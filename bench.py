@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- RTFx (audio-seconds / second) of the ASR inference hot path on B200.
+"""bench.py -- RTFx (audio-seconds / second) of the ASR inference hot path on H100.
 
-    python bench.py --gpus N --steps K --warmup W            # our sm_100a path
+    python bench.py --gpus N --steps K --warmup W            # our sm_90a path
+    python bench.py ... --dump-outputs DIR                   # + the last timed step's outputs as DIR/<name>.npy
     python bench.py --impl reference --gpus N --steps K ...   # the UNMODIFIED reference (baseline/_ref) on host CPU cores
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
@@ -12,7 +13,7 @@ SURVEY.md 8d).  One "step" = one pass of the whole path over one 32 x 10 s batch
 batches; the one exchange is an all-gather of the token ids (speechbrain_b200.parallel.gather_hypotheses, once per group
 call, inside the timed region).
 
-Other BASELINE configs (not the driver's line; run by hand, results in profiles/ and DESIGN.md):
+Other BASELINE configs (run by hand):
     --config small_enc     configs[1]: Conformer-small (12L/144d/4h RelPosMHAXL) encoder-only, 8 x 5 s
     --config beam10_lm     configs[3]: Conformer-L, beam 10 + TransformerLM (0.6) + CTC (0.4) scorers, 16 x 10 s, 48 steps
     --config beam10_shard  configs[4]: Conformer-L, beam 10 (no scorer), 32 x 10 s per GPU, NCCL gather of the hypotheses
@@ -22,7 +23,7 @@ value  : device-timed throughput, wav already resident in HBM.  The K-step regio
 e2e    : the same K steps through the host-buffer C-ABI call EncoderDecoderASR.transcribe_batches_async ->
          sbk_asr_transcribe_greedy_group_host_async: pinned host wav -> H2D -> pipeline -> D2H token ids, all inside the
          timed region.
-roofline: the dominant kernel (gemm_tc2_kernel, 2-CTA tcgen05) timed live per launch with CUDA events in a separate pass.
+roofline: the dominant kernels (the wgmma GEMMs) timed live per launch with CUDA events in a separate pass.
 cpu_baseline / --impl reference: the reference's own modules (pip-installed copy under baseline/_ref) on the host cores.
 """
 import argparse
@@ -44,11 +45,13 @@ METRIC = "audio-sec/sec (RTFx) Conformer-L ASR, batch=32x10s@16kHz"
 
 
 def peaks():
+    """HBM GB/s, sustained and burst dense fp16 TFLOP/s: MEASURED_PEAKS.json when present, else the H100 SXM data sheet
+    (3.35 TB/s, 989 TFLOP/s dense fp16 at 700 W; a card with a lower power limit sustains less)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1400.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet"
 
 
 def encoder_flops_per_utt(cfg, T):
@@ -300,6 +303,8 @@ def main():
     ap.add_argument("--group", type=int, default=16, help="max batches whose decode is coalesced into one greedy loop")
     ap.add_argument("--decode-steps", type=int, default=48, help="diagnostic: override the pinned 48 decode steps")
     ap.add_argument("--fuse-dec-ln", type=int, default=1)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the timed path computed in its last step to DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     args.ref_threads = args.ref_threads or None
     global DECODE_STEPS
@@ -347,7 +352,7 @@ def run_greedy32(args):
     wav_dev, lens_dev = wav_host.to(dev), lens_host.to(dev)
     L = wav_host.shape[1]
     T_f, T = eng.num_frames(L)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
     lib = _lib.lib()
 
     # ---- schedule: K steps = n_calls group calls (G <= --group batches each, balanced), NL groups in flight on NL streams.
@@ -454,6 +459,9 @@ def run_greedy32(args):
     launches = (lib.sbk_launch_count() - launches0) // R  # libsbk kernels inside one K-step region (graph nodes included)
     ms_host_all, _ = repeat(step_host)
     barrier()
+    if rank == 0 and args.dump_outputs:  # the device leg is the timed path; its last step = last batch of the last call
+        ln, g = (n_calls - 1) % NL, sizes[n_calls - 1]
+        dump_outputs(args.dump_outputs, tokens=preds[ln][g - 1])
     # parity of the two legs: same inputs -> same token ids
     e2e_matches_dev = all(bool(torch.equal(preds_host[0][g], preds[0][g].cpu())) for g in range(sizes[0])) if world == 1 else None
 
@@ -474,7 +482,7 @@ def run_greedy32(args):
     value = audio / (ms_dev / 1e3)
     e2e = audio / (ms_host / 1e3)
 
-    # ---- roofline leg: dominant kernel = the 2-CTA tcgen05 GEMM, timed live per launch with CUDA events (rank 0)
+    # ---- roofline leg: dominant kernels = the wgmma GEMMs, timed live per launch with CUDA events (rank 0)
     roof = None
     if rank == 0:
         import ctypes
@@ -493,10 +501,10 @@ def run_greedy32(args):
         ach = fl.value / (ms.value * 1e-3) / 1e12 if ms.value > 0 else 0.0
         enc_fl = BATCH * encoder_flops_per_utt(cfg, T)
         roof = {"bound": "tensor",
-                "kernel": "gemm_tc2_kernel (2-CTA tcgen05.mma cta_group::2 kind::f16, 256x256x64 tiles, fp16 in / fp32 acc in "
-                          "TMEM) -- all encoder / cross-K,V GEMM launches of one 32 x 10 s batch",
+                "kernel": "gemm_tc2_kernel / gemm_tc_kernel (wgmma m64nNk16, 128x256x64 and 128x128x64 tiles, fp16 in / fp32 "
+                          "acc in registers) -- all encoder / cross-K,V GEMM launches of one 32 x 10 s batch",
                 "achieved": ach, "peak": tf_sus, "unit": "TFLOP/s", "frac": ach / tf_sus,
-                "traffic": None,  # dram__bytes per launch is only available under ncu: see profiles/ (not hard-coded here)
+                "traffic": None,  # dram__bytes per launch is only available under ncu (not hard-coded here)
                 "peak_source": f"{src} bf16_tflops_sustained (kernel timed inside a long step)",
                 "launches_per_step": n.value, "gemm_ms_per_step": ms.value, "gemm_flops_per_step": fl.value,
                 "gemm_share_of_gpu_time_per_step": ms.value / (ms_dev / K),
@@ -519,7 +527,7 @@ def run_greedy32(args):
             times = time_reference(cfg, sd, BATCH, UTT_SECONDS, DECODE_STEPS, str(dev), 3, 1, 60.0)
             gpu_eager = {"value": BATCH * UTT_SECONDS / statistics.median(times), "unit": "audio-sec/sec",
                          "ms_per_step": 1e3 * statistics.median(times),
-                         "what": "the reference's own nn.Modules in eager PyTorch on this same B200 (TF32 on, as "
+                         "what": "the reference's own nn.Modules in eager PyTorch on this same GPU (TF32 on, as "
                                  "speechbrain/utils/quirks.py enables), wav on the device; informational competitor (SURVEY 2.3)"}
     if rank == 0:
         def spread(xs):
@@ -532,7 +540,7 @@ def run_greedy32(args):
                            "lanes": NL, "decode_group": G, "group_sizes": sizes, "decoder_ln_fused": bool(args.fuse_dec_ln),
                            "repeats": R, "ms_per_region": spread(ms_dev_all), "host_enqueue_ms_per_step": host_enqueue_ms,
                            "l2": "no flush inside the K-step bracket: per-step working set (0.25 GB weights + 0.3 GB "
-                                 "activations/KV per lane) exceeds the 126 MB L2; single_batch is flushed (256 MiB) per step",
+                                 "activations/KV per lane) exceeds the 50 MB L2; single_batch is flushed (256 MiB) per step",
                            "timing": f"median of {R} repetitions; each = one CUDA-event pair around K steps (= {n_calls} group "
                                      f"calls, sizes {sizes}), {NL} groups in flight on {NL} streams; max over ranks per repetition"},
                 "e2e": {"value": e2e, "unit": "audio-sec/sec", "ms_per_step": ms_host / K, "ms_per_region": spread(ms_host_all),
@@ -548,6 +556,17 @@ def run_greedy32(args):
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, **arrays):
+    """Each array -> out_dir/<name>.npy as float32 (float64 when the source is float64), so that two builds can be compared
+    output for output on the same seeded inputs."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.numpy().astype(np.float64 if t.dtype == torch.float64 else np.float32))
 
 
 def build_product_asr(cfg, sd, dev, decoder="greedy", beam=10, lm=False, ctc=False, coverage=None):
@@ -660,10 +679,18 @@ def run_other(args):
         dec = asr.mods["decoder"]
         T = asr.engine().num_frames(L)[1]
         hyp_buf = torch.full((B, DECODE_STEPS), -1, dtype=torch.int32, device=dev)
+        last = {}
+
+        def last_hyps():  # best hypothesis per utterance, padded with -1 to the decode limit
+            out = torch.full((B, DECODE_STEPS), -1, dtype=torch.int32)
+            for b, h in enumerate(last["hyps"]):
+                out[b, : len(h)] = torch.tensor(h, dtype=torch.int32)
+            return out
 
         def step(host):
             w, l_ = (wav_host, lens_host) if host else (wav_dev, lens_dev)
             words, hyps = asr.transcribe_batch(w, l_)  # public API: encode (fused pipeline) + beam search + host replay
+            last["hyps"] = hyps
             if world > 1:
                 hyp_buf.fill_(-1)
                 for b, h in enumerate(hyps):
@@ -695,6 +722,11 @@ def run_other(args):
     l0 = lib.sbk_launch_count()
     dev_ms = [region(False) for _ in range(R)]
     launches = (lib.sbk_launch_count() - l0) // R
+    if rank == 0 and args.dump_outputs:
+        if small:
+            dump_outputs(args.dump_outputs, encoder_out=enc_out)
+        else:
+            dump_outputs(args.dump_outputs, tokens=last_hyps())
     host_ms = [region(True) for _ in range(R)]
     t = torch.tensor([dev_ms, host_ms], device=dev, dtype=torch.float64)
     if world > 1:

@@ -1,4 +1,4 @@
-/* sbk.h -- C ABI of libsbk.so: the B200-native (sm_100a) ASR inference hot path behind SpeechBrain's
+/* sbk.h -- C ABI of libsbk.so: the H100-native (sm_90a) ASR inference hot path behind SpeechBrain's
  * module API.  Plain C: raw pointers + sizes, int error codes (0 = ok, <0 = error; text via
  * sbk_last_error()), an opaque CUDA stream (cudaStream_t passed as void*).  No torch types.
  *
@@ -69,7 +69,7 @@ typedef struct {
 const char* sbk_last_error(void); /* thread-local message of the last failing call */
 int sbk_version(void);
 long long sbk_launch_count(void); /* kernels launched by this library so far (graph replays included) */
-/* live per-launch timing of the tcgen05 GEMM (CUDA events on the launching stream); read after a sync */
+/* live per-launch timing of the wgmma GEMMs (CUDA events on the launching stream); read after a sync */
 void sbk_gemm_profile_enable(int on);
 int sbk_gemm_profile_read(int* n_launches, double* total_ms, double* total_flops);
 
@@ -91,7 +91,7 @@ int sbk_input_norm_global(const float* x_dev, float* out_dev, int B, int T, int 
 int sbk_input_norm_sentence(const float* x_dev, float* out_dev, const float* rel_len_dev, int B, int T, int F,
                             int std_norm, int avoid_padding_norm, float eps, void* stream);
 
-/* ---- tcgen05 GEMM self-test hook: out[M,N] = act(A[M,K] W[N,K]^T + bias) (fp16 in, fp32 accumulate) */
+/* ---- wgmma GEMM self-test hook: out[M,N] = act(A[M,K] W[N,K]^T + bias) (fp16 in, fp32 accumulate) */
 int sbk_gemm_f16_test(const void* A_dev, const void* W_dev, const float* bias_dev, void* out_dev, int out_is_f32,
                       int act, int M, int N, int K, void* stream);
 /* same kernel, residual epilogue (every Linear that closes a Conformer sub-block): x[M,N] += alpha * (A W^T + bias), fp32 in place */
@@ -115,7 +115,7 @@ int sbk_asr_set_poll_interval(sbk_asr* m, int every_n_steps);
  * 0 = separate LayerNorm kernel (less total GPU time when several batches are in flight). Same numerics. */
 int sbk_asr_set_decoder_ln_fusion(sbk_asr* m, int on);
 /* Decode steps with at least `rows` live hypotheses (several batches decoded together, wide beams) run their projections
- * on the tcgen05 GEMM instead of the weight-streaming kernel (default 64; a huge value = never, 1 = always). */
+ * on the wgmma GEMM instead of the weight-streaming kernel (default 64; a huge value = never, 1 = always). */
 int sbk_asr_set_decoder_tc_min_rows(sbk_asr* m, int rows);
 /* TransformerLMRescorer.rescore_hyps (decoders/scorer.py:1835-1882), device part: tokens_dev [n, L] int32 rows
  * "bos ... eos pad pad", lens_dev [n] int32 (tokens incl. bos/eos) -> scores_dev [n] fp32 = sum of log p(token | prefix) at

@@ -58,7 +58,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
-                f"{LIB_PATH} not found: the sm_100a CUDA library is required (no CPU fallback). "
+                f"{LIB_PATH} not found: the sm_90a CUDA library is required (no CPU fallback). "
                 "Build it with `make -C speechbrain_b200/csrc` or `__graft_entry__.build()`.")
         L = ctypes.CDLL(LIB_PATH)
         L.sbk_last_error.restype = ctypes.c_char_p

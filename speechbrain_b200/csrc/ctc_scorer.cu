@@ -1,4 +1,4 @@
-// CTC prefix scorer for joint CTC/attention beam search (full-vocabulary scoring), sm_100a.
+// CTC prefix scorer for joint CTC/attention beam search (full-vocabulary scoring), sm_90a.
 //
 // Reference: speechbrain/decoders/ctc.py:46-295 (CTCPrefixScore.__init__/forward_step/permute_mem) driven by
 // CTCScorer (decoders/scorer.py:183-249) as a *full* scorer of ScorerBuilder.score (:1221-1268), ctc_window_size = 0.
@@ -149,12 +149,10 @@ struct CtcArgs {
 // STREAMED through a shared-memory ring by bulk copies (one 1 KB row segment per copy, CTC_STAGE_ROWS rows per stage,
 // CTC_STAGES stages in flight, the first ones issued at kernel entry); the A tables arrive by ONE bulk copy from where
 // ctc_init / ctc_update left them.
-// History of this kernel (ncu: profiles/r2w_beam_ncu_full_summary.csv, r2aa_ctc_ncu_full_summary.csv): thread per
-// (hypothesis, token) log-domain recurrence 218 us (L2-bound: x re-read per hypothesis, one ex2 per term) -> linear domain,
-// 69-80 us in FIVE variants of the main loop (1 or 2 tokens per thread, 1 or 4 frame groups, register prefetch, bulk-copy
-// ring) because the main loop was never the problem: source-level samples put 45 % of the kernel in the prologue that built
-// the tables (two passes with integer divisions over 2 R T elements, redone by all 20 CTAs of an utterance), 17 % waiting
-// for data, 15 % in the FMAs -> tables moved to the kernels that produce the forward variables: 47 us.
+// History of this kernel: thread per (hypothesis, token) log-domain recurrence (L2-bound: x re-read per hypothesis, one ex2
+// per term) -> linear domain; the prologue that built the operand tables (two passes with integer divisions over 2 R T
+// elements, redone by all 20 CTAs of an utterance) then dominated, so the tables moved to the kernels that produce the
+// forward variables.
 // Every token uses the `rsum` table in the main loop; the one token per hypothesis that equals its last token (Alg.2-10:
 // phi = r_b instead) is recomputed from the second table by one warp of CTA column 0.
 constexpr int CTC_THREADS = 128;

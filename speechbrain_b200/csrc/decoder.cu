@@ -3,7 +3,7 @@
 // The reference (decoders/seq2seq.py:360-367,1929-1934 -> TransformerASR.decode
 // lobes/models/transformer/TransformerASR.py:426-473 -> Transformer.py:751-834,915-963) re-embeds and
 // re-runs all decoder layers over the WHOLE prefix every step and re-projects the encoder memory to K/V in
-// every layer every step. Here: cross-attention K/V are projected once per utterance (one tcgen05 GEMM
+// every layer every step. Here: cross-attention K/V are projected once per utterance (one wgmma GEMM
 // over all layers), self-attention K/V are appended to a cache, and one step touches only the newest token.
 // Numerically the step computes exactly the reference's last-position output.
 //
@@ -246,7 +246,7 @@ int skinny_gemm(const SkinnyArgs& a, cudaStream_t stream) {
     if (a.n_rows == 0) return SBK_OK;
     cudaError_t e;
     const int ry = ceil_div(a.n_rows, 32);
-    if (a.X == nullptr && a.n_rows >= 96 && getenv("SBK_SKINNY_MT8") != nullptr) {  // 128-row tiles: measured slower (64 fat CTAs), opt-in only
+    if (a.X == nullptr && a.n_rows >= 96 && getenv("SBK_SKINNY_MT8") != nullptr) {  // 128-row tiles (64 fat CTAs), opt-in only
         const dim3 grid(ceil_div(a.N, 8), ceil_div(a.n_rows, 128));
         if (a.K <= 1024) e = launch_k(skinny_gemm_kernel<2, 1, 0, 8>, grid, dim3(SK_WARPS * 32), 0, stream, a);
         else e = launch_k(skinny_gemm_kernel<4, 1, 0, 8>, grid, dim3(SK_WARPS * 32), 0, stream, a);
@@ -764,8 +764,7 @@ int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t s
     DecAttnArgs b = a;
     b.n_keys_fixed = max_keys;
     // cross-attention over an utterance's frames: optional TMA-staged variant (one box per (utterance, head), T <= 256).
-    // Measured equal to the register version (34.0 vs 32.1 us per 256-row layer-step = 4.1 TB/s, 62 % of the measured
-    // HBM copy peak): bytes in flight are not what limits it -> opt-in only.
+    // Opt-in only: bytes in flight are not what limits this kernel, so the register version stays the default.
     static const bool xatt_tma = getenv("SBK_DEC_XATT_TMA") != nullptr;
     if (a.n_keys_ptr == nullptr && a.lineage == nullptr && a.tok_cache == nullptr && max_keys <= 256 && xatt_tma &&
         a.vbase == a.kbase + a.H * 64 && (n_rows % a.rows_per_block) == 0) {
@@ -783,11 +782,11 @@ int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t s
         SBK_LAUNCH_CHECK();
         return SBK_OK;
     }
-    // persistent double-buffered TMA variant: measured SLOWER (42 us vs 32 us per 256-row layer-step -- with one 8-warp CTA
-    // per SM the two block barriers + merge per item cost more than the load/compute overlap wins) -> opt-in only
+    // persistent double-buffered TMA variant (opt-in only: with one 8-warp CTA per SM the two block barriers + merge per
+    // item cost about what the load/compute overlap wins)
     static const bool xatt_persist = getenv("SBK_DEC_XATT_PERSIST") != nullptr;
     if (a.n_keys_ptr == nullptr && a.lineage == nullptr && a.tok_cache == nullptr && max_keys <= 256 && xatt_persist &&
-        a.vbase == a.kbase + a.H * 64 && (n_rows % a.rows_per_block) == 0 && n_rows * a.H >= 4 * 148) {
+        a.vbase == a.kbase + a.H * 64 && (n_rows % a.rows_per_block) == 0 && n_rows * a.H >= 4 * SBK_NUM_SMS) {
         CUtensorMap tm;
         int rc = make_tmap_kv_f16(&tm, a.kbase, n_rows / a.rows_per_block, max_keys, a.H, a.key_stride, a.row_stride, max_keys);
         if (rc) return rc;

@@ -196,7 +196,7 @@ __global__ void cast_f32_f16_kernel(const float* __restrict__ in, __half* __rest
 }
 int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream) {
     if (n == 0) return SBK_OK;
-    const int blocks = static_cast<int>(std::min<size_t>((n + 255) / 256, 148 * 16));
+    const int blocks = static_cast<int>(std::min<size_t>((n + 255) / 256, SBK_NUM_SMS * 16));
     cast_f32_f16_kernel<<<blocks, 256, 0, stream>>>(in, out, n);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
@@ -205,8 +205,7 @@ int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream) {
 // --------------------------------------------------------------------------- depthwise conv + LN + Swish
 // glu [B*T, D] fp32 (GLU output) -> out [B*T, D] fp16 = Swish(LN(dwconv(glu) + bias)).  The tap weights arrive TAP-MAJOR
 // ([K, D], repacked from the reference's (D, 1, K) at load time): thread = channel, so the 31 weight loads of a thread are
-// coalesced across the warp (the channel-major layout made every load touch 32 cache lines -- ncu: lg_throttle the top
-// stall of the kernel).
+// coalesced across the warp (the channel-major layout made every load touch 32 cache lines).
 // Zero padding at utterance edges only: padded frames inside T are real inputs (Conformer.py:318-325
 // runs the conv before masking). One CTA per (utterance, tile of DW_TT frames); the (DW_TT + K - 1) x D
 // input slab is staged in shared memory once.

@@ -139,7 +139,7 @@ struct AsrModel {
     cudaGraphExec_t pipe_graph = nullptr;
     long long pipe_nodes = 0;
     int* weight_refs = nullptr;  // weights (arena + fbank plan) are shared between a handle and its clones (lanes)
-    int dec_tc_rows = getenv("SBK_DEC_TC_ROWS") ? atoi(getenv("SBK_DEC_TC_ROWS")) : 64;  // >= this many live hypotheses: tcgen05 decode GEMMs
+    int dec_tc_rows = getenv("SBK_DEC_TC_ROWS") ? atoi(getenv("SBK_DEC_TC_ROWS")) : 64;  // >= this many live hypotheses: wgmma decode GEMMs
     int dyn_chunk = 0, dyn_left = -1;  // DynChunkTrainConfig of the next encode calls (chunk frames, left-context chunks; 0 = off)
     int fuse_dec_ln = 1;         // 1: LayerNorm inside the projection kernel (latency); 0: separate LN kernel (throughput)
     int poll_every = 8;          // greedy early-exit poll interval in steps; 0 = never sync, run exactly max_steps
@@ -709,14 +709,14 @@ static int dec_ln(AsrModel* m, SkinnyArgs& a, const float* g, const float* bta, 
 }
 
 // Decode step when many hypotheses are live (several batches decoded together, or a wide beam): the projections run on
-// the tcgen05 GEMM (128 x 32/64 tiles, a handful of CTAs each, so concurrent lanes share the GPU) instead of the
+// the wgmma GEMM (128 x 32/64 tiles, a handful of CTAs each, so concurrent lanes share the GPU) instead of the
 // weight-streaming kernel whose cost grows with every 32 rows.  Same maths: fp16 operands, fp32 accumulate / residual.
 // Cross-attention K/V of every decoder layer, projected once per utterance from the encoder states (b.enc16).  Layout per
 // layer (default): [K | V] parts, each [utt][head][T][64] -- the decode-step attention of (utterance, head) then streams one
 // contiguous T x 128 B block of K and one of V instead of 128-byte pieces 2 KB apart (SBK_XATT_ROWMAJOR=1: the round-1
 // [utt * T][K(d) | V(d)] rows).  Needs head_dim 64.
 static bool xatt_headmajor(const AsrModel* m) {
-    static const bool legacy = getenv("SBK_XATT_ROWMAJOR") != nullptr || getenv("SBK_GEMM_V1") != nullptr;  // (scatter epilogue: 2-CTA kernel only)
+    static const bool legacy = getenv("SBK_XATT_ROWMAJOR") != nullptr || getenv("SBK_GEMM_V1") != nullptr;  // (scatter epilogue: wide-tile kernel only)
     return !legacy && m->cfg.d_model / m->cfg.nhead == 64 && m->cfg.d_model % 256 == 0;
 }
 static int project_cross_kv(AsrModel* m, int M, int T, cudaStream_t st) {
@@ -864,7 +864,7 @@ static int enqueue_decode_step(AsrModel* m, int rows, int rows_per_utt, int T, i
 // One TransformerLM step over `rows` hypotheses (post-norm encoder layers with a lineage-indexed KV cache), ending in
 // b.lm_extra[rows, V] = weight * log_softmax(lm_logits / temperature): TransformerLMScorer.score (scorer.py:510-543)
 // scaled by ScorerBuilder's weight.  b.lx / b.lx16 hold emb[token] * sqrt(d) + pe[step] (beam_reset / beam_step).
-// The same step with the projections on the tcgen05 GEMM (128 x 32/64 tiles): used when many hypotheses are live (wide beams,
+// The same step with the projections on the wgmma GEMM (128 x 32/64 tiles): used when many hypotheses are live (wide beams,
 // B * beam >= dec_tc_rows), where the weight-streaming kernel's cost grows with every 32 rows.
 static int enqueue_lm_step_tc(AsrModel* m, int rows, int S_max, float temperature, float weight, cudaStream_t st) {
     const sbk_asr_config& c = m->cfg;
@@ -1122,7 +1122,7 @@ static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos
     if (max_steps <= 0) return SBK_OK;
     RC(project_cross_kv(m, M, T, st));  // cross-attention K/V of all layers, once per utterance
     RC(greedy_reset(b.tokens, S_max + 1, rows, bos, b.step, b.has_ended, b.ended_count, m->emb, m->dec_pe, d, b.dx, st));
-    set_pdl(getenv("SBK_PDL") != nullptr);  // programmatic dependent launch measured slower here: opt-in only
+    set_pdl(getenv("SBK_PDL") != nullptr);  // programmatic dependent launch: opt-in only
     const bool use_graph = !in_capture && getenv("SBK_NO_GRAPH") == nullptr && log_probs == nullptr;
     if (in_capture) {  // the caller is capturing the whole pipeline: enqueue exactly max_steps steps, no polling
         for (int i = 0; i < max_steps; ++i) RC(enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, st));
@@ -1463,7 +1463,7 @@ static int transcribe_enqueue(AsrModel* m, const float* wav_dev, const float* re
 
 // G independent batches of B utterances: each batch goes through Fbank..encoder on its own (B-utterance kernels),
 // then ONE greedy loop decodes all G*B hypotheses together.  A decode step is ~50 dependent, latency-bound kernels
-// whose cost barely depends on the row count (measured: 0.32 ms for 32 rows), so coalescing the decode of the
+// whose cost barely depends on the row count, so coalescing the decode of the
 // batches in flight amortises it G-fold; per-utterance results are unchanged (rows are independent).
 static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_dev, const float* const* rel_dev, int B, int L,
                                     int max_steps, int bos, int eos, int* const* pred_dev, int* steps_done, cudaStream_t st,

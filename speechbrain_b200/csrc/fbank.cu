@@ -406,7 +406,7 @@ int fbank_forward(const Fbank* fb, const float* wav, int B, int L, float* out, i
     kern<<<grid, FB_THREADS, smem, stream>>>(wmap, wav, use_tma, B, L, T_f, d, out, utt_max);
     SBK_LAUNCH_CHECK();
     const size_t total = static_cast<size_t>(B) * T_f * d.n_mels;
-    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 8));
+    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, SBK_NUM_SMS * 8));
     fbank_finalize_kernel<<<blocks, 256, 0, stream>>>(out, out, utt_max, d.top_db, T_f * d.n_mels, d.n_mels, mean, stdv,
                                                       eps, total);
     SBK_LAUNCH_CHECK();
@@ -417,7 +417,7 @@ int global_norm_forward(const float* x, float* out, int B, int T, int F, const f
                         float eps, cudaStream_t stream) {
     const size_t total = static_cast<size_t>(B) * T * F;
     if (total == 0) return SBK_OK;
-    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 8));
+    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, SBK_NUM_SMS * 8));
     fbank_finalize_kernel<<<blocks, 256, 0, stream>>>(x, out, nullptr, 0.0f, T * F, F, mean, stdv, eps, total);
     SBK_LAUNCH_CHECK();
     return SBK_OK;

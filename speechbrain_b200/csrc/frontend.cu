@@ -26,8 +26,8 @@ __device__ __forceinline__ float leaky(float x) { return x > 0.0f ? x : 0.01f * 
 // w1: [C1, 3(kf), 3(kt)] fp32 (reference weight (C1,1,kf,kt)), b1: [C1]; g/be: [F1, C1].
 // One WARP per output frame (8 frames per CTA): lane l owns channels 2l, 2l+1 for all F1 feature rows, the frame's
 // F1 x C1 outputs stay in registers, so the LayerNorm over (F1, C1) needs only warp shuffles (no block barriers) and
-// every store is a 128-byte half2 row segment.  (The first version used one 256-thread CTA per frame with three block
-// barriers and 2-byte stores: 136 us per 32 x 10 s batch, 10x its HBM roofline.)
+// every store is a 128-byte half2 row segment (instead of one 256-thread CTA per frame with three block barriers and
+// 2-byte stores).
 constexpr int C1_WARPS = 8;
 
 template <int C1, int MAXF>
@@ -217,7 +217,7 @@ conv2_ln_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int F2,
 
 // --------------------------------------------------------------------------- conv1 + conv2 fused
 // The two-kernel version wrote conv1's output (B x T1 x F1 x 64 fp16 = 82 MB per 32 x 10 s batch) to global memory and read
-// it back: conv2 alone took 141 us on 82 MB of DRAM reads at 15 % occupancy (ncu, profiles/r2b_enc_summary.csv), conv1 92 us.
+// it back: conv2 was bound by those 82 MB of DRAM reads at low occupancy.
 // Here one CTA produces C2_FRAMES output frames from the input features directly: its 9 warps each compute one conv1 frame
 // (3x3 conv, LayerNorm over (F1, 64), LeakyReLU) with the frame held in registers, and write it -- fp16, reflect columns
 // included -- straight into the shared-memory patch the implicit-GEMM conv2 reads.  Global traffic per batch: the 10 MB of

@@ -1,5 +1,5 @@
-// Fused GEMM epilogues shared by the 1-CTA and the 2-CTA tcgen05 kernels: applied to 32 consecutive fp32
-// accumulator columns of one output row straight out of TMEM (tcgen05.ld 32x32b.x32).
+// Fused GEMM epilogues shared by the wgmma kernels: applied to 32 consecutive fp32 accumulator columns of one output row,
+// read from the staged accumulator tile (gemm_mainloop.cuh).
 #pragma once
 #include "common.cuh"
 #include "sbk_internal.h"
@@ -179,9 +179,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& e, const uint
 
 
 // ---------------------------------------------------------------------------------------------------------
-// Warp-cooperative, COALESCED variant (used by the 2-CTA kernel; needs N % 32 == 0 columns per chunk).
-// After tcgen05.ld each lane owns one row x 32 columns; storing that directly makes every warp-wide store touch
-// 32 different 128-byte lines (measured: the epilogue, not the MMA, bounded the GEMM).  Here the chunk is staged
+// Warp-cooperative, COALESCED variant (used by the wide-tile kernel; needs N % 32 == 0 columns per chunk).
+// With one row x 32 columns per lane, storing that directly makes every warp-wide store touch
+// 32 different 128-byte lines (the epilogue, not the MMA, would bound the GEMM).  Here the chunk is staged
 // through a per-warp shared-memory tile (row pitch 144 B, conflict-free for 16-byte accesses) and written back
 // with each instruction covering whole row segments (4 rows x 128 B or 8 rows x 64 B).
 constexpr int EPI_STG_PITCH = 144;                 // bytes per staged row (32 fp32 + 16 B pad)
@@ -193,8 +193,8 @@ __host__ __device__ constexpr int epi_stg_pitch() { return (MODE == EPI_F32 || M
 
 // EPI_RESID: out aliases resid (x += ...).  The 8 residual loads of a chunk are issued through this helper one chunk AHEAD
 // of the epilogue math (the first one before the accumulator is even complete), so their L2/HBM round trip hides behind
-// the main loop / the previous chunk instead of being eaten once per chunk (measured as the dominant long-scoreboard
-// stall of the N=512 GEMMs); they must also precede the first store or the compiler serialises load i after store i-1.
+// the main loop / the previous chunk instead of being eaten once per chunk (a long-scoreboard stall in every chunk
+// of the N=512 GEMMs otherwise); they must also precede the first store or the compiler serialises load i after store i-1.
 __device__ __forceinline__ void epilogue_resid_prefetch(const GemmEpilogue& e, float4 (&res)[8], int row_base, int col0, int M,
                                                         int lane) {
     const int seg = lane & 7, rsub = lane >> 3;
@@ -208,7 +208,7 @@ __device__ __forceinline__ void epilogue_resid_prefetch(const GemmEpilogue& e, f
 
 // EPI_ROPE: the rotation is applied in the write-back phase, where 4 lanes cover 32 consecutive columns of a row (8 rows
 // per instruction): each lane needs 4 cos + 4 sin of its row -- one 16-byte load each, 64 contiguous bytes per row.  (With
-// one row per lane, as after tcgen05.ld, every table load touched 32 different lines and the L1 tag stage, not the tensor
+// one row per lane, every table load touched 32 different lines and the L1 tag stage, not the tensor
 // pipe, bounded the QKV GEMM: tensor pipe 18 %, issue slots 12 % busy.)  The 8 loads of a chunk are fetched one chunk
 // ahead: with ~200 KB of the SM carved out as shared memory the tables do not survive in L1.
 __device__ __forceinline__ void epilogue_rope_prefetch(const GemmEpilogue& e, float4 (&rc)[4], float4 (&rs)[4], int row_base,

@@ -1,0 +1,135 @@
+// TMA + wgmma main loop shared by the GEMM kernels of gemm_tc.cu and gemm_tc2.cu:
+//
+//     acc = A[m0 .. m0 + 128, k-blocks] x W[n0 .. n0 + BN, k-blocks]^T    (fp16 operands, fp32 accumulate in registers)
+//
+// 288 threads: warps 0..7 are two consumer warpgroups (warpgroup g owns tile rows 64 g .. 64 g + 63), warp 8 is the TMA
+// producer (one elected lane).  A ring of STAGES (A 16 KB | W BN x 128 B, both 128B-swizzled K-major) is guarded by
+// full / empty mbarriers; a consumer warpgroup frees a stage as soon as the wgmma that read it has retired
+// (wait_group 1 keeps one k-block of MMAs in flight behind the next stage's).  After the loop the accumulators are
+// staged as an fp32 [128][BN] tile over the (then idle) ring, so that the epilogues can work on rows of 32 columns.
+#pragma once
+#include "common.cuh"
+
+namespace sbk {
+
+constexpr int WG_BM = 128;
+constexpr int WG_BK = 64;
+constexpr int WG_CONSUMERS = 256;
+constexpr int WG_THREADS = WG_CONSUMERS + 32;
+
+template <int BN>
+struct WgAcc {
+    static constexpr int WN = BN < 128 ? BN : 128;  // wgmma width: BN = 256 issues two n128 instructions per k step
+    static constexpr int NI = BN / WN;
+    float r[NI][WN / 2];
+};
+
+template <int BN, int STAGES>
+struct WgRing {
+    static constexpr int A_BYTES = WG_BM * WG_BK * 2;
+    static constexpr int B_BYTES = BN * WG_BK * 2;
+    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+    static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+    static constexpr int END = BAR_OFFSET + 2 * STAGES * 8;
+    // fp32 accumulator staging row; the 16-byte pad makes 16-byte accesses of 8 consecutive rows conflict-free
+    static constexpr int STG_PITCH = BN * 4 + 16;
+    static_assert(STAGE_BYTES % 1024 == 0, "128B-swizzled stages must stay 1 KB aligned");
+    static_assert(WG_BM * STG_PITCH <= BAR_OFFSET, "the accumulator staging tile reuses the operand ring");
+};
+
+// consumer warpgroups only (256 threads): named barrier 1
+__device__ __forceinline__ void wg_consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS) : "memory"); }
+
+// all threads: barriers initialised before any role starts
+template <int BN, int STAGES>
+__device__ __forceinline__ void wg_init(uint8_t* smem, const CUtensorMap* ta, const CUtensorMap* tb) {
+    using R = WgRing<BN, STAGES>;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + R::BAR_OFFSET);
+    uint64_t* empty_bar = full_bar + STAGES;
+    if (threadIdx.x == WG_CONSUMERS) {
+        tma_prefetch_desc(ta);
+        tma_prefetch_desc(tb);
+        for (int s = 0; s < STAGES; ++s) {
+            mbar_init(&full_bar[s], 1);   // producer's expect_tx arrive
+            mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+}
+
+// producer warp: k-blocks kb0 .. kb0 + num_kb of rows m0 (A) and n0 (W)
+template <int BN, int STAGES>
+__device__ __forceinline__ void wg_produce(uint8_t* smem, const CUtensorMap* ta, const CUtensorMap* tb, int m0, int n0,
+                                           int kb0, int num_kb) {
+    using R = WgRing<BN, STAGES>;
+    if (threadIdx.x != WG_CONSUMERS) return;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + R::BAR_OFFSET);
+    uint64_t* empty_bar = full_bar + STAGES;
+    for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % STAGES;
+        const uint32_t ph = (kb / STAGES) & 1;
+        mbar_wait(&empty_bar[s], ph ^ 1);
+        mbar_arrive_expect_tx(&full_bar[s], R::STAGE_BYTES);
+        uint8_t* a_dst = smem + s * R::STAGE_BYTES;
+        tma_load_2d(a_dst, ta, &full_bar[s], (kb0 + kb) * WG_BK, m0);
+        tma_load_2d(a_dst + R::A_BYTES, tb, &full_bar[s], (kb0 + kb) * WG_BK, n0);
+    }
+}
+
+// consumer warpgroups: the whole k loop, then the accumulators -> fp32 staging tile at smem (row pitch STG_PITCH).
+// Ends with the staging tile complete and visible to all 256 consumer threads.
+template <int BN, int STAGES>
+__device__ __forceinline__ void wg_consume_and_stage(uint8_t* smem, int num_kb) {
+    using R = WgRing<BN, STAGES>;
+    using Acc = WgAcc<BN>;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + R::BAR_OFFSET);
+    uint64_t* empty_bar = full_bar + STAGES;
+    const int wg = threadIdx.x >> 7;
+    Acc acc;
+#pragma unroll
+    for (int i = 0; i < Acc::NI; ++i)
+#pragma unroll
+        for (int j = 0; j < Acc::WN / 2; ++j) acc.r[i][j] = 0.0f;
+    for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % STAGES;
+        const uint32_t ph = (kb / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t a_addr = smem_u32(smem + s * R::STAGE_BYTES) + wg * 64 * 128;
+        const uint32_t b_addr = smem_u32(smem + s * R::STAGE_BYTES) + R::A_BYTES;
+        const uint64_t da = make_kmajor_sw128_desc(a_addr);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < WG_BK / 16; ++k)  // +32 B per k16 step -> +2 in (addr >> 4)
+#pragma unroll
+            for (int i = 0; i < Acc::NI; ++i)
+                wgmma_f16<Acc::WN>(acc.r[i], da + 2 * k, make_kmajor_sw128_desc(b_addr + i * Acc::WN * 128) + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(kb - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    wg_consumers_sync();  // both warpgroups are done reading the ring before it is overwritten
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    uint8_t* base = smem + (wg * 64 + w * 16 + (l >> 2)) * R::STG_PITCH + (l & 3) * 8;
+#pragma unroll
+    for (int i = 0; i < Acc::NI; ++i)
+#pragma unroll
+        for (int j = 0; j < Acc::WN / 8; ++j) {
+            const int col = i * Acc::WN + j * 8;
+            *reinterpret_cast<float2*>(base + col * 4) = make_float2(acc.r[i][4 * j], acc.r[i][4 * j + 1]);
+            *reinterpret_cast<float2*>(base + 8 * R::STG_PITCH + col * 4) = make_float2(acc.r[i][4 * j + 2], acc.r[i][4 * j + 3]);
+        }
+    wg_consumers_sync();
+}
+
+// 32 consecutive staged fp32 columns of one row (16-byte aligned shared-memory address)
+__device__ __forceinline__ void wg_load_row32(uint32_t addr, uint32_t (&a)[32]) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const uint4 v = lds128(addr + 16 * j);
+        a[4 * j] = v.x; a[4 * j + 1] = v.y; a[4 * j + 2] = v.z; a[4 * j + 3] = v.w;
+    }
+}
+
+}  // namespace sbk

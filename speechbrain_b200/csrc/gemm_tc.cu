@@ -1,44 +1,31 @@
-// tcgen05 / TMEM / TMA GEMM for the Conformer encoder (and decoder prefill):
+// wgmma / TMA GEMM for the Conformer encoder (and decoder prefill, decode-step projections):
 //
-//     out = epilogue( A[M,K] (fp16, K-major) x W[N,K]^T (fp16, K-major) ), fp32 accumulate in TMEM
+//     out = epilogue( A[M,K] (fp16, K-major) x W[N,K]^T (fp16, K-major) ), fp32 accumulate in registers
 //
 // Replaces the reference's F.linear / nn.Linear / Conv1d(k=1) call sites
 // (nnet/attention.py:623,739,932-936,1344; Conformer.py:126-157; TransformerASR.py:308-316).
 //
-// One 128 x BN output tile per CTA, 192 threads:
-//   warp 0      : TMA producer (one elected lane), 128B-swizzled K-major tiles of 64 halfs
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128 x BN x 16)
-//   warps 2..5  : epilogue; warp w drains TMEM lanes 32*(w%4).. with tcgen05.ld 32x32b.x32
-// smem ring of STAGES (A 16 KB + B BN*128 B) guarded by full/empty mbarriers; the MMA
-// completion is published with tcgen05.commit.  Two CTAs fit per SM (3 x 32 KB stages,
-// 128 TMEM columns each) so one CTA's epilogue overlaps the other's main loop.
+// One 128 x BN output tile per CTA (main loop: gemm_mainloop.cuh).  The epilogue runs row-wise on 32-column chunks of
+// the staged accumulator tile, so it handles any N and every epilogue mode, including partial column chunks.  With
+// BN <= 128 two CTAs fit per SM, so one CTA's epilogue overlaps the other's main loop.
 #include <stdlib.h>
 
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
+#include "gemm_mainloop.cuh"
 #include "sbk_internal.h"
 
 namespace sbk {
 
-constexpr int GEMM_BM = 128;
-constexpr int GEMM_BK = 64;
-constexpr int GEMM_THREADS = 192;
-
 template <int BN, int STAGES, int SPLIT = 1>
 struct GemmSmem {
-    static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
-    static constexpr int B_BYTES = BN * GEMM_BK * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-    static constexpr int PART_OFFSET = BAR_OFFSET + 256;                 // split-K: partial tiles of ranks 1..SPLIT-1
-    static constexpr int PART_BYTES = (SPLIT - 1) * GEMM_BM * BN * 4;    // (fp32 [SPLIT-1][128][BN], in rank 0's smem)
-    static constexpr int TOTAL = PART_OFFSET + PART_BYTES + 1024;        // + alignment slack
+    static constexpr int TOTAL = WgRing<BN, STAGES>::END + 1024;  // + alignment slack
 };
 
-// ---- split-K over a thread-block cluster (1, 1, SPLIT): CTA `rank` accumulates k-blocks [rank, rank+1) * num_kb / SPLIT
-// in its own TMEM, ranks > 0 ship their fp32 partial tile into rank 0's shared memory (DSMEM), rank 0 adds them in rank
-// order (deterministic) and runs the epilogue.  For the decode-step GEMMs with K = d_ffn: one CTA would have to stream
-// 128 x K of activations through a single SM (~10 us); four CTAs each stream a quarter.
+// ---- split-K over a thread-block cluster (1, 1, SPLIT): CTA `rank` accumulates k-blocks [rank, rank+1) * num_kb / SPLIT,
+// rank 0 reads the other ranks' staged fp32 partial tiles out of their shared memory (DSMEM), adds them in rank order
+// (deterministic) and runs the epilogue.  For the decode-step GEMMs with K = d_ffn: one CTA would have to stream
+// 128 x K of activations through a single SM; four CTAs each stream a quarter.
 __device__ __forceinline__ uint32_t gemm_cluster_rank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -48,139 +35,59 @@ __device__ __forceinline__ void gemm_cluster_sync() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void st_cluster_f4(const void* local_ptr, uint32_t cta, float a, float b, float c, float d) {
+__device__ __forceinline__ uint4 ld_cluster_u4(uint32_t local_addr, uint32_t cta) {
     uint32_t raddr;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(local_ptr)), "r"(cta));
-    asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(raddr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(local_addr), "r"(cta));
+    uint4 v;
+    asm volatile("ld.shared::cluster.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(raddr)
+                 : "memory");
+    return v;
 }
 
 template <int BN, int STAGES, int SPLIT = 1>
-__global__ void __launch_bounds__(GEMM_THREADS, (BN <= 128 ? 2 : 1))
+__global__ void __launch_bounds__(WG_THREADS, (BN <= 128 ? 2 : 1))
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmEpilogue epi, int M, int N, int K) {
-    using S = GemmSmem<BN, STAGES, SPLIT>;
+    using R = WgRing<BN, STAGES>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BAR_OFFSET);
-    uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full_bar = empty_bar + STAGES;
-    uint32_t* tmem_base_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * GEMM_BM;
+    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * WG_BM;
     const uint32_t rank = SPLIT > 1 ? gemm_cluster_rank() : 0u;
-    const int num_kb = (K + GEMM_BK - 1) / GEMM_BK / SPLIT;   // k-blocks of this CTA (host checks divisibility)
+    const int num_kb = (K + WG_BK - 1) / WG_BK / SPLIT;   // k-blocks of this CTA (host checks divisibility)
     const int kb0 = static_cast<int>(rank) * num_kb;
 
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_a);
-        tma_prefetch_desc(&tmap_b);
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(tmem_full_bar, 1);
-        mbar_fence_init();
-    }
-    if (warp == 1) tmem_alloc(tmem_base_ptr, BN);
-    tc_fence_before();
-    __syncthreads();
-    if constexpr (SPLIT > 1) gemm_cluster_sync();  // every CTA of the cluster is resident before any DSMEM traffic
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_ptr;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const int s = kb % STAGES;
-                const uint32_t ph = (kb / STAGES) & 1;
-                mbar_wait(&empty_bar[s], ph ^ 1);
-                mbar_arrive_expect_tx(&full_bar[s], S::STAGE_BYTES);
-                uint8_t* a_dst = smem + s * S::STAGE_BYTES;
-                tma_load_2d(a_dst, &tmap_a, &full_bar[s], (kb0 + kb) * GEMM_BK, m0);
-                tma_load_2d(a_dst + S::A_BYTES, &tmap_b, &full_bar[s], (kb0 + kb) * GEMM_BK, n0);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_f16(GEMM_BM, BN, 0);
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const int s = kb % STAGES;
-                const uint32_t ph = (kb / STAGES) & 1;
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES);
-                const uint64_t da = make_kmajor_sw128_desc(a_addr);
-                const uint64_t db = make_kmajor_sw128_desc(a_addr + S::A_BYTES);
-#pragma unroll
-                for (int k = 0; k < GEMM_BK / 16; ++k)  // +32 B per UMMA_K=16 halfs -> +2 in (addr>>4)
-                    umma_f16(tmem_base, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                umma_commit(&empty_bar[s]);
-            }
-            umma_commit(tmem_full_bar);
-        }
+    wg_init<BN, STAGES>(smem, &tmap_a, &tmap_b);
+    EpiPrefetch pre;
+    if (threadIdx.x >= WG_CONSUMERS) {
+        wg_produce<BN, STAGES>(smem, &tmap_a, &tmap_b, m0, n0, kb0, num_kb);
     } else {
-        const int q = warp & 3;  // TMEM lane quarter this warp may access
-        const int row = m0 + q * 32 + lane;
-        EpiPrefetch pre;
-        if constexpr (BN == 32 && SPLIT == 1) epilogue_prefetch(epi, pre, row, n0, M, N);  // while the main loop runs
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-        if constexpr (SPLIT == 1) {
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t acc[32];
-                tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c * 32, acc);
-                tmem_ld_wait();
-                epilogue_chunk(epi, acc, row, n0 + c * 32, M, N, pre);
-            }
-        } else if (rank != 0) {
-            float* part = reinterpret_cast<float*>(smem + S::PART_OFFSET) +
-                          (static_cast<size_t>(rank - 1) * GEMM_BM + q * 32 + lane) * BN;
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t acc[32];
-                tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c * 32, acc);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    st_cluster_f4(part + c * 32 + j, 0, __uint_as_float(acc[j]), __uint_as_float(acc[j + 1]),
-                                  __uint_as_float(acc[j + 2]), __uint_as_float(acc[j + 3]));
-            }
-        }
+        if constexpr (BN == 32 && SPLIT == 1)  // while the main loop runs
+            if (threadIdx.x < WG_BM) epilogue_prefetch(epi, pre, m0 + threadIdx.x, n0, M, N);
+        wg_consume_and_stage<BN, STAGES>(smem, num_kb);
     }
-    if constexpr (SPLIT > 1) {
-        tc_fence_before();
-        gemm_cluster_sync();  // partial tiles have landed in rank 0's shared memory (release / acquire)
-        if (rank == 0 && warp >= 2) {
-            tc_fence_after();
-            const int q = warp & 3;
-            const int row = m0 + q * 32 + lane;
+    if constexpr (SPLIT > 1) gemm_cluster_sync();  // every rank's partial tile is staged (release / acquire)
+    if (threadIdx.x < WG_CONSUMERS && rank == 0) {
+        const int r = threadIdx.x & (WG_BM - 1);
 #pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t acc[32];
-                tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c * 32, acc);
-                tmem_ld_wait();
+        for (int c = threadIdx.x / WG_BM; c < BN / 32; c += WG_CONSUMERS / WG_BM) {
+            const uint32_t src = smem_u32(smem) + r * R::STG_PITCH + c * 128;
+            uint32_t acc[32];
+            wg_load_row32(src, acc);
 #pragma unroll 1
-                for (int r = 0; r < SPLIT - 1; ++r) {  // fixed order: deterministic sum
-                    const float* part = reinterpret_cast<const float*>(smem + S::PART_OFFSET) +
-                                        (static_cast<size_t>(r) * GEMM_BM + q * 32 + lane) * BN + c * 32;
+            for (int p = 1; p < SPLIT; ++p) {  // fixed order: deterministic sum
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const float4 p4 = *reinterpret_cast<const float4*>(part + j);
-                        acc[j] = __float_as_uint(__uint_as_float(acc[j]) + p4.x);
-                        acc[j + 1] = __float_as_uint(__uint_as_float(acc[j + 1]) + p4.y);
-                        acc[j + 2] = __float_as_uint(__uint_as_float(acc[j + 2]) + p4.z);
-                        acc[j + 3] = __float_as_uint(__uint_as_float(acc[j + 3]) + p4.w);
-                    }
+                for (int j = 0; j < 8; ++j) {
+                    const uint4 v = ld_cluster_u4(src + 16 * j, static_cast<uint32_t>(p));
+                    acc[4 * j] = __float_as_uint(__uint_as_float(acc[4 * j]) + __uint_as_float(v.x));
+                    acc[4 * j + 1] = __float_as_uint(__uint_as_float(acc[4 * j + 1]) + __uint_as_float(v.y));
+                    acc[4 * j + 2] = __float_as_uint(__uint_as_float(acc[4 * j + 2]) + __uint_as_float(v.z));
+                    acc[4 * j + 3] = __float_as_uint(__uint_as_float(acc[4 * j + 3]) + __uint_as_float(v.w));
                 }
-                epilogue_chunk(epi, acc, row, n0 + c * 32, M, N, EpiPrefetch());
             }
+            epilogue_chunk(epi, acc, m0 + r, n0 + c * 32, M, N, pre);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, BN);
+    if constexpr (SPLIT > 1) gemm_cluster_sync();  // the other ranks keep their shared memory until rank 0 has read it
 }
 
 template <int BN, int STAGES, int SPLIT = 1>
@@ -188,13 +95,13 @@ static int launch_gemm(const void* A, int lda, const void* W, int ldw, const Gem
                        cudaStream_t stream) {
     using S = GemmSmem<BN, STAGES, SPLIT>;
     CUtensorMap ta, tb;
-    int rc = make_tmap_2d_f16(&ta, A, M, K, lda, GEMM_BM, GEMM_BK);
+    int rc = make_tmap_2d_f16(&ta, A, M, K, lda, WG_BM, WG_BK);
     if (rc) return rc;
-    rc = make_tmap_2d_f16(&tb, W, N, K, ldw, BN, GEMM_BK);
+    rc = make_tmap_2d_f16(&tb, W, N, K, ldw, BN, WG_BK);
     if (rc) return rc;
     auto kern = gemm_tc_kernel<BN, STAGES, SPLIT>;
     SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    dim3 grid(ceil_div(N, BN), ceil_div(M, GEMM_BM), SPLIT);
+    dim3 grid(ceil_div(N, BN), ceil_div(M, WG_BM), SPLIT);
     GemmProfile* prof = gemm_profile();
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (prof->enabled) {
@@ -203,11 +110,11 @@ static int launch_gemm(const void* A, int lda, const void* W, int ldw, const Gem
         cudaEventRecord(e0, stream);
     }
     if constexpr (SPLIT == 1) {
-        kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(ta, tb, epi, M, N, K);
+        kern<<<grid, WG_THREADS, S::TOTAL, stream>>>(ta, tb, epi, M, N, K);
     } else {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = grid;
-        cfg.blockDim = dim3(GEMM_THREADS);
+        cfg.blockDim = dim3(WG_THREADS);
         cfg.dynamicSmemBytes = S::TOTAL;
         cfg.stream = stream;
         cudaLaunchAttribute attr[1];
@@ -243,10 +150,10 @@ int gemm_f16_small(const void* A, int lda, const void* W, int ldw, const GemmEpi
                     "gemm_f16_small: bad EPI_QKV_CACHE arguments");
     // few, latency-bound CTAs: narrow N tiles spread the weight stream over more SMs; the ring holds a whole K = 512 panel
     if (N > 2048) return launch_gemm<64, 6>(A, lda, W, ldw, epi, M, N, K, stream);
-    // K = d_ffn: 4-way cluster split-K (deterministic DSMEM reduce) shortens that one kernel (16.8 -> 13.9 us at 256 rows)
-    // but its 4x CTAs take SMs from the other lanes: measured 2 % slower end to end with 4 lanes in flight -> opt-in
+    // K = d_ffn: 4-way cluster split-K (deterministic DSMEM reduce) shortens that one kernel, but its 4x CTAs take SMs from
+    // the other lanes in flight -> opt-in
     static const bool split = getenv("SBK_DEC_SPLITK") != nullptr;
-    if (K >= 2048 && K % (4 * GEMM_BK) == 0 && split)
+    if (K >= 2048 && K % (4 * WG_BK) == 0 && split)
         return launch_gemm<32, 8, 4>(A, lda, W, ldw, epi, M, N, K, stream);
     return launch_gemm<32, 8>(A, lda, W, ldw, epi, M, N, K, stream);
 }
@@ -260,7 +167,7 @@ int gemm_f16(const void* A, int lda, const void* W, int ldw, const GemmEpilogue&
     if (epi.mode == EPI_GLU || epi.mode == EPI_ROPE)
         SBK_REQUIRE(N % 32 == 0, "gemm_f16: GLU/RoPE epilogues need N %% 32 == 0");
     if (epi.mode == EPI_ROPE) SBK_REQUIRE(epi.head_dim % 32 == 0, "gemm_f16: RoPE epilogue needs head_dim %% 32 == 0");
-    if (N % 256 == 0 && getenv("SBK_GEMM_V1") == nullptr) return gemm_f16_2cta(A, lda, W, ldw, epi, M, N, K, stream);
+    if (N % 256 == 0 && getenv("SBK_GEMM_V1") == nullptr) return gemm_f16_wide(A, lda, W, ldw, epi, M, N, K, stream);
     return launch_gemm<128, 3>(A, lda, W, ldw, epi, M, N, K, stream);
 }
 

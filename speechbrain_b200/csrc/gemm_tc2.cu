@@ -1,332 +1,93 @@
-// 2-CTA (cta_group::2) persistent tcgen05 GEMM: out = epilogue(A[M,K] x W[N,K]^T), fp16 in / fp32 accumulate.
+// Wide-tile wgmma GEMM for N % 256 == 0: out = epilogue(A[M,K] x W[N,K]^T), fp16 in / fp32 accumulate.
 //
-// A CTA pair (cluster 2x1x1, two SMs of one TPC) owns a 256 x 256 output tile: CTA r holds rows
-// [m0 + 128 r, +128) of A and rows [n0 + 128 r, +128) of W in its shared memory, the leader issues
-// tcgen05.mma.cta_group::2 (UMMA 256 x 256 x 16) which reads both halves, and each CTA's TMEM receives its
-// own 128 accumulator rows.  Versus the 1-CTA 128x128 kernel this halves the L2->SM operand traffic per FLOP
-// (32 KB per 2 MMACs per CTA instead of 32 KB per 1 MMAC), which is what bounds these K = 512..2048 GEMMs.
-//
-// Persistent: 74 pairs loop over the tiles (n fastest, so pairs working on the same rows of A run together).
-// Warp roles per CTA: warp 0 TMA producer (6-stage ring, loads signal the LEADER's full barrier through the
-// cta_group::2 TMA form), warp 1 MMA issuer (leader only; commits multicast to both CTAs' barriers),
-// warps 2..5 epilogue.  TMEM holds two 256-column accumulator buffers, so the epilogue of tile i overlaps
-// the main loop of tile i+1.
+// One 128 x 256 output tile per CTA (main loop: gemm_mainloop.cuh; each consumer warpgroup issues two m64n128k16 per k
+// step), a 4-stage ring of 48 KB stages.  Versus the 128 x 128 tiles of gemm_tc.cu this halves the L2 -> SM traffic of
+// the A operand per FLOP, which is what bounds these K = 512..2048 GEMMs.  The grid runs n fastest, so the CTAs that
+// share the rows of A are resident together.
+// Epilogue: the 8 consumer warps each own 32 rows x 128 columns of the staged tile and run the warp-cooperative,
+// coalesced epilogue (gemm_epilogue.cuh) on it chunk by chunk, the staged rows doubling as its staging area.
 #include <stdio.h>
 #include <stdlib.h>
 
-#include <algorithm>
-
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
+#include "gemm_mainloop.cuh"
 #include "sbk_internal.h"
 
 namespace sbk {
 
-constexpr int G2_BM = 128;        // rows per CTA (256 per pair)
-constexpr int G2_BN = 256;        // columns per pair tile (default; template parameter BN of the kernel)
-constexpr int G2_BK = 64;
-constexpr int G2_STAGES = 5;
-// epilogue warps: EW / 4 warps per TMEM lane quarter, each drains 1 / (EW / 4) of the tile's columns.  The modes that
-// prefetch per-chunk operands (residual, RoPE tables: 32 more registers) keep 8; the MUFU/ALU-heavy fp16 modes (SiLU, GLU)
-// use 16 so every scheduler has 4 epilogue warps to hide latencies behind.
-template <int MODE>
-constexpr int g2_epi_warps() { return (MODE == EPI_F32 || MODE == EPI_RESID || MODE == EPI_ROPE) ? 8 : 16; }
-constexpr int G2_A_BYTES = G2_BM * G2_BK * 2;            // 16 KB
-// shared-memory map for a tile width BN and a ring of ST stages: [ST x (A 16 KB | this CTA's BN/2 rows of W)] [barriers]
-// [per-epilogue-warp staging tiles (32 rows x pitch)]
+constexpr int G2_BN = 256;       // columns per tile (default; template parameter BN of the kernel)
+constexpr int G2_STAGES = 4;
+// shared-memory map: [ring | barriers] [BN floats: the tile's bias vector] (+ alignment slack)
 template <int BN, int ST>
-struct G2Cfg {
-    static constexpr int B_BYTES = (BN / 2) * G2_BK * 2;
-    static constexpr int STAGE_BYTES = G2_A_BYTES + B_BYTES;
-    static constexpr int BAR_OFFSET = ST * STAGE_BYTES;
-    static constexpr int STG_OFFSET = BAR_OFFSET + 256;
-    static_assert(STAGE_BYTES % 1024 == 0, "128B-swizzled stages must stay 1 KB aligned");
-    static_assert((2 * ST + 4) * 8 + 4 <= 256, "barrier block");
-};
-// (+ BN floats: the tile's bias vector, staged once per tile by the epilogue warps)
-template <int MODE, int EW, int BN, int ST>
-constexpr int g2_bias_offset() { return G2Cfg<BN, ST>::STG_OFFSET + EW * 32 * epi_stg_pitch<MODE>(); }
-template <int MODE, int EW, int BN, int ST>
-constexpr int g2_smem() { return g2_bias_offset<MODE, EW, BN, ST>() + BN * 4 + 1024; }
+__host__ __device__ constexpr int g2_bias_offset() { return (WgRing<BN, ST>::END + 15) / 16 * 16; }
+template <int BN, int ST>
+__host__ __device__ constexpr int g2_smem() { return g2_bias_offset<BN, ST>() + BN * 4 + 1024; }
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// bounded wait: a protocol bug must trap (and fail the test), never hang the GPU
-__device__ __forceinline__ void mbar_wait_b(uint64_t* bar, uint32_t parity, int tag) {
-    for (uint32_t spins = 0; !mbar_try_wait(bar, parity); ++spins) {
-        if (spins > (1u << 26)) {
-            printf("gemm2: barrier timeout tag=%d block=%d thread=%d\n", tag, blockIdx.x, threadIdx.x);
-            __trap();
-        }
-    }
-}
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-    uint32_t raddr;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(bar)), "r"(cta));
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
-}
-// 2-SM TMA load: data lands in THIS CTA's shared memory, the transaction bytes are counted on the LEADER's barrier
-// (peer bit of the barrier address cleared, cute::Sm100MmaPeerBitMask).
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive (once) on the barrier at this offset in BOTH CTAs when all prior MMAs of this thread complete
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint32_t lead_rank) {
-    const uint16_t mask = static_cast<uint16_t>(3u << lead_rank);
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask)
-                 : "memory");
-}
-__device__ __forceinline__ void umma_commit_mask(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask)
-                 : "memory");
-}
-// 2-SM TMA load multicast to the CTAs in `mask` (same shared-memory offset in each; each destination's bytes are counted on
-// the barrier at this offset of ITS pair leader)
-__device__ __forceinline__ void tma_load_2d_2sm_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                   uint16_t mask) {
-    const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_leader), "r"(c0), "r"(c1), "h"(mask)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// Cluster size is a launch attribute: 2 (one pair) or 4 (two pairs working on the two n-neighbour tiles of the same 256
-// rows, so that both pairs pull the same A tiles from L2 at the same time -- see gemm_f16_2cta).
-template <int MODE, int ACT, int EW, int BN = G2_BN, int ST = G2_STAGES>
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
+template <int MODE, int ACT, int BN = G2_BN, int ST = G2_STAGES>
+__global__ void __launch_bounds__(WG_THREADS, 1)
 gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                const __grid_constant__ CUtensorMap tmap_a64, const GemmEpilogue epi, int M, int N, int K, int mc) {
-    using C = G2Cfg<BN, ST>;
+                const GemmEpilogue epi, int M, int N, int K) {
+    using R = WgRing<BN, ST>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);   // [STAGES]  (used on the leader)
-    uint64_t* empty_bar = full_bar + ST;                               // [STAGES]  (each CTA its own)
-    uint64_t* tmem_full_bar = empty_bar + ST;                          // [2]       (each CTA its own)
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;                             // [2]       (used on the leader)
-    uint32_t* tmem_base_ptr = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
+    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * WG_BM;
+    const int num_kb = (K + WG_BK - 1) / WG_BK;
 
+    wg_init<BN, ST>(smem, &tmap_a, &tmap_b);
+    if (threadIdx.x >= WG_CONSUMERS) {
+        wg_produce<BN, ST>(smem, &tmap_a, &tmap_b, m0, n0, 0, num_kb);
+        return;
+    }
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t crank = cluster_ctarank();
-    const uint32_t rank = crank & 1u;        // rank inside the CTA pair
-    const uint32_t lead_rank = crank & ~1u;  // cluster rank of this pair's leader
-    const bool leader = rank == 0;
-    const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-    const int n_tiles = (N + BN - 1) / BN, m_tiles = (M + 2 * G2_BM - 1) / (2 * G2_BM);
-    const int total_tiles = n_tiles * m_tiles;
-    const int num_kb = (K + G2_BK - 1) / G2_BK;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_a);
-        tma_prefetch_desc(&tmap_b);
-        for (int s = 0; s < ST; ++s) {
-            mbar_init(&full_bar[s], 2);   // leader's expect_tx arrive + the peer's remote arrive
-            mbar_init(&empty_bar[s], mc ? 2 : 1);  // multicast tcgen05.commit (A-multicast: of both pairs of the cluster)
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full_bar[i], 1);   // multicast tcgen05.commit
-            mbar_init(&tmem_empty_bar[i], 2);  // one elected epilogue thread per CTA
-        }
-        mbar_fence_init();
-    }
-    cluster_sync_all();  // both CTAs' barriers exist before any remote arrive / multicast
-    if (warp == 1) tmem_alloc_2sm(tmem_base_ptr, 512);
-    tc_fence_before();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_ptr;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int it = 0;  // running k-block counter across tiles (ring position)
-            for (int tile = pair; tile < total_tiles; tile += num_pairs) {
-                const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-                const int m_row = mt * 2 * G2_BM + static_cast<int>(rank) * G2_BM;
-                const int n_row = nt * BN + static_cast<int>(rank) * (BN / 2);
-                for (int kb = 0; kb < num_kb; ++kb, ++it) {
-                    const int s = it % ST;
-                    const uint32_t ph = (it / ST) & 1;
-                    mbar_wait_b(&empty_bar[s], ph ^ 1, 1);
-                    uint8_t* a_dst = smem + s * C::STAGE_BYTES;
-                    if (mc) {  // this CTA fetches half of its 128 A rows and multicasts them to its twin in the other pair
-                        const int half = static_cast<int>(crank >> 1);
-                        tma_load_2d_2sm_mc(a_dst + half * (G2_A_BYTES / 2), &tmap_a64, &full_bar[s], kb * G2_BK,
-                                           m_row + half * (G2_BM / 2), static_cast<uint16_t>((1u << crank) | (1u << (crank ^ 2u))));
-                    } else {
-                        tma_load_2d_2sm(a_dst, &tmap_a, &full_bar[s], kb * G2_BK, m_row);
-                    }
-                    tma_load_2d_2sm(a_dst + G2_A_BYTES, &tmap_b, &full_bar[s], kb * G2_BK, n_row);
-                    if (leader) mbar_arrive_expect_tx(&full_bar[s], 2 * C::STAGE_BYTES);
-                    else mbar_arrive_remote(&full_bar[s], lead_rank);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (leader && lane == 0) {
-            const uint32_t idesc = make_idesc_f16(2 * G2_BM, BN, 0);
-            int it = 0, local_tile = 0;
-            for (int tile = pair; tile < total_tiles; tile += num_pairs, ++local_tile) {
-                const int buf = local_tile & 1;
-                const uint32_t acc_ph = (local_tile >> 1) & 1;
-                mbar_wait_b(&tmem_empty_bar[buf], acc_ph ^ 1, 2);  // epilogues of both CTAs drained this buffer
-                tc_fence_after();
-                const uint32_t d_addr = tmem_base + buf * BN;
-                for (int kb = 0; kb < num_kb; ++kb, ++it) {
-                    const int s = it % ST;
-                    const uint32_t ph = (it / ST) & 1;
-                    mbar_wait_b(&full_bar[s], ph, 3);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + s * C::STAGE_BYTES);
-                    const uint64_t da = make_kmajor_sw128_desc(a_addr);
-                    const uint64_t db = make_kmajor_sw128_desc(a_addr + G2_A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < G2_BK / 16; ++k)
-                        umma_f16_2sm(d_addr, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                    if (mc) umma_commit_mask(&empty_bar[s], 0xF);  // the twin pair's producers write into this stage too
-                    else umma_commit_2sm(&empty_bar[s], lead_rank);  // frees this stage in both CTAs
-                }
-                umma_commit_2sm(&tmem_full_bar[buf], lead_rank);  // accumulators ready in both CTAs
-            }
-        }
-    } else {
-        const int q = warp & 3;             // TMEM lane quarter this warp may access
-        constexpr int PARTS = EW / 4, PART_COLS = BN / PARTS, PITCH = epi_stg_pitch<MODE>();
-        const int part = (warp - 2) >> 2;   // which slice of the tile's columns this warp drains
-        constexpr int CHUNKS = PART_COLS / 32;
-        static_assert(CHUNKS % 2 == 0, "epilogue double buffer needs an even chunk count");
-        uint8_t* stg = smem + C::STG_OFFSET + (warp - 2) * 32 * PITCH;
-        int local_tile = 0;
-        for (int tile = pair; tile < total_tiles; tile += num_pairs, ++local_tile) {
-            const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-            const int buf = local_tile & 1;
-            const uint32_t acc_ph = (local_tile >> 1) & 1;
-            const int row_base = mt * 2 * G2_BM + static_cast<int>(rank) * G2_BM + q * 32;
-            const int n0 = nt * BN + part * PART_COLS;
-            // residual operands are fetched TWO chunks ahead (two register sets): one chunk of work (~0.3 us) does not cover
-            // an L2 / HBM round trip, and with one tile per pair (N = 512) nothing else hides it
-            // the tile's bias vector -> shared memory, before the wait for the accumulators (read per chunk from global memory
-            // it was a dependent L2 / HBM round trip in every chunk: ~20 % of the epilogue warps' samples in ncu)
-            constexpr int BIAS_OFF = C::STG_OFFSET + EW * 32 * PITCH;   // = g2_bias_offset<MODE, EW, BN, ST>()
-            float* sbias_tile = reinterpret_cast<float*>(smem + BIAS_OFF);
-            {
-                const int e_tid = (warp - 2) * 32 + lane;
-                for (int j = e_tid; j < BN; j += 32 * EW) sbias_tile[j] = epi.bias ? __ldg(epi.bias + nt * BN + j) : 0.0f;
-                asm volatile("bar.sync 2, %0;" ::"n"(32 * EW) : "memory");
-            }
-            const float* sb = sbias_tile + part * PART_COLS;
-            float4 res[2][8];
-            float4 rcs[4], rsn[4];
-            if constexpr (MODE == EPI_RESID) {
-                epilogue_resid_prefetch(epi, res[0], row_base, n0, M, lane);
-                epilogue_resid_prefetch(epi, res[1], row_base, n0 + 32, M, lane);
-            }
-            if constexpr (MODE == EPI_ROPE) epilogue_rope_prefetch(epi, rcs, rsn, row_base, n0, lane);
-            mbar_wait_b(&tmem_full_bar[buf], acc_ph, 4);
-            tc_fence_after();
-            const uint32_t t0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * BN + part * PART_COLS;
-            if constexpr (MODE == EPI_RESID) {
-                // one accumulator buffer (a TMEM read is short next to the residual's memory round trip; the registers go to
-                // the second residual set instead)
-                uint32_t acc1[32];
+    const int rg = warp & 3;                 // rows rg * 32 .. + 31 of the tile
+    constexpr int PART_COLS = BN / 2, CHUNKS = PART_COLS / 32;
+    const int c0 = (warp >> 2) * PART_COLS;  // this warp's half of the columns
+    const int row_base = m0 + rg * 32;
+    // the tile's bias vector -> shared memory (read by every lane of every chunk: a broadcast instead of an L2 round trip);
+    // visible after the consumer barriers of the main loop
+    float* sbias = reinterpret_cast<float*>(smem + g2_bias_offset<BN, ST>());
+    for (int j = threadIdx.x; j < BN; j += WG_CONSUMERS) sbias[j] = epi.bias ? __ldg(epi.bias + n0 + j) : 0.0f;
+    // residual / RoPE-table operands of the first chunk are fetched before the main loop, so their memory round trip
+    // overlaps it; each chunk then fetches the next one's ahead of its own math
+    float4 res[8];
+    float4 rcs[4], rsn[4];
+    if constexpr (MODE == EPI_RESID) epilogue_resid_prefetch(epi, res, row_base, n0 + c0, M, lane);
+    if constexpr (MODE == EPI_ROPE) epilogue_rope_prefetch(epi, rcs, rsn, row_base, n0 + c0, lane);
+    wg_consume_and_stage<BN, ST>(smem, num_kb);
+    uint8_t* stg = smem + rg * 32 * R::STG_PITCH + c0 * 4;
 #pragma unroll 1
-                for (int c = 0; c < CHUNKS; c += 2) {
-                    tmem_ld_32x32(t0 + c * 32, acc1);
-                    tmem_ld_wait();
-                    epilogue_chunk_coalesced<MODE, ACT, PITCH>(epi, acc1, stg, row_base, n0 + c * 32, M, lane, res[0],
-                                                               c + 2 < CHUNKS ? n0 + (c + 2) * 32 : -1, rcs, rsn, sb + c * 32);
-                    tmem_ld_32x32(t0 + (c + 1) * 32, acc1);
-                    tmem_ld_wait();
-                    epilogue_chunk_coalesced<MODE, ACT, PITCH>(epi, acc1, stg, row_base, n0 + (c + 1) * 32, M, lane, res[1],
-                                                               c + 3 < CHUNKS ? n0 + (c + 3) * 32 : -1, rcs, rsn, sb + (c + 1) * 32);
-                }
-            } else {
-                uint32_t acc[2][32];
-                tmem_ld_32x32(t0, acc[0]);
-#pragma unroll 1
-                for (int c = 0; c < CHUNKS; c += 2) {  // two chunks per iteration keep the double buffers statically indexed
-                    tmem_ld_wait();
-                    tmem_ld_32x32(t0 + (c + 1) * 32, acc[1]);  // next chunk in flight
-                    epilogue_chunk_coalesced<MODE, ACT, PITCH>(epi, acc[0], stg, row_base, n0 + c * 32, M, lane, res[0],
-                                                               n0 + (c + 1) * 32, rcs, rsn, sb + c * 32);
-                    tmem_ld_wait();
-                    if (c + 2 < CHUNKS) tmem_ld_32x32(t0 + (c + 2) * 32, acc[0]);
-                    epilogue_chunk_coalesced<MODE, ACT, PITCH>(epi, acc[1], stg, row_base, n0 + (c + 1) * 32, M, lane, res[0],
-                                                               c + 2 < CHUNKS ? n0 + (c + 2) * 32 : -1, rcs, rsn, sb + (c + 1) * 32);
-                }
-            }
-            tc_fence_before();
-            asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");  // all epilogue warps are done with `buf`
-            if (warp == 2 && lane == 0) {
-                if (leader) mbar_arrive(&tmem_empty_bar[buf]);
-                else mbar_arrive_remote(&tmem_empty_bar[buf], lead_rank);
-            }
-        }
+    for (int c = 0; c < CHUNKS; ++c) {
+        uint32_t acc[32];
+        wg_load_row32(smem_u32(stg + lane * R::STG_PITCH + c * 128), acc);
+        epilogue_chunk_coalesced<MODE, ACT, R::STG_PITCH>(epi, acc, stg + c * 128, row_base, n0 + c0 + c * 32, M, lane, res,
+                                                          c + 1 < CHUNKS ? n0 + c0 + (c + 1) * 32 : -1, rcs, rsn,
+                                                          sbias + c0 + c * 32);
     }
-    tc_fence_before();
-    cluster_sync_all();
-    if (warp == 1) tmem_dealloc_2sm(tmem_base, 512);
 }
 
-int gemm_f16_2cta(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
+int gemm_f16_wide(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
                   cudaStream_t stream) {
     CUtensorMap ta, tb;
-    int rc = make_tmap_2d_f16(&ta, A, M, K, lda, G2_BM, G2_BK);
+    int rc = make_tmap_2d_f16(&ta, A, M, K, lda, WG_BM, WG_BK);
     if (rc) return rc;
-    // optional 256 x 128 tiles with a 7-stage ring for the fp32-output modes (N = 512 GEMMs: two rounds of tiles so the
-    // epilogue of the first overlaps the main loop of the second).  Measured: parity-green but 4 % slower end to end
-    // (5.28 vs 5.07 ms per batch) -> opt-in only.
+    // optional 128 x 128 tiles with a 4-stage ring for the fp32-output modes (N = 512 GEMMs: twice the CTAs) -> opt-in
     static const bool bn128_env = getenv("SBK_GEMM_BN128") != nullptr;
     const bool bn128 = bn128_env && (epi.mode == EPI_RESID || epi.mode == EPI_F32) && N % 128 == 0 && N <= 1024;
     const int bn = bn128 ? 128 : G2_BN;
-    rc = make_tmap_2d_f16(&tb, W, N, K, ldw, bn / 2, G2_BK);
+    rc = make_tmap_2d_f16(&tb, W, N, K, ldw, bn, WG_BK);
     if (rc) return rc;
-    void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmEpilogue, int, int, int, int) = nullptr;
-    int smem = 0, threads = 0;
+    void (*kern)(const CUtensorMap, const CUtensorMap, const GemmEpilogue, int, int, int) = nullptr;
+    int smem = 0;
 #define G2_PICK(MODE, ACT)                                                        \
     do {                                                                          \
-        constexpr int EW = g2_epi_warps<MODE>();                                  \
-        kern = gemm_tc2_kernel<MODE, ACT, EW>;                                    \
-        smem = g2_smem<MODE, EW, G2_BN, G2_STAGES>();                             \
-        threads = 64 + 32 * EW;                                                   \
+        kern = gemm_tc2_kernel<MODE, ACT>;                                        \
+        smem = g2_smem<G2_BN, G2_STAGES>();                                       \
     } while (0)
 #define G2_PICK_BN128(MODE)                                                       \
     do {                                                                          \
-        kern = gemm_tc2_kernel<MODE, ACT_NONE, 8, 128, 7>;                        \
-        smem = g2_smem<MODE, 8, 128, 7>();                                        \
-        threads = 64 + 32 * 8;                                                    \
+        kern = gemm_tc2_kernel<MODE, ACT_NONE, 128, 4>;                           \
+        smem = g2_smem<128, 4>();                                                 \
     } while (0)
     // SiLU / GLU-gate sigmoid through one tanh.approx MUFU per element (default) or the exact-form EX2 + RCP (SBK_SILU_EXACT=1)
     static const bool fast_act = getenv("SBK_SILU_EXACT") == nullptr;
@@ -336,7 +97,7 @@ int gemm_f16_2cta(const void* A, int lda, const void* W, int ldw, const GemmEpil
             else if (epi.act == ACT_SILU) G2_PICK(EPI_F16, ACT_SILU);
             else if (epi.act == ACT_GELU) G2_PICK(EPI_F16, ACT_GELU);
             else if (epi.act == ACT_NONE) G2_PICK(EPI_F16, ACT_NONE);
-            else { set_error("gemm_f16_2cta: activation %d not built", epi.act); return SBK_ERR_ARG; }
+            else { set_error("gemm_f16_wide: activation %d not built", epi.act); return SBK_ERR_ARG; }
             break;
         case EPI_F32:
             if (bn128) G2_PICK_BN128(EPI_F32);
@@ -351,56 +112,11 @@ int gemm_f16_2cta(const void* A, int lda, const void* W, int ldw, const GemmEpil
             else G2_PICK(EPI_GLU, ACT_NONE);
             break;
         case EPI_ROPE: G2_PICK(EPI_ROPE, ACT_NONE); break;
-        default: set_error("gemm_f16_2cta: bad epilogue mode %d", epi.mode); return SBK_ERR_ARG;
+        default: set_error("gemm_f16_wide: bad epilogue mode %d", epi.mode); return SBK_ERR_ARG;
     }
 #undef G2_PICK
 #undef G2_PICK_BN128
     SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    static int num_sms = 0;
-    if (num_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    const int n_tiles = ceil_div(N, bn), m_tiles = ceil_div(M, 2 * G2_BM);
-    // CTA pairs: no more than needed for the wave count the full machine would give (256 tiles: 4 rounds on 64 pairs as on 74;
-    // 96 tiles: 2 rounds on 48) -- the kernel takes the same time, and the SMs it leaves alone run other lanes' decode-step
-    // kernels, which cannot share an SM with a 200 KB GEMM CTA.  SBK_GEMM_PAIRS=n caps the pair count instead (74 = round-1 rule).
-    static const int pairs_env = getenv("SBK_GEMM_PAIRS") ? atoi(getenv("SBK_GEMM_PAIRS")) : 0;
-    const int max_pairs = num_sms / 2, tiles = n_tiles * m_tiles;
-    int pairs = std::min(max_pairs, tiles);
-    if (pairs_env > 0) pairs = std::min(pairs, pairs_env);
-    else pairs = ceil_div(tiles, ceil_div(tiles, max_pairs));
-    // SBK_GEMM_CL4=1: clusters of two pairs (needs an even tile count per row of tiles and an even pair count)
-    // SBK_GEMM_MC=1 (implies clusters of 4): the A tile is fetched once per cluster, each CTA multicasting half of its rows
-    static const bool mc_env = getenv("SBK_GEMM_MC") != nullptr;
-    static const bool cl4_env = getenv("SBK_GEMM_CL4") != nullptr || mc_env;
-    int cluster = 2, mc = 0;
-    CUtensorMap ta64 = ta;
-    if (cl4_env && n_tiles % 2 == 0 && pairs >= 2) {
-        if (mc_env) {
-            mc = 1;
-            rc = make_tmap_2d_f16(&ta64, A, M, K, lda, G2_BM / 2, G2_BK);
-            if (rc) return rc;
-        }
-        cluster = 4;
-        pairs &= ~1;
-        static int max_cl4[64] = {0};  // resident clusters of 4 the device can hold for this kernel / shared-memory size
-        int& cap = max_cl4[(epi.mode * 8 + epi.act) & 63];
-        if (cap == 0) {
-            cudaLaunchConfig_t q = {};
-            q.gridDim = dim3(num_sms / 4 * 4); q.blockDim = dim3(threads); q.dynamicSmemBytes = smem;
-            cudaLaunchAttribute qa[1];
-            qa[0].id = cudaLaunchAttributeClusterDimension;
-            qa[0].val.clusterDim.x = 4; qa[0].val.clusterDim.y = 1; qa[0].val.clusterDim.z = 1;
-            q.attrs = qa; q.numAttrs = 1;
-            int nc = 0;
-            if (cudaOccupancyMaxActiveClusters(&nc, reinterpret_cast<const void*>(kern), &q) != cudaSuccess || nc < 1) nc = 1;
-            cap = nc;
-            if (getenv("SBK_GEMM_TRACE")) fprintf(stderr, "gemm2: %d resident clusters of 4 for mode %d\n", nc, epi.mode);
-        }
-        pairs = std::min(pairs, 2 * cap);
-    }
     GemmProfile* prof = gemm_profile();
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (prof->enabled) {
@@ -408,15 +124,7 @@ int gemm_f16_2cta(const void* A, int lda, const void* W, int ldw, const GemmEpil
         cudaEventCreate(&e1);
         cudaEventRecord(e0, stream);
     }
-    {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        SBK_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ta, tb, ta64, epi, M, N, K, mc));
-    }
+    kern<<<dim3(N / bn, ceil_div(M, WG_BM)), WG_THREADS, smem, stream>>>(ta, tb, epi, M, N, K);
     if (prof->enabled) {
         cudaEventRecord(e1, stream);
         prof->ev.push_back(e0);

@@ -27,20 +27,20 @@ struct GemmEpilogue {
     // EPI_QKV_CACHE (decoder self-attention in_proj, columns [q | k | v] of width qkv_d): q -> out (fp16, ldo), k / v ->
     // cache[(row * S_max + step_ptr[row]) * qkv_d + col]
     __half* kcache = nullptr; __half* vcache = nullptr; const int* step_ptr = nullptr; int S_max = 0; int qkv_d = 0;
-    // EPI_F16 (2-CTA kernel) scatter of the cross-attention [K | V] projection (N = 2 * kv_heads * 64, row = utt * T + t) to
+    // EPI_F16 (wide-tile kernel) scatter of the cross-attention [K | V] projection (N = 2 * kv_heads * 64, row = utt * T + t) to
     // part[K|V][utt][head][t][64]; kv_part_stride = elements between the K part and the V part.  0 = plain row-major store.
     int kv_heads = 0; size_t kv_part_stride = 0;
 };
 
-// out = epilogue(A[M,K] fp16 x W[N,K]^T fp16), tcgen05 tensor cores. gemm_tc.cu
+// out = epilogue(A[M,K] fp16 x W[N,K]^T fp16), wgmma tensor cores. gemm_tc.cu
 int gemm_f16(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
              cudaStream_t stream);
 // Small-M variant for the decode steps of several batches (M = live hypotheses, 64..512): 128 x 32/64 tiles, deep TMA
 // ring; any epilogue mode incl. EPI_QKV_CACHE. gemm_tc.cu
 int gemm_f16_small(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
                    cudaStream_t stream);
-// 2-CTA (cta_group::2) persistent variant, N % 256 == 0. gemm_tc2.cu
-int gemm_f16_2cta(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
+// 128 x 256 tile variant with the coalesced epilogue, N % 256 == 0. gemm_tc2.cu
+int gemm_f16_wide(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
                   cudaStream_t stream);
 
 
@@ -50,7 +50,7 @@ long long launch_count_end_capture();
 void launch_count_add(long long n);
 long long launch_count();
 
-// Optional live timing of every tcgen05 GEMM launch (CUDA events on the launching stream).
+// Optional live timing of every wgmma GEMM launch (CUDA events on the launching stream).
 struct GemmProfile {
     bool enabled = false;
     std::vector<cudaEvent_t> ev;   // start/stop pairs

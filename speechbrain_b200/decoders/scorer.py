@@ -1,4 +1,4 @@
-"""Scorer interfaces of the beam search -- mirrors of speechbrain.decoders.scorer for what is built on the B200 path:
+"""Scorer interfaces of the beam search -- mirrors of speechbrain.decoders.scorer for what is built on the H100 path:
 ``TransformerLMScorer`` (scorer.py:455-560) and ``CTCScorer`` (scorer.py:81-249, CTCPrefixScore decoders/ctc.py:46-295)
 as *full* scorers of a ``ScorerBuilder`` (scorer.py:1075-1341), i.e. the recipe's ``scorer_test_search`` /
 ``scorer_valid_search`` (conformer_large.yaml:209-228), plus ``CoverageScorer`` (:788-955) and ``LengthScorer`` (:956-1072).

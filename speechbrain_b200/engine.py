@@ -155,7 +155,7 @@ class AsrEngine:
         return scores
 
     def set_decoder_tc_min_rows(self, rows):
-        """Decode steps with >= rows live hypotheses use the tcgen05 GEMM for the decoder projections (default 64)."""
+        """Decode steps with >= rows live hypotheses use the wgmma GEMM for the decoder projections (default 64)."""
         check(lib().sbk_asr_set_decoder_tc_min_rows(self._h, int(rows)), "sbk_asr_set_decoder_tc_min_rows")
 
     def set_decoder_ln_fusion(self, on):

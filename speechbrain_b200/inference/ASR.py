@@ -54,7 +54,7 @@ class EncoderDecoderASR(torch.nn.Module):
         self.tokenizer = self.hparams.get("tokenizer")
         self.transformer_beam_search = bool(self.hparams.get("transformer_beam_search", False))
         if self.hparams.get("transducer_beam_search", False):
-            raise NotImplementedError("speechbrain_b200.EncoderDecoderASR: transducer decoding is not on the B200 hot path")
+            raise NotImplementedError("speechbrain_b200.EncoderDecoderASR: transducer decoding is not on the H100 hot path")
         self.device = torch.device((run_opts or {}).get("device", "cuda:0"))
         dec = self.mods["decoder"]
         if not isinstance(dec, (S2STransformerGreedySearcher, S2STransformerBeamSearcher)):

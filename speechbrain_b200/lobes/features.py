@@ -1,4 +1,4 @@
-"""Fbank -- drop-in for speechbrain.lobes.features.Fbank (lobes/features.py:22-173) on the sm_100a kernel.
+"""Fbank -- drop-in for speechbrain.lobes.features.Fbank (lobes/features.py:22-173) on the sm_90a kernel.
 
 Same constructor, ``forward(wav) -> [B, T_f, n_mels]`` and ``state_dict`` keys ({"compute_deltas.kernel"}).
 Built natively: frozen triangular filters, no deltas, no context, mono [B, L] input -- i.e. what every ASR
@@ -25,7 +25,7 @@ class Fbank(torch.nn.Module):
                  left_frames=5, right_frames=5, win_length=25, hop_length=10):
         super().__init__()
         if deltas or context:
-            raise NotImplementedError("speechbrain_b200.Fbank: deltas/context are not on the B200 hot path")
+            raise NotImplementedError("speechbrain_b200.Fbank: deltas/context are not on the H100 hot path")
         if requires_grad:
             raise NotImplementedError("speechbrain_b200.Fbank: learnable filters are not supported (inference only)")
         if filter_shape != "triangular":

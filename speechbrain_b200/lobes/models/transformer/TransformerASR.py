@@ -2,7 +2,7 @@
 (TransformerASR.py:167-675) restricted to what the Conformer ASR recipes instantiate:
 encoder_module="conformer", attention_type in {"RoPEMHA", "RelPosMHAXL"}, normalize_before=True, causal=False.
 
-Same constructor kwargs, same state_dict keys (incl. the positional buffers), ``encode()`` on the sm_100a
+Same constructor kwargs, same state_dict keys (incl. the positional buffers), ``encode()`` on the sm_90a
 kernels.  ``decode()`` / ``forward()`` run teacher-forced on the KV-cached decoder step (the searchers in
 speechbrain_b200.decoders drive the same step one token at a time).
 """

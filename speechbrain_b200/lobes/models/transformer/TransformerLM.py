@@ -1,5 +1,5 @@
 """TransformerLM -- parameter container mirroring speechbrain.lobes.models.transformer.TransformerLM.TransformerLM
-(TransformerLM.py:22-187) for its use as a shallow-fusion scorer inside the B200 beam search: same constructor kwargs and
+(TransformerLM.py:22-187) for its use as a shallow-fusion scorer inside the H100 beam search: same constructor kwargs and
 state_dict keys (so ``lm.ckpt`` loads unchanged); the forward pass runs inside the engine with a KV cache
 (csrc/engine.cu enqueue_lm_step), so calling the module directly is not part of the hot path."""
 import torch

@@ -1,5 +1,5 @@
 """Linear -- drop-in for speechbrain.nnet.linear.Linear (nnet/linear.py:16-91): keys ``w.weight`` / ``w.bias``.
-On CUDA the product runs on the tcgen05 GEMM (fp16 operands, fp32 accumulate)."""
+On CUDA the product runs on the wgmma GEMM (fp16 operands, fp32 accumulate)."""
 import torch
 
 from .._lib import check, lib, ptr, require_cuda, stream_ptr

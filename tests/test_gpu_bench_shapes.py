@@ -85,7 +85,7 @@ def test_bench_shape_encoder_and_greedy(dev, tag):
     assert abs(chk - g["weight_checksum"]) / g["weight_checksum"] < 1e-9, "seeded weights differ from the golden run"
     wav, lens = _inputs(g)
     S = g["greedy_tokens"].shape[1]
-    for tc_rows, name in ((1 << 30, "weight-streaming"), (1, "tcgen05")):
+    for tc_rows, name in ((1 << 30, "weight-streaming"), (1, "wgmma")):
         eng.set_decoder_tc_min_rows(tc_rows)
         pred, score, enc, done = eng.transcribe_greedy_dev(wav.to(dev), lens.to(dev), S, 1, 2, want_enc=True)
         torch.cuda.synchronize()
@@ -179,12 +179,12 @@ def _check_beam(dev, g, gb, case):
     enc, lens = g["enc_out"].to(dev), g["wav_lens"].to(dev)
     hyps, hlens, scores, lp = bs(enc, lens)
     if gb["with_lm"] or case.endswith("eos16"):
-        # the same search with every projection (decoder AND TransformerLM step) on the tcgen05 GEMM instead of the
+        # the same search with every projection (decoder AND TransformerLM step) on the wgmma GEMM instead of the
         # weight-streaming kernel (what wide beams / many utterances use): same hypotheses, scores within 2e-3
         bs._get_engine(dev).set_decoder_tc_min_rows(1)
         h2, l2, s2, _ = bs(enc, lens)
         bs._get_engine(dev).set_decoder_tc_min_rows(64)
-        print(f"beam[{case}] tcgen05 projections: best scores {s2[:, 0].tolist()}")
+        print(f"beam[{case}] wgmma GEMM projections: best scores {s2[:, 0].tolist()}")
         assert (s2[:, 0].cpu() - scores[:, 0].cpu()).abs().max() < 2e-3
     hyps, hlens, scores = hyps.cpu(), hlens.cpu(), scores.cpu()
     B, L = hyps.shape[0], hyps.shape[2]

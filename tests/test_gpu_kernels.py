@@ -21,7 +21,7 @@ def dev():
     return torch.device("cuda:0")
 
 
-# ----------------------------------------------------------------------------------------- tcgen05 GEMM
+# ------------------------------------------------------------------------------------------- wgmma GEMM
 @pytest.mark.parametrize("M,N,K", [(128, 128, 64), (128, 128, 512), (200, 256, 512), (251, 5000, 512),
                                    (1000, 1536, 640), (8032, 2048, 512), (8032, 512, 2048), (300, 144, 144),
                                    (8032, 1536, 512), (8032, 1024, 512), (37, 512, 640), (20000, 256, 64)])
@@ -182,8 +182,8 @@ def test_model_stages_golden(dev, tag):
     top2 = g["greedy_logits"].topk(2, -1).values
     margin = top2[..., 0] - top2[..., 1]
     ref_tok = g["greedy_logits"].argmax(-1)
-    # both decode-step implementations: weight-streaming projections (default below 64 rows) and tcgen05 projections
-    for tc_rows, name in ((1 << 30, "skinny"), (1, "tcgen05")):
+    # both decode-step implementations: weight-streaming projections (default below 64 rows) and wgmma GEMM projections
+    for tc_rows, name in ((1 << 30, "skinny"), (1, "wgmma")):
         eng.set_decoder_tc_min_rows(tc_rows)
         pred, score, lp, done = eng.greedy_from_enc(g["enc_out"].to(dev), g["wav_lens"].to(dev), n_steps, 1, 2, want_log_probs=True)
         pred = pred.cpu()
@@ -236,7 +236,7 @@ def test_beam_search_golden(dev, case):
     lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
     bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, max_decode_ratio=gb["max_decode_ratio"],
                                     **gb["kwargs"])
-    for name, tc_rows in (("skinny", None), ("tcgen05", 1)):  # both decode-step projection implementations
+    for name, tc_rows in (("skinny", None), ("wgmma", 1)):  # both decode-step projection implementations
         if tc_rows is not None:
             bs._get_engine(dev).set_decoder_tc_min_rows(tc_rows)
         hyps, lens, scores, lp = bs(g["enc_out"].to(dev), g["wav_lens"].to(dev))
@@ -283,13 +283,13 @@ def test_full_size_properties(dev):
     eng.transcribe_greedy_group_dev([wav, wav_b], [ones, ones.clone()], steps, 1, 2, outs)
     torch.cuda.synchronize()
     assert torch.equal(outs[0], pred) and torch.equal(outs[1], pb)
-    # default: 64 live rows switch the projections to the tcgen05 GEMM (other summation order): ids may only differ after
+    # default: 64 live rows switch the projections to the wgmma GEMM (other summation order): ids may only differ after
     # a near-tie, so almost every utterance must still agree
     eng.set_decoder_tc_min_rows(64)
     eng.transcribe_greedy_group_dev([wav, wav_b], [ones, ones.clone()], steps, 1, 2, outs)
     torch.cuda.synchronize()
     same = sum(int(torch.equal(outs[0][i], pred[i])) + int(torch.equal(outs[1][i], pb[i])) for i in range(B))
-    print(f"coalesced decode (tcgen05 projections) vs separate (weight-streaming): {same}/{2 * B} utterances identical")
+    print(f"coalesced decode (wgmma GEMM projections) vs separate (weight-streaming): {same}/{2 * B} utterances identical")
     assert same >= int(0.9 * 2 * B)
     eng.set_decoder_tc_min_rows(1 << 30)
     # ragged: shortening utterance 5 must not change any other utterance

@@ -1,4 +1,4 @@
-"""Fixed cost vs per-k-block cost of the tcgen05 GEMM at the encoder's shapes: M = 8032 rows, N in {512, 2048}, K swept from one
+"""Fixed cost vs per-k-block cost of the wgmma GEMMs at the encoder's shapes: M = 8032 rows, N in {512, 2048}, K swept from one
 k-block (64) upward, fp16 / fp32 outputs.  Event-timed over back-to-back launches (after warm-up); prints one line per shape and
 a least-squares (intercept, slope per 64-wide k-block)."""
 import ctypes
@@ -41,10 +41,10 @@ for N in (512, 1024, 2048):
         sxx = sum(p[0] ** 2 for p in pts); sxy = sum(p[0] * p[1] for p in pts)
         slope = (n * sxy - sx * sy) / (n * sxx - sx * sx)
         icpt = (sy - slope * sx) / n
-        print(f"  -> N={N} out={'f32' if f32 else 'f16'}: fixed {icpt:.2f} us + {slope:.3f} us per k-block (tiles per pair: {((M + 255) // 256) * (N // 256) / 74:.2f})", flush=True)
+        print(f"  -> N={N} out={'f32' if f32 else 'f16'}: fixed {icpt:.2f} us + {slope:.3f} us per k-block (128 x 256 tiles per SM: {((M + 127) // 128) * (N // 256) / 132:.2f})", flush=True)
 
 # The encoder's own conditions for the N = 512 residual GEMMs: residual epilogue, operands not L2-hot (rotate over buffer sets
-# larger than the 126 MB L2), and one CUDA-event pair per launch (what bench.py's roofline pass does) vs pipelined launches.
+# larger than the 50 MB L2), and one CUDA-event pair per launch (what bench.py's roofline pass does) vs pipelined launches.
 print("--- residual epilogue (x += A W^T + b), M=%d N=512" % M, flush=True)
 for K in (512, 2048):
     for nset in (1, 12):
