@@ -97,6 +97,14 @@ int sbk_gemm_f16_test(const void* A_dev, const void* W_dev, const float* bias_de
 /* same kernel, residual epilogue (every Linear that closes a Conformer sub-block): x[M,N] += alpha * (A W^T + bias), fp32 in place */
 int sbk_gemm_f16_resid_test(const void* A_dev, const void* W_dev, const float* bias_dev, float* x_dev, float alpha,
                             int M, int N, int K, void* stream);
+/* any fused epilogue of the encoder GEMMs: mode 0 fp16 (act 0 none, 1 SiLU, 2 GELU; kv_heads > 0: cross-attention K/V
+ * scatter to [layer][K|V][utt][head][t][64] with the given element strides), 1 fp32, 2 residual (out = resid + alpha *
+ * (acc + bias), rows t >= row_lens[utt] get alpha 0; out may alias resid), 3 GLU (fp32 [M, N / 2]; weight rows
+ * interleaved [16 values | 16 gates] per 32), 4 RoPE (columns per head [q | k | v], q scaled by alpha; tables [T, dh / 2]) */
+int sbk_gemm_epilogue_test(const void* A_dev, const void* W_dev, const float* bias_dev, void* out_dev, int ldo, int mode,
+                           int act, float alpha, const float* resid_dev, const int* row_lens_dev, int T,
+                           const float* rope_cos_dev, const float* rope_sin_dev, int head_dim, int kv_heads,
+                           long long kv_part_stride, long long kv_layer_stride, int M, int N, int K, void* stream);
 
 /* ---- model handle: repacks the reference state_dict once */
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out);

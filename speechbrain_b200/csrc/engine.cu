@@ -724,10 +724,15 @@ static int project_cross_kv(AsrModel* m, int M, int T, cudaStream_t st) {
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, Ld = c.num_decoder_layers;
     RC(cast_f32_f16(b.enc_out, b.enc16, (size_t)M * d, st));
+    if (xatt_headmajor(m)) {  // w_ckv / b_ckv are [Ld * 2d] rows: every layer's K and V in ONE GEMM, scattered per layer
+        GemmEpilogue e;
+        e.mode = EPI_F16; e.bias = m->b_ckv; e.out = b.ckv16; e.ldo = Ld * 2 * d;
+        e.kv_heads = c.nhead; e.kv_part_stride = (size_t)M * d; e.kv_layer_stride = (size_t)M * 2 * d; e.T = T;
+        return gemm_f16(b.enc16, d, m->w_ckv, d, e, M, Ld * 2 * d, d, st);
+    }
     for (int l = 0; l < Ld; ++l) {
         GemmEpilogue e;
         e.mode = EPI_F16; e.bias = m->b_ckv + (size_t)l * 2 * d; e.out = b.ckv16 + (size_t)l * M * 2 * d; e.ldo = 2 * d;
-        if (xatt_headmajor(m)) { e.kv_heads = c.nhead; e.kv_part_stride = (size_t)M * d; e.T = T; }
         RC(gemm_f16(b.enc16, d, m->w_ckv + (size_t)l * 2 * d * d, d, e, M, 2 * d, d, st));
     }
     return SBK_OK;
@@ -1331,6 +1336,19 @@ int sbk_gemm_f16_resid_test(const void* A_dev, const void* W_dev, const float* b
     e.resid = x_dev;
     e.alpha = alpha;
     e.ldo = N;
+    return gemm_f16(A_dev, K, W_dev, K, e, M, N, K, static_cast<cudaStream_t>(stream));
+}
+
+int sbk_gemm_epilogue_test(const void* A_dev, const void* W_dev, const float* bias_dev, void* out_dev, int ldo, int mode,
+                           int act, float alpha, const float* resid_dev, const int* row_lens_dev, int T,
+                           const float* rope_cos_dev, const float* rope_sin_dev, int head_dim, int kv_heads,
+                           long long kv_part_stride, long long kv_layer_stride, int M, int N, int K, void* stream) {
+    GemmEpilogue e;
+    e.mode = mode; e.act = act; e.bias = bias_dev; e.out = out_dev; e.ldo = ldo; e.alpha = alpha;
+    e.resid = resid_dev; e.row_lens = row_lens_dev; e.T = T;
+    e.rope_cos = rope_cos_dev; e.rope_sin = rope_sin_dev; e.head_dim = head_dim;
+    e.kv_heads = kv_heads; e.kv_part_stride = (size_t)kv_part_stride; e.kv_layer_stride = (size_t)kv_layer_stride;
+    if (mode < EPI_F16 || mode > EPI_ROPE) { set_error("sbk_gemm_epilogue_test: mode %d", mode); return SBK_ERR_ARG; }
     return gemm_f16(A_dev, K, W_dev, K, e, M, N, K, static_cast<cudaStream_t>(stream));
 }
 

@@ -1,4 +1,4 @@
-// TMA + wgmma main loop shared by the GEMM kernels of gemm_tc.cu and gemm_tc2.cu:
+// TMA + wgmma main loop of the GEMM kernels of gemm_tc.cu:
 //
 //     acc = A[m0 .. m0 + 128, k-blocks] x W[n0 .. n0 + BN, k-blocks]^T    (fp16 operands, fp32 accumulate in registers)
 //

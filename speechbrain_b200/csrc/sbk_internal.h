@@ -27,9 +27,11 @@ struct GemmEpilogue {
     // EPI_QKV_CACHE (decoder self-attention in_proj, columns [q | k | v] of width qkv_d): q -> out (fp16, ldo), k / v ->
     // cache[(row * S_max + step_ptr[row]) * qkv_d + col]
     __half* kcache = nullptr; __half* vcache = nullptr; const int* step_ptr = nullptr; int S_max = 0; int qkv_d = 0;
-    // EPI_F16 (wide-tile kernel) scatter of the cross-attention [K | V] projection (N = 2 * kv_heads * 64, row = utt * T + t) to
-    // part[K|V][utt][head][t][64]; kv_part_stride = elements between the K part and the V part.  0 = plain row-major store.
-    int kv_heads = 0; size_t kv_part_stride = 0;
+    // EPI_F16 (wide-tile kernel) scatter of the cross-attention [K | V] projections of one or several decoder layers
+    // (N = layers * 2 * kv_heads * 64, row = utt * T + t) to layer[l][K|V][utt][head][t][64]; kv_part_stride = elements
+    // between the K part and the V part of a layer, kv_layer_stride = elements between layers.  kv_heads 0 = plain
+    // row-major store.
+    int kv_heads = 0; size_t kv_part_stride = 0; size_t kv_layer_stride = 0;
 };
 
 // out = epilogue(A[M,K] fp16 x W[N,K]^T fp16), wgmma tensor cores. gemm_tc.cu
