@@ -46,6 +46,37 @@ __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; 
 // SMs of the target GPU (H100 SXM): caps the grids of grid-stride kernels at a few waves
 constexpr int SBK_NUM_SMS = 132;
 
+// ---------------------------------------------------------------- programmatic dependent launch
+// A kernel launched by launch_pdl may start while its predecessor in the stream is still running; pdl_wait() blocks
+// until that predecessor has completed and its writes are visible (a no-op when the kernel was launched without the
+// attribute).  pdl_trigger() lets the successor start launching.  Rules for the code a kernel runs before pdl_wait(),
+// which may overlap not only the predecessor but, through its early trigger, kernels further back in the stream:
+//   * read only data no kernel of the decode loop writes (weights, biases, LayerNorm parameters, the cross-attention
+//     K/V ckv16, enc_len), and that data must come from kernels that never trigger early (project_cross_kv,
+//     abs_len_kernel);
+//   * write nothing to global memory: a predecessor that is still running could read the overwritten values;
+//   * never read step, dx, dh16, dq16, datt16, df16, the self-attention K/V caches, logits or tokens.
+// Every kernel launched this way executes pdl_wait() in at least one thread, so its completion implies its
+// predecessor's, and a chain of such kernels stays ordered.
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl,
+                              Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, kern, args...);
+}
+
 // ---------------------------------------------------------------- warp utils
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -25,28 +25,15 @@ __device__ __forceinline__ void mma16816_d(float (&d)[4], const uint32_t (&a)[4]
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// Programmatic dependent launch: every decode-step kernel lets its successor start launching immediately and
-// waits for its predecessor's memory only right before it touches activations, so launch latency and the
+// Programmatic dependent launch (common.cuh): every decode-step kernel lets its successor start launching immediately
+// and waits for its predecessor's memory only right before it touches activations, so launch latency and the
 // weight prefetch of kernel N+1 overlap the tail of kernel N.
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
 static bool g_use_pdl = true;
 void set_pdl(bool on) { g_use_pdl = on; }
 
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = g_use_pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kern, args...);
+    return launch_pdl(kern, grid, block, smem, st, g_use_pdl, args...);
 }
 
 // --------------------------------------------------------------------------- skinny GEMM (weight streaming)
@@ -306,8 +293,12 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
     // co-scheduled, so each DRAM page / L2 line set is consumed while it is open
     const int r = blockIdx.y, h = blockIdx.x;
     const int blk = r / a.rows_per_block;
+    // cross-attention reads only ckv16 and enc_len before pdl_wait() (see common.cuh): enc_len and the first chunk's K/V
+    // loads are issued before it.  Self-attention waits first: its keys are this step's cache writes and its length is
+    // the step counter.
+    const bool xatt = a.n_keys_ptr == nullptr && a.lineage == nullptr && a.tok_cache == nullptr;
     pdl_trigger();
-    pdl_wait();
+    if (!xatt) pdl_wait();
     int n_keys;
     if (a.n_keys_ptr) n_keys = *a.n_keys_ptr + 1;
     else n_keys = a.enc_len ? min(a.enc_len[blk], a.n_keys_fixed) : a.n_keys_fixed;
@@ -321,25 +312,10 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
     const int* lin = nullptr;
     if (a.lineage) lin = a.lineage + static_cast<size_t>((n_keys - 1) & 1) * gridDim.y * a.lin_stride + static_cast<size_t>(r) * a.lin_stride;
     const int* tokc = a.tok_cache;  // TransformerLM.make_masks: keys whose token id is pad_idx (0) are masked
-    // this lane's 8 dims of the query
-    float qf[8];
-    {
-        const uint4 qv = *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * 64 + dl);
-        const __half2* q2 = reinterpret_cast<const __half2*>(&qv);
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const float2 f = __half22float2(q2[u]);
-            qf[2 * u] = f.x; qf[2 * u + 1] = f.y;
-        }
-    }
-    float m_run = -INFINITY, l_run = 0.0f;
-    float o[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) o[e] = 0.0f;
-    for (int c0 = kb; c0 < ke; c0 += DA_CHUNK) {
-        // ---- issue every load of this chunk up front: 8 keys x (16 B of K + 16 B of V) per lane
-        uint4 kv[DA_KPG], vv[DA_KPG];
-        bool live[DA_KPG];
+    // every load of the chunk at c0: 8 keys x (16 B of K + 16 B of V) per lane
+    uint4 kv[DA_KPG], vv[DA_KPG];
+    bool live[DA_KPG];
+    auto load_chunk = [&](int c0) {
 #pragma unroll
         for (int i = 0; i < DA_KPG; ++i) {
             const int j = c0 + gq + 4 * i;
@@ -356,6 +332,28 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
                 vv[i] = make_uint4(0u, 0u, 0u, 0u);
             }
         }
+    };
+    if (xatt) {
+        load_chunk(kb);
+        pdl_wait();
+    }
+    // this lane's 8 dims of the query
+    float qf[8];
+    {
+        const uint4 qv = *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * 64 + dl);
+        const __half2* q2 = reinterpret_cast<const __half2*>(&qv);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const float2 f = __half22float2(q2[u]);
+            qf[2 * u] = f.x; qf[2 * u + 1] = f.y;
+        }
+    }
+    float m_run = -INFINITY, l_run = 0.0f;
+    float o[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) o[e] = 0.0f;
+    for (int c0 = kb; c0 < ke; c0 += DA_CHUNK) {
+        if (!xatt || c0 != kb) load_chunk(c0);  // issue every load of this chunk up front
         // ---- scores: 8-dim partial dot per lane, summed over the 8 lanes of the key's group
         float sc[DA_KPG];
         float cm = -INFINITY;

@@ -13,19 +13,33 @@ namespace sbk {
 
 // --------------------------------------------------------------------------- LayerNorm
 // One warp per row, two-pass statistics in registers. D <= 32 * LN_MAX_PER_LANE.
+// PDL (decode step, launched with programmatic stream serialisation): gamma / beta are fetched before pdl_wait(), x after.
 constexpr int LN_MAX_PER_LANE = 32;
 
-template <bool OUT_HALF>
+template <bool OUT_HALF, bool PDL>
 __global__ void __launch_bounds__(256)
 layernorm_rows_kernel(const float* __restrict__ x, void* __restrict__ out, const float* __restrict__ gamma,
                       const float* __restrict__ beta, int M, int D, float eps, int act_silu) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (row >= M) return;
     const int lane = threadIdx.x & 31;
+    const int nv = D >> 2;  // float4 vectors per row (D % 4 == 0)
+    float4 gp[PDL ? LN_MAX_PER_LANE / 4 : 1], bp[PDL ? LN_MAX_PER_LANE / 4 : 1];
+    if constexpr (PDL) {
+#pragma unroll
+        for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
+            const int vi = lane + i * 32;
+            if (vi < nv && row < M) {
+                gp[i] = __ldg(reinterpret_cast<const float4*>(gamma + vi * 4));
+                bp[i] = __ldg(reinterpret_cast<const float4*>(beta + vi * 4));
+            }
+        }
+        pdl_trigger();
+        pdl_wait();
+    }
+    if (row >= M) return;
     const float* xr = x + static_cast<size_t>(row) * D;
     float v[LN_MAX_PER_LANE];
     float s = 0.0f;
-    const int nv = D >> 2;  // float4 vectors per row (D % 4 == 0)
 #pragma unroll
     for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
         const int vi = lane + i * 32;
@@ -55,8 +69,8 @@ layernorm_rows_kernel(const float* __restrict__ x, void* __restrict__ out, const
     for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
         const int vi = lane + i * 32;
         if (vi < nv) {
-            const float4 g = __ldg(reinterpret_cast<const float4*>(gamma + vi * 4));
-            const float4 b = __ldg(reinterpret_cast<const float4*>(beta + vi * 4));
+            const float4 g = PDL ? gp[PDL ? i : 0] : __ldg(reinterpret_cast<const float4*>(gamma + vi * 4));
+            const float4 b = PDL ? bp[PDL ? i : 0] : __ldg(reinterpret_cast<const float4*>(beta + vi * 4));
             float y0 = (v[4 * i] - mean) * rstd * g.x + b.x;
             float y1 = (v[4 * i + 1] - mean) * rstd * g.y + b.y;
             float y2 = (v[4 * i + 2] - mean) * rstd * g.z + b.z;
@@ -77,16 +91,20 @@ layernorm_rows_kernel(const float* __restrict__ x, void* __restrict__ out, const
 }
 
 int layernorm_rows(const float* x, void* out, bool out_half, const float* gamma, const float* beta, int M, int D,
-                   float eps, bool act_silu, cudaStream_t stream) {
+                   float eps, bool act_silu, cudaStream_t stream, bool pdl) {
     SBK_REQUIRE(D % 4 == 0 && D <= 32 * LN_MAX_PER_LANE, "layernorm_rows: D=%d unsupported", D);
     if (M == 0) return SBK_OK;
     const int rows_per_cta = 8;
-    if (out_half)
-        layernorm_rows_kernel<true><<<ceil_div(M, rows_per_cta), rows_per_cta * 32, 0, stream>>>(x, out, gamma, beta, M, D,
-                                                                                              eps, act_silu);
-    else
-        layernorm_rows_kernel<false><<<ceil_div(M, rows_per_cta), rows_per_cta * 32, 0, stream>>>(x, out, gamma, beta, M,
-                                                                                               D, eps, act_silu);
+    const dim3 grid(ceil_div(M, rows_per_cta)), block(rows_per_cta * 32);
+    if (pdl) {
+        SBK_REQUIRE(out_half, "layernorm_rows: the PDL variant writes fp16");
+        SBK_CUDA_CHECK(launch_pdl(layernorm_rows_kernel<true, true>, grid, block, 0, stream, true, x, out, gamma, beta, M, D,
+                                  eps, static_cast<int>(act_silu)));
+    } else if (out_half) {
+        layernorm_rows_kernel<true, false><<<grid, block, 0, stream>>>(x, out, gamma, beta, M, D, eps, act_silu);
+    } else {
+        layernorm_rows_kernel<false, false><<<grid, block, 0, stream>>>(x, out, gamma, beta, M, D, eps, act_silu);
+    }
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }

@@ -759,7 +759,7 @@ static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int
         const DecLayerW& w = m->dec[l];
         __half* kc = b.kcache + (size_t)l * rows * S_max * d;
         __half* vc = b.vcache + (size_t)l * rows * S_max * d;
-        RC(layernorm_rows(b.dx, b.dh16, true, w.n1g, w.n1b, rows, d, 1e-6f, false, st));
+        RC(layernorm_rows(b.dx, b.dh16, true, w.n1g, w.n1b, rows, d, 1e-6f, false, st, true));
         GemmEpilogue e;
         e.mode = EPI_QKV_CACHE; e.bias = w.b_self_in; e.out = b.dq16; e.ldo = d; e.kcache = kc; e.vcache = vc;
         e.step_ptr = b.step; e.S_max = S_max; e.qkv_d = d;
@@ -771,7 +771,7 @@ static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int
         RC(dec_attention(t, rows, S_max, st));
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_self_out; e.out = b.dx; e.resid = b.dx; e.ldo = d;
         RC(gemm_f16_small(b.datt16, d, w.w_self_out, d, e, rows, d, d, st));
-        RC(layernorm_rows(b.dx, b.dh16, true, w.n2g, w.n2b, rows, d, 1e-6f, false, st));
+        RC(layernorm_rows(b.dx, b.dh16, true, w.n2g, w.n2b, rows, d, 1e-6f, false, st, true));
         e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.b_cross_q; e.out = b.dq16; e.ldo = d;
         RC(gemm_f16_small(b.dh16, d, w.w_cross_q, d, e, rows, d, d, st));
         t = DecAttnArgs{};
@@ -780,7 +780,7 @@ static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int
         RC(dec_attention(t, rows, T, st));
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_cross_out; e.out = b.dx; e.resid = b.dx; e.ldo = d;
         RC(gemm_f16_small(b.datt16, d, w.w_cross_out, d, e, rows, d, d, st));
-        RC(layernorm_rows(b.dx, b.dh16, true, w.n3g, w.n3b, rows, d, 1e-6f, false, st));
+        RC(layernorm_rows(b.dx, b.dh16, true, w.n3g, w.n3b, rows, d, 1e-6f, false, st, true));
         e = GemmEpilogue(); e.mode = EPI_F16; e.act = c.decoder_activation == SBK_ACT_GELU ? ACT_GELU : ACT_RELU;
         e.bias = w.b_ffn1; e.out = b.df16; e.ldo = F;
         RC(gemm_f16_small(b.dh16, d, w.w_ffn1, d, e, rows, F, d, st));
@@ -789,16 +789,24 @@ static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int
     }
     if (!with_head) return SBK_OK;
     SBK_REQUIRE(m->w_lin != nullptr, "decode step: this handle was created without the output head (seq_lin.w.*)");
-    RC(layernorm_rows(b.dx, b.dh16, true, m->dec_norm_g, m->dec_norm_b, rows, d, 1e-6f, false, st));
+    RC(layernorm_rows(b.dx, b.dh16, true, m->dec_norm_g, m->dec_norm_b, rows, d, 1e-6f, false, st, true));
     GemmEpilogue e;
     e.mode = EPI_F32; e.bias = m->b_lin; e.out = b.logits; e.ldo = c.vocab;
     RC(gemm_f16_small(b.dh16, d, m->w_lin, d, e, rows, c.vocab, d, st));
     return SBK_OK;
 }
 
+// the wgmma decode path (enqueue_decode_layers_tc) for `rows` live hypotheses
+static bool decode_tc(const AsrModel* m, int rows) {
+    return rows >= m->dec_tc_rows && m->cfg.d_model % 32 == 0;  // (the QKV -> cache scatter epilogue works on 32-column chunks)
+}
+// Programmatic dependent launch is always on for the wgmma decode path (its GEMMs and LayerNorms are launched with it
+// unconditionally); on the weight-streaming path it is opt-in (SBK_PDL=1), where it measured no faster.
+static void set_decode_pdl(const AsrModel* m, int rows) { set_pdl(decode_tc(m, rows) || getenv("SBK_PDL") != nullptr); }
+
 static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage,
                                  cudaStream_t st, bool with_head = true) {
-    if (rows >= m->dec_tc_rows && m->cfg.d_model % 32 == 0)  // (the QKV -> cache scatter epilogue works on 32-column chunks)
+    if (decode_tc(m, rows))
         return enqueue_decode_layers_tc(m, rows, rows_per_utt, T, S_max, lineage, st, with_head);
     const sbk_asr_config& c = m->cfg;
     AsrModel::Buf& b = m->b;
@@ -966,7 +974,7 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
     *steps_done = 0;
     if (p.max_steps <= 0) return SBK_OK;
     RC(project_cross_kv(m, M, T, st));
-    set_pdl(getenv("SBK_PDL") != nullptr);
+    set_decode_pdl(m, rows);
     const bool use_lm = p.lm_weight != 0.0f;
     SBK_REQUIRE(!use_lm || m->has_lm, "beam: lm_weight != 0 but this handle has no TransformerLM weights");
     const bool use_ctc = p.ctc_weight != 0.0f;
@@ -1127,7 +1135,7 @@ static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos
     if (max_steps <= 0) return SBK_OK;
     RC(project_cross_kv(m, M, T, st));  // cross-attention K/V of all layers, once per utterance
     RC(greedy_reset(b.tokens, S_max + 1, rows, bos, b.step, b.has_ended, b.ended_count, m->emb, m->dec_pe, d, b.dx, st));
-    set_pdl(getenv("SBK_PDL") != nullptr);  // programmatic dependent launch: opt-in only
+    set_decode_pdl(m, rows);
     const bool use_graph = !in_capture && getenv("SBK_NO_GRAPH") == nullptr && log_probs == nullptr;
     if (in_capture) {  // the caller is capturing the whole pipeline: enqueue exactly max_steps steps, no polling
         for (int i = 0; i < max_steps; ++i) RC(enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, st));

@@ -9,19 +9,22 @@ namespace sbk {
 
 // Apply the epilogue to 32 consecutive accumulator columns of one row.
 // `pre`: bias (and, for EPI_RESID, residual) values of this full, in-range chunk were fetched by the caller before the
-// accumulator was ready (the latency-bound decode-step GEMMs hide two L2 round trips that way).
+// accumulator was ready (the latency-bound decode-step GEMMs hide two L2 round trips that way).  The bias is a weight
+// and may be fetched before pdl_wait(); the residual is the previous kernel's output and only after it.
 struct EpiPrefetch {
     float4 bias[8];
     float4 res[8];
     bool on = false;
 };
-__device__ __forceinline__ void epilogue_prefetch(const GemmEpilogue& e, EpiPrefetch& p, int row, int col0, int M, int N) {
+__device__ __forceinline__ void epilogue_prefetch_bias(const GemmEpilogue& e, EpiPrefetch& p, int row, int col0, int M, int N) {
     p.on = row < M && col0 + 32 <= N;
     if (!p.on) return;
 #pragma unroll
     for (int j = 0; j < 8; ++j)
         p.bias[j] = e.bias != nullptr ? __ldg(reinterpret_cast<const float4*>(e.bias + col0) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-    if (e.mode == EPI_RESID) {
+}
+__device__ __forceinline__ void epilogue_prefetch_resid(const GemmEpilogue& e, EpiPrefetch& p, int row, int col0) {
+    if (p.on && e.mode == EPI_RESID) {
         const float4* r = reinterpret_cast<const float4*>(e.resid + static_cast<size_t>(row) * e.ldo + col0);
 #pragma unroll
         for (int j = 0; j < 8; ++j) p.res[j] = __ldcg(r + j);

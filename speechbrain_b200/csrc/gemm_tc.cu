@@ -5,9 +5,9 @@
 // Replaces the reference's F.linear / nn.Linear / Conv1d(k=1) call sites
 // (nnet/attention.py:623,739,932-936,1344; Conformer.py:126-157; TransformerASR.py:308-316).
 //
-// One 128 x BN output tile per CTA (main loop: gemm_mainloop.cuh).  The epilogue runs row-wise on 32-column chunks of
-// the staged accumulator tile, so it handles any N and every epilogue mode, including partial column chunks.  With
-// BN <= 128 two CTAs fit per SM, so one CTA's epilogue overlaps the other's main loop.
+// One BM x BN output tile per CTA (BM = 64 or 128; main loop: gemm_mainloop.cuh).  The epilogue runs row-wise on
+// 32-column chunks of the staged accumulator tile, so it handles any N and every epilogue mode, including partial column
+// chunks.  With BN <= 128 two CTAs fit per SM, so one CTA's epilogue overlaps the other's main loop.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -17,9 +17,9 @@
 
 namespace sbk {
 
-template <int BN, int STAGES, int SPLIT = 1>
+template <int BM, int BN, int STAGES>
 struct GemmSmem {
-    static constexpr int TOTAL = WgRing<BN, STAGES>::END + 1024;  // + alignment slack
+    static constexpr int TOTAL = WgRing<BM, BN, STAGES>::END + 1024;  // + alignment slack
 };
 
 // ---- split-K over a thread-block cluster (1, 1, SPLIT): CTA `rank` accumulates k-blocks [rank, rank+1) * num_kb / SPLIT,
@@ -44,32 +44,40 @@ __device__ __forceinline__ uint4 ld_cluster_u4(uint32_t local_addr, uint32_t cta
     return v;
 }
 
-template <int BN, int STAGES, int SPLIT = 1>
-__global__ void __launch_bounds__(WG_THREADS, (BN <= 128 ? 2 : 1))
+template <int BM, int BN, int STAGES, int SPLIT = 1>
+__global__ void __launch_bounds__(WgRoles<BM>::THREADS, (BN <= 128 ? 2 : 1))
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmEpilogue epi, int M, int N, int K) {
-    using R = WgRing<BN, STAGES>;
+    using R = WgRing<BM, BN, STAGES>;
+    constexpr int CONSUMERS = WgRoles<BM>::CONSUMERS;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * WG_BM;
+    const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
     const uint32_t rank = SPLIT > 1 ? gemm_cluster_rank() : 0u;
     const int num_kb = (K + WG_BK - 1) / WG_BK / SPLIT;   // k-blocks of this CTA (host checks divisibility)
     const int kb0 = static_cast<int>(rank) * num_kb;
 
-    wg_init<BN, STAGES>(smem, &tmap_a, &tmap_b);
+    // Before pdl_wait() (launched with programmatic stream serialisation, see common.cuh): barrier init, tensor-map
+    // prefetch, the first stages' weight loads and the bias.  Activations, the residual, the step counter and every
+    // global write come after it.
+    wg_init<BM, BN, STAGES>(smem, &tmap_a, &tmap_b);
     EpiPrefetch pre;
-    if (threadIdx.x >= WG_CONSUMERS) {
-        wg_produce<BN, STAGES>(smem, &tmap_a, &tmap_b, m0, n0, kb0, num_kb);
+    if (threadIdx.x >= CONSUMERS) {
+        wg_produce<BM, BN, STAGES>(smem, &tmap_a, &tmap_b, m0, n0, kb0, num_kb);
     } else {
-        if constexpr (BN == 32 && SPLIT == 1)  // while the main loop runs
-            if (threadIdx.x < WG_BM) epilogue_prefetch(epi, pre, m0 + threadIdx.x, n0, M, N);
-        wg_consume_and_stage<BN, STAGES>(smem, num_kb);
+        constexpr bool prefetch = BN == 32 && SPLIT == 1;  // while the main loop runs
+        if constexpr (prefetch)
+            if (threadIdx.x < BM) epilogue_prefetch_bias(epi, pre, m0 + threadIdx.x, n0, M, N);
+        pdl_wait();  // the consumers' own: the producer's wait does not order this thread's reads and writes
+        if constexpr (prefetch)
+            if (threadIdx.x < BM) epilogue_prefetch_resid(epi, pre, m0 + threadIdx.x, n0);
+        wg_consume_and_stage<BM, BN, STAGES>(smem, num_kb);
     }
     if constexpr (SPLIT > 1) gemm_cluster_sync();  // every rank's partial tile is staged (release / acquire)
-    if (threadIdx.x < WG_CONSUMERS && rank == 0) {
-        const int r = threadIdx.x & (WG_BM - 1);
+    if (threadIdx.x < CONSUMERS && rank == 0) {
+        const int r = threadIdx.x & (BM - 1);
 #pragma unroll 1
-        for (int c = threadIdx.x / WG_BM; c < BN / 32; c += WG_CONSUMERS / WG_BM) {
+        for (int c = threadIdx.x / BM; c < BN / 32; c += CONSUMERS / BM) {
             const uint32_t src = smem_u32(smem) + r * R::STG_PITCH + c * 128;
             uint32_t acc[32];
             wg_load_row32(src, acc);
@@ -90,18 +98,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     if constexpr (SPLIT > 1) gemm_cluster_sync();  // the other ranks keep their shared memory until rank 0 has read it
 }
 
-template <int BN, int STAGES, int SPLIT = 1>
+// pdl: launch with programmatic stream serialisation (the decode-step projections; not the cluster split-K variant);
+// the kernel's pre-wait section obeys the rules of common.cuh either way.
+template <int BM, int BN, int STAGES, int SPLIT = 1>
 static int launch_gemm(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
-                       cudaStream_t stream) {
-    using S = GemmSmem<BN, STAGES, SPLIT>;
+                       cudaStream_t stream, bool pdl) {
+    using S = GemmSmem<BM, BN, STAGES>;
     CUtensorMap ta, tb;
-    int rc = make_tmap_2d_f16(&ta, A, M, K, lda, WG_BM, WG_BK);
+    int rc = make_tmap_2d_f16(&ta, A, M, K, lda, BM, WG_BK);
     if (rc) return rc;
     rc = make_tmap_2d_f16(&tb, W, N, K, ldw, BN, WG_BK);
     if (rc) return rc;
-    auto kern = gemm_tc_kernel<BN, STAGES, SPLIT>;
+    auto kern = gemm_tc_kernel<BM, BN, STAGES, SPLIT>;
     SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    dim3 grid(ceil_div(N, BN), ceil_div(M, WG_BM), SPLIT);
+    dim3 grid(ceil_div(N, BN), ceil_div(M, BM), SPLIT);
     GemmProfile* prof = gemm_profile();
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (prof->enabled) {
@@ -110,11 +120,11 @@ static int launch_gemm(const void* A, int lda, const void* W, int ldw, const Gem
         cudaEventRecord(e0, stream);
     }
     if constexpr (SPLIT == 1) {
-        kern<<<grid, WG_THREADS, S::TOTAL, stream>>>(ta, tb, epi, M, N, K);
+        SBK_CUDA_CHECK(launch_pdl(kern, grid, dim3(WgRoles<BM>::THREADS), S::TOTAL, stream, pdl, ta, tb, epi, M, N, K));
     } else {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = grid;
-        cfg.blockDim = dim3(WG_THREADS);
+        cfg.blockDim = dim3(WgRoles<BM>::THREADS);
         cfg.dynamicSmemBytes = S::TOTAL;
         cfg.stream = stream;
         cudaLaunchAttribute attr[1];
@@ -148,14 +158,16 @@ int gemm_f16_small(const void* A, int lda, const void* W, int ldw, const GemmEpi
     if (epi.mode == EPI_QKV_CACHE)
         SBK_REQUIRE(epi.qkv_d % 32 == 0 && N == 3 * epi.qkv_d && epi.kcache && epi.vcache && epi.step_ptr,
                     "gemm_f16_small: bad EPI_QKV_CACHE arguments");
-    // few, latency-bound CTAs: narrow N tiles spread the weight stream over more SMs; the ring holds a whole K = 512 panel
-    if (N > 2048) return launch_gemm<64, 6>(A, lda, W, ldw, epi, M, N, K, stream);
+    // few, latency-bound CTAs: narrow N tiles spread the weight stream over more SMs; the ring holds a whole K = 512 panel.
+    // 64-row tiles (one consumer warpgroup): twice the CTAs of 128-row tiles, each streaming half the activations -- at
+    // 96 - 224 rows they measured faster for every decode shape (FFN2 K = 2048 and the vocabulary head included).
+    if (N > 2048) return launch_gemm<64, 64, 6>(A, lda, W, ldw, epi, M, N, K, stream, true);
     // K = d_ffn: 4-way cluster split-K (deterministic DSMEM reduce) shortens that one kernel, but its 4x CTAs take SMs from
     // the other lanes in flight -> opt-in
     static const bool split = getenv("SBK_DEC_SPLITK") != nullptr;
     if (K >= 2048 && K % (4 * WG_BK) == 0 && split)
-        return launch_gemm<32, 8, 4>(A, lda, W, ldw, epi, M, N, K, stream);
-    return launch_gemm<32, 8>(A, lda, W, ldw, epi, M, N, K, stream);
+        return launch_gemm<128, 32, 8, 4>(A, lda, W, ldw, epi, M, N, K, stream, false);
+    return launch_gemm<64, 32, 8>(A, lda, W, ldw, epi, M, N, K, stream, true);
 }
 
 int gemm_f16(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
@@ -168,7 +180,7 @@ int gemm_f16(const void* A, int lda, const void* W, int ldw, const GemmEpilogue&
         SBK_REQUIRE(N % 32 == 0, "gemm_f16: GLU/RoPE epilogues need N %% 32 == 0");
     if (epi.mode == EPI_ROPE) SBK_REQUIRE(epi.head_dim % 32 == 0, "gemm_f16: RoPE epilogue needs head_dim %% 32 == 0");
     if (N % 256 == 0 && getenv("SBK_GEMM_V1") == nullptr) return gemm_f16_wide(A, lda, W, ldw, epi, M, N, K, stream);
-    return launch_gemm<128, 3>(A, lda, W, ldw, epi, M, N, K, stream);
+    return launch_gemm<128, 128, 3>(A, lda, W, ldw, epi, M, N, K, stream, false);
 }
 
 }  // namespace sbk

@@ -81,8 +81,9 @@ int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float*
                          cudaStream_t stream);
 
 // ---- encoder_ops.cu
+// pdl: launched with programmatic stream serialisation (fp16 output only; the decode step's pre-norms)
 int layernorm_rows(const float* x, void* out, bool out_half, const float* gamma, const float* beta, int M, int D,
-                   float eps, bool act_silu, cudaStream_t stream);
+                   float eps, bool act_silu, cudaStream_t stream, bool pdl = false);
 // y = LN_a(x) (fp32, stored when y_out != null), z = LN_b(y) -> z_out (fp16 or fp32): two chained LayerNorms in one pass
 int layernorm2_rows(const float* x, float* y_out, void* z_out, bool z_half, const float* ga, const float* ba, float eps_a,
                     const float* gb, const float* bb, float eps_b, int M, int D, cudaStream_t stream);
@@ -107,6 +108,8 @@ struct SkinnyArgs {
     // LayerNorm-fused variant: A = LayerNorm(X fp32 [n_rows, K]) computed in-kernel (X != nullptr)
     const float* X; const float* ln_g; const float* ln_b; float ln_eps;
 };
+// programmatic dependent launch of the decode-step kernels launched by decoder.cu (attention, skinny GEMM, greedy /
+// beam bookkeeping, TransformerLM helpers)
 void set_pdl(bool on);
 int skinny_gemm(const SkinnyArgs& a, cudaStream_t stream);
 struct DecAttnArgs {
