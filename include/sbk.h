@@ -130,6 +130,19 @@ int sbk_asr_set_decoder_tc_min_rows(sbk_asr* m, int rows);
  * `temperature` with the pad column excluded from the normalisation.  Needs a handle created with SBK_PART_LM. */
 int sbk_asr_lm_rescore(sbk_asr* m, const int* tokens_dev, const int* lens_dev, int n, int L, float temperature, int pad_index,
                        float* scores_dev, void* stream);
+/* TransformerLM.forward(src) (lobes/models/transformer/TransformerLM.py:127-169), whole sequences at once: tokens_dev [n, s]
+ * int32 ids in [0, vocab), 0 = padding (make_masks' key-padding mask; pad positions still get logits, computed like the
+ * reference's) -> logits_dev [n, s, vocab] fp32, written directly.  Causal self-attention with the look-ahead and key-padding
+ * masks; every layer runs on all n * s rows at once.  Needs a handle created with SBK_PART_LM, s <= max_len and
+ * n <= 65535; the call grows a workspace of its own (14 * d_model + 2 * d_ffn bytes per token row) on first use.  Ids are
+ * not checked on the host (that would need a synchronise): an id outside [0, vocab) is never used as a table index, it
+ * turns its sequence's logits into NaN (other sequences are unaffected).  Enqueue only. */
+int sbk_asr_lm_forward(sbk_asr* m, const int* tokens_dev, int n, int s, float* logits_dev, void* stream);
+/* The same logits from the KV-cached TransformerLM step that the beam search's scorer and the rescorer run: position by
+ * position, teacher-forced, keys with id 0 masked through the token cache.  tokens_dev [n, L] int32 in [0, vocab) ->
+ * logits_dev [n, L, vocab] fp32.  L dependent steps: for checking sbk_asr_lm_forward against the step path, not a fast
+ * way to get logits.  Needs SBK_PART_LM and L <= max_len. */
+int sbk_asr_lm_step_logits(sbk_asr* m, const int* tokens_dev, int n, int L, float* logits_dev, void* stream);
 int sbk_asr_num_frames(const sbk_asr* m, int n_samples, int* T_feat, int* T_enc);
 
 /* ConvolutionFrontEnd.forward (lobes/models/convolution.py:116-320): feats [B,T0,n_mels] -> out [B,T2,F2*C2] fp32 */

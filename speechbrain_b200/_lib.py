@@ -50,6 +50,7 @@ EXPORTS = [
     "sbk_asr_transcribe_greedy_host", "sbk_asr_transcribe_greedy_host_async", "sbk_asr_clone",
     "sbk_asr_set_poll_interval", "sbk_asr_beam_from_enc", "sbk_asr_set_decoder_ln_fusion", "sbk_asr_transcribe_greedy_group_dev",
     "sbk_asr_set_decoder_tc_min_rows", "sbk_asr_lm_rescore", "sbk_asr_transcribe_greedy_group_host_async", "sbk_asr_decode_teacher_forced", "sbk_asr_ctc_head", "sbk_rows_argmax_f32", "sbk_asr_set_dynchunk",
+    "sbk_asr_lm_forward", "sbk_asr_lm_step_logits",
 ]
 
 

@@ -771,4 +771,173 @@ int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_d
     return SBK_ERR_UNSUPPORTED;
 }
 
+// =========================================================================== TransformerLM causal self-attention
+// Whole-sequence attention of TransformerLM.forward (TransformerLM.py:127-169: nn.MultiheadAttention under make_masks'
+// look-ahead mask and key-padding mask on pad_idx).  qkv [n*s, 3d] fp16 with columns [q | k | v] (nn.MultiheadAttention's
+// in_proj order, heads of 64 side by side, q pre-scaled by 1/sqrt(64)) -> out [n*s, d] fp16.
+// One CTA = (64 query rows, head, sequence), 4 warps x 16 rows, mma.sync m16n8k16 with an fp32 online softmax like
+// encoder_attention_kernel.  Query block qb reads key blocks 0..qb only: blocks above the diagonal are never loaded.
+// Masked: keys j > i (diagonal block only) and keys whose token id is pad_tok -- the rule the KV-cached step applies
+// through tok_cache / pad_tok (dec_attention_kernel).  A query whose visible keys are all padding (a sequence that starts
+// with the pad id) has an empty softmax and yields NaN, as in the reference and the step path.
+constexpr int LMA_B = 64;
+
+__global__ void __launch_bounds__(128)
+lm_causal_attention_kernel(const __half* __restrict__ qkv, int s, int d, const int* __restrict__ tokens, int pad_tok,
+                           __half* __restrict__ out) {
+    constexpr int DH = 64, STR = DH + 8, KS = DH / 16;
+    __shared__ __align__(16) __half Qs[LMA_B * STR];
+    __shared__ __align__(16) __half KVs[2][2][LMA_B * STR];  // [buffer][K | V]
+    __shared__ bool s_masked[2][LMA_B];                       // [buffer][key]: pad token or past the sequence
+    const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z, i0 = qb * LMA_B;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
+    const int ld = 3 * d;
+    const __half* base = qkv + static_cast<size_t>(b) * s * ld + h * DH;
+    const int* tok = tokens + static_cast<size_t>(b) * s;
+
+    auto cp16 = [](__half* dst, const __half* src, bool ok) {  // rows past the sequence are zero-filled
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(ok ? 16u : 0u)
+                     : "memory");
+    };
+    auto stage = [&](int jb, int buf) {  // key block jb -> buffer buf (one cp.async group)
+        const int j0 = jb * LMA_B;
+        for (int i = threadIdx.x; i < LMA_B * (DH / 8); i += blockDim.x) {
+            const int r = i / (DH / 8), v8 = i - r * (DH / 8);
+            const bool ok = j0 + r < s;
+            const __half* rowp = base + static_cast<size_t>(ok ? j0 + r : 0) * ld + v8 * 8;
+            cp16(KVs[buf][0] + r * STR + v8 * 8, rowp + d, ok);
+            cp16(KVs[buf][1] + r * STR + v8 * 8, rowp + 2 * d, ok);
+        }
+        if (threadIdx.x < LMA_B) {
+            const int j = j0 + threadIdx.x;
+            s_masked[buf][threadIdx.x] = j >= s || tok[j] == pad_tok;
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    for (int i = threadIdx.x; i < LMA_B * (DH / 8); i += blockDim.x) {  // Q rides in key block 0's group
+        const int r = i / (DH / 8), v8 = i - r * (DH / 8);
+        const bool ok = i0 + r < s;
+        cp16(Qs + r * STR + v8 * 8, base + static_cast<size_t>(ok ? i0 + r : 0) * ld + v8 * 8, ok);
+    }
+    stage(0, 0);
+
+    uint32_t qa[KS][4];
+    float o[DH / 8][4];
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.0f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.0f, 0.0f};
+    const float LOG2E = 1.4426950408889634f;
+    const int qi[2] = {i0 + warp * 16 + g, i0 + warp * 16 + g + 8};  // this thread's two query rows
+
+    for (int jb = 0; jb <= qb; ++jb) {
+        const int buf = jb & 1, j0 = jb * LMA_B;
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        __syncthreads();  // block jb has landed for everyone; block jb-1 (the other buffer) is fully consumed
+        if (jb + 1 <= qb) stage(jb + 1, buf ^ 1);
+        if (jb == 0) {
+            const __half* q0 = Qs + (warp * 16 + g) * STR + 2 * c;
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) {
+                qa[ks][0] = *reinterpret_cast<const uint32_t*>(q0 + ks * 16);
+                qa[ks][1] = *reinterpret_cast<const uint32_t*>(q0 + 8 * STR + ks * 16);
+                qa[ks][2] = *reinterpret_cast<const uint32_t*>(q0 + ks * 16 + 8);
+                qa[ks][3] = *reinterpret_cast<const uint32_t*>(q0 + 8 * STR + ks * 16 + 8);
+            }
+        }
+        const __half* Kc = KVs[buf][0];
+        const __half* Vc = KVs[buf][1];
+        float sc[LMA_B / 8][4];
+#pragma unroll
+        for (int nt = 0; nt < LMA_B / 8; ++nt) {
+            sc[nt][0] = sc[nt][1] = sc[nt][2] = sc[nt][3] = 0.0f;
+            const __half* kp = Kc + (nt * 8 + (lane & 7)) * STR + (lane >> 3) * 8;
+#pragma unroll
+            for (int ks = 0; ks < KS; ks += 2) {
+                uint32_t b0, b1, b2, b3;
+                ldmatrix_x4(b0, b1, b2, b3, kp + ks * 16);
+                mma16816(sc[nt], qa[ks], b0, b1);
+                mma16816(sc[nt], qa[ks + 1], b2, b3);
+            }
+        }
+        // ---- key-padding and (diagonal block) look-ahead mask, then the online softmax of rows g and g + 8
+        const bool diag = jb == qb;
+#pragma unroll
+        for (int nt = 0; nt < LMA_B / 8; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int lj = nt * 8 + 2 * c + (e & 1);
+                if (s_masked[buf][lj] || (diag && j0 + lj > qi[e >> 1])) sc[nt][e] = -INFINITY;
+            }
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int nt = 0; nt < LMA_B / 8; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) mx[e >> 1] = fmaxf(mx[e >> 1], sc[nt][e]);
+        float alpha[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+            const float m_new = fmaxf(m_run[r], mx[r]);
+            // (a block whose keys are all padding leaves a row with no visible key so far)
+            alpha[r] = m_new == -INFINITY ? 1.0f : ex2_ftz((m_run[r] - m_new) * LOG2E);
+            m_run[r] = m_new;
+        }
+        float rs[2] = {0.0f, 0.0f};
+        uint32_t pa[LMA_B / 16][4];
+        const float ms0 = m_run[0] == -INFINITY ? 0.0f : m_run[0] * LOG2E, ms1 = m_run[1] == -INFINITY ? 0.0f : m_run[1] * LOG2E;
+#pragma unroll
+        for (int nt = 0; nt < LMA_B / 8; ++nt) {
+            const float p0 = ex2_ftz(fmaf(sc[nt][0], LOG2E, -ms0)), p1 = ex2_ftz(fmaf(sc[nt][1], LOG2E, -ms0));
+            const float p2 = ex2_ftz(fmaf(sc[nt][2], LOG2E, -ms1)), p3 = ex2_ftz(fmaf(sc[nt][3], LOG2E, -ms1));
+            rs[0] += p0 + p1;
+            rs[1] += p2 + p3;
+            pa[nt >> 1][(nt & 1) * 2 + 0] = pack_half2(p0, p1);
+            pa[nt >> 1][(nt & 1) * 2 + 1] = pack_half2(p2, p3);
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            rs[r] += __shfl_xor_sync(0xffffffffu, rs[r], 1);
+            rs[r] += __shfl_xor_sync(0xffffffffu, rs[r], 2);
+            l_run[r] = l_run[r] * alpha[r] + rs[r];
+        }
+#pragma unroll
+        for (int nt = 0; nt < DH / 8; ++nt) {
+            o[nt][0] *= alpha[0]; o[nt][1] *= alpha[0];
+            o[nt][2] *= alpha[1]; o[nt][3] *= alpha[1];
+        }
+        // ---- O += P V : B fragments of V[key][dim] via ldmatrix.trans
+#pragma unroll
+        for (int kk = 0; kk < LMA_B / 16; ++kk) {
+#pragma unroll
+            for (int nt = 0; nt < DH / 8; nt += 2) {
+                uint32_t b0, b1, b2, b3;
+                ldmatrix_x4_trans(b0, b1, b2, b3, Vc + (kk * 16 + (lane & 15)) * STR + nt * 8 + (lane >> 4) * 8);
+                mma16816(o[nt], pa[kk], b0, b1);
+                mma16816(o[nt + 1], pa[kk], b2, b3);
+            }
+        }
+    }
+    // ---- normalise and store (l == 0 only for a row without any visible key: 0 * inf = NaN, see above)
+    const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+    __half* ob = out + static_cast<size_t>(b) * s * d + h * DH;
+#pragma unroll
+    for (int nt = 0; nt < DH / 8; ++nt) {
+        const int col = nt * 8 + 2 * c;
+        if (qi[0] < s) *reinterpret_cast<uint32_t*>(ob + static_cast<size_t>(qi[0]) * d + col) = pack_half2(o[nt][0] * inv0, o[nt][1] * inv0);
+        if (qi[1] < s) *reinterpret_cast<uint32_t*>(ob + static_cast<size_t>(qi[1]) * d + col) = pack_half2(o[nt][2] * inv1, o[nt][3] * inv1);
+    }
+}
+
+int lm_causal_attention(const __half* qkv, int n, int s, int d, int H, const int* tokens, int pad_tok, __half* out,
+                        cudaStream_t stream) {
+    SBK_REQUIRE(d == H * 64 && d % 8 == 0, "lm_causal_attention: head_dim must be 64 (d=%d, H=%d)", d, H);
+    SBK_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 3) == 0,
+                "lm_causal_attention: misaligned operands");
+    if (n == 0 || s == 0) return SBK_OK;
+    lm_causal_attention_kernel<<<dim3(ceil_div(s, LMA_B), H, n), 128, 0, stream>>>(qkv, s, d, tokens, pad_tok, out);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
 }  // namespace sbk

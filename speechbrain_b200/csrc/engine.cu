@@ -96,6 +96,13 @@ struct AsrModel {
     // xb [B, T], rsum/rb [2][rows, T] and psi [2][rows] ping-pong by step parity, add [rows, V] when there is no LM buffer
     struct CtcBuf { float* base = nullptr; size_t cap = 0; float *x, *xlin, *xb, *rsum, *rb, *psi, *add, *tab, *tabM; } ctc;
     struct CovBuf { float* base = nullptr; size_t cap = 0; } cov;  // CoverageScorer: [2][rows][T] coverage + [rows] scores
+    // TransformerLM whole-sequence forward (run_lm_forward), carved for `rows` = n * s token rows, independent of the
+    // decode / beam workspace: residual stream x [rows, d] fp32, its fp16 copy x16, qkv16 [rows, 3d], att16 [rows, d],
+    // f16 [rows, d_ffn]
+    struct LmFwdBuf {
+        uint8_t* base = nullptr; size_t cap = 0; int rows = 0;
+        float* x; __half *x16, *qkv16, *att16, *f16;
+    } lmf;
     // shapes the workspace is carved for
     int wsB = 0, wsL = 0, ws_rows = 0, ws_steps = 0;
     struct Buf {
@@ -479,6 +486,7 @@ int asr_clone(AsrModel* src, AsrModel** out) {
     m->b = AsrModel::Buf();
     m->ctc = AsrModel::CtcBuf();
     m->cov = AsrModel::CovBuf();
+    m->lmf = AsrModel::LmFwdBuf();
     m->step_graph = nullptr;
     m->pipe_graph = nullptr;
     m->group_graph = nullptr;
@@ -519,6 +527,7 @@ void asr_destroy(AsrModel* m) {
     cudaFree(m->ws.base);
     cudaFree(m->ctc.base);
     cudaFree(m->cov.base);
+    cudaFree(m->lmf.base);
     if (m->host_flag) cudaFreeHost(m->host_flag);
     if (m->cap_stream) cudaStreamDestroy(m->cap_stream);
     if (m->side_stream) cudaStreamDestroy(m->side_stream);
@@ -1260,6 +1269,98 @@ static int run_lm_rescore(AsrModel* m, const int* tokens, const int* lens, int n
     return SBK_OK;
 }
 
+// The same teacher-forced step path, keeping each position's raw logits: out[:, s, :] = lm_logits after feeding
+// tokens[:, s].  Keys are masked through tok_cache exactly as in the rescorer and the beam search's LM scorer.
+static int run_lm_step_logits(AsrModel* m, const int* tokens, int n, int L, float* out, cudaStream_t st) {
+    const sbk_asr_config& c = m->cfg;
+    AsrModel::Buf& b = m->b;
+    const int S_max = m->ws_steps + 1, dl = c.lm_d_model, V = c.vocab;
+    lm_teacher_reset_kernel<<<n, 128, 0, st>>>(tokens, n, L, S_max, 0, b.lineage, b.tok_cache, b.score);
+    SBK_LAUNCH_CHECK();
+    for (int s = 0; s < L; ++s) {
+        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->lm_emb, m->lm_pe, dl, sqrtf((float)dl), b.lx, b.lx16, b.step);
+        SBK_LAUNCH_CHECK();
+        RC(enqueue_lm_step(m, n, S_max, 1.0f, 1.0f, st));
+        SBK_CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s * V, (size_t)L * V * 4, b.lm_logits, (size_t)V * 4, (size_t)V * 4, n,
+                                         cudaMemcpyDeviceToDevice, st));
+    }
+    return SBK_OK;
+}
+
+// ---------------------------------------------------------------------------- TransformerLM.forward (TransformerLM.py:127-169)
+// Whole sequences at once: the n * s token rows go through every layer together on the encoder's wgmma GEMMs, attention is
+// the causal flash kernel (lm_causal_attention).  Same weights, epilogues and LayerNorm kernel as the KV-cached step.
+// Row r = (sequence r / s, position r % s): x = emb[token] * sqrt(d) + pe[pos], fp32 residual stream + fp16 GEMM operand
+// (the whole-sequence counterpart of lm_teacher_embed_kernel).  An id outside [0, vocab) is not read from the table: its
+// row becomes NaN (and, through attention, its sequence) instead of an out-of-bounds read.
+__global__ void lm_embed_kernel(const int* __restrict__ tokens, int s, int vocab, const float* __restrict__ emb,
+                                const float* __restrict__ pe, int d, float sqrt_d, float* __restrict__ x,
+                                __half* __restrict__ x16) {
+    const int r = blockIdx.x, pos = r % s;
+    const int tok = tokens[r];
+    const bool ok = tok >= 0 && tok < vocab;
+    for (int i = threadIdx.x; i < d; i += blockDim.x) {
+        const float v = ok ? emb[static_cast<size_t>(tok) * d + i] * sqrt_d + pe[static_cast<size_t>(pos) * d + i] : NAN;
+        x[static_cast<size_t>(r) * d + i] = v;
+        x16[static_cast<size_t>(r) * d + i] = float2half_sat(v);
+    }
+}
+
+static int ensure_lm_workspace(AsrModel* m, int rows, cudaStream_t st) {
+    AsrModel::LmFwdBuf& w = m->lmf;
+    if (w.base && rows <= w.rows) return SBK_OK;
+    const size_t R = rows, dl = m->cfg.lm_d_model, Fl = m->cfg.lm_d_ffn;
+    auto al = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
+    const size_t need = al(R * dl * 4) + al(R * dl * 2) + al(R * 3 * dl * 2) + al(R * dl * 2) + al(R * Fl * 2);
+    if (need > w.cap) {
+        if (w.base) { SBK_CUDA_CHECK(cudaStreamSynchronize(st)); cudaFree(w.base); w.base = nullptr; w.cap = 0; w.rows = 0; }
+        if (cudaMalloc(&w.base, need) != cudaSuccess) { set_error("lm_forward: workspace cudaMalloc(%zu) failed", need); return SBK_ERR_NOMEM; }
+        w.cap = need;
+    }
+    uint8_t* q = w.base;
+    w.x = reinterpret_cast<float*>(q); q += al(R * dl * 4);
+    w.x16 = reinterpret_cast<__half*>(q); q += al(R * dl * 2);
+    w.qkv16 = reinterpret_cast<__half*>(q); q += al(R * 3 * dl * 2);
+    w.att16 = reinterpret_cast<__half*>(q); q += al(R * dl * 2);
+    w.f16 = reinterpret_cast<__half*>(q);
+    w.rows = rows;
+    return SBK_OK;
+}
+
+static int run_lm_forward(AsrModel* m, const int* tokens, int n, int s, float* logits, cudaStream_t st) {
+    const sbk_asr_config& c = m->cfg;
+    const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead, M = n * s;
+    RC(ensure_lm_workspace(m, M, st));
+    const AsrModel::LmFwdBuf& b = m->lmf;
+    lm_embed_kernel<<<M, 128, 0, st>>>(tokens, s, c.vocab, m->lm_emb, m->lm_pe, dl, sqrtf((float)dl), b.x, b.x16);
+    SBK_LAUNCH_CHECK();
+    for (int l = 0; l < c.lm_layers; ++l) {  // post-norm TransformerEncoderLayer (Transformer.py:466-481)
+        const LmLayerW& w = m->lm[l];
+        GemmEpilogue e;
+        e.mode = EPI_F16; e.bias = w.b_in; e.out = b.qkv16; e.ldo = 3 * dl;
+        RC(gemm_f16(b.x16, dl, w.w_in, dl, e, M, 3 * dl, dl, st));
+        RC(lm_causal_attention(b.qkv16, n, s, dl, H, tokens, 0, b.att16, st));
+        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_out; e.out = b.x; e.resid = b.x; e.ldo = dl;
+        RC(gemm_f16(b.att16, dl, w.w_out, dl, e, M, dl, dl, st));
+        RC(layernorm_dual(b.x, b.x16, w.n1g, w.n1b, M, dl, 1e-6f, true, st));
+        e = GemmEpilogue(); e.mode = EPI_F16; e.act = c.lm_activation == SBK_ACT_GELU ? ACT_GELU : ACT_RELU;
+        e.bias = w.b1; e.out = b.f16; e.ldo = Fl;
+        RC(gemm_f16(b.x16, dl, w.w1, dl, e, M, Fl, dl, st));
+        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b2; e.out = b.x; e.resid = b.x; e.ldo = dl;
+        RC(gemm_f16(b.f16, Fl, w.w2, Fl, e, M, dl, Fl, st));
+        RC(layernorm_dual(b.x, b.x16, w.n2g, w.n2b, M, dl, 1e-6f, true, st));
+    }
+    RC(layernorm_dual(b.x, b.x16, m->lm_norm_g, m->lm_norm_b, M, dl, 1e-6f, false, st));  // encoder.norm
+    // output_proj: Linear d -> d (fp32, into the free residual buffer), LayerNorm, Linear d -> vocab into the caller's logits
+    GemmEpilogue e;
+    e.mode = EPI_F32; e.bias = m->lm_bp0; e.out = b.x; e.ldo = dl;
+    RC(gemm_f16(b.x16, dl, m->lm_wp0, dl, e, M, dl, dl, st));
+    RC(layernorm_dual(b.x, b.x16, m->lm_lnp_g, m->lm_lnp_b, M, dl, 1e-6f, false, st));
+    e = GemmEpilogue(); e.mode = EPI_F32; e.bias = m->lm_bp2; e.out = logits; e.ldo = c.vocab;
+    RC(gemm_f16(b.x16, dl, m->lm_wp2, dl, e, M, c.vocab, dl, st));
+    return SBK_OK;
+}
+
 }  // namespace sbk
 
 // ============================================================================ C ABI
@@ -1885,6 +1986,29 @@ int sbk_asr_lm_rescore(sbk_asr* mm, const int* tokens_dev, const int* lens_dev, 
     SBK_REQUIRE(pad_index == 0, "lm_rescore: pad_index must be 0 (TransformerLM.make_masks pads with index 0)");
     RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
     return run_lm_rescore(m, tokens_dev, lens_dev, n, L, temperature, pad_index, scores_dev, st);
+}
+
+// TransformerLM.forward(src) (TransformerLM.py:127-169): tokens_dev [n, s] int32 (pad id 0) -> logits_dev [n, s, vocab] fp32.
+int sbk_asr_lm_forward(sbk_asr* mm, const int* tokens_dev, int n, int s, float* logits_dev, void* stream) {
+    AsrModel* m = reinterpret_cast<AsrModel*>(mm);
+    SBK_REQUIRE(m != nullptr && tokens_dev && logits_dev, "lm_forward: null argument");
+    SBK_REQUIRE(m->has_lm, "lm_forward: this handle was created without TransformerLM weights");
+    SBK_REQUIRE(n >= 1 && s >= 1, "lm_forward: bad shape n=%d s=%d", n, s);
+    SBK_REQUIRE(n <= 65535, "lm_forward: n=%d sequences exceed the 65535 of one call (attention grid z)", n);
+    SBK_REQUIRE(s <= m->cfg.max_len, "lm_forward: s=%d exceeds max_len=%d", s, m->cfg.max_len);
+    SBK_REQUIRE((long long)n * s * std::max(m->cfg.vocab, 3 * m->cfg.lm_d_model) < (1LL << 31),
+                "lm_forward: n * s = %lld token rows is too many for one call", (long long)n * s);
+    return run_lm_forward(m, tokens_dev, n, s, logits_dev, static_cast<cudaStream_t>(stream));
+}
+
+// Step-by-step counterpart of sbk_asr_lm_forward on the KV-cached LM step: tokens_dev [n, L] -> logits_dev [n, L, vocab].
+int sbk_asr_lm_step_logits(sbk_asr* mm, const int* tokens_dev, int n, int L, float* logits_dev, void* stream) {
+    AsrModel* m = reinterpret_cast<AsrModel*>(mm);
+    SBK_REQUIRE(m != nullptr && tokens_dev && logits_dev, "lm_step_logits: null argument");
+    SBK_REQUIRE(m->has_lm, "lm_step_logits: this handle was created without TransformerLM weights");
+    SBK_REQUIRE(n >= 1 && L >= 1 && L <= m->cfg.max_len, "lm_step_logits: bad shape n=%d L=%d (max_len %d)", n, L, m->cfg.max_len);
+    RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
+    return run_lm_step_logits(m, tokens_dev, n, L, logits_dev, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -171,6 +171,7 @@ __device__ __forceinline__ void pp_epilogue_chunk(const GemmEpilogue& e, const f
                     if constexpr (ACT == ACT_SILU) v[q][i][c] = silu_f(v[q][i][c]);
                     else if constexpr (ACT == ACT_SILU_FAST) v[q][i][c] = silu_fast(v[q][i][c]);
                     else if constexpr (ACT == ACT_GELU) v[q][i][c] = gelu_erf_f(v[q][i][c]);
+                    else if constexpr (ACT == ACT_RELU) v[q][i][c] = fmaxf(v[q][i][c], 0.0f);
                 }
                 sts32(stg + (r0 + 8 * i) * P + (8 * q + qc) * 2, half2_bits(v[q][i][0], v[q][i][1]));
             }
@@ -411,6 +412,7 @@ static WideKernel pick_wide_kernel(const GemmEpilogue& epi, bool fast_act) {
         case EPI_F16:
             if (epi.act == ACT_SILU) return fast_act ? gemm_tc2_kernel<EPI_F16, ACT_SILU_FAST, BN> : gemm_tc2_kernel<EPI_F16, ACT_SILU, BN>;
             if (epi.act == ACT_GELU) return gemm_tc2_kernel<EPI_F16, ACT_GELU, BN>;
+            if (epi.act == ACT_RELU) return gemm_tc2_kernel<EPI_F16, ACT_RELU, BN>;  // ReLU TransformerLM FFN
             if (epi.act == ACT_NONE) return gemm_tc2_kernel<EPI_F16, ACT_NONE, BN>;
             return nullptr;
         case EPI_F32: return gemm_tc2_kernel<EPI_F32, ACT_NONE, BN>;

@@ -94,6 +94,10 @@ int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* w
 int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_dim, const int* lens, bool relpos,
                       const float* pos_u, const float* pos_v, const __half* P, int ldp, float scale, __half* out,
                       int ldo, cudaStream_t stream, int chunk = 0, int left_chunks = -1);
+// TransformerLM whole-sequence causal self-attention: qkv [n*s, 3d] fp16 ([q | k | v], head_dim 64, q pre-scaled), tokens
+// [n, s] int32 (keys whose id == pad_tok are masked) -> out [n*s, d] fp16
+int lm_causal_attention(const __half* qkv, int n, int s, int d, int H, const int* tokens, int pad_tok, __half* out,
+                        cudaStream_t stream);
 
 // ---- decoder.cu
 enum SkinnyEpi { SK_F16 = 0, SK_F16_GELU = 1, SK_F32 = 2, SK_RESID = 3, SK_QKV_CACHE = 4, SK_F16_RELU = 5 };

@@ -154,6 +154,30 @@ class AsrEngine:
                                            ptr(scores), self._sp()), "sbk_asr_lm_rescore")
         return scores
 
+    def lm_forward(self, tokens):
+        """TransformerLM.forward(src): ``tokens`` [n, s] integer CUDA (pad id 0) -> [n, s, vocab] fp32 CUDA logits, all
+        positions in one whole-sequence pass (causal attention, key-padding mask on id 0)."""
+        _lib.require_cuda(tokens, "AsrEngine.lm_forward")
+        if tokens.dim() != 2:
+            raise ValueError(f"AsrEngine.lm_forward: expected [n, s] token ids, got shape {tuple(tokens.shape)}")
+        tokens = tokens.to(torch.int32).contiguous()
+        n, s = tokens.shape
+        logits = torch.empty(n, s, self.cfg["vocab"], device=tokens.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(lib().sbk_asr_lm_forward(self._h, ptr(tokens), n, s, ptr(logits), self._sp()), "sbk_asr_lm_forward")
+        return logits
+
+    def lm_step_logits(self, tokens):
+        """The logits of ``lm_forward`` computed position by position on the KV-cached LM step (the path the beam search's
+        scorer and the rescorer run): ``tokens`` [n, L] integer CUDA -> [n, L, vocab] fp32 CUDA.  For comparing the two."""
+        _lib.require_cuda(tokens, "AsrEngine.lm_step_logits")
+        tokens = tokens.to(torch.int32).contiguous()
+        n, L = tokens.shape
+        logits = torch.empty(n, L, self.cfg["vocab"], device=tokens.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(lib().sbk_asr_lm_step_logits(self._h, ptr(tokens), n, L, ptr(logits), self._sp()), "sbk_asr_lm_step_logits")
+        return logits
+
     def set_decoder_tc_min_rows(self, rows):
         """Decode steps with >= rows live hypotheses use the wgmma GEMM for the decoder projections (default 64)."""
         check(lib().sbk_asr_set_decoder_tc_min_rows(self._h, int(rows)), "sbk_asr_set_decoder_tc_min_rows")
