@@ -105,6 +105,17 @@ int sbk_gemm_epilogue_test(const void* A_dev, const void* W_dev, const float* bi
                            int act, float alpha, const float* resid_dev, const int* row_lens_dev, int T,
                            const float* rope_cos_dev, const float* rope_sin_dev, int head_dim, int kv_heads,
                            long long kv_part_stride, long long kv_layer_stride, int M, int N, int K, void* stream);
+/* the CTC prefix scorer alone (CTCPrefixScore.forward_step + permute_mem, decoders/ctc.py:80-295), driven by a forced search
+ * history in the order the beam search runs it: reset, then per step s the state update of the survivors of step s - 1 and
+ * the full-vocabulary score.  logits_dev [B, T, V] fp32 ctc_lin output before log_softmax (copied, not modified);
+ * enc_len_dev [B] in [0, T]; hist_tok_dev / hist_pred_dev [n_steps, B * beam]: the token and GLOBAL parent row of every
+ * hypothesis after step s (the last row is not read).  scores_dev [n_steps, B * beam, V]: step s writes
+ * weight * (psi - psi_prev) for every extension of the prefixes given by history rows < s (accumulate != 0: added to what
+ * scores_dev holds).  group_width (may be NULL) receives the hypotheses per score CTA.  Allocates and frees its own
+ * buffers and synchronises the stream. */
+int sbk_ctc_prefix_test(const float* logits_dev, const int* enc_len_dev, int B, int T, int V, int beam, int blank, int bos,
+                        int eos, float weight, int accumulate, const int* hist_tok_dev, const int* hist_pred_dev, int n_steps,
+                        float* scores_dev, int* group_width, void* stream);
 
 /* ---- model handle: repacks the reference state_dict once */
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out);

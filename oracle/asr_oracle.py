@@ -705,6 +705,137 @@ def ctc_prefix_permute(st, memory, cand):
     return r_sel, psi_sel
 
 
+def ctc_prefix_scores(logits, enc_len, beam, blank, bos, eos, hist_tok, hist_pred, n_steps, minus_inf=-1e20, chunk=256,
+                      pick=None):
+    """The CTC prefix scorer along a forced search history, in float64: CTCPrefixScore.__init__ + n_steps x (forward_step,
+    permute_mem) (ctc.py:46-295), candidates = None.  Same inputs as the sbk_ctc_prefix_test hook: ``logits`` (B, T, V)
+    ctc_lin output before log_softmax, ``enc_len`` (B,) in [0, T], ``hist_tok`` / ``hist_pred`` (>= n_steps - 1, B * beam)
+    int tensors: token and global parent row of every hypothesis after each step.  With ``pick`` the history is chosen on
+    the way: ``pick(s, score_s, last_tokens)`` returns row s of (hist_tok, hist_pred), which are filled in place.
+
+    Unlike ctc_prefix_step it never materialises the (T, 2, n_bh, V) forward variables: psi(h, c) = logsumexp over frames
+    of phi_h[t - 1] + x[t, c] (Alg.2-13, plus the seed x[0, c] at step 0) is evaluated directly, token chunk by token chunk,
+    and the recurrence (Alg.2-11/12) runs only for the (parent, token) pairs the history keeps.  So it scales to T = 10240
+    and V = 5000.  It follows the reference's start = max(1, prefix_length), its padded frames (minus_inf everywhere but 0
+    in channel 0, ctc.py:59-62), its eos column r_sum[enc_len - 1] (a Python index: enc_len = 0 reads frame T - 1) and its
+    blank column.
+
+    Returns a dict of float64 tensors: ``score`` (n_steps, n_bh, V) = psi - psi_prev, ``psi`` (same shape), ``psi_prev``
+    (n_steps, n_bh), and ``low`` (n_steps, n_bh, V) bool: entries whose largest term lies more than 69 + log(T) nats below
+    the maximum of the phi variant it uses -- where a linear-domain sum of exp(phi - max) * exp(x) underflows fp32."""
+    x = torch.log_softmax(logits.double(), dim=-1)
+    B, T, V = x.shape
+    n_bh = B * beam
+    enc_len = enc_len.long()
+    pad = ~(torch.arange(T).unsqueeze(0) < enc_len.unsqueeze(1))
+    x = x.masked_fill(pad.unsqueeze(-1), minus_inf)
+    x[:, :, 0] = x[:, :, 0].masked_fill(pad, 0.0)
+    xb = x[:, :, blank]                                   # (B, T)
+    last_frame = torch.where(enc_len > 0, enc_len - 1, T - 1)
+    utt = torch.arange(n_bh) // beam
+    neg = torch.tensor(minus_inf, dtype=torch.float64)
+    # states = None (ctc.py:108-123)
+    r_nb = torch.full((n_bh, T), minus_inf, dtype=torch.float64)
+    r_b = torch.cumsum(xb, dim=1)[utt]
+    psi_prev = torch.zeros(n_bh, dtype=torch.float64)
+    score = torch.empty(n_steps, n_bh, V, dtype=torch.float64)
+    psi_all = torch.empty(n_steps, n_bh, V, dtype=torch.float64)
+    prev_all = torch.empty(n_steps, n_bh, dtype=torch.float64)
+    low = torch.zeros(n_steps, n_bh, V, dtype=torch.bool)
+    thr = -69.0 - math.log(T)
+    for s in range(n_steps):
+        last = torch.full((n_bh,), bos, dtype=torch.long) if s == 0 else hist_tok[s - 1].long()
+        r_sum = torch.logaddexp(r_nb, r_b)                # (n_bh, T)
+        start = max(1, s)
+        psi = torch.empty(n_bh, V, dtype=torch.float64)
+        for b in range(B):
+            rows = slice(b * beam, (b + 1) * beam)
+            for var, phi_all in ((0, r_sum), (1, r_b)):   # variant 1: phi = r_b for the row's last token (Alg.2-10)
+                phi = phi_all[rows, start - 1:T - 1]      # phi[t - 1] for t in [start, T)
+                m = phi.max(dim=1).values if phi.shape[1] else torch.full((beam,), -math.inf, dtype=torch.float64)
+                if s == 0:
+                    m = torch.maximum(m, torch.zeros_like(m))  # the seed term: phi = 0 before frame 0
+                for c0 in range(0, V, chunk):
+                    xc = x[b, start:, c0:c0 + chunk]      # (T - start, C)
+                    terms = phi.unsqueeze(2) + xc.unsqueeze(0)
+                    seed = x[b, 0, c0:c0 + chunk].expand(beam, -1) if s == 0 else neg.expand(beam, xc.shape[1])
+                    allt = torch.cat([terms, seed.unsqueeze(1)], dim=1)
+                    val = torch.logsumexp(allt, dim=1)
+                    if s == 0 or terms.shape[1]:          # largest term of the sum, relative to the variant's maximum
+                        top = allt.max(dim=1).values if s == 0 else terms.max(dim=1).values
+                        top = top - m.unsqueeze(1)
+                    else:                                  # no frame left: an empty sum
+                        top = torch.zeros_like(val)
+                    cols = torch.arange(c0, c0 + xc.shape[1])
+                    sel = (last[rows].unsqueeze(1) == cols.unsqueeze(0))
+                    if var == 0:
+                        psi[rows, c0:c0 + chunk] = val
+                        low[s, rows, c0:c0 + chunk] = top < thr
+                    else:
+                        psi[rows, c0:c0 + chunk] = torch.where(sel, val, psi[rows, c0:c0 + chunk])
+                        low[s, rows, c0:c0 + chunk] = torch.where(sel, top < thr, low[s, rows, c0:c0 + chunk])
+        psi[:, eos] = r_sum[torch.arange(n_bh), last_frame[utt]]   # Alg.2-3
+        if eos != blank:
+            psi[:, blank] = minus_inf
+        low[s, :, eos] = False
+        low[s, :, blank] = False
+        score[s] = psi - psi_prev.unsqueeze(1)
+        psi_all[s] = psi
+        prev_all[s] = psi_prev
+        if s + 1 == n_steps:
+            break
+        if pick is not None:
+            tok_s, par_s = pick(s, score[s], last)
+            hist_tok[s], hist_pred[s] = tok_s, par_s
+        # permute_mem: forward variables of the kept (parent, token) pairs only (Alg.2-11/12)
+        par, tok = hist_pred[s].long(), hist_tok[s].long()
+        bu = utt[par]
+        xn = x[bu, :, tok]                                # (n_bh, T)
+        phi = torch.where((tok == last[par]).unsqueeze(1), r_b[par], r_sum[par])
+        nb = torch.full((n_bh, T), minus_inf, dtype=torch.float64)
+        bl = torch.full((n_bh, T), minus_inf, dtype=torch.float64)
+        if s == 0:
+            nb[:, 0] = xn[:, 0]
+        xbu = xb[bu]
+        for t in range(start, T):
+            nb[:, t] = torch.logaddexp(nb[:, t - 1], phi[:, t - 1]) + xn[:, t]
+            bl[:, t] = torch.logaddexp(nb[:, t - 1], bl[:, t - 1]) + xbu[:, t]
+        r_nb, r_b = nb, bl
+        psi_prev = psi[par, tok]
+    return dict(score=score, psi=psi_all, psi_prev=prev_all, low=low, hist_tok=hist_tok, hist_pred=hist_pred)
+
+
+def ctc_history_picker(B, beam, V, blank, eos, seed):
+    """A ``pick`` for ctc_prefix_scores that makes search-like histories: parents drawn within each utterance with
+    replacement (some parents get several children, some none; slots 0 and 1 always share one), and tokens that cycle
+    through the parent's best-scoring token, the parent's own last token (phi = r_b, Alg.2-10) and a random token.
+    Never blank or eos (those end or void a prefix)."""
+    gen = torch.Generator().manual_seed(seed)
+    banned = torch.zeros(V, dtype=torch.bool)
+    banned[[blank, eos]] = True
+    allowed = (~banned).nonzero().squeeze(1)
+
+    def pick(s, score, last):
+        tok = torch.empty(B * beam, dtype=torch.int32)
+        par = torch.empty(B * beam, dtype=torch.int32)
+        for b in range(B):
+            loc = torch.randint(0, beam, (beam,), generator=gen)
+            if beam >= 2:
+                loc[1] = loc[0]
+            for k in range(beam):
+                p = b * beam + int(loc[k])
+                kind = (k + s) % 3
+                if kind == 1 and not banned[int(last[p])]:
+                    t = int(last[p])
+                elif kind == 0:
+                    t = int(score[p].masked_fill(banned, -math.inf).argmax())
+                else:
+                    t = int(allowed[torch.randint(0, allowed.numel(), (1,), generator=gen)])
+                tok[b * beam + k], par[b * beam + k] = t, p
+        return tok, par
+    return pick
+
+
 # --------------------------------------------------------------------------
 # TransformerLMRescorer.rescore_hyps (decoders/scorer.py:1793-1882) + RescorerBuilder.rescore (:2113-2162)
 # --------------------------------------------------------------------------

@@ -27,6 +27,10 @@ namespace {
 
 constexpr float CTC_NEG = -1e20f;  // CTCPrefixScore.minus_inf (ctc.py:54)
 
+// Frame of the eos column (Alg.2-3): the reference indexes r_sum with last_frame_index = enc_len - 1 as a Python index, so
+// enc_len = 0 reads the last frame T - 1 (never the element before the hypothesis' row).
+__device__ __forceinline__ int ctc_eos_frame(int enc_len, int T) { return enc_len > 0 ? enc_len - 1 : T - 1; }
+
 // log(exp(a) + exp(b))
 __device__ __forceinline__ float logaddexp_acc(float a, float b) {
     const float m = fmaxf(a, b);
@@ -182,7 +186,7 @@ __device__ __forceinline__ void ctc_emit(const CtcArgs& a, int row, int b, int c
                                          const float* rsum_row, float psi_prev) {
     float psi;
     if (c == a.blank && a.eos != a.blank) psi = CTC_NEG;
-    else if (c == a.eos) psi = rsum_row[a.enc_len[b] - 1];   // Alg.2-3
+    else if (c == a.eos) psi = rsum_row[ctc_eos_frame(a.enc_len[b], a.T)];   // Alg.2-3
     else if (acc > 1e-30f) psi = M + __logf(acc);
     else psi = ctc_psi_logdomain(a, b, c, step, phi_row);
     const float sc = a.weight * (psi - psi_prev);
@@ -309,9 +313,10 @@ __global__ void __launch_bounds__(CTC_THREADS) ctc_score_kernel(const CtcArgs a)
             old[q][h] = (a.accumulate && c < V) ? __ldcg(a.out + static_cast<size_t>(row0 + h) * V + c) : 0.0f;
     }
     float eos_psi[R], pprev[R];
+    const int t_eos = ctc_eos_frame(a.enc_len[b], T);
 #pragma unroll
     for (int h = 0; h < R; ++h) {
-        eos_psi[h] = rsum_in[static_cast<size_t>(row0 + h) * T + a.enc_len[b] - 1];   // Alg.2-3
+        eos_psi[h] = rsum_in[static_cast<size_t>(row0 + h) * T + t_eos];   // Alg.2-3
         pprev[h] = psi_prev[row0 + h];
     }
 #pragma unroll
@@ -401,7 +406,7 @@ __global__ void __launch_bounds__(128) ctc_update_kernel(const CtcArgs a) {
             s_nb[t] = nb; s_bl[t] = bl;
         }
         float psi = pm + logf(ps);
-        if (tok == a.eos) psi = rsum_in[static_cast<size_t>(prow) * T + a.enc_len[b] - 1];
+        if (tok == a.eos) psi = rsum_in[static_cast<size_t>(prow) * T + ctc_eos_frame(a.enc_len[b], T)];
         if (tok == a.blank && a.eos != a.blank) psi = CTC_NEG;
         psi_out[row] = psi;
     }
@@ -476,10 +481,19 @@ static int ctc_group_width(int beam, int T) {
     for (int w : widths) if (beam % w == 0 && w <= fit) return w;
     return 1;
 }
+int ctc_prefix_group_width(int beam, int T) { return ctc_group_width(beam, T); }
 
 int ctc_prefix_reset(float* x, float* xlin, float* xb, const int* enc_len, int B, int T, int V, int blank, int beam, float* rsum,
                      float* rb, float* psi_prev, float* tab, float* tabM, cudaStream_t stream) {
     SBK_REQUIRE(T >= 1 && T * 5 * 4 <= 200 * 1024, "ctc scorer: T=%d out of range", T);
+    // ctc_init (2 T floats) and ctc_update (5 T floats) exceed the default 48 KB of dynamic shared memory from T = 6145 and
+    // T = 2458 on; the reset runs before either is launched (the update is enqueued ahead of the score kernel in a step)
+    static bool attr = false;
+    if (!attr) {
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(ctc_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(ctc_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        attr = true;
+    }
     ctc_logsoftmax_mask_kernel<<<B * T, 256, 0, stream>>>(x, xlin, xb, enc_len, T, V, blank);
     SBK_LAUNCH_CHECK();
     ctc_init_kernel<<<B * beam, 128, 2 * T * 4, stream>>>(xb, T, beam, rsum, rb, psi_prev, tab, tabM, ctc_group_width(beam, T));
@@ -512,11 +526,6 @@ static int launch_score(const CtcArgs& a, cudaStream_t stream) {
 
 int ctc_prefix_score(const CtcStep& p, cudaStream_t stream) {
     const CtcArgs a = make_args(p, 0);   // runs before the beam kernel advances the step counters
-    static bool attr = false;
-    if (!attr) {
-        SBK_CUDA_CHECK(cudaFuncSetAttribute(ctc_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr = true;
-    }
     const int R = a.R;
     switch (R) {
         case 16: return launch_score<16>(a, stream);

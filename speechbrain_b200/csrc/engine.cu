@@ -1461,6 +1461,59 @@ int sbk_gemm_epilogue_test(const void* A_dev, const void* W_dev, const float* bi
     return gemm_f16(A_dev, K, W_dev, K, e, M, N, K, static_cast<cudaStream_t>(stream));
 }
 
+int sbk_ctc_prefix_test(const float* logits_dev, const int* enc_len_dev, int B, int T, int V, int beam, int blank, int bos,
+                        int eos, float weight, int accumulate, const int* hist_tok_dev, const int* hist_pred_dev, int n_steps,
+                        float* scores_dev, int* group_width, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(logits_dev && enc_len_dev && hist_tok_dev && hist_pred_dev && scores_dev, "ctc_prefix_test: null pointer");
+    SBK_REQUIRE(B >= 1 && T >= 1 && V >= 1 && beam >= 1 && n_steps >= 1, "ctc_prefix_test: bad sizes");
+    SBK_REQUIRE(blank >= 0 && blank < V && bos >= 0 && bos < V && eos >= 0 && eos < V, "ctc_prefix_test: bad token ids");
+    const int rows = B * beam;
+    // the kernels index frames, parents and token columns with these: check them on the host first
+    std::vector<int> len(B), tok((size_t)n_steps * rows), pred((size_t)n_steps * rows);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), enc_len_dev, B * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(tok.data(), hist_tok_dev, tok.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(pred.data(), hist_pred_dev, pred.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int v : len) SBK_REQUIRE(v >= 0 && v <= T, "ctc_prefix_test: enc_len %d outside [0, %d]", v, T);
+    for (size_t i = 0; i < tok.size(); ++i)
+        SBK_REQUIRE(tok[i] >= 0 && tok[i] < V && pred[i] >= 0 && pred[i] < rows, "ctc_prefix_test: history entry %zu out of range", i);
+    struct DevBufs {   // freed on every return path
+        std::vector<void*> p;
+        ~DevBufs() { for (void* q : p) cudaFree(q); }
+    } bufs;
+    auto alloc = [&](size_t n4, void** out) -> int {   // n4 4-byte elements
+        if (cudaMalloc(out, n4 * 4) != cudaSuccess) { set_error("ctc_prefix_test: cudaMalloc(%zu) failed", n4 * 4); return SBK_ERR_NOMEM; }
+        bufs.p.push_back(*out);
+        return SBK_OK;
+    };
+    const size_t M = (size_t)B * T;
+    float *x, *xlin, *xb, *rsum, *rb, *psi, *tab, *tabM;
+    int* steps;
+    RC(alloc(M * V, (void**)&x)); RC(alloc(M * V, (void**)&xlin)); RC(alloc(M, (void**)&xb));
+    RC(alloc((size_t)2 * rows * T, (void**)&rsum)); RC(alloc((size_t)2 * rows * T, (void**)&rb)); RC(alloc((size_t)2 * rows, (void**)&psi));
+    RC(alloc((size_t)2 * rows * (T + 4), (void**)&tab)); RC(alloc((size_t)2 * rows, (void**)&tabM));
+    RC(alloc((size_t)n_steps * rows, (void**)&steps));
+    std::vector<int> step_val((size_t)n_steps * rows);   // the beam search's per-row step counters, one row of them per step
+    for (size_t i = 0; i < step_val.size(); ++i) step_val[i] = static_cast<int>(i / rows);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(steps, step_val.data(), step_val.size() * 4, cudaMemcpyHostToDevice, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(x, logits_dev, M * V * 4, cudaMemcpyDeviceToDevice, st));
+    RC(ctc_prefix_reset(x, xlin, xb, enc_len_dev, B, T, V, blank, beam, rsum, rb, psi, tab, tabM, st));
+    CtcStep cs{};
+    cs.x = x; cs.xlin = xlin; cs.xb = xb; cs.enc_len = enc_len_dev; cs.hist_tok = hist_tok_dev; cs.hist_pred = hist_pred_dev;
+    cs.n_bh = rows; cs.rsum_base = rsum; cs.rb_base = rb; cs.psi_base = psi; cs.tab = tab; cs.tabM = tabM;
+    cs.bos = bos; cs.T = T; cs.V = V; cs.beam = beam; cs.blank = blank; cs.eos = eos; cs.weight = weight; cs.accumulate = accumulate ? 1 : 0;
+    for (int s = 0; s < n_steps; ++s) {   // run_beam's order: update of the previous survivors, then the score
+        cs.step_ptr = steps + (size_t)s * rows;
+        cs.out = scores_dev + (size_t)s * rows * V;
+        RC(ctc_prefix_update(cs, st));
+        RC(ctc_prefix_score(cs, st));
+    }
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    if (group_width) *group_width = ctc_prefix_group_width(beam, T);
+    return SBK_OK;
+}
+
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out) {
     return asr_create(cfg, weights, n_weights, reinterpret_cast<AsrModel**>(out));
 }

@@ -174,6 +174,7 @@ struct CtcStep {
 int ctc_prefix_reset(float* x, float* xlin, float* xb, const int* enc_len, int B, int T, int V, int blank, int beam, float* rsum,
                      float* rb, float* psi_prev, float* tab, float* tabM, cudaStream_t stream);
 int ctc_prefix_score(const CtcStep& p, cudaStream_t stream);
+int ctc_prefix_group_width(int beam, int T);   // hypotheses per score CTA (the R of ctc_score_kernel<R>)
 // x [rows, V] fp32: optional in-place log_softmax per row, arg-max per row -> idx (may be null)
 int rows_logsoftmax_argmax(float* x, int rows, int V, bool do_logsoftmax, int* idx, cudaStream_t stream);
 int ctc_prefix_update(const CtcStep& p, cudaStream_t stream);
