@@ -19,6 +19,7 @@ typedef struct sbk_asr sbk_asr;     /* opaque */
 
 enum { SBK_ATT_ROPE = 0, SBK_ATT_RELPOS = 1 };
 enum { SBK_ACT_RELU = 0, SBK_ACT_GELU = 1 };
+enum { SBK_ENC_CONFORMER = 0, SBK_ENC_BRANCHFORMER = 1 };
 enum { SBK_PART_FBANK = 1, SBK_PART_CNN = 2, SBK_PART_ENCODER = 4, SBK_PART_DECODER = 8, SBK_PART_ALL = 15, SBK_PART_LM = 16 };
 
 typedef struct {
@@ -43,6 +44,11 @@ typedef struct {
     /* Filterbank amin / top_db (processing/features.py:437-475) and InputNormalization epsilon (:1360-1455) of the fused
        wav -> features front end; 0 = the reference defaults (1e-10, 80 dB, 1e-10) */
     float fbank_amin, fbank_top_db, norm_eps;
+    /* TransformerASR encoder_module: SBK_ENC_CONFORMER (0, so a zeroed config stays a Conformer) or SBK_ENC_BRANCHFORMER
+       (Branchformer.py:92-234: RelPosMHAXL attention, no FFN modules, d_ffn only sizes the decoder) with the CSGU width
+       csgu_linear_units (even, csgu_linear_units / 2 % 8 == 0) and kernel_size the CSGU's odd depthwise kernel (<= 31);
+       branchformer_activation (SBK_ACT_RELU | SBK_ACT_GELU) follows pre_channel_proj */
+    int encoder_module, csgu_linear_units, branchformer_activation;
 } sbk_asr_config;
 
 typedef struct {
@@ -116,6 +122,13 @@ int sbk_gemm_epilogue_test(const void* A_dev, const void* W_dev, const float* bi
 int sbk_ctc_prefix_test(const float* logits_dev, const int* enc_len_dev, int B, int T, int V, int beam, int blank, int bos,
                         int eos, float weight, int accumulate, const int* hist_tok_dev, const int* hist_pred_dev, int n_steps,
                         float* scores_dev, int* group_width, void* stream);
+
+/* the Branchformer CSGU alone (ConvolutionalSpatialGatingUnit.forward, lobes/models/convolution.py:22-113, gate Identity):
+ * u_dev [B*T, C] fp16 -> out_dev [B*T, C/2] fp16 = u[:, :C/2] * (Conv1d_K(LayerNorm(u[:, C/2:])) + bias), the conv "same" with
+ * reflect padding inside the batch-padded T (T > (K-1)/2).  ln_g / ln_b [C/2], taps_dev in the reference layout [C/2, 1, K],
+ * bias [C/2] fp32; odd K <= 31, C/2 % 8 == 0.  Allocates and frees its own scratch and synchronises the stream. */
+int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev, const float* ln_b_dev, const float* taps_dev,
+                  const float* bias_dev, int K, void* out_dev, void* stream);
 
 /* ---- model handle: repacks the reference state_dict once */
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out);

@@ -23,7 +23,8 @@ class sbk_asr_config(ctypes.Structure):
         "n_fft", "hop", "n_mels", "cnn_c1", "cnn_c2", "input_size", "d_model", "nhead", "num_encoder_layers",
         "num_decoder_layers", "d_ffn", "vocab", "kernel_size", "attention_type", "decoder_activation", "max_len",
         "parts", "lm_d_model", "lm_nhead", "lm_layers", "lm_d_ffn", "lm_activation")] + [
-        (k, ctypes.c_float) for k in ("fbank_amin", "fbank_top_db", "norm_eps")]
+        (k, ctypes.c_float) for k in ("fbank_amin", "fbank_top_db", "norm_eps")] + [
+        (k, ctypes.c_int) for k in ("encoder_module", "csgu_linear_units", "branchformer_activation")]
 
 
 class sbk_beam_params(ctypes.Structure):
@@ -38,13 +39,14 @@ class sbk_beam_params(ctypes.Structure):
 
 SBK_ATT_ROPE, SBK_ATT_RELPOS = 0, 1
 SBK_ACT_RELU, SBK_ACT_GELU = 0, 1
+SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER = 0, 1
 SBK_PARTS = {"fbank": 1, "cnn": 2, "encoder": 4, "decoder": 8, "lm": 16}
 
 # every symbol include/sbk.h declares (tests check the library exports all of them)
 EXPORTS = [
     "sbk_last_error", "sbk_version", "sbk_launch_count", "sbk_gemm_profile_enable", "sbk_gemm_profile_read", "sbk_fbank_create", "sbk_fbank_destroy", "sbk_fbank_num_frames",
     "sbk_fbank_forward", "sbk_input_norm_global", "sbk_input_norm_sentence", "sbk_gemm_f16_test", "sbk_gemm_f16_resid_test",
-    "sbk_gemm_epilogue_test", "sbk_ctc_prefix_test",
+    "sbk_gemm_epilogue_test", "sbk_ctc_prefix_test", "sbk_csgu_test",
     "sbk_asr_create", "sbk_asr_destroy", "sbk_asr_num_frames", "sbk_asr_cnn_forward", "sbk_asr_encode_from_cnn",
     "sbk_asr_encode_feats", "sbk_asr_greedy_from_enc", "sbk_asr_transcribe_greedy_dev",
     "sbk_asr_transcribe_greedy_host", "sbk_asr_transcribe_greedy_host_async", "sbk_asr_clone",

@@ -14,12 +14,16 @@ namespace sbk {
 // --------------------------------------------------------------------------- LayerNorm
 // One warp per row, two-pass statistics in registers. D <= 32 * LN_MAX_PER_LANE.
 // PDL (decode step, launched with programmatic stream serialisation): gamma / beta are fetched before pdl_wait(), x after.
+// DUAL: a second fp16 output out2 = LN(x; gamma2, beta2) from the same statistics (the Branchformer layer's two pre-norms
+// norm_mhsa / norm_conv of the same x, Branchformer.py:204-221).
 constexpr int LN_MAX_PER_LANE = 32;
 
-template <bool OUT_HALF, bool PDL>
+template <bool OUT_HALF, bool PDL, bool DUAL = false>
 __global__ void __launch_bounds__(256)
 layernorm_rows_kernel(const float* __restrict__ x, void* __restrict__ out, const float* __restrict__ gamma,
-                      const float* __restrict__ beta, int M, int D, float eps, int act_silu) {
+                      const float* __restrict__ beta, int M, int D, float eps, int act_silu,
+                      __half* __restrict__ out2 = nullptr, const float* __restrict__ gamma2 = nullptr,
+                      const float* __restrict__ beta2 = nullptr) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     const int nv = D >> 2;  // float4 vectors per row (D % 4 == 0)
@@ -86,8 +90,29 @@ layernorm_rows_kernel(const float* __restrict__ x, void* __restrict__ out, const
                 *reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + static_cast<size_t>(row) * D + vi * 4) =
                     make_float4(y0, y1, y2, y3);
             }
+            if constexpr (DUAL) {
+                const float4 g2 = __ldg(reinterpret_cast<const float4*>(gamma2 + vi * 4));
+                const float4 b2 = __ldg(reinterpret_cast<const float4*>(beta2 + vi * 4));
+                __half2 h0 = floats2half2_sat((v[4 * i] - mean) * rstd * g2.x + b2.x, (v[4 * i + 1] - mean) * rstd * g2.y + b2.y);
+                __half2 h1 = floats2half2_sat((v[4 * i + 2] - mean) * rstd * g2.z + b2.z, (v[4 * i + 3] - mean) * rstd * g2.w + b2.w);
+                uint2 u;
+                u.x = *reinterpret_cast<uint32_t*>(&h0);
+                u.y = *reinterpret_cast<uint32_t*>(&h1);
+                *reinterpret_cast<uint2*>(out2 + static_cast<size_t>(row) * D + vi * 4) = u;
+            }
         }
     }
+}
+
+int layernorm_rows_dual(const float* x, __half* out, const float* gamma, const float* beta, __half* out2, const float* gamma2,
+                        const float* beta2, int M, int D, float eps, cudaStream_t stream) {
+    SBK_REQUIRE(D % 4 == 0 && D <= 32 * LN_MAX_PER_LANE, "layernorm_rows_dual: D=%d unsupported", D);
+    if (M == 0) return SBK_OK;
+    const int rows_per_cta = 8;
+    layernorm_rows_kernel<true, false, true><<<ceil_div(M, rows_per_cta), rows_per_cta * 32, 0, stream>>>(
+        x, out, gamma, beta, M, D, eps, 0, out2, gamma2, beta2);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
 }
 
 int layernorm_rows(const float* x, void* out, bool out_half, const float* gamma, const float* beta, int M, int D,
@@ -99,7 +124,8 @@ int layernorm_rows(const float* x, void* out, bool out_half, const float* gamma,
     if (pdl) {
         SBK_REQUIRE(out_half, "layernorm_rows: the PDL variant writes fp16");
         SBK_CUDA_CHECK(launch_pdl(layernorm_rows_kernel<true, true>, grid, block, 0, stream, true, x, out, gamma, beta, M, D,
-                                  eps, static_cast<int>(act_silu)));
+                                  eps, static_cast<int>(act_silu), static_cast<__half*>(nullptr),
+                                  static_cast<const float*>(nullptr), static_cast<const float*>(nullptr)));
     } else if (out_half) {
         layernorm_rows_kernel<true, false><<<grid, block, 0, stream>>>(x, out, gamma, beta, M, D, eps, act_silu);
     } else {
@@ -389,6 +415,149 @@ int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* w
     kern<<<dim3(ceil_div(T, DW_TT), B), 256, smem, stream>>>(glu, T, D, K, wdw, bdw, gamma, beta, eps, out, chunk);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
+}
+
+// --------------------------------------------------------------------------- CSGU (Branchformer convolution branch)
+// ConvolutionalSpatialGatingUnit.forward (lobes/models/convolution.py:22-113) on u = GELU(pre_channel_proj(x)) [B*T, C] fp16:
+//     a, b = u[:, :C/2], u[:, C/2:]          (x.chunk(2, dim=-1): the first half gates)
+//     g    = a * (dwconv_K(LN(b)) + bias)     (gate activation Identity, no linear after the conv)
+// The conv is speechbrain's Conv1d(padding="same"), padding_mode "reflect": (K-1)/2 frames on each side of the batch-padded
+// length T, mirrored about frames 0 and T-1 (so T > (K-1)/2).  Padded frames inside T are real inputs: the reference never
+// masks this branch (Branchformer.py:225).
+//   pass 1: fp32 LayerNorm statistics (mean, rstd) of b for every row, padded rows included;
+//   pass 2: one CTA per (CSGU_CC channels, CSGU_TT frames, utterance): the normalised halo'd b slab in shared memory (fp32),
+//           31 taps per output in registers, then a * (conv + bias) -> g fp16.
+// The taps arrive tap-major [CSGU_KMAX, C/2] with a kernel of K < CSGU_KMAX centred in zero rows, so every odd K <= 31
+// runs the same fully unrolled loop.
+constexpr int CSGU_KMAX = CSGU_TAP_ROWS, CSGU_HALO = (CSGU_KMAX - 1) / 2;
+constexpr int CSGU_TT = 64, CSGU_CC = 64, CSGU_THREADS = 256;
+constexpr int CSGU_FPT = CSGU_TT / (CSGU_THREADS / CSGU_CC);  // output frames per thread
+constexpr int CSGU_ROWS = CSGU_TT + CSGU_KMAX - 1;
+
+__global__ void __launch_bounds__(256)
+csgu_stats_kernel(const __half* __restrict__ u, int M, int C, float eps, float2* __restrict__ stats) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= M) return;
+    const int lane = threadIdx.x & 31, C2 = C >> 1, nv = C2 >> 3;
+    const uint4* src = reinterpret_cast<const uint4*>(u + static_cast<size_t>(row) * C + C2);
+    float s = 0.0f;
+    for (int j = lane; j < nv; j += 32) {
+        const uint4 w = __ldg(src + j);
+        const __half2* h = reinterpret_cast<const __half2*>(&w);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { const float2 f = __half22float2(h[q]); s += f.x + f.y; }
+    }
+    const float mean = warp_sum(s) / C2;
+    float v = 0.0f;  // second pass over the (L1-resident) row: exact two-pass variance, robust to large row means
+    for (int j = lane; j < nv; j += 32) {
+        const uint4 w = __ldg(src + j);
+        const __half2* h = reinterpret_cast<const __half2*>(&w);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const float2 f = __half22float2(h[q]);
+            v += (f.x - mean) * (f.x - mean) + (f.y - mean) * (f.y - mean);
+        }
+    }
+    const float rstd = rsqrtf(warp_sum(v) / C2 + eps);
+    if (lane == 0) stats[row] = make_float2(mean, rstd);
+}
+
+__global__ void __launch_bounds__(CSGU_THREADS)
+csgu_conv_gate_kernel(const __half* __restrict__ u, int T, int C, const float2* __restrict__ stats,
+                      const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ taps,
+                      const float* __restrict__ bias, __half* __restrict__ g) {
+    __shared__ __align__(16) float slab[CSGU_ROWS][CSGU_CC];  // slab row r = frame t0 - CSGU_HALO + r; rows [0, TT) reused for the outputs
+    const int C2 = C >> 1, c0 = blockIdx.x * CSGU_CC, t0 = blockIdx.y * CSGU_TT, b = blockIdx.z;
+    const size_t row0 = static_cast<size_t>(b) * T;
+    // normalised b slab: 8 channels (16 B) per load, reflect at the batch-padded edges
+    for (int i = threadIdx.x; i < CSGU_ROWS * (CSGU_CC / 8); i += CSGU_THREADS) {
+        const int r = i / (CSGU_CC / 8), j = (i % (CSGU_CC / 8)) * 8, ch = c0 + j;
+        int t = t0 - CSGU_HALO + r;
+        t = t < 0 ? -t : (t >= T ? 2 * (T - 1) - t : t);
+        t = min(max(t, 0), T - 1);  // rows only a zero tap (K < 31) or an output frame >= T reads
+        float y[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (ch < C2) {  // C/2 % 8 == 0: a vector lies entirely inside or outside the channels
+            const float2 st = __ldg(stats + row0 + t);
+            const uint4 w = __ldg(reinterpret_cast<const uint4*>(u + (row0 + t) * C + C2 + ch));
+            const __half2* h = reinterpret_cast<const __half2*>(&w);
+            const float4 ga = __ldg(reinterpret_cast<const float4*>(gamma + ch)), gb = __ldg(reinterpret_cast<const float4*>(gamma + ch + 4));
+            const float4 ba = __ldg(reinterpret_cast<const float4*>(beta + ch)), bb = __ldg(reinterpret_cast<const float4*>(beta + ch + 4));
+            const float gg[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
+            const float bt[8] = {ba.x, ba.y, ba.z, ba.w, bb.x, bb.y, bb.z, bb.w};
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const float2 f = __half22float2(h[q]);
+                y[2 * q] = (f.x - st.x) * st.y * gg[2 * q] + bt[2 * q];
+                y[2 * q + 1] = (f.y - st.x) * st.y * gg[2 * q + 1] + bt[2 * q + 1];
+            }
+        }
+        *reinterpret_cast<float4*>(&slab[r][j]) = make_float4(y[0], y[1], y[2], y[3]);
+        *reinterpret_cast<float4*>(&slab[r][j + 4]) = make_float4(y[4], y[5], y[6], y[7]);
+    }
+    // this thread: channel c0 + cl, output frames f0 .. f0 + CSGU_FPT - 1 of the tile
+    const int cl = threadIdx.x % CSGU_CC, f0 = (threadIdx.x / CSGU_CC) * CSGU_FPT, ch = c0 + cl;
+    float w[CSGU_KMAX], acc[CSGU_FPT];
+    const float bz = ch < C2 ? __ldg(bias + ch) : 0.0f;
+#pragma unroll
+    for (int k = 0; k < CSGU_KMAX; ++k) w[k] = ch < C2 ? __ldg(taps + static_cast<size_t>(k) * C2 + ch) : 0.0f;
+#pragma unroll
+    for (int i = 0; i < CSGU_FPT; ++i) acc[i] = bz;
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < CSGU_FPT + CSGU_KMAX - 1; ++r) {
+        const float xv = slab[f0 + r][cl];
+#pragma unroll
+        for (int i = 0; i < CSGU_FPT; ++i)
+            if (r - i >= 0 && r - i < CSGU_KMAX) acc[i] = fmaf(xv, w[r - i], acc[i]);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < CSGU_FPT; ++i) slab[f0 + i][cl] = acc[i];
+    __syncthreads();
+    // gate with a and store g: 8 channels per 16 B access
+    for (int i = threadIdx.x; i < CSGU_TT * (CSGU_CC / 8); i += CSGU_THREADS) {
+        const int r = i / (CSGU_CC / 8), j = (i % (CSGU_CC / 8)) * 8, t = t0 + r;
+        if (t >= T || c0 + j >= C2) continue;
+        const uint4 av = __ldg(reinterpret_cast<const uint4*>(u + (row0 + t) * C + c0 + j));
+        const __half2* ah = reinterpret_cast<const __half2*>(&av);
+        const float4 x0 = *reinterpret_cast<const float4*>(&slab[r][j]), x1 = *reinterpret_cast<const float4*>(&slab[r][j + 4]);
+        const float xs[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+        uint4 o;
+        uint32_t* op = reinterpret_cast<uint32_t*>(&o);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const float2 af = __half22float2(ah[q]);
+            __half2 hv = floats2half2_sat(af.x * xs[2 * q], af.y * xs[2 * q + 1]);
+            op[q] = *reinterpret_cast<uint32_t*>(&hv);
+        }
+        *reinterpret_cast<uint4*>(g + (row0 + t) * C2 + c0 + j) = o;
+    }
+}
+
+int csgu_forward(const __half* u, int B, int T, int C, const float* gamma, const float* beta, float eps, const float* taps,
+                 const float* bias, int K, float2* stats, __half* g, cudaStream_t stream) {
+    SBK_REQUIRE(C % 16 == 0, "csgu: csgu_linear_units=%d must be a multiple of 16 (C/2 %% 8 == 0)", C);
+    SBK_REQUIRE((K & 1) == 1 && K <= CSGU_KMAX, "csgu: kernel_size=%d must be odd and <= %d", K, CSGU_KMAX);
+    SBK_REQUIRE(T > (K - 1) / 2, "csgu: reflect padding needs T > (kernel_size - 1) / 2 (T=%d, kernel_size=%d)", T, K);
+    SBK_REQUIRE(B <= 65535, "csgu: B=%d", B);
+    SBK_REQUIRE(((reinterpret_cast<uintptr_t>(u) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(gamma) |
+                  reinterpret_cast<uintptr_t>(beta)) & 15) == 0, "csgu: operands must be 16-byte aligned");
+    const int M = B * T;
+    if (M == 0) return SBK_OK;
+    csgu_stats_kernel<<<ceil_div(M, 8), 256, 0, stream>>>(u, M, C, eps, stats);
+    SBK_LAUNCH_CHECK();
+    csgu_conv_gate_kernel<<<dim3(ceil_div(C / 2, CSGU_CC), ceil_div(T, CSGU_TT), B), CSGU_THREADS, 0, stream>>>(
+        u, T, C, stats, gamma, beta, taps, bias, g);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
+// (C/2, 1, K) reference taps -> tap-major [CSGU_KMAX, C/2], K centred (the layout csgu_forward reads)
+void csgu_repack_taps(const float* src, int C2, int K, float* dst) {
+    const int off = CSGU_HALO - (K - 1) / 2;
+    for (size_t i = 0; i < static_cast<size_t>(CSGU_KMAX) * C2; ++i) dst[i] = 0.0f;
+    for (int ch = 0; ch < C2; ++ch)
+        for (int k = 0; k < K; ++k) dst[static_cast<size_t>(k + off) * C2 + ch] = src[static_cast<size_t>(ch) * K + k];
 }
 
 // =========================================================================== self-attention

@@ -39,6 +39,12 @@ struct EncLayerW {
     const float *ffn2_ln_g, *ffn2_ln_b, *ffn2_b1, *ffn2_b2;
     const __half *ffn2_w1, *ffn2_w2;
     const float *norm2_g, *norm2_b;
+    // Branchformer layer (Branchformer.py:92-234; the attention uses norm1_g/b = norm_mhsa and wqkv / wo / bo / wpos / pos_u /
+    // pos_v above)
+    const float *nconv_g, *nconv_b;   // norm_conv
+    const __half *wpre, *wpost, *wmerge;  // pre_channel_proj [C, d], post_channel_proj [d, C/2], merge_proj [d, 2d]
+    const float *bpre, *bpost, *bmerge;
+    const float *csgu_ln_g, *csgu_ln_b, *csgu_taps, *csgu_bias;  // taps tap-major [CSGU_TAP_ROWS, C/2] (csgu_repack_taps)
 };
 
 struct DecLayerW {
@@ -114,6 +120,10 @@ struct AsrModel {
         __half *lx16, *lq16, *latt16, *lf16, *lh16, *lkc, *lvc;
         int* tok_cache;
         __half *act1, *a_in, *h16, *f16, *qkv16, *att16, *P16, *enc16, *ckv16, *kcache, *vcache, *dh16, *dq16, *datt16, *df16;
+        // Branchformer encoder only: norm_conv output [M, d], [attention | conv branch] [M, 2d], CSGU output [M, C/2], CSGU
+        // LayerNorm statistics [M]
+        __half *hc16, *cat16, *g16;
+        float2* csgu_stats;
     } b;
     cudaGraphExec_t step_graph = nullptr;
     int graph_rows = -1, graph_T = -1, graph_B = -1, graph_eos = -1, graph_S = -1;
@@ -203,6 +213,11 @@ struct Packer {
 static size_t weight_arena_bytes(const sbk_asr_config& c) {
     const size_t d = c.d_model, f = c.d_ffn;
     size_t enc = (size_t)c.num_encoder_layers * (4 * d * f + 3 * d * d + d * d + d * d + 2 * d * d + d * d) * 2;
+    if (c.encoder_module == SBK_ENC_BRANCHFORMER) {  // qkv, out, linear_pos, pre / post channel proj, merge (fp16) + CSGU taps
+        const size_t C = c.csgu_linear_units;
+        enc = (size_t)c.num_encoder_layers * ((3 * d * d + d * d + d * d + C * d + d * C / 2 + 2 * d * d) * 2 +
+                                              (size_t)CSGU_TAP_ROWS * C / 2 * 4 + (4 * C + 16 * d) * 4);
+    }
     size_t dec = (size_t)c.num_decoder_layers * (3 * d * d + d * d + 3 * d * d + d * d + 2 * d * f) * 2;
     size_t misc = (size_t)c.vocab * d * (4 + 2 + 2) + (size_t)c.max_len * d * (4 + 2) + (size_t)c.input_size * d * 2;
     size_t lm = 0;
@@ -225,6 +240,13 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
     SBK_REQUIRE(!((c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0) || (dh <= 64 && dh % 4 == 0 && d % 16 == 0),
                 "asr_create: decoder head_dim must be a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)", dh, d);
     SBK_REQUIRE(c.attention_type != SBK_ATT_ROPE || dh % 32 == 0, "asr_create: RoPEMHA needs head_dim %% 32 == 0");
+    SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER || c.encoder_module == SBK_ENC_BRANCHFORMER,
+                "asr_create: encoder_module %d (0 Conformer, 1 Branchformer)", c.encoder_module);
+    SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER ||
+                    (c.attention_type == SBK_ATT_RELPOS && c.csgu_linear_units > 0 && c.csgu_linear_units % 16 == 0 &&
+                     (K & 1) == 1 && K <= CSGU_TAP_ROWS),
+                "asr_create: the Branchformer needs RelPosMHAXL, csgu_linear_units / 2 %% 8 == 0 and an odd kernel_size <= %d "
+                "(got %d, %d)", CSGU_TAP_ROWS, c.csgu_linear_units, K);
     std::map<std::string, std::pair<const float*, int64_t>> w;
     for (int i = 0; i < n_weights; ++i) w[weights[i].name] = {weights[i].data, weights[i].numel};
 
@@ -281,7 +303,30 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
     m->w_in = p.f16("Transformer.custom_src_module.layers.0.w.weight", (int64_t)d * c.input_size);
     m->b_in = p.f32("Transformer.custom_src_module.layers.0.w.bias", d);
     m->enc.resize(c.num_encoder_layers);
-    for (int l = 0; l < c.num_encoder_layers && p.ok; ++l) {
+    for (int l = 0; l < c.num_encoder_layers && p.ok && c.encoder_module == SBK_ENC_BRANCHFORMER; ++l) {
+        const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".", cb = q + "convolution_branch.";
+        const int C = c.csgu_linear_units, C2 = C / 2;
+        EncLayerW& e = m->enc[l];
+        e.norm1_g = p.f32(q + "norm_mhsa.norm.weight", d); e.norm1_b = p.f32(q + "norm_mhsa.norm.bias", d);
+        e.nconv_g = p.f32(q + "norm_conv.norm.weight", d); e.nconv_b = p.f32(q + "norm_conv.norm.bias", d);
+        e.wqkv = p.f16(q + "mha_layer.in_proj_weight", (int64_t)3 * d * d);
+        e.wo = p.f16(q + "mha_layer.out_proj.weight", (int64_t)d * d); e.bo = p.f32(q + "mha_layer.out_proj.bias", d);
+        e.wpos = p.f16(q + "mha_layer.linear_pos.weight", (int64_t)d * d);
+        e.pos_u = p.f32(q + "mha_layer.pos_bias_u", d); e.pos_v = p.f32(q + "mha_layer.pos_bias_v", d);
+        e.wpre = p.f16(cb + "pre_channel_proj.weight", (int64_t)C * d); e.bpre = p.f32(cb + "pre_channel_proj.bias", C);
+        e.wpost = p.f16(cb + "post_channel_proj.weight", (int64_t)d * C2); e.bpost = p.f32(cb + "post_channel_proj.bias", d);
+        e.csgu_ln_g = p.f32(cb + "csgu.norm.norm.weight", C2); e.csgu_ln_b = p.f32(cb + "csgu.norm.norm.bias", C2);
+        {   // depthwise taps (C/2, 1, K) -> tap-major, K centred in CSGU_TAP_ROWS rows
+            const float* src = find(w, cb + "csgu.conv.conv.weight", (int64_t)C2 * K);
+            if (!src) { p.ok = false; break; }
+            std::vector<float> wt((size_t)CSGU_TAP_ROWS * C2);
+            csgu_repack_taps(src, C2, K, wt.data());
+            e.csgu_taps = p.f32_raw(wt.data(), wt.size());
+        }
+        e.csgu_bias = p.f32(cb + "csgu.conv.conv.bias", C2);
+        e.wmerge = p.f16(q + "merge_proj.weight", (int64_t)d * 2 * d); e.bmerge = p.f32(q + "merge_proj.bias", d);
+    }
+    for (int l = 0; l < c.num_encoder_layers && p.ok && c.encoder_module == SBK_ENC_CONFORMER; ++l) {
         const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".";
         EncLayerW& e = m->enc[l];
         e.ffn1_ln_g = p.f32(q + "ffn_module1.0.weight", d); e.ffn1_ln_b = p.f32(q + "ffn_module1.0.bias", d);
@@ -563,6 +608,8 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
     frames(c, L, &T0, &T1, &T2);
     const int F1 = (c.n_mels - 1) / 2 + 1;
     const size_t M = (size_t)B * T2, d = c.d_model, F = c.d_ffn, Ld = c.num_decoder_layers, S = steps + 1;
+    const bool bfm = c.encoder_module == SBK_ENC_BRANCHFORMER && m->has_enc;
+    const size_t Cu = bfm ? (size_t)c.csgu_linear_units : 0, Fu = std::max(F, Cu);  // f16 also holds the CSGU input u
     const size_t Md = (size_t)std::max(B, rows) * T2;  // encoder states / cross K,V of every utterance the decoder sees
     size_t need = 0;
     auto sz = [&](size_t bytes) { need += (bytes + 255) & ~size_t(255); };
@@ -570,7 +617,7 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
     sz((size_t)B * T1 * F1 * c.cnn_c1 * 4); sz(M * c.input_size * 4); sz((size_t)rows * d * 4);
     sz((size_t)rows * c.vocab * 4); sz((size_t)rows * S * 4);
     sz(B * 4); sz((size_t)std::max(B, rows) * 4); sz((size_t)rows * (S + 1) * 4); sz(rows * 4 + 64); sz(rows * 4); sz(64); sz((size_t)rows * S * 4); sz(B * 4);
-    sz((size_t)B * T1 * F1 * c.cnn_c1 * 2); sz(M * c.input_size * 2); sz(M * d * 2); sz(M * F * 2); sz(M * 3 * d * 2);
+    sz((size_t)B * T1 * F1 * c.cnn_c1 * 2); sz(M * c.input_size * 2); sz(M * d * 2); sz(M * Fu * 2); sz(M * 3 * d * 2);
     sz(M * d * 2); sz((size_t)T2 * d * 2); sz(Md * d * 2); sz(Md * Ld * 2 * d * 2);
     sz((size_t)Ld * rows * S * d * 2); sz((size_t)Ld * rows * S * d * 2);
     sz((size_t)rows * d * 2); sz((size_t)rows * d * 2); sz((size_t)rows * d * 2); sz((size_t)rows * F * 2);
@@ -582,6 +629,7 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
         sz(rows * dl * 2); sz(rows * dl * 2); sz(rows * dl * 2); sz(rows * Fl * 2); sz(rows * dl * 2);
         sz(Ll * rows * S * dl * 2); sz(Ll * rows * S * dl * 2); sz((size_t)rows * S * 4);
     }
+    if (bfm) { sz(M * d * 2); sz(M * 2 * d * 2); sz(M * Cu / 2 * 2); sz(M * 8); }
     need += 1 << 20;
     if (need > m->ws.cap) {
         if (m->ws.base) { cudaDeviceSynchronize(); cudaFree(m->ws.base); m->ws.base = nullptr; }
@@ -603,7 +651,7 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
     TAKE(utt_max, int, B * 4); TAKE(enc_len, int, (size_t)std::max(B, rows) * 4); TAKE(tokens, int, (size_t)rows * (S + 1) * 4); TAKE(step, int, rows * 4 + 64);
     TAKE(has_ended, int, rows * 4); TAKE(ended_count, int, 64); TAKE(pred, int, (size_t)rows * S * 4); TAKE(rel_len, float, B * 4);
     TAKE(act1, __half, (size_t)B * T1 * F1 * c.cnn_c1 * 2); TAKE(a_in, __half, M * c.input_size * 2); TAKE(h16, __half, M * d * 2);
-    TAKE(f16, __half, M * F * 2); TAKE(qkv16, __half, M * 3 * d * 2); TAKE(att16, __half, M * d * 2);
+    TAKE(f16, __half, M * Fu * 2); TAKE(qkv16, __half, M * 3 * d * 2); TAKE(att16, __half, M * d * 2);
     TAKE(P16, __half, (size_t)T2 * d * 2); TAKE(enc16, __half, Md * d * 2); TAKE(ckv16, __half, Md * Ld * 2 * d * 2);
     TAKE(kcache, __half, (size_t)Ld * rows * S * d * 2); TAKE(vcache, __half, (size_t)Ld * rows * S * d * 2);
     TAKE(dh16, __half, (size_t)rows * d * 2); TAKE(dq16, __half, (size_t)rows * d * 2); TAKE(datt16, __half, (size_t)rows * d * 2);
@@ -620,6 +668,11 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
         TAKE(lkc, __half, Ll * rows * S * dl * 2); TAKE(lvc, __half, Ll * rows * S * dl * 2); TAKE(tok_cache, int, (size_t)rows * S * 4);
         if (!b.tok_cache) { set_error("workspace carve failed (LM)"); return SBK_ERR_NOMEM; }
     }
+    if (bfm) {
+        TAKE(hc16, __half, M * d * 2); TAKE(cat16, __half, M * 2 * d * 2); TAKE(g16, __half, M * Cu / 2 * 2);
+        TAKE(csgu_stats, float2, M * 8);
+        if (!b.csgu_stats) { set_error("workspace carve failed (Branchformer)"); return SBK_ERR_NOMEM; }
+    }
     if (!b.df16 || !b.seq_scores || !b.lnout || !b.hist_lp) { set_error("workspace carve failed"); return SBK_ERR_NOMEM; }
 #undef TAKE
     m->wsB = B; m->wsL = L; m->ws_rows = rows; m->ws_steps = steps;
@@ -627,6 +680,44 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
 }
 
 #define RC(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
+
+// Branchformer layers (Branchformer.py:92-234, 330-410) on the fp32 residual stream b.x [B*T, d] -> enc_out = encoder.norm(x):
+//     x1 = RelPosMHAXL(norm_mhsa(x));  x2 = post_channel_proj(CSGU(act(pre_channel_proj(norm_conv(x)))))
+//     x  = x + merge_proj(cat[x1, x2])
+// Neither branch masks padded frames (the attention masks padded keys only).  x1 and x2 are written into the two column
+// halves of one [B*T, 2d] fp16 buffer so that merge_proj is one K = 2d GEMM with the residual epilogue.
+static int run_branchformer_layers(AsrModel* m, int B, int T, const int* enc_len, float* enc_out, cudaStream_t st) {
+    const sbk_asr_config& c = m->cfg;
+    AsrModel::Buf& b = m->b;
+    const int M = B * T, d = c.d_model, H = c.nhead, dh = d / H, C = c.csgu_linear_units;
+    SBK_REQUIRE(m->dyn_chunk == 0, "encode: the Branchformer has no chunked (DynChunkTrainConfig) mode");
+    const float att_scale = 1.0f / sqrtf((float)d);  // nnet/attention.py:521: 1/sqrt(embed_dim)
+    const int act = c.branchformer_activation == SBK_ACT_RELU ? ACT_RELU : ACT_GELU;
+    GemmEpilogue e;
+    for (int l = 0; l < c.num_encoder_layers; ++l) {
+        const EncLayerW& w = m->enc[l];
+        RC(layernorm_rows_dual(b.x, b.h16, w.norm1_g, w.norm1_b, b.hc16, w.nconv_g, w.nconv_b, M, d, 1e-5f, st));
+        // --- attention branch -> cat16[:, :d]
+        e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.qkv16; e.ldo = 3 * d;
+        RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
+        e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
+        RC(gemm_f16(m->relpos_pe, d, w.wpos, d, e, T, d, d, st));
+        RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, true, w.pos_u, w.pos_v, b.P16, d, att_scale, b.att16, d, st));
+        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bo; e.out = b.cat16; e.ldo = 2 * d;
+        RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
+        // --- convolution branch -> cat16[:, d:]
+        e = GemmEpilogue(); e.mode = EPI_F16; e.act = act; e.bias = w.bpre; e.out = b.f16; e.ldo = C;
+        RC(gemm_f16(b.hc16, d, w.wpre, d, e, M, C, d, st));
+        RC(csgu_forward(b.f16, B, T, C, w.csgu_ln_g, w.csgu_ln_b, 1e-5f, w.csgu_taps, w.csgu_bias, c.kernel_size, b.csgu_stats,
+                        b.g16, st));
+        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bpost; e.out = b.cat16 + d; e.ldo = 2 * d;
+        RC(gemm_f16(b.g16, C / 2, w.wpost, C / 2, e, M, d, C / 2, st));
+        // --- x += merge_proj(cat[x1, x2]): every row, padded frames included
+        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bmerge; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
+        RC(gemm_f16(b.cat16, 2 * d, w.wmerge, 2 * d, e, M, d, 2 * d, st));
+    }
+    return layernorm_rows(b.x, enc_out, false, m->enc_norm_g, m->enc_norm_b, M, d, 1e-6f, false, st);
+}
 
 // feats [B, T0, n_mels] fp32 (already normalised) -> enc_out fp32 [B, T2, d] (+ enc16). enc_len device int[B].
 static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int* enc_len, float* cnn_out_f,
@@ -638,12 +729,15 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
     SBK_REQUIRE(m->has_enc, "encode: this handle was created without encoder weights");
     SBK_REQUIRE(feats == nullptr || m->has_cnn, "encode: this handle was created without CNN weights");
     SBK_REQUIRE(T <= m->pos_len, "encode: %d frames exceed max_len=%d", T, m->pos_len);
+    SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER || T > (c.kernel_size - 1) / 2,
+                "encode: the Branchformer's reflect-padded conv needs more than %d frames (got %d)", (c.kernel_size - 1) / 2, T);
     if (feats != nullptr)
         RC(cnn_frontend_forward(feats, B, T0, c.n_mels, m->c1_w, m->c1_b, m->c1_g, m->c1_be, c.cnn_c1, m->c2_w, m->c2_b,
                                 m->c2_g, m->c2_be, c.cnn_c2, b.act1, nullptr, b.a_in, cnn_out_f, st));
     GemmEpilogue e;
     e.mode = EPI_F32; e.bias = m->b_in; e.out = b.x; e.ldo = d;
     RC(gemm_f16(b.a_in, c.input_size, m->w_in, c.input_size, e, M, d, c.input_size, st));
+    if (c.encoder_module == SBK_ENC_BRANCHFORMER) return run_branchformer_layers(m, B, T, enc_len, enc_out, st);
     const float att_scale = 1.0f / sqrtf((float)d);  // nnet/attention.py:521,1272: 1/sqrt(embed_dim), not head_dim
     for (int l = 0; l < c.num_encoder_layers; ++l) {
         const EncLayerW& w = m->enc[l];
@@ -1512,6 +1606,34 @@ int sbk_ctc_prefix_test(const float* logits_dev, const int* enc_len_dev, int B, 
     SBK_CUDA_CHECK(cudaStreamSynchronize(st));
     if (group_width) *group_width = ctc_prefix_group_width(beam, T);
     return SBK_OK;
+}
+
+int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev, const float* ln_b_dev, const float* taps_dev,
+                  const float* bias_dev, int K, void* out_dev, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(u_dev && ln_g_dev && ln_b_dev && taps_dev && bias_dev && out_dev, "csgu_test: null pointer");
+    SBK_REQUIRE(B >= 1 && T >= 1 && C >= 16 && C % 16 == 0 && K >= 1 && (K & 1) && K <= CSGU_TAP_ROWS,
+                "csgu_test: bad sizes B=%d T=%d C=%d K=%d", B, T, C, K);
+    const int C2 = C / 2;
+    std::vector<float> src((size_t)C2 * K), wt((size_t)CSGU_TAP_ROWS * C2);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(src.data(), taps_dev, src.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    csgu_repack_taps(src.data(), C2, K, wt.data());
+    float* taps = nullptr;
+    float2* stats = nullptr;
+    if (cudaMalloc(&taps, wt.size() * 4) != cudaSuccess || cudaMalloc(&stats, (size_t)B * T * 8) != cudaSuccess) {
+        cudaFree(taps);
+        set_error("csgu_test: cudaMalloc failed");
+        return SBK_ERR_NOMEM;
+    }
+    int rc = cudaMemcpyAsync(taps, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess ? SBK_OK : SBK_ERR_CUDA;
+    if (rc == SBK_OK)
+        rc = csgu_forward(static_cast<const __half*>(u_dev), B, T, C, ln_g_dev, ln_b_dev, 1e-5f, taps, bias_dev, K, stats,
+                          static_cast<__half*>(out_dev), st);
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("csgu_test: device error"); rc = SBK_ERR_CUDA; }
+    cudaFree(taps);
+    cudaFree(stats);
+    return rc;
 }
 
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out) {

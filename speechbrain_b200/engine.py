@@ -72,7 +72,8 @@ class FbankHandle:
 class AsrEngine:
     """One repacked model on one GPU.  ``cfg`` keys: n_fft, hop, win (samples), n_mels, cnn_channels, input_size,
     d_model, nhead, num_encoder_layers, num_decoder_layers, d_ffn, vocab, kernel_size, attention_type
-    ("RoPEMHA"|"RelPosMHAXL"), decoder_activation ("gelu"|"relu"), max_length.
+    ("RoPEMHA"|"RelPosMHAXL"), decoder_activation ("gelu"|"relu"), max_length; encoder_module ("conformer" (default) |
+    "branchformer") with csgu_linear_units and branchformer_activation ("gelu" (default) | "relu").
     ``state``: {reference key with recipe prefix: CPU fp32 tensor}."""
 
     def __init__(self, cfg, state, device="cuda", parts=("fbank", "cnn", "encoder", "decoder")):
@@ -91,6 +92,13 @@ class AsrEngine:
         c.attention_type = _lib.SBK_ATT_ROPE if att == "RoPEMHA" else _lib.SBK_ATT_RELPOS
         c.decoder_activation = _lib.SBK_ACT_GELU if cfg.get("decoder_activation", "gelu") == "gelu" else _lib.SBK_ACT_RELU
         c.max_len = cfg.get("max_length", 2500)
+        enc_module = cfg.get("encoder_module", "conformer")
+        if enc_module not in ("conformer", "branchformer"):
+            raise NotImplementedError(f"encoder_module={enc_module!r}: only conformer and branchformer are built")
+        if enc_module == "branchformer":
+            c.encoder_module, c.csgu_linear_units = _lib.SBK_ENC_BRANCHFORMER, cfg["csgu_linear_units"]
+            c.branchformer_activation = (_lib.SBK_ACT_GELU if cfg.get("branchformer_activation", "gelu") == "gelu"
+                                         else _lib.SBK_ACT_RELU)
         lm = cfg.get("lm")  # dict(d_model, nhead, num_encoder_layers, d_ffn, activation) of a TransformerLM scorer
         if lm is not None:
             c.lm_d_model, c.lm_nhead, c.lm_layers, c.lm_d_ffn = lm["d_model"], lm["nhead"], lm["num_encoder_layers"], lm["d_ffn"]

@@ -1,6 +1,7 @@
 """TransformerASR -- drop-in for speechbrain.lobes.models.transformer.TransformerASR.TransformerASR
-(TransformerASR.py:167-675) restricted to what the Conformer ASR recipes instantiate:
-encoder_module="conformer", attention_type in {"RoPEMHA", "RelPosMHAXL"}, normalize_before=True, causal=False.
+(TransformerASR.py:167-675) restricted to what the Conformer and Branchformer ASR recipes instantiate:
+encoder_module="conformer" with attention_type in {"RoPEMHA", "RelPosMHAXL"} and normalize_before=True, or
+encoder_module="branchformer" with attention_type="RelPosMHAXL" (Branchformer.py:92-410); causal=False.
 
 Same constructor kwargs, same state_dict keys (incl. the positional buffers), ``encode()`` on the sm_90a
 kernels.  ``decode()`` / ``forward()`` run teacher-forced on the KV-cached decoder step (the searchers in
@@ -43,17 +44,33 @@ class TransformerASR(torch.nn.Module):
         if causal is None:
             causal = True  # the reference warns and assumes True (TransformerASR.py:274-282)
         unsupported = []
-        if encoder_module != "conformer":
+        if encoder_module not in ("conformer", "branchformer"):
             unsupported.append(f"encoder_module={encoder_module!r}")
         if attention_type not in ("RoPEMHA", "RelPosMHAXL"):
             unsupported.append(f"attention_type={attention_type!r}")
+        bf_act = "gelu"
+        if encoder_module == "branchformer":
+            if attention_type != "RelPosMHAXL":
+                unsupported.append(f"Branchformer with attention_type={attention_type!r} (RelPosMHAXL only)")
+            name = getattr(branchformer_activation, "__name__", "GELU") if branchformer_activation is not None else "GELU"
+            if name not in ("GELU", "ReLU"):
+                unsupported.append(f"branchformer_activation={name} (GELU or ReLU)")
+            bf_act = "relu" if name == "ReLU" else "gelu"
+            if gate_activation is not None and getattr(gate_activation, "__name__", "") != "Identity":
+                unsupported.append("gate_activation other than Identity")
+            if use_linear_after_conv:
+                unsupported.append("use_linear_after_conv=True")
+            if kernel_size % 2 == 0 or kernel_size > 31:
+                unsupported.append(f"Branchformer kernel_size={kernel_size} (odd, <= 31)")
+            if csgu_linear_units % 2 or (csgu_linear_units // 2) % 8:
+                unsupported.append(f"csgu_linear_units={csgu_linear_units} (even, with csgu_linear_units / 2 a multiple of 8)")
         if causal:
             unsupported.append("causal=True (streaming / chunked masks)")
         if not bias:
             unsupported.append("bias=False")
         if output_hidden_states:
             unsupported.append("output_hidden_states=True")
-        if conformer_activation is not None and getattr(conformer_activation, "__name__", "") not in ("Swish", "SiLU"):
+        if encoder_module == "conformer" and conformer_activation is not None and getattr(conformer_activation, "__name__", "") not in ("Swish", "SiLU"):
             unsupported.append("conformer_activation other than Swish")
         if d_model % nhead or d_model // nhead not in (64, 36, 32):
             unsupported.append(f"head_dim={d_model // max(nhead, 1)} (64, 36 or 32)")
@@ -69,8 +86,10 @@ class TransformerASR(torch.nn.Module):
         self.num_encoder_layers, self.num_decoder_layers, self.d_ffn = num_encoder_layers, num_decoder_layers, d_ffn
         self.kernel_size, self.attention_type, self.max_length, self.causal = kernel_size, attention_type, max_length, causal
         self.positional_encoding_type = positional_encoding
+        self.encoder_module, self.csgu_linear_units, self.branchformer_activation = encoder_module, csgu_linear_units, bf_act
         build_param_tree(self, transformer_asr_shapes(tgt_vocab, input_size, d_model, nhead, num_encoder_layers,
-                                                      num_decoder_layers, d_ffn, kernel_size, attention_type), default_init)
+                                                      num_decoder_layers, d_ffn, kernel_size, attention_type, encoder_module,
+                                                      csgu_linear_units), default_init)
         # buffers the reference keeps in its state_dict (Transformer.py:150-163)
         if attention_type == "RelPosMHAXL":
             self.positional_encoding = _Node()
@@ -89,7 +108,9 @@ class TransformerASR(torch.nn.Module):
                     d_model=self.d_model, nhead=self.nhead, num_encoder_layers=self.num_encoder_layers,
                     num_decoder_layers=self.num_decoder_layers, d_ffn=self.d_ffn, vocab=self.tgt_vocab,
                     kernel_size=self.kernel_size, attention_type=self.attention_type,
-                    decoder_activation=self.decoder_activation, max_length=self.max_length)
+                    decoder_activation=self.decoder_activation, max_length=self.max_length,
+                    encoder_module=self.encoder_module, csgu_linear_units=self.csgu_linear_units,
+                    branchformer_activation=self.branchformer_activation)
 
     def prefixed_state(self, prefix="Transformer."):
         return {prefix + k: v for k, v in self.state_dict().items()}
@@ -123,11 +144,19 @@ class TransformerASR(torch.nn.Module):
         """src [B, T, F] or [B, T, F', C] -> encoder_out [B, T, d_model] (TransformerASR.py:475-544).
 
         ``dynchunktrain_config`` (a ``DynChunkTrainConfig``): chunked attention + Dynamic Chunk Convolution, i.e. the masked
-        evaluation mode whose outputs equal chunk-by-chunk streaming (TransformerASR.py:46-105, Conformer.py:190-313)."""
-        require_cuda(src, "TransformerASR.encode")
+        evaluation mode whose outputs equal chunk-by-chunk streaming (TransformerASR.py:46-105, Conformer.py:190-313).
+        The Branchformer has no such mode (an AssertionError, like Branchformer.py:369) and needs more than
+        (kernel_size - 1) / 2 frames: its reflect-padded CSGU convolution fails on shorter inputs in the reference."""
         if src.dim() == 4:
             bz, t, ch1, ch2 = src.shape
             src = src.reshape(bz, t, ch1 * ch2)
+        if self.encoder_module == "branchformer":
+            assert dynchunktrain_config is None, "Dynamic Chunk Training unsupported for this encoder"
+            halo = (self.kernel_size - 1) // 2
+            if src.shape[1] <= halo:
+                raise RuntimeError(f"TransformerASR.encode: the Branchformer's reflect padding ({halo} frames) needs more than "
+                                   f"{halo} frames, got {src.shape[1]}")
+        require_cuda(src, "TransformerASR.encode")
         if wav_len is not None and float(wav_len.max()) < 1.0 - 1e-6:
             # the reference builds its mask with width max(abs_len) and then fails to broadcast (dataio.py:836)
             raise ValueError("wav_len: the longest utterance must have relative length 1.0")
@@ -145,6 +174,8 @@ class TransformerASR(torch.nn.Module):
     # ------------------------------------------------------------------ streaming (TransformerASR.py:546-670)
     def make_streaming_context(self, dynchunktrain_config):
         """Streaming context for ``encode_streaming`` (TransformerASR.py:645-670)."""
+        if self.encoder_module == "branchformer":
+            raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
         if dynchunktrain_config is None or dynchunktrain_config.chunk_size <= 0:
             raise ValueError("make_streaming_context needs a DynChunkTrainConfig with chunk_size > 0")
         return TransformerASRStreamingContext(dynchunktrain_config)
@@ -158,6 +189,8 @@ class TransformerASR(torch.nn.Module):
         *inputs* seen so far in the context and re-runs that masked encode over the window the new chunk can depend on
         (12 layers x (left context + convolution halo); everything, for an infinite left context), returning the rows of the
         new chunk: the same values, at the cost of recomputing the window instead of reusing per-layer caches."""
+        if self.encoder_module == "branchformer":
+            raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
         require_cuda(src, "TransformerASR.encode_streaming")
         cfg = context.dynchunktrain_config
         if src.dim() == 4:

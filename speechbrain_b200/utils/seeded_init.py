@@ -77,6 +77,33 @@ CONFORMER_LARGE = dict(name="conformer_large", sample_rate=16000, n_fft=512, win
                        cnn_channels=(64, 32), input_size=640, d_model=512, nhead=8, num_encoder_layers=12,
                        num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="RoPEMHA",
                        decoder_activation="gelu", max_length=2500)
+def scale_csgu_conv(sd, tap_gain=1.4, bias_center=1.0):
+    """In place: the seeded depthwise taps of every ``csgu.conv.conv.weight`` (C/2, 1, K) rescaled to std tap_gain / sqrt(K)
+    and ``bias_center`` added to ``csgu.conv.conv.bias`` (the reference initialises it to ones, convolution.py:88).  With
+    the xavier-like seeded taps (std ~0.0065 at C/2 = 1536) the conv hardly changes the gate, so errors in its padding or
+    tap order would not show in the outputs."""
+    for k in list(sd):
+        if k.endswith("csgu.conv.conv.weight"):
+            w = sd[k]
+            xavier = math.sqrt(2.0 / (w.shape[1] * w.shape[2] + w.shape[0] * w.shape[2]))
+            sd[k] = w * (tap_gain / math.sqrt(w.shape[2]) / xavier)
+        elif k.endswith("csgu.conv.conv.bias"):
+            sd[k] = sd[k] + bias_center
+    return sd
+
+
+# recipes/LibriSpeech/ASR/transformer/hparams/branchformer_large.yaml (seq2seq + CTC, 18 Branchformer layers) and
+# recipes/LibriSpeech/ASR/CTC/hparams/branchformer_large.yaml (encoder-only, CTC over 31 characters)
+BRANCHFORMER_LARGE = dict(name="branchformer_large", sample_rate=16000, n_fft=512, win=512, hop=160, n_mels=80,
+                          cnn_channels=(64, 32), input_size=640, d_model=512, nhead=8, num_encoder_layers=18,
+                          num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="RelPosMHAXL",
+                          decoder_activation="gelu", max_length=2500, encoder_module="branchformer",
+                          csgu_linear_units=3072, branchformer_activation="gelu")
+BRANCHFORMER_CTC = dict(name="branchformer_ctc", sample_rate=16000, n_fft=512, win=400, hop=160, n_mels=80,
+                        cnn_channels=(64, 32), input_size=640, d_model=256, nhead=4, num_encoder_layers=18,
+                        num_decoder_layers=0, d_ffn=1024, vocab=31, kernel_size=31, attention_type="RelPosMHAXL",
+                        decoder_activation="gelu", max_length=2500, encoder_module="branchformer",
+                        csgu_linear_units=2400, branchformer_activation="gelu")
 CONFORMER_SMALL = dict(name="conformer_small", sample_rate=16000, n_fft=400, win=400, hop=160, n_mels=80,
                        cnn_channels=(64, 32), input_size=640, d_model=144, nhead=4, num_encoder_layers=12,
                        num_decoder_layers=4, d_ffn=1024, vocab=5000, kernel_size=31, attention_type="RelPosMHAXL",
