@@ -47,13 +47,11 @@ constexpr int SK_WARPS = 8;
 
 // UNR: k-steps whose loads are issued back to back; NT: 8-column tiles per CTA; VPL: LayerNorm-fused variant
 // when > 0, with K == 128 * VPL (each lane holds VPL float4 of each of its 4 rows).
-// MT: 16-row tiles per CTA (2 -> 32 rows, the single-batch case; 8 -> 128 rows when several batches are decoded
-// together, so W is streamed once per 128 rows instead of once per 32).
-template <int UNR, int NT, int VPL, int MT = 2>
-__global__ void __launch_bounds__(SK_WARPS * 32, ((VPL <= 4 && MT == 2) ? 2 : 1)) skinny_gemm_kernel(const SkinnyArgs a) {
+template <int UNR, int NT, int VPL>
+__global__ void __launch_bounds__(SK_WARPS * 32, (VPL <= 4 ? 2 : 1)) skinny_gemm_kernel(const SkinnyArgs a) {
     constexpr bool LN = VPL > 0;
+    constexpr int MT = 2;  // 16-row mma tiles per CTA
     constexpr int SK_ROWS = 16 * MT;
-    static_assert(!LN || MT == 2, "the LayerNorm-fused variant owns 32 rows per CTA");
     __shared__ float red[SK_WARPS][SK_ROWS][8 * NT + 1];
     extern __shared__ __align__(16) __half a_sm[];  // LN: [32][K + 8]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
@@ -233,14 +231,6 @@ int skinny_gemm(const SkinnyArgs& a, cudaStream_t stream) {
     if (a.n_rows == 0) return SBK_OK;
     cudaError_t e;
     const int ry = ceil_div(a.n_rows, 32);
-    if (a.X == nullptr && a.n_rows >= 96 && getenv("SBK_SKINNY_MT8") != nullptr) {  // 128-row tiles (64 fat CTAs), opt-in only
-        const dim3 grid(ceil_div(a.N, 8), ceil_div(a.n_rows, 128));
-        if (a.K <= 1024) e = launch_k(skinny_gemm_kernel<2, 1, 0, 8>, grid, dim3(SK_WARPS * 32), 0, stream, a);
-        else e = launch_k(skinny_gemm_kernel<4, 1, 0, 8>, grid, dim3(SK_WARPS * 32), 0, stream, a);
-        SBK_CUDA_CHECK(e);
-        SBK_LAUNCH_CHECK();
-        return SBK_OK;
-    }
     if (a.X != nullptr) {
         const size_t smem = static_cast<size_t>(32) * (a.K + 8) * 2;
         dim3 grid(ceil_div(a.N, 16), ry);
@@ -424,262 +414,6 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
     }
 }
 
-// Cross-attention variant: the (utterance, head) K and V tiles ([T][64] halfs each, T <= 256) are fetched by TWO 4-D TMA
-// loads into shared memory -- the whole 2 x 32 KB of a CTA is in flight at once without holding it in registers (the
-// register version keeps 128 KB per SM in flight and reached 57 % of the HBM peak), then the 4 warps run the same
-// 8-lanes-per-key q.k / p.V as above out of shared memory (a quarter-warp reads one 128-byte row: conflict-free).
-__global__ void __launch_bounds__(DA_WARPS * 32)
-dec_cross_attention_tma_kernel(const __grid_constant__ CUtensorMap tmap_kv, const DecAttnArgs a, int box_T) {
-    extern __shared__ __align__(128) uint8_t xa_smem[];
-    __shared__ uint64_t bar;
-    __shared__ float part_o[DA_WARPS][64];
-    __shared__ float part_m[DA_WARPS], part_l[DA_WARPS];
-    const __half* Ks = reinterpret_cast<const __half*>(xa_smem);
-    const __half* Vs = Ks + static_cast<size_t>(box_T) * 64;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int r = blockIdx.y, h = blockIdx.x;
-    const int blk = r / a.rows_per_block;
-    if (threadIdx.x == 0) {
-        mbar_init(&bar, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_arrive_expect_tx(&bar, static_cast<uint32_t>(box_T) * 256u);
-        tma_load_4d(const_cast<__half*>(Ks), &tmap_kv, &bar, 0, h, 0, blk);
-        tma_load_4d(const_cast<__half*>(Vs), &tmap_kv, &bar, 0, a.H + h, 0, blk);
-    }
-    const int n_keys = a.enc_len ? min(a.enc_len[blk], a.n_keys_fixed) : a.n_keys_fixed;
-    const int per = (n_keys + DA_WARPS - 1) / DA_WARPS;
-    const int kb = warp * per, ke = min(n_keys, kb + per);
-    const int gq = lane >> 3, dl = (lane & 7) * 8;
-    float qf[8];
-    {
-        const uint4 qv = *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * 64 + dl);
-        const __half2* q2 = reinterpret_cast<const __half2*>(&qv);
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const float2 f = __half22float2(q2[u]);
-            qf[2 * u] = f.x; qf[2 * u + 1] = f.y;
-        }
-    }
-    float m_run = -INFINITY, l_run = 0.0f;
-    float o[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) o[e] = 0.0f;
-    mbar_wait(&bar, 0);
-    for (int c0 = kb; c0 < ke; c0 += DA_CHUNK) {
-        float sc[DA_KPG];
-        float cm = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < DA_KPG; ++i) {
-            const int j = c0 + gq + 4 * i;
-            float dot = 0.0f;
-            if (j < ke) {
-                const uint4 kv = *reinterpret_cast<const uint4*>(Ks + static_cast<size_t>(j) * 64 + dl);
-                const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const float2 kf = __half22float2(k2[u]);
-                    dot = fmaf(kf.x, qf[2 * u], dot);
-                    dot = fmaf(kf.y, qf[2 * u + 1], dot);
-                }
-            }
-            dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-            dot += __shfl_xor_sync(0xffffffffu, dot, 2);
-            dot += __shfl_xor_sync(0xffffffffu, dot, 4);
-            sc[i] = j < ke ? dot : -INFINITY;
-            cm = fmaxf(cm, sc[i]);
-        }
-        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 8));
-        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 16));
-        const float m_new = fmaxf(m_run, cm);
-        const float alpha = (m_run == -INFINITY) ? 0.0f : __expf(m_run - m_new);
-        float psum = 0.0f;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] *= alpha;
-#pragma unroll
-        for (int i = 0; i < DA_KPG; ++i) {
-            const int j = c0 + gq + 4 * i;
-            const float p = (sc[i] == -INFINITY) ? 0.0f : __expf(sc[i] - m_new);
-            psum += p;
-            if (j < ke) {
-                const uint4 vv = *reinterpret_cast<const uint4*>(Vs + static_cast<size_t>(j) * 64 + dl);
-                const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const float2 vf = __half22float2(v2[u]);
-                    o[2 * u] = fmaf(p, vf.x, o[2 * u]);
-                    o[2 * u + 1] = fmaf(p, vf.y, o[2 * u + 1]);
-                }
-            }
-        }
-        psum += __shfl_xor_sync(0xffffffffu, psum, 8);
-        psum += __shfl_xor_sync(0xffffffffu, psum, 16);
-        l_run = l_run * alpha + psum;
-        m_run = m_new;
-    }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-        o[e] += __shfl_xor_sync(0xffffffffu, o[e], 8);
-        o[e] += __shfl_xor_sync(0xffffffffu, o[e], 16);
-    }
-    if (lane < 8) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) part_o[warp][dl + e] = o[e];
-    }
-    if (lane == 0) { part_m[warp] = m_run; part_l[warp] = l_run; }
-    __syncthreads();
-    if (threadIdx.x < 64) {
-        float M = part_m[0];
-#pragma unroll
-        for (int w = 1; w < DA_WARPS; ++w) M = fmaxf(M, part_m[w]);
-        float num = 0.0f, den = 0.0f;
-#pragma unroll
-        for (int w = 0; w < DA_WARPS; ++w) {
-            const float sc = part_m[w] == -INFINITY ? 0.0f : __expf(part_m[w] - M);
-            num += part_o[w][threadIdx.x] * sc;
-            den += part_l[w] * sc;
-        }
-        a.out[static_cast<size_t>(r) * a.ldo + h * 64 + threadIdx.x] = float2half_sat(num / den);
-    }
-}
-
-// Persistent, double-buffered cross-attention: one CTA per SM loops over (row, head) items; while the 8 warps work on
-// item i out of stage i & 1, the two TMA loads of item i + 1 are already in flight into the other stage, so HBM requests
-// are outstanding all the time (the one-shot kernels alternate load and compute phases and reach ~60 % of the copy
-// peak).  8 warps x one 32-key chunk cover T <= 256 frames.
-constexpr int XP_WARPS = 8;
-__global__ void __launch_bounds__(XP_WARPS * 32, 1)
-dec_cross_attention_persist_kernel(const __grid_constant__ CUtensorMap tmap_kv, const DecAttnArgs a, int box_T, int n_items) {
-    extern __shared__ __align__(128) uint8_t xp_smem[];
-    __shared__ uint64_t full[2];
-    __shared__ float part_o[XP_WARPS][64];
-    __shared__ float part_m[XP_WARPS], part_l[XP_WARPS];
-    const size_t stage_halfs = static_cast<size_t>(box_T) * 128;  // K [T][64] then V [T][64]
-    __half* stage0 = reinterpret_cast<__half*>(xp_smem);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int gq = lane >> 3, dl = (lane & 7) * 8;
-    const int H = a.H;
-    if (threadIdx.x == 0) {
-        mbar_init(&full[0], 1);
-        mbar_init(&full[1], 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
-    auto issue = [&](int item, int s) {  // thread 0 only
-        const int r = item / H, h = item - r * H, blk = r / a.rows_per_block;
-        __half* dst = stage0 + s * stage_halfs;
-        mbar_arrive_expect_tx(&full[s], static_cast<uint32_t>(box_T) * 256u);
-        tma_load_4d(dst, &tmap_kv, &full[s], 0, h, 0, blk);
-        tma_load_4d(dst + static_cast<size_t>(box_T) * 64, &tmap_kv, &full[s], 0, H + h, 0, blk);
-    };
-    const int first = blockIdx.x, stride = gridDim.x;
-    if (threadIdx.x == 0) {
-        if (first < n_items) issue(first, 0);
-        if (first + stride < n_items) issue(first + stride, 1);
-    }
-    auto load_q = [&](int item) {
-        const int r = item / H, h = item - r * H;
-        return *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * 64 + dl);
-    };
-    uint4 qv = make_uint4(0u, 0u, 0u, 0u);
-    if (first < n_items) qv = load_q(first);
-    int it = 0;
-    for (int item = first; item < n_items; item += stride, ++it) {
-        const int s = it & 1;
-        const int r = item / H, h = item - r * H, blk = r / a.rows_per_block;
-        float qf[8];
-        {
-            const __half2* q2 = reinterpret_cast<const __half2*>(&qv);
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const float2 f = __half22float2(q2[u]);
-                qf[2 * u] = f.x; qf[2 * u + 1] = f.y;
-            }
-        }
-        if (item + stride < n_items) qv = load_q(item + stride);  // next item's query while this one is computed
-        const int n_keys = a.enc_len ? min(a.enc_len[blk], a.n_keys_fixed) : a.n_keys_fixed;
-        const __half* Ks = stage0 + s * stage_halfs;
-        const __half* Vs = Ks + static_cast<size_t>(box_T) * 64;
-        mbar_wait(&full[s], (it >> 1) & 1);
-        const int c0 = warp * DA_CHUNK;
-        float sc[DA_KPG];
-        float cm = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < DA_KPG; ++i) {
-            const int j = c0 + gq + 4 * i;
-            float dot = 0.0f;
-            if (j < n_keys) {
-                const uint4 kv = *reinterpret_cast<const uint4*>(Ks + static_cast<size_t>(j) * 64 + dl);
-                const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const float2 kf = __half22float2(k2[u]);
-                    dot = fmaf(kf.x, qf[2 * u], dot);
-                    dot = fmaf(kf.y, qf[2 * u + 1], dot);
-                }
-            }
-            dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-            dot += __shfl_xor_sync(0xffffffffu, dot, 2);
-            dot += __shfl_xor_sync(0xffffffffu, dot, 4);
-            sc[i] = j < n_keys ? dot : -INFINITY;
-            cm = fmaxf(cm, sc[i]);
-        }
-        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 8));
-        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 16));
-        float o[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] = 0.0f;
-        float psum = 0.0f;
-#pragma unroll
-        for (int i = 0; i < DA_KPG; ++i) {
-            const int j = c0 + gq + 4 * i;
-            const float p = (sc[i] == -INFINITY) ? 0.0f : __expf(sc[i] - cm);
-            psum += p;
-            if (j < n_keys) {
-                const uint4 vv = *reinterpret_cast<const uint4*>(Vs + static_cast<size_t>(j) * 64 + dl);
-                const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const float2 vf = __half22float2(v2[u]);
-                    o[2 * u] = fmaf(p, vf.x, o[2 * u]);
-                    o[2 * u + 1] = fmaf(p, vf.y, o[2 * u + 1]);
-                }
-            }
-        }
-        psum += __shfl_xor_sync(0xffffffffu, psum, 8);
-        psum += __shfl_xor_sync(0xffffffffu, psum, 16);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            o[e] += __shfl_xor_sync(0xffffffffu, o[e], 8);
-            o[e] += __shfl_xor_sync(0xffffffffu, o[e], 16);
-        }
-        if (lane < 8) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) part_o[warp][dl + e] = o[e];
-        }
-        if (lane == 0) { part_m[warp] = cm; part_l[warp] = psum; }
-        __syncthreads();  // partials visible; every warp is done with stage s
-        if (threadIdx.x == 0 && item + 2 * stride < n_items) issue(item + 2 * stride, s);
-        if (threadIdx.x < 64) {
-            float M = part_m[0];
-#pragma unroll
-            for (int w = 1; w < XP_WARPS; ++w) M = fmaxf(M, part_m[w]);
-            float num = 0.0f, den = 0.0f;
-#pragma unroll
-            for (int w = 0; w < XP_WARPS; ++w) {
-                const float scl = part_m[w] == -INFINITY ? 0.0f : __expf(part_m[w] - M);
-                num += part_o[w][threadIdx.x] * scl;
-                den += part_l[w] * scl;
-            }
-            a.out[static_cast<size_t>(r) * a.ldo + h * 64 + threadIdx.x] = float2half_sat(num / den);
-        }
-        __syncthreads();  // partials consumed before the next item overwrites them
-    }
-}
-
-
 // Generic head_dim (<= 64, multiple of 4) variant of dec_attention_kernel: conformer_small's decoder has 4 heads of 36
 // (conformer_small.yaml).  One CTA (128 threads) per (row, head): thread-per-key scores into shared memory, block softmax,
 // then thread-per-dim p.V.  Small models only: no attempt at bandwidth efficiency.
@@ -761,47 +495,6 @@ int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t s
     if (n_rows == 0) return SBK_OK;
     DecAttnArgs b = a;
     b.n_keys_fixed = max_keys;
-    // cross-attention over an utterance's frames: optional TMA-staged variant (one box per (utterance, head), T <= 256).
-    // Opt-in only: bytes in flight are not what limits this kernel, so the register version stays the default.
-    static const bool xatt_tma = getenv("SBK_DEC_XATT_TMA") != nullptr;
-    if (a.n_keys_ptr == nullptr && a.lineage == nullptr && a.tok_cache == nullptr && max_keys <= 256 && xatt_tma &&
-        a.vbase == a.kbase + a.H * 64 && (n_rows % a.rows_per_block) == 0) {
-        CUtensorMap tm;
-        int rc = make_tmap_kv_f16(&tm, a.kbase, n_rows / a.rows_per_block, max_keys, a.H, a.key_stride, a.row_stride, max_keys);
-        if (rc) return rc;
-        const size_t smem = static_cast<size_t>(max_keys) * 256 + 128;
-        static bool attr = false;
-        if (!attr) {
-            SBK_CUDA_CHECK(cudaFuncSetAttribute(dec_cross_attention_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                256 * 256 + 128));
-            attr = true;
-        }
-        dec_cross_attention_tma_kernel<<<dim3(a.H, n_rows), DA_WARPS * 32, smem, stream>>>(tm, b, max_keys);
-        SBK_LAUNCH_CHECK();
-        return SBK_OK;
-    }
-    // persistent double-buffered TMA variant (opt-in only: with one 8-warp CTA per SM the two block barriers + merge per
-    // item cost about what the load/compute overlap wins)
-    static const bool xatt_persist = getenv("SBK_DEC_XATT_PERSIST") != nullptr;
-    if (a.n_keys_ptr == nullptr && a.lineage == nullptr && a.tok_cache == nullptr && max_keys <= 256 && xatt_persist &&
-        a.vbase == a.kbase + a.H * 64 && (n_rows % a.rows_per_block) == 0 && n_rows * a.H >= 4 * SBK_NUM_SMS) {
-        CUtensorMap tm;
-        int rc = make_tmap_kv_f16(&tm, a.kbase, n_rows / a.rows_per_block, max_keys, a.H, a.key_stride, a.row_stride, max_keys);
-        if (rc) return rc;
-        const size_t smem = static_cast<size_t>(max_keys) * 512 + 128;  // two stages of K + V
-        static int num_sms = 0;
-        if (num_sms == 0) {
-            int dev = 0;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-            SBK_CUDA_CHECK(cudaFuncSetAttribute(dec_cross_attention_persist_kernel,
-                                                cudaFuncAttributeMaxDynamicSharedMemorySize, 256 * 512 + 128));
-        }
-        const int n_items = n_rows * a.H;
-        dec_cross_attention_persist_kernel<<<std::min(num_sms, n_items), XP_WARPS * 32, smem, stream>>>(tm, b, max_keys, n_items);
-        SBK_LAUNCH_CHECK();
-        return SBK_OK;
-    }
     SBK_CUDA_CHECK(launch_k(dec_attention_kernel, dim3(a.H, n_rows), dim3(DA_WARPS * 32), 0, stream, b));
     SBK_LAUNCH_CHECK();
     return SBK_OK;

@@ -112,7 +112,7 @@ struct AsrModel {
     // shapes the workspace is carved for
     int wsB = 0, wsL = 0, ws_rows = 0, ws_steps = 0;
     struct Buf {
-        float *wav, *feats, *x, *glu, *enc_out, *act1_f, *cnn_f, *dx, *logits, *score, *seq_scores, *lnout, *beam_scr;
+        float *wav, *feats, *x, *glu, *enc_out, *dx, *logits, *score, *seq_scores, *lnout, *beam_scr;
         int *utt_max, *enc_len, *tokens, *step, *has_ended, *ended_count, *pred, *lineage, *finished, *hist_tok, *hist_pred;
         float *hist_score, *hist_lp;
         float* rel_len;
@@ -614,8 +614,7 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
     size_t need = 0;
     auto sz = [&](size_t bytes) { need += (bytes + 255) & ~size_t(255); };
     sz((size_t)B * L * 4); sz((size_t)B * T0 * c.n_mels * 4); sz(M * d * 4); sz(M * d * 4); sz(Md * d * 4);
-    sz((size_t)B * T1 * F1 * c.cnn_c1 * 4); sz(M * c.input_size * 4); sz((size_t)rows * d * 4);
-    sz((size_t)rows * c.vocab * 4); sz((size_t)rows * S * 4);
+    sz((size_t)rows * d * 4); sz((size_t)rows * c.vocab * 4); sz((size_t)rows * S * 4);
     sz(B * 4); sz((size_t)std::max(B, rows) * 4); sz((size_t)rows * (S + 1) * 4); sz(rows * 4 + 64); sz(rows * 4); sz(64); sz((size_t)rows * S * 4); sz(B * 4);
     sz((size_t)B * T1 * F1 * c.cnn_c1 * 2); sz(M * c.input_size * 2); sz(M * d * 2); sz(M * Fu * 2); sz(M * 3 * d * 2);
     sz(M * d * 2); sz((size_t)T2 * d * 2); sz(Md * d * 2); sz(Md * Ld * 2 * d * 2);
@@ -645,9 +644,8 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
     AsrModel::Buf& b = m->b;
 #define TAKE(field, type, bytes) b.field = reinterpret_cast<type*>(m->ws.take(bytes))
     TAKE(wav, float, (size_t)B * L * 4); TAKE(feats, float, (size_t)B * T0 * c.n_mels * 4); TAKE(x, float, M * d * 4);
-    TAKE(glu, float, M * d * 4); TAKE(enc_out, float, Md * d * 4); TAKE(act1_f, float, (size_t)B * T1 * F1 * c.cnn_c1 * 4);
-    TAKE(cnn_f, float, M * c.input_size * 4); TAKE(dx, float, (size_t)rows * d * 4); TAKE(logits, float, (size_t)rows * c.vocab * 4);
-    TAKE(score, float, (size_t)rows * S * 4);
+    TAKE(glu, float, M * d * 4); TAKE(enc_out, float, Md * d * 4); TAKE(dx, float, (size_t)rows * d * 4);
+    TAKE(logits, float, (size_t)rows * c.vocab * 4); TAKE(score, float, (size_t)rows * S * 4);
     TAKE(utt_max, int, B * 4); TAKE(enc_len, int, (size_t)std::max(B, rows) * 4); TAKE(tokens, int, (size_t)rows * (S + 1) * 4); TAKE(step, int, rows * 4 + 64);
     TAKE(has_ended, int, rows * 4); TAKE(ended_count, int, 64); TAKE(pred, int, (size_t)rows * S * 4); TAKE(rel_len, float, B * 4);
     TAKE(act1, __half, (size_t)B * T1 * F1 * c.cnn_c1 * 2); TAKE(a_in, __half, M * c.input_size * 2); TAKE(h16, __half, M * d * 2);
@@ -733,7 +731,7 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
                 "encode: the Branchformer's reflect-padded conv needs more than %d frames (got %d)", (c.kernel_size - 1) / 2, T);
     if (feats != nullptr)
         RC(cnn_frontend_forward(feats, B, T0, c.n_mels, m->c1_w, m->c1_b, m->c1_g, m->c1_be, c.cnn_c1, m->c2_w, m->c2_b,
-                                m->c2_g, m->c2_be, c.cnn_c2, b.act1, nullptr, b.a_in, cnn_out_f, st));
+                                m->c2_g, m->c2_be, c.cnn_c2, b.act1, b.a_in, cnn_out_f, st));
     GemmEpilogue e;
     e.mode = EPI_F32; e.bias = m->b_in; e.out = b.x; e.ldo = d;
     RC(gemm_f16(b.a_in, c.input_size, m->w_in, c.input_size, e, M, d, c.input_size, st));
@@ -812,14 +810,14 @@ static int dec_ln(AsrModel* m, SkinnyArgs& a, const float* g, const float* bta, 
 }
 
 // Decode step when many hypotheses are live (several batches decoded together, or a wide beam): the projections run on
-// the wgmma GEMM (128 x 32/64 tiles, a handful of CTAs each, so concurrent lanes share the GPU) instead of the
+// the wgmma GEMM (64 x 32/64 tiles, a handful of CTAs each, so concurrent lanes share the GPU) instead of the
 // weight-streaming kernel whose cost grows with every 32 rows.  Same maths: fp16 operands, fp32 accumulate / residual.
 // Cross-attention K/V of every decoder layer, projected once per utterance from the encoder states (b.enc16).  Layout per
 // layer (default): [K | V] parts, each [utt][head][T][64] -- the decode-step attention of (utterance, head) then streams one
 // contiguous T x 128 B block of K and one of V instead of 128-byte pieces 2 KB apart (SBK_XATT_ROWMAJOR=1: the round-1
 // [utt * T][K(d) | V(d)] rows).  Needs head_dim 64.
 static bool xatt_headmajor(const AsrModel* m) {
-    static const bool legacy = getenv("SBK_XATT_ROWMAJOR") != nullptr || getenv("SBK_GEMM_V1") != nullptr;  // (scatter epilogue: wide-tile kernel only)
+    static const bool legacy = getenv("SBK_XATT_ROWMAJOR") != nullptr;
     return !legacy && m->cfg.d_model / m->cfg.nhead == 64 && m->cfg.d_model % 256 == 0;
 }
 static int project_cross_kv(AsrModel* m, int M, int T, cudaStream_t st) {
@@ -903,9 +901,10 @@ static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int
 static bool decode_tc(const AsrModel* m, int rows) {
     return rows >= m->dec_tc_rows && m->cfg.d_model % 32 == 0;  // (the QKV -> cache scatter epilogue works on 32-column chunks)
 }
-// Programmatic dependent launch is always on for the wgmma decode path (its GEMMs and LayerNorms are launched with it
-// unconditionally); on the weight-streaming path it is opt-in (SBK_PDL=1), where it measured no faster.
-static void set_decode_pdl(const AsrModel* m, int rows) { set_pdl(decode_tc(m, rows) || getenv("SBK_PDL") != nullptr); }
+// Programmatic dependent launch is on for the wgmma decode path (its GEMMs and LayerNorms are launched with it
+// unconditionally) and off on the weight-streaming path, where it measured no faster (single_batch, H100 SXM at 400 W:
+// 24.8 / 28.2 ms with it against 23.4 / 23.3 ms without).
+static void set_decode_pdl(const AsrModel* m, int rows) { set_pdl(decode_tc(m, rows)); }
 
 static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage,
                                  cudaStream_t st, bool with_head = true) {
@@ -1685,7 +1684,7 @@ int sbk_asr_cnn_forward(sbk_asr* mm, const float* feats_dev, int B, int T0, floa
     const int L = (T0 - 1) * c.hop;
     RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
     return cnn_frontend_forward(feats_dev, B, T0, c.n_mels, m->c1_w, m->c1_b, m->c1_g, m->c1_be, c.cnn_c1, m->c2_w, m->c2_b,
-                                m->c2_g, m->c2_be, c.cnn_c2, m->b.act1, nullptr, m->b.a_in, out_dev,
+                                m->c2_g, m->c2_be, c.cnn_c2, m->b.act1, m->b.a_in, out_dev,
                                 static_cast<cudaStream_t>(stream));
 }
 

@@ -10,7 +10,7 @@
 //
 // Layout: wav [B, L] fp32 -> out [B, T_f, n_mels] fp32.  HBM-bound: 4*L + 4*T_f*n_mels bytes per utterance.
 //
-// Kernel 1 (fbank_tile_kernel): one CTA per (utterance, tile of FR frames).
+// Kernel 1 (fbank_tile_kernel): one CTA per (utterance, tile of FB_FRAMES frames).
 //   * the zero-padded wav segment is staged into shared memory by TMA (2-D tensor map over
 //     [B, L]; negative / past-the-end coordinates are zero-filled by the hardware, which is
 //     exactly torch.stft's center=True constant padding) -- or by guarded loads if L % 4 != 0;
@@ -20,7 +20,6 @@
 //     block-reduced atomicMax of the per-utterance maximum (ordered-int encoding).
 // Kernel 2 (fbank_finalize_kernel): x = max(x, max_b - top_db) [, (x - mean) / max(std, eps)].
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
@@ -34,8 +33,9 @@ namespace sbk {
 
 constexpr int FB_MAX_PASSES = 12;
 constexpr int FB_THREADS = 256;
-// frames per CTA (packed two per complex FFT) is a template parameter of the tile kernel: 8 frames = 42 KB of shared memory
-// = 4-5 CTAs per SM hide the kernel's many short barrier-separated phases better than 16 frames = 80 KB = 2 CTAs per SM
+// frames per CTA (packed two per complex FFT): 8 frames = 42 KB of shared memory = 4-5 CTAs per SM hide the kernel's many
+// short barrier-separated phases better than 16 frames = 80 KB = 2 CTAs per SM
+constexpr int FB_FRAMES = 8;
 
 struct FbankDev {
     int n_fft, hop, n_stft, n_mels, max_band;
@@ -134,7 +134,6 @@ __device__ __forceinline__ void stockham_pass(const float2* __restrict__ src, fl
     }
 }
 
-template <int FB_FRAMES>
 __global__ void __launch_bounds__(FB_THREADS)
 fbank_tile_kernel(const __grid_constant__ CUtensorMap wav_map, const float* __restrict__ wav, int use_tma, int B, int L,
                   int T_f, const FbankDev p, float* __restrict__ out, int* __restrict__ utt_max) {
@@ -389,21 +388,18 @@ int fbank_forward(const Fbank* fb, const float* wav, int B, int L, float* out, i
     const FbankDev& d = fb->d;
     SBK_REQUIRE(B > 0 && L > 0, "fbank_forward: empty input B=%d L=%d", B, L);
     const int T_f = 1 + L / d.hop;
-    static const int frames_per_cta = getenv("SBK_FBANK_FR16") != nullptr ? 16 : 8;
-    const int FR = frames_per_cta;
-    const int seg_len = (FR - 1) * d.hop + d.n_fft;
+    const int seg_len = (FB_FRAMES - 1) * d.hop + d.n_fft;
     const int seg_pad = (seg_len + 255) & ~255;
-    const size_t smem = static_cast<size_t>(seg_pad) * 4 + 2ull * (FR / 2) * d.n_fft * 8 + d.n_fft * 8ull;
+    const size_t smem = static_cast<size_t>(seg_pad) * 4 + 2ull * (FB_FRAMES / 2) * d.n_fft * 8 + d.n_fft * 8ull;
     SBK_REQUIRE(smem <= 200 * 1024, "fbank_forward: tile does not fit shared memory (hop=%d n_fft=%d)", d.hop, d.n_fft);
     CUtensorMap wmap;
     memset(&wmap, 0, sizeof(wmap));
     int use_tma = (L % 4 == 0) && ((reinterpret_cast<uintptr_t>(wav) & 15) == 0);
     if (use_tma && make_wav_map(&wmap, wav, B, L) != SBK_OK) use_tma = 0;
-    auto kern = FR == 16 ? fbank_tile_kernel<16> : fbank_tile_kernel<8>;
-    SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SBK_CUDA_CHECK(cudaFuncSetAttribute(fbank_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     fbank_init_max_kernel<<<ceil_div(B, 128), 128, 0, stream>>>(utt_max, B);
-    dim3 grid(ceil_div(T_f, FR), B);
-    kern<<<grid, FB_THREADS, smem, stream>>>(wmap, wav, use_tma, B, L, T_f, d, out, utt_max);
+    dim3 grid(ceil_div(T_f, FB_FRAMES), B);
+    fbank_tile_kernel<<<grid, FB_THREADS, smem, stream>>>(wmap, wav, use_tma, B, L, T_f, d, out, utt_max);
     SBK_LAUNCH_CHECK();
     const size_t total = static_cast<size_t>(B) * T_f * d.n_mels;
     const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, SBK_NUM_SMS * 8));

@@ -5,13 +5,11 @@
 // nnet/normalization.py:185-242 (LayerNorm over the last two dims), activation LeakyReLU(0.01).
 //
 // Layouts (channels-last, as the reference exposes them):
-//   feats [B, T0, F0] fp32 -> act1 [B, T1, F1, C1] fp16 (+ optional fp32) -> act2 [B, T2, F2*C2] fp16 (+ fp32)
+//   feats [B, T0, F0] fp32 -> act1 [B, T1, F1, C1] fp16 -> act2 [B, T2, F2*C2] fp16 (+ fp32)
 //   T1 = (T0-1)/2+1, F1 = (F0-1)/2+1, likewise T2/F2.
 // conv1 (C_in = 1) is HBM/latency bound: one CTA per output frame, fused LN + LeakyReLU.
 // conv2 (C1 -> C2, K = 9*C1 = 576) is an implicit GEMM on mma.sync.m16n8k16 (fp16 in, fp32 accumulate);
 // the weight matrix and a 9-frame input patch live in shared memory; LN + LeakyReLU fused.
-#include <stdlib.h>
-
 #include <algorithm>
 
 #include "common.cuh"
@@ -34,7 +32,7 @@ template <int C1, int MAXF>
 __global__ void __launch_bounds__(C1_WARPS * 32)
 conv1_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1, const float* __restrict__ w1,
                 const float* __restrict__ b1, const float* __restrict__ gamma, const float* __restrict__ beta,
-                __half* __restrict__ out_h, float* __restrict__ out_f) {
+                __half* __restrict__ out_h) {
     static_assert(C1 == 64, "two channels per lane");
     extern __shared__ float c1_smem[];
     const int FP = F0 + 2;
@@ -93,7 +91,6 @@ conv1_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1,
             const float y0 = leaky((va[f1] - mean) * rstd * g.x + be.x);
             const float y1 = leaky((vb[f1] - mean) * rstd * g.y + be.y);
             *reinterpret_cast<__half2*>(out_h + obase + gi) = floats2half2_sat(y0, y1);
-            if (out_f) *reinterpret_cast<float2*>(out_f + obase + gi) = make_float2(y0, y1);
         }
 }
 
@@ -383,17 +380,15 @@ cnn_fused_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1
 
 int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float* w1, const float* b1, const float* g1,
                          const float* be1, int C1, const __half* w2p, const float* b2, const float* g2,
-                         const float* be2, int C2, __half* act1_h, float* act1_f, __half* out_h, float* out_f,
-                         cudaStream_t stream) {
+                         const float* be2, int C2, __half* act1_h, __half* out_h, float* out_f, cudaStream_t stream) {
     SBK_REQUIRE(C1 == 64 && C2 == 32, "cnn_frontend: only out_channels=(64, 32) is built (got %d, %d)", C1, C2);
     SBK_REQUIRE(T0 >= 2 && F0 >= 2, "cnn_frontend: input too small for reflect padding");
     const int T1 = (T0 - 1) / 2 + 1, F1 = (F0 - 1) / 2 + 1;
     const int T2 = (T1 - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
     SBK_REQUIRE(F1 <= 64 && F2 * C2_FRAMES <= 96, "cnn_frontend: feature dim too large (F0=%d)", F0);
-    // default: the fused kernel (conv1 output never leaves the SM); SBK_CNN_UNFUSED=1 or a caller that wants conv1's output
-    // runs the two-kernel version
-    static const bool unfused = getenv("SBK_CNN_UNFUSED") != nullptr;
-    if (!unfused && act1_f == nullptr && F1 <= 40 && F1 >= 3 && C2_FRAMES * F2 <= 16 * CF_WARPS) {
+    // the fused kernel (conv1 output never leaves the SM) for 3 <= F1 <= 40: it holds a conv1 frame in 40 registers per lane
+    // and writes the reflect columns itself.  The two-kernel version otherwise (n_mels > 80, or n_mels <= 4).
+    if (F1 <= 40 && F1 >= 3 && C2_FRAMES * F2 <= 16 * CF_WARPS) {
         const size_t smem = static_cast<size_t>(CF_WARPS) * (F1 + 2) * C2_CELL * 2 + C2_COUT * C2_WROW * 2 +
                             static_cast<size_t>(C2_FRAMES) * F2 * 33 * 4 + static_cast<size_t>(CF_WARPS) * 3 * (F0 + 2) * 4;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(cnn_fused_kernel<40>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -405,10 +400,7 @@ int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float*
     {
         const size_t smem = static_cast<size_t>(C1_WARPS) * 3 * (F0 + 2) * sizeof(float);
         const dim3 grid(ceil_div(T1, C1_WARPS), B);
-        if (F1 <= 40)
-            conv1_ln_kernel<64, 40><<<grid, C1_WARPS * 32, smem, stream>>>(feats, T0, F0, T1, F1, w1, b1, g1, be1, act1_h, act1_f);
-        else
-            conv1_ln_kernel<64, 64><<<grid, C1_WARPS * 32, smem, stream>>>(feats, T0, F0, T1, F1, w1, b1, g1, be1, act1_h, act1_f);
+        conv1_ln_kernel<64, 64><<<grid, C1_WARPS * 32, smem, stream>>>(feats, T0, F0, T1, F1, w1, b1, g1, be1, act1_h);
         SBK_LAUNCH_CHECK();
     }
     {

@@ -66,12 +66,12 @@ __device__ __forceinline__ void wg_init(uint8_t* smem, const CUtensorMap* ta, co
     __syncthreads();
 }
 
-// producer warp: k-blocks kb0 .. kb0 + num_kb of rows m0 (A) and n0 (W).  The weights of the first min(STAGES, num_kb)
+// producer warp: the num_kb k-blocks of rows m0 (A) and n0 (W).  The weights of the first min(STAGES, num_kb)
 // k-blocks are requested before pdl_wait() -- they do not depend on the previous kernel -- and every A tile after it.
 // Each stage's full barrier still expects both loads' bytes.
 template <int BM, int BN, int STAGES>
 __device__ __forceinline__ void wg_produce(uint8_t* smem, const CUtensorMap* ta, const CUtensorMap* tb, int m0, int n0,
-                                           int kb0, int num_kb) {
+                                           int num_kb) {
     using R = WgRing<BM, BN, STAGES>;
     if (threadIdx.x != WgRoles<BM>::CONSUMERS) return;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + R::BAR_OFFSET);
@@ -79,7 +79,7 @@ __device__ __forceinline__ void wg_produce(uint8_t* smem, const CUtensorMap* ta,
     const int pre = num_kb < STAGES ? num_kb : STAGES;
     for (int kb = 0; kb < pre; ++kb) {  // first use of each stage: nothing to wait for
         mbar_arrive_expect_tx(&full_bar[kb], R::STAGE_BYTES);
-        tma_load_2d(smem + kb * R::STAGE_BYTES + R::A_BYTES, tb, &full_bar[kb], (kb0 + kb) * WG_BK, n0);
+        tma_load_2d(smem + kb * R::STAGE_BYTES + R::A_BYTES, tb, &full_bar[kb], kb * WG_BK, n0);
     }
     pdl_trigger();  // after this CTA's weight loads are in flight (measured faster than triggering at the top)
     pdl_wait();
@@ -89,9 +89,9 @@ __device__ __forceinline__ void wg_produce(uint8_t* smem, const CUtensorMap* ta,
         if (kb >= pre) {
             mbar_wait(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
             mbar_arrive_expect_tx(&full_bar[s], R::STAGE_BYTES);
-            tma_load_2d(a_dst + R::A_BYTES, tb, &full_bar[s], (kb0 + kb) * WG_BK, n0);
+            tma_load_2d(a_dst + R::A_BYTES, tb, &full_bar[s], kb * WG_BK, n0);
         }
-        tma_load_2d(a_dst, ta, &full_bar[s], (kb0 + kb) * WG_BK, m0);
+        tma_load_2d(a_dst, ta, &full_bar[s], kb * WG_BK, m0);
     }
 }
 

@@ -8,8 +8,6 @@
 // One BM x BN output tile per CTA (BM = 64 or 128; main loop: gemm_mainloop.cuh).  The epilogue runs row-wise on
 // 32-column chunks of the staged accumulator tile, so it handles any N and every epilogue mode, including partial column
 // chunks.  With BN <= 128 two CTAs fit per SM, so one CTA's epilogue overlaps the other's main loop.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
 #include "gemm_mainloop.cuh"
@@ -22,29 +20,7 @@ struct GemmSmem {
     static constexpr int TOTAL = WgRing<BM, BN, STAGES>::END + 1024;  // + alignment slack
 };
 
-// ---- split-K over a thread-block cluster (1, 1, SPLIT): CTA `rank` accumulates k-blocks [rank, rank+1) * num_kb / SPLIT,
-// rank 0 reads the other ranks' staged fp32 partial tiles out of their shared memory (DSMEM), adds them in rank order
-// (deterministic) and runs the epilogue.  For the decode-step GEMMs with K = d_ffn: one CTA would have to stream
-// 128 x K of activations through a single SM; four CTAs each stream a quarter.
-__device__ __forceinline__ uint32_t gemm_cluster_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void gemm_cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint4 ld_cluster_u4(uint32_t local_addr, uint32_t cta) {
-    uint32_t raddr;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(local_addr), "r"(cta));
-    uint4 v;
-    asm volatile("ld.shared::cluster.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(raddr)
-                 : "memory");
-    return v;
-}
-
-template <int BM, int BN, int STAGES, int SPLIT = 1>
+template <int BM, int BN, int STAGES>
 __global__ void __launch_bounds__(WgRoles<BM>::THREADS, (BN <= 128 ? 2 : 1))
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmEpilogue epi, int M, int N, int K) {
@@ -53,9 +29,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
-    const uint32_t rank = SPLIT > 1 ? gemm_cluster_rank() : 0u;
-    const int num_kb = (K + WG_BK - 1) / WG_BK / SPLIT;   // k-blocks of this CTA (host checks divisibility)
-    const int kb0 = static_cast<int>(rank) * num_kb;
+    const int num_kb = (K + WG_BK - 1) / WG_BK;
 
     // Before pdl_wait() (launched with programmatic stream serialisation, see common.cuh): barrier init, tensor-map
     // prefetch, the first stages' weight loads and the bias.  Activations, the residual, the step counter and every
@@ -63,9 +37,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     wg_init<BM, BN, STAGES>(smem, &tmap_a, &tmap_b);
     EpiPrefetch pre;
     if (threadIdx.x >= CONSUMERS) {
-        wg_produce<BM, BN, STAGES>(smem, &tmap_a, &tmap_b, m0, n0, kb0, num_kb);
+        wg_produce<BM, BN, STAGES>(smem, &tmap_a, &tmap_b, m0, n0, num_kb);
     } else {
-        constexpr bool prefetch = BN == 32 && SPLIT == 1;  // while the main loop runs
+        constexpr bool prefetch = BN == 32;  // while the main loop runs
         if constexpr (prefetch)
             if (threadIdx.x < BM) epilogue_prefetch_bias(epi, pre, m0 + threadIdx.x, n0, M, N);
         pdl_wait();  // the consumers' own: the producer's wait does not order this thread's reads and writes
@@ -73,34 +47,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
             if (threadIdx.x < BM) epilogue_prefetch_resid(epi, pre, m0 + threadIdx.x, n0);
         wg_consume_and_stage<BM, BN, STAGES>(smem, num_kb);
     }
-    if constexpr (SPLIT > 1) gemm_cluster_sync();  // every rank's partial tile is staged (release / acquire)
-    if (threadIdx.x < CONSUMERS && rank == 0) {
+    if (threadIdx.x < CONSUMERS) {
         const int r = threadIdx.x & (BM - 1);
 #pragma unroll 1
         for (int c = threadIdx.x / BM; c < BN / 32; c += CONSUMERS / BM) {
-            const uint32_t src = smem_u32(smem) + r * R::STG_PITCH + c * 128;
             uint32_t acc[32];
-            wg_load_row32(src, acc);
-#pragma unroll 1
-            for (int p = 1; p < SPLIT; ++p) {  // fixed order: deterministic sum
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const uint4 v = ld_cluster_u4(src + 16 * j, static_cast<uint32_t>(p));
-                    acc[4 * j] = __float_as_uint(__uint_as_float(acc[4 * j]) + __uint_as_float(v.x));
-                    acc[4 * j + 1] = __float_as_uint(__uint_as_float(acc[4 * j + 1]) + __uint_as_float(v.y));
-                    acc[4 * j + 2] = __float_as_uint(__uint_as_float(acc[4 * j + 2]) + __uint_as_float(v.z));
-                    acc[4 * j + 3] = __float_as_uint(__uint_as_float(acc[4 * j + 3]) + __uint_as_float(v.w));
-                }
-            }
+            wg_load_row32(smem_u32(smem) + r * R::STG_PITCH + c * 128, acc);
             epilogue_chunk(epi, acc, m0 + r, n0 + c * 32, M, N, pre);
         }
     }
-    if constexpr (SPLIT > 1) gemm_cluster_sync();  // the other ranks keep their shared memory until rank 0 has read it
 }
 
-// pdl: launch with programmatic stream serialisation (the decode-step projections; not the cluster split-K variant);
-// the kernel's pre-wait section obeys the rules of common.cuh either way.
-template <int BM, int BN, int STAGES, int SPLIT = 1>
+// pdl: launch with programmatic stream serialisation (the decode-step projections); the kernel's pre-wait section obeys
+// the rules of common.cuh either way.
+template <int BM, int BN, int STAGES>
 static int launch_gemm(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
                        cudaStream_t stream, bool pdl) {
     using S = GemmSmem<BM, BN, STAGES>;
@@ -109,9 +69,9 @@ static int launch_gemm(const void* A, int lda, const void* W, int ldw, const Gem
     if (rc) return rc;
     rc = make_tmap_2d_f16(&tb, W, N, K, ldw, BN, WG_BK);
     if (rc) return rc;
-    auto kern = gemm_tc_kernel<BM, BN, STAGES, SPLIT>;
+    auto kern = gemm_tc_kernel<BM, BN, STAGES>;
     SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    dim3 grid(ceil_div(N, BN), ceil_div(M, BM), SPLIT);
+    dim3 grid(ceil_div(N, BN), ceil_div(M, BM));
     GemmProfile* prof = gemm_profile();
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (prof->enabled) {
@@ -119,23 +79,7 @@ static int launch_gemm(const void* A, int lda, const void* W, int ldw, const Gem
         cudaEventCreate(&e1);
         cudaEventRecord(e0, stream);
     }
-    if constexpr (SPLIT == 1) {
-        SBK_CUDA_CHECK(launch_pdl(kern, grid, dim3(WgRoles<BM>::THREADS), S::TOTAL, stream, pdl, ta, tb, epi, M, N, K));
-    } else {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = grid;
-        cfg.blockDim = dim3(WgRoles<BM>::THREADS);
-        cfg.dynamicSmemBytes = S::TOTAL;
-        cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 1;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = SPLIT;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        SBK_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ta, tb, epi, M, N, K));
-    }
+    SBK_CUDA_CHECK(launch_pdl(kern, grid, dim3(WgRoles<BM>::THREADS), S::TOTAL, stream, pdl, ta, tb, epi, M, N, K));
     if (prof->enabled) {
         cudaEventRecord(e1, stream);
         prof->ev.push_back(e0);
@@ -162,11 +106,6 @@ int gemm_f16_small(const void* A, int lda, const void* W, int ldw, const GemmEpi
     // 64-row tiles (one consumer warpgroup): twice the CTAs of 128-row tiles, each streaming half the activations -- at
     // 96 - 224 rows they measured faster for every decode shape (FFN2 K = 2048 and the vocabulary head included).
     if (N > 2048) return launch_gemm<64, 64, 6>(A, lda, W, ldw, epi, M, N, K, stream, true);
-    // K = d_ffn: 4-way cluster split-K (deterministic DSMEM reduce) shortens that one kernel, but its 4x CTAs take SMs from
-    // the other lanes in flight -> opt-in
-    static const bool split = getenv("SBK_DEC_SPLITK") != nullptr;
-    if (K >= 2048 && K % (4 * WG_BK) == 0 && split)
-        return launch_gemm<128, 32, 8, 4>(A, lda, W, ldw, epi, M, N, K, stream, false);
     return launch_gemm<64, 32, 8>(A, lda, W, ldw, epi, M, N, K, stream, true);
 }
 
@@ -179,7 +118,7 @@ int gemm_f16(const void* A, int lda, const void* W, int ldw, const GemmEpilogue&
     if (epi.mode == EPI_GLU || epi.mode == EPI_ROPE)
         SBK_REQUIRE(N % 32 == 0, "gemm_f16: GLU/RoPE epilogues need N %% 32 == 0");
     if (epi.mode == EPI_ROPE) SBK_REQUIRE(epi.head_dim % 32 == 0, "gemm_f16: RoPE epilogue needs head_dim %% 32 == 0");
-    if (N % 256 == 0 && getenv("SBK_GEMM_V1") == nullptr) return gemm_f16_wide(A, lda, W, ldw, epi, M, N, K, stream);
+    if (N % 256 == 0) return gemm_f16_wide(A, lda, W, ldw, epi, M, N, K, stream);
     return launch_gemm<128, 128, 3>(A, lda, W, ldw, epi, M, N, K, stream, false);
 }
 

@@ -17,7 +17,6 @@
 //    only what the coalesced stores need, 16 rows x 32 columns at a time, in a per-warp buffer outside the ring.
 // The k-summation order of every output element is that of a plain k loop (no split-K), the same as gemm_tc.cu.
 #include <stdio.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "sbk_internal.h"
@@ -168,8 +167,7 @@ __device__ __forceinline__ void pp_epilogue_chunk(const GemmEpilogue& e, const f
             for (int i = 0; i < 2; ++i) {
 #pragma unroll
                 for (int c = 0; c < 2; ++c) {
-                    if constexpr (ACT == ACT_SILU) v[q][i][c] = silu_f(v[q][i][c]);
-                    else if constexpr (ACT == ACT_SILU_FAST) v[q][i][c] = silu_fast(v[q][i][c]);
+                    if constexpr (ACT == ACT_SILU_FAST) v[q][i][c] = silu_fast(v[q][i][c]);
                     else if constexpr (ACT == ACT_GELU) v[q][i][c] = gelu_erf_f(v[q][i][c]);
                     else if constexpr (ACT == ACT_RELU) v[q][i][c] = fmaxf(v[q][i][c], 0.0f);
                 }
@@ -183,8 +181,7 @@ __device__ __forceinline__ void pp_epilogue_chunk(const GemmEpilogue& e, const f
             for (int i = 0; i < 2; ++i) {
                 float o[2];
 #pragma unroll
-                for (int c = 0; c < 2; ++c)
-                    o[c] = ACT == ACT_SILU_FAST ? v[q][i][c] * sigmoid_fast(v[q + 2][i][c]) : v[q][i][c] * sigmoid_f(v[q + 2][i][c]);
+                for (int c = 0; c < 2; ++c) o[c] = v[q][i][c] * sigmoid_fast(v[q + 2][i][c]);
                 sts64(stg + (r0 + 8 * i) * P + (8 * q + qc) * 4, o[0], o[1]);
             }
     } else {  // EPI_F32, EPI_RESID (alpha-scaled; the residual is added in the store phase), EPI_ROPE (rotated there)
@@ -406,18 +403,19 @@ gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
 }
 
 using WideKernel = void (*)(const CUtensorMap, const CUtensorMap, const GemmEpilogue, int, int, int);
+// SiLU and the GLU gate's sigmoid: one tanh.approx MUFU per element
 template <int BN>
-static WideKernel pick_wide_kernel(const GemmEpilogue& epi, bool fast_act) {
+static WideKernel pick_wide_kernel(const GemmEpilogue& epi) {
     switch (epi.mode) {
         case EPI_F16:
-            if (epi.act == ACT_SILU) return fast_act ? gemm_tc2_kernel<EPI_F16, ACT_SILU_FAST, BN> : gemm_tc2_kernel<EPI_F16, ACT_SILU, BN>;
+            if (epi.act == ACT_SILU) return gemm_tc2_kernel<EPI_F16, ACT_SILU_FAST, BN>;
             if (epi.act == ACT_GELU) return gemm_tc2_kernel<EPI_F16, ACT_GELU, BN>;
             if (epi.act == ACT_RELU) return gemm_tc2_kernel<EPI_F16, ACT_RELU, BN>;  // ReLU TransformerLM FFN
             if (epi.act == ACT_NONE) return gemm_tc2_kernel<EPI_F16, ACT_NONE, BN>;
             return nullptr;
         case EPI_F32: return gemm_tc2_kernel<EPI_F32, ACT_NONE, BN>;
         case EPI_RESID: return gemm_tc2_kernel<EPI_RESID, ACT_NONE, BN>;
-        case EPI_GLU: return fast_act ? gemm_tc2_kernel<EPI_GLU, ACT_SILU_FAST, BN> : gemm_tc2_kernel<EPI_GLU, ACT_NONE, BN>;
+        case EPI_GLU: return gemm_tc2_kernel<EPI_GLU, ACT_SILU_FAST, BN>;
         case EPI_ROPE: return gemm_tc2_kernel<EPI_ROPE, ACT_NONE, BN>;
         default: return nullptr;
     }
@@ -436,9 +434,7 @@ int gemm_f16_wide(const void* A, int lda, const void* W, int ldw, const GemmEpil
     if (rc) return rc;
     rc = make_tmap_2d_f16(&tb, W, N, K, ldw, bn, PP_BK);
     if (rc) return rc;
-    // SiLU / GLU-gate sigmoid through one tanh.approx MUFU per element (default) or the exact-form EX2 + RCP (SBK_SILU_EXACT=1)
-    static const bool fast_act = getenv("SBK_SILU_EXACT") == nullptr;
-    const WideKernel kern = bn == 128 ? pick_wide_kernel<128>(epi, fast_act) : pick_wide_kernel<256>(epi, fast_act);
+    const WideKernel kern = bn == 128 ? pick_wide_kernel<128>(epi) : pick_wide_kernel<256>(epi);
     if (kern == nullptr) { set_error("gemm_f16_wide: epilogue mode %d / activation %d not built", epi.mode, epi.act); return SBK_ERR_ARG; }
     const int smem = bn == 128 ? PpCfg<128>::SMEM : PpCfg<256>::SMEM;
     SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

@@ -37,7 +37,7 @@ struct GemmEpilogue {
 // out = epilogue(A[M,K] fp16 x W[N,K]^T fp16), wgmma tensor cores. gemm_tc.cu
 int gemm_f16(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
              cudaStream_t stream);
-// Small-M variant for the decode steps of several batches (M = live hypotheses, 64..512): 128 x 32/64 tiles, deep TMA
+// Small-M variant for the decode steps of several batches (M = live hypotheses, 64..512): 64 x 32/64 tiles, deep TMA
 // ring; any epilogue mode incl. EPI_QKV_CACHE. gemm_tc.cu
 int gemm_f16_small(const void* A, int lda, const void* W, int ldw, const GemmEpilogue& epi, int M, int N, int K,
                    cudaStream_t stream);
@@ -77,8 +77,7 @@ int sentence_norm_forward(const float* x, float* out, const float* rel_len, int 
 // ---- frontend.cu
 int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float* w1, const float* b1, const float* g1,
                          const float* be1, int C1, const __half* w2p, const float* b2, const float* g2,
-                         const float* be2, int C2, __half* act1_h, float* act1_f, __half* out_h, float* out_f,
-                         cudaStream_t stream);
+                         const float* be2, int C2, __half* act1_h, __half* out_h, float* out_f, cudaStream_t stream);
 
 // ---- encoder_ops.cu
 // pdl: launched with programmatic stream serialisation (fp16 output only; the decode step's pre-norms)
@@ -141,8 +140,6 @@ struct DecAttnArgs {
     const int* tok_cache; int pad_tok;   // LM pad mask: keys whose token (tok_cache[phys_row][pos]) == pad_tok are masked
 };
 int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t stream);
-int make_tmap_kv_f16(CUtensorMap* out, const void* base, int n_utt, int T, int H, uint64_t key_stride_elems,
-                     uint64_t utt_stride_elems, int box_T);
 struct BeamLm {  // TransformerLM scorer state the beam step feeds (all null/0 when there is no LM)
     const float* emb = nullptr; const float* pe = nullptr; int d = 0;
     float* x = nullptr; __half* x16 = nullptr; int* tok_cache = nullptr;

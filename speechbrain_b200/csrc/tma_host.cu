@@ -69,31 +69,6 @@ int make_tmap_2d_f16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t
     return SBK_OK;
 }
 
-
-// Cross-attention K/V of one decoder layer: fp16 [n_utt][T][2 * H * 64] (K heads then V heads per frame) seen as the 4-D
-// tensor (64 | 2H slots | T | n_utt); one box = one head's K (or V) for all T frames of one utterance, landing densely
-// as [T][64] halfs in shared memory (no swizzle).
-int make_tmap_kv_f16(CUtensorMap* out, const void* base, int n_utt, int T, int H, uint64_t key_stride_elems,
-                     uint64_t utt_stride_elems, int box_T) {
-    auto fn = get_encode_fn();
-    if (!fn) {
-        set_error("cuTensorMapEncodeTiled driver entry point unavailable (no CUDA driver?)");
-        return SBK_ERR_CUDA;
-    }
-    cuuint64_t gdim[4] = {64, static_cast<cuuint64_t>(2 * H), static_cast<cuuint64_t>(T), static_cast<cuuint64_t>(n_utt)};
-    cuuint64_t gstride[3] = {128, key_stride_elems * 2, utt_stride_elems * 2};  // bytes, dims 1..3
-    cuuint32_t box[4] = {64, 1, static_cast<cuuint32_t>(box_T), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), gdim, gstride, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled(kv) failed (%d) n_utt=%d T=%d H=%d", (int)r, n_utt, T, H);
-        return SBK_ERR_CUDA;
-    }
-    return SBK_OK;
-}
-
 // fp32 [rows, cols] row-major, box [1, box_cols], no swizzle; OOB (incl. negative coords) reads 0.
 int make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint32_t box_cols) {
     auto fn = get_encode_fn();

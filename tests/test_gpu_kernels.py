@@ -199,6 +199,27 @@ def test_model_stages_golden(dev, tag):
         print(f"[{tag}] greedy[{name}] tokens {pred.tolist()} ref {g['hyps']} max log-prob err {worst:.2e}")
 
 
+@pytest.mark.parametrize("n_mels", [90, 96, 4])
+def test_cnn_frontend_two_kernel_golden(dev, n_mels):
+    """ConvolutionFrontEnd at feature widths the fused front-end kernel does not take (n_mels 81-96: F1 > 40; n_mels <= 4:
+    F1 < 3), which run conv1_ln_kernel + conv2_ln_kernel, vs the CPU oracle.  Same bar as the CNN check of
+    test_model_stages_golden."""
+    from oracle import asr_oracle as O
+    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
+    from speechbrain_b200.utils.seeded_init import seeded_state_dict
+    cnn = ConvolutionFrontEnd(input_shape=(8, 10, n_mels), num_blocks=2, num_layers_per_block=1, out_channels=(64, 32),
+                              kernel_sizes=(3, 3), strides=(2, 2), residuals=(False, False))
+    sd = seeded_state_dict(cnn, 0)
+    cnn.load_state_dict(sd)
+    x = torch.randn(2, 151, n_mels, generator=torch.Generator().manual_seed(n_mels))
+    out = cnn(x.to(dev)).cpu()
+    ref = O.cnn_frontend(x, sd)
+    assert out.shape == ref.shape, (out.shape, ref.shape)
+    e = (out - ref).abs().max().item()
+    print(f"[n_mels={n_mels}] cnn max abs err {e:.3e} (ref absmax {ref.abs().max():.2f})")
+    assert e < 5e-3
+
+
 def test_transcribe_end_to_end(dev):
     """wav -> tokens through the fused device pipeline and through the host-buffer entry point."""
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))

@@ -1,8 +1,8 @@
-"""Every diagnostic / experimental kernel variant that is compiled into libsbk.so (DESIGN.md section 8, "Diagnostic switches")
-must stay parity-green: the switches are read once per process, so each variant runs the 2 s golden in its own interpreter --
-fused wav -> ids pipeline for one 32-utterance batch (weight-streaming decode) and a 3-batch group (96 live rows: tensor-core GEMM decode
-projections, and enough (row, head) items for the TMA / persistent cross-attention variants) -- and must reproduce the
-reference's encoder states (1e-3 rel-L2) and greedy tokens."""
+"""Every diagnostic switch that selects a code path of libsbk.so (DESIGN.md section 8, "Diagnostic switches") must stay
+parity-green: the switches are read once per process, so each variant runs the 2 s golden in its own interpreter -- fused
+wav -> ids pipeline for one 32-utterance batch (weight-streaming decode) and a 3-batch group (96 live rows: tensor-core GEMM
+decode projections, or the weight-streaming kernels with SBK_DEC_TC_ROWS=128) -- and must reproduce the reference's encoder
+states (1e-3 rel-L2) and greedy tokens.  Every variant runs with both encoder attention types (RoPEMHA, RelPosMHAXL)."""
 import json
 import os
 import subprocess
@@ -19,8 +19,8 @@ import json, os, sys, torch
 sys.path.insert(0, %r)
 from speechbrain_b200.engine import AsrEngine
 from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
-g = torch.load(os.path.join(%r, "tests", "golden", "conformer_large_rope.pt"))
-cfg = dict(CONFORMER_LARGE)
+g = torch.load(os.path.join(%r, "tests", "golden", sys.argv[1] + ".pt"))
+cfg = dict(CONFORMER_LARGE, attention_type=g["cfg"]["attention_type"])
 eng = AsrEngine(cfg, seeded_asr_state(cfg, 0), device="cuda:0")
 wav = g["wav"].repeat(16, 1).cuda(); lens = g["wav_lens"].repeat(16).cuda()
 S = g["greedy_logits"].shape[1]
@@ -38,23 +38,27 @@ print(json.dumps({"rel": rel, "finite": bool(torch.isfinite(enc).all()), "tok": 
                   "group_equal": bool(all(torch.equal(o, outs[0]) for o in outs) and all(torch.equal(a, b) for a, b in zip(outs, outs2)))}))
 """ % (ROOT, ROOT)
 
-VARIANTS = [{}, {"SBK_GEMM_BN128": "1"}, {"SBK_GEMM_V1": "1"}, {"SBK_SILU_EXACT": "1"},
-            {"SBK_CNN_UNFUSED": "1"}, {"SBK_FBANK_FR16": "1"}, {"SBK_XATT_ROWMAJOR": "1"},
-            {"SBK_XATT_ROWMAJOR": "1", "SBK_DEC_XATT_TMA": "1"}, {"SBK_XATT_ROWMAJOR": "1", "SBK_DEC_XATT_PERSIST": "1"},
-            {"SBK_DEC_SPLITK": "1"}, {"SBK_PDL": "1"}, {"SBK_SKINNY_MT8": "1"}, {"SBK_NO_GRAPH": "1"}, {"SBK_DEC_TC_ROWS": "1"},
-            {"SBK_DEC_PRIORITY": "0"}]
+VARIANTS = [{}, {"SBK_XATT_ROWMAJOR": "1"}, {"SBK_NO_GRAPH": "1"}, {"SBK_DEC_TC_ROWS": "1"}, {"SBK_DEC_PRIORITY": "0"},
+            {"SBK_DEC_TC_ROWS": "128"}, {"SBK_XATT_ROWMAJOR": "1", "SBK_DEC_TC_ROWS": "128"},
+            {"SBK_NO_GRAPH": "1", "SBK_DEC_TC_ROWS": "128"}]
+GOLDENS = {"conformer_large_rope": "", "conformer_large_relpos": "-relpos"}  # golden -> test id suffix
 
 
-@pytest.mark.parametrize("env", VARIANTS, ids=lambda e: "+".join(sorted(e)) or "default")
-def test_kernel_variant_parity(env):
+def _env_id(env):
+    return "+".join(k if v in ("0", "1") else f"{k}={v}" for k, v in sorted(env.items())) or "default"
+
+
+@pytest.mark.parametrize("env,tag", [(e, t) for t in GOLDENS for e in VARIANTS],
+                         ids=[_env_id(e) + s for s in GOLDENS.values() for e in VARIANTS])
+def test_kernel_variant_parity(env, tag):
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
-    g = torch.load(os.path.join(ROOT, "tests", "golden", "conformer_large_rope.pt"))
+    g = torch.load(os.path.join(ROOT, "tests", "golden", tag + ".pt"))
     full_env = dict(os.environ, **env)
-    p = subprocess.run([sys.executable, "-c", SCRIPT], env=full_env, capture_output=True, text=True, timeout=600)
+    p = subprocess.run([sys.executable, "-c", SCRIPT, tag], env=full_env, capture_output=True, text=True, timeout=600)
     assert p.returncode == 0, p.stderr[-2000:]
     r = json.loads(p.stdout.strip().splitlines()[-1])
-    print(env, r)
+    print(tag, env, r)
     assert r["finite"] and r["rel"] < 1e-3
     assert r["tok"] == g["hyps"] and r["group_tok"] == g["hyps"] and r["rows_equal"] and r["group_equal"]
 
