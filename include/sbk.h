@@ -17,7 +17,7 @@ extern "C" {
 typedef struct sbk_fbank sbk_fbank; /* opaque */
 typedef struct sbk_asr sbk_asr;     /* opaque */
 
-enum { SBK_ATT_ROPE = 0, SBK_ATT_RELPOS = 1 };
+enum { SBK_ATT_ROPE = 0, SBK_ATT_RELPOS = 1, SBK_ATT_HYPERMIX = 2 };
 enum { SBK_ACT_RELU = 0, SBK_ACT_GELU = 1 };
 enum { SBK_ENC_CONFORMER = 0, SBK_ENC_BRANCHFORMER = 1 };
 enum { SBK_PART_FBANK = 1, SBK_PART_CNN = 2, SBK_PART_ENCODER = 4, SBK_PART_DECODER = 8, SBK_PART_ALL = 15, SBK_PART_LM = 16 };
@@ -35,7 +35,9 @@ typedef struct {
     int cnn_c1, cnn_c2;
     /* TransformerASR (lobes/models/transformer/TransformerASR.py:247-325) */
     int input_size, d_model, nhead, num_encoder_layers, num_decoder_layers, d_ffn, vocab, kernel_size;
-    int attention_type;     /* SBK_ATT_ROPE (RoPEMHA) | SBK_ATT_RELPOS (RelPosMHAXL) */
+    int attention_type;     /* SBK_ATT_ROPE (RoPEMHA) | SBK_ATT_RELPOS (RelPosMHAXL) | SBK_ATT_HYPERMIX (hypermixing: Conformer
+                               encoder only, head width d_model / nhead 32 or 64, hypernetwork width d_ffn / nhead a multiple
+                               of 16 up to 256; inputs up to 3000 frames) */
     int decoder_activation; /* SBK_ACT_RELU | SBK_ACT_GELU (the `activation` ctor kwarg) */
     int max_len;            /* positional tables (ctor kwarg max_length, default 2500) */
     int parts;              /* bitmask of SBK_PART_*: which sub-models the weight table carries */
@@ -129,6 +131,17 @@ int sbk_ctc_prefix_test(const float* logits_dev, const int* enc_len_dev, int B, 
  * bias [C/2] fp32; odd K <= 31, C/2 % 8 == 0.  Allocates and frees its own scratch and synchronises the stream. */
 int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev, const float* ln_b_dev, const float* taps_dev,
                   const float* bias_dev, int K, void* out_dev, void* stream);
+
+/* the HyperConformer's HyperMixing block alone (HyperMixing.forward, nnet/hypermixing.py:90-195, tied=False, nhead heads of
+ * e = d / nhead in {32, 64} channels, k = d_ffn / nhead a multiple of 16 up to 256): x_dev [B*T, d] fp16 (the norm1 output),
+ * lens_dev [B] valid frames (NULL: all T; frames t >= lens[b] are the key_padding_mask) -> out_dev [B*T, d] fp32 =
+ * layer_norm(mixing), before the residual add.  Weights fp32 in the reference layout: w{1,2}_gen fc1 [nhead, e, e],
+ * fc1 biases [nhead, e], fc2 [nhead, k, e], fc2 biases [nhead, k]; ln_g / ln_b [d].  T <= 3000.  Allocates and frees
+ * its own scratch and synchronises the stream. */
+int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int d, int nhead, int k, const float* w1_fc1_w_dev,
+                      const float* w1_fc1_b_dev, const float* w1_fc2_w_dev, const float* w1_fc2_b_dev, const float* w2_fc1_w_dev,
+                      const float* w2_fc1_b_dev, const float* w2_fc2_w_dev, const float* w2_fc2_b_dev, const float* ln_g_dev,
+                      const float* ln_b_dev, float* out_dev, void* stream);
 
 /* ---- model handle: repacks the reference state_dict once */
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out);

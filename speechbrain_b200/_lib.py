@@ -37,7 +37,7 @@ class sbk_beam_params(ctypes.Structure):
                 ("coverage_weight", ctypes.c_float), ("coverage_threshold", ctypes.c_float)]
 
 
-SBK_ATT_ROPE, SBK_ATT_RELPOS = 0, 1
+SBK_ATT_ROPE, SBK_ATT_RELPOS, SBK_ATT_HYPERMIX = 0, 1, 2
 SBK_ACT_RELU, SBK_ACT_GELU = 0, 1
 SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER = 0, 1
 SBK_PARTS = {"fbank": 1, "cnn": 2, "encoder": 4, "decoder": 8, "lm": 16}
@@ -46,7 +46,7 @@ SBK_PARTS = {"fbank": 1, "cnn": 2, "encoder": 4, "decoder": 8, "lm": 16}
 EXPORTS = [
     "sbk_last_error", "sbk_version", "sbk_launch_count", "sbk_gemm_profile_enable", "sbk_gemm_profile_read", "sbk_fbank_create", "sbk_fbank_destroy", "sbk_fbank_num_frames",
     "sbk_fbank_forward", "sbk_input_norm_global", "sbk_input_norm_sentence", "sbk_gemm_f16_test", "sbk_gemm_f16_resid_test",
-    "sbk_gemm_epilogue_test", "sbk_ctc_prefix_test", "sbk_csgu_test",
+    "sbk_gemm_epilogue_test", "sbk_ctc_prefix_test", "sbk_csgu_test", "sbk_hypermix_test",
     "sbk_asr_create", "sbk_asr_destroy", "sbk_asr_num_frames", "sbk_asr_cnn_forward", "sbk_asr_encode_from_cnn",
     "sbk_asr_encode_feats", "sbk_asr_greedy_from_enc", "sbk_asr_transcribe_greedy_dev",
     "sbk_asr_transcribe_greedy_host", "sbk_asr_transcribe_greedy_host_async", "sbk_asr_clone",

@@ -940,6 +940,298 @@ int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_d
     return SBK_ERR_UNSUPPORTED;
 }
 
+// =========================================================================== HyperMixing (HyperConformer token mixing)
+// HyperMixing.forward (nnet/hypermixing.py:90-195, 249-372; tied=False, keep_output_size=False) on the norm1 output
+// h16 [B*T, d] fp16, with M heads of e = d/M channels and a hypernetwork width of k = d_ffn/M per head:
+//     xm = h16 * valid;  hin = xm + PE_hm[t]                       (the module's own sine table, HM_PE_ROWS rows)
+//     per head m:  W1 = fc2_1(GELU(fc1_1(hin_m))), W2 = fc2_2(GELU(fc1_2(hin_m)))   [T, k], padded rows 0
+//                  H_m = xm_m^T W1 [e, k] over every frame,  y_m = W2 GELU(H_m)^T [T, e]
+//     x += LayerNorm_hm(y)   over the d channels of a frame (a padded frame has y = 0 and gets beta)
+// W1 and W2 never go through global memory: each is regenerated from hin in shared memory where it is consumed.
+//   hypermix_reduce:   one CTA per (HM_CHUNK frames, head, utterance).  Per 64-frame tile: w1_gen on tensor cores into
+//                      shared memory, then H += xm^T W1 in registers.  Writes the chunk's fp32 partial H.
+//   hypermix_finalize: per (head, utterance) the chunk partials summed in chunk order, G = GELU(H), stored fp16 as
+//                      G * 2^-s with the power of two s that puts max |G| in [2^13, 2^14): H grows with the number of
+//                      frames, and the scale keeps G finite and at full fp16 precision.  No atomics: chunks are aligned
+//                      to frame 0 and chunks past an utterance's length are not read, so reruns are bit-identical and
+//                      batch padding does not change an utterance's sums.
+//   hypermix_expand:   one CTA per (TR frames, utterance) over all heads: w2_gen into shared memory, y = W2 G^T times 2^s
+//                      in fp32 into a [TR, d] tile, then LayerNorm_hm of each frame and the residual add into x.
+// 8 warps share every product; the 16 x 8 output tiles of an m16n8k16 product are dealt round-robin to the warps, with
+// both operands K-contiguous in shared memory (ldmatrix without transposition).
+constexpr int HM_WARPS = 8, HM_THREADS = 32 * HM_WARPS, HM_TILE = 64, HM_CHUNK = 256;
+
+// acc[16 x 8] += A[16 rows, 0..K) . Bm[8 rows, 0..K)^T; row strides lda / ldb in halfs (multiples of 8), K % 16 == 0
+__device__ __forceinline__ void hm_mma_tile(float (&acc)[4], const __half* A, int lda, const __half* Bm, int ldb, int K) {
+    const int lane = threadIdx.x & 31;
+    const __half* pa = A + (lane & 15) * lda + (lane >> 4) * 8;
+    const __half* pb = Bm + (lane & 7) * ldb + ((lane >> 3) & 1) * 8;
+    for (int k0 = 0; k0 < K; k0 += 16) {
+        uint32_t a[4], b0, b1;
+        ldmatrix_x4(a[0], a[1], a[2], a[3], pa + k0);
+        ldmatrix_x2(b0, b1, pb + k0);
+        mma16816(acc, a, b0, b1);
+    }
+}
+
+// epi(r, n, C[r][n], C[r][n+1]) for every even n of C = A[R, K] . Bm[N, K]^T (R % 16 == 0, N % 8 == 0)
+template <typename Epi>
+__device__ __forceinline__ void hm_gemm(const __half* A, int lda, const __half* Bm, int ldb, int R, int N, int K, Epi epi) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
+    const int nt = N / 8, tiles = (R / 16) * nt;
+    for (int t = warp; t < tiles; t += HM_WARPS) {
+        const int r0 = (t / nt) * 16, n0 = (t % nt) * 8;
+        float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+        hm_mma_tile(acc, A + r0 * lda, lda, Bm + n0 * ldb, ldb, K);
+        epi(r0 + g, n0 + 2 * c, acc[0], acc[1]);
+        epi(r0 + g + 8, n0 + 2 * c, acc[2], acc[3]);
+    }
+}
+
+// rows x cols fp16 matrix (row-major, contiguous) -> shared memory with row stride ld halfs; cols % 8 == 0
+__device__ __forceinline__ void hm_copy_rows(__half* dst, int ld, const __half* __restrict__ src, int rows, int cols) {
+    const int v = cols / 8;
+    for (int i = threadIdx.x; i < rows * v; i += blockDim.x) {
+        const int r = i / v, j = (i - r * v) * 8;
+        *reinterpret_cast<uint4*>(dst + r * ld + j) = __ldg(reinterpret_cast<const uint4*>(src + static_cast<size_t>(r) * cols + j));
+    }
+}
+
+// hin = xm + PE (fp16, [rows][ldh]) and, when xmT != null, xm transposed ([E][ldx]) for the frames t0 .. t0 + rows - 1 of
+// the utterance at row0, channels ch0 .. ch0 + E - 1: xm = h16 for t < len, 0 otherwise; frames t >= T are 0 in both
+template <int E>
+__device__ __forceinline__ void hm_stage(const __half* __restrict__ h16, const float* __restrict__ pe, int d, int T, int len,
+                                         size_t row0, int t0, int rows, int ch0, __half* hin, int ldh, __half* xmT, int ldx) {
+    constexpr int V = E / 8;
+    for (int i = threadIdx.x; i < rows * V; i += blockDim.x) {
+        const int r = i / V, v = (i - r * V) * 8, t = t0 + r;
+        uint4 raw = make_uint4(0u, 0u, 0u, 0u), hv = make_uint4(0u, 0u, 0u, 0u);
+        if (t < len) raw = __ldg(reinterpret_cast<const uint4*>(h16 + (row0 + t) * d + ch0 + v));
+        const __half* xh = reinterpret_cast<const __half*>(&raw);
+        if (t < T) {
+            const float4 p0 = __ldg(reinterpret_cast<const float4*>(pe + static_cast<size_t>(t) * d + ch0 + v));
+            const float4 p1 = __ldg(reinterpret_cast<const float4*>(pe + static_cast<size_t>(t) * d + ch0 + v + 4));
+            hv.x = pack_half2(__half2float(xh[0]) + p0.x, __half2float(xh[1]) + p0.y);
+            hv.y = pack_half2(__half2float(xh[2]) + p0.z, __half2float(xh[3]) + p0.w);
+            hv.z = pack_half2(__half2float(xh[4]) + p1.x, __half2float(xh[5]) + p1.y);
+            hv.w = pack_half2(__half2float(xh[6]) + p1.z, __half2float(xh[7]) + p1.w);
+        }
+        *reinterpret_cast<uint4*>(hin + r * ldh + v) = hv;
+        if (xmT != nullptr) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) xmT[(v + j) * ldx + r] = xh[j];
+        }
+    }
+}
+
+template <int E>
+__global__ void __launch_bounds__(HM_THREADS)
+hypermix_reduce_kernel(const __half* __restrict__ h16, int T, int d, int KH, const int* __restrict__ lens,
+                       const float* __restrict__ pe, const __half* __restrict__ fc1w, const float* __restrict__ fc1b,
+                       const __half* __restrict__ fc2w, const float* __restrict__ fc2b, float* __restrict__ part, int nchunk) {
+    constexpr int LE = E + 8, LT = HM_TILE + 8;
+    constexpr int MAXT = E / 4;  // 16 x 8 tiles of H per warp at k = 256: (E / 16) * (256 / 8) / HM_WARPS
+    extern __shared__ __align__(16) uint8_t hm_smem[];
+    __half* w1s = reinterpret_cast<__half*>(hm_smem);  // fc1 of head m [E][LE]
+    __half* w2s = w1s + E * LE;                        // fc2 of head m [KH][LE]
+    __half* hin = w2s + KH * LE;                       // [64][LE]
+    __half* hid = hin + HM_TILE * LE;                  // GELU(fc1 hin) [64][LE]
+    __half* xmT = hid + HM_TILE * LE;                  // xm^T [E][LT]
+    __half* w1T = xmT + E * LT;                        // W1^T [KH][LT]
+    const int chunk = blockIdx.x, m = blockIdx.y, b = blockIdx.z, M = gridDim.y;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
+    const int len = lens ? min(max(lens[b], 0), T) : T;
+    const size_t row0 = static_cast<size_t>(b) * T;
+    const float* b1 = fc1b + m * E;
+    const float* b2 = fc2b + m * KH;
+    hm_copy_rows(w1s, LE, fc1w + static_cast<size_t>(m) * E * E, E, E);
+    hm_copy_rows(w2s, LE, fc2w + static_cast<size_t>(m) * KH * E, KH, E);
+    const int nt = KH / 8, tiles = (E / 16) * nt;
+    float acc[MAXT][4];
+#pragma unroll
+    for (int i = 0; i < MAXT; ++i) acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.0f;
+    const int te = min(chunk * HM_CHUNK + HM_CHUNK, len);
+    for (int t0 = chunk * HM_CHUNK; t0 < te; t0 += HM_TILE) {
+        __syncthreads();  // the previous tile is consumed (first tile: the weights are staged)
+        hm_stage<E>(h16, pe, d, T, len, row0, t0, HM_TILE, m * E, hin, LE, xmT, LT);
+        __syncthreads();
+        hm_gemm(hin, LE, w1s, LE, HM_TILE, E, E, [&](int r, int n, float v0, float v1) {
+            *reinterpret_cast<uint32_t*>(hid + r * LE + n) =
+                pack_half2(gelu_erf_f(v0 + __ldg(b1 + n)), gelu_erf_f(v1 + __ldg(b1 + n + 1)));
+        });
+        __syncthreads();
+        hm_gemm(hid, LE, w2s, LE, HM_TILE, KH, E, [&](int r, int n, float v0, float v1) {
+            const bool ok = t0 + r < len;  // padded frames: W1 row 0
+            w1T[n * LT + r] = float2half_sat(ok ? v0 + __ldg(b2 + n) : 0.0f);
+            w1T[(n + 1) * LT + r] = float2half_sat(ok ? v1 + __ldg(b2 + n + 1) : 0.0f);
+        });
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < MAXT; ++i) {
+            const int t = warp + HM_WARPS * i;
+            if (t < tiles) hm_mma_tile(acc[i], xmT + (t / nt) * 16 * LT, LT, w1T + (t % nt) * 8 * LT, LT, HM_TILE);
+        }
+    }
+    float* out = part + ((static_cast<size_t>(b) * M + m) * nchunk + chunk) * E * KH;
+#pragma unroll
+    for (int i = 0; i < MAXT; ++i) {
+        const int t = warp + HM_WARPS * i;
+        if (t >= tiles) continue;
+        const int r = (t / nt) * 16 + g, n = (t % nt) * 8 + 2 * c;
+        *reinterpret_cast<float2*>(out + static_cast<size_t>(r) * KH + n) = make_float2(acc[i][0], acc[i][1]);
+        *reinterpret_cast<float2*>(out + static_cast<size_t>(r + 8) * KH + n) = make_float2(acc[i][2], acc[i][3]);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+hypermix_finalize_kernel(float* __restrict__ part, int nchunk, int T, const int* __restrict__ lens, int EK,
+                         __half* __restrict__ G, float* __restrict__ gscale) {
+    __shared__ float red[8];
+    const int m = blockIdx.x, b = blockIdx.y, M = gridDim.x;
+    const int len = lens ? min(max(lens[b], 0), T) : T;
+    const int nc = max(1, ceil_div(len, HM_CHUNK));  // chunks holding valid frames (chunk 0 is always written)
+    float* p = part + (static_cast<size_t>(b) * M + m) * nchunk * EK;
+    float mx = 0.0f;
+    for (int i = threadIdx.x; i < EK; i += blockDim.x) {
+        float s = p[i];
+        for (int ch = 1; ch < nc; ++ch) s += p[static_cast<size_t>(ch) * EK + i];
+        const float gv = gelu_erf_f(s);
+        p[i] = gv;  // read back below by the same thread
+        mx = fmaxf(mx, fabsf(gv));
+    }
+    mx = warp_max(mx);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    mx = red[0];
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) mx = fmaxf(mx, red[w]);
+    int ex = 0;
+    frexpf(mx, &ex);  // mx < 2^ex
+    const int s = mx > 0.0f ? ex - 14 : 0;
+    const float down = ldexpf(1.0f, -s);
+    __half* gp = G + (static_cast<size_t>(b) * M + m) * EK;
+    for (int i = threadIdx.x; i < EK; i += blockDim.x) gp[i] = float2half_sat(p[i] * down);
+    if (threadIdx.x == 0) gscale[b * M + m] = ldexpf(1.0f, s);
+}
+
+template <int E, int TR>
+__global__ void __launch_bounds__(HM_THREADS)
+hypermix_expand_kernel(const __half* __restrict__ h16, int T, int d, int KH, const int* __restrict__ lens,
+                       const float* __restrict__ pe, const __half* __restrict__ fc1w, const float* __restrict__ fc1b,
+                       const __half* __restrict__ fc2w, const float* __restrict__ fc2b, const __half* __restrict__ G,
+                       const float* __restrict__ gscale, const float* __restrict__ ln_g, const float* __restrict__ ln_b,
+                       float eps, float* __restrict__ x) {
+    constexpr int LE = E + 8;
+    const int LK = KH + 8, LY = d + 4;
+    extern __shared__ __align__(16) uint8_t hm_smem[];
+    float* ys = reinterpret_cast<float*>(hm_smem);     // y of every head [TR][LY]
+    __half* w1s = reinterpret_cast<__half*>(ys + TR * LY);  // [E][LE]
+    __half* w2s = w1s + E * LE;                        // [KH][LE]
+    __half* hin = w2s + KH * LE;                       // [TR][LE]
+    __half* hid = hin + TR * LE;                       // [TR][LE]
+    __half* w2t = hid + TR * LE;                       // W2 [TR][LK]
+    __half* gs = w2t + TR * LK;                        // G * 2^-s [E][LK]
+    const int t0 = blockIdx.x * TR, b = blockIdx.y, M = d / E;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int len = lens ? min(max(lens[b], 0), T) : T;
+    const size_t row0 = static_cast<size_t>(b) * T;
+    for (int m = 0; m < M; ++m) {
+        const float* b1 = fc1b + m * E;
+        const float* b2 = fc2b + m * KH;
+        __syncthreads();  // the previous head's operands are consumed
+        hm_copy_rows(w1s, LE, fc1w + static_cast<size_t>(m) * E * E, E, E);
+        hm_copy_rows(w2s, LE, fc2w + static_cast<size_t>(m) * KH * E, KH, E);
+        hm_copy_rows(gs, LK, G + (static_cast<size_t>(b) * M + m) * E * KH, E, KH);
+        hm_stage<E>(h16, pe, d, T, len, row0, t0, TR, m * E, hin, LE, nullptr, 0);
+        __syncthreads();
+        hm_gemm(hin, LE, w1s, LE, TR, E, E, [&](int r, int n, float v0, float v1) {
+            *reinterpret_cast<uint32_t*>(hid + r * LE + n) =
+                pack_half2(gelu_erf_f(v0 + __ldg(b1 + n)), gelu_erf_f(v1 + __ldg(b1 + n + 1)));
+        });
+        __syncthreads();
+        hm_gemm(hid, LE, w2s, LE, TR, KH, E, [&](int r, int n, float v0, float v1) {
+            const bool ok = t0 + r < len;  // padded frames: W2 row 0
+            *reinterpret_cast<uint32_t*>(w2t + r * LK + n) =
+                pack_half2(ok ? v0 + __ldg(b2 + n) : 0.0f, ok ? v1 + __ldg(b2 + n + 1) : 0.0f);
+        });
+        __syncthreads();
+        const float sc = __ldg(gscale + b * M + m);
+        hm_gemm(w2t, LK, gs, LK, TR, E, KH, [&](int r, int n, float v0, float v1) {
+            *reinterpret_cast<float2*>(ys + r * LY + m * E + n) = make_float2(v0 * sc, v1 * sc);
+        });
+    }
+    __syncthreads();
+    // LayerNorm_hm (fp32, two-pass) of each frame and x += it, for every frame < T (padded frames get + beta)
+    for (int r = warp; r < TR; r += HM_WARPS) {
+        const int t = t0 + r;
+        if (t >= T) break;
+        const float* yr = ys + r * LY;
+        float s = 0.0f;
+        for (int j = lane; j < d; j += 32) s += yr[j];
+        const float mean = warp_sum(s) / d;
+        float v = 0.0f;
+        for (int j = lane; j < d; j += 32) v += (yr[j] - mean) * (yr[j] - mean);
+        const float rstd = rsqrtf(warp_sum(v) / d + eps);
+        float* xr = x + (row0 + t) * d;
+        for (int j = lane; j < d; j += 32) xr[j] += (yr[j] - mean) * rstd * __ldg(ln_g + j) + __ldg(ln_b + j);
+    }
+}
+
+size_t hypermix_part_floats(int B, int T, int d, int KH) {
+    return static_cast<size_t>(B) * d * KH * ceil_div(std::max(T, 1), HM_CHUNK);
+}
+
+template <int E>
+static size_t hm_reduce_smem(int KH) { return 2ull * (E * (E + 8) + KH * (E + 8) + 2 * HM_TILE * (E + 8) + (E + KH) * (HM_TILE + 8)); }
+template <int E, int TR>
+static size_t hm_expand_smem(int d, int KH) {
+    return 4ull * TR * (d + 4) + 2ull * (E * (E + 8) + KH * (E + 8) + 2 * TR * (E + 8) + (TR + E) * (KH + 8));
+}
+
+template <int E>
+static int launch_hypermix(const __half* h16, int B, int T, int d, int KH, const int* lens, const float* pe,
+                           const HyperMixWeights& w, float* part, __half* G, float* gscale, float* x, cudaStream_t st) {
+    constexpr int TR = E == 32 ? 64 : 32;
+    const int M = d / E, nchunk = ceil_div(T, HM_CHUNK);
+    const size_t sm_r = hm_reduce_smem<E>(KH), sm_e = hm_expand_smem<E, TR>(d, KH);
+    SBK_REQUIRE(sm_e <= 227 * 1024, "hypermix: d_model=%d with k=%d needs %zu bytes of shared memory", d, KH, sm_e);
+    auto kr = hypermix_reduce_kernel<E>;
+    SBK_CUDA_CHECK(cudaFuncSetAttribute(kr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_r));
+    kr<<<dim3(nchunk, M, B), HM_THREADS, sm_r, st>>>(h16, T, d, KH, lens, pe, w.fc1w[0], w.fc1b[0], w.fc2w[0], w.fc2b[0], part,
+                                                    nchunk);
+    SBK_LAUNCH_CHECK();
+    hypermix_finalize_kernel<<<dim3(M, B), 256, 0, st>>>(part, nchunk, T, lens, E * KH, G, gscale);
+    SBK_LAUNCH_CHECK();
+    auto ke = hypermix_expand_kernel<E, TR>;
+    SBK_CUDA_CHECK(cudaFuncSetAttribute(ke, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_e));
+    ke<<<dim3(ceil_div(T, TR), B), HM_THREADS, sm_e, st>>>(h16, T, d, KH, lens, pe, w.fc1w[1], w.fc1b[1], w.fc2w[1], w.fc2b[1],
+                                                           G, gscale, w.ln_g, w.ln_b, 1e-5f, x);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
+int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, const int* lens, const float* pe,
+                     const HyperMixWeights& w, float* part, __half* G, float* gscale, float* x, cudaStream_t st) {
+    SBK_REQUIRE(M > 0 && d % M == 0, "hypermix: d_model=%d, nhead=%d", d, M);
+    const int E = d / M;
+    SBK_REQUIRE(E == 32 || E == 64, "hypermix: head width d_model / nhead = %d not built (32, 64)", E);
+    SBK_REQUIRE(KH > 0 && KH % 16 == 0 && KH <= 256, "hypermix: k = d_ffn / nhead = %d must be a multiple of 16 up to 256", KH);
+    SBK_REQUIRE(T <= HM_PE_ROWS, "hypermix: %d frames exceed the HyperMixing positional table (%d)", T, HM_PE_ROWS);
+    SBK_REQUIRE(B <= 65535, "hypermix: B=%d", B);
+    if (B == 0 || T == 0) return SBK_OK;
+    return E == 32 ? launch_hypermix<32>(h16, B, T, d, KH, lens, pe, w, part, G, gscale, x, st)
+                   : launch_hypermix<64>(h16, B, T, d, KH, lens, pe, w, part, G, gscale, x, st);
+}
+
+void hypermix_pe_table(int d, float* dst) {
+    for (int i = 0; i < d / 2; ++i) {  // Transformer.py:252-303 PositionalEncoding, computed in fp32 like the reference
+        const float den = expf((float)(2 * i) * -(logf(10000.0f) / (float)d));
+        for (int t = 0; t < HM_PE_ROWS; ++t) {
+            dst[(size_t)t * d + 2 * i] = sinf((float)t * den);
+            dst[(size_t)t * d + 2 * i + 1] = cosf((float)t * den);
+        }
+    }
+}
+
 // =========================================================================== TransformerLM causal self-attention
 // Whole-sequence attention of TransformerLM.forward (TransformerLM.py:127-169: nn.MultiheadAttention under make_masks'
 // look-ahead mask and key-padding mask on pad_idx).  qkv [n*s, 3d] fp16 with columns [q | k | v] (nn.MultiheadAttention's

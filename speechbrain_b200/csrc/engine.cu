@@ -45,6 +45,7 @@ struct EncLayerW {
     const __half *wpre, *wpost, *wmerge;  // pre_channel_proj [C, d], post_channel_proj [d, C/2], merge_proj [d, 2d]
     const float *bpre, *bpost, *bmerge;
     const float *csgu_ln_g, *csgu_ln_b, *csgu_taps, *csgu_bias;  // taps tap-major [CSGU_TAP_ROWS, C/2] (csgu_repack_taps)
+    HyperMixWeights hm;               // HyperConformer: mha_layer = HyperMixing (replaces wqkv / wo / bo)
 };
 
 struct DecLayerW {
@@ -84,6 +85,7 @@ struct AsrModel {
     const float *enc_norm_g, *enc_norm_b;
     const float *rope_cos = nullptr, *rope_sin = nullptr;  // [max_len, dh/2]
     const __half* relpos_pe = nullptr;                     // [max_len, d] rows = |r|
+    const float* hm_pe = nullptr;                          // HyperMixing's own sine table [HM_PE_ROWS, d]
     int pos_len = 0;
     // decoder
     const float* emb; const float* dec_pe;
@@ -124,6 +126,9 @@ struct AsrModel {
         // LayerNorm statistics [M]
         __half *hc16, *cat16, *g16;
         float2* csgu_stats;
+        // HyperConformer encoder only: per-chunk partial H, G = GELU(H) scaled to fp16 [B, d, k], its scales [B, nhead]
+        float *hm_part, *hm_gscale;
+        __half* hm_G;
     } b;
     cudaGraphExec_t step_graph = nullptr;
     int graph_rows = -1, graph_T = -1, graph_B = -1, graph_eos = -1, graph_S = -1;
@@ -218,6 +223,11 @@ static size_t weight_arena_bytes(const sbk_asr_config& c) {
         enc = (size_t)c.num_encoder_layers * ((3 * d * d + d * d + d * d + C * d + d * C / 2 + 2 * d * d) * 2 +
                                               (size_t)CSGU_TAP_ROWS * C / 2 * 4 + (4 * C + 16 * d) * 4);
     }
+    if (c.attention_type == SBK_ATT_HYPERMIX && c.nhead > 0) {  // two hypernetworks (fp16 + fp32 biases), LayerNorm, PE table
+        const size_t e = d / c.nhead, k = f / c.nhead, M = c.nhead;
+        enc += (size_t)c.num_encoder_layers * (2 * M * (e * e + k * e) * 2 + (2 * M * (e + k) + 2 * d) * 4 + 4 * 256) +
+               (size_t)HM_PE_ROWS * d * 4;
+    }
     size_t dec = (size_t)c.num_decoder_layers * (3 * d * d + d * d + 3 * d * d + d * d + 2 * d * f) * 2;
     size_t misc = (size_t)c.vocab * d * (4 + 2 + 2) + (size_t)c.max_len * d * (4 + 2) + (size_t)c.input_size * d * 2;
     size_t lm = 0;
@@ -233,10 +243,15 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
     SBK_REQUIRE(cfg && weights && out, "asr_create: null argument");
     const sbk_asr_config& c = *cfg;
     SBK_REQUIRE(c.d_model % 8 == 0 && c.d_model % c.nhead == 0, "asr_create: bad d_model/nhead");
-    SBK_REQUIRE(c.attention_type == SBK_ATT_ROPE || c.attention_type == SBK_ATT_RELPOS,
-                "asr_create: attention_type must be RoPEMHA or RelPosMHAXL");
+    SBK_REQUIRE(c.attention_type == SBK_ATT_ROPE || c.attention_type == SBK_ATT_RELPOS || c.attention_type == SBK_ATT_HYPERMIX,
+                "asr_create: attention_type must be RoPEMHA, RelPosMHAXL or hypermixing");
     const int d = c.d_model, dh = d / c.nhead, F = c.d_ffn, K = c.kernel_size;
-    SBK_REQUIRE(dh == 64 || dh == 36 || dh == 32, "asr_create: encoder head_dim=%d not built (64, 36, 32)", dh);
+    const bool hypermix = c.attention_type == SBK_ATT_HYPERMIX;
+    SBK_REQUIRE(hypermix || dh == 64 || dh == 36 || dh == 32, "asr_create: encoder head_dim=%d not built (64, 36, 32)", dh);
+    SBK_REQUIRE(!hypermix || (c.encoder_module == SBK_ENC_CONFORMER && (dh == 32 || dh == 64) && F % c.nhead == 0 &&
+                              (F / c.nhead) % 16 == 0 && F / c.nhead <= 256),
+                "asr_create: hypermixing needs the Conformer encoder, a head width d_model / nhead of 32 or 64 and "
+                "k = d_ffn / nhead a multiple of 16 up to 256 (got %d, %d)", dh, c.nhead > 0 ? F / c.nhead : 0);
     SBK_REQUIRE(!((c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0) || (dh <= 64 && dh % 4 == 0 && d % 16 == 0),
                 "asr_create: decoder head_dim must be a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)", dh, d);
     SBK_REQUIRE(c.attention_type != SBK_ATT_ROPE || dh % 32 == 0, "asr_create: RoPEMHA needs head_dim %% 32 == 0");
@@ -333,9 +348,22 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
         e.ffn1_w1 = p.f16(q + "ffn_module1.1.ffn.0.weight", (int64_t)F * d); e.ffn1_b1 = p.f32(q + "ffn_module1.1.ffn.0.bias", F);
         e.ffn1_w2 = p.f16(q + "ffn_module1.1.ffn.3.weight", (int64_t)d * F); e.ffn1_b2 = p.f32(q + "ffn_module1.1.ffn.3.bias", d);
         e.norm1_g = p.f32(q + "norm1.norm.weight", d); e.norm1_b = p.f32(q + "norm1.norm.bias", d);
-        e.wqkv = p.f16(q + "mha_layer.in_proj_weight", (int64_t)3 * d * d);
-        e.wo = p.f16(q + "mha_layer.out_proj.weight", (int64_t)d * d); e.bo = p.f32(q + "mha_layer.out_proj.bias", d);
         e.wpos = nullptr; e.pos_u = e.pos_v = nullptr;
+        if (hypermix) {  // hypermixing.py:52-81, 274-337: w{1,2}_gen fc1 (M, e, e) / fc2 (M, k, e), then layer_norm (d)
+            const int Mh = c.nhead, kh = F / c.nhead;
+            const char* gen[2] = {"mha_layer.hyper.w1_gen.", "mha_layer.hyper.w2_gen."};
+            for (int gi = 0; gi < 2; ++gi) {
+                e.hm.fc1w[gi] = p.f16(q + gen[gi] + "fc1_weights", (int64_t)Mh * dh * dh);
+                e.hm.fc1b[gi] = p.f32(q + gen[gi] + "fc1_biases", (int64_t)Mh * dh);
+                e.hm.fc2w[gi] = p.f16(q + gen[gi] + "fc2_weights", (int64_t)Mh * kh * dh);
+                e.hm.fc2b[gi] = p.f32(q + gen[gi] + "fc2_biases", (int64_t)Mh * kh);
+            }
+            e.hm.ln_g = p.f32(q + "mha_layer.layer_norm.weight", d); e.hm.ln_b = p.f32(q + "mha_layer.layer_norm.bias", d);
+            e.wqkv = e.wo = nullptr; e.bo = nullptr;
+        } else {
+            e.wqkv = p.f16(q + "mha_layer.in_proj_weight", (int64_t)3 * d * d);
+            e.wo = p.f16(q + "mha_layer.out_proj.weight", (int64_t)d * d); e.bo = p.f32(q + "mha_layer.out_proj.bias", d);
+        }
         if (c.attention_type == SBK_ATT_RELPOS) {
             e.wpos = p.f16(q + "mha_layer.linear_pos.weight", (int64_t)d * d);
             e.pos_u = p.f32(q + "mha_layer.pos_bias_u", d); e.pos_v = p.f32(q + "mha_layer.pos_bias_v", d);
@@ -390,6 +418,11 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
         }
         m->rope_cos = p.f32_raw(cs.data(), cs.size());
         m->rope_sin = p.f32_raw(sn.data(), sn.size());
+    } else if (hypermix) {
+        std::vector<float> pe((size_t)HM_PE_ROWS * d);
+        hypermix_pe_table(d, pe.data());
+        m->hm_pe = p.f32_raw(pe.data(), pe.size());
+        m->pos_len = HM_PE_ROWS;
     } else {
         // nnet/attention.py:360-408: row |r|: even cols sin(|r| f_i), odd cols cos(|r| f_i)
         std::vector<float> pe((size_t)c.max_len * d);
@@ -609,6 +642,8 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
     const int F1 = (c.n_mels - 1) / 2 + 1;
     const size_t M = (size_t)B * T2, d = c.d_model, F = c.d_ffn, Ld = c.num_decoder_layers, S = steps + 1;
     const bool bfm = c.encoder_module == SBK_ENC_BRANCHFORMER && m->has_enc;
+    const bool hmx = c.attention_type == SBK_ATT_HYPERMIX && m->has_enc;
+    const size_t hm_part = hmx ? hypermix_part_floats(B, T2, c.d_model, c.d_ffn / c.nhead) : 0;
     const size_t Cu = bfm ? (size_t)c.csgu_linear_units : 0, Fu = std::max(F, Cu);  // f16 also holds the CSGU input u
     const size_t Md = (size_t)std::max(B, rows) * T2;  // encoder states / cross K,V of every utterance the decoder sees
     size_t need = 0;
@@ -629,6 +664,7 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
         sz(Ll * rows * S * dl * 2); sz(Ll * rows * S * dl * 2); sz((size_t)rows * S * 4);
     }
     if (bfm) { sz(M * d * 2); sz(M * 2 * d * 2); sz(M * Cu / 2 * 2); sz(M * 8); }
+    if (hmx) { sz(hm_part * 4); sz((size_t)B * d * (F / c.nhead) * 2); sz((size_t)B * c.nhead * 4); }
     need += 1 << 20;
     if (need > m->ws.cap) {
         if (m->ws.base) { cudaDeviceSynchronize(); cudaFree(m->ws.base); m->ws.base = nullptr; }
@@ -670,6 +706,11 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
         TAKE(hc16, __half, M * d * 2); TAKE(cat16, __half, M * 2 * d * 2); TAKE(g16, __half, M * Cu / 2 * 2);
         TAKE(csgu_stats, float2, M * 8);
         if (!b.csgu_stats) { set_error("workspace carve failed (Branchformer)"); return SBK_ERR_NOMEM; }
+    }
+    if (hmx) {
+        TAKE(hm_part, float, hm_part * 4); TAKE(hm_G, __half, (size_t)B * d * (F / c.nhead) * 2);
+        TAKE(hm_gscale, float, (size_t)B * c.nhead * 4);
+        if (!b.hm_gscale) { set_error("workspace carve failed (HyperMixing)"); return SBK_ERR_NOMEM; }
     }
     if (!b.df16 || !b.seq_scores || !b.lnout || !b.hist_lp) { set_error("workspace carve failed"); return SBK_ERR_NOMEM; }
 #undef TAKE
@@ -726,7 +767,12 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
     const int M = B * T, d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H;
     SBK_REQUIRE(m->has_enc, "encode: this handle was created without encoder weights");
     SBK_REQUIRE(feats == nullptr || m->has_cnn, "encode: this handle was created without CNN weights");
-    SBK_REQUIRE(T <= m->pos_len, "encode: %d frames exceed max_len=%d", T, m->pos_len);
+    if (c.attention_type == SBK_ATT_HYPERMIX)  // HyperMixing adds its own 3000-row table: longer inputs fail in the reference
+        SBK_REQUIRE(T <= HM_PE_ROWS, "encode: %d frames exceed HyperMixing's %d-row positional table", T, HM_PE_ROWS);
+    else
+        SBK_REQUIRE(T <= m->pos_len, "encode: %d frames exceed max_len=%d", T, m->pos_len);
+    SBK_REQUIRE(c.attention_type != SBK_ATT_HYPERMIX || m->dyn_chunk == 0,
+                "encode: HyperMixing has no chunked (DynChunkTrainConfig) mode");
     SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER || T > (c.kernel_size - 1) / 2,
                 "encode: the Branchformer's reflect-padded conv needs more than %d frames (got %d)", (c.kernel_size - 1) / 2, T);
     if (feats != nullptr)
@@ -747,21 +793,25 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
         RC(gemm_f16(b.f16, F, w.ffn1_w2, F, e, M, d, F, st));
         // --- self-attention (Conformer.py:481-492)
         RC(layernorm_rows(b.x, b.h16, true, w.norm1_g, w.norm1_b, M, d, 1e-5f, false, st));
-        e = GemmEpilogue(); e.out = b.qkv16; e.ldo = 3 * d;
-        if (c.attention_type == SBK_ATT_ROPE) {
-            e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->rope_cos; e.rope_sin = m->rope_sin; e.head_dim = dh;
+        if (c.attention_type == SBK_ATT_HYPERMIX) {  // x += HyperMixing(norm1(x)) (hypermixing.py:90-195)
+            RC(hypermix_forward(b.h16, B, T, d, H, F / H, enc_len, m->hm_pe, w.hm, b.hm_part, b.hm_G, b.hm_gscale, b.x, st));
         } else {
-            e.mode = EPI_F16;
+            e = GemmEpilogue(); e.out = b.qkv16; e.ldo = 3 * d;
+            if (c.attention_type == SBK_ATT_ROPE) {
+                e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->rope_cos; e.rope_sin = m->rope_sin; e.head_dim = dh;
+            } else {
+                e.mode = EPI_F16;
+            }
+            RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
+            if (c.attention_type == SBK_ATT_RELPOS) {
+                e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
+                RC(gemm_f16(m->relpos_pe, d, w.wpos, d, e, T, d, d, st));
+            }
+            RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, c.attention_type == SBK_ATT_RELPOS, w.pos_u, w.pos_v,
+                                 b.P16, d, att_scale, b.att16, d, st, m->dyn_chunk, m->dyn_left));
+            e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bo; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
+            RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
         }
-        RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
-        if (c.attention_type == SBK_ATT_RELPOS) {
-            e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
-            RC(gemm_f16(m->relpos_pe, d, w.wpos, d, e, T, d, d, st));
-        }
-        RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, c.attention_type == SBK_ATT_RELPOS, w.pos_u, w.pos_v,
-                             b.P16, d, att_scale, b.att16, d, st, m->dyn_chunk, m->dyn_left));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bo; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
-        RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
         // --- convolution module (Conformer.py:314-330, 494)
         RC(layernorm_rows(b.x, b.h16, true, w.conv_ln_g, w.conv_ln_b, M, d, 1e-5f, false, st));
         e = GemmEpilogue(); e.mode = EPI_GLU; e.bias = w.bpw1; e.out = b.glu; e.ldo = d;
@@ -1632,6 +1682,48 @@ int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev,
     if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("csgu_test: device error"); rc = SBK_ERR_CUDA; }
     cudaFree(taps);
     cudaFree(stats);
+    return rc;
+}
+
+int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int d, int nhead, int k, const float* w1_fc1_w_dev,
+                      const float* w1_fc1_b_dev, const float* w1_fc2_w_dev, const float* w1_fc2_b_dev, const float* w2_fc1_w_dev,
+                      const float* w2_fc1_b_dev, const float* w2_fc2_w_dev, const float* w2_fc2_b_dev, const float* ln_g_dev,
+                      const float* ln_b_dev, float* out_dev, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(x_dev && w1_fc1_w_dev && w1_fc1_b_dev && w1_fc2_w_dev && w1_fc2_b_dev && w2_fc1_w_dev && w2_fc1_b_dev &&
+                    w2_fc2_w_dev && w2_fc2_b_dev && ln_g_dev && ln_b_dev && out_dev, "hypermix_test: null pointer");
+    SBK_REQUIRE(B >= 1 && T >= 1 && nhead >= 1 && d % nhead == 0 && k >= 1, "hypermix_test: bad sizes B=%d T=%d d=%d nhead=%d k=%d",
+                B, T, d, nhead, k);
+    const int e = d / nhead;
+    const size_t n1 = (size_t)nhead * e * e, n2 = (size_t)nhead * k * e;
+    std::vector<float> pe((size_t)HM_PE_ROWS * d);
+    hypermix_pe_table(d, pe.data());
+    const size_t part_n = hypermix_part_floats(B, T, d, k);
+    uint8_t* base = nullptr;
+    const size_t off_w = 0, off_pe = off_w + ((2 * (n1 + n2) * 2 + 255) & ~size_t(255)), off_part = off_pe + pe.size() * 4,
+                 off_g = off_part + part_n * 4, off_s = off_g + (((size_t)B * d * k * 2 + 255) & ~size_t(255)),
+                 total = off_s + (size_t)B * nhead * 4;
+    if (cudaMalloc(&base, total) != cudaSuccess) { set_error("hypermix_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
+    __half* w16 = reinterpret_cast<__half*>(base + off_w);
+    HyperMixWeights w;
+    w.fc1w[0] = w16; w.fc2w[0] = w16 + n1; w.fc1w[1] = w16 + n1 + n2; w.fc2w[1] = w16 + 2 * n1 + n2;
+    w.fc1b[0] = w1_fc1_b_dev; w.fc2b[0] = w1_fc2_b_dev; w.fc1b[1] = w2_fc1_b_dev; w.fc2b[1] = w2_fc2_b_dev;
+    w.ln_g = ln_g_dev; w.ln_b = ln_b_dev;
+    int rc = cast_f32_f16(w1_fc1_w_dev, const_cast<__half*>(w.fc1w[0]), n1, st);
+    if (rc == SBK_OK) rc = cast_f32_f16(w1_fc2_w_dev, const_cast<__half*>(w.fc2w[0]), n2, st);
+    if (rc == SBK_OK) rc = cast_f32_f16(w2_fc1_w_dev, const_cast<__half*>(w.fc1w[1]), n1, st);
+    if (rc == SBK_OK) rc = cast_f32_f16(w2_fc2_w_dev, const_cast<__half*>(w.fc2w[1]), n2, st);
+    if (rc == SBK_OK && (cudaMemcpyAsync(base + off_pe, pe.data(), pe.size() * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+                         cudaMemsetAsync(out_dev, 0, (size_t)B * T * d * 4, st) != cudaSuccess)) {
+        set_error("hypermix_test: copy failed");
+        rc = SBK_ERR_CUDA;
+    }
+    if (rc == SBK_OK)
+        rc = hypermix_forward(static_cast<const __half*>(x_dev), B, T, d, nhead, k, lens_dev,
+                              reinterpret_cast<const float*>(base + off_pe), w, reinterpret_cast<float*>(base + off_part),
+                              reinterpret_cast<__half*>(base + off_g), reinterpret_cast<float*>(base + off_s), out_dev, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("hypermix_test: device error"); rc = SBK_ERR_CUDA; }
+    cudaFree(base);
     return rc;
 }
 

@@ -96,6 +96,21 @@ int csgu_forward(const __half* u, int B, int T, int C, const float* gamma, const
                  const float* bias, int K, float2* stats, __half* g, cudaStream_t stream);
 constexpr int CSGU_TAP_ROWS = 31;
 void csgu_repack_taps(const float* src, int C2, int K, float* dst);  // (C/2, 1, K) -> [CSGU_TAP_ROWS, C/2] (host)
+// HyperConformer token mixing (HyperMixing, tied=False): generator g = 0 (w1_gen) / 1 (w2_gen) with fc1 [M, e, e] and
+// fc2 [M, k, e] fp16 in the reference layout, fp32 biases [M, e] / [M, k]; ln_g / ln_b the module's LayerNorm [d]
+struct HyperMixWeights {
+    const __half *fc1w[2], *fc2w[2];
+    const float *fc1b[2], *fc2b[2];
+    const float *ln_g, *ln_b;
+};
+constexpr int HM_PE_ROWS = 3000;  // HyperMixing's own PositionalEncoding(d, max_length=3000)
+// x [B*T, d] fp32 += LayerNorm_hm(HyperMixing(h16)), h16 the norm1 output [B*T, d] fp16; M heads of e = d / M in {32, 64},
+// KH = d_ffn / M (multiple of 16, <= 256); pe [HM_PE_ROWS, d] fp32 (hypermix_pe_table); lens device int[B] (null: all T).
+// Scratch: part (hypermix_part_floats), G [B * d * KH] fp16, gscale [B * M] fp32.  T <= HM_PE_ROWS.
+int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, const int* lens, const float* pe,
+                     const HyperMixWeights& w, float* part, __half* G, float* gscale, float* x, cudaStream_t stream);
+size_t hypermix_part_floats(int B, int T, int d, int KH);
+void hypermix_pe_table(int d, float* dst);  // [HM_PE_ROWS, d] (host)
 // chunk > 0: Dynamic Chunk Convolution (inputs past the end of the output frame's chunk are zero)
 int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw,
                     const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk = 0);

@@ -72,7 +72,7 @@ class FbankHandle:
 class AsrEngine:
     """One repacked model on one GPU.  ``cfg`` keys: n_fft, hop, win (samples), n_mels, cnn_channels, input_size,
     d_model, nhead, num_encoder_layers, num_decoder_layers, d_ffn, vocab, kernel_size, attention_type
-    ("RoPEMHA"|"RelPosMHAXL"), decoder_activation ("gelu"|"relu"), max_length; encoder_module ("conformer" (default) |
+    ("RoPEMHA"|"RelPosMHAXL"|"hypermixing", the last with the Conformer only), decoder_activation ("gelu"|"relu"), max_length; encoder_module ("conformer" (default) |
     "branchformer") with csgu_linear_units and branchformer_activation ("gelu" (default) | "relu").
     ``state``: {reference key with recipe prefix: CPU fp32 tensor}."""
 
@@ -87,9 +87,10 @@ class AsrEngine:
         c.num_encoder_layers, c.num_decoder_layers = cfg["num_encoder_layers"], cfg["num_decoder_layers"]
         c.d_ffn, c.vocab, c.kernel_size = cfg["d_ffn"], cfg["vocab"], cfg.get("kernel_size", 31)
         att = cfg["attention_type"]
-        if att not in ("RoPEMHA", "RelPosMHAXL"):
-            raise NotImplementedError(f"attention_type={att!r}: only RoPEMHA and RelPosMHAXL are built")
-        c.attention_type = _lib.SBK_ATT_ROPE if att == "RoPEMHA" else _lib.SBK_ATT_RELPOS
+        att_types = {"RoPEMHA": _lib.SBK_ATT_ROPE, "RelPosMHAXL": _lib.SBK_ATT_RELPOS, "hypermixing": _lib.SBK_ATT_HYPERMIX}
+        if att not in att_types:
+            raise NotImplementedError(f"attention_type={att!r}: only RoPEMHA, RelPosMHAXL and hypermixing are built")
+        c.attention_type = att_types[att]
         c.decoder_activation = _lib.SBK_ACT_GELU if cfg.get("decoder_activation", "gelu") == "gelu" else _lib.SBK_ACT_RELU
         c.max_len = cfg.get("max_length", 2500)
         enc_module = cfg.get("encoder_module", "conformer")

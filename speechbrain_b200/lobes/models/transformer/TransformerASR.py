@@ -1,7 +1,9 @@
 """TransformerASR -- drop-in for speechbrain.lobes.models.transformer.TransformerASR.TransformerASR
-(TransformerASR.py:167-675) restricted to what the Conformer and Branchformer ASR recipes instantiate:
-encoder_module="conformer" with attention_type in {"RoPEMHA", "RelPosMHAXL"} and normalize_before=True, or
-encoder_module="branchformer" with attention_type="RelPosMHAXL" (Branchformer.py:92-410); causal=False.
+(TransformerASR.py:167-675) restricted to what the Conformer, HyperConformer and Branchformer ASR recipes instantiate:
+encoder_module="conformer" with attention_type in {"RoPEMHA", "RelPosMHAXL", "hypermixing"} and normalize_before=True
+(hypermixing: HyperMixing token mixing, nnet/hypermixing.py, with head width d_model / nhead of 32 or 64 and
+d_ffn / nhead a multiple of 16 up to 256), or encoder_module="branchformer" with attention_type="RelPosMHAXL"
+(Branchformer.py:92-410); causal=False.
 
 Same constructor kwargs, same state_dict keys (incl. the positional buffers), ``encode()`` on the sm_90a
 kernels.  ``decode()`` / ``forward()`` run teacher-forced on the KV-cached decoder step (the searchers in
@@ -14,6 +16,9 @@ import torch
 from ...._lib import require_cuda
 from ....utils.param_tree import _Node, build_param_tree, default_init
 from ....utils.shapes import transformer_asr_shapes
+
+
+HYPERMIXING_MAX_FRAMES = 3000  # HyperMixing(max_length=3000) (hypermixing.py:60): longer inputs fail in the reference
 
 
 def _sine_table(max_len, d):
@@ -46,8 +51,13 @@ class TransformerASR(torch.nn.Module):
         unsupported = []
         if encoder_module not in ("conformer", "branchformer"):
             unsupported.append(f"encoder_module={encoder_module!r}")
-        if attention_type not in ("RoPEMHA", "RelPosMHAXL"):
+        if attention_type not in ("RoPEMHA", "RelPosMHAXL", "hypermixing"):
             unsupported.append(f"attention_type={attention_type!r}")
+        if attention_type == "hypermixing" and encoder_module == "conformer":
+            if d_model % nhead or d_model // nhead not in (64, 32):
+                unsupported.append(f"hypermixing head width d_model / nhead = {d_model / max(nhead, 1):g} (32 or 64)")
+            if d_ffn % nhead or (d_ffn // nhead) % 16 or d_ffn // nhead > 256:
+                unsupported.append(f"hypermixing d_ffn / nhead = {d_ffn / max(nhead, 1):g} (a multiple of 16 up to 256)")
         bf_act = "gelu"
         if encoder_module == "branchformer":
             if attention_type != "RelPosMHAXL":
@@ -98,8 +108,17 @@ class TransformerASR(torch.nn.Module):
         elif positional_encoding == "fixed_abs_sine":
             self.positional_encoding = _Node()
             self.positional_encoding.register_buffer("pe", _sine_table(max_length, d_model))
-        self.positional_encoding_decoder = _Node()
-        self.positional_encoding_decoder.register_buffer("pe", _sine_table(max_length, d_model))
+        if attention_type == "hypermixing":
+            # no positional_encoding_decoder: the decoder adds positional_encoding (TransformerASR.py:455-466), the same
+            # table the engine computes; every HyperMixing layer keeps its own 3000-row table (hypermixing.py:74-81),
+            # one shared tensor here
+            pe_hm = _sine_table(HYPERMIXING_MAX_FRAMES, d_model)
+            for i in range(num_encoder_layers):
+                getattr(self.encoder.layers, str(i)).mha_layer.add_module("positional_encoding", _Node())
+                getattr(self.encoder.layers, str(i)).mha_layer.positional_encoding.register_buffer("pe", pe_hm)
+        else:
+            self.positional_encoding_decoder = _Node()
+            self.positional_encoding_decoder.register_buffer("pe", _sine_table(max_length, d_model))
         # engine slots (plain dict, not sub-modules): one shared device engine per set of modules wired to this model
         object.__setattr__(self, "_slots", {})
 
@@ -146,7 +165,10 @@ class TransformerASR(torch.nn.Module):
         ``dynchunktrain_config`` (a ``DynChunkTrainConfig``): chunked attention + Dynamic Chunk Convolution, i.e. the masked
         evaluation mode whose outputs equal chunk-by-chunk streaming (TransformerASR.py:46-105, Conformer.py:190-313).
         The Branchformer has no such mode (an AssertionError, like Branchformer.py:369) and needs more than
-        (kernel_size - 1) / 2 frames: its reflect-padded CSGU convolution fails on shorter inputs in the reference."""
+        (kernel_size - 1) / 2 frames: its reflect-padded CSGU convolution fails on shorter inputs in the reference.
+        HyperMixing ignores the chunked attention mask and mixes the whole utterance, so the masked mode would not equal
+        streaming (NotImplementedError), and it takes at most 3000 frames: its positional table fails to broadcast on
+        longer inputs in the reference (RuntimeError, raised here before any device work)."""
         if src.dim() == 4:
             bz, t, ch1, ch2 = src.shape
             src = src.reshape(bz, t, ch1 * ch2)
@@ -156,6 +178,13 @@ class TransformerASR(torch.nn.Module):
             if src.shape[1] <= halo:
                 raise RuntimeError(f"TransformerASR.encode: the Branchformer's reflect padding ({halo} frames) needs more than "
                                    f"{halo} frames, got {src.shape[1]}")
+        if self.attention_type == "hypermixing":
+            if dynchunktrain_config is not None:
+                raise NotImplementedError("TransformerASR: HyperMixing has no chunked (streaming-equivalent) mode: it "
+                                          "ignores the attention mask and mixes the whole utterance")
+            if src.shape[1] > HYPERMIXING_MAX_FRAMES:
+                raise RuntimeError(f"TransformerASR.encode: HyperMixing's positional table has {HYPERMIXING_MAX_FRAMES} "
+                                   f"rows, got {src.shape[1]} frames")
         require_cuda(src, "TransformerASR.encode")
         if wav_len is not None and float(wav_len.max()) < 1.0 - 1e-6:
             # the reference builds its mask with width max(abs_len) and then fails to broadcast (dataio.py:836)
@@ -176,6 +205,8 @@ class TransformerASR(torch.nn.Module):
         """Streaming context for ``encode_streaming`` (TransformerASR.py:645-670)."""
         if self.encoder_module == "branchformer":
             raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
+        if self.attention_type == "hypermixing":
+            raise NotImplementedError("TransformerASR: HyperMixing has no streaming mode")
         if dynchunktrain_config is None or dynchunktrain_config.chunk_size <= 0:
             raise ValueError("make_streaming_context needs a DynChunkTrainConfig with chunk_size > 0")
         return TransformerASRStreamingContext(dynchunktrain_config)
@@ -191,6 +222,8 @@ class TransformerASR(torch.nn.Module):
         new chunk: the same values, at the cost of recomputing the window instead of reusing per-layer caches."""
         if self.encoder_module == "branchformer":
             raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
+        if self.attention_type == "hypermixing":
+            raise NotImplementedError("TransformerASR: HyperMixing has no streaming mode")
         require_cuda(src, "TransformerASR.encode_streaming")
         cfg = context.dynchunktrain_config
         if src.dim() == 4:

@@ -104,6 +104,26 @@ BRANCHFORMER_CTC = dict(name="branchformer_ctc", sample_rate=16000, n_fft=512, w
                         num_decoder_layers=0, d_ffn=1024, vocab=31, kernel_size=31, attention_type="RelPosMHAXL",
                         decoder_activation="gelu", max_length=2500, encoder_module="branchformer",
                         csgu_linear_units=2400, branchformer_activation="gelu")
+def scale_hypernet(sd, gain=1.0):
+    """In place: every HyperMixing hypernetwork matrix (``hyper.w{1,2}_gen.fc{1,2}_weights``, (M, out, in)) rescaled to the
+    per-head xavier std gain * sqrt(2 / (in + out)).  seeded_tensor treats the (M, out, in) stack as one conv-like kernel and
+    gives it std sqrt(2 / (out * in + M * in)), 4-6x smaller: the generated W1 / W2 are then nearly the biases, the same for
+    every frame, and errors in the positional input or the per-frame hypernetwork would not show in the outputs."""
+    for k in list(sd):
+        if k.endswith("_gen.fc1_weights") or k.endswith("_gen.fc2_weights"):
+            w = sd[k]
+            M, o, i = w.shape
+            seeded = math.sqrt(2.0 / (o * i + M * i))
+            sd[k] = w * (gain * math.sqrt(2.0 / (i + o)) / seeded)
+    return sd
+
+
+# recipes/LibriSpeech/ASR/transformer/hparams/hyperconformer_22M.yaml: 10 Conformer layers with HyperMixing (8 heads of 32
+# channels, hypernetwork width d_ffn / 8 = 128 per head), 4 decoder layers, 5000 tokens
+HYPERCONFORMER_22M = dict(name="hyperconformer_22m", sample_rate=16000, n_fft=400, win=400, hop=160, n_mels=80,
+                          cnn_channels=(64, 32), input_size=640, d_model=256, nhead=8, num_encoder_layers=10,
+                          num_decoder_layers=4, d_ffn=1024, vocab=5000, kernel_size=31, attention_type="hypermixing",
+                          decoder_activation="gelu", max_length=2500)
 CONFORMER_SMALL = dict(name="conformer_small", sample_rate=16000, n_fft=400, win=400, hop=160, n_mels=80,
                        cnn_channels=(64, 32), input_size=640, d_model=144, nhead=4, num_encoder_layers=12,
                        num_decoder_layers=4, d_ffn=1024, vocab=5000, kernel_size=31, attention_type="RelPosMHAXL",
