@@ -243,6 +243,32 @@ int sbk_asr_transcribe_greedy_host_async(sbk_asr* m, const float* wav_host, cons
                                          int max_steps, int bos, int eos, int* pred_host, float* score_host,
                                          int* steps_done, void* stream);
 
+/* ---- CTC beam search without a language model: the frame loop of CTCBeamSearcher (decoders/ctc.py:1155-1485).
+ * Beams are keyed by polynomial hashes modulo 2^61 - 1 of their text and partial word, with base SBK_CTC_HASH_BASE over
+ * (code point + 1) per character, plus the string lengths.  The caller describes vocab_list[0 .. n_vocab) per token:
+ * tok_info [n_vocab][3] int32 = kind (SBK_CTC_TOK_*), string id (first index holding the same string), length in code
+ * points of the string the token appends (token[1:] for a word start, the token for a plain one, else 0);
+ * tok_hash [n_vocab][2] uint64 = hash of that string, base^length mod 2^61 - 1. */
+#define SBK_CTC_HASH_BASE 0x1F3D5B79A2C4E6F1ull
+enum { SBK_CTC_TOK_PLAIN = 0, SBK_CTC_TOK_BLANK = 1, SBK_CTC_TOK_WORD = 2, SBK_CTC_TOK_SPACE = 3 };
+typedef struct {
+    int blank, beam_size, prune_history;
+    /* float32 thresholds: token_prune_min_logp, beam_prune_logp, log(blank_skip_threshold) */
+    float token_prune_min_logp, beam_prune_logp, blank_skip_logp;
+} sbk_ctc_beam_params;
+/* Workspace for one search: runs the token-count pre-pass over log_probs_dev [B, T, V] fp32 with lens_dev [B] int32
+ * absolute frame counts (0..T) and synchronises the stream.  1 <= beam_size <= 256, V <= 8192, n_vocab <= V. */
+int sbk_ctc_beam_workspace_bytes(const float* log_probs_dev, const int* lens_dev, int B, int T, int V, int n_vocab,
+                                 const sbk_ctc_beam_params* params, size_t* bytes, void* stream);
+/* The search, one CTA per utterance.  Outputs: frame_beams [B, T] int32 = beams after frame f (-1: frame skipped;
+ * frames >= lens[b] untouched), parent / token [B, T, beam_size] int32 = each surviving beam's parent (rank at the previous
+ * processed frame) and token, score [B, beam_size] fp32 = final beam scores, n_final [B] int32 = final beam count (-1: a
+ * frame had no candidate token, which the reference fails on).  Synchronises the stream once (the pre-pass), then enqueues. */
+int sbk_ctc_beam_search(const float* log_probs_dev, const int* lens_dev, int B, int T, int V, int n_vocab,
+                        const int* tok_info_dev, const uint64_t* tok_hash_dev, const sbk_ctc_beam_params* params,
+                        void* workspace_dev, size_t workspace_bytes, int* frame_beams_dev, int* parent_dev, int* token_dev,
+                        float* score_dev, int* n_final_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

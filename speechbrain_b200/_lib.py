@@ -37,6 +37,12 @@ class sbk_beam_params(ctypes.Structure):
                 ("coverage_weight", ctypes.c_float), ("coverage_threshold", ctypes.c_float)]
 
 
+class sbk_ctc_beam_params(ctypes.Structure):
+    _fields_ = [("blank", ctypes.c_int), ("beam_size", ctypes.c_int), ("prune_history", ctypes.c_int),
+                ("token_prune_min_logp", ctypes.c_float), ("beam_prune_logp", ctypes.c_float),
+                ("blank_skip_logp", ctypes.c_float)]
+
+
 SBK_ATT_ROPE, SBK_ATT_RELPOS, SBK_ATT_HYPERMIX = 0, 1, 2
 SBK_ACT_RELU, SBK_ACT_GELU = 0, 1
 SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER = 0, 1
@@ -52,7 +58,7 @@ EXPORTS = [
     "sbk_asr_transcribe_greedy_host", "sbk_asr_transcribe_greedy_host_async", "sbk_asr_clone",
     "sbk_asr_set_poll_interval", "sbk_asr_beam_from_enc", "sbk_asr_set_decoder_ln_fusion", "sbk_asr_transcribe_greedy_group_dev",
     "sbk_asr_set_decoder_tc_min_rows", "sbk_asr_lm_rescore", "sbk_asr_transcribe_greedy_group_host_async", "sbk_asr_decode_teacher_forced", "sbk_asr_ctc_head", "sbk_rows_argmax_f32", "sbk_asr_set_dynchunk",
-    "sbk_asr_lm_forward", "sbk_asr_lm_step_logits",
+    "sbk_asr_lm_forward", "sbk_asr_lm_step_logits", "sbk_ctc_beam_workspace_bytes", "sbk_ctc_beam_search",
 ]
 
 

@@ -1,0 +1,527 @@
+// CTC beam search without a language model, sm_90a: the frame loop of CTCBeamSearcher.partial_decoding
+// (speechbrain/decoders/ctc.py:1298-1485) with merge_beams (:782-809), the beam prune and sort_beams (:811-824) and
+// _prune_history (:826-866).
+//
+// One persistent CTA per utterance walks all of that utterance's frames.  The reference keys a beam by STRINGS
+// (text, partial_word, last_token); here a beam carries polynomial hashes modulo 2^61 - 1 of its text and partial word
+// together with their lengths, the string id of its last token (the first vocabulary index holding the same string) and
+// the hash of the last word of its text (for the history pruning).  Per frame:
+//   1. skip the frame if lp[blank] > log(blank_skip_threshold);
+//   2. candidate tokens = {t < n_vocab : lp[t] > token_prune_min_logp} + argmax(lp), ascending;
+//   3. candidates (token-major, beams in rank order inside a token) extend their parent by the string rules and write
+//      their key and score to the workspace;
+//   4. an open-addressing table merges equal keys: the merged beam keeps the FIRST candidate's position and the LAST
+//      candidate's (parent, token), and its score folds the candidates' scores with np.logaddexp's float32 formula in
+//      candidate order;
+//   5. beams below max + beam_prune_logp go; a radix select finds the beam_size-th largest score and the kept beams are
+//      ranked by (score desc, position asc) -- heapq.nlargest's stable order;
+//   6. with prune_history, only the first beam per (last word of the text, partial word, last token) stays.
+// The CTA writes, per processed frame, the surviving beams' (parent, token) and their count, and the final scores; the
+// host replays the token chains of the final beams with exact strings (decoders/ctc.py in this package).
+#include <vector>
+
+#include "common.cuh"
+#include "sbk_internal.h"
+#include "../../include/sbk.h"
+
+namespace sbk {
+
+namespace {
+
+constexpr int CB_THREADS = 512;
+constexpr int CB_NW = CB_THREADS / 32;
+constexpr int CB_MAX_BEAM = 256;
+constexpr int CB_MAX_VOCAB = 8192;
+constexpr uint64_t HP = (1ull << 61) - 1;
+constexpr uint64_t HBASE = SBK_CTC_HASH_BASE;
+constexpr uint64_t HSEP = 33;   // ' ': characters are hashed as code point + 1
+
+__device__ __forceinline__ uint64_t hmul(uint64_t a, uint64_t b) {   // a * b mod 2^61 - 1, a, b < 2^61 - 1
+    const uint64_t lo = a * b, hi = __umul64hi(a, b);
+    uint64_t r = (lo & HP) + ((lo >> 61) | (hi << 3));
+    r = (r & HP) + (r >> 61);
+    return r >= HP ? r - HP : r;
+}
+__device__ __forceinline__ uint64_t hadd(uint64_t a, uint64_t b) {
+    const uint64_t r = a + b;
+    return r >= HP ? r - HP : r;
+}
+
+// np.logaddexp for float32 (npy_logaddexpf)
+__device__ __forceinline__ float logaddexp_np(float x, float y) {
+    if (x == y) return __fadd_rn(x, 0.693147180559945309417232121458176568f);
+    const float tmp = __fsub_rn(x, y);
+    if (tmp > 0.0f) return __fadd_rn(x, log1pf(expf(-tmp)));
+    if (tmp <= 0.0f) return __fadd_rn(y, log1pf(expf(tmp)));
+    return tmp;
+}
+
+// order-preserving float -> uint32 (-0 and +0 map to the same key); 0 is never a finite score's key
+__device__ __forceinline__ uint32_t score_key(float s) {
+    const uint32_t u = __float_as_uint(s == 0.0f ? 0.0f : s);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+struct BeamS {
+    uint64_t th, ph, pp, wh;   // hash of text, of partial word, P^len(partial), hash of the text's last word
+    int tl, pl, wl, sid;       // their lengths; string id of the last token (-1 = None)
+};
+
+// One candidate: beam s extended by token t (decoders/ctc.py:1359-1459).
+__device__ __forceinline__ BeamS extend(const BeamS& s, int kind, int tsid, uint64_t thash, uint64_t tpow, int tlen) {
+    BeamS n = s;
+    n.sid = tsid;
+    if (kind == SBK_CTC_TOK_BLANK || tsid == s.sid) return n;   // blank or repeated token: only the last token changes
+    if (kind == SBK_CTC_TOK_WORD || kind == SBK_CTC_TOK_SPACE) {   // the partial word is committed: merge_tokens(text, partial)
+        if (s.pl > 0) {
+            if (s.tl == 0) { n.th = s.ph; n.tl = s.pl; }
+            else { n.th = hadd(hmul(hadd(hmul(s.th, HBASE), HSEP), s.pp), s.ph); n.tl = s.tl + 1 + s.pl; }
+            n.wh = s.ph; n.wl = s.pl;
+        }
+        if (kind == SBK_CTC_TOK_WORD) { n.ph = thash; n.pl = tlen; n.pp = tpow; }
+        else { n.ph = 0; n.pl = 0; n.pp = 1; }
+        return n;
+    }
+    n.ph = hadd(hmul(s.ph, tpow), thash);
+    n.pl = s.pl + tlen;
+    n.pp = hmul(s.pp, tpow);
+    return n;
+}
+
+__device__ __forceinline__ uint32_t key_slot(uint64_t th, uint64_t ph, int tl, int pl, int sid) {
+    uint64_t h = th * 0x9E3779B97F4A7C15ull;
+    h ^= (ph + 0x632BE59BD9B4E019ull) * 0xC2B2AE3D27D4EB4Full;
+    h ^= ((static_cast<uint64_t>(tl) << 40) ^ (static_cast<uint64_t>(pl) << 20) ^ static_cast<uint32_t>(sid)) * 0x165667B19E3779F9ull;
+    h ^= h >> 29;
+    h *= 0xBF58476D1CE4E5B9ull;
+    h ^= h >> 32;
+    return static_cast<uint32_t>(h);
+}
+
+// Ordered compaction: the rank of this thread's flag among the set flags of lower threads; *total = set flags in the block.
+// Every thread must call it; it synchronises the block twice.
+__device__ __forceinline__ int block_rank(bool flag, int* s_w, int* total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const unsigned m = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) s_w[w] = __popc(m);
+    __syncthreads();
+    int off = 0, tot = 0;
+#pragma unroll
+    for (int i = 0; i < CB_NW; ++i) {
+        const int v = s_w[i];
+        off += i < w ? v : 0;
+        tot += v;
+    }
+    __syncthreads();
+    *total = tot;
+    return off + __popc(m & ((1u << lane) - 1u));
+}
+
+__device__ __forceinline__ float block_max(float v, float* s_f) {
+    v = warp_max(v);
+    if ((threadIdx.x & 31) == 0) s_f[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float r = s_f[0];
+    for (int i = 1; i < static_cast<int>(blockDim.x >> 5); ++i) r = fmaxf(r, s_f[i]);
+    __syncthreads();
+    return r;
+}
+
+// arg-max of a row, first index on ties (np.argmax)
+__device__ __forceinline__ int block_argmax(const float* col, int V, float* s_f, int* s_i) {
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int j = threadIdx.x; j < V; j += blockDim.x) {
+        const float v = col[j];
+        if (v > best || (v == best && j < bi)) { best = v; bi = j; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+    }
+    if ((threadIdx.x & 31) == 0) { s_f[threadIdx.x >> 5] = best; s_i[threadIdx.x >> 5] = bi; }
+    __syncthreads();
+    best = s_f[0]; bi = s_i[0];
+    for (int w = 1; w < static_cast<int>(blockDim.x >> 5); ++w)
+        if (s_f[w] > best || (s_f[w] == best && s_i[w] < bi)) { best = s_f[w]; bi = s_i[w]; }
+    __syncthreads();
+    return bi;
+}
+
+// Pre-pass: the largest candidate-token count of any processed frame (sizes the candidate workspace).
+__global__ void __launch_bounds__(256) ctc_beam_count_kernel(const float* __restrict__ lp, const int* __restrict__ lens, int T, int V,
+                                                             int nv, int blank, float tok_thr, float skip_thr, int* max_count) {
+    __shared__ float s_f[8];
+    __shared__ int s_i[8];
+    const int row = blockIdx.x, b = row / T, f = row - b * T;
+    if (f >= lens[b]) return;
+    const float* col = lp + static_cast<size_t>(row) * V;
+    if (col[blank] > skip_thr) return;
+    const int am = block_argmax(col, V, s_f, s_i);
+    int cnt = 0;
+    for (int j = threadIdx.x; j < nv; j += blockDim.x) cnt += (col[j] > tok_thr || j == am) ? 1 : 0;
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    if ((threadIdx.x & 31) == 0) s_i[threadIdx.x >> 5] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int tot = 0;
+        for (int w = 0; w < 8; ++w) tot += s_i[w];
+        atomicMax(max_count, tot);
+    }
+}
+
+struct CbArgs {
+    const float* lp; const int* lens;
+    int T, V, nv;
+    const int* tok_i;          // [nv][3]: kind, string id, length of the appended string
+    const uint64_t* tok_u;     // [nv][2]: hash of the appended string, P^length
+    int blank, beam, prune_history;
+    float tok_thr, beam_thr, skip_thr;
+    char* ws; size_t ws_stride; int cmax, hcap;
+    int* out_n; int* out_par; int* out_tok; float* out_score; int* out_final;
+};
+
+__host__ __device__ inline size_t cb_align(size_t x) { return (x + 255) & ~static_cast<size_t>(255); }
+
+__host__ __device__ inline size_t cb_stride(int cmax, int hcap) {
+    return 2 * cb_align(static_cast<size_t>(cmax) * 8) + 9 * cb_align(static_cast<size_t>(cmax) * 4) +
+           3 * cb_align(static_cast<size_t>(hcap) * 4);
+}
+
+__global__ void __launch_bounds__(CB_THREADS, 1) ctc_beam_kernel(const CbArgs a) {
+    extern __shared__ int s_tok[];   // [nv] candidate tokens of the frame, ascending
+    __shared__ float s_sc[2][CB_MAX_BEAM];
+    __shared__ uint64_t s_th[2][CB_MAX_BEAM], s_ph[2][CB_MAX_BEAM], s_pp[2][CB_MAX_BEAM], s_wh[2][CB_MAX_BEAM];
+    __shared__ int s_tl[2][CB_MAX_BEAM], s_pl[2][CB_MAX_BEAM], s_wl[2][CB_MAX_BEAM], s_sid[2][CB_MAX_BEAM];
+    __shared__ int s_kept[CB_MAX_BEAM];
+    __shared__ uint32_t s_kkey[CB_MAX_BEAM];
+    __shared__ int s_ord[CB_MAX_BEAM];
+    __shared__ int s_hist[256];
+    __shared__ int s_w[CB_NW];
+    __shared__ float s_f[CB_NW];
+    __shared__ int s_i[CB_NW];
+    const int b = blockIdx.x, tid = threadIdx.x, T = a.T, V = a.V, beam = a.beam;
+
+    // workspace of this utterance (layout: cb_stride)
+    char* w = a.ws + static_cast<size_t>(b) * a.ws_stride;
+    const size_t c8 = cb_align(static_cast<size_t>(a.cmax) * 8), c4 = cb_align(static_cast<size_t>(a.cmax) * 4);
+    uint64_t* c_th = reinterpret_cast<uint64_t*>(w); w += c8;
+    uint64_t* c_ph = reinterpret_cast<uint64_t*>(w); w += c8;
+    float* c_sc = reinterpret_cast<float*>(w); w += c4;
+    int* c_tl = reinterpret_cast<int*>(w); w += c4;
+    int* c_pl = reinterpret_cast<int*>(w); w += c4;
+    int* c_sid = reinterpret_cast<int*>(w); w += c4;
+    int* c_slot = reinterpret_cast<int*>(w); w += c4;
+    int* u_cand = reinterpret_cast<int*>(w); w += c4;
+    int* u_last = reinterpret_cast<int*>(w); w += c4;
+    float* u_sc = reinterpret_cast<float*>(w); w += c4;
+    uint32_t* u_key = reinterpret_cast<uint32_t*>(w); w += c4;
+    const size_t h4 = cb_align(static_cast<size_t>(a.hcap) * 4);
+    int* tab_idx = reinterpret_cast<int*>(w); w += h4;
+    int* tab_first = reinterpret_cast<int*>(w); w += h4;
+    int* tab_last = reinterpret_cast<int*>(w);
+
+    const int n = a.lens[b];
+    int cur = 0, nb = 1;
+    if (tid == 0) {
+        s_sc[0][0] = 0.0f;
+        s_th[0][0] = 0; s_ph[0][0] = 0; s_pp[0][0] = 1; s_wh[0][0] = 0;
+        s_tl[0][0] = 0; s_pl[0][0] = 0; s_wl[0][0] = 0; s_sid[0][0] = -1;
+    }
+    __syncthreads();
+    auto load = [&](int buf, int i) {
+        BeamS s;
+        s.th = s_th[buf][i]; s.ph = s_ph[buf][i]; s.pp = s_pp[buf][i]; s.wh = s_wh[buf][i];
+        s.tl = s_tl[buf][i]; s.pl = s_pl[buf][i]; s.wl = s_wl[buf][i]; s.sid = s_sid[buf][i];
+        return s;
+    };
+    auto store = [&](int buf, int i, const BeamS& s) {
+        s_th[buf][i] = s.th; s_ph[buf][i] = s.ph; s_pp[buf][i] = s.pp; s_wh[buf][i] = s.wh;
+        s_tl[buf][i] = s.tl; s_pl[buf][i] = s.pl; s_wl[buf][i] = s.wl; s_sid[buf][i] = s.sid;
+    };
+    auto extend_tok = [&](const BeamS& s, int t) {
+        const int* ti = a.tok_i + 3 * t;
+        return extend(s, ti[0], ti[1], a.tok_u[2 * t], a.tok_u[2 * t + 1], ti[2]);
+    };
+
+    for (int f = 0; f < n; ++f) {
+        const float* col = a.lp + (static_cast<size_t>(b) * T + f) * V;
+        int* on = a.out_n + static_cast<size_t>(b) * T + f;
+        if (col[a.blank] > a.skip_thr) {   // skipped frames still count in the frame numbering
+            if (tid == 0) *on = -1;
+            continue;
+        }
+        // ---- 2. candidate tokens
+        const int am = block_argmax(col, V, s_f, s_i);
+        int ntok = 0;
+        for (int base = 0; base < a.nv; base += CB_THREADS) {
+            const int j = base + tid;
+            const bool fl = j < a.nv && (col[j] > a.tok_thr || j == am);
+            int tot;
+            const int r = block_rank(fl, s_w, &tot);
+            if (fl) s_tok[ntok + r] = j;
+            ntok += tot;
+        }
+        if (ntok == 0) {   // the arg-max lies outside vocab_list and nothing passes the token threshold: no candidate
+            if (tid == 0) { *on = -2; a.out_final[b] = -1; }
+            return;
+        }
+        __syncthreads();
+        // ---- 3. candidates, token-major
+        const int C = ntok * nb;
+        int H = 64;
+        while (H < 2 * C) H <<= 1;
+        for (int c = tid; c < C; c += CB_THREADS) {
+            const int q = c / nb, p = c - q * nb, t = s_tok[q];
+            const BeamS s = extend_tok(load(cur, p), t);
+            c_th[c] = s.th; c_ph[c] = s.ph; c_tl[c] = s.tl; c_pl[c] = s.pl; c_sid[c] = s.sid;
+            c_sc[c] = __fadd_rn(s_sc[cur][p], col[t]);
+        }
+        for (int h = tid; h < H; h += CB_THREADS) { tab_idx[h] = -1; tab_first[h] = 0x7fffffff; tab_last[h] = -1; }
+        __syncthreads();
+        // ---- 4. merge equal keys
+        for (int c = tid; c < C; c += CB_THREADS) {
+            const uint64_t th = c_th[c], ph = c_ph[c];
+            const int tl = c_tl[c], pl = c_pl[c], sid = c_sid[c];
+            uint32_t slot = key_slot(th, ph, tl, pl, sid) & (H - 1);
+            for (;;) {
+                const int o = atomicCAS(&tab_idx[slot], -1, c);
+                if (o == -1 || (c_th[o] == th && c_ph[o] == ph && c_tl[o] == tl && c_pl[o] == pl && c_sid[o] == sid)) break;
+                slot = (slot + 1) & (H - 1);
+            }
+            c_slot[c] = static_cast<int>(slot);
+            atomicMin(&tab_first[slot], c);
+            atomicMax(&tab_last[slot], c);
+        }
+        __syncthreads();
+        int U = 0;
+        for (int base = 0; base < C; base += CB_THREADS) {
+            const int c = base + tid;
+            const bool fl = c < C && tab_first[c_slot[c]] == c;
+            int tot;
+            const int r = block_rank(fl, s_w, &tot);
+            if (fl) u_cand[U + r] = c;
+            U += tot;
+        }
+        __syncthreads();
+        float lmax = -INFINITY;
+        for (int u = tid; u < U; u += CB_THREADS) {
+            const int r = u_cand[u], slot = c_slot[r], last = tab_last[slot];
+            float s = c_sc[r];
+            for (int c = r + 1; c <= last; ++c)
+                if (c_slot[c] == slot) s = logaddexp_np(s, c_sc[c]);
+            u_sc[u] = s;
+            u_last[u] = last;
+            lmax = fmaxf(lmax, s);
+        }
+        const float mx = block_max(lmax, s_f);
+        // ---- 5. prune: score >= max + beam_prune_logp, then the beam_size best (stable)
+        const float thr = __fadd_rn(mx, a.beam_thr);
+        int ns_loc = 0;
+        for (int u = tid; u < U; u += CB_THREADS) {
+            const float s = u_sc[u];
+            const bool ok = s >= thr;
+            u_key[u] = ok ? score_key(s) : 0u;
+            ns_loc += ok ? 1 : 0;
+        }
+        ns_loc = __reduce_add_sync(0xffffffffu, ns_loc);
+        if ((tid & 31) == 0) s_w[tid >> 5] = ns_loc;
+        __syncthreads();
+        int ns = 0;
+        for (int i = 0; i < CB_NW; ++i) ns += s_w[i];
+        __syncthreads();
+        uint32_t K = 0;
+        int rem = 0;
+        const bool select = ns > beam;
+        if (select) {   // radix select of the beam-th largest key, 8 bits per pass
+            uint32_t prefix = 0, mask = 0;
+            rem = beam;
+            for (int shift = 24; shift >= 0; shift -= 8) {
+                for (int i = tid; i < 256; i += CB_THREADS) s_hist[i] = 0;
+                __syncthreads();
+                for (int u = tid; u < U; u += CB_THREADS) {
+                    const uint32_t k = u_key[u];
+                    if (k != 0u && (k & mask) == prefix) atomicAdd(&s_hist[(k >> shift) & 255u], 1);
+                }
+                __syncthreads();
+                if (tid == 0) {
+                    int acc = 0, d = 255;
+                    for (; d > 0; --d) {
+                        if (acc + s_hist[d] >= rem) break;
+                        acc += s_hist[d];
+                    }
+                    s_i[0] = d;
+                    s_i[1] = rem - acc;
+                }
+                __syncthreads();
+                prefix |= static_cast<uint32_t>(s_i[0]) << shift;
+                mask |= 255u << shift;
+                rem = s_i[1];
+                __syncthreads();
+            }
+            K = prefix;   // beam - rem keys are larger than K; the first rem keys equal to K (by position) are kept too
+        }
+        int nk = 0, neq = 0;
+        for (int base = 0; base < U; base += CB_THREADS) {
+            const int u = base + tid;
+            const uint32_t k = u < U ? u_key[u] : 0u;
+            const bool eq = select && k != 0u && k == K;
+            int tot_eq;
+            const int r_eq = block_rank(eq, s_w, &tot_eq);
+            const bool keep = k != 0u && (!select || k > K || (eq && neq + r_eq < rem));
+            int tot;
+            const int r = block_rank(keep, s_w, &tot);
+            if (keep) { s_kept[nk + r] = u; s_kkey[nk + r] = k; }
+            nk += tot;
+            neq += tot_eq;
+        }
+        __syncthreads();
+        if (tid < nk) {
+            const uint32_t k = s_kkey[tid];
+            int rk = 0;
+            for (int j = 0; j < nk; ++j) {
+                const uint32_t kj = s_kkey[j];
+                rk += (kj > k || (kj == k && j < tid)) ? 1 : 0;
+            }
+            s_ord[rk] = tid;
+        }
+        __syncthreads();
+        // the kept beams in rank order: state from the LAST merged candidate's (parent, token)
+        const int nxt = cur ^ 1;
+        BeamS ns_state = {};
+        float my_sc = 0.0f;
+        int my_par = 0, my_tok = 0;
+        if (tid < nk) {
+            const int u = s_kept[s_ord[tid]], c = u_last[u];
+            const int q = c / nb;
+            my_par = c - q * nb;
+            my_tok = s_tok[q];
+            my_sc = u_sc[u];
+            ns_state = extend_tok(load(cur, my_par), my_tok);
+            store(nxt, tid, ns_state);
+        }
+        __syncthreads();
+        // ---- 6. history pruning: the first beam per (last word of the text, partial word, last token)
+        bool keep = tid < nk;
+        if (a.prune_history && keep) {
+            for (int j = 0; j < tid; ++j)
+                if (s_wl[nxt][j] == ns_state.wl && s_wh[nxt][j] == ns_state.wh && s_pl[nxt][j] == ns_state.pl &&
+                    s_ph[nxt][j] == ns_state.ph && s_sid[nxt][j] == ns_state.sid) { keep = false; break; }
+        }
+        int nfin;
+        const int r = block_rank(keep, s_w, &nfin);   // (its barriers also separate the reads above from the writes below)
+        if (keep) {
+            store(nxt, r, ns_state);
+            s_sc[nxt][r] = my_sc;
+            const size_t o = (static_cast<size_t>(b) * T + f) * beam + r;
+            a.out_par[o] = my_par;
+            a.out_tok[o] = my_tok;
+        }
+        if (tid == 0) *on = nfin;
+        __syncthreads();
+        cur = nxt;
+        nb = nfin;
+    }
+    if (tid < nb) a.out_score[static_cast<size_t>(b) * beam + tid] = s_sc[cur][tid];
+    if (tid == 0) a.out_final[b] = nb;
+}
+
+int cb_check(const float* lp, const int* lens, int B, int T, int V, int nv, const sbk_ctc_beam_params* p, cudaStream_t st,
+             std::vector<int>& len_host) {
+    SBK_REQUIRE(lp && lens && p, "ctc_beam: null pointer");
+    SBK_REQUIRE(B >= 1 && T >= 1 && V >= 1, "ctc_beam: bad sizes B=%d T=%d V=%d", B, T, V);
+    SBK_REQUIRE(V <= CB_MAX_VOCAB, "ctc_beam: V=%d above the supported %d", V, CB_MAX_VOCAB);
+    SBK_REQUIRE(nv >= 1 && nv <= V, "ctc_beam: n_vocab=%d outside [1, V=%d]", nv, V);
+    SBK_REQUIRE(p->beam_size >= 1 && p->beam_size <= CB_MAX_BEAM, "ctc_beam: beam_size=%d outside [1, %d]", p->beam_size, CB_MAX_BEAM);
+    SBK_REQUIRE(p->blank >= 0 && p->blank < V, "ctc_beam: blank index %d outside [0, %d)", p->blank, V);
+    len_host.resize(B);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(len_host.data(), lens, B * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int v : len_host) SBK_REQUIRE(v >= 0 && v <= T, "ctc_beam: length %d outside [0, %d]", v, T);
+    return SBK_OK;
+}
+
+// largest candidate-token count over the processed frames (synchronises the stream)
+int cb_max_tokens(const float* lp, const int* lens, int B, int T, int V, int nv, const sbk_ctc_beam_params* p, cudaStream_t st,
+                  int* out) {
+    int* d = nullptr;
+    SBK_CUDA_CHECK(cudaMallocAsync(&d, sizeof(int), st));
+    SBK_CUDA_CHECK(cudaMemsetAsync(d, 0, sizeof(int), st));
+    ctc_beam_count_kernel<<<B * T, 256, 0, st>>>(lp, lens, T, V, nv, p->blank, p->token_prune_min_logp, p->blank_skip_logp, d);
+    cudaError_t e = cudaGetLastError();
+    count_launch();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d, sizeof(int), cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(d, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    SBK_CUDA_CHECK(e);
+    return SBK_OK;
+}
+
+void cb_sizes(int max_tok, int beam, int* cmax, int* hcap) {
+    *cmax = std::max(1, max_tok * beam);
+    int h = 64;
+    while (h < 2 * *cmax) h <<= 1;
+    *hcap = h;
+}
+
+}  // namespace
+
+}  // namespace sbk
+
+extern "C" {
+
+int sbk_ctc_beam_workspace_bytes(const float* log_probs_dev, const int* lens_dev, int B, int T, int V, int n_vocab,
+                                 const sbk_ctc_beam_params* p, size_t* bytes, void* stream) {
+    using namespace sbk;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(bytes, "ctc_beam: null pointer");
+    std::vector<int> len;
+    int rc = cb_check(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, len);
+    if (rc) return rc;
+    int mt = 0, cmax, hcap;
+    rc = cb_max_tokens(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, &mt);
+    if (rc) return rc;
+    cb_sizes(mt, p->beam_size, &cmax, &hcap);
+    *bytes = static_cast<size_t>(B) * cb_stride(cmax, hcap);
+    return SBK_OK;
+}
+
+int sbk_ctc_beam_search(const float* log_probs_dev, const int* lens_dev, int B, int T, int V, int n_vocab,
+                        const int* tok_info_dev, const uint64_t* tok_hash_dev, const sbk_ctc_beam_params* p,
+                        void* workspace_dev, size_t workspace_bytes, int* frame_beams_dev, int* parent_dev, int* token_dev,
+                        float* score_dev, int* n_final_dev, void* stream) {
+    using namespace sbk;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(tok_info_dev && tok_hash_dev && workspace_dev && frame_beams_dev && parent_dev && token_dev && score_dev &&
+                n_final_dev, "ctc_beam: null pointer");
+    std::vector<int> len;
+    int rc = cb_check(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, len);
+    if (rc) return rc;
+    int mt = 0, cmax, hcap;
+    rc = cb_max_tokens(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, &mt);
+    if (rc) return rc;
+    cb_sizes(mt, p->beam_size, &cmax, &hcap);
+    const size_t stride = cb_stride(cmax, hcap);
+    SBK_REQUIRE(workspace_bytes >= static_cast<size_t>(B) * stride,
+                "ctc_beam: workspace of %zu bytes, this input needs %zu (sbk_ctc_beam_workspace_bytes)", workspace_bytes,
+                static_cast<size_t>(B) * stride);
+    static bool attr = false;
+    if (!attr) {
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(ctc_beam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CB_MAX_VOCAB * 4));
+        attr = true;
+    }
+    CbArgs a;
+    a.lp = log_probs_dev; a.lens = lens_dev; a.T = T; a.V = V; a.nv = n_vocab;
+    a.tok_i = tok_info_dev; a.tok_u = tok_hash_dev;
+    a.blank = p->blank; a.beam = p->beam_size; a.prune_history = p->prune_history ? 1 : 0;
+    a.tok_thr = p->token_prune_min_logp; a.beam_thr = p->beam_prune_logp; a.skip_thr = p->blank_skip_logp;
+    a.ws = static_cast<char*>(workspace_dev); a.ws_stride = stride; a.cmax = cmax; a.hcap = hcap;
+    a.out_n = frame_beams_dev; a.out_par = parent_dev; a.out_tok = token_dev; a.out_score = score_dev; a.out_final = n_final_dev;
+    ctc_beam_kernel<<<B, CB_THREADS, static_cast<size_t>(n_vocab) * 4, st>>>(a);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
+}  // extern "C"

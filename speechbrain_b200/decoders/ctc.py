@@ -1,9 +1,20 @@
 """CTC greedy decoding -- mirror of speechbrain.decoders.ctc.{filter_ctc_output, ctc_greedy_decode} (decoders/ctc.py:298-378)
 for CUDA tensors: the per-frame arg-max runs in ``rows_logsoftmax_argmax_kernel`` (csrc/ctc_scorer.cu), the merge / blank
-filter of at most T integers per utterance stays on the host like in the reference."""
+filter of at most T integers per utterance stays on the host like in the reference.  CTCBeamSearcher (decoders/ctc.py:510-1485,
+no language model): the frame loop runs in ``ctc_beam_kernel`` (csrc/ctc_beam.cu), the replay of the surviving token chains
+and finalize_decoding on the host."""
+import dataclasses
+import heapq
+import logging
+import math
+import warnings
 from itertools import groupby
+from typing import Optional
 
+import numpy as np
 import torch
+
+logger = logging.getLogger(__name__)
 
 
 def filter_ctc_output(string_pred, blank_id=-1):
@@ -44,3 +55,231 @@ def greedy_from_argmax(pred, seq_lens, blank_id, batch_max_len=None):
         actual_size = int(torch.round(seq_len * batch_max_len))
         out.append(filter_ctc_output(seq[:actual_size], blank_id=blank_id))
     return out
+
+
+# --------------------------------------------------------------------------------------------------- CTC beam search
+@dataclasses.dataclass
+class CTCHypothesis:
+    """decoders/ctc.py:510-537."""
+    text: str
+    last_lm_state: None
+    score: float
+    lm_score: float
+    text_frames: Optional[list] = None
+
+
+_HASH_P = (1 << 61) - 1
+_HASH_BASE = 0x1F3D5B79A2C4E6F1  # SBK_CTC_HASH_BASE (include/sbk.h)
+_PLAIN, _BLANK, _WORD, _SPACE = 0, 1, 2, 3  # SBK_CTC_TOK_*
+MAX_BEAM, MAX_VOCAB = 256, 8192
+
+
+def _merge_words(a, b):
+    """CTCBaseSearcher.merge_tokens (decoders/ctc.py:757-780)."""
+    if not b:
+        return a
+    if not a:
+        return b
+    return a + " " + b
+
+
+class CTCBeamSearcher(torch.nn.Module):
+    """Mirror of speechbrain.decoders.ctc.CTCBeamSearcher (decoders/ctc.py:540-1485) without a language model, for CUDA
+    log-probabilities [B, T, V] fp32.  The frame loop (token pruning, extension, merging of beams with equal
+    (text, partial word, last token), beam pruning, stable top-beam_size sort and history pruning) runs in
+    ``ctc_beam_kernel`` (csrc/ctc_beam.cu), one CTA per utterance, on string hashes; the host then replays the string
+    rules on the surviving token chains and runs finalize_decoding (commit, merge by text, prune, sort) exactly, in
+    NumPy float32.  Constructor keywords and defaults are the reference's; ``kenlm_model_path`` raises
+    NotImplementedError, ``beam_size`` is limited to 256 and the log-probabilities' last dimension to 8192."""
+
+    def __init__(self, blank_index, vocab_list, space_token=" ", kenlm_model_path=None, unigrams=None, alpha=0.5, beta=1.5,
+                 unk_score_offset=-10.0, score_boundary=True, beam_size=100, beam_prune_logp=-10.0,
+                 token_prune_min_logp=-5.0, prune_history=True, blank_skip_threshold=1.0, topk=1, spm_token="▁"):
+        super().__init__()
+        if kenlm_model_path is not None:
+            raise NotImplementedError("speechbrain_b200.CTCBeamSearcher: KenLM scoring is not built")
+        if not 1 <= int(beam_size) <= MAX_BEAM:
+            raise ValueError(f"CTCBeamSearcher: beam_size={beam_size} outside [1, {MAX_BEAM}]")
+        self.blank_index = blank_index
+        self.vocab_list = vocab_list
+        self.space_token = space_token
+        self.kenlm_model_path = kenlm_model_path
+        self.unigrams = unigrams
+        self.alpha, self.beta, self.unk_score_offset, self.score_boundary = alpha, beta, unk_score_offset, score_boundary
+        self.beam_size = int(beam_size)
+        self.beam_prune_logp = beam_prune_logp
+        self.token_prune_min_logp = token_prune_min_logp
+        self.prune_history = prune_history
+        self.blank_skip_threshold = math.log(blank_skip_threshold)
+        self.topk = topk
+        self.spm_token = spm_token
+        self.lm = None
+        self.is_spm = any(str(s).startswith(spm_token) for s in vocab_list)
+        if not self.is_spm:
+            try:
+                self.space_index = vocab_list.index(space_token)
+            except ValueError:
+                logger.warning(f"space_token `{space_token}` not found in the vocabulary.Using value -1 as `space_index`."
+                               "Note: If your transcription is not expected to contain spaces, you can ignore this warning.")
+                self.space_index = -1
+        # per-token tables: kind, string id, appended string (its hash, base^length, length)
+        kinds, sids, app, first = [], [], [], {}
+        for i, s in enumerate(vocab_list):
+            if i == blank_index:
+                k = _BLANK
+            elif self.is_spm and s[:1] == spm_token:
+                k = _WORD
+            elif not self.is_spm and i == self.space_index:
+                k = _SPACE
+            else:
+                k = _PLAIN
+            kinds.append(k)
+            sids.append(first.setdefault(s, i))
+            app.append(s[1:] if k == _WORD else (s if k == _PLAIN else ""))
+        if prune_history and any(a and a.split() != [a] for a in app):
+            # the device keys the history by the last committed word, which needs whitespace-free token strings
+            raise NotImplementedError("CTCBeamSearcher: prune_history with tokens that contain whitespace is not built")
+        info, hashes = [], []
+        for k, sid, a in zip(kinds, sids, app):
+            h = 0
+            for ch in a:
+                h = (h * _HASH_BASE + ord(ch) + 1) % _HASH_P
+            info.append((k, sid, len(a)))
+            hashes.append((h, pow(_HASH_BASE, len(a), _HASH_P)))
+        self._kind = np.array(kinds, dtype=np.int64)
+        self._sid = np.array(sids + [-1], dtype=np.int64)  # [-1]: "no token yet"
+        self._app = app
+        self._info = torch.tensor(info, dtype=torch.int32).reshape(-1, 3)
+        self._hash = torch.tensor(np.array(hashes, dtype=np.uint64).view(np.int64)).reshape(-1, 2)
+        self._dev_tables = {}
+
+    def _tables(self, device):
+        if device not in self._dev_tables:
+            self._dev_tables[device] = (self._info.to(device).contiguous(), self._hash.to(device).contiguous())
+        return self._dev_tables[device]
+
+    def _params(self, blank):
+        from .._lib import sbk_ctc_beam_params
+        return sbk_ctc_beam_params(blank=blank, beam_size=self.beam_size, prune_history=int(bool(self.prune_history)),
+                                   token_prune_min_logp=float(np.float32(self.token_prune_min_logp)),
+                                   beam_prune_logp=float(np.float32(self.beam_prune_logp)),
+                                   blank_skip_logp=float(np.float32(self.blank_skip_threshold)))
+
+    @torch.no_grad()
+    def search(self, log_probs, lens):
+        """The device search alone: log_probs [B, T, V] fp32 CUDA, lens list of absolute frame counts -> per-frame beam
+        counts [B, T], parents and tokens [B, T, beam_size], final scores [B, beam_size], final counts [B] (device)."""
+        import ctypes
+
+        from .._lib import check, lib, ptr, stream_ptr
+        B, T, V = log_probs.shape
+        dev = log_probs.device
+        nv = min(V, len(self.vocab_list))
+        blank = self.blank_index
+        if not (isinstance(blank, int) and 0 <= blank < V):
+            raise ValueError(f"CTCBeamSearcher: blank_index {blank} outside [0, {V})")
+        if V > MAX_VOCAB:
+            raise ValueError(f"CTCBeamSearcher: vocabulary dimension {V} above the supported {MAX_VOCAB}")
+        x = log_probs.contiguous()
+        lens_d = torch.tensor(lens, dtype=torch.int32).to(dev)
+        info, hsh = self._tables(dev)
+        prm = self._params(blank)
+        K = self.beam_size
+        with torch.cuda.device(dev):
+            st = stream_ptr(dev)
+            nbytes = ctypes.c_size_t(0)
+            check(lib().sbk_ctc_beam_workspace_bytes(ptr(x), ptr(lens_d), B, T, V, nv, ctypes.byref(prm),
+                                                     ctypes.byref(nbytes), st), "sbk_ctc_beam_workspace_bytes")
+            ws = torch.empty(max(1, nbytes.value), dtype=torch.uint8, device=dev)
+            fb = torch.empty(B, T, dtype=torch.int32, device=dev)
+            par = torch.empty(B, T, K, dtype=torch.int32, device=dev)
+            tok = torch.empty(B, T, K, dtype=torch.int32, device=dev)
+            score = torch.empty(B, K, dtype=torch.float32, device=dev)
+            nfin = torch.empty(B, dtype=torch.int32, device=dev)
+            check(lib().sbk_ctc_beam_search(ptr(x), ptr(lens_d), B, T, V, nv, ptr(info), ptr(hsh), ctypes.byref(prm), ptr(ws),
+                                            ctypes.c_size_t(ws.numel()), ptr(fb), ptr(par), ptr(tok), ptr(score), ptr(nfin), st),
+                  "sbk_ctc_beam_search")
+        return fb, par, tok, score, nfin
+
+    def _replay(self, n, fb, par, tok, score, nfin):
+        """The final beams of one utterance from the search history: text, partial word, word frames, partial frames."""
+        if nfin < 0:
+            raise ValueError("max() arg is an empty sequence (a frame had no candidate token inside vocab_list)")
+        proc = np.flatnonzero(fb[:n] >= 0)
+        if len(proc) == 0:
+            return [("", "", (), (-1, -1), 0.0)]
+        P, K = len(proc), nfin
+        chain = np.empty((P, K), dtype=np.int64)
+        idx = np.arange(K)
+        for j in range(P - 1, -1, -1):
+            chain[j] = tok[proc[j], idx]
+            idx = par[proc[j], idx]
+        sid = self._sid[chain]
+        prev = np.concatenate([np.full((1, K), -1, dtype=np.int64), sid[:-1]], 0)
+        nonblank = chain != self.blank_index
+        rep = (nonblank & (sid == prev)).T.tolist()
+        kind, app, frames_of = self._kind, self._app, proc.tolist()
+        chain_t = chain.T.tolist()
+        out = []
+        for k in range(K):
+            text, part, words, pf = "", "", [], (-1, -1)
+            ck, rk = chain_t[k], rep[k]
+            for j in np.flatnonzero(nonblank[:, k]).tolist():
+                f, t = frames_of[j], ck[j]
+                if rk[j]:
+                    pf = (pf[0], f + 1)
+                    continue
+                kd = kind[t]
+                if kd == _WORD or kd == _SPACE:
+                    if part:
+                        words.append(pf)
+                        text = _merge_words(text, part)
+                    part, pf = (app[t], (f, f + 1)) if kd == _WORD else ("", (-1, -1))
+                else:
+                    part += app[t]
+                    pf = (f, f + 1) if pf[0] < 0 else (pf[0], f + 1)
+            out.append((text, part, tuple(words), pf, score[k]))
+        return out
+
+    def _finalize(self, beams):
+        """finalize_decoding(force_next_word=True, is_end=True) + decode_log_probs' CTCHypothesis list (:868-934, :1127-1152)."""
+        fin = {}
+        for text, part, words, pf, sc in beams:
+            nw = words + (pf,) if part else words
+            key = _merge_words(text, part)
+            fin[key] = (np.logaddexp(fin[key][0], sc), nw) if key in fin else (sc, nw)
+        items = [(s, text, nw) for text, (s, nw) in fin.items()]
+        top = max(it[0] for it in items)
+        items = [it for it in items if it[0] >= top + self.beam_prune_logp]
+        items = heapq.nlargest(self.beam_size, items, key=lambda it: it[0])
+        return [CTCHypothesis(text=" ".join(text.split()), last_lm_state=None, text_frames=list(zip(text.split(), nw)),
+                              score=s, lm_score=s) for s, text, nw in items][: self.topk]
+
+    def decode_beams(self, log_probs, wav_lens=None, lm_start_state=None):
+        """decoders/ctc.py:936-986: log_probs [B, T, V] fp32 CUDA log-probabilities, wav_lens relative (or None) ->
+        B lists of at most topk CTCHypothesis."""
+        from .._lib import require_cuda
+        if lm_start_state is not None:
+            raise NotImplementedError("speechbrain_b200.CTCBeamSearcher: lm_start_state needs a language model (not built)")
+        require_cuda(log_probs, "CTCBeamSearcher")
+        if log_probs.dtype != torch.float32:
+            raise ValueError(f"CTCBeamSearcher: expected float32 log-probabilities, got {log_probs.dtype}")
+        if log_probs.dim() != 3:
+            raise ValueError(f"CTCBeamSearcher: expected [batch, time, vocab] log-probabilities, got {tuple(log_probs.shape)}")
+        if log_probs.size(2) != len(self.vocab_list):
+            warnings.warn(f"Vocab size mismatch: log_probs vocab dim is {log_probs.size(2)} while vocab_list is "
+                          f"{len(self.vocab_list)}. During decoding, going to truncate the log_probs vocab dim to match vocab_list.")
+        B, T = log_probs.shape[0], log_probs.shape[1]
+        if wav_lens is not None:
+            raw = (T * wav_lens).cpu().numpy().astype(int).tolist()
+        else:
+            raw = [T] * B
+        lens = [len(range(T)[:n]) for n in raw]  # used as a slice bound, like log_probs[:wav_len]
+        fb, par, tok, score, nfin = (t.cpu().numpy() for t in self.search(log_probs, lens))
+        return [self._finalize(self._replay(lens[b], fb[b], par[b], tok[b], score[b], int(nfin[b]))) for b in range(B)]
+
+    def forward(self, log_probs, wav_lens=None, lm_start_state=None):
+        return self.decode_beams(log_probs, wav_lens, lm_start_state)
+
+    def __call__(self, log_probs, wav_lens=None, lm_start_state=None):
+        return self.decode_beams(log_probs, wav_lens, lm_start_state)

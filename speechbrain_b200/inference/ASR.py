@@ -166,8 +166,10 @@ class EncoderASR(torch.nn.Module):
 
     ``modules["encoder"]``: ``LengthsCapableSequential`` of Fbank, InputNormalization, ConvolutionFrontEnd,
     ``EncoderWrapper(TransformerASR)``, the CTC ``Linear`` and a log-softmax (``torch.nn.LogSoftmax`` /
-    ``speechbrain_b200.nnet.activations.Softmax(apply_log=True)``); ``hparams["decoding_function"]`` must be a
-    ``functools.partial`` of ``ctc_greedy_decode`` (the CTC beam searchers of the reference are not built)."""
+    ``speechbrain_b200.nnet.activations.Softmax(apply_log=True)``); ``hparams["decoding_function"]`` is a
+    ``functools.partial`` of ``ctc_greedy_decode`` or the ``CTCBeamSearcher`` class (inference/ASR.py:212-282), which is
+    instantiated with ``hparams["test_beam_search"]`` (or no keywords) and the tokenizer's vocabulary; the log-posteriors
+    then stay on the device and go to the beam search kernel (csrc/ctc_beam.cu).  The prefix beam searchers are not built."""
     HPARAMS_NEEDED = ["tokenizer", "decoding_function"]
     MODULES_NEEDED = ["encoder"]
 
@@ -175,7 +177,7 @@ class EncoderASR(torch.nn.Module):
         super().__init__()
         import functools
 
-        from ..decoders.ctc import ctc_greedy_decode
+        from ..decoders.ctc import CTCBeamSearcher, ctc_greedy_decode
         from ..nnet.linear import Linear
         modules = dict(modules or {})
         if "encoder" not in modules:
@@ -187,11 +189,16 @@ class EncoderASR(torch.nn.Module):
                 raise ValueError(f"Need hparams['{k}']")
         self.tokenizer = self.hparams["tokenizer"]
         fn = self.hparams["decoding_function"]
-        if not (isinstance(fn, functools.partial) and fn.func is ctc_greedy_decode):
+        self.beam_search = isinstance(fn, type) and issubclass(fn, CTCBeamSearcher)
+        if self.beam_search:
+            opts = dict(self.hparams.get("test_beam_search") or {})
+            self.decoding_function = fn(**opts, vocab_list=self._vocab_list())
+        elif isinstance(fn, functools.partial) and fn.func is ctc_greedy_decode:
+            self.decoding_function = fn
+            self.blank_id = fn.keywords.get("blank_id", -1)
+        else:
             raise NotImplementedError("speechbrain_b200.EncoderASR: decoding_function must be functools.partial(ctc_greedy_decode, "
-                                      "blank_id=...) (CTC beam searchers are not built)")
-        self.decoding_function = fn
-        self.blank_id = fn.keywords.get("blank_id", -1)
+                                      "blank_id=...) or CTCBeamSearcher (the CTC prefix beam searchers are not built)")
         self.device = torch.device((run_opts or {}).get("device", "cuda:0"))
         vals = list(self.mods.values())
         wrap = _find(vals, EncoderWrapper)
@@ -203,6 +210,19 @@ class EncoderASR(torch.nn.Module):
             object.__setattr__(self, name, m)
         if self.normalize.norm_type != "global":
             raise NotImplementedError("EncoderASR: fused pipeline needs InputNormalization(norm_type='global')")
+
+    def _vocab_list(self):
+        """inference/ASR.py:240-255: the beam searcher's vocab_list from a sentencepiece model or a label encoder."""
+        tok = self.tokenizer
+        try:
+            import sentencepiece
+        except ImportError:
+            sentencepiece = None
+        if sentencepiece is not None and isinstance(tok, sentencepiece.SentencePieceProcessor):
+            return [tok.id_to_piece(i) for i in range(tok.vocab_size())]
+        if hasattr(tok, "ind2lab"):
+            return [tok.ind2lab[i] for i in range(len(tok.ind2lab))]
+        raise ValueError("The tokenizer must be sentencepiece or CTCTextEncoder")
 
     @classmethod
     def from_hparams(cls, source, hparams_file="hyperparams.yaml", overrides=None, savedir=None, run_opts=None, **kwargs):
@@ -228,9 +248,14 @@ class EncoderASR(torch.nn.Module):
 
     @torch.no_grad()
     def transcribe_batch(self, wavs, wav_lens):
-        """inference/ASR.py:325-373: -> (predicted_words, predicted_tokens)."""
+        """inference/ASR.py:325-373: -> (predicted_words, predicted_tokens); with a CTCBeamSearcher
+        -> ([best text per utterance], the searcher's List[List[CTCHypothesis]])."""
         from ..decoders.ctc import greedy_from_argmax
         eng, enc = self._encode(wavs, wav_lens)
+        if self.beam_search:
+            lp, _ = eng.ctc_head(enc, want_log_probs=True, want_argmax=False)
+            hyps = self.decoding_function(lp, wav_lens.to(self.device))
+            return [h[0].text for h in hyps], hyps
         _, idx = eng.ctc_head(enc, want_log_probs=False, want_argmax=True)
         V = eng.cfg["vocab"]
         blank = self.blank_id + V if isinstance(self.blank_id, int) and self.blank_id < 0 else self.blank_id
