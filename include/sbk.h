@@ -146,7 +146,9 @@ int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int 
 /* ---- model handle: repacks the reference state_dict once */
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out);
 void sbk_asr_destroy(sbk_asr* m);
-/* A clone shares the repacked weights and owns its own workspace: one clone ("lane") per batch in flight. */
+/* A clone is a new lane on the same repacked weights: it owns its workspace, graphs, streams and events, and inherits the
+   source's settings (set_decoder_ln_fusion, set_decoder_tc_min_rows, set_poll_interval, set_dynchunk).  One clone per batch
+   in flight. */
 int sbk_asr_clone(sbk_asr* src, sbk_asr** out);
 /* DynChunkTrainConfig(chunk_size, left_context_size) for the following encode calls (TransformerASR.encode(...,
  * dynchunktrain_config=...), TransformerASR.py:46-105,475-544; Conformer.py:190-313): chunked attention (a frame sees its own

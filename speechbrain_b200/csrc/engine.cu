@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -70,11 +71,14 @@ struct Arena {
     }
 };
 
-struct AsrModel {
+#define RC(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
+
+// What asr_create uploads and nothing changes afterwards: the configuration, the Fbank plan and the repacked weights in
+// one device arena.  A handle and its clones (lanes) hold it jointly; the last one to go frees it.
+struct AsrWeights {
     sbk_asr_config cfg;
     Fbank* fbank = nullptr;
-    Arena warena;  // weights
-    Arena ws;      // workspace (re-carved per shape)
+    Arena warena;
     // frontend
     const float *glob_mean = nullptr, *glob_std = nullptr;
     const float *c1_w, *c1_b, *c1_g, *c1_be, *c2_b, *c2_g, *c2_be;
@@ -100,15 +104,92 @@ struct AsrModel {
     std::vector<LmLayerW> lm;
     const float *lm_norm_g, *lm_norm_b, *lm_bp0, *lm_lnp_g, *lm_lnp_b, *lm_bp2;
     const __half *lm_wp0, *lm_wp2;
-    // CTC prefix scorer state (allocated on the first beam search that uses it): x [B, T, V] masked log-posteriors,
-    // xb [B, T], rsum/rb [2][rows, T] and psi [2][rows] ping-pong by step parity, add [rows, V] when there is no LM buffer
-    struct CtcBuf { float* base = nullptr; size_t cap = 0; float *x, *xlin, *xb, *rsum, *rb, *psi, *add, *tab, *tabM; } ctc;
-    struct CovBuf { float* base = nullptr; size_t cap = 0; } cov;  // CoverageScorer: [2][rows][T] coverage + [rows] scores
+    bool has_fbank = false, has_cnn = false, has_enc = false, has_dec = false;
+    ~AsrWeights() {
+        if (fbank) fbank_destroy(fbank);
+        cudaFree(warena.base);
+    }
+};
+
+// One cached CUDA graph and the key it was captured for.  Keys are compared bytewise, so callers zero their padding.
+struct GraphCache {
+    cudaGraphExec_t exec = nullptr;
+    long long nodes = 0;  // kernel launches the graph replays (bench.py's launch count)
+    std::string key;
+    GraphCache() = default;
+    GraphCache(const GraphCache&) = delete;
+    GraphCache& operator=(const GraphCache&) = delete;
+    ~GraphCache() { reset(); }
+    void reset() {
+        if (exec) cudaGraphExecDestroy(exec);
+        exec = nullptr;
+    }
+    // Captures enqueue(cap_stream) (creating cap_stream on first use) unless a graph for the same key exists.
+    template <class Key, class Enqueue>
+    int ensure(const Key& k, cudaStream_t& cap_stream, Enqueue&& enqueue) {
+        if (exec && key.size() == sizeof(Key) && memcmp(key.data(), &k, sizeof(Key)) == 0) return SBK_OK;
+        reset();
+        if (!cap_stream) SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&cap_stream, cudaStreamNonBlocking));
+        cudaGraph_t g;
+        SBK_CUDA_CHECK(cudaStreamBeginCapture(cap_stream, cudaStreamCaptureModeThreadLocal));
+        launch_count_begin_capture();
+        const int rc = enqueue(cap_stream);
+        nodes = launch_count_end_capture();
+        const cudaError_t ce = cudaStreamEndCapture(cap_stream, &g);
+        if (rc) return rc;
+        SBK_CUDA_CHECK(ce);
+        const cudaError_t ie = cudaGraphInstantiate(&exec, g, 0);
+        cudaGraphDestroy(g);
+        SBK_CUDA_CHECK(ie);
+        key.assign(reinterpret_cast<const char*>(&k), sizeof(Key));
+        return SBK_OK;
+    }
+    int launch(cudaStream_t st) {
+        SBK_CUDA_CHECK(cudaGraphLaunch(exec, st));
+        launch_count_add(nodes);
+        return SBK_OK;
+    }
+};
+
+// A lane's device buffer that only grows (grow_buffer).  Graphs capture pointers into it.
+struct DevBuf {
+    void* base = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { cudaFree(base); }
+};
+
+// Lays fields out one after another in a buffer, each at a 256-byte boundary.  A buffer's layout is one function that runs
+// twice: with base == nullptr to measure the bytes it needs (`used`), then with the buffer to set the fields.
+struct Carver {
+    uint8_t* base = nullptr;
+    size_t used = 0;
+    template <class T>
+    void operator()(T*& field, size_t bytes) {
+        if (base) field = reinterpret_cast<T*>(base + used);
+        used += (bytes + 255) & ~size_t(255);
+    }
+};
+
+// A handle: the shared weights plus one lane's state.  A clone is another lane on the same weights with its own workspace,
+// graphs, streams and flags: one clone per in-flight batch lets independent batches overlap on different streams (the
+// decode loop is latency-bound and leaves most SMs idle, so concurrent lanes raise throughput without touching per-batch
+// numerics).  Streams, events and buffers are created on first use; the destructor releases all of them.
+struct AsrModel {
+    std::shared_ptr<const AsrWeights> wt;
+    DevBuf ws;  // workspace (re-carved per shape)
+    // CTC prefix scorer state (grown by the first beam search that uses it, see run_beam), or the logits of an arg-max-only
+    // ctc_head call
+    DevBuf ctc;
+    DevBuf cov;  // CoverageScorer: [2][rows][T] coverage + [rows] scores
     // TransformerLM whole-sequence forward (run_lm_forward), carved for `rows` = n * s token rows, independent of the
     // decode / beam workspace: residual stream x [rows, d] fp32, its fp16 copy x16, qkv16 [rows, 3d], att16 [rows, d],
     // f16 [rows, d_ffn]
+    DevBuf lmf_mem;
     struct LmFwdBuf {
-        uint8_t* base = nullptr; size_t cap = 0; int rows = 0;
+        int rows = 0;
         float* x; __half *x16, *qkv16, *att16, *f16;
     } lmf;
     // shapes the workspace is carved for
@@ -130,43 +211,39 @@ struct AsrModel {
         float *hm_part, *hm_gscale;
         __half* hm_G;
     } b;
-    cudaGraphExec_t step_graph = nullptr;
-    int graph_rows = -1, graph_T = -1, graph_B = -1, graph_eos = -1, graph_S = -1;
-    long long graph_nodes = 0;
+    GraphCache step_graph;    // one greedy decode step (run_greedy)
+    GraphCache group_graph;   // a whole group call (sbk_asr_transcribe_greedy_group_dev)
+    GraphCache hgroup_graph;  // the same from host buffers, H2D / D2H memcpy nodes included
+    GraphCache beam_graph;    // one whole beam-search step (run_beam)
+    GraphCache pipe_graph;    // the whole Fbank .. last decode step pipeline (sbk_asr_transcribe_greedy_dev)
     int* host_flag = nullptr;  // pinned
-    struct GroupKey { const void *wav[16], *rel[16], *pred[16]; int G, B, L, steps, bos, eos; };
-    GroupKey group_key{};
-    cudaGraphExec_t group_graph = nullptr;
-    long long group_nodes = 0;
     // host-buffer group entry point: device staging of the G batches' wav / lengths, a copy stream forked from the caller's
-    // stream (so batch g+1's H2D overlaps batch g's encoder) and its own graph (H2D / D2H memcpy nodes included)
-    float* gwav = nullptr; float* grel = nullptr; size_t gwav_cap = 0;
+    // stream (so batch g+1's H2D overlaps batch g's encoder)
+    DevBuf gwav;
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_ready[16] = {};
     cudaStream_t side_stream = nullptr;     // beam search: the LM scorer's branch of a search step
     cudaStream_t dec_stream = nullptr;      // group calls: the decode loop, on a high-priority stream (see transcribe_group_enqueue)
     cudaEvent_t ev_dfork = nullptr, ev_djoin = nullptr;
     cudaEvent_t ev_bfork = nullptr, ev_bjoin = nullptr;
-    struct HostGroupKey { const void *wav[16], *rel[16], *pred[16], *pred_dev[16]; int G, B, L, steps, bos, eos; };
-    HostGroupKey hgroup_key{};
-    cudaGraphExec_t hgroup_graph = nullptr;
-    long long hgroup_nodes = 0;
-    // beam search: ONE graph of a whole search step (decoder layers + LM step + CTC scorer + beam kernel), replayed per step
-    struct BeamKey { sbk_beam_params p; int B, T, rows, S_max, fuse_ln, tc_rows, fork; };
-    BeamKey beam_key{};
-    cudaGraphExec_t beam_graph = nullptr;
-    long long beam_nodes = 0;
-    struct PipeKey { const void *wav, *rel, *enc, *pred, *score; int B, L, steps, bos, eos; };
-    PipeKey pipe_key{};
-    cudaGraphExec_t pipe_graph = nullptr;
-    long long pipe_nodes = 0;
-    int* weight_refs = nullptr;  // weights (arena + fbank plan) are shared between a handle and its clones (lanes)
+    cudaStream_t cap_stream = nullptr;  // private stream for graph capture (the legacy default stream cannot capture)
     int dec_tc_rows = getenv("SBK_DEC_TC_ROWS") ? atoi(getenv("SBK_DEC_TC_ROWS")) : 64;  // >= this many live hypotheses: wgmma decode GEMMs
     int dyn_chunk = 0, dyn_left = -1;  // DynChunkTrainConfig of the next encode calls (chunk frames, left-context chunks; 0 = off)
     int fuse_dec_ln = 1;         // 1: LayerNorm inside the projection kernel (latency); 0: separate LN kernel (throughput)
     int poll_every = 8;          // greedy early-exit poll interval in steps; 0 = never sync, run exactly max_steps
-    bool has_fbank = false, has_cnn = false, has_enc = false, has_dec = false;
-    cudaStream_t cap_stream = nullptr;  // private stream for graph capture (the legacy default stream cannot capture)
+
+    AsrModel() = default;
+    AsrModel(const AsrModel&) = delete;
+    AsrModel& operator=(const AsrModel&) = delete;
+    ~AsrModel() {
+        if (host_flag) cudaFreeHost(host_flag);
+        for (cudaStream_t s : {copy_stream, side_stream, dec_stream, cap_stream})
+            if (s) cudaStreamDestroy(s);
+        for (cudaEvent_t e : {ev_fork, ev_dfork, ev_djoin, ev_bfork, ev_bjoin})
+            if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : ev_ready)
+            if (e) cudaEventDestroy(e);
+    }
 };
 
 static const float* find(const std::map<std::string, std::pair<const float*, int64_t>>& m, const std::string& k,
@@ -184,7 +261,7 @@ static const float* find(const std::map<std::string, std::pair<const float*, int
 }
 
 struct Packer {
-    AsrModel* m;
+    AsrWeights* W;
     const std::map<std::string, std::pair<const float*, int64_t>>* w;
     bool ok = true;
     std::vector<float> tmpf;
@@ -195,7 +272,7 @@ struct Packer {
         return f32_raw(src, n);
     }
     const float* f32_raw(const float* src, int64_t n) {
-        void* d = m->warena.take(n * 4);
+        void* d = W->warena.take(n * 4);
         if (!d) { ok = false; set_error("weight arena exhausted"); return nullptr; }
         if (cudaMemcpy(d, src, n * 4, cudaMemcpyHostToDevice) != cudaSuccess) { ok = false; set_error("weight upload failed"); }
         return reinterpret_cast<const float*>(d);
@@ -203,7 +280,7 @@ struct Packer {
     const __half* f16_raw(const float* src, int64_t n, float scale = 1.0f) {
         tmph.resize(n);
         for (int64_t i = 0; i < n; ++i) tmph[i] = __float2half_rn(src[i] * scale);
-        void* d = m->warena.take(n * 2);
+        void* d = W->warena.take(n * 2);
         if (!d) { ok = false; set_error("weight arena exhausted"); return nullptr; }
         if (cudaMemcpy(d, tmph.data(), n * 2, cudaMemcpyHostToDevice) != cudaSuccess) { ok = false; set_error("weight upload failed"); }
         return reinterpret_cast<const __half*>(d);
@@ -239,6 +316,19 @@ static size_t weight_arena_bytes(const sbk_asr_config& c) {
     return enc + dec + misc + lm + (64u << 20);
 }
 
+// A new lane on the weights of `wt`.
+static int new_lane(std::shared_ptr<const AsrWeights> wt, AsrModel** out) {
+    AsrModel* m = new AsrModel();
+    m->wt = std::move(wt);
+    if (cudaMallocHost(&m->host_flag, 64) != cudaSuccess) {
+        delete m;
+        set_error("cudaMallocHost failed");
+        return SBK_ERR_NOMEM;
+    }
+    *out = m;
+    return SBK_OK;
+}
+
 int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, AsrModel** out) {
     SBK_REQUIRE(cfg && weights && out, "asr_create: null argument");
     const sbk_asr_config& c = *cfg;
@@ -265,63 +355,61 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
     std::map<std::string, std::pair<const float*, int64_t>> w;
     for (int i = 0; i < n_weights; ++i) w[weights[i].name] = {weights[i].data, weights[i].numel};
 
-    AsrModel* m = new AsrModel();
-    m->cfg = c;
-    m->warena.cap = weight_arena_bytes(c);
-    if (cudaMalloc(&m->warena.base, m->warena.cap) != cudaSuccess) {
-        set_error("asr_create: cudaMalloc(%zu) for weights failed", m->warena.cap);
-        delete m;
+    auto wt = std::make_shared<AsrWeights>();
+    AsrWeights* W = wt.get();
+    W->cfg = c;
+    W->warena.cap = weight_arena_bytes(c);
+    if (cudaMalloc(&W->warena.base, W->warena.cap) != cudaSuccess) {
+        set_error("asr_create: cudaMalloc(%zu) for weights failed", W->warena.cap);
         return SBK_ERR_NOMEM;
     }
-    Packer p{m, &w};
-    int rc = SBK_OK;
+    Packer p{W, &w};
     const bool has_fbank = c.parts & SBK_PART_FBANK, has_cnn = c.parts & SBK_PART_CNN;
     const bool has_enc = (c.parts & SBK_PART_ENCODER) && c.num_encoder_layers >= 0;
     const bool has_dec = (c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0;
-    m->has_fbank = has_fbank; m->has_cnn = has_cnn; m->has_enc = has_enc; m->has_dec = has_dec;
+    W->has_fbank = has_fbank; W->has_cnn = has_cnn; W->has_enc = has_enc; W->has_dec = has_dec;
     // ---- Fbank + CMVN
     if (has_fbank) {
         const float* win = find(w, "fbank.window", c.n_fft);
         const float* mel = find(w, "fbank.mel_matrix", (int64_t)(c.n_fft / 2 + 1) * c.n_mels);
-        if (!win || !mel) { rc = SBK_ERR_ARG; goto fail; }
-        rc = fbank_create(&m->fbank, c.n_fft, c.hop, c.n_mels, win, mel, c.fbank_amin > 0.0f ? c.fbank_amin : 1e-10f,
-                          c.fbank_top_db > 0.0f ? c.fbank_top_db : 80.0f);
-        if (rc) goto fail;
+        if (!win || !mel) return SBK_ERR_ARG;
+        RC(fbank_create(&W->fbank, c.n_fft, c.hop, c.n_mels, win, mel, c.fbank_amin > 0.0f ? c.fbank_amin : 1e-10f,
+                        c.fbank_top_db > 0.0f ? c.fbank_top_db : 80.0f));
         if (w.count("normalize.glob_mean")) {
-            m->glob_mean = p.f32("normalize.glob_mean", c.n_mels);
-            m->glob_std = p.f32("normalize.glob_std", c.n_mels);
+            W->glob_mean = p.f32("normalize.glob_mean", c.n_mels);
+            W->glob_std = p.f32("normalize.glob_std", c.n_mels);
         }
     }
     // ---- CNN front-end
     if (has_cnn) {
         const int F1 = (c.n_mels - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
-        if (F2 * c.cnn_c2 != c.input_size) { set_error("asr_create: CNN output %d != input_size %d", F2 * c.cnn_c2, c.input_size); rc = SBK_ERR_ARG; goto fail; }
-        m->c1_w = p.f32("CNN.convblock_0.convs.conv_0.conv.weight", (int64_t)c.cnn_c1 * 9);
-        m->c1_b = p.f32("CNN.convblock_0.convs.conv_0.conv.bias", c.cnn_c1);
-        m->c1_g = p.f32("CNN.convblock_0.convs.norm_0.norm.weight", (int64_t)F1 * c.cnn_c1);
-        m->c1_be = p.f32("CNN.convblock_0.convs.norm_0.norm.bias", (int64_t)F1 * c.cnn_c1);
+        if (F2 * c.cnn_c2 != c.input_size) { set_error("asr_create: CNN output %d != input_size %d", F2 * c.cnn_c2, c.input_size); return SBK_ERR_ARG; }
+        W->c1_w = p.f32("CNN.convblock_0.convs.conv_0.conv.weight", (int64_t)c.cnn_c1 * 9);
+        W->c1_b = p.f32("CNN.convblock_0.convs.conv_0.conv.bias", c.cnn_c1);
+        W->c1_g = p.f32("CNN.convblock_0.convs.norm_0.norm.weight", (int64_t)F1 * c.cnn_c1);
+        W->c1_be = p.f32("CNN.convblock_0.convs.norm_0.norm.bias", (int64_t)F1 * c.cnn_c1);
         const float* w2 = find(w, "CNN.convblock_1.convs.conv_0.conv.weight", (int64_t)c.cnn_c2 * c.cnn_c1 * 9);
-        if (!w2) { rc = SBK_ERR_ARG; goto fail; }
+        if (!w2) return SBK_ERR_ARG;
         std::vector<float> w2p((size_t)c.cnn_c2 * 9 * c.cnn_c1);
         for (int o = 0; o < c.cnn_c2; ++o)
             for (int ch = 0; ch < c.cnn_c1; ++ch)
                 for (int kf = 0; kf < 3; ++kf)
                     for (int kt = 0; kt < 3; ++kt)
                         w2p[((size_t)o * 9 + kf * 3 + kt) * c.cnn_c1 + ch] = w2[(((size_t)o * c.cnn_c1 + ch) * 3 + kf) * 3 + kt];
-        m->c2_w = p.f16_raw(w2p.data(), w2p.size());
-        m->c2_b = p.f32("CNN.convblock_1.convs.conv_0.conv.bias", c.cnn_c2);
-        m->c2_g = p.f32("CNN.convblock_1.convs.norm_0.norm.weight", (int64_t)F2 * c.cnn_c2);
-        m->c2_be = p.f32("CNN.convblock_1.convs.norm_0.norm.bias", (int64_t)F2 * c.cnn_c2);
+        W->c2_w = p.f16_raw(w2p.data(), w2p.size());
+        W->c2_b = p.f32("CNN.convblock_1.convs.conv_0.conv.bias", c.cnn_c2);
+        W->c2_g = p.f32("CNN.convblock_1.convs.norm_0.norm.weight", (int64_t)F2 * c.cnn_c2);
+        W->c2_be = p.f32("CNN.convblock_1.convs.norm_0.norm.bias", (int64_t)F2 * c.cnn_c2);
     }
     // ---- encoder
     if (has_enc) {
-    m->w_in = p.f16("Transformer.custom_src_module.layers.0.w.weight", (int64_t)d * c.input_size);
-    m->b_in = p.f32("Transformer.custom_src_module.layers.0.w.bias", d);
-    m->enc.resize(c.num_encoder_layers);
+    W->w_in = p.f16("Transformer.custom_src_module.layers.0.w.weight", (int64_t)d * c.input_size);
+    W->b_in = p.f32("Transformer.custom_src_module.layers.0.w.bias", d);
+    W->enc.resize(c.num_encoder_layers);
     for (int l = 0; l < c.num_encoder_layers && p.ok && c.encoder_module == SBK_ENC_BRANCHFORMER; ++l) {
         const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".", cb = q + "convolution_branch.";
         const int C = c.csgu_linear_units, C2 = C / 2;
-        EncLayerW& e = m->enc[l];
+        EncLayerW& e = W->enc[l];
         e.norm1_g = p.f32(q + "norm_mhsa.norm.weight", d); e.norm1_b = p.f32(q + "norm_mhsa.norm.bias", d);
         e.nconv_g = p.f32(q + "norm_conv.norm.weight", d); e.nconv_b = p.f32(q + "norm_conv.norm.bias", d);
         e.wqkv = p.f16(q + "mha_layer.in_proj_weight", (int64_t)3 * d * d);
@@ -343,7 +431,7 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
     }
     for (int l = 0; l < c.num_encoder_layers && p.ok && c.encoder_module == SBK_ENC_CONFORMER; ++l) {
         const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".";
-        EncLayerW& e = m->enc[l];
+        EncLayerW& e = W->enc[l];
         e.ffn1_ln_g = p.f32(q + "ffn_module1.0.weight", d); e.ffn1_ln_b = p.f32(q + "ffn_module1.0.bias", d);
         e.ffn1_w1 = p.f16(q + "ffn_module1.1.ffn.0.weight", (int64_t)F * d); e.ffn1_b1 = p.f32(q + "ffn_module1.1.ffn.0.bias", F);
         e.ffn1_w2 = p.f16(q + "ffn_module1.1.ffn.3.weight", (int64_t)d * F); e.ffn1_b2 = p.f32(q + "ffn_module1.1.ffn.3.bias", d);
@@ -400,11 +488,11 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
         e.ffn2_w2 = p.f16(q + "ffn_module2.1.ffn.3.weight", (int64_t)d * F); e.ffn2_b2 = p.f32(q + "ffn_module2.1.ffn.3.bias", d);
         e.norm2_g = p.f32(q + "norm2.norm.weight", d); e.norm2_b = p.f32(q + "norm2.norm.bias", d);
     }
-    if (!p.ok) { rc = SBK_ERR_ARG; goto fail; }
-    m->enc_norm_g = p.f32("Transformer.encoder.norm.norm.weight", d);
-    m->enc_norm_b = p.f32("Transformer.encoder.norm.norm.bias", d);
+    if (!p.ok) return SBK_ERR_ARG;
+    W->enc_norm_g = p.f32("Transformer.encoder.norm.norm.weight", d);
+    W->enc_norm_b = p.f32("Transformer.encoder.norm.norm.bias", d);
     // positional tables
-    m->pos_len = c.max_len;
+    W->pos_len = c.max_len;
     if (c.attention_type == SBK_ATT_ROPE) {
         // nnet/attention.py:1012-1055: angle_{t,i} = t * exp(-2i * ln(1e4) / d_h), computed in fp32 like the reference
         std::vector<float> cs((size_t)c.max_len * dh / 2), sn(cs.size());
@@ -416,13 +504,13 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
                 sn[(size_t)t * (dh / 2) + i] = sinf(ta);
             }
         }
-        m->rope_cos = p.f32_raw(cs.data(), cs.size());
-        m->rope_sin = p.f32_raw(sn.data(), sn.size());
+        W->rope_cos = p.f32_raw(cs.data(), cs.size());
+        W->rope_sin = p.f32_raw(sn.data(), sn.size());
     } else if (hypermix) {
         std::vector<float> pe((size_t)HM_PE_ROWS * d);
         hypermix_pe_table(d, pe.data());
-        m->hm_pe = p.f32_raw(pe.data(), pe.size());
-        m->pos_len = HM_PE_ROWS;
+        W->hm_pe = p.f32_raw(pe.data(), pe.size());
+        W->pos_len = HM_PE_ROWS;
     } else {
         // nnet/attention.py:360-408: row |r|: even cols sin(|r| f_i), odd cols cos(|r| f_i)
         std::vector<float> pe((size_t)c.max_len * d);
@@ -433,12 +521,12 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
                 pe[(size_t)t * d + 2 * i + 1] = cosf((float)t * fr);
             }
         }
-        m->relpos_pe = p.f16_raw(pe.data(), pe.size());
+        W->relpos_pe = p.f16_raw(pe.data(), pe.size());
     }
     }  // has_enc
     // ---- decoder
     if (has_dec) {
-        m->emb = p.f32("Transformer.custom_tgt_module.layers.0.emb.Embedding.weight", (int64_t)c.vocab * d);
+        W->emb = p.f32("Transformer.custom_tgt_module.layers.0.emb.Embedding.weight", (int64_t)c.vocab * d);
         {
             std::vector<float> pe((size_t)c.max_len * d);  // Transformer.py:252-303
             for (int i = 0; i < d / 2; ++i) {
@@ -448,15 +536,15 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
                     pe[(size_t)t * d + 2 * i + 1] = cosf((float)t * den);
                 }
             }
-            m->dec_pe = p.f32_raw(pe.data(), pe.size());
+            W->dec_pe = p.f32_raw(pe.data(), pe.size());
         }
         const int L = c.num_decoder_layers;
-        m->dec.resize(L);
+        W->dec.resize(L);
         std::vector<float> wckv((size_t)L * 2 * d * d), bckv((size_t)L * 2 * d);
         const float qs = 1.0f / sqrtf((float)dh);
         for (int l = 0; l < L && p.ok; ++l) {
             const std::string q = "Transformer.decoder.layers." + std::to_string(l) + ".";
-            DecLayerW& e = m->dec[l];
+            DecLayerW& e = W->dec[l];
             e.n1g = p.f32(q + "norm1.norm.weight", d); e.n1b = p.f32(q + "norm1.norm.bias", d);
             e.n2g = p.f32(q + "norm2.norm.weight", d); e.n2b = p.f32(q + "norm2.norm.bias", d);
             e.n3g = p.f32(q + "norm3.norm.weight", d); e.n3b = p.f32(q + "norm3.norm.bias", d);
@@ -484,22 +572,22 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
             e.w_ffn1 = p.f16(q + "pos_ffn.ffn.0.weight", (int64_t)F * d); e.b_ffn1 = p.f32(q + "pos_ffn.ffn.0.bias", F);
             e.w_ffn2 = p.f16(q + "pos_ffn.ffn.3.weight", (int64_t)d * F); e.b_ffn2 = p.f32(q + "pos_ffn.ffn.3.bias", d);
         }
-        if (!p.ok) { rc = SBK_ERR_ARG; goto fail; }
-        m->w_ckv = p.f16_raw(wckv.data(), wckv.size());
-        m->b_ckv = p.f32_raw(bckv.data(), bckv.size());
-        m->dec_norm_g = p.f32("Transformer.decoder.norm.norm.weight", d);
-        m->dec_norm_b = p.f32("Transformer.decoder.norm.norm.bias", d);
-        m->w_lin = nullptr; m->b_lin = nullptr;
+        if (!p.ok) return SBK_ERR_ARG;
+        W->w_ckv = p.f16_raw(wckv.data(), wckv.size());
+        W->b_ckv = p.f32_raw(bckv.data(), bckv.size());
+        W->dec_norm_g = p.f32("Transformer.decoder.norm.norm.weight", d);
+        W->dec_norm_b = p.f32("Transformer.decoder.norm.norm.bias", d);
+        W->w_lin = nullptr; W->b_lin = nullptr;
         if (w.count("seq_lin.w.weight")) {  // the output head belongs to the searchers; TransformerASR.decode runs without it
-            m->w_lin = p.f16("seq_lin.w.weight", (int64_t)c.vocab * d);
-            m->b_lin = p.f32("seq_lin.w.bias", c.vocab);
+            W->w_lin = p.f16("seq_lin.w.weight", (int64_t)c.vocab * d);
+            W->b_lin = p.f32("seq_lin.w.bias", c.vocab);
         }
     }
     if ((c.parts & SBK_PART_LM) && c.lm_layers > 0) {
         const int dl = c.lm_d_model, Fl = c.lm_d_ffn, dhl = dl / c.lm_nhead;
-        if (dhl != 64 || dl % 128 != 0) { set_error("asr_create: LM head_dim must be 64 and d_model %% 128 == 0"); rc = SBK_ERR_UNSUPPORTED; goto fail; }
-        m->has_lm = true;
-        m->lm_emb = p.f32("lm.custom_src_module.emb.Embedding.weight", (int64_t)c.vocab * dl);
+        if (dhl != 64 || dl % 128 != 0) { set_error("asr_create: LM head_dim must be 64 and d_model %% 128 == 0"); return SBK_ERR_UNSUPPORTED; }
+        W->has_lm = true;
+        W->lm_emb = p.f32("lm.custom_src_module.emb.Embedding.weight", (int64_t)c.vocab * dl);
         {
             std::vector<float> pe((size_t)c.max_len * dl);
             for (int i = 0; i < dl / 2; ++i) {
@@ -509,13 +597,13 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
                     pe[(size_t)t * dl + 2 * i + 1] = cosf((float)t * den);
                 }
             }
-            m->lm_pe = p.f32_raw(pe.data(), pe.size());
+            W->lm_pe = p.f32_raw(pe.data(), pe.size());
         }
-        m->lm.resize(c.lm_layers);
+        W->lm.resize(c.lm_layers);
         const float qs = 1.0f / sqrtf((float)dhl);
         for (int l = 0; l < c.lm_layers && p.ok; ++l) {
             const std::string q = "lm.encoder.layers." + std::to_string(l) + ".";
-            LmLayerW& e = m->lm[l];
+            LmLayerW& e = W->lm[l];
             const float* wi = find(w, q + "self_att.att.in_proj_weight", (int64_t)3 * dl * dl);
             const float* bi = find(w, q + "self_att.att.in_proj_bias", 3 * dl);
             if (!wi || !bi) { p.ok = false; break; }
@@ -530,100 +618,61 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
             e.n1g = p.f32(q + "norm1.norm.weight", dl); e.n1b = p.f32(q + "norm1.norm.bias", dl);
             e.n2g = p.f32(q + "norm2.norm.weight", dl); e.n2b = p.f32(q + "norm2.norm.bias", dl);
         }
-        m->lm_norm_g = p.f32("lm.encoder.norm.norm.weight", dl); m->lm_norm_b = p.f32("lm.encoder.norm.norm.bias", dl);
-        m->lm_wp0 = p.f16("lm.output_proj.layers.0.w.weight", (int64_t)dl * dl); m->lm_bp0 = p.f32("lm.output_proj.layers.0.w.bias", dl);
-        m->lm_lnp_g = p.f32("lm.output_proj.layers.1.norm.weight", dl); m->lm_lnp_b = p.f32("lm.output_proj.layers.1.norm.bias", dl);
-        m->lm_wp2 = p.f16("lm.output_proj.layers.2.w.weight", (int64_t)c.vocab * dl); m->lm_bp2 = p.f32("lm.output_proj.layers.2.w.bias", c.vocab);
-        if (!p.ok) { rc = SBK_ERR_ARG; goto fail; }
+        W->lm_norm_g = p.f32("lm.encoder.norm.norm.weight", dl); W->lm_norm_b = p.f32("lm.encoder.norm.norm.bias", dl);
+        W->lm_wp0 = p.f16("lm.output_proj.layers.0.w.weight", (int64_t)dl * dl); W->lm_bp0 = p.f32("lm.output_proj.layers.0.w.bias", dl);
+        W->lm_lnp_g = p.f32("lm.output_proj.layers.1.norm.weight", dl); W->lm_lnp_b = p.f32("lm.output_proj.layers.1.norm.bias", dl);
+        W->lm_wp2 = p.f16("lm.output_proj.layers.2.w.weight", (int64_t)c.vocab * dl); W->lm_bp2 = p.f32("lm.output_proj.layers.2.w.bias", c.vocab);
+        if (!p.ok) return SBK_ERR_ARG;
     }
     if (w.count("ctc_lin.w.weight")) {
-        m->w_ctc = p.f16("ctc_lin.w.weight", (int64_t)c.vocab * d);
-        m->b_ctc = p.f32("ctc_lin.w.bias", c.vocab);
+        W->w_ctc = p.f16("ctc_lin.w.weight", (int64_t)c.vocab * d);
+        W->b_ctc = p.f32("ctc_lin.w.bias", c.vocab);
     }
-    if (!p.ok) { rc = SBK_ERR_ARG; goto fail; }
-    if (cudaMallocHost(&m->host_flag, 64) != cudaSuccess) { set_error("cudaMallocHost failed"); rc = SBK_ERR_NOMEM; goto fail; }
-    m->weight_refs = new int(1);
-    if (cudaDeviceSynchronize() != cudaSuccess) { set_error("asr_create: device error after upload"); rc = SBK_ERR_CUDA; goto fail; }
-    *out = m;
-    return SBK_OK;
-fail:
-    if (m->fbank) fbank_destroy(m->fbank);
-    cudaFree(m->warena.base);
-    delete m;
-    return rc;
+    if (!p.ok) return SBK_ERR_ARG;
+    if (cudaDeviceSynchronize() != cudaSuccess) { set_error("asr_create: device error after upload"); return SBK_ERR_CUDA; }
+    return new_lane(std::move(wt), out);
 }
 
-// A clone shares the repacked weights but owns its workspace, decode graph and flags: one clone per in-flight
-// batch ("lane") lets independent batches overlap on different streams (the decode loop is latency-bound and
-// leaves most SMs idle, so concurrent lanes raise throughput without touching per-batch numerics).
+// A clone is a new lane on the same weights; it inherits the source's settings.
 int asr_clone(AsrModel* src, AsrModel** out) {
     SBK_REQUIRE(src && out, "asr_clone: null argument");
-    AsrModel* m = new AsrModel(*src);
-    m->ws = Arena();
-    m->wsB = m->wsL = m->ws_rows = m->ws_steps = 0;
-    m->b = AsrModel::Buf();
-    m->ctc = AsrModel::CtcBuf();
-    m->cov = AsrModel::CovBuf();
-    m->lmf = AsrModel::LmFwdBuf();
-    m->step_graph = nullptr;
-    m->pipe_graph = nullptr;
-    m->group_graph = nullptr;
-    m->hgroup_graph = nullptr;
-    m->beam_graph = nullptr;
-    m->gwav = m->grel = nullptr; m->gwav_cap = 0;
-    m->copy_stream = nullptr; m->ev_fork = nullptr;
-    for (auto& e : m->ev_ready) e = nullptr;
-    m->graph_rows = m->graph_T = m->graph_B = -1;
-    m->cap_stream = nullptr;
-    m->host_flag = nullptr;
-    if (cudaMallocHost(&m->host_flag, 64) != cudaSuccess) {
-        delete m;
-        set_error("asr_clone: cudaMallocHost failed");
-        return SBK_ERR_NOMEM;
-    }
-    ++*m->weight_refs;
+    AsrModel* m = nullptr;
+    RC(new_lane(src->wt, &m));
+    m->fuse_dec_ln = src->fuse_dec_ln;
+    m->dec_tc_rows = src->dec_tc_rows;
+    m->poll_every = src->poll_every;
+    m->dyn_chunk = src->dyn_chunk;
+    m->dyn_left = src->dyn_left;
     *out = m;
     return SBK_OK;
-}
-
-void asr_destroy(AsrModel* m) {
-    if (!m) return;
-    if (m->step_graph) cudaGraphExecDestroy(m->step_graph);
-    if (m->pipe_graph) cudaGraphExecDestroy(m->pipe_graph);
-    if (m->group_graph) cudaGraphExecDestroy(m->group_graph);
-    if (m->hgroup_graph) cudaGraphExecDestroy(m->hgroup_graph);
-    if (m->beam_graph) cudaGraphExecDestroy(m->beam_graph);
-    cudaFree(m->gwav);
-    if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
-    if (m->ev_fork) cudaEventDestroy(m->ev_fork);
-    for (auto e : m->ev_ready) if (e) cudaEventDestroy(e);
-    if (m->weight_refs && --*m->weight_refs == 0) {
-        if (m->fbank) fbank_destroy(m->fbank);
-        cudaFree(m->warena.base);
-        delete m->weight_refs;
-    }
-    cudaFree(m->ws.base);
-    cudaFree(m->ctc.base);
-    cudaFree(m->cov.base);
-    cudaFree(m->lmf.base);
-    if (m->host_flag) cudaFreeHost(m->host_flag);
-    if (m->cap_stream) cudaStreamDestroy(m->cap_stream);
-    if (m->side_stream) cudaStreamDestroy(m->side_stream);
-    if (m->dec_stream) cudaStreamDestroy(m->dec_stream);
-    if (m->ev_dfork) cudaEventDestroy(m->ev_dfork);
-    if (m->ev_djoin) cudaEventDestroy(m->ev_djoin);
-    if (m->ev_bfork) cudaEventDestroy(m->ev_bfork);
-    if (m->ev_bjoin) cudaEventDestroy(m->ev_bjoin);
-    delete m;
 }
 
 // cached graphs bake in workspace pointers / kernel choices: drop them whenever either changes
 static void drop_graphs(AsrModel* m) {
-    if (m->step_graph) { cudaGraphExecDestroy(m->step_graph); m->step_graph = nullptr; m->graph_rows = -1; }
-    if (m->pipe_graph) { cudaGraphExecDestroy(m->pipe_graph); m->pipe_graph = nullptr; }
-    if (m->group_graph) { cudaGraphExecDestroy(m->group_graph); m->group_graph = nullptr; }
-    if (m->hgroup_graph) { cudaGraphExecDestroy(m->hgroup_graph); m->hgroup_graph = nullptr; }
-    if (m->beam_graph) { cudaGraphExecDestroy(m->beam_graph); m->beam_graph = nullptr; }
+    m->step_graph.reset();
+    m->pipe_graph.reset();
+    m->group_graph.reset();
+    m->hgroup_graph.reset();
+    m->beam_graph.reset();
+}
+
+// Makes `buf` hold at least `need` bytes.  Replacing a buffer waits for the device (work on any of the lane's streams may
+// still use it) and drops the lane's graphs, which captured pointers into it.
+static int grow_buffer(AsrModel* m, DevBuf& buf, size_t need, const char* what) {
+    if (need <= buf.cap) return SBK_OK;
+    if (buf.base) {
+        SBK_CUDA_CHECK(cudaDeviceSynchronize());
+        cudaFree(buf.base);
+        buf.base = nullptr;
+        buf.cap = 0;
+        drop_graphs(m);
+    }
+    if (cudaMalloc(&buf.base, need) != cudaSuccess) {
+        set_error("%s: cudaMalloc(%zu) failed", what, need);
+        return SBK_ERR_NOMEM;
+    }
+    buf.cap = need;
+    return SBK_OK;
 }
 
 static void frames(const sbk_asr_config& c, int L, int* T0, int* T1, int* T2) {
@@ -632,93 +681,64 @@ static void frames(const sbk_asr_config& c, int L, int* T0, int* T1, int* T2) {
     *T2 = (*T1 - 1) / 2 + 1;
 }
 
-// (Re)carve the workspace for a batch of B utterances of L samples, `rows` decoder hypotheses, `steps` max steps.
-static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
-    if (m->ws.base && B <= m->wsB && L <= m->wsL && rows <= m->ws_rows && steps <= m->ws_steps) return SBK_OK;
-    B = std::max(B, m->wsB); L = std::max(L, m->wsL); rows = std::max(rows, m->ws_rows); steps = std::max(steps, m->ws_steps);
-    const sbk_asr_config& c = m->cfg;
+// The workspace for a batch of B utterances of L samples, `rows` decoder hypotheses, `steps` max steps.
+static void workspace_layout(const AsrModel* m, int B, int L, int rows, int steps, AsrModel::Buf& b, Carver& take) {
+    const sbk_asr_config& c = m->wt->cfg;
     int T0, T1, T2;
     frames(c, L, &T0, &T1, &T2);
     const int F1 = (c.n_mels - 1) / 2 + 1;
     const size_t M = (size_t)B * T2, d = c.d_model, F = c.d_ffn, Ld = c.num_decoder_layers, S = steps + 1;
-    const bool bfm = c.encoder_module == SBK_ENC_BRANCHFORMER && m->has_enc;
-    const bool hmx = c.attention_type == SBK_ATT_HYPERMIX && m->has_enc;
-    const size_t hm_part = hmx ? hypermix_part_floats(B, T2, c.d_model, c.d_ffn / c.nhead) : 0;
+    const bool bfm = c.encoder_module == SBK_ENC_BRANCHFORMER && m->wt->has_enc;
+    const bool hmx = c.attention_type == SBK_ATT_HYPERMIX && m->wt->has_enc;
     const size_t Cu = bfm ? (size_t)c.csgu_linear_units : 0, Fu = std::max(F, Cu);  // f16 also holds the CSGU input u
     const size_t Md = (size_t)std::max(B, rows) * T2;  // encoder states / cross K,V of every utterance the decoder sees
-    size_t need = 0;
-    auto sz = [&](size_t bytes) { need += (bytes + 255) & ~size_t(255); };
-    sz((size_t)B * L * 4); sz((size_t)B * T0 * c.n_mels * 4); sz(M * d * 4); sz(M * d * 4); sz(Md * d * 4);
-    sz((size_t)rows * d * 4); sz((size_t)rows * c.vocab * 4); sz((size_t)rows * S * 4);
-    sz(B * 4); sz((size_t)std::max(B, rows) * 4); sz((size_t)rows * (S + 1) * 4); sz(rows * 4 + 64); sz(rows * 4); sz(64); sz((size_t)rows * S * 4); sz(B * 4);
-    sz((size_t)B * T1 * F1 * c.cnn_c1 * 2); sz(M * c.input_size * 2); sz(M * d * 2); sz(M * Fu * 2); sz(M * 3 * d * 2);
-    sz(M * d * 2); sz((size_t)T2 * d * 2); sz(Md * d * 2); sz(Md * Ld * 2 * d * 2);
-    sz((size_t)Ld * rows * S * d * 2); sz((size_t)Ld * rows * S * d * 2);
-    sz((size_t)rows * d * 2); sz((size_t)rows * d * 2); sz((size_t)rows * d * 2); sz((size_t)rows * F * 2);
-    sz((size_t)2 * rows * S * 4); sz(B * 4 + 64); sz((size_t)2 * rows * 4); sz((size_t)rows * d * 4); sz((size_t)rows * 33 * 4);
-    sz((size_t)rows * S * 4); sz((size_t)rows * S * 4); sz((size_t)rows * S * 4); sz((size_t)rows * S * 4);
-    const size_t dl = m->has_lm ? c.lm_d_model : 0, Fl = m->has_lm ? c.lm_d_ffn : 0, Ll = m->has_lm ? c.lm_layers : 0;
-    if (m->has_lm) {
-        sz(rows * dl * 4); sz(rows * dl * 4); sz((size_t)rows * c.vocab * 4); sz((size_t)rows * c.vocab * 4);
-        sz(rows * dl * 2); sz(rows * dl * 2); sz(rows * dl * 2); sz(rows * Fl * 2); sz(rows * dl * 2);
-        sz(Ll * rows * S * dl * 2); sz(Ll * rows * S * dl * 2); sz((size_t)rows * S * 4);
-    }
-    if (bfm) { sz(M * d * 2); sz(M * 2 * d * 2); sz(M * Cu / 2 * 2); sz(M * 8); }
-    if (hmx) { sz(hm_part * 4); sz((size_t)B * d * (F / c.nhead) * 2); sz((size_t)B * c.nhead * 4); }
-    need += 1 << 20;
-    if (need > m->ws.cap) {
-        if (m->ws.base) { cudaDeviceSynchronize(); cudaFree(m->ws.base); m->ws.base = nullptr; }
-        if (cudaMalloc(&m->ws.base, need) != cudaSuccess) {
-            m->ws.cap = 0;
-            set_error("workspace cudaMalloc(%zu) failed", need);
-            return SBK_ERR_NOMEM;
-        }
-        m->ws.cap = need;
-    }
-    drop_graphs(m);
-    m->ws.used = 0;
-    AsrModel::Buf& b = m->b;
-#define TAKE(field, type, bytes) b.field = reinterpret_cast<type*>(m->ws.take(bytes))
-    TAKE(wav, float, (size_t)B * L * 4); TAKE(feats, float, (size_t)B * T0 * c.n_mels * 4); TAKE(x, float, M * d * 4);
-    TAKE(glu, float, M * d * 4); TAKE(enc_out, float, Md * d * 4); TAKE(dx, float, (size_t)rows * d * 4);
-    TAKE(logits, float, (size_t)rows * c.vocab * 4); TAKE(score, float, (size_t)rows * S * 4);
-    TAKE(utt_max, int, B * 4); TAKE(enc_len, int, (size_t)std::max(B, rows) * 4); TAKE(tokens, int, (size_t)rows * (S + 1) * 4); TAKE(step, int, rows * 4 + 64);
-    TAKE(has_ended, int, rows * 4); TAKE(ended_count, int, 64); TAKE(pred, int, (size_t)rows * S * 4); TAKE(rel_len, float, B * 4);
-    TAKE(act1, __half, (size_t)B * T1 * F1 * c.cnn_c1 * 2); TAKE(a_in, __half, M * c.input_size * 2); TAKE(h16, __half, M * d * 2);
-    TAKE(f16, __half, M * Fu * 2); TAKE(qkv16, __half, M * 3 * d * 2); TAKE(att16, __half, M * d * 2);
-    TAKE(P16, __half, (size_t)T2 * d * 2); TAKE(enc16, __half, Md * d * 2); TAKE(ckv16, __half, Md * Ld * 2 * d * 2);
-    TAKE(kcache, __half, (size_t)Ld * rows * S * d * 2); TAKE(vcache, __half, (size_t)Ld * rows * S * d * 2);
-    TAKE(dh16, __half, (size_t)rows * d * 2); TAKE(dq16, __half, (size_t)rows * d * 2); TAKE(datt16, __half, (size_t)rows * d * 2);
-    TAKE(df16, __half, (size_t)rows * F * 2);
-    TAKE(lineage, int, (size_t)2 * rows * S * 4); TAKE(finished, int, B * 4 + 64); TAKE(seq_scores, float, (size_t)2 * rows * 4);
-    TAKE(lnout, float, (size_t)rows * d * 4); TAKE(beam_scr, float, (size_t)rows * 33 * 4);
-    TAKE(hist_tok, int, (size_t)rows * S * 4); TAKE(hist_pred, int, (size_t)rows * S * 4);
-    TAKE(hist_score, float, (size_t)rows * S * 4); TAKE(hist_lp, float, (size_t)rows * S * 4);
-    if (m->has_lm) {
-        TAKE(lx, float, rows * dl * 4); TAKE(lh32, float, rows * dl * 4); TAKE(lm_logits, float, (size_t)rows * c.vocab * 4);
-        TAKE(lm_extra, float, (size_t)rows * c.vocab * 4);
-        TAKE(lx16, __half, rows * dl * 2); TAKE(lq16, __half, rows * dl * 2); TAKE(latt16, __half, rows * dl * 2);
-        TAKE(lf16, __half, rows * Fl * 2); TAKE(lh16, __half, rows * dl * 2);
-        TAKE(lkc, __half, Ll * rows * S * dl * 2); TAKE(lvc, __half, Ll * rows * S * dl * 2); TAKE(tok_cache, int, (size_t)rows * S * 4);
-        if (!b.tok_cache) { set_error("workspace carve failed (LM)"); return SBK_ERR_NOMEM; }
+    take(b.wav, (size_t)B * L * 4); take(b.feats, (size_t)B * T0 * c.n_mels * 4); take(b.x, M * d * 4);
+    take(b.glu, M * d * 4); take(b.enc_out, Md * d * 4); take(b.dx, (size_t)rows * d * 4);
+    take(b.logits, (size_t)rows * c.vocab * 4); take(b.score, (size_t)rows * S * 4);
+    take(b.utt_max, B * 4); take(b.enc_len, (size_t)std::max(B, rows) * 4); take(b.tokens, (size_t)rows * (S + 1) * 4); take(b.step, rows * 4 + 64);
+    take(b.has_ended, rows * 4); take(b.ended_count, 64); take(b.pred, (size_t)rows * S * 4); take(b.rel_len, B * 4);
+    take(b.act1, (size_t)B * T1 * F1 * c.cnn_c1 * 2); take(b.a_in, M * c.input_size * 2); take(b.h16, M * d * 2);
+    take(b.f16, M * Fu * 2); take(b.qkv16, M * 3 * d * 2); take(b.att16, M * d * 2);
+    take(b.P16, (size_t)T2 * d * 2); take(b.enc16, Md * d * 2); take(b.ckv16, Md * Ld * 2 * d * 2);
+    take(b.kcache, (size_t)Ld * rows * S * d * 2); take(b.vcache, (size_t)Ld * rows * S * d * 2);
+    take(b.dh16, (size_t)rows * d * 2); take(b.dq16, (size_t)rows * d * 2); take(b.datt16, (size_t)rows * d * 2);
+    take(b.df16, (size_t)rows * F * 2);
+    take(b.lineage, (size_t)2 * rows * S * 4); take(b.finished, B * 4 + 64); take(b.seq_scores, (size_t)2 * rows * 4);
+    take(b.lnout, (size_t)rows * d * 4); take(b.beam_scr, (size_t)rows * 33 * 4);
+    take(b.hist_tok, (size_t)rows * S * 4); take(b.hist_pred, (size_t)rows * S * 4);
+    take(b.hist_score, (size_t)rows * S * 4); take(b.hist_lp, (size_t)rows * S * 4);
+    if (m->wt->has_lm) {
+        const size_t dl = c.lm_d_model, Fl = c.lm_d_ffn, Ll = c.lm_layers;
+        take(b.lx, rows * dl * 4); take(b.lh32, rows * dl * 4); take(b.lm_logits, (size_t)rows * c.vocab * 4);
+        take(b.lm_extra, (size_t)rows * c.vocab * 4);
+        take(b.lx16, rows * dl * 2); take(b.lq16, rows * dl * 2); take(b.latt16, rows * dl * 2);
+        take(b.lf16, rows * Fl * 2); take(b.lh16, rows * dl * 2);
+        take(b.lkc, Ll * rows * S * dl * 2); take(b.lvc, Ll * rows * S * dl * 2); take(b.tok_cache, (size_t)rows * S * 4);
     }
     if (bfm) {
-        TAKE(hc16, __half, M * d * 2); TAKE(cat16, __half, M * 2 * d * 2); TAKE(g16, __half, M * Cu / 2 * 2);
-        TAKE(csgu_stats, float2, M * 8);
-        if (!b.csgu_stats) { set_error("workspace carve failed (Branchformer)"); return SBK_ERR_NOMEM; }
+        take(b.hc16, M * d * 2); take(b.cat16, M * 2 * d * 2); take(b.g16, M * Cu / 2 * 2);
+        take(b.csgu_stats, M * 8);
     }
     if (hmx) {
-        TAKE(hm_part, float, hm_part * 4); TAKE(hm_G, __half, (size_t)B * d * (F / c.nhead) * 2);
-        TAKE(hm_gscale, float, (size_t)B * c.nhead * 4);
-        if (!b.hm_gscale) { set_error("workspace carve failed (HyperMixing)"); return SBK_ERR_NOMEM; }
+        take(b.hm_part, hypermix_part_floats(B, T2, c.d_model, c.d_ffn / c.nhead) * 4);
+        take(b.hm_G, (size_t)B * d * (F / c.nhead) * 2);
+        take(b.hm_gscale, (size_t)B * c.nhead * 4);
     }
-    if (!b.df16 || !b.seq_scores || !b.lnout || !b.hist_lp) { set_error("workspace carve failed"); return SBK_ERR_NOMEM; }
-#undef TAKE
+}
+
+// (Re)carve the workspace for at least the given shapes and the ones it is already carved for.
+static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
+    if (m->ws.base && B <= m->wsB && L <= m->wsL && rows <= m->ws_rows && steps <= m->ws_steps) return SBK_OK;
+    B = std::max(B, m->wsB); L = std::max(L, m->wsL); rows = std::max(rows, m->ws_rows); steps = std::max(steps, m->ws_steps);
+    Carver measure;
+    workspace_layout(m, B, L, rows, steps, m->b, measure);
+    RC(grow_buffer(m, m->ws, measure.used + (1 << 20), "workspace"));
+    drop_graphs(m);
+    Carver carve{static_cast<uint8_t*>(m->ws.base)};
+    workspace_layout(m, B, L, rows, steps, m->b, carve);
     m->wsB = B; m->wsL = L; m->ws_rows = rows; m->ws_steps = steps;
     return SBK_OK;
 }
-
-#define RC(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
 
 // Branchformer layers (Branchformer.py:92-234, 330-410) on the fp32 residual stream b.x [B*T, d] -> enc_out = encoder.norm(x):
 //     x1 = RelPosMHAXL(norm_mhsa(x));  x2 = post_channel_proj(CSGU(act(pre_channel_proj(norm_conv(x)))))
@@ -726,7 +746,7 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
 // Neither branch masks padded frames (the attention masks padded keys only).  x1 and x2 are written into the two column
 // halves of one [B*T, 2d] fp16 buffer so that merge_proj is one K = 2d GEMM with the residual epilogue.
 static int run_branchformer_layers(AsrModel* m, int B, int T, const int* enc_len, float* enc_out, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int M = B * T, d = c.d_model, H = c.nhead, dh = d / H, C = c.csgu_linear_units;
     SBK_REQUIRE(m->dyn_chunk == 0, "encode: the Branchformer has no chunked (DynChunkTrainConfig) mode");
@@ -734,13 +754,13 @@ static int run_branchformer_layers(AsrModel* m, int B, int T, const int* enc_len
     const int act = c.branchformer_activation == SBK_ACT_RELU ? ACT_RELU : ACT_GELU;
     GemmEpilogue e;
     for (int l = 0; l < c.num_encoder_layers; ++l) {
-        const EncLayerW& w = m->enc[l];
+        const EncLayerW& w = m->wt->enc[l];
         RC(layernorm_rows_dual(b.x, b.h16, w.norm1_g, w.norm1_b, b.hc16, w.nconv_g, w.nconv_b, M, d, 1e-5f, st));
         // --- attention branch -> cat16[:, :d]
         e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.qkv16; e.ldo = 3 * d;
         RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
         e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
-        RC(gemm_f16(m->relpos_pe, d, w.wpos, d, e, T, d, d, st));
+        RC(gemm_f16(m->wt->relpos_pe, d, w.wpos, d, e, T, d, d, st));
         RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, true, w.pos_u, w.pos_v, b.P16, d, att_scale, b.att16, d, st));
         e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bo; e.out = b.cat16; e.ldo = 2 * d;
         RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
@@ -755,36 +775,36 @@ static int run_branchformer_layers(AsrModel* m, int B, int T, const int* enc_len
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bmerge; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
         RC(gemm_f16(b.cat16, 2 * d, w.wmerge, 2 * d, e, M, d, 2 * d, st));
     }
-    return layernorm_rows(b.x, enc_out, false, m->enc_norm_g, m->enc_norm_b, M, d, 1e-6f, false, st);
+    return layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, false, st);
 }
 
 // feats [B, T0, n_mels] fp32 (already normalised) -> enc_out fp32 [B, T2, d] (+ enc16). enc_len device int[B].
 static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int* enc_len, float* cnn_out_f,
                        float* enc_out, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int T1 = (T0 - 1) / 2 + 1, T = feats ? (T1 - 1) / 2 + 1 : T0;  // feats == nullptr: b.a_in holds [B*T0, input_size]
     const int M = B * T, d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H;
-    SBK_REQUIRE(m->has_enc, "encode: this handle was created without encoder weights");
-    SBK_REQUIRE(feats == nullptr || m->has_cnn, "encode: this handle was created without CNN weights");
+    SBK_REQUIRE(m->wt->has_enc, "encode: this handle was created without encoder weights");
+    SBK_REQUIRE(feats == nullptr || m->wt->has_cnn, "encode: this handle was created without CNN weights");
     if (c.attention_type == SBK_ATT_HYPERMIX)  // HyperMixing adds its own 3000-row table: longer inputs fail in the reference
         SBK_REQUIRE(T <= HM_PE_ROWS, "encode: %d frames exceed HyperMixing's %d-row positional table", T, HM_PE_ROWS);
     else
-        SBK_REQUIRE(T <= m->pos_len, "encode: %d frames exceed max_len=%d", T, m->pos_len);
+        SBK_REQUIRE(T <= m->wt->pos_len, "encode: %d frames exceed max_len=%d", T, m->wt->pos_len);
     SBK_REQUIRE(c.attention_type != SBK_ATT_HYPERMIX || m->dyn_chunk == 0,
                 "encode: HyperMixing has no chunked (DynChunkTrainConfig) mode");
     SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER || T > (c.kernel_size - 1) / 2,
                 "encode: the Branchformer's reflect-padded conv needs more than %d frames (got %d)", (c.kernel_size - 1) / 2, T);
     if (feats != nullptr)
-        RC(cnn_frontend_forward(feats, B, T0, c.n_mels, m->c1_w, m->c1_b, m->c1_g, m->c1_be, c.cnn_c1, m->c2_w, m->c2_b,
-                                m->c2_g, m->c2_be, c.cnn_c2, b.act1, b.a_in, cnn_out_f, st));
+        RC(cnn_frontend_forward(feats, B, T0, c.n_mels, m->wt->c1_w, m->wt->c1_b, m->wt->c1_g, m->wt->c1_be, c.cnn_c1, m->wt->c2_w, m->wt->c2_b,
+                                m->wt->c2_g, m->wt->c2_be, c.cnn_c2, b.act1, b.a_in, cnn_out_f, st));
     GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->b_in; e.out = b.x; e.ldo = d;
-    RC(gemm_f16(b.a_in, c.input_size, m->w_in, c.input_size, e, M, d, c.input_size, st));
+    e.mode = EPI_F32; e.bias = m->wt->b_in; e.out = b.x; e.ldo = d;
+    RC(gemm_f16(b.a_in, c.input_size, m->wt->w_in, c.input_size, e, M, d, c.input_size, st));
     if (c.encoder_module == SBK_ENC_BRANCHFORMER) return run_branchformer_layers(m, B, T, enc_len, enc_out, st);
     const float att_scale = 1.0f / sqrtf((float)d);  // nnet/attention.py:521,1272: 1/sqrt(embed_dim), not head_dim
     for (int l = 0; l < c.num_encoder_layers; ++l) {
-        const EncLayerW& w = m->enc[l];
+        const EncLayerW& w = m->wt->enc[l];
         // --- ffn module 1 (Conformer.py:479); its LayerNorm was fused into the previous layer's norm2 kernel
         if (l == 0) RC(layernorm_rows(b.x, b.h16, true, w.ffn1_ln_g, w.ffn1_ln_b, M, d, 1e-5f, false, st));
         e = GemmEpilogue(); e.mode = EPI_F16; e.act = ACT_SILU; e.bias = w.ffn1_b1; e.out = b.f16; e.ldo = F;
@@ -794,18 +814,18 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
         // --- self-attention (Conformer.py:481-492)
         RC(layernorm_rows(b.x, b.h16, true, w.norm1_g, w.norm1_b, M, d, 1e-5f, false, st));
         if (c.attention_type == SBK_ATT_HYPERMIX) {  // x += HyperMixing(norm1(x)) (hypermixing.py:90-195)
-            RC(hypermix_forward(b.h16, B, T, d, H, F / H, enc_len, m->hm_pe, w.hm, b.hm_part, b.hm_G, b.hm_gscale, b.x, st));
+            RC(hypermix_forward(b.h16, B, T, d, H, F / H, enc_len, m->wt->hm_pe, w.hm, b.hm_part, b.hm_G, b.hm_gscale, b.x, st));
         } else {
             e = GemmEpilogue(); e.out = b.qkv16; e.ldo = 3 * d;
             if (c.attention_type == SBK_ATT_ROPE) {
-                e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->rope_cos; e.rope_sin = m->rope_sin; e.head_dim = dh;
+                e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->wt->rope_cos; e.rope_sin = m->wt->rope_sin; e.head_dim = dh;
             } else {
                 e.mode = EPI_F16;
             }
             RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
             if (c.attention_type == SBK_ATT_RELPOS) {
                 e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
-                RC(gemm_f16(m->relpos_pe, d, w.wpos, d, e, T, d, d, st));
+                RC(gemm_f16(m->wt->relpos_pe, d, w.wpos, d, e, T, d, d, st));
             }
             RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, c.attention_type == SBK_ATT_RELPOS, w.pos_u, w.pos_v,
                                  b.P16, d, att_scale, b.att16, d, st, m->dyn_chunk, m->dyn_left));
@@ -827,15 +847,15 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.ffn2_b2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 0.5f;
         RC(gemm_f16(b.f16, F, w.ffn2_w2, F, e, M, d, F, st));
         if (l + 1 < c.num_encoder_layers) {  // norm2 (fp32 residual stream) + the next layer's ffn1 LayerNorm (fp16 operand)
-            const EncLayerW& nx = m->enc[l + 1];
+            const EncLayerW& nx = m->wt->enc[l + 1];
             RC(layernorm2_rows(b.x, b.x, b.h16, true, w.norm2_g, w.norm2_b, 1e-5f, nx.ffn1_ln_g, nx.ffn1_ln_b, 1e-5f, M, d, st));
         } else {                             // norm2 + the encoder's final LayerNorm (Conformer.py:700)
-            RC(layernorm2_rows(b.x, nullptr, enc_out, false, w.norm2_g, w.norm2_b, 1e-5f, m->enc_norm_g, m->enc_norm_b, 1e-6f, M,
+            RC(layernorm2_rows(b.x, nullptr, enc_out, false, w.norm2_g, w.norm2_b, 1e-5f, m->wt->enc_norm_g, m->wt->enc_norm_b, 1e-6f, M,
                                d, st));
         }
     }
     if (c.num_encoder_layers == 0)
-        RC(layernorm_rows(b.x, enc_out, false, m->enc_norm_g, m->enc_norm_b, M, d, 1e-6f, false, st));
+        RC(layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, false, st));
     return SBK_OK;
 }
 
@@ -845,12 +865,34 @@ __global__ void abs_len_kernel(const float* rel, int B, int T, int* out) {
     if (i < B) out[i] = min(T, max(0, __float2int_rn(rel[i] * static_cast<float>(T))));
 }
 
+// enc_len [B] = round(rel_len * T), or T for every utterance when rel_len is null
+static int set_enc_len(int* enc_len, const float* rel_len, int B, int T, cudaStream_t st) {
+    if (rel_len) {
+        abs_len_kernel<<<ceil_div(B, 128), 128, 0, st>>>(rel_len, B, T, enc_len);
+        SBK_LAUNCH_CHECK();
+        return SBK_OK;
+    }
+    std::vector<int> full(B, T);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(enc_len, full.data(), B * 4, cudaMemcpyHostToDevice, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));  // before `full` goes out of scope
+    return SBK_OK;
+}
+
+// Copies the first `steps` columns of a [rows, S_max] per-step workspace array (b.pred, b.score) into dst [rows, ld];
+// nothing when dst is null.
+static int copy_steps(const AsrModel* m, void* dst, int ld, const void* src, int steps, int rows, cudaMemcpyKind kind,
+                      cudaStream_t st) {
+    const size_t S_max = m->ws_steps + 1;
+    if (dst) SBK_CUDA_CHECK(cudaMemcpy2DAsync(dst, (size_t)ld * 4, src, S_max * 4, (size_t)steps * 4, rows, kind, st));
+    return SBK_OK;
+}
+
 // Decoder pre-norm feeding a projection: either fused into the projection kernel (a.X) or a separate tiny kernel
 // writing fp16 (a.A).  Fusion saves a launch per projection (single-batch latency); the separate kernel avoids
 // recomputing the same 32-row LayerNorm in ~100-300 CTAs (GPU time when several batches are in flight).
 static int dec_ln(AsrModel* m, SkinnyArgs& a, const float* g, const float* bta, int rows, cudaStream_t st) {
     AsrModel::Buf& b = m->b;
-    const int d = m->cfg.d_model;
+    const int d = m->wt->cfg.d_model;
     if (m->fuse_dec_ln && (d == 256 || d == 512 || d == 768 || d == 1024)) {  // widths the LN-fused projection is built for
         a.X = b.dx; a.ln_g = g; a.ln_b = bta; a.ln_eps = 1e-6f;
         return SBK_OK;
@@ -868,29 +910,29 @@ static int dec_ln(AsrModel* m, SkinnyArgs& a, const float* g, const float* bta, 
 // [utt * T][K(d) | V(d)] rows).  Needs head_dim 64.
 static bool xatt_headmajor(const AsrModel* m) {
     static const bool legacy = getenv("SBK_XATT_ROWMAJOR") != nullptr;
-    return !legacy && m->cfg.d_model / m->cfg.nhead == 64 && m->cfg.d_model % 256 == 0;
+    return !legacy && m->wt->cfg.d_model / m->wt->cfg.nhead == 64 && m->wt->cfg.d_model % 256 == 0;
 }
 static int project_cross_kv(AsrModel* m, int M, int T, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, Ld = c.num_decoder_layers;
     RC(cast_f32_f16(b.enc_out, b.enc16, (size_t)M * d, st));
     if (xatt_headmajor(m)) {  // w_ckv / b_ckv are [Ld * 2d] rows: every layer's K and V in ONE GEMM, scattered per layer
         GemmEpilogue e;
-        e.mode = EPI_F16; e.bias = m->b_ckv; e.out = b.ckv16; e.ldo = Ld * 2 * d;
+        e.mode = EPI_F16; e.bias = m->wt->b_ckv; e.out = b.ckv16; e.ldo = Ld * 2 * d;
         e.kv_heads = c.nhead; e.kv_part_stride = (size_t)M * d; e.kv_layer_stride = (size_t)M * 2 * d; e.T = T;
-        return gemm_f16(b.enc16, d, m->w_ckv, d, e, M, Ld * 2 * d, d, st);
+        return gemm_f16(b.enc16, d, m->wt->w_ckv, d, e, M, Ld * 2 * d, d, st);
     }
     for (int l = 0; l < Ld; ++l) {
         GemmEpilogue e;
-        e.mode = EPI_F16; e.bias = m->b_ckv + (size_t)l * 2 * d; e.out = b.ckv16 + (size_t)l * M * 2 * d; e.ldo = 2 * d;
-        RC(gemm_f16(b.enc16, d, m->w_ckv + (size_t)l * 2 * d * d, d, e, M, 2 * d, d, st));
+        e.mode = EPI_F16; e.bias = m->wt->b_ckv + (size_t)l * 2 * d; e.out = b.ckv16 + (size_t)l * M * 2 * d; e.ldo = 2 * d;
+        RC(gemm_f16(b.enc16, d, m->wt->w_ckv + (size_t)l * 2 * d * d, d, e, M, 2 * d, d, st));
     }
     return SBK_OK;
 }
 // fills the K/V addressing of a cross-attention call for layer l
 static void cross_kv_args(const AsrModel* m, DecAttnArgs& t, int l, int n_utt, int T) {
-    const int d = m->cfg.d_model;
+    const int d = m->wt->cfg.d_model;
     const size_t M = (size_t)n_utt * T;
     t.kbase = m->b.ckv16 + (size_t)l * M * 2 * d;
     if (xatt_headmajor(m)) {
@@ -902,12 +944,12 @@ static void cross_kv_args(const AsrModel* m, DecAttnArgs& t, int l, int n_utt, i
 
 static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage,
                                     cudaStream_t st, bool with_head) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H, Ld = c.num_decoder_layers;
     const int n_utt = rows / rows_per_utt;
     for (int l = 0; l < Ld; ++l) {
-        const DecLayerW& w = m->dec[l];
+        const DecLayerW& w = m->wt->dec[l];
         __half* kc = b.kcache + (size_t)l * rows * S_max * d;
         __half* vc = b.vcache + (size_t)l * rows * S_max * d;
         RC(layernorm_rows(b.dx, b.dh16, true, w.n1g, w.n1b, rows, d, 1e-6f, false, st, true));
@@ -939,17 +981,17 @@ static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int
         RC(gemm_f16_small(b.df16, F, w.w_ffn2, F, e, rows, d, F, st));
     }
     if (!with_head) return SBK_OK;
-    SBK_REQUIRE(m->w_lin != nullptr, "decode step: this handle was created without the output head (seq_lin.w.*)");
-    RC(layernorm_rows(b.dx, b.dh16, true, m->dec_norm_g, m->dec_norm_b, rows, d, 1e-6f, false, st, true));
+    SBK_REQUIRE(m->wt->w_lin != nullptr, "decode step: this handle was created without the output head (seq_lin.w.*)");
+    RC(layernorm_rows(b.dx, b.dh16, true, m->wt->dec_norm_g, m->wt->dec_norm_b, rows, d, 1e-6f, false, st, true));
     GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->b_lin; e.out = b.logits; e.ldo = c.vocab;
-    RC(gemm_f16_small(b.dh16, d, m->w_lin, d, e, rows, c.vocab, d, st));
+    e.mode = EPI_F32; e.bias = m->wt->b_lin; e.out = b.logits; e.ldo = c.vocab;
+    RC(gemm_f16_small(b.dh16, d, m->wt->w_lin, d, e, rows, c.vocab, d, st));
     return SBK_OK;
 }
 
 // the wgmma decode path (enqueue_decode_layers_tc) for `rows` live hypotheses
 static bool decode_tc(const AsrModel* m, int rows) {
-    return rows >= m->dec_tc_rows && m->cfg.d_model % 32 == 0;  // (the QKV -> cache scatter epilogue works on 32-column chunks)
+    return rows >= m->dec_tc_rows && m->wt->cfg.d_model % 32 == 0;  // (the QKV -> cache scatter epilogue works on 32-column chunks)
 }
 // Programmatic dependent launch is on for the wgmma decode path (its GEMMs and LayerNorms are launched with it
 // unconditionally) and off on the weight-streaming path, where it measured no faster (single_batch, H100 SXM at 400 W:
@@ -960,14 +1002,14 @@ static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T,
                                  cudaStream_t st, bool with_head = true) {
     if (decode_tc(m, rows))
         return enqueue_decode_layers_tc(m, rows, rows_per_utt, T, S_max, lineage, st, with_head);
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H, Ld = c.num_decoder_layers;
     const int ffn_epi = c.decoder_activation == SBK_ACT_GELU ? SK_F16_GELU : SK_F16_RELU;
     const int n_utt = rows / rows_per_utt;
     // b.dx already holds emb[token] * sqrt(d) + pe[step] (written by greedy_reset / the previous greedy_select)
     for (int l = 0; l < Ld; ++l) {
-        const DecLayerW& w = m->dec[l];
+        const DecLayerW& w = m->wt->dec[l];
         __half* kc = b.kcache + (size_t)l * rows * S_max * d;
         __half* vc = b.vcache + (size_t)l * rows * S_max * d;
         SkinnyArgs a{};  // LN1 + self-attention in_proj; k/v appended to the cache at position step
@@ -1008,10 +1050,10 @@ static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T,
         RC(skinny_gemm(a, st));
     }
     if (!with_head) return SBK_OK;
-    SBK_REQUIRE(m->w_lin != nullptr, "decode step: this handle was created without the output head (seq_lin.w.*)");
+    SBK_REQUIRE(m->wt->w_lin != nullptr, "decode step: this handle was created without the output head (seq_lin.w.*)");
     SkinnyArgs a{};  // final LayerNorm + seq_lin
-    RC(dec_ln(m, a, m->dec_norm_g, m->dec_norm_b, rows, st));
-    a.W = m->w_lin; a.ldw = d; a.bias = m->b_lin; a.n_rows = rows; a.N = c.vocab; a.K = d;
+    RC(dec_ln(m, a, m->wt->dec_norm_g, m->wt->dec_norm_b, rows, st));
+    a.W = m->wt->w_lin; a.ldw = d; a.bias = m->wt->b_lin; a.n_rows = rows; a.N = c.vocab; a.K = d;
     a.epi = SK_F32; a.out = b.logits; a.ldo = c.vocab;
     RC(skinny_gemm(a, st));
     return SBK_OK;
@@ -1021,8 +1063,8 @@ static int enqueue_decode_step(AsrModel* m, int rows, int rows_per_utt, int T, i
                                int L_lp, cudaStream_t st) {
     AsrModel::Buf& b = m->b;
     RC(enqueue_decode_layers(m, rows, rows_per_utt, T, S_max, nullptr, st));
-    RC(greedy_select(b.logits, rows, m->cfg.vocab, b.step, eos, b.tokens, S_max + 1, b.has_ended, b.ended_count, b.pred,
-                     b.score, S_max, log_probs, L_lp, m->emb, m->dec_pe, m->cfg.d_model, b.dx, st));
+    RC(greedy_select(b.logits, rows, m->wt->cfg.vocab, b.step, eos, b.tokens, S_max + 1, b.has_ended, b.ended_count, b.pred,
+                     b.score, S_max, log_probs, L_lp, m->wt->emb, m->wt->dec_pe, m->wt->cfg.d_model, b.dx, st));
     return SBK_OK;
 }
 
@@ -1032,11 +1074,11 @@ static int enqueue_decode_step(AsrModel* m, int rows, int rows_per_utt, int T, i
 // The same step with the projections on the wgmma GEMM (128 x 32/64 tiles): used when many hypotheses are live (wide beams,
 // B * beam >= dec_tc_rows), where the weight-streaming kernel's cost grows with every 32 rows.
 static int enqueue_lm_step_tc(AsrModel* m, int rows, int S_max, float temperature, float weight, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead;
     for (int l = 0; l < c.lm_layers; ++l) {
-        const LmLayerW& w = m->lm[l];
+        const LmLayerW& w = m->wt->lm[l];
         __half* kc = b.lkc + (size_t)l * rows * S_max * dl;
         __half* vc = b.lvc + (size_t)l * rows * S_max * dl;
         GemmEpilogue e;
@@ -1058,24 +1100,24 @@ static int enqueue_lm_step_tc(AsrModel* m, int rows, int S_max, float temperatur
         RC(gemm_f16_small(b.lf16, Fl, w.w2, Fl, e, rows, dl, Fl, st));
         RC(layernorm_dual(b.lx, b.lx16, w.n2g, w.n2b, rows, dl, 1e-6f, true, st));
     }
-    RC(layernorm_dual(b.lx, b.lx16, m->lm_norm_g, m->lm_norm_b, rows, dl, 1e-6f, false, st));  // encoder.norm
+    RC(layernorm_dual(b.lx, b.lx16, m->wt->lm_norm_g, m->wt->lm_norm_b, rows, dl, 1e-6f, false, st));  // encoder.norm
     GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->lm_bp0; e.out = b.lh32; e.ldo = dl;
-    RC(gemm_f16_small(b.lx16, dl, m->lm_wp0, dl, e, rows, dl, dl, st));
-    RC(layernorm_dual(b.lh32, b.lh16, m->lm_lnp_g, m->lm_lnp_b, rows, dl, 1e-6f, false, st));
-    e = GemmEpilogue(); e.mode = EPI_F32; e.bias = m->lm_bp2; e.out = b.lm_logits; e.ldo = c.vocab;
-    RC(gemm_f16_small(b.lh16, dl, m->lm_wp2, dl, e, rows, c.vocab, dl, st));
+    e.mode = EPI_F32; e.bias = m->wt->lm_bp0; e.out = b.lh32; e.ldo = dl;
+    RC(gemm_f16_small(b.lx16, dl, m->wt->lm_wp0, dl, e, rows, dl, dl, st));
+    RC(layernorm_dual(b.lh32, b.lh16, m->wt->lm_lnp_g, m->wt->lm_lnp_b, rows, dl, 1e-6f, false, st));
+    e = GemmEpilogue(); e.mode = EPI_F32; e.bias = m->wt->lm_bp2; e.out = b.lm_logits; e.ldo = c.vocab;
+    RC(gemm_f16_small(b.lh16, dl, m->wt->lm_wp2, dl, e, rows, c.vocab, dl, st));
     RC(weighted_log_softmax(b.lm_logits, b.lm_extra, rows, c.vocab, temperature, weight, st));
     return SBK_OK;
 }
 
 static int enqueue_lm_step(AsrModel* m, int rows, int S_max, float temperature, float weight, cudaStream_t st) {
     if (rows >= m->dec_tc_rows) return enqueue_lm_step_tc(m, rows, S_max, temperature, weight, st);
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead;
     for (int l = 0; l < c.lm_layers; ++l) {
-        const LmLayerW& w = m->lm[l];
+        const LmLayerW& w = m->wt->lm[l];
         __half* kc = b.lkc + (size_t)l * rows * S_max * dl;
         __half* vc = b.lvc + (size_t)l * rows * S_max * dl;
         SkinnyArgs a{};
@@ -1100,13 +1142,13 @@ static int enqueue_lm_step(AsrModel* m, int rows, int S_max, float temperature, 
         RC(skinny_gemm(a, st));
         RC(layernorm_dual(b.lx, b.lx16, w.n2g, w.n2b, rows, dl, 1e-6f, true, st));
     }
-    RC(layernorm_dual(b.lx, b.lx16, m->lm_norm_g, m->lm_norm_b, rows, dl, 1e-6f, false, st));  // encoder.norm
+    RC(layernorm_dual(b.lx, b.lx16, m->wt->lm_norm_g, m->wt->lm_norm_b, rows, dl, 1e-6f, false, st));  // encoder.norm
     SkinnyArgs a{};
-    a.A = b.lx16; a.lda = dl; a.W = m->lm_wp0; a.ldw = dl; a.bias = m->lm_bp0; a.n_rows = rows; a.N = dl; a.K = dl;
+    a.A = b.lx16; a.lda = dl; a.W = m->wt->lm_wp0; a.ldw = dl; a.bias = m->wt->lm_bp0; a.n_rows = rows; a.N = dl; a.K = dl;
     a.epi = SK_F32; a.out = b.lh32; a.ldo = dl;
     RC(skinny_gemm(a, st));
-    RC(layernorm_dual(b.lh32, b.lh16, m->lm_lnp_g, m->lm_lnp_b, rows, dl, 1e-6f, false, st));
-    a = SkinnyArgs{}; a.A = b.lh16; a.lda = dl; a.W = m->lm_wp2; a.ldw = dl; a.bias = m->lm_bp2; a.n_rows = rows;
+    RC(layernorm_dual(b.lh32, b.lh16, m->wt->lm_lnp_g, m->wt->lm_lnp_b, rows, dl, 1e-6f, false, st));
+    a = SkinnyArgs{}; a.A = b.lh16; a.lda = dl; a.W = m->wt->lm_wp2; a.ldw = dl; a.bias = m->wt->lm_bp2; a.n_rows = rows;
     a.N = c.vocab; a.K = dl; a.epi = SK_F32; a.out = b.lm_logits; a.ldo = c.vocab;
     RC(skinny_gemm(a, st));
     RC(weighted_log_softmax(b.lm_logits, b.lm_extra, rows, c.vocab, temperature, weight, st));
@@ -1118,79 +1160,67 @@ static int enqueue_lm_step(AsrModel* m, int rows, int S_max, float temperature, 
 // on the host from that history (speechbrain_b200/decoders/seq2seq.py).
 static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hist_tok_out, int* hist_pred_out,
                     float* hist_score_out, float* hist_lp_out, int* steps_done, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, Ld = c.num_decoder_layers, M = B * T, beam = p.beam_size, rows = B * beam, S_max = m->ws_steps + 1;
-    SBK_REQUIRE(m->has_dec, "beam: this handle was created without decoder weights");
+    SBK_REQUIRE(m->wt->has_dec, "beam: this handle was created without decoder weights");
     SBK_REQUIRE(p.max_steps <= m->ws_steps && p.max_steps + 1 <= c.max_len, "beam: max_steps=%d too large", p.max_steps);
     *steps_done = 0;
     if (p.max_steps <= 0) return SBK_OK;
     RC(project_cross_kv(m, M, T, st));
     set_decode_pdl(m, rows);
     const bool use_lm = p.lm_weight != 0.0f;
-    SBK_REQUIRE(!use_lm || m->has_lm, "beam: lm_weight != 0 but this handle has no TransformerLM weights");
+    SBK_REQUIRE(!use_lm || m->wt->has_lm, "beam: lm_weight != 0 but this handle has no TransformerLM weights");
     const bool use_ctc = p.ctc_weight != 0.0f;
     // the search history lives in the workspace (fixed addresses: the step graph bakes them in) and is copied out at the end
     int* hist_tok = b.hist_tok; int* hist_pred = b.hist_pred; float* hist_score = b.hist_score; float* hist_lp = b.hist_lp;
     CtcStep cs{};
     if (use_ctc) {  // CTCScorer.reset_mem (scorer.py:243-249) + CTCPrefixScore.__init__ (ctc.py:46-78)
-        SBK_REQUIRE(m->w_ctc, "beam: ctc_weight != 0 but this handle has no ctc_lin weights");
+        SBK_REQUIRE(m->wt->w_ctc, "beam: ctc_weight != 0 but this handle has no ctc_lin weights");
         SBK_REQUIRE(p.blank_index >= 0 && p.blank_index < c.vocab && p.blank_index != p.bos && p.blank_index != p.eos &&
                     p.bos != p.eos, "Set blank, eos and bos to different indexes for joint ATT/CTC or CTC decoding");
         const size_t V = c.vocab;
-        auto al = [](size_t n) { return (n * 4 + 255) & ~size_t(255); };
-        const size_t need = 2 * al((size_t)M * V) + al(M) + 2 * al((size_t)2 * rows * T) + al(2 * rows) + (use_lm ? 0 : al(rows * V)) +
-                            al((size_t)2 * rows * (T + 4)) + al(2 * rows);
-        AsrModel::CtcBuf& cb = m->ctc;
-        if (need > cb.cap) {
-            if (cb.base) { SBK_CUDA_CHECK(cudaStreamSynchronize(st)); cudaFree(cb.base); cb.base = nullptr; cb.cap = 0; }
-            if (m->beam_graph) { cudaGraphExecDestroy(m->beam_graph); m->beam_graph = nullptr; }
-            if (cudaMalloc(&cb.base, need) != cudaSuccess) { set_error("beam: CTC scorer cudaMalloc(%zu) failed", need); return SBK_ERR_NOMEM; }
-            cb.cap = need;
-        }
-        char* q = reinterpret_cast<char*>(cb.base);
-        cb.x = reinterpret_cast<float*>(q); q += al((size_t)M * V);
-        cb.xlin = reinterpret_cast<float*>(q); q += al((size_t)M * V);
-        cb.xb = reinterpret_cast<float*>(q); q += al(M);
-        cb.rsum = reinterpret_cast<float*>(q); q += al((size_t)2 * rows * T);
-        cb.rb = reinterpret_cast<float*>(q); q += al((size_t)2 * rows * T);
-        cb.psi = reinterpret_cast<float*>(q); q += al(2 * rows);
-        cb.tab = reinterpret_cast<float*>(q); q += al((size_t)2 * rows * (T + 4));
-        cb.tabM = reinterpret_cast<float*>(q); q += al(2 * rows);
-        cb.add = use_lm ? b.lm_extra : reinterpret_cast<float*>(q);
+        float *x = nullptr, *xlin = nullptr, *xb = nullptr, *rsum = nullptr, *rb = nullptr, *psi = nullptr, *tab = nullptr,
+              *tabM = nullptr, *add = b.lm_extra;  // with an LM the CTC scores are added to the LM's
+        auto layout = [&](Carver& take) {
+            take(x, (size_t)M * V * 4); take(xlin, (size_t)M * V * 4); take(xb, (size_t)M * 4);
+            take(rsum, (size_t)2 * rows * T * 4); take(rb, (size_t)2 * rows * T * 4); take(psi, (size_t)2 * rows * 4);
+            take(tab, (size_t)2 * rows * (T + 4) * 4); take(tabM, (size_t)2 * rows * 4);
+            if (!use_lm) take(add, (size_t)rows * V * 4);
+        };
+        Carver measure;
+        layout(measure);
+        RC(grow_buffer(m, m->ctc, measure.used, "beam: CTC scorer"));
+        Carver carve{static_cast<uint8_t*>(m->ctc.base)};
+        layout(carve);
         GemmEpilogue e;
-        e.mode = EPI_F32; e.bias = m->b_ctc; e.out = cb.x; e.ldo = c.vocab;
-        RC(gemm_f16(b.enc16, d, m->w_ctc, d, e, M, c.vocab, d, st));
-        RC(ctc_prefix_reset(cb.x, cb.xlin, cb.xb, b.enc_len, B, T, c.vocab, p.blank_index, beam, cb.rsum, cb.rb, cb.psi, cb.tab, cb.tabM, st));
-        cs.x = cb.x; cs.xlin = cb.xlin; cs.xb = cb.xb; cs.enc_len = b.enc_len; cs.hist_tok = hist_tok; cs.hist_pred = hist_pred; cs.n_bh = rows;
-        cs.rsum_base = cb.rsum; cs.rb_base = cb.rb; cs.psi_base = cb.psi; cs.step_ptr = b.step; cs.tab = cb.tab; cs.tabM = cb.tabM;
+        e.mode = EPI_F32; e.bias = m->wt->b_ctc; e.out = x; e.ldo = c.vocab;
+        RC(gemm_f16(b.enc16, d, m->wt->w_ctc, d, e, M, c.vocab, d, st));
+        RC(ctc_prefix_reset(x, xlin, xb, b.enc_len, B, T, c.vocab, p.blank_index, beam, rsum, rb, psi, tab, tabM, st));
+        cs.x = x; cs.xlin = xlin; cs.xb = xb; cs.enc_len = b.enc_len; cs.hist_tok = hist_tok; cs.hist_pred = hist_pred; cs.n_bh = rows;
+        cs.rsum_base = rsum; cs.rb_base = rb; cs.psi_base = psi; cs.step_ptr = b.step; cs.tab = tab; cs.tabM = tabM;
         cs.bos = p.bos; cs.T = T; cs.V = c.vocab; cs.beam = beam; cs.blank = p.blank_index; cs.eos = p.eos;
-        cs.weight = p.ctc_weight; cs.out = cb.add; cs.accumulate = use_lm ? 1 : 0;
+        cs.weight = p.ctc_weight; cs.out = add; cs.accumulate = use_lm ? 1 : 0;
     }
     const bool use_cov = p.coverage_weight != 0.0f;
     CoverageStep cv{};
     if (use_cov) {  // CoverageScorer (scorer.py:788-955) on the last decoder layer's head-averaged cross-attention
         SBK_REQUIRE(d / c.nhead == 64, "beam: the coverage scorer is built for head_dim 64");
-        const size_t need = ((size_t)2 * rows * T + rows) * 4 + 256;
-        if (need > m->cov.cap) {
-            if (m->cov.base) { SBK_CUDA_CHECK(cudaStreamSynchronize(st)); cudaFree(m->cov.base); m->cov.base = nullptr; m->cov.cap = 0; }
-            if (m->beam_graph) { cudaGraphExecDestroy(m->beam_graph); m->beam_graph = nullptr; }
-            if (cudaMalloc(&m->cov.base, need) != cudaSuccess) { set_error("beam: coverage scorer cudaMalloc(%zu) failed", need); return SBK_ERR_NOMEM; }
-            m->cov.cap = need;
-        }
+        RC(grow_buffer(m, m->cov, ((size_t)2 * rows * T + rows) * 4 + 256, "beam: coverage scorer"));
+        float* cov = static_cast<float*>(m->cov.base);
         cv.q = b.dq16; cv.ldq = d; cv.kbase = b.ckv16 + (size_t)(Ld - 1) * M * 2 * d;
         if (xatt_headmajor(m)) { cv.utt_stride = (size_t)T * d; cv.key_stride = 64; cv.head_stride = T * 64; }
         else { cv.utt_stride = (size_t)T * 2 * d; cv.key_stride = 2 * d; cv.head_stride = 64; }
         cv.enc_len = b.enc_len; cv.rows_per_utt = beam; cv.T = T; cv.H = c.nhead;
-        cv.cov_base = m->cov.base; cv.hist_pred = hist_pred; cv.step_ptr = b.step; cv.n_bh = rows;
-        cv.threshold = p.coverage_threshold; cv.weight = p.coverage_weight; cv.out = m->cov.base + (size_t)2 * rows * T;
+        cv.cov_base = cov; cv.hist_pred = hist_pred; cv.step_ptr = b.step; cv.n_bh = rows;
+        cv.threshold = p.coverage_threshold; cv.weight = p.coverage_weight; cv.out = cov + (size_t)2 * rows * T;
     }
     BeamLm lm;
-    if (use_lm) { lm.emb = m->lm_emb; lm.pe = m->lm_pe; lm.d = c.lm_d_model; lm.x = b.lx; lm.x16 = b.lx16; lm.tok_cache = b.tok_cache; }
-    RC(beam_reset(rows, beam, S_max, p.bos, b.step, b.seq_scores, b.lineage, b.finished, b.ended_count, m->emb, m->dec_pe, d,
+    if (use_lm) { lm.emb = m->wt->lm_emb; lm.pe = m->wt->lm_pe; lm.d = c.lm_d_model; lm.x = b.lx; lm.x16 = b.lx16; lm.tok_cache = b.tok_cache; }
+    RC(beam_reset(rows, beam, S_max, p.bos, b.step, b.seq_scores, b.lineage, b.finished, b.ended_count, m->wt->emb, m->wt->dec_pe, d,
                   b.dx, use_lm ? &lm : nullptr, st));
     BeamStepArgs a{};
-    a.add_scores = use_lm ? b.lm_extra : (use_ctc ? m->ctc.add : nullptr);
+    a.add_scores = use_lm ? b.lm_extra : (use_ctc ? cs.out : nullptr);
     a.lm = lm;
     if (use_ctc) { a.attn_weight = 1.0f - p.ctc_weight; a.blank = p.blank_index; }
     a.add_const = p.length_weight;
@@ -1200,7 +1230,7 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
     a.hist_tok = hist_tok; a.hist_pred = hist_pred; a.hist_score = hist_score; a.hist_lp = hist_lp;
     a.temperature = p.temperature; a.eos_threshold = p.eos_threshold; a.minus_inf = p.minus_inf; a.min_steps = p.min_steps;
     a.eos = p.eos; a.use_eos_threshold = p.using_eos_threshold; a.length_norm = p.length_normalization;
-    a.emb = m->emb; a.pe = m->dec_pe; a.d = d; a.x_next = b.dx; a.scratch = b.beam_scr;
+    a.emb = m->wt->emb; a.pe = m->wt->dec_pe; a.d = d; a.x_next = b.dx; a.scratch = b.beam_scr;
     // One whole search step; every kernel takes the step index from the device counters, so the sequence is the same
     // for every step and can be replayed from a graph.  The scorers that do not read the decoder's output of this step --
     // the TransformerLM step and the CTC state update of the PREVIOUS step's survivors -- run as a second branch beside
@@ -1232,32 +1262,17 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
     };
     const bool use_graph = getenv("SBK_NO_GRAPH") == nullptr;
     if (use_graph) {
-        AsrModel::BeamKey key;
+        struct BeamKey { sbk_beam_params p; int B, T, rows, S_max, fuse_ln, tc_rows, fork; } key;
         memset(&key, 0, sizeof(key));
         key.p = p; key.B = B; key.T = T; key.rows = rows; key.S_max = S_max; key.fuse_ln = m->fuse_dec_ln; key.tc_rows = m->dec_tc_rows; key.fork = fork ? 1 : 0;
-        if (m->beam_graph == nullptr || memcmp(&key, &m->beam_key, sizeof(key)) != 0) {
-            if (m->beam_graph) { cudaGraphExecDestroy(m->beam_graph); m->beam_graph = nullptr; }
-            if (!m->cap_stream) SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-            cudaGraph_t g;
-            SBK_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-            launch_count_begin_capture();
-            int rc = enqueue_step(m->cap_stream);
-            m->beam_nodes = launch_count_end_capture();
-            cudaError_t ce = cudaStreamEndCapture(m->cap_stream, &g);
-            if (rc) return rc;
-            SBK_CUDA_CHECK(ce);
-            SBK_CUDA_CHECK(cudaGraphInstantiate(&m->beam_graph, g, 0));
-            cudaGraphDestroy(g);
-            m->beam_key = key;
-        }
+        RC(m->beam_graph.ensure(key, m->cap_stream, enqueue_step));
     }
     const int check_every = m->poll_every > 0 ? m->poll_every : p.max_steps;
     int s = 0;
     while (s < p.max_steps) {
         const int chunk = std::min(check_every, p.max_steps - s);
         for (int i = 0; i < chunk; ++i) {
-            if (use_graph) { SBK_CUDA_CHECK(cudaGraphLaunch(m->beam_graph, st)); launch_count_add(m->beam_nodes); }
-            else RC(enqueue_step(st));
+            RC(use_graph ? m->beam_graph.launch(st) : enqueue_step(st));
         }
         s += chunk;
         if (s < p.max_steps && m->poll_every > 0) {  // `_check_full_beams` (:806-822), polled once per chunk
@@ -1278,15 +1293,15 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
 // Greedy search over encoder states already in the workspace (b.enc_out / b.enc_len).
 static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos, float* log_probs, int* steps_done,
                       cudaStream_t st, bool in_capture = false) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, M = B * T, rows = B, S_max = m->ws_steps + 1;
-    SBK_REQUIRE(m->has_dec, "greedy: this handle was created without decoder weights");
+    SBK_REQUIRE(m->wt->has_dec, "greedy: this handle was created without decoder weights");
     SBK_REQUIRE(max_steps <= m->ws_steps && max_steps + 1 <= c.max_len, "greedy: max_steps=%d too large", max_steps);
     *steps_done = 0;
     if (max_steps <= 0) return SBK_OK;
     RC(project_cross_kv(m, M, T, st));  // cross-attention K/V of all layers, once per utterance
-    RC(greedy_reset(b.tokens, S_max + 1, rows, bos, b.step, b.has_ended, b.ended_count, m->emb, m->dec_pe, d, b.dx, st));
+    RC(greedy_reset(b.tokens, S_max + 1, rows, bos, b.step, b.has_ended, b.ended_count, m->wt->emb, m->wt->dec_pe, d, b.dx, st));
     set_decode_pdl(m, rows);
     const bool use_graph = !in_capture && getenv("SBK_NO_GRAPH") == nullptr && log_probs == nullptr;
     if (in_capture) {  // the caller is capturing the whole pipeline: enqueue exactly max_steps steps, no polling
@@ -1294,29 +1309,18 @@ static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos
         *steps_done = max_steps;
         return SBK_OK;
     }
-    if (use_graph && (m->step_graph == nullptr || m->graph_rows != rows || m->graph_T != T || m->graph_B != B ||
-                      m->graph_eos != eos || m->graph_S != S_max)) {
-        if (m->step_graph) { cudaGraphExecDestroy(m->step_graph); m->step_graph = nullptr; }
-        cudaGraph_t g;
-        if (!m->cap_stream) SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        SBK_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        launch_count_begin_capture();
-        int rc = enqueue_decode_step(m, rows, 1, T, S_max, eos, nullptr, 0, m->cap_stream);
-        m->graph_nodes = launch_count_end_capture();
-        cudaError_t ce = cudaStreamEndCapture(m->cap_stream, &g);
-        if (rc) return rc;
-        SBK_CUDA_CHECK(ce);
-        SBK_CUDA_CHECK(cudaGraphInstantiate(&m->step_graph, g, 0));
-        cudaGraphDestroy(g);
-        m->graph_rows = rows; m->graph_T = T; m->graph_B = B; m->graph_eos = eos; m->graph_S = S_max;
+    if (use_graph) {
+        const struct StepKey { int rows, T, B, eos, S_max; } key = {rows, T, B, eos, S_max};
+        RC(m->step_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
+            return enqueue_decode_step(m, rows, 1, T, S_max, eos, nullptr, 0, cs);
+        }));
     }
     const int check_every = m->poll_every > 0 ? m->poll_every : max_steps;
     int s = 0;
     while (s < max_steps) {
         const int chunk = std::min(check_every, max_steps - s);
         for (int i = 0; i < chunk; ++i) {
-            if (use_graph) { SBK_CUDA_CHECK(cudaGraphLaunch(m->step_graph, st)); launch_count_add(m->graph_nodes); }
-            else RC(enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, st));
+            RC(use_graph ? m->step_graph.launch(st) : enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, st));
         }
         s += chunk;
         if (s < max_steps && m->poll_every > 0) {  // seq2seq.py:256 `has_ended.all()` early exit, polled once per chunk
@@ -1378,17 +1382,17 @@ __global__ void dec_teacher_embed_kernel(const int* __restrict__ tokens, int S, 
 }
 
 static int run_decode_teacher(AsrModel* m, const int* tokens, int n, int S, int T, float* out, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, M = n * T, S_max = m->ws_steps + 1;
-    SBK_REQUIRE(m->has_dec, "decode: this handle was created without decoder weights");
+    SBK_REQUIRE(m->wt->has_dec, "decode: this handle was created without decoder weights");
     SBK_REQUIRE(S <= m->ws_steps && S <= c.max_len, "decode: %d target positions exceed the workspace / max_len", S);
     RC(project_cross_kv(m, M, T, st));
     for (int s = 0; s < S; ++s) {
-        dec_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, S, s, m->emb, m->dec_pe, d, sqrtf((float)d), b.dx, b.step);
+        dec_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, S, s, m->wt->emb, m->wt->dec_pe, d, sqrtf((float)d), b.dx, b.step);
         SBK_LAUNCH_CHECK();
         RC(enqueue_decode_layers(m, n, 1, T, S_max, nullptr, st, false));
-        RC(layernorm_rows(b.dx, b.lnout, false, m->dec_norm_g, m->dec_norm_b, n, d, 1e-6f, false, st));
+        RC(layernorm_rows(b.dx, b.lnout, false, m->wt->dec_norm_g, m->wt->dec_norm_b, n, d, 1e-6f, false, st));
         SBK_CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s * d, (size_t)S * d * 4, b.lnout, (size_t)d * 4, (size_t)d * 4, n,
                                          cudaMemcpyDeviceToDevice, st));
     }
@@ -1397,13 +1401,13 @@ static int run_decode_teacher(AsrModel* m, const int* tokens, int n, int S, int 
 
 static int run_lm_rescore(AsrModel* m, const int* tokens, const int* lens, int n, int L, float temperature, int pad,
                           float* scores, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int S_max = m->ws_steps + 1, dl = c.lm_d_model;
     lm_teacher_reset_kernel<<<n, 128, 0, st>>>(tokens, n, L, S_max, pad, b.lineage, b.tok_cache, scores);
     SBK_LAUNCH_CHECK();
     for (int s = 0; s + 1 < L; ++s) {
-        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->lm_emb, m->lm_pe, dl, sqrtf((float)dl), b.lx, b.lx16, b.step);
+        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->wt->lm_emb, m->wt->lm_pe, dl, sqrtf((float)dl), b.lx, b.lx16, b.step);
         SBK_LAUNCH_CHECK();
         RC(enqueue_lm_step(m, n, S_max, temperature, 1.0f, st));
         lm_teacher_score_kernel<<<ceil_div(n, 128), 128, 0, st>>>(b.lm_extra, c.vocab, tokens, L, s, lens, pad, scores, n);
@@ -1415,13 +1419,13 @@ static int run_lm_rescore(AsrModel* m, const int* tokens, const int* lens, int n
 // The same teacher-forced step path, keeping each position's raw logits: out[:, s, :] = lm_logits after feeding
 // tokens[:, s].  Keys are masked through tok_cache exactly as in the rescorer and the beam search's LM scorer.
 static int run_lm_step_logits(AsrModel* m, const int* tokens, int n, int L, float* out, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int S_max = m->ws_steps + 1, dl = c.lm_d_model, V = c.vocab;
     lm_teacher_reset_kernel<<<n, 128, 0, st>>>(tokens, n, L, S_max, 0, b.lineage, b.tok_cache, b.score);
     SBK_LAUNCH_CHECK();
     for (int s = 0; s < L; ++s) {
-        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->lm_emb, m->lm_pe, dl, sqrtf((float)dl), b.lx, b.lx16, b.step);
+        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->wt->lm_emb, m->wt->lm_pe, dl, sqrtf((float)dl), b.lx, b.lx16, b.step);
         SBK_LAUNCH_CHECK();
         RC(enqueue_lm_step(m, n, S_max, 1.0f, 1.0f, st));
         SBK_CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s * V, (size_t)L * V * 4, b.lm_logits, (size_t)V * 4, (size_t)V * 4, n,
@@ -1449,36 +1453,32 @@ __global__ void lm_embed_kernel(const int* __restrict__ tokens, int s, int vocab
     }
 }
 
-static int ensure_lm_workspace(AsrModel* m, int rows, cudaStream_t st) {
+static int ensure_lm_workspace(AsrModel* m, int rows) {
     AsrModel::LmFwdBuf& w = m->lmf;
-    if (w.base && rows <= w.rows) return SBK_OK;
-    const size_t R = rows, dl = m->cfg.lm_d_model, Fl = m->cfg.lm_d_ffn;
-    auto al = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
-    const size_t need = al(R * dl * 4) + al(R * dl * 2) + al(R * 3 * dl * 2) + al(R * dl * 2) + al(R * Fl * 2);
-    if (need > w.cap) {
-        if (w.base) { SBK_CUDA_CHECK(cudaStreamSynchronize(st)); cudaFree(w.base); w.base = nullptr; w.cap = 0; w.rows = 0; }
-        if (cudaMalloc(&w.base, need) != cudaSuccess) { set_error("lm_forward: workspace cudaMalloc(%zu) failed", need); return SBK_ERR_NOMEM; }
-        w.cap = need;
-    }
-    uint8_t* q = w.base;
-    w.x = reinterpret_cast<float*>(q); q += al(R * dl * 4);
-    w.x16 = reinterpret_cast<__half*>(q); q += al(R * dl * 2);
-    w.qkv16 = reinterpret_cast<__half*>(q); q += al(R * 3 * dl * 2);
-    w.att16 = reinterpret_cast<__half*>(q); q += al(R * dl * 2);
-    w.f16 = reinterpret_cast<__half*>(q);
+    if (m->lmf_mem.base && rows <= w.rows) return SBK_OK;
+    const size_t R = rows, dl = m->wt->cfg.lm_d_model, Fl = m->wt->cfg.lm_d_ffn;
+    auto layout = [&](Carver& take) {
+        take(w.x, R * dl * 4); take(w.x16, R * dl * 2); take(w.qkv16, R * 3 * dl * 2); take(w.att16, R * dl * 2);
+        take(w.f16, R * Fl * 2);
+    };
+    Carver measure;
+    layout(measure);
+    RC(grow_buffer(m, m->lmf_mem, measure.used, "lm_forward: workspace"));
+    Carver carve{static_cast<uint8_t*>(m->lmf_mem.base)};
+    layout(carve);
     w.rows = rows;
     return SBK_OK;
 }
 
 static int run_lm_forward(AsrModel* m, const int* tokens, int n, int s, float* logits, cudaStream_t st) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead, M = n * s;
-    RC(ensure_lm_workspace(m, M, st));
+    RC(ensure_lm_workspace(m, M));
     const AsrModel::LmFwdBuf& b = m->lmf;
-    lm_embed_kernel<<<M, 128, 0, st>>>(tokens, s, c.vocab, m->lm_emb, m->lm_pe, dl, sqrtf((float)dl), b.x, b.x16);
+    lm_embed_kernel<<<M, 128, 0, st>>>(tokens, s, c.vocab, m->wt->lm_emb, m->wt->lm_pe, dl, sqrtf((float)dl), b.x, b.x16);
     SBK_LAUNCH_CHECK();
     for (int l = 0; l < c.lm_layers; ++l) {  // post-norm TransformerEncoderLayer (Transformer.py:466-481)
-        const LmLayerW& w = m->lm[l];
+        const LmLayerW& w = m->wt->lm[l];
         GemmEpilogue e;
         e.mode = EPI_F16; e.bias = w.b_in; e.out = b.qkv16; e.ldo = 3 * dl;
         RC(gemm_f16(b.x16, dl, w.w_in, dl, e, M, 3 * dl, dl, st));
@@ -1493,14 +1493,14 @@ static int run_lm_forward(AsrModel* m, const int* tokens, int n, int s, float* l
         RC(gemm_f16(b.f16, Fl, w.w2, Fl, e, M, dl, Fl, st));
         RC(layernorm_dual(b.x, b.x16, w.n2g, w.n2b, M, dl, 1e-6f, true, st));
     }
-    RC(layernorm_dual(b.x, b.x16, m->lm_norm_g, m->lm_norm_b, M, dl, 1e-6f, false, st));  // encoder.norm
+    RC(layernorm_dual(b.x, b.x16, m->wt->lm_norm_g, m->wt->lm_norm_b, M, dl, 1e-6f, false, st));  // encoder.norm
     // output_proj: Linear d -> d (fp32, into the free residual buffer), LayerNorm, Linear d -> vocab into the caller's logits
     GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->lm_bp0; e.out = b.x; e.ldo = dl;
-    RC(gemm_f16(b.x16, dl, m->lm_wp0, dl, e, M, dl, dl, st));
-    RC(layernorm_dual(b.x, b.x16, m->lm_lnp_g, m->lm_lnp_b, M, dl, 1e-6f, false, st));
-    e = GemmEpilogue(); e.mode = EPI_F32; e.bias = m->lm_bp2; e.out = logits; e.ldo = c.vocab;
-    RC(gemm_f16(b.x16, dl, m->lm_wp2, dl, e, M, c.vocab, dl, st));
+    e.mode = EPI_F32; e.bias = m->wt->lm_bp0; e.out = b.x; e.ldo = dl;
+    RC(gemm_f16(b.x16, dl, m->wt->lm_wp0, dl, e, M, dl, dl, st));
+    RC(layernorm_dual(b.x, b.x16, m->wt->lm_lnp_g, m->wt->lm_lnp_b, M, dl, 1e-6f, false, st));
+    e = GemmEpilogue(); e.mode = EPI_F32; e.bias = m->wt->lm_bp2; e.out = logits; e.ldo = c.vocab;
+    RC(gemm_f16(b.x16, dl, m->wt->lm_wp2, dl, e, M, c.vocab, dl, st));
     return SBK_OK;
 }
 
@@ -1699,12 +1699,18 @@ int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int 
     std::vector<float> pe((size_t)HM_PE_ROWS * d);
     hypermix_pe_table(d, pe.data());
     const size_t part_n = hypermix_part_floats(B, T, d, k);
+    __half *w16 = nullptr, *G = nullptr;
+    float *pe_dev = nullptr, *part = nullptr, *gscale = nullptr;
+    auto layout = [&](Carver& take) {
+        take(w16, 2 * (n1 + n2) * 2); take(pe_dev, pe.size() * 4); take(part, part_n * 4); take(G, (size_t)B * d * k * 2);
+        take(gscale, (size_t)B * nhead * 4);
+    };
+    Carver measure;
+    layout(measure);
     uint8_t* base = nullptr;
-    const size_t off_w = 0, off_pe = off_w + ((2 * (n1 + n2) * 2 + 255) & ~size_t(255)), off_part = off_pe + pe.size() * 4,
-                 off_g = off_part + part_n * 4, off_s = off_g + (((size_t)B * d * k * 2 + 255) & ~size_t(255)),
-                 total = off_s + (size_t)B * nhead * 4;
-    if (cudaMalloc(&base, total) != cudaSuccess) { set_error("hypermix_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
-    __half* w16 = reinterpret_cast<__half*>(base + off_w);
+    if (cudaMalloc(&base, measure.used) != cudaSuccess) { set_error("hypermix_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
+    Carver carve{base};
+    layout(carve);
     HyperMixWeights w;
     w.fc1w[0] = w16; w.fc2w[0] = w16 + n1; w.fc1w[1] = w16 + n1 + n2; w.fc2w[1] = w16 + 2 * n1 + n2;
     w.fc1b[0] = w1_fc1_b_dev; w.fc2b[0] = w1_fc2_b_dev; w.fc1b[1] = w2_fc1_b_dev; w.fc2b[1] = w2_fc2_b_dev;
@@ -1713,15 +1719,14 @@ int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int 
     if (rc == SBK_OK) rc = cast_f32_f16(w1_fc2_w_dev, const_cast<__half*>(w.fc2w[0]), n2, st);
     if (rc == SBK_OK) rc = cast_f32_f16(w2_fc1_w_dev, const_cast<__half*>(w.fc1w[1]), n1, st);
     if (rc == SBK_OK) rc = cast_f32_f16(w2_fc2_w_dev, const_cast<__half*>(w.fc2w[1]), n2, st);
-    if (rc == SBK_OK && (cudaMemcpyAsync(base + off_pe, pe.data(), pe.size() * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+    if (rc == SBK_OK && (cudaMemcpyAsync(pe_dev, pe.data(), pe.size() * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
                          cudaMemsetAsync(out_dev, 0, (size_t)B * T * d * 4, st) != cudaSuccess)) {
         set_error("hypermix_test: copy failed");
         rc = SBK_ERR_CUDA;
     }
     if (rc == SBK_OK)
         rc = hypermix_forward(static_cast<const __half*>(x_dev), B, T, d, nhead, k, lens_dev,
-                              reinterpret_cast<const float*>(base + off_pe), w, reinterpret_cast<float*>(base + off_part),
-                              reinterpret_cast<__half*>(base + off_g), reinterpret_cast<float*>(base + off_s), out_dev, st);
+                              pe_dev, w, part, G, gscale, out_dev, st);
     if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("hypermix_test: device error"); rc = SBK_ERR_CUDA; }
     cudaFree(base);
     return rc;
@@ -1730,7 +1735,7 @@ int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int 
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out) {
     return asr_create(cfg, weights, n_weights, reinterpret_cast<AsrModel**>(out));
 }
-void sbk_asr_destroy(sbk_asr* m) { asr_destroy(reinterpret_cast<AsrModel*>(m)); }
+void sbk_asr_destroy(sbk_asr* m) { delete reinterpret_cast<AsrModel*>(m); }
 int sbk_asr_clone(sbk_asr* src, sbk_asr** out) {
     return asr_clone(reinterpret_cast<AsrModel*>(src), reinterpret_cast<AsrModel**>(out));
 }
@@ -1763,7 +1768,7 @@ int sbk_asr_set_poll_interval(sbk_asr* m, int every_n_steps) {
 int sbk_asr_num_frames(const sbk_asr* mm, int n_samples, int* T_feat, int* T_enc) {
     const AsrModel* m = reinterpret_cast<const AsrModel*>(mm);
     int T0, T1, T2;
-    frames(m->cfg, n_samples, &T0, &T1, &T2);
+    frames(m->wt->cfg, n_samples, &T0, &T1, &T2);
     if (T_feat) *T_feat = T0;
     if (T_enc) *T_enc = T2;
     return SBK_OK;
@@ -1771,12 +1776,12 @@ int sbk_asr_num_frames(const sbk_asr* mm, int n_samples, int* T_feat, int* T_enc
 
 int sbk_asr_cnn_forward(sbk_asr* mm, const float* feats_dev, int B, int T0, float* out_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
-    const sbk_asr_config& c = m->cfg;
-    SBK_REQUIRE(m->has_cnn, "cnn_forward: this handle was created without CNN weights");
+    const sbk_asr_config& c = m->wt->cfg;
+    SBK_REQUIRE(m->wt->has_cnn, "cnn_forward: this handle was created without CNN weights");
     const int L = (T0 - 1) * c.hop;
     RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
-    return cnn_frontend_forward(feats_dev, B, T0, c.n_mels, m->c1_w, m->c1_b, m->c1_g, m->c1_be, c.cnn_c1, m->c2_w, m->c2_b,
-                                m->c2_g, m->c2_be, c.cnn_c2, m->b.act1, m->b.a_in, out_dev,
+    return cnn_frontend_forward(feats_dev, B, T0, c.n_mels, m->wt->c1_w, m->wt->c1_b, m->wt->c1_g, m->wt->c1_be, c.cnn_c1, m->wt->c2_w, m->wt->c2_b,
+                                m->wt->c2_g, m->wt->c2_be, c.cnn_c2, m->b.act1, m->b.a_in, out_dev,
                                 static_cast<cudaStream_t>(stream));
 }
 
@@ -1785,14 +1790,13 @@ int sbk_asr_encode_feats(sbk_asr* mm, const float* feats_dev, const float* rel_l
                          float* cnn_out_dev, float* enc_out_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     const int L = (T0 - 1) * c.hop;
     RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
     const int T1 = (T0 - 1) / 2 + 1, T = (T1 - 1) / 2 + 1;
     const int* enc_len = nullptr;
     if (rel_len_dev) {
-        abs_len_kernel<<<ceil_div(B, 128), 128, 0, st>>>(rel_len_dev, B, T, m->b.enc_len);
-        SBK_LAUNCH_CHECK();
+        RC(set_enc_len(m->b.enc_len, rel_len_dev, B, T, st));
         enc_len = m->b.enc_len;
     }
     return run_encoder(m, feats_dev, B, T0, enc_len, cnn_out_dev, enc_out_dev ? enc_out_dev : m->b.enc_out, st);
@@ -1802,14 +1806,13 @@ int sbk_asr_encode_from_cnn(sbk_asr* mm, const float* src_dev, const float* rel_
                             float* enc_out_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     const int L = ((T - 1) * 4) * c.hop;  // any L whose frame count maps to >= T encoder frames
     RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
     RC(cast_f32_f16(src_dev, m->b.a_in, (size_t)B * T * c.input_size, st));
     const int* enc_len = nullptr;
     if (rel_len_dev) {
-        abs_len_kernel<<<ceil_div(B, 128), 128, 0, st>>>(rel_len_dev, B, T, m->b.enc_len);
-        SBK_LAUNCH_CHECK();
+        RC(set_enc_len(m->b.enc_len, rel_len_dev, B, T, st));
         enc_len = m->b.enc_len;
     }
     return run_encoder(m, nullptr, B, T, enc_len, nullptr, enc_out_dev ? enc_out_dev : m->b.enc_out, st);
@@ -1820,35 +1823,20 @@ int sbk_asr_encode_from_cnn(sbk_asr* mm, const float* src_dev, const float* rel_
 static int transcribe_enqueue(AsrModel* m, const float* wav_dev, const float* rel_len_dev, int B, int L, int max_steps,
                               int bos, int eos, float* enc_out_dev, int* pred_dev, float* score_dev, float* log_probs_dev,
                               int* steps_done, cudaStream_t st, bool in_capture) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     int T0, T1, T;
     frames(c, L, &T0, &T1, &T);
     AsrModel::Buf& b = m->b;
-    RC(fbank_forward(m->fbank, wav_dev, B, L, b.feats, b.utt_max, m->glob_mean, m->glob_std, c.norm_eps > 0.0f ? c.norm_eps : 1e-10f, st));
-    const int* enc_len = nullptr;
-    if (rel_len_dev) {
-        abs_len_kernel<<<ceil_div(B, 128), 128, 0, st>>>(rel_len_dev, B, T, b.enc_len);
-        SBK_LAUNCH_CHECK();
-        enc_len = b.enc_len;
-    } else {
-        std::vector<int> full(B, T);
-        SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_len, full.data(), B * 4, cudaMemcpyHostToDevice, st));
-        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-        enc_len = b.enc_len;
-    }
-    RC(run_encoder(m, b.feats, B, T0, enc_len, nullptr, b.enc_out, st));
+    RC(fbank_forward(m->wt->fbank, wav_dev, B, L, b.feats, b.utt_max, m->wt->glob_mean, m->wt->glob_std, c.norm_eps > 0.0f ? c.norm_eps : 1e-10f, st));
+    RC(set_enc_len(b.enc_len, rel_len_dev, B, T, st));
+    RC(run_encoder(m, b.feats, B, T0, b.enc_len, nullptr, b.enc_out, st));
     if (enc_out_dev)
         SBK_CUDA_CHECK(cudaMemcpyAsync(enc_out_dev, b.enc_out, (size_t)B * T * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
     int done = 0;
-    if (max_steps > 0 && m->has_dec) {
+    if (max_steps > 0 && m->wt->has_dec) {
         RC(run_greedy(m, B, T, max_steps, bos, eos, log_probs_dev, &done, st, in_capture));
-        const int S_max = m->ws_steps + 1;
-        if (pred_dev)
-            SBK_CUDA_CHECK(cudaMemcpy2DAsync(pred_dev, (size_t)max_steps * 4, b.pred, (size_t)S_max * 4, (size_t)done * 4, B,
-                                             cudaMemcpyDeviceToDevice, st));
-        if (score_dev)
-            SBK_CUDA_CHECK(cudaMemcpy2DAsync(score_dev, (size_t)max_steps * 4, b.score, (size_t)S_max * 4, (size_t)done * 4, B,
-                                             cudaMemcpyDeviceToDevice, st));
+        RC(copy_steps(m, pred_dev, max_steps, b.pred, done, B, cudaMemcpyDeviceToDevice, st));
+        RC(copy_steps(m, score_dev, max_steps, b.score, done, B, cudaMemcpyDeviceToDevice, st));
     }
     if (steps_done) *steps_done = done;
     return SBK_OK;
@@ -1861,16 +1849,15 @@ static int transcribe_enqueue(AsrModel* m, const float* wav_dev, const float* re
 static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_dev, const float* const* rel_dev, int B, int L,
                                     int max_steps, int bos, int eos, int* const* pred_dev, int* steps_done, cudaStream_t st,
                                     bool in_capture, const cudaEvent_t* ready = nullptr, int* const* pred_host = nullptr) {
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     int T0, T1, T;
     frames(c, L, &T0, &T1, &T);
     AsrModel::Buf& b = m->b;
     for (int g = 0; g < G; ++g) {
         if (ready) SBK_CUDA_CHECK(cudaStreamWaitEvent(st, ready[g], 0));  // batch g's wav has landed in the staging buffer
-        RC(fbank_forward(m->fbank, wav_dev[g], B, L, b.feats, b.utt_max, m->glob_mean, m->glob_std, c.norm_eps > 0.0f ? c.norm_eps : 1e-10f, st));
+        RC(fbank_forward(m->wt->fbank, wav_dev[g], B, L, b.feats, b.utt_max, m->wt->glob_mean, m->wt->glob_std, c.norm_eps > 0.0f ? c.norm_eps : 1e-10f, st));
         int* enc_len = b.enc_len + (size_t)g * B;
-        abs_len_kernel<<<ceil_div(B, 128), 128, 0, st>>>(rel_dev[g], B, T, enc_len);
-        SBK_LAUNCH_CHECK();
+        RC(set_enc_len(enc_len, rel_dev[g], B, T, st));
         RC(run_encoder(m, b.feats, B, T0, enc_len, nullptr, b.enc_out + (size_t)g * B * T * c.d_model, st));
     }
     // The decode loop is a chain of ~3300 small, latency-bound kernels; the encoders of the other lanes are machine-filling
@@ -1893,14 +1880,10 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
     }
     int done = 0;
     RC(run_greedy(m, G * B, T, max_steps, bos, eos, nullptr, &done, ds, in_capture));
-    const int S_max = m->ws_steps + 1;
     for (int g = 0; g < G; ++g) {
-        if (pred_dev && pred_dev[g])
-            SBK_CUDA_CHECK(cudaMemcpy2DAsync(pred_dev[g], (size_t)max_steps * 4, b.pred + (size_t)g * B * S_max, (size_t)S_max * 4,
-                                             (size_t)done * 4, B, cudaMemcpyDeviceToDevice, ds));
-        if (pred_host && pred_host[g])
-            SBK_CUDA_CHECK(cudaMemcpy2DAsync(pred_host[g], (size_t)max_steps * 4, b.pred + (size_t)g * B * S_max, (size_t)S_max * 4,
-                                             (size_t)done * 4, B, cudaMemcpyDeviceToHost, ds));
+        const int* pred = b.pred + (size_t)g * B * (m->ws_steps + 1);
+        RC(copy_steps(m, pred_dev ? pred_dev[g] : nullptr, max_steps, pred, done, B, cudaMemcpyDeviceToDevice, ds));
+        RC(copy_steps(m, pred_host ? pred_host[g] : nullptr, max_steps, pred, done, B, cudaMemcpyDeviceToHost, ds));
     }
     if (prio) {
         SBK_CUDA_CHECK(cudaEventRecord(m->ev_djoin, ds));
@@ -1920,9 +1903,11 @@ static int transcribe_group_host_enqueue(AsrModel* m, int G, const float* const*
     SBK_CUDA_CHECK(cudaStreamWaitEvent(m->copy_stream, m->ev_fork, 0));  // the previous call no longer reads the staging buffers
     const float* wav_dev[16];
     const float* rel_dev[16];
+    float* gwav = static_cast<float*>(m->gwav.base);
+    float* grel = gwav + (size_t)G * B * L;  // lengths behind the G waveforms
     for (int g = 0; g < G; ++g) {
-        float* w = m->gwav + (size_t)g * B * L;
-        float* r = m->grel + (size_t)g * B;
+        float* w = gwav + (size_t)g * B * L;
+        float* r = grel + (size_t)g * B;
         SBK_CUDA_CHECK(cudaMemcpyAsync(w, wav_host[g], (size_t)B * L * 4, cudaMemcpyHostToDevice, m->copy_stream));
         SBK_CUDA_CHECK(cudaMemcpyAsync(r, rel_host[g], (size_t)B * 4, cudaMemcpyHostToDevice, m->copy_stream));
         SBK_CUDA_CHECK(cudaEventRecord(m->ev_ready[g], m->copy_stream));
@@ -1938,34 +1923,21 @@ int sbk_asr_transcribe_greedy_group_dev(sbk_asr* mm, int G, const float* const* 
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SBK_REQUIRE(G >= 1 && G <= 16, "transcribe_group: G=%d not in [1, 16]", G);
-    SBK_REQUIRE(m->has_fbank && m->has_cnn && m->has_enc && m->has_dec, "transcribe_group: handle lacks model parts");
-    SBK_REQUIRE(m->glob_mean != nullptr, "transcribe_group: model has no normalize.glob_mean/std weights");
+    SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc && m->wt->has_dec, "transcribe_group: handle lacks model parts");
+    SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe_group: model has no normalize.glob_mean/std weights");
     for (int g = 0; g < G; ++g) SBK_REQUIRE(wav_dev[g] && rel_len_dev[g], "transcribe_group: null batch pointer");
     RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps)));
     const bool whole_graph = m->poll_every == 0 && getenv("SBK_NO_GRAPH") == nullptr && max_steps > 0;
     if (!whole_graph) return transcribe_group_enqueue(m, G, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, pred_dev, steps_done, st, false);
-    AsrModel::GroupKey key;
+    struct GroupKey { const void *wav[16], *rel[16], *pred[16]; int G, B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));
     key.G = G; key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
     for (int g = 0; g < G; ++g) { key.wav[g] = wav_dev[g]; key.rel[g] = rel_len_dev[g]; key.pred[g] = pred_dev[g]; }
-    if (m->group_graph == nullptr || memcmp(&key, &m->group_key, sizeof(key)) != 0) {
-        if (m->group_graph) { cudaGraphExecDestroy(m->group_graph); m->group_graph = nullptr; }
-        if (!m->cap_stream) SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        cudaGraph_t gr;
-        SBK_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        launch_count_begin_capture();
+    RC(m->group_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
         int done = 0;
-        int rc = transcribe_group_enqueue(m, G, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, pred_dev, &done, m->cap_stream, true);
-        m->group_nodes = launch_count_end_capture();
-        cudaError_t ce = cudaStreamEndCapture(m->cap_stream, &gr);
-        if (rc) return rc;
-        SBK_CUDA_CHECK(ce);
-        SBK_CUDA_CHECK(cudaGraphInstantiate(&m->group_graph, gr, 0));
-        cudaGraphDestroy(gr);
-        m->group_key = key;
-    }
-    SBK_CUDA_CHECK(cudaGraphLaunch(m->group_graph, st));
-    launch_count_add(m->group_nodes);
+        return transcribe_group_enqueue(m, G, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, pred_dev, &done, cs, true);
+    }));
+    RC(m->group_graph.launch(st));
     if (steps_done) *steps_done = max_steps;
     return SBK_OK;
 }
@@ -1979,19 +1951,12 @@ int sbk_asr_transcribe_greedy_group_host_async(sbk_asr* mm, int G, const float* 
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SBK_REQUIRE(G >= 1 && G <= 16, "transcribe_group_host: G=%d not in [1, 16]", G);
-    SBK_REQUIRE(m->has_fbank && m->has_cnn && m->has_enc && m->has_dec, "transcribe_group_host: handle lacks model parts");
-    SBK_REQUIRE(m->glob_mean != nullptr, "transcribe_group_host: model has no normalize.glob_mean/std weights");
+    SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc && m->wt->has_dec, "transcribe_group_host: handle lacks model parts");
+    SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe_group_host: model has no normalize.glob_mean/std weights");
     SBK_REQUIRE(wav_host && rel_len_host && pred_host, "transcribe_group_host: null argument");
     for (int g = 0; g < G; ++g) SBK_REQUIRE(wav_host[g] && rel_len_host[g] && pred_host[g], "transcribe_group_host: null batch pointer");
     RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps)));
-    const size_t need = (size_t)G * B * L * 4 + (size_t)G * B * 4 + 256;
-    if (need > m->gwav_cap) {
-        if (m->gwav) { SBK_CUDA_CHECK(cudaDeviceSynchronize()); cudaFree(m->gwav); m->gwav = nullptr; m->gwav_cap = 0; }
-        if (m->hgroup_graph) { cudaGraphExecDestroy(m->hgroup_graph); m->hgroup_graph = nullptr; }
-        if (cudaMalloc(&m->gwav, need) != cudaSuccess) { set_error("transcribe_group_host: cudaMalloc(%zu) failed", need); return SBK_ERR_NOMEM; }
-        m->gwav_cap = need;
-    }
-    m->grel = m->gwav + (size_t)G * B * L;  // lengths behind the G waveforms
+    RC(grow_buffer(m, m->gwav, (size_t)G * B * L * 4 + (size_t)G * B * 4 + 256, "transcribe_group_host"));
     if (!m->copy_stream) {
         SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
         SBK_CUDA_CHECK(cudaEventCreateWithFlags(&m->ev_fork, cudaEventDisableTiming));
@@ -2001,32 +1966,19 @@ int sbk_asr_transcribe_greedy_group_host_async(sbk_asr* mm, int G, const float* 
     if (!whole_graph)
         return transcribe_group_host_enqueue(m, G, wav_host, rel_len_host, B, L, max_steps, bos, eos, pred_host, pred_dev,
                                              steps_done, st, false);
-    AsrModel::HostGroupKey key;
+    struct HostGroupKey { const void *wav[16], *rel[16], *pred[16], *pred_dev[16]; int G, B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));
     key.G = G; key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
     for (int g = 0; g < G; ++g) {
         key.wav[g] = wav_host[g]; key.rel[g] = rel_len_host[g]; key.pred[g] = pred_host[g];
         key.pred_dev[g] = pred_dev ? pred_dev[g] : nullptr;
     }
-    if (m->hgroup_graph == nullptr || memcmp(&key, &m->hgroup_key, sizeof(key)) != 0) {
-        if (m->hgroup_graph) { cudaGraphExecDestroy(m->hgroup_graph); m->hgroup_graph = nullptr; }
-        if (!m->cap_stream) SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        cudaGraph_t gr;
-        SBK_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        launch_count_begin_capture();
+    RC(m->hgroup_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
         int done = 0;
-        int rc = transcribe_group_host_enqueue(m, G, wav_host, rel_len_host, B, L, max_steps, bos, eos, pred_host, pred_dev, &done,
-                                               m->cap_stream, true);
-        m->hgroup_nodes = launch_count_end_capture();
-        cudaError_t ce = cudaStreamEndCapture(m->cap_stream, &gr);
-        if (rc) return rc;
-        SBK_CUDA_CHECK(ce);
-        SBK_CUDA_CHECK(cudaGraphInstantiate(&m->hgroup_graph, gr, 0));
-        cudaGraphDestroy(gr);
-        m->hgroup_key = key;
-    }
-    SBK_CUDA_CHECK(cudaGraphLaunch(m->hgroup_graph, st));
-    launch_count_add(m->hgroup_nodes);
+        return transcribe_group_host_enqueue(m, G, wav_host, rel_len_host, B, L, max_steps, bos, eos, pred_host, pred_dev, &done,
+                                             cs, true);
+    }));
+    RC(m->hgroup_graph.launch(st));
     if (steps_done) *steps_done = max_steps;
     return SBK_OK;
 }
@@ -2036,39 +1988,26 @@ int sbk_asr_transcribe_greedy_dev(sbk_asr* mm, const float* wav_dev, const float
                                   float* log_probs_dev, int* steps_done, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(m->has_fbank && m->has_cnn && m->has_enc, "transcribe: handle lacks fbank/CNN/encoder weights");
-    SBK_REQUIRE(m->glob_mean != nullptr, "transcribe: model has no normalize.glob_mean/std (global CMVN) weights");
+    SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc, "transcribe: handle lacks fbank/CNN/encoder weights");
+    SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe: model has no normalize.glob_mean/std (global CMVN) weights");
     RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(max_steps, m->ws_steps)));
     // Fixed-length runs (poll interval 0) replay ONE CUDA graph of the whole pipeline (Fbank .. last decode step):
     // ~2.6k kernel nodes, a single host-side launch per batch.
     const bool whole_graph = m->poll_every == 0 && rel_len_dev != nullptr && log_probs_dev == nullptr &&
-                             getenv("SBK_NO_GRAPH") == nullptr && (max_steps == 0 || m->has_dec);
+                             getenv("SBK_NO_GRAPH") == nullptr && (max_steps == 0 || m->wt->has_dec);
     if (!whole_graph)
         return transcribe_enqueue(m, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, enc_out_dev, pred_dev, score_dev,
                                   log_probs_dev, steps_done, st, false);
-    AsrModel::PipeKey key;
-    memset(&key, 0, sizeof(key));  // the struct has tail padding and is compared with memcmp
+    struct PipeKey { const void *wav, *rel, *enc, *pred, *score; int B, L, steps, bos, eos; } key;
+    memset(&key, 0, sizeof(key));  // the struct has tail padding and is compared bytewise
     key.wav = wav_dev; key.rel = rel_len_dev; key.enc = enc_out_dev; key.pred = pred_dev; key.score = score_dev;
     key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
-    if (m->pipe_graph == nullptr || memcmp(&key, &m->pipe_key, sizeof(key)) != 0) {
-        if (m->pipe_graph) { cudaGraphExecDestroy(m->pipe_graph); m->pipe_graph = nullptr; }
-        if (!m->cap_stream) SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->cap_stream, cudaStreamNonBlocking));
-        cudaGraph_t g;
-        SBK_CUDA_CHECK(cudaStreamBeginCapture(m->cap_stream, cudaStreamCaptureModeThreadLocal));
-        launch_count_begin_capture();
+    RC(m->pipe_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
         int done = 0;
-        int rc = transcribe_enqueue(m, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, enc_out_dev, pred_dev, score_dev,
-                                    nullptr, &done, m->cap_stream, true);
-        m->pipe_nodes = launch_count_end_capture();
-        cudaError_t ce = cudaStreamEndCapture(m->cap_stream, &g);
-        if (rc) return rc;
-        SBK_CUDA_CHECK(ce);
-        SBK_CUDA_CHECK(cudaGraphInstantiate(&m->pipe_graph, g, 0));
-        cudaGraphDestroy(g);
-        m->pipe_key = key;
-    }
-    SBK_CUDA_CHECK(cudaGraphLaunch(m->pipe_graph, st));
-    launch_count_add(m->pipe_nodes);
+        return transcribe_enqueue(m, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, enc_out_dev, pred_dev, score_dev, nullptr,
+                                  &done, cs, true);
+    }));
+    RC(m->pipe_graph.launch(st));
     if (steps_done) *steps_done = max_steps;
     return SBK_OK;
 }
@@ -2079,29 +2018,19 @@ int sbk_asr_greedy_from_enc(sbk_asr* mm, const float* enc_dev, const float* rel_
                             void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     // workspace sized from T: pick L such that frames(L) -> T
     const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
     RC(ensure_workspace(m, std::max(B, m->wsB), L, std::max(B, m->ws_rows), std::max(max_steps, m->ws_steps)));
     AsrModel::Buf& b = m->b;
     SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, (size_t)B * T * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
-    if (rel_len_dev) {
-        abs_len_kernel<<<ceil_div(B, 128), 128, 0, st>>>(rel_len_dev, B, T, b.enc_len);
-        SBK_LAUNCH_CHECK();
-    } else {
-        std::vector<int> full(B, T);
-        SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_len, full.data(), B * 4, cudaMemcpyHostToDevice, st));
-        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    }
+    RC(set_enc_len(b.enc_len, rel_len_dev, B, T, st));
     int done = 0;
     RC(run_greedy(m, B, T, max_steps, bos, eos, log_probs_dev, &done, st));
-    const int S_max = m->ws_steps + 1;
-    if (pred_dev && done > 0)
-        SBK_CUDA_CHECK(cudaMemcpy2DAsync(pred_dev, (size_t)max_steps * 4, b.pred, (size_t)S_max * 4, (size_t)done * 4, B,
-                                         cudaMemcpyDeviceToDevice, st));
-    if (score_dev && done > 0)
-        SBK_CUDA_CHECK(cudaMemcpy2DAsync(score_dev, (size_t)max_steps * 4, b.score, (size_t)S_max * 4, (size_t)done * 4, B,
-                                         cudaMemcpyDeviceToDevice, st));
+    if (done > 0) {
+        RC(copy_steps(m, pred_dev, max_steps, b.pred, done, B, cudaMemcpyDeviceToDevice, st));
+        RC(copy_steps(m, score_dev, max_steps, b.score, done, B, cudaMemcpyDeviceToDevice, st));
+    }
     if (steps_done) *steps_done = done;
     return SBK_OK;
 }
@@ -2112,21 +2041,14 @@ int sbk_asr_beam_from_enc(sbk_asr* mm, const float* enc_dev, const float* rel_le
                           float* hist_lp_dev, int* steps_done, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     SBK_REQUIRE(params && params->beam_size >= 1, "beam: bad params");
     const int rows = B * params->beam_size;
     const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
     RC(ensure_workspace(m, std::max(B, m->wsB), L, std::max(rows, m->ws_rows), std::max(params->max_steps, m->ws_steps)));
     AsrModel::Buf& b = m->b;
     SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, (size_t)B * T * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
-    if (rel_len_dev) {
-        abs_len_kernel<<<ceil_div(B, 128), 128, 0, st>>>(rel_len_dev, B, T, b.enc_len);
-        SBK_LAUNCH_CHECK();
-    } else {
-        std::vector<int> full(B, T);
-        SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_len, full.data(), B * 4, cudaMemcpyHostToDevice, st));
-        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    }
+    RC(set_enc_len(b.enc_len, rel_len_dev, B, T, st));
     int done = 0;
     RC(run_beam(m, B, T, *params, hist_tok_dev, hist_pred_dev, hist_score_dev, hist_lp_dev, &done, st));
     if (steps_done) *steps_done = done;
@@ -2151,14 +2073,9 @@ static int transcribe_greedy_host_impl(sbk_asr* mm, const float* wav_host, const
     int done = 0;
     RC(sbk_asr_transcribe_greedy_dev(mm, b.wav, rel_dev, B, L, max_steps, bos, eos, nullptr, nullptr, nullptr, nullptr, &done,
                                      stream));
-    const int S_max = m->ws_steps + 1;
     if (done > 0) {
-        if (pred_host)
-            SBK_CUDA_CHECK(cudaMemcpy2DAsync(pred_host, (size_t)max_steps * 4, b.pred, (size_t)S_max * 4, (size_t)done * 4, B,
-                                             cudaMemcpyDeviceToHost, st));
-        if (score_host)
-            SBK_CUDA_CHECK(cudaMemcpy2DAsync(score_host, (size_t)max_steps * 4, b.score, (size_t)S_max * 4, (size_t)done * 4, B,
-                                             cudaMemcpyDeviceToHost, st));
+        RC(copy_steps(m, pred_host, max_steps, b.pred, done, B, cudaMemcpyDeviceToHost, st));
+        RC(copy_steps(m, score_host, max_steps, b.score, done, B, cudaMemcpyDeviceToHost, st));
     }
     if (sync) SBK_CUDA_CHECK(cudaStreamSynchronize(st));
     if (steps_done) *steps_done = done;
@@ -2191,8 +2108,8 @@ int sbk_rows_argmax_f32(const float* x_dev, int rows, int V, int* idx_dev, void*
 int sbk_asr_ctc_head(sbk_asr* mm, const float* enc_dev, int B, int T, float* log_probs_dev, int* argmax_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->cfg;
-    SBK_REQUIRE(m->w_ctc != nullptr, "ctc_head: this handle was created without ctc_lin.w.* weights");
+    const sbk_asr_config& c = m->wt->cfg;
+    SBK_REQUIRE(m->wt->w_ctc != nullptr, "ctc_head: this handle was created without ctc_lin.w.* weights");
     SBK_REQUIRE(B >= 1 && T >= 1 && (log_probs_dev || argmax_dev), "ctc_head: bad arguments");
     const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
     RC(ensure_workspace(m, std::max(B, m->wsB), L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
@@ -2201,19 +2118,13 @@ int sbk_asr_ctc_head(sbk_asr* mm, const float* enc_dev, int B, int T, float* log
     if (enc_dev) SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, M * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
     float* logits = log_probs_dev;
     if (!logits) {  // arg-max only: the logits live in the (lazily grown) CTC scratch buffer
-        AsrModel::CtcBuf& cb = m->ctc;
-        const size_t need = M * V * 4 + 256;
-        if (need > cb.cap) {
-            if (cb.base) { SBK_CUDA_CHECK(cudaStreamSynchronize(st)); cudaFree(cb.base); cb.base = nullptr; cb.cap = 0; }
-            if (cudaMalloc(&cb.base, need) != cudaSuccess) { set_error("ctc_head: cudaMalloc(%zu) failed", need); return SBK_ERR_NOMEM; }
-            cb.cap = need;
-        }
-        logits = cb.base;
+        RC(grow_buffer(m, m->ctc, M * V * 4 + 256, "ctc_head"));
+        logits = static_cast<float*>(m->ctc.base);
     }
     RC(cast_f32_f16(b.enc_out, b.enc16, M * c.d_model, st));
     GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->b_ctc; e.out = logits; e.ldo = c.vocab;
-    RC(gemm_f16(b.enc16, c.d_model, m->w_ctc, c.d_model, e, (int)M, c.vocab, c.d_model, st));
+    e.mode = EPI_F32; e.bias = m->wt->b_ctc; e.out = logits; e.ldo = c.vocab;
+    RC(gemm_f16(b.enc16, c.d_model, m->wt->w_ctc, c.d_model, e, (int)M, c.vocab, c.d_model, st));
     return rows_logsoftmax_argmax(logits, (int)M, c.vocab, log_probs_dev != nullptr, argmax_dev, st);
 }
 
@@ -2224,19 +2135,16 @@ int sbk_asr_decode_teacher_forced(sbk_asr* mm, const int* tgt_dev, const float* 
                                   int T, float* out_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->cfg;
+    const sbk_asr_config& c = m->wt->cfg;
     SBK_REQUIRE(tgt_dev && enc_dev && out_dev && n >= 1 && S >= 1 && T >= 1, "decode: bad arguments");
     const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
     RC(ensure_workspace(m, std::max(n, m->wsB), L, std::max(n, m->ws_rows), std::max(S, m->ws_steps)));
     AsrModel::Buf& b = m->b;
     SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, (size_t)n * T * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
-    if (enc_len_dev) {
+    if (enc_len_dev)
         SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_len, enc_len_dev, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-    } else {
-        std::vector<int> full(n, T);
-        SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_len, full.data(), n * 4, cudaMemcpyHostToDevice, st));
-        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    }
+    else
+        RC(set_enc_len(b.enc_len, nullptr, n, T, st));
     return run_decode_teacher(m, tgt_dev, n, S, T, out_dev, st);
 }
 
@@ -2246,11 +2154,11 @@ int sbk_asr_lm_rescore(sbk_asr* mm, const int* tokens_dev, const int* lens_dev, 
                        float* scores_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(m->has_lm, "lm_rescore: this handle was created without TransformerLM weights");
-    SBK_REQUIRE(n >= 1 && L >= 2 && L <= m->cfg.max_len && pad_index >= 0 && pad_index < m->cfg.vocab && temperature > 0.0f,
+    SBK_REQUIRE(m->wt->has_lm, "lm_rescore: this handle was created without TransformerLM weights");
+    SBK_REQUIRE(n >= 1 && L >= 2 && L <= m->wt->cfg.max_len && pad_index >= 0 && pad_index < m->wt->cfg.vocab && temperature > 0.0f,
                 "lm_rescore: bad arguments (n=%d L=%d pad=%d)", n, L, pad_index);
     SBK_REQUIRE(pad_index == 0, "lm_rescore: pad_index must be 0 (TransformerLM.make_masks pads with index 0)");
-    RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
+    RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->wt->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
     return run_lm_rescore(m, tokens_dev, lens_dev, n, L, temperature, pad_index, scores_dev, st);
 }
 
@@ -2258,11 +2166,11 @@ int sbk_asr_lm_rescore(sbk_asr* mm, const int* tokens_dev, const int* lens_dev, 
 int sbk_asr_lm_forward(sbk_asr* mm, const int* tokens_dev, int n, int s, float* logits_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     SBK_REQUIRE(m != nullptr && tokens_dev && logits_dev, "lm_forward: null argument");
-    SBK_REQUIRE(m->has_lm, "lm_forward: this handle was created without TransformerLM weights");
+    SBK_REQUIRE(m->wt->has_lm, "lm_forward: this handle was created without TransformerLM weights");
     SBK_REQUIRE(n >= 1 && s >= 1, "lm_forward: bad shape n=%d s=%d", n, s);
     SBK_REQUIRE(n <= 65535, "lm_forward: n=%d sequences exceed the 65535 of one call (attention grid z)", n);
-    SBK_REQUIRE(s <= m->cfg.max_len, "lm_forward: s=%d exceeds max_len=%d", s, m->cfg.max_len);
-    SBK_REQUIRE((long long)n * s * std::max(m->cfg.vocab, 3 * m->cfg.lm_d_model) < (1LL << 31),
+    SBK_REQUIRE(s <= m->wt->cfg.max_len, "lm_forward: s=%d exceeds max_len=%d", s, m->wt->cfg.max_len);
+    SBK_REQUIRE((long long)n * s * std::max(m->wt->cfg.vocab, 3 * m->wt->cfg.lm_d_model) < (1LL << 31),
                 "lm_forward: n * s = %lld token rows is too many for one call", (long long)n * s);
     return run_lm_forward(m, tokens_dev, n, s, logits_dev, static_cast<cudaStream_t>(stream));
 }
@@ -2271,9 +2179,9 @@ int sbk_asr_lm_forward(sbk_asr* mm, const int* tokens_dev, int n, int s, float* 
 int sbk_asr_lm_step_logits(sbk_asr* mm, const int* tokens_dev, int n, int L, float* logits_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     SBK_REQUIRE(m != nullptr && tokens_dev && logits_dev, "lm_step_logits: null argument");
-    SBK_REQUIRE(m->has_lm, "lm_step_logits: this handle was created without TransformerLM weights");
-    SBK_REQUIRE(n >= 1 && L >= 1 && L <= m->cfg.max_len, "lm_step_logits: bad shape n=%d L=%d (max_len %d)", n, L, m->cfg.max_len);
-    RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
+    SBK_REQUIRE(m->wt->has_lm, "lm_step_logits: this handle was created without TransformerLM weights");
+    SBK_REQUIRE(n >= 1 && L >= 1 && L <= m->wt->cfg.max_len, "lm_step_logits: bad shape n=%d L=%d (max_len %d)", n, L, m->wt->cfg.max_len);
+    RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->wt->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
     return run_lm_step_logits(m, tokens_dev, n, L, logits_dev, static_cast<cudaStream_t>(stream));
 }
 
