@@ -271,6 +271,30 @@ int sbk_ctc_beam_search(const float* log_probs_dev, const int* lens_dev, int B, 
                         void* workspace_dev, size_t workspace_bytes, int* frame_beams_dev, int* parent_dev, int* token_dev,
                         float* score_dev, int* n_final_dev, void* stream);
 
+/* ---- Transducer greedy search: TransducerBeamSearcher.transducer_greedy_decode (decoders/transducer.py:156-291) with
+ * the prediction network Embedding -> LSTM (1 layer, unidirectional, with biases, gate order i, f, g, o) ->
+ * Linear(bias=False), the joint GELU(tn + out_PN) (exact erf form) and the output Linear(bias=False) + log-softmax.
+ * Weights (HOST fp32, torch layouts): "emb.weight" [vocab, emb_dim], "lstm.weight_ih" [4 hidden, emb_dim],
+ * "lstm.weight_hh" [4 hidden, hidden], "lstm.bias_ih" / "lstm.bias_hh" [4 hidden], "proj_dec.weight" [joint, hidden],
+ * "out.weight" [vocab, joint].  hidden and joint are multiples of 64 up to 1024, vocab <= 4096, and the fp16 weight
+ * slices must fit the shared memory of the device's SMs. */
+typedef struct sbk_transducer sbk_transducer; /* opaque */
+typedef struct {
+    int vocab, emb_dim, hidden, joint;
+} sbk_transducer_config;
+int sbk_transducer_create(const sbk_transducer_config* cfg, const sbk_tensor* weights, int n_weights, sbk_transducer** out);
+void sbk_transducer_destroy(sbk_transducer* m);
+/* CTAs per search call (one per SM) and the shared memory one CTA uses at batch size 1 */
+int sbk_transducer_info(const sbk_transducer* m, int* ctas, int* smem_bytes_at_b1);
+/* One cooperative kernel for the whole call.  tn_dev [B, T, joint] fp32; every frame is decoded.  State in / out (fp32):
+ * h_dev, c_dev [B, hidden] and out_pn_dev [B, joint]; with start_from_blank they are overwritten with PN(blank) from a
+ * zero LSTM state first.  Outputs: tokens_dev [B, T * (max_symbols_per_step + 1)] int32 (the first n_tokens_dev[b]
+ * entries of row b), frames_dev (same shape, may be null) = the frame each token was emitted at, logp_sum_dev [B] = sum of the emitted tokens' log-probabilities, and, if stats_dev is not null,
+ * stats_dev[0..1] = rounds (decisions of the longest row) and grid barriers.  1 <= B <= 1024, 0 <= blank < vocab. */
+int sbk_transducer_greedy(sbk_transducer* m, const float* tn_dev, int B, int T, int blank, int max_symbols_per_step,
+                          int start_from_blank, float* h_dev, float* c_dev, float* out_pn_dev, int* tokens_dev,
+                          int* frames_dev, int* n_tokens_dev, float* logp_sum_dev, int* stats_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,8 @@ Two module layouts are accepted:
   ``hparams["transformer_beam_search"]`` the model itself sits under ``modules["transformer"]`` -- i.e. what
   ``speechbrain/asr-conformer-transformerlm-librispeech``'s hyperparams.yaml builds (``from_hparams`` loads such a file
   from a local directory, see ``speechbrain_b200.utils.hparams``);
+* the Conformer-Transducer layout (``hparams["transducer_beam_search"]``): ``encoder`` ends in the ``proj_enc`` Linear and
+  ``decoder`` is a ``TransducerBeamSearcher`` (greedy, decoders/transducer.py) that gets every frame of the batch;
 * the flat layout the recipes' training YAML uses (compute_features, normalize, CNN, Transformer, seq_lin, decoder).
 
 The waveform -> encoder states part runs as ONE fused device pipeline (Fbank + CMVN + CNN + Conformer encoder, C ABI
@@ -53,10 +55,12 @@ class EncoderDecoderASR(torch.nn.Module):
         self.hparams = dict(hparams) if isinstance(hparams, dict) else (dict(vars(hparams)) if hparams is not None else {})
         self.tokenizer = self.hparams.get("tokenizer")
         self.transformer_beam_search = bool(self.hparams.get("transformer_beam_search", False))
-        if self.hparams.get("transducer_beam_search", False):
-            raise NotImplementedError("speechbrain_b200.EncoderDecoderASR: transducer decoding is not on the H100 hot path")
+        self.transducer_beam_search = bool(self.hparams.get("transducer_beam_search", False))
         self.device = torch.device((run_opts or {}).get("device", "cuda:0"))
         dec = self.mods["decoder"]
+        if self.transducer_beam_search:
+            self._init_transducer()
+            return
         if not isinstance(dec, (S2STransformerGreedySearcher, S2STransformerBeamSearcher)):
             raise NotImplementedError("EncoderDecoderASR: the decoder must be a speechbrain_b200 S2STransformerGreedySearcher "
                                       "or S2STransformerBeamSearcher")
@@ -76,6 +80,27 @@ class EncoderDecoderASR(torch.nn.Module):
         if self.normalize.norm_type != "global":
             raise NotImplementedError("EncoderDecoderASR: fused pipeline needs InputNormalization(norm_type='global')")
 
+    def _init_transducer(self):
+        """The Conformer-Transducer layout: ``encoder`` = LengthsCapableSequential(Fbank, InputNormalization,
+        ConvolutionFrontEnd, EncoderWrapper(TransformerASR), Linear proj_enc), ``decoder`` = TransducerBeamSearcher."""
+        from ..decoders.transducer import TransducerBeamSearcher
+        from ..nnet.linear import Linear
+        if not isinstance(self.mods["decoder"], TransducerBeamSearcher):
+            raise NotImplementedError("EncoderDecoderASR(transducer_beam_search=True): the decoder must be a "
+                                      "speechbrain_b200 TransducerBeamSearcher")
+        if "encoder" not in self.mods:
+            raise ValueError("EncoderDecoderASR(transducer_beam_search=True): need modules['encoder']")
+        vals = list(self.mods["encoder"].children()) if isinstance(self.mods["encoder"], torch.nn.Module) else []
+        wrap = _find(vals, EncoderWrapper)
+        tr = _find(vals, TransformerASR) or (wrap.transformer if wrap is not None else None)
+        for name, m in (("fbank", _find(vals, Fbank)), ("normalize", _find(vals, InputNormalization)),
+                        ("cnn", _find(vals, ConvolutionFrontEnd)), ("transformer", tr), ("proj_enc", _find(vals, Linear))):
+            if m is None:
+                raise ValueError(f"EncoderDecoderASR: could not find the {name} module in modules['encoder']")
+            object.__setattr__(self, name, m)
+        if self.normalize.norm_type != "global":
+            raise NotImplementedError("EncoderDecoderASR: fused pipeline needs InputNormalization(norm_type='global')")
+
     @classmethod
     def from_hparams(cls, source, hparams_file="hyperparams.yaml", overrides=None, savedir=None, run_opts=None, **kwargs):
         """inference/interfaces.py:385-489 for a LOCAL directory: loads ``source/hparams_file`` with the HyperPyYAML-subset
@@ -88,6 +113,8 @@ class EncoderDecoderASR(torch.nn.Module):
     def engine(self):
         dec = self.mods["decoder"]
         src = {"fbank": self.fbank, "normalize": self.normalize, "CNN.": self.cnn}
+        if self.transducer_beam_search:
+            return self.transformer.engine_slot(("transducer",)).get(self.device, ("fbank", "cnn", "encoder"), src)
         return dec._get_engine(self.device, parts=("fbank", "cnn", "encoder"), extra_sources=src)
 
     def _steps(self, n_samples):
@@ -101,6 +128,8 @@ class EncoderDecoderASR(torch.nn.Module):
         """inference/ASR.py:100-128: wavs [B, L] (+ relative lengths) -> encoder states [B, T, d]."""
         wavs = wavs.float().to(self.device)
         wav_lens = wav_lens.to(self.device)
+        if self.transducer_beam_search:  # the fused wav -> encoder pipeline, then proj_enc on the wgmma GEMM
+            return self.proj_enc(self.engine().encode_wav(wavs, wav_lens))
         dec = self.mods["decoder"]
         _, _, enc, _ = self.engine().transcribe_greedy_dev(wavs, wav_lens, 0, dec.bos_index, dec.eos_index, want_enc=True)
         return enc
@@ -109,7 +138,11 @@ class EncoderDecoderASR(torch.nn.Module):
     def transcribe_batch(self, wavs, wav_lens):
         """inference/ASR.py:131-169: -> (predicted_words list[str], predicted_tokens list[list[int]])."""
         dec = self.mods["decoder"]
-        if isinstance(dec, S2STransformerBeamSearcher):
+        if self.transducer_beam_search:
+            # inference/ASR.py:160-164: the search gets every frame of the padded batch (no lengths), as the reference's
+            # does, so a short utterance is also decoded over its padded frames
+            hyps = dec(self.encode_batch(wavs, wav_lens))[0]
+        elif isinstance(dec, S2STransformerBeamSearcher):
             enc = self.encode_batch(wavs, wav_lens)
             hyps = dec(enc, wav_lens.to(self.device))[0]
             if dec.return_topk:  # padded (B, topk, L) tensor: the best hypothesis of every utterance, like hyps[0]
