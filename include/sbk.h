@@ -17,9 +17,9 @@ extern "C" {
 typedef struct sbk_fbank sbk_fbank; /* opaque */
 typedef struct sbk_asr sbk_asr;     /* opaque */
 
-enum { SBK_ATT_ROPE = 0, SBK_ATT_RELPOS = 1, SBK_ATT_HYPERMIX = 2 };
+enum { SBK_ATT_ROPE = 0, SBK_ATT_RELPOS = 1, SBK_ATT_HYPERMIX = 2, SBK_ATT_REGULAR = 3 };
 enum { SBK_ACT_RELU = 0, SBK_ACT_GELU = 1 };
-enum { SBK_ENC_CONFORMER = 0, SBK_ENC_BRANCHFORMER = 1 };
+enum { SBK_ENC_CONFORMER = 0, SBK_ENC_BRANCHFORMER = 1, SBK_ENC_TRANSFORMER = 2 };
 enum { SBK_PART_FBANK = 1, SBK_PART_CNN = 2, SBK_PART_ENCODER = 4, SBK_PART_DECODER = 8, SBK_PART_ALL = 15, SBK_PART_LM = 16 };
 
 typedef struct {
@@ -31,13 +31,14 @@ typedef struct {
 typedef struct {
     /* Fbank (lobes/features.py:98-145) -- sizes in samples */
     int n_fft, hop, n_mels;
-    /* ConvolutionFrontEnd (lobes/models/convolution.py:162-203): 2 blocks, 3x3, stride 2 */
+    /* ConvolutionFrontEnd (lobes/models/convolution.py:162-203): 2 blocks, 3x3, stride 2 (or 3 blocks, see cnn_blocks) */
     int cnn_c1, cnn_c2;
     /* TransformerASR (lobes/models/transformer/TransformerASR.py:247-325) */
     int input_size, d_model, nhead, num_encoder_layers, num_decoder_layers, d_ffn, vocab, kernel_size;
     int attention_type;     /* SBK_ATT_ROPE (RoPEMHA) | SBK_ATT_RELPOS (RelPosMHAXL) | SBK_ATT_HYPERMIX (hypermixing: Conformer
                                encoder only, head width d_model / nhead 32 or 64, hypernetwork width d_ffn / nhead a multiple
-                               of 16 up to 256; inputs up to 3000 frames) */
+                               of 16 up to 256; inputs up to 3000 frames) | SBK_ATT_REGULAR (regularMHA: the Transformer
+                               encoder only, head width 64 or 128) */
     int decoder_activation; /* SBK_ACT_RELU | SBK_ACT_GELU (the `activation` ctor kwarg) */
     int max_len;            /* positional tables (ctor kwarg max_length, default 2500) */
     int parts;              /* bitmask of SBK_PART_*: which sub-models the weight table carries */
@@ -49,8 +50,13 @@ typedef struct {
     /* TransformerASR encoder_module: SBK_ENC_CONFORMER (0, so a zeroed config stays a Conformer) or SBK_ENC_BRANCHFORMER
        (Branchformer.py:92-234: RelPosMHAXL attention, no FFN modules, d_ffn only sizes the decoder) with the CSGU width
        csgu_linear_units (even, csgu_linear_units / 2 % 8 == 0) and kernel_size the CSGU's odd depthwise kernel (<= 31);
-       branchformer_activation (SBK_ACT_RELU | SBK_ACT_GELU) follows pre_channel_proj */
+       branchformer_activation (SBK_ACT_RELU | SBK_ACT_GELU) follows pre_channel_proj; or SBK_ENC_TRANSFORMER
+       (TransformerEncoderLayer, Transformer.py:311-490: pre-norm, regularMHA, Linear + GELU + Linear, the absolute sine table
+       added to the input Linear's output) */
     int encoder_module, csgu_linear_units, branchformer_activation;
+    /* ConvolutionFrontEnd blocks: 0 or 2 = the Conformer recipes' 2 x (3x3, stride 2), channels (cnn_c1, cnn_c2) = (64, 32);
+       3 = the Transformer recipes' (5x5, stride 2), (5x5, stride 2), (1x1 + residual 1x1), 64 channels each */
+    int cnn_blocks;
 } sbk_asr_config;
 
 typedef struct {

@@ -24,7 +24,7 @@ class sbk_asr_config(ctypes.Structure):
         "num_decoder_layers", "d_ffn", "vocab", "kernel_size", "attention_type", "decoder_activation", "max_len",
         "parts", "lm_d_model", "lm_nhead", "lm_layers", "lm_d_ffn", "lm_activation")] + [
         (k, ctypes.c_float) for k in ("fbank_amin", "fbank_top_db", "norm_eps")] + [
-        (k, ctypes.c_int) for k in ("encoder_module", "csgu_linear_units", "branchformer_activation")]
+        (k, ctypes.c_int) for k in ("encoder_module", "csgu_linear_units", "branchformer_activation", "cnn_blocks")]
 
 
 class sbk_beam_params(ctypes.Structure):
@@ -43,9 +43,9 @@ class sbk_ctc_beam_params(ctypes.Structure):
                 ("blank_skip_logp", ctypes.c_float)]
 
 
-SBK_ATT_ROPE, SBK_ATT_RELPOS, SBK_ATT_HYPERMIX = 0, 1, 2
+SBK_ATT_ROPE, SBK_ATT_RELPOS, SBK_ATT_HYPERMIX, SBK_ATT_REGULAR = 0, 1, 2, 3
 SBK_ACT_RELU, SBK_ACT_GELU = 0, 1
-SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER = 0, 1
+SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER, SBK_ENC_TRANSFORMER = 0, 1, 2
 SBK_PARTS = {"fbank": 1, "cnn": 2, "encoder": 4, "decoder": 8, "lm": 16}
 
 # every symbol include/sbk.h declares (tests check the library exports all of them)

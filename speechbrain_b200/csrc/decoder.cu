@@ -270,13 +270,16 @@ int skinny_gemm(const SkinnyArgs& a, cudaStream_t stream) {
 // 3 shuffles, and the probabilities stay in registers for p.V.  The 4 warps' (max, sum, out) triples are merged
 // through shared memory.
 // Self-attention: keys = cache positions [0, step]; cross-attention: keys = encoder frames [0, enc_len[utt]).
-// (nn.MultiheadAttention semantics, scale 1/sqrt(d_h) already folded into q.)  head_dim == 64.
+// (nn.MultiheadAttention semantics, scale 1/sqrt(d_h) already folded into q.)  head_dim DH == 64, or 128 (the Transformer
+// recipes' 4 heads of 128): a lane then owns dims [8 (lane % 8), +8) of each 64-dim half, NV = 2 16-byte vectors per key.
 constexpr int DA_WARPS = 4;
 constexpr int DA_CHUNK = 32;  // keys a warp handles per round (8 per lane group)
 constexpr int DA_KPG = DA_CHUNK / 4;
 
-__global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const DecAttnArgs a) {
-    __shared__ float part_o[DA_WARPS][64];
+template <int DH>
+__global__ void __launch_bounds__(DA_WARPS * 32, DH == 64 ? 4 : 2) dec_attention_kernel(const DecAttnArgs a) {
+    constexpr int NV = DH / 64;
+    __shared__ float part_o[DA_WARPS][DH];
     __shared__ float part_m[DA_WARPS], part_l[DA_WARPS];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // heads on the fast grid axis: the 8 CTAs that share an utterance's K/V rows (2 KB per frame, 128 B per head) are
@@ -295,7 +298,7 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
     const int per = (n_keys + DA_WARPS - 1) / DA_WARPS;
     const int kb = warp * per, ke = min(n_keys, kb + per);
     const int gq = lane >> 3, dl = (lane & 7) * 8;
-    const int hs = a.head_stride > 0 ? a.head_stride : 64;
+    const int hs = a.head_stride > 0 ? a.head_stride : DH;
     const __half* kbase = a.kbase + static_cast<size_t>(blk) * a.row_stride + static_cast<size_t>(h) * hs + dl;
     const __half* vbase = a.vbase + static_cast<size_t>(blk) * a.row_stride + static_cast<size_t>(h) * hs + dl;
     // beam search: position j of hypothesis r lives in the cache row of the ancestor that wrote it
@@ -303,7 +306,7 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
     if (a.lineage) lin = a.lineage + static_cast<size_t>((n_keys - 1) & 1) * gridDim.y * a.lin_stride + static_cast<size_t>(r) * a.lin_stride;
     const int* tokc = a.tok_cache;  // TransformerLM.make_masks: keys whose token id is pad_idx (0) are masked
     // every load of the chunk at c0: 8 keys x (16 B of K + 16 B of V) per lane
-    uint4 kv[DA_KPG], vv[DA_KPG];
+    uint4 kv[DA_KPG][NV], vv[DA_KPG][NV];
     bool live[DA_KPG];
     auto load_chunk = [&](int c0) {
 #pragma unroll
@@ -314,12 +317,18 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
                 ptrdiff_t off = static_cast<ptrdiff_t>(j) * a.key_stride;
                 int src_row = r;
                 if (lin) { src_row = lin[j]; off += (static_cast<ptrdiff_t>(src_row) - r) * static_cast<ptrdiff_t>(a.row_stride); }
-                kv[i] = *reinterpret_cast<const uint4*>(kbase + off);
-                vv[i] = *reinterpret_cast<const uint4*>(vbase + off);
+#pragma unroll
+                for (int v = 0; v < NV; ++v) {
+                    kv[i][v] = *reinterpret_cast<const uint4*>(kbase + off + 64 * v);
+                    vv[i][v] = *reinterpret_cast<const uint4*>(vbase + off + 64 * v);
+                }
                 if (tokc) live[i] = tokc[static_cast<size_t>(src_row) * a.lin_stride + j] != a.pad_tok;
             } else {
-                kv[i] = make_uint4(0u, 0u, 0u, 0u);
-                vv[i] = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+                for (int v = 0; v < NV; ++v) {
+                    kv[i][v] = make_uint4(0u, 0u, 0u, 0u);
+                    vv[i][v] = make_uint4(0u, 0u, 0u, 0u);
+                }
             }
         }
     };
@@ -328,20 +337,21 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
         pdl_wait();
     }
     // this lane's 8 dims of the query
-    float qf[8];
-    {
-        const uint4 qv = *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * 64 + dl);
+    float qf[8 * NV];
+#pragma unroll
+    for (int v = 0; v < NV; ++v) {
+        const uint4 qv = *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * DH + 64 * v + dl);
         const __half2* q2 = reinterpret_cast<const __half2*>(&qv);
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
             const float2 f = __half22float2(q2[u]);
-            qf[2 * u] = f.x; qf[2 * u + 1] = f.y;
+            qf[8 * v + 2 * u] = f.x; qf[8 * v + 2 * u + 1] = f.y;
         }
     }
     float m_run = -INFINITY, l_run = 0.0f;
-    float o[8];
+    float o[8 * NV];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) o[e] = 0.0f;
+    for (int e = 0; e < 8 * NV; ++e) o[e] = 0.0f;
     for (int c0 = kb; c0 < ke; c0 += DA_CHUNK) {
         if (!xatt || c0 != kb) load_chunk(c0);  // issue every load of this chunk up front
         // ---- scores: 8-dim partial dot per lane, summed over the 8 lanes of the key's group
@@ -349,13 +359,16 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
         float cm = -INFINITY;
 #pragma unroll
         for (int i = 0; i < DA_KPG; ++i) {
-            const __half2* k2 = reinterpret_cast<const __half2*>(&kv[i]);
             float dot = 0.0f;
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const float2 kf = __half22float2(k2[u]);
-                dot = fmaf(kf.x, qf[2 * u], dot);
-                dot = fmaf(kf.y, qf[2 * u + 1], dot);
+            for (int v = 0; v < NV; ++v) {
+                const __half2* k2 = reinterpret_cast<const __half2*>(&kv[i][v]);
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const float2 kf = __half22float2(k2[u]);
+                    dot = fmaf(kf.x, qf[8 * v + 2 * u], dot);
+                    dot = fmaf(kf.y, qf[8 * v + 2 * u + 1], dot);
+                }
             }
             dot += __shfl_xor_sync(0xffffffffu, dot, 1);
             dot += __shfl_xor_sync(0xffffffffu, dot, 2);
@@ -370,17 +383,20 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
         // ---- p.V with the probabilities still in registers
         float psum = 0.0f;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] *= alpha;
+        for (int e = 0; e < 8 * NV; ++e) o[e] *= alpha;
 #pragma unroll
         for (int i = 0; i < DA_KPG; ++i) {
             const float p = (sc[i] == -INFINITY) ? 0.0f : __expf(sc[i] - m_new);
             psum += p;
-            const __half2* v2 = reinterpret_cast<const __half2*>(&vv[i]);
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const float2 vf = __half22float2(v2[u]);
-                o[2 * u] = fmaf(p, vf.x, o[2 * u]);
-                o[2 * u + 1] = fmaf(p, vf.y, o[2 * u + 1]);
+            for (int v = 0; v < NV; ++v) {
+                const __half2* v2 = reinterpret_cast<const __half2*>(&vv[i][v]);
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const float2 vf = __half22float2(v2[u]);
+                    o[8 * v + 2 * u] = fmaf(p, vf.x, o[8 * v + 2 * u]);
+                    o[8 * v + 2 * u + 1] = fmaf(p, vf.y, o[8 * v + 2 * u + 1]);
+                }
             }
         }
         psum += __shfl_xor_sync(0xffffffffu, psum, 8);
@@ -389,17 +405,17 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
         m_run = m_new;
     }
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
+    for (int e = 0; e < 8 * NV; ++e) {
         o[e] += __shfl_xor_sync(0xffffffffu, o[e], 8);
         o[e] += __shfl_xor_sync(0xffffffffu, o[e], 16);
     }
     if (lane < 8) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) part_o[warp][dl + e] = o[e];
+        for (int e = 0; e < 8 * NV; ++e) part_o[warp][64 * (e >> 3) + dl + (e & 7)] = o[e];
     }
     if (lane == 0) { part_m[warp] = m_run; part_l[warp] = l_run; }
     __syncthreads();
-    if (threadIdx.x < 64) {
+    if (threadIdx.x < DH) {
         float M = part_m[0];
 #pragma unroll
         for (int w = 1; w < DA_WARPS; ++w) M = fmaxf(M, part_m[w]);
@@ -410,7 +426,7 @@ __global__ void __launch_bounds__(DA_WARPS * 32, 4) dec_attention_kernel(const D
             num += part_o[w][threadIdx.x] * sc;
             den += part_l[w] * sc;
         }
-        a.out[static_cast<size_t>(r) * a.ldo + h * 64 + threadIdx.x] = float2half_sat(num / den);
+        a.out[static_cast<size_t>(r) * a.ldo + h * DH + threadIdx.x] = float2half_sat(num / den);
     }
 }
 
@@ -480,9 +496,9 @@ __global__ void __launch_bounds__(128) dec_attention_generic_kernel(const DecAtt
 }
 
 int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t stream) {
-    if (a.dh != 64) {
+    if (a.dh != 64 && a.dh != 128) {
         SBK_REQUIRE(a.dh >= 4 && a.dh <= 64 && a.dh % 4 == 0 && a.key_stride % 4 == 0 && a.row_stride % 4 == 0,
-                    "dec_attention: head_dim=%d not built (64, or a multiple of 4 below 64)", a.dh);
+                    "dec_attention: head_dim=%d not built (128, 64, or a multiple of 4 below 64)", a.dh);
         SBK_REQUIRE(max_keys <= DG_MAXKEYS, "dec_attention: %d keys exceed the generic kernel's limit %d", max_keys, DG_MAXKEYS);
         if (n_rows == 0) return SBK_OK;
         DecAttnArgs g = a;
@@ -495,7 +511,13 @@ int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t s
     if (n_rows == 0) return SBK_OK;
     DecAttnArgs b = a;
     b.n_keys_fixed = max_keys;
-    SBK_CUDA_CHECK(launch_k(dec_attention_kernel, dim3(a.H, n_rows), dim3(DA_WARPS * 32), 0, stream, b));
+    if (a.dh == 128) {
+        SBK_REQUIRE(a.key_stride % 8 == 0 && a.row_stride % 8 == 0 && a.ldq % 8 == 0,
+                    "dec_attention: head_dim 128 needs 16-byte aligned key rows");
+        SBK_CUDA_CHECK(launch_k(dec_attention_kernel<128>, dim3(a.H, n_rows), dim3(DA_WARPS * 32), 0, stream, b));
+    } else {
+        SBK_CUDA_CHECK(launch_k(dec_attention_kernel<64>, dim3(a.H, n_rows), dim3(DA_WARPS * 32), 0, stream, b));
+    }
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }

@@ -909,6 +909,9 @@ static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int
         auto kern = encoder_attention_kernel<DH, DHP, false>;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, nullptr, nullptr, nullptr, 0, scale, out, ldo, chunk, left_chunks);
+    } else if constexpr (DH > 64) {  // the RelPos band and P_h table are built for head widths up to 64
+        set_error("encoder_attention: RelPosMHAXL with head_dim=%d not built", DH);
+        return SBK_ERR_UNSUPPORTED;
     } else {
         SBK_REQUIRE(ldp % 4 == 0, "encoder_attention: bad ldp");
         const size_t smem = 4ull * ATT_BQ * STR * 2 + static_cast<size_t>(T) * STR * 2 + 4ull * 16 * 81 * 4 +
@@ -936,7 +939,9 @@ int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_d
         return launch_encoder_attention<36, 48>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
     if (head_dim == 32)
         return launch_encoder_attention<32, 32>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
-    set_error("encoder_attention: head_dim=%d not built (64, 36, 32)", head_dim);
+    if (head_dim == 128)  // the Transformer recipes' regularMHA (512 / 4 heads); no positional term
+        return launch_encoder_attention<128, 128>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
+    set_error("encoder_attention: head_dim=%d not built (128, 64, 36, 32)", head_dim);
     return SBK_ERR_UNSUPPORTED;
 }
 

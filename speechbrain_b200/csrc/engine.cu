@@ -47,6 +47,9 @@ struct EncLayerW {
     const float *bpre, *bpost, *bmerge;
     const float *csgu_ln_g, *csgu_ln_b, *csgu_taps, *csgu_bias;  // taps tap-major [CSGU_TAP_ROWS, C/2] (csgu_repack_taps)
     HyperMixWeights hm;               // HyperConformer: mha_layer = HyperMixing (replaces wqkv / wo / bo)
+    // Transformer layer (Transformer.py:311-490): self_att.att in_proj bias, repacked like wqkv; norm1 / norm2 and the FFN
+    // (ffn1_w1 / ffn1_b1 / ffn1_w2 / ffn1_b2) use the fields above
+    const float* bqkv;
 };
 
 struct DecLayerW {
@@ -83,6 +86,7 @@ struct AsrWeights {
     const float *glob_mean = nullptr, *glob_std = nullptr;
     const float *c1_w, *c1_b, *c1_g, *c1_be, *c2_b, *c2_g, *c2_be;
     const __half* c2_w;
+    Cnn3Weights cnn3{};  // cfg.cnn_blocks == 3
     // encoder
     const __half* w_in; const float* b_in;
     std::vector<EncLayerW> enc;
@@ -90,6 +94,7 @@ struct AsrWeights {
     const float *rope_cos = nullptr, *rope_sin = nullptr;  // [max_len, dh/2]
     const __half* relpos_pe = nullptr;                     // [max_len, d] rows = |r|
     const float* hm_pe = nullptr;                          // HyperMixing's own sine table [HM_PE_ROWS, d]
+    const float* enc_pe = nullptr;                         // regularMHA: the absolute sine table [max_len, d]
     int pos_len = 0;
     // decoder
     const float* emb; const float* dec_pe;
@@ -333,20 +338,27 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
     SBK_REQUIRE(cfg && weights && out, "asr_create: null argument");
     const sbk_asr_config& c = *cfg;
     SBK_REQUIRE(c.d_model % 8 == 0 && c.d_model % c.nhead == 0, "asr_create: bad d_model/nhead");
-    SBK_REQUIRE(c.attention_type == SBK_ATT_ROPE || c.attention_type == SBK_ATT_RELPOS || c.attention_type == SBK_ATT_HYPERMIX,
-                "asr_create: attention_type must be RoPEMHA, RelPosMHAXL or hypermixing");
+    SBK_REQUIRE(c.attention_type == SBK_ATT_ROPE || c.attention_type == SBK_ATT_RELPOS || c.attention_type == SBK_ATT_HYPERMIX ||
+                    c.attention_type == SBK_ATT_REGULAR,
+                "asr_create: attention_type must be RoPEMHA, RelPosMHAXL, hypermixing or regularMHA");
     const int d = c.d_model, dh = d / c.nhead, F = c.d_ffn, K = c.kernel_size;
     const bool hypermix = c.attention_type == SBK_ATT_HYPERMIX;
-    SBK_REQUIRE(hypermix || dh == 64 || dh == 36 || dh == 32, "asr_create: encoder head_dim=%d not built (64, 36, 32)", dh);
+    const bool tfm = c.encoder_module == SBK_ENC_TRANSFORMER;
+    SBK_REQUIRE(tfm == (c.attention_type == SBK_ATT_REGULAR),
+                "asr_create: regularMHA is built for the Transformer encoder only, and the Transformer encoder with regularMHA only");
+    SBK_REQUIRE(!tfm || dh == 64 || dh == 128, "asr_create: Transformer encoder head_dim=%d not built (128, 64)", dh);
+    SBK_REQUIRE(tfm || hypermix || dh == 64 || dh == 36 || dh == 32, "asr_create: encoder head_dim=%d not built (64, 36, 32)", dh);
+    SBK_REQUIRE(c.cnn_blocks == 0 || c.cnn_blocks == 2 || (c.cnn_blocks == 3 && c.cnn_c1 == 64 && c.cnn_c2 == 64),
+                "asr_create: cnn_blocks=%d with channels (%d, %d) not built (2, or 3 with 64 channels)", c.cnn_blocks, c.cnn_c1, c.cnn_c2);
     SBK_REQUIRE(!hypermix || (c.encoder_module == SBK_ENC_CONFORMER && (dh == 32 || dh == 64) && F % c.nhead == 0 &&
                               (F / c.nhead) % 16 == 0 && F / c.nhead <= 256),
                 "asr_create: hypermixing needs the Conformer encoder, a head width d_model / nhead of 32 or 64 and "
                 "k = d_ffn / nhead a multiple of 16 up to 256 (got %d, %d)", dh, c.nhead > 0 ? F / c.nhead : 0);
-    SBK_REQUIRE(!((c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0) || (dh <= 64 && dh % 4 == 0 && d % 16 == 0),
-                "asr_create: decoder head_dim must be a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)", dh, d);
+    SBK_REQUIRE(!((c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0) || ((dh <= 64 || dh == 128) && dh % 4 == 0 && d % 16 == 0),
+                "asr_create: decoder head_dim must be 128 or a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)", dh, d);
     SBK_REQUIRE(c.attention_type != SBK_ATT_ROPE || dh % 32 == 0, "asr_create: RoPEMHA needs head_dim %% 32 == 0");
-    SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER || c.encoder_module == SBK_ENC_BRANCHFORMER,
-                "asr_create: encoder_module %d (0 Conformer, 1 Branchformer)", c.encoder_module);
+    SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER || c.encoder_module == SBK_ENC_BRANCHFORMER || tfm,
+                "asr_create: encoder_module %d (0 Conformer, 1 Branchformer, 2 Transformer)", c.encoder_module);
     SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER ||
                     (c.attention_type == SBK_ATT_RELPOS && c.csgu_linear_units > 0 && c.csgu_linear_units % 16 == 0 &&
                      (K & 1) == 1 && K <= CSGU_TAP_ROWS),
@@ -381,7 +393,33 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
         }
     }
     // ---- CNN front-end
-    if (has_cnn) {
+    if (has_cnn && c.cnn_blocks == 3) {  // convolution.py:116-320 with kernel_sizes (5, 5, 1), residuals (False, False, True)
+        const int C = 64, F1 = (c.n_mels - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
+        if (F2 * C != c.input_size) { set_error("asr_create: CNN output %d != input_size %d", F2 * C, c.input_size); return SBK_ERR_ARG; }
+        const std::string b0 = "CNN.convblock_0.convs.", b1 = "CNN.convblock_1.convs.", b2 = "CNN.convblock_2.";
+        Cnn3Weights& k = W->cnn3;
+        k.w1 = p.f32(b0 + "conv_0.conv.weight", (int64_t)C * 25); k.b1 = p.f32(b0 + "conv_0.conv.bias", C);
+        k.g1 = p.f32(b0 + "norm_0.norm.weight", (int64_t)F1 * C); k.be1 = p.f32(b0 + "norm_0.norm.bias", (int64_t)F1 * C);
+        const float* w2 = find(w, b1 + "conv_0.conv.weight", (int64_t)C * C * 25);
+        const float* w3a = find(w, b2 + "convs.conv_0.conv.weight", (int64_t)C * C);
+        const float* w3r = find(w, b2 + "reduce_conv.conv.conv.weight", (int64_t)C * C);
+        const float* b3a = find(w, b2 + "convs.conv_0.conv.bias", C);
+        const float* b3r = find(w, b2 + "reduce_conv.conv.conv.bias", C);
+        if (!w2 || !w3a || !w3r || !b3a || !b3r) return SBK_ERR_ARG;
+        std::vector<float> w2p((size_t)C * 25 * C);  // (o, ch, kf, kt) -> [o][(kf * 5 + kt) * 64 + ch]
+        for (int o = 0; o < C; ++o)
+            for (int ch = 0; ch < C; ++ch)
+                for (int t = 0; t < 25; ++t) w2p[((size_t)o * 25 + t) * C + ch] = w2[((size_t)o * C + ch) * 25 + t];
+        k.w2p = p.f16_raw(w2p.data(), w2p.size());
+        k.b2 = p.f32(b1 + "conv_0.conv.bias", C);
+        k.g2 = p.f32(b1 + "norm_0.norm.weight", (int64_t)F2 * C); k.be2 = p.f32(b1 + "norm_0.norm.bias", (int64_t)F2 * C);
+        std::vector<float> w3((size_t)2 * C * C), b3(2 * C);  // [convs.conv_0 | reduce_conv.conv] output channels
+        memcpy(w3.data(), w3a, (size_t)C * C * 4); memcpy(w3.data() + (size_t)C * C, w3r, (size_t)C * C * 4);
+        memcpy(b3.data(), b3a, C * 4); memcpy(b3.data() + C, b3r, C * 4);
+        k.w3 = p.f32_raw(w3.data(), w3.size()); k.b3 = p.f32_raw(b3.data(), b3.size());
+        k.g3 = p.f32(b2 + "convs.norm_0.norm.weight", (int64_t)F2 * C); k.be3 = p.f32(b2 + "convs.norm_0.norm.bias", (int64_t)F2 * C);
+        k.gr = p.f32(b2 + "reduce_conv.norm.norm.weight", (int64_t)F2 * C); k.ber = p.f32(b2 + "reduce_conv.norm.norm.bias", (int64_t)F2 * C);
+    } else if (has_cnn) {
         const int F1 = (c.n_mels - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
         if (F2 * c.cnn_c2 != c.input_size) { set_error("asr_create: CNN output %d != input_size %d", F2 * c.cnn_c2, c.input_size); return SBK_ERR_ARG; }
         W->c1_w = p.f32("CNN.convblock_0.convs.conv_0.conv.weight", (int64_t)c.cnn_c1 * 9);
@@ -428,6 +466,31 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
         }
         e.csgu_bias = p.f32(cb + "csgu.conv.conv.bias", C2);
         e.wmerge = p.f16(q + "merge_proj.weight", (int64_t)d * 2 * d); e.bmerge = p.f32(q + "merge_proj.bias", d);
+    }
+    for (int l = 0; l < c.num_encoder_layers && p.ok && tfm; ++l) {
+        const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".";
+        EncLayerW& e = W->enc[l];
+        e.norm1_g = p.f32(q + "norm1.norm.weight", d); e.norm1_b = p.f32(q + "norm1.norm.bias", d);
+        e.norm2_g = p.f32(q + "norm2.norm.weight", d); e.norm2_b = p.f32(q + "norm2.norm.bias", d);
+        const float* wi = find(w, q + "self_att.att.in_proj_weight", (int64_t)3 * d * d);
+        const float* bi = find(w, q + "self_att.att.in_proj_bias", 3 * d);
+        if (!wi || !bi) { p.ok = false; break; }
+        // nn.MultiheadAttention's [Wq; Wk; Wv] rows -> per-head [q | k | v] blocks (the encoder attention's layout), with
+        // 1/sqrt(d_h) folded into the query rows
+        std::vector<float> wr((size_t)3 * d * d), br(3 * d);
+        const float qs = 1.0f / sqrtf((float)dh);
+        for (int h = 0; h < c.nhead; ++h)
+            for (int part = 0; part < 3; ++part)
+                for (int j = 0; j < dh; ++j) {
+                    const size_t src = (size_t)part * d + h * dh + j, dst = (size_t)h * 3 * dh + part * dh + j;
+                    const float sc = part == 0 ? qs : 1.0f;
+                    for (int k = 0; k < d; ++k) wr[dst * d + k] = wi[src * d + k] * sc;
+                    br[dst] = bi[src] * sc;
+                }
+        e.wqkv = p.f16_raw(wr.data(), wr.size()); e.bqkv = p.f32_raw(br.data(), br.size());
+        e.wo = p.f16(q + "self_att.att.out_proj.weight", (int64_t)d * d); e.bo = p.f32(q + "self_att.att.out_proj.bias", d);
+        e.ffn1_w1 = p.f16(q + "pos_ffn.ffn.0.weight", (int64_t)F * d); e.ffn1_b1 = p.f32(q + "pos_ffn.ffn.0.bias", F);
+        e.ffn1_w2 = p.f16(q + "pos_ffn.ffn.3.weight", (int64_t)d * F); e.ffn1_b2 = p.f32(q + "pos_ffn.ffn.3.bias", d);
     }
     for (int l = 0; l < c.num_encoder_layers && p.ok && c.encoder_module == SBK_ENC_CONFORMER; ++l) {
         const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".";
@@ -506,6 +569,16 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
         }
         W->rope_cos = p.f32_raw(cs.data(), cs.size());
         W->rope_sin = p.f32_raw(sn.data(), sn.size());
+    } else if (tfm) {  // Transformer.py:252-303 PositionalEncoding, fp32 like the reference's buffer
+        std::vector<float> pe((size_t)c.max_len * d);
+        for (int i = 0; i < d / 2; ++i) {
+            const float den = expf((float)(2 * i) * -(logf(10000.0f) / (float)d));
+            for (int t = 0; t < c.max_len; ++t) {
+                pe[(size_t)t * d + 2 * i] = sinf((float)t * den);
+                pe[(size_t)t * d + 2 * i + 1] = cosf((float)t * den);
+            }
+        }
+        W->enc_pe = p.f32_raw(pe.data(), pe.size());
     } else if (hypermix) {
         std::vector<float> pe((size_t)HM_PE_ROWS * d);
         hypermix_pe_table(d, pe.data());
@@ -778,6 +851,53 @@ static int run_branchformer_layers(AsrModel* m, int B, int T, const int* enc_len
     return layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, false, st);
 }
 
+// x [B*T, d] += pe[t]: TransformerASR.encode adds the absolute sine table to the input Linear's output (TransformerASR.py:519)
+__global__ void add_pos_table_kernel(float* __restrict__ x, const float* __restrict__ pe, int T, int d, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) x[i] += pe[(i / d) % T * d + i % d];
+}
+
+// Transformer layers (Transformer.py:311-490, normalize_before=True, regularMHA, Linear + GELU + Linear) on the fp32
+// residual stream b.x [B*T, d] -> enc_out = encoder.norm(x):
+//     x = x + out_proj(MHA(norm1(x)));  x = x + ffn(norm2(x))
+// The attention masks padded keys only (make_transformer_src_tgt_masks), so padded frames are computed like the reference.
+static int run_transformer_layers(AsrModel* m, int B, int T, const int* enc_len, float* enc_out, cudaStream_t st) {
+    const sbk_asr_config& c = m->wt->cfg;
+    AsrModel::Buf& b = m->b;
+    const int M = B * T, d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H;
+    SBK_REQUIRE(m->dyn_chunk == 0, "encode: the Transformer encoder has no chunked (DynChunkTrainConfig) mode");
+    const size_t n = (size_t)M * d;
+    add_pos_table_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(b.x, m->wt->enc_pe, T, d, n);
+    SBK_LAUNCH_CHECK();
+    GemmEpilogue e;
+    for (int l = 0; l < c.num_encoder_layers; ++l) {
+        const EncLayerW& w = m->wt->enc[l];
+        RC(layernorm_rows(b.x, b.h16, true, w.norm1_g, w.norm1_b, M, d, 1e-6f, false, st));
+        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bqkv; e.out = b.qkv16; e.ldo = 3 * d;
+        RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
+        // 1/sqrt(d_h) is folded into the query rows of wqkv / bqkv
+        RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, false, nullptr, nullptr, nullptr, 0, 1.0f, b.att16, d, st));
+        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bo; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
+        RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
+        RC(layernorm_rows(b.x, b.h16, true, w.norm2_g, w.norm2_b, M, d, 1e-6f, false, st));
+        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ACT_GELU; e.bias = w.ffn1_b1; e.out = b.f16; e.ldo = F;
+        RC(gemm_f16(b.h16, d, w.ffn1_w1, d, e, M, F, d, st));
+        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.ffn1_b2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
+        RC(gemm_f16(b.f16, F, w.ffn1_w2, F, e, M, d, F, st));
+    }
+    return layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, false, st);
+}
+
+// The fused front-end of the configured ConvolutionFrontEnd: feats [B, T0, n_mels] -> b.a_in [B*T2, input_size] fp16
+// (+ cnn_out_f fp32 when set).
+static int run_cnn(AsrModel* m, const float* feats, int B, int T0, float* cnn_out_f, cudaStream_t st) {
+    const sbk_asr_config& c = m->wt->cfg;
+    const AsrWeights& W = *m->wt;
+    if (c.cnn_blocks == 3) return cnn3_frontend_forward(feats, B, T0, c.n_mels, W.cnn3, m->b.act1, m->b.a_in, cnn_out_f, st);
+    return cnn_frontend_forward(feats, B, T0, c.n_mels, W.c1_w, W.c1_b, W.c1_g, W.c1_be, c.cnn_c1, W.c2_w, W.c2_b, W.c2_g,
+                                W.c2_be, c.cnn_c2, m->b.act1, m->b.a_in, cnn_out_f, st);
+}
+
 // feats [B, T0, n_mels] fp32 (already normalised) -> enc_out fp32 [B, T2, d] (+ enc16). enc_len device int[B].
 static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int* enc_len, float* cnn_out_f,
                        float* enc_out, cudaStream_t st) {
@@ -795,13 +915,12 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
                 "encode: HyperMixing has no chunked (DynChunkTrainConfig) mode");
     SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER || T > (c.kernel_size - 1) / 2,
                 "encode: the Branchformer's reflect-padded conv needs more than %d frames (got %d)", (c.kernel_size - 1) / 2, T);
-    if (feats != nullptr)
-        RC(cnn_frontend_forward(feats, B, T0, c.n_mels, m->wt->c1_w, m->wt->c1_b, m->wt->c1_g, m->wt->c1_be, c.cnn_c1, m->wt->c2_w, m->wt->c2_b,
-                                m->wt->c2_g, m->wt->c2_be, c.cnn_c2, b.act1, b.a_in, cnn_out_f, st));
+    if (feats != nullptr) RC(run_cnn(m, feats, B, T0, cnn_out_f, st));
     GemmEpilogue e;
     e.mode = EPI_F32; e.bias = m->wt->b_in; e.out = b.x; e.ldo = d;
     RC(gemm_f16(b.a_in, c.input_size, m->wt->w_in, c.input_size, e, M, d, c.input_size, st));
     if (c.encoder_module == SBK_ENC_BRANCHFORMER) return run_branchformer_layers(m, B, T, enc_len, enc_out, st);
+    if (c.encoder_module == SBK_ENC_TRANSFORMER) return run_transformer_layers(m, B, T, enc_len, enc_out, st);
     const float att_scale = 1.0f / sqrtf((float)d);  // nnet/attention.py:521,1272: 1/sqrt(embed_dim), not head_dim
     for (int l = 0; l < c.num_encoder_layers; ++l) {
         const EncLayerW& w = m->wt->enc[l];
@@ -1780,9 +1899,7 @@ int sbk_asr_cnn_forward(sbk_asr* mm, const float* feats_dev, int B, int T0, floa
     SBK_REQUIRE(m->wt->has_cnn, "cnn_forward: this handle was created without CNN weights");
     const int L = (T0 - 1) * c.hop;
     RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
-    return cnn_frontend_forward(feats_dev, B, T0, c.n_mels, m->wt->c1_w, m->wt->c1_b, m->wt->c1_g, m->wt->c1_be, c.cnn_c1, m->wt->c2_w, m->wt->c2_b,
-                                m->wt->c2_g, m->wt->c2_be, c.cnn_c2, m->b.act1, m->b.a_in, out_dev,
-                                static_cast<cudaStream_t>(stream));
+    return run_cnn(m, feats_dev, B, T0, out_dev, static_cast<cudaStream_t>(stream));
 }
 
 // src_dev: CNN output [B, T, input_size] fp32 -> enc_out_dev [B, T, d] fp32 (TransformerASR.encode)

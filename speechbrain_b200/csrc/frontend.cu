@@ -416,4 +416,258 @@ int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float*
     return SBK_OK;
 }
 
+// =========================================================================== 3-block front-end (Transformer recipes)
+// ConvolutionFrontEnd(num_blocks=3, num_layers_per_block=1, out_channels=(64, 64, 64), kernel_sizes=(5, 5, 1),
+// strides=(2, 2, 1), residuals=(False, False, True)):
+//   block 1: reflect-pad 2 + Conv2d(5x5, 1 -> 64, stride 2) + LayerNorm(F1, 64) + LeakyReLU      -> act1 fp16
+//   block 2: reflect-pad 2 + Conv2d(5x5, 64 -> 64, stride 2) + LayerNorm(F2, 64) + LeakyReLU     -> y (fp32, in smem)
+//   block 3: LeakyReLU(LayerNorm(Conv2d_1x1(y))) + LayerNorm(Conv2d_1x1 reduce_conv(y))          -> out [B, T2, F2*64]
+// Blocks 2 and 3 are one kernel: block 3 is per-pixel work plus a per-frame LayerNorm, so it runs on block 2's
+// LayerNorm output while that is still in shared memory, and only the 1280-wide row the input Linear reads is written.
+constexpr int K5_C = 64;                   // channels of every block
+constexpr int K5_FRAMES = 4;               // block-2 output frames per CTA
+constexpr int K5_WARPS = 5;                // 16 GEMM rows per warp: K5_FRAMES * F2 <= 80
+constexpr int K5_PROWS = 2 * K5_FRAMES + 3;  // act1 frames a CTA's patch holds
+constexpr int K5_CELL = 72;                // padded channel stride (halfs) of a patch cell
+constexpr int K5_WROW = 5 * K5_C + 8;      // padded weight row (halfs) of one kf slice: k = kt * 64 + ch
+constexpr int K5_YS = K5_C + 1;            // fp32 row stride of y
+constexpr int K5_ZS = 2 * K5_C + 1;        // fp32 row stride of the two block-3 convolutions
+
+// block 1: one warp per output frame, lane l owns channels 2l, 2l+1 (as conv1_ln_kernel, with 5x5 taps).
+// w1: [64, 5(kf), 5(kt)] fp32, g/be: [F1, 64].
+template <int MAXF>
+__global__ void __launch_bounds__(C1_WARPS * 32)
+conv1k5_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1, const float* __restrict__ w1,
+                  const float* __restrict__ b1, const float* __restrict__ gamma, const float* __restrict__ beta,
+                  __half* __restrict__ out_h) {
+    extern __shared__ float k5_in[];
+    const int FP = F0 + 4;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float* in = k5_in + warp * 5 * FP;  // [5][F0 + 4] of this warp's frame (reflect padded)
+    const int b = blockIdx.y, t1 = blockIdx.x * C1_WARPS + warp;
+    if (t1 >= T1) return;
+    for (int i = lane; i < 5 * FP; i += 32) {
+        const int kt = i / FP, fp = i - kt * FP;
+        const int t = reflect_idx(2 * t1 + kt - 2, T0);
+        const int f = reflect_idx(fp - 2, F0);
+        in[i] = __ldg(feats + (static_cast<size_t>(b) * T0 + t) * F0 + f);
+    }
+    const int c0 = 2 * lane;
+    float wa[25], wb[25];
+#pragma unroll
+    for (int i = 0; i < 25; ++i) { wa[i] = __ldg(w1 + c0 * 25 + i); wb[i] = __ldg(w1 + (c0 + 1) * 25 + i); }
+    const float ba = __ldg(b1 + c0), bb = __ldg(b1 + c0 + 1);
+    __syncwarp();
+    float va[MAXF], vb[MAXF];
+    float s = 0.0f;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1) {
+        va[f1] = 0.0f; vb[f1] = 0.0f;
+        if (f1 < F1) {
+            float a = ba, bq = bb;
+#pragma unroll
+            for (int kf = 0; kf < 5; ++kf)
+#pragma unroll
+                for (int kt = 0; kt < 5; ++kt) {
+                    const float x = in[kt * FP + 2 * f1 + kf];
+                    a = fmaf(wa[kf * 5 + kt], x, a);
+                    bq = fmaf(wb[kf * 5 + kt], x, bq);
+                }
+            va[f1] = a; vb[f1] = bq;
+            s += a + bq;
+        }
+    }
+    const float n = static_cast<float>(F1 * K5_C);
+    const float mean = warp_sum(s) / n;
+    float q = 0.0f;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1)
+        if (f1 < F1) {
+            const float da = va[f1] - mean, db = vb[f1] - mean;
+            q += da * da + db * db;
+        }
+    const float rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
+    const size_t obase = (static_cast<size_t>(b) * T1 + t1) * F1 * K5_C;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1)
+        if (f1 < F1) {
+            const int gi = f1 * K5_C + c0;
+            const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + gi));
+            const float2 be = __ldg(reinterpret_cast<const float2*>(beta + gi));
+            const float y0 = leaky((va[f1] - mean) * rstd * g.x + be.x);
+            const float y1 = leaky((vb[f1] - mean) * rstd * g.y + be.y);
+            *reinterpret_cast<__half2*>(out_h + obase + gi) = floats2half2_sat(y0, y1);
+        }
+}
+
+// LayerNorm over the n = F2 * 64 values of one frame held in smem rows [F2][stride] (columns col0 .. col0 + 63), one warp.
+__device__ __forceinline__ void k5_frame_stats(const float* src, int stride, int col0, int n, int lane, float& mean,
+                                               float& rstd) {
+    float s = 0.0f;
+    for (int i = lane; i < n; i += 32) s += src[(i >> 6) * stride + col0 + (i & 63)];
+    mean = warp_sum(s) / n;
+    float q = 0.0f;
+    for (int i = lane; i < n; i += 32) {
+        const float d = src[(i >> 6) * stride + col0 + (i & 63)] - mean;
+        q += d * d;
+    }
+    rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
+}
+
+// Bytes of the shared-memory region block 2 (patch + weight slice) and then block 3 (w3 + z) use.
+__host__ __device__ __forceinline__ size_t k5_shared_region(int F1, int F2) {
+    const size_t gemm = static_cast<size_t>(K5_PROWS) * (F1 + 4) * K5_CELL * 2 + K5_C * K5_WROW * 2;
+    const size_t blk3 = (2ull * K5_C * K5_YS + static_cast<size_t>(K5_FRAMES) * F2 * K5_ZS) * 4;
+    return ((gemm > blk3 ? gemm : blk3) + 15) & ~size_t(15);
+}
+
+// blocks 2 + 3.  act1 [B, T1, F1, 64] fp16; w2p [64, 1600] fp16 with k = (kf * 5 + kt) * 64 + ch; w3 [128, 64] fp32 rows
+// = [convs.conv_0 | reduce_conv.conv] output channels, b3 [128]; g2/be2, g3/be3, gr/ber: [F2, 64].
+// Block 2 is an implicit GEMM (M = K5_FRAMES * F2 pixels, N = 64, K = 1600) on mma.sync.m16n8k16 with fp16 operands and
+// fp32 accumulation; the weight slice of one kf (64 x 320) is staged per pass.  Block 3 runs in fp32.
+__global__ void __launch_bounds__(K5_WARPS * 32)
+cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int F2, const __half* __restrict__ w2p,
+                    const float* __restrict__ b2, const float* __restrict__ g2, const float* __restrict__ be2,
+                    const float* __restrict__ w3, const float* __restrict__ b3, const float* __restrict__ g3,
+                    const float* __restrict__ be3, const float* __restrict__ gr, const float* __restrict__ ber,
+                    __half* __restrict__ out_h, float* __restrict__ out_f) {
+    extern __shared__ __align__(16) uint8_t k5_smem[];
+    const int FPAD = F1 + 4;
+    __half* patch = reinterpret_cast<__half*>(k5_smem);              // [K5_PROWS][FPAD][K5_CELL]
+    __half* wsm = patch + K5_PROWS * FPAD * K5_CELL;                  // [64][K5_WROW]
+    // after block 2 the patch / weight region is free: block 3's weights and outputs reuse it
+    float* w3s = reinterpret_cast<float*>(k5_smem);                   // [128][K5_YS]
+    float* zs = w3s + 2 * K5_C * K5_YS;                               // [rows][K5_ZS]
+    const int rows = K5_FRAMES * F2;
+    float* ys = reinterpret_cast<float*>(k5_smem + k5_shared_region(F1, F2));  // [rows][K5_YS], behind both
+    const int b = blockIdx.y, t0 = blockIdx.x * K5_FRAMES;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    for (int i = threadIdx.x; i < K5_PROWS * FPAD * (K5_C / 8); i += blockDim.x) {
+        const int cell = i / (K5_C / 8), v8 = i - cell * (K5_C / 8);
+        const int tr = cell / FPAD, fp = cell - tr * FPAD;
+        int t = reflect_idx(2 * t0 + tr - 2, T1);
+        t = min(max(t, 0), T1 - 1);  // tail tiles: keep loads in range (results discarded)
+        const int f = reflect_idx(fp - 2, F1);
+        *reinterpret_cast<uint4*>(patch + cell * K5_CELL + v8 * 8) =
+            *reinterpret_cast<const uint4*>(act1 + ((static_cast<size_t>(b) * T1 + t) * F1 + f) * K5_C + v8 * 8);
+    }
+    const int g = lane >> 2, c = lane & 3;
+    const int r0 = warp * 16 + g, r1 = r0 + 8;
+    const int rr0 = min(r0, rows - 1), rr1 = min(r1, rows - 1);
+    const int fr0 = rr0 / F2, f20 = rr0 - fr0 * F2;
+    const int fr1 = rr1 / F2, f21 = rr1 - fr1 * F2;
+    const bool active = warp * 16 < rows;
+    float acc[8][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.0f;
+#pragma unroll 1
+    for (int kf = 0; kf < 5; ++kf) {
+        __syncthreads();  // the previous slice is consumed (kf == 0: nothing to wait for but the patch)
+        for (int i = threadIdx.x; i < K5_C * (5 * K5_C / 8); i += blockDim.x) {
+            const int o = i / (5 * K5_C / 8), v8 = i - o * (5 * K5_C / 8);
+            *reinterpret_cast<uint4*>(wsm + o * K5_WROW + v8 * 8) =
+                *reinterpret_cast<const uint4*>(w2p + static_cast<size_t>(o) * 25 * K5_C + kf * 5 * K5_C + v8 * 8);
+        }
+        __syncthreads();
+        if (active) {
+#pragma unroll  // a rolled kt loop inside the rolled kf loop kept one loop counter in local memory (8-byte spill)
+            for (int kt = 0; kt < 5; ++kt) {
+                const __half* a0p = patch + ((2 * fr0 + kt) * FPAD + 2 * f20 + kf) * K5_CELL + 2 * c;
+                const __half* a1p = patch + ((2 * fr1 + kt) * FPAD + 2 * f21 + kf) * K5_CELL + 2 * c;
+#pragma unroll
+                for (int ks = 0; ks < K5_C / 16; ++ks) {
+                    uint32_t a[4];
+                    a[0] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16);
+                    a[1] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16);
+                    a[2] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16 + 8);
+                    a[3] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16 + 8);
+                    const int kk = kt * K5_C + ks * 16 + 2 * c;
+#pragma unroll
+                    for (int nt = 0; nt < 8; ++nt) {
+                        uint32_t bb[2];
+                        const __half* wp = wsm + (nt * 8 + g) * K5_WROW + kk;
+                        bb[0] = *reinterpret_cast<const uint32_t*>(wp);
+                        bb[1] = *reinterpret_cast<const uint32_t*>(wp + 8);
+                        mma_16816(acc[nt], a, bb);
+                    }
+                }
+            }
+        }
+    }
+    if (active) {
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+            const int col = nt * 8 + 2 * c;
+            const float bz0 = __ldg(b2 + col), bz1 = __ldg(b2 + col + 1);
+            if (r0 < rows) { ys[r0 * K5_YS + col] = acc[nt][0] + bz0; ys[r0 * K5_YS + col + 1] = acc[nt][1] + bz1; }
+            if (r1 < rows) { ys[r1 * K5_YS + col] = acc[nt][2] + bz0; ys[r1 * K5_YS + col + 1] = acc[nt][3] + bz1; }
+        }
+    }
+    __syncthreads();
+    // block 2's LayerNorm + LeakyReLU in place (one warp per frame); block 3's weights into the freed region
+    for (int i = threadIdx.x; i < 2 * K5_C * K5_C; i += blockDim.x) w3s[(i >> 6) * K5_YS + (i & 63)] = __ldg(w3 + i);
+    const int n = F2 * K5_C;
+    if (warp < K5_FRAMES) {
+        float* src = ys + warp * F2 * K5_YS;
+        float mean, rstd;
+        k5_frame_stats(src, K5_YS, 0, n, lane, mean, rstd);
+        for (int i = lane; i < n; i += 32) {
+            float& v = src[(i >> 6) * K5_YS + (i & 63)];
+            v = leaky((v - mean) * rstd * __ldg(g2 + i) + __ldg(be2 + i));
+        }
+    }
+    __syncthreads();
+    // block 3's two 1x1 convolutions: z[r][0:64] = convs.conv_0(y[r]), z[r][64:128] = reduce_conv.conv(y[r])
+    for (int i = threadIdx.x; i < rows * 2 * K5_C; i += blockDim.x) {
+        const int r = i >> 7, o = i & 127;
+        const float* yr = ys + r * K5_YS;
+        const float* wr = w3s + o * K5_YS;
+        float z = __ldg(b3 + o);
+#pragma unroll 8
+        for (int k = 0; k < K5_C; ++k) z = fmaf(wr[k], yr[k], z);
+        zs[r * K5_ZS + o] = z;
+    }
+    __syncthreads();
+    if (warp < K5_FRAMES) {
+        const int t = t0 + warp;
+        if (t < T2) {
+            const float* src = zs + warp * F2 * K5_ZS;
+            float ma, ra, mr, rr;
+            k5_frame_stats(src, K5_ZS, 0, n, lane, ma, ra);
+            k5_frame_stats(src, K5_ZS, K5_C, n, lane, mr, rr);
+            const size_t ob = (static_cast<size_t>(b) * T2 + t) * n;
+            for (int i = lane; i < n; i += 32) {
+                const float* zr = src + (i >> 6) * K5_ZS + (i & 63);
+                const float y = leaky((zr[0] - ma) * ra * __ldg(g3 + i) + __ldg(be3 + i)) +
+                                ((zr[K5_C] - mr) * rr * __ldg(gr + i) + __ldg(ber + i));
+                out_h[ob + i] = float2half_sat(y);
+                if (out_f) out_f[ob + i] = y;
+            }
+        }
+    }
+}
+
+int cnn3_frontend_forward(const float* feats, int B, int T0, int F0, const Cnn3Weights& w, __half* act1_h, __half* out_h,
+                          float* out_f, cudaStream_t stream) {
+    const int T1 = (T0 - 1) / 2 + 1, F1 = (F0 - 1) / 2 + 1;
+    const int T2 = (T1 - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
+    // the reference's reflect padding of 2 needs 3 rows / columns at both strided convolutions
+    SBK_REQUIRE(T1 >= 3 && F1 >= 3, "cnn_frontend: the 5x5 reflect padding needs at least 5 frames and 5 features "
+                "(got %d frames, %d features)", T0, F0);
+    SBK_REQUIRE(F1 <= 64 && K5_FRAMES * F2 <= 16 * K5_WARPS, "cnn_frontend: feature dim too large (F0=%d)", F0);
+    {
+        const size_t smem = static_cast<size_t>(C1_WARPS) * 5 * (F0 + 4) * sizeof(float);
+        conv1k5_ln_kernel<64><<<dim3(ceil_div(T1, C1_WARPS), B), C1_WARPS * 32, smem, stream>>>(
+            feats, T0, F0, T1, F1, w.w1, w.b1, w.g1, w.be1, act1_h);
+        SBK_LAUNCH_CHECK();
+    }
+    const size_t smem = k5_shared_region(F1, F2) + static_cast<size_t>(K5_FRAMES) * F2 * K5_YS * 4;
+    SBK_CUDA_CHECK(cudaFuncSetAttribute(cnn3_block23_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cnn3_block23_kernel<<<dim3(ceil_div(T2, K5_FRAMES), B), K5_WARPS * 32, smem, stream>>>(
+        act1_h, T1, F1, T2, F2, w.w2p, w.b2, w.g2, w.be2, w.w3, w.b3, w.g3, w.be3, w.gr, w.ber, out_h, out_f);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
 }  // namespace sbk

@@ -72,8 +72,10 @@ class FbankHandle:
 class AsrEngine:
     """One repacked model on one GPU.  ``cfg`` keys: n_fft, hop, win (samples), n_mels, cnn_channels, input_size,
     d_model, nhead, num_encoder_layers, num_decoder_layers, d_ffn, vocab, kernel_size, attention_type
-    ("RoPEMHA"|"RelPosMHAXL"|"hypermixing", the last with the Conformer only), decoder_activation ("gelu"|"relu"), max_length; encoder_module ("conformer" (default) |
-    "branchformer") with csgu_linear_units and branchformer_activation ("gelu" (default) | "relu").
+    ("RoPEMHA"|"RelPosMHAXL"|"hypermixing"|"regularMHA", hypermixing with the Conformer only, regularMHA with the Transformer
+    only), decoder_activation ("gelu"|"relu"), max_length; encoder_module ("conformer" (default) | "branchformer" |
+    "transformer") with csgu_linear_units and branchformer_activation ("gelu" (default) | "relu"); cnn_blocks (2 (default),
+    or 3: the Transformer recipes' front-end, cnn_channels (64, 64)).
     ``state``: {reference key with recipe prefix: CPU fp32 tensor}."""
 
     def __init__(self, cfg, state, device="cuda", parts=("fbank", "cnn", "encoder", "decoder")):
@@ -87,15 +89,19 @@ class AsrEngine:
         c.num_encoder_layers, c.num_decoder_layers = cfg["num_encoder_layers"], cfg["num_decoder_layers"]
         c.d_ffn, c.vocab, c.kernel_size = cfg["d_ffn"], cfg["vocab"], cfg.get("kernel_size", 31)
         att = cfg["attention_type"]
-        att_types = {"RoPEMHA": _lib.SBK_ATT_ROPE, "RelPosMHAXL": _lib.SBK_ATT_RELPOS, "hypermixing": _lib.SBK_ATT_HYPERMIX}
+        att_types = {"RoPEMHA": _lib.SBK_ATT_ROPE, "RelPosMHAXL": _lib.SBK_ATT_RELPOS, "hypermixing": _lib.SBK_ATT_HYPERMIX,
+                     "regularMHA": _lib.SBK_ATT_REGULAR}
         if att not in att_types:
-            raise NotImplementedError(f"attention_type={att!r}: only RoPEMHA, RelPosMHAXL and hypermixing are built")
+            raise NotImplementedError(f"attention_type={att!r}: only RoPEMHA, RelPosMHAXL, hypermixing and regularMHA are built")
         c.attention_type = att_types[att]
         c.decoder_activation = _lib.SBK_ACT_GELU if cfg.get("decoder_activation", "gelu") == "gelu" else _lib.SBK_ACT_RELU
         c.max_len = cfg.get("max_length", 2500)
         enc_module = cfg.get("encoder_module", "conformer")
-        if enc_module not in ("conformer", "branchformer"):
-            raise NotImplementedError(f"encoder_module={enc_module!r}: only conformer and branchformer are built")
+        if enc_module not in ("conformer", "branchformer", "transformer"):
+            raise NotImplementedError(f"encoder_module={enc_module!r}: only conformer, branchformer and transformer are built")
+        if enc_module == "transformer":
+            c.encoder_module = _lib.SBK_ENC_TRANSFORMER
+        c.cnn_blocks = cfg.get("cnn_blocks", 2)
         if enc_module == "branchformer":
             c.encoder_module, c.csgu_linear_units = _lib.SBK_ENC_BRANCHFORMER, cfg["csgu_linear_units"]
             c.branchformer_activation = (_lib.SBK_ACT_GELU if cfg.get("branchformer_activation", "gelu") == "gelu"

@@ -75,6 +75,7 @@ class EngineSlot:
                 sd.update({prefix + k: v for k, v in src.state_dict().items()})
                 if prefix == "CNN.":
                     cfg["cnn_channels"] = tuple(src.out_channels)
+                    cfg["cnn_blocks"] = src.num_blocks  # the front-end actually wired to the model
         return cfg, sd
 
     def get(self, device, parts, sources=None):

@@ -3,7 +3,8 @@
 encoder_module="conformer" with attention_type in {"RoPEMHA", "RelPosMHAXL", "hypermixing"} and normalize_before=True
 (hypermixing: HyperMixing token mixing, nnet/hypermixing.py, with head width d_model / nhead of 32 or 64 and
 d_ffn / nhead a multiple of 16 up to 256), or encoder_module="branchformer" with attention_type="RelPosMHAXL"
-(Branchformer.py:92-410); causal=False.
+(Branchformer.py:92-410), or encoder_module="transformer" with attention_type="regularMHA",
+positional_encoding="fixed_abs_sine" and normalize_before=True (Transformer.py:311-490, head width 64 or 128); causal=False.
 
 Same constructor kwargs, same state_dict keys (incl. the positional buffers), ``encode()`` on the sm_90a
 kernels.  ``decode()`` / ``forward()`` run teacher-forced on the KV-cached decoder step (the searchers in
@@ -49,9 +50,18 @@ class TransformerASR(torch.nn.Module):
         if causal is None:
             causal = True  # the reference warns and assumes True (TransformerASR.py:274-282)
         unsupported = []
-        if encoder_module not in ("conformer", "branchformer"):
+        if encoder_module not in ("conformer", "branchformer", "transformer"):
             unsupported.append(f"encoder_module={encoder_module!r}")
-        if attention_type not in ("RoPEMHA", "RelPosMHAXL", "hypermixing"):
+        if encoder_module == "transformer":
+            if attention_type != "regularMHA":
+                unsupported.append(f"Transformer encoder with attention_type={attention_type!r} (regularMHA only)")
+            if not normalize_before:
+                unsupported.append("Transformer encoder with normalize_before=False (post-norm)")
+            if positional_encoding != "fixed_abs_sine":
+                unsupported.append(f"Transformer encoder with positional_encoding={positional_encoding!r}")
+            if d_model % nhead or d_model // nhead not in (128, 64):
+                unsupported.append(f"Transformer encoder head_dim={d_model // max(nhead, 1)} (128 or 64)")
+        elif attention_type not in ("RoPEMHA", "RelPosMHAXL", "hypermixing"):
             unsupported.append(f"attention_type={attention_type!r}")
         if attention_type == "hypermixing" and encoder_module == "conformer":
             if d_model % nhead or d_model // nhead not in (64, 32):
@@ -82,7 +92,7 @@ class TransformerASR(torch.nn.Module):
             unsupported.append("output_hidden_states=True")
         if encoder_module == "conformer" and conformer_activation is not None and getattr(conformer_activation, "__name__", "") not in ("Swish", "SiLU"):
             unsupported.append("conformer_activation other than Swish")
-        if d_model % nhead or d_model // nhead not in (64, 36, 32):
+        if encoder_module != "transformer" and (d_model % nhead or d_model // nhead not in (64, 36, 32)):
             unsupported.append(f"head_dim={d_model // max(nhead, 1)} (64, 36 or 32)")
         if d_model % 16:
             unsupported.append("d_model not a multiple of 16")
@@ -116,14 +126,17 @@ class TransformerASR(torch.nn.Module):
             for i in range(num_encoder_layers):
                 getattr(self.encoder.layers, str(i)).mha_layer.add_module("positional_encoding", _Node())
                 getattr(self.encoder.layers, str(i)).mha_layer.positional_encoding.register_buffer("pe", pe_hm)
-        else:
+        elif attention_type != "regularMHA":  # with regularMHA the decoder adds positional_encoding, as HyperMixing's does
             self.positional_encoding_decoder = _Node()
             self.positional_encoding_decoder.register_buffer("pe", _sine_table(max_length, d_model))
         # engine slots (plain dict, not sub-modules): one shared device engine per set of modules wired to this model
         object.__setattr__(self, "_slots", {})
 
     def engine_cfg(self):
-        return dict(n_fft=400, hop=160, win=400, n_mels=80, cnn_channels=(64, 32), input_size=self.input_size,
+        # the front-end each encoder's recipes pair it with: the 3-block one for the Transformer, else the 2-block one
+        tfm = self.encoder_module == "transformer"
+        return dict(n_fft=400, hop=160, win=400, n_mels=80, cnn_channels=(64, 64) if tfm else (64, 32),
+                    cnn_blocks=3 if tfm else 2, input_size=self.input_size,
                     d_model=self.d_model, nhead=self.nhead, num_encoder_layers=self.num_encoder_layers,
                     num_decoder_layers=self.num_decoder_layers, d_ffn=self.d_ffn, vocab=self.tgt_vocab,
                     kernel_size=self.kernel_size, attention_type=self.attention_type,
@@ -172,6 +185,8 @@ class TransformerASR(torch.nn.Module):
         if src.dim() == 4:
             bz, t, ch1, ch2 = src.shape
             src = src.reshape(bz, t, ch1 * ch2)
+        if self.encoder_module == "transformer" and dynchunktrain_config is not None:
+            raise NotImplementedError("TransformerASR: the Transformer encoder's chunked (streaming-equivalent) mode is not built")
         if self.encoder_module == "branchformer":
             assert dynchunktrain_config is None, "Dynamic Chunk Training unsupported for this encoder"
             halo = (self.kernel_size - 1) // 2
@@ -203,6 +218,8 @@ class TransformerASR(torch.nn.Module):
     # ------------------------------------------------------------------ streaming (TransformerASR.py:546-670)
     def make_streaming_context(self, dynchunktrain_config):
         """Streaming context for ``encode_streaming`` (TransformerASR.py:645-670)."""
+        if self.encoder_module == "transformer":
+            raise NotImplementedError("TransformerASR: streaming for the Transformer encoder is not built")
         if self.encoder_module == "branchformer":
             raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
         if self.attention_type == "hypermixing":
@@ -220,6 +237,8 @@ class TransformerASR(torch.nn.Module):
         *inputs* seen so far in the context and re-runs that masked encode over the window the new chunk can depend on
         (12 layers x (left context + convolution halo); everything, for an infinite left context), returning the rows of the
         new chunk: the same values, at the cost of recomputing the window instead of reusing per-layer caches."""
+        if self.encoder_module == "transformer":
+            raise NotImplementedError("TransformerASR: streaming for the Transformer encoder is not built")
         if self.encoder_module == "branchformer":
             raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
         if self.attention_type == "hypermixing":

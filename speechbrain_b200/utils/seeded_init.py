@@ -128,3 +128,9 @@ CONFORMER_SMALL = dict(name="conformer_small", sample_rate=16000, n_fft=400, win
                        cnn_channels=(64, 32), input_size=640, d_model=144, nhead=4, num_encoder_layers=12,
                        num_decoder_layers=4, d_ffn=1024, vocab=5000, kernel_size=31, attention_type="RelPosMHAXL",
                        decoder_activation="gelu", max_length=2500)
+# recipes/LibriSpeech/ASR/transformer/hparams/transformer.yaml: the 3-block front-end (5x5 / 5x5 / 1x1 + residual, 64
+# channels), 12 pre-norm Transformer encoder layers with regularMHA (4 heads of 128), 6 decoder layers, 5000 tokens
+TRANSFORMER_LARGE = dict(name="transformer_large", sample_rate=16000, n_fft=400, win=400, hop=160, n_mels=80,
+                         cnn_channels=(64, 64), cnn_blocks=3, input_size=1280, d_model=512, nhead=4, num_encoder_layers=12,
+                         num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="regularMHA",
+                         decoder_activation="gelu", max_length=2500, encoder_module="transformer")
