@@ -138,6 +138,25 @@ int sbk_ctc_prefix_test(const float* logits_dev, const int* enc_len_dev, int B, 
 int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev, const float* ln_b_dev, const float* taps_dev,
                   const float* bias_dev, int K, void* out_dev, void* stream);
 
+/* the encoder self-attention kernel alone, in the engine's layouts: qkv_dev [B*T, 3*H*head_dim] fp16 in per-head
+ * [q | k | v] blocks; lens_dev [B] valid frames (NULL: all T; keys j >= lens[b] are masked, padded query rows are computed
+ * like any other row).  relpos == 0 (RoPE / regularMHA): scores = q.k, q already scaled, scale unused.  relpos != 0
+ * (RelPosMHAXL, head_dim <= 64): scores = ((q+u).k + (q+v).P[|i-j|]) * scale with pos_u_dev / pos_v_dev [H*head_dim] fp32
+ * and P_dev [T, H*head_dim] fp16 (row r = linear_pos of relative distance r).  chunk > 0: Dynamic Chunk attention, query i
+ * sees keys [max(0, (i/chunk - left_chunks) * chunk), min(len, (i/chunk + 1) * chunk)), left_chunks < 0 = the whole past.
+ * A row that sees no key is 0.  out_dev [B*T, H*head_dim] fp16.  Synchronises the stream. */
+int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int head_dim, const int* lens_dev, int relpos,
+                               const float* pos_u_dev, const float* pos_v_dev, const void* P_dev, float scale, int chunk,
+                               int left_chunks, void* out_dev, void* stream);
+
+/* the Conformer convolution module's depthwise conv + LayerNorm + Swish alone (Conformer.py:314-330): x_dev [B*T, D] fp32
+ * (the GLU output) -> out_dev [B*T, D] fp16 = SiLU(LayerNorm(Conv1d_K(x) + bias)), eps 1e-5, zero padding outside [0, T)
+ * only (padded frames inside T are inputs).  taps_dev in the reference layout [D, 1, K], bias / ln_g / ln_b [D] fp32; odd K,
+ * D % 4 == 0, D <= 1024.  chunk > 0: Dynamic Chunk Convolution (inputs past the end of the output frame's chunk are zero).
+ * Allocates and frees its own scratch and synchronises the stream. */
+int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
+                    const float* ln_g_dev, const float* ln_b_dev, int chunk, void* out_dev, void* stream);
+
 /* the HyperConformer's HyperMixing block alone (HyperMixing.forward, nnet/hypermixing.py:90-195, tied=False, nhead heads of
  * e = d / nhead in {32, 64} channels, k = d_ffn / nhead a multiple of 16 up to 256): x_dev [B*T, d] fp16 (the norm1 output),
  * lens_dev [B] valid frames (NULL: all T; frames t >= lens[b] are the key_padding_mask) -> out_dev [B*T, d] fp32 =

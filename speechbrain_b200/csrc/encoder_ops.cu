@@ -417,6 +417,12 @@ int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* w
     return SBK_OK;
 }
 
+// (D, 1, K) reference taps -> tap-major [K, D] (the layout dwconv_ln_swish reads)
+void dwconv_repack_taps(const float* src, int D, int K, float* dst) {
+    for (int ch = 0; ch < D; ++ch)
+        for (int k = 0; k < K; ++k) dst[static_cast<size_t>(k) * D + ch] = src[static_cast<size_t>(ch) * K + k];
+}
+
 // --------------------------------------------------------------------------- CSGU (Branchformer convolution branch)
 // ConvolutionalSpatialGatingUnit.forward (lobes/models/convolution.py:22-113) on u = GELU(pre_channel_proj(x)) [B*T, C] fp16:
 //     a, b = u[:, :C/2], u[:, C/2:]          (x.chunk(2, dim=-1): the first half gates)
@@ -570,11 +576,17 @@ void csgu_repack_taps(const float* src, int C2, int K, float* dst) {
 //        (2T-1)-row table and rel_shifts it (:537-553); row r of the table depends only on |r| (RelPosEncXL
 //        :360-408 uses +sin for both halves), so BD[i,j] = (q_i+v).P[|i-j|] with P = linear_pos(pe[0..T-1]).
 //        Per key block each warp computes the 16 x 80 band G = Qv.Pband^T on tensor cores, parks it in
-//        shared memory and re-reads it diagonally shifted.
+//        shared memory and re-reads it diagonally shifted.  The four warps' bands of key block j0 read
+//        P[min(|a + x|, T - 1)], x in [0, 128), a = i0 - j0 - 63.  That window moves down by 64 rows per key
+//        block: a 192-row ring holds it, and each key block's 64 new rows stream in (cp.async) while the block
+//        before it is multiplied, so shared memory does not grow with T.
 //  Padded *query* rows are computed like any other row (the reference does; they leak into valid frames
 //  through the depthwise conv), only padded *keys* are masked.
 constexpr int ATT_BQ = 64;
 constexpr int ATT_BK = 64;
+constexpr int ATT_GW = 80;                      // relpos band width per warp (16 + 64 - 1 rounded to 8)
+constexpr int ATT_PW = ATT_BQ - 16 + ATT_GW;    // relpos P window rows per key block: 4 warp bands, 16 rows apart
+constexpr int ATT_PR = ATT_PW + ATT_BK;         // relpos P ring rows: one block's window + the next block's new rows
 
 __device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, const void* p) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(smem_u32(p)));
@@ -614,15 +626,15 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
                          int chunk, int left_chunks) {
     constexpr int STR = DHP + 8;  // padded row stride (halfs): conflict-free fragment loads
     constexpr int KS = DHP / 16;
-    constexpr int GW = 80;        // relpos band width (16 + 64 - 1 rounded to 8)
+    constexpr int GW = ATT_GW;
     constexpr int VPR = DH / 4;   // 8-byte vectors per row (DH % 4 == 0)
     extern __shared__ __align__(16) uint8_t att_smem[];
     __half* Qs = reinterpret_cast<__half*>(att_smem);  // [64][STR]   (RELPOS: Qu)
     __half* Ks = Qs + ATT_BQ * STR;                    // [64][STR]
     __half* Vs = Ks + ATT_BK * STR;                    // [64][STR]
     __half* Qv = Vs + ATT_BK * STR;                    // RELPOS: [64][STR]
-    __half* Ps = Qv + ATT_BQ * STR;                    // RELPOS: [T][STR]
-    float* Gs = reinterpret_cast<float*>(Ps + (RELPOS ? T : 0) * STR);  // RELPOS: [4 warps][16][GW+1]
+    __half* Ps = Qv + ATT_BQ * STR;                    // RELPOS: [ATT_PR][STR] ring of P rows (p_slot)
+    float* Gs = reinterpret_cast<float*>(Ps + (RELPOS ? ATT_PR : 0) * STR);  // RELPOS: [4 warps][16][GW+1]
     // head dims that are whole 16-byte vectors: K/V blocks are double-buffered with cp.async (block jb+1 streams in while
     // block jb is multiplied); the second buffer pair sits behind everything else
     constexpr bool ASYNC = (DH % 8 == 0) && (DHP == DH);
@@ -635,13 +647,13 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
 
     if constexpr (DHP != DH) {  // zero the padding columns once (they take part in the k-loop / PV n-tiles)
         constexpr int PADC = DHP - DH;
-        const int n_rows_pad = 4 * ATT_BQ + (RELPOS ? T : 0);
+        const int n_rows_pad = 4 * ATT_BQ + (RELPOS ? ATT_PR : 0);
         for (int i = threadIdx.x; i < n_rows_pad * PADC; i += blockDim.x) {
             const int r = i / PADC, cc = i - r * PADC;
             Qs[r * STR + DH + cc] = __float2half(0.0f);  // Qs, Ks, Vs, Qv, Ps are contiguous with the same stride
         }
     }
-    // ---- stage Q (and RELPOS: Qu/Qv, P_h)
+    // ---- stage Q (RELPOS: Qu/Qv)
     for (int i = threadIdx.x; i < ATT_BQ * VPR; i += blockDim.x) {
         const int r = i / VPR, v4 = i - r * VPR;
         uint2 val = make_uint2(0, 0);
@@ -659,13 +671,6 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
             *reinterpret_cast<uint2*>(Qv + r * STR + v4 * 4) = *reinterpret_cast<uint2*>(qv);
         } else {
             *reinterpret_cast<uint2*>(Qs + r * STR + v4 * 4) = val;
-        }
-    }
-    if constexpr (RELPOS) {
-        for (int i = threadIdx.x; i < T * VPR; i += blockDim.x) {
-            const int r = i / VPR, v4 = i - r * VPR;
-            *reinterpret_cast<uint2*>(Ps + r * STR + v4 * 4) =
-                *reinterpret_cast<const uint2*>(P + static_cast<size_t>(r) * ldp + h * DH + v4 * 4);
         }
     }
     __syncthreads();
@@ -715,6 +720,17 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
         }
     }
 
+    // RELPOS: the band of key block jb reads P[min(|v|, T - 1)] for v = a + x, x in [0, ATT_PW), a = i0 - j0 - (ATT_BK - 1);
+    // row v lives in ring slot v mod ATT_PR.  Block jb + 1's window is block jb's moved down by ATT_BK rows, so after the
+    // first block only its ATT_BK new rows [a, a + ATT_BK) are staged.  They take the slots of rows
+    // [a + ATT_PR, a + ATT_PR + ATT_BK), which lie above the window of the block before it (the one being multiplied while
+    // they stream in).
+    auto p_first = [&](int jb) { return i0 - jb * ATT_BK - (ATT_BK - 1); };
+    auto p_slot = [](int v) {
+        const int s = v % ATT_PR;
+        return s < 0 ? s + ATT_PR : s;
+    };
+    auto p_src = [&](int v) { return P + static_cast<size_t>(min(v < 0 ? -v : v, T - 1)) * ldp + h * DH; };
     auto stage_async = [&](int jb, __half* kd, __half* vd) {  // 16-byte cp.async, rows >= T zero-filled
         const int j0 = jb * ATT_BK;
         constexpr int V8 = DH / 8;
@@ -728,10 +744,29 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(vd + r * STR + v8 * 8)),
                          "l"(rowp + 2 * DH), "r"(nbytes) : "memory");
         }
+        if constexpr (RELPOS) {
+            const int a = p_first(jb), n = jb == blk_begin ? ATT_PW : ATT_BK;
+            for (int i = threadIdx.x; i < n * V8; i += blockDim.x) {
+                const int x = i / V8, v8 = i - x * V8;
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(Ps + p_slot(a + x) * STR + v8 * 8)),
+                             "l"(p_src(a + x) + v8 * 8) : "memory");
+            }
+        }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
-    if constexpr (ASYNC) {
-        if (n_blk > blk_begin) stage_async(blk_begin, Ks, Vs);
+    // RELPOS without 16-byte rows: only the P rows go through cp.async, in 8-byte pieces, one key block ahead
+    auto stage_p8 = [&](int jb) {
+        const int a = p_first(jb), n = jb == blk_begin ? ATT_PW : ATT_BK;
+        for (int i = threadIdx.x; i < n * VPR; i += blockDim.x) {
+            const int x = i / VPR, v4 = i - x * VPR;
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(Ps + p_slot(a + x) * STR + v4 * 4)),
+                         "l"(p_src(a + x) + v4 * 4) : "memory");
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    if (n_blk > blk_begin) {
+        if constexpr (ASYNC) stage_async(blk_begin, Ks, Vs);
+        else if constexpr (RELPOS) stage_p8(blk_begin);
     }
 
     for (int jb = blk_begin; jb < n_blk; ++jb) {
@@ -747,7 +782,11 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
                 else stage_async(jb + 1, KV1, KV1 + ATT_BK * STR);
             }
         } else {
-            __syncthreads();  // previous block's K/V fully consumed
+            if constexpr (RELPOS) asm volatile("cp.async.wait_group 0;" ::: "memory");
+            __syncthreads();  // previous block's K/V fully consumed (RELPOS: block jb's P rows have landed for everyone)
+            if constexpr (RELPOS) {
+                if (jb + 1 < n_blk) stage_p8(jb + 1);
+            }
             for (int i = threadIdx.x; i < ATT_BK * VPR; i += blockDim.x) {
                 const int r = i / VPR, v4 = i - r * VPR;
                 uint2 kv = make_uint2(0, 0), vv = make_uint2(0, 0);
@@ -782,16 +821,14 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
             }
         }
         if constexpr (RELPOS) {
-            // band G[li][rr] = Qv[li] . P[|rmin + rr|], rr in [0, 80): rmin = iw - j0 - 63
+            // band G[li][rr] = Qv[li] . P[|rmin + rr|], rr in [0, 80): rmin = iw - j0 - 63 = a + warp * 16
+            // (rows past T - 1 repeat row T - 1: columns outside the band that are never read back)
             float* Gw = Gs + warp * 16 * (GW + 1);
-            const int rmin = (i0 + warp * 16) - j0 - (ATT_BK - 1);
+            const int rmin = p_first(jb) + warp * 16;
 #pragma unroll 1
             for (int nt = 0; nt < GW / 8; ++nt) {
                 float gacc[4] = {0.f, 0.f, 0.f, 0.f};
-                int pr = rmin + nt * 8 + g;
-                pr = pr < 0 ? -pr : pr;
-                pr = min(pr, T - 1);  // columns outside the band that are never read back
-                const __half* pp = Ps + pr * STR + 2 * c;
+                const __half* pp = Ps + p_slot(rmin + nt * 8 + g) * STR + 2 * c;
 #pragma unroll
                 for (int ks = 0; ks < KS; ++ks)
                     mma16816(gacc, qva[ks], *reinterpret_cast<const uint32_t*>(pp + ks * 16),
@@ -909,14 +946,18 @@ static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int
         auto kern = encoder_attention_kernel<DH, DHP, false>;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, nullptr, nullptr, nullptr, 0, scale, out, ldo, chunk, left_chunks);
-    } else if constexpr (DH > 64) {  // the RelPos band and P_h table are built for head widths up to 64
+    } else if constexpr (DH > 64) {  // the RelPos band and P window are built for head widths up to 64
         set_error("encoder_attention: RelPosMHAXL with head_dim=%d not built", DH);
         return SBK_ERR_UNSUPPORTED;
     } else {
-        SBK_REQUIRE(ldp % 4 == 0, "encoder_attention: bad ldp");
-        const size_t smem = 4ull * ATT_BQ * STR * 2 + static_cast<size_t>(T) * STR * 2 + 4ull * 16 * 81 * 4 +
-                            2ull * ATT_BK * STR * 2;
-        SBK_REQUIRE(smem <= 220 * 1024, "encoder_attention(RelPos): T=%d too long for the shared-memory table", T);
+        constexpr bool ASYNC = (DH % 8 == 0) && (DHP == DH);  // as in the kernel: a second K/V buffer pair
+        if (ASYNC)
+            SBK_REQUIRE(ldp % 8 == 0 && (reinterpret_cast<uintptr_t>(P) & 15) == 0, "encoder_attention: P must be 16-byte aligned");
+        else
+            SBK_REQUIRE(ldp % 4 == 0 && (reinterpret_cast<uintptr_t>(P) & 7) == 0, "encoder_attention: P must be 8-byte aligned");
+        // independent of T: 101 KB at head_dim 64 (two CTAs per SM), 69 KB at 36 and 65 KB at 32 (three)
+        const size_t smem = (4ull * ATT_BQ + ATT_PR) * STR * 2 + 4ull * 16 * (ATT_GW + 1) * 4 +
+                            (ASYNC ? 2ull * ATT_BK * STR * 2 : 0);
         auto kern = encoder_attention_kernel<DH, DHP, true>;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks);

@@ -539,8 +539,7 @@ int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weigh
             const float* src = find(w, q + "convolution_module.conv.weight", (int64_t)d * K);
             if (!src) { p.ok = false; break; }
             std::vector<float> wt((size_t)K * d);
-            for (int ch = 0; ch < d; ++ch)
-                for (int k = 0; k < K; ++k) wt[(size_t)k * d + ch] = src[(size_t)ch * K + k];
+            dwconv_repack_taps(src, d, K, wt.data());
             e.wdw = p.f32_raw(wt.data(), wt.size());
         }
         e.bdw = p.f32(q + "convolution_module.conv.bias", d);
@@ -1801,6 +1800,41 @@ int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev,
     if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("csgu_test: device error"); rc = SBK_ERR_CUDA; }
     cudaFree(taps);
     cudaFree(stats);
+    return rc;
+}
+
+int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int head_dim, const int* lens_dev, int relpos,
+                               const float* pos_u_dev, const float* pos_v_dev, const void* P_dev, float scale, int chunk,
+                               int left_chunks, void* out_dev, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(qkv_dev && out_dev && (!relpos || (pos_u_dev && pos_v_dev && P_dev)), "encoder_attention_test: null pointer");
+    SBK_REQUIRE(B >= 1 && T >= 1 && H >= 1 && head_dim >= 1, "encoder_attention_test: bad sizes B=%d T=%d H=%d head_dim=%d", B,
+                T, H, head_dim);
+    const int d = H * head_dim;
+    int rc = encoder_attention(static_cast<const __half*>(qkv_dev), 3 * d, B, T, H, head_dim, lens_dev, relpos != 0, pos_u_dev,
+                               pos_v_dev, static_cast<const __half*>(P_dev), d, scale, static_cast<__half*>(out_dev), d, st,
+                               chunk, left_chunks);
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("encoder_attention_test: device error"); rc = SBK_ERR_CUDA; }
+    return rc;
+}
+
+int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
+                    const float* ln_g_dev, const float* ln_b_dev, int chunk, void* out_dev, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(x_dev && taps_dev && bias_dev && ln_g_dev && ln_b_dev && out_dev, "dwconv_test: null pointer");
+    SBK_REQUIRE(B >= 1 && T >= 1 && D >= 1 && K >= 1 && chunk >= 0, "dwconv_test: bad sizes B=%d T=%d D=%d K=%d chunk=%d", B, T,
+                D, K, chunk);
+    std::vector<float> src((size_t)D * K), wt((size_t)K * D);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(src.data(), taps_dev, src.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    dwconv_repack_taps(src.data(), D, K, wt.data());
+    float* taps = nullptr;
+    if (cudaMalloc(&taps, wt.size() * 4) != cudaSuccess) { set_error("dwconv_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
+    int rc = cudaMemcpyAsync(taps, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess ? SBK_OK : SBK_ERR_CUDA;
+    if (rc == SBK_OK)
+        rc = dwconv_ln_swish(x_dev, B, T, D, K, taps, bias_dev, ln_g_dev, ln_b_dev, 1e-5f, static_cast<__half*>(out_dev), st, chunk);
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("dwconv_test: device error"); rc = SBK_ERR_CUDA; }
+    cudaFree(taps);
     return rc;
 }
 

@@ -125,6 +125,7 @@ void hypermix_pe_table(int d, float* dst);  // [HM_PE_ROWS, d] (host)
 // chunk > 0: Dynamic Chunk Convolution (inputs past the end of the output frame's chunk are zero)
 int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw,
                     const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk = 0);
+void dwconv_repack_taps(const float* src, int D, int K, float* dst);  // (D, 1, K) -> tap-major [K, D] (host)
 int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_dim, const int* lens, bool relpos,
                       const float* pos_u, const float* pos_v, const __half* P, int ldp, float scale, __half* out,
                       int ldo, cudaStream_t stream, int chunk = 0, int left_chunks = -1);

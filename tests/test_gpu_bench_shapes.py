@@ -529,22 +529,24 @@ def test_edge_shapes_vs_oracle(dev, B, L, lens, att):
 
 
 def test_long_utterance_vs_oracle(dev):
-    """Maximum-size direction: 2 x 40 s (T = 1001 encoder frames = 16 key blocks, 8 x the bench length), ragged, 2 Conformer
-    layers, RoPE: encoder vs the CPU oracle."""
+    """Maximum-size direction, ragged, 2 Conformer layers, encoder vs the CPU oracle: RoPE at 2 x 40 s (T = 1001 encoder
+    frames = 16 key blocks, 8 x the bench length); RelPosMHAXL at 2 x 48 s (T = 1201: past the 1036 frames at which a
+    T-row shared-memory P table no longer fits)."""
     from oracle import asr_oracle as O
     from speechbrain_b200.engine import AsrEngine
     from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
-    cfg = dict(CONFORMER_LARGE, num_encoder_layers=2, num_decoder_layers=1)
-    sd = seeded_asr_state(cfg, 0)
-    eng = AsrEngine(cfg, sd, device=dev, parts=("fbank", "cnn", "encoder"))
-    gen = torch.Generator().manual_seed(40)
-    L = 640000
-    wav = torch.randn(2, L, generator=gen)
-    wl = torch.tensor([1.0, 0.73])
-    wav[1, int(0.73 * L):] = 0
-    enc = eng.encode_wav(wav.to(dev), wl.to(dev)).cpu()
-    with torch.no_grad():
-        ref = O.encode(O.full_pipeline_features(wav, wl, sd, dict(cfg, win_length=32)), wl, sd, cfg, "Transformer.")
-    r = _rel(enc, ref)
-    print(f"long utterance: T={ref.shape[1]} encoder rel-L2 {r:.3e}")
-    assert enc.shape == ref.shape and r < 1e-3
+    for att, L, frac, seed in (("RoPEMHA", 640000, 0.73, 40), ("RelPosMHAXL", 768000, 0.66, 48)):
+        cfg = dict(CONFORMER_LARGE, attention_type=att, num_encoder_layers=2, num_decoder_layers=1)
+        sd = seeded_asr_state(cfg, 0)
+        eng = AsrEngine(cfg, sd, device=dev, parts=("fbank", "cnn", "encoder"))
+        gen = torch.Generator().manual_seed(seed)
+        wav = torch.randn(2, L, generator=gen)
+        wl = torch.tensor([1.0, frac])
+        wav[1, int(frac * L):] = 0
+        enc = eng.encode_wav(wav.to(dev), wl.to(dev)).cpu()
+        del eng
+        with torch.no_grad():
+            ref = O.encode(O.full_pipeline_features(wav, wl, sd, dict(cfg, win_length=32)), wl, sd, cfg, "Transformer.")
+        r = _rel(enc, ref)
+        print(f"long utterance {att}: T={ref.shape[1]} encoder rel-L2 {r:.3e}")
+        assert enc.shape == ref.shape and r < 1e-3, f"{att}: rel-L2 {r:.3e}"
