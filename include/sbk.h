@@ -149,6 +149,13 @@ int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int hea
                                const float* pos_u_dev, const float* pos_v_dev, const void* P_dev, float scale, int chunk,
                                int left_chunks, void* out_dev, void* stream);
 
+/* the streaming encoder's ring write alone (stream_qkv_kernel): qkv_dev [B*n, 3*H*head_dim] fp32 (per head [q | k | v]) ->
+ * q_out_dev [B*n, H*head_dim] fp16 and each row's per-head [k | v] into slot (slot0 + i) % cap of kv_out_dev
+ * [B][cap][2*H*head_dim] fp16.  inv_freq_dev [head_dim / 2] fp32: RoPE at stream positions pos0 + i with q scaled by
+ * q_scale; NULL: no rotation.  Synchronises the stream. */
+int sbk_stream_qkv_test(const float* qkv_dev, int B, int n, int H, int head_dim, const float* inv_freq_dev, long long pos0,
+                        float q_scale, void* q_out_dev, void* kv_out_dev, int cap, int slot0, void* stream);
+
 /* the Conformer convolution module's depthwise conv + LayerNorm + Swish alone (Conformer.py:314-330): x_dev [B*T, D] fp32
  * (the GLU output) -> out_dev [B*T, D] fp16 = SiLU(LayerNorm(Conv1d_K(x) + bias)), eps 1e-5, zero padding outside [0, T)
  * only (padded frames inside T are inputs).  taps_dev in the reference layout [D, 1, K], bias / ln_g / ln_b [D] fp32; odd K,
@@ -215,6 +222,26 @@ int sbk_asr_cnn_forward(sbk_asr* m, const float* feats_dev, int B, int T0, float
  * rel_len_dev: relative lengths (wav_len) or NULL. */
 int sbk_asr_encode_from_cnn(sbk_asr* m, const float* src_dev, const float* rel_len_dev, int B, int T,
                             float* enc_out_dev, void* stream);
+/* Chunk-by-chunk streaming encoder (TransformerASR.encode_streaming, TransformerASR.py:546-643; Conformer.py:501-586) for
+ * the Conformer encoder with RoPEMHA or RelPosMHAXL.  A stream holds a batch of B streams that advance together: per layer
+ * the attention's left context (the projected keys / values of the last `left_frames` frames; -1 = every frame so far) and
+ * the Dynamic Chunk Convolution's carry.  Each chunk costs the same whatever the stream's age.  The outputs equal the
+ * masked full-sequence run (sbk_asr_set_dynchunk with left_context_chunks = left_frames / chunk_size).  With RelPosMHAXL an
+ * unlimited left context holds at most max_len frames.  The weights are the handle's: use a stream with the handle (or a
+ * clone) it was created from. */
+typedef struct sbk_asr_stream sbk_asr_stream; /* opaque */
+int sbk_asr_stream_create(sbk_asr* m, int B, int chunk_size, int left_frames, sbk_asr_stream** out);
+/* cnn_out [B, n, input_size] fp32 -> enc_out [B, n, d_model] fp32, 1 <= n <= chunk_size; only the last chunk may be
+ * shorter.  No host synchronisation, except when an unlimited left context outgrows its buffer (it doubles). */
+int sbk_asr_stream_encode_chunk(sbk_asr* m, sbk_asr_stream* s, const float* cnn_out_dev, int n_frames, float* enc_out_dev,
+                                void* stream);
+int sbk_asr_stream_reset(sbk_asr_stream* s); /* back to an empty context */
+void sbk_asr_stream_destroy(sbk_asr_stream* s);
+/* Layer `layer`'s context: *n_rows = cached frames; kv_out [B, n_rows, 2 * d_model] fp16 (per head [key | value], keys
+ * RoPE-rotated by stream position) and carry_out [B, (kernel_size - 1) / 2, d_model] fp32 (depthwise-conv inputs), each
+ * written when non-null. */
+int sbk_asr_stream_context(sbk_asr* m, const sbk_asr_stream* s, int layer, void* kv_out_dev, float* carry_out_dev,
+                           int* n_rows, void* stream);
 /* normalised feats [B,T0,n_mels] -> CNN -> encode in one call (inference/ASR.py:100-128 encode_batch, minus Fbank) */
 int sbk_asr_encode_feats(sbk_asr* m, const float* feats_dev, const float* rel_len_dev, int B, int T0,
                          float* cnn_out_dev, float* enc_out_dev, void* stream);

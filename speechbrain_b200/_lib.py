@@ -61,6 +61,8 @@ EXPORTS = [
     "sbk_asr_set_decoder_tc_min_rows", "sbk_asr_lm_rescore", "sbk_asr_transcribe_greedy_group_host_async", "sbk_asr_decode_teacher_forced", "sbk_asr_ctc_head", "sbk_rows_argmax_f32", "sbk_asr_set_dynchunk",
     "sbk_asr_lm_forward", "sbk_asr_lm_step_logits", "sbk_ctc_beam_workspace_bytes", "sbk_ctc_beam_search",
     "sbk_transducer_create", "sbk_transducer_destroy", "sbk_transducer_info", "sbk_transducer_greedy",
+    "sbk_asr_stream_create", "sbk_asr_stream_encode_chunk", "sbk_asr_stream_reset", "sbk_asr_stream_destroy",
+    "sbk_asr_stream_context", "sbk_stream_qkv_test",
 ]
 
 
@@ -78,7 +80,7 @@ def lib():
             getattr(L, name)  # AttributeError if the ABI is incomplete
         for name in EXPORTS:
             if name not in ("sbk_last_error", "sbk_fbank_destroy", "sbk_asr_destroy", "sbk_launch_count",
-                            "sbk_gemm_profile_enable", "sbk_transducer_destroy"):
+                            "sbk_gemm_profile_enable", "sbk_transducer_destroy", "sbk_asr_stream_destroy"):
                 getattr(L, name).restype = ctypes.c_int
         L.sbk_launch_count.restype = ctypes.c_longlong
         L.sbk_gemm_profile_enable.restype = None

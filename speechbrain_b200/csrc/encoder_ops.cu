@@ -258,11 +258,12 @@ constexpr int DW_TT = 16;
 // KT > 0: compile-time kernel size (taps held in registers); KT == 0: runtime K.  MAXC: channels per thread (D <= 256 * MAXC)
 // CHUNKED: Dynamic Chunk Convolution (Conformer.py:190-313): for every output frame the inputs beyond the end of its own
 // chunk of `chunk` frames count as zero (the past, other chunks included, is visible as usual).
+// left: [B, (K-1)/2, D] inputs of the frames just before frame 0 (a stream's previous chunks), or null for zero padding.
 template <int KT, int MAXC, bool CHUNKED = false>
 __global__ void __launch_bounds__(256, 2)
 dwconv_ln_swish_kernel(const float* __restrict__ glu, int T, int D, int K, const float* __restrict__ wdw /*[K,D] tap-major*/,
                        const float* __restrict__ bdw, const float* __restrict__ gamma, const float* __restrict__ beta,
-                       float eps, __half* __restrict__ out, int chunk) {
+                       float eps, __half* __restrict__ out, int chunk, const float* __restrict__ left) {
     extern __shared__ __align__(128) float dw_smem[];
     __shared__ uint64_t bar;
     const int halo = (K - 1) / 2;
@@ -287,12 +288,12 @@ dwconv_ln_swish_kernel(const float* __restrict__ glu, int T, int D, int K, const
             bulk_load_1d(slab + r * D, src + static_cast<size_t>(t0 - halo + r) * D, row_bytes * nr, &bar);
         }
     }
-    // zero rows outside the utterance (Conv1d zero padding)
+    // zero rows outside the utterance (Conv1d zero padding); rows before frame 0 come from `left` when it is set
     for (int i = threadIdx.x; i < (r_lo + rows_in - r_hi) * D; i += blockDim.x) {
         int r = i / D;
         const int ch = i - r * D;
         if (r >= r_lo) r += r_hi - r_lo;
-        slab[r * D + ch] = 0.0f;
+        slab[r * D + ch] = left && r < r_lo ? left[(static_cast<size_t>(b) * halo + t0 + r) * D + ch] : 0.0f;  // frame t0 - halo + r
     }
     // tap weights and biases of this thread's channels: fetched while the slab is still in flight
     float wreg[KT > 0 ? MAXC : 1][KT > 0 ? KT : 1];
@@ -398,7 +399,8 @@ dwconv_ln_swish_kernel(const float* __restrict__ glu, int T, int D, int K, const
 }
 
 int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw,
-                    const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk) {
+                    const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk,
+                    const float* left) {
     SBK_REQUIRE(D % 4 == 0 && D <= 1024 && (K & 1) == 1, "dwconv_ln_swish: D %% 4, D <= 1024 and odd K required (D=%d K=%d)", D, K);
     SBK_REQUIRE((reinterpret_cast<uintptr_t>(glu) & 15) == 0, "dwconv_ln_swish: input must be 16-byte aligned");
     const size_t smem = static_cast<size_t>(DW_TT + K - 1) * D * sizeof(float);
@@ -412,7 +414,28 @@ int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* w
         kern = D <= 256 ? dwconv_ln_swish_kernel<31, 1> : D <= 512 ? dwconv_ln_swish_kernel<31, 2> : dwconv_ln_swish_kernel<31, 4>;
     }
     SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<dim3(ceil_div(T, DW_TT), B), 256, smem, stream>>>(glu, T, D, K, wdw, bdw, gamma, beta, eps, out, chunk);
+    kern<<<dim3(ceil_div(T, DW_TT), B), 256, smem, stream>>>(glu, T, D, K, wdw, bdw, gamma, beta, eps, out, chunk, left);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
+// carry [B, halo, D] <- the last halo rows of [carry; glu [B, n, D]] (has_old == 0: the carry counts as zeros).  Thread =
+// (utterance, channel); rows ascend, so row j is written only after row j + n, which it may read, has been read.
+__global__ void dwconv_carry_kernel(const float* __restrict__ glu, int n, int D, int halo, int has_old, float* carry) {
+    const int ch = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (ch >= D) return;
+    float* cb = carry + static_cast<size_t>(b) * halo * D + ch;
+    for (int j = 0; j < halo; ++j) {
+        const int src = j + n - halo;  // row of the chunk, or (when < 0) of the old carry at j + n
+        cb[static_cast<size_t>(j) * D] = src >= 0 ? glu[(static_cast<size_t>(b) * n + src) * D + ch]
+                                                  : (has_old ? cb[static_cast<size_t>(j + n) * D] : 0.0f);
+    }
+}
+
+int dwconv_carry(const float* glu, int B, int n, int D, int K, bool has_old, float* carry, cudaStream_t stream) {
+    const int halo = (K - 1) / 2;
+    if (halo == 0) return SBK_OK;
+    dwconv_carry_kernel<<<dim3(ceil_div(D, 128), B), 128, 0, stream>>>(glu, n, D, halo, has_old ? 1 : 0, carry);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }
@@ -618,12 +641,14 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
     return *reinterpret_cast<uint32_t*>(&h);
 }
 
-template <int DH, int DHP, bool RELPOS>  // DHP = DH rounded up to a multiple of 16 (zero-padded in shared memory)
+// STREAM: one chunk of a stream (AttStream): T is the window [cached rows; chunk rows], the queries are its last sa.nq rows
+// (from sa.q), keys / values come from the ring sa.kv, every key of the window is visible, and out holds the chunk's rows.
+template <int DH, int DHP, bool RELPOS, bool STREAM = false>  // DHP = DH rounded up to a multiple of 16 (zero-padded in shared memory)
 __global__ void __launch_bounds__(128)
 encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const int* __restrict__ lens,
                          const float* __restrict__ pos_u, const float* __restrict__ pos_v,
                          const __half* __restrict__ P, int ldp, float scale, __half* __restrict__ out, int ldo,
-                         int chunk, int left_chunks) {
+                         int chunk, int left_chunks, AttStream sa) {
     constexpr int STR = DHP + 8;  // padded row stride (halfs): conflict-free fragment loads
     constexpr int KS = DHP / 16;
     constexpr int GW = ATT_GW;
@@ -640,10 +665,23 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
     constexpr bool ASYNC = (DH % 8 == 0) && (DHP == DH);
     __half* KV1 = reinterpret_cast<__half*>(Gs + (RELPOS ? 4 * 16 * (GW + 1) : 0));  // [2][64][STR] when ASYNC
 
-    const int b = blockIdx.z, h = blockIdx.y, i0 = blockIdx.x * ATT_BQ;
+    const int q_off = STREAM ? T - sa.nq : 0;  // window row of the first query
+    const int b = blockIdx.z, h = blockIdx.y, i0 = q_off + blockIdx.x * ATT_BQ;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
     const int len = lens ? min(lens[b], T) : T;
-    const __half* base = qkv + static_cast<size_t>(b) * T * ld + h * 3 * DH;
+    const __half* base = STREAM ? nullptr : qkv + static_cast<size_t>(b) * T * ld + h * 3 * DH;
+    auto q_row = [&](int i) {
+        if constexpr (STREAM) return sa.q + (static_cast<size_t>(b) * sa.nq + (i - q_off)) * sa.ldq + h * DH;
+        else return base + static_cast<size_t>(i) * ld;
+    };
+    auto k_row = [&](int j) {  // the row's V follows its K at + DH
+        if constexpr (STREAM) {
+            const int slot = sa.start + j < sa.cap ? sa.start + j : sa.start + j - sa.cap;
+            return sa.kv + (static_cast<size_t>(b) * sa.cap + slot) * sa.ldkv + h * 2 * DH;
+        } else {
+            return base + static_cast<size_t>(j) * ld + DH;
+        }
+    };
 
     if constexpr (DHP != DH) {  // zero the padding columns once (they take part in the k-loop / PV n-tiles)
         constexpr int PADC = DHP - DH;
@@ -657,7 +695,7 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
     for (int i = threadIdx.x; i < ATT_BQ * VPR; i += blockDim.x) {
         const int r = i / VPR, v4 = i - r * VPR;
         uint2 val = make_uint2(0, 0);
-        if (i0 + r < T) val = *reinterpret_cast<const uint2*>(base + static_cast<size_t>(i0 + r) * ld + v4 * 4);
+        if (i0 + r < T) val = *reinterpret_cast<const uint2*>(q_row(i0 + r) + v4 * 4);
         if constexpr (RELPOS) {
             const __half* hv = reinterpret_cast<const __half*>(&val);
             __half qu[4], qv[4];
@@ -737,12 +775,12 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
         for (int i = threadIdx.x; i < ATT_BK * V8; i += blockDim.x) {
             const int r = i / V8, v8 = i - r * V8;
             const bool ok = j0 + r < T;
-            const __half* rowp = base + static_cast<size_t>(ok ? j0 + r : 0) * ld + v8 * 8;
+            const __half* rowp = k_row(ok ? j0 + r : 0) + v8 * 8;
             const uint32_t nbytes = ok ? 16u : 0u;
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(kd + r * STR + v8 * 8)),
-                         "l"(rowp + DH), "r"(nbytes) : "memory");
+                         "l"(rowp), "r"(nbytes) : "memory");
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(vd + r * STR + v8 * 8)),
-                         "l"(rowp + 2 * DH), "r"(nbytes) : "memory");
+                         "l"(rowp + DH), "r"(nbytes) : "memory");
         }
         if constexpr (RELPOS) {
             const int a = p_first(jb), n = jb == blk_begin ? ATT_PW : ATT_BK;
@@ -791,9 +829,9 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
                 const int r = i / VPR, v4 = i - r * VPR;
                 uint2 kv = make_uint2(0, 0), vv = make_uint2(0, 0);
                 if (j0 + r < T) {
-                    const __half* rowp = base + static_cast<size_t>(j0 + r) * ld + v4 * 4;
-                    kv = *reinterpret_cast<const uint2*>(rowp + DH);
-                    vv = *reinterpret_cast<const uint2*>(rowp + 2 * DH);
+                    const __half* rowp = k_row(j0 + r) + v4 * 4;
+                    kv = *reinterpret_cast<const uint2*>(rowp);
+                    vv = *reinterpret_cast<const uint2*>(rowp + DH);
                 }
                 *reinterpret_cast<uint2*>(Ks + r * STR + v4 * 4) = kv;
                 *reinterpret_cast<uint2*>(Vs + r * STR + v4 * 4) = vv;
@@ -925,27 +963,32 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
     const int r0 = i0 + warp * 16 + g, r1 = r0 + 8;
     // (l == 0: a padded query row whose whole window is padding -- only possible with chunked attention; emit zeros)
     const float inv0 = l_run[0] > 0.0f ? 1.0f / l_run[0] : 0.0f, inv1 = l_run[1] > 0.0f ? 1.0f / l_run[1] : 0.0f;
-    __half* ob = out + static_cast<size_t>(b) * T * ldo + h * DH;
+    // output row of window row r (STREAM: the chunk's rows, [B * sa.nq, ldo])
+    auto o_row = [&](int r) {
+        const size_t row = STREAM ? static_cast<size_t>(b) * sa.nq + (r - q_off) : static_cast<size_t>(b) * T + r;
+        return out + row * ldo + h * DH;
+    };
 #pragma unroll
     for (int nt = 0; nt < DHP / 8; ++nt) {
         const int col = nt * 8 + 2 * c;
         if (col >= DH) continue;  // zero-padding columns
-        if (r0 < T) *reinterpret_cast<uint32_t*>(ob + static_cast<size_t>(r0) * ldo + col) = pack_half2(o[nt][0] * inv0, o[nt][1] * inv0);
-        if (r1 < T) *reinterpret_cast<uint32_t*>(ob + static_cast<size_t>(r1) * ldo + col) = pack_half2(o[nt][2] * inv1, o[nt][3] * inv1);
+        if (r0 < T) *reinterpret_cast<uint32_t*>(o_row(r0) + col) = pack_half2(o[nt][0] * inv0, o[nt][1] * inv0);
+        if (r1 < T) *reinterpret_cast<uint32_t*>(o_row(r1) + col) = pack_half2(o[nt][2] * inv1, o[nt][3] * inv1);
     }
 }
 
-template <int DH, int DHP>
+template <int DH, int DHP, bool STREAM = false>
 static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int H, const int* lens, bool relpos,
                                     const float* pos_u, const float* pos_v, const __half* P, int ldp, float scale,
-                                    __half* out, int ldo, int chunk, int left_chunks, cudaStream_t stream) {
+                                    __half* out, int ldo, int chunk, int left_chunks, cudaStream_t stream,
+                                    const AttStream& sa = AttStream{}) {
     constexpr int STR = DHP + 8;
-    dim3 grid(ceil_div(T, ATT_BQ), H, B);
+    dim3 grid(ceil_div(STREAM ? sa.nq : T, ATT_BQ), H, B);
     if (!relpos) {
         const size_t smem = 4ull * ATT_BQ * STR * 2 + 2ull * ATT_BK * STR * 2;  // + second K/V buffer pair
-        auto kern = encoder_attention_kernel<DH, DHP, false>;
+        auto kern = encoder_attention_kernel<DH, DHP, false, STREAM>;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, nullptr, nullptr, nullptr, 0, scale, out, ldo, chunk, left_chunks);
+        kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, nullptr, nullptr, nullptr, 0, scale, out, ldo, chunk, left_chunks, sa);
     } else if constexpr (DH > 64) {  // the RelPos band and P window are built for head widths up to 64
         set_error("encoder_attention: RelPosMHAXL with head_dim=%d not built", DH);
         return SBK_ERR_UNSUPPORTED;
@@ -958,9 +1001,9 @@ static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int
         // independent of T: 101 KB at head_dim 64 (two CTAs per SM), 69 KB at 36 and 65 KB at 32 (three)
         const size_t smem = (4ull * ATT_BQ + ATT_PR) * STR * 2 + 4ull * 16 * (ATT_GW + 1) * 4 +
                             (ASYNC ? 2ull * ATT_BK * STR * 2 : 0);
-        auto kern = encoder_attention_kernel<DH, DHP, true>;
+        auto kern = encoder_attention_kernel<DH, DHP, true, STREAM>;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks);
+        kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, sa);
     }
     SBK_LAUNCH_CHECK();
     return SBK_OK;
@@ -984,6 +1027,64 @@ int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_d
         return launch_encoder_attention<128, 128>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
     set_error("encoder_attention: head_dim=%d not built (128, 64, 36, 32)", head_dim);
     return SBK_ERR_UNSUPPORTED;
+}
+
+int encoder_attention_stream(const AttStream& sa, int B, int W, int H, int head_dim, bool relpos, const float* pos_u,
+                             const float* pos_v, const __half* P, int ldp, float scale, __half* out, int ldo,
+                             cudaStream_t stream) {
+    SBK_REQUIRE(sa.nq >= 1 && sa.nq <= W && W <= sa.cap && sa.start >= 0 && sa.start < sa.cap,
+                "encoder_attention_stream: bad window (%d queries, %d rows, ring of %d from %d)", sa.nq, W, sa.cap, sa.start);
+    SBK_REQUIRE(sa.ldq % 8 == 0 && sa.ldkv % 8 == 0 && ldo % 2 == 0 && (reinterpret_cast<uintptr_t>(sa.q) & 15) == 0 &&
+                    (reinterpret_cast<uintptr_t>(sa.kv) & 15) == 0,
+                "encoder_attention_stream: q / kv must be 16-byte aligned");
+    if (head_dim == 64)
+        return launch_encoder_attention<64, 64, true>(nullptr, 0, B, W, H, nullptr, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, 0, -1, stream, sa);
+    if (head_dim == 36 && relpos)
+        return launch_encoder_attention<36, 48, true>(nullptr, 0, B, W, H, nullptr, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, 0, -1, stream, sa);
+    if (head_dim == 32)
+        return launch_encoder_attention<32, 32, true>(nullptr, 0, B, W, H, nullptr, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, 0, -1, stream, sa);
+    set_error("encoder_attention_stream: head_dim=%d not built (64, 36 with RelPosMHAXL, 32)", head_dim);
+    return SBK_ERR_UNSUPPORTED;
+}
+
+// One chunk's QKV projection qkv [B*n, 3d] fp32 (per-head [q | k | v] blocks) -> the attention's operands: q [B*n, d] fp16
+// (RoPE: rotated and scaled by q_scale, as the full-sequence epilogue does; RelPos: as projected) and each row's [k | v]
+// per head into the ring slot (slot0 + i) % cap of kv [B][cap][2d] fp16.  RoPE rotates q and k by the row's position in the
+// stream: the angle pos * inv_freq is formed and reduced in double precision, so it stays exact however long the stream,
+// and the scores, which depend on the position difference only, equal those of a window-local rotation.  Each cached key
+// is rotated and rounded to fp16 once, like the full-sequence path's keys.
+__global__ void stream_qkv_kernel(const float* __restrict__ qkv, int n, int H, int DH, const float* __restrict__ inv_freq,
+                                  long long pos0, float q_scale, __half* __restrict__ q, __half* __restrict__ kv, int cap,
+                                  int slot0) {
+    const int half_dh = DH >> 1, d = H * DH;
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // (pair, head) of row blockIdx.y
+    if (idx >= H * half_dh) return;
+    const int h = idx / half_dh, p = idx - h * half_dh, row = blockIdx.y, b = row / n, i = row - b * n;
+    const float* src = qkv + static_cast<size_t>(row) * 3 * d + h * 3 * DH + 2 * p;
+    float q0 = src[0], q1 = src[1], k0 = src[DH], k1 = src[DH + 1];
+    if (inv_freq) {
+        double sd, cd;
+        sincos(static_cast<double>(pos0 + i) * static_cast<double>(inv_freq[p]), &sd, &cd);
+        const float c = static_cast<float>(cd), s = static_cast<float>(sd);
+        const float rq0 = (q0 * c - q1 * s) * q_scale, rq1 = (q1 * c + q0 * s) * q_scale;
+        const float rk0 = k0 * c - k1 * s, rk1 = k1 * c + k0 * s;
+        q0 = rq0; q1 = rq1; k0 = rk0; k1 = rk1;
+    }
+    *reinterpret_cast<__half2*>(q + static_cast<size_t>(row) * d + h * DH + 2 * p) = floats2half2_sat(q0, q1);
+    const int slot = (slot0 + i) % cap;
+    __half* dst = kv + (static_cast<size_t>(b) * cap + slot) * 2 * d + h * 2 * DH + 2 * p;
+    *reinterpret_cast<__half2*>(dst) = floats2half2_sat(k0, k1);
+    *reinterpret_cast<__half2*>(dst + DH) = floats2half2_sat(src[2 * DH], src[2 * DH + 1]);
+}
+
+int stream_qkv(const float* qkv, int B, int n, int H, int DH, const float* inv_freq, long long pos0, float q_scale,
+               __half* q, __half* kv, int cap, int slot0, cudaStream_t stream) {
+    SBK_REQUIRE(DH % 2 == 0 && n >= 1 && cap >= n && slot0 >= 0, "stream_qkv: bad shape");
+    const int pairs = H * DH / 2;
+    stream_qkv_kernel<<<dim3(ceil_div(pairs, 128), B * n), 128, 0, stream>>>(qkv, n, H, DH, inv_freq, pos0, q_scale, q, kv,
+                                                                            cap, slot0);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
 }
 
 // =========================================================================== HyperMixing (HyperConformer token mixing)

@@ -897,9 +897,34 @@ static int run_cnn(AsrModel* m, const float* feats, int B, int T0, float* cnn_ou
                                 W.c2_be, c.cnn_c2, m->b.act1, m->b.a_in, cnn_out_f, st);
 }
 
+// One chunk-by-chunk stream (or a batch of B streams advancing together) of a Conformer encoder: per layer the attention's
+// left context as a ring of projected [k | v] rows (RoPE keys rotated by stream position) and the Dynamic Chunk
+// Convolution's carry, the last (kernel_size - 1) / 2 depthwise-conv inputs.  The window of a chunk is [cached rows; chunk]:
+// exactly the keys the masked full-sequence mode lets the chunk's frames see, so its outputs are the same.
+struct AsrStream {
+    int B = 0, chunk = 0, left = -1;  // left-context frames (-1: the whole past)
+    int cap = 0;                      // ring rows per layer and stream (grows for an infinite left context)
+    long long total = 0;              // frames encoded so far
+    int clen = 0, start = 0;          // cached rows, ring slot of the oldest
+    bool ended = false;               // a chunk shorter than `chunk` was seen: it must be the last
+    int prow = 0;                     // RelPos: rows of P
+    DevBuf kv;     // [L][B][cap][2d] fp16
+    DevBuf carry;  // [L][B][halo][d] fp32
+    DevBuf P;      // RelPos: [L][prow][d] fp16 = linear_pos(pe[r])
+    DevBuf scr;    // inv_freq [dh/2] fp32 (RoPE), qkv [B*chunk, 3d] fp32, q [B*chunk, d] fp16
+    const float* inv_freq = nullptr; float* qkv32 = nullptr; __half* q16 = nullptr;
+    __half* kv_layer(const sbk_asr_config& c, int l) const {
+        return static_cast<__half*>(kv.base) + (size_t)l * B * cap * 2 * c.d_model;
+    }
+    float* carry_layer(const sbk_asr_config& c, int l) const {
+        return static_cast<float*>(carry.base) + (size_t)l * B * ((c.kernel_size - 1) / 2) * c.d_model;
+    }
+};
+
 // feats [B, T0, n_mels] fp32 (already normalised) -> enc_out fp32 [B, T2, d] (+ enc16). enc_len device int[B].
+// s: one chunk of a stream (T0 = the chunk's frames, feats null): attention over s's window, the conv over its carry.
 static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int* enc_len, float* cnn_out_f,
-                       float* enc_out, cudaStream_t st) {
+                       float* enc_out, cudaStream_t st, const AsrStream* s = nullptr) {
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int T1 = (T0 - 1) / 2 + 1, T = feats ? (T1 - 1) / 2 + 1 : T0;  // feats == nullptr: b.a_in holds [B*T0, input_size]
@@ -934,19 +959,33 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
         if (c.attention_type == SBK_ATT_HYPERMIX) {  // x += HyperMixing(norm1(x)) (hypermixing.py:90-195)
             RC(hypermix_forward(b.h16, B, T, d, H, F / H, enc_len, m->wt->hm_pe, w.hm, b.hm_part, b.hm_G, b.hm_gscale, b.x, st));
         } else {
-            e = GemmEpilogue(); e.out = b.qkv16; e.ldo = 3 * d;
-            if (c.attention_type == SBK_ATT_ROPE) {
-                e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->wt->rope_cos; e.rope_sin = m->wt->rope_sin; e.head_dim = dh;
+            if (s) {  // the chunk's q and its [k | v] rows in the ring, then attention over [cached rows; chunk]
+                const bool rope = c.attention_type == SBK_ATT_ROPE;
+                __half* kv = s->kv_layer(c, l);
+                e = GemmEpilogue(); e.mode = EPI_F32; e.out = s->qkv32; e.ldo = 3 * d;
+                RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
+                RC(stream_qkv(s->qkv32, B, T, H, dh, rope ? s->inv_freq : nullptr, s->total, att_scale, s->q16, kv, s->cap,
+                              (s->start + s->clen) % s->cap, st));
+                AttStream sa;
+                sa.q = s->q16; sa.ldq = d; sa.kv = kv; sa.ldkv = 2 * d; sa.cap = s->cap; sa.start = s->start; sa.nq = T;
+                RC(encoder_attention_stream(sa, B, s->clen + T, H, dh, !rope, w.pos_u, w.pos_v,
+                                            rope ? nullptr : static_cast<const __half*>(s->P.base) + (size_t)l * s->prow * d, d,
+                                            att_scale, b.att16, d, st));
             } else {
-                e.mode = EPI_F16;
+                e = GemmEpilogue(); e.out = b.qkv16; e.ldo = 3 * d;
+                if (c.attention_type == SBK_ATT_ROPE) {
+                    e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->wt->rope_cos; e.rope_sin = m->wt->rope_sin; e.head_dim = dh;
+                } else {
+                    e.mode = EPI_F16;
+                }
+                RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
+                if (c.attention_type == SBK_ATT_RELPOS) {
+                    e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
+                    RC(gemm_f16(m->wt->relpos_pe, d, w.wpos, d, e, T, d, d, st));
+                }
+                RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, c.attention_type == SBK_ATT_RELPOS, w.pos_u, w.pos_v,
+                                     b.P16, d, att_scale, b.att16, d, st, m->dyn_chunk, m->dyn_left));
             }
-            RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
-            if (c.attention_type == SBK_ATT_RELPOS) {
-                e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
-                RC(gemm_f16(m->wt->relpos_pe, d, w.wpos, d, e, T, d, d, st));
-            }
-            RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, c.attention_type == SBK_ATT_RELPOS, w.pos_u, w.pos_v,
-                                 b.P16, d, att_scale, b.att16, d, st, m->dyn_chunk, m->dyn_left));
             e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bo; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
             RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
         }
@@ -954,7 +993,15 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
         RC(layernorm_rows(b.x, b.h16, true, w.conv_ln_g, w.conv_ln_b, M, d, 1e-5f, false, st));
         e = GemmEpilogue(); e.mode = EPI_GLU; e.bias = w.bpw1; e.out = b.glu; e.ldo = d;
         RC(gemm_f16(b.h16, d, w.wpw1, d, e, M, 2 * d, d, st));
-        RC(dwconv_ln_swish(b.glu, B, T, d, c.kernel_size, w.wdw, w.bdw, w.aconv_ln_g, w.aconv_ln_b, 1e-5f, b.h16, st, m->dyn_chunk));
+        if (s) {  // the chunk after the carry, zeros after the chunk (its right edge); then the carry moves on
+            float* carry = s->carry_layer(c, l);
+            RC(dwconv_ln_swish(b.glu, B, T, d, c.kernel_size, w.wdw, w.bdw, w.aconv_ln_g, w.aconv_ln_b, 1e-5f, b.h16, st, 0,
+                               s->total > 0 ? carry : nullptr));
+            RC(dwconv_carry(b.glu, B, T, d, c.kernel_size, s->total > 0, carry, st));
+        } else {
+            RC(dwconv_ln_swish(b.glu, B, T, d, c.kernel_size, w.wdw, w.bdw, w.aconv_ln_g, w.aconv_ln_b, 1e-5f, b.h16, st,
+                               m->dyn_chunk));
+        }
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bpw2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
         e.row_lens = enc_len; e.T = T;
         RC(gemm_f16(b.h16, d, w.wpw2, d, e, M, d, d, st));
@@ -1818,6 +1865,17 @@ int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int hea
     return rc;
 }
 
+int sbk_stream_qkv_test(const float* qkv_dev, int B, int n, int H, int head_dim, const float* inv_freq_dev, long long pos0,
+                        float q_scale, void* q_out_dev, void* kv_out_dev, int cap, int slot0, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(qkv_dev && q_out_dev && kv_out_dev, "stream_qkv_test: null pointer");
+    SBK_REQUIRE(B >= 1 && H >= 1 && head_dim >= 2 && pos0 >= 0, "stream_qkv_test: bad sizes");
+    int rc = stream_qkv(qkv_dev, B, n, H, head_dim, inv_freq_dev, pos0, q_scale, static_cast<__half*>(q_out_dev),
+                        static_cast<__half*>(kv_out_dev), cap, slot0, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("stream_qkv_test: device error"); rc = SBK_ERR_CUDA; }
+    return rc;
+}
+
 int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
                     const float* ln_g_dev, const float* ln_b_dev, int chunk, void* out_dev, void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1967,6 +2025,144 @@ int sbk_asr_encode_from_cnn(sbk_asr* mm, const float* src_dev, const float* rel_
         enc_len = m->b.enc_len;
     }
     return run_encoder(m, nullptr, B, T, enc_len, nullptr, enc_out_dev ? enc_out_dev : m->b.enc_out, st);
+}
+
+// ---- chunk-by-chunk streaming encoder (AsrStream)
+static size_t stream_kv_bytes(const sbk_asr_config& c, int B, int cap) {
+    return (size_t)c.num_encoder_layers * B * cap * 2 * c.d_model * 2;
+}
+
+int sbk_asr_stream_create(sbk_asr* mm, int B, int chunk_size, int left_frames, sbk_asr_stream** out) {
+    AsrModel* m = reinterpret_cast<AsrModel*>(mm);
+    SBK_REQUIRE(m && out, "stream_create: null argument");
+    const sbk_asr_config& c = m->wt->cfg;
+    const int d = c.d_model, dh = d / c.nhead, L = c.num_encoder_layers, halo = (c.kernel_size - 1) / 2;
+    SBK_REQUIRE(m->wt->has_enc, "stream_create: this handle was created without encoder weights");
+    SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER && (c.attention_type == SBK_ATT_ROPE || c.attention_type == SBK_ATT_RELPOS),
+                "stream_create: streaming is built for the Conformer encoder with RoPEMHA or RelPosMHAXL");
+    SBK_REQUIRE(c.attention_type == SBK_ATT_RELPOS ? (dh == 64 || dh == 36 || dh == 32) : (dh == 64 || dh == 32),
+                "stream_create: head_dim=%d not built for streaming (RoPEMHA 64 or 32, RelPosMHAXL 64, 36 or 32)", dh);
+    SBK_REQUIRE(B >= 1 && chunk_size >= 1 && left_frames >= -1, "stream_create: B >= 1, chunk_size >= 1, left_frames >= -1");
+    const bool relpos = c.attention_type == SBK_ATT_RELPOS;
+    const int cap = left_frames >= 0 ? left_frames + chunk_size : std::max(4 * chunk_size, 256);
+    SBK_REQUIRE(!relpos || left_frames < 0 || cap <= m->wt->pos_len,
+                "stream_create: a window of %d frames exceeds RelPosMHAXL's max_len=%d", cap, m->wt->pos_len);
+    std::unique_ptr<AsrStream> st(new AsrStream());
+    st->B = B; st->chunk = chunk_size; st->left = left_frames; st->cap = cap;
+    auto alloc = [](DevBuf& buf, size_t bytes) {
+        if (cudaMalloc(&buf.base, std::max<size_t>(bytes, 256)) != cudaSuccess) {
+            set_error("stream_create: cudaMalloc(%zu) failed", bytes);
+            return SBK_ERR_NOMEM;
+        }
+        buf.cap = bytes;
+        return SBK_OK;
+    };
+    RC(alloc(st->kv, stream_kv_bytes(c, B, cap)));
+    RC(alloc(st->carry, (size_t)L * B * halo * d * 4));
+    const size_t rows = (size_t)B * chunk_size;
+    for (int pass = 0; pass < 2; ++pass) {
+        Carver take{pass ? static_cast<uint8_t*>(st->scr.base) : nullptr};
+        float* inv = nullptr;
+        take(inv, (size_t)dh / 2 * 4); take(st->qkv32, rows * 3 * d * 4); take(st->q16, rows * d * 2);
+        st->inv_freq = inv;
+        if (!pass) RC(alloc(st->scr, take.used));
+    }
+    if (!relpos) {  // nnet/attention.py:1012-1055: inv_freq_i = exp(-2i * ln(1e4) / d_h) in fp32, as the full-sequence table
+        std::vector<float> inv(dh / 2);
+        for (int i = 0; i < dh / 2; ++i) inv[i] = expf((float)(2 * i) * -(logf(10000.0f) / (float)dh));
+        SBK_CUDA_CHECK(cudaMemcpy(const_cast<float*>(st->inv_freq), inv.data(), inv.size() * 4, cudaMemcpyHostToDevice));
+    } else {  // P = linear_pos(pe[r]) for every row a window can reach, once per stream
+        st->prow = left_frames >= 0 ? cap : m->wt->pos_len;
+        RC(alloc(st->P, (size_t)L * st->prow * d * 2));
+        for (int l = 0; l < L; ++l) {
+            GemmEpilogue e; e.mode = EPI_F16; e.out = static_cast<__half*>(st->P.base) + (size_t)l * st->prow * d; e.ldo = d;
+            RC(gemm_f16(m->wt->relpos_pe, d, m->wt->enc[l].wpos, d, e, st->prow, d, d, 0));
+        }
+        SBK_CUDA_CHECK(cudaStreamSynchronize(0));
+    }
+    *out = reinterpret_cast<sbk_asr_stream*>(st.release());
+    return SBK_OK;
+}
+
+void sbk_asr_stream_destroy(sbk_asr_stream* s) { delete reinterpret_cast<AsrStream*>(s); }
+
+int sbk_asr_stream_reset(sbk_asr_stream* ss) {
+    AsrStream* s = reinterpret_cast<AsrStream*>(ss);
+    SBK_REQUIRE(s, "stream_reset: null stream");
+    s->total = 0; s->clen = 0; s->start = 0; s->ended = false;  // the first chunk reads no cache and a zero carry
+    return SBK_OK;
+}
+
+int sbk_asr_stream_encode_chunk(sbk_asr* mm, sbk_asr_stream* ss, const float* cnn_out_dev, int n, float* enc_out_dev,
+                                void* stream) {
+    AsrModel* m = reinterpret_cast<AsrModel*>(mm);
+    AsrStream* s = reinterpret_cast<AsrStream*>(ss);
+    SBK_REQUIRE(m && s && cnn_out_dev && enc_out_dev, "stream_encode_chunk: null argument");
+    const sbk_asr_config& c = m->wt->cfg;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(n >= 1 && n <= s->chunk, "stream_encode_chunk: %d frames, the chunk size is %d", n, s->chunk);
+    SBK_REQUIRE(!s->ended, "stream_encode_chunk: only the last chunk of a stream may be shorter than the chunk size");
+    const int W = s->clen + n;
+    SBK_REQUIRE(s->prow == 0 || W <= s->prow,
+                "stream_encode_chunk: an unlimited left context holds at most max_len=%d frames with RelPosMHAXL", s->prow);
+    if (W > s->cap) {  // unlimited left context (nothing is ever evicted, so the ring starts at slot 0): grow it
+        const int ncap = std::max(W, 2 * s->cap);
+        DevBuf nb;
+        if (cudaMalloc(&nb.base, stream_kv_bytes(c, s->B, ncap)) != cudaSuccess) {
+            set_error("stream_encode_chunk: cudaMalloc(%zu) failed", stream_kv_bytes(c, s->B, ncap));
+            return SBK_ERR_NOMEM;
+        }
+        const size_t row = (size_t)2 * c.d_model * 2;
+        if (s->clen > 0)
+            SBK_CUDA_CHECK(cudaMemcpy2DAsync(nb.base, ncap * row, s->kv.base, s->cap * row, s->clen * row,
+                                             (size_t)c.num_encoder_layers * s->B, cudaMemcpyDeviceToDevice, st));
+        SBK_CUDA_CHECK(cudaStreamSynchronize(st));  // the old ring is freed below
+        std::swap(nb.base, s->kv.base);
+        s->kv.cap = stream_kv_bytes(c, s->B, ncap);
+        s->cap = ncap;
+    }
+    const int L = ((n - 1) * 4) * c.hop;  // a sample count whose frame count maps to n encoder frames
+    RC(ensure_workspace(m, s->B, L, std::max(s->B, m->ws_rows), std::max(1, m->ws_steps)));
+    RC(cast_f32_f16(cnn_out_dev, m->b.a_in, (size_t)s->B * n * c.input_size, st));
+    RC(run_encoder(m, nullptr, s->B, n, nullptr, nullptr, enc_out_dev, st, s));
+    s->total += n;
+    if (n < s->chunk) s->ended = true;
+    if (s->left >= 0) {  // keep the last `left` rows of the window
+        const int keep = std::min(W, s->left);
+        s->start = (s->start + W - keep) % s->cap;
+        s->clen = keep;
+    } else {
+        s->clen = W;
+    }
+    return SBK_OK;
+}
+
+int sbk_asr_stream_context(sbk_asr* mm, const sbk_asr_stream* ss, int layer, void* kv_out_dev, float* carry_out_dev,
+                           int* n_rows, void* stream) {
+    const AsrModel* m = reinterpret_cast<const AsrModel*>(mm);
+    const AsrStream* s = reinterpret_cast<const AsrStream*>(ss);
+    SBK_REQUIRE(m && s, "stream_context: null argument");
+    const sbk_asr_config& c = m->wt->cfg;
+    SBK_REQUIRE(layer >= 0 && layer < c.num_encoder_layers, "stream_context: layer %d of %d", layer, c.num_encoder_layers);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (n_rows) *n_rows = s->clen;
+    const size_t row = (size_t)2 * c.d_model * 2;
+    if (kv_out_dev && s->clen > 0) {  // the ring in window order: slots [start, cap) then [0, ...)
+        const uint8_t* src = reinterpret_cast<const uint8_t*>(s->kv_layer(c, layer));
+        const int n1 = std::min(s->clen, s->cap - s->start), n2 = s->clen - n1;
+        uint8_t* dst = static_cast<uint8_t*>(kv_out_dev);
+        SBK_CUDA_CHECK(cudaMemcpy2DAsync(dst, s->clen * row, src + s->start * row, s->cap * row, n1 * row, s->B,
+                                         cudaMemcpyDeviceToDevice, st));
+        if (n2 > 0)
+            SBK_CUDA_CHECK(cudaMemcpy2DAsync(dst + n1 * row, s->clen * row, src, s->cap * row, n2 * row, s->B,
+                                             cudaMemcpyDeviceToDevice, st));
+    }
+    if (carry_out_dev) {
+        const size_t bytes = (size_t)s->B * ((c.kernel_size - 1) / 2) * c.d_model * 4;
+        if (s->total > 0) SBK_CUDA_CHECK(cudaMemcpyAsync(carry_out_dev, s->carry_layer(c, layer), bytes, cudaMemcpyDeviceToDevice, st));
+        else SBK_CUDA_CHECK(cudaMemsetAsync(carry_out_dev, 0, bytes, st));
+    }
+    return SBK_OK;
 }
 
 // Full device pipeline on device-resident wav: Fbank -> global CMVN -> CNN -> encoder -> greedy.

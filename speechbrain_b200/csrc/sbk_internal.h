@@ -122,13 +122,32 @@ int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, cons
                      const HyperMixWeights& w, float* part, __half* G, float* gscale, float* x, cudaStream_t stream);
 size_t hypermix_part_floats(int B, int T, int d, int KH);
 void hypermix_pe_table(int d, float* dst);  // [HM_PE_ROWS, d] (host)
-// chunk > 0: Dynamic Chunk Convolution (inputs past the end of the output frame's chunk are zero)
+// chunk > 0: Dynamic Chunk Convolution (inputs past the end of the output frame's chunk are zero).  left: [B, (K-1)/2, D]
+// inputs of the frames before frame 0 (a stream's carry), null = zero padding.
 int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw,
-                    const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk = 0);
+                    const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk = 0,
+                    const float* left = nullptr);
+// carry [B, (K-1)/2, D] <- the last (K-1)/2 rows of [carry; glu [B, n, D]]; has_old false: the old carry counts as zeros
+int dwconv_carry(const float* glu, int B, int n, int D, int K, bool has_old, float* carry, cudaStream_t stream);
 void dwconv_repack_taps(const float* src, int D, int K, float* dst);  // (D, 1, K) -> tap-major [K, D] (host)
 int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_dim, const int* lens, bool relpos,
                       const float* pos_u, const float* pos_v, const __half* P, int ldp, float scale, __half* out,
                       int ldo, cudaStream_t stream, int chunk = 0, int left_chunks = -1);
+// One chunk of a stream: the window is W rows [cached rows; the chunk's nq rows], all visible to every query.
+struct AttStream {
+    const __half* q = nullptr; int ldq = 0;  // [B * nq, ldq] the chunk's queries, head h at column h * head_dim
+    const __half* kv = nullptr; int ldkv = 0;  // ring [B][cap][ldkv]: head h's [k | v] at column h * 2 * head_dim
+    int cap = 0, start = 0;                    // window row r lives in slot (start + r) % cap
+    int nq = 0;
+};
+// out [B * nq, ldo] fp16; RelPos: P [>= W rows, ldp] = linear_pos(pe[|r|]); RoPE: q and k arrive rotated, q scaled
+int encoder_attention_stream(const AttStream& sa, int B, int W, int H, int head_dim, bool relpos, const float* pos_u,
+                             const float* pos_v, const __half* P, int ldp, float scale, __half* out, int ldo,
+                             cudaStream_t stream);
+// qkv [B*n, 3d] fp32 -> q [B*n, d] fp16 and the rows' [k | v] into ring slots (slot0 + i) % cap of kv [B][cap][2d] fp16;
+// inv_freq [head_dim / 2] set: RoPE at stream positions pos0 + i, q scaled by q_scale
+int stream_qkv(const float* qkv, int B, int n, int H, int DH, const float* inv_freq, long long pos0, float q_scale,
+               __half* q, __half* kv, int cap, int slot0, cudaStream_t stream);
 // TransformerLM whole-sequence causal self-attention: qkv [n*s, 3d] fp16 ([q | k | v], head_dim 64, q pre-scaled), tokens
 // [n, s] int32 (keys whose id == pad_tok are masked) -> out [n*s, d] fp16
 int lm_causal_attention(const __half* qkv, int n, int s, int d, int H, const int* tokens, int pad_tok, __half* out,

@@ -228,6 +228,10 @@ class AsrEngine:
                   "sbk_asr_encode_from_cnn")
         return out
 
+    def stream_create(self, B, chunk_size, left_frames=None):
+        """A chunk-by-chunk encoder stream of B streams on this engine's weights (left_frames None = the whole past)."""
+        return EncoderStream(self, B, chunk_size, left_frames)
+
     def encode_feats(self, feats, wav_lens=None, want_cnn=False):
         feats = feats.float().contiguous()
         B, T0, _ = feats.shape
@@ -401,3 +405,57 @@ class AsrEngine:
                                                        ptr(pred_host), None, ctypes.byref(done), self._sp()),
                   "sbk_asr_transcribe_greedy_host")
         return pred_host, done.value
+
+
+class EncoderStream:
+    """Per-layer left-context caches of B Conformer streams that advance together (sbk_asr_stream_*): ``encode_chunk`` maps
+    the CNN output of one chunk [B, n <= chunk_size, input_size] to the encoder output [B, n, d_model] at a cost that does
+    not grow with the stream's length."""
+
+    def __init__(self, engine, B, chunk_size, left_frames=None):
+        self.engine, self.B, self.chunk_size = engine, int(B), int(chunk_size)
+        self.left_frames = None if left_frames is None else int(left_frames)
+        self._s = ctypes.c_void_p()
+        with torch.cuda.device(engine.device):
+            check(lib().sbk_asr_stream_create(engine._h, self.B, self.chunk_size, -1 if left_frames is None else self.left_frames,
+                                              ctypes.byref(self._s)), "sbk_asr_stream_create")
+
+    def __del__(self):
+        try:
+            if getattr(self, "_s", None) and self._s.value:
+                lib().sbk_asr_stream_destroy(self._s)
+                self._s = None
+        except Exception:  # interpreter shutdown
+            pass
+
+    def encode_chunk(self, src):
+        src = src.float().contiguous()
+        B, n, F = src.shape
+        if B != self.B or F != self.engine.cfg["input_size"]:
+            raise ValueError(f"EncoderStream: expected [{self.B}, n, {self.engine.cfg['input_size']}], got {list(src.shape)}")
+        out = torch.empty(B, n, self.engine.cfg["d_model"], device=src.device, dtype=torch.float32)
+        with torch.cuda.device(self.engine.device):
+            check(lib().sbk_asr_stream_encode_chunk(self.engine._h, self._s, ptr(src), n, ptr(out), self.engine._sp()),
+                  "sbk_asr_stream_encode_chunk")
+        return out
+
+    def reset(self):
+        check(lib().sbk_asr_stream_reset(self._s), "sbk_asr_stream_reset")
+
+    def cached_frames(self):
+        n = ctypes.c_int()
+        check(lib().sbk_asr_stream_context(self.engine._h, self._s, 0, None, None, ctypes.byref(n), None), "sbk_asr_stream_context")
+        return n.value
+
+    def layer_context(self, layer):
+        """Copies of layer ``layer``'s caches: (kv [B, cached, 2 * d_model] fp16, per head [key | value]; carry
+        [B, (kernel_size - 1) / 2, d_model] fp32, the depthwise-conv inputs of the last frames)."""
+        d, K = self.engine.cfg["d_model"], self.engine.cfg.get("kernel_size", 31)
+        n = self.cached_frames()
+        dev = self.engine.device
+        kv = torch.empty(self.B, n, 2 * d, device=dev, dtype=torch.float16)
+        carry = torch.empty(self.B, (K - 1) // 2, d, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            check(lib().sbk_asr_stream_context(self.engine._h, self._s, int(layer), ptr(kv), ptr(carry), None, self.engine._sp()),
+                  "sbk_asr_stream_context")
+        return kv, carry

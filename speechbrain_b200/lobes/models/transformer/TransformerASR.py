@@ -216,49 +216,45 @@ class TransformerASR(torch.nn.Module):
             eng.set_dynchunk(0)
 
     # ------------------------------------------------------------------ streaming (TransformerASR.py:546-670)
-    def make_streaming_context(self, dynchunktrain_config):
-        """Streaming context for ``encode_streaming`` (TransformerASR.py:645-670)."""
+    def _check_streaming(self):
         if self.encoder_module == "transformer":
             raise NotImplementedError("TransformerASR: streaming for the Transformer encoder is not built")
         if self.encoder_module == "branchformer":
             raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
         if self.attention_type == "hypermixing":
             raise NotImplementedError("TransformerASR: HyperMixing has no streaming mode")
+
+    def make_streaming_context(self, dynchunktrain_config):
+        """Streaming context for ``encode_streaming`` (TransformerASR.py:645-670).  An infinite left context
+        (``left_context_size=None``) is accepted: the context then keeps every frame (with RelPosMHAXL, up to max_length)."""
+        self._check_streaming()
         if dynchunktrain_config is None or dynchunktrain_config.chunk_size <= 0:
             raise ValueError("make_streaming_context needs a DynChunkTrainConfig with chunk_size > 0")
-        return TransformerASRStreamingContext(dynchunktrain_config)
+        return TransformerASRStreamingContext(dynchunktrain_config, ConformerEncoderStreamingContext(
+            dynchunktrain_config, self.num_encoder_layers, self.nhead))
 
     @torch.no_grad()
     def encode_streaming(self, src, context):
-        """Encoder output for one more chunk of ``src`` [B, chunk_size, F] (TransformerASR.py:546-643).
+        """Encoder output for one more chunk of ``src`` [B, n <= chunk_size, F] (TransformerASR.py:546-643).
 
-        The reference carries per-layer left-context caches; its outputs equal the masked full-sequence run
-        (``encode(..., dynchunktrain_config)``, tests/unittests/test_conformer.py).  This implementation keeps the chunk
-        *inputs* seen so far in the context and re-runs that masked encode over the window the new chunk can depend on
-        (12 layers x (left context + convolution halo); everything, for an infinite left context), returning the rows of the
-        new chunk: the same values, at the cost of recomputing the window instead of reusing per-layer caches."""
-        if self.encoder_module == "transformer":
-            raise NotImplementedError("TransformerASR: streaming for the Transformer encoder is not built")
-        if self.encoder_module == "branchformer":
-            raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
-        if self.attention_type == "hypermixing":
-            raise NotImplementedError("TransformerASR: HyperMixing has no streaming mode")
+        The context keeps, per layer, the projected keys / values of the left context and the Dynamic Chunk Convolution's
+        last (kernel_size - 1) / 2 inputs on the device, so every chunk costs the same however long the stream.  The outputs
+        equal the masked full-sequence run ``encode(..., dynchunktrain_config)`` (tests/unittests/test_conformer.py).  The B
+        streams of a batch advance together; only the last chunk of a stream may be shorter than chunk_size."""
+        self._check_streaming()
         require_cuda(src, "TransformerASR.encode_streaming")
-        cfg = context.dynchunktrain_config
         if src.dim() == 4:
             src = src.reshape(src.shape[0], src.shape[1], -1)
-        if context.history is not None and context.history.shape[1] % cfg.chunk_size != 0:
-            raise ValueError("encode_streaming: only the last chunk of a stream may be shorter than chunk_size")
-        hist = src if context.history is None else torch.cat([context.history, src], dim=1)
-        out = self.encode(hist, None, dynchunktrain_config=cfg)[:, -src.shape[1]:].contiguous()
-        if not cfg.is_infinite_left_context():  # trim to the receptive field of the next chunk, on a chunk boundary
-            halo = (self.kernel_size - 1) // 2
-            per_layer = max(cfg.left_context_size * cfg.chunk_size + cfg.chunk_size - 1, halo)
-            keep = self.num_encoder_layers * per_layer + cfg.chunk_size
-            keep = -(-keep // cfg.chunk_size) * cfg.chunk_size
-            if hist.shape[1] > keep and hist.shape[1] % cfg.chunk_size == 0:
-                hist = hist[:, -keep:]
-        context.history = hist
+        ec = context.encoder_context
+        eng = self._get_engine(src.device)
+        if ec.stream is None or ec.stream.engine is not eng or ec.stream.B != src.shape[0]:
+            if ec.stream is not None and ec.frames > 0:
+                raise ValueError("encode_streaming: the batch size or the model's weights changed inside a stream")
+            cfg = context.dynchunktrain_config
+            left = None if cfg.is_infinite_left_context() else cfg.left_context_size * cfg.chunk_size
+            ec.stream = eng.stream_create(src.shape[0], cfg.chunk_size, left)
+        out = ec.stream.encode_chunk(src)
+        ec.frames += src.shape[1]
         return out
 
     def _decoder_engine(self, device):
@@ -294,12 +290,72 @@ class TransformerASR(torch.nn.Module):
         return enc, dec
 
 
-class TransformerASRStreamingContext:
-    """Mutable streaming state (TransformerASR.py:26-43): the DynChunkTrainConfig and the chunk inputs seen so far."""
+class ConformerEncoderLayerStreamingContext:
+    """One layer's streaming state (Conformer.py:27-60), read from the device caches on access."""
 
-    def __init__(self, dynchunktrain_config):
+    def __init__(self, parent, index, mha_left_context_size):
+        self._parent, self._index = parent, index
+        self.mha_left_context_size = mha_left_context_size
+
+    def _caches(self):
+        st = self._parent.stream
+        return None if st is None or self._parent.frames == 0 else st.layer_context(self._index)
+
+    @property
+    def mha_left_context(self):
+        """The projected keys of the cached frames [B, frames, d_model] (fp16; RoPE keys rotated by stream position), or
+        None before the first chunk.  The shape is the reference's, the values are not: the reference keeps the layer
+        inputs of the same frames and projects them again for every chunk."""
+        c = self._caches()
+        if c is None:
+            return None
+        kv = c[0]
+        B, n, _ = kv.shape
+        H = self._parent.nhead
+        return kv.view(B, n, H, 2, kv.shape[2] // (2 * H))[:, :, :, 0].reshape(B, n, kv.shape[2] // 2)
+
+    @property
+    def dcconv_left_context(self):
+        """The depthwise convolution's inputs of the last (kernel_size - 1) / 2 frames [B, (kernel_size - 1) / 2, d_model]
+        (fp32, after the GLU; LayerNorm, pointwise conv and GLU act per frame), or None before the first chunk."""
+        c = self._caches()
+        return None if c is None else c[1]
+
+
+class ConformerEncoderStreamingContext:
+    """Streaming state of a Conformer encoder (Conformer.py:63-80): ``layers[i]`` per layer, backed by one device stream."""
+
+    def __init__(self, dynchunktrain_config, num_layers, nhead):
+        cfg = dynchunktrain_config
+        # frames of left context per layer; None: every frame so far (the reference has no such mode)
+        size = None if cfg.is_infinite_left_context() else cfg.left_context_size * cfg.chunk_size
+        self.stream = None  # speechbrain_b200.engine.EncoderStream, created by the first chunk
+        self.frames = 0
+        self.nhead = nhead
+        self.layers = [ConformerEncoderLayerStreamingContext(self, i, size) for i in range(num_layers)]
+
+    def reset(self):
+        """Back to an empty context (the device buffers are kept for the next stream of the same batch size)."""
+        if self.stream is not None:
+            self.stream.reset()
+        self.frames = 0
+
+
+class TransformerASRStreamingContext:
+    """Mutable streaming state (TransformerASR.py:26-43): the DynChunkTrainConfig and the encoder's per-layer context."""
+
+    def __init__(self, dynchunktrain_config, encoder_context):
         self.dynchunktrain_config = dynchunktrain_config
-        self.history = None
+        self.encoder_context = encoder_context
+
+    def reset(self):
+        """Forget the stream: the next chunk starts a new one, with the same configuration."""
+        self.encoder_context.reset()
+
+    @property
+    def history(self):
+        """The frames the context retains (layer 0's left context [B, frames, d_model]), or None before the first chunk."""
+        return self.encoder_context.layers[0].mha_left_context if self.encoder_context.layers else None
 
 
 class EncoderWrapper(torch.nn.Module):
