@@ -1052,23 +1052,6 @@ static int copy_steps(const AsrModel* m, void* dst, int ld, const void* src, int
     return SBK_OK;
 }
 
-// Decoder pre-norm feeding a projection: either fused into the projection kernel (a.X) or a separate tiny kernel
-// writing fp16 (a.A).  Fusion saves a launch per projection (single-batch latency); the separate kernel avoids
-// recomputing the same 32-row LayerNorm in ~100-300 CTAs (GPU time when several batches are in flight).
-static int dec_ln(AsrModel* m, SkinnyArgs& a, const float* g, const float* bta, int rows, cudaStream_t st) {
-    AsrModel::Buf& b = m->b;
-    const int d = m->wt->cfg.d_model;
-    if (m->fuse_dec_ln && (d == 256 || d == 512 || d == 768 || d == 1024)) {  // widths the LN-fused projection is built for
-        a.X = b.dx; a.ln_g = g; a.ln_b = bta; a.ln_eps = 1e-6f;
-        return SBK_OK;
-    }
-    a.A = b.dh16; a.lda = d;
-    return layernorm_rows(b.dx, b.dh16, true, g, bta, rows, d, 1e-6f, false, st);
-}
-
-// Decode step when many hypotheses are live (several batches decoded together, or a wide beam): the projections run on
-// the wgmma GEMM (64 x 32/64 tiles, a handful of CTAs each, so concurrent lanes share the GPU) instead of the
-// weight-streaming kernel whose cost grows with every 32 rows.  Same maths: fp16 operands, fp32 accumulate / residual.
 // Cross-attention K/V of every decoder layer, projected once per utterance from the encoder states (b.enc16).  Layout per
 // layer (default): [K | V] parts, each [utt][head][T][64] -- the decode-step attention of (utterance, head) then streams one
 // contiguous T x 128 B block of K and one of V instead of 128-byte pieces 2 KB apart (SBK_XATT_ROWMAJOR=1: the round-1
@@ -1107,121 +1090,113 @@ static void cross_kv_args(const AsrModel* m, DecAttnArgs& t, int l, int n_utt, i
     }
 }
 
-static int enqueue_decode_layers_tc(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage,
-                                    cudaStream_t st, bool with_head) {
-    const sbk_asr_config& c = m->wt->cfg;
-    AsrModel::Buf& b = m->b;
-    const int d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H, Ld = c.num_decoder_layers;
-    const int n_utt = rows / rows_per_utt;
-    for (int l = 0; l < Ld; ++l) {
-        const DecLayerW& w = m->wt->dec[l];
-        __half* kc = b.kcache + (size_t)l * rows * S_max * d;
-        __half* vc = b.vcache + (size_t)l * rows * S_max * d;
-        RC(layernorm_rows(b.dx, b.dh16, true, w.n1g, w.n1b, rows, d, 1e-6f, false, st, true));
-        GemmEpilogue e;
-        e.mode = EPI_QKV_CACHE; e.bias = w.b_self_in; e.out = b.dq16; e.ldo = d; e.kcache = kc; e.vcache = vc;
-        e.step_ptr = b.step; e.S_max = S_max; e.qkv_d = d;
-        RC(gemm_f16_small(b.dh16, d, w.w_self_in, d, e, rows, 3 * d, d, st));
-        DecAttnArgs t{};
-        t.q = b.dq16; t.ldq = d; t.kbase = kc; t.vbase = vc; t.row_stride = (size_t)S_max * d; t.key_stride = d;
-        t.rows_per_block = 1; t.n_keys_ptr = b.step; t.enc_len = nullptr; t.H = H; t.dh = dh; t.out = b.datt16; t.ldo = d;
-        t.lineage = lineage; t.lin_stride = S_max;
-        RC(dec_attention(t, rows, S_max, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_self_out; e.out = b.dx; e.resid = b.dx; e.ldo = d;
-        RC(gemm_f16_small(b.datt16, d, w.w_self_out, d, e, rows, d, d, st));
-        RC(layernorm_rows(b.dx, b.dh16, true, w.n2g, w.n2b, rows, d, 1e-6f, false, st, true));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.b_cross_q; e.out = b.dq16; e.ldo = d;
-        RC(gemm_f16_small(b.dh16, d, w.w_cross_q, d, e, rows, d, d, st));
-        t = DecAttnArgs{};
-        t.q = b.dq16; t.ldq = d; cross_kv_args(m, t, l, n_utt, T); t.rows_per_block = rows_per_utt;
-        t.n_keys_ptr = nullptr; t.enc_len = b.enc_len; t.H = H; t.dh = dh; t.out = b.datt16; t.ldo = d;
-        RC(dec_attention(t, rows, T, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_cross_out; e.out = b.dx; e.resid = b.dx; e.ldo = d;
-        RC(gemm_f16_small(b.datt16, d, w.w_cross_out, d, e, rows, d, d, st));
-        RC(layernorm_rows(b.dx, b.dh16, true, w.n3g, w.n3b, rows, d, 1e-6f, false, st, true));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = c.decoder_activation == SBK_ACT_GELU ? ACT_GELU : ACT_RELU;
-        e.bias = w.b_ffn1; e.out = b.df16; e.ldo = F;
-        RC(gemm_f16_small(b.dh16, d, w.w_ffn1, d, e, rows, F, d, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_ffn2; e.out = b.dx; e.resid = b.dx; e.ldo = d;
-        RC(gemm_f16_small(b.df16, F, w.w_ffn2, F, e, rows, d, F, st));
+// ---------------------------------------------------------------------------- decode / TransformerLM step projections
+// The GEMM that runs a step's Linears.  The weight-streaming kernel (skinny_gemm) suits few live rows, but its cost grows
+// with every 32 rows; from dec_tc_rows rows on (several batches decoded together, or a wide beam) the wgmma GEMM
+// (gemm_f16_small: 64 x 32/64 tiles, a handful of CTAs each, so concurrent lanes share the GPU) takes over.  The
+// whole-sequence LM runs on the encoder's GEMM (gemm_f16).  Same maths on all three: fp16 operands, fp32 accumulate /
+// residual.
+enum StepGemm { SG_STREAM, SG_SMALL, SG_WIDE };
+
+// The back end of a step over `rows` live rows of width `width` (the wgmma QKV -> cache scatter epilogue works on 32-column
+// chunks).
+static StepGemm step_gemm(const AsrModel* m, int rows, int width) {
+    return rows >= m->dec_tc_rows && width % 32 == 0 ? SG_SMALL : SG_STREAM;
+}
+// Programmatic dependent launch is on for the wgmma step (its GEMMs and LayerNorms are launched with it unconditionally)
+// and off for weight streaming, where it measured no faster (single_batch, H100 SXM at 400 W: 24.8 / 28.2 ms with it
+// against 23.4 / 23.3 ms without).  Every entry that runs a step loop sets it before the loop.
+static void set_step_pdl(const AsrModel* m, int rows, int width) { set_pdl(step_gemm(m, rows, width) == SG_SMALL); }
+
+// What a step's Linear writes: fp16 (optionally through GELU / ReLU), fp32, fp32 added in place to `out` (the residual
+// stream), or the self-attention in_proj's [q | k | v]: q to `out`, k and v into the caches at (row, step_ptr[row]).
+enum ProjOut { PO_F16, PO_F16_GELU, PO_F16_RELU, PO_F32, PO_RESID, PO_QKV_CACHE };
+// One Linear of a step: out[rows, N] (row stride ldo) = epilogue(A[rows, K] (row stride lda) x W[N, K]^T + bias).
+struct Proj {
+    const __half* W; const float* bias; int N, K;
+    ProjOut kind; void* out; int ldo;
+    const __half* A = nullptr; int lda = 0;
+    __half* kcache = nullptr; __half* vcache = nullptr; const int* step_ptr = nullptr; int S_max = 0;  // PO_QKV_CACHE
+    const float* X = nullptr; const float* ln_g = nullptr; const float* ln_b = nullptr;  // SG_STREAM: A = LayerNorm(X) in-kernel
+};
+
+static int project(StepGemm g, const Proj& p, int rows, cudaStream_t st) {
+    if (g == SG_STREAM) {
+        static const int skinny_epi[] = {SK_F16, SK_F16_GELU, SK_F16_RELU, SK_F32, SK_RESID, SK_QKV_CACHE};
+        SkinnyArgs a{};
+        a.A = p.A; a.lda = p.lda; a.W = p.W; a.ldw = p.K; a.bias = p.bias; a.n_rows = rows; a.N = p.N; a.K = p.K;
+        a.epi = skinny_epi[p.kind]; a.out = p.out; a.ldo = p.ldo;
+        if (p.kind == PO_QKV_CACHE) {
+            a.kcache = p.kcache; a.vcache = p.vcache; a.step_ptr = p.step_ptr; a.S_max = p.S_max; a.d = p.N / 3; a.q_scale = 1.0f;
+        }
+        if (p.X) { a.X = p.X; a.ln_g = p.ln_g; a.ln_b = p.ln_b; a.ln_eps = 1e-6f; }
+        return skinny_gemm(a, st);
     }
-    if (!with_head) return SBK_OK;
-    SBK_REQUIRE(m->wt->w_lin != nullptr, "decode step: this handle was created without the output head (seq_lin.w.*)");
-    RC(layernorm_rows(b.dx, b.dh16, true, m->wt->dec_norm_g, m->wt->dec_norm_b, rows, d, 1e-6f, false, st, true));
     GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->wt->b_lin; e.out = b.logits; e.ldo = c.vocab;
-    RC(gemm_f16_small(b.dh16, d, m->wt->w_lin, d, e, rows, c.vocab, d, st));
-    return SBK_OK;
+    e.mode = p.kind == PO_F32 ? EPI_F32 : p.kind == PO_RESID ? EPI_RESID : p.kind == PO_QKV_CACHE ? EPI_QKV_CACHE : EPI_F16;
+    e.act = p.kind == PO_F16_GELU ? ACT_GELU : p.kind == PO_F16_RELU ? ACT_RELU : ACT_NONE;
+    e.bias = p.bias; e.out = p.out; e.ldo = p.ldo;
+    if (p.kind == PO_RESID) e.resid = static_cast<const float*>(p.out);
+    if (p.kind == PO_QKV_CACHE) {
+        e.kcache = p.kcache; e.vcache = p.vcache; e.step_ptr = p.step_ptr; e.S_max = p.S_max; e.qkv_d = p.N / 3;
+    }
+    if (g == SG_SMALL) return gemm_f16_small(p.A, p.lda, p.W, p.K, e, rows, p.N, p.K, st);
+    return gemm_f16(p.A, p.lda, p.W, p.K, e, rows, p.N, p.K, st);
 }
 
-// the wgmma decode path (enqueue_decode_layers_tc) for `rows` live hypotheses
-static bool decode_tc(const AsrModel* m, int rows) {
-    return rows >= m->dec_tc_rows && m->wt->cfg.d_model % 32 == 0;  // (the QKV -> cache scatter epilogue works on 32-column chunks)
+// A decoder pre-norm LN(b.dx) and the projection it feeds.  Weight streaming fuses the LayerNorm into the projection kernel
+// where that kernel is built for the width, which saves a launch per projection (single-batch latency); with fusion off it
+// runs a separate kernel into b.dh16, which avoids recomputing the same 32-row LayerNorm in ~100-300 CTAs (GPU time when
+// several batches are in flight).  The wgmma step always runs the separate kernel, launched with PDL.
+static int dec_norm_project(AsrModel* m, StepGemm g, Proj p, const float* gamma, const float* beta, int rows, cudaStream_t st) {
+    AsrModel::Buf& b = m->b;
+    const int d = m->wt->cfg.d_model;
+    if (g == SG_STREAM && m->fuse_dec_ln && (d == 256 || d == 512 || d == 768 || d == 1024)) {
+        p.X = b.dx; p.ln_g = gamma; p.ln_b = beta;
+    } else {
+        RC(layernorm_rows(b.dx, b.dh16, true, gamma, beta, rows, d, 1e-6f, false, st, g != SG_STREAM));
+        p.A = b.dh16; p.lda = d;
+    }
+    return project(g, p, rows, st);
 }
-// Programmatic dependent launch is on for the wgmma decode path (its GEMMs and LayerNorms are launched with it
-// unconditionally) and off on the weight-streaming path, where it measured no faster (single_batch, H100 SXM at 400 W:
-// 24.8 / 28.2 ms with it against 23.4 / 23.3 ms without).
-static void set_decode_pdl(const AsrModel* m, int rows) { set_pdl(decode_tc(m, rows)); }
 
 static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage,
                                  cudaStream_t st, bool with_head = true) {
-    if (decode_tc(m, rows))
-        return enqueue_decode_layers_tc(m, rows, rows_per_utt, T, S_max, lineage, st, with_head);
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H, Ld = c.num_decoder_layers;
-    const int ffn_epi = c.decoder_activation == SBK_ACT_GELU ? SK_F16_GELU : SK_F16_RELU;
+    const ProjOut ffn_act = c.decoder_activation == SBK_ACT_GELU ? PO_F16_GELU : PO_F16_RELU;
     const int n_utt = rows / rows_per_utt;
+    const StepGemm g = step_gemm(m, rows, d);
     // b.dx already holds emb[token] * sqrt(d) + pe[step] (written by greedy_reset / the previous greedy_select)
     for (int l = 0; l < Ld; ++l) {
         const DecLayerW& w = m->wt->dec[l];
         __half* kc = b.kcache + (size_t)l * rows * S_max * d;
         __half* vc = b.vcache + (size_t)l * rows * S_max * d;
-        SkinnyArgs a{};  // LN1 + self-attention in_proj; k/v appended to the cache at position step
-        RC(dec_ln(m, a, w.n1g, w.n1b, rows, st));
-        a.W = w.w_self_in; a.ldw = d; a.bias = w.b_self_in; a.n_rows = rows; a.N = 3 * d; a.K = d;
-        a.epi = SK_QKV_CACHE; a.out = b.dq16; a.ldo = d; a.kcache = kc; a.vcache = vc; a.step_ptr = b.step; a.S_max = S_max;
-        a.d = d; a.q_scale = 1.0f;
-        RC(skinny_gemm(a, st));
+        Proj qkv{w.w_self_in, w.b_self_in, 3 * d, d, PO_QKV_CACHE, b.dq16, d};  // LN1 + self-attention in_proj
+        qkv.kcache = kc; qkv.vcache = vc; qkv.step_ptr = b.step; qkv.S_max = S_max;
+        RC(dec_norm_project(m, g, qkv, w.n1g, w.n1b, rows, st));
         DecAttnArgs t{};
         t.q = b.dq16; t.ldq = d; t.kbase = kc; t.vbase = vc; t.row_stride = (size_t)S_max * d; t.key_stride = d;
         t.rows_per_block = 1; t.n_keys_ptr = b.step; t.enc_len = nullptr; t.H = H; t.dh = dh; t.out = b.datt16; t.ldo = d;
         t.lineage = lineage; t.lin_stride = S_max;
         RC(dec_attention(t, rows, S_max, st));
-        a = SkinnyArgs{}; a.A = b.datt16; a.lda = d; a.W = w.w_self_out; a.ldw = d; a.bias = w.b_self_out; a.n_rows = rows;
-        a.N = d; a.K = d; a.epi = SK_RESID; a.out = b.dx; a.ldo = d;
-        RC(skinny_gemm(a, st));
+        RC(project(g, {w.w_self_out, w.b_self_out, d, d, PO_RESID, b.dx, d, b.datt16, d}, rows, st));
         // cross attention: LN2 + (pre-scaled) query projection
-        a = SkinnyArgs{};
-        RC(dec_ln(m, a, w.n2g, w.n2b, rows, st));
-        a.W = w.w_cross_q; a.ldw = d; a.bias = w.b_cross_q; a.n_rows = rows;
-        a.N = d; a.K = d; a.epi = SK_F16; a.out = b.dq16; a.ldo = d;
-        RC(skinny_gemm(a, st));
+        RC(dec_norm_project(m, g, {w.w_cross_q, w.b_cross_q, d, d, PO_F16, b.dq16, d}, w.n2g, w.n2b, rows, st));
         t = DecAttnArgs{};
         t.q = b.dq16; t.ldq = d; cross_kv_args(m, t, l, n_utt, T); t.rows_per_block = rows_per_utt;
         t.n_keys_ptr = nullptr; t.enc_len = b.enc_len; t.H = H; t.dh = dh; t.out = b.datt16; t.ldo = d;
         RC(dec_attention(t, rows, T, st));
-        a = SkinnyArgs{}; a.A = b.datt16; a.lda = d; a.W = w.w_cross_out; a.ldw = d; a.bias = w.b_cross_out; a.n_rows = rows;
-        a.N = d; a.K = d; a.epi = SK_RESID; a.out = b.dx; a.ldo = d;
-        RC(skinny_gemm(a, st));
+        RC(project(g, {w.w_cross_out, w.b_cross_out, d, d, PO_RESID, b.dx, d, b.datt16, d}, rows, st));
         // feed-forward: LN3 + ffn1 + activation, then ffn2 + residual
-        a = SkinnyArgs{};
-        RC(dec_ln(m, a, w.n3g, w.n3b, rows, st));
-        a.W = w.w_ffn1; a.ldw = d; a.bias = w.b_ffn1; a.n_rows = rows;
-        a.N = F; a.K = d; a.epi = ffn_epi; a.out = b.df16; a.ldo = F;
-        RC(skinny_gemm(a, st));
-        a = SkinnyArgs{}; a.A = b.df16; a.lda = F; a.W = w.w_ffn2; a.ldw = F; a.bias = w.b_ffn2; a.n_rows = rows;
-        a.N = d; a.K = F; a.epi = SK_RESID; a.out = b.dx; a.ldo = d;
-        RC(skinny_gemm(a, st));
+        RC(dec_norm_project(m, g, {w.w_ffn1, w.b_ffn1, F, d, ffn_act, b.df16, F}, w.n3g, w.n3b, rows, st));
+        RC(project(g, {w.w_ffn2, w.b_ffn2, d, F, PO_RESID, b.dx, d, b.df16, F}, rows, st));
     }
     if (!with_head) return SBK_OK;
     SBK_REQUIRE(m->wt->w_lin != nullptr, "decode step: this handle was created without the output head (seq_lin.w.*)");
-    SkinnyArgs a{};  // final LayerNorm + seq_lin
-    RC(dec_ln(m, a, m->wt->dec_norm_g, m->wt->dec_norm_b, rows, st));
-    a.W = m->wt->w_lin; a.ldw = d; a.bias = m->wt->b_lin; a.n_rows = rows; a.N = c.vocab; a.K = d;
-    a.epi = SK_F32; a.out = b.logits; a.ldo = c.vocab;
-    RC(skinny_gemm(a, st));
-    return SBK_OK;
+    return dec_norm_project(m, g, {m->wt->w_lin, m->wt->b_lin, c.vocab, d, PO_F32, b.logits, c.vocab}, m->wt->dec_norm_g,
+                            m->wt->dec_norm_b, rows, st);  // final LayerNorm + seq_lin
 }
 
 static int enqueue_decode_step(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, int eos, float* log_probs,
@@ -1233,91 +1208,56 @@ static int enqueue_decode_step(AsrModel* m, int rows, int rows_per_utt, int T, i
     return SBK_OK;
 }
 
+// A post-norm TransformerLM layer after its self-attention (Transformer.py:466-481): x = norm1(x + out_proj(att)), then
+// x = norm2(x + ffn(x)).  x is the fp32 residual stream [rows, d] and x16 its fp16 copy; f16 [rows, d_ffn] is scratch.
+static int lm_layer_tail(const AsrModel* m, StepGemm g, const LmLayerW& w, int rows, const __half* att16, float* x,
+                         __half* x16, __half* f16, cudaStream_t st) {
+    const sbk_asr_config& c = m->wt->cfg;
+    const int dl = c.lm_d_model, Fl = c.lm_d_ffn;
+    const ProjOut act = c.lm_activation == SBK_ACT_GELU ? PO_F16_GELU : PO_F16_RELU;
+    RC(project(g, {w.w_out, w.b_out, dl, dl, PO_RESID, x, dl, att16, dl}, rows, st));
+    RC(layernorm_dual(x, x16, w.n1g, w.n1b, rows, dl, 1e-6f, true, st));
+    RC(project(g, {w.w1, w.b1, Fl, dl, act, f16, Fl, x16, dl}, rows, st));
+    RC(project(g, {w.w2, w.b2, dl, Fl, PO_RESID, x, dl, f16, Fl}, rows, st));
+    return layernorm_dual(x, x16, w.n2g, w.n2b, rows, dl, 1e-6f, true, st);
+}
+
+// The LM's encoder.norm, then output_proj: Linear d -> d (fp32 into h32), LayerNorm (fp16 into h16), Linear d -> vocab
+// (fp32 into logits).
+static int lm_output(const AsrModel* m, StepGemm g, int rows, float* x, __half* x16, float* h32, __half* h16, float* logits,
+                     cudaStream_t st) {
+    const AsrWeights& W = *m->wt;
+    const int dl = W.cfg.lm_d_model, V = W.cfg.vocab;
+    RC(layernorm_dual(x, x16, W.lm_norm_g, W.lm_norm_b, rows, dl, 1e-6f, false, st));
+    RC(project(g, {W.lm_wp0, W.lm_bp0, dl, dl, PO_F32, h32, dl, x16, dl}, rows, st));
+    RC(layernorm_dual(h32, h16, W.lm_lnp_g, W.lm_lnp_b, rows, dl, 1e-6f, false, st));
+    return project(g, {W.lm_wp2, W.lm_bp2, V, dl, PO_F32, logits, V, h16, dl}, rows, st);
+}
+
 // One TransformerLM step over `rows` hypotheses (post-norm encoder layers with a lineage-indexed KV cache), ending in
 // b.lm_extra[rows, V] = weight * log_softmax(lm_logits / temperature): TransformerLMScorer.score (scorer.py:510-543)
 // scaled by ScorerBuilder's weight.  b.lx / b.lx16 hold emb[token] * sqrt(d) + pe[step] (beam_reset / beam_step).
-// The same step with the projections on the wgmma GEMM (128 x 32/64 tiles): used when many hypotheses are live (wide beams,
-// B * beam >= dec_tc_rows), where the weight-streaming kernel's cost grows with every 32 rows.
-static int enqueue_lm_step_tc(AsrModel* m, int rows, int S_max, float temperature, float weight, cudaStream_t st) {
-    const sbk_asr_config& c = m->wt->cfg;
-    AsrModel::Buf& b = m->b;
-    const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead;
-    for (int l = 0; l < c.lm_layers; ++l) {
-        const LmLayerW& w = m->wt->lm[l];
-        __half* kc = b.lkc + (size_t)l * rows * S_max * dl;
-        __half* vc = b.lvc + (size_t)l * rows * S_max * dl;
-        GemmEpilogue e;
-        e.mode = EPI_QKV_CACHE; e.bias = w.b_in; e.out = b.lq16; e.ldo = dl; e.kcache = kc; e.vcache = vc;
-        e.step_ptr = b.step; e.S_max = S_max; e.qkv_d = dl;
-        RC(gemm_f16_small(b.lx16, dl, w.w_in, dl, e, rows, 3 * dl, dl, st));
-        DecAttnArgs t{};
-        t.q = b.lq16; t.ldq = dl; t.kbase = kc; t.vbase = vc; t.row_stride = (size_t)S_max * dl; t.key_stride = dl;
-        t.rows_per_block = 1; t.n_keys_ptr = b.step; t.H = H; t.dh = 64; t.out = b.latt16; t.ldo = dl;
-        t.lineage = b.lineage; t.lin_stride = S_max; t.tok_cache = b.tok_cache; t.pad_tok = 0;
-        RC(dec_attention(t, rows, S_max, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_out; e.out = b.lx; e.resid = b.lx; e.ldo = dl;
-        RC(gemm_f16_small(b.latt16, dl, w.w_out, dl, e, rows, dl, dl, st));
-        RC(layernorm_dual(b.lx, b.lx16, w.n1g, w.n1b, rows, dl, 1e-6f, true, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = c.lm_activation == SBK_ACT_GELU ? ACT_GELU : ACT_RELU;
-        e.bias = w.b1; e.out = b.lf16; e.ldo = Fl;
-        RC(gemm_f16_small(b.lx16, dl, w.w1, dl, e, rows, Fl, dl, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b2; e.out = b.lx; e.resid = b.lx; e.ldo = dl;
-        RC(gemm_f16_small(b.lf16, Fl, w.w2, Fl, e, rows, dl, Fl, st));
-        RC(layernorm_dual(b.lx, b.lx16, w.n2g, w.n2b, rows, dl, 1e-6f, true, st));
-    }
-    RC(layernorm_dual(b.lx, b.lx16, m->wt->lm_norm_g, m->wt->lm_norm_b, rows, dl, 1e-6f, false, st));  // encoder.norm
-    GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->wt->lm_bp0; e.out = b.lh32; e.ldo = dl;
-    RC(gemm_f16_small(b.lx16, dl, m->wt->lm_wp0, dl, e, rows, dl, dl, st));
-    RC(layernorm_dual(b.lh32, b.lh16, m->wt->lm_lnp_g, m->wt->lm_lnp_b, rows, dl, 1e-6f, false, st));
-    e = GemmEpilogue(); e.mode = EPI_F32; e.bias = m->wt->lm_bp2; e.out = b.lm_logits; e.ldo = c.vocab;
-    RC(gemm_f16_small(b.lh16, dl, m->wt->lm_wp2, dl, e, rows, c.vocab, dl, st));
-    RC(weighted_log_softmax(b.lm_logits, b.lm_extra, rows, c.vocab, temperature, weight, st));
-    return SBK_OK;
-}
-
 static int enqueue_lm_step(AsrModel* m, int rows, int S_max, float temperature, float weight, cudaStream_t st) {
-    if (rows >= m->dec_tc_rows) return enqueue_lm_step_tc(m, rows, S_max, temperature, weight, st);
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
-    const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead;
+    const int dl = c.lm_d_model, H = c.lm_nhead;
+    const StepGemm g = step_gemm(m, rows, dl);
     for (int l = 0; l < c.lm_layers; ++l) {
         const LmLayerW& w = m->wt->lm[l];
         __half* kc = b.lkc + (size_t)l * rows * S_max * dl;
         __half* vc = b.lvc + (size_t)l * rows * S_max * dl;
-        SkinnyArgs a{};
-        a.A = b.lx16; a.lda = dl; a.W = w.w_in; a.ldw = dl; a.bias = w.b_in; a.n_rows = rows; a.N = 3 * dl; a.K = dl;
-        a.epi = SK_QKV_CACHE; a.out = b.lq16; a.ldo = dl; a.kcache = kc; a.vcache = vc; a.step_ptr = b.step; a.S_max = S_max;
-        a.d = dl; a.q_scale = 1.0f;
-        RC(skinny_gemm(a, st));
+        Proj qkv{w.w_in, w.b_in, 3 * dl, dl, PO_QKV_CACHE, b.lq16, dl, b.lx16, dl};
+        qkv.kcache = kc; qkv.vcache = vc; qkv.step_ptr = b.step; qkv.S_max = S_max;
+        RC(project(g, qkv, rows, st));
         DecAttnArgs t{};
         t.q = b.lq16; t.ldq = dl; t.kbase = kc; t.vbase = vc; t.row_stride = (size_t)S_max * dl; t.key_stride = dl;
         t.rows_per_block = 1; t.n_keys_ptr = b.step; t.H = H; t.dh = 64; t.out = b.latt16; t.ldo = dl;
         t.lineage = b.lineage; t.lin_stride = S_max; t.tok_cache = b.tok_cache; t.pad_tok = 0;
         RC(dec_attention(t, rows, S_max, st));
-        a = SkinnyArgs{}; a.A = b.latt16; a.lda = dl; a.W = w.w_out; a.ldw = dl; a.bias = w.b_out; a.n_rows = rows;
-        a.N = dl; a.K = dl; a.epi = SK_RESID; a.out = b.lx; a.ldo = dl;
-        RC(skinny_gemm(a, st));
-        RC(layernorm_dual(b.lx, b.lx16, w.n1g, w.n1b, rows, dl, 1e-6f, true, st));
-        a = SkinnyArgs{}; a.A = b.lx16; a.lda = dl; a.W = w.w1; a.ldw = dl; a.bias = w.b1; a.n_rows = rows;
-        a.N = Fl; a.K = dl; a.epi = c.lm_activation == SBK_ACT_GELU ? SK_F16_GELU : SK_F16_RELU; a.out = b.lf16; a.ldo = Fl;
-        RC(skinny_gemm(a, st));
-        a = SkinnyArgs{}; a.A = b.lf16; a.lda = Fl; a.W = w.w2; a.ldw = Fl; a.bias = w.b2; a.n_rows = rows;
-        a.N = dl; a.K = Fl; a.epi = SK_RESID; a.out = b.lx; a.ldo = dl;
-        RC(skinny_gemm(a, st));
-        RC(layernorm_dual(b.lx, b.lx16, w.n2g, w.n2b, rows, dl, 1e-6f, true, st));
+        RC(lm_layer_tail(m, g, w, rows, b.latt16, b.lx, b.lx16, b.lf16, st));
     }
-    RC(layernorm_dual(b.lx, b.lx16, m->wt->lm_norm_g, m->wt->lm_norm_b, rows, dl, 1e-6f, false, st));  // encoder.norm
-    SkinnyArgs a{};
-    a.A = b.lx16; a.lda = dl; a.W = m->wt->lm_wp0; a.ldw = dl; a.bias = m->wt->lm_bp0; a.n_rows = rows; a.N = dl; a.K = dl;
-    a.epi = SK_F32; a.out = b.lh32; a.ldo = dl;
-    RC(skinny_gemm(a, st));
-    RC(layernorm_dual(b.lh32, b.lh16, m->wt->lm_lnp_g, m->wt->lm_lnp_b, rows, dl, 1e-6f, false, st));
-    a = SkinnyArgs{}; a.A = b.lh16; a.lda = dl; a.W = m->wt->lm_wp2; a.ldw = dl; a.bias = m->wt->lm_bp2; a.n_rows = rows;
-    a.N = c.vocab; a.K = dl; a.epi = SK_F32; a.out = b.lm_logits; a.ldo = c.vocab;
-    RC(skinny_gemm(a, st));
-    RC(weighted_log_softmax(b.lm_logits, b.lm_extra, rows, c.vocab, temperature, weight, st));
-    return SBK_OK;
+    RC(lm_output(m, g, rows, b.lx, b.lx16, b.lh32, b.lh16, b.lm_logits, st));
+    return weighted_log_softmax(b.lm_logits, b.lm_extra, rows, c.vocab, temperature, weight, st);
 }
 
 // Beam search (decoders/seq2seq.py:1632-1723 with scorer=None): the device runs decoder step + beam_step_kernel and
@@ -1333,7 +1273,7 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
     *steps_done = 0;
     if (p.max_steps <= 0) return SBK_OK;
     RC(project_cross_kv(m, M, T, st));
-    set_decode_pdl(m, rows);
+    set_step_pdl(m, rows, d);
     const bool use_lm = p.lm_weight != 0.0f;
     SBK_REQUIRE(!use_lm || m->wt->has_lm, "beam: lm_weight != 0 but this handle has no TransformerLM weights");
     const bool use_ctc = p.ctc_weight != 0.0f;
@@ -1467,7 +1407,7 @@ static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos
     if (max_steps <= 0) return SBK_OK;
     RC(project_cross_kv(m, M, T, st));  // cross-attention K/V of all layers, once per utterance
     RC(greedy_reset(b.tokens, S_max + 1, rows, bos, b.step, b.has_ended, b.ended_count, m->wt->emb, m->wt->dec_pe, d, b.dx, st));
-    set_decode_pdl(m, rows);
+    set_step_pdl(m, rows, d);
     const bool use_graph = !in_capture && getenv("SBK_NO_GRAPH") == nullptr && log_probs == nullptr;
     if (in_capture) {  // the caller is capturing the whole pipeline: enqueue exactly max_steps steps, no polling
         for (int i = 0; i < max_steps; ++i) RC(enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, st));
@@ -1553,6 +1493,7 @@ static int run_decode_teacher(AsrModel* m, const int* tokens, int n, int S, int 
     SBK_REQUIRE(m->wt->has_dec, "decode: this handle was created without decoder weights");
     SBK_REQUIRE(S <= m->ws_steps && S <= c.max_len, "decode: %d target positions exceed the workspace / max_len", S);
     RC(project_cross_kv(m, M, T, st));
+    set_step_pdl(m, n, d);
     for (int s = 0; s < S; ++s) {
         dec_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, S, s, m->wt->emb, m->wt->dec_pe, d, sqrtf((float)d), b.dx, b.step);
         SBK_LAUNCH_CHECK();
@@ -1569,6 +1510,7 @@ static int run_lm_rescore(AsrModel* m, const int* tokens, const int* lens, int n
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int S_max = m->ws_steps + 1, dl = c.lm_d_model;
+    set_step_pdl(m, n, dl);
     lm_teacher_reset_kernel<<<n, 128, 0, st>>>(tokens, n, L, S_max, pad, b.lineage, b.tok_cache, scores);
     SBK_LAUNCH_CHECK();
     for (int s = 0; s + 1 < L; ++s) {
@@ -1587,6 +1529,7 @@ static int run_lm_step_logits(AsrModel* m, const int* tokens, int n, int L, floa
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int S_max = m->ws_steps + 1, dl = c.lm_d_model, V = c.vocab;
+    set_step_pdl(m, n, dl);
     lm_teacher_reset_kernel<<<n, 128, 0, st>>>(tokens, n, L, S_max, 0, b.lineage, b.tok_cache, b.score);
     SBK_LAUNCH_CHECK();
     for (int s = 0; s < L; ++s) {
@@ -1637,36 +1580,19 @@ static int ensure_lm_workspace(AsrModel* m, int rows) {
 
 static int run_lm_forward(AsrModel* m, const int* tokens, int n, int s, float* logits, cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
-    const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead, M = n * s;
+    const int dl = c.lm_d_model, H = c.lm_nhead, M = n * s;
     RC(ensure_lm_workspace(m, M));
     const AsrModel::LmFwdBuf& b = m->lmf;
     lm_embed_kernel<<<M, 128, 0, st>>>(tokens, s, c.vocab, m->wt->lm_emb, m->wt->lm_pe, dl, sqrtf((float)dl), b.x, b.x16);
     SBK_LAUNCH_CHECK();
     for (int l = 0; l < c.lm_layers; ++l) {  // post-norm TransformerEncoderLayer (Transformer.py:466-481)
         const LmLayerW& w = m->wt->lm[l];
-        GemmEpilogue e;
-        e.mode = EPI_F16; e.bias = w.b_in; e.out = b.qkv16; e.ldo = 3 * dl;
-        RC(gemm_f16(b.x16, dl, w.w_in, dl, e, M, 3 * dl, dl, st));
+        RC(project(SG_WIDE, {w.w_in, w.b_in, 3 * dl, dl, PO_F16, b.qkv16, 3 * dl, b.x16, dl}, M, st));
         RC(lm_causal_attention(b.qkv16, n, s, dl, H, tokens, 0, b.att16, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b_out; e.out = b.x; e.resid = b.x; e.ldo = dl;
-        RC(gemm_f16(b.att16, dl, w.w_out, dl, e, M, dl, dl, st));
-        RC(layernorm_dual(b.x, b.x16, w.n1g, w.n1b, M, dl, 1e-6f, true, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = c.lm_activation == SBK_ACT_GELU ? ACT_GELU : ACT_RELU;
-        e.bias = w.b1; e.out = b.f16; e.ldo = Fl;
-        RC(gemm_f16(b.x16, dl, w.w1, dl, e, M, Fl, dl, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.b2; e.out = b.x; e.resid = b.x; e.ldo = dl;
-        RC(gemm_f16(b.f16, Fl, w.w2, Fl, e, M, dl, Fl, st));
-        RC(layernorm_dual(b.x, b.x16, w.n2g, w.n2b, M, dl, 1e-6f, true, st));
+        RC(lm_layer_tail(m, SG_WIDE, w, M, b.att16, b.x, b.x16, b.f16, st));
     }
-    RC(layernorm_dual(b.x, b.x16, m->wt->lm_norm_g, m->wt->lm_norm_b, M, dl, 1e-6f, false, st));  // encoder.norm
-    // output_proj: Linear d -> d (fp32, into the free residual buffer), LayerNorm, Linear d -> vocab into the caller's logits
-    GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->wt->lm_bp0; e.out = b.x; e.ldo = dl;
-    RC(gemm_f16(b.x16, dl, m->wt->lm_wp0, dl, e, M, dl, dl, st));
-    RC(layernorm_dual(b.x, b.x16, m->wt->lm_lnp_g, m->wt->lm_lnp_b, M, dl, 1e-6f, false, st));
-    e = GemmEpilogue(); e.mode = EPI_F32; e.bias = m->wt->lm_bp2; e.out = logits; e.ldo = c.vocab;
-    RC(gemm_f16(b.x16, dl, m->wt->lm_wp2, dl, e, M, c.vocab, dl, st));
-    return SBK_OK;
+    // output_proj's fp32 Linear d -> d goes into the free residual buffer, its logits into the caller's
+    return lm_output(m, SG_WIDE, M, b.x, b.x16, b.x, b.x16, logits, st);
 }
 
 }  // namespace sbk
