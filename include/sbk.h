@@ -275,8 +275,9 @@ int sbk_asr_beam_from_enc(sbk_asr* m, const float* enc_dev, const float* rel_len
 int sbk_asr_transcribe_greedy_dev(sbk_asr* m, const float* wav_dev, const float* rel_len_dev, int B, int L,
                                   int max_steps, int bos, int eos, float* enc_out_dev, int* pred_dev,
                                   float* score_dev, float* log_probs_dev, int* steps_done, void* stream);
-/* Decode coalescing: G batches (B utterances each, separate device buffers) are encoded batch by batch and decoded
- * by ONE greedy loop over G*B hypotheses; pred_dev[g] receives batch g's [B, max_steps] token ids. */
+/* Decode coalescing: G batches (B utterances each, separate device buffers) are encoded several batches per encoder pass
+ * (up to 65536 encoder rows, or one batch when a batch alone is larger) and decoded by ONE greedy loop over G*B
+ * hypotheses; pred_dev[g] receives batch g's [B, max_steps] token ids. */
 int sbk_asr_transcribe_greedy_group_dev(sbk_asr* m, int G, const float* const* wav_dev, const float* const* rel_len_dev,
                                         int B, int L, int max_steps, int bos, int eos, int* const* pred_dev,
                                         int* steps_done, void* stream);
@@ -285,7 +286,7 @@ int sbk_asr_transcribe_greedy_host(sbk_asr* m, const float* wav_host, const floa
                                    int* steps_done, void* stream);
 
 /* The group call from HOST buffers (pinned): per batch g, wav_host[g] [B, L] fp32 and rel_len_host[g] [B] are copied to the
- * device on an internal copy stream (batch g+1's copy overlaps batch g's encoder), pred_host[g] [B, max_steps] receives the
+ * device on an internal copy stream (a later encoder pass's copies overlap an earlier pass), pred_host[g] [B, max_steps] receives the
  * token ids; pred_dev (NULL, or an array whose entries may be NULL) additionally keeps them on the device.  Enqueue only:
  * the caller synchronises `stream`.  With poll interval 0 the whole call (copies included) replays one CUDA graph. */
 int sbk_asr_transcribe_greedy_group_host_async(sbk_asr* m, int G, const float* const* wav_host,

@@ -197,8 +197,8 @@ struct AsrModel {
         int rows = 0;
         float* x; __half *x16, *qkv16, *att16, *f16;
     } lmf;
-    // shapes the workspace is carved for
-    int wsB = 0, wsL = 0, ws_rows = 0, ws_steps = 0;
+    // shapes the workspace is carved for (wsBe: utterances per encoder pass, >= wsB)
+    int wsB = 0, wsBe = 0, wsL = 0, ws_rows = 0, ws_steps = 0;
     struct Buf {
         float *wav, *feats, *x, *glu, *enc_out, *dx, *logits, *score, *seq_scores, *lnout, *beam_scr;
         int *utt_max, *enc_len, *tokens, *step, *has_ended, *ended_count, *pred, *lineage, *finished, *hist_tok, *hist_pred;
@@ -223,7 +223,7 @@ struct AsrModel {
     GraphCache pipe_graph;    // the whole Fbank .. last decode step pipeline (sbk_asr_transcribe_greedy_dev)
     int* host_flag = nullptr;  // pinned
     // host-buffer group entry point: device staging of the G batches' wav / lengths, a copy stream forked from the caller's
-    // stream (so batch g+1's H2D overlaps batch g's encoder)
+    // stream (so the H2D of a later encoder pass's batches overlaps an earlier pass)
     DevBuf gwav;
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_ready[16] = {};
@@ -753,23 +753,26 @@ static void frames(const sbk_asr_config& c, int L, int* T0, int* T1, int* T2) {
     *T2 = (*T1 - 1) / 2 + 1;
 }
 
-// The workspace for a batch of B utterances of L samples, `rows` decoder hypotheses, `steps` max steps.
-static void workspace_layout(const AsrModel* m, int B, int L, int rows, int steps, AsrModel::Buf& b, Carver& take) {
+// The workspace for calls of B utterances of L samples whose encoder passes take up to Be utterances (Be > B: a group call
+// encodes several of its batches in one pass), `rows` decoder hypotheses, `steps` max steps.  Encoder activations are sized
+// for Be utterances, the per-call buffers (wav, Fbank scratch, lengths, flags) for B.
+static void workspace_layout(const AsrModel* m, int B, int Be, int L, int rows, int steps, AsrModel::Buf& b, Carver& take) {
     const sbk_asr_config& c = m->wt->cfg;
     int T0, T1, T2;
     frames(c, L, &T0, &T1, &T2);
     const int F1 = (c.n_mels - 1) / 2 + 1;
-    const size_t M = (size_t)B * T2, d = c.d_model, F = c.d_ffn, Ld = c.num_decoder_layers, S = steps + 1;
+    const size_t M = (size_t)Be * T2, d = c.d_model, F = c.d_ffn, Ld = c.num_decoder_layers, S = steps + 1;
     const bool bfm = c.encoder_module == SBK_ENC_BRANCHFORMER && m->wt->has_enc;
     const bool hmx = c.attention_type == SBK_ATT_HYPERMIX && m->wt->has_enc;
     const size_t Cu = bfm ? (size_t)c.csgu_linear_units : 0, Fu = std::max(F, Cu);  // f16 also holds the CSGU input u
-    const size_t Md = (size_t)std::max(B, rows) * T2;  // encoder states / cross K,V of every utterance the decoder sees
-    take(b.wav, (size_t)B * L * 4); take(b.feats, (size_t)B * T0 * c.n_mels * 4); take(b.x, M * d * 4);
+    const int Bd = std::max(Be, rows);          // utterances whose encoder states the decoder sees
+    const size_t Md = (size_t)Bd * T2;          // encoder states / cross K,V of those utterances
+    take(b.wav, (size_t)B * L * 4); take(b.feats, (size_t)Be * T0 * c.n_mels * 4); take(b.x, M * d * 4);
     take(b.glu, M * d * 4); take(b.enc_out, Md * d * 4); take(b.dx, (size_t)rows * d * 4);
     take(b.logits, (size_t)rows * c.vocab * 4); take(b.score, (size_t)rows * S * 4);
-    take(b.utt_max, B * 4); take(b.enc_len, (size_t)std::max(B, rows) * 4); take(b.tokens, (size_t)rows * (S + 1) * 4); take(b.step, rows * 4 + 64);
+    take(b.utt_max, B * 4); take(b.enc_len, (size_t)Bd * 4); take(b.tokens, (size_t)rows * (S + 1) * 4); take(b.step, rows * 4 + 64);
     take(b.has_ended, rows * 4); take(b.ended_count, 64); take(b.pred, (size_t)rows * S * 4); take(b.rel_len, B * 4);
-    take(b.act1, (size_t)B * T1 * F1 * c.cnn_c1 * 2); take(b.a_in, M * c.input_size * 2); take(b.h16, M * d * 2);
+    take(b.act1, (size_t)Be * T1 * F1 * c.cnn_c1 * 2); take(b.a_in, M * c.input_size * 2); take(b.h16, M * d * 2);
     take(b.f16, M * Fu * 2); take(b.qkv16, M * 3 * d * 2); take(b.att16, M * d * 2);
     take(b.P16, (size_t)T2 * d * 2); take(b.enc16, Md * d * 2); take(b.ckv16, Md * Ld * 2 * d * 2);
     take(b.kcache, (size_t)Ld * rows * S * d * 2); take(b.vcache, (size_t)Ld * rows * S * d * 2);
@@ -792,23 +795,26 @@ static void workspace_layout(const AsrModel* m, int B, int L, int rows, int step
         take(b.csgu_stats, M * 8);
     }
     if (hmx) {
-        take(b.hm_part, hypermix_part_floats(B, T2, c.d_model, c.d_ffn / c.nhead) * 4);
-        take(b.hm_G, (size_t)B * d * (F / c.nhead) * 2);
-        take(b.hm_gscale, (size_t)B * c.nhead * 4);
+        take(b.hm_part, hypermix_part_floats(Be, T2, c.d_model, c.d_ffn / c.nhead) * 4);
+        take(b.hm_G, (size_t)Be * d * (F / c.nhead) * 2);
+        take(b.hm_gscale, (size_t)Be * c.nhead * 4);
     }
 }
 
-// (Re)carve the workspace for at least the given shapes and the ones it is already carved for.
-static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps) {
-    if (m->ws.base && B <= m->wsB && L <= m->wsL && rows <= m->ws_rows && steps <= m->ws_steps) return SBK_OK;
-    B = std::max(B, m->wsB); L = std::max(L, m->wsL); rows = std::max(rows, m->ws_rows); steps = std::max(steps, m->ws_steps);
+// (Re)carve the workspace for at least the given shapes and the ones it is already carved for.  Be: utterances per encoder
+// pass (0: B).
+static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps, int Be = 0) {
+    Be = std::max(Be, B);
+    if (m->ws.base && B <= m->wsB && Be <= m->wsBe && L <= m->wsL && rows <= m->ws_rows && steps <= m->ws_steps) return SBK_OK;
+    B = std::max(B, m->wsB); Be = std::max(Be, m->wsBe); L = std::max(L, m->wsL); rows = std::max(rows, m->ws_rows);
+    steps = std::max(steps, m->ws_steps);
     Carver measure;
-    workspace_layout(m, B, L, rows, steps, m->b, measure);
+    workspace_layout(m, B, Be, L, rows, steps, m->b, measure);
     RC(grow_buffer(m, m->ws, measure.used + (1 << 20), "workspace"));
     drop_graphs(m);
     Carver carve{static_cast<uint8_t*>(m->ws.base)};
-    workspace_layout(m, B, L, rows, steps, m->b, carve);
-    m->wsB = B; m->wsL = L; m->ws_rows = rows; m->ws_steps = steps;
+    workspace_layout(m, B, Be, L, rows, steps, m->b, carve);
+    m->wsB = B; m->wsBe = Be; m->wsL = L; m->ws_rows = rows; m->ws_steps = steps;
     return SBK_OK;
 }
 
@@ -928,6 +934,10 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int T1 = (T0 - 1) / 2 + 1, T = feats ? (T1 - 1) / 2 + 1 : T0;  // feats == nullptr: b.a_in holds [B*T0, input_size]
+    // row counts are int (offsets into the activations are size_t); the CNN, attention and conv kernels launch one grid row
+    // or layer per utterance
+    SBK_REQUIRE(B <= 65535 && (long long)B * T0 <= INT_MAX, "encode: %d utterances of %d frames exceed the kernels' index range",
+                B, T0);
     const int M = B * T, d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H;
     SBK_REQUIRE(m->wt->has_enc, "encode: this handle was created without encoder weights");
     SBK_REQUIRE(feats == nullptr || m->wt->has_cnn, "encode: this handle was created without CNN weights");
@@ -2115,10 +2125,26 @@ static int transcribe_enqueue(AsrModel* m, const float* wav_dev, const float* re
     return SBK_OK;
 }
 
-// G independent batches of B utterances: each batch goes through Fbank..encoder on its own (B-utterance kernels),
-// then ONE greedy loop decodes all G*B hypotheses together.  A decode step is ~50 dependent, latency-bound kernels
-// whose cost barely depends on the row count, so coalescing the decode of the
-// batches in flight amortises it G-fold; per-utterance results are unchanged (rows are independent).
+// Batches per encoder pass of a group call of G >= 1 batches of B >= 1 utterances of L samples: as many batches as fit in
+// GROUP_PASS_ROWS encoder rows (at least one), then the batches spread evenly over that many passes, so no pass exceeds
+// GROUP_PASS_ROWS rows unless a single batch does.  Conformer-L, 32 x 10 s batches (8032 rows), one H100 SXM at 700 W
+// (tools/group_encode.py): the encode per batch falls up to about 7 batches per pass and is flat from 7 to 16, while the
+// pass's activations grow with it.
+constexpr long long GROUP_PASS_ROWS = 1 << 16;
+static int group_encode_batches(const sbk_asr_config& c, int G, int B, int L) {
+    int T0, T1, T;
+    frames(c, L, &T0, &T1, &T);
+    const long long fit = std::max(1LL, GROUP_PASS_ROWS / std::max(1LL, (long long)B * T));
+    const int E = (int)std::min<long long>(G, fit);
+    return ceil_div(G, ceil_div(G, E));
+}
+
+// G independent batches of B utterances: Fbank and the lengths run per batch (each batch is its own waveform pointer), the
+// CNN and encoder once per chunk of group_encode_batches() consecutive batches over all of the chunk's utterances, then ONE
+// greedy loop decodes all G*B hypotheses together.  Every encoder kernel works per row or per utterance, so an utterance's
+// encoder states do not depend on how many batches share its pass.  A decode step is ~50 dependent, latency-bound kernels
+// whose cost barely depends on the row count, so coalescing the decode of the batches in flight amortises it G-fold;
+// per-utterance results are unchanged (rows are independent).
 static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_dev, const float* const* rel_dev, int B, int L,
                                     int max_steps, int bos, int eos, int* const* pred_dev, int* steps_done, cudaStream_t st,
                                     bool in_capture, const cudaEvent_t* ready = nullptr, int* const* pred_host = nullptr) {
@@ -2126,12 +2152,16 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
     int T0, T1, T;
     frames(c, L, &T0, &T1, &T);
     AsrModel::Buf& b = m->b;
-    for (int g = 0; g < G; ++g) {
-        if (ready) SBK_CUDA_CHECK(cudaStreamWaitEvent(st, ready[g], 0));  // batch g's wav has landed in the staging buffer
-        RC(fbank_forward(m->wt->fbank, wav_dev[g], B, L, b.feats, b.utt_max, m->wt->glob_mean, m->wt->glob_std, c.norm_eps > 0.0f ? c.norm_eps : 1e-10f, st));
-        int* enc_len = b.enc_len + (size_t)g * B;
-        RC(set_enc_len(enc_len, rel_dev[g], B, T, st));
-        RC(run_encoder(m, b.feats, B, T0, enc_len, nullptr, b.enc_out + (size_t)g * B * T * c.d_model, st));
+    const int E = group_encode_batches(c, G, B, L);
+    for (int g0 = 0; g0 < G; g0 += E) {
+        const int n = std::min(E, G - g0);
+        for (int g = g0; g < g0 + n; ++g) {
+            if (ready) SBK_CUDA_CHECK(cudaStreamWaitEvent(st, ready[g], 0));  // batch g's wav has landed in the staging buffer
+            RC(fbank_forward(m->wt->fbank, wav_dev[g], B, L, b.feats + (size_t)(g - g0) * B * T0 * c.n_mels, b.utt_max,
+                             m->wt->glob_mean, m->wt->glob_std, c.norm_eps > 0.0f ? c.norm_eps : 1e-10f, st));
+            RC(set_enc_len(b.enc_len + (size_t)g * B, rel_dev[g], B, T, st));
+        }
+        RC(run_encoder(m, b.feats, n * B, T0, b.enc_len + (size_t)g0 * B, nullptr, b.enc_out + (size_t)g0 * B * T * c.d_model, st));
     }
     // The decode loop is a chain of ~3300 small, latency-bound kernels; the encoders of the other lanes are machine-filling
     // ones.  Its kernels go to a stream of the highest priority (under capture: kernel nodes of that priority), so that a ready
@@ -2166,9 +2196,9 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
     return SBK_OK;
 }
 
-// Host-buffer form of the group call: H2D of every batch on a copy stream forked from `st` (batch g+1's copy overlaps
-// batch g's encoder), the group pipeline, D2H of the token ids.  Works both eagerly and under stream capture (the fork /
-// join events become graph edges, the copies memcpy nodes).
+// Host-buffer form of the group call: H2D of every batch on a copy stream forked from `st` (batch g's Fbank waits for its
+// own copy only, so a later encoder pass's copies overlap an earlier pass), the group pipeline, D2H of the token ids.
+// Works both eagerly and under stream capture (the fork / join events become graph edges, the copies memcpy nodes).
 static int transcribe_group_host_enqueue(AsrModel* m, int G, const float* const* wav_host, const float* const* rel_host, int B,
                                          int L, int max_steps, int bos, int eos, int* const* pred_host, int* const* pred_dev,
                                          int* steps_done, cudaStream_t st, bool in_capture) {
@@ -2199,7 +2229,9 @@ int sbk_asr_transcribe_greedy_group_dev(sbk_asr* mm, int G, const float* const* 
     SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc && m->wt->has_dec, "transcribe_group: handle lacks model parts");
     SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe_group: model has no normalize.glob_mean/std weights");
     for (int g = 0; g < G; ++g) SBK_REQUIRE(wav_dev[g] && rel_len_dev[g], "transcribe_group: null batch pointer");
-    RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps)));
+    SBK_REQUIRE(B >= 1 && L >= 1, "transcribe_group: empty batch (B=%d, L=%d)", B, L);
+    RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps),
+                        group_encode_batches(m->wt->cfg, G, B, L) * B));
     const bool whole_graph = m->poll_every == 0 && getenv("SBK_NO_GRAPH") == nullptr && max_steps > 0;
     if (!whole_graph) return transcribe_group_enqueue(m, G, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, pred_dev, steps_done, st, false);
     struct GroupKey { const void *wav[16], *rel[16], *pred[16]; int G, B, L, steps, bos, eos; } key;
@@ -2228,7 +2260,9 @@ int sbk_asr_transcribe_greedy_group_host_async(sbk_asr* mm, int G, const float* 
     SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe_group_host: model has no normalize.glob_mean/std weights");
     SBK_REQUIRE(wav_host && rel_len_host && pred_host, "transcribe_group_host: null argument");
     for (int g = 0; g < G; ++g) SBK_REQUIRE(wav_host[g] && rel_len_host[g] && pred_host[g], "transcribe_group_host: null batch pointer");
-    RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps)));
+    SBK_REQUIRE(B >= 1 && L >= 1, "transcribe_group_host: empty batch (B=%d, L=%d)", B, L);
+    RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps),
+                        group_encode_batches(m->wt->cfg, G, B, L) * B));
     RC(grow_buffer(m, m->gwav, (size_t)G * B * L * 4 + (size_t)G * B * 4 + 256, "transcribe_group_host"));
     if (!m->copy_stream) {
         SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));

@@ -342,7 +342,9 @@ class AsrEngine:
 
     def transcribe_greedy_group_dev(self, wavs, lens, max_steps, bos, eos, preds):
         """Decode coalescing: ``wavs`` / ``lens`` / ``preds`` are lists of G per-batch device tensors ([B, L] fp32,
-        [B] fp32, [B, max_steps] int32).  Each batch is encoded on its own, all G*B hypotheses are decoded together."""
+        [B] fp32, [B, max_steps] int32).  The batches are encoded several at a time (up to 65536 encoder rows per pass, or
+        one batch when a batch alone is larger), all G*B
+        hypotheses are decoded together."""
         G = len(wavs)
         B, L = wavs[0].shape
         VP = ctypes.c_void_p * G

@@ -18,7 +18,7 @@ from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
 att = sys.argv[1] if len(sys.argv) > 1 else "RoPEMHA"
 steps = int(sys.argv[2]) if len(sys.argv) > 2 else 48
 B = int(sys.argv[3]) if len(sys.argv) > 3 else 32
-G = int(sys.argv[4]) if len(sys.argv) > 4 else 1  # > 1: G batches encoded one by one and decoded together (bench default 8)
+G = int(sys.argv[4]) if len(sys.argv) > 4 else 1  # > 1: G batches encoded in passes of up to 8 and decoded together
 out_dir = sys.argv[5] if len(sys.argv) > 5 else None
 cfg = dict(CONFORMER_LARGE, attention_type=att)
 eng = AsrEngine(cfg, seeded_asr_state(cfg, 0), device="cuda:0")
