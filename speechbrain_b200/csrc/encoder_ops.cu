@@ -1369,16 +1369,6 @@ int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, cons
                    : launch_hypermix<64>(h16, B, T, d, KH, lens, pe, w, part, G, gscale, x, st);
 }
 
-void hypermix_pe_table(int d, float* dst) {
-    for (int i = 0; i < d / 2; ++i) {  // Transformer.py:252-303 PositionalEncoding, computed in fp32 like the reference
-        const float den = expf((float)(2 * i) * -(logf(10000.0f) / (float)d));
-        for (int t = 0; t < HM_PE_ROWS; ++t) {
-            dst[(size_t)t * d + 2 * i] = sinf((float)t * den);
-            dst[(size_t)t * d + 2 * i + 1] = cosf((float)t * den);
-        }
-    }
-}
-
 // =========================================================================== TransformerLM causal self-attention
 // Whole-sequence attention of TransformerLM.forward (TransformerLM.py:127-169: nn.MultiheadAttention under make_masks'
 // look-ahead mask and key-padding mask on pad_idx).  qkv [n*s, 3d] fp16 with columns [q | k | v] (nn.MultiheadAttention's

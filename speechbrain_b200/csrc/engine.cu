@@ -1,120 +1,21 @@
-// Model engine: weight repacking, workspace, the encode pipeline (CNN front-end -> Conformer encoder)
-// and the KV-cached greedy decode loop.  Host-side orchestration only; all math is in the kernels.
-//
-// Weights arrive as HOST fp32 arrays named exactly like the reference state_dict (SURVEY.md 8b) with
-// the recipe's module prefixes:  "CNN.", "Transformer.", "seq_lin.", plus "normalize.glob_mean/std"
-// and "fbank.window" / "fbank.mel_matrix".  They are repacked once (fp16 GEMM operands, interleaved GLU
-// rows, concatenated cross-attention K/V projections, pre-scaled decoder queries) into one device arena.
+// Model engine: workspace, the encode pipeline (CNN front-end -> Conformer encoder) and the KV-cached greedy decode
+// loop.  Host-side orchestration only; all math is in the kernels.  The weights are loaded and repacked by asr_weights.cu.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
 
+#include "asr_weights.h"
 #include "common.cuh"
-#include "sbk_internal.h"
-#include "../../include/sbk.h"
 
 namespace sbk {
 
-struct EncLayerW {
-    const float *ffn1_ln_g, *ffn1_ln_b, *ffn1_b1, *ffn1_b2;
-    const __half *ffn1_w1, *ffn1_w2;
-    const float *norm1_g, *norm1_b;
-    const __half *wqkv, *wo;
-    const float* bo;
-    const __half* wpos;               // RelPos linear_pos
-    const float *pos_u, *pos_v;       // RelPos biases, raw (d_h, H) buffer viewed (H, d_h)
-    const float *conv_ln_g, *conv_ln_b;
-    const __half* wpw1;               // [2d, d] rows interleaved 16 value / 16 gate
-    const float* bpw1;                // interleaved the same way
-    const float *wdw, *bdw;           // [d, K], [d]
-    const float *aconv_ln_g, *aconv_ln_b;
-    const __half* wpw2;
-    const float* bpw2;
-    const float *ffn2_ln_g, *ffn2_ln_b, *ffn2_b1, *ffn2_b2;
-    const __half *ffn2_w1, *ffn2_w2;
-    const float *norm2_g, *norm2_b;
-    // Branchformer layer (Branchformer.py:92-234; the attention uses norm1_g/b = norm_mhsa and wqkv / wo / bo / wpos / pos_u /
-    // pos_v above)
-    const float *nconv_g, *nconv_b;   // norm_conv
-    const __half *wpre, *wpost, *wmerge;  // pre_channel_proj [C, d], post_channel_proj [d, C/2], merge_proj [d, 2d]
-    const float *bpre, *bpost, *bmerge;
-    const float *csgu_ln_g, *csgu_ln_b, *csgu_taps, *csgu_bias;  // taps tap-major [CSGU_TAP_ROWS, C/2] (csgu_repack_taps)
-    HyperMixWeights hm;               // HyperConformer: mha_layer = HyperMixing (replaces wqkv / wo / bo)
-    // Transformer layer (Transformer.py:311-490): self_att.att in_proj bias, repacked like wqkv; norm1 / norm2 and the FFN
-    // (ffn1_w1 / ffn1_b1 / ffn1_w2 / ffn1_b2) use the fields above
-    const float* bqkv;
-};
-
-struct DecLayerW {
-    const float *n1g, *n1b, *n2g, *n2b, *n3g, *n3b;
-    const __half *w_self_in, *w_self_out, *w_cross_q, *w_cross_out, *w_ffn1, *w_ffn2;
-    const float *b_self_in, *b_self_out, *b_cross_q, *b_cross_out, *b_ffn1, *b_ffn2;
-};
-
-struct LmLayerW {
-    const __half *w_in, *w_out, *w1, *w2;
-    const float *b_in, *b_out, *b1, *b2, *n1g, *n1b, *n2g, *n2b;
-};
-
-struct Arena {
-    uint8_t* base = nullptr;
-    size_t cap = 0, used = 0;
-    void* take(size_t bytes) {
-        const size_t off = (used + 255) & ~size_t(255);
-        if (off + bytes > cap) return nullptr;
-        used = off + bytes;
-        return base + off;
-    }
-};
-
 #define RC(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
-
-// What asr_create uploads and nothing changes afterwards: the configuration, the Fbank plan and the repacked weights in
-// one device arena.  A handle and its clones (lanes) hold it jointly; the last one to go frees it.
-struct AsrWeights {
-    sbk_asr_config cfg;
-    Fbank* fbank = nullptr;
-    Arena warena;
-    // frontend
-    const float *glob_mean = nullptr, *glob_std = nullptr;
-    const float *c1_w, *c1_b, *c1_g, *c1_be, *c2_b, *c2_g, *c2_be;
-    const __half* c2_w;
-    Cnn3Weights cnn3{};  // cfg.cnn_blocks == 3
-    // encoder
-    const __half* w_in; const float* b_in;
-    std::vector<EncLayerW> enc;
-    const float *enc_norm_g, *enc_norm_b;
-    const float *rope_cos = nullptr, *rope_sin = nullptr;  // [max_len, dh/2]
-    const __half* relpos_pe = nullptr;                     // [max_len, d] rows = |r|
-    const float* hm_pe = nullptr;                          // HyperMixing's own sine table [HM_PE_ROWS, d]
-    const float* enc_pe = nullptr;                         // regularMHA: the absolute sine table [max_len, d]
-    int pos_len = 0;
-    // decoder
-    const float* emb; const float* dec_pe;
-    std::vector<DecLayerW> dec;
-    const __half* w_ckv; const float* b_ckv;  // [L*2d, d]
-    const float *dec_norm_g, *dec_norm_b;
-    const __half* w_lin; const float* b_lin;
-    const __half* w_ctc = nullptr; const float* b_ctc = nullptr;
-    // TransformerLM scorer (optional part)
-    bool has_lm = false;
-    const float *lm_emb = nullptr, *lm_pe = nullptr;
-    std::vector<LmLayerW> lm;
-    const float *lm_norm_g, *lm_norm_b, *lm_bp0, *lm_lnp_g, *lm_lnp_b, *lm_bp2;
-    const __half *lm_wp0, *lm_wp2;
-    bool has_fbank = false, has_cnn = false, has_enc = false, has_dec = false;
-    ~AsrWeights() {
-        if (fbank) fbank_destroy(fbank);
-        cudaFree(warena.base);
-    }
-};
 
 // One cached CUDA graph and the key it was captured for.  Keys are compared bytewise, so callers zero their padding.
 struct GraphCache {
@@ -164,18 +65,6 @@ struct DevBuf {
     DevBuf(const DevBuf&) = delete;
     DevBuf& operator=(const DevBuf&) = delete;
     ~DevBuf() { cudaFree(base); }
-};
-
-// Lays fields out one after another in a buffer, each at a 256-byte boundary.  A buffer's layout is one function that runs
-// twice: with base == nullptr to measure the bytes it needs (`used`), then with the buffer to set the fields.
-struct Carver {
-    uint8_t* base = nullptr;
-    size_t used = 0;
-    template <class T>
-    void operator()(T*& field, size_t bytes) {
-        if (base) field = reinterpret_cast<T*>(base + used);
-        used += (bytes + 255) & ~size_t(255);
-    }
 };
 
 // A handle: the shared weights plus one lane's state.  A clone is another lane on the same weights with its own workspace,
@@ -251,76 +140,6 @@ struct AsrModel {
     }
 };
 
-static const float* find(const std::map<std::string, std::pair<const float*, int64_t>>& m, const std::string& k,
-                         int64_t numel, bool required = true) {
-    auto it = m.find(k);
-    if (it == m.end()) {
-        if (required) set_error("missing weight '%s'", k.c_str());
-        return nullptr;
-    }
-    if (numel >= 0 && it->second.second != numel) {
-        set_error("weight '%s' has %lld elements, expected %lld", k.c_str(), (long long)it->second.second, (long long)numel);
-        return nullptr;
-    }
-    return it->second.first;
-}
-
-struct Packer {
-    AsrWeights* W;
-    const std::map<std::string, std::pair<const float*, int64_t>>* w;
-    bool ok = true;
-    std::vector<float> tmpf;
-    std::vector<__half> tmph;
-    const float* f32(const std::string& k, int64_t n) {
-        const float* src = find(*w, k, n);
-        if (!src) { ok = false; return nullptr; }
-        return f32_raw(src, n);
-    }
-    const float* f32_raw(const float* src, int64_t n) {
-        void* d = W->warena.take(n * 4);
-        if (!d) { ok = false; set_error("weight arena exhausted"); return nullptr; }
-        if (cudaMemcpy(d, src, n * 4, cudaMemcpyHostToDevice) != cudaSuccess) { ok = false; set_error("weight upload failed"); }
-        return reinterpret_cast<const float*>(d);
-    }
-    const __half* f16_raw(const float* src, int64_t n, float scale = 1.0f) {
-        tmph.resize(n);
-        for (int64_t i = 0; i < n; ++i) tmph[i] = __float2half_rn(src[i] * scale);
-        void* d = W->warena.take(n * 2);
-        if (!d) { ok = false; set_error("weight arena exhausted"); return nullptr; }
-        if (cudaMemcpy(d, tmph.data(), n * 2, cudaMemcpyHostToDevice) != cudaSuccess) { ok = false; set_error("weight upload failed"); }
-        return reinterpret_cast<const __half*>(d);
-    }
-    const __half* f16(const std::string& k, int64_t n) {
-        const float* src = find(*w, k, n);
-        if (!src) { ok = false; return nullptr; }
-        return f16_raw(src, n);
-    }
-};
-
-static size_t weight_arena_bytes(const sbk_asr_config& c) {
-    const size_t d = c.d_model, f = c.d_ffn;
-    size_t enc = (size_t)c.num_encoder_layers * (4 * d * f + 3 * d * d + d * d + d * d + 2 * d * d + d * d) * 2;
-    if (c.encoder_module == SBK_ENC_BRANCHFORMER) {  // qkv, out, linear_pos, pre / post channel proj, merge (fp16) + CSGU taps
-        const size_t C = c.csgu_linear_units;
-        enc = (size_t)c.num_encoder_layers * ((3 * d * d + d * d + d * d + C * d + d * C / 2 + 2 * d * d) * 2 +
-                                              (size_t)CSGU_TAP_ROWS * C / 2 * 4 + (4 * C + 16 * d) * 4);
-    }
-    if (c.attention_type == SBK_ATT_HYPERMIX && c.nhead > 0) {  // two hypernetworks (fp16 + fp32 biases), LayerNorm, PE table
-        const size_t e = d / c.nhead, k = f / c.nhead, M = c.nhead;
-        enc += (size_t)c.num_encoder_layers * (2 * M * (e * e + k * e) * 2 + (2 * M * (e + k) + 2 * d) * 4 + 4 * 256) +
-               (size_t)HM_PE_ROWS * d * 4;
-    }
-    size_t dec = (size_t)c.num_decoder_layers * (3 * d * d + d * d + 3 * d * d + d * d + 2 * d * f) * 2;
-    size_t misc = (size_t)c.vocab * d * (4 + 2 + 2) + (size_t)c.max_len * d * (4 + 2) + (size_t)c.input_size * d * 2;
-    size_t lm = 0;
-    if (c.parts & SBK_PART_LM) {
-        const size_t dl = c.lm_d_model, fl = c.lm_d_ffn;
-        lm = (size_t)c.lm_layers * (4 * dl * dl + 2 * dl * fl) * 2 + (size_t)c.vocab * dl * (4 + 2) + dl * dl * 2 +
-             (size_t)c.max_len * dl * 4 + (8u << 20);
-    }
-    return enc + dec + misc + lm + (64u << 20);
-}
-
 // A new lane on the weights of `wt`.
 static int new_lane(std::shared_ptr<const AsrWeights> wt, AsrModel** out) {
     AsrModel* m = new AsrModel();
@@ -336,372 +155,8 @@ static int new_lane(std::shared_ptr<const AsrWeights> wt, AsrModel** out) {
 
 int asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, AsrModel** out) {
     SBK_REQUIRE(cfg && weights && out, "asr_create: null argument");
-    const sbk_asr_config& c = *cfg;
-    SBK_REQUIRE(c.d_model % 8 == 0 && c.d_model % c.nhead == 0, "asr_create: bad d_model/nhead");
-    SBK_REQUIRE(c.attention_type == SBK_ATT_ROPE || c.attention_type == SBK_ATT_RELPOS || c.attention_type == SBK_ATT_HYPERMIX ||
-                    c.attention_type == SBK_ATT_REGULAR,
-                "asr_create: attention_type must be RoPEMHA, RelPosMHAXL, hypermixing or regularMHA");
-    const int d = c.d_model, dh = d / c.nhead, F = c.d_ffn, K = c.kernel_size;
-    const bool hypermix = c.attention_type == SBK_ATT_HYPERMIX;
-    const bool tfm = c.encoder_module == SBK_ENC_TRANSFORMER;
-    SBK_REQUIRE(tfm == (c.attention_type == SBK_ATT_REGULAR),
-                "asr_create: regularMHA is built for the Transformer encoder only, and the Transformer encoder with regularMHA only");
-    SBK_REQUIRE(!tfm || dh == 64 || dh == 128, "asr_create: Transformer encoder head_dim=%d not built (128, 64)", dh);
-    SBK_REQUIRE(tfm || hypermix || dh == 64 || dh == 36 || dh == 32, "asr_create: encoder head_dim=%d not built (64, 36, 32)", dh);
-    SBK_REQUIRE(c.cnn_blocks == 0 || c.cnn_blocks == 2 || (c.cnn_blocks == 3 && c.cnn_c1 == 64 && c.cnn_c2 == 64),
-                "asr_create: cnn_blocks=%d with channels (%d, %d) not built (2, or 3 with 64 channels)", c.cnn_blocks, c.cnn_c1, c.cnn_c2);
-    SBK_REQUIRE(!hypermix || (c.encoder_module == SBK_ENC_CONFORMER && (dh == 32 || dh == 64) && F % c.nhead == 0 &&
-                              (F / c.nhead) % 16 == 0 && F / c.nhead <= 256),
-                "asr_create: hypermixing needs the Conformer encoder, a head width d_model / nhead of 32 or 64 and "
-                "k = d_ffn / nhead a multiple of 16 up to 256 (got %d, %d)", dh, c.nhead > 0 ? F / c.nhead : 0);
-    SBK_REQUIRE(!((c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0) || ((dh <= 64 || dh == 128) && dh % 4 == 0 && d % 16 == 0),
-                "asr_create: decoder head_dim must be 128 or a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)", dh, d);
-    SBK_REQUIRE(c.attention_type != SBK_ATT_ROPE || dh % 32 == 0, "asr_create: RoPEMHA needs head_dim %% 32 == 0");
-    SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER || c.encoder_module == SBK_ENC_BRANCHFORMER || tfm,
-                "asr_create: encoder_module %d (0 Conformer, 1 Branchformer, 2 Transformer)", c.encoder_module);
-    SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER ||
-                    (c.attention_type == SBK_ATT_RELPOS && c.csgu_linear_units > 0 && c.csgu_linear_units % 16 == 0 &&
-                     (K & 1) == 1 && K <= CSGU_TAP_ROWS),
-                "asr_create: the Branchformer needs RelPosMHAXL, csgu_linear_units / 2 %% 8 == 0 and an odd kernel_size <= %d "
-                "(got %d, %d)", CSGU_TAP_ROWS, c.csgu_linear_units, K);
-    std::map<std::string, std::pair<const float*, int64_t>> w;
-    for (int i = 0; i < n_weights; ++i) w[weights[i].name] = {weights[i].data, weights[i].numel};
-
-    auto wt = std::make_shared<AsrWeights>();
-    AsrWeights* W = wt.get();
-    W->cfg = c;
-    W->warena.cap = weight_arena_bytes(c);
-    if (cudaMalloc(&W->warena.base, W->warena.cap) != cudaSuccess) {
-        set_error("asr_create: cudaMalloc(%zu) for weights failed", W->warena.cap);
-        return SBK_ERR_NOMEM;
-    }
-    Packer p{W, &w};
-    const bool has_fbank = c.parts & SBK_PART_FBANK, has_cnn = c.parts & SBK_PART_CNN;
-    const bool has_enc = (c.parts & SBK_PART_ENCODER) && c.num_encoder_layers >= 0;
-    const bool has_dec = (c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0;
-    W->has_fbank = has_fbank; W->has_cnn = has_cnn; W->has_enc = has_enc; W->has_dec = has_dec;
-    // ---- Fbank + CMVN
-    if (has_fbank) {
-        const float* win = find(w, "fbank.window", c.n_fft);
-        const float* mel = find(w, "fbank.mel_matrix", (int64_t)(c.n_fft / 2 + 1) * c.n_mels);
-        if (!win || !mel) return SBK_ERR_ARG;
-        RC(fbank_create(&W->fbank, c.n_fft, c.hop, c.n_mels, win, mel, c.fbank_amin > 0.0f ? c.fbank_amin : 1e-10f,
-                        c.fbank_top_db > 0.0f ? c.fbank_top_db : 80.0f));
-        if (w.count("normalize.glob_mean")) {
-            W->glob_mean = p.f32("normalize.glob_mean", c.n_mels);
-            W->glob_std = p.f32("normalize.glob_std", c.n_mels);
-        }
-    }
-    // ---- CNN front-end
-    if (has_cnn && c.cnn_blocks == 3) {  // convolution.py:116-320 with kernel_sizes (5, 5, 1), residuals (False, False, True)
-        const int C = 64, F1 = (c.n_mels - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
-        if (F2 * C != c.input_size) { set_error("asr_create: CNN output %d != input_size %d", F2 * C, c.input_size); return SBK_ERR_ARG; }
-        const std::string b0 = "CNN.convblock_0.convs.", b1 = "CNN.convblock_1.convs.", b2 = "CNN.convblock_2.";
-        Cnn3Weights& k = W->cnn3;
-        k.w1 = p.f32(b0 + "conv_0.conv.weight", (int64_t)C * 25); k.b1 = p.f32(b0 + "conv_0.conv.bias", C);
-        k.g1 = p.f32(b0 + "norm_0.norm.weight", (int64_t)F1 * C); k.be1 = p.f32(b0 + "norm_0.norm.bias", (int64_t)F1 * C);
-        const float* w2 = find(w, b1 + "conv_0.conv.weight", (int64_t)C * C * 25);
-        const float* w3a = find(w, b2 + "convs.conv_0.conv.weight", (int64_t)C * C);
-        const float* w3r = find(w, b2 + "reduce_conv.conv.conv.weight", (int64_t)C * C);
-        const float* b3a = find(w, b2 + "convs.conv_0.conv.bias", C);
-        const float* b3r = find(w, b2 + "reduce_conv.conv.conv.bias", C);
-        if (!w2 || !w3a || !w3r || !b3a || !b3r) return SBK_ERR_ARG;
-        std::vector<float> w2p((size_t)C * 25 * C);  // (o, ch, kf, kt) -> [o][(kf * 5 + kt) * 64 + ch]
-        for (int o = 0; o < C; ++o)
-            for (int ch = 0; ch < C; ++ch)
-                for (int t = 0; t < 25; ++t) w2p[((size_t)o * 25 + t) * C + ch] = w2[((size_t)o * C + ch) * 25 + t];
-        k.w2p = p.f16_raw(w2p.data(), w2p.size());
-        k.b2 = p.f32(b1 + "conv_0.conv.bias", C);
-        k.g2 = p.f32(b1 + "norm_0.norm.weight", (int64_t)F2 * C); k.be2 = p.f32(b1 + "norm_0.norm.bias", (int64_t)F2 * C);
-        std::vector<float> w3((size_t)2 * C * C), b3(2 * C);  // [convs.conv_0 | reduce_conv.conv] output channels
-        memcpy(w3.data(), w3a, (size_t)C * C * 4); memcpy(w3.data() + (size_t)C * C, w3r, (size_t)C * C * 4);
-        memcpy(b3.data(), b3a, C * 4); memcpy(b3.data() + C, b3r, C * 4);
-        k.w3 = p.f32_raw(w3.data(), w3.size()); k.b3 = p.f32_raw(b3.data(), b3.size());
-        k.g3 = p.f32(b2 + "convs.norm_0.norm.weight", (int64_t)F2 * C); k.be3 = p.f32(b2 + "convs.norm_0.norm.bias", (int64_t)F2 * C);
-        k.gr = p.f32(b2 + "reduce_conv.norm.norm.weight", (int64_t)F2 * C); k.ber = p.f32(b2 + "reduce_conv.norm.norm.bias", (int64_t)F2 * C);
-    } else if (has_cnn) {
-        const int F1 = (c.n_mels - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
-        if (F2 * c.cnn_c2 != c.input_size) { set_error("asr_create: CNN output %d != input_size %d", F2 * c.cnn_c2, c.input_size); return SBK_ERR_ARG; }
-        W->c1_w = p.f32("CNN.convblock_0.convs.conv_0.conv.weight", (int64_t)c.cnn_c1 * 9);
-        W->c1_b = p.f32("CNN.convblock_0.convs.conv_0.conv.bias", c.cnn_c1);
-        W->c1_g = p.f32("CNN.convblock_0.convs.norm_0.norm.weight", (int64_t)F1 * c.cnn_c1);
-        W->c1_be = p.f32("CNN.convblock_0.convs.norm_0.norm.bias", (int64_t)F1 * c.cnn_c1);
-        const float* w2 = find(w, "CNN.convblock_1.convs.conv_0.conv.weight", (int64_t)c.cnn_c2 * c.cnn_c1 * 9);
-        if (!w2) return SBK_ERR_ARG;
-        std::vector<float> w2p((size_t)c.cnn_c2 * 9 * c.cnn_c1);
-        for (int o = 0; o < c.cnn_c2; ++o)
-            for (int ch = 0; ch < c.cnn_c1; ++ch)
-                for (int kf = 0; kf < 3; ++kf)
-                    for (int kt = 0; kt < 3; ++kt)
-                        w2p[((size_t)o * 9 + kf * 3 + kt) * c.cnn_c1 + ch] = w2[(((size_t)o * c.cnn_c1 + ch) * 3 + kf) * 3 + kt];
-        W->c2_w = p.f16_raw(w2p.data(), w2p.size());
-        W->c2_b = p.f32("CNN.convblock_1.convs.conv_0.conv.bias", c.cnn_c2);
-        W->c2_g = p.f32("CNN.convblock_1.convs.norm_0.norm.weight", (int64_t)F2 * c.cnn_c2);
-        W->c2_be = p.f32("CNN.convblock_1.convs.norm_0.norm.bias", (int64_t)F2 * c.cnn_c2);
-    }
-    // ---- encoder
-    if (has_enc) {
-    W->w_in = p.f16("Transformer.custom_src_module.layers.0.w.weight", (int64_t)d * c.input_size);
-    W->b_in = p.f32("Transformer.custom_src_module.layers.0.w.bias", d);
-    W->enc.resize(c.num_encoder_layers);
-    for (int l = 0; l < c.num_encoder_layers && p.ok && c.encoder_module == SBK_ENC_BRANCHFORMER; ++l) {
-        const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".", cb = q + "convolution_branch.";
-        const int C = c.csgu_linear_units, C2 = C / 2;
-        EncLayerW& e = W->enc[l];
-        e.norm1_g = p.f32(q + "norm_mhsa.norm.weight", d); e.norm1_b = p.f32(q + "norm_mhsa.norm.bias", d);
-        e.nconv_g = p.f32(q + "norm_conv.norm.weight", d); e.nconv_b = p.f32(q + "norm_conv.norm.bias", d);
-        e.wqkv = p.f16(q + "mha_layer.in_proj_weight", (int64_t)3 * d * d);
-        e.wo = p.f16(q + "mha_layer.out_proj.weight", (int64_t)d * d); e.bo = p.f32(q + "mha_layer.out_proj.bias", d);
-        e.wpos = p.f16(q + "mha_layer.linear_pos.weight", (int64_t)d * d);
-        e.pos_u = p.f32(q + "mha_layer.pos_bias_u", d); e.pos_v = p.f32(q + "mha_layer.pos_bias_v", d);
-        e.wpre = p.f16(cb + "pre_channel_proj.weight", (int64_t)C * d); e.bpre = p.f32(cb + "pre_channel_proj.bias", C);
-        e.wpost = p.f16(cb + "post_channel_proj.weight", (int64_t)d * C2); e.bpost = p.f32(cb + "post_channel_proj.bias", d);
-        e.csgu_ln_g = p.f32(cb + "csgu.norm.norm.weight", C2); e.csgu_ln_b = p.f32(cb + "csgu.norm.norm.bias", C2);
-        {   // depthwise taps (C/2, 1, K) -> tap-major, K centred in CSGU_TAP_ROWS rows
-            const float* src = find(w, cb + "csgu.conv.conv.weight", (int64_t)C2 * K);
-            if (!src) { p.ok = false; break; }
-            std::vector<float> wt((size_t)CSGU_TAP_ROWS * C2);
-            csgu_repack_taps(src, C2, K, wt.data());
-            e.csgu_taps = p.f32_raw(wt.data(), wt.size());
-        }
-        e.csgu_bias = p.f32(cb + "csgu.conv.conv.bias", C2);
-        e.wmerge = p.f16(q + "merge_proj.weight", (int64_t)d * 2 * d); e.bmerge = p.f32(q + "merge_proj.bias", d);
-    }
-    for (int l = 0; l < c.num_encoder_layers && p.ok && tfm; ++l) {
-        const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".";
-        EncLayerW& e = W->enc[l];
-        e.norm1_g = p.f32(q + "norm1.norm.weight", d); e.norm1_b = p.f32(q + "norm1.norm.bias", d);
-        e.norm2_g = p.f32(q + "norm2.norm.weight", d); e.norm2_b = p.f32(q + "norm2.norm.bias", d);
-        const float* wi = find(w, q + "self_att.att.in_proj_weight", (int64_t)3 * d * d);
-        const float* bi = find(w, q + "self_att.att.in_proj_bias", 3 * d);
-        if (!wi || !bi) { p.ok = false; break; }
-        // nn.MultiheadAttention's [Wq; Wk; Wv] rows -> per-head [q | k | v] blocks (the encoder attention's layout), with
-        // 1/sqrt(d_h) folded into the query rows
-        std::vector<float> wr((size_t)3 * d * d), br(3 * d);
-        const float qs = 1.0f / sqrtf((float)dh);
-        for (int h = 0; h < c.nhead; ++h)
-            for (int part = 0; part < 3; ++part)
-                for (int j = 0; j < dh; ++j) {
-                    const size_t src = (size_t)part * d + h * dh + j, dst = (size_t)h * 3 * dh + part * dh + j;
-                    const float sc = part == 0 ? qs : 1.0f;
-                    for (int k = 0; k < d; ++k) wr[dst * d + k] = wi[src * d + k] * sc;
-                    br[dst] = bi[src] * sc;
-                }
-        e.wqkv = p.f16_raw(wr.data(), wr.size()); e.bqkv = p.f32_raw(br.data(), br.size());
-        e.wo = p.f16(q + "self_att.att.out_proj.weight", (int64_t)d * d); e.bo = p.f32(q + "self_att.att.out_proj.bias", d);
-        e.ffn1_w1 = p.f16(q + "pos_ffn.ffn.0.weight", (int64_t)F * d); e.ffn1_b1 = p.f32(q + "pos_ffn.ffn.0.bias", F);
-        e.ffn1_w2 = p.f16(q + "pos_ffn.ffn.3.weight", (int64_t)d * F); e.ffn1_b2 = p.f32(q + "pos_ffn.ffn.3.bias", d);
-    }
-    for (int l = 0; l < c.num_encoder_layers && p.ok && c.encoder_module == SBK_ENC_CONFORMER; ++l) {
-        const std::string q = "Transformer.encoder.layers." + std::to_string(l) + ".";
-        EncLayerW& e = W->enc[l];
-        e.ffn1_ln_g = p.f32(q + "ffn_module1.0.weight", d); e.ffn1_ln_b = p.f32(q + "ffn_module1.0.bias", d);
-        e.ffn1_w1 = p.f16(q + "ffn_module1.1.ffn.0.weight", (int64_t)F * d); e.ffn1_b1 = p.f32(q + "ffn_module1.1.ffn.0.bias", F);
-        e.ffn1_w2 = p.f16(q + "ffn_module1.1.ffn.3.weight", (int64_t)d * F); e.ffn1_b2 = p.f32(q + "ffn_module1.1.ffn.3.bias", d);
-        e.norm1_g = p.f32(q + "norm1.norm.weight", d); e.norm1_b = p.f32(q + "norm1.norm.bias", d);
-        e.wpos = nullptr; e.pos_u = e.pos_v = nullptr;
-        if (hypermix) {  // hypermixing.py:52-81, 274-337: w{1,2}_gen fc1 (M, e, e) / fc2 (M, k, e), then layer_norm (d)
-            const int Mh = c.nhead, kh = F / c.nhead;
-            const char* gen[2] = {"mha_layer.hyper.w1_gen.", "mha_layer.hyper.w2_gen."};
-            for (int gi = 0; gi < 2; ++gi) {
-                e.hm.fc1w[gi] = p.f16(q + gen[gi] + "fc1_weights", (int64_t)Mh * dh * dh);
-                e.hm.fc1b[gi] = p.f32(q + gen[gi] + "fc1_biases", (int64_t)Mh * dh);
-                e.hm.fc2w[gi] = p.f16(q + gen[gi] + "fc2_weights", (int64_t)Mh * kh * dh);
-                e.hm.fc2b[gi] = p.f32(q + gen[gi] + "fc2_biases", (int64_t)Mh * kh);
-            }
-            e.hm.ln_g = p.f32(q + "mha_layer.layer_norm.weight", d); e.hm.ln_b = p.f32(q + "mha_layer.layer_norm.bias", d);
-            e.wqkv = e.wo = nullptr; e.bo = nullptr;
-        } else {
-            e.wqkv = p.f16(q + "mha_layer.in_proj_weight", (int64_t)3 * d * d);
-            e.wo = p.f16(q + "mha_layer.out_proj.weight", (int64_t)d * d); e.bo = p.f32(q + "mha_layer.out_proj.bias", d);
-        }
-        if (c.attention_type == SBK_ATT_RELPOS) {
-            e.wpos = p.f16(q + "mha_layer.linear_pos.weight", (int64_t)d * d);
-            e.pos_u = p.f32(q + "mha_layer.pos_bias_u", d); e.pos_v = p.f32(q + "mha_layer.pos_bias_v", d);
-        }
-        e.conv_ln_g = p.f32(q + "convolution_module.layer_norm.weight", d); e.conv_ln_b = p.f32(q + "convolution_module.layer_norm.bias", d);
-        {   // pointwise conv 1 (Conv1d k=1, weight (2d, d, 1)): interleave 16 value rows / 16 gate rows for the GLU epilogue
-            const float* src = find(w, q + "convolution_module.bottleneck.0.weight", (int64_t)2 * d * d);
-            const float* bs = find(w, q + "convolution_module.bottleneck.0.bias", 2 * d);
-            if (!src || !bs) { p.ok = false; break; }
-            std::vector<float> wi((size_t)2 * d * d), bi(2 * d);
-            for (int ch = 0; ch < d; ++ch) {
-                const int blk = ch / 16, j = ch % 16;
-                memcpy(&wi[((size_t)blk * 32 + j) * d], &src[(size_t)ch * d], d * 4);
-                memcpy(&wi[((size_t)blk * 32 + 16 + j) * d], &src[(size_t)(d + ch) * d], d * 4);
-                bi[blk * 32 + j] = bs[ch];
-                bi[blk * 32 + 16 + j] = bs[d + ch];
-            }
-            e.wpw1 = p.f16_raw(wi.data(), wi.size());
-            e.bpw1 = p.f32_raw(bi.data(), bi.size());
-        }
-        {   // depthwise taps (d, 1, K) -> tap-major [K, d] so that a warp's channels read one cache line per tap
-            const float* src = find(w, q + "convolution_module.conv.weight", (int64_t)d * K);
-            if (!src) { p.ok = false; break; }
-            std::vector<float> wt((size_t)K * d);
-            dwconv_repack_taps(src, d, K, wt.data());
-            e.wdw = p.f32_raw(wt.data(), wt.size());
-        }
-        e.bdw = p.f32(q + "convolution_module.conv.bias", d);
-        e.aconv_ln_g = p.f32(q + "convolution_module.after_conv.0.weight", d); e.aconv_ln_b = p.f32(q + "convolution_module.after_conv.0.bias", d);
-        e.wpw2 = p.f16(q + "convolution_module.after_conv.2.weight", (int64_t)d * d); e.bpw2 = p.f32(q + "convolution_module.after_conv.2.bias", d);
-        e.ffn2_ln_g = p.f32(q + "ffn_module2.0.weight", d); e.ffn2_ln_b = p.f32(q + "ffn_module2.0.bias", d);
-        e.ffn2_w1 = p.f16(q + "ffn_module2.1.ffn.0.weight", (int64_t)F * d); e.ffn2_b1 = p.f32(q + "ffn_module2.1.ffn.0.bias", F);
-        e.ffn2_w2 = p.f16(q + "ffn_module2.1.ffn.3.weight", (int64_t)d * F); e.ffn2_b2 = p.f32(q + "ffn_module2.1.ffn.3.bias", d);
-        e.norm2_g = p.f32(q + "norm2.norm.weight", d); e.norm2_b = p.f32(q + "norm2.norm.bias", d);
-    }
-    if (!p.ok) return SBK_ERR_ARG;
-    W->enc_norm_g = p.f32("Transformer.encoder.norm.norm.weight", d);
-    W->enc_norm_b = p.f32("Transformer.encoder.norm.norm.bias", d);
-    // positional tables
-    W->pos_len = c.max_len;
-    if (c.attention_type == SBK_ATT_ROPE) {
-        // nnet/attention.py:1012-1055: angle_{t,i} = t * exp(-2i * ln(1e4) / d_h), computed in fp32 like the reference
-        std::vector<float> cs((size_t)c.max_len * dh / 2), sn(cs.size());
-        for (int i = 0; i < dh / 2; ++i) {
-            const float ang = expf((float)(2 * i) * -(logf(10000.0f) / (float)dh));
-            for (int t = 0; t < c.max_len; ++t) {
-                const float ta = (float)t * ang;
-                cs[(size_t)t * (dh / 2) + i] = cosf(ta);
-                sn[(size_t)t * (dh / 2) + i] = sinf(ta);
-            }
-        }
-        W->rope_cos = p.f32_raw(cs.data(), cs.size());
-        W->rope_sin = p.f32_raw(sn.data(), sn.size());
-    } else if (tfm) {  // Transformer.py:252-303 PositionalEncoding, fp32 like the reference's buffer
-        std::vector<float> pe((size_t)c.max_len * d);
-        for (int i = 0; i < d / 2; ++i) {
-            const float den = expf((float)(2 * i) * -(logf(10000.0f) / (float)d));
-            for (int t = 0; t < c.max_len; ++t) {
-                pe[(size_t)t * d + 2 * i] = sinf((float)t * den);
-                pe[(size_t)t * d + 2 * i + 1] = cosf((float)t * den);
-            }
-        }
-        W->enc_pe = p.f32_raw(pe.data(), pe.size());
-    } else if (hypermix) {
-        std::vector<float> pe((size_t)HM_PE_ROWS * d);
-        hypermix_pe_table(d, pe.data());
-        W->hm_pe = p.f32_raw(pe.data(), pe.size());
-        W->pos_len = HM_PE_ROWS;
-    } else {
-        // nnet/attention.py:360-408: row |r|: even cols sin(|r| f_i), odd cols cos(|r| f_i)
-        std::vector<float> pe((size_t)c.max_len * d);
-        for (int i = 0; i < d / 2; ++i) {
-            const float fr = expf((float)(2 * i) * -(logf(10000.0f) / (float)d));
-            for (int t = 0; t < c.max_len; ++t) {
-                pe[(size_t)t * d + 2 * i] = sinf((float)t * fr);
-                pe[(size_t)t * d + 2 * i + 1] = cosf((float)t * fr);
-            }
-        }
-        W->relpos_pe = p.f16_raw(pe.data(), pe.size());
-    }
-    }  // has_enc
-    // ---- decoder
-    if (has_dec) {
-        W->emb = p.f32("Transformer.custom_tgt_module.layers.0.emb.Embedding.weight", (int64_t)c.vocab * d);
-        {
-            std::vector<float> pe((size_t)c.max_len * d);  // Transformer.py:252-303
-            for (int i = 0; i < d / 2; ++i) {
-                const float den = expf((float)(2 * i) * -(logf(10000.0f) / (float)d));
-                for (int t = 0; t < c.max_len; ++t) {
-                    pe[(size_t)t * d + 2 * i] = sinf((float)t * den);
-                    pe[(size_t)t * d + 2 * i + 1] = cosf((float)t * den);
-                }
-            }
-            W->dec_pe = p.f32_raw(pe.data(), pe.size());
-        }
-        const int L = c.num_decoder_layers;
-        W->dec.resize(L);
-        std::vector<float> wckv((size_t)L * 2 * d * d), bckv((size_t)L * 2 * d);
-        const float qs = 1.0f / sqrtf((float)dh);
-        for (int l = 0; l < L && p.ok; ++l) {
-            const std::string q = "Transformer.decoder.layers." + std::to_string(l) + ".";
-            DecLayerW& e = W->dec[l];
-            e.n1g = p.f32(q + "norm1.norm.weight", d); e.n1b = p.f32(q + "norm1.norm.bias", d);
-            e.n2g = p.f32(q + "norm2.norm.weight", d); e.n2b = p.f32(q + "norm2.norm.bias", d);
-            e.n3g = p.f32(q + "norm3.norm.weight", d); e.n3b = p.f32(q + "norm3.norm.bias", d);
-            const float* wi = find(w, q + "self_attn.att.in_proj_weight", (int64_t)3 * d * d);
-            const float* bi = find(w, q + "self_attn.att.in_proj_bias", 3 * d);
-            const float* wc = find(w, q + "multihead_attn.att.in_proj_weight", (int64_t)3 * d * d);
-            const float* bc = find(w, q + "multihead_attn.att.in_proj_bias", 3 * d);
-            if (!wi || !bi || !wc || !bc) { p.ok = false; break; }
-            {   // fold 1/sqrt(d_h) into the query rows
-                std::vector<float> ws(wi, wi + (size_t)3 * d * d), bs(bi, bi + 3 * d);
-                for (size_t i = 0; i < (size_t)d * d; ++i) ws[i] *= qs;
-                for (int i = 0; i < d; ++i) bs[i] *= qs;
-                e.w_self_in = p.f16_raw(ws.data(), ws.size());
-                e.b_self_in = p.f32_raw(bs.data(), bs.size());
-                std::vector<float> wq(wc, wc + (size_t)d * d), bq(bc, bc + d);
-                for (auto& v : wq) v *= qs;
-                for (auto& v : bq) v *= qs;
-                e.w_cross_q = p.f16_raw(wq.data(), wq.size());
-                e.b_cross_q = p.f32_raw(bq.data(), bq.size());
-            }
-            memcpy(&wckv[(size_t)l * 2 * d * d], wc + (size_t)d * d, (size_t)2 * d * d * 4);
-            memcpy(&bckv[(size_t)l * 2 * d], bc + d, (size_t)2 * d * 4);
-            e.w_self_out = p.f16(q + "self_attn.att.out_proj.weight", (int64_t)d * d); e.b_self_out = p.f32(q + "self_attn.att.out_proj.bias", d);
-            e.w_cross_out = p.f16(q + "multihead_attn.att.out_proj.weight", (int64_t)d * d); e.b_cross_out = p.f32(q + "multihead_attn.att.out_proj.bias", d);
-            e.w_ffn1 = p.f16(q + "pos_ffn.ffn.0.weight", (int64_t)F * d); e.b_ffn1 = p.f32(q + "pos_ffn.ffn.0.bias", F);
-            e.w_ffn2 = p.f16(q + "pos_ffn.ffn.3.weight", (int64_t)d * F); e.b_ffn2 = p.f32(q + "pos_ffn.ffn.3.bias", d);
-        }
-        if (!p.ok) return SBK_ERR_ARG;
-        W->w_ckv = p.f16_raw(wckv.data(), wckv.size());
-        W->b_ckv = p.f32_raw(bckv.data(), bckv.size());
-        W->dec_norm_g = p.f32("Transformer.decoder.norm.norm.weight", d);
-        W->dec_norm_b = p.f32("Transformer.decoder.norm.norm.bias", d);
-        W->w_lin = nullptr; W->b_lin = nullptr;
-        if (w.count("seq_lin.w.weight")) {  // the output head belongs to the searchers; TransformerASR.decode runs without it
-            W->w_lin = p.f16("seq_lin.w.weight", (int64_t)c.vocab * d);
-            W->b_lin = p.f32("seq_lin.w.bias", c.vocab);
-        }
-    }
-    if ((c.parts & SBK_PART_LM) && c.lm_layers > 0) {
-        const int dl = c.lm_d_model, Fl = c.lm_d_ffn, dhl = dl / c.lm_nhead;
-        if (dhl != 64 || dl % 128 != 0) { set_error("asr_create: LM head_dim must be 64 and d_model %% 128 == 0"); return SBK_ERR_UNSUPPORTED; }
-        W->has_lm = true;
-        W->lm_emb = p.f32("lm.custom_src_module.emb.Embedding.weight", (int64_t)c.vocab * dl);
-        {
-            std::vector<float> pe((size_t)c.max_len * dl);
-            for (int i = 0; i < dl / 2; ++i) {
-                const float den = expf((float)(2 * i) * -(logf(10000.0f) / (float)dl));
-                for (int t = 0; t < c.max_len; ++t) {
-                    pe[(size_t)t * dl + 2 * i] = sinf((float)t * den);
-                    pe[(size_t)t * dl + 2 * i + 1] = cosf((float)t * den);
-                }
-            }
-            W->lm_pe = p.f32_raw(pe.data(), pe.size());
-        }
-        W->lm.resize(c.lm_layers);
-        const float qs = 1.0f / sqrtf((float)dhl);
-        for (int l = 0; l < c.lm_layers && p.ok; ++l) {
-            const std::string q = "lm.encoder.layers." + std::to_string(l) + ".";
-            LmLayerW& e = W->lm[l];
-            const float* wi = find(w, q + "self_att.att.in_proj_weight", (int64_t)3 * dl * dl);
-            const float* bi = find(w, q + "self_att.att.in_proj_bias", 3 * dl);
-            if (!wi || !bi) { p.ok = false; break; }
-            std::vector<float> ws(wi, wi + (size_t)3 * dl * dl), bs(bi, bi + 3 * dl);
-            for (size_t i = 0; i < (size_t)dl * dl; ++i) ws[i] *= qs;  // fold 1/sqrt(d_h) into the query rows
-            for (int i = 0; i < dl; ++i) bs[i] *= qs;
-            e.w_in = p.f16_raw(ws.data(), ws.size());
-            e.b_in = p.f32_raw(bs.data(), bs.size());
-            e.w_out = p.f16(q + "self_att.att.out_proj.weight", (int64_t)dl * dl); e.b_out = p.f32(q + "self_att.att.out_proj.bias", dl);
-            e.w1 = p.f16(q + "pos_ffn.ffn.0.weight", (int64_t)Fl * dl); e.b1 = p.f32(q + "pos_ffn.ffn.0.bias", Fl);
-            e.w2 = p.f16(q + "pos_ffn.ffn.3.weight", (int64_t)dl * Fl); e.b2 = p.f32(q + "pos_ffn.ffn.3.bias", dl);
-            e.n1g = p.f32(q + "norm1.norm.weight", dl); e.n1b = p.f32(q + "norm1.norm.bias", dl);
-            e.n2g = p.f32(q + "norm2.norm.weight", dl); e.n2b = p.f32(q + "norm2.norm.bias", dl);
-        }
-        W->lm_norm_g = p.f32("lm.encoder.norm.norm.weight", dl); W->lm_norm_b = p.f32("lm.encoder.norm.norm.bias", dl);
-        W->lm_wp0 = p.f16("lm.output_proj.layers.0.w.weight", (int64_t)dl * dl); W->lm_bp0 = p.f32("lm.output_proj.layers.0.w.bias", dl);
-        W->lm_lnp_g = p.f32("lm.output_proj.layers.1.norm.weight", dl); W->lm_lnp_b = p.f32("lm.output_proj.layers.1.norm.bias", dl);
-        W->lm_wp2 = p.f16("lm.output_proj.layers.2.w.weight", (int64_t)c.vocab * dl); W->lm_bp2 = p.f32("lm.output_proj.layers.2.w.bias", c.vocab);
-        if (!p.ok) return SBK_ERR_ARG;
-    }
-    if (w.count("ctc_lin.w.weight")) {
-        W->w_ctc = p.f16("ctc_lin.w.weight", (int64_t)c.vocab * d);
-        W->b_ctc = p.f32("ctc_lin.w.bias", c.vocab);
-    }
-    if (!p.ok) return SBK_ERR_ARG;
-    if (cudaDeviceSynchronize() != cudaSuccess) { set_error("asr_create: device error after upload"); return SBK_ERR_CUDA; }
+    std::shared_ptr<const AsrWeights> wt;
+    RC(load_asr_weights(*cfg, weights, n_weights, &wt));
     return new_lane(std::move(wt), out);
 }
 
@@ -1843,8 +1298,7 @@ int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int 
                 B, T, d, nhead, k);
     const int e = d / nhead;
     const size_t n1 = (size_t)nhead * e * e, n2 = (size_t)nhead * k * e;
-    std::vector<float> pe((size_t)HM_PE_ROWS * d);
-    hypermix_pe_table(d, pe.data());
+    const std::vector<float> pe = sine_table(HM_PE_ROWS, d);
     const size_t part_n = hypermix_part_floats(B, T, d, k);
     __half *w16 = nullptr, *G = nullptr;
     float *pe_dev = nullptr, *part = nullptr, *gscale = nullptr;

@@ -8,6 +8,18 @@
 
 namespace sbk {
 
+// Lays fields out one after another in a buffer, each at a 256-byte boundary.  A buffer's layout is one function that runs
+// twice: with base == nullptr to measure the bytes it needs (`used`), then with the buffer to set the fields.
+struct Carver {
+    uint8_t* base = nullptr;
+    size_t used = 0;
+    template <class T>
+    void operator()(T*& field, size_t bytes) {
+        if (base) field = reinterpret_cast<T*>(base + used);
+        used += (bytes + 255) & ~size_t(255);
+    }
+};
+
 enum GemmEpiMode { EPI_F16 = 0, EPI_F32 = 1, EPI_RESID = 2, EPI_GLU = 3, EPI_ROPE = 4, EPI_QKV_CACHE = 5 };
 enum GemmAct { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU = 2, ACT_RELU = 3, ACT_SILU_FAST = 4 /* tanh.approx form; for EPI_GLU: fast gate sigmoid */ };
 
@@ -116,12 +128,11 @@ struct HyperMixWeights {
 };
 constexpr int HM_PE_ROWS = 3000;  // HyperMixing's own PositionalEncoding(d, max_length=3000)
 // x [B*T, d] fp32 += LayerNorm_hm(HyperMixing(h16)), h16 the norm1 output [B*T, d] fp16; M heads of e = d / M in {32, 64},
-// KH = d_ffn / M (multiple of 16, <= 256); pe [HM_PE_ROWS, d] fp32 (hypermix_pe_table); lens device int[B] (null: all T).
+// KH = d_ffn / M (multiple of 16, <= 256); pe [HM_PE_ROWS, d] fp32 (sine_table); lens device int[B] (null: all T).
 // Scratch: part (hypermix_part_floats), G [B * d * KH] fp16, gscale [B * M] fp32.  T <= HM_PE_ROWS.
 int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, const int* lens, const float* pe,
                      const HyperMixWeights& w, float* part, __half* G, float* gscale, float* x, cudaStream_t stream);
 size_t hypermix_part_floats(int B, int T, int d, int KH);
-void hypermix_pe_table(int d, float* dst);  // [HM_PE_ROWS, d] (host)
 // chunk > 0: Dynamic Chunk Convolution (inputs past the end of the output frame's chunk are zero).  left: [B, (K-1)/2, D]
 // inputs of the frames before frame 0 (a stream's carry), null = zero padding.
 int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw,
