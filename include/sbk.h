@@ -149,6 +149,32 @@ int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int hea
                                const float* pos_u_dev, const float* pos_v_dev, const void* P_dev, float scale, int chunk,
                                int left_chunks, void* out_dev, void* stream);
 
+/* one Linear of a decode / TransformerLM step alone, through the engine's step projection: out[rows, N] (row stride ldo) =
+ * epilogue(A[rows, K] W[N, K]^T + bias), fp16 operands, fp32 accumulate.  backend 0 = weight streaming, 1 = the wgmma GEMM
+ * (each launched with the programmatic-dependent-launch setting the step loops give it).  epilogue: 0 fp16, 1 fp16 GELU
+ * (erf), 2 fp16 ReLU, 3 fp32, 4 fp32 residual (out += ...), 5 QKV_CACHE: columns [q | k | v] of width N / 3, q (fp16) to out,
+ * k and v to kcache_dev / vcache_dev [rows][S_max][N / 3] fp16 at position step.  fp16 stores saturate at +-65504.  The A
+ * operand is either A_dev fp16 (row stride lda; X_dev NULL) or LayerNorm(X_dev) of X_dev fp32 [rows, K] with ln_g / ln_b [K]
+ * and eps 1e-6 (A_dev NULL): the decoder's pre-norm, fused into the weight-streaming kernel where it is built for K (256,
+ * 512, 768, 1024), otherwise a separate LayerNorm kernel.  K % 16 == 0; the wgmma back end needs K, lda and ldo % 8 == 0
+ * and, for QKV_CACHE, N / 3 % 32 == 0.  Allocates and frees its own scratch and synchronises the stream. */
+int sbk_step_proj_test(int backend, int epilogue, const void* A_dev, int lda, const float* X_dev, const float* ln_g_dev,
+                       const float* ln_b_dev, const void* W_dev, const float* bias_dev, int rows, int N, int K, void* out_dev,
+                       int ldo, void* kcache_dev, void* vcache_dev, int S_max, int step, void* stream);
+
+/* the decode-step attention alone (one query per row, nn.MultiheadAttention with the scale folded into q): q_dev fp16, row r
+ * head h at q_dev[r * ldq + h * dh]; key j of head h for row block b = r / rows_per_block at kbase_dev / vbase_dev
+ * [b * row_stride + h * head_stride + j * key_stride] (head_stride 0 = dh) -> out_dev [r * ldo + h * dh] fp16.  dh 64, 128
+ * or a multiple of 4 up to 64 (at most 2560 keys).  step >= 0: self-attention over the step + 1 cached keys [0, step]; with
+ * lineage_dev [2][rows][lin_stride] (rows_per_block 1) key j of row r lives in cache row lineage[step % 2][r][j], every
+ * entry in [0, rows); with tok_cache_dev [rows][lin_stride] keys whose token tok_cache[cache row][j] == pad_tok are masked.
+ * step < 0: cross-attention over the first enc_len_dev[b] of max_keys frames (enc_len_dev NULL: all max_keys), in [0,
+ * max_keys].  A row with no visible key is NaN, as in the reference.  Synchronises the stream. */
+int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, const void* vbase_dev, long long row_stride,
+                           int key_stride, int head_stride, int rows_per_block, int rows, int H, int dh, int max_keys, int step,
+                           const int* enc_len_dev, const int* lineage_dev, const int* tok_cache_dev, int lin_stride,
+                           int pad_tok, void* out_dev, int ldo, void* stream);
+
 /* the streaming encoder's ring write alone (stream_qkv_kernel): qkv_dev [B*n, 3*H*head_dim] fp32 (per head [q | k | v]) ->
  * q_out_dev [B*n, H*head_dim] fp16 and each row's per-head [k | v] into slot (slot0 + i) % cap of kv_out_dev
  * [B][cap][2*H*head_dim] fp16.  inv_freq_dev [head_dim / 2] fp32: RoPE at stream positions pos0 + i with q scaled by

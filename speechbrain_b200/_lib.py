@@ -62,7 +62,7 @@ EXPORTS = [
     "sbk_asr_lm_forward", "sbk_asr_lm_step_logits", "sbk_ctc_beam_workspace_bytes", "sbk_ctc_beam_search",
     "sbk_transducer_create", "sbk_transducer_destroy", "sbk_transducer_info", "sbk_transducer_greedy",
     "sbk_asr_stream_create", "sbk_asr_stream_encode_chunk", "sbk_asr_stream_reset", "sbk_asr_stream_destroy",
-    "sbk_asr_stream_context", "sbk_stream_qkv_test",
+    "sbk_asr_stream_context", "sbk_stream_qkv_test", "sbk_step_proj_test", "sbk_dec_attention_test",
 ]
 
 

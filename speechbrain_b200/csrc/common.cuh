@@ -312,6 +312,14 @@ __device__ __forceinline__ float4 u4_as_f4(uint4 u) {
 __device__ __forceinline__ float silu_f(float x) { return x * sigmoid_f(x); }
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
+// One merge step of an arg-max, in torch.argmax's order: NaN counts as the largest value, and the lower index wins ties.
+// True when (v, i) replaces (best, bi); start from (-INFINITY, INT_MAX).  A row of NaN (the logits of an utterance with no
+// encoder frame) thus gives its first index, as the reference does, instead of the start index.
+__device__ __forceinline__ bool argmax_takes(float v, int i, float best, int bi) {
+    if (isnan(v)) return !isnan(best) || i < bi;
+    return !isnan(best) && (v > best || (v == best && i < bi));
+}
+
 // ordered-int encoding so that atomicMax on int orders floats correctly
 __device__ __forceinline__ int float_to_ordered(float f) {
     int i = __float_as_int(f);

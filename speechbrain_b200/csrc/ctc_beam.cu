@@ -133,19 +133,19 @@ __device__ __forceinline__ int block_argmax(const float* col, int V, float* s_f,
     int bi = 0x7fffffff;
     for (int j = threadIdx.x; j < V; j += blockDim.x) {
         const float v = col[j];
-        if (v > best || (v == best && j < bi)) { best = v; bi = j; }
+        if (argmax_takes(v, j, best, bi)) { best = v; bi = j; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         const float ov = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+        if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
     if ((threadIdx.x & 31) == 0) { s_f[threadIdx.x >> 5] = best; s_i[threadIdx.x >> 5] = bi; }
     __syncthreads();
     best = s_f[0]; bi = s_i[0];
     for (int w = 1; w < static_cast<int>(blockDim.x >> 5); ++w)
-        if (s_f[w] > best || (s_f[w] == best && s_i[w] < bi)) { best = s_f[w]; bi = s_i[w]; }
+        if (argmax_takes(s_f[w], s_i[w], best, bi)) { best = s_f[w]; bi = s_i[w]; }
     __syncthreads();
     return bi;
 }

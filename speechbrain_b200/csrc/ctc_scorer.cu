@@ -438,19 +438,19 @@ rows_logsoftmax_argmax_kernel(float* __restrict__ x, int V, int do_logsoftmax, i
     int bi = 0x7fffffff;
     for (int j = tid; j < V; j += 256) {
         const float v = xr[j];
-        if (v > best || (v == best && j < bi)) { best = v; bi = j; }
+        if (argmax_takes(v, j, best, bi)) { best = v; bi = j; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         const float ov = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+        if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
     if ((tid & 31) == 0) { s_val[tid >> 5] = best; s_idx[tid >> 5] = bi; }
     __syncthreads();
     best = s_val[0]; bi = s_idx[0];
     for (int w = 1; w < 8; ++w)
-        if (s_val[w] > best || (s_val[w] == best && s_idx[w] < bi)) { best = s_val[w]; bi = s_idx[w]; }
+        if (argmax_takes(s_val[w], s_idx[w], best, bi)) { best = s_val[w]; bi = s_idx[w]; }
     if (idx != nullptr && tid == 0) idx[row] = bi;
     if (!do_logsoftmax) return;
     __syncthreads();

@@ -545,19 +545,19 @@ greedy_select_kernel(const float* __restrict__ logits, int V, int* __restrict__ 
     int bi = 0x7fffffff;
     for (int i = threadIdx.x; i < V; i += blockDim.x) {
         const float v = lg[i];
-        if (v > best || (v == best && i < bi)) { best = v; bi = i; }
+        if (argmax_takes(v, i, best, bi)) { best = v; bi = i; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         const float ov = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+        if (argmax_takes(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
     if ((threadIdx.x & 31) == 0) { s_val[threadIdx.x >> 5] = best; s_idx[threadIdx.x >> 5] = bi; }
     __syncthreads();
     best = s_val[0]; bi = s_idx[0];
     for (int w = 1; w < 8; ++w)
-        if (s_val[w] > best || (s_val[w] == best && s_idx[w] < bi)) { best = s_val[w]; bi = s_idx[w]; }
+        if (argmax_takes(s_val[w], s_idx[w], best, bi)) { best = s_val[w]; bi = s_idx[w]; }
     float sum = 0.0f;
     for (int i = threadIdx.x; i < V; i += blockDim.x) sum += expf(lg[i] - best);
     sum = warp_sum(sum);

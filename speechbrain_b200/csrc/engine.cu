@@ -609,20 +609,24 @@ static int project(StepGemm g, const Proj& p, int rows, cudaStream_t st) {
     return gemm_f16(p.A, p.lda, p.W, p.K, e, rows, p.N, p.K, st);
 }
 
-// A decoder pre-norm LN(b.dx) and the projection it feeds.  Weight streaming fuses the LayerNorm into the projection kernel
-// where that kernel is built for the width, which saves a launch per projection (single-batch latency); with fusion off it
-// runs a separate kernel into b.dh16, which avoids recomputing the same 32-row LayerNorm in ~100-300 CTAs (GPU time when
-// several batches are in flight).  The wgmma step always runs the separate kernel, launched with PDL.
-static int dec_norm_project(AsrModel* m, StepGemm g, Proj p, const float* gamma, const float* beta, int rows, cudaStream_t st) {
-    AsrModel::Buf& b = m->b;
-    const int d = m->wt->cfg.d_model;
-    if (g == SG_STREAM && m->fuse_dec_ln && (d == 256 || d == 512 || d == 768 || d == 1024)) {
-        p.X = b.dx; p.ln_g = gamma; p.ln_b = beta;
+// A decoder pre-norm LN(x) (x fp32 [rows, p.K], eps 1e-6) and the projection it feeds.  Weight streaming fuses the LayerNorm
+// into the projection kernel where that kernel is built for the width, which saves a launch per projection (single-batch
+// latency); with fusion off it runs a separate kernel into h16 [rows, p.K], which avoids recomputing the same 32-row LayerNorm
+// in ~100-300 CTAs (GPU time when several batches are in flight).  The wgmma step always runs the separate kernel, launched
+// with PDL.
+static int norm_project(StepGemm g, bool fuse_ln, Proj p, const float* x, const float* gamma, const float* beta, __half* h16,
+                        int rows, cudaStream_t st) {
+    const int d = p.K;
+    if (g == SG_STREAM && fuse_ln && (d == 256 || d == 512 || d == 768 || d == 1024)) {
+        p.X = x; p.ln_g = gamma; p.ln_b = beta;
     } else {
-        RC(layernorm_rows(b.dx, b.dh16, true, gamma, beta, rows, d, 1e-6f, false, st, g != SG_STREAM));
-        p.A = b.dh16; p.lda = d;
+        RC(layernorm_rows(x, h16, true, gamma, beta, rows, d, 1e-6f, false, st, g != SG_STREAM));
+        p.A = h16; p.lda = d;
     }
     return project(g, p, rows, st);
+}
+static int dec_norm_project(AsrModel* m, StepGemm g, Proj p, const float* gamma, const float* beta, int rows, cudaStream_t st) {
+    return norm_project(g, m->fuse_dec_ln, p, m->b.dx, gamma, beta, m->b.dh16, rows, st);
 }
 
 static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage,
@@ -1253,6 +1257,112 @@ int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int hea
                                pos_v_dev, static_cast<const __half*>(P_dev), d, scale, static_cast<__half*>(out_dev), d, st,
                                chunk, left_chunks);
     if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("encoder_attention_test: device error"); rc = SBK_ERR_CUDA; }
+    return rc;
+}
+
+int sbk_step_proj_test(int backend, int epilogue, const void* A_dev, int lda, const float* X_dev, const float* ln_g_dev,
+                       const float* ln_b_dev, const void* W_dev, const float* bias_dev, int rows, int N, int K, void* out_dev,
+                       int ldo, void* kcache_dev, void* vcache_dev, int S_max, int step, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(backend == 0 || backend == 1, "step_proj_test: backend %d (0 weight streaming, 1 wgmma)", backend);
+    SBK_REQUIRE(epilogue >= PO_F16 && epilogue <= PO_QKV_CACHE, "step_proj_test: epilogue %d", epilogue);
+    SBK_REQUIRE(W_dev && out_dev && (A_dev != nullptr) != (X_dev != nullptr) && (!X_dev || (ln_g_dev && ln_b_dev)),
+                "step_proj_test: null pointer, or not exactly one of A and X");
+    SBK_REQUIRE(rows >= 1 && N >= 1 && K >= 16 && K % 16 == 0 && (!A_dev || lda >= K),
+                "step_proj_test: bad sizes rows=%d N=%d K=%d lda=%d", rows, N, K, lda);
+    const bool qkv = epilogue == PO_QKV_CACHE;
+    SBK_REQUIRE(!qkv || (N % 3 == 0 && kcache_dev && vcache_dev && step >= 0 && step < S_max),
+                "step_proj_test: QKV_CACHE needs N %% 3 == 0, both caches and 0 <= step < S_max (N=%d step=%d S_max=%d)", N,
+                step, S_max);
+    SBK_REQUIRE(ldo >= (qkv ? N / 3 : N), "step_proj_test: ldo=%d below the output width", ldo);
+    // the wgmma epilogue stores 16-byte vectors
+    SBK_REQUIRE(backend == 0 || (ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(out_dev) & 15) == 0),
+                "step_proj_test: the wgmma back end needs ldo %% 8 == 0 and a 16-byte aligned out");
+    int* steps = nullptr;
+    __half* h16 = nullptr;
+    auto layout = [&](Carver& take) { take(steps, (size_t)rows * 4); take(h16, X_dev ? (size_t)rows * K * 2 : 0); };
+    Carver measure;
+    layout(measure);
+    uint8_t* base = nullptr;
+    if (cudaMalloc(&base, measure.used) != cudaSuccess) { set_error("step_proj_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
+    Carver carve{base};
+    layout(carve);
+    // one counter per row, all equal, as b.step holds them: the weight-streaming kernel reads row 0's, the wgmma epilogue
+    // each row's
+    const std::vector<int> step_val(rows, step);
+    int rc = cudaMemcpyAsync(steps, step_val.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, st) == cudaSuccess ? SBK_OK
+                                                                                                                 : SBK_ERR_CUDA;
+    if (rc == SBK_OK) {
+        const StepGemm g = backend == 1 ? SG_SMALL : SG_STREAM;
+        set_pdl(g == SG_SMALL);  // what set_step_pdl gives this back end
+        Proj p{static_cast<const __half*>(W_dev), bias_dev, N, K, static_cast<ProjOut>(epilogue), out_dev, ldo,
+               static_cast<const __half*>(A_dev), lda};
+        if (qkv) {
+            p.kcache = static_cast<__half*>(kcache_dev); p.vcache = static_cast<__half*>(vcache_dev);
+            p.step_ptr = steps; p.S_max = S_max;
+        }
+        rc = X_dev ? norm_project(g, true, p, X_dev, ln_g_dev, ln_b_dev, h16, rows, st) : project(g, p, rows, st);
+    }
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("step_proj_test: device error"); rc = SBK_ERR_CUDA; }
+    cudaFree(base);
+    return rc;
+}
+
+int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, const void* vbase_dev, long long row_stride,
+                           int key_stride, int head_stride, int rows_per_block, int rows, int H, int dh, int max_keys, int step,
+                           const int* enc_len_dev, const int* lineage_dev, const int* tok_cache_dev, int lin_stride,
+                           int pad_tok, void* out_dev, int ldo, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(q_dev && kbase_dev && vbase_dev && out_dev, "dec_attention_test: null pointer");
+    SBK_REQUIRE(rows >= 1 && H >= 1 && dh >= 1 && max_keys >= 1 && rows_per_block >= 1 && rows % rows_per_block == 0 &&
+                    ldq >= H * dh && ldo >= H * dh && key_stride >= 1 && row_stride >= 0 && head_stride >= 0,
+                "dec_attention_test: bad sizes rows=%d rows_per_block=%d H=%d dh=%d max_keys=%d", rows, rows_per_block, H, dh,
+                max_keys);
+    if (dh == 64 || dh == 128) {  // 16-byte loads of q, K and V
+        const uintptr_t al = reinterpret_cast<uintptr_t>(q_dev) | reinterpret_cast<uintptr_t>(kbase_dev) |
+                             reinterpret_cast<uintptr_t>(vbase_dev);
+        SBK_REQUIRE((al & 15) == 0 && ldq % 8 == 0 && key_stride % 8 == 0 && row_stride % 8 == 0 && head_stride % 8 == 0,
+                    "dec_attention_test: head_dim %d needs 16-byte aligned q / key rows", dh);
+    }
+    const bool self = step >= 0;
+    SBK_REQUIRE(self || (!lineage_dev && !tok_cache_dev), "dec_attention_test: a lineage or token mask needs self-attention");
+    SBK_REQUIRE(!lineage_dev || rows_per_block == 1, "dec_attention_test: a lineage table needs one cache row per query row");
+    SBK_REQUIRE(!self || step < max_keys, "dec_attention_test: step %d >= max_keys %d", step, max_keys);
+    SBK_REQUIRE(!(lineage_dev || tok_cache_dev) || step < lin_stride, "dec_attention_test: step %d >= lin_stride %d", step,
+                lin_stride);
+    // the kernels index rows and frames with these: check them on the host first
+    if (lineage_dev) {
+        std::vector<int> lin((size_t)2 * rows * lin_stride);
+        SBK_CUDA_CHECK(cudaMemcpyAsync(lin.data(), lineage_dev, lin.size() * 4, cudaMemcpyDeviceToHost, st));
+        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+        for (size_t i = 0; i < lin.size(); ++i)
+            SBK_REQUIRE(lin[i] >= 0 && lin[i] < rows, "dec_attention_test: lineage entry %zu = %d outside [0, %d)", i, lin[i], rows);
+    }
+    if (!self && enc_len_dev) {
+        std::vector<int> len(rows / rows_per_block);
+        SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), enc_len_dev, len.size() * 4, cudaMemcpyDeviceToHost, st));
+        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+        for (int v : len) SBK_REQUIRE(v >= 0 && v <= max_keys, "dec_attention_test: enc_len %d outside [0, %d]", v, max_keys);
+    }
+    int* step_dev = nullptr;
+    if (self) {
+        if (cudaMalloc(&step_dev, 4) != cudaSuccess) { set_error("dec_attention_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
+        if (cudaMemcpyAsync(step_dev, &step, 4, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+            cudaFree(step_dev);
+            set_error("dec_attention_test: copy failed");
+            return SBK_ERR_CUDA;
+        }
+    }
+    DecAttnArgs t{};
+    t.q = static_cast<const __half*>(q_dev); t.ldq = ldq;
+    t.kbase = static_cast<const __half*>(kbase_dev); t.vbase = static_cast<const __half*>(vbase_dev);
+    t.row_stride = (size_t)row_stride; t.key_stride = key_stride; t.head_stride = head_stride; t.rows_per_block = rows_per_block;
+    t.n_keys_ptr = step_dev; t.enc_len = self ? nullptr : enc_len_dev; t.H = H; t.dh = dh;
+    t.out = static_cast<__half*>(out_dev); t.ldo = ldo;
+    t.lineage = lineage_dev; t.tok_cache = tok_cache_dev; t.lin_stride = lin_stride; t.pad_tok = pad_tok;
+    int rc = dec_attention(t, rows, max_keys, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("dec_attention_test: device error"); rc = SBK_ERR_CUDA; }
+    cudaFree(step_dev);
     return rc;
 }
 
