@@ -25,6 +25,9 @@ void set_error(const char* fmt, ...);
         }                                                                                 \
     } while (0)
 
+// returns a failed call's error code
+#define RC(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
+
 // every kernel launch goes through this: counts launches (bench.py "gpu_launches") and checks the launch
 void count_launch();
 #define SBK_LAUNCH_CHECK()                   \

@@ -15,8 +15,6 @@
 
 namespace sbk {
 
-#define RC(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
-
 // One cached CUDA graph and the key it was captured for.  Keys are compared bytewise, so callers zero their padding.
 struct GraphCache {
     cudaGraphExec_t exec = nullptr;
@@ -67,6 +65,42 @@ struct DevBuf {
     ~DevBuf() { cudaFree(base); }
 };
 
+// A lane's second stream, created by ensure() on first use, with the events that fork work onto it and join it back.
+// Under stream capture the fork and join become graph edges.
+struct SideStream {
+    cudaStream_t s = nullptr;
+    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    SideStream() = default;
+    SideStream(const SideStream&) = delete;
+    SideStream& operator=(const SideStream&) = delete;
+    ~SideStream() {
+        if (s) cudaStreamDestroy(s);
+        if (ev_fork) cudaEventDestroy(ev_fork);
+        if (ev_join) cudaEventDestroy(ev_join);
+    }
+    int ensure(bool top_priority = false) {
+        if (s) return SBK_OK;
+        int lo = 0, hi = 0;  // numerically lowest = highest priority; 0 = the default
+        if (top_priority) SBK_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+        SBK_CUDA_CHECK(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, hi));
+        SBK_CUDA_CHECK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
+        SBK_CUDA_CHECK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
+        return SBK_OK;
+    }
+    // s waits for the work enqueued on `from` so far
+    int fork(cudaStream_t from) {
+        SBK_CUDA_CHECK(cudaEventRecord(ev_fork, from));
+        SBK_CUDA_CHECK(cudaStreamWaitEvent(s, ev_fork, 0));
+        return SBK_OK;
+    }
+    // `into` waits for the work enqueued on s so far
+    int join(cudaStream_t into) {
+        SBK_CUDA_CHECK(cudaEventRecord(ev_join, s));
+        SBK_CUDA_CHECK(cudaStreamWaitEvent(into, ev_join, 0));
+        return SBK_OK;
+    }
+};
+
 // A handle: the shared weights plus one lane's state.  A clone is another lane on the same weights with its own workspace,
 // graphs, streams and flags: one clone per in-flight batch lets independent batches overlap on different streams (the
 // decode loop is latency-bound and leaves most SMs idle, so concurrent lanes raise throughput without touching per-batch
@@ -114,12 +148,10 @@ struct AsrModel {
     // host-buffer group entry point: device staging of the G batches' wav / lengths, a copy stream forked from the caller's
     // stream (so the H2D of a later encoder pass's batches overlaps an earlier pass)
     DevBuf gwav;
-    cudaStream_t copy_stream = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_ready[16] = {};
-    cudaStream_t side_stream = nullptr;     // beam search: the LM scorer's branch of a search step
-    cudaStream_t dec_stream = nullptr;      // group calls: the decode loop, on a high-priority stream (see transcribe_group_enqueue)
-    cudaEvent_t ev_dfork = nullptr, ev_djoin = nullptr;
-    cudaEvent_t ev_bfork = nullptr, ev_bjoin = nullptr;
+    SideStream copy_stream;
+    cudaEvent_t ev_ready[16] = {};  // batch g's staging copies have landed
+    SideStream side_stream;  // beam search: the LM scorer's branch of a search step
+    SideStream dec_stream;   // group calls: the decode loop, on a high-priority stream (see transcribe_group_enqueue)
     cudaStream_t cap_stream = nullptr;  // private stream for graph capture (the legacy default stream cannot capture)
     int dec_tc_rows = getenv("SBK_DEC_TC_ROWS") ? atoi(getenv("SBK_DEC_TC_ROWS")) : 64;  // >= this many live hypotheses: wgmma decode GEMMs
     int dyn_chunk = 0, dyn_left = -1;  // DynChunkTrainConfig of the next encode calls (chunk frames, left-context chunks; 0 = off)
@@ -131,14 +163,26 @@ struct AsrModel {
     AsrModel& operator=(const AsrModel&) = delete;
     ~AsrModel() {
         if (host_flag) cudaFreeHost(host_flag);
-        for (cudaStream_t s : {copy_stream, side_stream, dec_stream, cap_stream})
-            if (s) cudaStreamDestroy(s);
-        for (cudaEvent_t e : {ev_fork, ev_dfork, ev_djoin, ev_bfork, ev_bjoin})
-            if (e) cudaEventDestroy(e);
+        if (cap_stream) cudaStreamDestroy(cap_stream);
         for (cudaEvent_t e : ev_ready)
             if (e) cudaEventDestroy(e);
     }
 };
+
+// A whole call as one CUDA graph: replays `graph` for `key` (capturing enqueue(cap_stream, &done, true) first when the key
+// is new), which runs exactly max_steps decode steps.  With use_graph false: enqueue(st, steps_done, false), eagerly.
+template <class Key, class Enqueue>
+static int replay_or_enqueue(AsrModel* m, GraphCache& graph, bool use_graph, const Key& key, int max_steps, int* steps_done,
+                             cudaStream_t st, Enqueue&& enqueue) {
+    if (!use_graph) return enqueue(st, steps_done, false);
+    RC(graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
+        int done = 0;
+        return enqueue(cs, &done, true);
+    }));
+    RC(graph.launch(st));
+    if (steps_done) *steps_done = max_steps;
+    return SBK_OK;
+}
 
 // A new lane on the weights of `wt`.
 static int new_lane(std::shared_ptr<const AsrWeights> wt, AsrModel** out) {
@@ -208,6 +252,9 @@ static void frames(const sbk_asr_config& c, int L, int* T0, int* T1, int* T2) {
     *T2 = (*T1 - 1) / 2 + 1;
 }
 
+// A sample count whose frames() give T encoder frames: sizes the workspace of entries that start from encoder states.
+static int enc_samples(const sbk_asr_config& c, int T) { return (T - 1) * 4 * c.hop; }
+
 // The workspace for calls of B utterances of L samples whose encoder passes take up to Be utterances (Be > B: a group call
 // encodes several of its batches in one pass), `rows` decoder hypotheses, `steps` max steps.  Encoder activations are sized
 // for Be utterances, the per-call buffers (wav, Fbank scratch, lengths, flags) for B.
@@ -256,8 +303,8 @@ static void workspace_layout(const AsrModel* m, int B, int Be, int L, int rows, 
     }
 }
 
-// (Re)carve the workspace for at least the given shapes and the ones it is already carved for.  Be: utterances per encoder
-// pass (0: B).
+// (Re)carve the workspace for at least the given shapes and the ones it is already carved for, so callers pass only what
+// they need.  Be: utterances per encoder pass (0: B).
 static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps, int Be = 0) {
     Be = std::max(Be, B);
     if (m->ws.base && B <= m->wsB && Be <= m->wsBe && L <= m->wsL && rows <= m->ws_rows && steps <= m->ws_steps) return SBK_OK;
@@ -508,6 +555,12 @@ static int set_enc_len(int* enc_len, const float* rel_len, int B, int T, cudaStr
     return SBK_OK;
 }
 
+// Copies a caller's encoder states enc [n, T, d] fp32 into b.enc_out, where the decoders and the CTC head read them.
+static int stage_enc(AsrModel* m, const float* enc, int n, int T, cudaStream_t st) {
+    SBK_CUDA_CHECK(cudaMemcpyAsync(m->b.enc_out, enc, (size_t)n * T * m->wt->cfg.d_model * 4, cudaMemcpyDeviceToDevice, st));
+    return SBK_OK;
+}
+
 // Copies the first `steps` columns of a [rows, S_max] per-step workspace array (b.pred, b.score) into dst [rows, ld];
 // nothing when dst is null.
 static int copy_steps(const AsrModel* m, void* dst, int ld, const void* src, int steps, int rows, cudaMemcpyKind kind,
@@ -729,6 +782,26 @@ static int enqueue_lm_step(AsrModel* m, int rows, int S_max, float temperature, 
     return weighted_log_softmax(b.lm_logits, b.lm_extra, rows, c.vocab, temperature, weight, st);
 }
 
+// Enqueues up to max_steps search steps, step(st) each.  Every poll_every steps (0: never) the host reads b.ended_count and
+// stops once it has reached `target`.  *done: the steps enqueued.
+template <class Step>
+static int run_steps(AsrModel* m, int max_steps, int target, cudaStream_t st, Step&& step, int* done) {
+    const int check_every = m->poll_every > 0 ? m->poll_every : max_steps;
+    int s = 0;
+    while (s < max_steps) {
+        const int chunk = std::min(check_every, max_steps - s);
+        for (int i = 0; i < chunk; ++i) RC(step(st));
+        s += chunk;
+        if (s < max_steps && m->poll_every > 0) {
+            SBK_CUDA_CHECK(cudaMemcpyAsync(m->host_flag, m->b.ended_count, 4, cudaMemcpyDeviceToHost, st));
+            SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+            if (*m->host_flag >= target) break;
+        }
+    }
+    *done = s;
+    return SBK_OK;
+}
+
 // Beam search (decoders/seq2seq.py:1632-1723 with scorer=None): the device runs decoder step + beam_step_kernel and
 // records the per-step (token, predecessor, normalised score, log-prob) history; hypothesis bookkeeping is replayed
 // on the host from that history (speechbrain_b200/decoders/seq2seq.py).
@@ -810,26 +883,18 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
     // the TransformerLM step and the CTC state update of the PREVIOUS step's survivors -- run as a second branch beside
     // the decoder layers (both are chains of small kernels that leave most SMs idle) and join before the scores are combined.
     const bool fork = (use_lm || use_ctc) && getenv("SBK_BEAM_SERIAL") == nullptr;
-    if (fork && !m->side_stream) {
-        SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->side_stream, cudaStreamNonBlocking));
-        SBK_CUDA_CHECK(cudaEventCreateWithFlags(&m->ev_bfork, cudaEventDisableTiming));
-        SBK_CUDA_CHECK(cudaEventCreateWithFlags(&m->ev_bjoin, cudaEventDisableTiming));
-    }
+    if (fork) RC(m->side_stream.ensure());
     auto enqueue_step = [&](cudaStream_t s_) -> int {
         cudaStream_t s2 = s_;
         if (fork) {
-            s2 = m->side_stream;
-            SBK_CUDA_CHECK(cudaEventRecord(m->ev_bfork, s_));
-            SBK_CUDA_CHECK(cudaStreamWaitEvent(s2, m->ev_bfork, 0));
+            RC(m->side_stream.fork(s_));
+            s2 = m->side_stream.s;
         }
         if (use_ctc) RC(ctc_prefix_update(cs, s2));  // permute_scorer_mem on the previous step's survivors (no-op at step 0)
         if (use_lm) RC(enqueue_lm_step(m, rows, S_max, p.lm_temperature, p.lm_weight, s2));
         RC(enqueue_decode_layers(m, rows, beam, T, S_max, b.lineage, s_));
         if (use_cov) RC(coverage_score(cv, s_));  // reads the last layer's cross-attention query left in b.dq16
-        if (fork) {
-            SBK_CUDA_CHECK(cudaEventRecord(m->ev_bjoin, s2));
-            SBK_CUDA_CHECK(cudaStreamWaitEvent(s_, m->ev_bjoin, 0));
-        }
+        if (fork) RC(m->side_stream.join(s_));
         if (use_ctc) RC(ctc_prefix_score(cs, s_));  // ScorerBuilder.score (ctc after transformerlm)
         RC(beam_step(a, B, s_));
         return SBK_OK;
@@ -841,20 +906,9 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
         key.p = p; key.B = B; key.T = T; key.rows = rows; key.S_max = S_max; key.fuse_ln = m->fuse_dec_ln; key.tc_rows = m->dec_tc_rows; key.fork = fork ? 1 : 0;
         RC(m->beam_graph.ensure(key, m->cap_stream, enqueue_step));
     }
-    const int check_every = m->poll_every > 0 ? m->poll_every : p.max_steps;
-    int s = 0;
-    while (s < p.max_steps) {
-        const int chunk = std::min(check_every, p.max_steps - s);
-        for (int i = 0; i < chunk; ++i) {
-            RC(use_graph ? m->beam_graph.launch(st) : enqueue_step(st));
-        }
-        s += chunk;
-        if (s < p.max_steps && m->poll_every > 0) {  // `_check_full_beams` (:806-822), polled once per chunk
-            SBK_CUDA_CHECK(cudaMemcpyAsync(m->host_flag, b.ended_count, 4, cudaMemcpyDeviceToHost, st));
-            SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-            if (*m->host_flag >= B) break;
-        }
-    }
+    int s = 0;  // `_check_full_beams` (:806-822): b.ended_count counts the utterances whose beams are full
+    RC(run_steps(m, p.max_steps, B, st, [&](cudaStream_t s_) { return use_graph ? m->beam_graph.launch(s_) : enqueue_step(s_); },
+                 &s));
     const size_t hb = (size_t)s * rows * 4;
     if (hist_tok_out) SBK_CUDA_CHECK(cudaMemcpyAsync(hist_tok_out, hist_tok, hb, cudaMemcpyDeviceToDevice, st));
     if (hist_pred_out) SBK_CUDA_CHECK(cudaMemcpyAsync(hist_pred_out, hist_pred, hb, cudaMemcpyDeviceToDevice, st));
@@ -889,22 +943,10 @@ static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos
             return enqueue_decode_step(m, rows, 1, T, S_max, eos, nullptr, 0, cs);
         }));
     }
-    const int check_every = m->poll_every > 0 ? m->poll_every : max_steps;
-    int s = 0;
-    while (s < max_steps) {
-        const int chunk = std::min(check_every, max_steps - s);
-        for (int i = 0; i < chunk; ++i) {
-            RC(use_graph ? m->step_graph.launch(st) : enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, st));
-        }
-        s += chunk;
-        if (s < max_steps && m->poll_every > 0) {  // seq2seq.py:256 `has_ended.all()` early exit, polled once per chunk
-            SBK_CUDA_CHECK(cudaMemcpyAsync(m->host_flag, b.ended_count, 4, cudaMemcpyDeviceToHost, st));
-            SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-            if (*m->host_flag >= rows) break;
-        }
-    }
-    *steps_done = s;
-    return SBK_OK;
+    // seq2seq.py:256 `has_ended.all()` early exit
+    return run_steps(m, max_steps, rows, st, [&](cudaStream_t s_) {
+        return use_graph ? m->step_graph.launch(s_) : enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, s_);
+    }, steps_done);
 }
 
 // ---------------------------------------------------------------------------- TransformerLMRescorer (scorer.py:1835-1882)
@@ -1128,138 +1170,6 @@ int sbk_input_norm_sentence(const float* x_dev, float* out_dev, const float* rel
                                  static_cast<cudaStream_t>(stream));
 }
 
-int sbk_gemm_f16_test(const void* A_dev, const void* W_dev, const float* bias_dev, void* out_dev, int out_is_f32, int act,
-                      int M, int N, int K, void* stream) {
-    GemmEpilogue e;
-    e.mode = out_is_f32 ? EPI_F32 : EPI_F16;
-    e.act = act;
-    e.bias = bias_dev;
-    e.out = out_dev;
-    e.ldo = N;
-    return gemm_f16(A_dev, K, W_dev, K, e, M, N, K, static_cast<cudaStream_t>(stream));
-}
-
-int sbk_gemm_f16_resid_test(const void* A_dev, const void* W_dev, const float* bias_dev, float* x_dev, float alpha, int M,
-                            int N, int K, void* stream) {
-    GemmEpilogue e;
-    e.mode = EPI_RESID;
-    e.bias = bias_dev;
-    e.out = x_dev;
-    e.resid = x_dev;
-    e.alpha = alpha;
-    e.ldo = N;
-    return gemm_f16(A_dev, K, W_dev, K, e, M, N, K, static_cast<cudaStream_t>(stream));
-}
-
-int sbk_gemm_epilogue_test(const void* A_dev, const void* W_dev, const float* bias_dev, void* out_dev, int ldo, int mode,
-                           int act, float alpha, const float* resid_dev, const int* row_lens_dev, int T,
-                           const float* rope_cos_dev, const float* rope_sin_dev, int head_dim, int kv_heads,
-                           long long kv_part_stride, long long kv_layer_stride, int M, int N, int K, void* stream) {
-    GemmEpilogue e;
-    e.mode = mode; e.act = act; e.bias = bias_dev; e.out = out_dev; e.ldo = ldo; e.alpha = alpha;
-    e.resid = resid_dev; e.row_lens = row_lens_dev; e.T = T;
-    e.rope_cos = rope_cos_dev; e.rope_sin = rope_sin_dev; e.head_dim = head_dim;
-    e.kv_heads = kv_heads; e.kv_part_stride = (size_t)kv_part_stride; e.kv_layer_stride = (size_t)kv_layer_stride;
-    if (mode < EPI_F16 || mode > EPI_ROPE) { set_error("sbk_gemm_epilogue_test: mode %d", mode); return SBK_ERR_ARG; }
-    return gemm_f16(A_dev, K, W_dev, K, e, M, N, K, static_cast<cudaStream_t>(stream));
-}
-
-int sbk_ctc_prefix_test(const float* logits_dev, const int* enc_len_dev, int B, int T, int V, int beam, int blank, int bos,
-                        int eos, float weight, int accumulate, const int* hist_tok_dev, const int* hist_pred_dev, int n_steps,
-                        float* scores_dev, int* group_width, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(logits_dev && enc_len_dev && hist_tok_dev && hist_pred_dev && scores_dev, "ctc_prefix_test: null pointer");
-    SBK_REQUIRE(B >= 1 && T >= 1 && V >= 1 && beam >= 1 && n_steps >= 1, "ctc_prefix_test: bad sizes");
-    SBK_REQUIRE(blank >= 0 && blank < V && bos >= 0 && bos < V && eos >= 0 && eos < V, "ctc_prefix_test: bad token ids");
-    const int rows = B * beam;
-    // the kernels index frames, parents and token columns with these: check them on the host first
-    std::vector<int> len(B), tok((size_t)n_steps * rows), pred((size_t)n_steps * rows);
-    SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), enc_len_dev, B * 4, cudaMemcpyDeviceToHost, st));
-    SBK_CUDA_CHECK(cudaMemcpyAsync(tok.data(), hist_tok_dev, tok.size() * 4, cudaMemcpyDeviceToHost, st));
-    SBK_CUDA_CHECK(cudaMemcpyAsync(pred.data(), hist_pred_dev, pred.size() * 4, cudaMemcpyDeviceToHost, st));
-    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int v : len) SBK_REQUIRE(v >= 0 && v <= T, "ctc_prefix_test: enc_len %d outside [0, %d]", v, T);
-    for (size_t i = 0; i < tok.size(); ++i)
-        SBK_REQUIRE(tok[i] >= 0 && tok[i] < V && pred[i] >= 0 && pred[i] < rows, "ctc_prefix_test: history entry %zu out of range", i);
-    struct DevBufs {   // freed on every return path
-        std::vector<void*> p;
-        ~DevBufs() { for (void* q : p) cudaFree(q); }
-    } bufs;
-    auto alloc = [&](size_t n4, void** out) -> int {   // n4 4-byte elements
-        if (cudaMalloc(out, n4 * 4) != cudaSuccess) { set_error("ctc_prefix_test: cudaMalloc(%zu) failed", n4 * 4); return SBK_ERR_NOMEM; }
-        bufs.p.push_back(*out);
-        return SBK_OK;
-    };
-    const size_t M = (size_t)B * T;
-    float *x, *xlin, *xb, *rsum, *rb, *psi, *tab, *tabM;
-    int* steps;
-    RC(alloc(M * V, (void**)&x)); RC(alloc(M * V, (void**)&xlin)); RC(alloc(M, (void**)&xb));
-    RC(alloc((size_t)2 * rows * T, (void**)&rsum)); RC(alloc((size_t)2 * rows * T, (void**)&rb)); RC(alloc((size_t)2 * rows, (void**)&psi));
-    RC(alloc((size_t)2 * rows * (T + 4), (void**)&tab)); RC(alloc((size_t)2 * rows, (void**)&tabM));
-    RC(alloc((size_t)n_steps * rows, (void**)&steps));
-    std::vector<int> step_val((size_t)n_steps * rows);   // the beam search's per-row step counters, one row of them per step
-    for (size_t i = 0; i < step_val.size(); ++i) step_val[i] = static_cast<int>(i / rows);
-    SBK_CUDA_CHECK(cudaMemcpyAsync(steps, step_val.data(), step_val.size() * 4, cudaMemcpyHostToDevice, st));
-    SBK_CUDA_CHECK(cudaMemcpyAsync(x, logits_dev, M * V * 4, cudaMemcpyDeviceToDevice, st));
-    RC(ctc_prefix_reset(x, xlin, xb, enc_len_dev, B, T, V, blank, beam, rsum, rb, psi, tab, tabM, st));
-    CtcStep cs{};
-    cs.x = x; cs.xlin = xlin; cs.xb = xb; cs.enc_len = enc_len_dev; cs.hist_tok = hist_tok_dev; cs.hist_pred = hist_pred_dev;
-    cs.n_bh = rows; cs.rsum_base = rsum; cs.rb_base = rb; cs.psi_base = psi; cs.tab = tab; cs.tabM = tabM;
-    cs.bos = bos; cs.T = T; cs.V = V; cs.beam = beam; cs.blank = blank; cs.eos = eos; cs.weight = weight; cs.accumulate = accumulate ? 1 : 0;
-    for (int s = 0; s < n_steps; ++s) {   // run_beam's order: update of the previous survivors, then the score
-        cs.step_ptr = steps + (size_t)s * rows;
-        cs.out = scores_dev + (size_t)s * rows * V;
-        RC(ctc_prefix_update(cs, st));
-        RC(ctc_prefix_score(cs, st));
-    }
-    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    if (group_width) *group_width = ctc_prefix_group_width(beam, T);
-    return SBK_OK;
-}
-
-int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev, const float* ln_b_dev, const float* taps_dev,
-                  const float* bias_dev, int K, void* out_dev, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(u_dev && ln_g_dev && ln_b_dev && taps_dev && bias_dev && out_dev, "csgu_test: null pointer");
-    SBK_REQUIRE(B >= 1 && T >= 1 && C >= 16 && C % 16 == 0 && K >= 1 && (K & 1) && K <= CSGU_TAP_ROWS,
-                "csgu_test: bad sizes B=%d T=%d C=%d K=%d", B, T, C, K);
-    const int C2 = C / 2;
-    std::vector<float> src((size_t)C2 * K), wt((size_t)CSGU_TAP_ROWS * C2);
-    SBK_CUDA_CHECK(cudaMemcpyAsync(src.data(), taps_dev, src.size() * 4, cudaMemcpyDeviceToHost, st));
-    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    csgu_repack_taps(src.data(), C2, K, wt.data());
-    float* taps = nullptr;
-    float2* stats = nullptr;
-    if (cudaMalloc(&taps, wt.size() * 4) != cudaSuccess || cudaMalloc(&stats, (size_t)B * T * 8) != cudaSuccess) {
-        cudaFree(taps);
-        set_error("csgu_test: cudaMalloc failed");
-        return SBK_ERR_NOMEM;
-    }
-    int rc = cudaMemcpyAsync(taps, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess ? SBK_OK : SBK_ERR_CUDA;
-    if (rc == SBK_OK)
-        rc = csgu_forward(static_cast<const __half*>(u_dev), B, T, C, ln_g_dev, ln_b_dev, 1e-5f, taps, bias_dev, K, stats,
-                          static_cast<__half*>(out_dev), st);
-    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("csgu_test: device error"); rc = SBK_ERR_CUDA; }
-    cudaFree(taps);
-    cudaFree(stats);
-    return rc;
-}
-
-int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int head_dim, const int* lens_dev, int relpos,
-                               const float* pos_u_dev, const float* pos_v_dev, const void* P_dev, float scale, int chunk,
-                               int left_chunks, void* out_dev, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(qkv_dev && out_dev && (!relpos || (pos_u_dev && pos_v_dev && P_dev)), "encoder_attention_test: null pointer");
-    SBK_REQUIRE(B >= 1 && T >= 1 && H >= 1 && head_dim >= 1, "encoder_attention_test: bad sizes B=%d T=%d H=%d head_dim=%d", B,
-                T, H, head_dim);
-    const int d = H * head_dim;
-    int rc = encoder_attention(static_cast<const __half*>(qkv_dev), 3 * d, B, T, H, head_dim, lens_dev, relpos != 0, pos_u_dev,
-                               pos_v_dev, static_cast<const __half*>(P_dev), d, scale, static_cast<__half*>(out_dev), d, st,
-                               chunk, left_chunks);
-    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("encoder_attention_test: device error"); rc = SBK_ERR_CUDA; }
-    return rc;
-}
-
 int sbk_step_proj_test(int backend, int epilogue, const void* A_dev, int lda, const float* X_dev, const float* ln_g_dev,
                        const float* ln_b_dev, const void* W_dev, const float* bias_dev, int rows, int N, int K, void* out_dev,
                        int ldo, void* kcache_dev, void* vcache_dev, int S_max, int step, void* stream) {
@@ -1280,13 +1190,8 @@ int sbk_step_proj_test(int backend, int epilogue, const void* A_dev, int lda, co
                 "step_proj_test: the wgmma back end needs ldo %% 8 == 0 and a 16-byte aligned out");
     int* steps = nullptr;
     __half* h16 = nullptr;
-    auto layout = [&](Carver& take) { take(steps, (size_t)rows * 4); take(h16, X_dev ? (size_t)rows * K * 2 : 0); };
-    Carver measure;
-    layout(measure);
-    uint8_t* base = nullptr;
-    if (cudaMalloc(&base, measure.used) != cudaSuccess) { set_error("step_proj_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
-    Carver carve{base};
-    layout(carve);
+    TestScratch scr;
+    RC(scr.carve("step_proj_test", [&](Carver& take) { take(steps, (size_t)rows * 4); take(h16, X_dev ? (size_t)rows * K * 2 : 0); }));
     // one counter per row, all equal, as b.step holds them: the weight-streaming kernel reads row 0's, the wgmma epilogue
     // each row's
     const std::vector<int> step_val(rows, step);
@@ -1303,144 +1208,7 @@ int sbk_step_proj_test(int backend, int epilogue, const void* A_dev, int lda, co
         }
         rc = X_dev ? norm_project(g, true, p, X_dev, ln_g_dev, ln_b_dev, h16, rows, st) : project(g, p, rows, st);
     }
-    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("step_proj_test: device error"); rc = SBK_ERR_CUDA; }
-    cudaFree(base);
-    return rc;
-}
-
-int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, const void* vbase_dev, long long row_stride,
-                           int key_stride, int head_stride, int rows_per_block, int rows, int H, int dh, int max_keys, int step,
-                           const int* enc_len_dev, const int* lineage_dev, const int* tok_cache_dev, int lin_stride,
-                           int pad_tok, void* out_dev, int ldo, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(q_dev && kbase_dev && vbase_dev && out_dev, "dec_attention_test: null pointer");
-    SBK_REQUIRE(rows >= 1 && H >= 1 && dh >= 1 && max_keys >= 1 && rows_per_block >= 1 && rows % rows_per_block == 0 &&
-                    ldq >= H * dh && ldo >= H * dh && key_stride >= 1 && row_stride >= 0 && head_stride >= 0,
-                "dec_attention_test: bad sizes rows=%d rows_per_block=%d H=%d dh=%d max_keys=%d", rows, rows_per_block, H, dh,
-                max_keys);
-    if (dh == 64 || dh == 128) {  // 16-byte loads of q, K and V
-        const uintptr_t al = reinterpret_cast<uintptr_t>(q_dev) | reinterpret_cast<uintptr_t>(kbase_dev) |
-                             reinterpret_cast<uintptr_t>(vbase_dev);
-        SBK_REQUIRE((al & 15) == 0 && ldq % 8 == 0 && key_stride % 8 == 0 && row_stride % 8 == 0 && head_stride % 8 == 0,
-                    "dec_attention_test: head_dim %d needs 16-byte aligned q / key rows", dh);
-    }
-    const bool self = step >= 0;
-    SBK_REQUIRE(self || (!lineage_dev && !tok_cache_dev), "dec_attention_test: a lineage or token mask needs self-attention");
-    SBK_REQUIRE(!lineage_dev || rows_per_block == 1, "dec_attention_test: a lineage table needs one cache row per query row");
-    SBK_REQUIRE(!self || step < max_keys, "dec_attention_test: step %d >= max_keys %d", step, max_keys);
-    SBK_REQUIRE(!(lineage_dev || tok_cache_dev) || step < lin_stride, "dec_attention_test: step %d >= lin_stride %d", step,
-                lin_stride);
-    // the kernels index rows and frames with these: check them on the host first
-    if (lineage_dev) {
-        std::vector<int> lin((size_t)2 * rows * lin_stride);
-        SBK_CUDA_CHECK(cudaMemcpyAsync(lin.data(), lineage_dev, lin.size() * 4, cudaMemcpyDeviceToHost, st));
-        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-        for (size_t i = 0; i < lin.size(); ++i)
-            SBK_REQUIRE(lin[i] >= 0 && lin[i] < rows, "dec_attention_test: lineage entry %zu = %d outside [0, %d)", i, lin[i], rows);
-    }
-    if (!self && enc_len_dev) {
-        std::vector<int> len(rows / rows_per_block);
-        SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), enc_len_dev, len.size() * 4, cudaMemcpyDeviceToHost, st));
-        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-        for (int v : len) SBK_REQUIRE(v >= 0 && v <= max_keys, "dec_attention_test: enc_len %d outside [0, %d]", v, max_keys);
-    }
-    int* step_dev = nullptr;
-    if (self) {
-        if (cudaMalloc(&step_dev, 4) != cudaSuccess) { set_error("dec_attention_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
-        if (cudaMemcpyAsync(step_dev, &step, 4, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-            cudaFree(step_dev);
-            set_error("dec_attention_test: copy failed");
-            return SBK_ERR_CUDA;
-        }
-    }
-    DecAttnArgs t{};
-    t.q = static_cast<const __half*>(q_dev); t.ldq = ldq;
-    t.kbase = static_cast<const __half*>(kbase_dev); t.vbase = static_cast<const __half*>(vbase_dev);
-    t.row_stride = (size_t)row_stride; t.key_stride = key_stride; t.head_stride = head_stride; t.rows_per_block = rows_per_block;
-    t.n_keys_ptr = step_dev; t.enc_len = self ? nullptr : enc_len_dev; t.H = H; t.dh = dh;
-    t.out = static_cast<__half*>(out_dev); t.ldo = ldo;
-    t.lineage = lineage_dev; t.tok_cache = tok_cache_dev; t.lin_stride = lin_stride; t.pad_tok = pad_tok;
-    int rc = dec_attention(t, rows, max_keys, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("dec_attention_test: device error"); rc = SBK_ERR_CUDA; }
-    cudaFree(step_dev);
-    return rc;
-}
-
-int sbk_stream_qkv_test(const float* qkv_dev, int B, int n, int H, int head_dim, const float* inv_freq_dev, long long pos0,
-                        float q_scale, void* q_out_dev, void* kv_out_dev, int cap, int slot0, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(qkv_dev && q_out_dev && kv_out_dev, "stream_qkv_test: null pointer");
-    SBK_REQUIRE(B >= 1 && H >= 1 && head_dim >= 2 && pos0 >= 0, "stream_qkv_test: bad sizes");
-    int rc = stream_qkv(qkv_dev, B, n, H, head_dim, inv_freq_dev, pos0, q_scale, static_cast<__half*>(q_out_dev),
-                        static_cast<__half*>(kv_out_dev), cap, slot0, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("stream_qkv_test: device error"); rc = SBK_ERR_CUDA; }
-    return rc;
-}
-
-int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
-                    const float* ln_g_dev, const float* ln_b_dev, int chunk, void* out_dev, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(x_dev && taps_dev && bias_dev && ln_g_dev && ln_b_dev && out_dev, "dwconv_test: null pointer");
-    SBK_REQUIRE(B >= 1 && T >= 1 && D >= 1 && K >= 1 && chunk >= 0, "dwconv_test: bad sizes B=%d T=%d D=%d K=%d chunk=%d", B, T,
-                D, K, chunk);
-    std::vector<float> src((size_t)D * K), wt((size_t)K * D);
-    SBK_CUDA_CHECK(cudaMemcpyAsync(src.data(), taps_dev, src.size() * 4, cudaMemcpyDeviceToHost, st));
-    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    dwconv_repack_taps(src.data(), D, K, wt.data());
-    float* taps = nullptr;
-    if (cudaMalloc(&taps, wt.size() * 4) != cudaSuccess) { set_error("dwconv_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
-    int rc = cudaMemcpyAsync(taps, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess ? SBK_OK : SBK_ERR_CUDA;
-    if (rc == SBK_OK)
-        rc = dwconv_ln_swish(x_dev, B, T, D, K, taps, bias_dev, ln_g_dev, ln_b_dev, 1e-5f, static_cast<__half*>(out_dev), st, chunk);
-    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("dwconv_test: device error"); rc = SBK_ERR_CUDA; }
-    cudaFree(taps);
-    return rc;
-}
-
-int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int d, int nhead, int k, const float* w1_fc1_w_dev,
-                      const float* w1_fc1_b_dev, const float* w1_fc2_w_dev, const float* w1_fc2_b_dev, const float* w2_fc1_w_dev,
-                      const float* w2_fc1_b_dev, const float* w2_fc2_w_dev, const float* w2_fc2_b_dev, const float* ln_g_dev,
-                      const float* ln_b_dev, float* out_dev, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(x_dev && w1_fc1_w_dev && w1_fc1_b_dev && w1_fc2_w_dev && w1_fc2_b_dev && w2_fc1_w_dev && w2_fc1_b_dev &&
-                    w2_fc2_w_dev && w2_fc2_b_dev && ln_g_dev && ln_b_dev && out_dev, "hypermix_test: null pointer");
-    SBK_REQUIRE(B >= 1 && T >= 1 && nhead >= 1 && d % nhead == 0 && k >= 1, "hypermix_test: bad sizes B=%d T=%d d=%d nhead=%d k=%d",
-                B, T, d, nhead, k);
-    const int e = d / nhead;
-    const size_t n1 = (size_t)nhead * e * e, n2 = (size_t)nhead * k * e;
-    const std::vector<float> pe = sine_table(HM_PE_ROWS, d);
-    const size_t part_n = hypermix_part_floats(B, T, d, k);
-    __half *w16 = nullptr, *G = nullptr;
-    float *pe_dev = nullptr, *part = nullptr, *gscale = nullptr;
-    auto layout = [&](Carver& take) {
-        take(w16, 2 * (n1 + n2) * 2); take(pe_dev, pe.size() * 4); take(part, part_n * 4); take(G, (size_t)B * d * k * 2);
-        take(gscale, (size_t)B * nhead * 4);
-    };
-    Carver measure;
-    layout(measure);
-    uint8_t* base = nullptr;
-    if (cudaMalloc(&base, measure.used) != cudaSuccess) { set_error("hypermix_test: cudaMalloc failed"); return SBK_ERR_NOMEM; }
-    Carver carve{base};
-    layout(carve);
-    HyperMixWeights w;
-    w.fc1w[0] = w16; w.fc2w[0] = w16 + n1; w.fc1w[1] = w16 + n1 + n2; w.fc2w[1] = w16 + 2 * n1 + n2;
-    w.fc1b[0] = w1_fc1_b_dev; w.fc2b[0] = w1_fc2_b_dev; w.fc1b[1] = w2_fc1_b_dev; w.fc2b[1] = w2_fc2_b_dev;
-    w.ln_g = ln_g_dev; w.ln_b = ln_b_dev;
-    int rc = cast_f32_f16(w1_fc1_w_dev, const_cast<__half*>(w.fc1w[0]), n1, st);
-    if (rc == SBK_OK) rc = cast_f32_f16(w1_fc2_w_dev, const_cast<__half*>(w.fc2w[0]), n2, st);
-    if (rc == SBK_OK) rc = cast_f32_f16(w2_fc1_w_dev, const_cast<__half*>(w.fc1w[1]), n1, st);
-    if (rc == SBK_OK) rc = cast_f32_f16(w2_fc2_w_dev, const_cast<__half*>(w.fc2w[1]), n2, st);
-    if (rc == SBK_OK && (cudaMemcpyAsync(pe_dev, pe.data(), pe.size() * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-                         cudaMemsetAsync(out_dev, 0, (size_t)B * T * d * 4, st) != cudaSuccess)) {
-        set_error("hypermix_test: copy failed");
-        rc = SBK_ERR_CUDA;
-    }
-    if (rc == SBK_OK)
-        rc = hypermix_forward(static_cast<const __half*>(x_dev), B, T, d, nhead, k, lens_dev,
-                              pe_dev, w, part, G, gscale, out_dev, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess && rc == SBK_OK) { set_error("hypermix_test: device error"); rc = SBK_ERR_CUDA; }
-    cudaFree(base);
-    return rc;
+    return finish_test("step_proj_test", rc, st);
 }
 
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out) {
@@ -1489,8 +1257,7 @@ int sbk_asr_cnn_forward(sbk_asr* mm, const float* feats_dev, int B, int T0, floa
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     const sbk_asr_config& c = m->wt->cfg;
     SBK_REQUIRE(m->wt->has_cnn, "cnn_forward: this handle was created without CNN weights");
-    const int L = (T0 - 1) * c.hop;
-    RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
+    RC(ensure_workspace(m, B, (T0 - 1) * c.hop, B, 1));
     return run_cnn(m, feats_dev, B, T0, out_dev, static_cast<cudaStream_t>(stream));
 }
 
@@ -1500,8 +1267,7 @@ int sbk_asr_encode_feats(sbk_asr* mm, const float* feats_dev, const float* rel_l
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const sbk_asr_config& c = m->wt->cfg;
-    const int L = (T0 - 1) * c.hop;
-    RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
+    RC(ensure_workspace(m, B, (T0 - 1) * c.hop, B, 1));
     const int T1 = (T0 - 1) / 2 + 1, T = (T1 - 1) / 2 + 1;
     const int* enc_len = nullptr;
     if (rel_len_dev) {
@@ -1516,8 +1282,7 @@ int sbk_asr_encode_from_cnn(sbk_asr* mm, const float* src_dev, const float* rel_
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const sbk_asr_config& c = m->wt->cfg;
-    const int L = ((T - 1) * 4) * c.hop;  // any L whose frame count maps to >= T encoder frames
-    RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
+    RC(ensure_workspace(m, B, enc_samples(c, T), B, 1));
     RC(cast_f32_f16(src_dev, m->b.a_in, (size_t)B * T * c.input_size, st));
     const int* enc_len = nullptr;
     if (rel_len_dev) {
@@ -1621,8 +1386,7 @@ int sbk_asr_stream_encode_chunk(sbk_asr* mm, sbk_asr_stream* ss, const float* cn
         s->kv.cap = stream_kv_bytes(c, s->B, ncap);
         s->cap = ncap;
     }
-    const int L = ((n - 1) * 4) * c.hop;  // a sample count whose frame count maps to n encoder frames
-    RC(ensure_workspace(m, s->B, L, std::max(s->B, m->ws_rows), std::max(1, m->ws_steps)));
+    RC(ensure_workspace(m, s->B, enc_samples(c, n), s->B, 1));
     RC(cast_f32_f16(cnn_out_dev, m->b.a_in, (size_t)s->B * n * c.input_size, st));
     RC(run_encoder(m, nullptr, s->B, n, nullptr, nullptr, enc_out_dev, st, s));
     s->total += n;
@@ -1703,6 +1467,18 @@ static int group_encode_batches(const sbk_asr_config& c, int G, int B, int L) {
     return ceil_div(G, ceil_div(G, E));
 }
 
+// The argument checks of the group entries `who`: G batches of B utterances of L samples, every batch's wav and lengths
+// given (and its output ids, when `pred` is given).
+static int check_group_call(const AsrModel* m, const char* who, int G, const float* const* wav, const float* const* rel,
+                            int* const* pred, int B, int L) {
+    SBK_REQUIRE(G >= 1 && G <= 16, "%s: G=%d not in [1, 16]", who, G);
+    SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc && m->wt->has_dec, "%s: handle lacks model parts", who);
+    SBK_REQUIRE(m->wt->glob_mean != nullptr, "%s: model has no normalize.glob_mean/std weights", who);
+    for (int g = 0; g < G; ++g) SBK_REQUIRE(wav[g] && rel[g] && (!pred || pred[g]), "%s: null batch pointer", who);
+    SBK_REQUIRE(B >= 1 && L >= 1, "%s: empty batch (B=%d, L=%d)", who, B, L);
+    return SBK_OK;
+}
+
 // G independent batches of B utterances: Fbank and the lengths run per batch (each batch is its own waveform pointer), the
 // CNN and encoder once per chunk of group_encode_batches() consecutive batches over all of the chunk's utterances, then ONE
 // greedy loop decodes all G*B hypotheses together.  Every encoder kernel works per row or per utterance, so an utterance's
@@ -1734,16 +1510,9 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
     static const bool prio = getenv("SBK_DEC_PRIORITY") == nullptr || atoi(getenv("SBK_DEC_PRIORITY")) != 0;
     cudaStream_t ds = st;
     if (prio) {
-        if (!m->dec_stream) {
-            int lo = 0, hi = 0;
-            SBK_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));  // numerically lowest = highest priority
-            SBK_CUDA_CHECK(cudaStreamCreateWithPriority(&m->dec_stream, cudaStreamNonBlocking, hi));
-            SBK_CUDA_CHECK(cudaEventCreateWithFlags(&m->ev_dfork, cudaEventDisableTiming));
-            SBK_CUDA_CHECK(cudaEventCreateWithFlags(&m->ev_djoin, cudaEventDisableTiming));
-        }
-        ds = m->dec_stream;
-        SBK_CUDA_CHECK(cudaEventRecord(m->ev_dfork, st));
-        SBK_CUDA_CHECK(cudaStreamWaitEvent(ds, m->ev_dfork, 0));
+        RC(m->dec_stream.ensure(true));
+        RC(m->dec_stream.fork(st));
+        ds = m->dec_stream.s;
     }
     int done = 0;
     RC(run_greedy(m, G * B, T, max_steps, bos, eos, nullptr, &done, ds, in_capture));
@@ -1752,10 +1521,7 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
         RC(copy_steps(m, pred_dev ? pred_dev[g] : nullptr, max_steps, pred, done, B, cudaMemcpyDeviceToDevice, ds));
         RC(copy_steps(m, pred_host ? pred_host[g] : nullptr, max_steps, pred, done, B, cudaMemcpyDeviceToHost, ds));
     }
-    if (prio) {
-        SBK_CUDA_CHECK(cudaEventRecord(m->ev_djoin, ds));
-        SBK_CUDA_CHECK(cudaStreamWaitEvent(st, m->ev_djoin, 0));
-    }
+    if (prio) RC(m->dec_stream.join(st));
     if (steps_done) *steps_done = done;
     return SBK_OK;
 }
@@ -1766,8 +1532,8 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
 static int transcribe_group_host_enqueue(AsrModel* m, int G, const float* const* wav_host, const float* const* rel_host, int B,
                                          int L, int max_steps, int bos, int eos, int* const* pred_host, int* const* pred_dev,
                                          int* steps_done, cudaStream_t st, bool in_capture) {
-    SBK_CUDA_CHECK(cudaEventRecord(m->ev_fork, st));
-    SBK_CUDA_CHECK(cudaStreamWaitEvent(m->copy_stream, m->ev_fork, 0));  // the previous call no longer reads the staging buffers
+    RC(m->copy_stream.fork(st));  // the previous call no longer reads the staging buffers
+    const cudaStream_t cs = m->copy_stream.s;
     const float* wav_dev[16];
     const float* rel_dev[16];
     float* gwav = static_cast<float*>(m->gwav.base);
@@ -1775,9 +1541,9 @@ static int transcribe_group_host_enqueue(AsrModel* m, int G, const float* const*
     for (int g = 0; g < G; ++g) {
         float* w = gwav + (size_t)g * B * L;
         float* r = grel + (size_t)g * B;
-        SBK_CUDA_CHECK(cudaMemcpyAsync(w, wav_host[g], (size_t)B * L * 4, cudaMemcpyHostToDevice, m->copy_stream));
-        SBK_CUDA_CHECK(cudaMemcpyAsync(r, rel_host[g], (size_t)B * 4, cudaMemcpyHostToDevice, m->copy_stream));
-        SBK_CUDA_CHECK(cudaEventRecord(m->ev_ready[g], m->copy_stream));
+        SBK_CUDA_CHECK(cudaMemcpyAsync(w, wav_host[g], (size_t)B * L * 4, cudaMemcpyHostToDevice, cs));
+        SBK_CUDA_CHECK(cudaMemcpyAsync(r, rel_host[g], (size_t)B * 4, cudaMemcpyHostToDevice, cs));
+        SBK_CUDA_CHECK(cudaEventRecord(m->ev_ready[g], cs));
         wav_dev[g] = w; rel_dev[g] = r;
     }
     return transcribe_group_enqueue(m, G, wav_dev, rel_dev, B, L, max_steps, bos, eos, pred_dev, steps_done, st, in_capture,
@@ -1788,27 +1554,17 @@ int sbk_asr_transcribe_greedy_group_dev(sbk_asr* mm, int G, const float* const* 
                                         int B, int L, int max_steps, int bos, int eos, int* const* pred_dev, int* steps_done,
                                         void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(G >= 1 && G <= 16, "transcribe_group: G=%d not in [1, 16]", G);
-    SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc && m->wt->has_dec, "transcribe_group: handle lacks model parts");
-    SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe_group: model has no normalize.glob_mean/std weights");
-    for (int g = 0; g < G; ++g) SBK_REQUIRE(wav_dev[g] && rel_len_dev[g], "transcribe_group: null batch pointer");
-    SBK_REQUIRE(B >= 1 && L >= 1, "transcribe_group: empty batch (B=%d, L=%d)", B, L);
-    RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps),
-                        group_encode_batches(m->wt->cfg, G, B, L) * B));
+    RC(check_group_call(m, "transcribe_group", G, wav_dev, rel_len_dev, nullptr, B, L));
+    RC(ensure_workspace(m, B, L, G * B, max_steps, group_encode_batches(m->wt->cfg, G, B, L) * B));
     const bool whole_graph = m->poll_every == 0 && getenv("SBK_NO_GRAPH") == nullptr && max_steps > 0;
-    if (!whole_graph) return transcribe_group_enqueue(m, G, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, pred_dev, steps_done, st, false);
     struct GroupKey { const void *wav[16], *rel[16], *pred[16]; int G, B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));
     key.G = G; key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
-    for (int g = 0; g < G; ++g) { key.wav[g] = wav_dev[g]; key.rel[g] = rel_len_dev[g]; key.pred[g] = pred_dev[g]; }
-    RC(m->group_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
-        int done = 0;
-        return transcribe_group_enqueue(m, G, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, pred_dev, &done, cs, true);
-    }));
-    RC(m->group_graph.launch(st));
-    if (steps_done) *steps_done = max_steps;
-    return SBK_OK;
+    for (int g = 0; g < G; ++g) { key.wav[g] = wav_dev[g]; key.rel[g] = rel_len_dev[g]; key.pred[g] = pred_dev ? pred_dev[g] : nullptr; }
+    return replay_or_enqueue(m, m->group_graph, whole_graph, key, max_steps, steps_done, static_cast<cudaStream_t>(stream),
+                             [&](cudaStream_t s, int* done, bool in_capture) {
+        return transcribe_group_enqueue(m, G, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, pred_dev, done, s, in_capture);
+    });
 }
 
 // Same pipeline from HOST buffers (pinned): the call EncoderDecoderASR.transcribe_batch makes, for G batches at once.
@@ -1818,25 +1574,14 @@ int sbk_asr_transcribe_greedy_group_host_async(sbk_asr* mm, int G, const float* 
                                                const float* const* rel_len_host, int B, int L, int max_steps, int bos, int eos,
                                                int* const* pred_host, int* const* pred_dev, int* steps_done, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    SBK_REQUIRE(G >= 1 && G <= 16, "transcribe_group_host: G=%d not in [1, 16]", G);
-    SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc && m->wt->has_dec, "transcribe_group_host: handle lacks model parts");
-    SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe_group_host: model has no normalize.glob_mean/std weights");
     SBK_REQUIRE(wav_host && rel_len_host && pred_host, "transcribe_group_host: null argument");
-    for (int g = 0; g < G; ++g) SBK_REQUIRE(wav_host[g] && rel_len_host[g] && pred_host[g], "transcribe_group_host: null batch pointer");
-    SBK_REQUIRE(B >= 1 && L >= 1, "transcribe_group_host: empty batch (B=%d, L=%d)", B, L);
-    RC(ensure_workspace(m, B, L, std::max(G * B, m->ws_rows), std::max(max_steps, m->ws_steps),
-                        group_encode_batches(m->wt->cfg, G, B, L) * B));
+    RC(check_group_call(m, "transcribe_group_host", G, wav_host, rel_len_host, pred_host, B, L));
+    RC(ensure_workspace(m, B, L, G * B, max_steps, group_encode_batches(m->wt->cfg, G, B, L) * B));
     RC(grow_buffer(m, m->gwav, (size_t)G * B * L * 4 + (size_t)G * B * 4 + 256, "transcribe_group_host"));
-    if (!m->copy_stream) {
-        SBK_CUDA_CHECK(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
-        SBK_CUDA_CHECK(cudaEventCreateWithFlags(&m->ev_fork, cudaEventDisableTiming));
-        for (auto& e : m->ev_ready) SBK_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
+    RC(m->copy_stream.ensure());
+    for (auto& e : m->ev_ready)
+        if (!e) SBK_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     const bool whole_graph = m->poll_every == 0 && getenv("SBK_NO_GRAPH") == nullptr && max_steps > 0;
-    if (!whole_graph)
-        return transcribe_group_host_enqueue(m, G, wav_host, rel_len_host, B, L, max_steps, bos, eos, pred_host, pred_dev,
-                                             steps_done, st, false);
     struct HostGroupKey { const void *wav[16], *rel[16], *pred[16], *pred_dev[16]; int G, B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));
     key.G = G; key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
@@ -1844,43 +1589,33 @@ int sbk_asr_transcribe_greedy_group_host_async(sbk_asr* mm, int G, const float* 
         key.wav[g] = wav_host[g]; key.rel[g] = rel_len_host[g]; key.pred[g] = pred_host[g];
         key.pred_dev[g] = pred_dev ? pred_dev[g] : nullptr;
     }
-    RC(m->hgroup_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
-        int done = 0;
-        return transcribe_group_host_enqueue(m, G, wav_host, rel_len_host, B, L, max_steps, bos, eos, pred_host, pred_dev, &done,
-                                             cs, true);
-    }));
-    RC(m->hgroup_graph.launch(st));
-    if (steps_done) *steps_done = max_steps;
-    return SBK_OK;
+    return replay_or_enqueue(m, m->hgroup_graph, whole_graph, key, max_steps, steps_done, static_cast<cudaStream_t>(stream),
+                             [&](cudaStream_t s, int* done, bool in_capture) {
+        return transcribe_group_host_enqueue(m, G, wav_host, rel_len_host, B, L, max_steps, bos, eos, pred_host, pred_dev, done, s,
+                                             in_capture);
+    });
 }
 
 int sbk_asr_transcribe_greedy_dev(sbk_asr* mm, const float* wav_dev, const float* rel_len_dev, int B, int L,
                                   int max_steps, int bos, int eos, float* enc_out_dev, int* pred_dev, float* score_dev,
                                   float* log_probs_dev, int* steps_done, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->has_enc, "transcribe: handle lacks fbank/CNN/encoder weights");
     SBK_REQUIRE(m->wt->glob_mean != nullptr, "transcribe: model has no normalize.glob_mean/std (global CMVN) weights");
-    RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(max_steps, m->ws_steps)));
+    RC(ensure_workspace(m, B, L, B, max_steps));
     // Fixed-length runs (poll interval 0) replay ONE CUDA graph of the whole pipeline (Fbank .. last decode step):
     // ~2.6k kernel nodes, a single host-side launch per batch.
     const bool whole_graph = m->poll_every == 0 && rel_len_dev != nullptr && log_probs_dev == nullptr &&
                              getenv("SBK_NO_GRAPH") == nullptr && (max_steps == 0 || m->wt->has_dec);
-    if (!whole_graph)
-        return transcribe_enqueue(m, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, enc_out_dev, pred_dev, score_dev,
-                                  log_probs_dev, steps_done, st, false);
     struct PipeKey { const void *wav, *rel, *enc, *pred, *score; int B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));  // the struct has tail padding and is compared bytewise
     key.wav = wav_dev; key.rel = rel_len_dev; key.enc = enc_out_dev; key.pred = pred_dev; key.score = score_dev;
     key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
-    RC(m->pipe_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
-        int done = 0;
-        return transcribe_enqueue(m, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, enc_out_dev, pred_dev, score_dev, nullptr,
-                                  &done, cs, true);
-    }));
-    RC(m->pipe_graph.launch(st));
-    if (steps_done) *steps_done = max_steps;
-    return SBK_OK;
+    return replay_or_enqueue(m, m->pipe_graph, whole_graph, key, max_steps, steps_done, static_cast<cudaStream_t>(stream),
+                             [&](cudaStream_t s, int* done, bool in_capture) {
+        return transcribe_enqueue(m, wav_dev, rel_len_dev, B, L, max_steps, bos, eos, enc_out_dev, pred_dev, score_dev,
+                                  log_probs_dev, done, s, in_capture);
+    });
 }
 
 // Greedy search from caller-provided encoder states (S2STransformerGreedySearcher.forward).
@@ -1889,12 +1624,9 @@ int sbk_asr_greedy_from_enc(sbk_asr* mm, const float* enc_dev, const float* rel_
                             void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->wt->cfg;
-    // workspace sized from T: pick L such that frames(L) -> T
-    const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
-    RC(ensure_workspace(m, std::max(B, m->wsB), L, std::max(B, m->ws_rows), std::max(max_steps, m->ws_steps)));
+    RC(ensure_workspace(m, B, enc_samples(m->wt->cfg, T), B, max_steps));
     AsrModel::Buf& b = m->b;
-    SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, (size_t)B * T * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
+    RC(stage_enc(m, enc_dev, B, T, st));
     RC(set_enc_len(b.enc_len, rel_len_dev, B, T, st));
     int done = 0;
     RC(run_greedy(m, B, T, max_steps, bos, eos, log_probs_dev, &done, st));
@@ -1912,14 +1644,10 @@ int sbk_asr_beam_from_enc(sbk_asr* mm, const float* enc_dev, const float* rel_le
                           float* hist_lp_dev, int* steps_done, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->wt->cfg;
     SBK_REQUIRE(params && params->beam_size >= 1, "beam: bad params");
-    const int rows = B * params->beam_size;
-    const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
-    RC(ensure_workspace(m, std::max(B, m->wsB), L, std::max(rows, m->ws_rows), std::max(params->max_steps, m->ws_steps)));
-    AsrModel::Buf& b = m->b;
-    SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, (size_t)B * T * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
-    RC(set_enc_len(b.enc_len, rel_len_dev, B, T, st));
+    RC(ensure_workspace(m, B, enc_samples(m->wt->cfg, T), B * params->beam_size, params->max_steps));
+    RC(stage_enc(m, enc_dev, B, T, st));
+    RC(set_enc_len(m->b.enc_len, rel_len_dev, B, T, st));
     int done = 0;
     RC(run_beam(m, B, T, *params, hist_tok_dev, hist_pred_dev, hist_score_dev, hist_lp_dev, &done, st));
     if (steps_done) *steps_done = done;
@@ -1933,7 +1661,7 @@ static int transcribe_greedy_host_impl(sbk_asr* mm, const float* wav_host, const
                                        void* stream, bool sync) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    RC(ensure_workspace(m, B, L, std::max(B, m->ws_rows), std::max(max_steps, m->ws_steps)));
+    RC(ensure_workspace(m, B, L, B, max_steps));
     AsrModel::Buf& b = m->b;
     SBK_CUDA_CHECK(cudaMemcpyAsync(b.wav, wav_host, (size_t)B * L * 4, cudaMemcpyHostToDevice, st));
     const float* rel_dev = nullptr;
@@ -1982,11 +1710,10 @@ int sbk_asr_ctc_head(sbk_asr* mm, const float* enc_dev, int B, int T, float* log
     const sbk_asr_config& c = m->wt->cfg;
     SBK_REQUIRE(m->wt->w_ctc != nullptr, "ctc_head: this handle was created without ctc_lin.w.* weights");
     SBK_REQUIRE(B >= 1 && T >= 1 && (log_probs_dev || argmax_dev), "ctc_head: bad arguments");
-    const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
-    RC(ensure_workspace(m, std::max(B, m->wsB), L, std::max(B, m->ws_rows), std::max(1, m->ws_steps)));
+    RC(ensure_workspace(m, B, enc_samples(c, T), B, 1));
     AsrModel::Buf& b = m->b;
     const size_t M = (size_t)B * T, V = c.vocab;
-    if (enc_dev) SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, M * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
+    if (enc_dev) RC(stage_enc(m, enc_dev, B, T, st));
     float* logits = log_probs_dev;
     if (!logits) {  // arg-max only: the logits live in the (lazily grown) CTC scratch buffer
         RC(grow_buffer(m, m->ctc, M * V * 4 + 256, "ctc_head"));
@@ -2006,12 +1733,10 @@ int sbk_asr_decode_teacher_forced(sbk_asr* mm, const int* tgt_dev, const float* 
                                   int T, float* out_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->wt->cfg;
     SBK_REQUIRE(tgt_dev && enc_dev && out_dev && n >= 1 && S >= 1 && T >= 1, "decode: bad arguments");
-    const int L = std::max(m->wsL, ((T - 1) * 4) * c.hop);
-    RC(ensure_workspace(m, std::max(n, m->wsB), L, std::max(n, m->ws_rows), std::max(S, m->ws_steps)));
+    RC(ensure_workspace(m, n, enc_samples(m->wt->cfg, T), n, S));
     AsrModel::Buf& b = m->b;
-    SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_out, enc_dev, (size_t)n * T * c.d_model * 4, cudaMemcpyDeviceToDevice, st));
+    RC(stage_enc(m, enc_dev, n, T, st));
     if (enc_len_dev)
         SBK_CUDA_CHECK(cudaMemcpyAsync(b.enc_len, enc_len_dev, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
     else
@@ -2029,7 +1754,7 @@ int sbk_asr_lm_rescore(sbk_asr* mm, const int* tokens_dev, const int* lens_dev, 
     SBK_REQUIRE(n >= 1 && L >= 2 && L <= m->wt->cfg.max_len && pad_index >= 0 && pad_index < m->wt->cfg.vocab && temperature > 0.0f,
                 "lm_rescore: bad arguments (n=%d L=%d pad=%d)", n, L, pad_index);
     SBK_REQUIRE(pad_index == 0, "lm_rescore: pad_index must be 0 (TransformerLM.make_masks pads with index 0)");
-    RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->wt->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
+    RC(ensure_workspace(m, 1, enc_samples(m->wt->cfg, 2), n, L));  // the LM reads no encoder states
     return run_lm_rescore(m, tokens_dev, lens_dev, n, L, temperature, pad_index, scores_dev, st);
 }
 
@@ -2052,7 +1777,7 @@ int sbk_asr_lm_step_logits(sbk_asr* mm, const int* tokens_dev, int n, int L, flo
     SBK_REQUIRE(m != nullptr && tokens_dev && logits_dev, "lm_step_logits: null argument");
     SBK_REQUIRE(m->wt->has_lm, "lm_step_logits: this handle was created without TransformerLM weights");
     SBK_REQUIRE(n >= 1 && L >= 1 && L <= m->wt->cfg.max_len, "lm_step_logits: bad shape n=%d L=%d (max_len %d)", n, L, m->wt->cfg.max_len);
-    RC(ensure_workspace(m, std::max(1, m->wsB), std::max(m->wsL, 4 * m->wt->cfg.hop), std::max(n, m->ws_rows), std::max(L, m->ws_steps)));
+    RC(ensure_workspace(m, 1, enc_samples(m->wt->cfg, 2), n, L));  // the LM reads no encoder states
     return run_lm_step_logits(m, tokens_dev, n, L, logits_dev, static_cast<cudaStream_t>(stream));
 }
 

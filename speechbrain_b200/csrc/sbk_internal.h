@@ -20,6 +20,28 @@ struct Carver {
     }
 };
 
+// ---- test_hooks.cu: what the kernel test hooks of the C ABI share
+// A hook's device scratch: laid out by one Carver function in a single cudaMalloc, freed when it goes out of scope.
+struct TestScratch {
+    uint8_t* base = nullptr;
+    TestScratch() = default;
+    TestScratch(const TestScratch&) = delete;
+    TestScratch& operator=(const TestScratch&) = delete;
+    ~TestScratch() { cudaFree(base); }
+    int reserve(const char* who, size_t bytes);  // no allocation for 0 bytes
+    template <class Layout>
+    int carve(const char* who, Layout&& layout) {
+        Carver measure;
+        layout(measure);
+        if (int rc = reserve(who, measure.used)) return rc;
+        Carver take{base};
+        layout(take);
+        return 0;
+    }
+};
+// A hook's last step: synchronises the stream; a device error becomes "<who>: device error" unless rc already holds one.
+int finish_test(const char* who, int rc, cudaStream_t stream);
+
 enum GemmEpiMode { EPI_F16 = 0, EPI_F32 = 1, EPI_RESID = 2, EPI_GLU = 3, EPI_ROPE = 4, EPI_QKV_CACHE = 5 };
 enum GemmAct { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU = 2, ACT_RELU = 3, ACT_SILU_FAST = 4 /* tanh.approx form; for EPI_GLU: fast gate sigmoid */ };
 
