@@ -18,7 +18,7 @@ typedef struct sbk_fbank sbk_fbank; /* opaque */
 typedef struct sbk_asr sbk_asr;     /* opaque */
 
 enum { SBK_ATT_ROPE = 0, SBK_ATT_RELPOS = 1, SBK_ATT_HYPERMIX = 2, SBK_ATT_REGULAR = 3 };
-enum { SBK_ACT_RELU = 0, SBK_ACT_GELU = 1 };
+enum { SBK_ACT_RELU = 0, SBK_ACT_GELU = 1, SBK_ACT_SILU = 2 };
 enum { SBK_ENC_CONFORMER = 0, SBK_ENC_BRANCHFORMER = 1, SBK_ENC_TRANSFORMER = 2 };
 enum { SBK_PART_FBANK = 1, SBK_PART_CNN = 2, SBK_PART_ENCODER = 4, SBK_PART_DECODER = 8, SBK_PART_ALL = 15, SBK_PART_LM = 16 };
 
@@ -39,7 +39,7 @@ typedef struct {
                                encoder only, head width d_model / nhead 32 or 64, hypernetwork width d_ffn / nhead a multiple
                                of 16 up to 256; inputs up to 3000 frames) | SBK_ATT_REGULAR (regularMHA: the Transformer
                                encoder only, head width 64 or 128) */
-    int decoder_activation; /* SBK_ACT_RELU | SBK_ACT_GELU (the `activation` ctor kwarg) */
+    int decoder_activation; /* SBK_ACT_RELU | SBK_ACT_GELU | SBK_ACT_SILU (the `activation` ctor kwarg) */
     int max_len;            /* positional tables (ctor kwarg max_length, default 2500) */
     int parts;              /* bitmask of SBK_PART_*: which sub-models the weight table carries */
     /* TransformerLM used as a shallow-fusion scorer (lobes/models/transformer/TransformerLM.py; weights "lm.*") */

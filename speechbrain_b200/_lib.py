@@ -44,7 +44,7 @@ class sbk_ctc_beam_params(ctypes.Structure):
 
 
 SBK_ATT_ROPE, SBK_ATT_RELPOS, SBK_ATT_HYPERMIX, SBK_ATT_REGULAR = 0, 1, 2, 3
-SBK_ACT_RELU, SBK_ACT_GELU = 0, 1
+SBK_ACT_RELU, SBK_ACT_GELU, SBK_ACT_SILU = 0, 1, 2
 SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER, SBK_ENC_TRANSFORMER = 0, 1, 2
 SBK_PARTS = {"fbank": 1, "cnn": 2, "encoder": 4, "decoder": 8, "lm": 16}
 

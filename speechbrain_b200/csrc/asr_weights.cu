@@ -398,15 +398,19 @@ static int check_config(const sbk_asr_config& c) {
     SBK_REQUIRE(tfm == (c.attention_type == SBK_ATT_REGULAR),
                 "asr_create: regularMHA is built for the Transformer encoder only, and the Transformer encoder with regularMHA only");
     SBK_REQUIRE(!tfm || dh == 64 || dh == 128, "asr_create: Transformer encoder head_dim=%d not built (128, 64)", dh);
-    SBK_REQUIRE(tfm || hypermix || dh == 64 || dh == 36 || dh == 32, "asr_create: encoder head_dim=%d not built (64, 36, 32)", dh);
+    SBK_REQUIRE(tfm || hypermix || dh == 64 || dh == 36 || dh == 32 ||
+                    (dh == 80 && c.encoder_module == SBK_ENC_CONFORMER && c.attention_type == SBK_ATT_RELPOS),
+                "asr_create: encoder head_dim=%d not built (64, 36, 32; 80 for the Conformer with RelPosMHAXL)", dh);
     SBK_REQUIRE(c.cnn_blocks == 0 || c.cnn_blocks == 2 || (c.cnn_blocks == 3 && c.cnn_c1 == 64 && c.cnn_c2 == 64),
                 "asr_create: cnn_blocks=%d with channels (%d, %d) not built (2, or 3 with 64 channels)", c.cnn_blocks, c.cnn_c1, c.cnn_c2);
     SBK_REQUIRE(!hypermix || (c.encoder_module == SBK_ENC_CONFORMER && (dh == 32 || dh == 64) && F % c.nhead == 0 &&
                               (F / c.nhead) % 16 == 0 && F / c.nhead <= 256),
                 "asr_create: hypermixing needs the Conformer encoder, a head width d_model / nhead of 32 or 64 and "
                 "k = d_ffn / nhead a multiple of 16 up to 256 (got %d, %d)", dh, c.nhead > 0 ? F / c.nhead : 0);
-    SBK_REQUIRE(!((c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0) || ((dh <= 64 || dh == 128) && dh % 4 == 0 && d % 16 == 0),
-                "asr_create: decoder head_dim must be 128 or a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)", dh, d);
+    SBK_REQUIRE(!((c.parts & SBK_PART_DECODER) && c.num_decoder_layers > 0) ||
+                    ((dh <= 64 || dh == 80 || dh == 128) && dh % 4 == 0 && d % 16 == 0),
+                "asr_create: decoder head_dim must be 128, 80 or a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)",
+                dh, d);
     SBK_REQUIRE(c.attention_type != SBK_ATT_ROPE || dh % 32 == 0, "asr_create: RoPEMHA needs head_dim %% 32 == 0");
     SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER || c.encoder_module == SBK_ENC_BRANCHFORMER || tfm,
                 "asr_create: encoder_module %d (0 Conformer, 1 Branchformer, 2 Transformer)", c.encoder_module);

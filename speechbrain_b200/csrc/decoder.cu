@@ -209,6 +209,9 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (VPL <= 4 ? 2 : 1)) skinny_gemm
                 case SK_F16_GELU:
                     reinterpret_cast<__half*>(a.out)[static_cast<size_t>(row) * a.ldo + col] = float2half_sat(gelu_erf_f(v));
                     break;
+                case SK_F16_SILU:
+                    reinterpret_cast<__half*>(a.out)[static_cast<size_t>(row) * a.ldo + col] = float2half_sat(silu_f(v));
+                    break;
                 case SK_F32: reinterpret_cast<float*>(a.out)[static_cast<size_t>(row) * a.ldo + col] = v; break;
                 case SK_RESID: reinterpret_cast<float*>(a.out)[static_cast<size_t>(row) * a.ldo + col] += v; break;
                 case SK_QKV_CACHE: {
@@ -270,15 +273,18 @@ int skinny_gemm(const SkinnyArgs& a, cudaStream_t stream) {
 // 3 shuffles, and the probabilities stay in registers for p.V.  The 4 warps' (max, sum, out) triples are merged
 // through shared memory.
 // Self-attention: keys = cache positions [0, step]; cross-attention: keys = encoder frames [0, enc_len[utt]).
-// (nn.MultiheadAttention semantics, scale 1/sqrt(d_h) already folded into q.)  head_dim DH == 64, or 128 (the Transformer
-// recipes' 4 heads of 128): a lane then owns dims [8 (lane % 8), +8) of each 64-dim half, NV = 2 16-byte vectors per key.
+// (nn.MultiheadAttention semantics, scale 1/sqrt(d_h) already folded into q.)  head_dim DH == 64, 80 (the d_model 640
+// recipes' 8 heads of 80) or 128 (the Transformer recipes' 4 heads of 128): a lane then owns dims [8 (lane % 8), +8) of
+// each 64-dim slice, NV = 2 16-byte vectors per key; at 80 the second slice is 16 dims wide, held by lanes 0 and 1 of each
+// group (the other lanes' second vector is zero and never stored).
 constexpr int DA_WARPS = 4;
 constexpr int DA_CHUNK = 32;  // keys a warp handles per round (8 per lane group)
 constexpr int DA_KPG = DA_CHUNK / 4;
 
 template <int DH>
 __global__ void __launch_bounds__(DA_WARPS * 32, DH == 64 ? 4 : 2) dec_attention_kernel(const DecAttnArgs a) {
-    constexpr int NV = DH / 64;
+    static_assert(DH % 8 == 0 && DH <= 128, "dec_attention_kernel: 16-byte vectors, at most two 64-dim slices");
+    constexpr int NV = (DH + 63) / 64;
     __shared__ float part_o[DA_WARPS][DH];
     __shared__ float part_m[DA_WARPS], part_l[DA_WARPS];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -298,6 +304,7 @@ __global__ void __launch_bounds__(DA_WARPS * 32, DH == 64 ? 4 : 2) dec_attention
     const int per = (n_keys + DA_WARPS - 1) / DA_WARPS;
     const int kb = warp * per, ke = min(n_keys, kb + per);
     const int gq = lane >> 3, dl = (lane & 7) * 8;
+    auto owns = [&](int v) { return DH % 64 == 0 || 64 * v + dl < DH; };  // this lane holds dims 64 v + dl .. + 8
     const int hs = a.head_stride > 0 ? a.head_stride : DH;
     const __half* kbase = a.kbase + static_cast<size_t>(blk) * a.row_stride + static_cast<size_t>(h) * hs + dl;
     const __half* vbase = a.vbase + static_cast<size_t>(blk) * a.row_stride + static_cast<size_t>(h) * hs + dl;
@@ -319,8 +326,8 @@ __global__ void __launch_bounds__(DA_WARPS * 32, DH == 64 ? 4 : 2) dec_attention
                 if (lin) { src_row = lin[j]; off += (static_cast<ptrdiff_t>(src_row) - r) * static_cast<ptrdiff_t>(a.row_stride); }
 #pragma unroll
                 for (int v = 0; v < NV; ++v) {
-                    kv[i][v] = *reinterpret_cast<const uint4*>(kbase + off + 64 * v);
-                    vv[i][v] = *reinterpret_cast<const uint4*>(vbase + off + 64 * v);
+                    kv[i][v] = owns(v) ? *reinterpret_cast<const uint4*>(kbase + off + 64 * v) : make_uint4(0u, 0u, 0u, 0u);
+                    vv[i][v] = owns(v) ? *reinterpret_cast<const uint4*>(vbase + off + 64 * v) : make_uint4(0u, 0u, 0u, 0u);
                 }
                 if (tokc) live[i] = tokc[static_cast<size_t>(src_row) * a.lin_stride + j] != a.pad_tok;
             } else {
@@ -340,7 +347,8 @@ __global__ void __launch_bounds__(DA_WARPS * 32, DH == 64 ? 4 : 2) dec_attention
     float qf[8 * NV];
 #pragma unroll
     for (int v = 0; v < NV; ++v) {
-        const uint4 qv = *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * DH + 64 * v + dl);
+        const uint4 qv = owns(v) ? *reinterpret_cast<const uint4*>(a.q + static_cast<size_t>(r) * a.ldq + h * DH + 64 * v + dl)
+                                 : make_uint4(0u, 0u, 0u, 0u);
         const __half2* q2 = reinterpret_cast<const __half2*>(&qv);
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
@@ -411,7 +419,8 @@ __global__ void __launch_bounds__(DA_WARPS * 32, DH == 64 ? 4 : 2) dec_attention
     }
     if (lane < 8) {
 #pragma unroll
-        for (int e = 0; e < 8 * NV; ++e) part_o[warp][64 * (e >> 3) + dl + (e & 7)] = o[e];
+        for (int e = 0; e < 8 * NV; ++e)
+            if (owns(e >> 3)) part_o[warp][64 * (e >> 3) + dl + (e & 7)] = o[e];
     }
     if (lane == 0) { part_m[warp] = m_run; part_l[warp] = l_run; }
     __syncthreads();
@@ -496,9 +505,9 @@ __global__ void __launch_bounds__(128) dec_attention_generic_kernel(const DecAtt
 }
 
 int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t stream) {
-    if (a.dh != 64 && a.dh != 128) {
+    if (a.dh != 64 && a.dh != 80 && a.dh != 128) {
         SBK_REQUIRE(a.dh >= 4 && a.dh <= 64 && a.dh % 4 == 0 && a.key_stride % 4 == 0 && a.row_stride % 4 == 0,
-                    "dec_attention: head_dim=%d not built (128, 64, or a multiple of 4 below 64)", a.dh);
+                    "dec_attention: head_dim=%d not built (128, 80, 64, or a multiple of 4 below 64)", a.dh);
         SBK_REQUIRE(max_keys <= DG_MAXKEYS, "dec_attention: %d keys exceed the generic kernel's limit %d", max_keys, DG_MAXKEYS);
         if (n_rows == 0) return SBK_OK;
         DecAttnArgs g = a;
@@ -511,10 +520,11 @@ int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t s
     if (n_rows == 0) return SBK_OK;
     DecAttnArgs b = a;
     b.n_keys_fixed = max_keys;
-    if (a.dh == 128) {
-        SBK_REQUIRE(a.key_stride % 8 == 0 && a.row_stride % 8 == 0 && a.ldq % 8 == 0,
-                    "dec_attention: head_dim 128 needs 16-byte aligned key rows");
-        SBK_CUDA_CHECK(launch_k(dec_attention_kernel<128>, dim3(a.H, n_rows), dim3(DA_WARPS * 32), 0, stream, b));
+    if (a.dh == 128 || a.dh == 80) {
+        SBK_REQUIRE(a.key_stride % 8 == 0 && a.row_stride % 8 == 0 && a.ldq % 8 == 0 && (a.dh == 128 || a.head_stride % 8 == 0),
+                    "dec_attention: head_dim %d needs 16-byte aligned key rows", a.dh);
+        SBK_CUDA_CHECK(launch_k(a.dh == 128 ? dec_attention_kernel<128> : dec_attention_kernel<80>, dim3(a.H, n_rows),
+                                dim3(DA_WARPS * 32), 0, stream, b));
     } else {
         SBK_CUDA_CHECK(launch_k(dec_attention_kernel<64>, dim3(a.H, n_rows), dim3(DA_WARPS * 32), 0, stream, b));
     }

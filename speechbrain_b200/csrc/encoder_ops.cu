@@ -643,6 +643,14 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
 
 // STREAM: one chunk of a stream (AttStream): T is the window [cached rows; chunk rows], the queries are its last sa.nq rows
 // (from sa.q), keys / values come from the ring sa.kv, every key of the window is visible, and out holds the chunk's rows.
+// Head dims that are whole 16-byte vectors stage K/V blocks with cp.async.  KV2: double-buffered (block jb+1 streams in while
+// block jb is multiplied; the second buffer pair sits behind everything else); otherwise one buffer pair, refilled after
+// the block has been multiplied.  RelPosMHAXL at head width 80 takes one pair: 97 KB of shared memory, two CTAs per SM,
+// against 119 KB and one CTA with two (H100 80GB HBM3, 700 W: B = 32, 8 heads, T = 251 113 us against 158 us; T = 2500
+// 5.56 ms against 7.92 ms).
+template <int DH, int DHP, bool RELPOS>
+__host__ __device__ constexpr bool att_kv2() { return (DH % 8 == 0) && (DHP == DH) && !(RELPOS && DH == 80); }
+
 template <int DH, int DHP, bool RELPOS, bool STREAM = false>  // DHP = DH rounded up to a multiple of 16 (zero-padded in shared memory)
 __global__ void __launch_bounds__(128)
 encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const int* __restrict__ lens,
@@ -660,10 +668,9 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
     __half* Qv = Vs + ATT_BK * STR;                    // RELPOS: [64][STR]
     __half* Ps = Qv + ATT_BQ * STR;                    // RELPOS: [ATT_PR][STR] ring of P rows (p_slot)
     float* Gs = reinterpret_cast<float*>(Ps + (RELPOS ? ATT_PR : 0) * STR);  // RELPOS: [4 warps][16][GW+1]
-    // head dims that are whole 16-byte vectors: K/V blocks are double-buffered with cp.async (block jb+1 streams in while
-    // block jb is multiplied); the second buffer pair sits behind everything else
     constexpr bool ASYNC = (DH % 8 == 0) && (DHP == DH);
-    __half* KV1 = reinterpret_cast<__half*>(Gs + (RELPOS ? 4 * 16 * (GW + 1) : 0));  // [2][64][STR] when ASYNC
+    constexpr bool KV2 = att_kv2<DH, DHP, RELPOS>();
+    __half* KV1 = reinterpret_cast<__half*>(Gs + (RELPOS ? 4 * 16 * (GW + 1) : 0));  // [2][64][STR] when KV2
 
     const int q_off = STREAM ? T - sa.nq : 0;  // window row of the first query
     const int b = blockIdx.z, h = blockIdx.y, i0 = q_off + blockIdx.x * ATT_BQ;
@@ -811,7 +818,7 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
         const int j0 = jb * ATT_BK;
         const __half* Kc = Ks;
         const __half* Vc = Vs;
-        if constexpr (ASYNC) {
+        if constexpr (KV2) {
             if ((jb - blk_begin) & 1) { Kc = KV1; Vc = KV1 + ATT_BK * STR; }
             asm volatile("cp.async.wait_group 0;" ::: "memory");
             __syncthreads();  // block jb has landed for everyone; block jb-1 (the other buffer) is fully consumed
@@ -819,6 +826,13 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
                 if ((jb - blk_begin) & 1) stage_async(jb + 1, Ks, Vs);
                 else stage_async(jb + 1, KV1, KV1 + ATT_BK * STR);
             }
+        } else if constexpr (ASYNC) {
+            if (jb != blk_begin) {  // block jb-1 has been multiplied by every warp: refill the buffer pair with block jb
+                __syncthreads();
+                stage_async(jb, Ks, Vs);
+            }
+            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            __syncthreads();  // block jb has landed for everyone
         } else {
             if constexpr (RELPOS) asm volatile("cp.async.wait_group 0;" ::: "memory");
             __syncthreads();  // previous block's K/V fully consumed (RELPOS: block jb's P rows have landed for everyone)
@@ -989,18 +1003,18 @@ static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int
         auto kern = encoder_attention_kernel<DH, DHP, false, STREAM>;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, nullptr, nullptr, nullptr, 0, scale, out, ldo, chunk, left_chunks, sa);
-    } else if constexpr (DH > 64) {  // the RelPos band and P window are built for head widths up to 64
+    } else if constexpr (DH > 64 && DH != 80) {  // RelPosMHAXL is built for the recipes' head widths: up to 64, and 80
         set_error("encoder_attention: RelPosMHAXL with head_dim=%d not built", DH);
         return SBK_ERR_UNSUPPORTED;
     } else {
-        constexpr bool ASYNC = (DH % 8 == 0) && (DHP == DH);  // as in the kernel: a second K/V buffer pair
+        constexpr bool ASYNC = (DH % 8 == 0) && (DHP == DH);  // as in the kernel
         if (ASYNC)
             SBK_REQUIRE(ldp % 8 == 0 && (reinterpret_cast<uintptr_t>(P) & 15) == 0, "encoder_attention: P must be 16-byte aligned");
         else
             SBK_REQUIRE(ldp % 4 == 0 && (reinterpret_cast<uintptr_t>(P) & 7) == 0, "encoder_attention: P must be 8-byte aligned");
-        // independent of T: 101 KB at head_dim 64 (two CTAs per SM), 69 KB at 36 and 65 KB at 32 (three)
+        // independent of T: 101 KB at head_dim 64 and 97 KB at 80 (two CTAs per SM), 69 KB at 36 and 65 KB at 32 (three)
         const size_t smem = (4ull * ATT_BQ + ATT_PR) * STR * 2 + 4ull * 16 * (ATT_GW + 1) * 4 +
-                            (ASYNC ? 2ull * ATT_BK * STR * 2 : 0);
+                            (att_kv2<DH, DHP, true>() ? 2ull * ATT_BK * STR * 2 : 0);
         auto kern = encoder_attention_kernel<DH, DHP, true, STREAM>;
         SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, sa);
@@ -1023,9 +1037,11 @@ int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_d
         return launch_encoder_attention<36, 48>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
     if (head_dim == 32)
         return launch_encoder_attention<32, 32>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
+    if (head_dim == 80)  // the d_model 640 conformer_large recipes (Libriheavy, People's Speech): 640 / 8 heads
+        return launch_encoder_attention<80, 80>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
     if (head_dim == 128)  // the Transformer recipes' regularMHA (512 / 4 heads); no positional term
         return launch_encoder_attention<128, 128>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
-    set_error("encoder_attention: head_dim=%d not built (128, 64, 36, 32)", head_dim);
+    set_error("encoder_attention: head_dim=%d not built (128, 80, 64, 36, 32)", head_dim);
     return SBK_ERR_UNSUPPORTED;
 }
 

@@ -626,9 +626,10 @@ static StepGemm step_gemm(const AsrModel* m, int rows, int width) {
 // against 23.4 / 23.3 ms without).  Every entry that runs a step loop sets it before the loop.
 static void set_step_pdl(const AsrModel* m, int rows, int width) { set_pdl(step_gemm(m, rows, width) == SG_SMALL); }
 
-// What a step's Linear writes: fp16 (optionally through GELU / ReLU), fp32, fp32 added in place to `out` (the residual
-// stream), or the self-attention in_proj's [q | k | v]: q to `out`, k and v into the caches at (row, step_ptr[row]).
-enum ProjOut { PO_F16, PO_F16_GELU, PO_F16_RELU, PO_F32, PO_RESID, PO_QKV_CACHE };
+// What a step's Linear writes: fp16 (optionally through GELU / ReLU / SiLU), fp32, fp32 added in place to `out` (the
+// residual stream), or the self-attention in_proj's [q | k | v]: q to `out`, k and v into the caches at (row, step_ptr[row]).
+// (sbk_step_proj_test takes the codes up to PO_QKV_CACHE.)
+enum ProjOut { PO_F16, PO_F16_GELU, PO_F16_RELU, PO_F32, PO_RESID, PO_QKV_CACHE, PO_F16_SILU };
 // One Linear of a step: out[rows, N] (row stride ldo) = epilogue(A[rows, K] (row stride lda) x W[N, K]^T + bias).
 struct Proj {
     const __half* W; const float* bias; int N, K;
@@ -640,7 +641,7 @@ struct Proj {
 
 static int project(StepGemm g, const Proj& p, int rows, cudaStream_t st) {
     if (g == SG_STREAM) {
-        static const int skinny_epi[] = {SK_F16, SK_F16_GELU, SK_F16_RELU, SK_F32, SK_RESID, SK_QKV_CACHE};
+        static const int skinny_epi[] = {SK_F16, SK_F16_GELU, SK_F16_RELU, SK_F32, SK_RESID, SK_QKV_CACHE, SK_F16_SILU};
         SkinnyArgs a{};
         a.A = p.A; a.lda = p.lda; a.W = p.W; a.ldw = p.K; a.bias = p.bias; a.n_rows = rows; a.N = p.N; a.K = p.K;
         a.epi = skinny_epi[p.kind]; a.out = p.out; a.ldo = p.ldo;
@@ -652,7 +653,7 @@ static int project(StepGemm g, const Proj& p, int rows, cudaStream_t st) {
     }
     GemmEpilogue e;
     e.mode = p.kind == PO_F32 ? EPI_F32 : p.kind == PO_RESID ? EPI_RESID : p.kind == PO_QKV_CACHE ? EPI_QKV_CACHE : EPI_F16;
-    e.act = p.kind == PO_F16_GELU ? ACT_GELU : p.kind == PO_F16_RELU ? ACT_RELU : ACT_NONE;
+    e.act = p.kind == PO_F16_GELU ? ACT_GELU : p.kind == PO_F16_RELU ? ACT_RELU : p.kind == PO_F16_SILU ? ACT_SILU : ACT_NONE;
     e.bias = p.bias; e.out = p.out; e.ldo = p.ldo;
     if (p.kind == PO_RESID) e.resid = static_cast<const float*>(p.out);
     if (p.kind == PO_QKV_CACHE) {
@@ -687,7 +688,9 @@ static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T,
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H, Ld = c.num_decoder_layers;
-    const ProjOut ffn_act = c.decoder_activation == SBK_ACT_GELU ? PO_F16_GELU : PO_F16_RELU;
+    const ProjOut ffn_act = c.decoder_activation == SBK_ACT_GELU   ? PO_F16_GELU
+                            : c.decoder_activation == SBK_ACT_SILU ? PO_F16_SILU
+                                                                   : PO_F16_RELU;
     const int n_utt = rows / rows_per_utt;
     const StepGemm g = step_gemm(m, rows, d);
     // b.dx already holds emb[token] * sqrt(d) + pe[step] (written by greedy_reset / the previous greedy_select)

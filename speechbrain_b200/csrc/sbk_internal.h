@@ -187,7 +187,7 @@ int lm_causal_attention(const __half* qkv, int n, int s, int d, int H, const int
                         cudaStream_t stream);
 
 // ---- decoder.cu
-enum SkinnyEpi { SK_F16 = 0, SK_F16_GELU = 1, SK_F32 = 2, SK_RESID = 3, SK_QKV_CACHE = 4, SK_F16_RELU = 5 };
+enum SkinnyEpi { SK_F16 = 0, SK_F16_GELU = 1, SK_F32 = 2, SK_RESID = 3, SK_QKV_CACHE = 4, SK_F16_RELU = 5, SK_F16_SILU = 6 };
 struct SkinnyArgs {
     const __half* A; int lda;
     const __half* W; int ldw;

@@ -161,7 +161,7 @@ int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, co
                     ldq >= H * dh && ldo >= H * dh && key_stride >= 1 && row_stride >= 0 && head_stride >= 0,
                 "dec_attention_test: bad sizes rows=%d rows_per_block=%d H=%d dh=%d max_keys=%d", rows, rows_per_block, H, dh,
                 max_keys);
-    if (dh == 64 || dh == 128) {  // 16-byte loads of q, K and V
+    if (dh == 64 || dh == 80 || dh == 128) {  // 16-byte loads of q, K and V
         const uintptr_t al = reinterpret_cast<uintptr_t>(q_dev) | reinterpret_cast<uintptr_t>(kbase_dev) |
                              reinterpret_cast<uintptr_t>(vbase_dev);
         SBK_REQUIRE((al & 15) == 0 && ldq % 8 == 0 && key_stride % 8 == 0 && row_stride % 8 == 0 && head_stride % 8 == 0,

@@ -73,7 +73,7 @@ class AsrEngine:
     """One repacked model on one GPU.  ``cfg`` keys: n_fft, hop, win (samples), n_mels, cnn_channels, input_size,
     d_model, nhead, num_encoder_layers, num_decoder_layers, d_ffn, vocab, kernel_size, attention_type
     ("RoPEMHA"|"RelPosMHAXL"|"hypermixing"|"regularMHA", hypermixing with the Conformer only, regularMHA with the Transformer
-    only), decoder_activation ("gelu"|"relu"), max_length; encoder_module ("conformer" (default) | "branchformer" |
+    only), decoder_activation ("gelu"|"relu"|"swish"), max_length; encoder_module ("conformer" (default) | "branchformer" |
     "transformer") with csgu_linear_units and branchformer_activation ("gelu" (default) | "relu"); cnn_blocks (2 (default),
     or 3: the Transformer recipes' front-end, cnn_channels (64, 64)).
     ``state``: {reference key with recipe prefix: CPU fp32 tensor}."""
@@ -94,7 +94,10 @@ class AsrEngine:
         if att not in att_types:
             raise NotImplementedError(f"attention_type={att!r}: only RoPEMHA, RelPosMHAXL, hypermixing and regularMHA are built")
         c.attention_type = att_types[att]
-        c.decoder_activation = _lib.SBK_ACT_GELU if cfg.get("decoder_activation", "gelu") == "gelu" else _lib.SBK_ACT_RELU
+        dec_acts = {"gelu": _lib.SBK_ACT_GELU, "relu": _lib.SBK_ACT_RELU, "swish": _lib.SBK_ACT_SILU}
+        if cfg.get("decoder_activation", "gelu") not in dec_acts:
+            raise NotImplementedError(f"decoder_activation={cfg['decoder_activation']!r}: only gelu, relu and swish are built")
+        c.decoder_activation = dec_acts[cfg.get("decoder_activation", "gelu")]
         c.max_len = cfg.get("max_length", 2500)
         enc_module = cfg.get("encoder_module", "conformer")
         if enc_module not in ("conformer", "branchformer", "transformer"):

@@ -1,10 +1,12 @@
 """TransformerASR -- drop-in for speechbrain.lobes.models.transformer.TransformerASR.TransformerASR
 (TransformerASR.py:167-675) restricted to what the Conformer, HyperConformer and Branchformer ASR recipes instantiate:
 encoder_module="conformer" with attention_type in {"RoPEMHA", "RelPosMHAXL", "hypermixing"} and normalize_before=True
-(hypermixing: HyperMixing token mixing, nnet/hypermixing.py, with head width d_model / nhead of 32 or 64 and
+(head width d_model / nhead of 64, 36 or 32, and 80 with RelPosMHAXL: the d_model 640 conformer_large recipes;
+hypermixing: HyperMixing token mixing, nnet/hypermixing.py, with head width d_model / nhead of 32 or 64 and
 d_ffn / nhead a multiple of 16 up to 256), or encoder_module="branchformer" with attention_type="RelPosMHAXL"
 (Branchformer.py:92-410), or encoder_module="transformer" with attention_type="regularMHA",
 positional_encoding="fixed_abs_sine" and normalize_before=True (Transformer.py:311-490, head width 64 or 128); causal=False.
+The decoder's FFN activation is GELU, ReLU or Swish / SiLU.
 
 Same constructor kwargs, same state_dict keys (incl. the positional buffers), ``encode()`` on the sm_90a
 kernels.  ``decode()`` / ``forward()`` run teacher-forced on the KV-cached decoder step (the searchers in
@@ -93,15 +95,17 @@ class TransformerASR(torch.nn.Module):
         if encoder_module == "conformer" and conformer_activation is not None and getattr(conformer_activation, "__name__", "") not in ("Swish", "SiLU"):
             unsupported.append("conformer_activation other than Swish")
         if encoder_module != "transformer" and (d_model % nhead or d_model // nhead not in (64, 36, 32)):
-            unsupported.append(f"head_dim={d_model // max(nhead, 1)} (64, 36 or 32)")
+            if not (encoder_module == "conformer" and attention_type == "RelPosMHAXL" and d_model == 80 * nhead):
+                unsupported.append(f"head_dim={d_model // max(nhead, 1)} (64, 36 or 32; 80 for the Conformer with RelPosMHAXL)")
         if d_model % 16:
             unsupported.append("d_model not a multiple of 16")
         if unsupported:
             raise NotImplementedError("speechbrain_b200.TransformerASR: not built: " + ", ".join(unsupported))
         act_name = getattr(activation, "__name__", str(activation))
-        if act_name not in ("GELU", "ReLU"):
+        dec_acts = {"GELU": "gelu", "ReLU": "relu", "Swish": "swish", "SiLU": "swish"}
+        if act_name not in dec_acts:
             raise NotImplementedError(f"speechbrain_b200.TransformerASR: decoder activation {act_name} not built")
-        self.decoder_activation = "gelu" if act_name == "GELU" else "relu"
+        self.decoder_activation = dec_acts[act_name]
         self.tgt_vocab, self.input_size, self.d_model, self.nhead = tgt_vocab, input_size, d_model, nhead
         self.num_encoder_layers, self.num_decoder_layers, self.d_ffn = num_encoder_layers, num_decoder_layers, d_ffn
         self.kernel_size, self.attention_type, self.max_length, self.causal = kernel_size, attention_type, max_length, causal
@@ -223,6 +227,8 @@ class TransformerASR(torch.nn.Module):
             raise NotImplementedError("TransformerASR: the Branchformer encoder has no streaming mode")
         if self.attention_type == "hypermixing":
             raise NotImplementedError("TransformerASR: HyperMixing has no streaming mode")
+        if self.d_model // self.nhead == 80:
+            raise NotImplementedError("TransformerASR: streaming is not built for head width 80")
 
     def make_streaming_context(self, dynchunktrain_config):
         """Streaming context for ``encode_streaming`` (TransformerASR.py:645-670).  An infinite left context

@@ -134,3 +134,11 @@ TRANSFORMER_LARGE = dict(name="transformer_large", sample_rate=16000, n_fft=400,
                          cnn_channels=(64, 64), cnn_blocks=3, input_size=1280, d_model=512, nhead=4, num_encoder_layers=12,
                          num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="regularMHA",
                          decoder_activation="gelu", max_length=2500, encoder_module="transformer")
+# recipes/Libriheavy/ASR/transformer/hparams/conformer_large.yaml: 14 Conformer layers at d_model 640 with RelPosMHAXL (8 heads
+# of 80), 6 GELU decoder layers, 5000 tokens; and recipes/PeoplesSpeech/ASR/transformer/hparams/conformer_large.yaml: the same
+# encoder, 6 decoder layers with a Swish FFN, 5120 tokens
+CONFORMER_640 = dict(name="conformer_640", sample_rate=16000, n_fft=512, win=512, hop=160, n_mels=80,
+                     cnn_channels=(64, 32), input_size=640, d_model=640, nhead=8, num_encoder_layers=14,
+                     num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="RelPosMHAXL",
+                     decoder_activation="gelu", max_length=2500)
+CONFORMER_640_PEOPLES = dict(CONFORMER_640, name="conformer_640_peoples", vocab=5120, decoder_activation="swish")
