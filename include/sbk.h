@@ -350,6 +350,36 @@ int sbk_ctc_beam_search(const float* log_probs_dev, const int* lens_dev, int B, 
                         void* workspace_dev, size_t workspace_bytes, int* frame_beams_dev, int* parent_dev, int* token_dev,
                         float* score_dev, int* n_final_dev, void* stream);
 
+/* ---- CTC prefix beam search without a language model: the frame loop of CTCPrefixBeamSearcher (decoders/ctc.py:
+ * 1488-1905), candidates in CPython's set order, float64 beam probabilities.  Strings are hashed as above.  Per token of
+ * vocab_list[0 .. n_vocab): tok_info [n_vocab][SBK_CTC_PREFIX_TOK_INTS] int32 = kind (SBK_CTC_TOK_*), string id, length
+ * of the token string, length of the string a new beam appends to its text (" " + token[1:] for a word start, else the
+ * token), length of token[1:] (word starts), whether the appended string holds whitespace, length of its part before the
+ * first whitespace, of its part after the last whitespace, of its last non-empty word between the two (0: none);
+ * tok_hash [n_vocab][SBK_CTC_PREFIX_TOK_WORDS] uint64 = hash and base^length of the token string, hash and base^length
+ * of the appended string, hash of token[1:], hash and base^length of the leading part, hash of the trailing part, hash
+ * of the inner word. */
+#define SBK_CTC_PREFIX_TOK_INTS 9
+#define SBK_CTC_PREFIX_TOK_WORDS 9
+typedef struct {
+    int blank, beam_size, prune_history;
+    /* float32 thresholds: token_prune_min_logp, log(blank_skip_threshold); float64 beam_prune_logp */
+    float token_prune_min_logp, blank_skip_logp;
+    double beam_prune_logp;
+} sbk_ctc_prefix_beam_params;
+/* Workspace for one search: runs the token-count pre-pass over log_probs_dev [B, T, V] fp32 with lens_dev [B] int32
+ * absolute frame counts (0..T) and synchronises the stream.  1 <= beam_size <= 256, V <= 8192, n_vocab <= V. */
+int sbk_ctc_prefix_beam_workspace_bytes(const float* log_probs_dev, const int* lens_dev, int B, int T, int V, int n_vocab,
+                                        const sbk_ctc_prefix_beam_params* params, size_t* bytes, void* stream);
+/* The search, one CTA per utterance.  Outputs: frame_beams [B, T] int32 = beams after frame f (-1: frame skipped;
+ * frames >= lens[b] untouched), parent / token [B, T, beam_size] int32 = each surviving beam's origin: its rank at the
+ * previous processed frame and the token that created it (-1: the beam was carried over), score [B, beam_size] fp64 =
+ * final beam scores, n_final [B] int32 = final beam count.  Synchronises the stream once (the pre-pass), then enqueues. */
+int sbk_ctc_prefix_beam_search(const float* log_probs_dev, const int* lens_dev, int B, int T, int V, int n_vocab,
+                               const int* tok_info_dev, const uint64_t* tok_hash_dev, const sbk_ctc_prefix_beam_params* params,
+                               void* workspace_dev, size_t workspace_bytes, int* frame_beams_dev, int* parent_dev,
+                               int* token_dev, double* score_dev, int* n_final_dev, void* stream);
+
 /* ---- Transducer greedy search: TransducerBeamSearcher.transducer_greedy_decode (decoders/transducer.py:156-291) with
  * the prediction network Embedding -> LSTM (1 layer, unidirectional, with biases, gate order i, f, g, o) ->
  * Linear(bias=False), the joint GELU(tn + out_PN) (exact erf form) and the output Linear(bias=False) + log-softmax.

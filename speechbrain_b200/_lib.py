@@ -43,6 +43,12 @@ class sbk_ctc_beam_params(ctypes.Structure):
                 ("blank_skip_logp", ctypes.c_float)]
 
 
+class sbk_ctc_prefix_beam_params(ctypes.Structure):
+    _fields_ = [("blank", ctypes.c_int), ("beam_size", ctypes.c_int), ("prune_history", ctypes.c_int),
+                ("token_prune_min_logp", ctypes.c_float), ("blank_skip_logp", ctypes.c_float),
+                ("beam_prune_logp", ctypes.c_double)]
+
+
 SBK_ATT_ROPE, SBK_ATT_RELPOS, SBK_ATT_HYPERMIX, SBK_ATT_REGULAR = 0, 1, 2, 3
 SBK_ACT_RELU, SBK_ACT_GELU, SBK_ACT_SILU = 0, 1, 2
 SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER, SBK_ENC_TRANSFORMER = 0, 1, 2
@@ -60,6 +66,7 @@ EXPORTS = [
     "sbk_asr_set_poll_interval", "sbk_asr_beam_from_enc", "sbk_asr_set_decoder_ln_fusion", "sbk_asr_transcribe_greedy_group_dev",
     "sbk_asr_set_decoder_tc_min_rows", "sbk_asr_lm_rescore", "sbk_asr_transcribe_greedy_group_host_async", "sbk_asr_decode_teacher_forced", "sbk_asr_ctc_head", "sbk_rows_argmax_f32", "sbk_asr_set_dynchunk",
     "sbk_asr_lm_forward", "sbk_asr_lm_step_logits", "sbk_ctc_beam_workspace_bytes", "sbk_ctc_beam_search",
+    "sbk_ctc_prefix_beam_workspace_bytes", "sbk_ctc_prefix_beam_search",
     "sbk_transducer_create", "sbk_transducer_destroy", "sbk_transducer_info", "sbk_transducer_greedy",
     "sbk_asr_stream_create", "sbk_asr_stream_encode_chunk", "sbk_asr_stream_reset", "sbk_asr_stream_destroy",
     "sbk_asr_stream_context", "sbk_stream_qkv_test", "sbk_step_proj_test", "sbk_dec_attention_test",

@@ -2,4 +2,5 @@
 from .scorer import (CoverageScorer, CTCScorer, LengthScorer, RescorerBuilder, ScorerBuilder, TransformerLMRescorer,  # noqa: F401
                      TransformerLMScorer)
 from .seq2seq import S2STransformerBeamSearcher, S2STransformerGreedySearcher  # noqa: F401
-from .ctc import CTCBeamSearcher, CTCHypothesis, ctc_greedy_decode, filter_ctc_output  # noqa: F401
+from .ctc import (CTCBeamSearcher, CTCHypothesis, CTCPrefixBeamSearcher, ctc_greedy_decode,  # noqa: F401
+                  filter_ctc_output)

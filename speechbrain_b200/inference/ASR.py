@@ -200,9 +200,10 @@ class EncoderASR(torch.nn.Module):
     ``modules["encoder"]``: ``LengthsCapableSequential`` of Fbank, InputNormalization, ConvolutionFrontEnd,
     ``EncoderWrapper(TransformerASR)``, the CTC ``Linear`` and a log-softmax (``torch.nn.LogSoftmax`` /
     ``speechbrain_b200.nnet.activations.Softmax(apply_log=True)``); ``hparams["decoding_function"]`` is a
-    ``functools.partial`` of ``ctc_greedy_decode`` or the ``CTCBeamSearcher`` class (inference/ASR.py:212-282), which is
-    instantiated with ``hparams["test_beam_search"]`` (or no keywords) and the tokenizer's vocabulary; the log-posteriors
-    then stay on the device and go to the beam search kernel (csrc/ctc_beam.cu).  The prefix beam searchers are not built."""
+    ``functools.partial`` of ``ctc_greedy_decode`` or the ``CTCBeamSearcher`` / ``CTCPrefixBeamSearcher`` class
+    (inference/ASR.py:212-282), which is instantiated with ``hparams["test_beam_search"]`` (or no keywords) and the
+    tokenizer's vocabulary; the log-posteriors then stay on the device and go to the beam search kernel (csrc/ctc_beam.cu,
+    csrc/ctc_prefix_beam.cu).  TorchAudioCTCPrefixBeamSearch is not built."""
     HPARAMS_NEEDED = ["tokenizer", "decoding_function"]
     MODULES_NEEDED = ["encoder"]
 
@@ -210,7 +211,7 @@ class EncoderASR(torch.nn.Module):
         super().__init__()
         import functools
 
-        from ..decoders.ctc import CTCBeamSearcher, ctc_greedy_decode
+        from ..decoders.ctc import CTCBaseSearcher, ctc_greedy_decode
         from ..nnet.linear import Linear
         modules = dict(modules or {})
         if "encoder" not in modules:
@@ -222,7 +223,7 @@ class EncoderASR(torch.nn.Module):
                 raise ValueError(f"Need hparams['{k}']")
         self.tokenizer = self.hparams["tokenizer"]
         fn = self.hparams["decoding_function"]
-        self.beam_search = isinstance(fn, type) and issubclass(fn, CTCBeamSearcher)
+        self.beam_search = isinstance(fn, type) and issubclass(fn, CTCBaseSearcher)
         if self.beam_search:
             opts = dict(self.hparams.get("test_beam_search") or {})
             self.decoding_function = fn(**opts, vocab_list=self._vocab_list())
@@ -231,7 +232,8 @@ class EncoderASR(torch.nn.Module):
             self.blank_id = fn.keywords.get("blank_id", -1)
         else:
             raise NotImplementedError("speechbrain_b200.EncoderASR: decoding_function must be functools.partial(ctc_greedy_decode, "
-                                      "blank_id=...) or CTCBeamSearcher (the CTC prefix beam searchers are not built)")
+                                      "blank_id=...), CTCBeamSearcher or CTCPrefixBeamSearcher (TorchAudioCTCPrefixBeamSearch "
+                                      "is not built)")
         self.device = torch.device((run_opts or {}).get("device", "cuda:0"))
         vals = list(self.mods.values())
         wrap = _find(vals, EncoderWrapper)
@@ -281,7 +283,7 @@ class EncoderASR(torch.nn.Module):
 
     @torch.no_grad()
     def transcribe_batch(self, wavs, wav_lens):
-        """inference/ASR.py:325-373: -> (predicted_words, predicted_tokens); with a CTCBeamSearcher
+        """inference/ASR.py:325-373: -> (predicted_words, predicted_tokens); with a CTC beam searcher
         -> ([best text per utterance], the searcher's List[List[CTCHypothesis]])."""
         from ..decoders.ctc import greedy_from_argmax
         eng, enc = self._encode(wavs, wav_lens)
