@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import asr_oracle as O
+from parity import lm_scorer_state, oracle_lm
 
 WAV_SEED, LENS, STEPS, BOS, EOS = 7, [1.0, 0.9, 0.6, 0.3], 48, 1, 2
 PREFIX = "Transformer."
@@ -76,20 +77,13 @@ def decode(cfg, sd, tgt, enc, abs_len):
 
 
 def lm_scorer(cfg):
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
-    from speechbrain_b200.utils.seeded_init import seeded_state_dict
-    lm = TransformerLM(vocab=cfg["vocab"], d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                       dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-    return seeded_state_dict(lm, seed=1)
+    return lm_scorer_state(cfg["vocab"])
 
 
 @torch.no_grad()
 def beam(cfg, sd, enc, lens, case, **extra):
     """O.beam_search with the recipe's test search of a fixture beam case (dict(beam, lm_weight, ctc_weight, steps))"""
-    lm = None
-    if case["lm_weight"]:
-        lm = dict(sd=lm_scorer(cfg), cfg=dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072, activation="gelu"),
-                  weight=case["lm_weight"], temperature=1.15)
+    lm = oracle_lm(case["lm_weight"], 1.15, cfg["vocab"]) if case["lm_weight"] else None
     ctc = dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=case["ctc_weight"], blank_index=0)
     kw = dict(beam_size=case["beam"], max_decode_ratio=(case["steps"] + 0.5) / enc.shape[1])
     kw.update(extra)

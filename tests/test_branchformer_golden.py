@@ -9,13 +9,10 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import case_wav, check_summary, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir  # noqa: E402
 import branchformer_oracle as BO  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
 
 
 @pytest.fixture(scope="module")
@@ -28,26 +25,8 @@ def _state(cfg, fx):
     return scale_csgu_conv(seeded_asr_state(cfg, fx["weight_seed"]), fx["tap_gain"], fx["bias_center"])
 
 
-def _wav(case):
-    B, L = case["wav_shape"]
-    g = torch.Generator().manual_seed(case["wav_seed"])
-    wav = torch.randn(B, L, generator=g)
-    for b in range(B):
-        wav[b, int(round(float(case["wav_lens"][b]) * L)):] = 0
-    assert abs(float(wav.double().abs().sum()) - case["wav_checksum"]) / case["wav_checksum"] < 1e-9
-    return wav, case["wav_lens"]
-
-
 def _oracle_encode(cfg, sd, case, q=None):
-    wav, lens = _wav(case)
-    return BO.wav_to_states(wav, lens, sd, cfg, q=q)
-
-
-def _summary_err(enc, case):
-    """rel-L2 of the per-frame norms of every frame and of the sampled full rows against the reference's (the fixture keeps
-    those instead of the whole states)."""
-    idx = case["sample_idx"].long()
-    return max(_rel(enc.double().norm(dim=-1), case["frame_norm"]), _rel(enc[idx[:, 0], idx[:, 1]], case["sample_rows"]))
+    return BO.wav_to_states(*case_wav(case), sd, cfg, q=q)
 
 
 @pytest.mark.parametrize("case", ["large", "short", "ctc"])
@@ -57,12 +36,16 @@ def test_oracle_matches_reference(fx, case):
     sd = _state(cfg, fx)
     with torch.no_grad():
         enc = _oracle_encode(cfg, sd, fx[case])
-    r = _rel(enc, fx[case]["enc_out"]) if case == "short" else _summary_err(enc, fx[case])
-    print(f"[{case}] oracle vs reference encoder rel-L2 {r:.2e}")
-    assert r <= 1e-6
+    if case == "short":
+        r = rel(enc, fx[case]["enc_out"])
+        print(f"[{case}] oracle vs reference encoder rel-L2 {r:.2e}")
+        assert r <= 1e-6
+    else:  # the fixture keeps the per-frame norms and sampled rows instead of the whole states
+        c = fx[case]
+        check_summary(f"{case} oracle", enc, c["frame_norm"], c["sample_idx"], c["sample_rows"], 1e-6)
     if case == "ctc":
         lp = torch.log_softmax(torch.nn.functional.linear(enc, sd["ctc_lin.w.weight"], sd["ctc_lin.w.bias"]), -1)
-        assert _rel(lp, fx["ctc"]["log_probs"]) <= 1e-6
+        assert rel(lp, fx["ctc"]["log_probs"]) <= 1e-6
 
 
 def _mirror(cfg, **kw):
@@ -234,14 +217,9 @@ def test_from_hparams_branchformer_recipe_layout(tmp_path):
 
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_LARGE, seeded_asr_state
-    tmp = str(tmp_path)
     cfg = dict(BRANCHFORMER_LARGE, num_encoder_layers=2, num_decoder_layers=1, vocab=60)
     sd = seeded_asr_state(cfg, 0)
-    prefix = {"CNN.": "0.", "Transformer.": "1.", "seq_lin.": "2.", "ctc_lin.": "3."}
-    torch.save({q + k[len(p):]: v for k, v in sd.items() for p, q in prefix.items() if k.startswith(p)},
-               os.path.join(tmp, "asr.ckpt"))
-    torch.save({"count": 1, "glob_mean": sd["normalize.glob_mean"], "glob_std": sd["normalize.glob_std"]},
-               os.path.join(tmp, "normalizer.ckpt"))
+    tmp = write_pretrained_dir(tmp_path, YAML, dict(asr=module_list_ckpt(sd), normalizer=normalizer_ckpt(sd)))
     with open(os.path.join(tmp, "corpus.txt"), "w") as f:
         words = ["branch", "former", "gating", "spatial", "conv", "reflect", "merge", "attention", "encoder", "decoder"]
         for i in range(400):
@@ -249,8 +227,6 @@ def test_from_hparams_branchformer_recipe_layout(tmp_path):
     spm.SentencePieceTrainer.train(input=os.path.join(tmp, "corpus.txt"), model_prefix=os.path.join(tmp, "tok"), vocab_size=60,
                                    model_type="bpe", bos_id=1, eos_id=2, unk_id=0, pad_id=-1, minloglevel=2)
     os.rename(os.path.join(tmp, "tok.model"), os.path.join(tmp, "tokenizer.ckpt"))
-    with open(os.path.join(tmp, "hyperparams.yaml"), "w") as f:
-        f.write(YAML.replace("<save_dir>", tmp))
     asr = EncoderDecoderASR.from_hparams(source=tmp, run_opts={"device": "cuda:0"})
     tr = asr.transformer
     assert tr.encoder_module == "branchformer" and tr.csgu_linear_units == 3072 and asr.mods["decoder"].model is tr
@@ -272,8 +248,8 @@ def test_fp16_operand_error_estimate(fx):
         enc = _oracle_encode(BRANCHFORMER_LARGE, sd, fx["large"], q=lambda t: t.half().float())
         ref = _oracle_encode(BRANCHFORMER_LARGE, sd, fx["large"])  # = the reference (test_oracle_matches_reference)
     lens = fx["large"]["abs_len"]
-    per_utt = [_rel(enc[b, :int(lens[b])], ref[b, :int(lens[b])]) for b in range(ref.shape[0])]
-    r = _rel(enc, ref)
+    per_utt = [rel(enc[b, :int(lens[b])], ref[b, :int(lens[b])]) for b in range(ref.shape[0])]
+    r = rel(enc, ref)
     print(f"fp16-operand oracle vs reference: encoder rel-L2 {r:.2e}, valid frames per utterance "
           f"{['%.2e' % x for x in per_utt]}")
     assert r <= 1.2e-3 and max(per_utt) <= 1.2e-3

@@ -10,6 +10,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import check_summary, rel  # noqa: E402
 import conformer640_oracle as CO  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "conformer640.pt")
@@ -53,15 +54,9 @@ def _cfg(recipe):
     return CONFORMER_640 if recipe == "libriheavy" else CONFORMER_640_PEOPLES
 
 
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
-
-
-def _check_summary(name, x, summ):
-    idx = summ["sample_idx"].long()
-    e = max(_rel(x.double().norm(dim=-1), summ["row_norm"]), _rel(x[idx[:, 0], idx[:, 1]], summ["sample_rows"]))
-    print(f"{name}: oracle vs reference rel-L2 {e:.2e}")
-    assert e < 1e-5, name
+def _check_summary(tag, x, summ):
+    """the fixture names the row norms row_norm"""
+    check_summary(tag, x, summ["row_norm"], summ["sample_idx"], summ["sample_rows"], 1e-5)
 
 
 @pytest.mark.parametrize("recipe", ["libriheavy", "peoples"])
@@ -101,7 +96,7 @@ def test_oracle_matches_reference(fx, recipe):
     if "short" in g:
         w1, l1 = CO.waveforms(seed=13, L=20800, lens=[1.0])
         e1 = CO.encode(cfg, sd, w1, l1)
-        assert _rel(e1, g["short"]["enc"]) < 1e-5 and CO.greedy(cfg, sd, e1, l1, ratio=1.0)[0] == g["short"]["greedy_hyps"]
+        assert rel(e1, g["short"]["enc"]) < 1e-5 and CO.greedy(cfg, sd, e1, l1, ratio=1.0)[0] == g["short"]["greedy_hyps"]
 
 
 def test_fp16_operand_error_estimate():

@@ -9,24 +9,18 @@ hypothesis, or -- when fp16 rounding made the search pick another near-tied hypo
 (pinned against the reference by the generator) scores within 3e-2 of what we report and no worse than the reference's best
 minus 3e-2."""
 import os
+import sys
 
 import pytest
 import torch
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import (best_tokens, case_wav, check_beam, check_ctc_argmax, check_encoder, check_greedy, dev,  # noqa: E402,F401
+                    oracle_lm, rel)
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 pytestmark = pytest.mark.gpu
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def _cfg(g):
@@ -35,43 +29,11 @@ def _cfg(g):
     return dict(base, attention_type=g["cfg"]["attention_type"])
 
 
-def _inputs(g):
-    """The generator's waveform, regenerated from its seed (a checksum pins the RNG stream)."""
-    B, L = g["wav_shape"]
-    gen = torch.Generator().manual_seed(g["wav_seed"])
-    wav = torch.randn(B, L, generator=gen)
-    lens = g["wav_lens"]
-    for b in range(B):
-        wav[b, int(round(float(lens[b]) * L)):] = 0
-    chk = float(wav.double().abs().sum())
-    assert abs(chk - g["wav_checksum"]) / g["wav_checksum"] < 1e-9, "regenerated waveform differs from the golden run"
-    return wav, lens
-
-
 def _engine(cfg, dev, parts=("fbank", "cnn", "encoder", "decoder")):
     from speechbrain_b200.engine import AsrEngine
     from speechbrain_b200.utils.seeded_init import seeded_asr_state
     sd = seeded_asr_state(cfg, 0)
     return AsrEngine(cfg, sd, device=dev, parts=parts), sd
-
-
-def _check_greedy(tag, name, pred, score, g):
-    ref_tok, margin, ref_lp = g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"]
-    B, S = ref_tok.shape
-    compared, worst, stops = 0, 0.0, []
-    for b in range(B):
-        for s in range(S):
-            if int(pred[b, s]) != int(ref_tok[b, s]):
-                assert float(margin[b, s]) < 5e-3, f"[{tag}/{name}] token mismatch at b={b} s={s}, reference margin {float(margin[b, s]):.4f}"
-                stops.append((b, s))
-                break
-            d = abs(float(score[b, s]) - float(ref_lp[b, s]))
-            worst = max(worst, d)
-            assert d < 2e-2, f"[{tag}/{name}] chosen log-prob err {d} at b={b} s={s}"
-            compared += 1
-    print(f"[{tag}] greedy[{name}]: {compared}/{B * S} decisions compared identical, max chosen-log-prob err {worst:.2e}, "
-          f"near-tie stops {stops}")
-    assert compared >= 0.6 * B * S, "too few decisions comparable"
 
 
 @pytest.mark.parametrize("tag", ["bench_conformer_large_rope_10s", "bench_conformer_large_relpos_10s"])
@@ -83,21 +45,16 @@ def test_bench_shape_encoder_and_greedy(dev, tag):
     eng, sd = _engine(cfg, dev)
     chk = float(sum(v.double().abs().sum() for k, v in sorted(sd.items())))
     assert abs(chk - g["weight_checksum"]) / g["weight_checksum"] < 1e-9, "seeded weights differ from the golden run"
-    wav, lens = _inputs(g)
+    wav, lens = case_wav(g)
     S = g["greedy_tokens"].shape[1]
     for tc_rows, name in ((1 << 30, "weight-streaming"), (1, "wgmma")):
         eng.set_decoder_tc_min_rows(tc_rows)
         pred, score, enc, done = eng.transcribe_greedy_dev(wav.to(dev), lens.to(dev), S, 1, 2, want_enc=True)
         torch.cuda.synchronize()
         assert done == S
-        enc = enc.cpu()
-        assert torch.isfinite(enc).all()
-        r_all = _rel(enc, g["enc_out"])
-        per_utt = [_rel(enc[b, : int(g["abs_len"][b])], g["enc_out"][b, : int(g["abs_len"][b])]) for b in range(enc.shape[0])]
-        print(f"[{tag}] encoder rel-L2 err {r_all:.3e} (valid frames per utterance: {['%.2e' % x for x in per_utt]}) "
-              f"max abs {(enc - g['enc_out']).abs().max():.3e}")
-        assert r_all < 1e-3 and max(per_utt) < 1e-3
-        _check_greedy(tag, name, pred.cpu(), score.cpu(), g)
+        check_encoder(f"{tag}/{name}", enc.cpu(), g["enc_out"], g["abs_len"], 1e-3)
+        check_greedy(f"{tag}/{name}", pred.cpu(), score.cpu(), g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"],
+                     min_compared=0.6)
 
 
 def test_bench_shape_conformer_small(dev):
@@ -106,9 +63,9 @@ def test_bench_shape_conformer_small(dev):
     g = torch.load(os.path.join(GOLDEN, "bench_conformer_small_relpos_5s.pt"))
     cfg = _cfg(g)
     eng, sd = _engine(cfg, dev, parts=("fbank", "cnn", "encoder"))
-    wav, lens = _inputs(g)
+    wav, lens = case_wav(g)
     enc = eng.encode_wav(wav.to(dev), lens.to(dev)).cpu()
-    r = _rel(enc, g["enc_out"])
+    r = rel(enc, g["enc_out"])
     print(f"[conformer_small 8x5s] encoder rel-L2 err {r:.3e} max abs {(enc - g['enc_out']).abs().max():.3e}")
     assert enc.shape == g["enc_out"].shape and r < 1e-3
     eng.set_poll_interval(0)  # the encode-only CUDA-graph path
@@ -127,7 +84,7 @@ def test_bench_shape_decode_teacher_forced(dev):
     asr = bench.build_product_asr(cfg, seeded_asr_state(cfg, 0), dev)
     tr = asr.transformer
     pred, attn = tr.decode(gd["tgt"].to(dev), g["enc_out"].to(dev), gd["enc_len"].to(dev))
-    r = _rel(pred.cpu(), gd["pred"])
+    r = rel(pred.cpu(), gd["pred"])
     print(f"decode(tgt, enc, enc_len): rel-L2 err {r:.3e} max abs {(pred.cpu() - gd['pred']).abs().max():.3e}")
     assert pred.shape == gd["pred"].shape and attn is None and r < 2e-3
 
@@ -143,7 +100,7 @@ def test_bench_shape_beam10(dev, file, case):
     search) for 24 steps, and scorer-less searches whose hypotheses finish gradually (up to 48 steps)."""
     g = torch.load(os.path.join(GOLDEN, "bench_conformer_large_rope_10s.pt"))
     gb = torch.load(os.path.join(GOLDEN, file + ".pt"))[case]
-    _check_beam(dev, g, gb, case)
+    _run_beam_case(dev, g, gb, case)
 
 
 def test_beam66_recipe_width(dev):
@@ -151,7 +108,7 @@ def test_beam66_recipe_width(dev):
     reference on the 2 s golden."""
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam66_conformer_large_rope.pt"))
-    _check_beam(dev, g, gb, "beam66")
+    _run_beam_case(dev, g, gb, "beam66")
 
 
 def test_beam_search_with_coverage_scorer(dev):
@@ -159,13 +116,13 @@ def test_beam_search_with_coverage_scorer(dev):
     vs the reference on the 2 s golden; the weight is large enough that the result differs from the scorer-less search."""
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_cov_conformer_large_rope.pt"))
-    _check_beam(dev, g, gb, "coverage")
+    _run_beam_case(dev, g, gb, "coverage")
 
 
-def _check_beam(dev, g, gb, case):
+def _run_beam_case(dev, g, gb, case):
     import bench
     from oracle import asr_oracle as O
-    from speechbrain_b200.utils.seeded_init import seeded_asr_state, seeded_state_dict
+    from speechbrain_b200.utils.seeded_init import seeded_asr_state
     cfg = _cfg(g)
     sd = seeded_asr_state(cfg, 0)
     sd["seq_lin.w.bias"] = sd["seq_lin.w.bias"].clone()
@@ -186,46 +143,17 @@ def _check_beam(dev, g, gb, case):
         bs._get_engine(dev).set_decoder_tc_min_rows(64)
         print(f"beam[{case}] wgmma GEMM projections: best scores {s2[:, 0].tolist()}")
         assert (s2[:, 0].cpu() - scores[:, 0].cpu()).abs().max() < 2e-3
-    hyps, hlens, scores = hyps.cpu(), hlens.cpu(), scores.cpu()
-    B, L = hyps.shape[0], hyps.shape[2]
-    ref_h, ref_len, ref_s = gb["hyps"].long(), gb["lens"], gb["scores"]
-    tol, diverged = 3e-2, []
-    for b in range(B):
-        n = int(torch.round(hlens[b, 0] * L)) + 1          # tokens the search stored for its best hypothesis
-        n_ref = int(torch.round(ref_len[b, 0] * ref_h.shape[2])) + 1
-        ours, ref = hyps[b, 0, :n].tolist(), ref_h[b, 0, :n_ref].tolist()
-        assert abs(float(scores[b, 0]) - float(ref_s[b, 0])) < tol, f"best score {float(scores[b, 0])} vs reference {float(ref_s[b, 0])}"
-        if ours != ref:
-            diverged.append((b, ours))
-    # the n-best list as a whole: sorted scores of all `beam` hypotheses track the reference's
-    k = min(scores.shape[1], ref_s.shape[1])
-    nbest_err = (scores[:, :k] - ref_s[:, :k]).abs().max().item()
-    print(f"beam[{case}] best scores {scores[:, 0].tolist()} ref {ref_s[:, 0].tolist()}; identical best hypothesis for "
-          f"{B - len(diverged)}/{B} utterances (reference top-1/top-2 gaps {(ref_s[:, 0] - ref_s[:, 1]).tolist()}); "
-          f"max |n-best score - reference| over all {k} ranks {nbest_err:.2e}")
-    assert nbest_err < tol
-    if diverged:  # judge the near-tied alternative with the CPU oracle walked along OUR tokens
-        lm = ctc = None
-        if gb["with_lm"]:
-            from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
-            lm_m = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                                 dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-            lm = dict(sd=seeded_state_dict(lm_m, seed=1), cfg=dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072,
-                                                                   activation="gelu"), weight=0.6, temperature=1.15)
-        if gb["with_ctc"]:
-            ctc = dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4, blank_index=0)
-        idx = [b for b, _ in diverged]
+
+    @torch.no_grad()
+    def rescore_forced(idx, tokens):  # the CPU oracle walked along our tokens, with the case's scorers
+        lm = oracle_lm(0.6, 1.15) if gb["with_lm"] else None
+        ctc = dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4, blank_index=0) if gb["with_ctc"] else None
         kw = {k_: v for k_, v in gb["kwargs"].items() if k_ != "beam_size"}
-        ocfg = dict(g["cfg"])
-        with torch.no_grad():
-            o = O.beam_search(g["enc_out"][idx], g["wav_lens"][idx], sd, ocfg, sd["seq_lin.w.weight"], sd["seq_lin.w.bias"], 1, 2,
-                              beam_size=1, prefix="Transformer.", lm=lm, ctc=ctc, forced=[t for _, t in diverged],
-                              coverage=dict(weight=cov[0], threshold=cov[1]) if cov else None, **kw)
-        for (b, toks), osc in zip(diverged, o.tolist()):
-            print(f"   utterance {b}: our hypothesis ({len(toks)} tokens) scores {float(scores[b, 0]):.5f}, the oracle gives it "
-                  f"{osc:.5f}; reference best {float(ref_s[b, 0]):.5f}")
-            assert abs(osc - float(scores[b, 0])) < tol, "our score for our own hypothesis is off"
-            assert osc > float(ref_s[b, 0]) - tol, "the search returned a clearly worse hypothesis than the reference"
+        return O.beam_search(g["enc_out"][idx], g["wav_lens"][idx], sd, dict(g["cfg"]), sd["seq_lin.w.weight"], sd["seq_lin.w.bias"],
+                             1, 2, beam_size=1, prefix="Transformer.", lm=lm, ctc=ctc, forced=tokens,
+                             coverage=dict(weight=cov[0], threshold=cov[1]) if cov else None, **kw)
+    check_beam(f"beam[{case}]", best_tokens(hyps, hlens), scores, best_tokens(gb["hyps"].long(), gb["lens"]), gb["scores"],
+               rescore_forced)
 
 
 def _sub_lens(g, idx):
@@ -248,7 +176,7 @@ def test_encoder_decoder_asr_interface(dev):
     n_steps = g["greedy_logits"].shape[1]
     asr.mods["decoder"].max_decode_ratio = (n_steps + 0.5) / T
     enc = asr.encode_batch(g["wav"], g["wav_lens"])
-    assert _rel(enc.cpu(), g["enc_out"]) < 1.5e-3
+    assert rel(enc.cpu(), g["enc_out"]) < 1.5e-3
     words_h, toks_h = asr.transcribe_batch(g["wav"].pin_memory(), g["wav_lens"])       # host tensors (C-ABI host entry)
     words_d, toks_d = asr(g["wav"].to(dev), g["wav_lens"].to(dev))                     # device tensors, forward()
     print("EncoderDecoderASR greedy tokens", toks_h, "reference", g["hyps"])
@@ -258,7 +186,7 @@ def test_encoder_decoder_asr_interface(dev):
     builds = slot.builds
     enc2 = asr.transformer.encode(g["cnn_out"].to(dev), g["wav_lens"].to(dev))
     hy, _, _, _ = asr.mods["decoder"](enc, g["wav_lens"].to(dev))
-    assert slot.builds == builds and hy == g["hyps"] and _rel(enc2.cpu(), g["enc_out"]) < 1e-3
+    assert slot.builds == builds and hy == g["hyps"] and rel(enc2.cpu(), g["enc_out"]) < 1e-3
     # load_state_dict after first use must take effect (ADVICE r1: stale snapshot)
     lin = asr.mods["decoder"].fc
     bias = sd["seq_lin.w.bias"].clone()
@@ -319,7 +247,7 @@ def test_encoder_asr_ctc_greedy(dev):
     exceeds 5e-3, and -- with the near-tie frames taken from the reference -- identical token lists (merge + blank filter)."""
     import functools
 
-    from speechbrain_b200.decoders.ctc import ctc_greedy_decode, greedy_from_argmax
+    from speechbrain_b200.decoders.ctc import ctc_greedy_decode
     from speechbrain_b200.inference.ASR import EncoderASR
     from speechbrain_b200.lobes.features import Fbank
     from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
@@ -357,19 +285,9 @@ def test_encoder_asr_ctc_greedy(dev):
                          run_opts={"device": str(dev)})
         lp = asr.encode_batch(g["wav"], g["wav_lens"]).cpu()
         assert lp.shape[:2] == g["enc_out"].shape[:2] and lp.shape[2] == 5000
-        e = (lp[:, :, :64] - c["log_probs_head"]).abs().max().item()
         words, toks = asr.transcribe_batch(g["wav"], g["wav_lens"])
-        am = lp.argmax(-1)
-        T = lp.shape[1]
-        bad = 0
-        for b in range(lp.shape[0]):
-            n = int(torch.round(g["wav_lens"][b] * T))
-            strong = c["margin"][b, :n] >= 5e-3
-            bad += int((am[b, :n][strong] != c["argmax"][b, :n].long()[strong]).sum())
-        patched = torch.where(c["margin"] >= 5e-3, am, c["argmax"].long())
-        hy = greedy_from_argmax(patched, g["wav_lens"], 0)
-        print(f"EncoderASR[{name}] log-prob err {e:.2e}; strong-margin frames with another arg-max: {bad}; tokens {toks} ref {c['hyps']}")
-        assert e < 2e-2 and bad == 0 and hy == c["hyps"]
+        print(f"EncoderASR[{name}] tokens {toks} ref {c['hyps']}")
+        check_ctc_argmax(f"EncoderASR[{name}]", lp, c["log_probs_head"], c["argmax"], c["margin"], g["wav_lens"], 0, c["hyps"])
         # module-by-module use of the mirror function on a CUDA tensor of log-probs
         assert ctc_greedy_decode(lp.to(dev), g["wav_lens"], blank_id=0) == toks
 
@@ -398,7 +316,7 @@ def test_fp16_range_scaled_weights(dev):
     for name, bar in (("ffn", 1e-3), ("attn", 3e-3)):
         eng = AsrEngine(cfg, scale_state(sd, gs[name]["scales"]), device=dev, parts=("encoder",))
         enc = eng.encode_from_cnn(cnn, g["wav_lens"].to(dev)).cpu()
-        r = _rel(enc, gs[name]["enc_out"])
+        r = rel(enc, gs[name]["enc_out"])
         print(f"scaled weights [{name}] {gs[name]['scales']} (max |FFN pre-activation| {gs[name]['ffn_hidden_absmax']:.0f} in the "
               f"reference): encoder rel-L2 err {r:.3e} (bar {bar:g})")
         results.append((name, bool(torch.isfinite(enc).all()), r, bar))
@@ -422,19 +340,11 @@ def test_conformer_small_decoder_greedy(dev):
     ref_tok = g["greedy_logits"].argmax(-1)
     pred, score, lp, done = eng.greedy_from_enc(g["enc_out"].to(dev), g["wav_lens"].to(dev), n_steps, 1, 2, want_log_probs=True)
     pred, lp = pred.cpu(), lp.cpu()
-    worst, compared = 0.0, 0
-    for b in range(pred.shape[0]):
-        for s in range(n_steps):
-            if pred[b, s] != ref_tok[b, s]:
-                assert margin[b, s] < 5e-3, f"token mismatch at b={b} s={s} with margin {margin[b, s]}"
-                break
-            worst = max(worst, (lp[b, s] - ref_lp[b, s]).abs().max().item())
-            compared += 1
-    print(f"[conformer_small] greedy tokens {pred.tolist()} ref {g['hyps']}; {compared} steps compared, max log-prob err {worst:.2e}")
-    assert worst < 2e-2 and compared >= n_steps
+    print(f"[conformer_small] greedy tokens {pred.tolist()} ref {g['hyps']}")
+    check_greedy("conformer_small", pred, lp, ref_tok, margin, ref_lp, min_compared=1 / pred.shape[0])  # n_steps decisions
     # and the whole path from the waveform
     p2, _, enc, _ = eng.transcribe_greedy_dev(g["wav"].to(dev), g["wav_lens"].to(dev), n_steps, 1, 2, want_enc=True)
-    assert _rel(enc.cpu(), g["enc_out"]) < 1.5e-3
+    assert rel(enc.cpu(), g["enc_out"]) < 1.5e-3
 
 
 def test_dynamic_chunk_encode(dev):
@@ -455,10 +365,10 @@ def test_dynamic_chunk_encode(dev):
         tr = asrs[att]
         src = g["cnn_out"].to(dev)
         enc = tr.encode(src, g["wav_lens"].to(dev), dynchunktrain_config=DynChunkTrainConfig(c["chunk_size"], c["left_context_size"])).cpu()
-        r = _rel(enc, c["enc_out"])
+        r = rel(enc, c["enc_out"])
         full = tr.encode(src, g["wav_lens"].to(dev)).cpu()  # the engine is back in full-context mode afterwards
-        print(f"[dynchunk {key}] encoder rel-L2 err {r:.3e}; full-context afterwards rel {_rel(full, g['enc_out']):.3e}")
-        assert r < 1e-3 and _rel(full, g["enc_out"]) < 1e-3
+        print(f"[dynchunk {key}] encoder rel-L2 err {r:.3e}; full-context afterwards rel {rel(full, g['enc_out']):.3e}")
+        assert r < 1e-3 and rel(full, g["enc_out"]) < 1e-3
 
 
 def test_encode_streaming_equals_masked(dev):
@@ -479,7 +389,7 @@ def test_encode_streaming_equals_masked(dev):
         ctx = tr.make_streaming_context(dc)
         outs = [tr.encode_streaming(src[:, t:t + cs].contiguous(), ctx) for t in range(0, T, cs)]
         stream = torch.cat(outs, dim=1)
-        r = _rel(stream.cpu(), full.cpu())
+        r = rel(stream.cpu(), full.cpu())
         print(f"[streaming {att} chunk {cs} left {lc}] {len(outs)} chunks, retained history {ctx.history.shape[1]} of {T} frames, "
               f"rel diff vs masked {r:.2e}")
         assert stream.shape == full.shape and r < 3e-4  # same maths; the online-softmax key-block partition differs with the window
@@ -514,18 +424,14 @@ def test_edge_shapes_vs_oracle(dev, B, L, lens, att):
         T = ref.shape[1]
         out = O.greedy_search(ref, wl, sd, cfg, sd["seq_lin.w.weight"], sd["seq_lin.w.bias"], 1, 2, 0.0, (steps + 0.5) / T,
                               "Transformer.", return_logits=True)
-    r = _rel(enc.cpu(), ref)
+    r = rel(enc.cpu(), ref)
     logits = out[4]
     n = logits.shape[1]
     top2 = logits.topk(2, -1).values
-    ok = True
-    for b in range(B):
-        for s in range(min(n, done)):
-            if int(pred[b, s]) != int(logits[b, s].argmax()):
-                ok = ok and float(top2[b, s, 0] - top2[b, s, 1]) < 5e-3
-                break
-    print(f"edge B={B} L={L} lens={lens} {att}: T={T} encoder rel-L2 {r:.3e}, steps {done}/{n}, tokens ok {ok}")
-    assert enc.shape == ref.shape and torch.isfinite(enc).all() and r < 1e-3 and ok
+    print(f"edge B={B} L={L} lens={lens} {att}: T={T} encoder rel-L2 {r:.3e}, steps {done}/{n}")
+    assert enc.shape == ref.shape and torch.isfinite(enc).all() and r < 1e-3
+    m = min(n, done)
+    check_greedy(f"edge B={B} L={L}", pred.cpu()[:, :m], None, logits.argmax(-1)[:, :m], (top2[..., 0] - top2[..., 1])[:, :m])
 
 
 def test_long_utterance_vs_oracle(dev):
@@ -547,6 +453,6 @@ def test_long_utterance_vs_oracle(dev):
         del eng
         with torch.no_grad():
             ref = O.encode(O.full_pipeline_features(wav, wl, sd, dict(cfg, win_length=32)), wl, sd, cfg, "Transformer.")
-        r = _rel(enc, ref)
+        r = rel(enc, ref)
         print(f"long utterance {att}: T={ref.shape[1]} encoder rel-L2 {r:.3e}")
         assert enc.shape == ref.shape and r < 1e-3, f"{att}: rel-L2 {r:.3e}"

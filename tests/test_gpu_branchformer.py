@@ -8,8 +8,7 @@ Encoder bar: rel-L2 <= 1.5e-3 over all frames and over each utterance's valid fr
 operand rounded to fp16 already sits at 1.0e-3 on this input (test_branchformer_golden.py::test_fp16_operand_error_estimate):
 18 layers without a LayerNorm on the residual stream let the operand rounding accumulate (5e-4 after layer 1, 1.0e-3 after
 layer 18), so the Conformer's 1e-3 bar is below what fp16 operands allow here.  Greedy: tokens identical up to the first
-decision whose reference top-1/top-2 margin is below 5e-3, chosen log-probs within 2e-2 (the rule of
-test_gpu_bench_shapes.py)."""
+decision whose reference top-1/top-2 margin is below 5e-3, chosen log-probs within 2e-2 (parity.check_greedy)."""
 import functools
 import os
 import sys
@@ -19,6 +18,8 @@ import torch
 import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import (case_wav, check_alone_vs_batch, check_ctc_argmax, check_encoder, check_greedy, check_summary,  # noqa: E402,F401
+                    dev, seeded_wav)
 import branchformer_oracle as BO  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -28,36 +29,13 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def fx():
     return torch.load(os.path.join(GOLDEN, "branchformer.pt"))
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
 
 
 def _state(cfg, fx):
     from speechbrain_b200.utils.seeded_init import scale_csgu_conv, seeded_asr_state
     return scale_csgu_conv(seeded_asr_state(cfg, fx["weight_seed"]), fx["tap_gain"], fx["bias_center"])
-
-
-def _wav(case, seed_key="wav_seed", shape_key="wav_shape", check=True):
-    B, L = case[shape_key]
-    g = torch.Generator().manual_seed(case[seed_key])
-    wav = torch.randn(B, L, generator=g)
-    lens = case["wav_lens"] if check else torch.ones(B)
-    for b in range(B):
-        wav[b, int(round(float(lens[b]) * L)):] = 0
-    if check:
-        assert abs(float(wav.double().abs().sum()) - case["wav_checksum"]) / case["wav_checksum"] < 1e-9
-    return wav, lens
 
 
 # ------------------------------------------------------------------------------------------------ CSGU kernel
@@ -128,72 +106,44 @@ def _engine(cfg, fx, dev, parts=("fbank", "cnn", "encoder", "decoder")):
     return AsrEngine(cfg, _state(cfg, fx), device=dev, parts=parts)
 
 
-def _reference_states(cfg, fx, case):
+def _oracle_states(cfg, fx, case):
     """The reference's encoder states of a fixture case, recomputed by the CPU oracle and checked against the stored
     per-frame norms and sampled rows."""
-    wav, lens = _wav(case)
     with torch.no_grad():
-        ref = BO.wav_to_states(wav, lens, _state(cfg, fx), cfg)
-    idx = case["sample_idx"].long()
-    assert _rel(ref.double().norm(dim=-1), case["frame_norm"]) <= 1e-5
-    assert _rel(ref[idx[:, 0], idx[:, 1]], case["sample_rows"]) <= 1e-5
+        ref = BO.wav_to_states(*case_wav(case), _state(cfg, fx), cfg)
+    check_summary(f"{cfg['name']} oracle", ref, case["frame_norm"], case["sample_idx"], case["sample_rows"], 1e-5)
     return ref
-
-
-def _check_encoder(tag, enc, ref, abs_len):
-    r_all = _rel(enc, ref)
-    per = [_rel(enc[b, :int(abs_len[b])], ref[b, :int(abs_len[b])]) for b in range(enc.shape[0])]
-    print(f"[{tag}] encoder rel-L2 {r_all:.3e} (valid frames per utterance {['%.2e' % x for x in per]}) "
-          f"max abs {(enc - ref).abs().max():.3e}")
-    assert torch.isfinite(enc).all() and r_all <= ENC_BAR and max(per) <= ENC_BAR
 
 
 def test_branchformer_large_encoder_and_greedy(dev, fx):
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_LARGE
     g = fx["large"]
     eng = _engine(BRANCHFORMER_LARGE, fx, dev)
-    wav, lens = _wav(g)
+    wav, lens = case_wav(g)
     S = g["greedy_tokens"].shape[1]
     pred, score, enc, done = eng.transcribe_greedy_dev(wav.to(dev), lens.to(dev), S, 1, 2, want_enc=True)
     torch.cuda.synchronize()
     assert done == S
-    _check_encoder("branchformer_large 4x10s", enc.cpu(), _reference_states(BRANCHFORMER_LARGE, fx, g), g["abs_len"])
-    pred, score = pred.cpu(), score.cpu()
-    ref_tok, margin, ref_lp = g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"]
-    compared, stops = 0, []
-    for b in range(ref_tok.shape[0]):
-        for s in range(S):
-            if int(pred[b, s]) != int(ref_tok[b, s]):
-                assert float(margin[b, s]) < 5e-3, f"token mismatch at b={b} s={s}, reference margin {float(margin[b, s]):.4f}"
-                stops.append((b, s))
-                break
-            assert abs(float(score[b, s]) - float(ref_lp[b, s])) < 2e-2, f"chosen log-prob at b={b} s={s}"
-            compared += 1
-    print(f"[branchformer_large] greedy: {compared}/{ref_tok.numel()} decisions identical, near-tie stops {stops}")
-    # batch invariance: utterance 0 (relative length 1.0, so the same T) alone and in the padded batch; reruns bit-identical
-    enc_b = eng.encode_wav(wav.to(dev), lens.to(dev)).cpu()
-    enc_1 = eng.encode_wav(wav[:1].to(dev), lens[:1].to(dev)).cpu()
-    assert torch.equal(enc_b, eng.encode_wav(wav.to(dev), lens.to(dev)).cpu())
-    d = float((enc_1[0] - enc_b[0]).abs().max())
-    print(f"[branchformer_large] utterance alone vs in the batch: max abs {d:.2e}")
-    assert d <= 1e-5
+    check_encoder("branchformer_large 4x10s", enc.cpu(), _oracle_states(BRANCHFORMER_LARGE, fx, g), g["abs_len"], ENC_BAR)
+    check_greedy("branchformer_large", pred.cpu(), score.cpu(), g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"])
+    check_alone_vs_batch(lambda w, ln: eng.encode_wav(w.to(dev), ln.to(dev)), wav, lens, 1e-5)
 
 
 def test_branchformer_shortest_input(dev, fx):
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_LARGE
     s = fx["short"]
     eng = _engine(BRANCHFORMER_LARGE, fx, dev, parts=("fbank", "cnn", "encoder"))
-    wav, lens = _wav(s)
+    wav, lens = case_wav(s)
     enc = eng.encode_wav(wav.to(dev), lens.to(dev)).cpu()
     assert enc.shape == (1, 16, 512)
-    _check_encoder("branchformer_large T=16", enc, s["enc_out"], torch.tensor([16]))
-    wav15, lens15 = _wav(s, "short_wav_seed", "short_wav_shape", check=False)
+    check_encoder("branchformer_large T=16", enc, s["enc_out"], torch.tensor([16]), ENC_BAR)
+    wav15, lens15 = seeded_wav(s["short_wav_seed"], s["short_wav_shape"])
     with pytest.raises(RuntimeError, match="reflect"):
         eng.encode_wav(wav15.to(dev), lens15.to(dev))
 
 
 def test_branchformer_ctc_encoder_asr(dev, fx):
-    from speechbrain_b200.decoders.ctc import ctc_greedy_decode, greedy_from_argmax
+    from speechbrain_b200.decoders.ctc import ctc_greedy_decode
     from speechbrain_b200.inference.ASR import EncoderASR
     from speechbrain_b200.lobes.features import Fbank
     from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
@@ -223,22 +173,11 @@ def test_branchformer_ctc_encoder_asr(dev, fx):
                                    ctc_lin=ctc_lin, log_softmax=Softmax(apply_log=True))
     asr = EncoderASR(modules=dict(encoder=enc), hparams=dict(tokenizer=None, decoding_function=functools.partial(ctc_greedy_decode, blank_id=0)),
                      run_opts={"device": str(dev)})
-    wav, lens = _wav(c)
+    wav, lens = case_wav(c)
     lp = asr.encode_batch(wav, lens).cpu()
     assert lp.shape == c["log_probs"].shape
-    e = float((lp - c["log_probs"]).abs().max())
+    check_ctc_argmax("branchformer_ctc", lp, c["log_probs"], c["argmax"], c["margin"], lens, 0, c["hyps"])
     _, toks = asr.transcribe_batch(wav, lens)
-    am = lp.argmax(-1)
-    T = lp.shape[1]
-    bad = 0
-    for b in range(lp.shape[0]):
-        n = int(torch.round(lens[b] * T))
-        strong = c["margin"][b, :n] >= 5e-3
-        bad += int((am[b, :n][strong] != c["argmax"][b, :n].long()[strong]).sum())
-    patched = torch.where(c["margin"] >= 5e-3, am, c["argmax"].long())
-    print(f"[branchformer_ctc] log-prob max err {e:.2e}; strong-margin frames with another arg-max: {bad}; "
-          f"tokens {toks} ref {c['hyps']}")
-    assert e <= 2e-2 and bad == 0 and greedy_from_argmax(patched, lens, 0) == c["hyps"]
     assert toks == c["hyps"]
     states = _engine(cfg, fx, dev, parts=("fbank", "cnn", "encoder")).encode_wav(wav.to(dev), lens.to(dev)).cpu()
-    _check_encoder("branchformer_ctc 3x8s", states, _reference_states(cfg, fx, c), torch.round(lens * T).int())
+    check_encoder("branchformer_ctc 3x8s", states, _oracle_states(cfg, fx, c), torch.round(lens * lp.shape[1]).int(), ENC_BAR)

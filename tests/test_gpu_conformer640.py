@@ -10,7 +10,7 @@ tests/golden/conformer640.pt (generator: tools/make_conformer640_golden.py) and 
 conformer640_oracle.py recomputed here (it equals the reference to 1e-5 on every fixture entry, test_conformer640_oracle.py):
 4 x 10 s ragged [1.0, 0.9, 0.6, 0.3] waveforms -> encoder states (all frames and each utterance's valid frames, rel-L2 <=
 ENC_BAR), 48 greedy steps and teacher-forced decode() on 48 positions, Libriheavy's beam 66 + TransformerLM 0.6 + CTC 0.4
-and People's Speech's beam 10 + CTC 0.3 for 24 steps (the rule of test_bench_shape_beam10), a 1.3 s utterance, and both
+and People's Speech's beam 10 + CTC 0.3 for 24 steps (parity.check_beam), a 1.3 s utterance, and both
 recipes' inference layouts loaded through EncoderDecoderASR.from_hparams from a local directory.
 
 ENC_BAR: the oracle with every GEMM operand rounded to fp16 sits at about 5e-4 of the fp32 oracle on this input
@@ -20,12 +20,13 @@ import sys
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import conformer640_oracle as CO  # noqa: E402
 import test_gpu_decoder_kernels as DKT  # noqa: E402
 import test_gpu_encoder_kernels as EKT  # noqa: E402
+from parity import (BEAM_TOL, check_alone_vs_batch, check_beam, check_encoder, check_greedy, check_summary,  # noqa: E402,F401
+                    dev, lm_scorer, lm_scorer_state, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir)
 
 ENC_BAR = 1e-3
 DEC_BAR = 2e-3  # teacher-forced decode(), rel-L2 (measured 4.4e-4)
@@ -33,13 +34,6 @@ BOS, EOS = CO.BOS, CO.EOS
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "conformer640.pt")
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 # ------------------------------------------------------------------------------------------------ kernels at head width 80
@@ -88,10 +82,6 @@ def test_decode_cross_attention80(dev):
 
 
 # ------------------------------------------------------------------------------------------------ model level
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
-
-
 @pytest.fixture(scope="module")
 def fx():
     return torch.load(GOLDEN)
@@ -118,38 +108,9 @@ def peoples(fx):
     return _case(CONFORMER_640_PEOPLES, fx["peoples"])
 
 
-def _check_summary(name, x, summ, bar):
-    """x [B, T, d] against a fixture summary: every row's L2 norm and the sampled rows, rel-L2 <= bar"""
-    idx = summ["sample_idx"].long()
-    e_norm = _rel(x.double().norm(dim=-1), summ["row_norm"])
-    e_rows = _rel(x[idx[:, 0], idx[:, 1]], summ["sample_rows"])
-    print(f"MEASURE {name} vs reference fixture: row norms rel-L2 {e_norm:.3e}, sampled rows {e_rows:.3e} (bar {bar})")
-    assert e_norm <= bar and e_rows <= bar
-
-
-def _check_encoder(name, enc, ref, lens):
-    T = ref.shape[1]
-    per = [_rel(enc[b, :int(round(float(lens[b]) * T))], ref[b, :int(round(float(lens[b]) * T))]) for b in range(ref.shape[0])]
-    r = _rel(enc, ref)
-    print(f"MEASURE {name} encoder vs oracle rel-L2 {r:.3e}, valid frames per utterance {['%.3e' % x for x in per]} "
-          f"(bar {ENC_BAR})")
-    assert torch.isfinite(enc).all() and r <= ENC_BAR and max(per) <= ENC_BAR
-
-
-def _check_greedy(name, pred, score, tokens, margin, chosen_lp):
-    """tokens identical up to the first decision whose reference top-1/top-2 margin is below 5e-3; chosen log-probs within
-    2e-2 (test_gpu_branchformer.py's rule)"""
-    compared = 0
-    for b in range(tokens.shape[0]):
-        for s in range(min(pred.shape[1], tokens.shape[1])):
-            if int(pred[b, s]) != int(tokens[b, s]):
-                assert float(margin[b, s]) < 5e-3, f"{name}: greedy token differs at b={b} step={s}"
-                break
-            assert abs(float(score[b, s]) - float(chosen_lp[b, s])) < 2e-2, f"{name}: log-prob at b={b} step={s}"
-            compared += 1
-            if int(tokens[b, s]) == EOS:
-                break
-    print(f"MEASURE {name} greedy: {compared} decisions identical")
+def _check_summary(tag, x, summ, bar):
+    """the fixture names the row norms row_norm"""
+    check_summary(tag, x, summ["row_norm"], summ["sample_idx"], summ["sample_rows"], bar)
 
 
 @pytest.mark.parametrize("recipe", ["libriheavy", "peoples"])
@@ -161,23 +122,20 @@ def test_wav_to_encoder_and_greedy(dev, recipe, request):
     g = case["fx"]
     eng = AsrEngine(case["cfg"], case["sd"], device=str(dev))
     wav, lens = case["wav"].to(dev), case["lens"].to(dev)
-    pred, score, enc, _ = eng.transcribe_greedy_dev(wav, lens, CO.STEPS, BOS, EOS, want_enc=True)
+    def greedy(w, ln):
+        pred, score, enc, _ = eng.transcribe_greedy_dev(w, ln, CO.STEPS, BOS, EOS, want_enc=True)
+        return enc, pred, score
+    enc, pred, score = greedy(wav, lens)
     torch.cuda.synchronize()
     enc = enc.cpu()
     _check_summary(f"{recipe} encoder", enc, g["enc"], ENC_BAR)
-    _check_encoder(recipe, enc, case["enc"], case["lens"])
-    _check_greedy(recipe, pred.cpu(), score.cpu(), g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"])
-    pred2, score2, enc2, _ = eng.transcribe_greedy_dev(wav, lens, CO.STEPS, BOS, EOS, want_enc=True)
-    assert torch.equal(enc, enc2.cpu()) and torch.equal(pred, pred2) and torch.equal(score, score2), "rerun differs"
-    _, _, alone, _ = eng.transcribe_greedy_dev(wav[:1].contiguous(), lens[:1].contiguous(), CO.STEPS, BOS, EOS,
-                                               want_enc=True)
-    d = float((alone[0].cpu() - enc[0]).abs().max() / enc[0].abs().max())
-    print(f"MEASURE {recipe} utterance 0 alone vs in the batch: max |d| / max |x| {d:.2e}")
-    assert d <= 1e-5
+    check_encoder(recipe, enc, case["enc"], [round(float(x) * case["T"]) for x in case["lens"]], ENC_BAR)
+    check_greedy(recipe, pred.cpu(), score.cpu(), g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"], stop_at=EOS)
+    check_alone_vs_batch(greedy, wav, lens, 1e-5, relative=True)
     if "short" in g:  # one 1.3 s utterance (T = 33)
         w1, l1 = CO.waveforms(seed=13, L=20800, lens=[1.0])
         _, _, e1, _ = eng.transcribe_greedy_dev(w1.to(dev), l1.to(dev), 4, BOS, EOS, want_enc=True)
-        r = _rel(e1.cpu(), g["short"]["enc"])
+        r = rel(e1.cpu(), g["short"]["enc"])
         print(f"MEASURE {recipe} 1.3 s utterance encoder vs reference rel-L2 {r:.3e}")
         assert r <= ENC_BAR
 
@@ -210,7 +168,7 @@ def test_decode_teacher_forced(dev, recipe, request):
         tr._decoder_engine(dev).set_decoder_tc_min_rows(rows)
         out, _ = tr.decode(tgt.to(dev), case["enc"].to(dev), enc_len.to(dev))
         out = out.cpu()
-        r = _rel(out, ref)
+        r = rel(out, ref)
         print(f"MEASURE {recipe} decode() tc_min_rows={rows} rel-L2 vs oracle {r:.3e}")
         assert torch.isfinite(out).all() and r <= DEC_BAR
         _check_summary(f"{recipe} decode() tc_min_rows={rows}", out, case["fx"]["decode"], DEC_BAR)
@@ -220,7 +178,6 @@ def test_decode_teacher_forced(dev, recipe, request):
 def _search_modules(cfg, beam, lm_weight, ctc_weight, max_decode_ratio):
     from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
     from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
     from speechbrain_b200.nnet.linear import Linear
     sd = CO.state(cfg)
     tr = _transformer(cfg)
@@ -230,10 +187,7 @@ def _search_modules(cfg, beam, lm_weight, ctc_weight, max_decode_ratio):
     ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
     full, weights = [], {}
     if lm_weight:  # the recipe's order: [transformerlm, ctc]
-        lm_m = TransformerLM(vocab=cfg["vocab"], d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0,
-                             d_ffn=3072, dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-        lm_m.load_state_dict(CO.lm_scorer(cfg))
-        full.append(TransformerLMScorer(language_model=lm_m, temperature=1.15))
+        full.append(TransformerLMScorer(language_model=lm_scorer(cfg["vocab"]), temperature=1.15))
         weights["transformerlm"] = lm_weight
     full.append(CTCScorer(eos_index=EOS, blank_index=0, ctc_fc=ctc_lin))
     weights["ctc"] = ctc_weight
@@ -249,36 +203,25 @@ def test_beam_search(dev, recipe, request):
     """the recipe's test search (Libriheavy: beam 66, TransformerLM 0.6, CTC 0.4 on utterances 0 and 3; People's Speech:
     beam 10, CTC 0.3) for 24 steps on the oracle's encoder states vs the reference fixture: best scores within 3e-2, and a
     best hypothesis that differs from the reference's must score, by the oracle walked along its tokens, within 3e-2 of its
-    own score and no worse than the reference's best (test_bench_shape_beam10's rule); the n-best list against the oracle's"""
+    own score and no worse than the reference's best (parity.check_beam); the n-best list against the oracle's"""
     case = request.getfixturevalue(recipe)
     cfg, sd, gb = case["cfg"], case["sd"], case["fx"]["beam"]
     utts = gb["utts"]
     _, _, _, bs = _search_modules(cfg, gb["beam"], gb["lm_weight"], gb["ctc_weight"], (gb["steps"] + 0.5) / case["T"])
     enc, lens = case["enc"][utts], case["lens"][utts]
     hyps, _, scores, _ = bs(enc.to(dev), lens.to(dev))
-    scores = scores.cpu().view(-1)
+    scores = scores.cpu().view(-1, 1)
     h2, _, s2, _ = bs(enc.to(dev), lens.to(dev))
-    assert h2 == hyps and torch.equal(s2.cpu().view(-1), scores), "rerun differs"
-    tol, diverged = 3e-2, []
-    B = len(hyps)
-    for b in range(B):
-        assert abs(float(scores[b]) - float(gb["scores"][b])) < tol, \
-            f"best score {float(scores[b])} vs reference {float(gb['scores'][b])}"
-        if list(hyps[b]) != list(gb["hyps"][b]):
-            diverged.append((b, list(hyps[b]) + [EOS]))
+    assert h2 == hyps and torch.equal(s2.cpu().view(-1, 1), scores), "rerun differs"
+    # the fixture keeps the reference's best hypotheses and scores; its n-best list is the oracle's
+    check_beam(f"{recipe} beam {gb['beam']}", [list(h) + [EOS] for h in hyps], scores, [list(h) + [EOS] for h in gb["hyps"]],
+               gb["scores"].view(-1, 1), lambda idx, tokens: CO.beam(cfg, sd, enc[idx], lens[idx], dict(gb, beam=1), forced=tokens))
     bs.return_topk, bs.topk = True, gb["beam"]
     _, _, nbest, _ = bs(enc.to(dev), lens.to(dev))
-    nbest = nbest.cpu()
     _, _, ref_s, _ = CO.beam(cfg, sd, enc, lens, gb, return_topk=True, topk=gb["beam"])
-    nbest_err = (nbest - ref_s).abs().max().item()
-    print(f"MEASURE {recipe} beam {gb['beam']}: best {scores.tolist()} reference {gb['scores'].tolist()}; identical "
-          f"best hypothesis for {B - len(diverged)}/{B}; max |n-best - oracle| {nbest_err:.2e}")
-    assert nbest_err < tol
-    if diverged:
-        idx = [b for b, _ in diverged]
-        o = CO.beam(cfg, sd, enc[idx], lens[idx], dict(gb, beam=1), forced=[t for _, t in diverged])
-        for (b, _), osc in zip(diverged, o.tolist()):
-            assert abs(osc - float(scores[b])) < tol and osc > float(gb["scores"][b]) - tol
+    nbest_err = (nbest.cpu() - ref_s).abs().max().item()
+    print(f"MEASURE {recipe} beam {gb['beam']}: max |n-best - oracle| {nbest_err:.2e}")
+    assert nbest_err < BEAM_TOL
 
 
 INFERENCE_YAML = """
@@ -401,21 +344,13 @@ def test_from_hparams_local_directory(dev, recipe, request, tmp_path):
     cfg, sd = case["cfg"], case["sd"]
     lm = recipe == "libriheavy"
     beam, ratio = (66, 0.6, 0.4) if lm else (10, 0.0, 0.3), (24 + 0.5) / case["T"]
-    tmp = str(tmp_path)
-    prefix = {"CNN.": "0.", "Transformer.": "1.", "seq_lin.": "2.", "ctc_lin.": "3."}
-    torch.save({q + k[len(p):]: v for k, v in sd.items() for p, q in prefix.items() if k.startswith(p)},
-               os.path.join(tmp, "asr.ckpt"))
-    torch.save({"count": 1, "glob_mean": sd["normalize.glob_mean"], "glob_std": sd["normalize.glob_std"]},
-               os.path.join(tmp, "normalizer.ckpt"))
-    if lm:
-        torch.save(CO.lm_scorer(cfg), os.path.join(tmp, "lm.ckpt"))
     yaml = INFERENCE_YAML.format(
         vocab=cfg["vocab"], ratio=ratio, beam=beam[0],
         activation="speechbrain.nnet.activations.Swish" if cfg["decoder_activation"] == "swish" else "torch.nn.GELU",
         lm_block=LM_BLOCK if lm else CTC_BLOCK, lm_loadable="\n        lm: !ref <lm_model>" if lm else "",
         lm_path="\n        lm: <save_dir>/lm.ckpt" if lm else "")
-    with open(os.path.join(tmp, "hyperparams.yaml"), "w") as f:
-        f.write(yaml.replace("<save_dir>", tmp))
+    ckpts = dict(asr=module_list_ckpt(sd), normalizer=normalizer_ckpt(sd), **(dict(lm=lm_scorer_state(cfg["vocab"])) if lm else {}))
+    tmp = write_pretrained_dir(tmp_path, yaml, ckpts)
     loaded = EncoderDecoderASR.from_hparams(source=tmp, run_opts={"device": str(dev)})
     assert torch.equal(loaded.mods["decoder"].fc.w.weight.cpu(), sd["seq_lin.w.weight"])
     tr, _, _, bs = _search_modules(cfg, beam[0], beam[1], beam[2], ratio)

@@ -254,7 +254,7 @@ def test_ctc_only_beam16_vs_oracle_search():
     search, judged like the beam goldens (near-tied alternatives scored by the oracle walked along our tokens)."""
     from oracle import asr_oracle as O
     from speechbrain_b200.utils.seeded_init import seeded_asr_state
-    from test_gpu_bench_shapes import _cfg, _check_beam
+    from test_gpu_bench_shapes import _cfg, _run_beam_case
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     cfg = _cfg(g)
     sd = seeded_asr_state(cfg, 0)
@@ -266,4 +266,4 @@ def test_ctc_only_beam16_vs_oracle_search():
                                                ctc=dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4,
                                                         blank_index=0), topk=16, return_topk=True, **kw)
     gb = dict(kwargs=kw, eos_bias=0.0, max_decode_ratio=mdr, with_lm=False, with_ctc=True, hyps=hyps, lens=lens, scores=scores)
-    _check_beam(torch.device("cuda:0"), g, gb, "ctc_beam16")
+    _run_beam_case(torch.device("cuda:0"), g, gb, "ctc_beam16")

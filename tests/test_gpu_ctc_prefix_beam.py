@@ -16,19 +16,13 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
 import ctc_beam_oracle as CO  # noqa: E402
 from test_ctc_prefix_beam_golden import CASES, oracle  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 RECIPE = dict(blank_index=0, beam_size=100, beam_prune_logp=-12.0, token_prune_min_logp=-1.2, prune_history=False)
 DEFAULTS = dict(blank_index=0, topk=5)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def tuples(hyps):

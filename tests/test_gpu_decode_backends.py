@@ -3,6 +3,8 @@ streaming with the pre-norms fused into the projections, weight streaming with s
 GEMM.  Every entry point that runs a step loop must enqueue the launches its layer structure implies, keep the step's
 projections on the back end its row count selects, and give bit-identical results when run again."""
 import ctypes
+import os
+import sys
 
 import pytest
 import torch
@@ -11,6 +13,9 @@ from speechbrain_b200 import _lib
 from speechbrain_b200.engine import AsrEngine
 from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, CONFORMER_SMALL, seeded_asr_state, seeded_tensor
 from speechbrain_b200.utils.shapes import transformer_lm_shapes
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 LM = dict(d_model=128, nhead=2, num_encoder_layers=2, d_ffn=256)
@@ -36,13 +41,6 @@ LM_STEP = LL * 7 + 5
 # wgmma GEMM launches of one teacher-forced step on that back end (none on weight streaming): 6 per decoder layer (no
 # head), 4 per LM layer and 2 for the LM's output projection
 DEC_GEMMS, LM_GEMMS = LD * 6, LL * 4 + 2
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")

@@ -35,6 +35,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
 import decoder_kernels_oracle as DK  # noqa: E402
 
 #                (max |d| / (|ref| + rms), rel-L2)   measured worst
@@ -46,13 +47,6 @@ ATT_BAR = (8e-4, 5e-4)               # 3.6e-4, 2.4e-4
 pytestmark = pytest.mark.gpu
 SENT = -777.0   # sentinel of output entries a call must not write (exact in fp16)
 BIG = 3e4       # keys / values that must not be seen
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def _vp(t, off=0):

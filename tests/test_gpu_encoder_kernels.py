@@ -27,6 +27,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
 import encoder_kernels_oracle as EK  # noqa: E402
 
 #                 (max |d| / (|ref| + rms), rel-L2)   measured worst
@@ -35,13 +36,6 @@ ATT_BARS = {False: (1.5e-3, 5e-4),                  # RoPE / regularMHA: 7.1e-4,
 DW_BAR = 9e-4                                       # 4.3e-4
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 # ------------------------------------------------------------------------------------------------ attention

@@ -1,12 +1,17 @@
 """-m gpu tests of what sbk_asr_create rejects (csrc/asr_weights.cu): a state_dict with a required tensor missing, or with
 one of the wrong element count, fails with an error that names the key, for every part of a model and every encoder family;
 the optional tensors stay optional; a failed create leaves the process able to create."""
+import os
 import pytest
+import sys
 import torch
 
 from speechbrain_b200.engine import AsrEngine
 from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, TRANSFORMER_LARGE, seeded_asr_state, seeded_tensor
 from speechbrain_b200.utils.shapes import transformer_lm_shapes
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 LM = dict(d_model=128, nhead=2, num_encoder_layers=1, d_ffn=256)
@@ -41,13 +46,6 @@ REQUIRED = [
     ("lm", "lm.encoder.layers.0.self_att.att.in_proj_weight"),
     ("lm", "lm.output_proj.layers.2.w.weight"),
 ]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def _state(name):

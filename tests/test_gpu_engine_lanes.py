@@ -2,6 +2,8 @@
 own streams, events, buffers and graphs, and growing a lane buffer drops the graphs that captured pointers into it.
 Results are compared with the same handle's or the source's own, not with goldens (those are checked elsewhere)."""
 import gc
+import os
+import sys
 
 import pytest
 import torch
@@ -11,17 +13,13 @@ from speechbrain_b200.engine import AsrEngine
 from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state, seeded_tensor
 from speechbrain_b200.utils.shapes import transformer_lm_shapes
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
+
 pytestmark = pytest.mark.gpu
 LM = dict(d_model=128, nhead=2, num_encoder_layers=2, d_ffn=256)
 CFG = dict(CONFORMER_LARGE, num_encoder_layers=2, num_decoder_layers=2, lm=LM)
 BEAM = dict(beam_size=4, max_steps=12, min_steps=0, bos=1, eos=2, lm_weight=0.6, ctc_weight=0.4, blank_index=0)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def _engine(dev):

@@ -2,21 +2,19 @@
 count (M = 8032 = 32 x 251 frames: 62 full 128-row tiles and a 96-row tail, several tiles per CTA), the M tail and M < 128,
 K not a multiple of 64, and the all-layer cross-attention K/V launch against one launch per layer."""
 import ctypes
+import os
+import sys
 
 import pytest
 import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 
 EPI_F16, EPI_F32, EPI_RESID, EPI_GLU, EPI_ROPE = 0, 1, 2, 3, 4
 ACT_NONE, ACT_SILU, ACT_GELU = 0, 1, 2
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def _operands(dev, M, N, K, seed):

@@ -5,22 +5,20 @@ kernel works per row or per utterance, so with the decode kernels of a single-ba
 one pass (G <= 8), a partial last pass (G = 9: 5 + 4 batches) and two full ones (G = 16), each batch with its own
 waveforms and ragged lengths."""
 import math
+import os
+import sys
 
 import pytest
 import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 
 B, L, S = 32, 160000, 6  # 32 x 10 s: 251 frames, 8032 encoder rows per batch
 PASS = 8                 # batches in one pass of at most 65536 rows
 GROUPS = (1, PASS, PASS + 1, 16)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def _engine(base, dev, **kw):

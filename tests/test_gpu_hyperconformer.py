@@ -8,8 +8,8 @@ states as per-frame norms and sampled rows; the whole states are recomputed with
 Encoder bar: rel-L2 <= 7.5e-3 over all frames and over each utterance's valid frames.  The CPU oracle with every product's
 operands rounded to fp16 already sits at 3.2e-3 (all frames) and 4.9e-3 (worst utterance) on this input
 (test_hyperconformer_golden.py::test_fp16_operand_error_estimate).  Greedy: tokens identical up to the first decision whose
-reference top-1/top-2 margin is below 5e-3, chosen log-probs within 2e-2 (the rule of test_gpu_bench_shapes.py).  Beam 10
-with [TransformerLM 0.6, CTC 0.4]: the rule of test_gpu_bench_shapes.py::test_bench_shape_beam10."""
+reference top-1/top-2 margin is below 5e-3, chosen log-probs within 2e-2 (parity.check_greedy).  Beam 10
+with [TransformerLM 0.6, CTC 0.4]: parity.check_beam."""
 import os
 import sys
 
@@ -17,6 +17,8 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import (best_tokens, case_wav, check_alone_vs_batch, check_beam, check_encoder, check_greedy,  # noqa: E402,F401
+                    check_summary, dev, oracle_lm, rel)
 import hyperconformer_oracle as HO  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -27,34 +29,13 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def fx():
     return torch.load(os.path.join(GOLDEN, "hyperconformer.pt"))
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
 
 
 def _state(fx, gain=None):
     from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M, scale_hypernet, seeded_asr_state
     return scale_hypernet(seeded_asr_state(HYPERCONFORMER_22M, fx["weight_seed"]), fx["hypernet_gain"] if gain is None else gain)
-
-
-def _wav(case):
-    B, L = case["wav_shape"]
-    g = torch.Generator().manual_seed(case["wav_seed"])
-    wav = torch.randn(B, L, generator=g)
-    for b in range(B):
-        wav[b, int(round(float(case["wav_lens"][b]) * L)):] = 0
-    assert abs(float(wav.double().abs().sum()) - case["wav_checksum"]) / case["wav_checksum"] < 1e-9
-    return wav, case["wav_lens"]
 
 
 # ------------------------------------------------------------------------------------------------ HyperMixing kernels
@@ -108,8 +89,8 @@ def test_hypermix_kernel_vs_torch(dev, T, d, nhead, k):
             assert HO.max_abs_h(x16.float(), sd, "m.", kpm) > 65504.0
         out = _hm_dev(x16.to(dev), None if ln is None else ln.to(dev), w, nhead, k).cpu()
         valid = torch.ones(B, T, dtype=torch.bool) if kpm is None else ~kpm
-        r_all = _rel(out, ref)
-        r_utt = [_rel(out[b][valid[b]], ref[b][valid[b]]) for b in range(B)]
+        r_all = rel(out, ref)
+        r_utt = [rel(out[b][valid[b]], ref[b][valid[b]]) for b in range(B)]
         print(f"hypermix T={T} d={d} nhead={nhead} k={k} {name}: rel-L2 {r_all:.2e}, valid frames per utterance "
               f"{['%.1e' % r for r in r_utt]}, max abs {float((out - ref).abs().max()):.2e}")
         assert torch.isfinite(out).all() and r_all <= KERNEL_BAR and max(r_utt) <= KERNEL_BAR
@@ -139,115 +120,64 @@ def _engine(fx, dev, parts=("fbank", "cnn", "encoder", "decoder"), gain=None):
     return AsrEngine(HYPERCONFORMER_22M, _state(fx, gain), device=dev, parts=parts)
 
 
-def _reference_states(fx, case):
+def _oracle_states(fx, case):
     """The reference's encoder states of a fixture case, recomputed by the CPU oracle and checked against the stored
     per-frame norms and sampled rows."""
     from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M
-    wav, lens = _wav(case)
     with torch.no_grad():
-        ref = HO.wav_to_states(wav, lens, _state(fx), HYPERCONFORMER_22M)
-    idx = case["sample_idx"].long()
-    assert _rel(ref.double().norm(dim=-1), case["frame_norm"]) <= 1e-5
-    assert _rel(ref[idx[:, 0], idx[:, 1]], case["sample_rows"]) <= 1e-5
+        ref = HO.wav_to_states(*case_wav(case), _state(fx), HYPERCONFORMER_22M)
+    check_summary("hyperconformer_22M oracle", ref, case["frame_norm"], case["sample_idx"], case["sample_rows"], 1e-5)
     return ref
-
-
-def _check_encoder(tag, enc, ref, abs_len):
-    r_all = _rel(enc, ref)
-    per = [_rel(enc[b, :int(abs_len[b])], ref[b, :int(abs_len[b])]) for b in range(enc.shape[0])]
-    print(f"[{tag}] encoder rel-L2 {r_all:.3e} (valid frames per utterance {['%.2e' % x for x in per]}) "
-          f"max abs {(enc - ref).abs().max():.3e}")
-    assert torch.isfinite(enc).all() and r_all <= ENC_BAR and max(per) <= ENC_BAR
 
 
 def test_hyperconformer_encoder_and_greedy(dev, fx):
     g = fx["main"]
     eng = _engine(fx, dev)
-    wav, lens = _wav(g)
+    wav, lens = case_wav(g)
     S = g["greedy_tokens"].shape[1]
     pred, score, enc, done = eng.transcribe_greedy_dev(wav.to(dev), lens.to(dev), S, 1, 2, want_enc=True)
     torch.cuda.synchronize()
     assert done == S
-    _check_encoder("hyperconformer_22M 4x10s", enc.cpu(), _reference_states(fx, g), g["abs_len"])
-    pred, score = pred.cpu(), score.cpu()
-    ref_tok, margin, ref_lp = g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"]
-    compared, stops = 0, []
-    for b in range(ref_tok.shape[0]):
-        for s in range(S):
-            if int(pred[b, s]) != int(ref_tok[b, s]):
-                assert float(margin[b, s]) < 5e-3, f"token mismatch at b={b} s={s}, reference margin {float(margin[b, s]):.4f}"
-                stops.append((b, s))
-                break
-            assert abs(float(score[b, s]) - float(ref_lp[b, s])) < 2e-2, f"chosen log-prob at b={b} s={s}"
-            compared += 1
-    print(f"[hyperconformer_22M] greedy: {compared}/{ref_tok.numel()} decisions identical, near-tie stops {stops}")
-    # batch invariance: utterance 0 (relative length 1.0, so the same T) alone and in the padded batch; reruns bit-identical
-    enc_b = eng.encode_wav(wav.to(dev), lens.to(dev)).cpu()
-    enc_1 = eng.encode_wav(wav[:1].to(dev), lens[:1].to(dev)).cpu()
-    assert torch.equal(enc_b, eng.encode_wav(wav.to(dev), lens.to(dev)).cpu())
-    d = float((enc_1[0] - enc_b[0]).abs().max())
-    print(f"[hyperconformer_22M] utterance alone vs in the batch: max abs {d:.2e}")
-    assert d <= 1e-5
+    check_encoder("hyperconformer_22M 4x10s", enc.cpu(), _oracle_states(fx, g), g["abs_len"], ENC_BAR)
+    check_greedy("hyperconformer_22M", pred.cpu(), score.cpu(), g["greedy_tokens"], g["greedy_margin"], g["greedy_chosen_lp"])
+    check_alone_vs_batch(lambda w, ln: eng.encode_wav(w.to(dev), ln.to(dev)), wav, lens, 1e-5)
 
 
 def test_hyperconformer_short_utterance(dev, fx):
     s = fx["short"]
     eng = _engine(fx, dev, parts=("fbank", "cnn", "encoder"))
-    wav, lens = _wav(s)
+    wav, lens = case_wav(s)
     enc = eng.encode_wav(wav.to(dev), lens.to(dev)).cpu()
     assert enc.shape == s["enc_out"].shape
-    _check_encoder("hyperconformer_22M short", enc, s["enc_out"], torch.tensor([enc.shape[1]]))
+    check_encoder("hyperconformer_22M short", enc, s["enc_out"], torch.tensor([enc.shape[1]]), ENC_BAR)
 
 
 def test_hyperconformer_beam10_lm_ctc(dev, fx):
     """The recipe's test search (beam 10, [TransformerLM 0.6, CTC 0.4], temperature 1.15) on the reference's encoder states,
-    judged like test_gpu_bench_shapes.py::test_bench_shape_beam10: best scores and every rank of the n-best within 3e-2; a
+    judged by parity.check_beam: best scores and every rank of the n-best within 3e-2; a
     different best hypothesis only where the oracle, walked along our tokens, scores it within 3e-2 of ours and no worse
     than the reference's best."""
     import bench
     from oracle import asr_oracle as O
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
-    from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M, seeded_state_dict
+    from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M
     g, gb = fx["main"], fx["main"]["beam"]
     sd = _state(fx)
     asr = bench.build_product_asr(HYPERCONFORMER_22M, sd, dev, decoder="beam", beam=gb["kwargs"]["beam_size"], lm=True, ctc=True)
     bs = asr.mods["decoder"]
     bs.max_decode_ratio, bs.min_decode_ratio = gb["max_decode_ratio"], 0.0
     bs.return_topk, bs.topk = True, gb["kwargs"]["beam_size"]
-    ref_enc = _reference_states(fx, g)
+    ref_enc = _oracle_states(fx, g)
     lens = g["wav_lens"]
     hyps, hlens, scores, _ = bs(ref_enc.to(dev), lens.to(dev))
-    hyps, hlens, scores = hyps.cpu(), hlens.cpu(), scores.cpu()
-    B, L = hyps.shape[0], hyps.shape[2]
-    ref_h, ref_len, ref_s = gb["hyps"].long(), gb["lens"], gb["scores"]
-    tol, diverged = 3e-2, []
-    for b in range(B):
-        n = int(torch.round(hlens[b, 0] * L)) + 1
-        n_ref = int(torch.round(ref_len[b, 0] * ref_h.shape[2])) + 1
-        ours, ref = hyps[b, 0, :n].tolist(), ref_h[b, 0, :n_ref].tolist()
-        assert abs(float(scores[b, 0]) - float(ref_s[b, 0])) < tol, f"best score {float(scores[b, 0])} vs {float(ref_s[b, 0])}"
-        if ours != ref:
-            diverged.append((b, ours))
-    k = min(scores.shape[1], ref_s.shape[1])
-    nbest_err = (scores[:, :k] - ref_s[:, :k]).abs().max().item()
-    print(f"beam10 lm+ctc: best scores {scores[:, 0].tolist()} ref {ref_s[:, 0].tolist()}; identical best hypothesis for "
-          f"{B - len(diverged)}/{B}; max |n-best score - reference| {nbest_err:.2e}")
-    assert nbest_err < tol
-    if diverged:
-        lm_m = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                             dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-        lm = dict(sd=seeded_state_dict(lm_m, seed=1), cfg=dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072,
-                                                               activation="gelu"), weight=0.6, temperature=1.15)
-        ctc = dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4, blank_index=0)
-        idx = [b for b, _ in diverged]
+
+    @torch.no_grad()
+    def rescore_forced(idx, tokens):
         kw = {k_: v for k_, v in gb["kwargs"].items() if k_ != "beam_size"}
-        with torch.no_grad():
-            o = O.beam_search(ref_enc[idx], lens[idx], sd, dict(HYPERCONFORMER_22M), sd["seq_lin.w.weight"],
-                              sd["seq_lin.w.bias"], 1, 2, beam_size=1, prefix="Transformer.", lm=lm, ctc=ctc,
-                              forced=[t for _, t in diverged], **kw)
-        for (b, toks), osc in zip(diverged, o.tolist()):
-            print(f"   utterance {b}: ours scores {float(scores[b, 0]):.5f}, oracle {osc:.5f}; reference best {float(ref_s[b, 0]):.5f}")
-            assert abs(osc - float(scores[b, 0])) < tol and osc > float(ref_s[b, 0]) - tol
+        ctc = dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4, blank_index=0)
+        return O.beam_search(ref_enc[idx], lens[idx], sd, dict(HYPERCONFORMER_22M), sd["seq_lin.w.weight"], sd["seq_lin.w.bias"],
+                             1, 2, beam_size=1, prefix="Transformer.", lm=oracle_lm(0.6, 1.15), ctc=ctc, forced=tokens, **kw)
+    check_beam("beam10 lm+ctc", best_tokens(hyps, hlens), scores, best_tokens(gb["hyps"].long(), gb["lens"]), gb["scores"],
+               rescore_forced)
 
 
 def test_group_host_entry_matches_device(dev, fx):
@@ -283,12 +213,12 @@ def test_load_state_dict_after_first_use(dev, fx):
     from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M
     cfg = dict(HYPERCONFORMER_22M, num_encoder_layers=2, num_decoder_layers=1)
     asr = bench.build_product_asr(cfg, _state(fx), dev)
-    wav, lens = _wav(fx["short"])
+    wav, lens = case_wav(fx["short"])
     before = asr.encode_batch(wav.to(dev), lens.to(dev)).cpu()
     sd2 = _state(fx, gain=0.7)
     tr = asr.transformer
     tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd2.items() if k.startswith("Transformer.")}, strict=False)
     after = asr.encode_batch(wav.to(dev), lens.to(dev)).cpu()
     fresh = bench.build_product_asr(cfg, sd2, dev).encode_batch(wav.to(dev), lens.to(dev)).cpu()
-    print(f"load_state_dict: change {_rel(after, before):.2e}, vs a fresh engine max abs {float((after - fresh).abs().max()):.2e}")
-    assert _rel(after, before) > 1e-2 and torch.equal(after, fresh)
+    print(f"load_state_dict: change {rel(after, before):.2e}, vs a fresh engine max abs {float((after - fresh).abs().max()):.2e}")
+    assert rel(after, before) > 1e-2 and torch.equal(after, fresh)

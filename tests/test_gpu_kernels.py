@@ -1,24 +1,17 @@
 """-m gpu parity tests: every CUDA path is called through the C ABI (libsbk.so) and compared with the
 CPU oracle / the committed reference goldens on the same seeded inputs."""
 import os
+import sys
 
 import pytest
 import torch
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import check_greedy, dev, lm_scorer, rel  # noqa: E402,F401
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 pytestmark = pytest.mark.gpu
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 # ------------------------------------------------------------------------------------------- wgmma GEMM
@@ -151,7 +144,7 @@ def test_conformer_small_encoder_golden(dev):
     eng, sd = _engine(cfg, dev, parts=("cnn", "encoder"))
     cnn_shape = (g["cnn_out"].shape[0], g["cnn_out"].shape[1], -1)
     enc = eng.encode_from_cnn(g["cnn_out"].reshape(cnn_shape).to(dev), g["wav_lens"].to(dev)).cpu()
-    r = _rel(enc, g["enc_out"])
+    r = rel(enc, g["enc_out"])
     print(f"[conformer_small_relpos] encoder rel-L2 err {r:.3e} max abs {(enc - g['enc_out']).abs().max():.3e}")
     assert r < 1e-3
 
@@ -174,7 +167,7 @@ def test_model_stages_golden(dev, tag):
     print(f"[{tag}] cnn max abs err {e:.3e} (ref absmax {ref_cnn.abs().max():.2f})")
     assert e < 5e-3
     enc = eng.encode_from_cnn(g["cnn_out"].reshape(cnn.shape).to(dev), g["wav_lens"].to(dev)).cpu()
-    r = _rel(enc, g["enc_out"])
+    r = rel(enc, g["enc_out"])
     print(f"[{tag}] encoder rel-L2 err {r:.3e} max abs {(enc - g['enc_out']).abs().max():.3e}")
     assert r < 1e-3
     n_steps = g["greedy_logits"].shape[1]
@@ -186,17 +179,8 @@ def test_model_stages_golden(dev, tag):
     for tc_rows, name in ((1 << 30, "skinny"), (1, "wgmma")):
         eng.set_decoder_tc_min_rows(tc_rows)
         pred, score, lp, done = eng.greedy_from_enc(g["enc_out"].to(dev), g["wav_lens"].to(dev), n_steps, 1, 2, want_log_probs=True)
-        pred = pred.cpu()
-        worst = 0.0
-        for b in range(pred.shape[0]):
-            for s in range(n_steps):
-                if pred[b, s] != ref_tok[b, s]:
-                    assert margin[b, s] < 5e-3, f"[{name}] token mismatch at b={b} s={s} with margin {margin[b, s]}"
-                    break
-                d = (lp[b, s].cpu() - ref_lp[b, s]).abs().max().item()
-                worst = max(worst, d)
-                assert d < 2e-2, f"[{name}] log-prob err {d} at b={b} s={s}"
-        print(f"[{tag}] greedy[{name}] tokens {pred.tolist()} ref {g['hyps']} max log-prob err {worst:.2e}")
+        print(f"[{tag}] greedy[{name}] tokens {pred.tolist()} ref {g['hyps']}")
+        check_greedy(f"{tag}/{name}", pred.cpu(), lp.cpu(), ref_tok, margin, ref_lp)
 
 
 @pytest.mark.parametrize("n_mels", [90, 96, 4])
@@ -227,7 +211,7 @@ def test_transcribe_end_to_end(dev):
     eng, sd = _engine(cfg, dev)
     n_steps = g["greedy_logits"].shape[1]
     pred, score, enc, done = eng.transcribe_greedy_dev(g["wav"].to(dev), g["wav_lens"].to(dev), n_steps, 1, 2, want_enc=True)
-    r = _rel(enc.cpu(), g["enc_out"])
+    r = rel(enc.cpu(), g["enc_out"])
     print("e2e encoder rel-L2", r, "tokens", pred.cpu().tolist(), "ref", g["hyps"])
     assert r < 1.5e-3
     pred_h, done_h = eng.transcribe_greedy_host(g["wav"].pin_memory(), g["wav_lens"], n_steps, 1, 2)
@@ -294,7 +278,7 @@ def test_full_size_properties(dev):
     assert torch.isfinite(enc).all()
     for i in (0, 17, 31):
         p1, _, e1, _ = eng.transcribe_greedy_dev(wav[i:i + 1].contiguous(), ones[:1], steps, 1, 2, want_enc=True)
-        assert _rel(e1[0].cpu(), enc[i].cpu()) < 1e-5, f"encoder states of utterance {i} depend on the batch"
+        assert rel(e1[0].cpu(), enc[i].cpu()) < 1e-5, f"encoder states of utterance {i} depend on the batch"
         assert torch.equal(p1[0], pred[i]), f"tokens of utterance {i} depend on the batch"
     # decode coalescing == separate calls
     wav_b = torch.randn(B, L, generator=g).to(dev)
@@ -329,9 +313,8 @@ def test_beam_search_with_transformerlm_scorer_golden(dev, case):
     from speechbrain_b200.decoders.scorer import ScorerBuilder, TransformerLMScorer
     from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
     from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
     from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state, seeded_state_dict
+    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_lm_conformer_large_rope.pt"))[case]
     sd = seeded_asr_state(dict(CONFORMER_LARGE), 0)
@@ -343,9 +326,7 @@ def test_beam_search_with_transformerlm_scorer_golden(dev, case):
     bias = sd["seq_lin.w.bias"].clone()
     bias[2] += gb["eos_bias"]
     lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
-    lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072, dropout=0.0,
-                       activation=torch.nn.GELU, normalize_before=False)
-    lm.load_state_dict(seeded_state_dict(lm, seed=1))
+    lm = lm_scorer()
     scorer = ScorerBuilder(full_scorers=[TransformerLMScorer(language_model=lm, temperature=gb["lm_temperature"])],
                            weights={"transformerlm": gb["lm_weight"]})
     bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, max_decode_ratio=gb["max_decode_ratio"],
@@ -365,9 +346,8 @@ def test_beam_search_with_ctc_scorer_golden(dev, case):
     from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
     from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
     from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
     from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state, seeded_state_dict
+    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_ctc_conformer_large_rope.pt"))[case]
     sd = seeded_asr_state(dict(CONFORMER_LARGE), 0)
@@ -383,9 +363,7 @@ def test_beam_search_with_ctc_scorer_golden(dev, case):
     ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
     ctc_scorer = CTCScorer(eos_index=2, blank_index=0, ctc_fc=ctc_lin)
     if gb["with_lm"]:
-        lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                           dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-        lm.load_state_dict(seeded_state_dict(lm, seed=1))
+        lm = lm_scorer()
         scorer = ScorerBuilder(full_scorers=[TransformerLMScorer(language_model=lm, temperature=gb["lm_temperature"]), ctc_scorer],
                                weights={"transformerlm": gb["lm_weight"], "ctc": gb["ctc_weight"]})
     else:
@@ -429,12 +407,8 @@ def test_lm_rescorer_golden(dev):
     rescoring: LM scores within 5e-2 of sums of up to 24 log-probs (|score| ~ 35..200), identical re-ranking."""
     from oracle.asr_oracle import StubTokenizer
     from speechbrain_b200.decoders.scorer import RescorerBuilder, TransformerLMRescorer
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
-    from speechbrain_b200.utils.seeded_init import seeded_state_dict
     gb = torch.load(os.path.join(GOLDEN, "lm_rescore.pt"))
-    lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072, dropout=0.0,
-                       activation=torch.nn.GELU, normalize_before=False)
-    lm.load_state_dict(seeded_state_dict(lm, seed=1))
+    lm = lm_scorer()
     resc = TransformerLMRescorer(language_model=lm, tokenizer=StubTokenizer(), device=dev, temperature=gb["temperature"],
                                  bos_index=1, eos_index=2, pad_index=0)
     scores = resc.rescore_hyps(gb["hyps"]).cpu()

@@ -3,24 +3,21 @@ engine's KV-cached step path (position by position, and summed as AsrEngine.lm_r
 properties.  Logits are compared on every position, pad positions included, and some batches hold id 0 inside the valid
 length: the key-padding mask removes keys that real positions would otherwise see."""
 import os
+import sys
 
 import pytest
 import torch
 
 from oracle import asr_oracle as O
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev  # noqa: E402,F401
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 pytestmark = pytest.mark.gpu
 
 CFG = dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 def _lm(act="gelu", seed=1):

@@ -5,21 +5,15 @@ rel-L2 (same maths; the chunk's keys are grouped into other 64-key blocks, so th
 A finite-context stream's per-chunk work does not grow with its length (equal kernel-launch counts at chunks 5 and 60, and
 a chunk past max_length frames equal to a fresh stream fed only that chunk's receptive field).  Reruns, reset and a stream
 inside a batch are bit-identical."""
+import os
 import pytest
+import sys
 import torch
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import dev, rel  # noqa: E402,F401
+
 pytestmark = pytest.mark.gpu
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 _MODELS = {}
@@ -59,8 +53,8 @@ def test_streaming_equals_masked(dev, base, att, cs, lc, B):
     dc = DynChunkTrainConfig(cs, lc)
     full = tr.encode(src, None, dynchunktrain_config=dc)
     out, ctx = _stream(tr, src, dc)
-    r = _rel(out.cpu(), full.cpu())
-    per_chunk = max(_rel(out[:, t:t + cs].cpu(), full[:, t:t + cs].cpu()) for t in range(0, T, cs))
+    r = rel(out.cpu(), full.cpu())
+    per_chunk = max(rel(out[:, t:t + cs].cpu(), full[:, t:t + cs].cpu()) for t in range(0, T, cs))
     print(f"[stream {base} {att} ({cs}, {lc}) B={B}] rel vs masked {r:.2e}, worst chunk {per_chunk:.2e}")
     assert out.shape == full.shape and r < 3e-4 and per_chunk < 6e-4
     layer = ctx.encoder_context.layers[0]
@@ -95,7 +89,7 @@ def test_cache_cost_is_constant(dev):
     R = 8
     first = n_chunks - 1 - R
     fresh, _ = _stream(tr, src[:, first * cs:].contiguous(), dc)
-    r = _rel(fresh[:, -cs:].cpu(), outs[-1].cpu())
+    r = rel(fresh[:, -cs:].cpu(), outs[-1].cpu())
     print(f"[stream cost] chunk {n_chunks - 1} (frames {(n_chunks - 1) * cs}..) vs a fresh stream over its receptive field: {r:.2e}")
     assert r < 3e-4
 
@@ -186,7 +180,7 @@ def test_rope_ring_write_far_into_a_stream(dev, pos0):
         blk = qkv.double().view(n, H, 3, dh)[:, h]
         ref = (rotate(blk[:, 0], win) * scale) @ rotate(blk[:, 1], win).T
         got = qh[:, h] @ ring[:, h, 0].T
-        worst = max(worst, _rel(got, ref))
+        worst = max(worst, rel(got, ref))
         assert torch.equal(ring[:, h, 1], blk[:, 2].half().double())  # values pass through
     print(f"[ring write pos0={pos0}] scores vs window-local float64 rotation: rel {worst:.2e}")
     assert worst < 1e-3
@@ -213,8 +207,8 @@ def test_encoder_vs_reference_golden(dev, name):
     worst = 0.0
     for k, t in enumerate(range(0, T, g["chunk"])):
         out = tr.encode_streaming(src[:, t:t + g["chunk"]].contiguous(), ctx).cpu()
-        worst = max(worst, _rel(out.double().norm(dim=-1), g["frame_norms"][k]))
+        worst = max(worst, rel(out.double().norm(dim=-1), g["frame_norms"][k]))
         if k == g["full_chunk_index"]:
-            full = _rel(out, g["full_chunk"])
+            full = rel(out, g["full_chunk"])
     print(f"[golden {name}] worst chunk frame-norm rel {worst:.2e}; chunk {g['full_chunk_index']} rel-L2 {full:.2e}")
     assert worst < 1e-3 and full < 1e-3

@@ -10,6 +10,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import transducer_oracle as TO  # noqa: E402
+from parity import normalizer_ckpt, write_pretrained_dir  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -366,12 +367,7 @@ def test_from_hparams_local_directory_matches_direct_construction(tmp_path):
     mods, parts = _transducer_modules(sd, w_enc, W)
     order = ["CNN", "Transformer", "proj_enc", "emb", "dec", "proj_dec", "transducer_lin"]
     ck = {f"{i}.{k}": v for i, n in enumerate(order) for k, v in parts[n].state_dict().items()}
-    tmp = str(tmp_path)
-    torch.save(ck, os.path.join(tmp, "asr.ckpt"))
-    torch.save({"count": 1, "glob_mean": sd["normalize.glob_mean"], "glob_std": sd["normalize.glob_std"]},
-               os.path.join(tmp, "normalizer.ckpt"))
-    with open(os.path.join(tmp, "hyperparams.yaml"), "w") as f:
-        f.write(HPARAMS.replace("<save_dir>", tmp))
+    tmp = write_pretrained_dir(tmp_path, HPARAMS, dict(asr=ck, normalizer=normalizer_ckpt(sd)))
     loaded = EncoderDecoderASR.from_hparams(source=tmp, run_opts={"device": "cuda:0"})
     assert isinstance(loaded.mods["decoder"], TransducerBeamSearcher) and loaded.transducer_beam_search
     direct = EncoderDecoderASR(modules=mods, hparams={"tokenizer": None, "transducer_beam_search": True},

@@ -6,8 +6,8 @@ beam-10 test search with the CTC and TransformerLM scorers (the lineage-indexed 
 from_hparams round trip of the recipe's module layout.
 
 Front-end bar: rel-L2 <= 5e-4 (3.0e-4 measured: fp16 act1 and block-2 operands).  Encoder bar: rel-L2 <= 1e-3 (the
-Conformer's).  Greedy: tokens identical up to the first decision whose reference top-1/top-2 margin is below 5e-3 (the rule
-of test_gpu_bench_shapes.py).  Beam: hypotheses identical, scores within 5e-2 (the rule of test_gpu_kernels.py's CTC+LM
+Conformer's).  Greedy: tokens identical up to the first decision whose reference top-1/top-2 margin is below 5e-3
+(parity.check_greedy; the fixture keeps no chosen log-probs).  Beam: hypotheses identical, scores within 5e-2 (the rule of test_gpu_kernels.py's CTC+LM
 beam test)."""
 import os
 import sys
@@ -16,19 +16,14 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import (case_wav, check_alone_vs_batch, check_encoder, check_greedy, check_summary, dev,  # noqa: E402,F401
+                    lm_scorer, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir)
 import transformer_oracle as TO  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 ENC_BAR = 1e-3
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")
@@ -40,20 +35,6 @@ def fx():
 def sd(fx):
     from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE, seeded_asr_state
     return seeded_asr_state(TRANSFORMER_LARGE, fx["weight_seed"])
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
-
-
-def _wav(case):
-    B, L = case["wav_shape"]
-    g = torch.Generator().manual_seed(case["wav_seed"])
-    wav = torch.randn(B, L, generator=g)
-    lens = case["wav_lens"]
-    for b in range(B):
-        wav[b, int(round(float(lens[b]) * L)):] = 0
-    return wav, lens
 
 
 def _front_end(sd, dev):
@@ -73,7 +54,7 @@ def test_front_end_kernel_vs_oracle(dev, sd, B, T0):
     feats = torch.randn(B, T0, 80, generator=g) * 2.0
     out = cnn(feats.to(dev)).cpu()
     ref = TO.cnn3(feats, sd)
-    err = _rel(out, ref)
+    err = rel(out, ref)
     print(f"front-end B={B} T0={T0} -> {tuple(out.shape)}: rel-L2 {err:.2e}, max abs {(out - ref).abs().max():.2e}")
     assert out.shape == ref.shape and torch.isfinite(out).all() and err <= 5e-4
     assert torch.equal(out, cnn(feats.to(dev)).cpu())
@@ -96,39 +77,18 @@ def _engine(sd, dev, parts=("fbank", "cnn", "encoder", "decoder")):
 def test_transformer_large_encoder_and_greedy(dev, fx, sd):
     from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE as cfg
     g = fx["large"]
-    wav, lens = _wav(g)
+    wav, lens = case_wav(g)
     with torch.no_grad():
         ref = TO.encode(TO.wav_to_cnn(wav, lens, sd, cfg), lens, sd, cfg)
-    idx = g["enc"]["sample_idx"].long()
-    assert _rel(ref[idx[:, 0], idx[:, 1]], g["enc"]["sample_rows"]) <= 1e-5
+    check_summary("transformer_large oracle", ref, g["enc"]["frame_norm"], g["enc"]["sample_idx"], g["enc"]["sample_rows"], 1e-5)
     eng = _engine(sd, dev)
     S = g["greedy_tokens"].shape[1]
     pred, score, enc, done = eng.transcribe_greedy_dev(wav.to(dev), lens.to(dev), S, 1, 2, want_enc=True)
     torch.cuda.synchronize()
-    enc = enc.cpu()
-    abs_len = g["abs_len"]
-    r_all = _rel(enc, ref)
-    per = [_rel(enc[b, :int(abs_len[b])], ref[b, :int(abs_len[b])]) for b in range(enc.shape[0])]
-    print(f"[transformer_large] encoder rel-L2 {r_all:.3e} (valid frames {['%.2e' % x for x in per]})")
-    assert torch.isfinite(enc).all() and r_all <= ENC_BAR and max(per) <= ENC_BAR
-    pred = pred.cpu()
-    ref_tok, margin = g["greedy_tokens"], g["greedy_margin"]
-    compared, stops = 0, []
-    for b in range(ref_tok.shape[0]):
-        for s in range(S):
-            if int(pred[b, s]) != int(ref_tok[b, s]):
-                assert float(margin[b, s]) < 5e-3, f"token mismatch at b={b} s={s}, reference margin {float(margin[b, s]):.4f}"
-                stops.append((b, s))
-                break
-            compared += 1
-    print(f"[transformer_large] greedy: {compared}/{ref_tok.numel()} decisions identical, near-tie stops {stops}")
-    # batch independence: utterance 0 (relative length 1.0, so the same T) alone and in the padded batch
-    enc_b = eng.encode_wav(wav.to(dev), lens.to(dev)).cpu()
-    enc_1 = eng.encode_wav(wav[:1].to(dev), lens[:1].to(dev)).cpu()
-    assert torch.equal(enc_b, eng.encode_wav(wav.to(dev), lens.to(dev)).cpu())
-    d = float((enc_1[0] - enc_b[0]).abs().max())
-    print(f"[transformer_large] utterance alone vs in the batch: max abs {d:.2e}")
-    assert d <= 1e-5
+    check_encoder("transformer_large", enc.cpu(), ref, g["abs_len"], ENC_BAR)
+    # the fixture keeps no chosen log-probs: tokens only
+    check_greedy("transformer_large", pred.cpu(), None, g["greedy_tokens"], g["greedy_margin"], chosen_lp=None)
+    check_alone_vs_batch(lambda w, ln: eng.encode_wav(w.to(dev), ln.to(dev)), wav, lens, 1e-5)
 
 
 def _transformer(sd):
@@ -159,28 +119,23 @@ def test_head_dim_128_decoder_attention_teacher_forced(dev, sd, n):
     out, _ = tr.to(dev).decode(tgt.to(dev), enc.to(dev), enc_len.to(dev))
     ref = O.decode(tgt, enc, enc_len, sd, cfg, "Transformer.")
     ref = ref[0] if isinstance(ref, tuple) else ref
-    err = _rel(out.cpu(), ref)
+    err = rel(out.cpu(), ref)
     print(f"decode head_dim 128: rel-L2 {err:.2e}")
     assert torch.isfinite(out).all() and err <= 2e-3
 
 
 
-def _asr_modules(sd, dev, beam, max_decode_ratio, lm_sd=None, lm_shape=(768, 12, 12, 3072)):
+def _asr_modules(sd, dev, beam, max_decode_ratio, lm):
     """The recipe's modules as this package's mirrors, wired like transformer.yaml's test search (beam, temperature 1.15,
     no EOS threshold, CTC 0.4 + TransformerLM 0.6)."""
     from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
     from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
     from speechbrain_b200.nnet.linear import Linear
     tr = _transformer(sd)
     V = sd["seq_lin.w.weight"].shape[0]
     seq_lin, ctc_lin = Linear(input_size=512, n_neurons=V), Linear(input_size=512, n_neurons=V)
     seq_lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": sd["seq_lin.w.bias"]})
     ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    d, h, L, f = lm_shape
-    lm = TransformerLM(vocab=V, d_model=d, nhead=h, num_encoder_layers=L, num_decoder_layers=0, d_ffn=f, dropout=0.0,
-                       activation=torch.nn.GELU, normalize_before=False)
-    lm.load_state_dict(lm_sd)
     scorer = ScorerBuilder(full_scorers=[CTCScorer(eos_index=2, blank_index=0, ctc_fc=ctc_lin),
                                          TransformerLMScorer(language_model=lm, temperature=1.15)],
                            weights={"ctc": 0.4, "transformerlm": 0.6})
@@ -193,16 +148,13 @@ def _asr_modules(sd, dev, beam, max_decode_ratio, lm_sd=None, lm_shape=(768, 12,
 def test_beam10_ctc_lm_matches_reference(dev, fx, sd):
     """The recipe's test search at beam 10 (40 live hypotheses: the beam step's lineage-indexed self-attention and the
     cross-attention at head width 128) on the reference's encoder states, recomputed by the oracle."""
-    from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE as cfg, seeded_state_dict
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
+    from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE as cfg
     g, gb = fx["large"], fx["beam10"]
-    wav, lens = _wav(g)
+    wav, lens = case_wav(g)
     with torch.no_grad():
         enc = TO.encode(TO.wav_to_cnn(wav, lens, sd, cfg), lens, sd, cfg)
-    lm_sd = seeded_state_dict(TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0,
-                                            d_ffn=3072, dropout=0.0, activation=torch.nn.GELU, normalize_before=False),
-                              seed=gb["lm_seed"])
-    _, bs = _asr_modules(sd, dev, gb["kwargs"]["beam_size"], gb["max_decode_ratio"], lm_sd)
+    assert gb["lm_seed"] == 1
+    _, bs = _asr_modules(sd, dev, gb["kwargs"]["beam_size"], gb["max_decode_ratio"], lm_scorer())
     hyps, _, scores, _ = bs(enc.to(dev), lens.to(dev))
     print(f"[transformer_large beam10 ctc+lm] hyps equal {hyps == gb['hyps']}; score err "
           f"{(scores.cpu() - gb['scores']).abs().max():.2e}")
@@ -321,20 +273,13 @@ def test_from_hparams_local_directory_round_trip(dev, fx, sd, tmp_path):
     from speechbrain_b200.nnet.containers import LengthsCapableSequential
     from speechbrain_b200.processing.features import InputNormalization
     from speechbrain_b200.utils.seeded_init import seeded_state_dict
-    tmp = str(tmp_path)
-    prefix = {"CNN.": "0.", "Transformer.": "1.", "seq_lin.": "2.", "ctc_lin.": "3."}
-    ck = {q + k[len(p):]: v for k, v in sd.items() for p, q in prefix.items() if k.startswith(p)}
-    torch.save(ck, os.path.join(tmp, "asr.ckpt"))
-    lm_sd = seeded_state_dict(TransformerLM(vocab=5000, d_model=128, nhead=2, num_encoder_layers=2, num_decoder_layers=0,
-                                            d_ffn=256, dropout=0.0, activation=torch.nn.GELU, normalize_before=False), seed=1)
-    torch.save(lm_sd, os.path.join(tmp, "lm.ckpt"))
-    torch.save({"count": 1, "glob_mean": sd["normalize.glob_mean"], "glob_std": sd["normalize.glob_std"]},
-               os.path.join(tmp, "normalizer.ckpt"))
-    with open(os.path.join(tmp, "hyperparams.yaml"), "w") as f:
-        f.write(HPARAMS.replace("<save_dir>", tmp))
+    lm = TransformerLM(vocab=5000, d_model=128, nhead=2, num_encoder_layers=2, num_decoder_layers=0, d_ffn=256, dropout=0.0,
+                       activation=torch.nn.GELU, normalize_before=False)
+    lm.load_state_dict(seeded_state_dict(lm, seed=1))
+    tmp = write_pretrained_dir(tmp_path, HPARAMS, dict(asr=module_list_ckpt(sd), lm=lm.state_dict(), normalizer=normalizer_ckpt(sd)))
     loaded = EncoderDecoderASR.from_hparams(source=tmp, run_opts={"device": str(dev)})
     # direct construction of the same layout
-    tr, bs = _asr_modules(sd, dev, 10, 0.05, lm_sd, lm_shape=(128, 2, 2, 256))
+    tr, bs = _asr_modules(sd, dev, 10, 0.05, lm)
     norm = InputNormalization(norm_type="global")
     norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
     norm.eval()
@@ -343,7 +288,7 @@ def test_from_hparams_local_directory_round_trip(dev, fx, sd, tmp_path):
     direct = EncoderDecoderASR(modules=dict(encoder=enc, transformer=tr, decoder=bs),
                                hparams=dict(tokenizer=None, transformer_beam_search=True), run_opts={"device": str(dev)})
     assert torch.equal(loaded.mods["decoder"].fc.w.weight.cpu(), sd["seq_lin.w.weight"])
-    wav, lens = _wav(fx["large"])
+    wav, lens = case_wav(fx["large"])
     w1, t1 = loaded.transcribe_batch(wav, lens)
     w2, t2 = direct.transcribe_batch(wav, lens)
     print("from_hparams tokens", t1)

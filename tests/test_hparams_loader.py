@@ -3,9 +3,13 @@ the way speechbrain/asr-conformer-transformerlm-librispeech writes it -- ``speec
 ``pretrainer`` with loadables -- is loaded from a LOCAL directory into this package's mirrors, the checkpoints land in the
 modules, and (GPU test) the interface transcribes like the directly constructed one."""
 import os
+import sys
 
 import pytest
 import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import module_list_ckpt, normalizer_ckpt, write_pretrained_dir  # noqa: E402
 
 YAML = """
 # Feature parameters
@@ -138,15 +142,6 @@ def _make_dir(tmp, n_enc=1, n_dec=1, vocab=60, max_ratio=0.2):
     from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     cfg = dict(CONFORMER_LARGE, num_encoder_layers=n_enc, num_decoder_layers=n_dec, vocab=vocab)
     sd = seeded_asr_state(cfg, 0)
-    prefix = {"CNN.": "0.", "Transformer.": "1.", "seq_lin.": "2.", "ctc_lin.": "3."}
-    ck = {}
-    for k, v in sd.items():
-        for p, q in prefix.items():
-            if k.startswith(p):
-                ck[q + k[len(p):]] = v
-    torch.save(ck, os.path.join(tmp, "asr.ckpt"))
-    torch.save({"count": 1, "glob_mean": sd["normalize.glob_mean"], "glob_std": sd["normalize.glob_std"]},
-               os.path.join(tmp, "normalizer.ckpt"))
     txt = os.path.join(tmp, "corpus.txt")
     with open(txt, "w") as f:
         words = ["speech", "brain", "blackwell", "tensor", "memory", "conformer", "encoder", "decoder", "beam", "search", "greedy",
@@ -156,8 +151,8 @@ def _make_dir(tmp, n_enc=1, n_dec=1, vocab=60, max_ratio=0.2):
     spm.SentencePieceTrainer.train(input=txt, model_prefix=os.path.join(tmp, "tok"), vocab_size=vocab, model_type="bpe",
                                    bos_id=1, eos_id=2, unk_id=0, pad_id=-1, minloglevel=2)
     os.rename(os.path.join(tmp, "tok.model"), os.path.join(tmp, "tokenizer.ckpt"))
-    with open(os.path.join(tmp, "hyperparams.yaml"), "w") as f:
-        f.write(YAML.format(n_enc=n_enc, n_dec=n_dec, vocab=vocab, max_ratio=max_ratio).replace("<save_dir>", tmp))
+    write_pretrained_dir(tmp, YAML.format(n_enc=n_enc, n_dec=n_dec, vocab=vocab, max_ratio=max_ratio),
+                         dict(asr=module_list_ckpt(sd), normalizer=normalizer_ckpt(sd)))
     return cfg, sd
 
 

@@ -10,13 +10,10 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import case_wav, check_summary, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir  # noqa: E402
 import hyperconformer_oracle as HO  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
 
 
 @pytest.fixture(scope="module")
@@ -29,34 +26,19 @@ def _state(fx):
     return scale_hypernet(seeded_asr_state(HYPERCONFORMER_22M, fx["weight_seed"]), fx["hypernet_gain"])
 
 
-def _wav(case):
-    B, L = case["wav_shape"]
-    g = torch.Generator().manual_seed(case["wav_seed"])
-    wav = torch.randn(B, L, generator=g)
-    for b in range(B):
-        wav[b, int(round(float(case["wav_lens"][b]) * L)):] = 0
-    assert abs(float(wav.double().abs().sum()) - case["wav_checksum"]) / case["wav_checksum"] < 1e-9
-    return wav, case["wav_lens"]
-
-
-def _summary_err(enc, case):
-    """rel-L2 of the per-frame norms of every frame and of the sampled full rows against the reference's."""
-    idx = case["sample_idx"].long()
-    return _rel(enc.double().norm(dim=-1), case["frame_norm"]), _rel(enc[idx[:, 0], idx[:, 1]], case["sample_rows"])
-
-
 def test_oracle_matches_reference(fx):
     """Frame norms and the full short-utterance states to 1e-6; the sampled full rows to 2e-6 (fp32 summation-order noise of
     individual channels: 1.2e-6 against the reference's einsum / bmm order)."""
     from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M
     sd = _state(fx)
     with torch.no_grad():
-        enc = HO.wav_to_states(*_wav(fx["main"]), sd, HYPERCONFORMER_22M)
-        short = HO.wav_to_states(*_wav(fx["short"]), sd, HYPERCONFORMER_22M)
-    r_norm, r_rows = _summary_err(enc, fx["main"])
-    r_short = _rel(short, fx["short"]["enc_out"])
-    print(f"oracle vs reference: frame norms {r_norm:.2e}, sampled rows {r_rows:.2e}, short utterance {r_short:.2e}")
-    assert r_norm <= 1e-6 and r_rows <= 2e-6 and r_short <= 1e-6
+        enc = HO.wav_to_states(*case_wav(fx["main"]), sd, HYPERCONFORMER_22M)
+        short = HO.wav_to_states(*case_wav(fx["short"]), sd, HYPERCONFORMER_22M)
+    m = fx["main"]
+    r_norm, _ = check_summary("hyperconformer_22M oracle", enc, m["frame_norm"], m["sample_idx"], m["sample_rows"], 2e-6)
+    r_short = rel(short, fx["short"]["enc_out"])
+    print(f"oracle vs reference: short utterance {r_short:.2e}")
+    assert r_norm <= 1e-6 and r_short <= 1e-6
 
 
 def _mirror(**kw):
@@ -259,14 +241,9 @@ def test_from_hparams_hyperconformer_recipe_layout(tmp_path):
 
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
     from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M, seeded_asr_state
-    tmp = str(tmp_path)
     cfg = dict(HYPERCONFORMER_22M, num_encoder_layers=2, num_decoder_layers=1, vocab=60)
     sd = seeded_asr_state(cfg, 0)
-    prefix = {"CNN.": "0.", "Transformer.": "1.", "seq_lin.": "2.", "ctc_lin.": "3."}
-    torch.save({q + k[len(p):]: v for k, v in sd.items() for p, q in prefix.items() if k.startswith(p)},
-               os.path.join(tmp, "asr.ckpt"))
-    torch.save({"count": 1, "glob_mean": sd["normalize.glob_mean"], "glob_std": sd["normalize.glob_std"]},
-               os.path.join(tmp, "normalizer.ckpt"))
+    tmp = write_pretrained_dir(tmp_path, YAML, dict(asr=module_list_ckpt(sd), normalizer=normalizer_ckpt(sd)))
     with open(os.path.join(tmp, "corpus.txt"), "w") as f:
         words = ["hyper", "mixing", "token", "conformer", "linear", "time", "network", "weights", "encoder", "decoder"]
         for i in range(400):
@@ -274,8 +251,6 @@ def test_from_hparams_hyperconformer_recipe_layout(tmp_path):
     spm.SentencePieceTrainer.train(input=os.path.join(tmp, "corpus.txt"), model_prefix=os.path.join(tmp, "tok"), vocab_size=60,
                                    model_type="bpe", bos_id=1, eos_id=2, unk_id=0, pad_id=-1, minloglevel=2)
     os.rename(os.path.join(tmp, "tok.model"), os.path.join(tmp, "tokenizer.ckpt"))
-    with open(os.path.join(tmp, "hyperparams.yaml"), "w") as f:
-        f.write(YAML.replace("<save_dir>", tmp))
     asr = EncoderDecoderASR.from_hparams(source=tmp, run_opts={"device": "cuda:0"})
     tr = asr.transformer
     assert tr.attention_type == "hypermixing" and asr.mods["decoder"].model is tr
@@ -295,11 +270,11 @@ def test_fp16_operand_error_estimate(fx):
     from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M
     sd = _state(fx)
     with torch.no_grad():
-        enc = HO.wav_to_states(*_wav(fx["main"]), sd, HYPERCONFORMER_22M, q=lambda t: t.half().float())
-        ref = HO.wav_to_states(*_wav(fx["main"]), sd, HYPERCONFORMER_22M)
+        enc = HO.wav_to_states(*case_wav(fx["main"]), sd, HYPERCONFORMER_22M, q=lambda t: t.half().float())
+        ref = HO.wav_to_states(*case_wav(fx["main"]), sd, HYPERCONFORMER_22M)
     lens = fx["main"]["abs_len"]
-    per_utt = [_rel(enc[b, :int(lens[b])], ref[b, :int(lens[b])]) for b in range(ref.shape[0])]
-    r = _rel(enc, ref)
+    per_utt = [rel(enc[b, :int(lens[b])], ref[b, :int(lens[b])]) for b in range(ref.shape[0])]
+    r = rel(enc, ref)
     print(f"fp16-operand oracle vs reference: encoder rel-L2 {r:.2e}, valid frames per utterance "
           f"{['%.2e' % x for x in per_utt]}")
     assert r <= 4e-3 and max(per_utt) <= 5.5e-3

@@ -9,6 +9,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from parity import case_wav, check_summary, rel  # noqa: E402
 import transformer_oracle as TO  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -19,42 +20,20 @@ def fx():
     return torch.load(os.path.join(GOLDEN, "transformer.pt"))
 
 
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
-
-
-def _wav(case):
-    B, L = case["wav_shape"]
-    g = torch.Generator().manual_seed(case["wav_seed"])
-    wav = torch.randn(B, L, generator=g)
-    lens = case.get("wav_lens", torch.ones(B))
-    for b in range(B):
-        wav[b, int(round(float(lens[b]) * L)):] = 0
-    return wav, lens
-
-
-def _check(x, summ):
-    B, T = x.shape[:2]
-    x = x.reshape(B, T, -1)
-    idx = summ["sample_idx"].long()
-    return max(_rel(x.double().norm(dim=-1), summ["frame_norm"]), _rel(x[idx[:, 0], idx[:, 1]], summ["sample_rows"]))
-
-
 def test_oracle_equals_reference(fx):
     from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE as cfg, seeded_asr_state
     sd = seeded_asr_state(cfg, fx["weight_seed"])
     g = fx["large"]
-    wav, lens = _wav(g)
-    assert abs(float(wav.double().abs().sum()) - g["wav_checksum"]) / g["wav_checksum"] < 1e-9
+    wav, lens = case_wav(g)
     with torch.no_grad():
         cnn = TO.wav_to_cnn(wav, lens, sd, cfg)
         enc = TO.encode(cnn, lens, sd, cfg)
     assert cnn.shape == (4, 251, 20, 64) and enc.shape == (4, 251, 512)
-    assert _check(cnn, g["cnn"]) <= 1e-5
-    assert _check(enc, g["enc"]) <= 1e-5
+    for name, x in (("cnn", cnn.flatten(2)), ("enc", enc)):
+        check_summary(f"transformer_large oracle {name}", x, g[name]["frame_norm"], g[name]["sample_idx"], g[name]["sample_rows"], 1e-5)
     s = fx["short"]
-    w5, l5 = _wav(s)
-    assert _rel(TO.wav_to_cnn(w5, l5, sd, cfg), s["cnn"]) <= 1e-5
+    w5, l5 = case_wav(s)
+    assert rel(TO.wav_to_cnn(w5, l5, sd, cfg), s["cnn"]) <= 1e-5
 
 
 def test_state_dict_keys_match_reference(fx):
