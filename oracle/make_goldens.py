@@ -1,28 +1,17 @@
-"""Generate tests/golden/*.pt by RUNNING THE REFERENCE (build container only).
+"""Generate tests/golden/*.pt of the Conformer recipes by RUNNING THE REFERENCE (how to run it: oracle/goldens.py).
 
-TEST INFRASTRUCTURE. Usage (needs /root/reference and a 2-function hyperpyyaml stub):
-
-    mkdir -p /tmp/stub && printf 'def resolve_references(*a,**k): raise RuntimeError\\n'\\
-        'def load_hyperpyyaml(*a,**k): raise RuntimeError\\n' > /tmp/stub/hyperpyyaml.py
-    PYTHONPATH=/tmp/stub:/root/reference:/root/repo python oracle/make_goldens.py
-
-For every case it (1) builds the reference modules with the recipe's kwargs
-(recipes/LibriSpeech/ASR/transformer/hparams/conformer_{large,small}.yaml), (2) loads
-seeded weights (speechbrain_b200.utils.seeded_init -- regenerated, not stored),
-(3) runs the reference on seeded inputs, (4) checks oracle/asr_oracle.py against
-it, and (5) stores inputs + reference outputs as small fixtures.
+TEST INFRASTRUCTURE.  For every case it (1) builds the reference modules with the recipe's kwargs
+(recipes/LibriSpeech/ASR/transformer/hparams/conformer_{large,small}.yaml), (2) loads seeded weights
+(speechbrain_b200.utils.seeded_init -- regenerated, not stored), (3) runs the reference on seeded inputs, (4) checks
+oracle/asr_oracle.py against it, and (5) stores inputs + reference outputs as small fixtures.
 """
-import os
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-from oracle import asr_oracle as O  # noqa: E402
-from speechbrain_b200.utils.seeded_init import seeded_asr_state, seeded_state_dict  # noqa: E402
-
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+from oracle import asr_oracle as O
+from oracle import goldens as G
+from speechbrain_b200.utils.seeded_init import seeded_asr_state
 
 CFG_L = dict(name="conformer_large", d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=6,
              d_ffn=2048, vocab=5000, n_fft=512, win_length=32, n_mels=80, kernel_size=31,
@@ -32,47 +21,18 @@ CFG_S = dict(name="conformer_small", d_model=144, nhead=4, num_encoder_layers=12
              cnn_channels=(64, 32), input_size=640)
 
 
-def _product_cfg(cfg, attention_type):
+def weight_checksum(cfg, attention_type):
+    """sum of |w| over the product's seeded state of the recipe (pins the seeded weights the tests regenerate)"""
     from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, CONFORMER_SMALL
     base = CONFORMER_LARGE if cfg["name"] == "conformer_large" else CONFORMER_SMALL
-    return dict(base, attention_type=attention_type)
+    state = seeded_asr_state(dict(base, attention_type=attention_type), 0)
+    return float(sum(v.double().abs().sum() for k, v in sorted(state.items())))
 
 
-def rel(a, b):
-    return float((a - b).norm() / b.norm().clamp_min(1e-30))
-
-
-def build_reference(cfg, attention_type):
-    import speechbrain  # noqa: F401
-    from speechbrain.lobes.features import Fbank
-    from speechbrain.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain.nnet.linear import Linear
-    from speechbrain.processing.features import InputNormalization
-
-    fb = Fbank(n_fft=cfg["n_fft"], n_mels=cfg["n_mels"], win_length=cfg["win_length"])
-    norm = InputNormalization(norm_type="global", update_until_epoch=4)
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=2, num_layers_per_block=1,
-                              out_channels=cfg["cnn_channels"], kernel_sizes=(3, 3), strides=(2, 2),
-                              residuals=(False, False))
-    tr = TransformerASR(input_size=cfg["input_size"], tgt_vocab=cfg["vocab"], d_model=cfg["d_model"],
-                        nhead=cfg["nhead"], num_encoder_layers=cfg["num_encoder_layers"],
-                        num_decoder_layers=cfg["num_decoder_layers"], d_ffn=cfg["d_ffn"], dropout=0.1,
-                        activation=torch.nn.GELU, encoder_module="conformer", attention_type=attention_type,
-                        normalize_before=True, causal=False)
-    seq_lin = Linear(input_size=cfg["d_model"], n_neurons=cfg["vocab"])
-    ctc_lin = Linear(input_size=cfg["d_model"], n_neurons=cfg["vocab"])
-    mods = torch.nn.ModuleDict(dict(CNN=cnn, Transformer=tr, seq_lin=seq_lin, ctc_lin=ctc_lin))
-    sd = seeded_state_dict(mods, seed=0)
-    mods.load_state_dict(sd)
-    mods.eval()
-    from speechbrain_b200.utils.seeded_init import seeded_tensor
-    norm.glob_mean = seeded_tensor(0, "normalize.glob_mean", (cfg["n_mels"],)) * 3.0 - 20.0
-    norm.glob_std = seeded_tensor(0, "normalize.glob_std", (cfg["n_mels"],)) * 8.0
-    norm.count = 1
-    norm.eval()
-    sd["normalize.glob_mean"], sd["normalize.glob_std"] = norm.glob_mean, norm.glob_std
-    return fb, norm, mods, sd
+def rope_case():
+    """the reference of conformer_large with RoPE and the encoder states of conformer_large_rope.pt"""
+    g = G.load("conformer_large_rope.pt")
+    return G.build_reference(CFG_L, "RoPEMHA"), g["enc_out"], g["wav_lens"]
 
 
 def fbank_cases():
@@ -98,7 +58,7 @@ def fbank_cases():
     # all-zero utterance: amin clamp + top_db
     wav = torch.zeros(1, 1600)
     out["zeros"] = dict(kwargs=dict(n_fft=400, n_mels=80), wav=wav, out=Fbank(n_fft=400, n_mels=80)(wav))
-    torch.save(out, os.path.join(OUT, "fbank.pt"))
+    G.save(out, "fbank.pt")
 
 
 def norm_cases():
@@ -125,108 +85,62 @@ def norm_cases():
     kat = InputNormalization(norm_type="sentence").eval()(torch.tensor([[[1.0], [3.0], [0.0], [0.0], [0.0]]]),
                                                             torch.tensor([0.4]))
     out["kat"] = kat
-    torch.save(out, os.path.join(OUT, "input_norm.pt"))
+    G.save(out, "input_norm.pt")
 
 
 def model_case(cfg, attention_type, B, L, lens, n_steps, tag):
-    from speechbrain.decoders.seq2seq import S2STransformerGreedySearcher
-    fb, norm, mods, sd = build_reference(cfg, attention_type)
-    g = torch.Generator().manual_seed(1234)
-    wav = torch.randn(B, L, generator=g)
-    wav_lens = torch.tensor(lens)
-    for b in range(B):
-        wav[b, int(round(lens[b] * L)):] = 0
-    ocfg = dict(cfg, attention_type=attention_type)
+    ref = G.build_reference(cfg, attention_type)
+    sd, mods = ref.sd, ref.mods
+    wav, wav_lens, _ = G.wav_case(1234, B, L, lens)
     with torch.no_grad():
-        f = fb(wav)
-        fn = norm(f, wav_lens)
+        f = ref.fb(wav)
+        fn = ref.norm(f, wav_lens)
         c = mods["CNN"](fn)
         enc = mods["Transformer"].encode(c, wav_lens)
         T = enc.shape[1]
-        gs = S2STransformerGreedySearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                          min_decode_ratio=0.0, max_decode_ratio=(n_steps + 0.5) / T)
-        hyps, top_len, top_scores, top_lp = gs(enc, wav_lens)
+        hyps, logits = G.greedy_case(ref, enc, wav_lens, n_steps, tag)
         ctc_logits = mods["ctc_lin"](enc)
         # oracle checks
         of = O.fbank(wav, n_fft=cfg["n_fft"], n_mels=cfg["n_mels"], win_length_ms=cfg["win_length"])
         ofn = O.input_norm(of, wav_lens, "global", sd["normalize.glob_mean"], sd["normalize.glob_std"])
         oc = O.cnn_frontend(fn, sd, "CNN.")
-        oenc, olayers = O.encode(c, wav_lens, sd, ocfg, "Transformer.", return_layers=True)
-        ohyps, olen, oscores, olp, ologits = O.greedy_search(
-            enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], sd["seq_lin.w.bias"], 1, 2, 0.0,
-            (n_steps + 0.5) / T, "Transformer.", return_logits=True)
+        oenc, olayers = O.encode(c, wav_lens, sd, ref.cfg, "Transformer.", return_layers=True)
     print(f"[{tag}] fbank err {(of - f).abs().max():.2e}  norm err {(ofn - fn).abs().max():.2e} "
-          f"cnn err {(oc - c).abs().max():.2e}  enc rel {rel(oenc, enc):.2e}  "
-          f"greedy equal {ohyps == hyps} lp err {(olp - top_lp).abs().max():.2e}")
-    assert (oc - c).abs().max() < 1e-4 and rel(oenc, enc) < 1e-5 and ohyps == hyps
-    logits = ologits
+          f"cnn err {(oc - c).abs().max():.2e}  enc rel {G.rel(oenc, enc):.2e}")
+    assert (oc - c).abs().max() < 1e-4 and G.rel(oenc, enc) < 1e-5
     top2 = logits.topk(2, dim=-1).values
     print(f"   T={T} steps={logits.shape[1]} min top1-top2 margin {float((top2[..., 0] - top2[..., 1]).min()):.4f}")
-    gold = dict(cfg=ocfg, wav=wav, wav_lens=wav_lens, fbank=f, cnn_out=c, enc_out=enc,
+    gold = dict(cfg=dict(cfg, attention_type=attention_type), wav=wav, wav_lens=wav_lens, fbank=f, cnn_out=c, enc_out=enc,
                 enc_layer0=olayers[0], enc_layer5=olayers[5], hyps=hyps, greedy_logits=logits,
-                ctc_logits_head=ctc_logits[:, :, :64].clone(),
-                weight_checksum=float(sum(v.double().abs().sum() for k, v in sorted(seeded_asr_state(_product_cfg(cfg, attention_type), 0).items()))))
-    torch.save(gold, os.path.join(OUT, f"{tag}.pt"))
+                ctc_logits_head=ctc_logits[:, :, :64].clone(), weight_checksum=weight_checksum(cfg, attention_type))
+    G.save(gold, f"{tag}.pt")
 
 
 def beam_case(tag="beam_conformer_large_rope"):
-    """S2STransformerBeamSearcher (no scorer) on the conformer_large_rope golden's encoder states.  seq_lin's EOS
-    bias is raised so that EOS hypotheses actually finish (random weights never emit EOS otherwise)."""
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
+    """S2STransformerBeamSearcher (no scorer) on the conformer_large_rope golden's encoder states."""
+    ref, enc, wav_lens = rope_case()
     T = enc.shape[1]
     out = {}
-    for name, kw, eos_bias in [("thr_on", dict(beam_size=4, using_eos_threshold=True, temperature=1.0), 4.0),
-                               ("recipe", dict(beam_size=5, using_eos_threshold=False, temperature=1.15, min_decode_ratio=2.5 / T), 5.5),
-                               ("no_eos", dict(beam_size=3, using_eos_threshold=False, length_normalization=False), 0.0)]:
-        with torch.no_grad():
-            bias = sd["seq_lin.w.bias"].clone()
-            bias[2] += eos_bias
-            mods["seq_lin"].w.bias.copy_(bias)
-            kwargs = dict(kw)
-            kwargs.setdefault("min_decode_ratio", 0.0)
-            bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                            max_decode_ratio=8.5 / T, **kwargs)
-            hyps, lens, scores, lp = bs(enc, wav_lens)
-            ocfg = dict(CFG_L, attention_type="RoPEMHA")
-            okw = dict(kwargs)
-            ohyps, olens, oscores, olp = O.beam_search(enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], bias, 1, 2,
-                                                       max_decode_ratio=8.5 / T, prefix="Transformer.", **okw)
-        print(f"[beam {name}] ref hyps {hyps} scores {scores.tolist()} | oracle equal: {ohyps == hyps} "
-              f"score err {(oscores - scores).abs().max():.2e} lp err {(olp - lp).abs().max():.2e}")
-        assert ohyps == hyps and (oscores - scores).abs().max() < 1e-4
-        out[name] = dict(kwargs=kwargs, eos_bias=eos_bias, max_decode_ratio=8.5 / T, hyps=hyps, lens=lens, scores=scores, log_probs=lp)
-    torch.save(out, os.path.join(OUT, f"{tag}.pt"))
+    for name, kwargs, eos_bias in [
+            ("thr_on", dict(beam_size=4, using_eos_threshold=True, temperature=1.0, min_decode_ratio=0.0), 4.0),
+            ("recipe", dict(beam_size=5, using_eos_threshold=False, temperature=1.15, min_decode_ratio=2.5 / T), 5.5),
+            ("no_eos", dict(beam_size=3, using_eos_threshold=False, length_normalization=False, min_decode_ratio=0.0), 0.0)]:
+        hyps, lens, scores, lp = G.run_beam(ref, enc, wav_lens, kwargs, 8.5 / T, eos_bias, tag=f"beam {name}")
+        out[name] = dict(kwargs=kwargs, eos_bias=eos_bias, max_decode_ratio=8.5 / T, hyps=hyps, lens=lens, scores=scores,
+                         log_probs=lp)
+    G.save(out, f"{tag}.pt")
 
 
 def beam_topk_case(tag="beam_topk_conformer_large_rope"):
     """return_topk=True, topk=3 (the n-best output the rescorers consume): padded (B, topk, L) hypotheses, lengths, scores and
     log-probs of the reference vs the oracle."""
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
+    ref, enc, wav_lens = rope_case()
     T = enc.shape[1]
     kwargs = dict(beam_size=5, using_eos_threshold=False, temperature=1.15, min_decode_ratio=2.5 / T)
     eos_bias = 5.5
-    with torch.no_grad():
-        bias = sd["seq_lin.w.bias"].clone()
-        bias[2] += eos_bias
-        mods["seq_lin"].w.bias.copy_(bias)
-        bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                        max_decode_ratio=8.5 / T, return_topk=True, topk=3, **kwargs)
-        tk_hyps, tk_len, tk_scores, tk_lp = bs(enc, wav_lens)
-        ocfg = dict(CFG_L, attention_type="RoPEMHA")
-        o_hyps, o_len, o_scores, o_lp = O.beam_search(enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], bias, 1, 2,
-                                                      max_decode_ratio=8.5 / T, prefix="Transformer.", topk=3,
-                                                      return_topk=True, **kwargs)
-    print(f"[beam topk] ref hyps {tk_hyps.tolist()} scores {tk_scores.tolist()} | oracle equal: {torch.equal(o_hyps, tk_hyps)} "
-          f"score err {(o_scores - tk_scores).abs().max():.2e}")
-    assert torch.equal(o_hyps, tk_hyps) and torch.allclose(o_len, tk_len) and (o_scores - tk_scores).abs().max() < 1e-4
-    torch.save(dict(kwargs=kwargs, eos_bias=eos_bias, max_decode_ratio=8.5 / T, topk=3, hyps=tk_hyps, lens=tk_len,
-                    scores=tk_scores, log_probs=tk_lp), os.path.join(OUT, f"{tag}.pt"))
+    hyps, lens, scores, lp = G.run_beam(ref, enc, wav_lens, kwargs, 8.5 / T, eos_bias, topk=3, tag="beam topk")
+    G.save(dict(kwargs=kwargs, eos_bias=eos_bias, max_decode_ratio=8.5 / T, topk=3, hyps=hyps, lens=lens, scores=scores,
+                log_probs=lp), f"{tag}.pt")
 
 
 def rescore_case(tag="lm_rescore"):
@@ -235,13 +149,7 @@ def rescore_case(tag="lm_rescore"):
     import copy
 
     from speechbrain.decoders.scorer import RescorerBuilder, TransformerLMRescorer
-    from speechbrain.lobes.models.transformer.TransformerLM import TransformerLM
-    lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                       dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-    sd_lm = seeded_state_dict(lm, seed=1)
-    lm.load_state_dict(sd_lm)
-    lm.eval()
-    cfg_lm = dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072, activation="gelu")
+    lm, sd_lm = G.reference_lm()
     tok = O.StubTokenizer()
     hyps = [["hello world", "hello word", "yellow world peace"], ["a b", "abc", "the cat sat on the mat"]]
     scores = [[-1.0, -1.2, -1.5], [-0.3, -0.35, -0.4]]
@@ -249,140 +157,89 @@ def rescore_case(tag="lm_rescore"):
                                  pad_index=0)
     with torch.no_grad():
         ref = resc.rescore_hyps(hyps)
-        ours = O.lm_rescore_hyps(hyps, tok, sd_lm, cfg_lm, 1.15, 1, 2, 0)
+        ours = O.lm_rescore_hyps(hyps, tok, sd_lm, G.CFG_LM, 1.15, 1, 2, 0)
         rb = RescorerBuilder(weights={"transformerlm": 0.5}, rescorers=[resc])
         out_c, out_s = rb.rescore(hyps, copy.deepcopy(scores))
     o_c, o_s = O.rescorer_builder_rescore(hyps, scores, ours, 0.5)
     print(f"[rescore] ref {ref.tolist()} oracle err {(ours - ref).abs().max():.2e}; reranked {out_c} equal: {o_c == out_c}")
     assert (ours - ref).abs().max() < 1e-3 and o_c == out_c
-    torch.save(dict(hyps=hyps, scores=scores, temperature=1.15, weight=0.5, lm_scores=ref, out_candidates=out_c, out_scores=out_s),
-               os.path.join(OUT, f"{tag}.pt"))
+    G.save(dict(hyps=hyps, scores=scores, temperature=1.15, weight=0.5, lm_scores=ref, out_candidates=out_c, out_scores=out_s),
+           f"{tag}.pt")
 
 
 def beam_len_case(tag="beam_len_conformer_large_rope"):
     """ScorerBuilder(full_scorers=[LengthScorer]) (length reward, no length normalisation): with the reward the search keeps
     longer hypotheses than without it."""
-    from speechbrain.decoders.scorer import LengthScorer, ScorerBuilder
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
+    ref, enc, wav_lens = rope_case()
     T = enc.shape[1]
     kwargs = dict(beam_size=4, using_eos_threshold=False, temperature=1.0, min_decode_ratio=0.0, length_normalization=False)
     eos_bias, w_len = 4.0, 8.3
-    with torch.no_grad():
-        bias = sd["seq_lin.w.bias"].clone()
-        bias[2] += eos_bias
-        mods["seq_lin"].w.bias.copy_(bias)
-        res = {}
-        for name, scorer in (("off", None), ("on", ScorerBuilder(full_scorers=[LengthScorer(5000)], weights={"length": w_len}))):
-            bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                            max_decode_ratio=8.5 / T, scorer=scorer, **kwargs)
-            res[name] = bs(enc, wav_lens)
-        ocfg = dict(CFG_L, attention_type="RoPEMHA")
-        ohyps, olens, oscores, olp = O.beam_search(enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], bias, 1, 2,
-                                                   max_decode_ratio=8.5 / T, prefix="Transformer.", length_weight=w_len, **kwargs)
-    hyps, lens, scores, lp = res["on"]
-    print(f"[beam len] without {res['off'][0]} with {hyps} scores {scores.tolist()} | oracle equal: {ohyps == hyps} "
-          f"score err {(oscores - scores).abs().max():.2e}")
-    assert ohyps == hyps and (oscores - scores).abs().max() < 1e-4 and res["off"][0] != hyps
-    torch.save(dict(kwargs=kwargs, eos_bias=eos_bias, length_weight=w_len, max_decode_ratio=8.5 / T, hyps=hyps, lens=lens,
-                    scores=scores, log_probs=lp, hyps_without=res["off"][0]), os.path.join(OUT, f"{tag}.pt"))
+    without = G.run_beam(ref, enc, wav_lens, kwargs, 8.5 / T, eos_bias, check=False)[0]
+    hyps, lens, scores, lp = G.run_beam(ref, enc, wav_lens, kwargs, 8.5 / T, eos_bias, scorers={"length": w_len},
+                                        tag="beam len")
+    print(f"[beam len] without {without} with {hyps}")
+    assert without != hyps
+    G.save(dict(kwargs=kwargs, eos_bias=eos_bias, length_weight=w_len, max_decode_ratio=8.5 / T, hyps=hyps, lens=lens,
+                scores=scores, log_probs=lp, hyps_without=without), f"{tag}.pt")
 
 
 def beam_lm_case(tag="beam_lm_conformer_large_rope"):
     """S2STransformerBeamSearcher + ScorerBuilder(full_scorers=[TransformerLMScorer]) -- shallow fusion with the recipe's
     12 x 768 TransformerLM (conformer_large.yaml:160-170, 215-223), weight 0.6, temperature 1.15."""
-    from speechbrain.decoders.scorer import ScorerBuilder, TransformerLMScorer
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain.lobes.models.transformer.TransformerLM import TransformerLM
     from speechbrain_b200.utils.shapes import transformer_lm_shapes
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
+    ref, enc, wav_lens = rope_case()
     T = enc.shape[1]
-    lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                       dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-    sd_lm = seeded_state_dict(lm, seed=1)
-    lm.load_state_dict(sd_lm)
-    lm.eval()
+    lm = G.reference_lm()
     ours = {k: tuple(v) for k, v in transformer_lm_shapes(5000).items()}
-    ref_shapes = {k: tuple(v.shape) for k, v in lm.state_dict().items() if not k.endswith(".pe")}
+    ref_shapes = {k: tuple(v.shape) for k, v in lm[0].state_dict().items() if not k.endswith(".pe")}
     assert ours == ref_shapes, (set(ours) ^ set(ref_shapes))
-    cfg_lm = dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072, activation="gelu")
     out = {}
-    for name, kw, eos_bias in [("lm_recipe", dict(beam_size=4, using_eos_threshold=False, temperature=1.15), 0.0),
-                               ("lm_eos", dict(beam_size=3, using_eos_threshold=True, temperature=1.0, min_decode_ratio=1.5 / T), 9.0)]:
-        with torch.no_grad():
-            bias = sd["seq_lin.w.bias"].clone()
-            bias[2] += eos_bias
-            mods["seq_lin"].w.bias.copy_(bias)
-            kwargs = dict(kw)
-            kwargs.setdefault("min_decode_ratio", 0.0)
-            scorer = ScorerBuilder(full_scorers=[TransformerLMScorer(language_model=lm, temperature=1.15)],
-                                   weights={"transformerlm": 0.6})
-            bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                            max_decode_ratio=6.5 / T, scorer=scorer, **kwargs)
-            hyps, lens, scores, lp = bs(enc, wav_lens)
-            ocfg = dict(CFG_L, attention_type="RoPEMHA")
-            ohyps, olens, oscores, olp = O.beam_search(
-                enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], bias, 1, 2, max_decode_ratio=6.5 / T, prefix="Transformer.",
-                lm=dict(sd=sd_lm, cfg=cfg_lm, weight=0.6, temperature=1.15), **kwargs)
-        print(f"[beam+lm {name}] ref hyps {hyps} scores {scores.tolist()} | oracle equal: {ohyps == hyps} "
-              f"score err {(oscores - scores).abs().max():.2e}")
-        assert ohyps == hyps and (oscores - scores).abs().max() < 1e-4
+    for name, kwargs, eos_bias in [
+            ("lm_recipe", dict(beam_size=4, using_eos_threshold=False, temperature=1.15, min_decode_ratio=0.0), 0.0),
+            ("lm_eos", dict(beam_size=3, using_eos_threshold=True, temperature=1.0, min_decode_ratio=1.5 / T), 9.0)]:
+        hyps, lens, scores, lp = G.run_beam(ref, enc, wav_lens, kwargs, 6.5 / T, eos_bias, scorers={"transformerlm": 0.6},
+                                            lm=lm, tag=f"beam+lm {name}")
         out[name] = dict(kwargs=kwargs, eos_bias=eos_bias, max_decode_ratio=6.5 / T, lm_weight=0.6, lm_temperature=1.15,
                          hyps=hyps, lens=lens, scores=scores, log_probs=lp)
-    torch.save(out, os.path.join(OUT, f"{tag}.pt"))
+    G.save(out, f"{tag}.pt")
+
+
+def scorers(with_lm, with_ctc):
+    """the recipe's full scorers (conformer_large.yaml:209-228): TransformerLM 0.6 and / or CTC 0.4, in its order"""
+    return dict(([("transformerlm", 0.6)] if with_lm else []) + ([("ctc", 0.4)] if with_ctc else []))
 
 
 def beam_ctc_case(tag="beam_ctc_conformer_large_rope"):
     """Joint CTC/attention decoding: ScorerBuilder(full_scorers=[TransformerLMScorer, CTCScorer]) (the recipe's test search,
     conformer_large.yaml:209-223: lm 0.60, ctc 0.40) and full_scorers=[CTCScorer] (the valid search, :225-228)."""
-    from speechbrain.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain.lobes.models.transformer.TransformerLM import TransformerLM
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
+    ref, enc, wav_lens = rope_case()
     T = enc.shape[1]
-    lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                       dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-    sd_lm = seeded_state_dict(lm, seed=1)
-    lm.load_state_dict(sd_lm)
-    lm.eval()
-    cfg_lm = dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072, activation="gelu")
+    lm = G.reference_lm()
     out = {}
-    cases = [("ctc_lm_test", True, dict(beam_size=4, using_eos_threshold=False, temperature=1.15), 0.0, 10.5),
-             ("ctc_valid", False, dict(beam_size=5, using_eos_threshold=False, temperature=1.15), 0.0, 10.5),
-             ("ctc_eos", False, dict(beam_size=3, using_eos_threshold=True, temperature=1.0, min_decode_ratio=1.5 / T), 9.0, 8.5)]
-    for name, with_lm, kw, eos_bias, steps in cases:
-        with torch.no_grad():
-            bias = sd["seq_lin.w.bias"].clone()
-            bias[2] += eos_bias
-            mods["seq_lin"].w.bias.copy_(bias)
-            kwargs = dict(kw)
-            kwargs.setdefault("min_decode_ratio", 0.0)
-            ctc_scorer = CTCScorer(eos_index=2, blank_index=0, ctc_fc=mods["ctc_lin"])
-            if with_lm:
-                scorer = ScorerBuilder(full_scorers=[TransformerLMScorer(language_model=lm, temperature=1.15), ctc_scorer],
-                                       weights={"transformerlm": 0.6, "ctc": 0.4})
-            else:
-                scorer = ScorerBuilder(full_scorers=[ctc_scorer], weights={"ctc": 0.4})
-            bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                            max_decode_ratio=steps / T, scorer=scorer, **kwargs)
-            hyps, lens, scores, lp = bs(enc, wav_lens)
-            ocfg = dict(CFG_L, attention_type="RoPEMHA")
-            ohyps, olens, oscores, olp = O.beam_search(
-                enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], bias, 1, 2, max_decode_ratio=steps / T, prefix="Transformer.",
-                lm=dict(sd=sd_lm, cfg=cfg_lm, weight=0.6, temperature=1.15) if with_lm else None,
-                ctc=dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4, blank_index=0), **kwargs)
-        print(f"[beam+ctc {name}] ref hyps {hyps} scores {scores.tolist()} | oracle equal: {ohyps == hyps} "
-              f"score err {(oscores - scores).abs().max():.2e} lp err {(olp - lp).abs().max():.2e}")
-        assert ohyps == hyps and (oscores - scores).abs().max() < 1e-3
+    for name, with_lm, kwargs, eos_bias, steps in [
+            ("ctc_lm_test", True, dict(beam_size=4, using_eos_threshold=False, temperature=1.15, min_decode_ratio=0.0), 0.0,
+             10.5),
+            ("ctc_valid", False, dict(beam_size=5, using_eos_threshold=False, temperature=1.15, min_decode_ratio=0.0), 0.0,
+             10.5),
+            ("ctc_eos", False, dict(beam_size=3, using_eos_threshold=True, temperature=1.0, min_decode_ratio=1.5 / T), 9.0,
+             8.5)]:
+        hyps, lens, scores, lp = G.run_beam(ref, enc, wav_lens, kwargs, steps / T, eos_bias, scorers=scorers(with_lm, True),
+                                            lm=lm, bar=1e-3, tag=f"beam+ctc {name}")
         out[name] = dict(kwargs=kwargs, eos_bias=eos_bias, max_decode_ratio=steps / T, with_lm=with_lm, lm_weight=0.6,
                          lm_temperature=1.15, ctc_weight=0.4, hyps=hyps, lens=lens, scores=scores, log_probs=lp)
-    torch.save(out, os.path.join(OUT, f"{tag}.pt"))
+    G.save(out, f"{tag}.pt")
+
+
+def bench_beam(ref, enc, wav_lens, kwargs, steps, eos_bias, tag, with_lm=False, with_ctc=False, lm=None, **record):
+    """A bench-shape beam case: the n-best of all beam_size hypotheses, best hypothesis and every score checked against
+    the oracle (1e-3); its fixture record"""
+    T, beam = enc.shape[1], kwargs["beam_size"]
+    hyps, lens, scores, lp = G.run_beam(ref, enc, wav_lens, kwargs, (steps + 0.5) / T, eos_bias,
+                                        scorers=scorers(with_lm, with_ctc), lm=lm, topk=beam, bar=1e-3, rank0=True, tag=tag)
+    print(f"   best lens {(lens[:, 0] * hyps.shape[2]).round().int().tolist()} max len {hyps.shape[2]}; "
+          f"top1-top2 score gap {(scores[:, 0] - scores[:, 1]).tolist()}")
+    return dict(kwargs=kwargs, with_lm=with_lm, with_ctc=with_ctc, eos_bias=eos_bias, max_decode_ratio=(steps + 0.5) / T,
+                **record, hyps=hyps.int(), lens=lens, scores=scores, log_probs=lp)
 
 
 def bench_shape_case(cfg, attention_type, B, L, lens, n_greedy, tag, beams=(), seed=4321):
@@ -390,133 +247,54 @@ def bench_shape_case(cfg, attention_type, B, L, lens, n_greedy, tag, beams=(), s
     lengths so that one trailing key block is partially and one fully masked, 48 greedy steps (KV-cache positions 0..47),
     beam = 10 with the recipe's scorers.  The waveform is regenerated from ``seed`` by the test (a checksum pins it); stored:
     reference enc_out (fp32), greedy tokens / chosen log-probs / top-2 margins, beam n-best (all `beam` hypotheses + scores)."""
-    from speechbrain.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher, S2STransformerGreedySearcher
-    from speechbrain.lobes.models.transformer.TransformerLM import TransformerLM
-    import time
-    fb, norm, mods, sd = build_reference(cfg, attention_type)
-    g = torch.Generator().manual_seed(seed)
-    wav = torch.randn(B, L, generator=g)
-    wav_lens = torch.tensor(lens)
-    for b in range(B):
-        wav[b, int(round(lens[b] * L)):] = 0
-    ocfg = dict(cfg, attention_type=attention_type)
-    gold = dict(cfg=ocfg, wav_seed=seed, wav_shape=(B, L), wav_lens=wav_lens, wav_checksum=float(wav.double().abs().sum()),
-                weight_checksum=float(sum(v.double().abs().sum() for k, v in sorted(seeded_asr_state(_product_cfg(cfg, attention_type), 0).items()))))
+    ref = G.build_reference(cfg, attention_type)
+    wav, wav_lens, record = G.wav_case(seed, B, L, lens)
+    gold = dict(cfg=dict(cfg, attention_type=attention_type), **record,
+                weight_checksum=weight_checksum(cfg, attention_type))
     with torch.no_grad():
-        t0 = time.time()
-        fn = norm(fb(wav), wav_lens)
-        c = mods["CNN"](fn)
-        enc = mods["Transformer"].encode(c, wav_lens)
+        enc = ref.encode(wav, wav_lens)
         T = enc.shape[1]
-        oc = O.full_pipeline_features(wav, wav_lens, sd, dict(cfg))
-        oenc = O.encode(oc, wav_lens, sd, ocfg, "Transformer.")
-        print(f"[{tag}] T={T} encoder: reference {time.time() - t0:.1f}s; oracle rel {rel(oenc, enc):.2e}")
-        assert rel(oenc, enc) < 1e-5
-        gold["enc_out"] = enc.clone()
-        gold["abs_len"] = torch.round(wav_lens * T).int()
-        if n_greedy > 0:
-            t0 = time.time()
-            gs = S2STransformerGreedySearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                              min_decode_ratio=0.0, max_decode_ratio=(n_greedy + 0.5) / T)
-            hyps, top_len, top_scores, top_lp = gs(enc, wav_lens)
-            ohyps, olen, oscores, olp, ologits = O.greedy_search(
-                enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], sd["seq_lin.w.bias"], 1, 2, 0.0,
-                (n_greedy + 0.5) / T, "Transformer.", return_logits=True)
-            assert ohyps == hyps, "oracle greedy != reference greedy"
-            top2 = ologits.topk(2, dim=-1).values
-            lp = torch.log_softmax(ologits, -1)
-            tok = ologits.argmax(-1)
-            gold.update(greedy_hyps=hyps, greedy_tokens=tok.int(), greedy_margin=(top2[..., 0] - top2[..., 1]).clone(),
-                        greedy_chosen_lp=lp.gather(-1, tok.unsqueeze(-1)).squeeze(-1).clone(),
-                        greedy_lp_sample=lp[:, :, :128].clone().half())
-            print(f"[{tag}] greedy {n_greedy} steps {time.time() - t0:.1f}s  min margin {float(gold['greedy_margin'].min()):.4f} "
-                  f"lens {[len(h) for h in hyps]}")
-        lm = None
-        for name, kw in beams:
-            kw = dict(kw)
-            t0 = time.time()
-            with_lm, with_ctc, eos_bias, steps = kw.pop("with_lm"), kw.pop("with_ctc"), kw.pop("eos_bias"), kw.pop("steps")
-            if with_lm and lm is None:
-                lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                                   dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-                sd_lm = seeded_state_dict(lm, seed=1)
-                lm.load_state_dict(sd_lm)
-                lm.eval()
-            cfg_lm = dict(d_model=768, nhead=12, num_encoder_layers=12, d_ffn=3072, activation="gelu")
-            bias = sd["seq_lin.w.bias"].clone()
-            bias[2] += eos_bias
-            mods["seq_lin"].w.bias.copy_(bias)
-            full, weights = [], {}
-            if with_lm:
-                full.append(TransformerLMScorer(language_model=lm, temperature=1.15)); weights["transformerlm"] = 0.6
-            if with_ctc:
-                full.append(CTCScorer(eos_index=2, blank_index=0, ctc_fc=mods["ctc_lin"])); weights["ctc"] = 0.4
-            scorer = ScorerBuilder(full_scorers=full, weights=weights) if full else None
-            kw.setdefault("min_decode_ratio", 0.0)
-            beam = kw["beam_size"]
-            bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                            max_decode_ratio=(steps + 0.5) / T, scorer=scorer, return_topk=True, topk=beam, **kw)
-            tk_hyps, tk_len, tk_scores, tk_lp = bs(enc, wav_lens)
-            t_ref = time.time() - t0
-            o_hyps, o_len, o_scores, o_lp = O.beam_search(
-                enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], bias, 1, 2, max_decode_ratio=(steps + 0.5) / T,
-                prefix="Transformer.", topk=beam, return_topk=True,
-                lm=dict(sd=sd_lm, cfg=cfg_lm, weight=0.6, temperature=1.15) if with_lm else None,
-                ctc=dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4, blank_index=0) if with_ctc else None, **kw)
-            print(f"[{tag} beam {name}] reference {t_ref:.1f}s; best lens {(tk_len[:, 0] * tk_hyps.shape[2]).round().int().tolist()} "
-                  f"scores {tk_scores[:, 0].tolist()}; oracle hyps equal {torch.equal(o_hyps, tk_hyps)} "
-                  f"score err {(o_scores - tk_scores).abs().max():.2e}; top1-top2 score gap {(tk_scores[:, 0] - tk_scores[:, 1]).tolist()}")
-            assert torch.equal(o_hyps[:, 0], tk_hyps[:, 0]) and (o_scores - tk_scores).abs().max() < 1e-3
-            gold["beam_" + name] = dict(kwargs=kw, with_lm=with_lm, with_ctc=with_ctc, eos_bias=eos_bias,
-                                        max_decode_ratio=(steps + 0.5) / T, lm_weight=0.6, lm_temperature=1.15, ctc_weight=0.4,
-                                        hyps=tk_hyps.int(), lens=tk_len, scores=tk_scores, log_probs=tk_lp)
-        mods["seq_lin"].w.bias.copy_(sd["seq_lin.w.bias"])
-    torch.save(gold, os.path.join(OUT, f"{tag}.pt"))
-    print(tag, os.path.getsize(os.path.join(OUT, f"{tag}.pt")))
+        oc = O.full_pipeline_features(wav, wav_lens, ref.sd, dict(cfg))
+        oenc = O.encode(oc, wav_lens, ref.sd, ref.cfg, "Transformer.")
+    print(f"[{tag}] T={T} encoder: oracle rel {G.rel(oenc, enc):.2e}")
+    assert G.rel(oenc, enc) < 1e-5
+    gold["enc_out"] = enc.clone()
+    gold["abs_len"] = torch.round(wav_lens * T).int()
+    if n_greedy > 0:
+        hyps, logits = G.greedy_case(ref, enc, wav_lens, n_greedy, tag)
+        gold.update(G.greedy_record(hyps, logits),
+                    greedy_lp_sample=torch.log_softmax(logits, -1)[:, :, :128].clone().half())
+    lm = G.reference_lm() if any(kw["with_lm"] for _, kw in beams) else None
+    for name, kw in beams:
+        kw = dict(kw)
+        with_lm, with_ctc, eos_bias, steps = kw.pop("with_lm"), kw.pop("with_ctc"), kw.pop("eos_bias"), kw.pop("steps")
+        kw.setdefault("min_decode_ratio", 0.0)
+        gold["beam_" + name] = bench_beam(ref, enc, wav_lens, kw, steps, eos_bias, f"{tag} beam {name}", with_lm, with_ctc,
+                                          lm, lm_weight=0.6, lm_temperature=1.15, ctc_weight=0.4)
+    G.save(gold, f"{tag}.pt")
 
 
 def bench_extra_case(tag="bench_decode_conformer_large_rope_10s"):
     """On the encoder states of the bench-shape RoPE golden: (1) TransformerASR.decode(tgt, enc, enc_len) of the reference,
     teacher-forced on the greedy tokens (48 positions, ragged memory lengths) -> decoder outputs [4, 48, 512];
     (2) beam = 10 without scorers, EOS bias chosen so that hypotheses finish gradually over many steps."""
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    import time
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "bench_conformer_large_rope_10s.pt"))
+    ref = G.build_reference(CFG_L, "RoPEMHA")
+    g = G.load("bench_conformer_large_rope_10s.pt")
     enc, wav_lens = g["enc_out"], g["wav_lens"]
     T = enc.shape[1]
-    ocfg = dict(CFG_L, attention_type="RoPEMHA")
     out = {}
     with torch.no_grad():
         tgt = torch.cat([torch.full((enc.shape[0], 1), 1, dtype=torch.long), g["greedy_tokens"].long()[:, :-1]], 1)
         enc_len = torch.round(wav_lens * T).int()
-        pred, attn = mods["Transformer"].decode(tgt, enc, enc_len)
-        opred, _ = O.decode(tgt, enc, enc_len, sd, ocfg, "Transformer.")
-        print(f"[decode] pred {tuple(pred.shape)} oracle rel {rel(opred, pred):.2e}")
-        assert rel(opred, pred) < 1e-5
-        out["decode"] = dict(tgt=tgt.int(), enc_len=enc_len, pred=pred.clone())
-        for name, eos_bias, steps in (("b10_plain_eos12", 1.2, 48), ("b10_plain_eos16", 1.6, 48)):
-            t0 = time.time()
-            kw = dict(beam_size=10, using_eos_threshold=False, temperature=1.15, min_decode_ratio=3.5 / T)
-            bias = sd["seq_lin.w.bias"].clone()
-            bias[2] += eos_bias
-            mods["seq_lin"].w.bias.copy_(bias)
-            bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                            max_decode_ratio=(steps + 0.5) / T, return_topk=True, topk=10, **kw)
-            tk_hyps, tk_len, tk_scores, tk_lp = bs(enc, wav_lens)
-            o_hyps, o_len, o_scores, o_lp = O.beam_search(enc, wav_lens, sd, ocfg, sd["seq_lin.w.weight"], bias, 1, 2,
-                                                          max_decode_ratio=(steps + 0.5) / T, prefix="Transformer.", topk=10,
-                                                          return_topk=True, **kw)
-            print(f"[beam {name}] reference {time.time() - t0:.1f}s; best lens {(tk_len[:, 0] * tk_hyps.shape[2]).round().int().tolist()} "
-                  f"max len {tk_hyps.shape[2]} scores {tk_scores[:, 0].tolist()} oracle equal {torch.equal(o_hyps, tk_hyps)} "
-                  f"gap {(tk_scores[:, 0] - tk_scores[:, 1]).tolist()}")
-            assert torch.equal(o_hyps[:, 0], tk_hyps[:, 0]) and (o_scores - tk_scores).abs().max() < 1e-3
-            out["beam_" + name] = dict(kwargs=kw, with_lm=False, with_ctc=False, eos_bias=eos_bias, max_decode_ratio=(steps + 0.5) / T,
-                                       hyps=tk_hyps.int(), lens=tk_len, scores=tk_scores, log_probs=tk_lp)
-        mods["seq_lin"].w.bias.copy_(sd["seq_lin.w.bias"])
-    torch.save(out, os.path.join(OUT, f"{tag}.pt"))
-    print(tag, os.path.getsize(os.path.join(OUT, f"{tag}.pt")))
+        pred, attn = ref.mods["Transformer"].decode(tgt, enc, enc_len)
+        opred, _ = O.decode(tgt, enc, enc_len, ref.sd, ref.cfg, "Transformer.")
+    print(f"[decode] pred {tuple(pred.shape)} oracle rel {G.rel(opred, pred):.2e}")
+    assert G.rel(opred, pred) < 1e-5
+    out["decode"] = dict(tgt=tgt.int(), enc_len=enc_len, pred=pred.clone())
+    for name, eos_bias, steps in (("b10_plain_eos12", 1.2, 48), ("b10_plain_eos16", 1.6, 48)):
+        kw = dict(beam_size=10, using_eos_threshold=False, temperature=1.15, min_decode_ratio=3.5 / T)
+        out["beam_" + name] = bench_beam(ref, enc, wav_lens, kw, steps, eos_bias, f"beam {name}")
+    G.save(out, f"{tag}.pt")
 
 
 def ctc_greedy_case(tag="ctc_greedy_conformer_large_rope"):
@@ -524,9 +302,8 @@ def ctc_greedy_case(tag="ctc_greedy_conformer_large_rope"):
     encoder states: log_softmax(ctc_lin(enc)) -> ctc_greedy_decode(blank 0).  Random-init posteriors almost never repeat, so a
     second case adds a bias to the blank and to one token to exercise the merge / blank-filter rules."""
     from speechbrain.decoders.ctc import ctc_greedy_decode
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
+    ref, enc, wav_lens = rope_case()
+    sd, mods = ref.sd, ref.mods
     out = {}
     for name, bias_blank, bias_tok in (("plain", 0.0, 0.0), ("merge", 1.2, 1.1)):
         with torch.no_grad():
@@ -546,7 +323,7 @@ def ctc_greedy_case(tag="ctc_greedy_conformer_large_rope"):
                          margin=(top2[..., 0] - top2[..., 1]).clone(), log_probs_head=lp[:, :, :64].clone())
     with torch.no_grad():
         mods["ctc_lin"].w.bias.copy_(sd["ctc_lin.w.bias"])
-    torch.save(out, os.path.join(OUT, f"{tag}.pt"))
+    G.save(out, f"{tag}.pt")
 
 
 # "ffn": first FFN layers x200 and second layers / 200: hidden activations (the fp16-stored tensor) in the hundreds while the
@@ -574,90 +351,53 @@ def scale_state(sd, scales):
 def scaled_case(tag="conformer_large_rope_scaled"):
     """fp16 range (VERDICT r1 #8): the 2 s RoPE golden re-run by the reference with (a) FFN pre-activations pushed into the
     hundreds, (b) attention logits x9 and GLU inputs x4 -- far above what random init gives."""
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
+    g = G.load("conformer_large_rope.pt")
     out = {}
     for name, sc in SCALES.items():
-        fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-        sds = scale_state(sd, sc)
-        mods.load_state_dict({k: v for k, v in sds.items() if not k.startswith("normalize.")})
+        ref = G.build_reference(CFG_L, "RoPEMHA")
+        sds = scale_state(ref.sd, sc)
+        ref.mods.load_state_dict({k: v for k, v in sds.items() if not k.startswith("normalize.")})
         stats = {"ffn_hidden_absmax": 0.0}
 
         def hook_ffn(m, i, o):
             stats["ffn_hidden_absmax"] = max(stats["ffn_hidden_absmax"], float(o.abs().max()))
-        for layer in mods["Transformer"].encoder.layers:
+        for layer in ref.mods["Transformer"].encoder.layers:
             layer.ffn_module1[1].ffn[0].register_forward_hook(hook_ffn)
             layer.ffn_module2[1].ffn[0].register_forward_hook(hook_ffn)
         with torch.no_grad():
-            enc = mods["Transformer"].encode(g["cnn_out"], g["wav_lens"])
+            enc = ref.mods["Transformer"].encode(g["cnn_out"], g["wav_lens"])
             oenc = O.encode(g["cnn_out"].reshape(g["cnn_out"].shape[0], g["cnn_out"].shape[1], -1), g["wav_lens"], sds,
-                            dict(CFG_L, attention_type="RoPEMHA"), "Transformer.")
-        print(f"[scaled {name}] enc finite {bool(torch.isfinite(enc).all())} oracle rel {rel(oenc, enc):.2e} max |FFN pre-activation| "
-              f"{stats['ffn_hidden_absmax']:.1f} enc absmax {float(enc.abs().max()):.2f}")
-        assert rel(oenc, enc) < 1e-5
+                            ref.cfg, "Transformer.")
+        print(f"[scaled {name}] enc finite {bool(torch.isfinite(enc).all())} oracle rel {G.rel(oenc, enc):.2e} max |FFN "
+              f"pre-activation| {stats['ffn_hidden_absmax']:.1f} enc absmax {float(enc.abs().max()):.2f}")
+        assert G.rel(oenc, enc) < 1e-5
         out[name] = dict(scales=sc, enc_out=enc, ffn_hidden_absmax=stats["ffn_hidden_absmax"])
-    torch.save(out, os.path.join(OUT, f"{tag}.pt"))
-
+    G.save(out, f"{tag}.pt")
 
 
 def beam66_case(tag="beam66_conformer_large_rope"):
     """beam_size = 66, the recipe's test_beam_size (conformer_large.yaml:132), on the 2 s golden: scorer-less, temperature
     1.15, a small EOS bias so that hypotheses finish at different steps.  All 66 hypotheses per utterance are stored."""
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
-    T = enc.shape[1]
-    kw = dict(beam_size=66, using_eos_threshold=False, temperature=1.15, min_decode_ratio=2.5 / T)
-    eos_bias, steps = 1.5, 10
-    with torch.no_grad():
-        bias = sd["seq_lin.w.bias"].clone()
-        bias[2] += eos_bias
-        mods["seq_lin"].w.bias.copy_(bias)
-        bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                        max_decode_ratio=(steps + 0.5) / T, return_topk=True, topk=66, **kw)
-        tk_hyps, tk_len, tk_scores, tk_lp = bs(enc, wav_lens)
-        o_hyps, o_len, o_scores, o_lp = O.beam_search(enc, wav_lens, sd, dict(CFG_L, attention_type="RoPEMHA"), sd["seq_lin.w.weight"],
-                                                      bias, 1, 2, max_decode_ratio=(steps + 0.5) / T, prefix="Transformer.", topk=66,
-                                                      return_topk=True, **kw)
-    print(f"[beam66] best lens {(tk_len[:, 0] * tk_hyps.shape[2]).round().int().tolist()} max len {tk_hyps.shape[2]} scores "
-          f"{tk_scores[:, 0].tolist()} oracle equal {torch.equal(o_hyps, tk_hyps)} gap {(tk_scores[:, 0] - tk_scores[:, 1]).tolist()}")
-    assert torch.equal(o_hyps[:, 0], tk_hyps[:, 0]) and (o_scores - tk_scores).abs().max() < 1e-3
-    torch.save(dict(kwargs=kw, with_lm=False, with_ctc=False, eos_bias=eos_bias, max_decode_ratio=(steps + 0.5) / T,
-                    hyps=tk_hyps.int(), lens=tk_len, scores=tk_scores, log_probs=tk_lp), os.path.join(OUT, f"{tag}.pt"))
+    ref, enc, wav_lens = rope_case()
+    kw = dict(beam_size=66, using_eos_threshold=False, temperature=1.15, min_decode_ratio=2.5 / enc.shape[1])
+    G.save(bench_beam(ref, enc, wav_lens, kw, 10, 1.5, "beam66"), f"{tag}.pt")
 
 
 def beam_cov_case(tag="beam_cov_conformer_large_rope"):
     """ScorerBuilder(full_scorers=[CoverageScorer]) (scorer.py:788-955): coverage penalty on the last decoder layer's
     head-averaged cross-attention, weight chosen large enough to change the result of the scorer-less search."""
-    from speechbrain.decoders.scorer import CoverageScorer, ScorerBuilder
-    from speechbrain.decoders.seq2seq import S2STransformerBeamSearcher
-    fb, norm, mods, sd = build_reference(CFG_L, "RoPEMHA")
-    g = torch.load(os.path.join(OUT, "conformer_large_rope.pt"))
-    enc, wav_lens = g["enc_out"], g["wav_lens"]
+    ref, enc, wav_lens = rope_case()
     T = enc.shape[1]
     kwargs = dict(beam_size=5, using_eos_threshold=False, temperature=1.15, min_decode_ratio=2.5 / T)
     eos_bias, w_cov, thr, steps = 1.5, 40.0, 0.05, 10
-    with torch.no_grad():
-        bias = sd["seq_lin.w.bias"].clone()
-        bias[2] += eos_bias
-        mods["seq_lin"].w.bias.copy_(bias)
-        res = {}
-        for name, scorer in (("off", None), ("on", ScorerBuilder(full_scorers=[CoverageScorer(5000, threshold=thr)],
-                                                                 weights={"coverage": w_cov}))):
-            bs = S2STransformerBeamSearcher(modules=[mods["Transformer"], mods["seq_lin"]], bos_index=1, eos_index=2,
-                                            max_decode_ratio=(steps + 0.5) / T, scorer=scorer, return_topk=True, topk=5, **kwargs)
-            res[name] = bs(enc, wav_lens)
-        o = O.beam_search(enc, wav_lens, sd, dict(CFG_L, attention_type="RoPEMHA"), sd["seq_lin.w.weight"], bias, 1, 2,
-                          max_decode_ratio=(steps + 0.5) / T, prefix="Transformer.", topk=5, return_topk=True,
-                          coverage=dict(weight=w_cov, threshold=thr), **kwargs)
-    hyps, lens, scores, lp = res["on"]
-    print(f"[beam cov] without {res['off'][0][:, 0].tolist()} {res['off'][2][:, 0].tolist()} with {hyps[:, 0].tolist()} scores "
-          f"{scores[:, 0].tolist()} | oracle equal: {torch.equal(o[0], hyps)} score err {(o[2] - scores).abs().max():.2e}")
-    assert torch.equal(o[0][:, 0], hyps[:, 0]) and (o[2] - scores).abs().max() < 1e-3
-    assert not torch.equal(res["off"][2], scores)
-    torch.save(dict(kwargs=kwargs, with_lm=False, with_ctc=False, eos_bias=eos_bias, coverage_weight=w_cov, coverage_threshold=thr,
-                    max_decode_ratio=(steps + 0.5) / T, hyps=hyps.int(), lens=lens, scores=scores, log_probs=lp,
-                    scores_without=res["off"][2]), os.path.join(OUT, f"{tag}.pt"))
+    without = G.run_beam(ref, enc, wav_lens, kwargs, (steps + 0.5) / T, eos_bias, topk=5, check=False)[2]
+    hyps, lens, scores, lp = G.run_beam(ref, enc, wav_lens, kwargs, (steps + 0.5) / T, eos_bias, scorers={"coverage": w_cov},
+                                        coverage_threshold=thr, topk=5, bar=1e-3, rank0=True, tag="beam cov")
+    print(f"[beam cov] best scores without {without[:, 0].tolist()} with {scores[:, 0].tolist()}")
+    assert not torch.equal(without, scores)
+    G.save(dict(kwargs=kwargs, with_lm=False, with_ctc=False, eos_bias=eos_bias, coverage_weight=w_cov, coverage_threshold=thr,
+                max_decode_ratio=(steps + 0.5) / T, hyps=hyps.int(), lens=lens, scores=scores, log_probs=lp,
+                scores_without=without), f"{tag}.pt")
 
 
 def dynchunk_case(tag="dynchunk_conformer_large"):
@@ -668,17 +408,17 @@ def dynchunk_case(tag="dynchunk_conformer_large"):
     from speechbrain.utils.dynamic_chunk_training import DynChunkTrainConfig
     out = {}
     for att, cs, lc in (("RoPEMHA", 8, 2), ("RelPosMHAXL", 16, None), ("RoPEMHA", 5, 3), ("RelPosMHAXL", 4, 4)):
-        fb, norm, mods, sd = build_reference(CFG_L, att)
-        g = torch.load(os.path.join(OUT, "conformer_large_rope.pt" if att == "RoPEMHA" else "conformer_large_relpos.pt"))
+        ref = G.build_reference(CFG_L, att)
+        g = G.load("conformer_large_rope.pt" if att == "RoPEMHA" else "conformer_large_relpos.pt")
         with torch.no_grad():
-            enc = mods["Transformer"].encode(g["cnn_out"], g["wav_lens"], dynchunktrain_config=DynChunkTrainConfig(cs, lc))
+            enc = ref.mods["Transformer"].encode(g["cnn_out"], g["wav_lens"], dynchunktrain_config=DynChunkTrainConfig(cs, lc))
             src = g["cnn_out"].reshape(g["cnn_out"].shape[0], g["cnn_out"].shape[1], -1)
-            oenc = O.encode(src, g["wav_lens"], sd, dict(CFG_L, attention_type=att), "Transformer.", dynchunk=(cs, lc))
-        print(f"[dynchunk {att} chunk {cs} left {lc}] oracle rel {rel(oenc, enc):.2e}; differs from full-context by "
-              f"{rel(enc, g['enc_out']):.2e}")
-        assert rel(oenc, enc) < 1e-5 and rel(enc, g["enc_out"]) > 1e-2
+            oenc = O.encode(src, g["wav_lens"], ref.sd, ref.cfg, "Transformer.", dynchunk=(cs, lc))
+        print(f"[dynchunk {att} chunk {cs} left {lc}] oracle rel {G.rel(oenc, enc):.2e}; differs from full-context by "
+              f"{G.rel(enc, g['enc_out']):.2e}")
+        assert G.rel(oenc, enc) < 1e-5 and G.rel(enc, g["enc_out"]) > 1e-2
         out[f"{att}_{cs}_{lc}"] = dict(attention_type=att, chunk_size=cs, left_context_size=lc, enc_out=enc)
-    torch.save(out, os.path.join(OUT, f"{tag}.pt"))
+    G.save(out, f"{tag}.pt")
 
 
 BEAMS_10S = (
@@ -688,52 +428,38 @@ BEAMS_10S = (
                            with_ctc=False, eos_bias=6.0, steps=48)),
 )
 
+CASES = {
+    "fbank": fbank_cases,
+    "norm": norm_cases,
+    "L_rope": lambda: model_case(CFG_L, "RoPEMHA", 2, 32000, [1.0, 0.7], 6, "conformer_large_rope"),
+    "L_relpos": lambda: model_case(CFG_L, "RelPosMHAXL", 2, 32000, [1.0, 0.7], 6, "conformer_large_relpos"),
+    "S_relpos": lambda: model_case(CFG_S, "RelPosMHAXL", 2, 24000, [0.8, 1.0], 6, "conformer_small_relpos"),
+    "beam": beam_case,
+    "beam_topk": beam_topk_case,
+    "beam_lm": beam_lm_case,
+    "rescore": rescore_case,
+    "beam_len": beam_len_case,
+    "beam_ctc": beam_ctc_case,
+    # not in the default list: minutes of CPU time each
+    "bench_L_rope": lambda: bench_shape_case(CFG_L, "RoPEMHA", 4, 160000, [1.0, 0.9, 0.6, 0.3], 48,
+                                             "bench_conformer_large_rope_10s", BEAMS_10S),
+    "bench_L_relpos": lambda: bench_shape_case(CFG_L, "RelPosMHAXL", 4, 160000, [1.0, 0.9, 0.6, 0.3], 48,
+                                               "bench_conformer_large_relpos_10s"),
+    "dynchunk": dynchunk_case,
+    "beam_cov": beam_cov_case,
+    "beam66": beam66_case,
+    "scaled": scaled_case,
+    "ctc_greedy": ctc_greedy_case,
+    "bench_extra": bench_extra_case,
+    "bench_S_relpos": lambda: bench_shape_case(CFG_S, "RelPosMHAXL", 8, 80000, [1.0, 0.95, 0.9, 0.8, 0.7, 0.55, 0.4, 0.25],
+                                               0, "bench_conformer_small_relpos_5s"),
+}
+DEFAULT = ["fbank", "norm", "L_rope", "L_relpos", "S_relpos", "beam", "beam_topk", "beam_lm", "beam_ctc", "rescore", "beam_len"]
+
 
 if __name__ == "__main__":
-    os.makedirs(OUT, exist_ok=True)
     torch.manual_seed(0)
-    which = sys.argv[1:] or ["fbank", "norm", "L_rope", "L_relpos", "S_relpos", "beam", "beam_topk", "beam_lm", "beam_ctc", "rescore", "beam_len"]
-    if "fbank" in which:
-        fbank_cases()
-    if "norm" in which:
-        norm_cases()
-    if "L_rope" in which:
-        model_case(CFG_L, "RoPEMHA", 2, 32000, [1.0, 0.7], 6, "conformer_large_rope")
-    if "L_relpos" in which:
-        model_case(CFG_L, "RelPosMHAXL", 2, 32000, [1.0, 0.7], 6, "conformer_large_relpos")
-    if "S_relpos" in which:
-        model_case(CFG_S, "RelPosMHAXL", 2, 24000, [0.8, 1.0], 6, "conformer_small_relpos")
-    if "beam" in which:
-        beam_case()
-    if "beam_topk" in which:
-        beam_topk_case()
-    if "beam_lm" in which:
-        beam_lm_case()
-    if "rescore" in which:
-        rescore_case()
-    if "beam_len" in which:
-        beam_len_case()
-    if "beam_ctc" in which:
-        beam_ctc_case()
-    # ---- bench-shape goldens (not in the default list: minutes of CPU time each)
-    if "bench_L_rope" in which:
-        bench_shape_case(CFG_L, "RoPEMHA", 4, 160000, [1.0, 0.9, 0.6, 0.3], 48, "bench_conformer_large_rope_10s", BEAMS_10S)
-    if "bench_L_relpos" in which:
-        bench_shape_case(CFG_L, "RelPosMHAXL", 4, 160000, [1.0, 0.9, 0.6, 0.3], 48, "bench_conformer_large_relpos_10s")
-    if "dynchunk" in which:
-        dynchunk_case()
-    if "beam_cov" in which:
-        beam_cov_case()
-    if "beam66" in which:
-        beam66_case()
-    if "scaled" in which:
-        scaled_case()
-    if "ctc_greedy" in which:
-        ctc_greedy_case()
-    if "bench_extra" in which:
-        bench_extra_case()
-    if "bench_S_relpos" in which:
-        bench_shape_case(CFG_S, "RelPosMHAXL", 8, 80000, [1.0, 0.95, 0.9, 0.8, 0.7, 0.55, 0.4, 0.25], 0,
-                         "bench_conformer_small_relpos_5s")
-    for fn in sorted(os.listdir(OUT)):
-        print(fn, os.path.getsize(os.path.join(OUT, fn)))
+    which = sys.argv[1:] or DEFAULT
+    for name, case in CASES.items():
+        if name in which:
+            case()

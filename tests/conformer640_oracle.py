@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import asr_oracle as O
+from oracle.goldens import wav_case
 from parity import lm_scorer_state, oracle_lm
 
 WAV_SEED, LENS, STEPS, BOS, EOS = 7, [1.0, 0.9, 0.6, 0.3], 48, 1, 2
@@ -28,11 +29,7 @@ def state(cfg):
 
 
 def waveforms(seed=WAV_SEED, L=160000, lens=LENS):
-    g = torch.Generator().manual_seed(seed)
-    wav = torch.randn(len(lens), L, generator=g)
-    for b, f in enumerate(lens):
-        wav[b, int(round(f * L)):] = 0
-    return wav, torch.tensor(lens)
+    return wav_case(seed, len(lens), L, lens)[:2]
 
 
 def swish_decoder(cfg):

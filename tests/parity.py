@@ -15,14 +15,11 @@ import os
 import pytest
 import torch
 
+from oracle.goldens import rel, seeded_wav  # noqa: F401  (the writers' waveform rule and rel-L2, re-exported)
+
 GREEDY_MARGIN = 5e-3
 GREEDY_LOGPROB = 2e-2
 BEAM_TOL = 3e-2
-
-
-def rel(a, b):
-    """rel-L2 of a against b, in float64"""
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-30))
 
 
 @pytest.fixture(scope="module")
@@ -30,19 +27,6 @@ def dev():
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     return torch.device("cuda:0")
-
-
-def seeded_wav(seed, shape, lens=None, checksum=None):
-    """A fixture generator's waveform, regenerated from its seed: [B, L] normal samples, row b zeroed past round(lens[b] L)
-    (lens None: all ones); the checksum (sum of |x|) pins the RNG stream"""
-    B, L = shape
-    wav = torch.randn(B, L, generator=torch.Generator().manual_seed(seed))
-    lens = torch.ones(B) if lens is None else lens
-    for b in range(B):
-        wav[b, int(round(float(lens[b]) * L)):] = 0
-    if checksum is not None:
-        assert abs(float(wav.double().abs().sum()) - checksum) / checksum < 1e-9, "regenerated waveform differs from the fixture's"
-    return wav, lens
 
 
 def case_wav(case):

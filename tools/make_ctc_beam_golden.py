@@ -1,25 +1,18 @@
 """Generate tests/golden/ctc_beam.pt by RUNNING THE REFERENCE CTCBeamSearcher (speechbrain.decoders.ctc, no LM).
 
-Run it the way oracle/make_goldens.py's docstring describes (reference package and hyperpyyaml stub on PYTHONPATH):
-
-    PYTHONPATH=/tmp/stub:<reference>:. python tools/make_ctc_beam_golden.py
-
-Every case's log-posteriors are regenerated from a seed (tests/ctc_beam_oracle.synthetic_log_probs; the fixture keeps the
+How to run it: oracle/goldens.py.  Every case's log-posteriors are regenerated from a seed (tests/ctc_beam_oracle.synthetic_log_probs; the fixture keeps the
 seed and a checksum) or, for the Branchformer CTC cases, read from tests/golden/branchformer.pt.  For every case the
 script asserts that the NumPy oracle (tests/ctc_beam_oracle.py) equals the reference: texts and text_frames identical,
 scores bit-equal, except where two hypotheses' scores tie exactly (reported).  It stores the reference hypotheses, the
 oracle's per-frame live-beam and merge counts (evidence that the beam fills and merges happen) and the reference's CPU
 time per case."""
-import os
-import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+from oracle import goldens as G  # also puts tests/, where the oracles live, on sys.path
+
 import ctc_beam_oracle as CO  # noqa: E402
 
 RECIPE = dict(blank_index=0, beam_size=100, beam_prune_logp=-12.0, token_prune_min_logp=-1.2, prune_history=False)
@@ -29,7 +22,7 @@ DEFAULTS = dict(blank_index=0, topk=5)
 def case_list():
     spm = CO.spm_vocab(5000, 0)
     spm_active = list(range(11)) + [17, 40, 99, 512, 1024, 2048, 3001, 4999]
-    bf = torch.load(os.path.join(ROOT, "tests", "golden", "branchformer.pt"))["ctc"]
+    bf = G.load("branchformer.pt")["ctc"]
     lens8 = [1.0, 0.9, 0.75, 0.6, 0.5, 0.33, 0.2, 0.1]   # 0.9 * 251 = 225.9: truncation 225, rounding 226
     return [
         dict(name="recipe", vocab=CO.CHAR_VOCAB, params=RECIPE, gen=dict(seed=101, B=8, T=251, V=31), lens=lens8),
@@ -104,9 +97,7 @@ def main():
         else:
             entry["stored"] = "branchformer.pt:ctc.log_probs"
         out["cases"].append(entry)
-    path = os.path.join(ROOT, "tests", "golden", "ctc_beam.pt")
-    torch.save(out, path)
-    print(f"wrote {path} ({os.path.getsize(path)} bytes)")
+    G.save(out, "ctc_beam.pt")
 
 
 if __name__ == "__main__":

@@ -1,24 +1,17 @@
 """Generate tests/golden/ctc_prefix_beam.pt by RUNNING THE REFERENCE CTCPrefixBeamSearcher (speechbrain.decoders.ctc, no LM).
 
-Run it the way oracle/make_goldens.py's docstring describes (reference package and hyperpyyaml stub on PYTHONPATH):
-
-    PYTHONPATH=/tmp/stub:<reference>:. python tools/make_ctc_prefix_beam_golden.py
-
-Every case's log-posteriors are regenerated from a seed (tests/ctc_beam_oracle.synthetic_log_probs; the fixture keeps the
+How to run it: oracle/goldens.py.  Every case's log-posteriors are regenerated from a seed (tests/ctc_beam_oracle.synthetic_log_probs; the fixture keeps the
 seed and a checksum) or, for the Branchformer CTC cases, read from tests/golden/branchformer.pt.  For every case the
 script asserts that the NumPy oracle (tests/ctc_prefix_beam_oracle.py) equals the reference exactly: texts, text_frames
 and float64 score bits.  It stores the reference hypotheses, the oracle's per-frame live and created beam counts, and the
 reference's CPU time per case."""
-import os
-import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+from oracle import goldens as G  # also puts tests/, where the oracles live, on sys.path
+
 import ctc_beam_oracle as CO  # noqa: E402
 import ctc_prefix_beam_oracle as PO  # noqa: E402
 
@@ -71,7 +64,7 @@ def duplicate_text_log_probs():
 def case_inputs(case):
     """(log_probs [B, T, V] float32, wav_lens float32) of a fixture case."""
     if case.get("stored"):
-        bf = torch.load(os.path.join(ROOT, "tests", "golden", "branchformer.pt"))["ctc"]
+        bf = G.load("branchformer.pt")["ctc"]
         return bf["log_probs"].float(), bf["wav_lens"].float()
     if "tied" in case:
         lp = CO.tied_log_probs(**case["tied"])
@@ -122,9 +115,7 @@ def main():
             if k in case:
                 entry[k] = case[k]
         out["cases"].append(entry)
-    path = os.path.join(ROOT, "tests", "golden", "ctc_prefix_beam.pt")
-    torch.save(out, path)
-    print(f"wrote {path} ({os.path.getsize(path)} bytes)")
+    G.save(out, "ctc_prefix_beam.pt")
 
 
 if __name__ == "__main__":

@@ -1,24 +1,17 @@
 """Generate tests/golden/ctc_prefix.pt by RUNNING THE REFERENCE's CTCPrefixScore (decoders/ctc.py:26-295) in float64.
 
-Run it the way oracle/make_goldens.py's docstring describes (reference package and hyperpyyaml stub on PYTHONPATH).
-
-Each case drives CTCPrefixScore.forward_step + permute_mem along a forced search history (the way ScorerBuilder /
+How to run it: oracle/goldens.py.  Each case drives CTCPrefixScore.forward_step + permute_mem along a forced search history (the way ScorerBuilder /
 S2SBeamSearcher drive it: inp_tokens = the previous step's tokens, permute_mem(memory, candidates)) for every step up to
 prefix_length = T, the last step the reference defines.  The history comes from oracle.ctc_history_picker (parents with
 several children and with none, repeated last tokens, the best and random tokens).  Cases: blank 0 and a nonzero blank,
 V = 61 (not a multiple of 4, below one 256-token CTA), ragged enc_len including 1 and T, beam 7.  The script checks
 oracle.ctc_prefix_scores against the reference on every entry, then stores the inputs and the reference's psi - psi_prev.
 """
-import os
-import sys
-
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle import asr_oracle as O
+from oracle import goldens as G
 
-from oracle import asr_oracle as O  # noqa: E402
-
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "ctc_prefix.pt")
 # name: (B, T, V, beam, blank, bos, eos, enc_len, seed)
 CASES = {
     "blank0_beam7": (3, 14, 61, 7, 0, 1, 2, [14, 1, 9], 11),
@@ -75,8 +68,7 @@ def main():
         assert err < 1e-9 and (ours["psi_prev"] - ref_prev).abs().max() < 1e-9
         gold[name] = dict(logits=logits, enc_len=enc_len, beam=beam, blank=blank, bos=bos, eos=eos, n_steps=n_steps,
                           hist_tok=ht, hist_pred=hp, score=ref.clone(), psi_prev=ref_prev.clone())
-    torch.save(gold, OUT)
-    print(OUT, os.path.getsize(OUT))
+    G.save(gold, "ctc_prefix.pt")
 
 
 if __name__ == "__main__":

@@ -1,22 +1,14 @@
 """Generate tests/golden/streaming.pt by RUNNING THE REFERENCE TransformerASR.encode_streaming (speechbrain.lobes.models.
 transformer.TransformerASR, Conformer.py forward_streaming with its per-layer mha / dcconv left contexts) chunk by chunk.
 
-Run it the way oracle/make_goldens.py's docstring describes (reference package and hyperpyyaml stub on PYTHONPATH):
-
-    PYTHONPATH=/tmp/stub:<reference>:. python tools/make_streaming_golden.py
-
-Models: the Conformer-L encoder (12 layers, d_model 512) with seeded weights (seeded_init.seeded_asr_state, seed 0), RoPEMHA
+How to run it: oracle/goldens.py.  Models: the Conformer-L encoder (12 layers, d_model 512) with seeded weights (seeded_init.seeded_asr_state, seed 0), RoPEMHA
 with DynChunkTrainConfig (24, 8), (8, 2) and (16, 1), and RelPosMHAXL with (16, 2).  Input: a 2-stream batch of encoder-input
 frames [2, T, 640] from a seed (checksummed), 14 full chunks and a short last one, so the (24, 8) caches fill.  Per case
 it stores the per-frame L2 norms of every chunk's output and the whole output of one chunk taken after the caches filled.
 The reference rejects an unlimited left context, so every case has a finite one."""
-import os
-import sys
-
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from oracle import goldens as G
 
 CASES = [dict(name="rope_24_8", att="RoPEMHA", chunk=24, left=8, seed=101),
          dict(name="rope_8_2", att="RoPEMHA", chunk=8, left=2, seed=102),
@@ -66,16 +58,14 @@ def main():
                 norms.append(o.double().norm(dim=-1).float())
             full = tr.encode(src, None, dynchunktrain_config=dc)
         stream = torch.cat(outs, dim=1)
-        r = float((stream - full).norm() / full.norm())
+        r = G.rel(stream, full)
         keep = FULL_CHUNKS - 2  # a chunk after every cache has filled
         print(f"[{case['name']}] {len(outs)} chunks; reference streaming vs its masked encode rel {r:.2e}; "
               f"layer 0 left context {tuple(ctx.encoder_context.layers[0].mha_left_context.shape)}")
         assert r < 1e-5
         out["cases"][case["name"]] = dict(case, src_checksum=float(src.double().abs().sum()), frame_norms=norms,
                                           full_chunk_index=keep, full_chunk=outs[keep].clone())
-    path = os.path.join(ROOT, "tests", "golden", "streaming.pt")
-    torch.save(out, path)
-    print(f"wrote {path} ({os.path.getsize(path)} bytes)")
+    G.save(out, "streaming.pt")
 
 
 if __name__ == "__main__":

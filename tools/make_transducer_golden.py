@@ -1,11 +1,7 @@
 """Generate tests/golden/transducer.pt by RUNNING THE REFERENCE TransducerBeamSearcher(beam_size=1) (speechbrain.decoders.
 transducer) with the reference Embedding / LSTM / Linear / Transducer_joint modules on seeded recipe-shaped weights.
 
-Run it the way oracle/make_goldens.py's docstring describes (reference package and hyperpyyaml stub on PYTHONPATH):
-
-    PYTHONPATH=/tmp/stub:<reference>:. python tools/make_transducer_golden.py
-
-The weights and tn_output of every case are regenerated from seeds (tests/transducer_oracle.seeded_weights / seeded_tn;
+How to run it: oracle/goldens.py.  The weights and tn_output of every case are regenerated from seeds (tests/transducer_oracle.seeded_weights / seeded_tn;
 the fixture keeps the seeds, the weight rescale and a checksum).  Per case it stores the reference's tokens, its score
 (exp of the summed log-probs, averaged over the batch) and, per joint evaluation, the top-two log-probs of every row
 (the reference margins); for the streaming case the tokens of chunked calls and the final (out_PN, h, c) norms.  It
@@ -20,15 +16,11 @@ the per-frame norms of the reference tn_output (padded frames included), the tok
 decisions (frame, token, top-1 / top-2 log-prob margin) as the reference took them.  The blank gain is the rescale that
 makes this search emit 0, 1 and >= 2 tokens per frame (asserted)."""
 import collections
-import os
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
+from oracle import goldens as G  # also puts tests/, where the oracles live, on sys.path
+
 import transducer_oracle as TO  # noqa: E402
 
 
@@ -84,14 +76,12 @@ E2E = dict(seed=21, pn_seed=23, wav_seed=22, lens=[1.0, 0.9, 0.6, 0.3], L=160000
 
 def e2e_inputs():
     """(encoder state dict, proj_enc weight, prediction-network weights, wav, lens) of the end-to-end case."""
-    from make_branchformer_golden import waveforms
-
     from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state, seeded_tensor
     cfg = dict(CONFORMER_LARGE, num_decoder_layers=0, vocab=1000)
     sd = seeded_asr_state(cfg, E2E["seed"])
     w_enc = seeded_tensor(E2E["seed"], "proj_enc.w.weight", (640, 512)) * E2E["enc_scale"]
     W = TO.seeded_weights(E2E["pn_seed"], 640, 512, 1000, 0, blank_gain=E2E["blank_gain"])
-    wav, lens = waveforms(E2E["wav_seed"], len(E2E["lens"]), E2E["L"], E2E["lens"])
+    wav, lens, _ = G.wav_case(E2E["wav_seed"], len(E2E["lens"]), E2E["L"], E2E["lens"])
     return cfg, sd, w_enc, W, wav, lens
 
 
@@ -214,9 +204,7 @@ def main():
         out["cases"].append(entry)
     assert all(total[k] > 0 for k in (0, 1, 2)), total   # frames with 0, 1 and >= 2 emissions
     out["e2e"] = e2e_case()
-    path = os.path.join(ROOT, "tests", "golden", "transducer.pt")
-    torch.save(out, path)
-    print("wrote", path, os.path.getsize(path), "bytes")
+    G.save(out, "transducer.pt")
 
 
 if __name__ == "__main__":
