@@ -20,6 +20,7 @@ typedef struct sbk_asr sbk_asr;     /* opaque */
 enum { SBK_ATT_ROPE = 0, SBK_ATT_RELPOS = 1, SBK_ATT_HYPERMIX = 2, SBK_ATT_REGULAR = 3 };
 enum { SBK_ACT_RELU = 0, SBK_ACT_GELU = 1, SBK_ACT_SILU = 2 };
 enum { SBK_ENC_CONFORMER = 0, SBK_ENC_BRANCHFORMER = 1, SBK_ENC_TRANSFORMER = 2 };
+enum { SBK_CONFORMER_ACT_SWISH = 0, SBK_CONFORMER_ACT_GELU = 1 };
 enum { SBK_PART_FBANK = 1, SBK_PART_CNN = 2, SBK_PART_ENCODER = 4, SBK_PART_DECODER = 8, SBK_PART_ALL = 15, SBK_PART_LM = 16 };
 
 typedef struct {
@@ -57,6 +58,10 @@ typedef struct {
     /* ConvolutionFrontEnd blocks: 0 or 2 = the Conformer recipes' 2 x (3x3, stride 2), channels (cnn_c1, cnn_c2) = (64, 32);
        3 = the Transformer recipes' (5x5, stride 2), (5x5, stride 2), (1x1 + residual 1x1), 64 channels each */
     int cnn_blocks;
+    /* The Conformer encoder's conformer_activation (Conformer.py: both FFN modules and the convolution module after its
+       LayerNorm): SBK_CONFORMER_ACT_SWISH (0, so a zeroed config stays Swish) or SBK_CONFORMER_ACT_GELU (torch.nn.GELU,
+       the exact erf form: the Loquacious recipes).  Other values are rejected by sbk_asr_create. */
+    int conformer_activation;
 } sbk_asr_config;
 
 typedef struct {
@@ -189,6 +194,10 @@ int sbk_stream_qkv_test(const float* qkv_dev, int B, int n, int H, int head_dim,
  * Allocates and frees its own scratch and synchronises the stream. */
 int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
                     const float* ln_g_dev, const float* ln_b_dev, int chunk, void* out_dev, void* stream);
+/* the same with the Conformer activation as an argument: act SBK_CONFORMER_ACT_SWISH (SiLU, as sbk_dwconv_test) or
+ * SBK_CONFORMER_ACT_GELU (exact erf GELU) after the LayerNorm. */
+int sbk_dwconv_act_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
+                        const float* ln_g_dev, const float* ln_b_dev, int chunk, int act, void* out_dev, void* stream);
 
 /* the HyperConformer's HyperMixing block alone (HyperMixing.forward, nnet/hypermixing.py:90-195, tied=False, nhead heads of
  * e = d / nhead in {32, 64} channels, k = d_ffn / nhead a multiple of 16 up to 256): x_dev [B*T, d] fp16 (the norm1 output),

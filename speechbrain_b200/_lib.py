@@ -24,7 +24,8 @@ class sbk_asr_config(ctypes.Structure):
         "num_decoder_layers", "d_ffn", "vocab", "kernel_size", "attention_type", "decoder_activation", "max_len",
         "parts", "lm_d_model", "lm_nhead", "lm_layers", "lm_d_ffn", "lm_activation")] + [
         (k, ctypes.c_float) for k in ("fbank_amin", "fbank_top_db", "norm_eps")] + [
-        (k, ctypes.c_int) for k in ("encoder_module", "csgu_linear_units", "branchformer_activation", "cnn_blocks")]
+        (k, ctypes.c_int) for k in ("encoder_module", "csgu_linear_units", "branchformer_activation", "cnn_blocks",
+                                    "conformer_activation")]
 
 
 class sbk_beam_params(ctypes.Structure):
@@ -52,6 +53,7 @@ class sbk_ctc_prefix_beam_params(ctypes.Structure):
 SBK_ATT_ROPE, SBK_ATT_RELPOS, SBK_ATT_HYPERMIX, SBK_ATT_REGULAR = 0, 1, 2, 3
 SBK_ACT_RELU, SBK_ACT_GELU, SBK_ACT_SILU = 0, 1, 2
 SBK_ENC_CONFORMER, SBK_ENC_BRANCHFORMER, SBK_ENC_TRANSFORMER = 0, 1, 2
+SBK_CONFORMER_ACT_SWISH, SBK_CONFORMER_ACT_GELU = 0, 1
 SBK_PARTS = {"fbank": 1, "cnn": 2, "encoder": 4, "decoder": 8, "lm": 16}
 
 # every symbol include/sbk.h declares (tests check the library exports all of them)
@@ -59,7 +61,7 @@ EXPORTS = [
     "sbk_last_error", "sbk_version", "sbk_launch_count", "sbk_gemm_profile_enable", "sbk_gemm_profile_read", "sbk_fbank_create", "sbk_fbank_destroy", "sbk_fbank_num_frames",
     "sbk_fbank_forward", "sbk_input_norm_global", "sbk_input_norm_sentence", "sbk_gemm_f16_test", "sbk_gemm_f16_resid_test",
     "sbk_gemm_epilogue_test", "sbk_ctc_prefix_test", "sbk_csgu_test", "sbk_hypermix_test",
-    "sbk_encoder_attention_test", "sbk_dwconv_test",
+    "sbk_encoder_attention_test", "sbk_dwconv_test", "sbk_dwconv_act_test",
     "sbk_asr_create", "sbk_asr_destroy", "sbk_asr_num_frames", "sbk_asr_cnn_forward", "sbk_asr_encode_from_cnn",
     "sbk_asr_encode_feats", "sbk_asr_greedy_from_enc", "sbk_asr_transcribe_greedy_dev",
     "sbk_asr_transcribe_greedy_host", "sbk_asr_transcribe_greedy_host_async", "sbk_asr_clone",

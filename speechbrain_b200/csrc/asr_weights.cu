@@ -412,6 +412,10 @@ static int check_config(const sbk_asr_config& c) {
                 "asr_create: decoder head_dim must be 128, 80 or a multiple of 4 up to 64 and d_model a multiple of 16 (got %d, %d)",
                 dh, d);
     SBK_REQUIRE(c.attention_type != SBK_ATT_ROPE || dh % 32 == 0, "asr_create: RoPEMHA needs head_dim %% 32 == 0");
+    SBK_REQUIRE(c.conformer_activation == SBK_CONFORMER_ACT_SWISH || c.conformer_activation == SBK_CONFORMER_ACT_GELU,
+                "asr_create: conformer_activation %d not built (0 Swish, 1 GELU)", c.conformer_activation);
+    SBK_REQUIRE(c.conformer_activation == SBK_CONFORMER_ACT_SWISH || c.encoder_module == SBK_ENC_CONFORMER,
+                "asr_create: conformer_activation GELU is for the Conformer encoder only");
     SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER || c.encoder_module == SBK_ENC_BRANCHFORMER || tfm,
                 "asr_create: encoder_module %d (0 Conformer, 1 Branchformer, 2 Transformer)", c.encoder_module);
     SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER ||

@@ -246,8 +246,9 @@ int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream) {
     return SBK_OK;
 }
 
-// --------------------------------------------------------------------------- depthwise conv + LN + Swish
-// glu [B*T, D] fp32 (GLU output) -> out [B*T, D] fp16 = Swish(LN(dwconv(glu) + bias)).  The tap weights arrive TAP-MAJOR
+// --------------------------------------------------------------------------- depthwise conv + LN + Swish / GELU
+// glu [B*T, D] fp32 (GLU output) -> out [B*T, D] fp16 = act(LN(dwconv(glu) + bias)), act the Conformer's activation: Swish,
+// or the exact erf GELU of the recipes with conformer_activation=torch.nn.GELU.  The tap weights arrive TAP-MAJOR
 // ([K, D], repacked from the reference's (D, 1, K) at load time): thread = channel, so the 31 weight loads of a thread are
 // coalesced across the warp (the channel-major layout made every load touch 32 cache lines).
 // Zero padding at utterance edges only: padded frames inside T are real inputs (Conformer.py:318-325
@@ -255,15 +256,22 @@ int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream) {
 // input slab is staged in shared memory once.
 constexpr int DW_TT = 16;
 
+template <bool GELU>
+__device__ __forceinline__ float conv_act(float x) {
+    if constexpr (GELU) return gelu_erf_f(x);
+    else return silu_f(x);
+}
+
 // KT > 0: compile-time kernel size (taps held in registers); KT == 0: runtime K.  MAXC: channels per thread (D <= 256 * MAXC)
 // CHUNKED: Dynamic Chunk Convolution (Conformer.py:190-313): for every output frame the inputs beyond the end of its own
 // chunk of `chunk` frames count as zero (the past, other chunks included, is visible as usual).
 // left: [B, (K-1)/2, D] inputs of the frames just before frame 0 (a stream's previous chunks), or null for zero padding.
-template <int KT, int MAXC, bool CHUNKED = false>
+// GELU: exact erf GELU after the LayerNorm instead of Swish.
+template <int KT, int MAXC, bool CHUNKED = false, bool GELU = false>
 __global__ void __launch_bounds__(256, 2)
-dwconv_ln_swish_kernel(const float* __restrict__ glu, int T, int D, int K, const float* __restrict__ wdw /*[K,D] tap-major*/,
-                       const float* __restrict__ bdw, const float* __restrict__ gamma, const float* __restrict__ beta,
-                       float eps, __half* __restrict__ out, int chunk, const float* __restrict__ left) {
+dwconv_ln_act_kernel(const float* __restrict__ glu, int T, int D, int K, const float* __restrict__ wdw /*[K,D] tap-major*/,
+                     const float* __restrict__ bdw, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     float eps, __half* __restrict__ out, int chunk, const float* __restrict__ left) {
     extern __shared__ __align__(128) float dw_smem[];
     __shared__ uint64_t bar;
     const int halo = (K - 1) / 2;
@@ -390,29 +398,35 @@ dwconv_ln_swish_kernel(const float* __restrict__ glu, int T, int D, int K, const
             const int j = 2 * lane + 64 * p;
             if (j < D) {
                 const float2 cv = *reinterpret_cast<const float2*>(c + j);
-                const float y0 = silu_f((cv.x - mean) * rstd * g2[p].x + b2[p].x);
-                const float y1 = silu_f((cv.y - mean) * rstd * g2[p].y + b2[p].y);
+                const float y0 = conv_act<GELU>((cv.x - mean) * rstd * g2[p].x + b2[p].x);
+                const float y1 = conv_act<GELU>((cv.y - mean) * rstd * g2[p].y + b2[p].y);
                 *reinterpret_cast<__half2*>(o + j) = floats2half2_sat(y0, y1);
             }
         }
     }
 }
 
-int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw,
-                    const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk,
-                    const float* left) {
-    SBK_REQUIRE(D % 4 == 0 && D <= 1024 && (K & 1) == 1, "dwconv_ln_swish: D %% 4, D <= 1024 and odd K required (D=%d K=%d)", D, K);
-    SBK_REQUIRE((reinterpret_cast<uintptr_t>(glu) & 15) == 0, "dwconv_ln_swish: input must be 16-byte aligned");
-    const size_t smem = static_cast<size_t>(DW_TT + K - 1) * D * sizeof(float);
-    SBK_REQUIRE(smem <= 200 * 1024, "dwconv_ln_swish: tile too large for shared memory (D=%d K=%d)", D, K);
-    auto kern = dwconv_ln_swish_kernel<0, 4>;
+// The instantiation for (D, K, chunk): taps in registers at K = 31 with 1, 2 or 4 channels per thread (D <= 1024), else
+// runtime K.  D = 768 takes the 4-channel form with its fourth channel slot idle.
+template <bool GELU>
+static auto dwconv_kernel_for(int D, int K, int chunk) {
     if (chunk > 0) {
-        kern = dwconv_ln_swish_kernel<0, 4, true>;
-        if (K == 31) kern = D <= 256 ? dwconv_ln_swish_kernel<31, 1, true> : D <= 512 ? dwconv_ln_swish_kernel<31, 2, true>
-                                                                                        : dwconv_ln_swish_kernel<31, 4, true>;
-    } else if (K == 31) {
-        kern = D <= 256 ? dwconv_ln_swish_kernel<31, 1> : D <= 512 ? dwconv_ln_swish_kernel<31, 2> : dwconv_ln_swish_kernel<31, 4>;
+        if (K != 31) return dwconv_ln_act_kernel<0, 4, true, GELU>;
+        return D <= 256 ? dwconv_ln_act_kernel<31, 1, true, GELU> : D <= 512 ? dwconv_ln_act_kernel<31, 2, true, GELU>
+                                                                             : dwconv_ln_act_kernel<31, 4, true, GELU>;
     }
+    if (K != 31) return dwconv_ln_act_kernel<0, 4, false, GELU>;
+    return D <= 256 ? dwconv_ln_act_kernel<31, 1, false, GELU> : D <= 512 ? dwconv_ln_act_kernel<31, 2, false, GELU>
+                                                                          : dwconv_ln_act_kernel<31, 4, false, GELU>;
+}
+
+int dwconv_ln_act(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw, const float* gamma,
+                  const float* beta, float eps, __half* out, cudaStream_t stream, bool gelu, int chunk, const float* left) {
+    SBK_REQUIRE(D % 4 == 0 && D <= 1024 && (K & 1) == 1, "dwconv_ln_act: D %% 4, D <= 1024 and odd K required (D=%d K=%d)", D, K);
+    SBK_REQUIRE((reinterpret_cast<uintptr_t>(glu) & 15) == 0, "dwconv_ln_act: input must be 16-byte aligned");
+    const size_t smem = static_cast<size_t>(DW_TT + K - 1) * D * sizeof(float);
+    SBK_REQUIRE(smem <= 200 * 1024, "dwconv_ln_act: tile too large for shared memory (D=%d K=%d)", D, K);
+    const auto kern = gelu ? dwconv_kernel_for<true>(D, K, chunk) : dwconv_kernel_for<false>(D, K, chunk);
     SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<dim3(ceil_div(T, DW_TT), B), 256, smem, stream>>>(glu, T, D, K, wdw, bdw, gamma, beta, eps, out, chunk, left);
     SBK_LAUNCH_CHECK();
@@ -440,7 +454,7 @@ int dwconv_carry(const float* glu, int B, int n, int D, int K, bool has_old, flo
     return SBK_OK;
 }
 
-// (D, 1, K) reference taps -> tap-major [K, D] (the layout dwconv_ln_swish reads)
+// (D, 1, K) reference taps -> tap-major [K, D] (the layout dwconv_ln_act reads)
 void dwconv_repack_taps(const float* src, int D, int K, float* dst) {
     for (int ch = 0; ch < D; ++ch)
         for (int k = 0; k < K; ++k) dst[static_cast<size_t>(k) * D + ch] = src[static_cast<size_t>(ch) * K + k];

@@ -458,11 +458,14 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
     if (c.encoder_module == SBK_ENC_BRANCHFORMER) return run_branchformer_layers(m, B, T, enc_len, enc_out, st);
     if (c.encoder_module == SBK_ENC_TRANSFORMER) return run_transformer_layers(m, B, T, enc_len, enc_out, st);
     const float att_scale = 1.0f / sqrtf((float)d);  // nnet/attention.py:521,1272: 1/sqrt(embed_dim), not head_dim
+    // conformer_activation: both FFN modules' hidden activation and the convolution module's after the LayerNorm
+    const bool gelu = c.conformer_activation == SBK_CONFORMER_ACT_GELU;
+    const int ffn_act = gelu ? ACT_GELU : ACT_SILU;
     for (int l = 0; l < c.num_encoder_layers; ++l) {
         const EncLayerW& w = m->wt->enc[l];
         // --- ffn module 1 (Conformer.py:479); its LayerNorm was fused into the previous layer's norm2 kernel
         if (l == 0) RC(layernorm_rows(b.x, b.h16, true, w.ffn1_ln_g, w.ffn1_ln_b, M, d, 1e-5f, false, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ACT_SILU; e.bias = w.ffn1_b1; e.out = b.f16; e.ldo = F;
+        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ffn_act; e.bias = w.ffn1_b1; e.out = b.f16; e.ldo = F;
         RC(gemm_f16(b.h16, d, w.ffn1_w1, d, e, M, F, d, st));
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.ffn1_b2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 0.5f;
         RC(gemm_f16(b.f16, F, w.ffn1_w2, F, e, M, d, F, st));
@@ -507,19 +510,19 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
         RC(gemm_f16(b.h16, d, w.wpw1, d, e, M, 2 * d, d, st));
         if (s) {  // the chunk after the carry, zeros after the chunk (its right edge); then the carry moves on
             float* carry = s->carry_layer(c, l);
-            RC(dwconv_ln_swish(b.glu, B, T, d, c.kernel_size, w.wdw, w.bdw, w.aconv_ln_g, w.aconv_ln_b, 1e-5f, b.h16, st, 0,
-                               s->total > 0 ? carry : nullptr));
+            RC(dwconv_ln_act(b.glu, B, T, d, c.kernel_size, w.wdw, w.bdw, w.aconv_ln_g, w.aconv_ln_b, 1e-5f, b.h16, st, gelu, 0,
+                             s->total > 0 ? carry : nullptr));
             RC(dwconv_carry(b.glu, B, T, d, c.kernel_size, s->total > 0, carry, st));
         } else {
-            RC(dwconv_ln_swish(b.glu, B, T, d, c.kernel_size, w.wdw, w.bdw, w.aconv_ln_g, w.aconv_ln_b, 1e-5f, b.h16, st,
-                               m->dyn_chunk));
+            RC(dwconv_ln_act(b.glu, B, T, d, c.kernel_size, w.wdw, w.bdw, w.aconv_ln_g, w.aconv_ln_b, 1e-5f, b.h16, st, gelu,
+                             m->dyn_chunk));
         }
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bpw2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
         e.row_lens = enc_len; e.T = T;
         RC(gemm_f16(b.h16, d, w.wpw2, d, e, M, d, d, st));
         // --- ffn module 2 + norm2 (Conformer.py:498)
         RC(layernorm_rows(b.x, b.h16, true, w.ffn2_ln_g, w.ffn2_ln_b, M, d, 1e-5f, false, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ACT_SILU; e.bias = w.ffn2_b1; e.out = b.f16; e.ldo = F;
+        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ffn_act; e.bias = w.ffn2_b1; e.out = b.f16; e.ldo = F;
         RC(gemm_f16(b.h16, d, w.ffn2_w1, d, e, M, F, d, st));
         e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.ffn2_b2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 0.5f;
         RC(gemm_f16(b.f16, F, w.ffn2_w2, F, e, M, d, F, st));

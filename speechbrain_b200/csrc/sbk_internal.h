@@ -156,10 +156,11 @@ int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, cons
                      const HyperMixWeights& w, float* part, __half* G, float* gscale, float* x, cudaStream_t stream);
 size_t hypermix_part_floats(int B, int T, int d, int KH);
 // chunk > 0: Dynamic Chunk Convolution (inputs past the end of the output frame's chunk are zero).  left: [B, (K-1)/2, D]
-// inputs of the frames before frame 0 (a stream's carry), null = zero padding.
-int dwconv_ln_swish(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw,
-                    const float* gamma, const float* beta, float eps, __half* out, cudaStream_t stream, int chunk = 0,
-                    const float* left = nullptr);
+// inputs of the frames before frame 0 (a stream's carry), null = zero padding.  gelu: exact erf GELU after the LayerNorm,
+// else Swish (the Conformer's conformer_activation).
+int dwconv_ln_act(const float* glu, int B, int T, int D, int K, const float* wdw, const float* bdw, const float* gamma,
+                  const float* beta, float eps, __half* out, cudaStream_t stream, bool gelu, int chunk = 0,
+                  const float* left = nullptr);
 // carry [B, (K-1)/2, D] <- the last (K-1)/2 rows of [carry; glu [B, n, D]]; has_old false: the old carry counts as zeros
 int dwconv_carry(const float* glu, int B, int n, int D, int K, bool has_old, float* carry, cudaStream_t stream);
 void dwconv_repack_taps(const float* src, int D, int K, float* dst);  // (D, 1, K) -> tap-major [K, D] (host)

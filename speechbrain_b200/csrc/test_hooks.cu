@@ -214,9 +214,8 @@ int sbk_stream_qkv_test(const float* qkv_dev, int B, int n, int H, int head_dim,
     return finish_test("stream_qkv_test", rc, st);
 }
 
-int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
-                    const float* ln_g_dev, const float* ln_b_dev, int chunk, void* out_dev, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
+static int dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
+                       const float* ln_g_dev, const float* ln_b_dev, int chunk, bool gelu, void* out_dev, cudaStream_t st) {
     SBK_REQUIRE(x_dev && taps_dev && bias_dev && ln_g_dev && ln_b_dev && out_dev, "dwconv_test: null pointer");
     SBK_REQUIRE(B >= 1 && T >= 1 && D >= 1 && K >= 1 && chunk >= 0, "dwconv_test: bad sizes B=%d T=%d D=%d K=%d chunk=%d", B, T,
                 D, K, chunk);
@@ -229,8 +228,22 @@ int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float*
     RC(scr.carve("dwconv_test", [&](Carver& take) { take(taps, wt.size() * 4); }));
     int rc = cudaMemcpyAsync(taps, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice, st) == cudaSuccess ? SBK_OK : SBK_ERR_CUDA;
     if (rc == SBK_OK)
-        rc = dwconv_ln_swish(x_dev, B, T, D, K, taps, bias_dev, ln_g_dev, ln_b_dev, 1e-5f, static_cast<__half*>(out_dev), st, chunk);
+        rc = dwconv_ln_act(x_dev, B, T, D, K, taps, bias_dev, ln_g_dev, ln_b_dev, 1e-5f, static_cast<__half*>(out_dev), st, gelu,
+                           chunk);
     return finish_test("dwconv_test", rc, st);
+}
+
+int sbk_dwconv_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
+                    const float* ln_g_dev, const float* ln_b_dev, int chunk, void* out_dev, void* stream) {
+    return dwconv_test(x_dev, B, T, D, K, taps_dev, bias_dev, ln_g_dev, ln_b_dev, chunk, false, out_dev,
+                       static_cast<cudaStream_t>(stream));
+}
+
+int sbk_dwconv_act_test(const float* x_dev, int B, int T, int D, int K, const float* taps_dev, const float* bias_dev,
+                        const float* ln_g_dev, const float* ln_b_dev, int chunk, int act, void* out_dev, void* stream) {
+    SBK_REQUIRE(act == SBK_CONFORMER_ACT_SWISH || act == SBK_CONFORMER_ACT_GELU, "dwconv_act_test: act %d (0 Swish, 1 GELU)", act);
+    return dwconv_test(x_dev, B, T, D, K, taps_dev, bias_dev, ln_g_dev, ln_b_dev, chunk, act == SBK_CONFORMER_ACT_GELU, out_dev,
+                       static_cast<cudaStream_t>(stream));
 }
 
 int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int d, int nhead, int k, const float* w1_fc1_w_dev,

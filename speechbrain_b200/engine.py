@@ -75,7 +75,8 @@ class AsrEngine:
     ("RoPEMHA"|"RelPosMHAXL"|"hypermixing"|"regularMHA", hypermixing with the Conformer only, regularMHA with the Transformer
     only), decoder_activation ("gelu"|"relu"|"swish"), max_length; encoder_module ("conformer" (default) | "branchformer" |
     "transformer") with csgu_linear_units and branchformer_activation ("gelu" (default) | "relu"); cnn_blocks (2 (default),
-    or 3: the Transformer recipes' front-end, cnn_channels (64, 64)).
+    or 3: the Transformer recipes' front-end, cnn_channels (64, 64)); conformer_activation ("swish" (default) | "gelu": the
+    Conformer's FFN and convolution-module activation).
     ``state``: {reference key with recipe prefix: CPU fp32 tensor}."""
 
     def __init__(self, cfg, state, device="cuda", parts=("fbank", "cnn", "encoder", "decoder")):
@@ -105,6 +106,10 @@ class AsrEngine:
         if enc_module == "transformer":
             c.encoder_module = _lib.SBK_ENC_TRANSFORMER
         c.cnn_blocks = cfg.get("cnn_blocks", 2)
+        conformer_acts = {"swish": _lib.SBK_CONFORMER_ACT_SWISH, "gelu": _lib.SBK_CONFORMER_ACT_GELU}
+        if cfg.get("conformer_activation", "swish") not in conformer_acts:
+            raise NotImplementedError(f"conformer_activation={cfg['conformer_activation']!r}: only swish and gelu are built")
+        c.conformer_activation = conformer_acts[cfg.get("conformer_activation", "swish")]
         if enc_module == "branchformer":
             c.encoder_module, c.csgu_linear_units = _lib.SBK_ENC_BRANCHFORMER, cfg["csgu_linear_units"]
             c.branchformer_activation = (_lib.SBK_ACT_GELU if cfg.get("branchformer_activation", "gelu") == "gelu"

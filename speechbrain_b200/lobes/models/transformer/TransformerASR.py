@@ -6,7 +6,8 @@ hypermixing: HyperMixing token mixing, nnet/hypermixing.py, with head width d_mo
 d_ffn / nhead a multiple of 16 up to 256), or encoder_module="branchformer" with attention_type="RelPosMHAXL"
 (Branchformer.py:92-410), or encoder_module="transformer" with attention_type="regularMHA",
 positional_encoding="fixed_abs_sine" and normalize_before=True (Transformer.py:311-490, head width 64 or 128); causal=False.
-The decoder's FFN activation is GELU, ReLU or Swish / SiLU.
+The decoder's FFN activation is GELU, ReLU or Swish / SiLU; the Conformer's (conformer_activation) is Swish / SiLU or
+torch.nn.GELU (exact erf, the Loquacious recipes).
 
 Same constructor kwargs, same state_dict keys (incl. the positional buffers), ``encode()`` on the sm_90a
 kernels.  ``decode()`` / ``forward()`` run teacher-forced on the KV-cached decoder step (the searchers in
@@ -92,8 +93,13 @@ class TransformerASR(torch.nn.Module):
             unsupported.append("bias=False")
         if output_hidden_states:
             unsupported.append("output_hidden_states=True")
-        if encoder_module == "conformer" and conformer_activation is not None and getattr(conformer_activation, "__name__", "") not in ("Swish", "SiLU"):
-            unsupported.append("conformer_activation other than Swish")
+        conf_act = "swish"
+        if encoder_module == "conformer" and conformer_activation is not None:
+            # torch.nn.GELU itself is the exact erf form; a partial or subclass (e.g. approximate="tanh") is another function
+            if conformer_activation is torch.nn.GELU:
+                conf_act = "gelu"
+            elif getattr(conformer_activation, "__name__", "") not in ("Swish", "SiLU"):
+                unsupported.append("conformer_activation other than Swish or torch.nn.GELU")
         if encoder_module != "transformer" and (d_model % nhead or d_model // nhead not in (64, 36, 32)):
             if not (encoder_module == "conformer" and attention_type == "RelPosMHAXL" and d_model == 80 * nhead):
                 unsupported.append(f"head_dim={d_model // max(nhead, 1)} (64, 36 or 32; 80 for the Conformer with RelPosMHAXL)")
@@ -111,6 +117,7 @@ class TransformerASR(torch.nn.Module):
         self.kernel_size, self.attention_type, self.max_length, self.causal = kernel_size, attention_type, max_length, causal
         self.positional_encoding_type = positional_encoding
         self.encoder_module, self.csgu_linear_units, self.branchformer_activation = encoder_module, csgu_linear_units, bf_act
+        self.conformer_activation = conf_act
         build_param_tree(self, transformer_asr_shapes(tgt_vocab, input_size, d_model, nhead, num_encoder_layers,
                                                       num_decoder_layers, d_ffn, kernel_size, attention_type, encoder_module,
                                                       csgu_linear_units), default_init)
@@ -146,7 +153,8 @@ class TransformerASR(torch.nn.Module):
                     kernel_size=self.kernel_size, attention_type=self.attention_type,
                     decoder_activation=self.decoder_activation, max_length=self.max_length,
                     encoder_module=self.encoder_module, csgu_linear_units=self.csgu_linear_units,
-                    branchformer_activation=self.branchformer_activation)
+                    branchformer_activation=self.branchformer_activation,
+                    conformer_activation=self.conformer_activation)
 
     def prefixed_state(self, prefix="Transformer."):
         return {prefix + k: v for k, v in self.state_dict().items()}

@@ -142,3 +142,16 @@ CONFORMER_640 = dict(name="conformer_640", sample_rate=16000, n_fft=512, win=512
                      num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="RelPosMHAXL",
                      decoder_activation="gelu", max_length=2500)
 CONFORMER_640_PEOPLES = dict(CONFORMER_640, name="conformer_640_peoples", vocab=5120, decoder_activation="swish")
+# recipes/Loquacious/ASR/transformer/hparams/conformer_{small,base,large,xlarge}.yaml: Conformer encoders with
+# conformer_activation=torch.nn.GELU and RelPosMHAXL (head width 64), GELU decoders, Fbank with n_fft 400 and the default
+# 25 ms window; xlarge is the released 480M model.  Token indices: blank 3, bos 1, eos 2, pad 0.
+LOQUACIOUS_SMALL = dict(name="loquacious_small", sample_rate=16000, n_fft=400, win=400, hop=160, n_mels=80,
+                        cnn_channels=(64, 32), input_size=640, d_model=256, nhead=4, num_encoder_layers=12,
+                        num_decoder_layers=6, d_ffn=1024, vocab=1024, kernel_size=31, attention_type="RelPosMHAXL",
+                        decoder_activation="gelu", max_length=2500, conformer_activation="gelu")
+LOQUACIOUS_BASE = dict(LOQUACIOUS_SMALL, name="loquacious_base", d_model=512, nhead=8, d_ffn=2048, vocab=5120)
+LOQUACIOUS_LARGE = dict(LOQUACIOUS_SMALL, name="loquacious_large", d_model=768, nhead=12, num_encoder_layers=14,
+                        d_ffn=3072, vocab=5120)
+LOQUACIOUS_XLARGE = dict(LOQUACIOUS_SMALL, name="loquacious_xlarge", d_model=1024, nhead=16, num_encoder_layers=18,
+                         d_ffn=3072, vocab=5120)
+LOQUACIOUS_BLANK, LOQUACIOUS_BOS, LOQUACIOUS_EOS, LOQUACIOUS_PAD = 3, 1, 2, 0
