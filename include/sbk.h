@@ -210,6 +210,36 @@ int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int 
                       const float* w2_fc1_b_dev, const float* w2_fc2_w_dev, const float* w2_fc2_b_dev, const float* ln_g_dev,
                       const float* ln_b_dev, float* out_dev, void* stream);
 
+/* one beam-search step alone (beam_step: S2SBeamSearcher.search_step, decoders/seq2seq.py:1478-1598, with the scorers'
+ * scores precomputed), on caller buffers, n_bh = B * beam_size rows.  From params: beam_size, min_steps, eos, temperature,
+ * using_eos_threshold, eos_threshold, length_normalization, minus_inf, length_weight (added to every token), and with
+ * ctc_weight != 0 blank_index (masked to minus_inf) and the decoder weight 1 - ctc_weight.  path 0 picks the kernels by
+ * width, 1 the rows + merge kernels (beam_size <= 16), 2 the radix select.  logits_dev [n_bh, V]; seq_scores_dev [2][n_bh]
+ * and lineage_dev [2][n_bh][S_max] ping-pong by step parity; step_dev [n_bh] (one step per utterance, step + 1 < S_max and
+ * step < n_hist; advanced by one); finished_dev [B] (eos hypotheses, capped at beam_size) and n_full_dev (utterances whose
+ * counter reached beam_size); hist_{tok,pred,score,lp}_dev [n_hist][n_bh] (row `step` written); add_scores_dev [n_bh, V]
+ * and add_row_dev [n_bh] optional; x_next_dev [n_bh, d] = emb_dev[token] * sqrt(d) + pe_dev[step + 1] (pe [S_max, d]).  With
+ * lm_emb_dev: lm_x_dev fp32 and lm_x16_dev fp16 (saturating) [n_bh, lm_d] from lm_emb_dev / lm_pe_dev the same way, and the
+ * token at tok_cache_dev[row * S_max + step + 1].  Every lineage entry in [0, n_bh).  Synchronises the stream. */
+int sbk_beam_step_test(const sbk_beam_params* params, int path, int B, int V, int S_max, int n_hist, const float* logits_dev,
+                       float* seq_scores_dev, int* lineage_dev, int* step_dev, int* finished_dev, int* n_full_dev,
+                       int* hist_tok_dev, int* hist_pred_dev, float* hist_score_dev, float* hist_lp_dev,
+                       const float* add_scores_dev, const float* add_row_dev, const float* emb_dev, const float* pe_dev, int d,
+                       float* x_next_dev, const float* lm_emb_dev, const float* lm_pe_dev, int lm_d, float* lm_x_dev,
+                       void* lm_x16_dev, int* tok_cache_dev, void* stream);
+
+/* the CoverageScorer step alone (coverage_score, decoders/scorer.py:788-955): row r of utterance u = r / rows_per_utt
+ * attends with q_dev fp16 (head h at q_dev[r * ldq + h * 64], scale folded in) to the first enc_len_dev[u] of T keys, key
+ * t of head h at kbase_dev[u * utt_stride + h * head_stride + t * key_stride] fp16 (head_stride 0 = 64, 16-byte aligned
+ * rows); coverage = the head average of that attention + the coverage of its predecessor hist_pred_dev[(step - 1) * n_bh +
+ * r] (step > 0) from cov_dev [2][n_bh][T] (ping-pong by step parity, step from step_dev [n_bh], the same in every row) ->
+ * out_dev[r] = weight * -(sum_t max(coverage_t, threshold) - T * threshold) / (step + 1).  A row with no visible key has
+ * NaN coverage and score, as in the reference.  T * 8 <= 96 KB.  Synchronises the stream. */
+int sbk_coverage_score_test(const void* q_dev, int ldq, const void* kbase_dev, long long utt_stride, int key_stride,
+                            int head_stride, const int* enc_len_dev, int rows_per_utt, int T, int H, float* cov_dev,
+                            const int* hist_pred_dev, const int* step_dev, int n_bh, float threshold, float weight, float* out_dev,
+                            void* stream);
+
 /* ---- model handle: repacks the reference state_dict once */
 int sbk_asr_create(const sbk_asr_config* cfg, const sbk_tensor* weights, int n_weights, sbk_asr** out);
 void sbk_asr_destroy(sbk_asr* m);

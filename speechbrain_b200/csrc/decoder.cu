@@ -794,7 +794,9 @@ struct BeamArgs {
 
 // Two kernels.  beam_rows_kernel, one CTA per hypothesis row (B * beam CTAs instead of B): the row's log-sum-exp, masked eos
 // log-prob and its own top-`beam` candidates under the final score -- the utterance's top-`beam` of beam * V is a subset
-// of the union of the rows' top-`beam` (same order: score descending, candidate index ascending).  beam_merge_kernel, one
+// of the union of the rows' top-`beam`.  Both kernels rank candidates in argmax_takes's order: NaN first whatever its sign,
+// then score descending, then candidate index ascending; every candidate counts, -inf ones included, so that an utterance
+// with fewer than `beam` finite candidates takes real (token, row) pairs as torch.topk does.  beam_merge_kernel, one
 // CTA per utterance: ranks the beam * beam survivors, then does the bookkeeping.  Scratch: [n_bh][BS_MAXB] scores,
 // [n_bh][BS_MAXB] candidate indices (k * V + token), [n_bh] log-sum-exp.
 __global__ void __launch_bounds__(BS_THREADS) beam_rows_kernel(const BeamArgs a) {
@@ -870,12 +872,12 @@ __global__ void __launch_bounds__(BS_THREADS) beam_rows_kernel(const BeamArgs a)
             if (a.add_row) lp += add_row;
         }
         const float sc = (seq + lp) * inv_len;
-        if (sc > bv[BS_MAXB - 1] && sc > -INFINITY) {  // insert (list sorted descending; only the first `beam` matter)
+        int ix = k * V + j;
+        if (argmax_takes(sc, ix, bv[BS_MAXB - 1], bi[BS_MAXB - 1])) {  // insert (list in candidate order; first `beam` matter)
             float v = sc;
-            int ix = k * V + j;
 #pragma unroll
             for (int i = 0; i < BS_MAXB; ++i) {
-                if (v > bv[i] || (v == bv[i] && ix < bi[i])) {
+                if (argmax_takes(v, ix, bv[i], bi[i])) {
                     const float tv = bv[i]; const int ti = bi[i];
                     bv[i] = v; bi[i] = ix;
                     v = tv; ix = ti;
@@ -899,7 +901,7 @@ __global__ void __launch_bounds__(BS_THREADS) beam_rows_kernel(const BeamArgs a)
             const float ov = __shfl_xor_sync(0xffffffffu, v, o);
             const int oi = __shfl_xor_sync(0xffffffffu, ix, o);
             const int ow = __shfl_xor_sync(0xffffffffu, who, o);
-            if (ov > v || (ov == v && (oi < ix || (oi == ix && ow < who)))) { v = ov; ix = oi; who = ow; }
+            if (argmax_takes(ov, oi, v, ix) || (oi == ix && ow < who)) { v = ov; ix = oi; who = ow; }
         }
         if (lane == 0) { s_red[warp] = v; s_redi[warp] = who; s_redx[warp] = ix; }
         __syncthreads();
@@ -907,7 +909,7 @@ __global__ void __launch_bounds__(BS_THREADS) beam_rows_kernel(const BeamArgs a)
             float best = s_red[0];
             int bw = s_redi[0], bx = s_redx[0];
             for (int w = 1; w < BS_THREADS / 32; ++w)
-                if (s_red[w] > best || (s_red[w] == best && s_redx[w] < bx)) { best = s_red[w]; bw = s_redi[w]; bx = s_redx[w]; }
+                if (argmax_takes(s_red[w], s_redx[w], best, bx)) { best = s_red[w]; bw = s_redi[w]; bx = s_redx[w]; }
             s_redi[0] = bw;
             a.scr_val[row * BS_MAXB + r] = best;
             a.scr_idx[row * BS_MAXB + r] = bx;
@@ -944,7 +946,7 @@ __global__ void __launch_bounds__(BS_THREADS) beam_merge_kernel(const BeamArgs a
         for (int j = 0; j < n; ++j) {
             const float ov = s_v[j];
             const int oi = s_i[j];
-            rank += (ov > v || (ov == v && (oi < ix || (oi == ix && j < tid)))) ? 1 : 0;
+            rank += (argmax_takes(ov, oi, v, ix) || (oi == ix && j < tid)) ? 1 : 0;
         }
         if (rank < beam) {
             int kk = 0, tok = 0;
@@ -1029,7 +1031,8 @@ __global__ void __launch_bounds__(256) coverage_score_kernel(const CoverageArgs 
     const int utt = r / a.rows_per_utt;
     const int n_keys = min(a.enc_len[utt], T);
     const int step = a.step_ptr[r];
-    for (int t = tid; t < T; t += 256) s_avg[t] = 0.0f;
+    // no visible key: the reference's attention row is NaN (nn.MultiheadAttention), and so are the coverage and the score
+    for (int t = tid; t < T; t += 256) s_avg[t] = n_keys > 0 ? 0.0f : NAN;
     for (int h = 0; h < a.H; ++h) {
         __syncthreads();
         if (tid < 64) s_q[tid] = __half2float(a.q[static_cast<size_t>(r) * a.ldq + h * 64 + tid]);
@@ -1082,7 +1085,7 @@ __global__ void __launch_bounds__(256) coverage_score_kernel(const CoverageArgs 
     for (int t = tid; t < T; t += 256) {
         const float c = (step == 0 ? 0.0f : cov_in[static_cast<size_t>(prow) * T + t]) + s_avg[t];
         cov_out[static_cast<size_t>(r) * T + t] = c;
-        pen += fmaxf(c, a.threshold);
+        pen += c < a.threshold ? a.threshold : c;   // torch.max: a NaN coverage stays NaN
     }
     pen = warp_sum(pen);
     if ((tid & 31) == 0) s_red[tid >> 5] = pen;
@@ -1121,7 +1124,9 @@ int coverage_score(const CoverageStep& p, cudaStream_t stream) {
 constexpr int BL_MAXB = 128;
 constexpr int BL_TIECAP = 1024;
 
-__device__ __forceinline__ uint32_t score_key(float v) {  // larger score <-> larger key; -inf is the smallest finite key
+// larger score <-> larger key, -inf the smallest; every NaN, whatever its sign, maps to the largest key (argmax_takes's order)
+__device__ __forceinline__ uint32_t score_key(float v) {
+    if (isnan(v)) return 0xFFFFFFFFu;
     const uint32_t u = __float_as_uint(v);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
@@ -1226,7 +1231,10 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
         }
     }
     __syncthreads();
-    {   // the lowest-index `remaining` ties complete the selection (ties beyond BL_TIECAP cannot occur with finite scores)
+    // the lowest-index `remaining` ties complete the selection.  Past BL_TIECAP ties (a row of equal logits gives V of them)
+    // the buffer keeps the first to arrive, which the scan order makes the lowest-index ones unless a warp lags four
+    // passes behind the others; test_gpu_beam_step.py checks a flat row at V = 5000.
+    {
         const int nsel = min(s_nsel, BL_MAXB), ntie = min(s_ntie, BL_TIECAP), want = min(s_remaining, beam - nsel);
         const float tv = [&] { const uint32_t k = thr; const uint32_t u = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k; return __uint_as_float(u); }();
         for (int r = 0; r < want; ++r) {
@@ -1260,7 +1268,7 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
                 if (ixj > tid) {
                     const float v0 = s_selv[tid], v1 = s_selv[ixj];
                     const int i0 = s_seli[tid], i1 = s_seli[ixj];
-                    const bool first_after = (v0 < v1) || (v0 == v1 && i0 > i1);  // element at tid should come after ixj
+                    const bool first_after = argmax_takes(v1, i1, v0, i0);  // element at tid should come after ixj
                     const bool up = (tid & k2) == 0;
                     if (first_after == up) { s_selv[tid] = v1; s_selv[ixj] = v0; s_seli[tid] = i1; s_seli[ixj] = i0; }
                 }
@@ -1364,6 +1372,9 @@ int beam_reset(int n_bh, int beam, int S_max, int bos, int* step_arr, float* seq
 int beam_step(const BeamStepArgs& p, int B, cudaStream_t stream) {
     SBK_REQUIRE(p.beam >= 1 && p.beam <= BL_MAXB, "beam_step: beam_size=%d not in [1, %d]", p.beam, BL_MAXB);
     SBK_REQUIRE(p.beam <= p.V, "beam_step: beam_size=%d exceeds the vocabulary (%d)", p.beam, p.V);
+    SBK_REQUIRE(p.path >= 0 && p.path <= 2, "beam_step: path %d (0 by width, 1 rows + merge, 2 radix select)", p.path);
+    SBK_REQUIRE(p.path != 1 || p.beam <= BS_MAXB, "beam_step: the rows + merge kernels take beam_size <= %d, not %d", BS_MAXB,
+                p.beam);
     BeamArgs a;
     a.logits = p.logits; a.V = p.V; a.beam = p.beam; a.n_bh = B * p.beam; a.S_max = p.S_max;
     a.seq_scores = p.seq_scores; a.lineage = p.lineage; a.step_arr = p.step_arr; a.finished = p.finished; a.n_full = p.n_full;
@@ -1375,8 +1386,8 @@ int beam_step(const BeamStepArgs& p, int B, cudaStream_t stream) {
     a.lm_emb = p.lm.emb; a.lm_pe = p.lm.pe; a.lm_d = p.lm.d; a.lm_sqrt_d = p.lm.d ? sqrtf(static_cast<float>(p.lm.d)) : 0.f;
     a.lm_x_next = p.lm.x; a.lm_x16_next = p.lm.x16; a.tok_cache = p.lm.tok_cache;
     a.scr_val = nullptr; a.scr_idx = nullptr; a.scr_lse = nullptr;
-    static const bool force_large = getenv("SBK_BEAM_RADIX") != nullptr;  // test hook: radix-select kernel for every width
-    if (p.beam > BS_MAXB || force_large) SBK_CUDA_CHECK(launch_k(beam_step_large_kernel, dim3(B), dim3(BS_THREADS), 0, stream, a));
+    if (p.path == 2 || (p.path == 0 && p.beam > BS_MAXB))
+        SBK_CUDA_CHECK(launch_k(beam_step_large_kernel, dim3(B), dim3(BS_THREADS), 0, stream, a));
     else {
         SBK_REQUIRE(p.scratch != nullptr, "beam_step: no scratch buffer");
         a.scr_val = p.scratch; a.scr_idx = reinterpret_cast<int*>(p.scratch + (size_t)a.n_bh * BS_MAXB);

@@ -238,6 +238,7 @@ struct BeamStepArgs {
     float add_const = 0.0f;    // LengthScorer: weight * 1 added to every token (scorer.py:1043-1071)
     const float* add_row = nullptr;  // CoverageScorer: [n_bh] weighted score added to every token of a hypothesis
     float* scratch = nullptr;        // [n_bh * 33] floats: per-row candidates between the two kernels of a step (beam <= 16)
+    int path = 0;  // 0: by width (rows + merge up to beam 16, radix select above), 1: rows + merge, 2: radix select
 };
 // CoverageScorer (decoders/scorer.py:788-955) on the last decoder layer's head-averaged cross-attention
 struct CoverageStep {

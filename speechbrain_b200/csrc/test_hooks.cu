@@ -285,4 +285,94 @@ int sbk_hypermix_test(const void* x_dev, const int* lens_dev, int B, int T, int 
     return finish_test("hypermix_test", rc, st);
 }
 
+int sbk_beam_step_test(const sbk_beam_params* params, int path, int B, int V, int S_max, int n_hist, const float* logits_dev,
+                       float* seq_scores_dev, int* lineage_dev, int* step_dev, int* finished_dev, int* n_full_dev,
+                       int* hist_tok_dev, int* hist_pred_dev, float* hist_score_dev, float* hist_lp_dev,
+                       const float* add_scores_dev, const float* add_row_dev, const float* emb_dev, const float* pe_dev, int d,
+                       float* x_next_dev, const float* lm_emb_dev, const float* lm_pe_dev, int lm_d, float* lm_x_dev,
+                       void* lm_x16_dev, int* tok_cache_dev, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(params && logits_dev && seq_scores_dev && lineage_dev && step_dev && finished_dev && n_full_dev && hist_tok_dev &&
+                    hist_pred_dev && hist_score_dev && hist_lp_dev && emb_dev && pe_dev && x_next_dev,
+                "beam_step_test: null pointer");
+    const sbk_beam_params& p = *params;
+    const int beam = p.beam_size;
+    SBK_REQUIRE(B >= 1 && V >= 1 && S_max >= 2 && n_hist >= 1 && d >= 1, "beam_step_test: bad sizes B=%d V=%d S_max=%d n_hist=%d d=%d",
+                B, V, S_max, n_hist, d);
+    SBK_REQUIRE(beam >= 1 && beam <= 128 && beam <= V, "beam_step_test: beam_size %d not in [1, min(128, V = %d)]", beam, V);
+    SBK_REQUIRE(path >= 0 && path <= 2 && !(path == 1 && beam > 16), "beam_step_test: path %d at beam_size %d", path, beam);
+    SBK_REQUIRE(p.eos >= 0 && p.eos < V, "beam_step_test: eos %d outside [0, %d)", p.eos, V);
+    SBK_REQUIRE(p.ctc_weight == 0.0f || (p.blank_index >= 0 && p.blank_index < V && p.blank_index != p.eos),
+                "beam_step_test: blank %d must be a token other than eos", p.blank_index);
+    const bool lm = lm_emb_dev != nullptr;
+    SBK_REQUIRE(!lm || (lm_pe_dev && lm_x_dev && lm_x16_dev && tok_cache_dev && lm_d >= 1), "beam_step_test: incomplete LM buffers");
+    const int rows = B * beam;
+    // the kernels index the history, the lineage, the positional tables and the token cache with these: check them first
+    std::vector<int> step((size_t)rows), lin((size_t)2 * rows * S_max);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(step.data(), step_dev, step.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(lin.data(), lineage_dev, lin.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int r = 0; r < rows; ++r) {
+        const int s = step[r];
+        SBK_REQUIRE(s == step[r - r % beam], "beam_step_test: rows of utterance %d at steps %d and %d", r / beam, step[r - r % beam], s);
+        SBK_REQUIRE(s >= 0 && s + 1 < S_max && s < n_hist, "beam_step_test: step %d outside [0, min(S_max - 1 = %d, n_hist = %d))", s,
+                    S_max - 1, n_hist);
+    }
+    for (size_t i = 0; i < lin.size(); ++i)
+        SBK_REQUIRE(lin[i] >= 0 && lin[i] < rows, "beam_step_test: lineage entry %zu = %d outside [0, %d)", i, lin[i], rows);
+    float* scr = nullptr;
+    TestScratch scratch;
+    const bool rows_merge = path == 1 || (path == 0 && beam <= 16);
+    RC(scratch.carve("beam_step_test", [&](Carver& take) { if (rows_merge) take(scr, (size_t)rows * 33 * 4); }));
+    BeamStepArgs a{};   // as run_beam fills it
+    a.logits = logits_dev; a.V = V; a.beam = beam; a.S_max = S_max; a.seq_scores = seq_scores_dev; a.lineage = lineage_dev;
+    a.step_arr = step_dev; a.finished = finished_dev; a.n_full = n_full_dev;
+    a.hist_tok = hist_tok_dev; a.hist_pred = hist_pred_dev; a.hist_score = hist_score_dev; a.hist_lp = hist_lp_dev;
+    a.temperature = p.temperature; a.eos_threshold = p.eos_threshold; a.minus_inf = p.minus_inf; a.min_steps = p.min_steps;
+    a.eos = p.eos; a.use_eos_threshold = p.using_eos_threshold; a.length_norm = p.length_normalization;
+    a.emb = emb_dev; a.pe = pe_dev; a.d = d; a.x_next = x_next_dev;
+    a.add_scores = add_scores_dev; a.add_row = add_row_dev; a.add_const = p.length_weight;
+    if (p.ctc_weight != 0.0f) { a.attn_weight = 1.0f - p.ctc_weight; a.blank = p.blank_index; }
+    if (lm) {
+        a.lm.emb = lm_emb_dev; a.lm.pe = lm_pe_dev; a.lm.d = lm_d; a.lm.x = lm_x_dev; a.lm.x16 = static_cast<__half*>(lm_x16_dev);
+        a.lm.tok_cache = tok_cache_dev;
+    }
+    a.scratch = scr; a.path = path;
+    return finish_test("beam_step_test", beam_step(a, B, st), st);
+}
+
+int sbk_coverage_score_test(const void* q_dev, int ldq, const void* kbase_dev, long long utt_stride, int key_stride,
+                            int head_stride, const int* enc_len_dev, int rows_per_utt, int T, int H, float* cov_dev,
+                            const int* hist_pred_dev, const int* step_dev, int n_bh, float threshold, float weight, float* out_dev,
+                            void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(q_dev && kbase_dev && enc_len_dev && cov_dev && hist_pred_dev && step_dev && out_dev, "coverage_test: null pointer");
+    SBK_REQUIRE(n_bh >= 1 && rows_per_utt >= 1 && n_bh % rows_per_utt == 0 && H >= 1 && ldq >= H * 64 && T >= 1 &&
+                    utt_stride >= 0 && key_stride >= 1 && head_stride >= 0,
+                "coverage_test: bad sizes n_bh=%d rows_per_utt=%d H=%d T=%d", n_bh, rows_per_utt, H, T);
+    const uintptr_t al = reinterpret_cast<uintptr_t>(kbase_dev);   // 16-byte key loads
+    SBK_REQUIRE((al & 15) == 0 && utt_stride % 8 == 0 && key_stride % 8 == 0 && head_stride % 8 == 0,
+                "coverage_test: key rows must be 16-byte aligned");
+    // the kernel indexes frames, the coverage rows and the history with these: check them first
+    std::vector<int> len(n_bh / rows_per_utt), step(n_bh);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), enc_len_dev, len.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(step.data(), step_dev, step.size() * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int v : len) SBK_REQUIRE(v >= 0 && v <= T, "coverage_test: enc_len %d outside [0, %d]", v, T);
+    for (int s : step) SBK_REQUIRE(s == step[0] && s >= 0, "coverage_test: rows at steps %d and %d", step[0], s);
+    if (step[0] > 0) {
+        std::vector<int> pred(n_bh);
+        SBK_CUDA_CHECK(cudaMemcpyAsync(pred.data(), hist_pred_dev + (size_t)(step[0] - 1) * n_bh, pred.size() * 4,
+                                       cudaMemcpyDeviceToHost, st));
+        SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+        for (int v : pred) SBK_REQUIRE(v >= 0 && v < n_bh, "coverage_test: predecessor %d outside [0, %d)", v, n_bh);
+    }
+    CoverageStep c{};
+    c.q = static_cast<const __half*>(q_dev); c.ldq = ldq; c.kbase = static_cast<const __half*>(kbase_dev);
+    c.utt_stride = (size_t)utt_stride; c.key_stride = key_stride; c.head_stride = head_stride; c.enc_len = enc_len_dev;
+    c.rows_per_utt = rows_per_utt; c.T = T; c.H = H; c.cov_base = cov_dev; c.hist_pred = hist_pred_dev; c.step_ptr = step_dev;
+    c.n_bh = n_bh; c.threshold = threshold; c.weight = weight; c.out = out_dev;
+    return finish_test("coverage_test", coverage_score(c, st), st);
+}
+
 }  // extern "C"

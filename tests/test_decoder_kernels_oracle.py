@@ -219,3 +219,118 @@ def test_zero_length_utterance_oracle():
     hyps, _, scores, _ = O.greedy_search(enc, torch.tensor([1.0, 0.0, 0.6]), sd, cfg, seq_w, seq_b, 1, 2)
     assert hyps[1] == [0] * T and torch.isnan(scores[1, 0]).all()
     assert torch.isfinite(scores[0, 0]).all() and torch.isfinite(scores[2, 0]).all()
+
+
+# ------------------------------------------------------------------------------------------------ beam step
+@pytest.fixture(scope="module")
+def small_model():
+    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
+    cfg = dict(CONFORMER_LARGE, num_encoder_layers=1, num_decoder_layers=2)
+    return cfg, seeded_asr_state(cfg, 0)
+
+
+def _beam_by_steps(enc, wav_len, sd, cfg, beam, max_steps, ctc=None, length_weight=0.0, coverage=None):
+    """oracle.asr_oracle.beam_search's loop with every step's selection and bookkeeping from DK.beam_step_ref (and the
+    coverage from DK.coverage_ref): -> (history [(tok, pred, score, lp)], smallest gap between the beam-th and the
+    (beam + 1)-th candidate of any utterance and step, relative to the scores' scale)"""
+    B, T, _ = enc.shape
+    V, n_bh = sd["seq_lin.w.weight"].shape[0], B * beam
+    enc_lens = torch.round(T * wav_len).int()
+    enc_r, enc_l = enc.repeat_interleave(beam, dim=0), enc_lens.repeat_interleave(beam, dim=0)
+    seq = torch.full((n_bh,), float("-inf"), dtype=torch.float64)
+    seq[::beam] = 0.0
+    memory = torch.full((n_bh, 1), 1, dtype=torch.long)
+    finished = torch.zeros(B, dtype=torch.long)
+    cov = torch.zeros(n_bh, T, dtype=torch.float64)
+    kw = {}
+    if ctc is not None:
+        kw = dict(ctc_weight=ctc["weight"], blank=ctc["blank_index"])
+        st = O.ctc_prefix_reset(torch.log_softmax(enc @ ctc["w"].T + ctc["b"], dim=-1), enc_lens, ctc["blank_index"], 2)
+        mem = None
+    hist, gap = [], float("inf")
+    for step in range(max_steps):
+        if bool((finished == beam).all()):
+            break
+        pred_out, attn = O.decode(memory, enc_r, enc_l, sd, cfg, "Transformer.")
+        logits = pred_out[:, -1] @ sd["seq_lin.w.weight"].T + sd["seq_lin.w.bias"]
+        add = add_row = None
+        if ctc is not None:
+            score, mem = O.ctc_prefix_step(st, memory[:, -1], mem, beam)
+            add = ctc["weight"] * score
+        if coverage is not None:
+            c, add_row = DK.coverage_ref(attn[:, -1], cov, step, coverage["threshold"], coverage["weight"])
+        r = DK.beam_step_ref(logits, seq, step, beam, 2, using_eos_threshold=True, eos_threshold=1.5, add_scores=add,
+                             add_row=add_row, length_weight=length_weight, finished=finished, **kw)
+        flat = r["sc"].view(B, -1)
+        top = flat.topk(beam + 1, dim=-1).values
+        scale = top[:, 0].abs().clamp_min(1.0)
+        gap = min(gap, float(((top[:, beam - 1] - top[:, beam]) / scale).min()))
+        if ctc is not None:
+            mem = O.ctc_prefix_permute(st, mem, ((r["pred"] % beam) * V + r["tok"]).view(B, beam))
+        if coverage is not None:
+            cov = c[r["pred"]]
+        memory = torch.cat([memory[r["pred"]], r["tok"].view(n_bh, 1)], dim=1)
+        seq, finished = r["seq"], r["finished"]
+        hist.append((r["tok"], r["pred"], r["score"], r["lp"]))
+    return hist, gap
+
+
+BEAM_SCORERS = ["none", "ctc", "length", "coverage"]
+SEED_SHIFT = {(20, "ctc"): 300}   # the first seed of this case has a near-tie at the beam boundary
+
+
+@pytest.mark.parametrize("scorer", BEAM_SCORERS)
+@pytest.mark.parametrize("beam", [4, 20])
+def test_beam_step_vs_oracle(small_model, beam, scorer):
+    """Conformer-L with 2 decoder layers (seeded), 2 utterances of 12 and 7 frames, 6 steps: DK.beam_step_ref driven one
+    step at a time reproduces O.beam_search's history, tokens and predecessors exactly and scores and log-probs within fp32
+    rounding (the oracle runs in fp32), on a case whose beam boundary has no near-tie."""
+    cfg, sd = small_model
+    g = torch.Generator().manual_seed(beam * 7 + len(scorer) + SEED_SHIFT.get((beam, scorer), 0))
+    enc = torch.randn(2, 12, cfg["d_model"], generator=g)
+    wl = torch.tensor([1.0, 0.6])
+    steps = 6
+    ctc = dict(w=sd["ctc_lin.w.weight"], b=sd["ctc_lin.w.bias"], weight=0.4, blank_index=0) if scorer == "ctc" else None
+    cov = dict(weight=0.5, threshold=0.3) if scorer == "coverage" else None
+    lw = 0.7 if scorer == "length" else 0.0
+    with torch.no_grad():
+        *_, ref = O.beam_search(enc, wl, sd, cfg, sd["seq_lin.w.weight"], sd["seq_lin.w.bias"], 1, 2, beam, 0.0,
+                                (steps + 0.5) / 12, prefix="Transformer.", return_history=True, ctc=ctc, length_weight=lw,
+                                coverage=cov)
+        got, gap = _beam_by_steps(enc, wl, sd, cfg, beam, steps, ctc=ctc, length_weight=lw, coverage=cov)
+    assert gap > 1e-5, f"near-tie at the beam boundary ({gap:.2e}): the case would pin fp32 noise"
+    assert len(got) == len(ref) and len(ref) >= 1
+    for s, (a, b) in enumerate(zip(got, ref)):
+        assert torch.equal(a[0], b[0].long()) and torch.equal(a[1], b[1].long()), f"step {s}"
+        for x, y, what in ((a[2], b[2], "score"), (a[3], b[3], "lp")):
+            fin = torch.isfinite(y)
+            assert torch.equal(fin, torch.isfinite(x)), f"step {s} {what}"
+            err = float(((x[fin] - y[fin].double()).abs() / y[fin].double().abs().clamp_min(1.0)).max()) if fin.any() else 0.0
+            assert err <= 2e-5, f"step {s} {what}: {err:.2e}"
+
+
+def test_beam_step_ref_order():
+    """candidate_order: NaN (either sign) first, lowest index first among NaN, among equal scores and among -inf"""
+    nan, inf = float("nan"), float("inf")
+    neg_nan = -torch.tensor(nan)
+    sc = torch.tensor([[1.0, nan, 2.0, float(neg_nan), 2.0, -inf, inf, -inf]], dtype=torch.float64)
+    assert DK.candidate_order(sc)[0].tolist() == [1, 3, 6, 2, 4, 0, 5, 7]
+    r = DK.beam_step_ref(torch.full((2, 5), -inf), torch.tensor([0.0, -inf]), 0, 2, 2)   # every log-prob NaN
+    assert r["tok"].tolist() == [0, 1] and r["pred"].tolist() == [0, 0] and torch.isnan(r["score"]).all()
+    lg = torch.tensor([[0.0, 0.0, -inf, -inf], [0.0, 0.0, 0.0, 0.0]])
+    r = DK.beam_step_ref(lg, torch.tensor([0.0, -inf]), 0, 2, 3, length_normalization=False, minus_inf=-inf)
+    assert r["tok"].tolist() == [0, 1]
+    r = DK.beam_step_ref(lg, torch.tensor([-inf, -inf]), 3, 2, 3, finished=torch.tensor([1]))   # only -inf candidates
+    assert r["tok"].tolist() == [0, 1] and r["pred"].tolist() == [0, 0] and r["finished"].tolist() == [1]
+
+
+def test_coverage_ref_empty_row():
+    """a row with no visible key: NaN coverage and score; others finite; coverage accumulates over the predecessor's"""
+    g = torch.Generator().manual_seed(3)
+    q, K = torch.randn(4, 2, 8, generator=g), torch.randn(2, 5, 2, 8, generator=g)
+    att = DK.cross_attention_probs(q, K, torch.tensor([5, 0]), 2)
+    assert torch.isnan(att[2:]).all() and torch.allclose(att[:2].sum(-1), torch.ones(2, dtype=torch.float64))
+    cov, s = DK.coverage_ref(att, torch.zeros(4, 5), 0, 0.5, 1.0)
+    assert torch.isnan(s[2:]).all() and torch.isfinite(s[:2]).all()
+    cov2, s2 = DK.coverage_ref(att, cov[[1, 0, 3, 2]], 1, 0.5, 1.0)
+    assert torch.allclose(cov2[0], att[0] + att[1]) and torch.isnan(s2[2:]).all()
