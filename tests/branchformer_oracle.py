@@ -5,7 +5,14 @@ running reference, and the Branchformer tests compare the device against it."""
 import torch
 import torch.nn.functional as F
 
+from mirrors import seeded
 from oracle import asr_oracle as O
+
+
+def state(cfg, fx):
+    """the fixture's weights: seeded with its weight_seed, the CSGU convolutions rescaled by its tap_gain and bias_center"""
+    from speechbrain_b200.utils.seeded_init import scale_csgu_conv
+    return seeded(cfg, fx["weight_seed"], lambda sd: scale_csgu_conv(sd, fx["tap_gain"], fx["bias_center"]))
 
 
 def csgu(u, sd, p, q=None):

@@ -3,29 +3,18 @@ inputs of tests/golden/conformer640.pt (generator: tools/make_conformer640_golde
 reference on every output).  oracle/asr_oracle.py builds the decoder FFN with GELU or ReLU; the People's Speech decoder's
 Swish FFN is its decode() with SiLU in place of GELU (swish_decoder)."""
 import contextlib
-import functools
 from unittest import mock
 
 import torch
 import torch.nn.functional as F
 
+from mirrors import seeded as state  # noqa: F401  (the seed-0 weights the oracle runs on)
 from oracle import asr_oracle as O
 from oracle.goldens import wav_case
 from parity import lm_scorer_state, oracle_lm
 
 WAV_SEED, LENS, STEPS, BOS, EOS = 7, [1.0, 0.9, 0.6, 0.3], 48, 1, 2
 PREFIX = "Transformer."
-
-
-@functools.lru_cache(maxsize=2)
-def _state(name):
-    from speechbrain_b200.utils import seeded_init as S
-    cfg = {S.CONFORMER_640["name"]: S.CONFORMER_640, S.CONFORMER_640_PEOPLES["name"]: S.CONFORMER_640_PEOPLES}[name]
-    return S.seeded_asr_state(cfg, 0)
-
-
-def state(cfg):
-    return _state(cfg["name"])
 
 
 def waveforms(seed=WAV_SEED, L=160000, lens=LENS):

@@ -1,9 +1,8 @@
 """The fp32 CPU oracle of the Loquacious Conformers (utils/seeded_init.LOQUACIOUS_*: conformer_activation=torch.nn.GELU) on
 the inputs of tests/golden/loquacious.pt (generator: tools/make_loquacious_golden.py, which asserts this module equals the
-reference on every output), and the device-side modules the tests and tools/loquacious.py build from the same seeded
-weights.  oracle/asr_oracle.py builds the Conformer with Swish; gelu_conformer() runs its two Conformer sub-modules that
-apply conformer_activation (conformer_ffn: both FFN modules; conv_module: after the convolution module's LayerNorm) with
-the exact erf GELU, and nothing else.  The decoders are GELU, as asr_oracle builds them."""
+reference on every output).  oracle/asr_oracle.py builds the Conformer with Swish; gelu_conformer() runs its two
+Conformer sub-modules that apply conformer_activation (conformer_ffn: both FFN modules; conv_module: after the convolution
+module's LayerNorm) with the exact erf GELU, and nothing else.  The decoders are GELU, as asr_oracle builds them."""
 import contextlib
 import functools
 from unittest import mock
@@ -11,6 +10,7 @@ from unittest import mock
 import torch
 import torch.nn.functional as F
 
+from mirrors import seeded as state  # noqa: F401  (the seed-0 weights the oracle runs on)
 from oracle import asr_oracle as O
 from oracle.goldens import wav_case
 
@@ -60,17 +60,6 @@ def gelu_conformer():
         yield
 
 
-@functools.lru_cache(maxsize=4)
-def _state(key):
-    from speechbrain_b200.utils.seeded_init import seeded_asr_state
-    return seeded_asr_state(dict(key), 0)
-
-
-def state(cfg):
-    """seed-0 weights of cfg (values depend only on the key and shape, so a reduced model's are the full one's first layers)"""
-    return _state(tuple(sorted(cfg.items())))
-
-
 def waveforms(seed=WAV_SEED, L=160000, lens=LENS):
     return wav_case(seed, len(lens), L, lens)[:2]
 
@@ -99,36 +88,3 @@ def beam(cfg, sd, enc, lens, case=BEAM, **extra):
     return O.beam_search(enc, lens, sd, cfg, sd["seq_lin.w.weight"], sd["seq_lin.w.bias"], BOS, EOS,
                          temperature=case["temperature"], using_eos_threshold=True, length_normalization=True,
                          prefix=PREFIX, ctc=ctc, **kw)
-
-
-# ------------------------------------------------------------------------------------------------ device-side modules
-def mirror(cfg):
-    """speechbrain_b200's TransformerASR built like the recipe (conformer_activation and activation torch.nn.GELU), holding
-    the seeded weights of cfg"""
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    tr = TransformerASR(tgt_vocab=cfg["vocab"], input_size=cfg["input_size"], d_model=cfg["d_model"], nhead=cfg["nhead"],
-                        num_encoder_layers=cfg["num_encoder_layers"], num_decoder_layers=cfg["num_decoder_layers"],
-                        d_ffn=cfg["d_ffn"], activation=torch.nn.GELU, encoder_module="conformer",
-                        attention_type=cfg["attention_type"], normalize_before=True, causal=False,
-                        conformer_activation=torch.nn.GELU)
-    sd = state(cfg)
-    tr.load_state_dict({k[len(PREFIX):]: v for k, v in sd.items() if k.startswith(PREFIX)}, strict=False)
-    return tr
-
-
-def search_modules(cfg, max_decode_ratio, case=BEAM):
-    """(TransformerASR, seq_lin, ctc_lin, S2STransformerBeamSearcher) of the recipe's test search on the seeded weights"""
-    from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.nnet.linear import Linear
-    sd = state(cfg)
-    tr = mirror(cfg)
-    lin, ctc_lin = (Linear(input_size=cfg["d_model"], n_neurons=cfg["vocab"]) for _ in range(2))
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": sd["seq_lin.w.bias"]})
-    ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    scorer = ScorerBuilder(full_scorers=[CTCScorer(eos_index=EOS, blank_index=BLANK, ctc_fc=ctc_lin)],
-                           weights=dict(ctc=case["ctc_weight"]), scorer_beam_scale=0.3)
-    bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=BOS, eos_index=EOS, min_decode_ratio=0.0,
-                                    max_decode_ratio=max_decode_ratio, beam_size=case["beam"],
-                                    temperature=case["temperature"], using_eos_threshold=True, scorer=scorer)
-    return tr, lin, ctc_lin, bs

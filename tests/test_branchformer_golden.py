@@ -20,11 +20,6 @@ def fx():
     return torch.load(os.path.join(GOLDEN, "branchformer.pt"))
 
 
-def _state(cfg, fx):
-    from speechbrain_b200.utils.seeded_init import scale_csgu_conv, seeded_asr_state
-    return scale_csgu_conv(seeded_asr_state(cfg, fx["weight_seed"]), fx["tap_gain"], fx["bias_center"])
-
-
 def _oracle_encode(cfg, sd, case, q=None):
     return BO.wav_to_states(*case_wav(case), sd, cfg, q=q)
 
@@ -33,7 +28,7 @@ def _oracle_encode(cfg, sd, case, q=None):
 def test_oracle_matches_reference(fx, case):
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_CTC, BRANCHFORMER_LARGE
     cfg = BRANCHFORMER_CTC if case == "ctc" else BRANCHFORMER_LARGE
-    sd = _state(cfg, fx)
+    sd = BO.state(cfg, fx)
     with torch.no_grad():
         enc = _oracle_encode(cfg, sd, fx[case])
     if case == "short":
@@ -243,7 +238,7 @@ def test_fp16_operand_error_estimate(fx):
     operands accumulates (5e-4 after layer 1).  That is why the device encoder bar for the Branchformer is 1.5e-3
     (test_gpu_branchformer.py); this test pins the estimate that bar rests on."""
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_LARGE
-    sd = _state(BRANCHFORMER_LARGE, fx)
+    sd = BO.state(BRANCHFORMER_LARGE, fx)
     with torch.no_grad():
         enc = _oracle_encode(BRANCHFORMER_LARGE, sd, fx["large"], q=lambda t: t.half().float())
         ref = _oracle_encode(BRANCHFORMER_LARGE, sd, fx["large"])  # = the reference (test_oracle_matches_reference)

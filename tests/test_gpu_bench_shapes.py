@@ -15,6 +15,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from mirrors import build_mirror, load, raise_bias, seeded  # noqa: E402
 from parity import (best_tokens, case_wav, check_beam, check_ctc_argmax, check_encoder, check_greedy, dev,  # noqa: E402,F401
                     oracle_lm, rel)
 
@@ -188,17 +189,11 @@ def test_encoder_decoder_asr_interface(dev):
     hy, _, _, _ = asr.mods["decoder"](enc, g["wav_lens"].to(dev))
     assert slot.builds == builds and hy == g["hyps"] and rel(enc2.cpu(), g["enc_out"]) < 1e-3
     # load_state_dict after first use must take effect (ADVICE r1: stale snapshot)
-    lin = asr.mods["decoder"].fc
-    bias = sd["seq_lin.w.bias"].clone()
-    bias[7] += 100.0
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
+    load(asr.mods["decoder"].fc, raise_bias(sd, "seq_lin", {7: 100.0}), "seq_lin.")
     _, toks_new = asr.transcribe_batch(g["wav"].to(dev), g["wav_lens"].to(dev))
     assert slot.builds == builds + 1 and all(set(t) == {7} for t in toks_new), toks_new
     # beam decoder through the same interface, reference wiring (eos bias so that hypotheses finish)
-    sd_b = dict(sd)
-    sd_b["seq_lin.w.bias"] = sd["seq_lin.w.bias"].clone()
-    sd_b["seq_lin.w.bias"][2] += gb["eos_bias"]
-    asr_b = bench.build_product_asr(cfg, sd_b, dev, decoder="beam", beam=gb["kwargs"]["beam_size"])
+    asr_b = bench.build_product_asr(cfg, raise_bias(sd, "seq_lin", {2: gb["eos_bias"]}), dev, decoder="beam", beam=gb["kwargs"]["beam_size"])
     bs = asr_b.mods["decoder"]
     bs.max_decode_ratio, bs.min_decode_ratio, bs.temperature = gb["max_decode_ratio"], gb["kwargs"]["min_decode_ratio"], gb["kwargs"]["temperature"]
     bs.using_eos_threshold = gb["kwargs"]["using_eos_threshold"]
@@ -249,38 +244,13 @@ def test_encoder_asr_ctc_greedy(dev):
 
     from speechbrain_b200.decoders.ctc import ctc_greedy_decode
     from speechbrain_b200.inference.ASR import EncoderASR
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import EncoderWrapper, TransformerASR
-    from speechbrain_b200.nnet.activations import Softmax
-    from speechbrain_b200.nnet.containers import LengthsCapableSequential
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.processing.features import InputNormalization
-    from speechbrain_b200.utils.seeded_init import seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gc = torch.load(os.path.join(GOLDEN, "ctc_greedy_conformer_large_rope.pt"))
     cfg = _cfg(g)
-    sd = seeded_asr_state(cfg, 0)
-    fb = Fbank(n_fft=512, n_mels=80, win_length=32)
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=2, num_layers_per_block=1, out_channels=(64, 32),
-                              kernel_sizes=(3, 3), strides=(2, 2), residuals=(False, False))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    tr = TransformerASR(input_size=640, tgt_vocab=5000, d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="conformer", attention_type="RoPEMHA",
-                        normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    ctc_lin = Linear(input_size=512, n_neurons=5000)
+    m = build_mirror(cfg, seeded(cfg))
     for name in ("plain", "merge"):
         c = gc[name]
-        bias = sd["ctc_lin.w.bias"].clone()
-        bias[0] += c["bias_blank"]
-        bias[17] += c["bias_tok"]
-        ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": bias})
-        enc = LengthsCapableSequential(compute_features=fb, normalize=norm, cnn=cnn, transformer_encoder=EncoderWrapper(tr),
-                                       ctc_lin=ctc_lin, log_softmax=Softmax(apply_log=True))
+        enc = m.front_end(m.head("ctc_lin", {0: c["bias_blank"], 17: c["bias_tok"]}))
         asr = EncoderASR(modules=dict(encoder=enc), hparams=dict(tokenizer=None, decoding_function=functools.partial(ctc_greedy_decode, blank_id=0)),
                          run_opts={"device": str(dev)})
         lp = asr.encode_batch(g["wav"], g["wav_lens"]).cpu()

@@ -21,6 +21,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from parity import (case_wav, check_alone_vs_batch, check_ctc_argmax, check_encoder, check_greedy, check_summary,  # noqa: E402,F401
                     dev, seeded_wav)
 import branchformer_oracle as BO  # noqa: E402
+from mirrors import build_mirror  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 ENC_BAR = 1.5e-3
@@ -31,11 +32,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def fx():
     return torch.load(os.path.join(GOLDEN, "branchformer.pt"))
-
-
-def _state(cfg, fx):
-    from speechbrain_b200.utils.seeded_init import scale_csgu_conv, seeded_asr_state
-    return scale_csgu_conv(seeded_asr_state(cfg, fx["weight_seed"]), fx["tap_gain"], fx["bias_center"])
 
 
 # ------------------------------------------------------------------------------------------------ CSGU kernel
@@ -103,14 +99,14 @@ def test_csgu_kernel_rejects_short_and_bad_shapes(dev):
 # ------------------------------------------------------------------------------------------------ whole encoder
 def _engine(cfg, fx, dev, parts=("fbank", "cnn", "encoder", "decoder")):
     from speechbrain_b200.engine import AsrEngine
-    return AsrEngine(cfg, _state(cfg, fx), device=dev, parts=parts)
+    return AsrEngine(cfg, BO.state(cfg, fx), device=dev, parts=parts)
 
 
 def _oracle_states(cfg, fx, case):
     """The reference's encoder states of a fixture case, recomputed by the CPU oracle and checked against the stored
     per-frame norms and sampled rows."""
     with torch.no_grad():
-        ref = BO.wav_to_states(*case_wav(case), _state(cfg, fx), cfg)
+        ref = BO.wav_to_states(*case_wav(case), BO.state(cfg, fx), cfg)
     check_summary(f"{cfg['name']} oracle", ref, case["frame_norm"], case["sample_idx"], case["sample_rows"], 1e-5)
     return ref
 
@@ -145,32 +141,10 @@ def test_branchformer_shortest_input(dev, fx):
 def test_branchformer_ctc_encoder_asr(dev, fx):
     from speechbrain_b200.decoders.ctc import ctc_greedy_decode
     from speechbrain_b200.inference.ASR import EncoderASR
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import EncoderWrapper, TransformerASR
-    from speechbrain_b200.nnet.activations import Softmax
-    from speechbrain_b200.nnet.containers import LengthsCapableSequential
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.processing.features import InputNormalization
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_CTC as cfg
     c = fx["ctc"]
-    sd = _state(cfg, fx)
-    fb = Fbank(n_fft=512, n_mels=80, win_length=25)
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=2, num_layers_per_block=1, out_channels=(64, 32),
-                              kernel_sizes=(3, 3), strides=(2, 2), residuals=(False, False))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    tr = TransformerASR(input_size=640, tgt_vocab=31, d_model=256, nhead=4, num_encoder_layers=18, num_decoder_layers=0,
-                        activation=torch.nn.GELU, branchformer_activation=torch.nn.GELU, encoder_module="branchformer",
-                        csgu_linear_units=2400, kernel_size=31, attention_type="RelPosMHAXL", normalize_before=True,
-                        causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    ctc_lin = Linear(input_size=256, n_neurons=31)
-    ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    enc = LengthsCapableSequential(compute_features=fb, normalize=norm, cnn=cnn, transformer_encoder=EncoderWrapper(tr),
-                                   ctc_lin=ctc_lin, log_softmax=Softmax(apply_log=True))
+    m = build_mirror(cfg, BO.state(cfg, fx))
+    enc = m.front_end(m.ctc_lin)
     asr = EncoderASR(modules=dict(encoder=enc), hparams=dict(tokenizer=None, decoding_function=functools.partial(ctc_greedy_decode, blank_id=0)),
                      run_opts={"device": str(dev)})
     wav, lens = case_wav(c)

@@ -25,8 +25,9 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import conformer640_oracle as CO  # noqa: E402
 import test_gpu_decoder_kernels as DKT  # noqa: E402
 import test_gpu_encoder_kernels as EKT  # noqa: E402
+from mirrors import build_mirror, seeded  # noqa: E402
 from parity import (BEAM_TOL, check_alone_vs_batch, check_beam, check_encoder, check_greedy, check_summary,  # noqa: E402,F401
-                    dev, lm_scorer, lm_scorer_state, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir)
+                    dev, lm_scorer_state, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir)
 
 ENC_BAR = 1e-3
 DEC_BAR = 2e-3  # teacher-forced decode(), rel-L2 (measured 4.4e-4)
@@ -89,7 +90,7 @@ def fx():
 
 def _case(cfg, fx_recipe):
     """seeded weights, the waveforms, the oracle's encoder states and greedy search (CPU), and the reference fixture"""
-    sd = CO.state(cfg)
+    sd = seeded(cfg)
     wav, lens = CO.waveforms()
     enc = CO.encode(cfg, sd, wav, lens)
     _, _, logits = CO.greedy(cfg, sd, enc, lens)
@@ -140,26 +141,13 @@ def test_wav_to_encoder_and_greedy(dev, recipe, request):
         assert r <= ENC_BAR
 
 
-def _transformer(cfg, conformer_swish=True):
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.nnet.activations import Swish
-    tr = TransformerASR(tgt_vocab=cfg["vocab"], input_size=cfg["input_size"], d_model=cfg["d_model"], nhead=cfg["nhead"],
-                        num_encoder_layers=cfg["num_encoder_layers"], num_decoder_layers=cfg["num_decoder_layers"],
-                        d_ffn=cfg["d_ffn"], activation=Swish if cfg["decoder_activation"] == "swish" else torch.nn.GELU,
-                        encoder_module="conformer", attention_type="RelPosMHAXL", normalize_before=True, causal=False,
-                        conformer_activation=Swish if conformer_swish else None)
-    sd = CO.state(cfg)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    return tr
-
-
 @pytest.mark.parametrize("recipe", ["libriheavy", "peoples"])
 def test_decode_teacher_forced(dev, recipe, request):
     """TransformerASR.decode() (the mirror, built with the recipe's decoder activation) on 48 positions of the oracle's
     encoder states vs the reference fixture and the oracle; covers the Swish FFN on both projection back ends"""
     case = request.getfixturevalue(recipe)
     cfg = case["cfg"]
-    tr = _transformer(cfg)
+    tr = build_mirror(cfg, case["sd"]).tr
     assert tr.decoder_activation == cfg["decoder_activation"]
     tgt = CO.teacher_tokens(cfg)
     enc_len = torch.round(case["lens"] * case["T"]).int()
@@ -175,27 +163,11 @@ def test_decode_teacher_forced(dev, recipe, request):
     tr._decoder_engine(dev).set_decoder_tc_min_rows(64)
 
 
-def _search_modules(cfg, beam, lm_weight, ctc_weight, max_decode_ratio):
-    from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.nnet.linear import Linear
-    sd = CO.state(cfg)
-    tr = _transformer(cfg)
-    lin = Linear(input_size=cfg["d_model"], n_neurons=cfg["vocab"])
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": sd["seq_lin.w.bias"]})
-    ctc_lin = Linear(input_size=cfg["d_model"], n_neurons=cfg["vocab"])
-    ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    full, weights = [], {}
-    if lm_weight:  # the recipe's order: [transformerlm, ctc]
-        full.append(TransformerLMScorer(language_model=lm_scorer(cfg["vocab"]), temperature=1.15))
-        weights["transformerlm"] = lm_weight
-    full.append(CTCScorer(eos_index=EOS, blank_index=0, ctc_fc=ctc_lin))
-    weights["ctc"] = ctc_weight
-    bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=BOS, eos_index=EOS, min_decode_ratio=0.0,
-                                    max_decode_ratio=max_decode_ratio, beam_size=beam, temperature=1.15,
-                                    using_eos_threshold=False, length_normalization=True,
-                                    scorer=ScorerBuilder(full_scorers=full, weights=weights))
-    return tr, lin, ctc_lin, bs
+def searcher(m, beam, lm_weight, ctc_weight, max_decode_ratio):
+    """the recipes' test search on the mirror m: [TransformerLM, CTC] (Libriheavy) or [CTC] (People's Speech)"""
+    scorers = dict(transformerlm=lm_weight, ctc=ctc_weight) if lm_weight else dict(ctc=ctc_weight)
+    kwargs = dict(min_decode_ratio=0.0, beam_size=beam, temperature=1.15, using_eos_threshold=False, length_normalization=True)
+    return m.searcher(kwargs, max_decode_ratio, scorers=scorers)
 
 
 @pytest.mark.parametrize("recipe", ["libriheavy", "peoples"])
@@ -207,7 +179,7 @@ def test_beam_search(dev, recipe, request):
     case = request.getfixturevalue(recipe)
     cfg, sd, gb = case["cfg"], case["sd"], case["fx"]["beam"]
     utts = gb["utts"]
-    _, _, _, bs = _search_modules(cfg, gb["beam"], gb["lm_weight"], gb["ctc_weight"], (gb["steps"] + 0.5) / case["T"])
+    bs = searcher(build_mirror(cfg, sd), gb["beam"], gb["lm_weight"], gb["ctc_weight"], (gb["steps"] + 0.5) / case["T"])
     enc, lens = case["enc"][utts], case["lens"][utts]
     hyps, _, scores, _ = bs(enc.to(dev), lens.to(dev))
     scores = scores.cpu().view(-1, 1)
@@ -336,10 +308,6 @@ def test_from_hparams_local_directory(dev, recipe, request, tmp_path):
     from a local directory, the checkpoints land in the mirrors, and transcribe_batch gives the tokens of the same modules
     constructed directly, 24 steps per utterance"""
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain_b200.nnet.containers import LengthsCapableSequential
-    from speechbrain_b200.processing.features import InputNormalization
     case = request.getfixturevalue(recipe)
     cfg, sd = case["cfg"], case["sd"]
     lm = recipe == "libriheavy"
@@ -353,17 +321,10 @@ def test_from_hparams_local_directory(dev, recipe, request, tmp_path):
     tmp = write_pretrained_dir(tmp_path, yaml, ckpts)
     loaded = EncoderDecoderASR.from_hparams(source=tmp, run_opts={"device": str(dev)})
     assert torch.equal(loaded.mods["decoder"].fc.w.weight.cpu(), sd["seq_lin.w.weight"])
-    tr, _, _, bs = _search_modules(cfg, beam[0], beam[1], beam[2], ratio)
-    assert loaded.mods["decoder"].model.decoder_activation == tr.decoder_activation == cfg["decoder_activation"]
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=2, num_layers_per_block=1, out_channels=(64, 32),
-                              kernel_sizes=(3, 3), strides=(2, 2), residuals=(False, False))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    enc = LengthsCapableSequential(compute_features=Fbank(sample_rate=16000, n_fft=512, n_mels=80, win_length=32),
-                                   normalize=norm, cnn=cnn)
-    direct = EncoderDecoderASR(modules=dict(encoder=enc, transformer=tr, decoder=bs),
+    m = build_mirror(cfg, sd)
+    bs = searcher(m, beam[0], beam[1], beam[2], ratio)
+    assert loaded.mods["decoder"].model.decoder_activation == m.tr.decoder_activation == cfg["decoder_activation"]
+    direct = EncoderDecoderASR(modules=dict(encoder=m.front_end(), transformer=m.tr, decoder=bs),
                                hparams=dict(tokenizer=None, transformer_beam_search=True), run_opts={"device": str(dev)})
     wav, lens = case["wav"], case["lens"]
     _, t1 = loaded.transcribe_batch(wav, lens)

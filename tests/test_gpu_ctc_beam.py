@@ -16,7 +16,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from parity import dev  # noqa: E402,F401
+import branchformer_oracle as BO  # noqa: E402
 import ctc_beam_oracle as CO  # noqa: E402
+from mirrors import build_mirror  # noqa: E402
 from test_ctc_beam_golden import CASES  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -148,33 +150,10 @@ class _LabelEncoder:
 
 def _branchformer_ctc_asr(dev, decoding_function, hparams_extra):
     from speechbrain_b200.inference.ASR import EncoderASR
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import EncoderWrapper, TransformerASR
-    from speechbrain_b200.nnet.activations import Softmax
-    from speechbrain_b200.nnet.containers import LengthsCapableSequential
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.processing.features import InputNormalization
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_CTC as cfg
-    from speechbrain_b200.utils.seeded_init import scale_csgu_conv, seeded_asr_state
     fx = torch.load(os.path.join(GOLDEN, "branchformer.pt"))
-    sd = scale_csgu_conv(seeded_asr_state(cfg, fx["weight_seed"]), fx["tap_gain"], fx["bias_center"])
-    fb = Fbank(n_fft=512, n_mels=80, win_length=25)
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=2, num_layers_per_block=1, out_channels=(64, 32),
-                              kernel_sizes=(3, 3), strides=(2, 2), residuals=(False, False))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    tr = TransformerASR(input_size=640, tgt_vocab=31, d_model=256, nhead=4, num_encoder_layers=18, num_decoder_layers=0,
-                        activation=torch.nn.GELU, branchformer_activation=torch.nn.GELU, encoder_module="branchformer",
-                        csgu_linear_units=2400, kernel_size=31, attention_type="RelPosMHAXL", normalize_before=True,
-                        causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    ctc_lin = Linear(input_size=256, n_neurons=31)
-    ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    enc = LengthsCapableSequential(compute_features=fb, normalize=norm, cnn=cnn, transformer_encoder=EncoderWrapper(tr),
-                                   ctc_lin=ctc_lin, log_softmax=Softmax(apply_log=True))
+    m = build_mirror(cfg, BO.state(cfg, fx))
+    enc = m.front_end(m.ctc_lin)
     hp = dict(tokenizer=_LabelEncoder(CO.CHAR_VOCAB), decoding_function=decoding_function, **hparams_extra)
     c = fx["ctc"]
     B, L = c["wav_shape"]

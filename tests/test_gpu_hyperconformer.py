@@ -20,6 +20,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from parity import (best_tokens, case_wav, check_alone_vs_batch, check_beam, check_encoder, check_greedy,  # noqa: E402,F401
                     check_summary, dev, oracle_lm, rel)
 import hyperconformer_oracle as HO  # noqa: E402
+from mirrors import load, seeded  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 ENC_BAR = 7.5e-3
@@ -33,9 +34,11 @@ def fx():
     return torch.load(os.path.join(GOLDEN, "hyperconformer.pt"))
 
 
-def _state(fx, gain=None):
-    from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M, scale_hypernet, seeded_asr_state
-    return scale_hypernet(seeded_asr_state(HYPERCONFORMER_22M, fx["weight_seed"]), fx["hypernet_gain"] if gain is None else gain)
+def _state(fx, gain=None, cfg=None):
+    """the fixture's weights of HYPERCONFORMER_22M (or of cfg: a reduced model's are the full one's first layers)"""
+    from speechbrain_b200.utils.seeded_init import HYPERCONFORMER_22M, scale_hypernet
+    return seeded(cfg or HYPERCONFORMER_22M, fx["weight_seed"],
+                  lambda sd: scale_hypernet(sd, fx["hypernet_gain"] if gain is None else gain))
 
 
 # ------------------------------------------------------------------------------------------------ HyperMixing kernels
@@ -215,9 +218,8 @@ def test_load_state_dict_after_first_use(dev, fx):
     asr = bench.build_product_asr(cfg, _state(fx), dev)
     wav, lens = case_wav(fx["short"])
     before = asr.encode_batch(wav.to(dev), lens.to(dev)).cpu()
-    sd2 = _state(fx, gain=0.7)
-    tr = asr.transformer
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd2.items() if k.startswith("Transformer.")}, strict=False)
+    sd2 = _state(fx, gain=0.7, cfg=cfg)
+    load(asr.transformer, sd2, "Transformer.")
     after = asr.encode_batch(wav.to(dev), lens.to(dev)).cpu()
     fresh = bench.build_product_asr(cfg, sd2, dev).encode_batch(wav.to(dev), lens.to(dev)).cpu()
     print(f"load_state_dict: change {rel(after, before):.2e}, vs a fresh engine max abs {float((after - fresh).abs().max()):.2e}")

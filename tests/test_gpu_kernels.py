@@ -7,6 +7,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from mirrors import build_mirror, seeded  # noqa: E402
 from parity import check_greedy, dev, lm_scorer, rel  # noqa: E402,F401
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -218,29 +219,20 @@ def test_transcribe_end_to_end(dev):
     assert torch.equal(pred_h, pred.cpu())
 
 
+def _conformer_large():
+    """the mirror of the seeded Conformer-L the beam fixtures were written from"""
+    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE
+    return build_mirror(CONFORMER_LARGE, seeded(CONFORMER_LARGE))
+
+
 @pytest.mark.parametrize("case", ["thr_on", "recipe", "no_eos"])
 def test_beam_search_golden(dev, case):
     """S2STransformerBeamSearcher (no scorer) vs the REFERENCE's hypotheses / scores / log-probs on the golden encoder
     states: EOS threshold on, the recipe's settings (temperature 1.15, min steps, no threshold), and the path where no
     hypothesis ever ends (final fill).  Scores within 2e-2 (fp16 decoder), hypotheses identical."""
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_conformer_large_rope.pt"))[case]
-    cfg = dict(CONFORMER_LARGE)
-    sd = seeded_asr_state(cfg, 0)
-    tr = TransformerASR(input_size=640, tgt_vocab=5000, d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="conformer", attention_type="RoPEMHA",
-                        normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    lin = Linear(input_size=512, n_neurons=5000)
-    bias = sd["seq_lin.w.bias"].clone()
-    bias[2] += gb["eos_bias"]
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
-    bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, max_decode_ratio=gb["max_decode_ratio"],
-                                    **gb["kwargs"])
+    bs = _conformer_large().searcher(gb["kwargs"], gb["max_decode_ratio"], gb["eos_bias"])
     for name, tc_rows in (("skinny", None), ("wgmma", 1)):  # both decode-step projection implementations
         if tc_rows is not None:
             bs._get_engine(dev).set_decoder_tc_min_rows(tc_rows)
@@ -310,27 +302,10 @@ def test_full_size_properties(dev):
 def test_beam_search_with_transformerlm_scorer_golden(dev, case):
     """S2STransformerBeamSearcher + ScorerBuilder(full_scorers=[TransformerLMScorer], weight 0.6, temperature 1.15) with the
     recipe's 12 x 768 TransformerLM vs the REFERENCE (shallow fusion, scorer.py:510-543,1221-1268)."""
-    from speechbrain_b200.decoders.scorer import ScorerBuilder, TransformerLMScorer
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_lm_conformer_large_rope.pt"))[case]
-    sd = seeded_asr_state(dict(CONFORMER_LARGE), 0)
-    tr = TransformerASR(input_size=640, tgt_vocab=5000, d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="conformer", attention_type="RoPEMHA",
-                        normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    lin = Linear(input_size=512, n_neurons=5000)
-    bias = sd["seq_lin.w.bias"].clone()
-    bias[2] += gb["eos_bias"]
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
-    lm = lm_scorer()
-    scorer = ScorerBuilder(full_scorers=[TransformerLMScorer(language_model=lm, temperature=gb["lm_temperature"])],
-                           weights={"transformerlm": gb["lm_weight"]})
-    bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, max_decode_ratio=gb["max_decode_ratio"],
-                                    scorer=scorer, **gb["kwargs"])
+    bs = _conformer_large().searcher(gb["kwargs"], gb["max_decode_ratio"], gb["eos_bias"],
+                                     scorers={"transformerlm": gb["lm_weight"]}, lm_temperature=gb["lm_temperature"])
     hyps, lens, scores, lp = bs(g["enc_out"].to(dev), g["wav_lens"].to(dev))
     print(f"beam+lm[{case}] hyps {hyps} ref {gb['hyps']} scores {scores.tolist()} ref {gb['scores'].tolist()}")
     assert hyps == gb["hyps"]
@@ -343,33 +318,11 @@ def test_beam_search_with_ctc_scorer_golden(dev, case):
     """Joint CTC/attention decoding: S2STransformerBeamSearcher + ScorerBuilder(full_scorers=[TransformerLMScorer, CTCScorer]
     (test search) or [CTCScorer] (valid search), ctc 0.4 / lm 0.6) vs the REFERENCE: hypotheses identical, scores within
     5e-2 (fp16 GEMM operands in the decoder, LM and CTC head; the prefix scores sum ~T log-posteriors)."""
-    from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_ctc_conformer_large_rope.pt"))[case]
-    sd = seeded_asr_state(dict(CONFORMER_LARGE), 0)
-    tr = TransformerASR(input_size=640, tgt_vocab=5000, d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="conformer", attention_type="RoPEMHA",
-                        normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    lin = Linear(input_size=512, n_neurons=5000)
-    bias = sd["seq_lin.w.bias"].clone()
-    bias[2] += gb["eos_bias"]
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
-    ctc_lin = Linear(input_size=512, n_neurons=5000)
-    ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    ctc_scorer = CTCScorer(eos_index=2, blank_index=0, ctc_fc=ctc_lin)
-    if gb["with_lm"]:
-        lm = lm_scorer()
-        scorer = ScorerBuilder(full_scorers=[TransformerLMScorer(language_model=lm, temperature=gb["lm_temperature"]), ctc_scorer],
-                               weights={"transformerlm": gb["lm_weight"], "ctc": gb["ctc_weight"]})
-    else:
-        scorer = ScorerBuilder(full_scorers=[ctc_scorer], weights={"ctc": gb["ctc_weight"]})
-    bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, max_decode_ratio=gb["max_decode_ratio"],
-                                    scorer=scorer, **gb["kwargs"])
+    scorers = dict(transformerlm=gb["lm_weight"], ctc=gb["ctc_weight"]) if gb["with_lm"] else dict(ctc=gb["ctc_weight"])
+    bs = _conformer_large().searcher(gb["kwargs"], gb["max_decode_ratio"], gb["eos_bias"], scorers=scorers,
+                                     lm_temperature=gb["lm_temperature"])
     hyps, lens, scores, lp = bs(g["enc_out"].to(dev), g["wav_lens"].to(dev))
     print(f"beam+ctc[{case}] hyps {hyps} ref {gb['hyps']} scores {scores.tolist()} ref {gb['scores'].tolist()}")
     assert hyps == gb["hyps"]
@@ -379,23 +332,9 @@ def test_beam_search_with_ctc_scorer_golden(dev, case):
 
 def test_beam_search_return_topk_golden(dev):
     """return_topk=True, topk=3: padded n-best hypotheses, lengths, scores and log-probs vs the REFERENCE."""
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_topk_conformer_large_rope.pt"))
-    sd = seeded_asr_state(dict(CONFORMER_LARGE), 0)
-    tr = TransformerASR(input_size=640, tgt_vocab=5000, d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="conformer", attention_type="RoPEMHA",
-                        normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    lin = Linear(input_size=512, n_neurons=5000)
-    bias = sd["seq_lin.w.bias"].clone()
-    bias[2] += gb["eos_bias"]
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
-    bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, max_decode_ratio=gb["max_decode_ratio"],
-                                    return_topk=True, topk=gb["topk"], **gb["kwargs"])
+    bs = _conformer_large().searcher(gb["kwargs"], gb["max_decode_ratio"], gb["eos_bias"], topk=gb["topk"])
     hyps, lens, scores, lp = bs(g["enc_out"].to(dev), g["wav_lens"].to(dev))
     print(f"beam topk hyps {hyps.tolist()} ref {gb['hyps'].tolist()} scores {scores.tolist()} ref {gb['scores'].tolist()}")
     assert torch.equal(hyps.cpu(), gb["hyps"]) and torch.allclose(lens.cpu(), gb["lens"])
@@ -425,25 +364,13 @@ def test_beam_search_with_length_scorer_golden(dev):
     """ScorerBuilder(full_scorers=[LengthScorer], weights={"length": w}) with length_normalization=False vs the REFERENCE."""
     from speechbrain_b200.decoders.scorer import LengthScorer, ScorerBuilder
     from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, seeded_asr_state
     g = torch.load(os.path.join(GOLDEN, "conformer_large_rope.pt"))
     gb = torch.load(os.path.join(GOLDEN, "beam_len_conformer_large_rope.pt"))
-    sd = seeded_asr_state(dict(CONFORMER_LARGE), 0)
-    tr = TransformerASR(input_size=640, tgt_vocab=5000, d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="conformer", attention_type="RoPEMHA",
-                        normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    lin = Linear(input_size=512, n_neurons=5000)
-    bias = sd["seq_lin.w.bias"].clone()
-    bias[2] += gb["eos_bias"]
-    lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": bias})
+    m = _conformer_large()
     scorer = ScorerBuilder(full_scorers=[LengthScorer(5000)], weights={"length": gb["length_weight"]})
     with pytest.raises(ValueError):  # "Length normalization is not compatible with length rewarding."
-        S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, beam_size=4, scorer=scorer)
-    bs = S2STransformerBeamSearcher(modules=[tr, lin], bos_index=1, eos_index=2, max_decode_ratio=gb["max_decode_ratio"],
-                                    scorer=scorer, **gb["kwargs"])
+        S2STransformerBeamSearcher(modules=[m.tr, m.seq_lin], bos_index=1, eos_index=2, beam_size=4, scorer=scorer)
+    bs = m.searcher(gb["kwargs"], gb["max_decode_ratio"], gb["eos_bias"], scorers={"length": gb["length_weight"]})
     hyps, lens, scores, lp = bs(g["enc_out"].to(dev), g["wav_lens"].to(dev))
     print(f"beam+length hyps {hyps} ref {gb['hyps']} scores {scores.tolist()} ref {gb['scores'].tolist()}")
     assert hyps == gb["hyps"]

@@ -17,6 +17,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import loquacious_oracle as LO  # noqa: E402
+from mirrors import build_mirror, raise_bias, seeded  # noqa: E402
 from parity import (BEAM_TOL, check_alone_vs_batch, check_beam, check_encoder, check_greedy, check_summary,  # noqa: E402,F401
                     dev, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir)
 
@@ -122,7 +123,7 @@ def test_create_rejects_unknown_activation(dev):
     from speechbrain_b200.engine import AsrEngine
     from speechbrain_b200.utils.seeded_init import BRANCHFORMER_CTC, seeded_asr_state
     cfg = LO.reduced(LO.sizes()["loquacious_small"])
-    sd = LO.state(cfg)
+    sd = seeded(cfg)
     with pytest.raises(NotImplementedError):
         AsrEngine(dict(cfg, conformer_activation="tanh_gelu"), sd, device=str(dev))
     bf = dict(BRANCHFORMER_CTC, num_encoder_layers=1, conformer_activation="gelu")
@@ -143,7 +144,7 @@ def wav():
 
 def _engine(cfg, dev):
     from speechbrain_b200.engine import AsrEngine
-    return AsrEngine(dict(cfg, conformer_activation="gelu"), LO.state(cfg), device=str(dev))
+    return AsrEngine(dict(cfg, conformer_activation="gelu"), seeded(cfg), device=str(dev))
 
 
 def _enc_case(tag, cfg, rec, wav, dev, dynchunk=None):
@@ -157,7 +158,7 @@ def _enc_case(tag, cfg, rec, wav, dev, dynchunk=None):
     T = enc.shape[1]
     s = rec["enc"]
     check_summary(f"{tag} encoder", enc, s["frame_norm"], s["sample_idx"], s["sample_rows"], ENC_BAR)
-    check_encoder(tag, enc, LO.encode(cfg, LO.state(cfg), w, lens, dynchunk), [round(float(x) * T) for x in lens], ENC_BAR)
+    check_encoder(tag, enc, LO.encode(cfg, seeded(cfg), w, lens, dynchunk), [round(float(x) * T) for x in lens], ENC_BAR)
     return eng
 
 
@@ -180,7 +181,7 @@ def test_encoder_rope(dev, fx, wav):
 def xlarge(fx, wav):
     from speechbrain_b200.utils.seeded_init import LOQUACIOUS_XLARGE
     w, lens = wav
-    return dict(cfg=LOQUACIOUS_XLARGE, enc=LO.encode(LOQUACIOUS_XLARGE, LO.state(LOQUACIOUS_XLARGE), w, lens), fx=fx)
+    return dict(cfg=LOQUACIOUS_XLARGE, enc=LO.encode(LOQUACIOUS_XLARGE, seeded(LOQUACIOUS_XLARGE), w, lens), fx=fx)
 
 
 def test_xlarge_encoder_and_greedy(dev, xlarge, wav):
@@ -204,6 +205,14 @@ def test_xlarge_encoder_and_greedy(dev, xlarge, wav):
     check_alone_vs_batch(greedy, w, lens, 1e-5, relative=True)
 
 
+def searcher(m, max_decode_ratio, case=LO.BEAM, eos_bias=0.0):
+    """the recipe's test search on the mirror m: beam 80, CTC 0.3 with blank 3 (scorer_beam_scale 0.3), temperature 1.15,
+    using_eos_threshold; seq_lin's EOS bias raised by eos_bias"""
+    kwargs = dict(min_decode_ratio=0.0, beam_size=case["beam"], temperature=case["temperature"], using_eos_threshold=True)
+    return m.searcher(kwargs, max_decode_ratio, eos_bias, scorers=dict(ctc=case["ctc_weight"]), blank=BLANK,
+                      scorer_beam_scale=0.3)
+
+
 @pytest.mark.parametrize("which", ["beam", "beam_eos"])
 def test_xlarge_beam80_ctc(dev, xlarge, wav, which):
     """the recipe's test search (beam 80, CTC 0.3 with blank 3, temperature 1.15, using_eos_threshold) on the oracle's
@@ -216,14 +225,11 @@ def test_xlarge_beam80_ctc(dev, xlarge, wav, which):
         cfg, enc = xlarge["cfg"], xlarge["enc"][utts]
     else:
         cfg = LO.reduced(xlarge["cfg"])
-        enc = LO.encode(cfg, LO.state(cfg), wav[0], wav[1])[utts]
+        enc = LO.encode(cfg, seeded(cfg), wav[0], wav[1])[utts]
         assert len({tuple(h) for h in gb["hyps"]}) > 1
-    sd = dict(LO.state(cfg))
     lens = wav[1][utts]
-    _, lin, _, bs = LO.search_modules(cfg, (gb["steps"] + 0.5) / enc.shape[1], gb)
-    with torch.no_grad():
-        lin.w.bias[EOS] += gb["eos_bias"]
-    sd["seq_lin.w.bias"] = lin.w.bias.detach().clone()
+    bs = searcher(build_mirror(cfg, seeded(cfg)), (gb["steps"] + 0.5) / enc.shape[1], gb, gb["eos_bias"])
+    sd = raise_bias(seeded(cfg), "seq_lin", {EOS: gb["eos_bias"]})
     hyps, _, scores, _ = bs(enc.to(dev), lens.to(dev))
     scores = scores.cpu().view(-1, 1)
     h2, _, s2, _ = bs(enc.to(dev), lens.to(dev))
@@ -237,7 +243,7 @@ def test_gelu_engine_differs_from_swish(dev, wav):
     """the engine built from engine_cfg() follows conformer_activation: the same weights as a Swish model give other
     encoder states"""
     cfg = LO.reduced(LO.sizes()["loquacious_base"])
-    tr = LO.mirror(cfg)
+    tr = build_mirror(cfg, seeded(cfg)).tr
     src = torch.randn(2, 60, 640, generator=torch.Generator().manual_seed(5)).to(dev)
     gelu = tr.encode(src).cpu()
     tr.conformer_activation = "swish"
@@ -250,7 +256,8 @@ def test_gelu_engine_differs_from_swish(dev, wav):
 def test_streaming_equals_masked(dev, att, cs, lc):
     """encode_streaming with GELU equals the masked Dynamic Chunk mode, as test_gpu_streaming.py checks for Swish"""
     from speechbrain_b200.utils.dynamic_chunk_training import DynChunkTrainConfig
-    tr = LO.mirror(dict(LO.sizes()["loquacious_large"], num_encoder_layers=3, num_decoder_layers=1, attention_type=att))
+    cfg = dict(LO.sizes()["loquacious_large"], num_encoder_layers=3, num_decoder_layers=1, attention_type=att)
+    tr = build_mirror(cfg, seeded(cfg)).tr
     B, T = 2, 14 * cs + 5
     src = torch.randn(B, T, 640, generator=torch.Generator().manual_seed(cs)).to(dev)
     dc = DynChunkTrainConfig(cs, lc)
@@ -365,13 +372,9 @@ def test_from_hparams_local_directory(dev, wav, tmp_path):
     Transformer is a GELU Conformer holding the checkpoint, and transcribe_batch gives the tokens of the same modules
     constructed directly, 10 steps per utterance"""
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain_b200.nnet.containers import LengthsCapableSequential
-    from speechbrain_b200.processing.features import InputNormalization
     from speechbrain_b200.utils.seeded_init import LOQUACIOUS_XLARGE
     cfg = LO.reduced(LOQUACIOUS_XLARGE)
-    sd = LO.state(cfg)
+    sd = seeded(cfg)
     ratio = (LO.BEAM["steps"] + 0.5) / 251
     yaml = INFERENCE_YAML.format(ratio=ratio, **{k: cfg[k] for k in ("d_model", "nhead", "num_encoder_layers",
                                                                    "num_decoder_layers", "d_ffn", "vocab")})
@@ -381,15 +384,8 @@ def test_from_hparams_local_directory(dev, wav, tmp_path):
     assert dec.model.conformer_activation == "gelu" and dec.model.engine_cfg()["conformer_activation"] == "gelu"
     assert torch.equal(dec.fc.w.weight.cpu(), sd["seq_lin.w.weight"])
     assert dec.ctc_scorer.blank_index == BLANK and dec.ctc_weight == 0.3 and (dec.bos_index, dec.eos_index) == (BOS, EOS)
-    tr, _, _, bs = LO.search_modules(cfg, ratio)
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=2, num_layers_per_block=1, out_channels=(64, 32),
-                              kernel_sizes=(3, 3), strides=(2, 2), residuals=(False, False))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    enc = LengthsCapableSequential(compute_features=Fbank(sample_rate=16000, n_fft=400, n_mels=80), normalize=norm, cnn=cnn)
-    direct = EncoderDecoderASR(modules=dict(encoder=enc, transformer=tr, decoder=bs),
+    m = build_mirror(cfg, sd)
+    direct = EncoderDecoderASR(modules=dict(encoder=m.front_end(), transformer=m.tr, decoder=searcher(m, ratio)),
                                hparams=dict(tokenizer=None, transformer_beam_search=True), run_opts={"device": str(dev)})
     w, lens = wav
     _, t1 = loaded.transcribe_batch(w, lens)

@@ -10,6 +10,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import transducer_oracle as TO  # noqa: E402
+from mirrors import build_mirror  # noqa: E402
 from parity import normalizer_ckpt, write_pretrained_dir  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -183,31 +184,18 @@ def _fixture_e2e():
     return fx, cfg, sd, w_enc, W, wav, lens
 
 
-def _transducer_modules(sd, w_enc, W):
+def _transducer_modules(cfg, sd, w_enc, W):
     """The reference's EncoderDecoderASR layout for the LibriSpeech transducer recipe: encoder = LengthsCapableSequential(
     Fbank, InputNormalization, ConvolutionFrontEnd, EncoderWrapper(12-layer RoPEMHA Conformer), proj_enc), decoder =
     TransducerBeamSearcher(beam_size=1)."""
     from speechbrain_b200.decoders.transducer import TransducerBeamSearcher
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import EncoderWrapper, TransformerASR
+    from speechbrain_b200.lobes.models.transformer.TransformerASR import EncoderWrapper
     from speechbrain_b200.nnet.containers import LengthsCapableSequential
     from speechbrain_b200.nnet.embedding import Embedding
     from speechbrain_b200.nnet.linear import Linear
     from speechbrain_b200.nnet.RNN import LSTM
     from speechbrain_b200.nnet.transducer.transducer_joint import Transducer_joint
-    from speechbrain_b200.processing.features import InputNormalization
-    fb = Fbank(n_fft=512, n_mels=80, win_length=32)
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=2, num_layers_per_block=1, out_channels=(64, 32),
-                              kernel_sizes=(3, 3), strides=(2, 2), residuals=(False, False))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    tr = TransformerASR(input_size=640, tgt_vocab=1000, d_model=512, nhead=8, num_encoder_layers=12, num_decoder_layers=0,
-                        d_ffn=2048, activation=torch.nn.GELU, kernel_size=31, attention_type="RoPEMHA",
-                        encoder_module="conformer", normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
+    mirror = build_mirror(cfg, sd)
     proj_enc = Linear(input_size=512, n_neurons=640, bias=False)
     proj_enc.load_state_dict({"w.weight": w_enc})
     emb = Embedding(num_embeddings=1000, consider_as_one_hot=True, blank_id=0)
@@ -218,8 +206,8 @@ def _transducer_modules(sd, w_enc, W):
         m.load_state_dict({k[len(prefix) + 1:]: v for k, v in W.items() if k.startswith(prefix + ".")})
     s = TransducerBeamSearcher([emb, dec, proj_dec], Transducer_joint(joint="sum", nonlinearity=torch.nn.GELU), [lin],
                                blank_id=0, beam_size=1, nbest=1)
-    enc = LengthsCapableSequential(fb, norm, cnn, EncoderWrapper(tr), proj_enc)
-    return dict(encoder=enc, decoder=s), dict(CNN=cnn, Transformer=tr, proj_enc=proj_enc, emb=emb, dec=dec,
+    enc = LengthsCapableSequential(mirror.fb, mirror.norm, mirror.cnn, EncoderWrapper(mirror.tr), proj_enc)
+    return dict(encoder=enc, decoder=s), dict(CNN=mirror.cnn, Transformer=mirror.tr, proj_enc=proj_enc, emb=emb, dec=dec,
                                                proj_dec=proj_dec, transducer_lin=lin)
 
 
@@ -245,7 +233,7 @@ def test_encoder_decoder_asr_transducer_end_to_end():
     with a reference margin < 5e-3, and from there the oracle walked along the device's decisions (check_rows)."""
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
     fx, cfg, sd, w_enc, W, wav, lens = _fixture_e2e()
-    mods, _ = _transducer_modules(sd, w_enc, W)
+    mods, _ = _transducer_modules(cfg, sd, w_enc, W)
     asr = EncoderDecoderASR(modules=mods, hparams={"tokenizer": None, "transducer_beam_search": True},
                             run_opts={"device": "cuda:0"})
     tn = asr.encode_batch(wav.cuda(), lens.cuda())
@@ -364,7 +352,7 @@ def test_from_hparams_local_directory_matches_direct_construction(tmp_path):
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
     from speechbrain_b200.decoders.transducer import TransducerBeamSearcher
     fx, cfg, sd, w_enc, W, wav, lens = _fixture_e2e()
-    mods, parts = _transducer_modules(sd, w_enc, W)
+    mods, parts = _transducer_modules(cfg, sd, w_enc, W)
     order = ["CNN", "Transformer", "proj_enc", "emb", "dec", "proj_dec", "transducer_lin"]
     ck = {f"{i}.{k}": v for i, n in enumerate(order) for k, v in parts[n].state_dict().items()}
     tmp = write_pretrained_dir(tmp_path, HPARAMS, dict(asr=ck, normalizer=normalizer_ckpt(sd)))

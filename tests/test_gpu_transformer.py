@@ -19,6 +19,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from parity import (case_wav, check_alone_vs_batch, check_encoder, check_greedy, check_summary, dev,  # noqa: E402,F401
                     lm_scorer, module_list_ckpt, normalizer_ckpt, rel, write_pretrained_dir)
 import transformer_oracle as TO  # noqa: E402
+from mirrors import build_mirror, seeded  # noqa: E402
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 ENC_BAR = 1e-3
@@ -33,16 +34,17 @@ def fx():
 
 @pytest.fixture(scope="module")
 def sd(fx):
-    from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE, seeded_asr_state
-    return seeded_asr_state(TRANSFORMER_LARGE, fx["weight_seed"])
+    from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE
+    return seeded(TRANSFORMER_LARGE, fx["weight_seed"])
+
+
+def _mirror(sd):
+    from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE
+    return build_mirror(TRANSFORMER_LARGE, sd)
 
 
 def _front_end(sd, dev):
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=3, num_layers_per_block=1, out_channels=(64, 64, 64),
-                              kernel_sizes=(5, 5, 1), strides=(2, 2, 1), residuals=(False, False, True))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    return cnn.to(dev)
+    return _mirror(sd).cnn.to(dev)
 
 
 @pytest.mark.parametrize("B,T0", [(2, 1001), (3, 1003), (1, 1002), (2, 5), (1, 6), (1, 7), (4, 37)])
@@ -91,24 +93,13 @@ def test_transformer_large_encoder_and_greedy(dev, fx, sd):
     check_alone_vs_batch(lambda w, ln: eng.encode_wav(w.to(dev), ln.to(dev)), wav, lens, 1e-5)
 
 
-def _transformer(sd):
-    """The TransformerASR mirror loaded with every reference key; the sine table is the only buffer not in ``sd``."""
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    tr = TransformerASR(input_size=1280, tgt_vocab=5000, d_model=512, nhead=4, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="transformer", attention_type="regularMHA",
-                        normalize_before=True, causal=False)
-    res = tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    assert list(res.unexpected_keys) == [] and list(res.missing_keys) == ["positional_encoding.pe"]
-    return tr
-
-
 @pytest.mark.parametrize("n", [3, 72])
 def test_head_dim_128_decoder_attention_teacher_forced(dev, sd, n):
     """TransformerASR.decode (self- and cross-attention at 4 heads of 128) against the oracle's decoder, on ragged
     encoder states: 3 rows run the weight-streaming decode path, 72 rows (>= 64) the wgmma one."""
     from oracle import asr_oracle as O
     from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE as cfg
-    tr = _transformer(sd)
+    tr = _mirror(sd).tr
     g = torch.Generator().manual_seed(7 + n)
     T, S = 97, 11
     enc = torch.randn(n, T, 512, generator=g)
@@ -124,25 +115,11 @@ def test_head_dim_128_decoder_attention_teacher_forced(dev, sd, n):
     assert torch.isfinite(out).all() and err <= 2e-3
 
 
-
-def _asr_modules(sd, dev, beam, max_decode_ratio, lm):
-    """The recipe's modules as this package's mirrors, wired like transformer.yaml's test search (beam, temperature 1.15,
-    no EOS threshold, CTC 0.4 + TransformerLM 0.6)."""
-    from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
-    from speechbrain_b200.nnet.linear import Linear
-    tr = _transformer(sd)
-    V = sd["seq_lin.w.weight"].shape[0]
-    seq_lin, ctc_lin = Linear(input_size=512, n_neurons=V), Linear(input_size=512, n_neurons=V)
-    seq_lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": sd["seq_lin.w.bias"]})
-    ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    scorer = ScorerBuilder(full_scorers=[CTCScorer(eos_index=2, blank_index=0, ctc_fc=ctc_lin),
-                                         TransformerLMScorer(language_model=lm, temperature=1.15)],
-                           weights={"ctc": 0.4, "transformerlm": 0.6})
-    bs = S2STransformerBeamSearcher(modules=[tr, seq_lin], bos_index=1, eos_index=2, min_decode_ratio=0.0,
-                                    max_decode_ratio=max_decode_ratio, beam_size=beam, temperature=1.15,
-                                    using_eos_threshold=False, length_normalization=True, scorer=scorer)
-    return tr, bs
+def _searcher(m, beam, max_decode_ratio, lm):
+    """transformer.yaml's test search on the mirror m: beam, temperature 1.15, no EOS threshold, CTC 0.4 + TransformerLM
+    0.6 (in that order)"""
+    kwargs = dict(min_decode_ratio=0.0, beam_size=beam, temperature=1.15, using_eos_threshold=False, length_normalization=True)
+    return m.searcher(kwargs, max_decode_ratio, scorers=dict(ctc=0.4, transformerlm=0.6), lm=lm)
 
 
 def test_beam10_ctc_lm_matches_reference(dev, fx, sd):
@@ -154,7 +131,7 @@ def test_beam10_ctc_lm_matches_reference(dev, fx, sd):
     with torch.no_grad():
         enc = TO.encode(TO.wav_to_cnn(wav, lens, sd, cfg), lens, sd, cfg)
     assert gb["lm_seed"] == 1
-    _, bs = _asr_modules(sd, dev, gb["kwargs"]["beam_size"], gb["max_decode_ratio"], lm_scorer())
+    bs = _searcher(_mirror(sd), gb["kwargs"]["beam_size"], gb["max_decode_ratio"], lm_scorer())
     hyps, _, scores, _ = bs(enc.to(dev), lens.to(dev))
     print(f"[transformer_large beam10 ctc+lm] hyps equal {hyps == gb['hyps']}; score err "
           f"{(scores.cpu() - gb['scores']).abs().max():.2e}")
@@ -267,11 +244,7 @@ def test_from_hparams_local_directory_round_trip(dev, fx, sd, tmp_path):
     seq_lin, TransformerLM, beam search with the CTC and LM scorers) loads through from_hparams, the checkpoints land in the
     mirrors, and it transcribes like the same modules wired directly."""
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
     from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
-    from speechbrain_b200.nnet.containers import LengthsCapableSequential
-    from speechbrain_b200.processing.features import InputNormalization
     from speechbrain_b200.utils.seeded_init import seeded_state_dict
     lm = TransformerLM(vocab=5000, d_model=128, nhead=2, num_encoder_layers=2, num_decoder_layers=0, d_ffn=256, dropout=0.0,
                        activation=torch.nn.GELU, normalize_before=False)
@@ -279,13 +252,8 @@ def test_from_hparams_local_directory_round_trip(dev, fx, sd, tmp_path):
     tmp = write_pretrained_dir(tmp_path, HPARAMS, dict(asr=module_list_ckpt(sd), lm=lm.state_dict(), normalizer=normalizer_ckpt(sd)))
     loaded = EncoderDecoderASR.from_hparams(source=tmp, run_opts={"device": str(dev)})
     # direct construction of the same layout
-    tr, bs = _asr_modules(sd, dev, 10, 0.05, lm)
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = _front_end(sd, dev)
-    enc = LengthsCapableSequential(compute_features=Fbank(sample_rate=16000, n_fft=400, n_mels=80), normalize=norm, cnn=cnn)
-    direct = EncoderDecoderASR(modules=dict(encoder=enc, transformer=tr, decoder=bs),
+    m = _mirror(sd)
+    direct = EncoderDecoderASR(modules=dict(encoder=m.front_end(), transformer=m.tr, decoder=_searcher(m, 10, 0.05, lm)),
                                hparams=dict(tokenizer=None, transformer_beam_search=True), run_opts={"device": str(dev)})
     assert torch.equal(loaded.mods["decoder"].fc.w.weight.cpu(), sd["seq_lin.w.weight"])
     wav, lens = case_wav(fx["large"])

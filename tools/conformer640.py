@@ -80,10 +80,11 @@ def dec_cross_attention(dev, rows, rpu, T, H, dh):
 def model_times(dev, B, reps):
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import conformer640_oracle as CO
+    from mirrors import build_mirror, seeded
     from speechbrain_b200.engine import AsrEngine
     from speechbrain_b200.utils.seeded_init import CONFORMER_640
     cfg = CONFORMER_640
-    sd = CO.state(cfg)
+    sd = seeded(cfg)
     eng = AsrEngine(cfg, sd, device=str(dev))
     g = torch.Generator().manual_seed(0)
     wav = torch.randn(B, 160000, generator=g).to(dev)
@@ -94,9 +95,9 @@ def model_times(dev, B, reps):
     enc = eng.encode_wav(wav, lens)
     import importlib
     T = importlib.import_module("test_gpu_conformer640")
-    times = {}
+    times, m = {}, build_mirror(cfg, sd)
     for steps in (1, 24):
-        _, _, _, bs = T._search_modules(cfg, 66, 0.6, 0.4, (steps + 0.5) / enc.shape[1])
+        bs = T.searcher(m, 66, 0.6, 0.4, (steps + 0.5) / enc.shape[1])
         times[steps] = events(lambda: bs(enc, lens), 1, reps)
     res["beam66_lm_ctc_step_ms"] = (times[24] - times[1]) / 23
     return res

@@ -61,6 +61,8 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("loquacious.py measures on a GPU; none found")
     import loquacious_oracle as LO
+    import test_gpu_loquacious as T
+    from mirrors import build_mirror, seeded
     from speechbrain_b200.engine import AsrEngine
     from speechbrain_b200.utils.seeded_init import LOQUACIOUS_LARGE, LOQUACIOUS_XLARGE
     dev = torch.device("cuda:0")
@@ -69,14 +71,15 @@ def main():
     wav = torch.randn(32, 160000, generator=g).to(dev)
     lens = torch.ones(32, device=dev)
     cfg = LOQUACIOUS_XLARGE
-    eng = AsrEngine(cfg, LO.state(cfg), device=str(dev))
+    eng = AsrEngine(cfg, seeded(cfg), device=str(dev))
     out = measure({"xlarge_encode_32x10s": lambda: eng.encode_wav(wav, lens),
                    "xlarge_encode_greedy48_32x10s": lambda: eng.transcribe_greedy_dev(wav, lens, 48, LO.BOS, LO.EOS)},
                   args.reps)
     res.update(out)
     enc, l8 = eng.encode_wav(wav[:8], lens[:8]), lens[:8]
     del eng
-    searchers = {s: LO.search_modules(cfg, (s + 0.5) / enc.shape[1])[3] for s in (1, 24)}
+    m = build_mirror(cfg, seeded(cfg))
+    searchers = {s: T.searcher(m, (s + 0.5) / enc.shape[1]) for s in (1, 24)}
     for b in searchers.values():
         b(enc, l8)
     torch.cuda.synchronize()
@@ -85,9 +88,9 @@ def main():
         t1, t24 = timed(lambda: searchers[1](enc, l8)), timed(lambda: searchers[24](enc, l8))
         steps.append((t24 - t1) / 23)
     res["xlarge_beam80_ctc_step_8x10s"] = stats(steps)
-    del searchers
+    del searchers, m
     cfg = LOQUACIOUS_LARGE
-    sd = LO.state(cfg)
+    sd = seeded(cfg)
     engs = {a: AsrEngine(dict(cfg, conformer_activation=a), sd, device=str(dev)) for a in ("swish", "gelu")}
     res.update(measure({f"large_{a}_encode_32x10s": (lambda e=e: e.encode_wav(wav, lens)) for a, e in engs.items()},
                        args.reps))

@@ -19,6 +19,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 B, L, STEPS = 32, 160000, 48
 
@@ -43,42 +44,15 @@ def front_end_flops(Bn, T0, F0=80, C=64):
     return 2.0 * macs
 
 
-def build_asr(sd, dev, lm_sd):
-    from speechbrain_b200.decoders.scorer import CTCScorer, ScorerBuilder, TransformerLMScorer
-    from speechbrain_b200.decoders.seq2seq import S2STransformerBeamSearcher
+def build_asr(sd, dev):
+    """EncoderDecoderASR of the recipe's modules with its test search: beam 10, CTC 0.4 + the 12 x 768 TransformerLM 0.6"""
+    from mirrors import build_mirror
     from speechbrain_b200.inference.ASR import EncoderDecoderASR
-    from speechbrain_b200.lobes.features import Fbank
-    from speechbrain_b200.lobes.models.convolution import ConvolutionFrontEnd
-    from speechbrain_b200.lobes.models.transformer.TransformerASR import TransformerASR
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
-    from speechbrain_b200.nnet.containers import LengthsCapableSequential
-    from speechbrain_b200.nnet.linear import Linear
-    from speechbrain_b200.processing.features import InputNormalization
-
-    norm = InputNormalization(norm_type="global")
-    norm.glob_mean, norm.glob_std, norm.count = sd["normalize.glob_mean"], sd["normalize.glob_std"], 1
-    norm.eval()
-    cnn = ConvolutionFrontEnd(input_shape=(8, 10, 80), num_blocks=3, num_layers_per_block=1, out_channels=(64, 64, 64),
-                              kernel_sizes=(5, 5, 1), strides=(2, 2, 1), residuals=(False, False, True))
-    cnn.load_state_dict({k[4:]: v for k, v in sd.items() if k.startswith("CNN.")})
-    tr = TransformerASR(input_size=1280, tgt_vocab=5000, d_model=512, nhead=4, num_encoder_layers=12, num_decoder_layers=6,
-                        d_ffn=2048, activation=torch.nn.GELU, encoder_module="transformer", attention_type="regularMHA",
-                        normalize_before=True, causal=False)
-    tr.load_state_dict({k[len("Transformer."):]: v for k, v in sd.items() if k.startswith("Transformer.")}, strict=False)
-    seq_lin, ctc_lin = Linear(input_size=512, n_neurons=5000), Linear(input_size=512, n_neurons=5000)
-    seq_lin.load_state_dict({"w.weight": sd["seq_lin.w.weight"], "w.bias": sd["seq_lin.w.bias"]})
-    ctc_lin.load_state_dict({"w.weight": sd["ctc_lin.w.weight"], "w.bias": sd["ctc_lin.w.bias"]})
-    lm = TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0, d_ffn=3072,
-                       dropout=0.0, activation=torch.nn.GELU, normalize_before=False)
-    lm.load_state_dict(lm_sd)
-    scorer = ScorerBuilder(full_scorers=[CTCScorer(eos_index=2, blank_index=0, ctc_fc=ctc_lin),
-                                         TransformerLMScorer(language_model=lm, temperature=1.15)],
-                           weights={"ctc": 0.4, "transformerlm": 0.6})
-    dec = S2STransformerBeamSearcher(modules=[tr, seq_lin], bos_index=1, eos_index=2, min_decode_ratio=0.0,
-                                     max_decode_ratio=(STEPS + 0.5) / 251.0, beam_size=10, temperature=1.15,
-                                     using_eos_threshold=False, length_normalization=True, scorer=scorer)
-    enc = LengthsCapableSequential(compute_features=Fbank(sample_rate=16000, n_fft=400, n_mels=80), normalize=norm, cnn=cnn)
-    return EncoderDecoderASR(modules=dict(encoder=enc, transformer=tr, decoder=dec),
+    from speechbrain_b200.utils.seeded_init import TRANSFORMER_LARGE
+    m = build_mirror(TRANSFORMER_LARGE, sd)
+    kwargs = dict(min_decode_ratio=0.0, beam_size=10, temperature=1.15, using_eos_threshold=False, length_normalization=True)
+    dec = m.searcher(kwargs, (STEPS + 0.5) / 251.0, scorers=dict(ctc=0.4, transformerlm=0.6))
+    return EncoderDecoderASR(modules=dict(encoder=m.front_end(), transformer=m.tr, decoder=dec),
                              hparams=dict(tokenizer=None, transformer_beam_search=True), run_opts={"device": str(dev)})
 
 
@@ -91,8 +65,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("transformer_encode.py needs a CUDA device")
     from speechbrain_b200.engine import AsrEngine
-    from speechbrain_b200.lobes.models.transformer.TransformerLM import TransformerLM
-    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, TRANSFORMER_LARGE, seeded_asr_state, seeded_state_dict
+    from speechbrain_b200.utils.seeded_init import CONFORMER_LARGE, TRANSFORMER_LARGE, seeded_asr_state
 
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                           text=True).stdout.strip()
@@ -120,9 +93,7 @@ def main():
     fe_ms = _time(lambda: eng_t.cnn(feats), args.reps * 5)
     flops = front_end_flops(B, T0)
     # transcribe_batch, beam 10 + CTC + LM
-    lm_sd = seeded_state_dict(TransformerLM(vocab=5000, d_model=768, nhead=12, num_encoder_layers=12, num_decoder_layers=0,
-                                            d_ffn=3072, dropout=0.0, activation=torch.nn.GELU, normalize_before=False), seed=1)
-    asr = build_asr(sd_t, dev, lm_sd)
+    asr = build_asr(sd_t, dev)
     asr.transcribe_batch(wav, lens)
     tb_ms = _time(lambda: asr.transcribe_batch(wav, lens), max(2, args.reps // 3))
     med = lambda xs: sorted(xs)[len(xs) // 2]  # noqa: E731
