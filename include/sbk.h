@@ -180,6 +180,16 @@ int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, co
                            const int* enc_len_dev, const int* lineage_dev, const int* tok_cache_dev, int lin_stride,
                            int pad_tok, void* out_dev, int ldo, void* stream);
 
+/* the folded cross-attention of a decode step alone (rows = utterances, one query row each): the folded query projection
+ * (gemm_f16_small, fp16 out), dec_xatt_fold_kernel, and the folded output projection added to x_dev [rows, ldx] fp32 in
+ * place (columns [0, d); the others are left alone).  h16_dev [rows, d] fp16 is the LayerNorm output feeding the query
+ * projection; in_proj_w / in_proj_b / out_w / out_b are the layer's multihead_attn weights as fp32 HOST arrays ([3d, d],
+ * [3d], [d, d], [d]), folded on the host like the weight loader does.  enc16_dev [rows, T, d] fp16, enc_len_dev [rows] in
+ * [0, T] (0: the row is NaN).  d = 64 H, d = 256 or 512.  Synchronises the stream. */
+int sbk_xatt_fold_test(const void* h16_dev, const float* in_proj_w, const float* in_proj_b, const float* out_w,
+                       const float* out_b, const void* enc16_dev, const int* enc_len_dev, int rows, int T, int H, int d,
+                       float* x_dev, int ldx, void* stream);
+
 /* the streaming encoder's ring write alone (stream_qkv_kernel): qkv_dev [B*n, 3*H*head_dim] fp32 (per head [q | k | v]) ->
  * q_out_dev [B*n, H*head_dim] fp16 and each row's per-head [k | v] into slot (slot0 + i) % cap of kv_out_dev
  * [B][cap][2*H*head_dim] fp16.  inv_freq_dev [head_dim / 2] fp32: RoPE at stream positions pos0 + i with q scaled by

@@ -58,6 +58,15 @@ struct Packer {
     }
     const float* f32_raw(const std::vector<float>& v) { return f32_raw(v.data(), v.size()); }
     const __half* f16_raw(const std::vector<float>& v) { return f16_raw(v.data(), v.size()); }
+    // float64 products, rounded once to the stored type
+    const float* f32_raw(const std::vector<double>& v) { return f32_raw(std::vector<float>(v.begin(), v.end())); }
+    const __half* f16_raw(const std::vector<double>& v) {
+        if (carve.base) {
+            tmph.resize(v.size());
+            for (size_t i = 0; i < v.size(); ++i) tmph[i] = __double2half(v[i]);
+        }
+        return static_cast<const __half*>(place(tmph.data(), v.size() * 2));
+    }
     const float* f32(const std::string& k, int64_t n) {
         const float* src = host(k, n);
         return src ? f32_raw(src, n) : nullptr;
@@ -312,6 +321,37 @@ static void pack_encoder(Packer& p, AsrWeights& W) {
     pack_positional_tables(p, W);
 }
 
+bool xatt_foldable(const sbk_asr_config& c) {
+    return c.d_model == 64 * c.nhead && c.d_model % 256 == 0 && c.nhead * c.d_model <= 4096;
+}
+
+void fold_cross_attention(const float* wc, const float* bc, const float* wo, const float* bo, int d, int H,
+                          std::vector<double>* xq, std::vector<double>* bxq, std::vector<double>* xo, std::vector<double>* bxo) {
+    const int dh = d / H;
+    const std::vector<float> wq = fold_query_scale(wc, (size_t)d * d, (size_t)d * d, dh);  // the unfolded path's W_q, b_q
+    const std::vector<float> bq = fold_query_scale(bc, d, d, dh);
+    const float *wk = wc + (size_t)d * d, *wv = wc + (size_t)2 * d * d, *bv = bc + 2 * d;
+    xq->assign((size_t)H * d * d, 0.0); bxq->assign((size_t)H * d, 0.0);
+    xo->assign((size_t)d * H * d, 0.0); bxo->assign(bo, bo + d);
+    for (int h = 0; h < H; ++h)
+        for (int a = 0; a < dh; ++a) {
+            const size_t r = (size_t)h * dh + a;  // row of W_q / W_k / W_v, column of W_o
+            const float* q = &wq[r * d];
+            for (int i = 0; i < d; ++i) {
+                const double k = wk[r * d + i];
+                double* row = &(*xq)[((size_t)h * d + i) * d];
+                for (int j = 0; j < d; ++j) row[j] += k * q[j];
+                (*bxq)[(size_t)h * d + i] += k * bq[r];
+            }
+            for (int o = 0; o < d; ++o) {
+                const double w = wo[(size_t)o * d + r];
+                double* row = &(*xo)[(size_t)o * H * d + (size_t)h * d];
+                for (int i = 0; i < d; ++i) row[i] += w * wv[r * d + i];
+                (*bxo)[o] += w * bv[r];
+            }
+        }
+}
+
 static void pack_decoder(Packer& p, AsrWeights& W) {
     const sbk_asr_config& c = W.cfg;
     const int d = c.d_model, dh = d / c.nhead, F = c.d_ffn, L = c.num_decoder_layers;
@@ -338,6 +378,15 @@ static void pack_decoder(Packer& p, AsrWeights& W) {
         memcpy(&bckv[(size_t)l * 2 * d], bc + d, (size_t)2 * d * 4);
         p.linear(q + "self_attn.att.out_proj", d, d, &e.w_self_out, &e.b_self_out);
         p.linear(q + "multihead_attn.att.out_proj", d, d, &e.w_cross_out, &e.b_cross_out);
+        if (xatt_foldable(c)) {  // the products are only formed when the arena is filled; measuring needs their sizes
+            const float* wo = p.host(q + "multihead_attn.att.out_proj.weight", (int64_t)d * d);
+            const float* bo = p.host(q + "multihead_attn.att.out_proj.bias", d);
+            if (!wo || !bo) return;
+            std::vector<double> xq((size_t)c.nhead * d * d), bxq((size_t)c.nhead * d), xo((size_t)d * c.nhead * d), bxo(d);
+            if (p.carve.base) fold_cross_attention(wc, bc, wo, bo, d, c.nhead, &xq, &bxq, &xo, &bxo);
+            e.w_xq = p.f16_raw(xq); e.b_xq = p.f32_raw(bxq);
+            e.w_xo = p.f16_raw(xo); e.b_xo = p.f32_raw(bxo);
+        }
         p.linear(q + "pos_ffn.ffn.0", F, d, &e.w_ffn1, &e.b_ffn1);
         p.linear(q + "pos_ffn.ffn.3", d, F, &e.w_ffn2, &e.b_ffn2);
         if (!p.ok) return;

@@ -46,6 +46,9 @@ struct DecLayerW {
     const float *n1g, *n1b, *n2g, *n2b, *n3g, *n3b;
     const __half *w_self_in, *w_self_out, *w_cross_q, *w_cross_out, *w_ffn1, *w_ffn2;
     const float *b_self_in, *b_self_out, *b_cross_q, *b_cross_out, *b_ffn1, *b_ffn2;
+    // folded cross-attention (fold_cross_attention), packed only where xatt_foldable(): query [H d, d] and output [d, H d]
+    const __half *w_xq = nullptr, *w_xo = nullptr;
+    const float *b_xq = nullptr, *b_xo = nullptr;
 };
 
 struct LmLayerW {
@@ -100,6 +103,16 @@ struct AsrWeights {
 // element count fails before anything is allocated on the device.
 int load_asr_weights(const sbk_asr_config& cfg, const sbk_tensor* weights, int n_weights,
                      std::shared_ptr<const AsrWeights>* out);
+
+// Whether a decoder's cross-attention is packed in folded form as well: head width 64, d_model 256 or 512 (the widths the
+// folded cross-attention kernel is built for: H d_model <= 4096).
+bool xatt_foldable(const sbk_asr_config& c);
+// The folded cross-attention weights of one decoder layer, in float64 from its fp32 multihead_attn in_proj (wc [3d, d],
+// bc [3d]) and out_proj (wo [d, d], bo [d]), H heads of dh = d / H:
+//   xq [H d, d] rows (h, i) = sum_a W_k[h dh + a][i] W_q[h dh + a][:] / sqrt(dh),  bxq [H d] = W_k,h^T b_q,h / sqrt(dh);
+//   xo [d, H d] columns (h, i) = sum_a W_o[:, h dh + a] W_v[h dh + a][i],         bxo [d] = b_o + W_o b_v.
+void fold_cross_attention(const float* wc, const float* bc, const float* wo, const float* bo, int d, int H,
+                          std::vector<double>* xq, std::vector<double>* bxq, std::vector<double>* xo, std::vector<double>* bxo);
 
 // Rows t = 0 .. rows - 1 of the reference's PositionalEncoding(d) (Transformer.py:252-303; row |r| of RelPosEncXL,
 // nnet/attention.py:360-408, is the same): even columns sin(t f_i), odd columns cos(t f_i), in fp32 like the reference's

@@ -55,8 +55,8 @@ constexpr int SBK_NUM_SMS = 132;
 // attribute).  pdl_trigger() lets the successor start launching.  Rules for the code a kernel runs before pdl_wait(),
 // which may overlap not only the predecessor but, through its early trigger, kernels further back in the stream:
 //   * read only data no kernel of the decode loop writes (weights, biases, LayerNorm parameters, the cross-attention
-//     K/V ckv16, enc_len), and that data must come from kernels that never trigger early (project_cross_kv,
-//     abs_len_kernel);
+//     K/V ckv16, the fp16 encoder states enc16 the folded cross-attention reads, enc_len), and that data must come from
+//     kernels that never trigger early (project_cross_kv, abs_len_kernel);
 //   * write nothing to global memory: a predecessor that is still running could read the overwritten values;
 //   * never read step, dx, dh16, dq16, datt16, df16, the self-attention K/V caches, logits or tokens.
 // Every kernel launched this way executes pdl_wait() in at least one thread, so its completion implies its
@@ -94,6 +94,22 @@ __device__ __forceinline__ float warp_max(float v) {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+
+// ---------------------------------------------------------------- ldmatrix (8 x 8 fp16 tiles from shared memory)
+__device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, const void* p) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(smem_u32(p)));
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(smem_u32(p)));
+}
+__device__ __forceinline__ void ldmatrix_x2(uint32_t& r0, uint32_t& r1, const void* p) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(smem_u32(p)));
+}
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(smem_u32(p)));
 }
 
 // ---------------------------------------------------------------- mbarrier

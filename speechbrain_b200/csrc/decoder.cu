@@ -532,6 +532,171 @@ int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t s
     return SBK_OK;
 }
 
+// --------------------------------------------------------------------------- folded cross-attention (1 row / utterance)
+// Every head's keys and values are linear in the same encoder states e: k_t = W_k,h e_t + b_k,h, v_t = W_v,h e_t + b_v,h.
+// So q_h . k_t = (W_k,h^T q_h) . e_t + q_h . b_k,h, whose last term is the same for every key and cancels in the softmax,
+// and sum_t p_t v_t = W_v,h (sum_t p_t e_t) + b_v,h since the p_t sum to 1.  The step's query projection writes the folded
+// queries q'_h = W_k,h^T q_h, this kernel the context vectors sum_t p_t e_t, and the output projection applies
+// W_o[:, h] W_v,h to them (asr_weights.cu packs both).  A layer then reads e (2 D bytes per frame) instead of its K and V
+// (4 D bytes per frame).
+// One CTA per utterance, warp w of 8 owning dims [w D / 8, (w + 1) D / 8) of e.  Blocks of XF_FRAMES frames stream through a
+// cp.async ring; per block each warp computes the H heads' partial scores over its dims (mma m16n8k16, the heads padded to
+// 16 rows), the 8 partials are summed through shared memory in a fixed order, every warp runs the same online softmax and
+// accumulates P e over its own dims.  Results depend on the utterance alone.
+constexpr int XF_WARPS = 8;
+constexpr int XF_FRAMES = 32;
+constexpr int XF_STAGES = 3;
+constexpr int XF_RED = XF_FRAMES + 8;  // row stride of the partial scores: at most 2-way bank conflicts
+template <int D>
+constexpr size_t xf_smem_bytes() {  // frame rows padded by 16 bytes: the 8 rows of an ldmatrix tile hit distinct banks
+    return (size_t)XF_STAGES * XF_FRAMES * (D + 8) * 2 + (size_t)XF_WARPS * 8 * XF_RED * 4;
+}
+
+template <int D>
+__global__ void __launch_bounds__(XF_WARPS * 32, 2) dec_xatt_fold_kernel(const XattFoldArgs a) {
+    constexpr int SROW = D + 8, KW = D / XF_WARPS, NKS = KW / 16, NNT = KW / 8, NJ = XF_FRAMES / 8;
+    constexpr int CHUNKS = XF_FRAMES * D / 8;  // 16-byte pieces of one block
+    static_assert(CHUNKS % (XF_WARPS * 32) == 0 && NKS % 2 == 0 && NNT % 2 == 0, "dec_xatt_fold_kernel: tile shape");
+    extern __shared__ __align__(16) uint8_t xf_sm[];
+    __half* ring = reinterpret_cast<__half*>(xf_sm);
+    float* red = reinterpret_cast<float*>(xf_sm + (size_t)XF_STAGES * XF_FRAMES * SROW * 2);  // [warp][head][frame]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
+    const int utt = blockIdx.x;
+    // enc16 and enc_len come from kernels that never trigger early (see common.cuh): the first blocks' loads are issued
+    // before pdl_wait().  The successor is only triggered after the main loop: its CTAs would otherwise sit on the SMs
+    // waiting, holding the shared memory this kernel's second CTA per SM needs.
+    const int n_keys = min(a.enc_len[utt], a.T);
+    const int n_blk = ceil_div(n_keys, XF_FRAMES);
+    const __half* e = a.e + static_cast<size_t>(utt) * a.T * D;
+    auto load_block = [&](int blk) {  // frames past n_keys are zero-filled: their p is 0, and 0 * garbage could be NaN
+        if (blk < n_blk) {
+            __half* dst = ring + static_cast<size_t>(blk % XF_STAGES) * XF_FRAMES * SROW;
+#pragma unroll
+            for (int i = 0; i < CHUNKS / (XF_WARPS * 32); ++i) {
+                const int idx = threadIdx.x + i * XF_WARPS * 32;
+                const int f = idx / (D / 8), v8 = idx % (D / 8);
+                const int t = blk * XF_FRAMES + f;
+                const __half* src = e + static_cast<size_t>(t < n_keys ? t : 0) * D + v8 * 8;
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst + f * SROW + v8 * 8)),
+                             "l"(src), "r"(t < n_keys ? 16 : 0));
+            }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+#pragma unroll
+    for (int s = 0; s < XF_STAGES - 1; ++s) load_block(s);
+    pdl_wait();
+    // A fragments of this warp's dims of q'_h, h = g (rows g + 8 and heads >= H are zero)
+    uint32_t qa[NKS][2];
+    const __half* qrow = a.q + static_cast<size_t>(utt) * a.ldq + static_cast<size_t>(g) * D + warp * KW + 2 * c;
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks) {
+        qa[ks][0] = g < a.H ? *reinterpret_cast<const uint32_t*>(qrow + 16 * ks) : 0u;
+        qa[ks][1] = g < a.H ? *reinterpret_cast<const uint32_t*>(qrow + 16 * ks + 8) : 0u;
+    }
+    float acc[NNT][4];
+#pragma unroll
+    for (int nt = 0; nt < NNT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.0f;
+    float m_run = -INFINITY, l_run = 0.0f;
+    for (int blk = 0; blk < n_blk; ++blk) {
+        asm volatile("cp.async.wait_group %0;" ::"n"(XF_STAGES - 2) : "memory");
+        __syncthreads();  // block blk landed for every thread; everyone is done with the stage and `red` reused below
+        load_block(blk + XF_STAGES - 1);
+        const __half* st = ring + static_cast<size_t>(blk % XF_STAGES) * XF_FRAMES * SROW + warp * KW;
+        // ---- partial scores over this warp's dims: frames 8 j .. 8 j + 7 per n8 tile, two k16 steps per ldmatrix.x4
+        float sp[NJ][4];
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+            sp[j][0] = sp[j][1] = sp[j][2] = sp[j][3] = 0.0f;
+#pragma unroll
+            for (int ks = 0; ks < NKS; ks += 2) {
+                uint32_t b0, b1, b2, b3;
+                ldmatrix_x4(b0, b1, b2, b3, st + (8 * j + (lane & 7)) * SROW + 16 * ks + 8 * (lane >> 3));
+                const uint32_t a0[4] = {qa[ks][0], 0u, qa[ks][1], 0u};
+                const uint32_t a1[4] = {qa[ks + 1][0], 0u, qa[ks + 1][1], 0u};
+                mma16816_d(sp[j], a0, b0, b1);
+                mma16816_d(sp[j], a1, b2, b3);
+            }
+            *reinterpret_cast<float2*>(red + (warp * 8 + g) * XF_RED + 8 * j + 2 * c) = make_float2(sp[j][0], sp[j][1]);
+        }
+        __syncthreads();
+        // ---- full scores of head g at this lane's frames 8 j + 2 c (+1), online softmax (same in every warp)
+        float s[NJ][2];
+        float cm = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                float v = 0.0f;
+#pragma unroll
+                for (int w = 0; w < XF_WARPS; ++w) v += red[(w * 8 + g) * XF_RED + 8 * j + 2 * c + u];
+                s[j][u] = blk * XF_FRAMES + 8 * j + 2 * c + u < n_keys ? v : -INFINITY;
+                cm = fmaxf(cm, s[j][u]);
+            }
+        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 1));
+        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 2));
+        const float m_new = fmaxf(m_run, cm);  // finite: every block processed has a visible key
+        const float alpha = m_run == -INFINITY ? 0.0f : __expf(m_run - m_new);
+        float psum = 0.0f;
+        uint32_t pa[NJ / 2][4];
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+            const float p0 = __expf(s[j][0] - m_new), p1 = __expf(s[j][1] - m_new);
+            psum += p0 + p1;
+            const __half2 h = floats2half2_sat(p0, p1);
+            pa[j / 2][(j & 1) * 2] = *reinterpret_cast<const uint32_t*>(&h);  // a0: frames 16 ks + 2c, a2: + 8
+            pa[j / 2][(j & 1) * 2 + 1] = 0u;                                  // rows g + 8
+        }
+        psum += __shfl_xor_sync(0xffffffffu, psum, 1);
+        psum += __shfl_xor_sync(0xffffffffu, psum, 2);
+        l_run = l_run * alpha + psum;
+        m_run = m_new;
+        // ---- context += P e over this warp's dims (B fragments of e[frame][dim] via ldmatrix.trans)
+#pragma unroll
+        for (int nt = 0; nt < NNT; ++nt) { acc[nt][0] *= alpha; acc[nt][1] *= alpha; }
+#pragma unroll
+        for (int ks = 0; ks < NJ / 2; ++ks)
+#pragma unroll
+            for (int nt = 0; nt < NNT; nt += 2) {
+                uint32_t b0, b1, b2, b3;
+                ldmatrix_x4_trans(b0, b1, b2, b3, st + (16 * ks + (lane & 15)) * SROW + 8 * nt + 8 * (lane >> 4));
+                mma16816_d(acc[nt], pa[ks], b0, b1);
+                mma16816_d(acc[nt + 1], pa[ks], b2, b3);
+            }
+    }
+    pdl_trigger();
+    if (g < a.H) {  // no visible key: 0 / 0 = NaN, like the unfolded path
+        __half* o = a.out + static_cast<size_t>(utt) * a.ldo + static_cast<size_t>(g) * D + warp * KW + 2 * c;
+#pragma unroll
+        for (int nt = 0; nt < NNT; ++nt)
+            *reinterpret_cast<__half2*>(o + 8 * nt) = floats2half2_sat(acc[nt][0] / l_run, acc[nt][1] / l_run);
+    }
+}
+
+int dec_xatt_fold(const XattFoldArgs& a, int n_utt, cudaStream_t stream) {
+    SBK_REQUIRE((a.D == 512 && a.H >= 1 && a.H <= 8) || (a.D == 256 && a.H >= 1 && a.H <= 4),
+                "dec_xatt_fold: D=%d with %d heads not built (512 with <= 8, 256 with <= 4)", a.D, a.H);
+    SBK_REQUIRE(a.ldq % 8 == 0 && a.ldo % 2 == 0 && a.ldq >= a.H * a.D && a.ldo >= a.H * a.D && a.T >= 1 &&
+                    (reinterpret_cast<uintptr_t>(a.q) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.e) & 15) == 0 &&
+                    (reinterpret_cast<uintptr_t>(a.out) & 3) == 0,
+                "dec_xatt_fold: bad strides or alignment");
+    if (n_utt == 0) return SBK_OK;
+    static bool attr_done = false;  // above the 48 KB default
+    if (!attr_done) {
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(dec_xatt_fold_kernel<512>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)xf_smem_bytes<512>()));
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(dec_xatt_fold_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)xf_smem_bytes<256>()));
+        attr_done = true;
+    }
+    if (a.D == 512)
+        SBK_CUDA_CHECK(launch_k(dec_xatt_fold_kernel<512>, dim3(n_utt), dim3(XF_WARPS * 32), xf_smem_bytes<512>(), stream, a));
+    else
+        SBK_CUDA_CHECK(launch_k(dec_xatt_fold_kernel<256>, dim3(n_utt), dim3(XF_WARPS * 32), xf_smem_bytes<256>(), stream, a));
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
 
 // --------------------------------------------------------------------------- greedy step bookkeeping
 // decoders/seq2seq.py:226-257: argmax, fp32 log_softmax, has_ended |= (tok == eos); ended rows get

@@ -278,8 +278,10 @@ static void workspace_layout(const AsrModel* m, int B, int Be, int L, int rows, 
     take(b.f16, M * Fu * 2); take(b.qkv16, M * 3 * d * 2); take(b.att16, M * d * 2);
     take(b.P16, (size_t)T2 * d * 2); take(b.enc16, Md * d * 2); take(b.ckv16, Md * Ld * 2 * d * 2);
     take(b.kcache, (size_t)Ld * rows * S * d * 2); take(b.vcache, (size_t)Ld * rows * S * d * 2);
-    take(b.dh16, (size_t)rows * d * 2); take(b.dq16, (size_t)rows * d * 2); take(b.datt16, (size_t)rows * d * 2);
-    take(b.df16, (size_t)rows * F * 2);
+    // a folded cross-attention keeps its H d-wide queries in dq16 and its context vectors in df16
+    const size_t Hd = m->wt->has_dec && m->wt->dec[0].w_xq ? (size_t)c.nhead * d : 0;
+    take(b.dh16, (size_t)rows * d * 2); take(b.dq16, (size_t)rows * std::max(d, Hd) * 2); take(b.datt16, (size_t)rows * d * 2);
+    take(b.df16, (size_t)rows * std::max(F, Hd) * 2);
     take(b.lineage, (size_t)2 * rows * S * 4); take(b.finished, B * 4 + 64); take(b.seq_scores, (size_t)2 * rows * 4);
     take(b.lnout, (size_t)rows * d * 4); take(b.beam_scr, (size_t)rows * 33 * 4);
     take(b.hist_tok, (size_t)rows * S * 4); take(b.hist_pred, (size_t)rows * S * 4);
@@ -581,11 +583,13 @@ static bool xatt_headmajor(const AsrModel* m) {
     static const bool legacy = getenv("SBK_XATT_ROWMAJOR") != nullptr;
     return !legacy && m->wt->cfg.d_model / m->wt->cfg.nhead == 64 && m->wt->cfg.d_model % 256 == 0;
 }
-static int project_cross_kv(AsrModel* m, int M, int T, cudaStream_t st) {
+// A folded call (xatt_fold) attends over enc16 itself and needs no K/V.
+static int project_cross_kv(AsrModel* m, int M, int T, bool fold, cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
     const int d = c.d_model, Ld = c.num_decoder_layers;
     RC(cast_f32_f16(b.enc_out, b.enc16, (size_t)M * d, st));
+    if (fold) return SBK_OK;
     if (xatt_headmajor(m)) {  // w_ckv / b_ckv are [Ld * 2d] rows: every layer's K and V in ONE GEMM, scattered per layer
         GemmEpilogue e;
         e.mode = EPI_F16; e.bias = m->wt->b_ckv; e.out = b.ckv16; e.ldo = Ld * 2 * d;
@@ -623,6 +627,23 @@ enum StepGemm { SG_STREAM, SG_SMALL, SG_WIDE };
 // chunks).
 static StepGemm step_gemm(const AsrModel* m, int rows, int width) {
     return rows >= m->dec_tc_rows && width % 32 == 0 ? SG_SMALL : SG_STREAM;
+}
+// Whether a decode call over n_utt utterances of T frames, one row each (greedy and teacher-forced decoding), runs the folded
+// cross-attention (dec_xatt_fold): each layer then streams the fp16 encoder states, 2 d bytes per frame, instead of its
+// cross-attention K and V, 4 d bytes per frame, and its query and output projections grow from d x d to H d x d weights;
+// the call also skips the K/V GEMM over all encoder frames.  By bytes alone the step would gain from n_utt T = 2 (H - 1) d
+// frames on, but the two grown projections cost far more than their extra weight bytes (H100 SXM at 700 W, 224 rows, d 512,
+// 8 heads: N = 4096 query projection 8 us, K = 4096 output projection 13 us, against 4 us each at d x d).  A folded
+// Conformer-L step at T = 251 measured +45 / +58 / +7 / -6 us against the K/V path at 64 / 96 / 160 / 224 live rows,
+// while the skipped K/V GEMM (6.3 MFLOP per frame) saves about 4.3 us per utterance once per call (at 370 TFLOP/s).
+// Over a 48-step call that crosses over near 150 utterances: the fold starts at n_utt T >= 11 (H - 1) d (39424 frames
+// for Conformer-L, 157 utterances of 10 s; DESIGN.md section 9), so 96 rows keep the K/V path and 160 rows fold.  Only
+// on the wgmma step back end, and only for decoders packed with folded weights (xatt_foldable).  Beam search keeps the K/V path: several
+// rows share an utterance's keys there, and the coverage scorer reads the last layer's K.
+static bool xatt_fold(const AsrModel* m, int n_utt, int T) {
+    const sbk_asr_config& c = m->wt->cfg;
+    return m->wt->dec[0].w_xq != nullptr && step_gemm(m, n_utt, c.d_model) == SG_SMALL &&
+           (size_t)n_utt * T >= (size_t)11 * (c.nhead - 1) * c.d_model;
 }
 // Programmatic dependent launch is on for the wgmma step (its GEMMs and LayerNorms are launched with it unconditionally)
 // and off for weight streaming, where it measured no faster (single_batch, H100 SXM at 400 W: 24.8 / 28.2 ms with it
@@ -686,7 +707,7 @@ static int dec_norm_project(AsrModel* m, StepGemm g, Proj p, const float* gamma,
     return norm_project(g, m->fuse_dec_ln, p, m->b.dx, gamma, beta, m->b.dh16, rows, st);
 }
 
-static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage,
+static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, const int* lineage, bool fold,
                                  cudaStream_t st, bool with_head = true) {
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
@@ -710,13 +731,21 @@ static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T,
         t.lineage = lineage; t.lin_stride = S_max;
         RC(dec_attention(t, rows, S_max, st));
         RC(project(g, {w.w_self_out, w.b_self_out, d, d, PO_RESID, b.dx, d, b.datt16, d}, rows, st));
-        // cross attention: LN2 + (pre-scaled) query projection
-        RC(dec_norm_project(m, g, {w.w_cross_q, w.b_cross_q, d, d, PO_F16, b.dq16, d}, w.n2g, w.n2b, rows, st));
-        t = DecAttnArgs{};
-        t.q = b.dq16; t.ldq = d; cross_kv_args(m, t, l, n_utt, T); t.rows_per_block = rows_per_utt;
-        t.n_keys_ptr = nullptr; t.enc_len = b.enc_len; t.H = H; t.dh = dh; t.out = b.datt16; t.ldo = d;
-        RC(dec_attention(t, rows, T, st));
-        RC(project(g, {w.w_cross_out, w.b_cross_out, d, d, PO_RESID, b.dx, d, b.datt16, d}, rows, st));
+        if (fold) {  // LN2 + folded query projection, attention over enc16, folded output projection (rows_per_utt == 1)
+            const int Hd = H * d;
+            RC(dec_norm_project(m, g, {w.w_xq, w.b_xq, Hd, d, PO_F16, b.dq16, Hd}, w.n2g, w.n2b, rows, st));
+            XattFoldArgs x{b.dq16, Hd, b.enc16, b.enc_len, T, H, d, b.df16, Hd};
+            RC(dec_xatt_fold(x, rows, st));
+            RC(project(g, {w.w_xo, w.b_xo, d, Hd, PO_RESID, b.dx, d, b.df16, Hd}, rows, st));
+        } else {
+            // cross attention: LN2 + (pre-scaled) query projection
+            RC(dec_norm_project(m, g, {w.w_cross_q, w.b_cross_q, d, d, PO_F16, b.dq16, d}, w.n2g, w.n2b, rows, st));
+            t = DecAttnArgs{};
+            t.q = b.dq16; t.ldq = d; cross_kv_args(m, t, l, n_utt, T); t.rows_per_block = rows_per_utt;
+            t.n_keys_ptr = nullptr; t.enc_len = b.enc_len; t.H = H; t.dh = dh; t.out = b.datt16; t.ldo = d;
+            RC(dec_attention(t, rows, T, st));
+            RC(project(g, {w.w_cross_out, w.b_cross_out, d, d, PO_RESID, b.dx, d, b.datt16, d}, rows, st));
+        }
         // feed-forward: LN3 + ffn1 + activation, then ffn2 + residual
         RC(dec_norm_project(m, g, {w.w_ffn1, w.b_ffn1, F, d, ffn_act, b.df16, F}, w.n3g, w.n3b, rows, st));
         RC(project(g, {w.w_ffn2, w.b_ffn2, d, F, PO_RESID, b.dx, d, b.df16, F}, rows, st));
@@ -727,10 +756,10 @@ static int enqueue_decode_layers(AsrModel* m, int rows, int rows_per_utt, int T,
                             m->wt->dec_norm_b, rows, st);  // final LayerNorm + seq_lin
 }
 
-static int enqueue_decode_step(AsrModel* m, int rows, int rows_per_utt, int T, int S_max, int eos, float* log_probs,
-                               int L_lp, cudaStream_t st) {
+static int enqueue_decode_step(AsrModel* m, int rows, int T, int S_max, bool fold, int eos, float* log_probs, int L_lp,
+                               cudaStream_t st) {
     AsrModel::Buf& b = m->b;
-    RC(enqueue_decode_layers(m, rows, rows_per_utt, T, S_max, nullptr, st));
+    RC(enqueue_decode_layers(m, rows, 1, T, S_max, nullptr, fold, st));
     RC(greedy_select(b.logits, rows, m->wt->cfg.vocab, b.step, eos, b.tokens, S_max + 1, b.has_ended, b.ended_count, b.pred,
                      b.score, S_max, log_probs, L_lp, m->wt->emb, m->wt->dec_pe, m->wt->cfg.d_model, b.dx, st));
     return SBK_OK;
@@ -820,7 +849,7 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
     SBK_REQUIRE(p.max_steps <= m->ws_steps && p.max_steps + 1 <= c.max_len, "beam: max_steps=%d too large", p.max_steps);
     *steps_done = 0;
     if (p.max_steps <= 0) return SBK_OK;
-    RC(project_cross_kv(m, M, T, st));
+    RC(project_cross_kv(m, M, T, false, st));
     set_step_pdl(m, rows, d);
     const bool use_lm = p.lm_weight != 0.0f;
     SBK_REQUIRE(!use_lm || m->wt->has_lm, "beam: lm_weight != 0 but this handle has no TransformerLM weights");
@@ -898,7 +927,7 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
         }
         if (use_ctc) RC(ctc_prefix_update(cs, s2));  // permute_scorer_mem on the previous step's survivors (no-op at step 0)
         if (use_lm) RC(enqueue_lm_step(m, rows, S_max, p.lm_temperature, p.lm_weight, s2));
-        RC(enqueue_decode_layers(m, rows, beam, T, S_max, b.lineage, s_));
+        RC(enqueue_decode_layers(m, rows, beam, T, S_max, b.lineage, false, s_));
         if (use_cov) RC(coverage_score(cv, s_));  // reads the last layer's cross-attention query left in b.dq16
         if (fork) RC(m->side_stream.join(s_));
         if (use_ctc) RC(ctc_prefix_score(cs, s_));  // ScorerBuilder.score (ctc after transformerlm)
@@ -934,24 +963,25 @@ static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos
     SBK_REQUIRE(max_steps <= m->ws_steps && max_steps + 1 <= c.max_len, "greedy: max_steps=%d too large", max_steps);
     *steps_done = 0;
     if (max_steps <= 0) return SBK_OK;
-    RC(project_cross_kv(m, M, T, st));  // cross-attention K/V of all layers, once per utterance
+    const bool fold = xatt_fold(m, B, T);
+    RC(project_cross_kv(m, M, T, fold, st));  // cross-attention K/V of all layers, once per utterance
     RC(greedy_reset(b.tokens, S_max + 1, rows, bos, b.step, b.has_ended, b.ended_count, m->wt->emb, m->wt->dec_pe, d, b.dx, st));
     set_step_pdl(m, rows, d);
     const bool use_graph = !in_capture && getenv("SBK_NO_GRAPH") == nullptr && log_probs == nullptr;
     if (in_capture) {  // the caller is capturing the whole pipeline: enqueue exactly max_steps steps, no polling
-        for (int i = 0; i < max_steps; ++i) RC(enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, st));
+        for (int i = 0; i < max_steps; ++i) RC(enqueue_decode_step(m, rows, T, S_max, fold, eos, log_probs, max_steps, st));
         *steps_done = max_steps;
         return SBK_OK;
     }
     if (use_graph) {
         const struct StepKey { int rows, T, B, eos, S_max; } key = {rows, T, B, eos, S_max};
         RC(m->step_graph.ensure(key, m->cap_stream, [&](cudaStream_t cs) {
-            return enqueue_decode_step(m, rows, 1, T, S_max, eos, nullptr, 0, cs);
+            return enqueue_decode_step(m, rows, T, S_max, fold, eos, nullptr, 0, cs);
         }));
     }
     // seq2seq.py:256 `has_ended.all()` early exit
     return run_steps(m, max_steps, rows, st, [&](cudaStream_t s_) {
-        return use_graph ? m->step_graph.launch(s_) : enqueue_decode_step(m, rows, 1, T, S_max, eos, log_probs, max_steps, s_);
+        return use_graph ? m->step_graph.launch(s_) : enqueue_decode_step(m, rows, T, S_max, fold, eos, log_probs, max_steps, s_);
     }, steps_done);
 }
 
@@ -1009,12 +1039,13 @@ static int run_decode_teacher(AsrModel* m, const int* tokens, int n, int S, int 
     const int d = c.d_model, M = n * T, S_max = m->ws_steps + 1;
     SBK_REQUIRE(m->wt->has_dec, "decode: this handle was created without decoder weights");
     SBK_REQUIRE(S <= m->ws_steps && S <= c.max_len, "decode: %d target positions exceed the workspace / max_len", S);
-    RC(project_cross_kv(m, M, T, st));
+    const bool fold = xatt_fold(m, n, T);
+    RC(project_cross_kv(m, M, T, fold, st));
     set_step_pdl(m, n, d);
     for (int s = 0; s < S; ++s) {
         dec_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, S, s, m->wt->emb, m->wt->dec_pe, d, sqrtf((float)d), b.dx, b.step);
         SBK_LAUNCH_CHECK();
-        RC(enqueue_decode_layers(m, n, 1, T, S_max, nullptr, st, false));
+        RC(enqueue_decode_layers(m, n, 1, T, S_max, nullptr, fold, st, false));
         RC(layernorm_rows(b.dx, b.lnout, false, m->wt->dec_norm_g, m->wt->dec_norm_b, n, d, 1e-6f, false, st));
         SBK_CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s * d, (size_t)S * d * 4, b.lnout, (size_t)d * 4, (size_t)d * 4, n,
                                          cudaMemcpyDeviceToDevice, st));

@@ -220,6 +220,16 @@ struct DecAttnArgs {
     const int* tok_cache; int pad_tok;   // LM pad mask: keys whose token (tok_cache[phys_row][pos]) == pad_tok are masked
 };
 int dec_attention(const DecAttnArgs& a, int n_rows, int max_keys, cudaStream_t stream);
+// Cross-attention of one query row per utterance over the fp16 encoder states e [n_utt][T][D] with folded weights:
+// q [n_utt, ldq] holds the H folded queries W_k,h^T q_h (D each), out [n_utt, ldo] gets the H context vectors
+// sum_t p_t e_t (D each).  D = 512 with H <= 8, or D = 256 with H <= 4.
+struct XattFoldArgs {
+    const __half* q; int ldq;
+    const __half* e; const int* enc_len; int T;
+    int H, D;
+    __half* out; int ldo;
+};
+int dec_xatt_fold(const XattFoldArgs& a, int n_utt, cudaStream_t stream);
 struct BeamLm {  // TransformerLM scorer state the beam step feeds (all null/0 when there is no LM)
     const float* emb = nullptr; const float* pe = nullptr; int d = 0;
     float* x = nullptr; __half* x16 = nullptr; int* tok_cache = nullptr;

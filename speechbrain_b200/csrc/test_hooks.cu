@@ -204,6 +204,47 @@ int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, co
     return finish_test("dec_attention_test", dec_attention(t, rows, max_keys, st), st);
 }
 
+int sbk_xatt_fold_test(const void* h16_dev, const float* in_proj_w, const float* in_proj_b, const float* out_w,
+                       const float* out_b, const void* enc16_dev, const int* enc_len_dev, int rows, int T, int H, int d,
+                       float* x_dev, int ldx, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(h16_dev && in_proj_w && in_proj_b && out_w && out_b && enc16_dev && enc_len_dev && x_dev,
+                "xatt_fold_test: null pointer");
+    SBK_REQUIRE(rows >= 1 && T >= 1 && H >= 1 && d == 64 * H && (d == 256 || d == 512) && ldx >= d,
+                "xatt_fold_test: bad sizes rows=%d T=%d H=%d d=%d ldx=%d", rows, T, H, d, ldx);
+    std::vector<int> len(rows);  // the kernel indexes frames with these: check them on the host first
+    SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), enc_len_dev, rows * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int v : len) SBK_REQUIRE(v >= 0 && v <= T, "xatt_fold_test: enc_len %d outside [0, %d]", v, T);
+    std::vector<double> xq, bxq, xo, bxo;
+    fold_cross_attention(in_proj_w, in_proj_b, out_w, out_b, d, H, &xq, &bxq, &xo, &bxo);
+    std::vector<__half> wq16(xq.size()), wo16(xo.size());
+    for (size_t i = 0; i < xq.size(); ++i) wq16[i] = __double2half(xq[i]);
+    for (size_t i = 0; i < xo.size(); ++i) wo16[i] = __double2half(xo[i]);
+    const std::vector<float> bq32(bxq.begin(), bxq.end()), bo32(bxo.begin(), bxo.end());
+    const int Hd = H * d;
+    __half *wq = nullptr, *wo = nullptr, *q = nullptr, *ctx = nullptr;
+    float *bq = nullptr, *bo = nullptr;
+    TestScratch scr;
+    RC(scr.carve("xatt_fold_test", [&](Carver& take) {
+        take(wq, wq16.size() * 2); take(wo, wo16.size() * 2); take(bq, (size_t)Hd * 4); take(bo, (size_t)d * 4);
+        take(q, (size_t)rows * Hd * 2); take(ctx, (size_t)rows * Hd * 2);
+    }));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(wq, wq16.data(), wq16.size() * 2, cudaMemcpyHostToDevice, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(wo, wo16.data(), wo16.size() * 2, cudaMemcpyHostToDevice, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(bq, bq32.data(), (size_t)Hd * 4, cudaMemcpyHostToDevice, st));
+    SBK_CUDA_CHECK(cudaMemcpyAsync(bo, bo32.data(), (size_t)d * 4, cudaMemcpyHostToDevice, st));
+    GemmEpilogue eq;
+    eq.mode = EPI_F16; eq.bias = bq; eq.out = q; eq.ldo = Hd;
+    int rc = gemm_f16_small(h16_dev, d, wq, d, eq, rows, Hd, d, st);
+    XattFoldArgs x{q, Hd, static_cast<const __half*>(enc16_dev), enc_len_dev, T, H, d, ctx, Hd};
+    if (rc == SBK_OK) rc = dec_xatt_fold(x, rows, st);
+    GemmEpilogue eo;
+    eo.mode = EPI_RESID; eo.bias = bo; eo.out = x_dev; eo.resid = x_dev; eo.ldo = ldx;
+    if (rc == SBK_OK) rc = gemm_f16_small(ctx, Hd, wo, Hd, eo, rows, d, Hd, st);
+    return finish_test("xatt_fold_test", rc, st);
+}
+
 int sbk_stream_qkv_test(const float* qkv_dev, int B, int n, int H, int head_dim, const float* inv_freq_dev, long long pos0,
                         float q_scale, void* q_out_dev, void* kv_out_dev, int cap, int slot0, void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
