@@ -32,7 +32,7 @@ typedef struct {
 typedef struct {
     /* Fbank (lobes/features.py:98-145) -- sizes in samples */
     int n_fft, hop, n_mels;
-    /* ConvolutionFrontEnd (lobes/models/convolution.py:162-203): 2 blocks, 3x3, stride 2 (or 3 blocks, see cnn_blocks) */
+    /* ConvolutionFrontEnd (lobes/models/convolution.py:162-203): 2 blocks, 3x3, stride 2 (or 3 blocks), see cnn_blocks */
     int cnn_c1, cnn_c2;
     /* TransformerASR (lobes/models/transformer/TransformerASR.py:247-325) */
     int input_size, d_model, nhead, num_encoder_layers, num_decoder_layers, d_ffn, vocab, kernel_size;
@@ -55,8 +55,9 @@ typedef struct {
        (TransformerEncoderLayer, Transformer.py:311-490: pre-norm, regularMHA, Linear + GELU + Linear, the absolute sine table
        added to the input Linear's output) */
     int encoder_module, csgu_linear_units, branchformer_activation;
-    /* ConvolutionFrontEnd blocks: 0 or 2 = the Conformer recipes' 2 x (3x3, stride 2), channels (cnn_c1, cnn_c2) = (64, 32);
-       3 = the Transformer recipes' (5x5, stride 2), (5x5, stride 2), (1x1 + residual 1x1), 64 channels each */
+    /* ConvolutionFrontEnd blocks: 0 or 2 = 2 x (3x3, stride 2) with channels (cnn_c1, cnn_c2) = (64, 32) (the Conformer
+       recipes') or (256, 256) (AISHELL-1's Transformer, up to 80 mels); 3 = the LibriSpeech Transformer recipes' (5x5,
+       stride 2), (5x5, stride 2), (1x1 + residual 1x1), 64 channels each; any other pair is refused */
     int cnn_blocks;
     /* The Conformer encoder's conformer_activation (Conformer.py: both FFN modules and the convolution module after its
        LayerNorm): SBK_CONFORMER_ACT_SWISH (0, so a zeroed config stays Swish) or SBK_CONFORMER_ACT_GELU (torch.nn.GELU,

@@ -144,6 +144,20 @@ static std::vector<float> conv_taps_channel_last(const float* src, int Co, int C
     return dst;
 }
 
+// Conv2d weight (o, ch, kf, kt), 3 x 3 taps -> the K-major operand [Co][(kf * 3 + kt) * Ci + ch] as 64-wide k-blocks,
+// each the 128B-swizzled shared-memory image the 256-channel conv2 kernel copies into one stage: block kb holds row o
+// (k = 64 kb .. 64 kb + 63) at 128 o bytes, with its 16-byte chunk j at chunk j ^ (o % 8)
+static std::vector<float> conv_taps_kblocks_sw128(const float* src, int Co, int Ci) {
+    const std::vector<float> km = conv_taps_channel_last(src, Co, Ci, 3);
+    const int K = 9 * Ci;
+    std::vector<float> dst(km.size());
+    for (int kb = 0; kb < K / 64; ++kb)
+        for (int o = 0; o < Co; ++o)
+            for (int k = 0; k < 64; ++k)
+                dst[((size_t)kb * Co + o) * 64 + (((k >> 3) ^ (o & 7)) << 3) + (k & 7)] = km[(size_t)o * K + kb * 64 + k];
+    return dst;
+}
+
 // ---- the parts of a model, each in the order its tensors lie in the arena
 
 static void pack_frontend(Packer& p, AsrWeights& W) {
@@ -185,7 +199,8 @@ static void pack_frontend(Packer& p, AsrWeights& W) {
         p.norm(b0 + "norm_0.norm", (int64_t)F1 * c.cnn_c1, &W.c1_g, &W.c1_be);
         const float* w2 = p.host(b1 + "conv_0.conv.weight", (int64_t)c.cnn_c2 * c.cnn_c1 * 9);
         if (!w2) return;
-        W.c2_w = p.f16_raw(conv_taps_channel_last(w2, c.cnn_c2, c.cnn_c1, 3));
+        W.c2_w = p.f16_raw(c.cnn_c1 == 256 ? conv_taps_kblocks_sw128(w2, c.cnn_c2, c.cnn_c1)
+                                           : conv_taps_channel_last(w2, c.cnn_c2, c.cnn_c1, 3));
         W.c2_b = p.f32(b1 + "conv_0.conv.bias", c.cnn_c2);
         p.norm(b1 + "norm_0.norm", (int64_t)F2 * c.cnn_c2, &W.c2_g, &W.c2_be);
     }
@@ -450,8 +465,11 @@ static int check_config(const sbk_asr_config& c) {
     SBK_REQUIRE(tfm || hypermix || dh == 64 || dh == 36 || dh == 32 ||
                     (dh == 80 && c.encoder_module == SBK_ENC_CONFORMER && c.attention_type == SBK_ATT_RELPOS),
                 "asr_create: encoder head_dim=%d not built (64, 36, 32; 80 for the Conformer with RelPosMHAXL)", dh);
-    SBK_REQUIRE(c.cnn_blocks == 0 || c.cnn_blocks == 2 || (c.cnn_blocks == 3 && c.cnn_c1 == 64 && c.cnn_c2 == 64),
-                "asr_create: cnn_blocks=%d with channels (%d, %d) not built (2, or 3 with 64 channels)", c.cnn_blocks, c.cnn_c1, c.cnn_c2);
+    SBK_REQUIRE(((c.cnn_blocks == 0 || c.cnn_blocks == 2) &&
+                 ((c.cnn_c1 == 64 && c.cnn_c2 == 32) || (c.cnn_c1 == 256 && c.cnn_c2 == 256))) ||
+                    (c.cnn_blocks == 3 && c.cnn_c1 == 64 && c.cnn_c2 == 64),
+                "asr_create: cnn_blocks=%d with channels (%d, %d) not built (2 blocks with (64, 32) or (256, 256), 3 with "
+                "(64, 64))", c.cnn_blocks, c.cnn_c1, c.cnn_c2);
     SBK_REQUIRE(!hypermix || (c.encoder_module == SBK_ENC_CONFORMER && (dh == 32 || dh == 64) && F % c.nhead == 0 &&
                               (F / c.nhead) % 16 == 0 && F / c.nhead <= 256),
                 "asr_create: hypermixing needs the Conformer encoder, a head width d_model / nhead of 32 or 64 and "

@@ -10,6 +10,7 @@
 // conv1 (C_in = 1) is HBM/latency bound: one CTA per output frame, fused LN + LeakyReLU.
 // conv2 (C1 -> C2, K = 9*C1 = 576) is an implicit GEMM on mma.sync.m16n8k16 (fp16 in, fp32 accumulate);
 // the weight matrix and a 9-frame input patch live in shared memory; LN + LeakyReLU fused.
+// out_channels (256, 256) has kernels of its own (conv2 on wgmma), further down; cnn_frontend_forward picks by channels.
 #include <algorithm>
 
 #include "common.cuh"
@@ -378,10 +379,290 @@ cnn_fused_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1
     }
 }
 
+// =========================================================================== 256-channel 2-block front-end (AISHELL-1)
+// ConvolutionFrontEnd(num_blocks=2, out_channels=(256, 256)), otherwise the blocks above:
+//   conv1 (1 -> 256): one CTA per output frame, LayerNorm over (F1, 256) with block reductions -> act1 [B, T1, F1, 256] fp16
+//   conv2 (256 -> 256): implicit GEMM, M = B * T2 * F2 pixels, N = 256, K = 9 * 256 = 2304 (k = tap * 256 + ch), on wgmma.
+// conv2's weights (1.18 MB) cannot stay in shared memory: they stream through a ring of 64-wide k-blocks, each one bulk
+// copy of an image packed at load time in the 128B-swizzled layout wgmma reads.  The A rows are gathered from act1 by a
+// producer warp with cp.async (TMA cannot reflect at the time and feature edges).  A CTA owns W2_BM = 128 GEMM rows =
+// the 128 / F2 whole frames they hold (6 at 80 mels, 120 rows), so the epilogue normalises each frame from the fp32
+// accumulator tile in shared memory: bias, LayerNorm over (F2, 256) and LeakyReLU, with no second pass over HBM.
+constexpr int W1_THREADS = 128;            // conv1: two channels per thread
+constexpr int W_C = 256;                   // channels of both blocks
+constexpr int W2_BK = 64;                  // k-block: 64 input channels of one tap
+constexpr int W2_KB = 9 * W_C / W2_BK;     // 36 k-blocks
+constexpr int W2_BM = 128;                 // GEMM rows per CTA: two consumer warpgroups of 64
+constexpr int W2_STAGES = 4;
+constexpr int W2_LAG = 2;                  // k-blocks of A rows the producer keeps in flight before it marks one full
+constexpr int W2_A_BYTES = W2_BM * W2_BK * 2;
+constexpr int W2_B_BYTES = W_C * W2_BK * 2;
+constexpr int W2_STAGE_BYTES = W2_A_BYTES + W2_B_BYTES;
+constexpr int W2_BAR_OFFSET = W2_STAGES * W2_STAGE_BYTES;
+constexpr int W2_SMEM = W2_BAR_OFFSET + 2 * W2_STAGES * 8 + 1024;  // + alignment slack
+constexpr int W2_STG_PITCH = W_C * 4 + 16;  // fp32 accumulator row in the epilogue
+constexpr int W2_CONSUMERS = 2 * 128;
+constexpr int W2_THREADS = W2_CONSUMERS + 32;
+static_assert(W2_STAGE_BYTES % 1024 == 0 && W2_BM * W2_STG_PITCH <= W2_BAR_OFFSET, "ring layout");
+static_assert(W2_LAG <= W2_STAGES - 2, "the producer must mark stage kb full before it waits for stage kb + 2 to drain");
+
+// w1: [256, 3(kf), 3(kt)] fp32, g/be: [F1, 256].  Same arithmetic per value as conv1_ln_kernel.
+template <int MAXF>
+__global__ void __launch_bounds__(W1_THREADS)
+conv1c256_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1, const float* __restrict__ w1,
+                    const float* __restrict__ b1, const float* __restrict__ gamma, const float* __restrict__ beta,
+                    __half* __restrict__ out_h) {
+    extern __shared__ float w1_in[];  // [3][F0 + 2] of the frame (reflect padded)
+    __shared__ float red[2][W1_THREADS / 32];
+    const int FP = F0 + 2;
+    const int t1 = blockIdx.x, b = blockIdx.y;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < 3 * FP; i += W1_THREADS) {
+        const int kt = i / FP, fp = i - kt * FP;
+        const int t = reflect_idx(2 * t1 + kt - 1, T0);
+        const int f = reflect_idx(fp - 1, F0);
+        w1_in[i] = __ldg(feats + (static_cast<size_t>(b) * T0 + t) * F0 + f);
+    }
+    const int c0 = 2 * threadIdx.x;
+    float wa[9], wb[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) { wa[i] = __ldg(w1 + c0 * 9 + i); wb[i] = __ldg(w1 + (c0 + 1) * 9 + i); }
+    const float ba = __ldg(b1 + c0), bb = __ldg(b1 + c0 + 1);
+    __syncthreads();
+    float va[MAXF], vb[MAXF];
+    float s = 0.0f;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1) {
+        va[f1] = 0.0f; vb[f1] = 0.0f;
+        if (f1 < F1) {
+            float a = ba, bq = bb;
+#pragma unroll
+            for (int kf = 0; kf < 3; ++kf)
+#pragma unroll
+                for (int kt = 0; kt < 3; ++kt) {
+                    const float x = w1_in[kt * FP + 2 * f1 + kf];
+                    a = fmaf(wa[kf * 3 + kt], x, a);
+                    bq = fmaf(wb[kf * 3 + kt], x, bq);
+                }
+            va[f1] = a; vb[f1] = bq;
+            s += a + bq;
+        }
+    }
+    const float n = static_cast<float>(F1 * W_C);
+    s = warp_sum(s);
+    if (lane == 0) red[0][warp] = s;
+    __syncthreads();
+    const float mean = (red[0][0] + red[0][1] + red[0][2] + red[0][3]) / n;
+    float q = 0.0f;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1)
+        if (f1 < F1) {
+            const float da = va[f1] - mean, db = vb[f1] - mean;
+            q += da * da + db * db;
+        }
+    q = warp_sum(q);
+    if (lane == 0) red[1][warp] = q;
+    __syncthreads();
+    const float rstd = rsqrtf((red[1][0] + red[1][1] + red[1][2] + red[1][3]) / n + 1e-5f);
+    const size_t obase = (static_cast<size_t>(b) * T1 + t1) * F1 * W_C;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1)
+        if (f1 < F1) {
+            const int gi = f1 * W_C + c0;
+            const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + gi));
+            const float2 be = __ldg(reinterpret_cast<const float2*>(beta + gi));
+            const float y0 = leaky((va[f1] - mean) * rstd * g.x + be.x);
+            const float y1 = leaky((vb[f1] - mean) * rstd * g.y + be.y);
+            *reinterpret_cast<__half2*>(out_h + obase + gi) = floats2half2_sat(y0, y1);
+        }
+}
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// generic-proxy writes to shared memory (cp.async, st.shared) made visible to the async proxy wgmma reads through
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// act1 [B, T1, F1, 256] fp16; w2s: W2_KB k-blocks of [256 out][64 k] fp16, each the 128B-swizzled image a stage holds
+// (k = (kf * 3 + kt) * 256 + ch); frames = W2_BM / F2 output frames per CTA; out [B, T2, F2 * 256].
+__global__ void __launch_bounds__(W2_THREADS, 1)
+conv2c256_ln_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int F2, int frames,
+                    const __half* __restrict__ w2s, const float* __restrict__ b2, const float* __restrict__ gamma,
+                    const float* __restrict__ beta, __half* __restrict__ out_h, float* __restrict__ out_f) {
+    extern __shared__ uint8_t w2_smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w2_smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + W2_BAR_OFFSET);
+    uint64_t* empty_bar = full_bar + W2_STAGES;
+    const int b = blockIdx.y, t0 = blockIdx.x * frames, rows = frames * F2;
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < W2_STAGES; ++s) {
+            mbar_init(&full_bar[s], 1 + 32);  // the weight copy's expect_tx arrive + one arrive per producer lane
+            mbar_init(&empty_bar[s], 2);      // one arrive per consumer warpgroup
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= W2_CONSUMERS) {
+        // ---- producer warp: lane l gathers GEMM rows l, l + 32, l + 64, l + 96 (8 x 16-byte chunks each per k-block)
+        int t2r[W2_BM / 32], f2r[W2_BM / 32];
+#pragma unroll
+        for (int j = 0; j < W2_BM / 32; ++j) {
+            const int r = lane + 32 * j, fr = r / F2;
+            t2r[j] = min(t0 + fr, T2 - 1);  // tail frames: keep loads in range (results discarded)
+            f2r[j] = r - fr * F2;
+        }
+        const __half* act1_b = act1 + static_cast<size_t>(b) * T1 * F1 * W_C;
+        for (int kb = 0; kb < W2_KB; ++kb) {
+            const int s = kb % W2_STAGES;
+            if (kb >= W2_STAGES) mbar_wait(&empty_bar[s], ((kb / W2_STAGES) & 1) ^ 1);
+            uint8_t* stage = smem + s * W2_STAGE_BYTES;
+            if (lane == 0) {
+                mbar_arrive_expect_tx(&full_bar[s], W2_B_BYTES);
+                bulk_load_1d(stage + W2_A_BYTES, w2s + static_cast<size_t>(kb) * W_C * W2_BK, W2_B_BYTES, &full_bar[s]);
+            }
+            const int tap = kb / (W_C / W2_BK), kf = tap / 3, kt = tap - 3 * kf;
+            const int ch0 = (kb - tap * (W_C / W2_BK)) * W2_BK;
+            const uint32_t a_base = smem_u32(stage);
+#pragma unroll
+            for (int j = 0; j < W2_BM / 32; ++j) {
+                const int r = lane + 32 * j;
+                if (r < rows) {  // rows past the last whole frame stay unwritten: their outputs are never read
+                    const int t1 = reflect_idx(2 * t2r[j] + kt - 1, T1), f1 = reflect_idx(2 * f2r[j] + kf - 1, F1);
+                    const __half* src = act1_b + (static_cast<size_t>(t1) * F1 + f1) * W_C + ch0;
+                    const uint32_t dst = a_base + r * 128;
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) cp_async16(dst + ((c ^ (r & 7)) << 4), src + c * 8);
+                }
+            }
+            cp_async_commit();
+            if (kb >= W2_LAG) {
+                cp_async_wait<W2_LAG>();
+                fence_proxy_async_smem();
+                mbar_arrive(&full_bar[(kb - W2_LAG) % W2_STAGES]);
+            }
+        }
+        cp_async_wait<0>();
+        fence_proxy_async_smem();
+        for (int kb = W2_KB - W2_LAG; kb < W2_KB; ++kb) mbar_arrive(&full_bar[kb % W2_STAGES]);
+        return;
+    }
+
+    // ---- consumers: warpgroup g computes rows 64 g .. 64 g + 63 x all 256 columns (two n128 wgmma per k16 step)
+    const int wg = threadIdx.x >> 7;
+    float acc[2][64];
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 64; ++j) acc[i][j] = 0.0f;
+    for (int kb = 0; kb < W2_KB; ++kb) {
+        const int s = kb % W2_STAGES;
+        mbar_wait(&full_bar[s], (kb / W2_STAGES) & 1);
+        const uint32_t a_addr = smem_u32(smem + s * W2_STAGE_BYTES) + wg * 64 * 128;
+        const uint32_t b_addr = smem_u32(smem + s * W2_STAGE_BYTES) + W2_A_BYTES;
+        const uint64_t da = make_kmajor_sw128_desc(a_addr);
+        const uint64_t db0 = make_kmajor_sw128_desc(b_addr), db1 = make_kmajor_sw128_desc(b_addr + 128 * 128);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < W2_BK / 16; ++k) {  // +32 B per k16 step -> +2 in (addr >> 4)
+            wgmma_f16<128>(acc[0], da + 2 * k, db0 + 2 * k, 1u);
+            wgmma_f16<128>(acc[1], da + 2 * k, db1 + 2 * k, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(kb - 1) % W2_STAGES]);
+    }
+    wgmma_wait<0>();
+    asm volatile("bar.sync 1, %0;" ::"n"(W2_CONSUMERS) : "memory");  // both warpgroups are done reading the ring
+    {
+        const int w = (threadIdx.x >> 5) & 3;
+        uint8_t* base = smem + (wg * 64 + w * 16 + (lane >> 2)) * W2_STG_PITCH + (lane & 3) * 8;
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int col = i * 128 + j * 8 + 2 * (lane & 3);
+                const float bz0 = __ldg(b2 + col), bz1 = __ldg(b2 + col + 1);
+                *reinterpret_cast<float2*>(base + (i * 128 + j * 8) * 4) =
+                    make_float2(acc[i][4 * j] + bz0, acc[i][4 * j + 1] + bz1);
+                *reinterpret_cast<float2*>(base + 8 * W2_STG_PITCH + (i * 128 + j * 8) * 4) =
+                    make_float2(acc[i][4 * j + 2] + bz0, acc[i][4 * j + 3] + bz1);
+            }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(W2_CONSUMERS) : "memory");
+    // LayerNorm over (F2, 256) per frame + LeakyReLU; one warp per frame, lane l owns columns 4 l .. 4 l + 3 and 128 + 4 l ..
+    const int warp = threadIdx.x >> 5;
+    const int n = F2 * W_C;
+    const uint32_t stg = smem_u32(smem);
+    for (int fr = warp; fr < frames; fr += W2_CONSUMERS / 32) {
+        const int t = t0 + fr;
+        if (t >= T2) break;
+        const uint32_t fbase = stg + fr * F2 * W2_STG_PITCH + lane * 16;
+        float s = 0.0f;
+        for (int r = 0; r < F2; ++r)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float4 v = u4_as_f4(lds128(fbase + r * W2_STG_PITCH + h * 512));
+                s += (v.x + v.y) + (v.z + v.w);
+            }
+        const float mean = warp_sum(s) / n;
+        float q = 0.0f;
+        for (int r = 0; r < F2; ++r)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float4 v = u4_as_f4(lds128(fbase + r * W2_STG_PITCH + h * 512));
+                const float d0 = v.x - mean, d1 = v.y - mean, d2 = v.z - mean, d3 = v.w - mean;
+                q += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
+            }
+        const float rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
+        const size_t ob = (static_cast<size_t>(b) * T2 + t) * n;
+        for (int r = 0; r < F2; ++r)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int i = r * W_C + h * 128 + 4 * lane;
+                const float4 v = u4_as_f4(lds128(fbase + r * W2_STG_PITCH + h * 512));
+                const float4 g = __ldg(reinterpret_cast<const float4*>(gamma + i));
+                const float4 be = __ldg(reinterpret_cast<const float4*>(beta + i));
+                const float4 y = make_float4(leaky((v.x - mean) * rstd * g.x + be.x), leaky((v.y - mean) * rstd * g.y + be.y),
+                                             leaky((v.z - mean) * rstd * g.z + be.z), leaky((v.w - mean) * rstd * g.w + be.w));
+                const __half2 lo = floats2half2_sat(y.x, y.y), hi = floats2half2_sat(y.z, y.w);
+                *reinterpret_cast<uint2*>(out_h + ob + i) =
+                    make_uint2(*reinterpret_cast<const uint32_t*>(&lo), *reinterpret_cast<const uint32_t*>(&hi));
+                if (out_f) *reinterpret_cast<float4*>(out_f + ob + i) = y;
+            }
+    }
+}
+
+static int cnn256_frontend_forward(const float* feats, int B, int T0, int F0, const float* w1, const float* b1,
+                                   const float* g1, const float* be1, const __half* w2s, const float* b2, const float* g2,
+                                   const float* be2, __half* act1_h, __half* out_h, float* out_f, cudaStream_t stream) {
+    // the reference's reflect padding of 1 needs 2 rows / columns at both strided convolutions
+    SBK_REQUIRE(T0 >= 3 && F0 >= 3, "cnn_frontend: the 3x3 reflect padding needs at least 3 frames and 3 features "
+                "(got %d frames, %d features)", T0, F0);
+    const int T1 = (T0 - 1) / 2 + 1, F1 = (F0 - 1) / 2 + 1;
+    const int T2 = (T1 - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
+    SBK_REQUIRE(F1 <= 40, "cnn_frontend: out_channels=(256, 256) is built for up to 80 features (F0=%d)", F0);
+    conv1c256_ln_kernel<40><<<dim3(T1, B), W1_THREADS, 3 * (F0 + 2) * sizeof(float), stream>>>(
+        feats, T0, F0, T1, F1, w1, b1, g1, be1, act1_h);
+    SBK_LAUNCH_CHECK();
+    const int frames = W2_BM / F2;
+    SBK_CUDA_CHECK(cudaFuncSetAttribute(conv2c256_ln_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM));
+    conv2c256_ln_kernel<<<dim3(ceil_div(T2, frames), B), W2_THREADS, W2_SMEM, stream>>>(
+        act1_h, T1, F1, T2, F2, frames, w2s, b2, g2, be2, out_h, out_f);
+    SBK_LAUNCH_CHECK();
+    return SBK_OK;
+}
+
 int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float* w1, const float* b1, const float* g1,
                          const float* be1, int C1, const __half* w2p, const float* b2, const float* g2,
                          const float* be2, int C2, __half* act1_h, __half* out_h, float* out_f, cudaStream_t stream) {
-    SBK_REQUIRE(C1 == 64 && C2 == 32, "cnn_frontend: only out_channels=(64, 32) is built (got %d, %d)", C1, C2);
+    if (C1 == W_C && C2 == W_C)
+        return cnn256_frontend_forward(feats, B, T0, F0, w1, b1, g1, be1, w2p, b2, g2, be2, act1_h, out_h, out_f, stream);
+    SBK_REQUIRE(C1 == 64 && C2 == 32, "cnn_frontend: only out_channels=(64, 32) and (256, 256) are built (got %d, %d)", C1, C2);
     SBK_REQUIRE(T0 >= 2 && F0 >= 2, "cnn_frontend: input too small for reflect padding");
     const int T1 = (T0 - 1) / 2 + 1, F1 = (F0 - 1) / 2 + 1;
     const int T2 = (T1 - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;

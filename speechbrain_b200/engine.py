@@ -75,7 +75,7 @@ class AsrEngine:
     ("RoPEMHA"|"RelPosMHAXL"|"hypermixing"|"regularMHA", hypermixing with the Conformer only, regularMHA with the Transformer
     only), decoder_activation ("gelu"|"relu"|"swish"), max_length; encoder_module ("conformer" (default) | "branchformer" |
     "transformer") with csgu_linear_units and branchformer_activation ("gelu" (default) | "relu"); cnn_blocks (2 (default),
-    or 3: the Transformer recipes' front-end, cnn_channels (64, 64)); conformer_activation ("swish" (default) | "gelu": the
+    with cnn_channels (64, 32) or (256, 256), or 3: the LibriSpeech Transformer recipes' front-end, cnn_channels (64, 64)); conformer_activation ("swish" (default) | "gelu": the
     Conformer's FFN and convolution-module activation).
     ``state``: {reference key with recipe prefix: CPU fp32 tensor}."""
 

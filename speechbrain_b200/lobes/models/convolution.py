@@ -1,7 +1,7 @@
 """ConvolutionFrontEnd -- drop-in for speechbrain.lobes.models.convolution.ConvolutionFrontEnd
 (lobes/models/convolution.py:116-320) for the two configurations the recipes use:
 - the Conformer recipes': 2 blocks x 1 Conv2d(3x3, stride 2, reflect 'same' padding) + LayerNorm + LeakyReLU, no residuals,
-  out_channels (64, 32);
+  out_channels (64, 32), and the AISHELL-1 Transformer recipe's, the same blocks with out_channels (256, 256);
 - the Transformer recipes': 3 blocks x 1 layer, out_channels (64, 64, 64), kernel_sizes (5, 5, 1), strides (2, 2, 1),
   residuals (False, False, True): the third block adds a 1x1 Conv2d + LayerNorm (reduce_conv) of its input.
 Same constructor and state_dict keys; other configurations raise (no CPU fallback)."""
@@ -21,14 +21,16 @@ class ConvolutionFrontEnd(torch.nn.Module):
         common = (num_layers_per_block == 1 and conv_module is None and activation is torch.nn.LeakyReLU
                   and norm == "LayerNorm" and conv_bias and padding == "same")
         conformer = (common and num_blocks == 2 and tuple(kernel_sizes[:2]) == (3, 3) and tuple(strides[:2]) == (2, 2)
-                     and not any(residuals[:2]) and tuple(dilations[:2]) == (1, 1) and tuple(out_channels[:2]) == (64, 32))
+                     and not any(residuals[:2]) and tuple(dilations[:2]) == (1, 1)
+                     and tuple(out_channels[:2]) in ((64, 32), (256, 256)))
         transformer = (common and num_blocks == 3 and tuple(kernel_sizes[:3]) == (5, 5, 1)
                        and tuple(strides[:3]) == (2, 2, 1) and tuple(bool(r) for r in residuals[:3]) == (False, False, True)
                        and tuple(dilations[:3]) == (1, 1, 1) and tuple(out_channels[:3]) == (64, 64, 64))
         if not (conformer or transformer):
             raise NotImplementedError(
                 "speechbrain_b200.ConvolutionFrontEnd: only the Conformer recipes' front-end (num_blocks=2, "
-                "num_layers_per_block=1, out_channels=(64, 32), 3x3, stride 2, no residuals) and the Transformer recipes' "
+                "num_layers_per_block=1, out_channels=(64, 32), 3x3, stride 2, no residuals), the same with "
+                "out_channels=(256, 256) (AISHELL-1's Transformer) and the LibriSpeech Transformer recipes' "
                 "(num_blocks=3, num_layers_per_block=1, out_channels=(64, 64, 64), kernel_sizes=(5, 5, 1), strides=(2, 2, 1), "
                 "residuals=(False, False, True)) are built")
         self.n_mels = int(input_shape[-1])

@@ -144,10 +144,13 @@ class TransformerASR(torch.nn.Module):
         object.__setattr__(self, "_slots", {})
 
     def engine_cfg(self):
-        # the front-end each encoder's recipes pair it with: the 3-block one for the Transformer, else the 2-block one
+        # the front-end each encoder's recipes pair it with: for the Transformer the LibriSpeech recipes' 3-block one, or
+        # AISHELL-1's 2-block one with 256 channels (20 x 256 = 5120 features at 80 mels); else the 2-block (64, 32) one
         tfm = self.encoder_module == "transformer"
-        return dict(n_fft=400, hop=160, win=400, n_mels=80, cnn_channels=(64, 64) if tfm else (64, 32),
-                    cnn_blocks=3 if tfm else 2, input_size=self.input_size,
+        cnn3 = tfm and self.input_size != 5120
+        return dict(n_fft=400, hop=160, win=400, n_mels=80,
+                    cnn_channels=(64, 64) if cnn3 else (256, 256) if tfm else (64, 32),
+                    cnn_blocks=3 if cnn3 else 2, input_size=self.input_size,
                     d_model=self.d_model, nhead=self.nhead, num_encoder_layers=self.num_encoder_layers,
                     num_decoder_layers=self.num_decoder_layers, d_ffn=self.d_ffn, vocab=self.tgt_vocab,
                     kernel_size=self.kernel_size, attention_type=self.attention_type,

@@ -134,6 +134,13 @@ TRANSFORMER_LARGE = dict(name="transformer_large", sample_rate=16000, n_fft=400,
                          cnn_channels=(64, 64), cnn_blocks=3, input_size=1280, d_model=512, nhead=4, num_encoder_layers=12,
                          num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="regularMHA",
                          decoder_activation="gelu", max_length=2500, encoder_module="transformer")
+# recipes/AISHELL-1/ASR/transformer/hparams/train_ASR_transformer.yaml: the 2-block front-end with 256 channels (input
+# 20 x 256 = 5120), 12 pre-norm Transformer encoder layers with regularMHA (4 heads of 64), 6 decoder layers, 5000 tokens;
+# blank 0, bos 1, eos 2
+AISHELL_TRANSFORMER = dict(name="aishell_transformer", sample_rate=16000, n_fft=400, win=400, hop=160, n_mels=80,
+                           cnn_channels=(256, 256), input_size=5120, d_model=256, nhead=4, num_encoder_layers=12,
+                           num_decoder_layers=6, d_ffn=2048, vocab=5000, kernel_size=31, attention_type="regularMHA",
+                           decoder_activation="gelu", max_length=2500, encoder_module="transformer")
 # recipes/Libriheavy/ASR/transformer/hparams/conformer_large.yaml: 14 Conformer layers at d_model 640 with RelPosMHAXL (8 heads
 # of 80), 6 GELU decoder layers, 5000 tokens; and recipes/PeoplesSpeech/ASR/transformer/hparams/conformer_large.yaml: the same
 # encoder, 6 decoder layers with a Swish FFN, 5120 tokens
