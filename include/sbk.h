@@ -43,7 +43,10 @@ typedef struct {
     int decoder_activation; /* SBK_ACT_RELU | SBK_ACT_GELU | SBK_ACT_SILU (the `activation` ctor kwarg) */
     int max_len;            /* positional tables (ctor kwarg max_length, default 2500) */
     int parts;              /* bitmask of SBK_PART_*: which sub-models the weight table carries */
-    /* TransformerLM used as a shallow-fusion scorer (lobes/models/transformer/TransformerLM.py; weights "lm.*") */
+    /* TransformerLM used as a shallow-fusion scorer (lobes/models/transformer/TransformerLM.py; weights "lm.*"): head width
+       64 with lm_d_model % 128 == 0, or the Switchboard LM (lm_d_model 264, 12 heads).  With "lm.embedding_proj.w.weight"
+       present (TransformerLM(d_embedding=...)) d_embedding is its numel / lm_d_model and the projection is folded into
+       the embedding table */
     int lm_d_model, lm_nhead, lm_layers, lm_d_ffn, lm_activation;
     /* Filterbank amin / top_db (processing/features.py:437-475) and InputNormalization epsilon (:1360-1455) of the fused
        wav -> features front end; 0 = the reference defaults (1e-10, 80 dB, 1e-10) */
@@ -180,6 +183,13 @@ int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, co
                            int key_stride, int head_stride, int rows_per_block, int rows, int H, int dh, int max_keys, int step,
                            const int* enc_len_dev, const int* lineage_dev, const int* tok_cache_dev, int lin_stride,
                            int pad_tok, void* out_dev, int ldo, void* stream);
+
+/* TransformerLM.forward's causal self-attention alone: qkv_dev [n * s, 3 d] fp16 with columns [q | k | v], H heads of
+ * d / H = 64 or 32 side by side (q pre-scaled), tokens_dev [n, s] int32 (keys whose id == pad_tok are masked, as are keys
+ * after the query) -> out_dev [n * s, d] fp16.  A query with no visible key is NaN, as in the reference.  Synchronises
+ * the stream. */
+int sbk_lm_causal_attention_test(const void* qkv_dev, int n, int s, int d, int H, const int* tokens_dev, int pad_tok,
+                                 void* out_dev, void* stream);
 
 /* the folded cross-attention of a decode step alone (rows = utterances, one query row each): the folded query projection
  * (gemm_f16_small, fp16 out), dec_xatt_fold_kernel, and the folded output projection added to x_dev [rows, ldx] fp32 in

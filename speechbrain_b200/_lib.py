@@ -72,7 +72,7 @@ EXPORTS = [
     "sbk_transducer_create", "sbk_transducer_destroy", "sbk_transducer_info", "sbk_transducer_greedy",
     "sbk_asr_stream_create", "sbk_asr_stream_encode_chunk", "sbk_asr_stream_reset", "sbk_asr_stream_destroy",
     "sbk_asr_stream_context", "sbk_stream_qkv_test", "sbk_step_proj_test", "sbk_dec_attention_test",
-    "sbk_beam_step_test", "sbk_coverage_score_test", "sbk_xatt_fold_test",
+    "sbk_beam_step_test", "sbk_coverage_score_test", "sbk_xatt_fold_test", "sbk_lm_causal_attention_test",
 ]
 
 

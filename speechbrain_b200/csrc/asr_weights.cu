@@ -26,6 +26,7 @@ struct Packer {
     bool ok = true;
     std::vector<__half> tmph;
     bool has(const std::string& k) const { return w.count(k) != 0; }
+    int64_t numel(const std::string& k) const { return has(k) ? w.at(k).second : 0; }
     // the host tensor itself, for a repack (null, with ok cleared and the error set, when it is missing or mis-sized)
     const float* host(const std::string& k, int64_t n) {
         auto it = w.find(k);
@@ -413,11 +414,84 @@ static void pack_decoder(Packer& p, AsrWeights& W) {
     if (p.has("seq_lin.w.weight")) p.linear("seq_lin.w", c.vocab, d, &W.w_lin, &W.b_lin);
 }
 
+bool lm_widths(int d, int H, int* dp, int* dhp) {
+    if (H > 0 && d == 64 * H && d % 128 == 0) { *dp = d; *dhp = 64; return true; }
+    if (d == 264 && H == 12) { *dp = 272; *dhp = 32; return true; }
+    return false;
+}
+
+// A [rows.size(), cols.size()] copy of the row-major matrix src (`ld` columns): element (i, j) = src[rows[i]][cols[j]], zero
+// where either index is -1.  Places a TransformerLM weight in its padded layout.
+static std::vector<float> gather2d(const float* src, int ld, const std::vector<int>& rows, const std::vector<int>& cols) {
+    std::vector<float> dst(rows.size() * cols.size(), 0.0f);
+    for (size_t i = 0; i < rows.size(); ++i)
+        if (rows[i] >= 0)
+            for (size_t j = 0; j < cols.size(); ++j)
+                if (cols[j] >= 0) dst[i * cols.size() + j] = src[(size_t)rows[i] * ld + cols[j]];
+    return dst;
+}
+
 static void pack_lm(Packer& p, AsrWeights& W) {
     const sbk_asr_config& c = W.cfg;
-    const int dl = c.lm_d_model, Fl = c.lm_d_ffn, dhl = dl / c.lm_nhead;
-    W.lm_emb = p.f32("lm.custom_src_module.emb.Embedding.weight", (int64_t)c.vocab * dl);
-    W.lm_pe = p.f32_raw(sine_table(c.max_len, dl));
+    const int dl = c.lm_d_model, Fl = c.lm_d_ffn, H = c.lm_nhead, dhl = dl / H, V = c.vocab;
+    int dp = 0, dhp = 0;
+    lm_widths(dl, H, &dp, &dhp);  // check_config has refused every other shape
+    W.lm_dp = dp; W.lm_dhp = dhp; W.lm_da = H * dhp;
+    // index maps into the reference's tensors: the residual stream (dp channels, the first dl real), the attention width
+    // (da channels, head h's first dhl real), the in_proj's [q | k | v] rows, and the identity over the FFN / vocabulary
+    std::vector<int> res(dp, -1), att(W.lm_da, -1), qkv(3 * W.lm_da, -1), ffn(Fl), voc(V), one{0};
+    for (int i = 0; i < dl; ++i) res[i] = i;
+    for (int h = 0; h < H; ++h)
+        for (int j = 0; j < dhl; ++j) att[h * dhp + j] = h * dhl + j;
+    for (int part = 0; part < 3; ++part)
+        for (int i = 0; i < W.lm_da; ++i) qkv[part * W.lm_da + i] = att[i] < 0 ? -1 : part * dl + att[i];
+    for (int i = 0; i < Fl; ++i) ffn[i] = i;
+    for (int i = 0; i < V; ++i) voc[i] = i;
+    // Linear prefix.weight [out, in] / prefix.bias [out] with their rows picked by `out` and columns by `in`
+    auto linear = [&](const std::string& prefix, const std::vector<int>& out, const std::vector<int>& in, int n_out, int n_in,
+                      const __half** wgt, const float** bias) {
+        const float* w = p.host(prefix + ".weight", (int64_t)n_out * n_in);
+        const float* b = p.host(prefix + ".bias", n_out);
+        if (!w || !b) return;
+        *wgt = p.f16_raw(gather2d(w, n_in, out, in));
+        *bias = p.f32_raw(gather2d(b, 1, out, one));
+    };
+
+    // the embedding table the step kernels read one row of, at pitch dp
+    const std::string proj = "lm.embedding_proj.w";
+    if (p.has(proj + ".weight")) {  // TransformerLM(d_embedding=...): NormalizedEmbedding(d_embedding) -> embedding_proj
+        const int64_t de = p.numel(proj + ".weight") / dl;
+        if (de < 1 || de * dl != p.numel(proj + ".weight")) {
+            set_error("weight '%s.weight' has %lld elements, not a multiple of d_model %d", proj.c_str(),
+                      (long long)p.numel(proj + ".weight"), dl);
+            p.ok = false;
+            return;
+        }
+        const float* E = p.host("lm.custom_src_module.emb.Embedding.weight", (int64_t)V * de);
+        const float* Wp = p.host(proj + ".weight", (int64_t)dl * de);
+        const float* bp = p.host(proj + ".bias", dl);
+        if (!E || !Wp || !bp) return;
+        std::vector<double> table((size_t)V * dp, 0.0);  // embedding_proj(sqrt(d_embedding) E[v]), formed only to upload
+        if (p.carve.base) {
+            const double s = sqrt((double)de);
+            for (int v = 0; v < V; ++v)
+                for (int o = 0; o < dl; ++o) {
+                    double acc = 0.0;
+                    for (int64_t i = 0; i < de; ++i) acc += (double)Wp[(size_t)o * de + i] * (s * E[(size_t)v * de + i]);
+                    table[(size_t)v * dp + o] = acc + bp[o];
+                }
+        }
+        W.lm_emb = p.f32_raw(table);
+        W.lm_emb_scale = 1.0f;
+    } else {
+        const float* emb = p.host("lm.custom_src_module.emb.Embedding.weight", (int64_t)V * dl);
+        if (!emb) return;
+        W.lm_emb = p.f32_raw(gather2d(emb, dl, voc, res));
+        W.lm_emb_scale = sqrtf((float)dl);
+    }
+    std::vector<int> pos(c.max_len);
+    for (int t = 0; t < c.max_len; ++t) pos[t] = t;
+    W.lm_pe = p.f32_raw(gather2d(sine_table(c.max_len, dl).data(), dl, pos, res));
     W.lm.resize(c.lm_layers);
     for (int l = 0; l < c.lm_layers; ++l) {
         const std::string q = "lm.encoder.layers." + std::to_string(l) + ".";
@@ -425,19 +499,20 @@ static void pack_lm(Packer& p, AsrWeights& W) {
         const float* wi = p.host(q + "self_att.att.in_proj_weight", (int64_t)3 * dl * dl);
         const float* bi = p.host(q + "self_att.att.in_proj_bias", 3 * dl);
         if (!wi || !bi) return;
-        e.w_in = p.f16_raw(fold_query_scale(wi, (size_t)3 * dl * dl, (size_t)dl * dl, dhl));
-        e.b_in = p.f32_raw(fold_query_scale(bi, 3 * dl, dl, dhl));
-        p.linear(q + "self_att.att.out_proj", dl, dl, &e.w_out, &e.b_out);
-        p.linear(q + "pos_ffn.ffn.0", Fl, dl, &e.w1, &e.b1);
-        p.linear(q + "pos_ffn.ffn.3", dl, Fl, &e.w2, &e.b2);
+        // 1 / sqrt(dh) of the true head width; the padded query dims are zero
+        e.w_in = p.f16_raw(gather2d(fold_query_scale(wi, (size_t)3 * dl * dl, (size_t)dl * dl, dhl).data(), dl, qkv, res));
+        e.b_in = p.f32_raw(gather2d(fold_query_scale(bi, 3 * dl, dl, dhl).data(), 1, qkv, one));
+        linear(q + "self_att.att.out_proj", res, att, dl, dl, &e.w_out, &e.b_out);
+        linear(q + "pos_ffn.ffn.0", ffn, res, Fl, dl, &e.w1, &e.b1);
+        linear(q + "pos_ffn.ffn.3", res, ffn, dl, Fl, &e.w2, &e.b2);
         p.norm(q + "norm1.norm", dl, &e.n1g, &e.n1b);
         p.norm(q + "norm2.norm", dl, &e.n2g, &e.n2b);
         if (!p.ok) return;
     }
     p.norm("lm.encoder.norm.norm", dl, &W.lm_norm_g, &W.lm_norm_b);
-    p.linear("lm.output_proj.layers.0.w", dl, dl, &W.lm_wp0, &W.lm_bp0);
+    linear("lm.output_proj.layers.0.w", res, res, dl, dl, &W.lm_wp0, &W.lm_bp0);
     p.norm("lm.output_proj.layers.1.norm", dl, &W.lm_lnp_g, &W.lm_lnp_b);
-    p.linear("lm.output_proj.layers.2.w", c.vocab, dl, &W.lm_wp2, &W.lm_bp2);
+    linear("lm.output_proj.layers.2.w", voc, res, V, dl, &W.lm_wp2, &W.lm_bp2);
 }
 
 // Everything that goes into the arena.  Stops at the first part with a missing or mis-sized tensor (p.ok cleared, the
@@ -494,8 +569,10 @@ static int check_config(const sbk_asr_config& c) {
         const int F1 = (c.n_mels - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
         SBK_REQUIRE(F2 * c.cnn_c2 == c.input_size, "asr_create: CNN output %d != input_size %d", F2 * c.cnn_c2, c.input_size);
     }
-    if ((c.parts & SBK_PART_LM) && c.lm_layers > 0 && (c.lm_d_model / c.lm_nhead != 64 || c.lm_d_model % 128 != 0)) {
-        set_error("asr_create: LM head_dim must be 64 and d_model %% 128 == 0");
+    int lm_dp, lm_dhp;
+    if ((c.parts & SBK_PART_LM) && c.lm_layers > 0 && !lm_widths(c.lm_d_model, c.lm_nhead, &lm_dp, &lm_dhp)) {
+        set_error("asr_create: LM d_model=%d with %d heads not built (head_dim 64 with d_model %% 128 == 0, or d_model 264 "
+                  "with 12 heads of 22)", c.lm_d_model, c.lm_nhead);
         return SBK_ERR_UNSUPPORTED;
     }
     return SBK_OK;

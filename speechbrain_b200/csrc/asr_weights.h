@@ -85,7 +85,12 @@ struct AsrWeights {
     const float *dec_norm_g = nullptr, *dec_norm_b = nullptr;
     const __half* w_lin = nullptr; const float* b_lin = nullptr;  // seq_lin, when the state has it
     const __half* w_ctc = nullptr; const float* b_ctc = nullptr;  // ctc_lin, when the state has it
-    // TransformerLM scorer (optional part)
+    // TransformerLM scorer (optional part).  Its kernels see padded widths (lm_widths): the residual stream at pitch lm_dp,
+    // heads of lm_dhp, attention width lm_da = lm_nhead * lm_dhp; the padding channels hold zero weights and stay zero.
+    // lm_emb [vocab, lm_dp] is the raw table (x = lm_emb[tok] * sqrt(d) + pe) or, with a d_embedding projection, the folded
+    // table embedding_proj(sqrt(d_embedding) E[tok]) (lm_emb_scale 1).
+    int lm_dp = 0, lm_dhp = 0, lm_da = 0;
+    float lm_emb_scale = 0.0f;
     const float *lm_emb = nullptr, *lm_pe = nullptr;
     std::vector<LmLayerW> lm;
     const float *lm_norm_g = nullptr, *lm_norm_b = nullptr, *lm_lnp_g = nullptr, *lm_lnp_b = nullptr;
@@ -103,6 +108,11 @@ struct AsrWeights {
 // element count fails before anything is allocated on the device.
 int load_asr_weights(const sbk_asr_config& cfg, const sbk_tensor* weights, int n_weights,
                      std::shared_ptr<const AsrWeights>* out);
+
+// The padded widths of a TransformerLM (d_model d, H heads of dh): head width 64 runs unpadded (dp = d, dhp = 64); the
+// Switchboard LM (d 264, 12 heads of 22) runs at dp = 272 (K % 16 for the skinny GEMM) and dhp = 32 (the k-step of the
+// causal flash kernel).  False for any other shape.
+bool lm_widths(int d, int H, int* dp, int* dhp);
 
 // Whether a decoder's cross-attention is packed in folded form as well: head width 64, d_model 256 or 512 (the widths the
 // folded cross-attention kernel is built for: H d_model <= 4096).

@@ -802,16 +802,17 @@ int greedy_select(const float* logits, int n_rows, int V, int* step_arr, int eos
 
 // --------------------------------------------------------------------------- post-norm helpers (TransformerLM)
 // x = LayerNorm(x) in place (fp32) + fp16 copy for the next projection: the post-norm residual stream of
-// TransformerEncoderLayer(normalize_before=False) (Transformer.py:466-481). One warp per row.
+// TransformerEncoderLayer(normalize_before=False) (Transformer.py:466-481). One warp per row.  Rows lie `pitch` apart; the
+// statistics are over the first D channels, and channels D .. pitch - 1 are written as zero (a padded LM's residual stream).
 __global__ void __launch_bounds__(256)
 layernorm_dual_kernel(float* __restrict__ x, __half* __restrict__ x16, const float* __restrict__ gamma,
-                      const float* __restrict__ beta, int M, int D, float eps, int write_f32) {
+                      const float* __restrict__ beta, int M, int D, int pitch, float eps, int write_f32) {
     pdl_trigger();
     pdl_wait();
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= M) return;
     const int lane = threadIdx.x & 31;
-    float* xr = x + static_cast<size_t>(row) * D;
+    float* xr = x + static_cast<size_t>(row) * pitch;
     float s = 0.0f;
     for (int j = lane; j < D; j += 32) s += xr[j];
     const float mean = warp_sum(s) / D;
@@ -821,10 +822,10 @@ layernorm_dual_kernel(float* __restrict__ x, __half* __restrict__ x16, const flo
         q += d0 * d0;
     }
     const float rstd = rsqrtf(warp_sum(q) / D + eps);
-    for (int j = lane; j < D; j += 32) {
-        const float y = (xr[j] - mean) * rstd * __ldg(gamma + j) + __ldg(beta + j);
+    for (int j = lane; j < pitch; j += 32) {
+        const float y = j < D ? (xr[j] - mean) * rstd * __ldg(gamma + j) + __ldg(beta + j) : 0.0f;
         if (write_f32) xr[j] = y;
-        x16[static_cast<size_t>(row) * D + j] = float2half_sat(y);
+        x16[static_cast<size_t>(row) * pitch + j] = float2half_sat(y);
     }
 }
 
@@ -870,19 +871,20 @@ layernorm_dual_reg_kernel(float* __restrict__ x, __half* __restrict__ x16, const
     }
 }
 
-int layernorm_dual(float* x, __half* x16, const float* gamma, const float* beta, int M, int D, float eps, bool write_f32,
-                   cudaStream_t stream) {
+int layernorm_dual(float* x, __half* x16, const float* gamma, const float* beta, int M, int D, int pitch, float eps,
+                   bool write_f32, cudaStream_t stream) {
+    SBK_REQUIRE(D >= 1 && pitch >= D, "layernorm_dual: D=%d, pitch=%d", D, pitch);
     if (M == 0) return SBK_OK;
     const int wf = write_f32 ? 1 : 0;
     const dim3 grid(ceil_div(M, 4)), block(128);
-    switch (D % 128 == 0 ? D / 128 : 0) {
+    switch (D % 128 == 0 && pitch == D ? D / 128 : 0) {
         case 2: SBK_CUDA_CHECK(launch_k(layernorm_dual_reg_kernel<2>, grid, block, 0, stream, x, x16, gamma, beta, M, eps, wf)); break;
         case 4: SBK_CUDA_CHECK(launch_k(layernorm_dual_reg_kernel<4>, grid, block, 0, stream, x, x16, gamma, beta, M, eps, wf)); break;
         case 6: SBK_CUDA_CHECK(launch_k(layernorm_dual_reg_kernel<6>, grid, block, 0, stream, x, x16, gamma, beta, M, eps, wf)); break;
         case 8: SBK_CUDA_CHECK(launch_k(layernorm_dual_reg_kernel<8>, grid, block, 0, stream, x, x16, gamma, beta, M, eps, wf)); break;
         default:
             SBK_CUDA_CHECK(launch_k(layernorm_dual_kernel, dim3(ceil_div(M, 8)), dim3(256), 0, stream, x, x16, gamma, beta, M, D,
-                                    eps, wf));
+                                    pitch, eps, wf));
     }
     SBK_LAUNCH_CHECK();
     return SBK_OK;
@@ -953,7 +955,7 @@ struct BeamArgs {
     const float* add_scores;
     const float* add_row;   // [n_bh] per-hypothesis score added to every token (CoverageScorer), or null
     float attn_weight; int blank; float add_const;
-    const float* lm_emb; const float* lm_pe; int lm_d; float lm_sqrt_d; float* lm_x_next; __half* lm_x16_next; int* tok_cache;
+    const float* lm_emb; const float* lm_pe; int lm_d; float lm_scale; float* lm_x_next; __half* lm_x16_next; int* tok_cache;
     float* scr_val; int* scr_idx; float* scr_lse;   // beam_rows_kernel -> beam_merge_kernel
 };
 
@@ -1155,7 +1157,7 @@ __global__ void __launch_bounds__(BS_THREADS) beam_merge_kernel(const BeamArgs a
     if (a.lm_emb) {
         for (int i = tid; i < beam * a.lm_d; i += BS_THREADS) {
             const int k = i / a.lm_d, c = i - k * a.lm_d;
-            const float v2 = a.lm_emb[static_cast<size_t>(s_wtok[k]) * a.lm_d + c] * a.lm_sqrt_d +
+            const float v2 = a.lm_emb[static_cast<size_t>(s_wtok[k]) * a.lm_d + c] * a.lm_scale +
                              a.lm_pe[static_cast<size_t>(step + 1) * a.lm_d + c];
             a.lm_x_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = v2;
             a.lm_x16_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = float2half_sat(v2);
@@ -1486,7 +1488,7 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
     if (a.lm_emb) {
         for (int i = tid; i < beam * a.lm_d; i += BS_THREADS) {
             const int k = i / a.lm_d, c = i - k * a.lm_d;
-            const float v = a.lm_emb[static_cast<size_t>(s_wtok[k]) * a.lm_d + c] * a.lm_sqrt_d +
+            const float v = a.lm_emb[static_cast<size_t>(s_wtok[k]) * a.lm_d + c] * a.lm_scale +
                             a.lm_pe[static_cast<size_t>(step + 1) * a.lm_d + c];
             a.lm_x_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = v;
             a.lm_x16_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = float2half_sat(v);
@@ -1497,11 +1499,12 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
     if (tid < beam) a.step_arr[row0 + tid] = step + 1;
 }
 
-// step = 0 state: x = emb[bos] * sqrt(d) + pe[0]; beam 0 alive (score 0), others -inf; identity lineage.
+// step = 0 state: x = emb[bos] * sqrt(d) + pe[0] (the LM's: lm_emb[bos] * lm_scale + lm_pe[0]); beam 0 alive (score 0),
+// others -inf; identity lineage.
 __global__ void beam_reset_kernel(int n_bh, int beam, int S_max, int bos, int* step_arr, float* seq_scores, int* lineage,
                                   int* finished, int* n_full, const float* __restrict__ emb, const float* __restrict__ pe,
                                   int d, float sqrt_d, float* __restrict__ x, const float* __restrict__ lm_emb,
-                                  const float* __restrict__ lm_pe, int lm_d, float lm_sqrt_d, float* __restrict__ lm_x,
+                                  const float* __restrict__ lm_pe, int lm_d, float lm_scale, float* __restrict__ lm_x,
                                   __half* __restrict__ lm_x16, int* __restrict__ tok_cache) {
     const int r = blockIdx.x;
     if (threadIdx.x == 0) {
@@ -1516,7 +1519,7 @@ __global__ void beam_reset_kernel(int n_bh, int beam, int S_max, int bos, int* s
     for (int i = threadIdx.x; i < d; i += blockDim.x) x[static_cast<size_t>(r) * d + i] = e[i] * sqrt_d + pe[i];
     if (lm_emb) {
         for (int i = threadIdx.x; i < lm_d; i += blockDim.x) {
-            const float v = lm_emb[static_cast<size_t>(bos) * lm_d + i] * lm_sqrt_d + lm_pe[i];
+            const float v = lm_emb[static_cast<size_t>(bos) * lm_d + i] * lm_scale + lm_pe[i];
             lm_x[static_cast<size_t>(r) * lm_d + i] = v;
             lm_x16[static_cast<size_t>(r) * lm_d + i] = float2half_sat(v);
         }
@@ -1528,7 +1531,7 @@ int beam_reset(int n_bh, int beam, int S_max, int bos, int* step_arr, float* seq
                int* n_full, const float* emb, const float* pe, int d, float* x, const BeamLm* lm, cudaStream_t stream) {
     beam_reset_kernel<<<n_bh, 128, 0, stream>>>(n_bh, beam, S_max, bos, step_arr, seq_scores, lineage, finished, n_full, emb,
                                                 pe, d, sqrtf(static_cast<float>(d)), x, lm ? lm->emb : nullptr,
-                                                lm ? lm->pe : nullptr, lm ? lm->d : 0, lm ? sqrtf(static_cast<float>(lm->d)) : 0.f,
+                                                lm ? lm->pe : nullptr, lm ? lm->d : 0, lm ? lm->scale : 0.f,
                                                 lm ? lm->x : nullptr, lm ? lm->x16 : nullptr, lm ? lm->tok_cache : nullptr);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
@@ -1548,7 +1551,7 @@ int beam_step(const BeamStepArgs& p, int B, cudaStream_t stream) {
     a.min_steps = p.min_steps; a.eos = p.eos; a.use_eos_threshold = p.use_eos_threshold; a.length_norm = p.length_norm;
     a.emb = p.emb; a.pe = p.pe; a.d = p.d; a.sqrt_d = sqrtf(static_cast<float>(p.d)); a.x_next = p.x_next;
     a.add_scores = p.add_scores; a.add_row = p.add_row; a.attn_weight = p.attn_weight; a.blank = p.blank; a.add_const = p.add_const;
-    a.lm_emb = p.lm.emb; a.lm_pe = p.lm.pe; a.lm_d = p.lm.d; a.lm_sqrt_d = p.lm.d ? sqrtf(static_cast<float>(p.lm.d)) : 0.f;
+    a.lm_emb = p.lm.emb; a.lm_pe = p.lm.pe; a.lm_d = p.lm.d; a.lm_scale = p.lm.scale;
     a.lm_x_next = p.lm.x; a.lm_x16_next = p.lm.x16; a.tok_cache = p.lm.tok_cache;
     a.scr_val = nullptr; a.scr_idx = nullptr; a.scr_lse = nullptr;
     if (p.path == 2 || (p.path == 0 && p.beam > BS_MAXB))

@@ -1388,7 +1388,9 @@ int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, cons
 // =========================================================================== TransformerLM causal self-attention
 // Whole-sequence attention of TransformerLM.forward (TransformerLM.py:127-169: nn.MultiheadAttention under make_masks'
 // look-ahead mask and key-padding mask on pad_idx).  qkv [n*s, 3d] fp16 with columns [q | k | v] (nn.MultiheadAttention's
-// in_proj order, heads of 64 side by side, q pre-scaled by 1/sqrt(64)) -> out [n*s, d] fp16.
+// in_proj order, heads of DH side by side, q pre-scaled by 1/sqrt(true head width)) -> out [n*s, d] fp16.  DH = 64, or 32:
+// the Switchboard LM's heads of 22 zero-padded to the 16-wide k-step of m16n8k16 (the padding adds zero to q.k and
+// gives zero output columns).
 // One CTA = (64 query rows, head, sequence), 4 warps x 16 rows, mma.sync m16n8k16 with an fp32 online softmax like
 // encoder_attention_kernel.  Query block qb reads key blocks 0..qb only: blocks above the diagonal are never loaded.
 // Masked: keys j > i (diagonal block only) and keys whose token id is pad_tok -- the rule the KV-cached step applies
@@ -1396,10 +1398,12 @@ int hypermix_forward(const __half* h16, int B, int T, int d, int M, int KH, cons
 // with the pad id) has an empty softmax and yields NaN, as in the reference and the step path.
 constexpr int LMA_B = 64;
 
+template <int DH>
 __global__ void __launch_bounds__(128)
 lm_causal_attention_kernel(const __half* __restrict__ qkv, int s, int d, const int* __restrict__ tokens, int pad_tok,
                            __half* __restrict__ out) {
-    constexpr int DH = 64, STR = DH + 8, KS = DH / 16;
+    static_assert(DH % 32 == 0, "lm_causal_attention_kernel: K fragments are loaded 32 dims at a time");
+    constexpr int STR = DH + 8, KS = DH / 16;  // row stride 16 B past a multiple of 64 B: ldmatrix rows hit distinct banks
     __shared__ __align__(16) __half Qs[LMA_B * STR];
     __shared__ __align__(16) __half KVs[2][2][LMA_B * STR];  // [buffer][K | V]
     __shared__ bool s_masked[2][LMA_B];                       // [buffer][key]: pad token or past the sequence
@@ -1545,11 +1549,13 @@ lm_causal_attention_kernel(const __half* __restrict__ qkv, int s, int d, const i
 
 int lm_causal_attention(const __half* qkv, int n, int s, int d, int H, const int* tokens, int pad_tok, __half* out,
                         cudaStream_t stream) {
-    SBK_REQUIRE(d == H * 64 && d % 8 == 0, "lm_causal_attention: head_dim must be 64 (d=%d, H=%d)", d, H);
+    SBK_REQUIRE(H >= 1 && (d == H * 64 || d == H * 32), "lm_causal_attention: head_dim must be 64 or 32 (d=%d, H=%d)", d, H);
     SBK_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 3) == 0,
                 "lm_causal_attention: misaligned operands");
     if (n == 0 || s == 0) return SBK_OK;
-    lm_causal_attention_kernel<<<dim3(ceil_div(s, LMA_B), H, n), 128, 0, stream>>>(qkv, s, d, tokens, pad_tok, out);
+    const dim3 grid(ceil_div(s, LMA_B), H, n);
+    if (d == H * 64) lm_causal_attention_kernel<64><<<grid, 128, 0, stream>>>(qkv, s, d, tokens, pad_tok, out);
+    else lm_causal_attention_kernel<32><<<grid, 128, 0, stream>>>(qkv, s, d, tokens, pad_tok, out);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }

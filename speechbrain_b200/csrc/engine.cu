@@ -286,13 +286,13 @@ static void workspace_layout(const AsrModel* m, int B, int Be, int L, int rows, 
     take(b.lnout, (size_t)rows * d * 4); take(b.beam_scr, (size_t)rows * 33 * 4);
     take(b.hist_tok, (size_t)rows * S * 4); take(b.hist_pred, (size_t)rows * S * 4);
     take(b.hist_score, (size_t)rows * S * 4); take(b.hist_lp, (size_t)rows * S * 4);
-    if (m->wt->has_lm) {
-        const size_t dl = c.lm_d_model, Fl = c.lm_d_ffn, Ll = c.lm_layers;
-        take(b.lx, rows * dl * 4); take(b.lh32, rows * dl * 4); take(b.lm_logits, (size_t)rows * c.vocab * 4);
+    if (m->wt->has_lm) {  // the residual stream at pitch lm_dp, queries / attention outputs / KV cache at lm_da
+        const size_t dp = m->wt->lm_dp, da = m->wt->lm_da, Fl = c.lm_d_ffn, Ll = c.lm_layers;
+        take(b.lx, rows * dp * 4); take(b.lh32, rows * dp * 4); take(b.lm_logits, (size_t)rows * c.vocab * 4);
         take(b.lm_extra, (size_t)rows * c.vocab * 4);
-        take(b.lx16, rows * dl * 2); take(b.lq16, rows * dl * 2); take(b.latt16, rows * dl * 2);
-        take(b.lf16, rows * Fl * 2); take(b.lh16, rows * dl * 2);
-        take(b.lkc, Ll * rows * S * dl * 2); take(b.lvc, Ll * rows * S * dl * 2); take(b.tok_cache, (size_t)rows * S * 4);
+        take(b.lx16, rows * dp * 2); take(b.lq16, rows * da * 2); take(b.latt16, rows * da * 2);
+        take(b.lf16, rows * Fl * 2); take(b.lh16, rows * dp * 2);
+        take(b.lkc, Ll * rows * S * da * 2); take(b.lvc, Ll * rows * S * da * 2); take(b.tok_cache, (size_t)rows * S * 4);
     }
     if (bfm) {
         take(b.hc16, M * d * 2); take(b.cat16, M * 2 * d * 2); take(b.g16, M * Cu / 2 * 2);
@@ -766,17 +766,18 @@ static int enqueue_decode_step(AsrModel* m, int rows, int T, int S_max, bool fol
 }
 
 // A post-norm TransformerLM layer after its self-attention (Transformer.py:466-481): x = norm1(x + out_proj(att)), then
-// x = norm2(x + ffn(x)).  x is the fp32 residual stream [rows, d] and x16 its fp16 copy; f16 [rows, d_ffn] is scratch.
+// x = norm2(x + ffn(x)).  x is the fp32 residual stream [rows, lm_dp] and x16 its fp16 copy, att16 [rows, lm_da]; f16
+// [rows, d_ffn] is scratch.  The LayerNorms take their statistics over the d_model real channels and write zero padding.
 static int lm_layer_tail(const AsrModel* m, StepGemm g, const LmLayerW& w, int rows, const __half* att16, float* x,
                          __half* x16, __half* f16, cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
-    const int dl = c.lm_d_model, Fl = c.lm_d_ffn;
+    const int dl = c.lm_d_model, dp = m->wt->lm_dp, da = m->wt->lm_da, Fl = c.lm_d_ffn;
     const ProjOut act = c.lm_activation == SBK_ACT_GELU ? PO_F16_GELU : PO_F16_RELU;
-    RC(project(g, {w.w_out, w.b_out, dl, dl, PO_RESID, x, dl, att16, dl}, rows, st));
-    RC(layernorm_dual(x, x16, w.n1g, w.n1b, rows, dl, 1e-6f, true, st));
-    RC(project(g, {w.w1, w.b1, Fl, dl, act, f16, Fl, x16, dl}, rows, st));
-    RC(project(g, {w.w2, w.b2, dl, Fl, PO_RESID, x, dl, f16, Fl}, rows, st));
-    return layernorm_dual(x, x16, w.n2g, w.n2b, rows, dl, 1e-6f, true, st);
+    RC(project(g, {w.w_out, w.b_out, dp, da, PO_RESID, x, dp, att16, da}, rows, st));
+    RC(layernorm_dual(x, x16, w.n1g, w.n1b, rows, dl, dp, 1e-6f, true, st));
+    RC(project(g, {w.w1, w.b1, Fl, dp, act, f16, Fl, x16, dp}, rows, st));
+    RC(project(g, {w.w2, w.b2, dp, Fl, PO_RESID, x, dp, f16, Fl}, rows, st));
+    return layernorm_dual(x, x16, w.n2g, w.n2b, rows, dl, dp, 1e-6f, true, st);
 }
 
 // The LM's encoder.norm, then output_proj: Linear d -> d (fp32 into h32), LayerNorm (fp16 into h16), Linear d -> vocab
@@ -784,31 +785,31 @@ static int lm_layer_tail(const AsrModel* m, StepGemm g, const LmLayerW& w, int r
 static int lm_output(const AsrModel* m, StepGemm g, int rows, float* x, __half* x16, float* h32, __half* h16, float* logits,
                      cudaStream_t st) {
     const AsrWeights& W = *m->wt;
-    const int dl = W.cfg.lm_d_model, V = W.cfg.vocab;
-    RC(layernorm_dual(x, x16, W.lm_norm_g, W.lm_norm_b, rows, dl, 1e-6f, false, st));
-    RC(project(g, {W.lm_wp0, W.lm_bp0, dl, dl, PO_F32, h32, dl, x16, dl}, rows, st));
-    RC(layernorm_dual(h32, h16, W.lm_lnp_g, W.lm_lnp_b, rows, dl, 1e-6f, false, st));
-    return project(g, {W.lm_wp2, W.lm_bp2, V, dl, PO_F32, logits, V, h16, dl}, rows, st);
+    const int dl = W.cfg.lm_d_model, dp = W.lm_dp, V = W.cfg.vocab;
+    RC(layernorm_dual(x, x16, W.lm_norm_g, W.lm_norm_b, rows, dl, dp, 1e-6f, false, st));
+    RC(project(g, {W.lm_wp0, W.lm_bp0, dp, dp, PO_F32, h32, dp, x16, dp}, rows, st));
+    RC(layernorm_dual(h32, h16, W.lm_lnp_g, W.lm_lnp_b, rows, dl, dp, 1e-6f, false, st));
+    return project(g, {W.lm_wp2, W.lm_bp2, V, dp, PO_F32, logits, V, h16, dp}, rows, st);
 }
 
 // One TransformerLM step over `rows` hypotheses (post-norm encoder layers with a lineage-indexed KV cache), ending in
 // b.lm_extra[rows, V] = weight * log_softmax(lm_logits / temperature): TransformerLMScorer.score (scorer.py:510-543)
-// scaled by ScorerBuilder's weight.  b.lx / b.lx16 hold emb[token] * sqrt(d) + pe[step] (beam_reset / beam_step).
+// scaled by ScorerBuilder's weight.  b.lx / b.lx16 hold emb[token] * scale + pe[step] (beam_reset / beam_step).
 static int enqueue_lm_step(AsrModel* m, int rows, int S_max, float temperature, float weight, cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
-    const int dl = c.lm_d_model, H = c.lm_nhead;
-    const StepGemm g = step_gemm(m, rows, dl);
+    const int dp = m->wt->lm_dp, da = m->wt->lm_da, H = c.lm_nhead;
+    const StepGemm g = step_gemm(m, rows, da);
     for (int l = 0; l < c.lm_layers; ++l) {
         const LmLayerW& w = m->wt->lm[l];
-        __half* kc = b.lkc + (size_t)l * rows * S_max * dl;
-        __half* vc = b.lvc + (size_t)l * rows * S_max * dl;
-        Proj qkv{w.w_in, w.b_in, 3 * dl, dl, PO_QKV_CACHE, b.lq16, dl, b.lx16, dl};
+        __half* kc = b.lkc + (size_t)l * rows * S_max * da;
+        __half* vc = b.lvc + (size_t)l * rows * S_max * da;
+        Proj qkv{w.w_in, w.b_in, 3 * da, dp, PO_QKV_CACHE, b.lq16, da, b.lx16, dp};
         qkv.kcache = kc; qkv.vcache = vc; qkv.step_ptr = b.step; qkv.S_max = S_max;
         RC(project(g, qkv, rows, st));
         DecAttnArgs t{};
-        t.q = b.lq16; t.ldq = dl; t.kbase = kc; t.vbase = vc; t.row_stride = (size_t)S_max * dl; t.key_stride = dl;
-        t.rows_per_block = 1; t.n_keys_ptr = b.step; t.H = H; t.dh = 64; t.out = b.latt16; t.ldo = dl;
+        t.q = b.lq16; t.ldq = da; t.kbase = kc; t.vbase = vc; t.row_stride = (size_t)S_max * da; t.key_stride = da;
+        t.rows_per_block = 1; t.n_keys_ptr = b.step; t.H = H; t.dh = m->wt->lm_dhp; t.out = b.latt16; t.ldo = da;
         t.lineage = b.lineage; t.lin_stride = S_max; t.tok_cache = b.tok_cache; t.pad_tok = 0;
         RC(dec_attention(t, rows, S_max, st));
         RC(lm_layer_tail(m, g, w, rows, b.latt16, b.lx, b.lx16, b.lf16, st));
@@ -898,7 +899,10 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
         cv.threshold = p.coverage_threshold; cv.weight = p.coverage_weight; cv.out = cov + (size_t)2 * rows * T;
     }
     BeamLm lm;
-    if (use_lm) { lm.emb = m->wt->lm_emb; lm.pe = m->wt->lm_pe; lm.d = c.lm_d_model; lm.x = b.lx; lm.x16 = b.lx16; lm.tok_cache = b.tok_cache; }
+    if (use_lm) {
+        lm.emb = m->wt->lm_emb; lm.pe = m->wt->lm_pe; lm.d = m->wt->lm_dp; lm.scale = m->wt->lm_emb_scale;
+        lm.x = b.lx; lm.x16 = b.lx16; lm.tok_cache = b.tok_cache;
+    }
     RC(beam_reset(rows, beam, S_max, p.bos, b.step, b.seq_scores, b.lineage, b.finished, b.ended_count, m->wt->emb, m->wt->dec_pe, d,
                   b.dx, use_lm ? &lm : nullptr, st));
     BeamStepArgs a{};
@@ -999,12 +1003,12 @@ __global__ void lm_teacher_reset_kernel(const int* __restrict__ tokens, int n, i
     if (threadIdx.x == 0) scores[r] = 0.0f;
 }
 __global__ void lm_teacher_embed_kernel(const int* __restrict__ tokens, int L, int s, const float* __restrict__ emb,
-                                        const float* __restrict__ pe, int d, float sqrt_d, float* __restrict__ x,
+                                        const float* __restrict__ pe, int d, float scale, float* __restrict__ x,
                                         __half* __restrict__ x16, int* __restrict__ step_arr) {
     const int r = blockIdx.x;
     const int tok = tokens[static_cast<size_t>(r) * L + s];
     for (int i = threadIdx.x; i < d; i += blockDim.x) {
-        const float v = emb[static_cast<size_t>(tok) * d + i] * sqrt_d + pe[static_cast<size_t>(s) * d + i];
+        const float v = emb[static_cast<size_t>(tok) * d + i] * scale + pe[static_cast<size_t>(s) * d + i];
         x[static_cast<size_t>(r) * d + i] = v;
         x16[static_cast<size_t>(r) * d + i] = float2half_sat(v);
     }
@@ -1057,12 +1061,13 @@ static int run_lm_rescore(AsrModel* m, const int* tokens, const int* lens, int n
                           float* scores, cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
-    const int S_max = m->ws_steps + 1, dl = c.lm_d_model;
-    set_step_pdl(m, n, dl);
+    const int S_max = m->ws_steps + 1, dp = m->wt->lm_dp;
+    set_step_pdl(m, n, m->wt->lm_da);
     lm_teacher_reset_kernel<<<n, 128, 0, st>>>(tokens, n, L, S_max, pad, b.lineage, b.tok_cache, scores);
     SBK_LAUNCH_CHECK();
     for (int s = 0; s + 1 < L; ++s) {
-        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->wt->lm_emb, m->wt->lm_pe, dl, sqrtf((float)dl), b.lx, b.lx16, b.step);
+        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->wt->lm_emb, m->wt->lm_pe, dp, m->wt->lm_emb_scale, b.lx,
+                                                   b.lx16, b.step);
         SBK_LAUNCH_CHECK();
         RC(enqueue_lm_step(m, n, S_max, temperature, 1.0f, st));
         lm_teacher_score_kernel<<<ceil_div(n, 128), 128, 0, st>>>(b.lm_extra, c.vocab, tokens, L, s, lens, pad, scores, n);
@@ -1076,12 +1081,13 @@ static int run_lm_rescore(AsrModel* m, const int* tokens, const int* lens, int n
 static int run_lm_step_logits(AsrModel* m, const int* tokens, int n, int L, float* out, cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
-    const int S_max = m->ws_steps + 1, dl = c.lm_d_model, V = c.vocab;
-    set_step_pdl(m, n, dl);
+    const int S_max = m->ws_steps + 1, dp = m->wt->lm_dp, V = c.vocab;
+    set_step_pdl(m, n, m->wt->lm_da);
     lm_teacher_reset_kernel<<<n, 128, 0, st>>>(tokens, n, L, S_max, 0, b.lineage, b.tok_cache, b.score);
     SBK_LAUNCH_CHECK();
     for (int s = 0; s < L; ++s) {
-        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->wt->lm_emb, m->wt->lm_pe, dl, sqrtf((float)dl), b.lx, b.lx16, b.step);
+        lm_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, L, s, m->wt->lm_emb, m->wt->lm_pe, dp, m->wt->lm_emb_scale, b.lx,
+                                                   b.lx16, b.step);
         SBK_LAUNCH_CHECK();
         RC(enqueue_lm_step(m, n, S_max, 1.0f, 1.0f, st));
         SBK_CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s * V, (size_t)L * V * 4, b.lm_logits, (size_t)V * 4, (size_t)V * 4, n,
@@ -1093,17 +1099,17 @@ static int run_lm_step_logits(AsrModel* m, const int* tokens, int n, int L, floa
 // ---------------------------------------------------------------------------- TransformerLM.forward (TransformerLM.py:127-169)
 // Whole sequences at once: the n * s token rows go through every layer together on the encoder's wgmma GEMMs, attention is
 // the causal flash kernel (lm_causal_attention).  Same weights, epilogues and LayerNorm kernel as the KV-cached step.
-// Row r = (sequence r / s, position r % s): x = emb[token] * sqrt(d) + pe[pos], fp32 residual stream + fp16 GEMM operand
+// Row r = (sequence r / s, position r % s): x = emb[token] * scale + pe[pos], fp32 residual stream + fp16 GEMM operand
 // (the whole-sequence counterpart of lm_teacher_embed_kernel).  An id outside [0, vocab) is not read from the table: its
 // row becomes NaN (and, through attention, its sequence) instead of an out-of-bounds read.
 __global__ void lm_embed_kernel(const int* __restrict__ tokens, int s, int vocab, const float* __restrict__ emb,
-                                const float* __restrict__ pe, int d, float sqrt_d, float* __restrict__ x,
+                                const float* __restrict__ pe, int d, float scale, float* __restrict__ x,
                                 __half* __restrict__ x16) {
     const int r = blockIdx.x, pos = r % s;
     const int tok = tokens[r];
     const bool ok = tok >= 0 && tok < vocab;
     for (int i = threadIdx.x; i < d; i += blockDim.x) {
-        const float v = ok ? emb[static_cast<size_t>(tok) * d + i] * sqrt_d + pe[static_cast<size_t>(pos) * d + i] : NAN;
+        const float v = ok ? emb[static_cast<size_t>(tok) * d + i] * scale + pe[static_cast<size_t>(pos) * d + i] : NAN;
         x[static_cast<size_t>(r) * d + i] = v;
         x16[static_cast<size_t>(r) * d + i] = float2half_sat(v);
     }
@@ -1112,9 +1118,9 @@ __global__ void lm_embed_kernel(const int* __restrict__ tokens, int s, int vocab
 static int ensure_lm_workspace(AsrModel* m, int rows) {
     AsrModel::LmFwdBuf& w = m->lmf;
     if (m->lmf_mem.base && rows <= w.rows) return SBK_OK;
-    const size_t R = rows, dl = m->wt->cfg.lm_d_model, Fl = m->wt->cfg.lm_d_ffn;
+    const size_t R = rows, dp = m->wt->lm_dp, da = m->wt->lm_da, Fl = m->wt->cfg.lm_d_ffn;
     auto layout = [&](Carver& take) {
-        take(w.x, R * dl * 4); take(w.x16, R * dl * 2); take(w.qkv16, R * 3 * dl * 2); take(w.att16, R * dl * 2);
+        take(w.x, R * dp * 4); take(w.x16, R * dp * 2); take(w.qkv16, R * 3 * da * 2); take(w.att16, R * da * 2);
         take(w.f16, R * Fl * 2);
     };
     Carver measure;
@@ -1128,15 +1134,15 @@ static int ensure_lm_workspace(AsrModel* m, int rows) {
 
 static int run_lm_forward(AsrModel* m, const int* tokens, int n, int s, float* logits, cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
-    const int dl = c.lm_d_model, H = c.lm_nhead, M = n * s;
+    const int dp = m->wt->lm_dp, da = m->wt->lm_da, H = c.lm_nhead, M = n * s;
     RC(ensure_lm_workspace(m, M));
     const AsrModel::LmFwdBuf& b = m->lmf;
-    lm_embed_kernel<<<M, 128, 0, st>>>(tokens, s, c.vocab, m->wt->lm_emb, m->wt->lm_pe, dl, sqrtf((float)dl), b.x, b.x16);
+    lm_embed_kernel<<<M, 128, 0, st>>>(tokens, s, c.vocab, m->wt->lm_emb, m->wt->lm_pe, dp, m->wt->lm_emb_scale, b.x, b.x16);
     SBK_LAUNCH_CHECK();
     for (int l = 0; l < c.lm_layers; ++l) {  // post-norm TransformerEncoderLayer (Transformer.py:466-481)
         const LmLayerW& w = m->wt->lm[l];
-        RC(project(SG_WIDE, {w.w_in, w.b_in, 3 * dl, dl, PO_F16, b.qkv16, 3 * dl, b.x16, dl}, M, st));
-        RC(lm_causal_attention(b.qkv16, n, s, dl, H, tokens, 0, b.att16, st));
+        RC(project(SG_WIDE, {w.w_in, w.b_in, 3 * da, dp, PO_F16, b.qkv16, 3 * da, b.x16, dp}, M, st));
+        RC(lm_causal_attention(b.qkv16, n, s, da, H, tokens, 0, b.att16, st));
         RC(lm_layer_tail(m, SG_WIDE, w, M, b.att16, b.x, b.x16, b.f16, st));
     }
     // output_proj's fp32 Linear d -> d goes into the free residual buffer, its logits into the caller's
@@ -1803,7 +1809,7 @@ int sbk_asr_lm_forward(sbk_asr* mm, const int* tokens_dev, int n, int s, float* 
     SBK_REQUIRE(n >= 1 && s >= 1, "lm_forward: bad shape n=%d s=%d", n, s);
     SBK_REQUIRE(n <= 65535, "lm_forward: n=%d sequences exceed the 65535 of one call (attention grid z)", n);
     SBK_REQUIRE(s <= m->wt->cfg.max_len, "lm_forward: s=%d exceeds max_len=%d", s, m->wt->cfg.max_len);
-    SBK_REQUIRE((long long)n * s * std::max(m->wt->cfg.vocab, 3 * m->wt->cfg.lm_d_model) < (1LL << 31),
+    SBK_REQUIRE((long long)n * s * std::max(m->wt->cfg.vocab, 3 * m->wt->lm_da) < (1LL << 31),
                 "lm_forward: n * s = %lld token rows is too many for one call", (long long)n * s);
     return run_lm_forward(m, tokens_dev, n, s, logits_dev, static_cast<cudaStream_t>(stream));
 }

@@ -182,7 +182,8 @@ int encoder_attention_stream(const AttStream& sa, int B, int W, int H, int head_
 // inv_freq [head_dim / 2] set: RoPE at stream positions pos0 + i, q scaled by q_scale
 int stream_qkv(const float* qkv, int B, int n, int H, int DH, const float* inv_freq, long long pos0, float q_scale,
                __half* q, __half* kv, int cap, int slot0, cudaStream_t stream);
-// TransformerLM whole-sequence causal self-attention: qkv [n*s, 3d] fp16 ([q | k | v], head_dim 64, q pre-scaled), tokens
+// TransformerLM whole-sequence causal self-attention: qkv [n*s, 3d] fp16 ([q | k | v], head_dim d / H of 64 or 32, q
+// pre-scaled), tokens
 // [n, s] int32 (keys whose id == pad_tok are masked) -> out [n*s, d] fp16
 int lm_causal_attention(const __half* qkv, int n, int s, int d, int H, const int* tokens, int pad_tok, __half* out,
                         cudaStream_t stream);
@@ -231,7 +232,8 @@ struct XattFoldArgs {
 };
 int dec_xatt_fold(const XattFoldArgs& a, int n_utt, cudaStream_t stream);
 struct BeamLm {  // TransformerLM scorer state the beam step feeds (all null/0 when there is no LM)
-    const float* emb = nullptr; const float* pe = nullptr; int d = 0;
+    const float* emb = nullptr; const float* pe = nullptr; int d = 0;  // d: the row pitch of emb, pe, x and x16
+    float scale = 0.0f;                                                 // x = emb[token] * scale + pe[step]
     float* x = nullptr; __half* x16 = nullptr; int* tok_cache = nullptr;
 };
 struct BeamStepArgs {
@@ -277,8 +279,10 @@ int rows_logsoftmax_argmax(float* x, int rows, int V, bool do_logsoftmax, int* i
 int ctc_prefix_update(const CtcStep& p, cudaStream_t stream);
 int beam_reset(int n_bh, int beam, int S_max, int bos, int* step_arr, float* seq_scores, int* lineage, int* finished,
                int* n_full, const float* emb, const float* pe, int d, float* x, const BeamLm* lm, cudaStream_t stream);
-int layernorm_dual(float* x, __half* x16, const float* gamma, const float* beta, int M, int D, float eps, bool write_f32,
-                   cudaStream_t stream);
+// x [M, pitch] fp32 rows of D channels and pitch - D zero padding -> LayerNorm over the D channels, in place (write_f32) and
+// into x16 [M, pitch] fp16, the padding written as zero; gamma, beta [D]
+int layernorm_dual(float* x, __half* x16, const float* gamma, const float* beta, int M, int D, int pitch, float eps,
+                   bool write_f32, cudaStream_t stream);
 int weighted_log_softmax(const float* logits, float* out, int rows, int V, float temperature, float weight,
                          cudaStream_t stream);
 int beam_step(const BeamStepArgs& p, int B, cudaStream_t stream);

@@ -151,6 +151,15 @@ int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int hea
     return finish_test("encoder_attention_test", rc, st);
 }
 
+int sbk_lm_causal_attention_test(const void* qkv_dev, int n, int s, int d, int H, const int* tokens_dev, int pad_tok,
+                                 void* out_dev, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(qkv_dev && tokens_dev && out_dev && n >= 1 && s >= 1 && n <= 65535, "lm_causal_attention_test: bad arguments");
+    return finish_test("lm_causal_attention_test",
+                       lm_causal_attention(static_cast<const __half*>(qkv_dev), n, s, d, H, tokens_dev, pad_tok,
+                                           static_cast<__half*>(out_dev), st), st);
+}
+
 int sbk_dec_attention_test(const void* q_dev, int ldq, const void* kbase_dev, const void* vbase_dev, long long row_stride,
                            int key_stride, int head_stride, int rows_per_block, int rows, int H, int dh, int max_keys, int step,
                            const int* enc_len_dev, const int* lineage_dev, const int* tok_cache_dev, int lin_stride,
@@ -375,7 +384,7 @@ int sbk_beam_step_test(const sbk_beam_params* params, int path, int B, int V, in
     a.add_scores = add_scores_dev; a.add_row = add_row_dev; a.add_const = p.length_weight;
     if (p.ctc_weight != 0.0f) { a.attn_weight = 1.0f - p.ctc_weight; a.blank = p.blank_index; }
     if (lm) {
-        a.lm.emb = lm_emb_dev; a.lm.pe = lm_pe_dev; a.lm.d = lm_d; a.lm.x = lm_x_dev; a.lm.x16 = static_cast<__half*>(lm_x16_dev);
+        a.lm.emb = lm_emb_dev; a.lm.pe = lm_pe_dev; a.lm.d = lm_d; a.lm.scale = sqrtf((float)lm_d); a.lm.x = lm_x_dev; a.lm.x16 = static_cast<__half*>(lm_x16_dev);
         a.lm.tok_cache = tok_cache_dev;
     }
     a.scratch = scr; a.path = path;

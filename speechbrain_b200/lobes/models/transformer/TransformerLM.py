@@ -1,7 +1,11 @@
 """TransformerLM -- mirror of speechbrain.lobes.models.transformer.TransformerLM.TransformerLM (TransformerLM.py:22-187):
 same constructor kwargs and state_dict keys (so ``lm.ckpt`` loads unchanged).  ``forward(src)`` runs the whole-sequence
 (prefill) pass on the device (csrc/engine.cu run_lm_forward); the beam search's shallow fusion and the n-best rescorer
-keep the KV-cached step (enqueue_lm_step)."""
+keep the KV-cached step (enqueue_lm_step).
+
+Built: head width 64 with d_model a multiple of 128, and the Switchboard recipe's LM (d_model 264, 12 heads of 22,
+d_embedding 128, whose embedding_proj the device folds into the embedding table)."""
+SWITCHBOARD_LM_SHAPE = (264, 12, 128)  # (d_model, nhead, d_embedding) of Switchboard/LM/hparams/transformer.yaml
 import torch
 
 from ....utils.param_tree import _Node, build_param_tree, default_init
@@ -19,11 +23,12 @@ class TransformerLM(torch.nn.Module):
             bad.append("num_decoder_layers != 0")
         if normalize_before:
             bad.append("normalize_before=True")
-        if d_embedding is not None and d_embedding != d_model:
-            bad.append("d_embedding != d_model")
+        switchboard = (d_model, nhead, d_embedding) == SWITCHBOARD_LM_SHAPE
+        if d_embedding is not None and d_embedding != d_model and not switchboard:
+            bad.append("d_embedding other than d_model (or 128 with the Switchboard LM's d_model 264 and 12 heads)")
         if attention_type != "regularMHA" or positional_encoding != "fixed_abs_sine" or not causal:
             bad.append("attention_type / positional_encoding / causal other than the recipe's")
-        if d_model % nhead or d_model // nhead != 64 or d_model % 128:
+        if not switchboard and (d_model % nhead or d_model // nhead != 64 or d_model % 128):
             bad.append("head_dim != 64 or d_model % 128 != 0")
         act = getattr(activation, "__name__", str(activation))
         if act not in ("GELU", "ReLU"):
@@ -33,7 +38,9 @@ class TransformerLM(torch.nn.Module):
         self.vocab, self.d_model, self.nhead, self.num_encoder_layers, self.d_ffn = vocab, d_model, nhead, num_encoder_layers, d_ffn
         self.activation = "gelu" if act == "GELU" else "relu"
         self.max_length = max_length
-        build_param_tree(self, transformer_lm_shapes(vocab, d_model, nhead, num_encoder_layers, d_ffn), default_init)
+        self.d_embedding = d_embedding if switchboard else None  # (d_embedding == d_model builds no projection)
+        build_param_tree(self, transformer_lm_shapes(vocab, d_model, nhead, num_encoder_layers, d_ffn, self.d_embedding),
+                         default_init)
         self.positional_encoding = _Node()
         self.positional_encoding.register_buffer("pe", _sine_table(max_length, d_model))
         self._slot = None

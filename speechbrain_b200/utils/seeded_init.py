@@ -162,3 +162,15 @@ LOQUACIOUS_LARGE = dict(LOQUACIOUS_SMALL, name="loquacious_large", d_model=768, 
 LOQUACIOUS_XLARGE = dict(LOQUACIOUS_SMALL, name="loquacious_xlarge", d_model=1024, nhead=16, num_encoder_layers=18,
                          d_ffn=3072, vocab=5120)
 LOQUACIOUS_BLANK, LOQUACIOUS_BOS, LOQUACIOUS_EOS, LOQUACIOUS_PAD = 3, 1, 2, 0
+# recipes/Switchboard/ASR/transformer/hparams/transformer.yaml: the 3-block front-end (64 channels, input 20 x 64 = 1280),
+# 12 pre-norm Transformer encoder layers with regularMHA (4 heads of 64) at d_model 256, 6 GELU decoder layers, 2000 tokens;
+# its lm_model (the same as recipes/Switchboard/LM/hparams/transformer.yaml) is SWITCHBOARD_LM, the TransformerLM keywords.
+# Token indices: blank 0, pad 0, bos 1, eos 2.
+SWITCHBOARD_TRANSFORMER = dict(name="switchboard_transformer", sample_rate=16000, n_fft=400, win=400, hop=160, n_mels=80,
+                               cnn_channels=(64, 64), cnn_blocks=3, input_size=1280, d_model=256, nhead=4,
+                               num_encoder_layers=12, num_decoder_layers=6, d_ffn=2048, vocab=2000, kernel_size=31,
+                               attention_type="regularMHA", decoder_activation="gelu", max_length=2500,
+                               encoder_module="transformer")
+SWITCHBOARD_LM = dict(vocab=2000, d_model=264, d_embedding=128, nhead=12, num_encoder_layers=12, num_decoder_layers=0,
+                      d_ffn=1024, normalize_before=False)
+SWITCHBOARD_BLANK, SWITCHBOARD_PAD, SWITCHBOARD_BOS, SWITCHBOARD_EOS = 0, 0, 1, 2
