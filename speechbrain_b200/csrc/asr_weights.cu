@@ -170,41 +170,38 @@ static void pack_frontend(Packer& p, AsrWeights& W) {
     if (!W.has_cnn) return;
     const int F1 = (c.n_mels - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
     const std::string b0 = "CNN.convblock_0.convs.", b1 = "CNN.convblock_1.convs.", b2 = "CNN.convblock_2.";
-    if (c.cnn_blocks == 3) {  // convolution.py:116-320 with kernel_sizes (5, 5, 1), residuals (False, False, True)
-        const int C = 64;
-        Cnn3Weights& k = W.cnn3;
-        k.w1 = p.f32(b0 + "conv_0.conv.weight", (int64_t)C * 25);
-        k.b1 = p.f32(b0 + "conv_0.conv.bias", C);
-        p.norm(b0 + "norm_0.norm", (int64_t)F1 * C, &k.g1, &k.be1);
-        const float* w2 = p.host(b1 + "conv_0.conv.weight", (int64_t)C * C * 25);
-        const float* w3a = p.host(b2 + "convs.conv_0.conv.weight", (int64_t)C * C);
-        const float* w3r = p.host(b2 + "reduce_conv.conv.conv.weight", (int64_t)C * C);
-        const float* b3a = p.host(b2 + "convs.conv_0.conv.bias", C);
-        const float* b3r = p.host(b2 + "reduce_conv.conv.conv.bias", C);
-        if (!w2 || !w3a || !w3r || !b3a || !b3r) return;
-        k.w2p = p.f16_raw(conv_taps_channel_last(w2, C, C, 5));
-        k.b2 = p.f32(b1 + "conv_0.conv.bias", C);
-        p.norm(b1 + "norm_0.norm", (int64_t)F2 * C, &k.g2, &k.be2);
-        std::vector<float> w3((size_t)2 * C * C), b3(2 * C);  // [convs.conv_0 | reduce_conv.conv] output channels
-        memcpy(w3.data(), w3a, (size_t)C * C * 4);
-        memcpy(w3.data() + (size_t)C * C, w3r, (size_t)C * C * 4);
-        memcpy(b3.data(), b3a, C * 4);
-        memcpy(b3.data() + C, b3r, C * 4);
-        k.w3 = p.f32_raw(w3);
-        k.b3 = p.f32_raw(b3);
-        p.norm(b2 + "convs.norm_0.norm", (int64_t)F2 * C, &k.g3, &k.be3);
-        p.norm(b2 + "reduce_conv.norm.norm", (int64_t)F2 * C, &k.gr, &k.ber);
-    } else {
-        W.c1_w = p.f32(b0 + "conv_0.conv.weight", (int64_t)c.cnn_c1 * 9);
-        W.c1_b = p.f32(b0 + "conv_0.conv.bias", c.cnn_c1);
-        p.norm(b0 + "norm_0.norm", (int64_t)F1 * c.cnn_c1, &W.c1_g, &W.c1_be);
-        const float* w2 = p.host(b1 + "conv_0.conv.weight", (int64_t)c.cnn_c2 * c.cnn_c1 * 9);
-        if (!w2) return;
-        W.c2_w = p.f16_raw(c.cnn_c1 == 256 ? conv_taps_kblocks_sw128(w2, c.cnn_c2, c.cnn_c1)
-                                           : conv_taps_channel_last(w2, c.cnn_c2, c.cnn_c1, 3));
-        W.c2_b = p.f32(b1 + "conv_0.conv.bias", c.cnn_c2);
-        p.norm(b1 + "norm_0.norm", (int64_t)F2 * c.cnn_c2, &W.c2_g, &W.c2_be);
+    // convolution.py:116-320; 3 blocks: kernel_sizes (5, 5, 1), residuals (False, False, True), 64 channels
+    CnnWeights& k = W.cnn;
+    k.blocks = c.cnn_blocks == 3 ? 3 : 2;
+    k.c1 = c.cnn_c1;
+    k.c2 = c.cnn_c2;
+    const int K = k.blocks == 3 ? 5 : 3, C = 64;
+    k.w1 = p.f32(b0 + "conv_0.conv.weight", (int64_t)k.c1 * K * K);
+    k.b1 = p.f32(b0 + "conv_0.conv.bias", k.c1);
+    p.norm(b0 + "norm_0.norm", (int64_t)F1 * k.c1, &k.g1, &k.be1);
+    const float* w2 = p.host(b1 + "conv_0.conv.weight", (int64_t)k.c2 * k.c1 * K * K);
+    const float *w3a = nullptr, *w3r = nullptr, *b3a = nullptr, *b3r = nullptr;
+    if (k.blocks == 3) {
+        w3a = p.host(b2 + "convs.conv_0.conv.weight", (int64_t)C * C);
+        w3r = p.host(b2 + "reduce_conv.conv.conv.weight", (int64_t)C * C);
+        b3a = p.host(b2 + "convs.conv_0.conv.bias", C);
+        b3r = p.host(b2 + "reduce_conv.conv.conv.bias", C);
+        if (!w3a || !w3r || !b3a || !b3r) return;
     }
+    if (!w2) return;
+    k.w2 = p.f16_raw(k.c1 == 256 ? conv_taps_kblocks_sw128(w2, k.c2, k.c1) : conv_taps_channel_last(w2, k.c2, k.c1, K));
+    k.b2 = p.f32(b1 + "conv_0.conv.bias", k.c2);
+    p.norm(b1 + "norm_0.norm", (int64_t)F2 * k.c2, &k.g2, &k.be2);
+    if (k.blocks != 3) return;
+    std::vector<float> w3((size_t)2 * C * C), b3(2 * C);  // [convs.conv_0 | reduce_conv.conv] output channels
+    memcpy(w3.data(), w3a, (size_t)C * C * 4);
+    memcpy(w3.data() + (size_t)C * C, w3r, (size_t)C * C * 4);
+    memcpy(b3.data(), b3a, C * 4);
+    memcpy(b3.data() + C, b3r, C * 4);
+    k.w3 = p.f32_raw(w3);
+    k.b3 = p.f32_raw(b3);
+    p.norm(b2 + "convs.norm_0.norm", (int64_t)F2 * C, &k.g3, &k.be3);
+    p.norm(b2 + "reduce_conv.norm.norm", (int64_t)F2 * C, &k.gr, &k.ber);
 }
 
 // mha_layer of a Conformer or Branchformer layer: RoPEMHA, or RelPosMHAXL with its linear_pos and position biases

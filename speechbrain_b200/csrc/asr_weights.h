@@ -65,10 +65,7 @@ struct AsrWeights {
     uint8_t* arena = nullptr;
     // frontend
     const float *glob_mean = nullptr, *glob_std = nullptr;
-    const float *c1_w = nullptr, *c1_b = nullptr, *c1_g = nullptr, *c1_be = nullptr;
-    const float *c2_b = nullptr, *c2_g = nullptr, *c2_be = nullptr;
-    const __half* c2_w = nullptr;
-    Cnn3Weights cnn3{};  // cfg.cnn_blocks == 3
+    CnnWeights cnn;
     // encoder
     const __half* w_in = nullptr; const float* b_in = nullptr;
     std::vector<EncLayerW> enc;

@@ -112,6 +112,33 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t& r0, uint32_t& r1, ui
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(smem_u32(p)));
 }
 
+// ---------------------------------------------------------------- mma.sync (warp MMA)
+// D[16 x 8] += A[16 x 16] * B[8 x 16]^T, fp16 in, fp32 accumulate; a: the four A registers, b0 / b1: the two B registers
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// ---------------------------------------------------------------- cp.async (global -> shared, bypassing registers)
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+// copies src_bytes (0 or 16) and zero-fills the rest of the 16 bytes: src_bytes 0 writes zeros without reading src
+__device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, uint32_t src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+// 8-byte copy through L1 (.cg takes 16-byte copies only)
+__device__ __forceinline__ void cp_async8(uint32_t dst, const void* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// generic-proxy writes to shared memory (cp.async, st.shared) made visible to the async proxy wgmma reads through
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -282,6 +309,11 @@ __device__ __forceinline__ __half2 floats2half2_sat(float lo, float hi) {
 __device__ __forceinline__ __half float2half_sat(float x) {
     const __half2 h = floats2half2_sat(x, 0.0f);
     return __low2half(h);
+}
+// the bits of floats2half2_sat(lo, hi), for 32-bit stores and mma operands
+__device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
+    const __half2 h = floats2half2_sat(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h);
 }
 
 // ---------------------------------------------------------------- misc math

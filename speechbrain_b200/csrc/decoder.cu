@@ -18,13 +18,6 @@
 
 namespace sbk {
 
-__device__ __forceinline__ void mma16816_d(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 // Programmatic dependent launch (common.cuh): every decode-step kernel lets its successor start launching immediately
 // and waits for its predecessor's memory only right before it touches activations, so launch latency and the
 // weight prefetch of kernel N+1 overlap the tail of kernel N.
@@ -177,7 +170,7 @@ __global__ void __launch_bounds__(SK_WARPS * 32, (VPL <= 4 ? 2 : 1)) skinny_gemm
 #pragma unroll
             for (int j = 0; j < NT; ++j)
 #pragma unroll
-                for (int mt = 0; mt < MT; ++mt) mma16816_d(acc[mt][j], af[u][mt], bf[u][j][0], bf[u][j][1]);
+                for (int mt = 0; mt < MT; ++mt) mma16816(acc[mt][j], af[u][mt], bf[u][j][0], bf[u][j][1]);
     }
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
@@ -577,11 +570,10 @@ __global__ void __launch_bounds__(XF_WARPS * 32, 2) dec_xatt_fold_kernel(const X
                 const int f = idx / (D / 8), v8 = idx % (D / 8);
                 const int t = blk * XF_FRAMES + f;
                 const __half* src = e + static_cast<size_t>(t < n_keys ? t : 0) * D + v8 * 8;
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst + f * SROW + v8 * 8)),
-                             "l"(src), "r"(t < n_keys ? 16 : 0));
+                cp_async16_zfill(smem_u32(dst + f * SROW + v8 * 8), src, t < n_keys ? 16u : 0u);
             }
         }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async_commit();
     };
 #pragma unroll
     for (int s = 0; s < XF_STAGES - 1; ++s) load_block(s);
@@ -599,7 +591,7 @@ __global__ void __launch_bounds__(XF_WARPS * 32, 2) dec_xatt_fold_kernel(const X
     for (int nt = 0; nt < NNT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.0f;
     float m_run = -INFINITY, l_run = 0.0f;
     for (int blk = 0; blk < n_blk; ++blk) {
-        asm volatile("cp.async.wait_group %0;" ::"n"(XF_STAGES - 2) : "memory");
+        cp_async_wait<XF_STAGES - 2>();
         __syncthreads();  // block blk landed for every thread; everyone is done with the stage and `red` reused below
         load_block(blk + XF_STAGES - 1);
         const __half* st = ring + static_cast<size_t>(blk % XF_STAGES) * XF_FRAMES * SROW + warp * KW;
@@ -614,8 +606,8 @@ __global__ void __launch_bounds__(XF_WARPS * 32, 2) dec_xatt_fold_kernel(const X
                 ldmatrix_x4(b0, b1, b2, b3, st + (8 * j + (lane & 7)) * SROW + 16 * ks + 8 * (lane >> 3));
                 const uint32_t a0[4] = {qa[ks][0], 0u, qa[ks][1], 0u};
                 const uint32_t a1[4] = {qa[ks + 1][0], 0u, qa[ks + 1][1], 0u};
-                mma16816_d(sp[j], a0, b0, b1);
-                mma16816_d(sp[j], a1, b2, b3);
+                mma16816(sp[j], a0, b0, b1);
+                mma16816(sp[j], a1, b2, b3);
             }
             *reinterpret_cast<float2*>(red + (warp * 8 + g) * XF_RED + 8 * j + 2 * c) = make_float2(sp[j][0], sp[j][1]);
         }
@@ -660,8 +652,8 @@ __global__ void __launch_bounds__(XF_WARPS * 32, 2) dec_xatt_fold_kernel(const X
             for (int nt = 0; nt < NNT; nt += 2) {
                 uint32_t b0, b1, b2, b3;
                 ldmatrix_x4_trans(b0, b1, b2, b3, st + (16 * ks + (lane & 15)) * SROW + 8 * nt + 8 * (lane >> 4));
-                mma16816_d(acc[nt], pa[ks], b0, b1);
-                mma16816_d(acc[nt + 1], pa[ks], b2, b3);
+                mma16816(acc[nt], pa[ks], b0, b1);
+                mma16816(acc[nt + 1], pa[ks], b2, b3);
             }
     }
     pdl_trigger();

@@ -630,16 +630,6 @@ __device__ __forceinline__ float ex2_ftz(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-    __half2 h = floats2half2_sat(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
 
 // STREAM: one chunk of a stream (AttStream): T is the window [cached rows; chunk rows], the queries are its last sa.nq rows
 // (from sa.q), keys / values come from the ring sa.kv, every key of the window is visible, and out holds the chunk's rows.
@@ -784,30 +774,26 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
             const bool ok = j0 + r < T;
             const __half* rowp = k_row(ok ? j0 + r : 0) + v8 * 8;
             const uint32_t nbytes = ok ? 16u : 0u;
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(kd + r * STR + v8 * 8)),
-                         "l"(rowp), "r"(nbytes) : "memory");
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(vd + r * STR + v8 * 8)),
-                         "l"(rowp + DH), "r"(nbytes) : "memory");
+            cp_async16_zfill(smem_u32(kd + r * STR + v8 * 8), rowp, nbytes);
+            cp_async16_zfill(smem_u32(vd + r * STR + v8 * 8), rowp + DH, nbytes);
         }
         if constexpr (RELPOS) {
             const int a = p_first(jb), n = jb == blk_begin ? ATT_PW : ATT_BK;
             for (int i = threadIdx.x; i < n * V8; i += blockDim.x) {
                 const int x = i / V8, v8 = i - x * V8;
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(Ps + p_slot(a + x) * STR + v8 * 8)),
-                             "l"(p_src(a + x) + v8 * 8) : "memory");
+                cp_async16(smem_u32(Ps + p_slot(a + x) * STR + v8 * 8), p_src(a + x) + v8 * 8);
             }
         }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async_commit();
     };
     // RELPOS without 16-byte rows: only the P rows go through cp.async, in 8-byte pieces, one key block ahead
     auto stage_p8 = [&](int jb) {
         const int a = p_first(jb), n = jb == blk_begin ? ATT_PW : ATT_BK;
         for (int i = threadIdx.x; i < n * VPR; i += blockDim.x) {
             const int x = i / VPR, v4 = i - x * VPR;
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(Ps + p_slot(a + x) * STR + v4 * 4)),
-                         "l"(p_src(a + x) + v4 * 4) : "memory");
+            cp_async8(smem_u32(Ps + p_slot(a + x) * STR + v4 * 4), p_src(a + x) + v4 * 4);
         }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async_commit();
     };
     if (n_blk > blk_begin) {
         if constexpr (ASYNC) stage_async(blk_begin, Ks, Vs);
@@ -820,7 +806,7 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
         const __half* Vc = Vs;
         if constexpr (KV2) {
             if ((jb - blk_begin) & 1) { Kc = KV1; Vc = KV1 + ATT_BK * STR; }
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            cp_async_wait<0>();
             __syncthreads();  // block jb has landed for everyone; block jb-1 (the other buffer) is fully consumed
             if (jb + 1 < n_blk) {
                 if ((jb - blk_begin) & 1) stage_async(jb + 1, Ks, Vs);
@@ -831,10 +817,10 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
                 __syncthreads();
                 stage_async(jb, Ks, Vs);
             }
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            cp_async_wait<0>();
             __syncthreads();  // block jb has landed for everyone
         } else {
-            if constexpr (RELPOS) asm volatile("cp.async.wait_group 0;" ::: "memory");
+            if constexpr (RELPOS) cp_async_wait<0>();
             __syncthreads();  // previous block's K/V fully consumed (RELPOS: block jb's P rows have landed for everyone)
             if constexpr (RELPOS) {
                 if (jb + 1 < n_blk) stage_p8(jb + 1);
@@ -1414,8 +1400,7 @@ lm_causal_attention_kernel(const __half* __restrict__ qkv, int s, int d, const i
     const int* tok = tokens + static_cast<size_t>(b) * s;
 
     auto cp16 = [](__half* dst, const __half* src, bool ok) {  // rows past the sequence are zero-filled
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(ok ? 16u : 0u)
-                     : "memory");
+        cp_async16_zfill(smem_u32(dst), src, ok ? 16u : 0u);
     };
     auto stage = [&](int jb, int buf) {  // key block jb -> buffer buf (one cp.async group)
         const int j0 = jb * LMA_B;
@@ -1430,7 +1415,7 @@ lm_causal_attention_kernel(const __half* __restrict__ qkv, int s, int d, const i
             const int j = j0 + threadIdx.x;
             s_masked[buf][threadIdx.x] = j >= s || tok[j] == pad_tok;
         }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async_commit();
     };
     for (int i = threadIdx.x; i < LMA_B * (DH / 8); i += blockDim.x) {  // Q rides in key block 0's group
         const int r = i / (DH / 8), v8 = i - r * (DH / 8);
@@ -1449,7 +1434,7 @@ lm_causal_attention_kernel(const __half* __restrict__ qkv, int s, int d, const i
 
     for (int jb = 0; jb <= qb; ++jb) {
         const int buf = jb & 1, j0 = jb * LMA_B;
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        cp_async_wait<0>();
         __syncthreads();  // block jb has landed for everyone; block jb-1 (the other buffer) is fully consumed
         if (jb + 1 <= qb) stage(jb + 1, buf ^ 1);
         if (jb == 0) {

@@ -400,11 +400,7 @@ static int run_transformer_layers(AsrModel* m, int B, int T, const int* enc_len,
 // The fused front-end of the configured ConvolutionFrontEnd: feats [B, T0, n_mels] -> b.a_in [B*T2, input_size] fp16
 // (+ cnn_out_f fp32 when set).
 static int run_cnn(AsrModel* m, const float* feats, int B, int T0, float* cnn_out_f, cudaStream_t st) {
-    const sbk_asr_config& c = m->wt->cfg;
-    const AsrWeights& W = *m->wt;
-    if (c.cnn_blocks == 3) return cnn3_frontend_forward(feats, B, T0, c.n_mels, W.cnn3, m->b.act1, m->b.a_in, cnn_out_f, st);
-    return cnn_frontend_forward(feats, B, T0, c.n_mels, W.c1_w, W.c1_b, W.c1_g, W.c1_be, c.cnn_c1, W.c2_w, W.c2_b, W.c2_g,
-                                W.c2_be, c.cnn_c2, m->b.act1, m->b.a_in, cnn_out_f, st);
+    return cnn_frontend_forward(feats, B, T0, m->wt->cfg.n_mels, m->wt->cnn, m->b.act1, m->b.a_in, cnn_out_f, st);
 }
 
 // One chunk-by-chunk stream (or a batch of B streams advancing together) of a Conformer encoder: per layer the attention's

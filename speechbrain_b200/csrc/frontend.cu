@@ -1,16 +1,24 @@
-// ConvolutionFrontEnd: 2 x [reflect-pad + Conv2d(3x3, stride 2) + LayerNorm(F', C) + LeakyReLU].
+// ConvolutionFrontEnd: 2 x [reflect-pad + Conv2d(3x3, stride 2) + LayerNorm(F', C) + LeakyReLU], or the Transformer
+// recipes' 3 blocks (5x5, 5x5, 1x1 with a residual 1x1).
 //
 // Replaces lobes/models/convolution.py:116-320 (ConvolutionFrontEnd / ConvBlock) with
 // nnet/CNN.py:654-751 (Conv2d.forward, "same" reflect padding k//2 for stride > 1) and
 // nnet/normalization.py:185-242 (LayerNorm over the last two dims), activation LeakyReLU(0.01).
 //
 // Layouts (channels-last, as the reference exposes them):
-//   feats [B, T0, F0] fp32 -> act1 [B, T1, F1, C1] fp16 -> act2 [B, T2, F2*C2] fp16 (+ fp32)
+//   feats [B, T0, F0] fp32 -> act1 [B, T1, F1, C1] fp16 -> out [B, T2, F2*C2] fp16 (+ fp32)
 //   T1 = (T0-1)/2+1, F1 = (F0-1)/2+1, likewise T2/F2.
-// conv1 (C_in = 1) is HBM/latency bound: one CTA per output frame, fused LN + LeakyReLU.
-// conv2 (C1 -> C2, K = 9*C1 = 576) is an implicit GEMM on mma.sync.m16n8k16 (fp16 in, fp32 accumulate);
-// the weight matrix and a 9-frame input patch live in shared memory; LN + LeakyReLU fused.
-// out_channels (256, 256) has kernels of its own (conv2 on wgmma), further down; cnn_frontend_forward picks by channels.
+// cnn_frontend_forward at the bottom makes every kernel choice from the weights' block count and channels.
+//
+// Each stage is written once and shared by the kernels that run it:
+//   conv1 (C_in = 1, K x K taps, K = 3 or 5): conv1_stage_rows / conv1_taps / conv1_frame / conv1_centred_sq /
+//     conv1_ln_pair.  A thread owns two channels of one frame in registers; conv1_warp_frame adds the warp-shuffle
+//     LayerNorm statistics.  conv1_ln_kernel (3x3) and conv1k5_ln_kernel (5x5) write act1 with one warp per frame,
+//     cnn_fused_kernel writes its frames into the conv2 patch in shared memory, conv1c256_ln_kernel reduces over 4 warps.
+//   conv2 (64 input channels, K = 9 or 25 taps x 64) is an implicit GEMM on mma.sync.m16n8k16 (fp16 in, fp32 accumulate)
+//     over a reflect-padded patch in shared memory (stage_patch, conv_tile_store); the 64 -> 32 conv2 of
+//     conv2_ln_kernel and cnn_fused_kernel is conv2_gemm + conv2_ln_store; the per-frame LayerNorm statistics are
+//     frame_ln_stats.  conv2c256_ln_kernel (256 -> 256) runs on wgmma.
 #include <algorithm>
 
 #include "common.cuh"
@@ -21,13 +29,119 @@ namespace sbk {
 __device__ __forceinline__ int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 __device__ __forceinline__ float leaky(float x) { return x > 0.0f ? x : 0.01f * x; }
 
-// --------------------------------------------------------------------------- conv1
-// w1: [C1, 3(kf), 3(kt)] fp32 (reference weight (C1,1,kf,kt)), b1: [C1]; g/be: [F1, C1].
-// One WARP per output frame (8 frames per CTA): lane l owns channels 2l, 2l+1 for all F1 feature rows, the frame's
-// F1 x C1 outputs stay in registers, so the LayerNorm over (F1, C1) needs only warp shuffles (no block barriers) and
-// every store is a 128-byte half2 row segment (instead of one 256-thread CTA per frame with three block barriers and
-// 2-byte stores).
+// --------------------------------------------------------------------------- conv1 stage
+// w1: [C1, K(kf), K(kt)] fp32 (reference weight (C1,1,kf,kt)), b1: [C1]; g/be: [F1, C1].  A thread owns channels c0, c0 + 1
+// for all F1 feature rows of one frame, so the frame's outputs stay in registers and every store is a half2.
+
+// in [K][F0 + K - 1] <- the K reflect-padded feature rows conv1 frame t1 reads; threads tid, tid + nthr, ...
+template <int K>
+__device__ __forceinline__ void conv1_stage_rows(float* in, const float* __restrict__ feats, int b, int t1, int T0, int F0,
+                                                 int tid, int nthr) {
+    const int FP = F0 + K - 1;
+    for (int i = tid; i < K * FP; i += nthr) {
+        const int kt = i / FP, fp = i - kt * FP;
+        const int t = reflect_idx(2 * t1 + kt - K / 2, T0);
+        const int f = reflect_idx(fp - K / 2, F0);
+        in[i] = __ldg(feats + (static_cast<size_t>(b) * T0 + t) * F0 + f);
+    }
+}
+
+template <int K>
+struct Conv1Taps {
+    float wa[K * K], wb[K * K], ba, bb;  // channels c0, c0 + 1
+};
+template <int K>
+__device__ __forceinline__ Conv1Taps<K> conv1_taps(const float* __restrict__ w1, const float* __restrict__ b1, int c0) {
+    Conv1Taps<K> w;
+#pragma unroll
+    for (int i = 0; i < K * K; ++i) { w.wa[i] = __ldg(w1 + c0 * K * K + i); w.wb[i] = __ldg(w1 + (c0 + 1) * K * K + i); }
+    w.ba = __ldg(b1 + c0);
+    w.bb = __ldg(b1 + c0 + 1);
+    return w;
+}
+
+// The channel pair's conv outputs at f1 < F1 into va / vb (0 beyond); returns their sum
+template <int K, int MAXF>
+__device__ __forceinline__ float conv1_frame(const float* in, int F0, int F1, const Conv1Taps<K>& w, float (&va)[MAXF],
+                                             float (&vb)[MAXF]) {
+    const int FP = F0 + K - 1;
+    float s = 0.0f;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1) {
+        va[f1] = 0.0f; vb[f1] = 0.0f;
+        if (f1 < F1) {
+            float a = w.ba, bq = w.bb;
+#pragma unroll
+            for (int kf = 0; kf < K; ++kf)
+#pragma unroll
+                for (int kt = 0; kt < K; ++kt) {
+                    const float x = in[kt * FP + 2 * f1 + kf];
+                    a = fmaf(w.wa[kf * K + kt], x, a);
+                    bq = fmaf(w.wb[kf * K + kt], x, bq);
+                }
+            va[f1] = a; vb[f1] = bq;
+            s += a + bq;
+        }
+    }
+    return s;
+}
+
+template <int MAXF>
+__device__ __forceinline__ float conv1_centred_sq(const float (&va)[MAXF], const float (&vb)[MAXF], int F1, float mean) {
+    float q = 0.0f;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1)
+        if (f1 < F1) {
+            const float da = va[f1] - mean, db = vb[f1] - mean;
+            q += da * da + db * db;
+        }
+    return q;
+}
+
+// LayerNorm (gamma / beta at gi = f1 * C1 + c0) + LeakyReLU of the channel pair (va, vb), as fp16
+__device__ __forceinline__ __half2 conv1_ln_pair(float va, float vb, float mean, float rstd, const float* __restrict__ gamma,
+                                                 const float* __restrict__ beta, int gi) {
+    const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + gi));
+    const float2 be = __ldg(reinterpret_cast<const float2*>(beta + gi));
+    return floats2half2_sat(leaky((va - mean) * rstd * g.x + be.x), leaky((vb - mean) * rstd * g.y + be.y));
+}
+
+// One warp computes 64-channel conv1 frame t1 (lane l: channels 2l, 2l+1) and its LayerNorm statistics over (F1, 64) with
+// warp shuffles only (no block barriers); in: this warp's [K][F0 + K - 1] staging rows.
+template <int K, int MAXF>
+__device__ __forceinline__ void conv1_warp_frame(float* in, const float* __restrict__ feats, int b, int t1, int T0, int F0,
+                                                 int F1, const float* __restrict__ w1, const float* __restrict__ b1,
+                                                 int lane, float (&va)[MAXF], float (&vb)[MAXF], float& mean, float& rstd) {
+    conv1_stage_rows<K>(in, feats, b, t1, T0, F0, lane, 32);
+    const Conv1Taps<K> w = conv1_taps<K>(w1, b1, 2 * lane);
+    __syncwarp();
+    const float n = static_cast<float>(F1 * 64);
+    mean = warp_sum(conv1_frame<K>(in, F0, F1, w, va, vb)) / n;
+    rstd = rsqrtf(warp_sum(conv1_centred_sq(va, vb, F1, mean)) / n + 1e-5f);
+}
+
+// One WARP per output frame (C1_WARPS frames per CTA) -> act1 [B, T1, F1, 64] fp16: every store is a 128-byte half2 row
+// segment (instead of one 256-thread CTA per frame with three block barriers and 2-byte stores).
 constexpr int C1_WARPS = 8;
+
+template <int K, int MAXF>
+__device__ __forceinline__ void conv1_warps_to_act1(float* smem, const float* __restrict__ feats, int T0, int F0, int T1,
+                                                    int F1, const float* __restrict__ w1, const float* __restrict__ b1,
+                                                    const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                    __half* __restrict__ out_h) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.y, t1 = blockIdx.x * C1_WARPS + warp;
+    if (t1 >= T1) return;
+    float va[MAXF], vb[MAXF], mean, rstd;
+    conv1_warp_frame<K>(smem + warp * K * (F0 + K - 1), feats, b, t1, T0, F0, F1, w1, b1, lane, va, vb, mean, rstd);
+    const size_t obase = (static_cast<size_t>(b) * T1 + t1) * F1 * 64;
+#pragma unroll
+    for (int f1 = 0; f1 < MAXF; ++f1)
+        if (f1 < F1) {
+            const int gi = f1 * 64 + 2 * lane;
+            *reinterpret_cast<__half2*>(out_h + obase + gi) = conv1_ln_pair(va[f1], vb[f1], mean, rstd, gamma, beta, gi);
+        }
+}
 
 template <int C1, int MAXF>
 __global__ void __launch_bounds__(C1_WARPS * 32)
@@ -36,192 +150,168 @@ conv1_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1,
                 __half* __restrict__ out_h) {
     static_assert(C1 == 64, "two channels per lane");
     extern __shared__ float c1_smem[];
-    const int FP = F0 + 2;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    float* in = c1_smem + warp * 3 * FP;  // [3][F0 + 2] of this warp's frame (reflect padded)
-    const int b = blockIdx.y, t1 = blockIdx.x * C1_WARPS + warp;
-    if (t1 >= T1) return;
-    for (int i = lane; i < 3 * FP; i += 32) {
-        const int kt = i / FP, fp = i - kt * FP;
-        const int t = reflect_idx(2 * t1 + kt - 1, T0);
-        const int f = reflect_idx(fp - 1, F0);
-        in[i] = __ldg(feats + (static_cast<size_t>(b) * T0 + t) * F0 + f);
+    conv1_warps_to_act1<3, MAXF>(c1_smem, feats, T0, F0, T1, F1, w1, b1, gamma, beta, out_h);
+}
+
+// block 1 of the 3-block front-end: w1 [64, 5(kf), 5(kt)]
+template <int MAXF>
+__global__ void __launch_bounds__(C1_WARPS * 32)
+conv1k5_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1, const float* __restrict__ w1,
+                  const float* __restrict__ b1, const float* __restrict__ gamma, const float* __restrict__ beta,
+                  __half* __restrict__ out_h) {
+    extern __shared__ float c1_smem[];
+    conv1_warps_to_act1<5, MAXF>(c1_smem, feats, T0, F0, T1, F1, w1, b1, gamma, beta, out_h);
+}
+
+// --------------------------------------------------------------------------- 64-channel conv2 stage (mma.sync)
+constexpr int CELL = 72;       // padded channel stride (halfs) of one (t, f) cell of a 64-channel patch in smem
+
+// patch [ROWS][F1 + K - 1][CELL] <- the reflect-padded act1 frames of the CTA's output frames from t0 (16-byte vectors)
+template <int K, int ROWS>
+__device__ __forceinline__ void stage_patch(__half* patch, const __half* __restrict__ act1, int b, int t0, int T1, int F1) {
+    const int FPAD = F1 + K - 1;
+    for (int i = threadIdx.x; i < ROWS * FPAD * 8; i += blockDim.x) {
+        const int cell = i / 8, v8 = i - cell * 8;
+        const int tr = cell / FPAD, fp = cell - tr * FPAD;
+        int t = reflect_idx(2 * t0 + tr - K / 2, T1);
+        t = min(max(t, 0), T1 - 1);  // tail tiles: keep loads in range (results discarded)
+        const int f = reflect_idx(fp - K / 2, F1);
+        *reinterpret_cast<uint4*>(patch + cell * CELL + v8 * 8) =
+            *reinterpret_cast<const uint4*>(act1 + ((static_cast<size_t>(b) * T1 + t) * F1 + f) * 64 + v8 * 8);
     }
-    const int c0 = 2 * lane;
-    float wa[9], wb[9];
+}
+
+// acc + bias -> out [rows][LD] fp32 at the warp's rows r0, r1 = r0 + 8 (those < rows)
+template <int NT, int LD>
+__device__ __forceinline__ void conv_tile_store(const float (&acc)[NT][4], const float* __restrict__ bias, float* out, int r0,
+                                                int r1, int rows, int c) {
 #pragma unroll
-    for (int i = 0; i < 9; ++i) { wa[i] = __ldg(w1 + c0 * 9 + i); wb[i] = __ldg(w1 + (c0 + 1) * 9 + i); }
-    const float ba = __ldg(b1 + c0), bb = __ldg(b1 + c0 + 1);
-    __syncwarp();
-    float va[MAXF], vb[MAXF];
+    for (int nt = 0; nt < NT; ++nt) {
+        const int col = nt * 8 + 2 * c;
+        const float bz0 = __ldg(bias + col), bz1 = __ldg(bias + col + 1);
+        if (r0 < rows) { out[r0 * LD + col] = acc[nt][0] + bz0; out[r0 * LD + col + 1] = acc[nt][1] + bz1; }
+        if (r1 < rows) { out[r1 * LD + col] = acc[nt][2] + bz0; out[r1 * LD + col + 1] = acc[nt][3] + bz1; }
+    }
+}
+
+// LayerNorm statistics over the n = F2 * C values of one frame held in smem rows [F2][stride] (C channels each); one warp
+template <int C>
+__device__ __forceinline__ void frame_ln_stats(const float* src, int stride, int n, int lane, float& mean, float& rstd) {
+    constexpr int LOG_C = C == 32 ? 5 : 6;
+    static_assert(C == 1 << LOG_C, "32 or 64 channels per pixel");
     float s = 0.0f;
+    for (int i = lane; i < n; i += 32) s += src[(i >> LOG_C) * stride + (i & (C - 1))];
+    mean = warp_sum(s) / n;
+    float q = 0.0f;
+    for (int i = lane; i < n; i += 32) {
+        const float d = src[(i >> LOG_C) * stride + (i & (C - 1))] - mean;
+        q += d * d;
+    }
+    rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
+}
+
+// conv2 64 -> 32: act1 [B, T1, F1, 64] fp16; w2p [32, 576] fp16 with k = (kf*3+kt)*64 + ch; out [B, T2, F2*32].
+// A CTA computes C2_FRAMES output frames from a 9-frame patch; the weight matrix lives in shared memory too.
+constexpr int C2_FRAMES = 4;   // output frames per CTA
+constexpr int C2_PROWS = 2 * C2_FRAMES + 1;  // act1 frames of the patch
+constexpr int C2_COUT = 32;
+constexpr int C2_WROW = 9 * 64 + 8;  // padded weight row (halfs)
+constexpr int C2_LD = C2_COUT + 1;   // fp32 row stride of cbuf
+
+__device__ __forceinline__ void conv2_stage_weights(__half* wsm, const __half* __restrict__ w2p) {
+    for (int i = threadIdx.x; i < C2_COUT * (9 * 64 / 8); i += blockDim.x) {
+        const int o = i / (9 * 64 / 8), v8 = i - o * (9 * 64 / 8);
+        *reinterpret_cast<uint4*>(wsm + o * C2_WROW + v8 * 8) =
+            *reinterpret_cast<const uint4*>(w2p + static_cast<size_t>(o) * 9 * 64 + v8 * 8);
+    }
+}
+
+// The implicit GEMM over patch [C2_PROWS][F1 + 2][CELL] and wsm [32][C2_WROW]: warp w computes GEMM rows 16 w .. 16 w + 15
+// (row r = frame r / F2, pixel r % F2) and stores them + bias into cbuf [C2_FRAMES * F2][C2_LD].
+__device__ __forceinline__ void conv2_gemm(const __half* patch, const __half* wsm, int F1, int F2, const float* __restrict__ b2,
+                                           float* cbuf, int warp, int lane) {
+    const int FPAD = F1 + 2, rows = C2_FRAMES * F2;
+    const int g = lane >> 2, c = lane & 3;
+    const int r0 = warp * 16 + g, r1 = r0 + 8;
+    if (warp * 16 >= rows) return;
+    float acc[4][4];
 #pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1) {
-        va[f1] = 0.0f; vb[f1] = 0.0f;
-        if (f1 < F1) {
-            float a = ba, bq = bb;
+    for (int i = 0; i < 4; ++i)
 #pragma unroll
-            for (int kf = 0; kf < 3; ++kf)
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+    const int rr0 = min(r0, rows - 1), rr1 = min(r1, rows - 1);
+    const int fr0 = rr0 / F2, f20 = rr0 - fr0 * F2;
+    const int fr1 = rr1 / F2, f21 = rr1 - fr1 * F2;
+#pragma unroll 1
+    for (int tap = 0; tap < 9; ++tap) {
+        const int kf = tap / 3, kt = tap - kf * 3;
+        const __half* a0p = patch + ((2 * fr0 + kt) * FPAD + 2 * f20 + kf) * CELL + 2 * c;
+        const __half* a1p = patch + ((2 * fr1 + kt) * FPAD + 2 * f21 + kf) * CELL + 2 * c;
 #pragma unroll
-                for (int kt = 0; kt < 3; ++kt) {
-                    const float x = in[kt * FP + 2 * f1 + kf];
-                    a = fmaf(wa[kf * 3 + kt], x, a);
-                    bq = fmaf(wb[kf * 3 + kt], x, bq);
-                }
-            va[f1] = a; vb[f1] = bq;
-            s += a + bq;
+        for (int ks = 0; ks < 4; ++ks) {
+            uint32_t a[4];
+            a[0] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16);
+            a[1] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16);
+            a[2] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16 + 8);
+            a[3] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16 + 8);
+            const int kk = tap * 64 + ks * 16 + 2 * c;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                const __half* wp = wsm + (nt * 8 + g) * C2_WROW + kk;
+                mma16816(acc[nt], a, *reinterpret_cast<const uint32_t*>(wp), *reinterpret_cast<const uint32_t*>(wp + 8));
+            }
         }
     }
-    const float n = static_cast<float>(F1 * C1);
-    const float mean = warp_sum(s) / n;
-    float q = 0.0f;
-#pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1)
-        if (f1 < F1) {
-            const float da = va[f1] - mean, db = vb[f1] - mean;
-            q += da * da + db * db;
-        }
-    const float rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
-    const size_t obase = (static_cast<size_t>(b) * T1 + t1) * F1 * C1;
-#pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1)
-        if (f1 < F1) {
-            const int gi = f1 * C1 + c0;
-            const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + gi));
-            const float2 be = __ldg(reinterpret_cast<const float2*>(beta + gi));
-            const float y0 = leaky((va[f1] - mean) * rstd * g.x + be.x);
-            const float y1 = leaky((vb[f1] - mean) * rstd * g.y + be.y);
-            *reinterpret_cast<__half2*>(out_h + obase + gi) = floats2half2_sat(y0, y1);
-        }
+    conv_tile_store<4, C2_LD>(acc, b2, cbuf, r0, r1, rows, c);
 }
 
-// --------------------------------------------------------------------------- conv2
-__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+// LayerNorm over (F2, 32) + LeakyReLU of output frame t0 + warp (one warp per frame) from cbuf -> out
+__device__ __forceinline__ void conv2_ln_store(const float* cbuf, int b, int t0, int T2, int F2, const float* __restrict__ gamma,
+                                               const float* __restrict__ beta, __half* __restrict__ out_h,
+                                               float* __restrict__ out_f, int warp, int lane) {
+    if (warp >= C2_FRAMES) return;
+    const int t = t0 + warp;
+    if (t >= T2) return;
+    const int n = F2 * C2_COUT;
+    const float* src = cbuf + warp * F2 * C2_LD;
+    float mean, rstd;
+    frame_ln_stats<C2_COUT>(src, C2_LD, n, lane, mean, rstd);
+    const size_t ob = (static_cast<size_t>(b) * T2 + t) * n;
+    for (int i = lane; i < n; i += 32) {
+        const float y = leaky((src[(i >> 5) * C2_LD + (i & 31)] - mean) * rstd * __ldg(gamma + i) + __ldg(beta + i));
+        out_h[ob + i] = float2half_sat(y);
+        if (out_f) out_f[ob + i] = y;
+    }
 }
 
-constexpr int C2_FRAMES = 4;   // output frames per CTA
-constexpr int C2_CIN = 64;     // input channels (k16 steps per tap = 4)
-constexpr int C2_COUT = 32;
-constexpr int C2_CELL = 72;    // padded channel stride (halfs) of one (t, f) cell in smem
-constexpr int C2_WROW = 9 * C2_CIN + 8;  // padded weight row (halfs)
-
-// act1 [B, T1, F1, 64] fp16; w2p [32, 576] fp16 with k = (kf*3+kt)*64 + ch; out [B, T2, F2*32].
 // Requires F2 * C2_FRAMES <= 16 * n_warps (launch with ceil(F2*4/16) warps) and F2 * 32 <= 1024.
 __global__ void __launch_bounds__(192)
 conv2_ln_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int F2, const __half* __restrict__ w2p,
                 const float* __restrict__ b2, const float* __restrict__ gamma, const float* __restrict__ beta,
                 __half* __restrict__ out_h, float* __restrict__ out_f) {
     extern __shared__ __align__(16) uint8_t c2_smem[];
-    const int FPAD = F1 + 2;
-    const int n_trows = 2 * C2_FRAMES + 1;
-    __half* patch = reinterpret_cast<__half*>(c2_smem);                 // [n_trows][FPAD][C2_CELL]
-    __half* wsm = patch + n_trows * FPAD * C2_CELL;                     // [32][C2_WROW]
-    float* cbuf = reinterpret_cast<float*>(wsm + C2_COUT * C2_WROW);    // [C2_FRAMES * F2][33]
+    __half* patch = reinterpret_cast<__half*>(c2_smem);                 // [C2_PROWS][F1 + 2][CELL]
+    __half* wsm = patch + C2_PROWS * (F1 + 2) * CELL;                   // [32][C2_WROW]
+    float* cbuf = reinterpret_cast<float*>(wsm + C2_COUT * C2_WROW);    // [C2_FRAMES * F2][C2_LD]
     const int b = blockIdx.y, t0 = blockIdx.x * C2_FRAMES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    // stage the input patch (reflect-padded) : 16-byte vectors of 8 channels
-    const int vec_per_cell = C2_CIN / 8;
-    for (int i = threadIdx.x; i < n_trows * FPAD * vec_per_cell; i += blockDim.x) {
-        const int cell = i / vec_per_cell, v8 = i - cell * vec_per_cell;
-        const int tr = cell / FPAD, fp = cell - tr * FPAD;
-        int t = reflect_idx(2 * t0 + tr - 1, T1);
-        t = min(max(t, 0), T1 - 1);  // tail tiles: keep loads in range (results discarded)
-        const int f = reflect_idx(fp - 1, F1);
-        const uint4 val =
-            *reinterpret_cast<const uint4*>(act1 + ((static_cast<size_t>(b) * T1 + t) * F1 + f) * C2_CIN + v8 * 8);
-        *reinterpret_cast<uint4*>(patch + cell * C2_CELL + v8 * 8) = val;
-    }
-    for (int i = threadIdx.x; i < C2_COUT * (9 * C2_CIN / 8); i += blockDim.x) {
-        const int o = i / (9 * C2_CIN / 8), v8 = i - o * (9 * C2_CIN / 8);
-        *reinterpret_cast<uint4*>(wsm + o * C2_WROW + v8 * 8) =
-            *reinterpret_cast<const uint4*>(w2p + static_cast<size_t>(o) * 9 * C2_CIN + v8 * 8);
-    }
+    stage_patch<3, C2_PROWS>(patch, act1, b, t0, T1, F1);
+    conv2_stage_weights(wsm, w2p);
     __syncthreads();
-
-    const int rows = C2_FRAMES * F2;
-    const int g = lane >> 2, c = lane & 3;
-    const int r0 = warp * 16 + g, r1 = r0 + 8;
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
-    if (warp * 16 < rows) {
-        const int rr0 = min(r0, rows - 1), rr1 = min(r1, rows - 1);
-        const int fr0 = rr0 / F2, f20 = rr0 - fr0 * F2;
-        const int fr1 = rr1 / F2, f21 = rr1 - fr1 * F2;
-#pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) {
-            const int kf = tap / 3, kt = tap - kf * 3;
-            const __half* a0p = patch + ((2 * fr0 + kt) * FPAD + 2 * f20 + kf) * C2_CELL + 2 * c;
-            const __half* a1p = patch + ((2 * fr1 + kt) * FPAD + 2 * f21 + kf) * C2_CELL + 2 * c;
-#pragma unroll
-            for (int ks = 0; ks < C2_CIN / 16; ++ks) {
-                uint32_t a[4];
-                a[0] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16);
-                a[1] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16);
-                a[2] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16 + 8);
-                a[3] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16 + 8);
-                const int kk = tap * C2_CIN + ks * 16 + 2 * c;
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    uint32_t bb[2];
-                    const __half* wp = wsm + (nt * 8 + g) * C2_WROW + kk;
-                    bb[0] = *reinterpret_cast<const uint32_t*>(wp);
-                    bb[1] = *reinterpret_cast<const uint32_t*>(wp + 8);
-                    mma_16816(acc[nt], a, bb);
-                }
-            }
-        }
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-            const int col = nt * 8 + 2 * c;
-            const float bz0 = __ldg(b2 + col), bz1 = __ldg(b2 + col + 1);
-            if (r0 < rows) { cbuf[r0 * 33 + col] = acc[nt][0] + bz0; cbuf[r0 * 33 + col + 1] = acc[nt][1] + bz1; }
-            if (r1 < rows) { cbuf[r1 * 33 + col] = acc[nt][2] + bz0; cbuf[r1 * 33 + col + 1] = acc[nt][3] + bz1; }
-        }
-    }
+    conv2_gemm(patch, wsm, F1, F2, b2, cbuf, warp, lane);
     __syncthreads();
-    // LayerNorm over (F2, 32) per frame + LeakyReLU; one warp per frame
-    if (warp < C2_FRAMES) {
-        const int t = t0 + warp;
-        if (t < T2) {
-            const int n = F2 * C2_COUT;
-            const float* src = cbuf + warp * F2 * 33;
-            float s = 0.0f;
-            for (int i = lane; i < n; i += 32) s += src[(i >> 5) * 33 + (i & 31)];
-            const float mean = warp_sum(s) / n;
-            float q = 0.0f;
-            for (int i = lane; i < n; i += 32) {
-                const float d = src[(i >> 5) * 33 + (i & 31)] - mean;
-                q += d * d;
-            }
-            const float rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
-            const size_t ob = (static_cast<size_t>(b) * T2 + t) * n;
-            for (int i = lane; i < n; i += 32) {
-                const float y = leaky((src[(i >> 5) * 33 + (i & 31)] - mean) * rstd * __ldg(gamma + i) + __ldg(beta + i));
-                out_h[ob + i] = float2half_sat(y);
-                if (out_f) out_f[ob + i] = y;
-            }
-        }
-    }
+    conv2_ln_store(cbuf, b, t0, T2, F2, gamma, beta, out_h, out_f, warp, lane);
 }
 
-
 // --------------------------------------------------------------------------- conv1 + conv2 fused
-// The two-kernel version wrote conv1's output (B x T1 x F1 x 64 fp16 = 82 MB per 32 x 10 s batch) to global memory and read
-// it back: conv2 was bound by those 82 MB of DRAM reads at low occupancy.
+// The two-kernel version writes conv1's output (B x T1 x F1 x 64 fp16 = 82 MB per 32 x 10 s batch) to global memory and
+// reads it back: conv2 is bound by those 82 MB of DRAM reads at low occupancy.
 // Here one CTA produces C2_FRAMES output frames from the input features directly: its 9 warps each compute one conv1 frame
 // (3x3 conv, LayerNorm over (F1, 64), LeakyReLU) with the frame held in registers, and write it -- fp16, reflect columns
 // included -- straight into the shared-memory patch the implicit-GEMM conv2 reads.  Global traffic per batch: the 10 MB of
-// features (re-read ~2.3x through L2) + the 10 MB output instead of 2 x 82 MB.  Same arithmetic as the two kernels
-// (conv1 fp32 -> LN -> fp16; conv2 fp16 operands, fp32 accumulate), so the results are bit-identical to them.
-constexpr int CF_WARPS = 2 * C2_FRAMES + 1;  // one per conv1 frame of the patch
+// features (re-read ~2.3x through L2) + the 10 MB output instead of 2 x 82 MB.  Same stage code as the two kernels, so the
+// results are bit-identical to them.
+constexpr int CF_WARPS = C2_PROWS;  // one per conv1 frame of the patch
 
 template <int MAXF>
 __global__ void __launch_bounds__(CF_WARPS * 32, 2)
@@ -230,153 +320,38 @@ cnn_fused_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1
                  const __half* __restrict__ w2p, const float* __restrict__ b2, const float* __restrict__ g2,
                  const float* __restrict__ be2, __half* __restrict__ out_h, float* __restrict__ out_f) {
     extern __shared__ __align__(16) uint8_t c2_smem[];
-    constexpr int C1 = C2_CIN;
-    const int FPAD = F1 + 2, FP0 = F0 + 2;
-    constexpr int n_trows = CF_WARPS;
-    __half* patch = reinterpret_cast<__half*>(c2_smem);                 // [n_trows][FPAD][C2_CELL]
-    __half* wsm = patch + n_trows * FPAD * C2_CELL;                     // [32][C2_WROW]
-    float* cbuf = reinterpret_cast<float*>(wsm + C2_COUT * C2_WROW);    // [C2_FRAMES * F2][33]
-    float* in_all = cbuf + C2_FRAMES * F2 * 33;                         // [CF_WARPS][3][F0 + 2]
+    const int FPAD = F1 + 2;
+    __half* patch = reinterpret_cast<__half*>(c2_smem);                 // [C2_PROWS][FPAD][CELL]
+    __half* wsm = patch + C2_PROWS * FPAD * CELL;                       // [32][C2_WROW]
+    float* cbuf = reinterpret_cast<float*>(wsm + C2_COUT * C2_WROW);    // [C2_FRAMES * F2][C2_LD]
+    float* in_all = cbuf + C2_FRAMES * F2 * C2_LD;                      // [CF_WARPS][3][F0 + 2]
     const int b = blockIdx.y, t0 = blockIdx.x * C2_FRAMES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    // conv2 weights -> shared memory (independent of everything else: issued first)
-    for (int i = threadIdx.x; i < C2_COUT * (9 * C2_CIN / 8); i += blockDim.x) {
-        const int o = i / (9 * C2_CIN / 8), v8 = i - o * (9 * C2_CIN / 8);
-        *reinterpret_cast<uint4*>(wsm + o * C2_WROW + v8 * 8) =
-            *reinterpret_cast<const uint4*>(w2p + static_cast<size_t>(o) * 9 * C2_CIN + v8 * 8);
-    }
+    conv2_stage_weights(wsm, w2p);  // independent of everything else: issued first
     // ---- stage 1: warp `warp` computes conv1 frame t1 = reflect(2 t0 + warp - 1) into patch row `warp`
     {
         int t1 = reflect_idx(2 * t0 + warp - 1, T1);
         t1 = min(max(t1, 0), T1 - 1);  // tail tiles: keep loads in range (results discarded)
-        float* in = in_all + warp * 3 * FP0;
-        for (int i = lane; i < 3 * FP0; i += 32) {
-            const int kt = i / FP0, fp = i - kt * FP0;
-            const int t = reflect_idx(2 * t1 + kt - 1, T0);
-            const int f = reflect_idx(fp - 1, F0);
-            in[i] = __ldg(feats + (static_cast<size_t>(b) * T0 + t) * F0 + f);
-        }
+        float va[MAXF], vb[MAXF], mean, rstd;
+        conv1_warp_frame<3>(in_all + warp * 3 * (F0 + 2), feats, b, t1, T0, F0, F1, w1, b1, lane, va, vb, mean, rstd);
         const int c0 = 2 * lane;
-        float wa[9], wb[9];
-#pragma unroll
-        for (int i = 0; i < 9; ++i) { wa[i] = __ldg(w1 + c0 * 9 + i); wb[i] = __ldg(w1 + (c0 + 1) * 9 + i); }
-        const float ba = __ldg(b1 + c0), bb = __ldg(b1 + c0 + 1);
-        __syncwarp();
-        float va[MAXF], vb[MAXF];
-        float s = 0.0f;
-#pragma unroll
-        for (int f1 = 0; f1 < MAXF; ++f1) {
-            va[f1] = 0.0f; vb[f1] = 0.0f;
-            if (f1 < F1) {
-                float a = ba, bq = bb;
-#pragma unroll
-                for (int kf = 0; kf < 3; ++kf)
-#pragma unroll
-                    for (int kt = 0; kt < 3; ++kt) {
-                        const float x = in[kt * FP0 + 2 * f1 + kf];
-                        a = fmaf(wa[kf * 3 + kt], x, a);
-                        bq = fmaf(wb[kf * 3 + kt], x, bq);
-                    }
-                va[f1] = a; vb[f1] = bq;
-                s += a + bq;
-            }
-        }
-        const float n = static_cast<float>(F1 * C1);
-        const float mean = warp_sum(s) / n;
-        float q = 0.0f;
+        __half* prow = patch + static_cast<size_t>(warp) * FPAD * CELL;
 #pragma unroll
         for (int f1 = 0; f1 < MAXF; ++f1)
             if (f1 < F1) {
-                const float da = va[f1] - mean, db = vb[f1] - mean;
-                q += da * da + db * db;
-            }
-        const float rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
-        __half* prow = patch + static_cast<size_t>(warp) * FPAD * C2_CELL;
-#pragma unroll
-        for (int f1 = 0; f1 < MAXF; ++f1)
-            if (f1 < F1) {
-                const int gi = f1 * C1 + c0;
-                const float2 g = __ldg(reinterpret_cast<const float2*>(g1 + gi));
-                const float2 be = __ldg(reinterpret_cast<const float2*>(be1 + gi));
-                const __half2 y = floats2half2_sat(leaky((va[f1] - mean) * rstd * g.x + be.x),
-                                                   leaky((vb[f1] - mean) * rstd * g.y + be.y));
-                *reinterpret_cast<__half2*>(prow + (f1 + 1) * C2_CELL + c0) = y;
+                const __half2 y = conv1_ln_pair(va[f1], vb[f1], mean, rstd, g1, be1, f1 * 64 + c0);
+                *reinterpret_cast<__half2*>(prow + (f1 + 1) * CELL + c0) = y;
                 // reflect padding of the feature axis: column -1 mirrors f1 = 1, column F1 mirrors f1 = F1 - 2
                 if (f1 == 1) *reinterpret_cast<__half2*>(prow + c0) = y;
-                if (f1 == F1 - 2) *reinterpret_cast<__half2*>(prow + (F1 + 1) * C2_CELL + c0) = y;
+                if (f1 == F1 - 2) *reinterpret_cast<__half2*>(prow + (F1 + 1) * CELL + c0) = y;
             }
     }
     __syncthreads();
-
-    // ---- stage 2: conv2 as an implicit GEMM over the patch (identical to conv2_ln_kernel from here on)
-    const int rows = C2_FRAMES * F2;
-    const int g = lane >> 2, c = lane & 3;
-    const int r0 = warp * 16 + g, r1 = r0 + 8;
-    if (warp * 16 < rows) {
-        float acc[4][4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
-        const int rr0 = min(r0, rows - 1), rr1 = min(r1, rows - 1);
-        const int fr0 = rr0 / F2, f20 = rr0 - fr0 * F2;
-        const int fr1 = rr1 / F2, f21 = rr1 - fr1 * F2;
-#pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) {
-            const int kf = tap / 3, kt = tap - kf * 3;
-            const __half* a0p = patch + ((2 * fr0 + kt) * FPAD + 2 * f20 + kf) * C2_CELL + 2 * c;
-            const __half* a1p = patch + ((2 * fr1 + kt) * FPAD + 2 * f21 + kf) * C2_CELL + 2 * c;
-#pragma unroll
-            for (int ks = 0; ks < C2_CIN / 16; ++ks) {
-                uint32_t a[4];
-                a[0] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16);
-                a[1] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16);
-                a[2] = *reinterpret_cast<const uint32_t*>(a0p + ks * 16 + 8);
-                a[3] = *reinterpret_cast<const uint32_t*>(a1p + ks * 16 + 8);
-                const int kk = tap * C2_CIN + ks * 16 + 2 * c;
-#pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    uint32_t bb[2];
-                    const __half* wp = wsm + (nt * 8 + g) * C2_WROW + kk;
-                    bb[0] = *reinterpret_cast<const uint32_t*>(wp);
-                    bb[1] = *reinterpret_cast<const uint32_t*>(wp + 8);
-                    mma_16816(acc[nt], a, bb);
-                }
-            }
-        }
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-            const int col = nt * 8 + 2 * c;
-            const float bz0 = __ldg(b2 + col), bz1 = __ldg(b2 + col + 1);
-            if (r0 < rows) { cbuf[r0 * 33 + col] = acc[nt][0] + bz0; cbuf[r0 * 33 + col + 1] = acc[nt][1] + bz1; }
-            if (r1 < rows) { cbuf[r1 * 33 + col] = acc[nt][2] + bz0; cbuf[r1 * 33 + col + 1] = acc[nt][3] + bz1; }
-        }
-    }
+    // ---- stage 2: conv2 as an implicit GEMM over the patch, then the per-frame LayerNorm
+    conv2_gemm(patch, wsm, F1, F2, b2, cbuf, warp, lane);
     __syncthreads();
-    // LayerNorm over (F2, 32) per frame + LeakyReLU; one warp per frame
-    if (warp < C2_FRAMES) {
-        const int t = t0 + warp;
-        if (t < T2) {
-            const int n = F2 * C2_COUT;
-            const float* src = cbuf + warp * F2 * 33;
-            float s = 0.0f;
-            for (int i = lane; i < n; i += 32) s += src[(i >> 5) * 33 + (i & 31)];
-            const float mean = warp_sum(s) / n;
-            float q = 0.0f;
-            for (int i = lane; i < n; i += 32) {
-                const float d = src[(i >> 5) * 33 + (i & 31)] - mean;
-                q += d * d;
-            }
-            const float rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
-            const size_t ob = (static_cast<size_t>(b) * T2 + t) * n;
-            for (int i = lane; i < n; i += 32) {
-                const float y = leaky((src[(i >> 5) * 33 + (i & 31)] - mean) * rstd * __ldg(g2 + i) + __ldg(be2 + i));
-                out_h[ob + i] = float2half_sat(y);
-                if (out_f) out_f[ob + i] = y;
-            }
-        }
-    }
+    conv2_ln_store(cbuf, b, t0, T2, F2, g2, be2, out_h, out_f, warp, lane);
 }
 
 // =========================================================================== 256-channel 2-block front-end (AISHELL-1)
@@ -406,7 +381,7 @@ constexpr int W2_THREADS = W2_CONSUMERS + 32;
 static_assert(W2_STAGE_BYTES % 1024 == 0 && W2_BM * W2_STG_PITCH <= W2_BAR_OFFSET, "ring layout");
 static_assert(W2_LAG <= W2_STAGES - 2, "the producer must mark stage kb full before it waits for stage kb + 2 to drain");
 
-// w1: [256, 3(kf), 3(kt)] fp32, g/be: [F1, 256].  Same arithmetic per value as conv1_ln_kernel.
+// w1: [256, 3(kf), 3(kt)] fp32, g/be: [F1, 256].  The conv1 stage above, with the LayerNorm sums reduced over 4 warps.
 template <int MAXF>
 __global__ void __launch_bounds__(W1_THREADS)
 conv1c256_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1, const float* __restrict__ w1,
@@ -414,53 +389,19 @@ conv1c256_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int
                     __half* __restrict__ out_h) {
     extern __shared__ float w1_in[];  // [3][F0 + 2] of the frame (reflect padded)
     __shared__ float red[2][W1_THREADS / 32];
-    const int FP = F0 + 2;
     const int t1 = blockIdx.x, b = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < 3 * FP; i += W1_THREADS) {
-        const int kt = i / FP, fp = i - kt * FP;
-        const int t = reflect_idx(2 * t1 + kt - 1, T0);
-        const int f = reflect_idx(fp - 1, F0);
-        w1_in[i] = __ldg(feats + (static_cast<size_t>(b) * T0 + t) * F0 + f);
-    }
+    conv1_stage_rows<3>(w1_in, feats, b, t1, T0, F0, threadIdx.x, W1_THREADS);
     const int c0 = 2 * threadIdx.x;
-    float wa[9], wb[9];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) { wa[i] = __ldg(w1 + c0 * 9 + i); wb[i] = __ldg(w1 + (c0 + 1) * 9 + i); }
-    const float ba = __ldg(b1 + c0), bb = __ldg(b1 + c0 + 1);
+    const Conv1Taps<3> w = conv1_taps<3>(w1, b1, c0);
     __syncthreads();
     float va[MAXF], vb[MAXF];
-    float s = 0.0f;
-#pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1) {
-        va[f1] = 0.0f; vb[f1] = 0.0f;
-        if (f1 < F1) {
-            float a = ba, bq = bb;
-#pragma unroll
-            for (int kf = 0; kf < 3; ++kf)
-#pragma unroll
-                for (int kt = 0; kt < 3; ++kt) {
-                    const float x = w1_in[kt * FP + 2 * f1 + kf];
-                    a = fmaf(wa[kf * 3 + kt], x, a);
-                    bq = fmaf(wb[kf * 3 + kt], x, bq);
-                }
-            va[f1] = a; vb[f1] = bq;
-            s += a + bq;
-        }
-    }
     const float n = static_cast<float>(F1 * W_C);
-    s = warp_sum(s);
+    const float s = warp_sum(conv1_frame<3>(w1_in, F0, F1, w, va, vb));
     if (lane == 0) red[0][warp] = s;
     __syncthreads();
     const float mean = (red[0][0] + red[0][1] + red[0][2] + red[0][3]) / n;
-    float q = 0.0f;
-#pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1)
-        if (f1 < F1) {
-            const float da = va[f1] - mean, db = vb[f1] - mean;
-            q += da * da + db * db;
-        }
-    q = warp_sum(q);
+    const float q = warp_sum(conv1_centred_sq(va, vb, F1, mean));
     if (lane == 0) red[1][warp] = q;
     __syncthreads();
     const float rstd = rsqrtf((red[1][0] + red[1][1] + red[1][2] + red[1][3]) / n + 1e-5f);
@@ -469,22 +410,9 @@ conv1c256_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int
     for (int f1 = 0; f1 < MAXF; ++f1)
         if (f1 < F1) {
             const int gi = f1 * W_C + c0;
-            const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + gi));
-            const float2 be = __ldg(reinterpret_cast<const float2*>(beta + gi));
-            const float y0 = leaky((va[f1] - mean) * rstd * g.x + be.x);
-            const float y1 = leaky((vb[f1] - mean) * rstd * g.y + be.y);
-            *reinterpret_cast<__half2*>(out_h + obase + gi) = floats2half2_sat(y0, y1);
+            *reinterpret_cast<__half2*>(out_h + obase + gi) = conv1_ln_pair(va[f1], vb[f1], mean, rstd, gamma, beta, gi);
         }
 }
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-// generic-proxy writes to shared memory (cp.async, st.shared) made visible to the async proxy wgmma reads through
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // act1 [B, T1, F1, 256] fp16; w2s: W2_KB k-blocks of [256 out][64 k] fp16, each the 128B-swizzled image a stage holds
 // (k = (kf * 3 + kt) * 256 + ch); frames = W2_BM / F2 output frames per CTA; out [B, T2, F2 * 256].
@@ -637,70 +565,11 @@ conv2c256_ln_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
     }
 }
 
-static int cnn256_frontend_forward(const float* feats, int B, int T0, int F0, const float* w1, const float* b1,
-                                   const float* g1, const float* be1, const __half* w2s, const float* b2, const float* g2,
-                                   const float* be2, __half* act1_h, __half* out_h, float* out_f, cudaStream_t stream) {
-    // the reference's reflect padding of 1 needs 2 rows / columns at both strided convolutions
-    SBK_REQUIRE(T0 >= 3 && F0 >= 3, "cnn_frontend: the 3x3 reflect padding needs at least 3 frames and 3 features "
-                "(got %d frames, %d features)", T0, F0);
-    const int T1 = (T0 - 1) / 2 + 1, F1 = (F0 - 1) / 2 + 1;
-    const int T2 = (T1 - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
-    SBK_REQUIRE(F1 <= 40, "cnn_frontend: out_channels=(256, 256) is built for up to 80 features (F0=%d)", F0);
-    conv1c256_ln_kernel<40><<<dim3(T1, B), W1_THREADS, 3 * (F0 + 2) * sizeof(float), stream>>>(
-        feats, T0, F0, T1, F1, w1, b1, g1, be1, act1_h);
-    SBK_LAUNCH_CHECK();
-    const int frames = W2_BM / F2;
-    SBK_CUDA_CHECK(cudaFuncSetAttribute(conv2c256_ln_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM));
-    conv2c256_ln_kernel<<<dim3(ceil_div(T2, frames), B), W2_THREADS, W2_SMEM, stream>>>(
-        act1_h, T1, F1, T2, F2, frames, w2s, b2, g2, be2, out_h, out_f);
-    SBK_LAUNCH_CHECK();
-    return SBK_OK;
-}
-
-int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float* w1, const float* b1, const float* g1,
-                         const float* be1, int C1, const __half* w2p, const float* b2, const float* g2,
-                         const float* be2, int C2, __half* act1_h, __half* out_h, float* out_f, cudaStream_t stream) {
-    if (C1 == W_C && C2 == W_C)
-        return cnn256_frontend_forward(feats, B, T0, F0, w1, b1, g1, be1, w2p, b2, g2, be2, act1_h, out_h, out_f, stream);
-    SBK_REQUIRE(C1 == 64 && C2 == 32, "cnn_frontend: only out_channels=(64, 32) and (256, 256) are built (got %d, %d)", C1, C2);
-    SBK_REQUIRE(T0 >= 2 && F0 >= 2, "cnn_frontend: input too small for reflect padding");
-    const int T1 = (T0 - 1) / 2 + 1, F1 = (F0 - 1) / 2 + 1;
-    const int T2 = (T1 - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
-    SBK_REQUIRE(F1 <= 64 && F2 * C2_FRAMES <= 96, "cnn_frontend: feature dim too large (F0=%d)", F0);
-    // the fused kernel (conv1 output never leaves the SM) for 3 <= F1 <= 40: it holds a conv1 frame in 40 registers per lane
-    // and writes the reflect columns itself.  The two-kernel version otherwise (n_mels > 80, or n_mels <= 4).
-    if (F1 <= 40 && F1 >= 3 && C2_FRAMES * F2 <= 16 * CF_WARPS) {
-        const size_t smem = static_cast<size_t>(CF_WARPS) * (F1 + 2) * C2_CELL * 2 + C2_COUT * C2_WROW * 2 +
-                            static_cast<size_t>(C2_FRAMES) * F2 * 33 * 4 + static_cast<size_t>(CF_WARPS) * 3 * (F0 + 2) * 4;
-        SBK_CUDA_CHECK(cudaFuncSetAttribute(cnn_fused_kernel<40>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        cnn_fused_kernel<40><<<dim3(ceil_div(T2, C2_FRAMES), B), CF_WARPS * 32, smem, stream>>>(
-            feats, T0, F0, T1, F1, T2, F2, w1, b1, g1, be1, w2p, b2, g2, be2, out_h, out_f);
-        SBK_LAUNCH_CHECK();
-        return SBK_OK;
-    }
-    {
-        const size_t smem = static_cast<size_t>(C1_WARPS) * 3 * (F0 + 2) * sizeof(float);
-        const dim3 grid(ceil_div(T1, C1_WARPS), B);
-        conv1_ln_kernel<64, 64><<<grid, C1_WARPS * 32, smem, stream>>>(feats, T0, F0, T1, F1, w1, b1, g1, be1, act1_h);
-        SBK_LAUNCH_CHECK();
-    }
-    {
-        const int n_trows = 2 * C2_FRAMES + 1;
-        const size_t smem = static_cast<size_t>(n_trows) * (F1 + 2) * C2_CELL * 2 + C2_COUT * C2_WROW * 2 +
-                            static_cast<size_t>(C2_FRAMES) * F2 * 33 * 4;
-        SBK_CUDA_CHECK(cudaFuncSetAttribute(conv2_ln_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const int warps = std::max(C2_FRAMES, ceil_div(C2_FRAMES * F2, 16));
-        conv2_ln_kernel<<<dim3(ceil_div(T2, C2_FRAMES), B), warps * 32, smem, stream>>>(act1_h, T1, F1, T2, F2, w2p, b2,
-                                                                                       g2, be2, out_h, out_f);
-        SBK_LAUNCH_CHECK();
-    }
-    return SBK_OK;
-}
-
 // =========================================================================== 3-block front-end (Transformer recipes)
 // ConvolutionFrontEnd(num_blocks=3, num_layers_per_block=1, out_channels=(64, 64, 64), kernel_sizes=(5, 5, 1),
 // strides=(2, 2, 1), residuals=(False, False, True)):
 //   block 1: reflect-pad 2 + Conv2d(5x5, 1 -> 64, stride 2) + LayerNorm(F1, 64) + LeakyReLU      -> act1 fp16
+//            (conv1k5_ln_kernel, above)
 //   block 2: reflect-pad 2 + Conv2d(5x5, 64 -> 64, stride 2) + LayerNorm(F2, 64) + LeakyReLU     -> y (fp32, in smem)
 //   block 3: LeakyReLU(LayerNorm(Conv2d_1x1(y))) + LayerNorm(Conv2d_1x1 reduce_conv(y))          -> out [B, T2, F2*64]
 // Blocks 2 and 3 are one kernel: block 3 is per-pixel work plus a per-frame LayerNorm, so it runs on block 2's
@@ -709,95 +578,13 @@ constexpr int K5_C = 64;                   // channels of every block
 constexpr int K5_FRAMES = 4;               // block-2 output frames per CTA
 constexpr int K5_WARPS = 5;                // 16 GEMM rows per warp: K5_FRAMES * F2 <= 80
 constexpr int K5_PROWS = 2 * K5_FRAMES + 3;  // act1 frames a CTA's patch holds
-constexpr int K5_CELL = 72;                // padded channel stride (halfs) of a patch cell
 constexpr int K5_WROW = 5 * K5_C + 8;      // padded weight row (halfs) of one kf slice: k = kt * 64 + ch
 constexpr int K5_YS = K5_C + 1;            // fp32 row stride of y
 constexpr int K5_ZS = 2 * K5_C + 1;        // fp32 row stride of the two block-3 convolutions
 
-// block 1: one warp per output frame, lane l owns channels 2l, 2l+1 (as conv1_ln_kernel, with 5x5 taps).
-// w1: [64, 5(kf), 5(kt)] fp32, g/be: [F1, 64].
-template <int MAXF>
-__global__ void __launch_bounds__(C1_WARPS * 32)
-conv1k5_ln_kernel(const float* __restrict__ feats, int T0, int F0, int T1, int F1, const float* __restrict__ w1,
-                  const float* __restrict__ b1, const float* __restrict__ gamma, const float* __restrict__ beta,
-                  __half* __restrict__ out_h) {
-    extern __shared__ float k5_in[];
-    const int FP = F0 + 4;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    float* in = k5_in + warp * 5 * FP;  // [5][F0 + 4] of this warp's frame (reflect padded)
-    const int b = blockIdx.y, t1 = blockIdx.x * C1_WARPS + warp;
-    if (t1 >= T1) return;
-    for (int i = lane; i < 5 * FP; i += 32) {
-        const int kt = i / FP, fp = i - kt * FP;
-        const int t = reflect_idx(2 * t1 + kt - 2, T0);
-        const int f = reflect_idx(fp - 2, F0);
-        in[i] = __ldg(feats + (static_cast<size_t>(b) * T0 + t) * F0 + f);
-    }
-    const int c0 = 2 * lane;
-    float wa[25], wb[25];
-#pragma unroll
-    for (int i = 0; i < 25; ++i) { wa[i] = __ldg(w1 + c0 * 25 + i); wb[i] = __ldg(w1 + (c0 + 1) * 25 + i); }
-    const float ba = __ldg(b1 + c0), bb = __ldg(b1 + c0 + 1);
-    __syncwarp();
-    float va[MAXF], vb[MAXF];
-    float s = 0.0f;
-#pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1) {
-        va[f1] = 0.0f; vb[f1] = 0.0f;
-        if (f1 < F1) {
-            float a = ba, bq = bb;
-#pragma unroll
-            for (int kf = 0; kf < 5; ++kf)
-#pragma unroll
-                for (int kt = 0; kt < 5; ++kt) {
-                    const float x = in[kt * FP + 2 * f1 + kf];
-                    a = fmaf(wa[kf * 5 + kt], x, a);
-                    bq = fmaf(wb[kf * 5 + kt], x, bq);
-                }
-            va[f1] = a; vb[f1] = bq;
-            s += a + bq;
-        }
-    }
-    const float n = static_cast<float>(F1 * K5_C);
-    const float mean = warp_sum(s) / n;
-    float q = 0.0f;
-#pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1)
-        if (f1 < F1) {
-            const float da = va[f1] - mean, db = vb[f1] - mean;
-            q += da * da + db * db;
-        }
-    const float rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
-    const size_t obase = (static_cast<size_t>(b) * T1 + t1) * F1 * K5_C;
-#pragma unroll
-    for (int f1 = 0; f1 < MAXF; ++f1)
-        if (f1 < F1) {
-            const int gi = f1 * K5_C + c0;
-            const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + gi));
-            const float2 be = __ldg(reinterpret_cast<const float2*>(beta + gi));
-            const float y0 = leaky((va[f1] - mean) * rstd * g.x + be.x);
-            const float y1 = leaky((vb[f1] - mean) * rstd * g.y + be.y);
-            *reinterpret_cast<__half2*>(out_h + obase + gi) = floats2half2_sat(y0, y1);
-        }
-}
-
-// LayerNorm over the n = F2 * 64 values of one frame held in smem rows [F2][stride] (columns col0 .. col0 + 63), one warp.
-__device__ __forceinline__ void k5_frame_stats(const float* src, int stride, int col0, int n, int lane, float& mean,
-                                               float& rstd) {
-    float s = 0.0f;
-    for (int i = lane; i < n; i += 32) s += src[(i >> 6) * stride + col0 + (i & 63)];
-    mean = warp_sum(s) / n;
-    float q = 0.0f;
-    for (int i = lane; i < n; i += 32) {
-        const float d = src[(i >> 6) * stride + col0 + (i & 63)] - mean;
-        q += d * d;
-    }
-    rstd = rsqrtf(warp_sum(q) / n + 1e-5f);
-}
-
 // Bytes of the shared-memory region block 2 (patch + weight slice) and then block 3 (w3 + z) use.
 __host__ __device__ __forceinline__ size_t k5_shared_region(int F1, int F2) {
-    const size_t gemm = static_cast<size_t>(K5_PROWS) * (F1 + 4) * K5_CELL * 2 + K5_C * K5_WROW * 2;
+    const size_t gemm = static_cast<size_t>(K5_PROWS) * (F1 + 4) * CELL * 2 + K5_C * K5_WROW * 2;
     const size_t blk3 = (2ull * K5_C * K5_YS + static_cast<size_t>(K5_FRAMES) * F2 * K5_ZS) * 4;
     return ((gemm > blk3 ? gemm : blk3) + 15) & ~size_t(15);
 }
@@ -814,8 +601,8 @@ cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
                     __half* __restrict__ out_h, float* __restrict__ out_f) {
     extern __shared__ __align__(16) uint8_t k5_smem[];
     const int FPAD = F1 + 4;
-    __half* patch = reinterpret_cast<__half*>(k5_smem);              // [K5_PROWS][FPAD][K5_CELL]
-    __half* wsm = patch + K5_PROWS * FPAD * K5_CELL;                  // [64][K5_WROW]
+    __half* patch = reinterpret_cast<__half*>(k5_smem);              // [K5_PROWS][FPAD][CELL]
+    __half* wsm = patch + K5_PROWS * FPAD * CELL;                     // [64][K5_WROW]
     // after block 2 the patch / weight region is free: block 3's weights and outputs reuse it
     float* w3s = reinterpret_cast<float*>(k5_smem);                   // [128][K5_YS]
     float* zs = w3s + 2 * K5_C * K5_YS;                               // [rows][K5_ZS]
@@ -824,15 +611,7 @@ cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
     const int b = blockIdx.y, t0 = blockIdx.x * K5_FRAMES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    for (int i = threadIdx.x; i < K5_PROWS * FPAD * (K5_C / 8); i += blockDim.x) {
-        const int cell = i / (K5_C / 8), v8 = i - cell * (K5_C / 8);
-        const int tr = cell / FPAD, fp = cell - tr * FPAD;
-        int t = reflect_idx(2 * t0 + tr - 2, T1);
-        t = min(max(t, 0), T1 - 1);  // tail tiles: keep loads in range (results discarded)
-        const int f = reflect_idx(fp - 2, F1);
-        *reinterpret_cast<uint4*>(patch + cell * K5_CELL + v8 * 8) =
-            *reinterpret_cast<const uint4*>(act1 + ((static_cast<size_t>(b) * T1 + t) * F1 + f) * K5_C + v8 * 8);
-    }
+    stage_patch<5, K5_PROWS>(patch, act1, b, t0, T1, F1);
     const int g = lane >> 2, c = lane & 3;
     const int r0 = warp * 16 + g, r1 = r0 + 8;
     const int rr0 = min(r0, rows - 1), rr1 = min(r1, rows - 1);
@@ -854,8 +633,8 @@ cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
         if (active) {
 #pragma unroll  // a rolled kt loop inside the rolled kf loop kept one loop counter in local memory (8-byte spill)
             for (int kt = 0; kt < 5; ++kt) {
-                const __half* a0p = patch + ((2 * fr0 + kt) * FPAD + 2 * f20 + kf) * K5_CELL + 2 * c;
-                const __half* a1p = patch + ((2 * fr1 + kt) * FPAD + 2 * f21 + kf) * K5_CELL + 2 * c;
+                const __half* a0p = patch + ((2 * fr0 + kt) * FPAD + 2 * f20 + kf) * CELL + 2 * c;
+                const __half* a1p = patch + ((2 * fr1 + kt) * FPAD + 2 * f21 + kf) * CELL + 2 * c;
 #pragma unroll
                 for (int ks = 0; ks < K5_C / 16; ++ks) {
                     uint32_t a[4];
@@ -866,25 +645,15 @@ cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
                     const int kk = kt * K5_C + ks * 16 + 2 * c;
 #pragma unroll
                     for (int nt = 0; nt < 8; ++nt) {
-                        uint32_t bb[2];
                         const __half* wp = wsm + (nt * 8 + g) * K5_WROW + kk;
-                        bb[0] = *reinterpret_cast<const uint32_t*>(wp);
-                        bb[1] = *reinterpret_cast<const uint32_t*>(wp + 8);
-                        mma_16816(acc[nt], a, bb);
+                        mma16816(acc[nt], a, *reinterpret_cast<const uint32_t*>(wp),
+                                 *reinterpret_cast<const uint32_t*>(wp + 8));
                     }
                 }
             }
         }
     }
-    if (active) {
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-            const int col = nt * 8 + 2 * c;
-            const float bz0 = __ldg(b2 + col), bz1 = __ldg(b2 + col + 1);
-            if (r0 < rows) { ys[r0 * K5_YS + col] = acc[nt][0] + bz0; ys[r0 * K5_YS + col + 1] = acc[nt][1] + bz1; }
-            if (r1 < rows) { ys[r1 * K5_YS + col] = acc[nt][2] + bz0; ys[r1 * K5_YS + col + 1] = acc[nt][3] + bz1; }
-        }
-    }
+    if (active) conv_tile_store<8, K5_YS>(acc, b2, ys, r0, r1, rows, c);
     __syncthreads();
     // block 2's LayerNorm + LeakyReLU in place (one warp per frame); block 3's weights into the freed region
     for (int i = threadIdx.x; i < 2 * K5_C * K5_C; i += blockDim.x) w3s[(i >> 6) * K5_YS + (i & 63)] = __ldg(w3 + i);
@@ -892,7 +661,7 @@ cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
     if (warp < K5_FRAMES) {
         float* src = ys + warp * F2 * K5_YS;
         float mean, rstd;
-        k5_frame_stats(src, K5_YS, 0, n, lane, mean, rstd);
+        frame_ln_stats<K5_C>(src, K5_YS, n, lane, mean, rstd);
         for (int i = lane; i < n; i += 32) {
             float& v = src[(i >> 6) * K5_YS + (i & 63)];
             v = leaky((v - mean) * rstd * __ldg(g2 + i) + __ldg(be2 + i));
@@ -915,8 +684,8 @@ cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
         if (t < T2) {
             const float* src = zs + warp * F2 * K5_ZS;
             float ma, ra, mr, rr;
-            k5_frame_stats(src, K5_ZS, 0, n, lane, ma, ra);
-            k5_frame_stats(src, K5_ZS, K5_C, n, lane, mr, rr);
+            frame_ln_stats<K5_C>(src, K5_ZS, n, lane, ma, ra);
+            frame_ln_stats<K5_C>(src + K5_C, K5_ZS, n, lane, mr, rr);
             const size_t ob = (static_cast<size_t>(b) * T2 + t) * n;
             for (int i = lane; i < n; i += 32) {
                 const float* zr = src + (i >> 6) * K5_ZS + (i & 63);
@@ -929,24 +698,65 @@ cnn3_block23_kernel(const __half* __restrict__ act1, int T1, int F1, int T2, int
     }
 }
 
-int cnn3_frontend_forward(const float* feats, int B, int T0, int F0, const Cnn3Weights& w, __half* act1_h, __half* out_h,
-                          float* out_f, cudaStream_t stream) {
+// =========================================================================== entry point
+int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const CnnWeights& w, __half* act1_h, __half* out_h,
+                         float* out_f, cudaStream_t stream) {
     const int T1 = (T0 - 1) / 2 + 1, F1 = (F0 - 1) / 2 + 1;
     const int T2 = (T1 - 1) / 2 + 1, F2 = (F1 - 1) / 2 + 1;
-    // the reference's reflect padding of 2 needs 3 rows / columns at both strided convolutions
-    SBK_REQUIRE(T1 >= 3 && F1 >= 3, "cnn_frontend: the 5x5 reflect padding needs at least 5 frames and 5 features "
-                "(got %d frames, %d features)", T0, F0);
-    SBK_REQUIRE(F1 <= 64 && K5_FRAMES * F2 <= 16 * K5_WARPS, "cnn_frontend: feature dim too large (F0=%d)", F0);
-    {
-        const size_t smem = static_cast<size_t>(C1_WARPS) * 5 * (F0 + 4) * sizeof(float);
-        conv1k5_ln_kernel<64><<<dim3(ceil_div(T1, C1_WARPS), B), C1_WARPS * 32, smem, stream>>>(
+    if (w.blocks == 3) {
+        // the reference's reflect padding of 2 needs 3 rows / columns at both strided convolutions
+        SBK_REQUIRE(T1 >= 3 && F1 >= 3, "cnn_frontend: the 5x5 reflect padding needs at least 5 frames and 5 features "
+                    "(got %d frames, %d features)", T0, F0);
+        SBK_REQUIRE(F1 <= 64 && K5_FRAMES * F2 <= 16 * K5_WARPS, "cnn_frontend: feature dim too large (F0=%d)", F0);
+        conv1k5_ln_kernel<64><<<dim3(ceil_div(T1, C1_WARPS), B), C1_WARPS * 32, C1_WARPS * 5 * (F0 + 4) * sizeof(float),
+                                stream>>>(feats, T0, F0, T1, F1, w.w1, w.b1, w.g1, w.be1, act1_h);
+        SBK_LAUNCH_CHECK();
+        const size_t smem = k5_shared_region(F1, F2) + static_cast<size_t>(K5_FRAMES) * F2 * K5_YS * 4;
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(cnn3_block23_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        cnn3_block23_kernel<<<dim3(ceil_div(T2, K5_FRAMES), B), K5_WARPS * 32, smem, stream>>>(
+            act1_h, T1, F1, T2, F2, w.w2, w.b2, w.g2, w.be2, w.w3, w.b3, w.g3, w.be3, w.gr, w.ber, out_h, out_f);
+        SBK_LAUNCH_CHECK();
+        return SBK_OK;
+    }
+    if (w.c1 == W_C && w.c2 == W_C) {
+        // the reference's reflect padding of 1 needs 2 rows / columns at both strided convolutions
+        SBK_REQUIRE(T0 >= 3 && F0 >= 3, "cnn_frontend: the 3x3 reflect padding needs at least 3 frames and 3 features "
+                    "(got %d frames, %d features)", T0, F0);
+        SBK_REQUIRE(F1 <= 40, "cnn_frontend: out_channels=(256, 256) is built for up to 80 features (F0=%d)", F0);
+        conv1c256_ln_kernel<40><<<dim3(T1, B), W1_THREADS, 3 * (F0 + 2) * sizeof(float), stream>>>(
             feats, T0, F0, T1, F1, w.w1, w.b1, w.g1, w.be1, act1_h);
         SBK_LAUNCH_CHECK();
+        const int frames = W2_BM / F2;
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(conv2c256_ln_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM));
+        conv2c256_ln_kernel<<<dim3(ceil_div(T2, frames), B), W2_THREADS, W2_SMEM, stream>>>(
+            act1_h, T1, F1, T2, F2, frames, w.w2, w.b2, w.g2, w.be2, out_h, out_f);
+        SBK_LAUNCH_CHECK();
+        return SBK_OK;
     }
-    const size_t smem = k5_shared_region(F1, F2) + static_cast<size_t>(K5_FRAMES) * F2 * K5_YS * 4;
-    SBK_CUDA_CHECK(cudaFuncSetAttribute(cnn3_block23_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cnn3_block23_kernel<<<dim3(ceil_div(T2, K5_FRAMES), B), K5_WARPS * 32, smem, stream>>>(
-        act1_h, T1, F1, T2, F2, w.w2p, w.b2, w.g2, w.be2, w.w3, w.b3, w.g3, w.be3, w.gr, w.ber, out_h, out_f);
+    SBK_REQUIRE(w.c1 == 64 && w.c2 == 32, "cnn_frontend: only out_channels=(64, 32) and (256, 256) are built (got %d, %d)",
+                w.c1, w.c2);
+    SBK_REQUIRE(T0 >= 2 && F0 >= 2, "cnn_frontend: input too small for reflect padding");
+    SBK_REQUIRE(F1 <= 64 && F2 * C2_FRAMES <= 96, "cnn_frontend: feature dim too large (F0=%d)", F0);
+    // patch + weights + cbuf, the shared memory of both (64, 32) conv2 kernels
+    const size_t c2_smem = static_cast<size_t>(C2_PROWS) * (F1 + 2) * CELL * 2 + C2_COUT * C2_WROW * 2 +
+                           static_cast<size_t>(C2_FRAMES) * F2 * C2_LD * 4;
+    // the fused kernel (conv1 output never leaves the SM) for 3 <= F1 <= 40: it holds a conv1 frame in 40 registers per lane
+    // and writes the reflect columns itself.  The two-kernel version otherwise (n_mels > 80, or n_mels <= 4).
+    if (F1 <= 40 && F1 >= 3 && C2_FRAMES * F2 <= 16 * CF_WARPS) {
+        const size_t smem = c2_smem + static_cast<size_t>(CF_WARPS) * 3 * (F0 + 2) * 4;
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(cnn_fused_kernel<40>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        cnn_fused_kernel<40><<<dim3(ceil_div(T2, C2_FRAMES), B), CF_WARPS * 32, smem, stream>>>(
+            feats, T0, F0, T1, F1, T2, F2, w.w1, w.b1, w.g1, w.be1, w.w2, w.b2, w.g2, w.be2, out_h, out_f);
+        SBK_LAUNCH_CHECK();
+        return SBK_OK;
+    }
+    conv1_ln_kernel<64, 64><<<dim3(ceil_div(T1, C1_WARPS), B), C1_WARPS * 32, C1_WARPS * 3 * (F0 + 2) * sizeof(float),
+                              stream>>>(feats, T0, F0, T1, F1, w.w1, w.b1, w.g1, w.be1, act1_h);
+    SBK_LAUNCH_CHECK();
+    SBK_CUDA_CHECK(cudaFuncSetAttribute(conv2_ln_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c2_smem));
+    const int warps = std::max(C2_FRAMES, ceil_div(C2_FRAMES * F2, 16));
+    conv2_ln_kernel<<<dim3(ceil_div(T2, C2_FRAMES), B), warps * 32, c2_smem, stream>>>(act1_h, T1, F1, T2, F2, w.w2, w.b2,
+                                                                                        w.g2, w.be2, out_h, out_f);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }

@@ -71,10 +71,6 @@ __device__ __forceinline__ float2 lds64(uint32_t addr) {
     asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
     return v;
 }
-__device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
-    const __half2 h = floats2half2_sat(lo, hi);
-    return *reinterpret_cast<const uint32_t*>(&h);
-}
 
 // Tile t -> (m0, n0): groups of PP_GROUP_M row panels, rows fastest inside a group.  The tiles in flight at one time (a
 // contiguous range of t) then read a few W column panels and the group's A row panels, all of which stay in L2.
@@ -171,7 +167,7 @@ __device__ __forceinline__ void pp_epilogue_chunk(const GemmEpilogue& e, const f
                     else if constexpr (ACT == ACT_GELU) v[q][i][c] = gelu_erf_f(v[q][i][c]);
                     else if constexpr (ACT == ACT_RELU) v[q][i][c] = fmaxf(v[q][i][c], 0.0f);
                 }
-                sts32(stg + (r0 + 8 * i) * P + (8 * q + qc) * 2, half2_bits(v[q][i][0], v[q][i][1]));
+                sts32(stg + (r0 + 8 * i) * P + (8 * q + qc) * 2, pack_half2(v[q][i][0], v[q][i][1]));
             }
     } else if constexpr (MODE == EPI_GLU) {  // weight rows interleaved [16 values | 16 gates] per 32 columns: the gate of
                                              // value column j (group q) is column j + 16 (group q + 2) of the same thread
@@ -233,7 +229,7 @@ __device__ __forceinline__ void pp_epilogue_chunk(const GemmEpilogue& e, const f
             }
             if (row < M)
                 *reinterpret_cast<uint4*>(outp + static_cast<size_t>(row) * e.ldo + col0 + seg * 8) =
-                    make_uint4(half2_bits(x0.x, x0.y), half2_bits(x0.z, x0.w), half2_bits(x1.x, x1.y), half2_bits(x1.z, x1.w));
+                    make_uint4(pack_half2(x0.x, x0.y), pack_half2(x0.z, x0.w), pack_half2(x1.x, x1.y), pack_half2(x1.z, x1.w));
         }
     } else {  // 64 B per row (32 fp16, or 16 fp32 GLU outputs): 4 lanes x 16 B per row, 8 rows per instruction
         const int seg = lane & 3, rsub = lane >> 2;

@@ -109,20 +109,20 @@ int sentence_norm_forward(const float* x, float* out, const float* rel_len, int 
                           int avoid_padding_norm, float eps, cudaStream_t stream);
 
 // ---- frontend.cu
-int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const float* w1, const float* b1, const float* g1,
-                         const float* be1, int C1, const __half* w2p, const float* b2, const float* g2,
-                         const float* be2, int C2, __half* act1_h, __half* out_h, float* out_f, cudaStream_t stream);
-// The Transformer recipes' 3-block front-end (5x5 / stride 2, 5x5 / stride 2, 1x1 with a residual 1x1), 64 channels:
-// feats [B, T0, F0] fp32 -> out [B, T2, F2 * 64] fp16 (+ fp32 when out_f is set); act1_h [B, T1, F1, 64] scratch.
-struct Cnn3Weights {
-    const float *w1, *b1, *g1, *be1;  // block 1: conv [64, 5, 5], LayerNorm [F1, 64]
-    const __half* w2p;                 // block 2: conv [64][(kf * 5 + kt) * 64 + ch]
-    const float *b2, *g2, *be2;
-    const float *w3, *b3;              // block 3: [convs.conv_0 | reduce_conv.conv] as [128, 64], [128]
-    const float *g3, *be3, *gr, *ber;  // block 3: convs.norm_0 and reduce_conv.norm, [F2, 64]
+// A ConvolutionFrontEnd's weights: 2 blocks of K x K convolutions (K = 3, out_channels (c1, c2) = (64, 32) or (256, 256)),
+// or the Transformer recipes' 3 blocks (5x5 / stride 2, 5x5 / stride 2, 1x1 with a residual 1x1), 64 channels.
+struct CnnWeights {
+    int blocks = 0, c1 = 0, c2 = 0;
+    const float *w1 = nullptr, *b1 = nullptr;   // block 1: conv [c1, K, K], bias [c1]
+    const float *g1 = nullptr, *be1 = nullptr;  // block 1: LayerNorm [F1, c1]
+    const __half* w2 = nullptr;  // block 2: conv [c2][(kf * K + kt) * c1 + ch]; at 256 channels as 128B-swizzled k-blocks
+    const float *b2 = nullptr, *g2 = nullptr, *be2 = nullptr;  // block 2: bias [c2], LayerNorm [F2, c2]
+    const float *w3 = nullptr, *b3 = nullptr;   // block 3: [convs.conv_0 | reduce_conv.conv] as [128, 64], [128]
+    const float *g3 = nullptr, *be3 = nullptr, *gr = nullptr, *ber = nullptr;  // block 3: convs.norm_0, reduce_conv.norm
 };
-int cnn3_frontend_forward(const float* feats, int B, int T0, int F0, const Cnn3Weights& w, __half* act1_h, __half* out_h,
-                          float* out_f, cudaStream_t stream);
+// feats [B, T0, F0] fp32 -> out [B, T2, F2 * c2] fp16 (+ fp32 when out_f is set); act1_h [B, T1, F1, c1] scratch
+int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const CnnWeights& w, __half* act1_h, __half* out_h,
+                         float* out_f, cudaStream_t stream);
 
 // ---- encoder_ops.cu
 // pdl: launched with programmatic stream serialisation (fp16 output only; the decode step's pre-norms)

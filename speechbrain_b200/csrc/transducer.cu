@@ -82,13 +82,7 @@ struct TdSmem {
     }
 };
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+// IEEE expf and division (sigmoid_f in common.cuh is the approximate one)
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // gates = U[tok] + W_hh h for this CTA's hidden units, then the LSTM cell (gate order i, f, g, o); rows with tok < 0 skip
@@ -202,7 +196,7 @@ __global__ void __launch_bounds__(TD_THREADS, 1) transducer_greedy_kernel(TdArgs
             for (int i = tid; i < TD_RB * J; i += TD_THREADS) {
                 const int r = i / J, k = i - r * J, b = rb0 + r;
                 if (b < B && st_t[b] < T)
-                    sZ[i] = gelu_erf(a.tn[(size_t(b) * T + st_t[b]) * J + k] + a.p[size_t(b) * J + k]);
+                    sZ[i] = gelu_erf_f(a.tn[(size_t(b) * T + st_t[b]) * J + k] + a.p[size_t(b) * J + k]);
             }
             __syncthreads();
             for (int pi = warp; pi < TD_RB * nvl; pi += TD_NW) {
