@@ -378,6 +378,60 @@ __device__ __forceinline__ int float_to_ordered(float f) {
 }
 __device__ __forceinline__ float ordered_to_float(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7FFFFFFF); }
 
+// Order-preserving unsigned key of a score, for radix_select: a larger score gives a larger key, -inf the smallest, every
+// NaN (whatever its sign) the largest key (argmax_takes's order), -0 the key of +0.  Key 0 is never produced.
+__device__ __forceinline__ uint32_t score_key(float s) {
+    if (isnan(s)) return 0xFFFFFFFFu;
+    const uint32_t u = __float_as_uint(s == 0.0f ? 0.0f : s);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ uint64_t score_key(double s) {
+    if (isnan(s)) return ~0ull;
+    const uint64_t u = static_cast<uint64_t>(__double_as_longlong(s == 0.0 ? 0.0 : s));
+    return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
+}
+// the score of a float key (the NaN key gives a NaN)
+__device__ __forceinline__ float key_score(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }
+
+template <typename Key>
+struct KthKey {
+    Key key;    // the k-th largest key
+    int ties;   // how many keys equal to it belong to the top k (the others of the top k are larger)
+};
+
+// Block-wide radix select, 8 bits per pass: the k-th largest of the nonzero keys key_of(0), ..., key_of(n - 1) (key 0:
+// not a candidate; there must be at least k others).  Every thread of the block calls it.
+template <typename Key, typename KeyOf>
+__device__ __forceinline__ KthKey<Key> radix_select(int n, int k, KeyOf key_of) {
+    __shared__ int s_hist[256];
+    __shared__ int s_sel[2];
+    Key prefix = 0, mask = 0;
+    int rem = k;
+    for (int shift = 8 * static_cast<int>(sizeof(Key)) - 8; shift >= 0; shift -= 8) {
+        for (int i = threadIdx.x; i < 256; i += blockDim.x) s_hist[i] = 0;
+        __syncthreads();
+        for (int u = threadIdx.x; u < n; u += blockDim.x) {
+            const Key key = key_of(u);
+            if (key != 0 && (key & mask) == prefix) atomicAdd(&s_hist[(key >> shift) & 255u], 1);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {   // walk the bins from the top until the bin that holds the rem-th largest key
+            int acc = 0, d = 255;
+            for (; d > 0; --d) {
+                if (acc + s_hist[d] >= rem) break;
+                acc += s_hist[d];
+            }
+            s_sel[0] = d;
+            s_sel[1] = rem - acc;
+        }
+        __syncthreads();
+        prefix |= static_cast<Key>(s_sel[0]) << shift;
+        mask |= static_cast<Key>(255) << shift;
+        rem = s_sel[1];
+    }
+    return {prefix, rem};
+}
+
 // Host: encode a 2-D row-major fp16 tensor [rows, cols] as a TMA map with box
 // [box_rows, 64 cols] and 128B swizzle. Implemented in tma_host.cu.
 int make_tmap_2d_f16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t row_stride_elems,

@@ -13,13 +13,11 @@
 //   4. an open-addressing table merges equal keys: the merged beam keeps the FIRST candidate's position and the LAST
 //      candidate's (parent, token), and its score folds the candidates' scores with np.logaddexp's float32 formula in
 //      candidate order;
-//   5. beams below max + beam_prune_logp go; a radix select finds the beam_size-th largest score and the kept beams are
-//      ranked by (score desc, position asc) -- heapq.nlargest's stable order;
+//   5. beams below max + beam_prune_logp go, the beam_size best stay, ranked by (score desc, position asc) --
+//      heapq.nlargest's stable order (prune_and_rank, ctc_search.cuh);
 //   6. with prune_history, only the first beam per (last word of the text, partial word, last token) stays.
 // The CTA writes, per processed frame, the surviving beams' (parent, token) and their count, and the final scores; the
 // host replays the token chains of the final beams with exact strings (decoders/ctc.py in this package).
-#include <vector>
-
 #include "ctc_search.cuh"
 #include "sbk_internal.h"
 
@@ -28,12 +26,6 @@ namespace sbk {
 namespace {
 
 constexpr uint64_t HSEP = 33;   // ' ': characters are hashed as code point + 1
-
-// order-preserving float -> uint32 (-0 and +0 map to the same key); 0 is never a finite score's key
-__device__ __forceinline__ uint32_t score_key(float s) {
-    const uint32_t u = __float_as_uint(s == 0.0f ? 0.0f : s);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 struct BeamS {
     uint64_t th, ph, pp, wh;   // hash of text, of partial word, P^len(partial), hash of the text's last word
@@ -71,16 +63,6 @@ __device__ __forceinline__ uint32_t key_slot(uint64_t th, uint64_t ph, int tl, i
     return static_cast<uint32_t>(h);
 }
 
-__device__ __forceinline__ float block_max(float v, float* s_f) {
-    v = warp_max(v);
-    if ((threadIdx.x & 31) == 0) s_f[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float r = s_f[0];
-    for (int i = 1; i < static_cast<int>(blockDim.x >> 5); ++i) r = fmaxf(r, s_f[i]);
-    __syncthreads();
-    return r;
-}
-
 struct CbArgs {
     const float* lp; const int* lens;
     int T, V, nv;
@@ -102,10 +84,7 @@ __global__ void __launch_bounds__(CB_THREADS, 1) ctc_beam_kernel(const CbArgs a)
     __shared__ float s_sc[2][CB_MAX_BEAM];
     __shared__ uint64_t s_th[2][CB_MAX_BEAM], s_ph[2][CB_MAX_BEAM], s_pp[2][CB_MAX_BEAM], s_wh[2][CB_MAX_BEAM];
     __shared__ int s_tl[2][CB_MAX_BEAM], s_pl[2][CB_MAX_BEAM], s_wl[2][CB_MAX_BEAM], s_sid[2][CB_MAX_BEAM];
-    __shared__ int s_kept[CB_MAX_BEAM];
-    __shared__ uint32_t s_kkey[CB_MAX_BEAM];
-    __shared__ int s_ord[CB_MAX_BEAM];
-    __shared__ int s_hist[256];
+    __shared__ int s_pos[CB_MAX_BEAM];
     __shared__ int s_w[CB_NW];
     __shared__ float s_f[CB_NW];
     __shared__ int s_i[CB_NW];
@@ -223,85 +202,15 @@ __global__ void __launch_bounds__(CB_THREADS, 1) ctc_beam_kernel(const CbArgs a)
             u_last[u] = last;
             lmax = fmaxf(lmax, s);
         }
-        const float mx = block_max(lmax, s_f);
         // ---- 5. prune: score >= max + beam_prune_logp, then the beam_size best (stable)
-        const float thr = __fadd_rn(mx, a.beam_thr);
-        int ns_loc = 0;
-        for (int u = tid; u < U; u += CB_THREADS) {
-            const float s = u_sc[u];
-            const bool ok = s >= thr;
-            u_key[u] = ok ? score_key(s) : 0u;
-            ns_loc += ok ? 1 : 0;
-        }
-        ns_loc = __reduce_add_sync(0xffffffffu, ns_loc);
-        if ((tid & 31) == 0) s_w[tid >> 5] = ns_loc;
-        __syncthreads();
-        int ns = 0;
-        for (int i = 0; i < CB_NW; ++i) ns += s_w[i];
-        __syncthreads();
-        uint32_t K = 0;
-        int rem = 0;
-        const bool select = ns > beam;
-        if (select) {   // radix select of the beam-th largest key, 8 bits per pass
-            uint32_t prefix = 0, mask = 0;
-            rem = beam;
-            for (int shift = 24; shift >= 0; shift -= 8) {
-                for (int i = tid; i < 256; i += CB_THREADS) s_hist[i] = 0;
-                __syncthreads();
-                for (int u = tid; u < U; u += CB_THREADS) {
-                    const uint32_t k = u_key[u];
-                    if (k != 0u && (k & mask) == prefix) atomicAdd(&s_hist[(k >> shift) & 255u], 1);
-                }
-                __syncthreads();
-                if (tid == 0) {
-                    int acc = 0, d = 255;
-                    for (; d > 0; --d) {
-                        if (acc + s_hist[d] >= rem) break;
-                        acc += s_hist[d];
-                    }
-                    s_i[0] = d;
-                    s_i[1] = rem - acc;
-                }
-                __syncthreads();
-                prefix |= static_cast<uint32_t>(s_i[0]) << shift;
-                mask |= 255u << shift;
-                rem = s_i[1];
-                __syncthreads();
-            }
-            K = prefix;   // beam - rem keys are larger than K; the first rem keys equal to K (by position) are kept too
-        }
-        int nk = 0, neq = 0;
-        for (int base = 0; base < U; base += CB_THREADS) {
-            const int u = base + tid;
-            const uint32_t k = u < U ? u_key[u] : 0u;
-            const bool eq = select && k != 0u && k == K;
-            int tot_eq;
-            const int r_eq = block_rank(eq, s_w, &tot_eq);
-            const bool keep = k != 0u && (!select || k > K || (eq && neq + r_eq < rem));
-            int tot;
-            const int r = block_rank(keep, s_w, &tot);
-            if (keep) { s_kept[nk + r] = u; s_kkey[nk + r] = k; }
-            nk += tot;
-            neq += tot_eq;
-        }
-        __syncthreads();
-        if (tid < nk) {
-            const uint32_t k = s_kkey[tid];
-            int rk = 0;
-            for (int j = 0; j < nk; ++j) {
-                const uint32_t kj = s_kkey[j];
-                rk += (kj > k || (kj == k && j < tid)) ? 1 : 0;
-            }
-            s_ord[rk] = tid;
-        }
-        __syncthreads();
+        const int nk = prune_and_rank(U, beam, lmax, a.beam_thr, [&](int u) { return u_sc[u]; }, u_key, s_w, s_pos);
         // the kept beams in rank order: state from the LAST merged candidate's (parent, token)
         const int nxt = cur ^ 1;
         BeamS ns_state = {};
         float my_sc = 0.0f;
         int my_par = 0, my_tok = 0;
         if (tid < nk) {
-            const int u = s_kept[s_ord[tid]], c = u_last[u];
+            const int u = s_pos[tid], c = u_last[u];
             const int q = c / nb;
             my_par = c - q * nb;
             my_tok = s_tok[q];
@@ -335,21 +244,6 @@ __global__ void __launch_bounds__(CB_THREADS, 1) ctc_beam_kernel(const CbArgs a)
     if (tid == 0) a.out_final[b] = nb;
 }
 
-int cb_check(const float* lp, const int* lens, int B, int T, int V, int nv, const sbk_ctc_beam_params* p, cudaStream_t st,
-             std::vector<int>& len_host) {
-    SBK_REQUIRE(lp && lens && p, "ctc_beam: null pointer");
-    SBK_REQUIRE(B >= 1 && T >= 1 && V >= 1, "ctc_beam: bad sizes B=%d T=%d V=%d", B, T, V);
-    SBK_REQUIRE(V <= CB_MAX_VOCAB, "ctc_beam: V=%d above the supported %d", V, CB_MAX_VOCAB);
-    SBK_REQUIRE(nv >= 1 && nv <= V, "ctc_beam: n_vocab=%d outside [1, V=%d]", nv, V);
-    SBK_REQUIRE(p->beam_size >= 1 && p->beam_size <= CB_MAX_BEAM, "ctc_beam: beam_size=%d outside [1, %d]", p->beam_size, CB_MAX_BEAM);
-    SBK_REQUIRE(p->blank >= 0 && p->blank < V, "ctc_beam: blank index %d outside [0, %d)", p->blank, V);
-    len_host.resize(B);
-    SBK_CUDA_CHECK(cudaMemcpyAsync(len_host.data(), lens, B * 4, cudaMemcpyDeviceToHost, st));
-    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int v : len_host) SBK_REQUIRE(v >= 0 && v <= T, "ctc_beam: length %d outside [0, %d]", v, T);
-    return SBK_OK;
-}
-
 // largest candidate-token count over the processed frames (synchronises the stream)
 int cb_max_tokens(const float* lp, const int* lens, int B, int T, int V, int nv, const sbk_ctc_beam_params* p, cudaStream_t st,
                   int* out) {
@@ -374,8 +268,7 @@ int sbk_ctc_beam_workspace_bytes(const float* log_probs_dev, const int* lens_dev
     using namespace sbk;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SBK_REQUIRE(bytes, "ctc_beam: null pointer");
-    std::vector<int> len;
-    int rc = cb_check(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, len);
+    int rc = ctc_check("ctc_beam", log_probs_dev, lens_dev, B, T, V, n_vocab, p, st);
     if (rc) return rc;
     int mt = 0, cmax, hcap;
     rc = cb_max_tokens(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, &mt);
@@ -393,8 +286,7 @@ int sbk_ctc_beam_search(const float* log_probs_dev, const int* lens_dev, int B, 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SBK_REQUIRE(tok_info_dev && tok_hash_dev && workspace_dev && frame_beams_dev && parent_dev && token_dev && score_dev &&
                 n_final_dev, "ctc_beam: null pointer");
-    std::vector<int> len;
-    int rc = cb_check(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, len);
+    int rc = ctc_check("ctc_beam", log_probs_dev, lens_dev, B, T, V, n_vocab, p, st);
     if (rc) return rc;
     int mt = 0, cmax, hcap;
     rc = cb_max_tokens(log_probs_dev, lens_dev, B, T, V, n_vocab, p, st, &mt);

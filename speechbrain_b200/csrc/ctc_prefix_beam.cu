@@ -14,13 +14,11 @@
 //      all beams (open addressing on (text hash, length), first beam in list order), created on a miss, and receives
 //      p_b + p or score + p.  The sums follow the reference's NumPy 2 types: score + p in float64 (float32 on the first
 //      processed frame, where the score is still the Python 0.0), p_nb + p and p_b + p in float32;
-//   4. every beam steps (score = logaddexp(p_b, p_nb) in float64), beams below max + beam_prune_logp go, a radix select
-//      finds the beam_size-th largest score and the kept beams are ranked by (score desc, position asc) -- heapq.nlargest's
-//      stable order; with prune_history only the first beam per (last word, partial word, last token) stays.
+//   4. every beam steps (score = logaddexp(p_b, p_nb) in float64), beams below max + beam_prune_logp go, the beam_size
+//      best stay, ranked by (score desc, position asc) -- heapq.nlargest's stable order (prune_and_rank, ctc_search.cuh);
+//      with prune_history only the first beam per (last word, partial word, last token) stays.
 // The CTA writes, per processed frame, each surviving beam's origin (previous rank, token or -1 when carried over) and
 // the final float64 scores; the host replays the texts and frames with exact strings (decoders/ctc.py in this package).
-#include <vector>
-
 #include "ctc_search.cuh"
 #include "sbk_internal.h"
 
@@ -51,12 +49,6 @@ __device__ __forceinline__ double logaddexp_np64(double x, double y) {
 }
 // np.logaddexp(python float, float32 value): both cast to float32
 __device__ __forceinline__ double lae32(double a, float b) { return logaddexp_np(__double2float_rn(a), b); }
-
-// order-preserving double -> uint64 (-0 and +0 map to the same key); 0 is never a score's key
-__device__ __forceinline__ uint64_t dkey(double s) {
-    const uint64_t u = static_cast<uint64_t>(__double_as_longlong(s == 0.0 ? 0.0 : s));
-    return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
-}
 
 // ---- CPython 3.12 set tables for non-negative int keys (hash(v) == v), no deletions (Objects/setobject.c)
 struct PySetT {
@@ -214,13 +206,10 @@ __global__ void __launch_bounds__(CB_THREADS, 1) ctc_prefix_beam_kernel(const Pb
     extern __shared__ int s_dyn[];
     int* s_above = s_dyn;          // [V] tokens above the threshold, ascending
     int* s_ord = s_dyn + a.V;      // [nv] candidate tokens in set order
-    __shared__ int s_kept[CB_MAX_BEAM], s_pos[CB_MAX_BEAM];
-    __shared__ uint64_t s_kkey[CB_MAX_BEAM];
-    __shared__ int s_hist[256];
+    __shared__ int s_pos[CB_MAX_BEAM];
     __shared__ int s_w[CB_NW];
     __shared__ float s_f[CB_NW];
     __shared__ int s_i[CB_NW];
-    __shared__ double s_d[CB_NW];
     const int b = blockIdx.x, tid = threadIdx.x, T = a.T, V = a.V, beam = a.beam;
 
     char* w = a.ws + static_cast<size_t>(b) * a.ws_stride;
@@ -318,82 +307,7 @@ __global__ void __launch_bounds__(CB_THREADS, 1) ctc_prefix_beam_kernel(const Pb
             x->score = logaddexp_np64(x->p_b, x->p_nb);
             lmax = fmax(lmax, x->score);
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) lmax = fmax(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
-        if ((tid & 31) == 0) s_d[tid >> 5] = lmax;
-        __syncthreads();
-        double mx = s_d[0];
-        for (int i = 1; i < CB_NW; ++i) mx = fmax(mx, s_d[i]);
-        const double thr = __dadd_rn(mx, a.beam_thr);
-        int ns_loc = 0;
-        for (int u = tid; u < U; u += CB_THREADS) {
-            const double s = bm[u].score;
-            const bool ok = s >= thr;
-            key[u] = ok ? dkey(s) : 0ull;
-            ns_loc += ok ? 1 : 0;
-        }
-        ns_loc = __reduce_add_sync(0xffffffffu, ns_loc);
-        if ((tid & 31) == 0) s_w[tid >> 5] = ns_loc;
-        __syncthreads();
-        int ns = 0;
-        for (int i = 0; i < CB_NW; ++i) ns += s_w[i];
-        __syncthreads();
-        uint64_t K = 0;
-        int rem = 0;
-        const bool select = ns > beam;
-        if (select) {   // radix select of the beam-th largest key, 8 bits per pass
-            uint64_t prefix = 0, mask = 0;
-            rem = beam;
-            for (int shift = 56; shift >= 0; shift -= 8) {
-                for (int i = tid; i < 256; i += CB_THREADS) s_hist[i] = 0;
-                __syncthreads();
-                for (int u = tid; u < U; u += CB_THREADS) {
-                    const uint64_t k = key[u];
-                    if (k != 0ull && (k & mask) == prefix) atomicAdd(&s_hist[(k >> shift) & 255u], 1);
-                }
-                __syncthreads();
-                if (tid == 0) {
-                    int acc = 0, dg = 255;
-                    for (; dg > 0; --dg) {
-                        if (acc + s_hist[dg] >= rem) break;
-                        acc += s_hist[dg];
-                    }
-                    s_i[0] = dg;
-                    s_i[1] = rem - acc;
-                }
-                __syncthreads();
-                prefix |= static_cast<uint64_t>(s_i[0]) << shift;
-                mask |= 255ull << shift;
-                rem = s_i[1];
-                __syncthreads();
-            }
-            K = prefix;   // beam - rem keys are larger than K; the first rem keys equal to K (by position) are kept too
-        }
-        int nk = 0, neq = 0;
-        for (int base = 0; base < U; base += CB_THREADS) {
-            const int u = base + tid;
-            const uint64_t k = u < U ? key[u] : 0ull;
-            const bool eq = select && k != 0ull && k == K;
-            int tot_eq;
-            const int r_eq = block_rank(eq, s_w, &tot_eq);
-            const bool keep = k != 0ull && (!select || k > K || (eq && neq + r_eq < rem));
-            int tot;
-            const int r = block_rank(keep, s_w, &tot);
-            if (keep) { s_kept[nk + r] = u; s_kkey[nk + r] = k; }
-            nk += tot;
-            neq += tot_eq;
-        }
-        __syncthreads();
-        if (tid < nk) {
-            const uint64_t k = s_kkey[tid];
-            int rk = 0;
-            for (int j = 0; j < nk; ++j) {
-                const uint64_t kj = s_kkey[j];
-                rk += (kj > k || (kj == k && j < tid)) ? 1 : 0;
-            }
-            s_pos[rk] = s_kept[tid];
-        }
-        __syncthreads();
+        const int nk = prune_and_rank(U, beam, lmax, a.beam_thr, [&](int u) { return bm[u].score; }, key, s_w, s_pos);
         PBeam me;
         if (tid < nk) {
             me = bm[s_pos[tid]];
@@ -429,26 +343,11 @@ __global__ void __launch_bounds__(CB_THREADS, 1) ctc_prefix_beam_kernel(const Pb
     if (tid == 0) a.out_final[b] = nb;
 }
 
-int pb_check(const float* lp, const int* lens, int B, int T, int V, int nv, const sbk_ctc_prefix_beam_params* p, cudaStream_t st) {
-    SBK_REQUIRE(lp && lens && p, "ctc_prefix_beam: null pointer");
-    SBK_REQUIRE(B >= 1 && T >= 1 && V >= 1, "ctc_prefix_beam: bad sizes B=%d T=%d V=%d", B, T, V);
-    SBK_REQUIRE(V <= CB_MAX_VOCAB, "ctc_prefix_beam: V=%d above the supported %d", V, CB_MAX_VOCAB);
-    SBK_REQUIRE(nv >= 1 && nv <= V, "ctc_prefix_beam: n_vocab=%d outside [1, V=%d]", nv, V);
-    SBK_REQUIRE(p->beam_size >= 1 && p->beam_size <= CB_MAX_BEAM, "ctc_prefix_beam: beam_size=%d outside [1, %d]", p->beam_size,
-                CB_MAX_BEAM);
-    SBK_REQUIRE(p->blank >= 0 && p->blank < V, "ctc_prefix_beam: blank index %d outside [0, %d)", p->blank, V);
-    std::vector<int> len(B);
-    SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), lens, B * 4, cudaMemcpyDeviceToHost, st));
-    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int v : len) SBK_REQUIRE(v >= 0 && v <= T, "ctc_prefix_beam: length %d outside [0, %d]", v, T);
-    return SBK_OK;
-}
-
 // Workspace shape from the pre-pass over all V columns: a frame has at most mt candidates, so at most beam * mt created
 // beams; the set tables of mt + 1 keys stay below 8 (mt + 1) slots.
 int pb_sizes(const float* lp, const int* lens, int B, int T, int V, int nv, const sbk_ctc_prefix_beam_params* p, cudaStream_t st,
              int* bcap, int* hcap, int* scap, size_t* stride) {
-    int rc = pb_check(lp, lens, B, T, V, nv, p, st);
+    int rc = ctc_check("ctc_prefix_beam", lp, lens, B, T, V, nv, p, st);
     if (rc) return rc;
     int mt = 0;
     rc = ctc_max_tokens(lp, lens, B, T, V, V, p->blank, p->token_prune_min_logp, p->blank_skip_logp, st, &mt);

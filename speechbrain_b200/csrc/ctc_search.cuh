@@ -1,7 +1,10 @@
 // Pieces shared by the two CTC beam searches without a language model (ctc_beam.cu, ctc_prefix_beam.cu): polynomial
-// string hashes modulo 2^61 - 1, np.logaddexp's float32 formula, the block-wide ordered compaction and arg-max, and the
-// token-count pre-pass that sizes their workspaces.
+// string hashes modulo 2^61 - 1, np.logaddexp's float32 formula, the block-wide ordered compaction, arg-max and max, the
+// prune and stable ranking of the merged beams (radix_select of common.cuh), the host input checks and the token-count
+// pre-pass that sizes their workspaces.
 #pragma once
+#include <vector>
+
 #include "common.cuh"
 #include "../../include/sbk.h"
 
@@ -75,6 +78,92 @@ __device__ __forceinline__ int block_argmax(const float* col, int V, float* s_f,
         if (argmax_takes(s_f[w], s_i[w], best, bi)) { best = s_f[w]; bi = s_i[w]; }
     __syncthreads();
     return bi;
+}
+
+template <typename T>
+__device__ __forceinline__ T block_max(T v, T* s_red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    T r = s_red[0];
+    for (int i = 1; i < static_cast<int>(blockDim.x >> 5); ++i) r = fmax(r, s_red[i]);
+    __syncthreads();
+    return r;
+}
+
+// The beam prune and sort_beams of both searches (decoders/ctc.py:811-824) over the U merged beams: the beams whose
+// score_of(u) >= max + beam_thr, and of those the `beam` best -- a radix select of the beam-th largest key, the ties at
+// it kept by position -- ranked by (score desc, position asc), heapq.nlargest's stable order.  lmax: the max of this
+// thread's scores (u = tid, tid + CB_THREADS, ...); key: U keys of workspace.  Leaves the kept positions in rank order in
+// s_pos and returns their count.  Every thread of the CB_THREADS block calls it.
+template <typename Score, typename Key, typename ScoreOf>
+__device__ __forceinline__ int prune_and_rank(int U, int beam, Score lmax, Score beam_thr, ScoreOf score_of, Key* key, int* s_w,
+                                              int* s_pos) {
+    __shared__ Score s_red[CB_NW];
+    __shared__ int s_kept[CB_MAX_BEAM];
+    __shared__ Key s_kkey[CB_MAX_BEAM];
+    const int tid = threadIdx.x;
+    const Score thr = block_max(lmax, s_red) + beam_thr;
+    int ns = 0;
+    for (int u = tid; u < U; u += CB_THREADS) {
+        const Score s = score_of(u);
+        const bool ok = s >= thr;
+        key[u] = ok ? score_key(s) : Key(0);   // no NaN passes: key 0 marks the pruned beams
+        ns += ok ? 1 : 0;
+    }
+    ns = __reduce_add_sync(0xffffffffu, ns);
+    if ((tid & 31) == 0) s_w[tid >> 5] = ns;
+    __syncthreads();
+    ns = 0;
+    for (int i = 0; i < CB_NW; ++i) ns += s_w[i];
+    __syncthreads();
+    const bool select = ns > beam;
+    KthKey<Key> kth = {0, 0};
+    if (select) kth = radix_select<Key>(U, beam, [&](int u) { return key[u]; });
+    int nk = 0, neq = 0;
+    for (int base = 0; base < U; base += CB_THREADS) {
+        const int u = base + tid;
+        const Key k = u < U ? key[u] : Key(0);
+        const bool eq = select && k != 0 && k == kth.key;
+        int tot_eq;
+        const int r_eq = block_rank(eq, s_w, &tot_eq);
+        const bool keep = k != 0 && (!select || k > kth.key || (eq && neq + r_eq < kth.ties));
+        int tot;
+        const int r = block_rank(keep, s_w, &tot);
+        if (keep) { s_kept[nk + r] = u; s_kkey[nk + r] = k; }
+        nk += tot;
+        neq += tot_eq;
+    }
+    __syncthreads();
+    if (tid < nk) {
+        const Key k = s_kkey[tid];
+        int rk = 0;
+        for (int j = 0; j < nk; ++j) {
+            const Key kj = s_kkey[j];
+            rk += (kj > k || (kj == k && j < tid)) ? 1 : 0;
+        }
+        s_pos[rk] = s_kept[tid];
+    }
+    __syncthreads();
+    return nk;
+}
+
+// Host checks of both searches' inputs (who: the message prefix); synchronises the stream to read the lengths.
+template <typename Params>
+int ctc_check(const char* who, const float* lp, const int* lens, int B, int T, int V, int nv, const Params* p, cudaStream_t st) {
+    SBK_REQUIRE(lp && lens && p, "%s: null pointer", who);
+    SBK_REQUIRE(B >= 1 && T >= 1 && V >= 1, "%s: bad sizes B=%d T=%d V=%d", who, B, T, V);
+    SBK_REQUIRE(V <= CB_MAX_VOCAB, "%s: V=%d above the supported %d", who, V, CB_MAX_VOCAB);
+    SBK_REQUIRE(nv >= 1 && nv <= V, "%s: n_vocab=%d outside [1, V=%d]", who, nv, V);
+    SBK_REQUIRE(p->beam_size >= 1 && p->beam_size <= CB_MAX_BEAM, "%s: beam_size=%d outside [1, %d]", who, p->beam_size,
+                CB_MAX_BEAM);
+    SBK_REQUIRE(p->blank >= 0 && p->blank < V, "%s: blank index %d outside [0, %d)", who, p->blank, V);
+    std::vector<int> len(B);
+    SBK_CUDA_CHECK(cudaMemcpyAsync(len.data(), lens, B * 4, cudaMemcpyDeviceToHost, st));
+    SBK_CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int v : len) SBK_REQUIRE(v >= 0 && v <= T, "%s: length %d outside [0, %d]", who, v, T);
+    return SBK_OK;
 }
 
 // Pre-pass: the largest candidate-token count of any processed frame (sizes the candidate workspace).

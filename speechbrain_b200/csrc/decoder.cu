@@ -947,9 +947,112 @@ struct BeamArgs {
     const float* add_scores;
     const float* add_row;   // [n_bh] per-hypothesis score added to every token (CoverageScorer), or null
     float attn_weight; int blank; float add_const;
-    const float* lm_emb; const float* lm_pe; int lm_d; float lm_scale; float* lm_x_next; __half* lm_x16_next; int* tok_cache;
+    BeamLm lm;
     float* scr_val; int* scr_idx; float* scr_lse;   // beam_rows_kernel -> beam_merge_kernel
 };
+
+// The scorers' add-ons to a token's log-prob, one at a time: ScorerBuilder.score's pre-weighted full scores (add: the
+// row's, or null), the LengthScorer's constant and the row's CoverageScorer score.
+__device__ __forceinline__ float add_ons(const BeamArgs& a, float lp, const float* add, int j, float add_row) {
+    if (add) lp += add[j];
+    lp += a.add_const;
+    if (a.add_row) lp += add_row;
+    return lp;
+}
+
+// The eos log-prob of a row with its add-ons, -inf'd (minus_inf) before min_decode_steps and under the eos threshold;
+// mne: the max over the row's other tokens of logit / T.
+__device__ __forceinline__ float eos_logprob(const BeamArgs& a, float logit, float lse, float mne, int step, const float* add,
+                                             float add_row) {
+    float lp = a.attn_weight * (logit * a.inv_temp - lse);
+    if (step < a.min_steps) lp = a.minus_inf;
+    if (a.use_eos_threshold) {
+        const float max_lp = fmaxf(a.attn_weight * (mne - lse), lp);
+        if (!(lp > a.eos_threshold * max_lp)) lp = a.minus_inf;
+    }
+    return add_ons(a, lp, add, a.eos, add_row);
+}
+
+// The final score of token j of a row (lg, add: the row's logits and add scores; eos_lp from eos_logprob), the CTC blank
+// blocked.  Never -0 (x - lse rounds to +0, sequence scores start at +0): score_key orders it as argmax_takes does.
+__device__ __forceinline__ float cand_score(const BeamArgs& a, const float* lg, const float* add, float add_row, int j,
+                                            float lse, float eos_lp, float seq, float inv_len) {
+    float lp = eos_lp;
+    if (j != a.eos) {
+        lp = a.attn_weight * (lg[j] * a.inv_temp - lse);
+        if (j == a.blank) lp = a.minus_inf;
+        lp = add_ons(a, lp, add, j, add_row);
+    }
+    return (seq + lp) * inv_len;
+}
+
+// Decoder input of the n rows row0 + k for token tok_of(k) at position pos: emb[tok] * scale + pe[pos]; with an LM also
+// its own input (lm.emb[tok] * lm.scale + lm.pe[pos], fp32 and fp16) and the token in its cache.  Element i = k * d + c
+// is written by calling thread i % nt (t: this thread's index among the nt callers).
+template <typename TokOf>
+__device__ __forceinline__ void write_inputs(int row0, int n, TokOf tok_of, int pos, int S_max, const float* emb, const float* pe,
+                                             int d, float scale, float* x, const BeamLm& lm, int t, int nt) {
+    for (int i = t; i < n * d; i += nt) {
+        const int k = i / d, c = i - k * d;
+        x[static_cast<size_t>(row0 + k) * d + c] =
+            emb[static_cast<size_t>(tok_of(k)) * d + c] * scale + pe[static_cast<size_t>(pos) * d + c];
+    }
+    if (lm.emb) {
+        for (int i = t; i < n * lm.d; i += nt) {
+            const int k = i / lm.d, c = i - k * lm.d;
+            const float v = lm.emb[static_cast<size_t>(tok_of(k)) * lm.d + c] * lm.scale +
+                            lm.pe[static_cast<size_t>(pos) * lm.d + c];
+            lm.x[static_cast<size_t>(row0 + k) * lm.d + c] = v;
+            lm.x16[static_cast<size_t>(row0 + k) * lm.d + c] = float2half_sat(v);
+        }
+        if (t < n) lm.tok_cache[static_cast<size_t>(row0 + t) * S_max + pos] = tok_of(t);
+    }
+}
+
+// The end of a beam step of utterance b, after the selection; every thread of the BS_THREADS block calls it.  The thread
+// holding rank `rank` < beam (score v, candidate ix = k * V + token or 0x7fffffff for none; lse: the log-sum-exps of the
+// utterance's rows) writes that winner's history and next sequence score (-inf after eos).  Then the finished counters,
+// the lineage of the new beams, their next decoder inputs and the step counters.  s_wtok, s_wpred: [beam] shared ints.
+__device__ __forceinline__ void finish_step(const BeamArgs& a, int b, int step, int rank, float v, int ix, const float* lse,
+                                            int* s_wtok, int* s_wpred) {
+    const int tid = threadIdx.x, beam = a.beam, V = a.V, row0 = b * beam;
+    if (rank < beam) {
+        int kk = 0, tok = 0;
+        if (ix != 0x7fffffff) { kk = ix / V; tok = ix - kk * V; }
+        const int row = row0 + rank, prow = row0 + kk;
+        const float raw_lp = a.attn_weight * (a.logits[static_cast<size_t>(prow) * V + tok] * a.inv_temp - lse[kk]);
+        const size_t h = static_cast<size_t>(step) * a.n_bh + row;
+        a.hist_tok[h] = tok; a.hist_pred[h] = prow; a.hist_score[h] = v; a.hist_lp[h] = raw_lp;
+        float ns = a.length_norm ? v * static_cast<float>(step + 1) : v;
+        if (tok == a.eos) ns = -INFINITY;
+        a.seq_scores[static_cast<size_t>((step + 1) & 1) * a.n_bh + row] = ns;
+        s_wtok[rank] = tok; s_wpred[rank] = prow;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int n_eos = 0;
+        for (int k = 0; k < beam; ++k) n_eos += (s_wtok[k] == a.eos) ? 1 : 0;
+        const int before = a.finished[b];
+        const int after = min(beam, before + n_eos);
+        a.finished[b] = after;
+        if (before < beam && after >= beam) atomicAdd(a.n_full, 1);
+    }
+    const int* lin_in = a.lineage + static_cast<size_t>(step & 1) * a.n_bh * a.S_max;
+    int* lin_out = a.lineage + static_cast<size_t>((step + 1) & 1) * a.n_bh * a.S_max;
+    for (int i = tid; i < beam * (step + 2); i += BS_THREADS) {
+        const int k = i / (step + 2), p = i - k * (step + 2);
+        const int row = row0 + k, prow = s_wpred[k];
+        int src;
+        if (p < step) src = lin_in[static_cast<size_t>(prow) * a.S_max + p];
+        else if (p == step) src = prow;   // this step's K/V were written at the predecessor's physical row
+        else src = row;                   // next step writes at the new row itself
+        lin_out[static_cast<size_t>(row) * a.S_max + p] = src;
+    }
+    write_inputs(row0, beam, [&](int k) { return s_wtok[k]; }, step + 1, a.S_max, a.emb, a.pe, a.d, a.sqrt_d, a.x_next, a.lm,
+                 tid, BS_THREADS);
+    __syncthreads();
+    if (tid < beam) a.step_arr[row0 + tid] = step + 1;
+}
 
 // Two kernels.  beam_rows_kernel, one CTA per hypothesis row (B * beam CTAs instead of B): the row's log-sum-exp, masked eos
 // log-prob and its own top-`beam` candidates under the final score -- the utterance's top-`beam` of beam * V is a subset
@@ -999,16 +1102,8 @@ __global__ void __launch_bounds__(BS_THREADS) beam_rows_kernel(const BeamArgs a)
             float tot = 0.0f, mne = -INFINITY;
             for (int w = 0; w < BS_THREADS / 32; ++w) { tot += s_red[w]; mne = fmaxf(mne, __int_as_float(s_redi[w])); }
             const float lse = mx + logf(tot);
-            float eos_lp = a.attn_weight * (lg[a.eos] * a.inv_temp - lse);
-            if (step < a.min_steps) eos_lp = a.minus_inf;
-            if (a.use_eos_threshold) {
-                const float max_lp = fmaxf(a.attn_weight * (mne - lse), eos_lp);
-                if (!(eos_lp > a.eos_threshold * max_lp)) eos_lp = a.minus_inf;
-            }
-            if (add) eos_lp += add[a.eos];  // ScorerBuilder.score
-            eos_lp += a.add_const + add_row;
             s_lse = lse;
-            s_eos = eos_lp;
+            s_eos = eos_logprob(a, lg[a.eos], lse, mne, step, add, add_row);
             a.scr_lse[row] = lse;
         }
         __syncthreads();
@@ -1021,16 +1116,7 @@ __global__ void __launch_bounds__(BS_THREADS) beam_rows_kernel(const BeamArgs a)
     const float inv_len = a.length_norm ? 1.0f / static_cast<float>(step + 1) : 1.0f;
     const float lse = s_lse, eos_lp = s_eos;
     for (int j = tid; j < V; j += BS_THREADS) {
-        float lp;
-        if (j == a.eos) lp = eos_lp;
-        else {
-            lp = a.attn_weight * (lg[j] * a.inv_temp - lse);
-            if (j == a.blank) lp = a.minus_inf;
-            if (add) lp += add[j];
-            lp += a.add_const;
-            if (a.add_row) lp += add_row;
-        }
-        const float sc = (seq + lp) * inv_len;
+        const float sc = cand_score(a, lg, add, add_row, j, lse, eos_lp, seq, inv_len);
         int ix = k * V + j;
         if (argmax_takes(sc, ix, bv[BS_MAXB - 1], bi[BS_MAXB - 1])) {  // insert (list in candidate order; first `beam` matter)
             float v = sc;
@@ -1086,10 +1172,9 @@ __global__ void __launch_bounds__(BS_THREADS) beam_merge_kernel(const BeamArgs a
     pdl_trigger();
     pdl_wait();
     const int b = blockIdx.x, tid = threadIdx.x;
-    const int beam = a.beam, V = a.V;
+    const int beam = a.beam;
     const int row0 = b * beam;
     const int step = a.step_arr[row0];
-    float* seq_out = a.seq_scores + static_cast<size_t>((step + 1) & 1) * a.n_bh;
     const int n = beam * beam;
     float v = -INFINITY;
     int ix = 0x7fffffff;
@@ -1100,67 +1185,17 @@ __global__ void __launch_bounds__(BS_THREADS) beam_merge_kernel(const BeamArgs a
         s_v[tid] = v; s_i[tid] = ix;
     }
     __syncthreads();
+    int rank = beam;   // threads past the beam * beam survivors hold no winner
     if (tid < n) {
-        int rank = 0;
+        rank = 0;
         for (int j = 0; j < n; ++j) {
             const float ov = s_v[j];
             const int oi = s_i[j];
             rank += (argmax_takes(ov, oi, v, ix) || (oi == ix && j < tid)) ? 1 : 0;
         }
-        if (rank < beam) {
-            int kk = 0, tok = 0;
-            if (ix != 0x7fffffff) { kk = ix / V; tok = ix - kk * V; }
-            const int row = row0 + rank, prow = row0 + kk;
-            const float raw_lp = a.attn_weight * (a.logits[static_cast<size_t>(prow) * V + tok] * a.inv_temp - a.scr_lse[prow]);
-            const size_t h = static_cast<size_t>(step) * a.n_bh + row;
-            a.hist_tok[h] = tok; a.hist_pred[h] = prow; a.hist_score[h] = v; a.hist_lp[h] = raw_lp;
-            float ns = a.length_norm ? v * static_cast<float>(step + 1) : v;
-            if (tok == a.eos) ns = -INFINITY;
-            seq_out[row] = ns;
-            s_wtok[rank] = tok; s_wpred[rank] = prow;
-        }
     }
-    __syncthreads();
-    // ---- finished counters, lineage of the new beams, next decoder inputs, step counters
-    if (tid == 0) {
-        int n_eos = 0;
-        for (int k = 0; k < beam; ++k) n_eos += (s_wtok[k] == a.eos) ? 1 : 0;
-        const int before = a.finished[b];
-        const int after = min(beam, before + n_eos);
-        a.finished[b] = after;
-        if (before < beam && after >= beam) atomicAdd(a.n_full, 1);
-    }
-    const int* lin_in = a.lineage + static_cast<size_t>(step & 1) * a.n_bh * a.S_max;
-    int* lin_out = a.lineage + static_cast<size_t>((step + 1) & 1) * a.n_bh * a.S_max;
-    for (int i = tid; i < beam * (step + 2); i += BS_THREADS) {
-        const int k = i / (step + 2), p = i - k * (step + 2);
-        const int row = row0 + k, prow = s_wpred[k];
-        int src;
-        if (p < step) src = lin_in[static_cast<size_t>(prow) * a.S_max + p];
-        else if (p == step) src = prow;   // this step's K/V were written at the predecessor's physical row
-        else src = row;                   // next step writes at the new row itself
-        lin_out[static_cast<size_t>(row) * a.S_max + p] = src;
-    }
-    for (int i = tid; i < beam * a.d; i += BS_THREADS) {
-        const int k = i / a.d, c = i - k * a.d;
-        a.x_next[static_cast<size_t>(row0 + k) * a.d + c] =
-            a.emb[static_cast<size_t>(s_wtok[k]) * a.d + c] * a.sqrt_d + a.pe[static_cast<size_t>(step + 1) * a.d + c];
-    }
-    if (a.lm_emb) {
-        for (int i = tid; i < beam * a.lm_d; i += BS_THREADS) {
-            const int k = i / a.lm_d, c = i - k * a.lm_d;
-            const float v2 = a.lm_emb[static_cast<size_t>(s_wtok[k]) * a.lm_d + c] * a.lm_scale +
-                             a.lm_pe[static_cast<size_t>(step + 1) * a.lm_d + c];
-            a.lm_x_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = v2;
-            a.lm_x16_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = float2half_sat(v2);
-        }
-        if (tid < beam) a.tok_cache[static_cast<size_t>(row0 + tid) * a.S_max + step + 1] = s_wtok[tid];
-    }
-    __syncthreads();
-    if (tid < beam) a.step_arr[row0 + tid] = step + 1;
+    finish_step(a, b, step, rank, v, ix, a.scr_lse + row0, s_wtok, s_wpred);
 }
-
-
 
 // --------------------------------------------------------------------------- CoverageScorer (decoders/scorer.py:788-955)
 // For the Transformer decoder `attn` is the LAST decoder layer's head-averaged cross-attention distribution of every
@@ -1277,26 +1312,17 @@ int coverage_score(const CoverageStep& p, cudaStream_t stream) {
 // --------------------------------------------------------------------------- beam step for wide beams (16 < beam <= 128)
 // Same contract as beam_step_kernel; the per-thread sorted lists of that kernel (beam registers per thread) do not scale to
 // the recipes' test_beam_size = 66 (conformer_large.yaml:132), so the top-`beam` of the beam * V candidates is found by an
-// exact radix select: 4 passes of 8 bits over an order-preserving integer image of the score find the beam-th largest value,
-// one more pass collects everything above it plus the lowest-index ties, a bitonic sort orders the <= 128 survivors by
-// (score descending, candidate index ascending) -- the order the small-beam kernel produces.
+// exact radix select: radix_select (common.cuh) finds the beam-th largest score_key in 4 passes of 8 bits over the
+// candidates, one more pass collects everything above it plus the lowest-index ties, a bitonic sort orders the <= 128
+// survivors by (score descending, candidate index ascending) -- the order the small-beam kernel produces.
 constexpr int BL_MAXB = 128;
 constexpr int BL_TIECAP = 1024;
-
-// larger score <-> larger key, -inf the smallest; every NaN, whatever its sign, maps to the largest key (argmax_takes's order)
-__device__ __forceinline__ uint32_t score_key(float v) {
-    if (isnan(v)) return 0xFFFFFFFFu;
-    const uint32_t u = __float_as_uint(v);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamArgs a) {
     __shared__ float s_red[BS_THREADS / 32];
     __shared__ int s_redi[BS_THREADS / 32];
     __shared__ float s_lse[BL_MAXB], s_eos[BL_MAXB], s_seq[BL_MAXB];
-    __shared__ int s_hist[256];
-    __shared__ uint32_t s_prefix;
-    __shared__ int s_remaining, s_nsel, s_ntie;
+    __shared__ int s_nsel, s_ntie;
     __shared__ float s_selv[BL_MAXB];
     __shared__ int s_seli[BL_MAXB];
     __shared__ int s_tie[BL_TIECAP];
@@ -1308,7 +1334,6 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
     const int row0 = b * beam;
     const int step = a.step_arr[row0];
     const float* seq_in = a.seq_scores + static_cast<size_t>(step & 1) * a.n_bh;
-    float* seq_out = a.seq_scores + static_cast<size_t>((step + 1) & 1) * a.n_bh;
     // ---- phase 1: per beam row log-sum-exp of logits / T and the (masked) eos log-prob (one warp per row)
     for (int k = warp; k < beam; k += BS_THREADS / 32) {
         const float* lg = a.logits + static_cast<size_t>(row0 + k) * V;
@@ -1325,61 +1350,28 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
         mne = warp_max(mne);
         if (lane == 0) {
             const float lse = mx + logf(sm);
-            float eos_lp = a.attn_weight * (lg[a.eos] * a.inv_temp - lse);
-            if (step < a.min_steps) eos_lp = a.minus_inf;
-            if (a.use_eos_threshold) {
-                const float max_lp = fmaxf(a.attn_weight * (mne - lse), eos_lp);
-                if (!(eos_lp > a.eos_threshold * max_lp)) eos_lp = a.minus_inf;
-            }
-            if (a.add_scores) eos_lp += a.add_scores[static_cast<size_t>(row0 + k) * V + a.eos];
-            eos_lp += a.add_const;
-            if (a.add_row) eos_lp += a.add_row[row0 + k];
             s_lse[k] = lse;
-            s_eos[k] = eos_lp;
+            const float* add = a.add_scores ? a.add_scores + static_cast<size_t>(row0 + k) * V : nullptr;
+            s_eos[k] = eos_logprob(a, lg[a.eos], lse, mne, step, add, a.add_row ? a.add_row[row0 + k] : 0.0f);
             s_seq[k] = seq_in[row0 + k];
         }
     }
-    if (tid == 0) { s_prefix = 0u; s_remaining = beam; s_nsel = 0; s_ntie = 0; }
+    if (tid == 0) { s_nsel = 0; s_ntie = 0; }
     __syncthreads();
     const float inv_len = a.length_norm ? 1.0f / static_cast<float>(step + 1) : 1.0f;
     const int n_cand = beam * V;
-    auto cand_score = [&](int cidx) -> float {
+    auto score_of = [&](int cidx) {
         const int k = cidx / V, j = cidx - k * V;
-        float lp = (j == a.eos) ? s_eos[k]
-                                : a.attn_weight * (a.logits[static_cast<size_t>(row0 + k) * V + j] * a.inv_temp - s_lse[k]);
-        if (j == a.blank) lp = a.minus_inf;
-        if (a.add_scores && j != a.eos) lp += a.add_scores[static_cast<size_t>(row0 + k) * V + j];
-        if (j != a.eos) lp += a.add_const;
-        if (a.add_row && j != a.eos) lp += a.add_row[row0 + k];
-        return (s_seq[k] + lp) * inv_len;
+        const size_t r = static_cast<size_t>(row0 + k) * V;
+        return cand_score(a, a.logits + r, a.add_scores ? a.add_scores + r : nullptr, a.add_row ? a.add_row[row0 + k] : 0.0f, j,
+                          s_lse[k], s_eos[k], s_seq[k], inv_len);
     };
     // ---- phase 2: radix select of the beam-th largest key
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 24 - 8 * pass;
-        s_hist[tid] = 0;
-        __syncthreads();
-        const uint32_t prefix = s_prefix;
-        const uint32_t himask = pass == 0 ? 0u : (0xFFFFFFFFu << (shift + 8));
-        for (int cidx = tid; cidx < n_cand; cidx += BS_THREADS) {
-            const uint32_t key = score_key(cand_score(cidx));
-            if ((key & himask) == (prefix & himask)) atomicAdd(&s_hist[(key >> shift) & 255u], 1);
-        }
-        __syncthreads();
-        if (tid == 0) {
-            int need = s_remaining, acc = 0, bin = 255;
-            for (; bin > 0; --bin) {
-                if (acc + s_hist[bin] >= need) break;
-                acc += s_hist[bin];
-            }
-            s_prefix = prefix | (static_cast<uint32_t>(bin) << shift);
-            s_remaining = need - acc;  // how many of the candidates inside this bin are still wanted
-        }
-        __syncthreads();
-    }
+    const KthKey<uint32_t> kth = radix_select<uint32_t>(n_cand, beam, [&](int cidx) { return score_key(score_of(cidx)); });
     // ---- phase 3: collect keys above the threshold, and the ties
-    const uint32_t thr = s_prefix;
+    const uint32_t thr = kth.key;
     for (int cidx = tid; cidx < n_cand; cidx += BS_THREADS) {
-        const float sc = cand_score(cidx);
+        const float sc = score_of(cidx);
         const uint32_t key = score_key(sc);
         if (key > thr) {
             const int p = atomicAdd(&s_nsel, 1);
@@ -1394,8 +1386,8 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
     // the buffer keeps the first to arrive, which the scan order makes the lowest-index ones unless a warp lags four
     // passes behind the others; test_gpu_beam_step.py checks a flat row at V = 5000.
     {
-        const int nsel = min(s_nsel, BL_MAXB), ntie = min(s_ntie, BL_TIECAP), want = min(s_remaining, beam - nsel);
-        const float tv = [&] { const uint32_t k = thr; const uint32_t u = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k; return __uint_as_float(u); }();
+        const int nsel = min(s_nsel, BL_MAXB), ntie = min(s_ntie, BL_TIECAP), want = min(kth.ties, beam - nsel);
+        const float tv = key_score(thr);
         for (int r = 0; r < want; ++r) {
             int best = 0x7fffffff, bp = -1;
             for (int i = tid; i < ntie; i += BS_THREADS)
@@ -1435,69 +1427,18 @@ __global__ void __launch_bounds__(BS_THREADS) beam_step_large_kernel(const BeamA
             __syncthreads();
         }
     }
-    // ---- winners (thread k handles new beam k)
-    if (tid < beam) {
-        const int k = tid;
-        const int cand = s_seli[k];
-        const float sc = s_selv[k];
-        int kk = 0, tok = 0;
-        if (cand != 0x7fffffff) { kk = cand / V; tok = cand - kk * V; }
-        const int row = row0 + k, prow = row0 + kk;
-        const float raw_lp = a.attn_weight * (a.logits[static_cast<size_t>(prow) * V + tok] * a.inv_temp - s_lse[kk]);
-        const size_t h = static_cast<size_t>(step) * a.n_bh + row;
-        a.hist_tok[h] = tok; a.hist_pred[h] = prow; a.hist_score[h] = sc; a.hist_lp[h] = raw_lp;
-        float ns = a.length_norm ? sc * static_cast<float>(step + 1) : sc;
-        if (tok == a.eos) ns = -INFINITY;
-        seq_out[row] = ns;
-        s_wtok[k] = tok; s_wpred[k] = prow;
-    }
-    __syncthreads();
-    // ---- phase 4: finished counters, lineage of the new beams, next decoder inputs, step counters (as beam_step_kernel)
-    if (tid == 0) {
-        int n_eos = 0;
-        for (int k = 0; k < beam; ++k) n_eos += (s_wtok[k] == a.eos) ? 1 : 0;
-        const int before = a.finished[b];
-        const int after = min(beam, before + n_eos);
-        a.finished[b] = after;
-        if (before < beam && after >= beam) atomicAdd(a.n_full, 1);
-    }
-    const int* lin_in = a.lineage + static_cast<size_t>(step & 1) * a.n_bh * a.S_max;
-    int* lin_out = a.lineage + static_cast<size_t>((step + 1) & 1) * a.n_bh * a.S_max;
-    for (int i = tid; i < beam * (step + 2); i += BS_THREADS) {
-        const int k = i / (step + 2), p = i - k * (step + 2);
-        const int row = row0 + k, prow = s_wpred[k];
-        int src;
-        if (p < step) src = lin_in[static_cast<size_t>(prow) * a.S_max + p];
-        else if (p == step) src = prow;
-        else src = row;
-        lin_out[static_cast<size_t>(row) * a.S_max + p] = src;
-    }
-    for (int i = tid; i < beam * a.d; i += BS_THREADS) {
-        const int k = i / a.d, c = i - k * a.d;
-        a.x_next[static_cast<size_t>(row0 + k) * a.d + c] =
-            a.emb[static_cast<size_t>(s_wtok[k]) * a.d + c] * a.sqrt_d + a.pe[static_cast<size_t>(step + 1) * a.d + c];
-    }
-    if (a.lm_emb) {
-        for (int i = tid; i < beam * a.lm_d; i += BS_THREADS) {
-            const int k = i / a.lm_d, c = i - k * a.lm_d;
-            const float v = a.lm_emb[static_cast<size_t>(s_wtok[k]) * a.lm_d + c] * a.lm_scale +
-                            a.lm_pe[static_cast<size_t>(step + 1) * a.lm_d + c];
-            a.lm_x_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = v;
-            a.lm_x16_next[static_cast<size_t>(row0 + k) * a.lm_d + c] = float2half_sat(v);
-        }
-        if (tid < beam) a.tok_cache[static_cast<size_t>(row0 + tid) * a.S_max + step + 1] = s_wtok[tid];
-    }
-    __syncthreads();
-    if (tid < beam) a.step_arr[row0 + tid] = step + 1;
+    // ---- winners (thread k handles new beam k) and the bookkeeping
+    float v = 0.0f;
+    int ix = 0, rank = beam;
+    if (tid < beam) { rank = tid; v = s_selv[tid]; ix = s_seli[tid]; }
+    finish_step(a, b, step, rank, v, ix, s_lse, s_wtok, s_wpred);
 }
 
-// step = 0 state: x = emb[bos] * sqrt(d) + pe[0] (the LM's: lm_emb[bos] * lm_scale + lm_pe[0]); beam 0 alive (score 0),
+// step = 0 state: x = emb[bos] * sqrt(d) + pe[0] (the LM's: lm.emb[bos] * lm.scale + lm.pe[0]); beam 0 alive (score 0),
 // others -inf; identity lineage.
 __global__ void beam_reset_kernel(int n_bh, int beam, int S_max, int bos, int* step_arr, float* seq_scores, int* lineage,
                                   int* finished, int* n_full, const float* __restrict__ emb, const float* __restrict__ pe,
-                                  int d, float sqrt_d, float* __restrict__ x, const float* __restrict__ lm_emb,
-                                  const float* __restrict__ lm_pe, int lm_d, float lm_scale, float* __restrict__ lm_x,
-                                  __half* __restrict__ lm_x16, int* __restrict__ tok_cache) {
+                                  int d, float sqrt_d, float* __restrict__ x, const BeamLm lm) {
     const int r = blockIdx.x;
     if (threadIdx.x == 0) {
         step_arr[r] = 0;
@@ -1507,24 +1448,13 @@ __global__ void beam_reset_kernel(int n_bh, int beam, int S_max, int bos, int* s
         if (r % beam == 0) finished[r / beam] = 0;
         if (r == 0) *n_full = 0;
     }
-    const float* e = emb + static_cast<size_t>(bos) * d;
-    for (int i = threadIdx.x; i < d; i += blockDim.x) x[static_cast<size_t>(r) * d + i] = e[i] * sqrt_d + pe[i];
-    if (lm_emb) {
-        for (int i = threadIdx.x; i < lm_d; i += blockDim.x) {
-            const float v = lm_emb[static_cast<size_t>(bos) * lm_d + i] * lm_scale + lm_pe[i];
-            lm_x[static_cast<size_t>(r) * lm_d + i] = v;
-            lm_x16[static_cast<size_t>(r) * lm_d + i] = float2half_sat(v);
-        }
-        if (threadIdx.x == 0) tok_cache[static_cast<size_t>(r) * S_max] = bos;
-    }
+    write_inputs(r, 1, [&](int) { return bos; }, 0, S_max, emb, pe, d, sqrt_d, x, lm, threadIdx.x, blockDim.x);
 }
 
 int beam_reset(int n_bh, int beam, int S_max, int bos, int* step_arr, float* seq_scores, int* lineage, int* finished,
                int* n_full, const float* emb, const float* pe, int d, float* x, const BeamLm* lm, cudaStream_t stream) {
     beam_reset_kernel<<<n_bh, 128, 0, stream>>>(n_bh, beam, S_max, bos, step_arr, seq_scores, lineage, finished, n_full, emb,
-                                                pe, d, sqrtf(static_cast<float>(d)), x, lm ? lm->emb : nullptr,
-                                                lm ? lm->pe : nullptr, lm ? lm->d : 0, lm ? lm->scale : 0.f,
-                                                lm ? lm->x : nullptr, lm ? lm->x16 : nullptr, lm ? lm->tok_cache : nullptr);
+                                                pe, d, sqrtf(static_cast<float>(d)), x, lm ? *lm : BeamLm{});
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }
@@ -1543,8 +1473,7 @@ int beam_step(const BeamStepArgs& p, int B, cudaStream_t stream) {
     a.min_steps = p.min_steps; a.eos = p.eos; a.use_eos_threshold = p.use_eos_threshold; a.length_norm = p.length_norm;
     a.emb = p.emb; a.pe = p.pe; a.d = p.d; a.sqrt_d = sqrtf(static_cast<float>(p.d)); a.x_next = p.x_next;
     a.add_scores = p.add_scores; a.add_row = p.add_row; a.attn_weight = p.attn_weight; a.blank = p.blank; a.add_const = p.add_const;
-    a.lm_emb = p.lm.emb; a.lm_pe = p.lm.pe; a.lm_d = p.lm.d; a.lm_scale = p.lm.scale;
-    a.lm_x_next = p.lm.x; a.lm_x16_next = p.lm.x16; a.tok_cache = p.lm.tok_cache;
+    a.lm = p.lm;
     a.scr_val = nullptr; a.scr_idx = nullptr; a.scr_lse = nullptr;
     if (p.path == 2 || (p.path == 0 && p.beam > BS_MAXB))
         SBK_CUDA_CHECK(launch_k(beam_step_large_kernel, dim3(B), dim3(BS_THREADS), 0, stream, a));
