@@ -321,7 +321,21 @@ int sbk_asr_stream_create(sbk_asr* m, int B, int chunk_size, int left_frames, sb
  * shorter.  No host synchronisation, except when an unlimited left context outgrows its buffer (it doubles). */
 int sbk_asr_stream_encode_chunk(sbk_asr* m, sbk_asr_stream* s, const float* cnn_out_dev, int n_frames, float* enc_out_dev,
                                 void* stream);
-int sbk_asr_stream_reset(sbk_asr_stream* s); /* back to an empty context */
+/* the same with the chunk's frames of row b at cnn_out_dev + b * batch_stride (batch_stride >= n_frames * input_size): a
+ * trimmed slice of sbk_asr_stream_frontend_chunk's window output, read in place */
+int sbk_asr_stream_encode_chunk_strided(sbk_asr* m, sbk_asr_stream* s, const float* cnn_out_dev, long long batch_stride,
+                                        int n_frames, float* enc_out_dev, void* stream);
+/* StreamingFeatureWrapper.forward (lobes/features.py:508-670) over LengthsCapableSequential(Fbank, InputNormalization
+ * (global, eval), ConvolutionFrontEnd): the stream keeps each row's last 2 * pad samples of audio context on the device
+ * (zeros before the first chunk).  wav_chunk_dev [B, n_samples] fp32 -> win_out_dev [B, T2, input_size] fp32, the front
+ * end over the whole window [context | chunk] of 2 * pad + n_samples samples (T2 from sbk_asr_num_frames of that count);
+ * the wrapper's output is frames [pad / stride, T2 - pad / stride) of each row, *n_frames of them, with stride = 4 * hop.
+ * pad: a positive multiple of the stride, the same for every chunk of a stream.  The window's Fbank top_db clamp, STFT
+ * centre padding and CNN reflect padding are those of the whole window, as in the reference.  The chunk must give at most
+ * chunk_size frames, and only the last chunk of a stream may give fewer.  Enqueue only. */
+int sbk_asr_stream_frontend_chunk(sbk_asr* m, sbk_asr_stream* s, const float* wav_chunk_dev, int n_samples, int pad,
+                                  float* win_out_dev, int* n_frames, void* stream);
+int sbk_asr_stream_reset(sbk_asr_stream* s); /* back to an empty context (encoder caches and front-end audio context) */
 void sbk_asr_stream_destroy(sbk_asr_stream* s);
 /* Layer `layer`'s context: *n_rows = cached frames; kv_out [B, n_rows, 2 * d_model] fp16 (per head [key | value], keys
  * RoPE-rotated by stream position) and carry_out [B, (kernel_size - 1) / 2, d_model] fp32 (depthwise-conv inputs), each

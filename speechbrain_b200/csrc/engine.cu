@@ -414,6 +414,12 @@ struct AsrStream {
     int clen = 0, start = 0;          // cached rows, ring slot of the oldest
     bool ended = false;               // a chunk shorter than `chunk` was seen: it must be the last
     int prow = 0;                     // RelPos: rows of P
+    // StreamingFeatureWrapper's audio context: the last 2 * pad samples of each row's previous front-end window, kept in
+    // two buffers that alternate (a chunk reads one and writes the other)
+    int pad = 0;                      // samples of padding on each side of a window (0: the front end has not run)
+    int fe_chunks = 0;                // front-end windows built since the last reset
+    bool fe_ended = false;            // a window gave fewer than `chunk` frames: it must be the last
+    DevBuf wav_carry;  // [2][B][2 * pad] fp32
     DevBuf kv;     // [L][B][cap][2d] fp16
     DevBuf carry;  // [L][B][halo][d] fp32
     DevBuf P;      // RelPos: [L][prow][d] fp16 = linear_pos(pe[r])
@@ -1394,17 +1400,26 @@ int sbk_asr_stream_reset(sbk_asr_stream* ss) {
     AsrStream* s = reinterpret_cast<AsrStream*>(ss);
     SBK_REQUIRE(s, "stream_reset: null stream");
     s->total = 0; s->clen = 0; s->start = 0; s->ended = false;  // the first chunk reads no cache and a zero carry
+    s->fe_chunks = 0; s->fe_ended = false;                        // and the first front-end window zero audio context
     return SBK_OK;
 }
 
-int sbk_asr_stream_encode_chunk(sbk_asr* mm, sbk_asr_stream* ss, const float* cnn_out_dev, int n, float* enc_out_dev,
-                                void* stream) {
-    AsrModel* m = reinterpret_cast<AsrModel*>(mm);
-    AsrStream* s = reinterpret_cast<AsrStream*>(ss);
+// rows [B][n][F] fp32 at src + b * batch_stride + t * F -> dst [B * n, F] fp16 (the fp32 -> fp16 cast of cast_f32_f16)
+__global__ void cast_rows_f16_kernel(const float* __restrict__ src, long long batch_stride, int nF, int B, __half* __restrict__ dst) {
+    const size_t total = (size_t)B * nF;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t b = i / nF, j = i % nF;
+        dst[i] = float2half_sat(src[b * batch_stride + j]);
+    }
+}
+
+static int stream_encode(AsrModel* m, AsrStream* s, const float* cnn_out_dev, long long batch_stride, int n, float* enc_out_dev,
+                         cudaStream_t st) {
     SBK_REQUIRE(m && s && cnn_out_dev && enc_out_dev, "stream_encode_chunk: null argument");
     const sbk_asr_config& c = m->wt->cfg;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     SBK_REQUIRE(n >= 1 && n <= s->chunk, "stream_encode_chunk: %d frames, the chunk size is %d", n, s->chunk);
+    SBK_REQUIRE(batch_stride >= (long long)n * c.input_size, "stream_encode_chunk: batch stride %lld below %d frames of %d",
+                batch_stride, n, c.input_size);
     SBK_REQUIRE(!s->ended, "stream_encode_chunk: only the last chunk of a stream may be shorter than the chunk size");
     const int W = s->clen + n;
     SBK_REQUIRE(s->prow == 0 || W <= s->prow,
@@ -1426,7 +1441,14 @@ int sbk_asr_stream_encode_chunk(sbk_asr* mm, sbk_asr_stream* ss, const float* cn
         s->cap = ncap;
     }
     RC(ensure_workspace(m, s->B, enc_samples(c, n), s->B, 1));
-    RC(cast_f32_f16(cnn_out_dev, m->b.a_in, (size_t)s->B * n * c.input_size, st));
+    if (batch_stride == (long long)n * c.input_size) {
+        RC(cast_f32_f16(cnn_out_dev, m->b.a_in, (size_t)s->B * n * c.input_size, st));
+    } else {  // the chunk's frames inside a longer window of each row (the streaming front end's output)
+        const size_t total = (size_t)s->B * n * c.input_size;
+        cast_rows_f16_kernel<<<(int)std::min<size_t>((total + 255) / 256, SBK_NUM_SMS * 16), 256, 0, st>>>(
+            cnn_out_dev, batch_stride, n * c.input_size, s->B, m->b.a_in);
+        SBK_LAUNCH_CHECK();
+    }
     RC(run_encoder(m, nullptr, s->B, n, nullptr, nullptr, enc_out_dev, st, s));
     s->total += n;
     if (n < s->chunk) s->ended = true;
@@ -1437,6 +1459,83 @@ int sbk_asr_stream_encode_chunk(sbk_asr* mm, sbk_asr_stream* ss, const float* cn
     } else {
         s->clen = W;
     }
+    return SBK_OK;
+}
+
+int sbk_asr_stream_encode_chunk(sbk_asr* mm, sbk_asr_stream* ss, const float* cnn_out_dev, int n, float* enc_out_dev,
+                                void* stream) {
+    AsrModel* m = reinterpret_cast<AsrModel*>(mm);
+    SBK_REQUIRE(m, "stream_encode_chunk: null argument");
+    return stream_encode(m, reinterpret_cast<AsrStream*>(ss), cnn_out_dev, (long long)n * m->wt->cfg.input_size, n,
+                         enc_out_dev, static_cast<cudaStream_t>(stream));
+}
+
+int sbk_asr_stream_encode_chunk_strided(sbk_asr* mm, sbk_asr_stream* ss, const float* cnn_out_dev, long long batch_stride,
+                                        int n, float* enc_out_dev, void* stream) {
+    return stream_encode(reinterpret_cast<AsrModel*>(mm), reinterpret_cast<AsrStream*>(ss), cnn_out_dev, batch_stride, n,
+                         enc_out_dev, static_cast<cudaStream_t>(stream));
+}
+
+// One front-end window per row: win [B][2 * pad + n] = [carry | chunk] (zeros for the carry before a stream's first chunk),
+// and the window's last 2 * pad samples into the other carry buffer.  StreamingFeatureWrapper.forward, lobes/features.py:
+// 615-660.
+__global__ void stream_window_kernel(const float* __restrict__ chunk, int n, int P2, const float* __restrict__ carry_in,
+                                     float* __restrict__ carry_out, float* __restrict__ win) {
+    const int b = blockIdx.y, Lw = P2 + n;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Lw; i += gridDim.x * blockDim.x) {
+        const float v = i < P2 ? (carry_in ? carry_in[(size_t)b * P2 + i] : 0.0f) : chunk[(size_t)b * n + i - P2];
+        win[(size_t)b * Lw + i] = v;
+        if (i >= n) carry_out[(size_t)b * P2 + i - n] = v;
+    }
+}
+
+int sbk_asr_stream_frontend_chunk(sbk_asr* mm, sbk_asr_stream* ss, const float* wav_chunk_dev, int n_samples, int pad,
+                                  float* win_out_dev, int* n_frames, void* stream) {
+    AsrModel* m = reinterpret_cast<AsrModel*>(mm);
+    AsrStream* s = reinterpret_cast<AsrStream*>(ss);
+    SBK_REQUIRE(m && s && wav_chunk_dev && win_out_dev, "stream_frontend_chunk: null argument");
+    const sbk_asr_config& c = m->wt->cfg;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SBK_REQUIRE(m->wt->has_fbank && m->wt->has_cnn && m->wt->glob_mean,
+                "stream_frontend_chunk: the handle needs Fbank, global InputNormalization and CNN weights");
+    const int stride = 4 * c.hop;  // the Fbank hop times the front end's two stride-2 blocks
+    SBK_REQUIRE(pad > 0 && pad % stride == 0, "stream_frontend_chunk: pad=%d is not a positive multiple of the stride %d",
+                pad, stride);
+    SBK_REQUIRE(s->pad == 0 || s->pad == pad, "stream_frontend_chunk: pad=%d, the stream was started with pad=%d", pad, s->pad);
+    SBK_REQUIRE(n_samples >= 1, "stream_frontend_chunk: empty chunk");
+    const int P2 = 2 * pad, Lw = P2 + n_samples, trim = pad / stride;
+    int T0, T1, T2;
+    frames(c, Lw, &T0, &T1, &T2);
+    const int n = T2 - 2 * trim;
+    SBK_REQUIRE(n >= 1 && n <= s->chunk, "stream_frontend_chunk: %d samples give %d frames, the chunk size is %d", n_samples,
+                n, s->chunk);
+    // the encoder's own limits too, so that a chunk it would refuse leaves the audio context where it was
+    SBK_REQUIRE(!s->fe_ended && !s->ended,
+                "stream_frontend_chunk: only the last chunk of a stream may be shorter than the chunk size");
+    SBK_REQUIRE(s->prow == 0 || s->clen + n <= s->prow,
+                "stream_frontend_chunk: an unlimited left context holds at most max_len=%d frames with RelPosMHAXL", s->prow);
+    if (s->pad == 0) {
+        if (cudaMalloc(&s->wav_carry.base, (size_t)2 * s->B * P2 * 4) != cudaSuccess) {
+            set_error("stream_frontend_chunk: cudaMalloc(%zu) failed", (size_t)2 * s->B * P2 * 4);
+            return SBK_ERR_NOMEM;
+        }
+        s->wav_carry.cap = (size_t)2 * s->B * P2 * 4;
+        s->pad = pad;
+    }
+    RC(ensure_workspace(m, s->B, Lw, s->B, 1));
+    float* carry = static_cast<float*>(s->wav_carry.base);
+    const int k = s->fe_chunks & 1;
+    dim3 grid(std::min(ceil_div(Lw, 256), 64), s->B);
+    stream_window_kernel<<<grid, 256, 0, st>>>(wav_chunk_dev, n_samples, P2, s->fe_chunks ? carry + (size_t)k * s->B * P2 : nullptr,
+                                              carry + (size_t)(1 - k) * s->B * P2, m->b.wav);
+    SBK_LAUNCH_CHECK();
+    AsrModel::Buf& b = m->b;
+    RC(fbank_forward(m->wt->fbank, b.wav, s->B, Lw, b.feats, b.utt_max, m->wt->glob_mean, m->wt->glob_std,
+                     c.norm_eps > 0.0f ? c.norm_eps : 1e-10f, st));
+    RC(run_cnn(m, b.feats, s->B, T0, win_out_dev, st));
+    s->fe_chunks += 1;
+    if (n < s->chunk) s->fe_ended = true;
+    if (n_frames) *n_frames = n;
     return SBK_OK;
 }
 

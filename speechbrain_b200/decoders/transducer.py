@@ -188,6 +188,18 @@ class TransducerBeamSearcher(torch.nn.Module):
         ``hidden_state`` = ``(out_PN [B, 1, J], (h [1, B, H], c [1, B, H]))`` as returned with ``return_hidden``.
         Returns (hyps list[list[int]], exp(score).mean() over the batch, None, None[, (out_PN, (h, c))]); the state
         tensors are new tensors (the reference updates the passed-in ones in place)."""
+        B, r = self._enqueue_search(tn_output, hidden_state, max_symbols_per_step)
+        n = r["n_tokens"].cpu().tolist()
+        toks = r["tokens"].cpu()
+        hyps = [toks[b, :n[b]].tolist() for b in range(B)]
+        score = r["logp_sum"].cpu().exp().mean()
+        ret = (hyps, score, None, None)
+        if return_hidden:
+            ret += ((r["out_pn"].unsqueeze(1), (r["h"].unsqueeze(0), r["c"].unsqueeze(0))),)
+        return ret
+
+    def _enqueue_search(self, tn_output, hidden_state, max_symbols_per_step):
+        """Checks the arguments and enqueues the device search: (B, the dict of device tensors of _DeviceSearch.greedy)."""
         require_cuda(tn_output, "TransducerBeamSearcher")
         if tn_output.ndim != 3:
             raise ValueError(f"TransducerBeamSearcher: tn_output must be [B, T, J], got {tuple(tn_output.shape)}")
@@ -206,21 +218,16 @@ class TransducerBeamSearcher(torch.nn.Module):
         if T == 0:
             raise ValueError("TransducerBeamSearcher: tn_output has no frames")
         tn = tn_output.detach().to(torch.float32).contiguous()
-        r = s.greedy(tn, self.blank_id, int(max_symbols_per_step), state)
-        n = r["n_tokens"].cpu().tolist()
-        toks = r["tokens"].cpu()
-        hyps = [toks[b, :n[b]].tolist() for b in range(B)]
-        score = r["logp_sum"].cpu().exp().mean()
-        ret = (hyps, score, None, None)
-        if return_hidden:
-            ret += ((r["out_pn"].unsqueeze(1), (r["h"].unsqueeze(0), r["c"].unsqueeze(0))),)
-        return ret
+        return B, s.greedy(tn, self.blank_id, int(max_symbols_per_step), state)
 
     def transducer_greedy_decode_streaming(self, x: torch.Tensor, context: TransducerGreedySearcherStreamingContext):
-        """decoders/transducer.py:293-318: decode a chunk, carrying ``(out_PN, hidden)`` in ``context``."""
-        hyp, _scores, _, _, hidden = self.transducer_greedy_decode(x, context.hidden, return_hidden=True)
-        context.hidden = hidden
-        return hyp
+        """decoders/transducer.py:293-318: decode a chunk, carrying ``(out_PN, hidden)`` in ``context`` on the device.  The
+        reference discards the score here, so it is not fetched: the token counts and ids come to the host in one copy,
+        the call's only host synchronisation."""
+        B, r = self._enqueue_search(x, context.hidden, 5)
+        packed = torch.cat([r["n_tokens"].unsqueeze(1), r["tokens"]], dim=1).cpu()
+        context.hidden = (r["out_pn"].unsqueeze(1), (r["h"].unsqueeze(0), r["c"].unsqueeze(0)))
+        return [packed[b, 1:1 + int(packed[b, 0])].tolist() for b in range(B)]
 
     def transducer_beam_search_decode(self, tn_output):
         raise NotImplementedError("speechbrain_b200.TransducerBeamSearcher: transducer beam search is not built")

@@ -439,15 +439,40 @@ class EncoderStream:
             pass
 
     def encode_chunk(self, src):
-        src = src.float().contiguous()
+        """src [B, n, input_size]; rows that are slices of longer contiguous rows (the front end's trimmed window) are read
+        in place."""
         B, n, F = src.shape
         if B != self.B or F != self.engine.cfg["input_size"]:
             raise ValueError(f"EncoderStream: expected [{self.B}, n, {self.engine.cfg['input_size']}], got {list(src.shape)}")
         out = torch.empty(B, n, self.engine.cfg["d_model"], device=src.device, dtype=torch.float32)
+        strided = src.dtype == torch.float32 and src.stride(2) == 1 and src.stride(1) == F and src.stride(0) > n * F
+        if not strided:
+            src = src.float().contiguous()
         with torch.cuda.device(self.engine.device):
-            check(lib().sbk_asr_stream_encode_chunk(self.engine._h, self._s, ptr(src), n, ptr(out), self.engine._sp()),
-                  "sbk_asr_stream_encode_chunk")
+            if strided:
+                check(lib().sbk_asr_stream_encode_chunk_strided(self.engine._h, self._s, ctypes.c_void_p(src.data_ptr()),
+                                                                ctypes.c_longlong(src.stride(0)),
+                                                                n, ptr(out), self.engine._sp()),
+                      "sbk_asr_stream_encode_chunk_strided")
+            else:
+                check(lib().sbk_asr_stream_encode_chunk(self.engine._h, self._s, ptr(src), n, ptr(out), self.engine._sp()),
+                      "sbk_asr_stream_encode_chunk")
         return out
+
+    def frontend_chunk(self, wav, pad):
+        """StreamingFeatureWrapper's device front end: wav [B, n_samples] behind the stream's last 2 * pad samples ->
+        (window output [B, T2, input_size] fp32, trimmed frames per side, frames kept)."""
+        wav = wav.float().contiguous()
+        B, L = wav.shape
+        if B != self.B:
+            raise ValueError(f"EncoderStream: a chunk of {B} rows for a stream of {self.B}")
+        _, T2 = self.engine.num_frames(2 * pad + L)
+        out = torch.empty(B, T2, self.engine.cfg["input_size"], device=wav.device, dtype=torch.float32)
+        n = ctypes.c_int()
+        with torch.cuda.device(self.engine.device):
+            check(lib().sbk_asr_stream_frontend_chunk(self.engine._h, self._s, ptr(wav), L, int(pad), ptr(out), ctypes.byref(n),
+                                                      self.engine._sp()), "sbk_asr_stream_frontend_chunk")
+        return out, pad // (4 * self.engine.cfg["hop"]), n.value
 
     def reset(self):
         check(lib().sbk_asr_stream_reset(self._s), "sbk_asr_stream_reset")

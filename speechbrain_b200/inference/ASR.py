@@ -17,6 +17,10 @@ The waveform -> encoder states part runs as ONE fused device pipeline (Fbank + C
 ``sbk_asr_transcribe_greedy_*`` / ``sbk_asr_encode``); a greedy decoder stays inside the same call (one CUDA-graph-able
 pipeline wav -> token ids), a beam decoder runs ``sbk_asr_beam_from_enc`` on the states.  One repacked engine is shared
 by every mirror involved (engine_cache.py)."""
+import types
+from dataclasses import dataclass
+from typing import Any, List, Optional
+
 import torch
 
 from ..decoders.seq2seq import (S2STransformerBeamSearcher, S2STransformerGreedySearcher, greedy_exit_step, greedy_outputs)
@@ -304,3 +308,130 @@ class EncoderASR(torch.nn.Module):
     def forward(self, wavs, wav_lens):
         """Runs the encoder (the reference's forward returns encode_batch)."""
         return self.encode_batch(wavs, wav_lens)
+
+
+@dataclass
+class ASRStreamingContext:
+    """inference/ASR.py:947-975: the mutable state of one streaming session, passed to every chunk call."""
+
+    config: Any
+    """The DynChunkTrainConfig the context was made for."""
+    fea_extractor_context: Any
+    """StreamingFeatureWrapperContext, bound to the encoder context's device stream (which holds the audio context)."""
+    encoder_context: Any
+    """TransformerASRStreamingContext: per-layer device caches."""
+    decoder_context: Any
+    """The decoder's streaming context (TransducerGreedySearcherStreamingContext)."""
+    tokenizer_context: Optional[List[Any]] = None
+    """One detokeniser context per row, made by the first ``decode_chunk``."""
+
+
+class StreamingASR(torch.nn.Module):
+    """Drop-in for speechbrain.inference.ASR.StreamingASR (inference/ASR.py:978-1363): audio chunks to text for the
+    streaming Conformer-Transducer.
+
+    Per chunk, on the caller's stream: the feature wrapper's device front end over [audio context | chunk]
+    (``sbk_asr_stream_frontend_chunk``), the encoder on its per-layer device caches (``enc.forward_streaming``), ``proj_enc``
+    on the wgmma GEMM and the greedy transducer kernel carrying ``(out_PN, (h, c))``; the tokens then come to the host
+    for the SentencePiece detokeniser.  ``hparams`` as the recipe's inference block builds them: ``fea_streaming_extractor``
+    (a ``StreamingFeatureWrapper`` over Fbank, global InputNormalization and the ConvolutionFrontEnd),
+    ``make_decoder_streaming_context``, ``decoding_function`` (``TransducerBeamSearcher.transducer_greedy_decode_streaming``
+    bound to a greedy searcher), ``make_tokenizer_streaming_context``, ``tokenizer_decode_streaming`` and ``tokenizer``.
+
+    The B rows of a batch advance together, and only the last chunk of a stream may be shorter than
+    ``get_chunk_size_frames``: to flush a stream, append the recommended zero chunks to its audio before splitting it.
+    ``transcribe_file`` / ``transcribe_file_streaming`` need audio file decoding, which is not built."""
+    HPARAMS_NEEDED = ["fea_streaming_extractor", "make_decoder_streaming_context", "decoding_function",
+                      "make_tokenizer_streaming_context", "tokenizer_decode_streaming"]
+    MODULES_NEEDED = ["enc", "proj_enc"]
+
+    def __init__(self, modules=None, hparams=None, run_opts=None, freeze_params=True):
+        super().__init__()
+        from ..lobes.features import StreamingFeatureWrapper
+        from ..nnet.linear import Linear
+        modules = dict(modules or {})
+        for k in self.MODULES_NEEDED:
+            if k not in modules:
+                raise ValueError(f"Need modules['{k}']")
+        self.mods = torch.nn.ModuleDict(modules)
+        hp = dict(hparams) if isinstance(hparams, dict) else (dict(vars(hparams)) if hparams is not None else {})
+        for k in self.HPARAMS_NEEDED:
+            if k not in hp:
+                raise ValueError(f"Need hparams['{k}']")
+        self.hparams = types.SimpleNamespace(**hp)
+        if not isinstance(self.mods["enc"], EncoderWrapper):
+            raise NotImplementedError("speechbrain_b200.StreamingASR: modules['enc'] must be an EncoderWrapper(TransformerASR)")
+        if not isinstance(self.mods["proj_enc"], Linear):
+            raise NotImplementedError("speechbrain_b200.StreamingASR: modules['proj_enc'] must be a speechbrain_b200 Linear")
+        fea = self.hparams.fea_streaming_extractor
+        if not isinstance(fea, StreamingFeatureWrapper):
+            raise NotImplementedError("speechbrain_b200.StreamingASR: fea_streaming_extractor must be a speechbrain_b200 "
+                                      "StreamingFeatureWrapper")
+        self.filter_props = fea.properties
+        self.device = torch.device((run_opts or {}).get("device", "cuda:0"))
+        object.__setattr__(self, "_slot", self.mods["enc"].transformer.engine_slot(("streaming", id(fea))))
+
+    @classmethod
+    def from_hparams(cls, source, hparams_file="hyperparams.yaml", overrides=None, savedir=None, run_opts=None, **kwargs):
+        """Loads a LOCAL directory in the layout of the recipe's inference hparams (see EncoderDecoderASR.from_hparams)."""
+        from ..utils.hparams import load_pretrained_interface
+        return load_pretrained_interface(cls, source, hparams_file, overrides or {}, run_opts or {})
+
+    def engine(self):
+        """The engine holding this model's front end and encoder: the one the streams run on."""
+        fea = self.hparams.fea_streaming_extractor
+        return self._slot.get(self.device, ("fbank", "cnn", "encoder"),
+                              {"fbank": fea.fbank, "normalize": fea.normalize, "CNN.": fea.cnn})
+
+    def transcribe_file_streaming(self, path, dynchunktrain_config, use_torchaudio_streaming=True, **kwargs):
+        raise NotImplementedError("speechbrain_b200.StreamingASR: audio file decoding is not built (this torchaudio has no "
+                                  "torchaudio.io); load the audio yourself and call transcribe_chunk per chunk")
+
+    def transcribe_file(self, path, dynchunktrain_config, use_torchaudio_streaming=True):
+        raise NotImplementedError("speechbrain_b200.StreamingASR: audio file decoding is not built (this torchaudio has no "
+                                  "torchaudio.io); load the audio yourself and call transcribe_chunk per chunk")
+
+    def make_streaming_context(self, dynchunktrain_config):
+        enc_ctx = self.mods["enc"].make_streaming_context(dynchunktrain_config)
+        enc_ctx.encoder_context.slot = self._slot
+        fea_ctx = self.hparams.fea_streaming_extractor.make_streaming_context()
+        fea_ctx.stream_owner = enc_ctx.encoder_context
+        return ASRStreamingContext(config=dynchunktrain_config, fea_extractor_context=fea_ctx, encoder_context=enc_ctx,
+                                   decoder_context=self.hparams.make_decoder_streaming_context(), tokenizer_context=None)
+
+    def get_chunk_size_frames(self, dynchunktrain_config) -> int:
+        """Samples per chunk, (stride - 1) * chunk_size, as the reference computes it."""
+        return (self.filter_props.stride - 1) * dynchunktrain_config.chunk_size
+
+    @torch.no_grad()
+    def encode_chunk(self, context, chunk, chunk_len=None):
+        """chunk [B, n_samples <= get_chunk_size_frames] -> proj_enc(encoder output) [B, frames, joint]."""
+        if chunk_len is None:
+            chunk_len = torch.ones((chunk.size(0),))
+        if chunk.dim() != 2 or chunk.shape[-1] > self.get_chunk_size_frames(context.config):
+            raise ValueError(f"StreamingASR.encode_chunk: a chunk of shape {tuple(chunk.shape)}; expected [batch, <= "
+                             f"{self.get_chunk_size_frames(context.config)}] samples")
+        # chunk_len stays where it is: with global statistics in eval mode it changes no value (see the wrapper)
+        chunk = chunk.float().to(self.device)
+        context.encoder_context.encoder_context.ensure_stream(self.engine(), chunk.shape[0])
+        x = self.hparams.fea_streaming_extractor(chunk, context=context.fea_extractor_context, lengths=chunk_len)
+        x = self.mods["enc"].forward_streaming(x, context.encoder_context)
+        return self.mods["proj_enc"](x)
+
+    @torch.no_grad()
+    def decode_chunk(self, context, x):
+        """-> (text per row for this chunk, tokens per row)."""
+        tokens = self.hparams.decoding_function(x, context.decoder_context)
+        if context.tokenizer_context is None:
+            context.tokenizer_context = [self.hparams.make_tokenizer_streaming_context() for _ in range(len(tokens))]
+        words = [self.hparams.tokenizer_decode_streaming(self.hparams.tokenizer, cur_tokens, context.tokenizer_context[i])
+                 for i, cur_tokens in enumerate(tokens)]
+        return words, tokens
+
+    def transcribe_chunk(self, context, chunk, chunk_len=None):
+        """The text of one more chunk of every row (possibly empty strings)."""
+        if chunk_len is None:
+            chunk_len = torch.ones((chunk.size(0),))
+        x = self.encode_chunk(context, chunk, chunk_len)
+        words, _ = self.decode_chunk(context, x)
+        return words

@@ -4,10 +4,14 @@ Same constructor, ``forward(wav) -> [B, T_f, n_mels]`` and ``state_dict`` keys (
 Built natively: frozen triangular filters, no deltas, no context, mono [B, L] input -- i.e. what every ASR
 recipe on the hot path uses (conformer_{small,large}.yaml).  Anything else raises (there is no CPU fallback).
 """
+from dataclasses import dataclass
+from typing import Any, Optional
+
 import torch
 
 from .._lib import require_cuda
 from ..engine import FbankHandle, mel_filter_matrix, stft_window
+from ..utils.filter_analysis import FilterProperties, upalign_value  # noqa: F401  (upalign_value: the reference's home)
 
 
 class _DeltasBuffer(torch.nn.Module):
@@ -60,7 +64,80 @@ class Fbank(torch.nn.Module):
         return self._get_handle().forward(wav)
 
     def get_filter_properties(self):
-        """(window_size, stride) of the STFT, as processing/features.py:190-198 reports them."""
-        if self.n_fft % 2 == 0:
-            raise ValueError("Cannot determine the filter properties of an even-sized window STFT")
-        return {"window_size": self.n_fft, "stride": self.hop_length}
+        """The centred STFT's window and hop in samples (lobes/features.py:171-173, processing/features.py:190-198)."""
+        return FilterProperties(window_size=self.win_length, stride=self.hop_length)
+
+
+@dataclass
+class StreamingFeatureWrapperContext:
+    """lobes/features.py:495-505.  ``left_context`` is None before the first chunk and then True: the carried samples
+    themselves stay on the device, in ``stream`` (the ``EncoderStream`` of the streaming encoder context this context
+    is bound to by ``StreamingASR.make_streaming_context``)."""
+
+    left_context: Optional[bool] = None
+    stream_owner: Any = None  # a ConformerEncoderStreamingContext: its ``stream`` holds the audio context
+
+
+class StreamingFeatureWrapper(torch.nn.Module):
+    """StreamingFeatureWrapper (lobes/features.py:508-670): runs a filter chunk by chunk, each chunk behind the last
+    2 * pad samples of the previous window (zeros before the first), and trims pad / stride output frames off each side,
+    with pad = upalign((window_size - 1) // 2, stride).
+
+    Built for one module: ``LengthsCapableSequential(Fbank, InputNormalization(norm_type="global"), ConvolutionFrontEnd)``
+    (the streaming Conformer-Transducer recipe's).  The window is assembled and the fused Fbank + CMVN and front-end
+    kernels run over it on the device (``sbk_asr_stream_frontend_chunk``), so the STFT's centre padding, the top_db clamp
+    and the CNN's reflect padding are those of the whole window, as in the reference.  With global statistics in eval
+    mode ``lengths`` changes no value (the reference also normalises the padded samples), so it is accepted and unused."""
+
+    def __init__(self, module, properties):
+        super().__init__()
+        self.module = module
+        self.properties = properties
+        if self.properties.causal:
+            raise ValueError("Causal streaming feature wrapper is not yet supported")
+        if self.properties.dilation != 1:
+            raise ValueError("Dilation not yet supported in streaming feature wrapper")
+        from ..lobes.models.convolution import ConvolutionFrontEnd
+        from ..nnet.containers import LengthsCapableSequential
+        from ..processing.features import InputNormalization
+        parts = list(module.values()) if isinstance(module, LengthsCapableSequential) else []
+        if (len(parts) != 3 or not isinstance(parts[0], Fbank) or not isinstance(parts[1], InputNormalization)
+                or parts[1].norm_type != "global" or not isinstance(parts[2], ConvolutionFrontEnd)):
+            raise NotImplementedError("speechbrain_b200.StreamingFeatureWrapper: the module must be LengthsCapableSequential("
+                                      "Fbank, InputNormalization(norm_type='global'), ConvolutionFrontEnd)")
+        self.fbank, self.normalize, self.cnn = parts
+        # the device trims pad / (hop * 4) frames: properties that are not this module's would trim differently
+        if self.properties.stride != 4 * self.fbank.hop_length:
+            raise ValueError(f"StreamingFeatureWrapper: properties.stride={self.properties.stride}, but the module's stride "
+                             f"is {4 * self.fbank.hop_length} (Fbank hop x the front end's two stride-2 blocks)")
+
+    def get_required_padding(self) -> int:
+        return upalign_value((self.properties.window_size - 1) // 2, self.properties.stride)
+
+    def get_output_count_per_pad_frame(self) -> int:
+        return self.get_required_padding() // self.properties.stride
+
+    def get_recommended_final_chunk_count(self, frames_per_chunk: int) -> int:
+        return upalign_value(self.get_required_padding(), frames_per_chunk) // frames_per_chunk
+
+    @torch.no_grad()
+    def forward(self, chunk, context, *extra_args, lengths=None, **extra_kwargs):
+        """chunk [B, n_samples] on the device -> features [B, frames, input_size]: a view of the window's front-end output
+        (the frames the reference keeps after trimming), enqueued on the current stream."""
+        del extra_args, extra_kwargs, lengths
+        require_cuda(chunk, "StreamingFeatureWrapper")
+        owner = context.stream_owner
+        if owner is None or owner.stream is None:
+            raise RuntimeError("StreamingFeatureWrapper: the device front end keeps its audio context in a streaming "
+                               "encoder's device stream; use a context from StreamingASR.make_streaming_context")
+        if chunk.dim() != 2:
+            raise ValueError(f"StreamingFeatureWrapper: expected a [batch, time] chunk, got {tuple(chunk.shape)}")
+        out, trim, n = owner.stream.frontend_chunk(chunk, self.get_required_padding())
+        context.left_context = owner.started = True
+        return out[:, trim:trim + n]
+
+    def get_filter_properties(self):
+        return self.properties
+
+    def make_streaming_context(self):
+        return StreamingFeatureWrapperContext(None)

@@ -8,6 +8,7 @@ Same constructor and state_dict keys; other configurations raise (no CPU fallbac
 import torch
 
 from ..._lib import require_cuda
+from ...utils.filter_analysis import FilterProperties, stack_filter_properties
 from ...utils.param_tree import build_param_tree, default_init
 from ...utils.shapes import cnn3_frontend_shapes, cnn_frontend_shapes
 
@@ -35,10 +36,17 @@ class ConvolutionFrontEnd(torch.nn.Module):
                 "residuals=(False, False, True)) are built")
         self.n_mels = int(input_shape[-1])
         self.num_blocks = num_blocks
+        # one Conv2d per block: its (kernel, stride) along time (ConvBlock.filter_properties, convolution.py:283-289)
+        self._block_filters = [FilterProperties(window_size=k, stride=s)
+                               for k, s in zip(kernel_sizes[:num_blocks], strides[:num_blocks])]
         self.out_channels = tuple(out_channels[:2])
         shapes = cnn3_frontend_shapes(self.n_mels) if transformer else cnn_frontend_shapes(self.n_mels, self.out_channels)
         build_param_tree(self, shapes, default_init)
         object.__setattr__(self, "_slot", None)
+
+    def get_filter_properties(self):
+        """The blocks' filters stacked (convolution.py:200-203, 319-320)."""
+        return stack_filter_properties(self._block_filters)
 
     def _engine_cfg(self):
         f2 = ((self.n_mels - 1) // 2 + 1 - 1) // 2 + 1

@@ -263,14 +263,8 @@ class TransformerASR(torch.nn.Module):
         if src.dim() == 4:
             src = src.reshape(src.shape[0], src.shape[1], -1)
         ec = context.encoder_context
-        eng = self._get_engine(src.device)
-        if ec.stream is None or ec.stream.engine is not eng or ec.stream.B != src.shape[0]:
-            if ec.stream is not None and ec.frames > 0:
-                raise ValueError("encode_streaming: the batch size or the model's weights changed inside a stream")
-            cfg = context.dynchunktrain_config
-            left = None if cfg.is_infinite_left_context() else cfg.left_context_size * cfg.chunk_size
-            ec.stream = eng.stream_create(src.shape[0], cfg.chunk_size, left)
-        out = ec.stream.encode_chunk(src)
+        eng = ec.slot.get(src.device, ("encoder",)) if ec.slot is not None else self._get_engine(src.device)
+        out = ec.ensure_stream(eng, src.shape[0]).encode_chunk(src)
         ec.frames += src.shape[1]
         return out
 
@@ -346,16 +340,31 @@ class ConformerEncoderStreamingContext:
         cfg = dynchunktrain_config
         # frames of left context per layer; None: every frame so far (the reference has no such mode)
         size = None if cfg.is_infinite_left_context() else cfg.left_context_size * cfg.chunk_size
+        self.config = cfg
         self.stream = None  # speechbrain_b200.engine.EncoderStream, created by the first chunk
         self.frames = 0
+        self.started = False  # the streaming front end has taken a chunk since the last reset
         self.nhead = nhead
+        self.slot = None  # the EngineSlot whose engine runs the stream (StreamingASR: the one that also holds the front end)
         self.layers = [ConformerEncoderLayerStreamingContext(self, i, size) for i in range(num_layers)]
+
+    def ensure_stream(self, eng, B):
+        """The device stream of B rows on ``eng``, created on first use (and again when the batch size or the weights
+        changed before the stream took any chunk)."""
+        if self.stream is None or self.stream.engine is not eng or self.stream.B != B:
+            if self.stream is not None and (self.frames > 0 or self.started):
+                raise ValueError("encode_streaming: the batch size or the model's weights changed inside a stream")
+            cfg = self.config
+            left = None if cfg.is_infinite_left_context() else cfg.left_context_size * cfg.chunk_size
+            self.stream = eng.stream_create(B, cfg.chunk_size, left)
+        return self.stream
 
     def reset(self):
         """Back to an empty context (the device buffers are kept for the next stream of the same batch size)."""
         if self.stream is not None:
             self.stream.reset()
         self.frames = 0
+        self.started = False
 
 
 class TransformerASRStreamingContext:

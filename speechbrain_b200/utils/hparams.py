@@ -210,7 +210,7 @@ def load_pretrained_interface(cls, source, hparams_file="hyperparams.yaml", over
     missing = [k for k in getattr(cls, "HPARAMS_NEEDED", []) if k not in hp]
     if missing:
         raise ValueError(f"Need hparams {missing}")
-    for opt in ("transformer_beam_search", "transducer_beam_search", "sample_rate", "test_beam_search"):
+    for opt in ("transformer_beam_search", "transducer_beam_search", "sample_rate", "test_beam_search", "tokenizer"):
         if opt in hp:
             needed[opt] = hp[opt]
     return cls(modules=modules, hparams=types.SimpleNamespace(**needed), run_opts=run_opts)
