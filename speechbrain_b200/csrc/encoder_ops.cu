@@ -18,88 +18,93 @@ namespace sbk {
 // norm_mhsa / norm_conv of the same x, Branchformer.py:204-221).
 constexpr int LN_MAX_PER_LANE = 32;
 
+// One warp's row of D values, float4 vi = lane + 32 i in v[4 i .. 4 i + 3] (zeros past the row).  The mean sums each float4
+// as (x + y) + (z + w) and the variance adds the centred squares one by one: every LayerNorm kernel here keeps that order, so
+// they agree bit for bit.
+struct LnRow {
+    float v[LN_MAX_PER_LANE];
+    float mean, rstd;
+    int lane, D, nv;  // nv: float4 vectors per row (D % 4 == 0)
+
+    __device__ __forceinline__ LnRow(const float* xr, int lane_, int D_) : lane(lane_), D(D_), nv(D_ >> 2) {
+#pragma unroll
+        for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
+            const int vi = lane + i * 32;
+            float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (vi < nv) t = *reinterpret_cast<const float4*>(xr + vi * 4);
+            v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+        }
+    }
+    __device__ __forceinline__ void stats(float eps) {
+        float s = 0.0f;
+#pragma unroll
+        for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) s += (v[4 * i] + v[4 * i + 1]) + (v[4 * i + 2] + v[4 * i + 3]);
+        mean = warp_sum(s) / D;
+        float q = 0.0f;
+#pragma unroll
+        for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i)
+            if (lane + i * 32 < nv) {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float d = v[4 * i + j] - mean;
+                    q += d * d;
+                }
+            }
+        rstd = rsqrtf(warp_sum(q) / D + eps);
+    }
+    // float4 i of the row normalised with gamma / beta float4s g, b
+    __device__ __forceinline__ float4 norm(int i, float4 g, float4 b) const {
+        return make_float4((v[4 * i] - mean) * rstd * g.x + b.x, (v[4 * i + 1] - mean) * rstd * g.y + b.y,
+                           (v[4 * i + 2] - mean) * rstd * g.z + b.z, (v[4 * i + 3] - mean) * rstd * g.w + b.w);
+    }
+    // y -> float4 vi of the row at out + off, fp16 or fp32
+    template <bool OUT_HALF>
+    __device__ __forceinline__ static void store(void* out, size_t off, int vi, float4 y) {
+        if constexpr (OUT_HALF) {
+            __half2 h0 = floats2half2_sat(y.x, y.y), h1 = floats2half2_sat(y.z, y.w);
+            uint2 u;
+            u.x = *reinterpret_cast<uint32_t*>(&h0);
+            u.y = *reinterpret_cast<uint32_t*>(&h1);
+            *reinterpret_cast<uint2*>(static_cast<__half*>(out) + off + vi * 4) = u;
+        } else {
+            *reinterpret_cast<float4*>(static_cast<float*>(out) + off + vi * 4) = y;
+        }
+    }
+};
+
+__device__ __forceinline__ float4 ldg4(const float* p, int vi) { return __ldg(reinterpret_cast<const float4*>(p + vi * 4)); }
+
 template <bool OUT_HALF, bool PDL, bool DUAL = false>
 __global__ void __launch_bounds__(256)
 layernorm_rows_kernel(const float* __restrict__ x, void* __restrict__ out, const float* __restrict__ gamma,
-                      const float* __restrict__ beta, int M, int D, float eps, int act_silu,
-                      __half* __restrict__ out2 = nullptr, const float* __restrict__ gamma2 = nullptr,
-                      const float* __restrict__ beta2 = nullptr) {
+                      const float* __restrict__ beta, int M, int D, float eps, __half* __restrict__ out2 = nullptr,
+                      const float* __restrict__ gamma2 = nullptr, const float* __restrict__ beta2 = nullptr) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
-    const int nv = D >> 2;  // float4 vectors per row (D % 4 == 0)
     float4 gp[PDL ? LN_MAX_PER_LANE / 4 : 1], bp[PDL ? LN_MAX_PER_LANE / 4 : 1];
     if constexpr (PDL) {
 #pragma unroll
         for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
             const int vi = lane + i * 32;
-            if (vi < nv && row < M) {
-                gp[i] = __ldg(reinterpret_cast<const float4*>(gamma + vi * 4));
-                bp[i] = __ldg(reinterpret_cast<const float4*>(beta + vi * 4));
+            if (vi < D >> 2 && row < M) {
+                gp[i] = ldg4(gamma, vi);
+                bp[i] = ldg4(beta, vi);
             }
         }
         pdl_trigger();
         pdl_wait();
     }
     if (row >= M) return;
-    const float* xr = x + static_cast<size_t>(row) * D;
-    float v[LN_MAX_PER_LANE];
-    float s = 0.0f;
+    const size_t off = static_cast<size_t>(row) * D;
+    LnRow r(x + off, lane, D);
+    r.stats(eps);
 #pragma unroll
     for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
         const int vi = lane + i * 32;
-        if (vi < nv) {
-            const float4 t = *reinterpret_cast<const float4*>(xr + vi * 4);
-            v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
-            s += (t.x + t.y) + (t.z + t.w);
-        } else {
-            v[4 * i] = v[4 * i + 1] = v[4 * i + 2] = v[4 * i + 3] = 0.0f;
-        }
-    }
-    const float mean = warp_sum(s) / D;
-    float q = 0.0f;
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
-        const int vi = lane + i * 32;
-        if (vi < nv) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float d = v[4 * i + j] - mean;
-                q += d * d;
-            }
-        }
-    }
-    const float rstd = rsqrtf(warp_sum(q) / D + eps);
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
-        const int vi = lane + i * 32;
-        if (vi < nv) {
-            const float4 g = PDL ? gp[PDL ? i : 0] : __ldg(reinterpret_cast<const float4*>(gamma + vi * 4));
-            const float4 b = PDL ? bp[PDL ? i : 0] : __ldg(reinterpret_cast<const float4*>(beta + vi * 4));
-            float y0 = (v[4 * i] - mean) * rstd * g.x + b.x;
-            float y1 = (v[4 * i + 1] - mean) * rstd * g.y + b.y;
-            float y2 = (v[4 * i + 2] - mean) * rstd * g.z + b.z;
-            float y3 = (v[4 * i + 3] - mean) * rstd * g.w + b.w;
-            if (act_silu) { y0 = silu_f(y0); y1 = silu_f(y1); y2 = silu_f(y2); y3 = silu_f(y3); }
-            if constexpr (OUT_HALF) {
-                __half2 h0 = floats2half2_sat(y0, y1), h1 = floats2half2_sat(y2, y3);
-                uint2 u;
-                u.x = *reinterpret_cast<uint32_t*>(&h0);
-                u.y = *reinterpret_cast<uint32_t*>(&h1);
-                *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(out) + static_cast<size_t>(row) * D + vi * 4) = u;
-            } else {
-                *reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + static_cast<size_t>(row) * D + vi * 4) =
-                    make_float4(y0, y1, y2, y3);
-            }
-            if constexpr (DUAL) {
-                const float4 g2 = __ldg(reinterpret_cast<const float4*>(gamma2 + vi * 4));
-                const float4 b2 = __ldg(reinterpret_cast<const float4*>(beta2 + vi * 4));
-                __half2 h0 = floats2half2_sat((v[4 * i] - mean) * rstd * g2.x + b2.x, (v[4 * i + 1] - mean) * rstd * g2.y + b2.y);
-                __half2 h1 = floats2half2_sat((v[4 * i + 2] - mean) * rstd * g2.z + b2.z, (v[4 * i + 3] - mean) * rstd * g2.w + b2.w);
-                uint2 u;
-                u.x = *reinterpret_cast<uint32_t*>(&h0);
-                u.y = *reinterpret_cast<uint32_t*>(&h1);
-                *reinterpret_cast<uint2*>(out2 + static_cast<size_t>(row) * D + vi * 4) = u;
-            }
+        if (vi < r.nv) {
+            LnRow::store<OUT_HALF>(out, off, vi, r.norm(i, PDL ? gp[PDL ? i : 0] : ldg4(gamma, vi),
+                                                            PDL ? bp[PDL ? i : 0] : ldg4(beta, vi)));
+            if constexpr (DUAL) LnRow::store<true>(out2, off, vi, r.norm(i, ldg4(gamma2, vi), ldg4(beta2, vi)));
         }
     }
 }
@@ -110,13 +115,13 @@ int layernorm_rows_dual(const float* x, __half* out, const float* gamma, const f
     if (M == 0) return SBK_OK;
     const int rows_per_cta = 8;
     layernorm_rows_kernel<true, false, true><<<ceil_div(M, rows_per_cta), rows_per_cta * 32, 0, stream>>>(
-        x, out, gamma, beta, M, D, eps, 0, out2, gamma2, beta2);
+        x, out, gamma, beta, M, D, eps, out2, gamma2, beta2);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }
 
 int layernorm_rows(const float* x, void* out, bool out_half, const float* gamma, const float* beta, int M, int D,
-                   float eps, bool act_silu, cudaStream_t stream, bool pdl) {
+                   float eps, cudaStream_t stream, bool pdl) {
     SBK_REQUIRE(D % 4 == 0 && D <= 32 * LN_MAX_PER_LANE, "layernorm_rows: D=%d unsupported", D);
     if (M == 0) return SBK_OK;
     const int rows_per_cta = 8;
@@ -124,12 +129,12 @@ int layernorm_rows(const float* x, void* out, bool out_half, const float* gamma,
     if (pdl) {
         SBK_REQUIRE(out_half, "layernorm_rows: the PDL variant writes fp16");
         SBK_CUDA_CHECK(launch_pdl(layernorm_rows_kernel<true, true>, grid, block, 0, stream, true, x, out, gamma, beta, M, D,
-                                  eps, static_cast<int>(act_silu), static_cast<__half*>(nullptr),
-                                  static_cast<const float*>(nullptr), static_cast<const float*>(nullptr)));
+                                  eps, static_cast<__half*>(nullptr), static_cast<const float*>(nullptr),
+                                  static_cast<const float*>(nullptr)));
     } else if (out_half) {
-        layernorm_rows_kernel<true, false><<<grid, block, 0, stream>>>(x, out, gamma, beta, M, D, eps, act_silu);
+        layernorm_rows_kernel<true, false><<<grid, block, 0, stream>>>(x, out, gamma, beta, M, D, eps);
     } else {
-        layernorm_rows_kernel<false, false><<<grid, block, 0, stream>>>(x, out, gamma, beta, M, D, eps, act_silu);
+        layernorm_rows_kernel<false, false><<<grid, block, 0, stream>>>(x, out, gamma, beta, M, D, eps);
     }
     SBK_LAUNCH_CHECK();
     return SBK_OK;
@@ -148,72 +153,23 @@ layernorm2_rows_kernel(const float* __restrict__ x, float* __restrict__ y_out, v
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= M) return;
     const int lane = threadIdx.x & 31;
-    const float* xr = x + static_cast<size_t>(row) * D;
-    float v[LN_MAX_PER_LANE];
-    const int nv = D >> 2;
-    float s = 0.0f;
+    const size_t off = static_cast<size_t>(row) * D;
+    LnRow r(x + off, lane, D);
+    r.stats(eps_a);
 #pragma unroll
     for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
         const int vi = lane + i * 32;
-        float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (vi < nv) t = *reinterpret_cast<const float4*>(xr + vi * 4);
-        v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
-        s += (t.x + t.y) + (t.z + t.w);
-    }
-    float mean = warp_sum(s) / D;
-    float q = 0.0f;
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i)
-        if (lane + i * 32 < nv) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { const float d = v[4 * i + j] - mean; q += d * d; }
-        }
-    float rstd = rsqrtf(warp_sum(q) / D + eps_a);
-    s = 0.0f;
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
-        const int vi = lane + i * 32;
-        if (vi < nv) {
-            const float4 g = __ldg(reinterpret_cast<const float4*>(ga + vi * 4));
-            const float4 b = __ldg(reinterpret_cast<const float4*>(ba + vi * 4));
-            v[4 * i] = (v[4 * i] - mean) * rstd * g.x + b.x;
-            v[4 * i + 1] = (v[4 * i + 1] - mean) * rstd * g.y + b.y;
-            v[4 * i + 2] = (v[4 * i + 2] - mean) * rstd * g.z + b.z;
-            v[4 * i + 3] = (v[4 * i + 3] - mean) * rstd * g.w + b.w;
-            if (y_out != nullptr)
-                *reinterpret_cast<float4*>(y_out + static_cast<size_t>(row) * D + vi * 4) =
-                    make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-            s += (v[4 * i] + v[4 * i + 1]) + (v[4 * i + 2] + v[4 * i + 3]);
+        if (vi < r.nv) {
+            const float4 y = r.norm(i, ldg4(ga, vi), ldg4(ba, vi));
+            if (y_out != nullptr) LnRow::store<false>(y_out, off, vi, y);
+            r.v[4 * i] = y.x; r.v[4 * i + 1] = y.y; r.v[4 * i + 2] = y.z; r.v[4 * i + 3] = y.w;
         }
     }
-    mean = warp_sum(s) / D;
-    q = 0.0f;
-#pragma unroll
-    for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i)
-        if (lane + i * 32 < nv) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { const float d = v[4 * i + j] - mean; q += d * d; }
-        }
-    rstd = rsqrtf(warp_sum(q) / D + eps_b);
+    r.stats(eps_b);
 #pragma unroll
     for (int i = 0; i < LN_MAX_PER_LANE / 4; ++i) {
         const int vi = lane + i * 32;
-        if (vi < nv) {
-            const float4 g = __ldg(reinterpret_cast<const float4*>(gb + vi * 4));
-            const float4 b = __ldg(reinterpret_cast<const float4*>(bb + vi * 4));
-            const float z0 = (v[4 * i] - mean) * rstd * g.x + b.x, z1 = (v[4 * i + 1] - mean) * rstd * g.y + b.y;
-            const float z2 = (v[4 * i + 2] - mean) * rstd * g.z + b.z, z3 = (v[4 * i + 3] - mean) * rstd * g.w + b.w;
-            if constexpr (OUT_HALF) {
-                __half2 h0 = floats2half2_sat(z0, z1), h1 = floats2half2_sat(z2, z3);
-                uint2 u;
-                u.x = *reinterpret_cast<uint32_t*>(&h0);
-                u.y = *reinterpret_cast<uint32_t*>(&h1);
-                *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(z_out) + static_cast<size_t>(row) * D + vi * 4) = u;
-            } else {
-                *reinterpret_cast<float4*>(reinterpret_cast<float*>(z_out) + static_cast<size_t>(row) * D + vi * 4) =
-                    make_float4(z0, z1, z2, z3);
-            }
-        }
+        if (vi < r.nv) LnRow::store<OUT_HALF>(z_out, off, vi, r.norm(i, ldg4(gb, vi), ldg4(bb, vi)));
     }
 }
 
@@ -232,16 +188,18 @@ int layernorm2_rows(const float* x, float* y_out, void* z_out, bool z_half, cons
     return SBK_OK;
 }
 
-// fp32 -> fp16 cast (used for goldens-driven tests and the decoder memory)
-__global__ void cast_f32_f16_kernel(const float* __restrict__ in, __half* __restrict__ out, size_t n) {
-    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-         i += static_cast<size_t>(gridDim.x) * blockDim.x)
-        out[i] = float2half_sat(in[i]);
+// fp32 -> fp16 cast of `rows` rows of n values, row r read at in + r * ld_in and written packed at out + r * n (used for
+// goldens-driven tests, the decoder memory and the CNN output, whole or a stream chunk's frames inside longer rows)
+__global__ void cast_f32_f16_kernel(const float* __restrict__ in, size_t ld_in, __half* __restrict__ out, size_t n, int rows) {
+    for (int r = blockIdx.y; r < rows; r += gridDim.y)
+        for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+             i += static_cast<size_t>(gridDim.x) * blockDim.x)
+            out[r * n + i] = float2half_sat(in[r * ld_in + i]);
 }
-int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream) {
-    if (n == 0) return SBK_OK;
-    const int blocks = static_cast<int>(std::min<size_t>((n + 255) / 256, SBK_NUM_SMS * 16));
-    cast_f32_f16_kernel<<<blocks, 256, 0, stream>>>(in, out, n);
+int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream, int rows, size_t ld_in) {
+    if (n == 0 || rows == 0) return SBK_OK;
+    const dim3 grid(static_cast<unsigned>(std::min<size_t>((n + 255) / 256, SBK_NUM_SMS * 16)), std::min(rows, 65535));
+    cast_f32_f16_kernel<<<grid, 256, 0, stream>>>(in, ld_in, out, n, rows);
     SBK_LAUNCH_CHECK();
     return SBK_OK;
 }

@@ -322,87 +322,6 @@ static int ensure_workspace(AsrModel* m, int B, int L, int rows, int steps, int 
     return SBK_OK;
 }
 
-// Branchformer layers (Branchformer.py:92-234, 330-410) on the fp32 residual stream b.x [B*T, d] -> enc_out = encoder.norm(x):
-//     x1 = RelPosMHAXL(norm_mhsa(x));  x2 = post_channel_proj(CSGU(act(pre_channel_proj(norm_conv(x)))))
-//     x  = x + merge_proj(cat[x1, x2])
-// Neither branch masks padded frames (the attention masks padded keys only).  x1 and x2 are written into the two column
-// halves of one [B*T, 2d] fp16 buffer so that merge_proj is one K = 2d GEMM with the residual epilogue.
-static int run_branchformer_layers(AsrModel* m, int B, int T, const int* enc_len, float* enc_out, cudaStream_t st) {
-    const sbk_asr_config& c = m->wt->cfg;
-    AsrModel::Buf& b = m->b;
-    const int M = B * T, d = c.d_model, H = c.nhead, dh = d / H, C = c.csgu_linear_units;
-    SBK_REQUIRE(m->dyn_chunk == 0, "encode: the Branchformer has no chunked (DynChunkTrainConfig) mode");
-    const float att_scale = 1.0f / sqrtf((float)d);  // nnet/attention.py:521: 1/sqrt(embed_dim)
-    const int act = c.branchformer_activation == SBK_ACT_RELU ? ACT_RELU : ACT_GELU;
-    GemmEpilogue e;
-    for (int l = 0; l < c.num_encoder_layers; ++l) {
-        const EncLayerW& w = m->wt->enc[l];
-        RC(layernorm_rows_dual(b.x, b.h16, w.norm1_g, w.norm1_b, b.hc16, w.nconv_g, w.nconv_b, M, d, 1e-5f, st));
-        // --- attention branch -> cat16[:, :d]
-        e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.qkv16; e.ldo = 3 * d;
-        RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
-        RC(gemm_f16(m->wt->relpos_pe, d, w.wpos, d, e, T, d, d, st));
-        RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, true, w.pos_u, w.pos_v, b.P16, d, att_scale, b.att16, d, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bo; e.out = b.cat16; e.ldo = 2 * d;
-        RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
-        // --- convolution branch -> cat16[:, d:]
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = act; e.bias = w.bpre; e.out = b.f16; e.ldo = C;
-        RC(gemm_f16(b.hc16, d, w.wpre, d, e, M, C, d, st));
-        RC(csgu_forward(b.f16, B, T, C, w.csgu_ln_g, w.csgu_ln_b, 1e-5f, w.csgu_taps, w.csgu_bias, c.kernel_size, b.csgu_stats,
-                        b.g16, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bpost; e.out = b.cat16 + d; e.ldo = 2 * d;
-        RC(gemm_f16(b.g16, C / 2, w.wpost, C / 2, e, M, d, C / 2, st));
-        // --- x += merge_proj(cat[x1, x2]): every row, padded frames included
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bmerge; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
-        RC(gemm_f16(b.cat16, 2 * d, w.wmerge, 2 * d, e, M, d, 2 * d, st));
-    }
-    return layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, false, st);
-}
-
-// x [B*T, d] += pe[t]: TransformerASR.encode adds the absolute sine table to the input Linear's output (TransformerASR.py:519)
-__global__ void add_pos_table_kernel(float* __restrict__ x, const float* __restrict__ pe, int T, int d, size_t n) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) x[i] += pe[(i / d) % T * d + i % d];
-}
-
-// Transformer layers (Transformer.py:311-490, normalize_before=True, regularMHA, Linear + GELU + Linear) on the fp32
-// residual stream b.x [B*T, d] -> enc_out = encoder.norm(x):
-//     x = x + out_proj(MHA(norm1(x)));  x = x + ffn(norm2(x))
-// The attention masks padded keys only (make_transformer_src_tgt_masks), so padded frames are computed like the reference.
-static int run_transformer_layers(AsrModel* m, int B, int T, const int* enc_len, float* enc_out, cudaStream_t st) {
-    const sbk_asr_config& c = m->wt->cfg;
-    AsrModel::Buf& b = m->b;
-    const int M = B * T, d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H;
-    SBK_REQUIRE(m->dyn_chunk == 0, "encode: the Transformer encoder has no chunked (DynChunkTrainConfig) mode");
-    const size_t n = (size_t)M * d;
-    add_pos_table_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(b.x, m->wt->enc_pe, T, d, n);
-    SBK_LAUNCH_CHECK();
-    GemmEpilogue e;
-    for (int l = 0; l < c.num_encoder_layers; ++l) {
-        const EncLayerW& w = m->wt->enc[l];
-        RC(layernorm_rows(b.x, b.h16, true, w.norm1_g, w.norm1_b, M, d, 1e-6f, false, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bqkv; e.out = b.qkv16; e.ldo = 3 * d;
-        RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
-        // 1/sqrt(d_h) is folded into the query rows of wqkv / bqkv
-        RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, false, nullptr, nullptr, nullptr, 0, 1.0f, b.att16, d, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bo; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
-        RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
-        RC(layernorm_rows(b.x, b.h16, true, w.norm2_g, w.norm2_b, M, d, 1e-6f, false, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ACT_GELU; e.bias = w.ffn1_b1; e.out = b.f16; e.ldo = F;
-        RC(gemm_f16(b.h16, d, w.ffn1_w1, d, e, M, F, d, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.ffn1_b2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
-        RC(gemm_f16(b.f16, F, w.ffn1_w2, F, e, M, d, F, st));
-    }
-    return layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, false, st);
-}
-
-// The fused front-end of the configured ConvolutionFrontEnd: feats [B, T0, n_mels] -> b.a_in [B*T2, input_size] fp16
-// (+ cnn_out_f fp32 when set).
-static int run_cnn(AsrModel* m, const float* feats, int B, int T0, float* cnn_out_f, cudaStream_t st) {
-    return cnn_frontend_forward(feats, B, T0, m->wt->cfg.n_mels, m->wt->cnn, m->b.act1, m->b.a_in, cnn_out_f, st);
-}
-
 // One chunk-by-chunk stream (or a batch of B streams advancing together) of a Conformer encoder: per layer the attention's
 // left context as a ring of projected [k | v] rows (RoPE keys rotated by stream position) and the Dynamic Chunk
 // Convolution's carry, the last (kernel_size - 1) / 2 depthwise-conv inputs.  The window of a chunk is [cached rows; chunk]:
@@ -433,83 +352,154 @@ struct AsrStream {
     }
 };
 
-// feats [B, T0, n_mels] fp32 (already normalised) -> enc_out fp32 [B, T2, d] (+ enc16). enc_len device int[B].
-// s: one chunk of a stream (T0 = the chunk's frames, feats null): attention over s's window, the conv over its carry.
-static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int* enc_len, float* cnn_out_f,
-                       float* enc_out, cudaStream_t st, const AsrStream* s = nullptr) {
+// RelPosMHAXL's positional projection of encoder layer l: P [rows, d] fp16 = linear_pos(pe[r]) for r < rows
+static int relpos_project(const AsrModel* m, int l, int rows, __half* P, cudaStream_t st) {
+    const int d = m->wt->cfg.d_model;
+    GemmEpilogue e; e.mode = EPI_F16; e.out = P; e.ldo = d;
+    return gemm_f16(m->wt->relpos_pe, d, m->wt->enc[l].wpos, d, e, rows, d, d, st);
+}
+
+// Self-attention of encoder layer l on its pre-norm b.h16 [B*T, d] fp16: the QKV projection, RoPEMHA, RelPosMHAXL or
+// regularMHA attention over the whole sequence (DynChunkTrain windows when set) or, with s, over one stream chunk's window,
+// then the output projection.  That adds to the residual stream b.x, or with cat16 set writes fp16 cat16[:, :d] (row stride
+// 2d, the Branchformer's concatenation).
+static int self_attention(AsrModel* m, int l, int B, int T, const int* enc_len, const AsrStream* s, __half* cat16,
+                          cudaStream_t st) {
     const sbk_asr_config& c = m->wt->cfg;
     AsrModel::Buf& b = m->b;
-    const int T1 = (T0 - 1) / 2 + 1, T = feats ? (T1 - 1) / 2 + 1 : T0;  // feats == nullptr: b.a_in holds [B*T0, input_size]
-    // row counts are int (offsets into the activations are size_t); the CNN, attention and conv kernels launch one grid row
-    // or layer per utterance
-    SBK_REQUIRE(B <= 65535 && (long long)B * T0 <= INT_MAX, "encode: %d utterances of %d frames exceed the kernels' index range",
-                B, T0);
-    const int M = B * T, d = c.d_model, F = c.d_ffn, H = c.nhead, dh = d / H;
-    SBK_REQUIRE(m->wt->has_enc, "encode: this handle was created without encoder weights");
-    SBK_REQUIRE(feats == nullptr || m->wt->has_cnn, "encode: this handle was created without CNN weights");
-    if (c.attention_type == SBK_ATT_HYPERMIX)  // HyperMixing adds its own 3000-row table: longer inputs fail in the reference
-        SBK_REQUIRE(T <= HM_PE_ROWS, "encode: %d frames exceed HyperMixing's %d-row positional table", T, HM_PE_ROWS);
-    else
-        SBK_REQUIRE(T <= m->wt->pos_len, "encode: %d frames exceed max_len=%d", T, m->wt->pos_len);
-    SBK_REQUIRE(c.attention_type != SBK_ATT_HYPERMIX || m->dyn_chunk == 0,
-                "encode: HyperMixing has no chunked (DynChunkTrainConfig) mode");
-    SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER || T > (c.kernel_size - 1) / 2,
-                "encode: the Branchformer's reflect-padded conv needs more than %d frames (got %d)", (c.kernel_size - 1) / 2, T);
-    if (feats != nullptr) RC(run_cnn(m, feats, B, T0, cnn_out_f, st));
+    const EncLayerW& w = m->wt->enc[l];
+    const int M = B * T, d = c.d_model, H = c.nhead, dh = d / H;
+    const bool rope = c.attention_type == SBK_ATT_ROPE, relpos = c.attention_type == SBK_ATT_RELPOS;
+    // nnet/attention.py:521,1272: 1/sqrt(embed_dim), not head_dim; regularMHA's 1/sqrt(d_h) is folded into the query rows of
+    // wqkv / bqkv
+    const float att_scale = c.attention_type == SBK_ATT_REGULAR ? 1.0f : 1.0f / sqrtf((float)d);
     GemmEpilogue e;
-    e.mode = EPI_F32; e.bias = m->wt->b_in; e.out = b.x; e.ldo = d;
-    RC(gemm_f16(b.a_in, c.input_size, m->wt->w_in, c.input_size, e, M, d, c.input_size, st));
-    if (c.encoder_module == SBK_ENC_BRANCHFORMER) return run_branchformer_layers(m, B, T, enc_len, enc_out, st);
-    if (c.encoder_module == SBK_ENC_TRANSFORMER) return run_transformer_layers(m, B, T, enc_len, enc_out, st);
-    const float att_scale = 1.0f / sqrtf((float)d);  // nnet/attention.py:521,1272: 1/sqrt(embed_dim), not head_dim
+    e.bias = w.bqkv; e.ldo = 3 * d;
+    if (s) {  // the chunk's q and its [k | v] rows in the ring, then attention over [cached rows; chunk]
+        __half* kv = s->kv_layer(c, l);
+        e.mode = EPI_F32; e.out = s->qkv32;
+        RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
+        RC(stream_qkv(s->qkv32, B, T, H, dh, rope ? s->inv_freq : nullptr, s->total, att_scale, s->q16, kv, s->cap,
+                      (s->start + s->clen) % s->cap, st));
+        AttStream sa;
+        sa.q = s->q16; sa.ldq = d; sa.kv = kv; sa.ldkv = 2 * d; sa.cap = s->cap; sa.start = s->start; sa.nq = T;
+        RC(encoder_attention_stream(sa, B, s->clen + T, H, dh, relpos, w.pos_u, w.pos_v,
+                                    relpos ? static_cast<const __half*>(s->P.base) + (size_t)l * s->prow * d : nullptr, d,
+                                    att_scale, b.att16, d, st));
+    } else {
+        e.out = b.qkv16;
+        if (rope) {
+            e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->wt->rope_cos; e.rope_sin = m->wt->rope_sin; e.head_dim = dh;
+        } else {
+            e.mode = EPI_F16;
+        }
+        RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
+        if (relpos) RC(relpos_project(m, l, T, b.P16, st));
+        RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, relpos, w.pos_u, w.pos_v, b.P16, d, att_scale, b.att16, d,
+                             st, m->dyn_chunk, m->dyn_left));
+    }
+    e = GemmEpilogue(); e.bias = w.bo;
+    if (cat16) {
+        e.mode = EPI_F16; e.out = cat16; e.ldo = 2 * d;
+    } else {
+        e.mode = EPI_RESID; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
+    }
+    return gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st);
+}
+
+// A feed-forward module on its pre-norm b.h16 [M, d] fp16: x += alpha * (act(h16 W1^T + b1) W2^T + b2), the hidden layer in
+// b.f16 [M, d_ffn]
+static int feed_forward(AsrModel* m, const __half* W1, const float* b1, const __half* W2, const float* b2, int act, float alpha,
+                        int M, cudaStream_t st) {
+    const int d = m->wt->cfg.d_model, F = m->wt->cfg.d_ffn;
+    GemmEpilogue e;
+    e.mode = EPI_F16; e.act = act; e.bias = b1; e.out = m->b.f16; e.ldo = F;
+    RC(gemm_f16(m->b.h16, d, W1, d, e, M, F, d, st));
+    e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = b2; e.out = m->b.x; e.resid = m->b.x; e.ldo = d; e.alpha = alpha;
+    return gemm_f16(m->b.f16, F, W2, F, e, M, d, F, st);
+}
+
+// Branchformer layers (Branchformer.py:92-234, 330-410) on the fp32 residual stream b.x [B*T, d]:
+//     x1 = RelPosMHAXL(norm_mhsa(x));  x2 = post_channel_proj(CSGU(act(pre_channel_proj(norm_conv(x)))))
+//     x  = x + merge_proj(cat[x1, x2])
+// Neither branch masks padded frames (the attention masks padded keys only).  x1 and x2 are written into the two column
+// halves of one [B*T, 2d] fp16 buffer so that merge_proj is one K = 2d GEMM with the residual epilogue.
+static int run_branchformer_layers(AsrModel* m, int B, int T, const int* enc_len, cudaStream_t st) {
+    const sbk_asr_config& c = m->wt->cfg;
+    AsrModel::Buf& b = m->b;
+    const int M = B * T, d = c.d_model, C = c.csgu_linear_units;
+    const int act = c.branchformer_activation == SBK_ACT_RELU ? ACT_RELU : ACT_GELU;
+    GemmEpilogue e;
+    for (int l = 0; l < c.num_encoder_layers; ++l) {
+        const EncLayerW& w = m->wt->enc[l];
+        RC(layernorm_rows_dual(b.x, b.h16, w.norm1_g, w.norm1_b, b.hc16, w.nconv_g, w.nconv_b, M, d, 1e-5f, st));
+        // --- attention branch -> cat16[:, :d]
+        RC(self_attention(m, l, B, T, enc_len, nullptr, b.cat16, st));
+        // --- convolution branch -> cat16[:, d:]
+        e = GemmEpilogue(); e.mode = EPI_F16; e.act = act; e.bias = w.bpre; e.out = b.f16; e.ldo = C;
+        RC(gemm_f16(b.hc16, d, w.wpre, d, e, M, C, d, st));
+        RC(csgu_forward(b.f16, B, T, C, w.csgu_ln_g, w.csgu_ln_b, 1e-5f, w.csgu_taps, w.csgu_bias, c.kernel_size, b.csgu_stats,
+                        b.g16, st));
+        e = GemmEpilogue(); e.mode = EPI_F16; e.bias = w.bpost; e.out = b.cat16 + d; e.ldo = 2 * d;
+        RC(gemm_f16(b.g16, C / 2, w.wpost, C / 2, e, M, d, C / 2, st));
+        // --- x += merge_proj(cat[x1, x2]): every row, padded frames included
+        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bmerge; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
+        RC(gemm_f16(b.cat16, 2 * d, w.wmerge, 2 * d, e, M, d, 2 * d, st));
+    }
+    return SBK_OK;
+}
+
+// x [B*T, d] += pe[t]: TransformerASR.encode adds the absolute sine table to the input Linear's output (TransformerASR.py:519)
+__global__ void add_pos_table_kernel(float* __restrict__ x, const float* __restrict__ pe, int T, int d, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) x[i] += pe[(i / d) % T * d + i % d];
+}
+
+// Transformer layers (Transformer.py:311-490, normalize_before=True, regularMHA, Linear + GELU + Linear) on the fp32
+// residual stream b.x [B*T, d]:
+//     x = x + out_proj(MHA(norm1(x)));  x = x + ffn(norm2(x))
+// The attention masks padded keys only (make_transformer_src_tgt_masks), so padded frames are computed like the reference.
+static int run_transformer_layers(AsrModel* m, int B, int T, const int* enc_len, cudaStream_t st) {
+    const sbk_asr_config& c = m->wt->cfg;
+    AsrModel::Buf& b = m->b;
+    const int M = B * T, d = c.d_model;
+    const size_t n = (size_t)M * d;
+    add_pos_table_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(b.x, m->wt->enc_pe, T, d, n);
+    SBK_LAUNCH_CHECK();
+    for (int l = 0; l < c.num_encoder_layers; ++l) {
+        const EncLayerW& w = m->wt->enc[l];
+        RC(layernorm_rows(b.x, b.h16, true, w.norm1_g, w.norm1_b, M, d, 1e-6f, st));
+        RC(self_attention(m, l, B, T, enc_len, nullptr, nullptr, st));
+        RC(layernorm_rows(b.x, b.h16, true, w.norm2_g, w.norm2_b, M, d, 1e-6f, st));
+        RC(feed_forward(m, w.ffn1_w1, w.ffn1_b1, w.ffn1_w2, w.ffn1_b2, ACT_GELU, 1.0f, M, st));
+    }
+    return SBK_OK;
+}
+
+// Conformer layers (Conformer.py:472-500) on the fp32 residual stream b.x [B*T, d]; the last layer's norm2 runs fused with
+// the encoder's final LayerNorm into enc_out.  s: one chunk of a stream (attention over s's window, the conv over its carry).
+static int run_conformer_layers(AsrModel* m, int B, int T, const int* enc_len, float* enc_out, cudaStream_t st,
+                                const AsrStream* s) {
+    const sbk_asr_config& c = m->wt->cfg;
+    AsrModel::Buf& b = m->b;
+    const int M = B * T, d = c.d_model, F = c.d_ffn, H = c.nhead;
     // conformer_activation: both FFN modules' hidden activation and the convolution module's after the LayerNorm
     const bool gelu = c.conformer_activation == SBK_CONFORMER_ACT_GELU;
     const int ffn_act = gelu ? ACT_GELU : ACT_SILU;
+    GemmEpilogue e;
     for (int l = 0; l < c.num_encoder_layers; ++l) {
         const EncLayerW& w = m->wt->enc[l];
         // --- ffn module 1 (Conformer.py:479); its LayerNorm was fused into the previous layer's norm2 kernel
-        if (l == 0) RC(layernorm_rows(b.x, b.h16, true, w.ffn1_ln_g, w.ffn1_ln_b, M, d, 1e-5f, false, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ffn_act; e.bias = w.ffn1_b1; e.out = b.f16; e.ldo = F;
-        RC(gemm_f16(b.h16, d, w.ffn1_w1, d, e, M, F, d, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.ffn1_b2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 0.5f;
-        RC(gemm_f16(b.f16, F, w.ffn1_w2, F, e, M, d, F, st));
+        if (l == 0) RC(layernorm_rows(b.x, b.h16, true, w.ffn1_ln_g, w.ffn1_ln_b, M, d, 1e-5f, st));
+        RC(feed_forward(m, w.ffn1_w1, w.ffn1_b1, w.ffn1_w2, w.ffn1_b2, ffn_act, 0.5f, M, st));
         // --- self-attention (Conformer.py:481-492)
-        RC(layernorm_rows(b.x, b.h16, true, w.norm1_g, w.norm1_b, M, d, 1e-5f, false, st));
-        if (c.attention_type == SBK_ATT_HYPERMIX) {  // x += HyperMixing(norm1(x)) (hypermixing.py:90-195)
+        RC(layernorm_rows(b.x, b.h16, true, w.norm1_g, w.norm1_b, M, d, 1e-5f, st));
+        if (c.attention_type == SBK_ATT_HYPERMIX)  // x += HyperMixing(norm1(x)) (hypermixing.py:90-195)
             RC(hypermix_forward(b.h16, B, T, d, H, F / H, enc_len, m->wt->hm_pe, w.hm, b.hm_part, b.hm_G, b.hm_gscale, b.x, st));
-        } else {
-            if (s) {  // the chunk's q and its [k | v] rows in the ring, then attention over [cached rows; chunk]
-                const bool rope = c.attention_type == SBK_ATT_ROPE;
-                __half* kv = s->kv_layer(c, l);
-                e = GemmEpilogue(); e.mode = EPI_F32; e.out = s->qkv32; e.ldo = 3 * d;
-                RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
-                RC(stream_qkv(s->qkv32, B, T, H, dh, rope ? s->inv_freq : nullptr, s->total, att_scale, s->q16, kv, s->cap,
-                              (s->start + s->clen) % s->cap, st));
-                AttStream sa;
-                sa.q = s->q16; sa.ldq = d; sa.kv = kv; sa.ldkv = 2 * d; sa.cap = s->cap; sa.start = s->start; sa.nq = T;
-                RC(encoder_attention_stream(sa, B, s->clen + T, H, dh, !rope, w.pos_u, w.pos_v,
-                                            rope ? nullptr : static_cast<const __half*>(s->P.base) + (size_t)l * s->prow * d, d,
-                                            att_scale, b.att16, d, st));
-            } else {
-                e = GemmEpilogue(); e.out = b.qkv16; e.ldo = 3 * d;
-                if (c.attention_type == SBK_ATT_ROPE) {
-                    e.mode = EPI_ROPE; e.alpha = att_scale; e.T = T; e.rope_cos = m->wt->rope_cos; e.rope_sin = m->wt->rope_sin; e.head_dim = dh;
-                } else {
-                    e.mode = EPI_F16;
-                }
-                RC(gemm_f16(b.h16, d, w.wqkv, d, e, M, 3 * d, d, st));
-                if (c.attention_type == SBK_ATT_RELPOS) {
-                    e = GemmEpilogue(); e.mode = EPI_F16; e.out = b.P16; e.ldo = d;
-                    RC(gemm_f16(m->wt->relpos_pe, d, w.wpos, d, e, T, d, d, st));
-                }
-                RC(encoder_attention(b.qkv16, 3 * d, B, T, H, dh, enc_len, c.attention_type == SBK_ATT_RELPOS, w.pos_u, w.pos_v,
-                                     b.P16, d, att_scale, b.att16, d, st, m->dyn_chunk, m->dyn_left));
-            }
-            e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.bo; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 1.0f;
-            RC(gemm_f16(b.att16, d, w.wo, d, e, M, d, d, st));
-        }
+        else
+            RC(self_attention(m, l, B, T, enc_len, s, nullptr, st));
         // --- convolution module (Conformer.py:314-330, 494)
-        RC(layernorm_rows(b.x, b.h16, true, w.conv_ln_g, w.conv_ln_b, M, d, 1e-5f, false, st));
+        RC(layernorm_rows(b.x, b.h16, true, w.conv_ln_g, w.conv_ln_b, M, d, 1e-5f, st));
         e = GemmEpilogue(); e.mode = EPI_GLU; e.bias = w.bpw1; e.out = b.glu; e.ldo = d;
         RC(gemm_f16(b.h16, d, w.wpw1, d, e, M, 2 * d, d, st));
         if (s) {  // the chunk after the carry, zeros after the chunk (its right edge); then the carry moves on
@@ -525,11 +515,8 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
         e.row_lens = enc_len; e.T = T;
         RC(gemm_f16(b.h16, d, w.wpw2, d, e, M, d, d, st));
         // --- ffn module 2 + norm2 (Conformer.py:498)
-        RC(layernorm_rows(b.x, b.h16, true, w.ffn2_ln_g, w.ffn2_ln_b, M, d, 1e-5f, false, st));
-        e = GemmEpilogue(); e.mode = EPI_F16; e.act = ffn_act; e.bias = w.ffn2_b1; e.out = b.f16; e.ldo = F;
-        RC(gemm_f16(b.h16, d, w.ffn2_w1, d, e, M, F, d, st));
-        e = GemmEpilogue(); e.mode = EPI_RESID; e.bias = w.ffn2_b2; e.out = b.x; e.resid = b.x; e.ldo = d; e.alpha = 0.5f;
-        RC(gemm_f16(b.f16, F, w.ffn2_w2, F, e, M, d, F, st));
+        RC(layernorm_rows(b.x, b.h16, true, w.ffn2_ln_g, w.ffn2_ln_b, M, d, 1e-5f, st));
+        RC(feed_forward(m, w.ffn2_w1, w.ffn2_b1, w.ffn2_w2, w.ffn2_b2, ffn_act, 0.5f, M, st));
         if (l + 1 < c.num_encoder_layers) {  // norm2 (fp32 residual stream) + the next layer's ffn1 LayerNorm (fp16 operand)
             const EncLayerW& nx = m->wt->enc[l + 1];
             RC(layernorm2_rows(b.x, b.x, b.h16, true, w.norm2_g, w.norm2_b, 1e-5f, nx.ffn1_ln_g, nx.ffn1_ln_b, 1e-5f, M, d, st));
@@ -538,8 +525,51 @@ static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int
                                d, st));
         }
     }
-    if (c.num_encoder_layers == 0)
-        RC(layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, false, st));
+    return SBK_OK;
+}
+
+// The fused front-end of the configured ConvolutionFrontEnd: feats [B, T0, n_mels] -> b.a_in [B*T2, input_size] fp16
+// (+ cnn_out_f fp32 when set).
+static int run_cnn(AsrModel* m, const float* feats, int B, int T0, float* cnn_out_f, cudaStream_t st) {
+    return cnn_frontend_forward(feats, B, T0, m->wt->cfg.n_mels, m->wt->cnn, m->b.act1, m->b.a_in, cnn_out_f, st);
+}
+
+// feats [B, T0, n_mels] fp32 (already normalised) -> enc_out fp32 [B, T2, d] (+ enc16). enc_len device int[B].
+// s: one chunk of a stream (T0 = the chunk's frames, feats null): attention over s's window, the conv over its carry.
+static int run_encoder(AsrModel* m, const float* feats, int B, int T0, const int* enc_len, float* cnn_out_f,
+                       float* enc_out, cudaStream_t st, const AsrStream* s = nullptr) {
+    const sbk_asr_config& c = m->wt->cfg;
+    AsrModel::Buf& b = m->b;
+    const int T1 = (T0 - 1) / 2 + 1, T = feats ? (T1 - 1) / 2 + 1 : T0;  // feats == nullptr: b.a_in holds [B*T0, input_size]
+    // row counts are int (offsets into the activations are size_t); the CNN, attention and conv kernels launch one grid row
+    // or layer per utterance
+    SBK_REQUIRE(B <= 65535 && (long long)B * T0 <= INT_MAX, "encode: %d utterances of %d frames exceed the kernels' index range",
+                B, T0);
+    const int M = B * T, d = c.d_model;
+    SBK_REQUIRE(m->wt->has_enc, "encode: this handle was created without encoder weights");
+    SBK_REQUIRE(feats == nullptr || m->wt->has_cnn, "encode: this handle was created without CNN weights");
+    if (c.attention_type == SBK_ATT_HYPERMIX)  // HyperMixing adds its own 3000-row table: longer inputs fail in the reference
+        SBK_REQUIRE(T <= HM_PE_ROWS, "encode: %d frames exceed HyperMixing's %d-row positional table", T, HM_PE_ROWS);
+    else
+        SBK_REQUIRE(T <= m->wt->pos_len, "encode: %d frames exceed max_len=%d", T, m->wt->pos_len);
+    SBK_REQUIRE(c.attention_type != SBK_ATT_HYPERMIX || m->dyn_chunk == 0,
+                "encode: HyperMixing has no chunked (DynChunkTrainConfig) mode");
+    SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER || T > (c.kernel_size - 1) / 2,
+                "encode: the Branchformer's reflect-padded conv needs more than %d frames (got %d)", (c.kernel_size - 1) / 2, T);
+    SBK_REQUIRE(c.encoder_module != SBK_ENC_BRANCHFORMER || m->dyn_chunk == 0,
+                "encode: the Branchformer has no chunked (DynChunkTrainConfig) mode");
+    SBK_REQUIRE(c.encoder_module != SBK_ENC_TRANSFORMER || m->dyn_chunk == 0,
+                "encode: the Transformer encoder has no chunked (DynChunkTrainConfig) mode");
+    if (feats != nullptr) RC(run_cnn(m, feats, B, T0, cnn_out_f, st));
+    GemmEpilogue e;
+    e.mode = EPI_F32; e.bias = m->wt->b_in; e.out = b.x; e.ldo = d;
+    RC(gemm_f16(b.a_in, c.input_size, m->wt->w_in, c.input_size, e, M, d, c.input_size, st));
+    if (c.encoder_module == SBK_ENC_BRANCHFORMER) RC(run_branchformer_layers(m, B, T, enc_len, st));
+    else if (c.encoder_module == SBK_ENC_TRANSFORMER) RC(run_transformer_layers(m, B, T, enc_len, st));
+    else RC(run_conformer_layers(m, B, T, enc_len, enc_out, st, s));
+    // encoder.norm, unless a Conformer layer ran it with its norm2
+    if (c.encoder_module != SBK_ENC_CONFORMER || c.num_encoder_layers == 0)
+        RC(layernorm_rows(b.x, enc_out, false, m->wt->enc_norm_g, m->wt->enc_norm_b, M, d, 1e-6f, st));
     return SBK_OK;
 }
 
@@ -700,7 +730,7 @@ static int norm_project(StepGemm g, bool fuse_ln, Proj p, const float* x, const 
     if (g == SG_STREAM && fuse_ln && (d == 256 || d == 512 || d == 768 || d == 1024)) {
         p.X = x; p.ln_g = gamma; p.ln_b = beta;
     } else {
-        RC(layernorm_rows(x, h16, true, gamma, beta, rows, d, 1e-6f, false, st, g != SG_STREAM));
+        RC(layernorm_rows(x, h16, true, gamma, beta, rows, d, 1e-6f, st, g != SG_STREAM));
         p.A = h16; p.lda = d;
     }
     return project(g, p, rows, st);
@@ -1052,7 +1082,7 @@ static int run_decode_teacher(AsrModel* m, const int* tokens, int n, int S, int 
         dec_teacher_embed_kernel<<<n, 128, 0, st>>>(tokens, S, s, m->wt->emb, m->wt->dec_pe, d, sqrtf((float)d), b.dx, b.step);
         SBK_LAUNCH_CHECK();
         RC(enqueue_decode_layers(m, n, 1, T, S_max, nullptr, fold, st, false));
-        RC(layernorm_rows(b.dx, b.lnout, false, m->wt->dec_norm_g, m->wt->dec_norm_b, n, d, 1e-6f, false, st));
+        RC(layernorm_rows(b.dx, b.lnout, false, m->wt->dec_norm_g, m->wt->dec_norm_b, n, d, 1e-6f, st));
         SBK_CUDA_CHECK(cudaMemcpy2DAsync(out + (size_t)s * d, (size_t)S * d * 4, b.lnout, (size_t)d * 4, (size_t)d * 4, n,
                                          cudaMemcpyDeviceToDevice, st));
     }
@@ -1306,20 +1336,23 @@ int sbk_asr_cnn_forward(sbk_asr* mm, const float* feats_dev, int B, int T0, floa
     return run_cnn(m, feats_dev, B, T0, out_dev, static_cast<cudaStream_t>(stream));
 }
 
+// The encoder of an encode entry: b.enc_len = round(rel_len * T) when rel_len is set (else every frame counts), then
+// run_encoder from feats (null: from the CNN output in b.a_in) into enc_out (null: b.enc_out).
+static int encode_entry(AsrModel* m, const float* feats, const float* rel_len, int B, int T0, int T, float* cnn_out,
+                        float* enc_out, cudaStream_t st) {
+    if (rel_len) RC(set_enc_len(m->b.enc_len, rel_len, B, T, st));
+    return run_encoder(m, feats, B, T0, rel_len ? m->b.enc_len : nullptr, cnn_out, enc_out ? enc_out : m->b.enc_out, st);
+}
+
 // src_dev: CNN output [B, T, input_size] fp32 -> enc_out_dev [B, T, d] fp32 (TransformerASR.encode)
 int sbk_asr_encode_feats(sbk_asr* mm, const float* feats_dev, const float* rel_len_dev, int B, int T0,
                          float* cnn_out_dev, float* enc_out_dev, void* stream) {
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const sbk_asr_config& c = m->wt->cfg;
-    RC(ensure_workspace(m, B, (T0 - 1) * c.hop, B, 1));
-    const int T1 = (T0 - 1) / 2 + 1, T = (T1 - 1) / 2 + 1;
-    const int* enc_len = nullptr;
-    if (rel_len_dev) {
-        RC(set_enc_len(m->b.enc_len, rel_len_dev, B, T, st));
-        enc_len = m->b.enc_len;
-    }
-    return run_encoder(m, feats_dev, B, T0, enc_len, cnn_out_dev, enc_out_dev ? enc_out_dev : m->b.enc_out, st);
+    const int L = (T0 - 1) * m->wt->cfg.hop;
+    RC(ensure_workspace(m, B, L, B, 1));
+    int T0_, T1, T;
+    frames(m->wt->cfg, L, &T0_, &T1, &T);
+    return encode_entry(m, feats_dev, rel_len_dev, B, T0, T, cnn_out_dev, enc_out_dev, static_cast<cudaStream_t>(stream));
 }
 
 int sbk_asr_encode_from_cnn(sbk_asr* mm, const float* src_dev, const float* rel_len_dev, int B, int T,
@@ -1329,12 +1362,7 @@ int sbk_asr_encode_from_cnn(sbk_asr* mm, const float* src_dev, const float* rel_
     const sbk_asr_config& c = m->wt->cfg;
     RC(ensure_workspace(m, B, enc_samples(c, T), B, 1));
     RC(cast_f32_f16(src_dev, m->b.a_in, (size_t)B * T * c.input_size, st));
-    const int* enc_len = nullptr;
-    if (rel_len_dev) {
-        RC(set_enc_len(m->b.enc_len, rel_len_dev, B, T, st));
-        enc_len = m->b.enc_len;
-    }
-    return run_encoder(m, nullptr, B, T, enc_len, nullptr, enc_out_dev ? enc_out_dev : m->b.enc_out, st);
+    return encode_entry(m, nullptr, rel_len_dev, B, T, T, nullptr, enc_out_dev, st);
 }
 
 // ---- chunk-by-chunk streaming encoder (AsrStream)
@@ -1384,10 +1412,8 @@ int sbk_asr_stream_create(sbk_asr* mm, int B, int chunk_size, int left_frames, s
     } else {  // P = linear_pos(pe[r]) for every row a window can reach, once per stream
         st->prow = left_frames >= 0 ? cap : m->wt->pos_len;
         RC(alloc(st->P, (size_t)L * st->prow * d * 2));
-        for (int l = 0; l < L; ++l) {
-            GemmEpilogue e; e.mode = EPI_F16; e.out = static_cast<__half*>(st->P.base) + (size_t)l * st->prow * d; e.ldo = d;
-            RC(gemm_f16(m->wt->relpos_pe, d, m->wt->enc[l].wpos, d, e, st->prow, d, d, 0));
-        }
+        for (int l = 0; l < L; ++l)
+            RC(relpos_project(m, l, st->prow, static_cast<__half*>(st->P.base) + (size_t)l * st->prow * d, 0));
         SBK_CUDA_CHECK(cudaStreamSynchronize(0));
     }
     *out = reinterpret_cast<sbk_asr_stream*>(st.release());
@@ -1402,15 +1428,6 @@ int sbk_asr_stream_reset(sbk_asr_stream* ss) {
     s->total = 0; s->clen = 0; s->start = 0; s->ended = false;  // the first chunk reads no cache and a zero carry
     s->fe_chunks = 0; s->fe_ended = false;                        // and the first front-end window zero audio context
     return SBK_OK;
-}
-
-// rows [B][n][F] fp32 at src + b * batch_stride + t * F -> dst [B * n, F] fp16 (the fp32 -> fp16 cast of cast_f32_f16)
-__global__ void cast_rows_f16_kernel(const float* __restrict__ src, long long batch_stride, int nF, int B, __half* __restrict__ dst) {
-    const size_t total = (size_t)B * nF;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t b = i / nF, j = i % nF;
-        dst[i] = float2half_sat(src[b * batch_stride + j]);
-    }
 }
 
 static int stream_encode(AsrModel* m, AsrStream* s, const float* cnn_out_dev, long long batch_stride, int n, float* enc_out_dev,
@@ -1441,14 +1458,8 @@ static int stream_encode(AsrModel* m, AsrStream* s, const float* cnn_out_dev, lo
         s->cap = ncap;
     }
     RC(ensure_workspace(m, s->B, enc_samples(c, n), s->B, 1));
-    if (batch_stride == (long long)n * c.input_size) {
-        RC(cast_f32_f16(cnn_out_dev, m->b.a_in, (size_t)s->B * n * c.input_size, st));
-    } else {  // the chunk's frames inside a longer window of each row (the streaming front end's output)
-        const size_t total = (size_t)s->B * n * c.input_size;
-        cast_rows_f16_kernel<<<(int)std::min<size_t>((total + 255) / 256, SBK_NUM_SMS * 16), 256, 0, st>>>(
-            cnn_out_dev, batch_stride, n * c.input_size, s->B, m->b.a_in);
-        SBK_LAUNCH_CHECK();
-    }
+    // each row's chunk, possibly inside a longer window of the row (the streaming front end's output)
+    RC(cast_f32_f16(cnn_out_dev, m->b.a_in, (size_t)n * c.input_size, st, s->B, batch_stride));
     RC(run_encoder(m, nullptr, s->B, n, nullptr, nullptr, enc_out_dev, st, s));
     s->total += n;
     if (n < s->chunk) s->ended = true;

@@ -127,14 +127,15 @@ int cnn_frontend_forward(const float* feats, int B, int T0, int F0, const CnnWei
 // ---- encoder_ops.cu
 // pdl: launched with programmatic stream serialisation (fp16 output only; the decode step's pre-norms)
 int layernorm_rows(const float* x, void* out, bool out_half, const float* gamma, const float* beta, int M, int D,
-                   float eps, bool act_silu, cudaStream_t stream, bool pdl = false);
+                   float eps, cudaStream_t stream, bool pdl = false);
 // y = LN_a(x) (fp32, stored when y_out != null), z = LN_b(y) -> z_out (fp16 or fp32): two chained LayerNorms in one pass
 int layernorm2_rows(const float* x, float* y_out, void* z_out, bool z_half, const float* ga, const float* ba, float eps_a,
                     const float* gb, const float* bb, float eps_b, int M, int D, cudaStream_t stream);
 // out = LN(x; gamma, beta), out2 = LN(x; gamma2, beta2): two fp16 LayerNorms of the same rows from one pass
 int layernorm_rows_dual(const float* x, __half* out, const float* gamma, const float* beta, __half* out2, const float* gamma2,
                         const float* beta2, int M, int D, float eps, cudaStream_t stream);
-int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream);
+// rows x n fp32 (row stride ld_in) -> rows x n fp16, packed
+int cast_f32_f16(const float* in, __half* out, size_t n, cudaStream_t stream, int rows = 1, size_t ld_in = 0);
 // Branchformer CSGU: u [B*T, C] fp16 -> g [B*T, C/2] fp16 = u[:, :C/2] * (dwconv_K(LN(u[:, C/2:])) + bias), reflect padding
 // inside T; taps tap-major [31, C/2] as csgu_repack_taps lays them out; stats: B*T float2 of scratch
 int csgu_forward(const __half* u, int B, int T, int C, const float* gamma, const float* beta, float eps, const float* taps,
