@@ -478,6 +478,31 @@ int sbk_transducer_greedy(sbk_transducer* m, const float* tn_dev, int B, int T, 
                           int start_from_blank, float* h_dev, float* c_dev, float* out_pn_dev, int* tokens_dev,
                           int* frames_dev, int* n_tokens_dev, float* logp_sum_dev, int* stats_dev, void* stream);
 
+/* ---- Transducer beam search: TransducerBeamSearcher.transducer_beam_search_decode (decoders/transducer.py:320-476)
+ * without a language model, on a handle of sbk_transducer_create.  Every utterance starts from [blank] with score 0 and
+ * a zero LSTM state and every frame of tn_dev [B, T, joint] fp32 is decoded.  A frame stops after
+ * SBK_TRANSDUCER_BEAM_POP_CAP(beam_size) pops at the most: an utterance that reaches it stops there.
+ * Outputs, per utterance b and rank n < nbest (rank order = the reference's sort by score / length):
+ *   out_tokens_dev [B, nbest, T * SBK_TRANSDUCER_BEAM_POP_CAP(beam_size)] int32: the first out_lens entries are the
+ *     hypothesis without its leading blank;
+ *   out_lens_dev [B, nbest] int32: the length, -1 when the last beam held fewer than n + 1 hypotheses, and in
+ *     out_lens_dev[b, 0] -2 - t when utterance b stopped at the pop cap in frame t;
+ *   out_scores_dev [B, nbest] fp32: score / (length + 1), the reference's normalised score.
+ * trace_dev (may be null) [B, T * cap, 6 + 2 beam_size] int32: one record per pop, in pop order per utterance, unused
+ * records set to -1: (utterance, frame, index of the popped hypothesis in the frame's list -- the previous beam, then the
+ * children in the order they were added --, how the frame ended right after this pop (0: it did not, 1: the state_beam
+ * test, 2: the beam is full), bit j = child j kept, the popped hypothesis' raw score (fp32 bits), the top beam_size tokens,
+ * their log-probabilities (fp32 bits)).  stats_dev (may be null) [4]: rounds, pops, prediction-network steps, grid
+ * barriers.  2 <= beam_size <= SBK_TRANSDUCER_BEAM_MAX, beam_size <= vocab, 1 <= nbest <= beam_size, 1 <= B <= 1024.
+ * Memory grows as B * T * cap: the token output (4 * nbest bytes per possible pop), a stream-ordered workspace of about
+ * B * (8 T cap + 4 (beam_size + cap) (2 hidden + joint) + 20 beam_size (cap + 1)) bytes, and the trace when requested;
+ * long inputs with a wide n-best are best searched in smaller batches. */
+#define SBK_TRANSDUCER_BEAM_MAX 32
+#define SBK_TRANSDUCER_BEAM_POP_CAP(beam_size) (4 * (beam_size))
+int sbk_transducer_beam(sbk_transducer* m, const float* tn_dev, int B, int T, int blank, int beam_size, int nbest,
+                        float state_beam, float expand_beam, int* out_tokens_dev, int* out_lens_dev, float* out_scores_dev,
+                        int* trace_dev, int* stats_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

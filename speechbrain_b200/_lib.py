@@ -70,6 +70,7 @@ EXPORTS = [
     "sbk_asr_lm_forward", "sbk_asr_lm_step_logits", "sbk_ctc_beam_workspace_bytes", "sbk_ctc_beam_search",
     "sbk_ctc_prefix_beam_workspace_bytes", "sbk_ctc_prefix_beam_search",
     "sbk_transducer_create", "sbk_transducer_destroy", "sbk_transducer_info", "sbk_transducer_greedy",
+    "sbk_transducer_beam",
     "sbk_asr_stream_create", "sbk_asr_stream_encode_chunk", "sbk_asr_stream_reset", "sbk_asr_stream_destroy",
     "sbk_asr_stream_context", "sbk_asr_stream_encode_chunk_strided", "sbk_asr_stream_frontend_chunk", "sbk_stream_qkv_test", "sbk_step_proj_test", "sbk_dec_attention_test",
     "sbk_beam_step_test", "sbk_coverage_score_test", "sbk_xatt_fold_test", "sbk_lm_causal_attention_test",

@@ -1,5 +1,6 @@
 """TransducerBeamSearcher -- drop-in for speechbrain.decoders.transducer.TransducerBeamSearcher (decoders/transducer.py:25-
-291) with ``beam_size=1``: the greedy search of the Conformer-Transducer recipes, on the device.
+476): the greedy search (``beam_size=1``) and the beam search without a language model (``beam_size > 1``) of the
+Conformer-Transducer recipes, on the device.
 
 The prediction network must be the recipes' ``[Embedding, LSTM, Linear(bias=False)]`` (one unidirectional LSTM layer with
 biases), the joint ``Transducer_joint(joint="sum", nonlinearity=torch.nn.GELU)`` and the classifier
@@ -15,8 +16,14 @@ Semantics kept from the reference:
   a short utterance can pick up tokens from them, exactly as in the reference.
 
 Rows are independent (a row that produced blank keeps producing blank for the rest of the frame), so the device walks
-each row on its own; the results do not depend on the other rows of the batch.  ``beam_size > 1`` (the beam search with
-the RNNLM) is not built."""
+each row on its own; the results do not depend on the other rows of the batch.
+
+The beam search (``transducer_beam_search_decode``, decoders/transducer.py:320-476, C ABI ``sbk_transducer_beam``) keeps
+the reference's order of pops, its key score / len(prediction), its state_beam and expand_beam tests and its fp32 score
+sums; each utterance is searched on its own, as in the reference.  Exact ties between top-K log-probabilities go to the
+lower token id.  A frame stops after ``4 * beam_size`` pops at the most (the reference would loop for ever on a frame whose
+top-K never holds blank); the call then raises naming the utterance and the frame.  RNNLM shallow fusion (``lm_weight >
+0``), ``nbest > beam_size`` and beams above 32 are not built."""
 import ctypes
 from dataclasses import dataclass
 from typing import Any, Optional
@@ -34,6 +41,12 @@ from ..nnet.transducer.transducer_joint import Transducer_joint
 MAX_HIDDEN = 1024  # LSTM hidden and joint sizes: multiples of 64 up to this
 MAX_VOCAB = 4096
 MAX_BATCH = 1024
+MAX_BEAM = 32  # SBK_TRANSDUCER_BEAM_MAX
+
+
+def pop_cap(beam_size):
+    """SBK_TRANSDUCER_BEAM_POP_CAP: the most pops of one frame of the beam search"""
+    return 4 * beam_size
 
 
 class sbk_transducer_config(ctypes.Structure):
@@ -103,9 +116,31 @@ class _DeviceSearch:
             out["stats"] = stats
         return out
 
+    def beam(self, tn, blank, beam_size, nbest, state_beam, expand_beam, want_trace=False, want_stats=False):
+        """tn [B, T, J] fp32 on the device -> dict of device tensors (tokens [B, nbest, T * pop_cap], lens [B, nbest],
+        scores [B, nbest][, trace [B, T * pop_cap, 6 + 2 beam_size], stats [4]]); enqueued on the current stream."""
+        B, T, _ = tn.shape
+        dev = tn.device
+        cap = pop_cap(beam_size)
+        i32 = dict(device=dev, dtype=torch.int32)
+        out = dict(tokens=torch.empty(B, nbest, T * cap, **i32), lens=torch.empty(B, nbest, **i32),
+                   scores=torch.empty(B, nbest, device=dev, dtype=torch.float32))
+        if want_trace:
+            out["trace"] = torch.empty(B, T * cap, 6 + 2 * beam_size, **i32)
+        if want_stats:
+            out["stats"] = torch.zeros(4, **i32)
+        with torch.cuda.device(dev):
+            check(lib().sbk_transducer_beam(self.handle, ptr(tn), B, T, blank, beam_size, nbest, ctypes.c_float(state_beam),
+                                            ctypes.c_float(expand_beam), ptr(out["tokens"]), ptr(out["lens"]),
+                                            ptr(out["scores"]), ptr(out.get("trace")), ptr(out.get("stats")),
+                                            stream_ptr(dev)),
+                  "sbk_transducer_beam")
+        return out
+
 
 class TransducerBeamSearcher(torch.nn.Module):
-    """decoders/transducer.py:25-154 with the reference's constructor; ``beam_size`` must be 1 (greedy)."""
+    """decoders/transducer.py:25-154 with the reference's constructor: ``beam_size=1`` selects the greedy search,
+    ``beam_size > 1`` the beam search without a language model."""
 
     def __init__(self, decode_network_lst, tjoint, classifier_network, blank_id, beam_size=4, nbest=5, lm_module=None,
                  lm_weight=0.0, state_beam=2.3, expand_beam=2.3):
@@ -123,10 +158,17 @@ class TransducerBeamSearcher(torch.nn.Module):
         self.state_beam = state_beam
         self.expand_beam = expand_beam
         if beam_size > 1:
-            raise NotImplementedError("speechbrain_b200.TransducerBeamSearcher: beam_size > 1 (transducer beam search) is "
-                                      "not built; use beam_size=1 (greedy)")
+            if lm_module is not None and lm_weight > 0:
+                raise NotImplementedError("speechbrain_b200.TransducerBeamSearcher: RNNLM shallow fusion (lm_weight > 0) "
+                                          "is not built")
+            if nbest > beam_size:
+                raise NotImplementedError(f"speechbrain_b200.TransducerBeamSearcher: nbest {nbest} above beam_size "
+                                          f"{beam_size} is not built")
+            if beam_size > MAX_BEAM:
+                raise NotImplementedError(f"speechbrain_b200.TransducerBeamSearcher: beam_size {beam_size} above "
+                                          f"{MAX_BEAM}")
         self._check_layout()
-        self.searcher = self.transducer_greedy_decode
+        self.searcher = self.transducer_beam_search_decode if beam_size > 1 else self.transducer_greedy_decode
         self._search = None
         self._fp = None
         self.builds = 0
@@ -163,6 +205,9 @@ class TransducerBeamSearcher(torch.nn.Module):
             raise NotImplementedError(f"speechbrain_b200.TransducerBeamSearcher: vocabulary {V} above {MAX_VOCAB}")
         if not 0 <= self.blank_id < V:
             raise ValueError(f"TransducerBeamSearcher: blank_id {self.blank_id} outside [0, {V})")
+        if self.beam_size > V:
+            raise NotImplementedError(f"speechbrain_b200.TransducerBeamSearcher: beam_size {self.beam_size} above the "
+                                      f"vocabulary size {V}")
 
     def _sources(self):
         dec = list(self.decode_network_lst)
@@ -198,8 +243,8 @@ class TransducerBeamSearcher(torch.nn.Module):
             ret += ((r["out_pn"].unsqueeze(1), (r["h"].unsqueeze(0), r["c"].unsqueeze(0))),)
         return ret
 
-    def _enqueue_search(self, tn_output, hidden_state, max_symbols_per_step):
-        """Checks the arguments and enqueues the device search: (B, the dict of device tensors of _DeviceSearch.greedy)."""
+    def _check_input(self, tn_output):
+        """Checks tn_output: (the device weights, B, T)."""
         require_cuda(tn_output, "TransducerBeamSearcher")
         if tn_output.ndim != 3:
             raise ValueError(f"TransducerBeamSearcher: tn_output must be [B, T, J], got {tuple(tn_output.shape)}")
@@ -209,6 +254,11 @@ class TransducerBeamSearcher(torch.nn.Module):
             raise ValueError(f"TransducerBeamSearcher: tn_output width {J}, the joint expects {s.J}")
         if not 1 <= B <= MAX_BATCH:
             raise NotImplementedError(f"speechbrain_b200.TransducerBeamSearcher: batch size {B} outside [1, {MAX_BATCH}]")
+        return s, B, T
+
+    def _enqueue_search(self, tn_output, hidden_state, max_symbols_per_step):
+        """Checks the arguments and enqueues the device search: (B, the dict of device tensors of _DeviceSearch.greedy)."""
+        s, B, T = self._check_input(tn_output)
         if max_symbols_per_step < 0:
             raise ValueError("max_symbols_per_step must be >= 0")
         state = None
@@ -229,5 +279,31 @@ class TransducerBeamSearcher(torch.nn.Module):
         context.hidden = (r["out_pn"].unsqueeze(1), (r["h"].unsqueeze(0), r["c"].unsqueeze(0)))
         return [packed[b, 1:1 + int(packed[b, 0])].tolist() for b in range(B)]
 
+    @torch.no_grad()
     def transducer_beam_search_decode(self, tn_output):
-        raise NotImplementedError("speechbrain_b200.TransducerBeamSearcher: transducer beam search is not built")
+        """decoders/transducer.py:320-476 without a language model.  tn_output [B, T, J] on a CUDA device; every frame is
+        decoded.  Returns (best hyps list[list[int]], exp(best normalised scores).mean(), nbest hyps per utterance, their
+        normalised scores as 0-dim tensors), the reference's return value."""
+        r, B = self._enqueue_beam(tn_output)
+        lens = r["lens"].cpu()
+        capped = [b for b in range(B) if int(lens[b, 0]) <= -2]
+        if capped:
+            b = capped[0]
+            raise RuntimeError(f"TransducerBeamSearcher: utterance {b} reached the limit of {pop_cap(self.beam_size)} pops "
+                               f"in frame {-2 - int(lens[b, 0])} (blank never entered the top {self.beam_size})")
+        n = max(1, int(lens.max()))
+        toks, scores = r["tokens"][:, :, :n].cpu(), r["scores"].cpu()
+        nbest_batch = [[toks[b, k, :int(lens[b, k])].tolist() for k in range(self.nbest) if int(lens[b, k]) >= 0]
+                       for b in range(B)]
+        nbest_batch_score = [[scores[b, k].clone() for k in range(self.nbest) if int(lens[b, k]) >= 0] for b in range(B)]
+        best = torch.Tensor([float(s[0]) for s in nbest_batch_score]).exp().mean()
+        return [h[0] for h in nbest_batch], best, nbest_batch, nbest_batch_score
+
+    def _enqueue_beam(self, tn_output, want_trace=False, want_stats=False):
+        """Checks tn_output and enqueues the device beam search: (the dict of _DeviceSearch.beam, B)."""
+        s, B, T = self._check_input(tn_output)
+        if T == 0:
+            raise ValueError("TransducerBeamSearcher: tn_output has no frames")
+        tn = tn_output.detach().to(torch.float32).contiguous()
+        return s.beam(tn, self.blank_id, int(self.beam_size), int(self.nbest), float(self.state_beam),
+                      float(self.expand_beam), want_trace, want_stats), B
