@@ -153,7 +153,7 @@ struct AsrModel {
     SideStream side_stream;  // beam search: the LM scorer's branch of a search step
     SideStream dec_stream;   // group calls: the decode loop, on a high-priority stream (see transcribe_group_enqueue)
     cudaStream_t cap_stream = nullptr;  // private stream for graph capture (the legacy default stream cannot capture)
-    int dec_tc_rows = getenv("SBK_DEC_TC_ROWS") ? atoi(getenv("SBK_DEC_TC_ROWS")) : 64;  // >= this many live hypotheses: wgmma decode GEMMs
+    int dec_tc_rows = 64;        // >= this many live hypotheses: wgmma decode GEMMs
     int dyn_chunk = 0, dyn_left = -1;  // DynChunkTrainConfig of the next encode calls (chunk frames, left-context chunks; 0 = off)
     int fuse_dec_ln = 1;         // 1: LayerNorm inside the projection kernel (latency); 0: separate LN kernel (throughput)
     int poll_every = 8;          // greedy early-exit poll interval in steps; 0 = never sync, run exactly max_steps
@@ -607,13 +607,12 @@ static int copy_steps(const AsrModel* m, void* dst, int ld, const void* src, int
     return SBK_OK;
 }
 
-// Cross-attention K/V of every decoder layer, projected once per utterance from the encoder states (b.enc16).  Layout per
-// layer (default): [K | V] parts, each [utt][head][T][64] -- the decode-step attention of (utterance, head) then streams one
-// contiguous T x 128 B block of K and one of V instead of 128-byte pieces 2 KB apart (SBK_XATT_ROWMAJOR=1: the round-1
-// [utt * T][K(d) | V(d)] rows).  Needs head_dim 64.
+// Cross-attention K/V of every decoder layer, projected once per utterance from the encoder states (b.enc16).  At head
+// width 64 and d_model a multiple of 256 the layout per layer is [K | V] parts, each [utt][head][T][64] -- the decode-step
+// attention of (utterance, head) then streams one contiguous T x 128 B block of K and one of V instead of 128-byte pieces
+// 2 KB apart.  Every other shape keeps [utt * T][K(d) | V(d)] rows.
 static bool xatt_headmajor(const AsrModel* m) {
-    static const bool legacy = getenv("SBK_XATT_ROWMAJOR") != nullptr;
-    return !legacy && m->wt->cfg.d_model / m->wt->cfg.nhead == 64 && m->wt->cfg.d_model % 256 == 0;
+    return m->wt->cfg.d_model / m->wt->cfg.nhead == 64 && m->wt->cfg.d_model % 256 == 0;
 }
 // A folded call (xatt_fold) attends over enc16 itself and needs no K/V.
 static int project_cross_kv(AsrModel* m, int M, int T, bool fold, cudaStream_t st) {
@@ -953,7 +952,7 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
     // for every step and can be replayed from a graph.  The scorers that do not read the decoder's output of this step --
     // the TransformerLM step and the CTC state update of the PREVIOUS step's survivors -- run as a second branch beside
     // the decoder layers (both are chains of small kernels that leave most SMs idle) and join before the scores are combined.
-    const bool fork = (use_lm || use_ctc) && getenv("SBK_BEAM_SERIAL") == nullptr;
+    const bool fork = use_lm || use_ctc;
     if (fork) RC(m->side_stream.ensure());
     auto enqueue_step = [&](cudaStream_t s_) -> int {
         cudaStream_t s2 = s_;
@@ -970,16 +969,12 @@ static int run_beam(AsrModel* m, int B, int T, const sbk_beam_params& p, int* hi
         RC(beam_step(a, B, s_));
         return SBK_OK;
     };
-    const bool use_graph = getenv("SBK_NO_GRAPH") == nullptr;
-    if (use_graph) {
-        struct BeamKey { sbk_beam_params p; int B, T, rows, S_max, fuse_ln, tc_rows, fork; } key;
-        memset(&key, 0, sizeof(key));
-        key.p = p; key.B = B; key.T = T; key.rows = rows; key.S_max = S_max; key.fuse_ln = m->fuse_dec_ln; key.tc_rows = m->dec_tc_rows; key.fork = fork ? 1 : 0;
-        RC(m->beam_graph.ensure(key, m->cap_stream, enqueue_step));
-    }
+    struct BeamKey { sbk_beam_params p; int B, T, rows, S_max; } key;
+    memset(&key, 0, sizeof(key));
+    key.p = p; key.B = B; key.T = T; key.rows = rows; key.S_max = S_max;
+    RC(m->beam_graph.ensure(key, m->cap_stream, enqueue_step));
     int s = 0;  // `_check_full_beams` (:806-822): b.ended_count counts the utterances whose beams are full
-    RC(run_steps(m, p.max_steps, B, st, [&](cudaStream_t s_) { return use_graph ? m->beam_graph.launch(s_) : enqueue_step(s_); },
-                 &s));
+    RC(run_steps(m, p.max_steps, B, st, [&](cudaStream_t s_) { return m->beam_graph.launch(s_); }, &s));
     const size_t hb = (size_t)s * rows * 4;
     if (hist_tok_out) SBK_CUDA_CHECK(cudaMemcpyAsync(hist_tok_out, hist_tok, hb, cudaMemcpyDeviceToDevice, st));
     if (hist_pred_out) SBK_CUDA_CHECK(cudaMemcpyAsync(hist_pred_out, hist_pred, hb, cudaMemcpyDeviceToDevice, st));
@@ -1003,7 +998,7 @@ static int run_greedy(AsrModel* m, int B, int T, int max_steps, int bos, int eos
     RC(project_cross_kv(m, M, T, fold, st));  // cross-attention K/V of all layers, once per utterance
     RC(greedy_reset(b.tokens, S_max + 1, rows, bos, b.step, b.has_ended, b.ended_count, m->wt->emb, m->wt->dec_pe, d, b.dx, st));
     set_step_pdl(m, rows, d);
-    const bool use_graph = !in_capture && getenv("SBK_NO_GRAPH") == nullptr && log_probs == nullptr;
+    const bool use_graph = !in_capture && log_probs == nullptr;
     if (in_capture) {  // the caller is capturing the whole pipeline: enqueue exactly max_steps steps, no polling
         for (int i = 0; i < max_steps; ++i) RC(enqueue_decode_step(m, rows, T, S_max, fold, eos, log_probs, max_steps, st));
         *steps_done = max_steps;
@@ -1655,14 +1650,10 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
     // The decode loop is a chain of ~3300 small, latency-bound kernels; the encoders of the other lanes are machine-filling
     // ones.  Its kernels go to a stream of the highest priority (under capture: kernel nodes of that priority), so that a ready
     // decode kernel gets the next free SM slots ahead of the remaining CTAs of an encoder kernel instead of queueing behind
-    // them.  SBK_DEC_PRIORITY=0: same stream as the encoders.
-    static const bool prio = getenv("SBK_DEC_PRIORITY") == nullptr || atoi(getenv("SBK_DEC_PRIORITY")) != 0;
-    cudaStream_t ds = st;
-    if (prio) {
-        RC(m->dec_stream.ensure(true));
-        RC(m->dec_stream.fork(st));
-        ds = m->dec_stream.s;
-    }
+    // them.
+    RC(m->dec_stream.ensure(true));
+    RC(m->dec_stream.fork(st));
+    const cudaStream_t ds = m->dec_stream.s;
     int done = 0;
     RC(run_greedy(m, G * B, T, max_steps, bos, eos, nullptr, &done, ds, in_capture));
     for (int g = 0; g < G; ++g) {
@@ -1670,7 +1661,7 @@ static int transcribe_group_enqueue(AsrModel* m, int G, const float* const* wav_
         RC(copy_steps(m, pred_dev ? pred_dev[g] : nullptr, max_steps, pred, done, B, cudaMemcpyDeviceToDevice, ds));
         RC(copy_steps(m, pred_host ? pred_host[g] : nullptr, max_steps, pred, done, B, cudaMemcpyDeviceToHost, ds));
     }
-    if (prio) RC(m->dec_stream.join(st));
+    RC(m->dec_stream.join(st));
     if (steps_done) *steps_done = done;
     return SBK_OK;
 }
@@ -1705,7 +1696,7 @@ int sbk_asr_transcribe_greedy_group_dev(sbk_asr* mm, int G, const float* const* 
     AsrModel* m = reinterpret_cast<AsrModel*>(mm);
     RC(check_group_call(m, "transcribe_group", G, wav_dev, rel_len_dev, nullptr, B, L));
     RC(ensure_workspace(m, B, L, G * B, max_steps, group_encode_batches(m->wt->cfg, G, B, L) * B));
-    const bool whole_graph = m->poll_every == 0 && getenv("SBK_NO_GRAPH") == nullptr && max_steps > 0;
+    const bool whole_graph = m->poll_every == 0 && max_steps > 0;
     struct GroupKey { const void *wav[16], *rel[16], *pred[16]; int G, B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));
     key.G = G; key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
@@ -1730,7 +1721,7 @@ int sbk_asr_transcribe_greedy_group_host_async(sbk_asr* mm, int G, const float* 
     RC(m->copy_stream.ensure());
     for (auto& e : m->ev_ready)
         if (!e) SBK_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    const bool whole_graph = m->poll_every == 0 && getenv("SBK_NO_GRAPH") == nullptr && max_steps > 0;
+    const bool whole_graph = m->poll_every == 0 && max_steps > 0;
     struct HostGroupKey { const void *wav[16], *rel[16], *pred[16], *pred_dev[16]; int G, B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));
     key.G = G; key.B = B; key.L = L; key.steps = max_steps; key.bos = bos; key.eos = eos;
@@ -1755,7 +1746,7 @@ int sbk_asr_transcribe_greedy_dev(sbk_asr* mm, const float* wav_dev, const float
     // Fixed-length runs (poll interval 0) replay ONE CUDA graph of the whole pipeline (Fbank .. last decode step):
     // ~2.6k kernel nodes, a single host-side launch per batch.
     const bool whole_graph = m->poll_every == 0 && rel_len_dev != nullptr && log_probs_dev == nullptr &&
-                             getenv("SBK_NO_GRAPH") == nullptr && (max_steps == 0 || m->wt->has_dec);
+                             (max_steps == 0 || m->wt->has_dec);
     struct PipeKey { const void *wav, *rel, *enc, *pred, *score; int B, L, steps, bos, eos; } key;
     memset(&key, 0, sizeof(key));  // the struct has tail padding and is compared bytewise
     key.wav = wav_dev; key.rel = rel_len_dev; key.enc = enc_out_dev; key.pred = pred_dev; key.score = score_dev;
