@@ -39,7 +39,8 @@ typedef struct {
     int attention_type;     /* SBK_ATT_ROPE (RoPEMHA) | SBK_ATT_RELPOS (RelPosMHAXL) | SBK_ATT_HYPERMIX (hypermixing: Conformer
                                encoder only, head width d_model / nhead 32 or 64, hypernetwork width d_ffn / nhead a multiple
                                of 16 up to 256; inputs up to 3000 frames) | SBK_ATT_REGULAR (regularMHA: the Transformer
-                               encoder only, head width 64 or 128) */
+                               encoder only, head width 64 or 128).  Head width 96 is built for the Conformer with
+                               RelPosMHAXL and no decoder layers (GigaSpeech's Conformer-Transducer) */
     int decoder_activation; /* SBK_ACT_RELU | SBK_ACT_GELU | SBK_ACT_SILU (the `activation` ctor kwarg) */
     int max_len;            /* positional tables (ctor kwarg max_length, default 2500) */
     int parts;              /* bitmask of SBK_PART_*: which sub-models the weight table carries */
@@ -150,13 +151,26 @@ int sbk_csgu_test(const void* u_dev, int B, int T, int C, const float* ln_g_dev,
 /* the encoder self-attention kernel alone, in the engine's layouts: qkv_dev [B*T, 3*H*head_dim] fp16 in per-head
  * [q | k | v] blocks; lens_dev [B] valid frames (NULL: all T; keys j >= lens[b] are masked, padded query rows are computed
  * like any other row).  relpos == 0 (RoPE / regularMHA): scores = q.k, q already scaled, scale unused.  relpos != 0
- * (RelPosMHAXL, head_dim <= 64): scores = ((q+u).k + (q+v).P[|i-j|]) * scale with pos_u_dev / pos_v_dev [H*head_dim] fp32
+ * (RelPosMHAXL, head_dim <= 64 or 80): scores = ((q+u).k + (q+v).P[|i-j|]) * scale with pos_u_dev / pos_v_dev [H*head_dim] fp32
  * and P_dev [T, H*head_dim] fp16 (row r = linear_pos of relative distance r).  chunk > 0: Dynamic Chunk attention, query i
  * sees keys [max(0, (i/chunk - left_chunks) * chunk), min(len, (i/chunk + 1) * chunk)), left_chunks < 0 = the whole past.
  * A row that sees no key is 0.  out_dev [B*T, H*head_dim] fp16.  Synchronises the stream. */
 int sbk_encoder_attention_test(const void* qkv_dev, int B, int T, int H, int head_dim, const int* lens_dev, int relpos,
                                const float* pos_u_dev, const float* pos_v_dev, const void* P_dev, float scale, int chunk,
                                int left_chunks, void* out_dev, void* stream);
+/* the same kernel at every head width the engine builds, in both of its forms.  head widths: 128, 80, 64, 36, 32, and 96
+ * with RelPosMHAXL.  kv_dev == NULL: the full-sequence form, arguments as sbk_encoder_attention_test.  kv_dev set: one
+ * stream chunk over a window of T rows whose last nq rows are the queries.  Then qkv_dev holds the queries [B*nq, H*head_dim]
+ * fp16 and kv_dev the ring [B][cap][2*H*head_dim] fp16 with head h's [k | v] at column h * 2 * head_dim; window row r lives
+ * in slot (start + r) % cap.  Every key of the window is visible (lens_dev NULL, chunk 0), P_dev has >= T rows and out_dev
+ * is [B*nq, H*head_dim].  Synchronises the stream. */
+int sbk_encoder_attention_window_test(const void* qkv_dev, const void* kv_dev, int B, int T, int H, int head_dim,
+                                      const int* lens_dev, int relpos, const float* pos_u_dev, const float* pos_v_dev,
+                                      const void* P_dev, float scale, int chunk, int left_chunks, int cap, int start, int nq,
+                                      void* out_dev, void* stream);
+/* CTAs per SM that the RelPosMHAXL encoder attention kernel reaches at head_dim (96, 80, 64, 36, 32; stream_form != 0: the
+ * stream form, built at 96, 64, 36 and 32), with the shared-memory attributes its launch sets. */
+int sbk_encoder_attention_occupancy(int head_dim, int stream_form, int* ctas_per_sm);
 
 /* one Linear of a decode / TransformerLM step alone, through the engine's step projection: out[rows, N] (row stride ldo) =
  * epilogue(A[rows, K] W[N, K]^T + bias), fp16 operands, fp32 accumulate.  backend 0 = weight streaming, 1 = the wgmma GEMM

@@ -61,7 +61,7 @@ EXPORTS = [
     "sbk_last_error", "sbk_version", "sbk_launch_count", "sbk_gemm_profile_enable", "sbk_gemm_profile_read", "sbk_fbank_create", "sbk_fbank_destroy", "sbk_fbank_num_frames",
     "sbk_fbank_forward", "sbk_input_norm_global", "sbk_input_norm_sentence", "sbk_gemm_f16_test", "sbk_gemm_f16_resid_test",
     "sbk_gemm_epilogue_test", "sbk_ctc_prefix_test", "sbk_csgu_test", "sbk_hypermix_test",
-    "sbk_encoder_attention_test", "sbk_dwconv_test", "sbk_dwconv_act_test",
+    "sbk_encoder_attention_test", "sbk_encoder_attention_window_test", "sbk_encoder_attention_occupancy", "sbk_dwconv_test", "sbk_dwconv_act_test",
     "sbk_asr_create", "sbk_asr_destroy", "sbk_asr_num_frames", "sbk_asr_cnn_forward", "sbk_asr_encode_from_cnn",
     "sbk_asr_encode_feats", "sbk_asr_greedy_from_enc", "sbk_asr_transcribe_greedy_dev",
     "sbk_asr_transcribe_greedy_host", "sbk_asr_transcribe_greedy_host_async", "sbk_asr_clone",

@@ -535,8 +535,8 @@ static int check_config(const sbk_asr_config& c) {
                 "asr_create: regularMHA is built for the Transformer encoder only, and the Transformer encoder with regularMHA only");
     SBK_REQUIRE(!tfm || dh == 64 || dh == 128, "asr_create: Transformer encoder head_dim=%d not built (128, 64)", dh);
     SBK_REQUIRE(tfm || hypermix || dh == 64 || dh == 36 || dh == 32 ||
-                    (dh == 80 && c.encoder_module == SBK_ENC_CONFORMER && c.attention_type == SBK_ATT_RELPOS),
-                "asr_create: encoder head_dim=%d not built (64, 36, 32; 80 for the Conformer with RelPosMHAXL)", dh);
+                    ((dh == 80 || dh == 96) && c.encoder_module == SBK_ENC_CONFORMER && c.attention_type == SBK_ATT_RELPOS),
+                "asr_create: encoder head_dim=%d not built (64, 36, 32; 80 and 96 for the Conformer with RelPosMHAXL)", dh);
     SBK_REQUIRE(((c.cnn_blocks == 0 || c.cnn_blocks == 2) &&
                  ((c.cnn_c1 == 64 && c.cnn_c2 == 32) || (c.cnn_c1 == 256 && c.cnn_c2 == 256))) ||
                     (c.cnn_blocks == 3 && c.cnn_c1 == 64 && c.cnn_c2 == 64),

@@ -595,9 +595,10 @@ __device__ __forceinline__ float ex2_ftz(float x) {
 // block jb is multiplied; the second buffer pair sits behind everything else); otherwise one buffer pair, refilled after
 // the block has been multiplied.  RelPosMHAXL at head width 80 takes one pair: 97 KB of shared memory, two CTAs per SM,
 // against 119 KB and one CTA with two (H100 80GB HBM3, 700 W: B = 32, 8 heads, T = 251 113 us against 158 us; T = 2500
-// 5.56 ms against 7.92 ms).
+// 5.56 ms against 7.92 ms).  At head width 96 one pair takes 111.25 KB, two CTAs per SM with the largest carveout, against
+// 137.25 KB and one CTA with two (DESIGN.md section 9, GigaSpeech Conformer-Transducer).
 template <int DH, int DHP, bool RELPOS>
-__host__ __device__ constexpr bool att_kv2() { return (DH % 8 == 0) && (DHP == DH) && !(RELPOS && DH == 80); }
+__host__ __device__ constexpr bool att_kv2() { return (DH % 8 == 0) && (DHP == DH) && !(RELPOS && (DH == 80 || DH == 96)); }
 
 template <int DH, int DHP, bool RELPOS, bool STREAM = false>  // DHP = DH rounded up to a multiple of 16 (zero-padded in shared memory)
 __global__ void __launch_bounds__(128)
@@ -935,6 +936,22 @@ encoder_attention_kernel(const __half* __restrict__ qkv, int ld, int T, const in
     }
 }
 
+// The RelPosMHAXL kernel's shared memory and the attributes its launch needs (encoder_attention_occupancy sets the same).
+// Independent of T: 101 KB at head_dim 64, 97 KB at 80 and 111.25 KB at 96 (two CTAs per SM), 69 KB at 36 and 65 KB at 32
+// (three).
+template <int DH, int DHP, bool STREAM>
+static int relpos_attention_prepare(size_t* smem) {
+    constexpr int STR = DHP + 8;
+    *smem = (4ull * ATT_BQ + ATT_PR) * STR * 2 + 4ull * 16 * (ATT_GW + 1) * 4 + (att_kv2<DH, DHP, true>() ? 2ull * ATT_BK * STR * 2 : 0);
+    auto kern = encoder_attention_kernel<DH, DHP, true, STREAM>;
+    SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
+    // two 111.25 KB CTAs and their 1 KB reservations take 224.5 KB of the SM's 228 KB: only the largest carveout holds them,
+    // so ask for it rather than leave the choice to the driver
+    if constexpr (DH == 96)
+        SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return SBK_OK;
+}
+
 template <int DH, int DHP, bool STREAM = false>
 static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int H, const int* lens, bool relpos,
                                     const float* pos_u, const float* pos_v, const __half* P, int ldp, float scale,
@@ -943,11 +960,16 @@ static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int
     constexpr int STR = DHP + 8;
     dim3 grid(ceil_div(STREAM ? sa.nq : T, ATT_BQ), H, B);
     if (!relpos) {
-        const size_t smem = 4ull * ATT_BQ * STR * 2 + 2ull * ATT_BK * STR * 2;  // + second K/V buffer pair
-        auto kern = encoder_attention_kernel<DH, DHP, false, STREAM>;
-        SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, nullptr, nullptr, nullptr, 0, scale, out, ldo, chunk, left_chunks, sa);
-    } else if constexpr (DH > 64 && DH != 80) {  // RelPosMHAXL is built for the recipes' head widths: up to 64, and 80
+        if constexpr (DH == 96) {  // GigaSpeech's head width: no recipe runs RoPEMHA or regularMHA at 96
+            set_error("encoder_attention: head_dim=96 is built for RelPosMHAXL only");
+            return SBK_ERR_UNSUPPORTED;
+        } else {
+            const size_t smem = 4ull * ATT_BQ * STR * 2 + 2ull * ATT_BK * STR * 2;  // + second K/V buffer pair
+            auto kern = encoder_attention_kernel<DH, DHP, false, STREAM>;
+            SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, nullptr, nullptr, nullptr, 0, scale, out, ldo, chunk, left_chunks, sa);
+        }
+    } else if constexpr (DH > 64 && DH != 80 && DH != 96) {  // RelPosMHAXL is built for the recipes' head widths: up to 64, 80, 96
         set_error("encoder_attention: RelPosMHAXL with head_dim=%d not built", DH);
         return SBK_ERR_UNSUPPORTED;
     } else {
@@ -956,12 +978,9 @@ static int launch_encoder_attention(const __half* qkv, int ld, int B, int T, int
             SBK_REQUIRE(ldp % 8 == 0 && (reinterpret_cast<uintptr_t>(P) & 15) == 0, "encoder_attention: P must be 16-byte aligned");
         else
             SBK_REQUIRE(ldp % 4 == 0 && (reinterpret_cast<uintptr_t>(P) & 7) == 0, "encoder_attention: P must be 8-byte aligned");
-        // independent of T: 101 KB at head_dim 64 and 97 KB at 80 (two CTAs per SM), 69 KB at 36 and 65 KB at 32 (three)
-        const size_t smem = (4ull * ATT_BQ + ATT_PR) * STR * 2 + 4ull * 16 * (ATT_GW + 1) * 4 +
-                            (att_kv2<DH, DHP, true>() ? 2ull * ATT_BK * STR * 2 : 0);
-        auto kern = encoder_attention_kernel<DH, DHP, true, STREAM>;
-        SBK_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, 128, smem, stream>>>(qkv, ld, T, lens, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, sa);
+        size_t smem = 0;
+        RC((relpos_attention_prepare<DH, DHP, STREAM>(&smem)));
+        encoder_attention_kernel<DH, DHP, true, STREAM><<<grid, 128, smem, stream>>>(qkv, ld, T, lens, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, sa);
     }
     SBK_LAUNCH_CHECK();
     return SBK_OK;
@@ -983,9 +1002,11 @@ int encoder_attention(const __half* qkv, int ld, int B, int T, int H, int head_d
         return launch_encoder_attention<32, 32>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
     if (head_dim == 80)  // the d_model 640 conformer_large recipes (Libriheavy, People's Speech): 640 / 8 heads
         return launch_encoder_attention<80, 80>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
+    if (head_dim == 96 && relpos)  // GigaSpeech's Conformer-Transducer: 768 / 8 heads with RelPosMHAXL
+        return launch_encoder_attention<96, 96>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
     if (head_dim == 128)  // the Transformer recipes' regularMHA (512 / 4 heads); no positional term
         return launch_encoder_attention<128, 128>(qkv, ld, B, T, H, lens, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, chunk, left_chunks, stream);
-    set_error("encoder_attention: head_dim=%d not built (128, 80, 64, 36, 32)", head_dim);
+    set_error("encoder_attention: head_dim=%d not built (128, 80, 64, 36, 32; 96 with RelPosMHAXL)", head_dim);
     return SBK_ERR_UNSUPPORTED;
 }
 
@@ -1003,7 +1024,35 @@ int encoder_attention_stream(const AttStream& sa, int B, int W, int H, int head_
         return launch_encoder_attention<36, 48, true>(nullptr, 0, B, W, H, nullptr, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, 0, -1, stream, sa);
     if (head_dim == 32)
         return launch_encoder_attention<32, 32, true>(nullptr, 0, B, W, H, nullptr, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, 0, -1, stream, sa);
-    set_error("encoder_attention_stream: head_dim=%d not built (64, 36 with RelPosMHAXL, 32)", head_dim);
+    if (head_dim == 96 && relpos)
+        return launch_encoder_attention<96, 96, true>(nullptr, 0, B, W, H, nullptr, relpos, pos_u, pos_v, P, ldp, scale, out, ldo, 0, -1, stream, sa);
+    set_error("encoder_attention_stream: head_dim=%d not built (64, 32; 36 and 96 with RelPosMHAXL)", head_dim);
+    return SBK_ERR_UNSUPPORTED;
+}
+
+template <int DH, int DHP, bool STREAM>
+static int relpos_attention_occupancy(int* ctas) {
+    size_t smem = 0;
+    RC((relpos_attention_prepare<DH, DHP, STREAM>(&smem)));
+    SBK_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas, encoder_attention_kernel<DH, DHP, true, STREAM>, 128, smem));
+    return SBK_OK;
+}
+
+int encoder_attention_occupancy(int head_dim, bool stream, int* ctas) {
+    if (!stream) {
+        if (head_dim == 96) return relpos_attention_occupancy<96, 96, false>(ctas);
+        if (head_dim == 80) return relpos_attention_occupancy<80, 80, false>(ctas);
+        if (head_dim == 64) return relpos_attention_occupancy<64, 64, false>(ctas);
+        if (head_dim == 36) return relpos_attention_occupancy<36, 48, false>(ctas);
+        if (head_dim == 32) return relpos_attention_occupancy<32, 32, false>(ctas);
+    } else {
+        if (head_dim == 96) return relpos_attention_occupancy<96, 96, true>(ctas);
+        if (head_dim == 64) return relpos_attention_occupancy<64, 64, true>(ctas);
+        if (head_dim == 36) return relpos_attention_occupancy<36, 48, true>(ctas);
+        if (head_dim == 32) return relpos_attention_occupancy<32, 32, true>(ctas);
+    }
+    set_error("encoder_attention_occupancy: RelPosMHAXL %s form not built at head_dim=%d", stream ? "stream" : "full-sequence",
+              head_dim);
     return SBK_ERR_UNSUPPORTED;
 }
 

@@ -1373,8 +1373,8 @@ int sbk_asr_stream_create(sbk_asr* mm, int B, int chunk_size, int left_frames, s
     SBK_REQUIRE(m->wt->has_enc, "stream_create: this handle was created without encoder weights");
     SBK_REQUIRE(c.encoder_module == SBK_ENC_CONFORMER && (c.attention_type == SBK_ATT_ROPE || c.attention_type == SBK_ATT_RELPOS),
                 "stream_create: streaming is built for the Conformer encoder with RoPEMHA or RelPosMHAXL");
-    SBK_REQUIRE(c.attention_type == SBK_ATT_RELPOS ? (dh == 64 || dh == 36 || dh == 32) : (dh == 64 || dh == 32),
-                "stream_create: head_dim=%d not built for streaming (RoPEMHA 64 or 32, RelPosMHAXL 64, 36 or 32)", dh);
+    SBK_REQUIRE(c.attention_type == SBK_ATT_RELPOS ? (dh == 64 || dh == 36 || dh == 32 || dh == 96) : (dh == 64 || dh == 32),
+                "stream_create: head_dim=%d not built for streaming (RoPEMHA 64 or 32, RelPosMHAXL 96, 64, 36 or 32)", dh);
     SBK_REQUIRE(B >= 1 && chunk_size >= 1 && left_frames >= -1, "stream_create: B >= 1, chunk_size >= 1, left_frames >= -1");
     const bool relpos = c.attention_type == SBK_ATT_RELPOS;
     const int cap = left_frames >= 0 ? left_frames + chunk_size : std::max(4 * chunk_size, 256);

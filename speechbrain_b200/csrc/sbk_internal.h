@@ -179,6 +179,8 @@ struct AttStream {
 int encoder_attention_stream(const AttStream& sa, int B, int W, int H, int head_dim, bool relpos, const float* pos_u,
                              const float* pos_v, const __half* P, int ldp, float scale, __half* out, int ldo,
                              cudaStream_t stream);
+// CTAs per SM of the RelPosMHAXL encoder attention at head_dim, full-sequence or stream form, with the attributes its launch sets
+int encoder_attention_occupancy(int head_dim, bool stream, int* ctas);
 // qkv [B*n, 3d] fp32 -> q [B*n, d] fp16 and the rows' [k | v] into ring slots (slot0 + i) % cap of kv [B][cap][2d] fp16;
 // inv_freq [head_dim / 2] set: RoPE at stream positions pos0 + i, q scaled by q_scale
 int stream_qkv(const float* qkv, int B, int n, int H, int DH, const float* inv_freq, long long pos0, float q_scale,

@@ -1,7 +1,8 @@
 """TransformerASR -- drop-in for speechbrain.lobes.models.transformer.TransformerASR.TransformerASR
 (TransformerASR.py:167-675) restricted to what the Conformer, HyperConformer and Branchformer ASR recipes instantiate:
 encoder_module="conformer" with attention_type in {"RoPEMHA", "RelPosMHAXL", "hypermixing"} and normalize_before=True
-(head width d_model / nhead of 64, 36 or 32, and 80 with RelPosMHAXL: the d_model 640 conformer_large recipes;
+(head width d_model / nhead of 64, 36 or 32; 80 with RelPosMHAXL: the d_model 640 conformer_large recipes; 96 with
+RelPosMHAXL and no decoder layers: GigaSpeech's d_model 768 Conformer-Transducer, full context, Dynamic Chunk and streaming;
 hypermixing: HyperMixing token mixing, nnet/hypermixing.py, with head width d_model / nhead of 32 or 64 and
 d_ffn / nhead a multiple of 16 up to 256), or encoder_module="branchformer" with attention_type="RelPosMHAXL"
 (Branchformer.py:92-410), or encoder_module="transformer" with attention_type="regularMHA",
@@ -101,8 +102,13 @@ class TransformerASR(torch.nn.Module):
             elif getattr(conformer_activation, "__name__", "") not in ("Swish", "SiLU"):
                 unsupported.append("conformer_activation other than Swish or torch.nn.GELU")
         if encoder_module != "transformer" and (d_model % nhead or d_model // nhead not in (64, 36, 32)):
-            if not (encoder_module == "conformer" and attention_type == "RelPosMHAXL" and d_model == 80 * nhead):
-                unsupported.append(f"head_dim={d_model // max(nhead, 1)} (64, 36 or 32; 80 for the Conformer with RelPosMHAXL)")
+            relpos_conformer = encoder_module == "conformer" and attention_type == "RelPosMHAXL"
+            if not (relpos_conformer and d_model in (80 * nhead, 96 * nhead)):
+                unsupported.append(f"head_dim={d_model // max(nhead, 1)} (64, 36 or 32; 80 and 96 for the Conformer with "
+                                   "RelPosMHAXL)")
+            elif d_model == 96 * nhead and num_decoder_layers > 0:
+                unsupported.append("decoder layers at head width 96 (the decoder attention is built for 128, 80 or a "
+                                   "multiple of 4 up to 64)")
         if d_model % 16:
             unsupported.append("d_model not a multiple of 16")
         if unsupported:

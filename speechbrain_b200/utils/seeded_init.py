@@ -174,3 +174,11 @@ SWITCHBOARD_TRANSFORMER = dict(name="switchboard_transformer", sample_rate=16000
 SWITCHBOARD_LM = dict(vocab=2000, d_model=264, d_embedding=128, nhead=12, num_encoder_layers=12, num_decoder_layers=0,
                       d_ffn=1024, normalize_before=False)
 SWITCHBOARD_BLANK, SWITCHBOARD_PAD, SWITCHBOARD_BOS, SWITCHBOARD_EOS = 0, 0, 1, 2
+# recipes/GigaSpeech/ASR/transducer/hparams/conformer_transducer.yaml (released as asr-streaming-conformer-gigaspeech): Fbank
+# with n_fft 512 and a 32 ms window, the 2-block (64, 32) front end, 12 Conformer layers at d_model 768 with RelPosMHAXL (8
+# heads of 96) and the default Swish (TransformerASR passes conformer_activation, not activation, to the encoder), no decoder
+# layers; proj_enc 768 -> 512, LSTM 512, joint 512 with GELU over 1024 tokens, blank 0
+GIGASPEECH_TRANSDUCER = dict(name="gigaspeech_transducer", sample_rate=16000, n_fft=512, win=512, hop=160, n_mels=80,
+                             cnn_channels=(64, 32), input_size=640, d_model=768, nhead=8, num_encoder_layers=12,
+                             num_decoder_layers=0, d_ffn=2048, vocab=1024, kernel_size=31, attention_type="RelPosMHAXL",
+                             decoder_activation="gelu", max_length=2500)
